@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - ICP iterations/s (whole-job) and Mpoints/s of the J^T J / J^T r reduction on B200.
+"""bench.py - ICP iterations/s (whole-job) and Mpoints/s of the J^T J / J^T r reduction on H100.
 
 Contract (see the task statement): `python bench.py --gpus N --steps K --warmup W [--impl reference]`
 prints ONE JSON line on rank 0.  A "step" is one full registration of the C2 workload (synthetic
@@ -16,6 +16,9 @@ N > 1: replicas (one independent scan pair per GPU, no data-path collective, "we
 10M-slot reduction with its 32-double ncclAllReduce is reported under "sharded".
 `--impl reference` times the reference's own CPU algorithm (oracle port; the reference binary cannot
 be built here: Eigen/PCL/yaml-cpp absent and its "Ours" stage is a stub) on the same config.
+`--dump-outputs DIR` writes, after the timed steps, what the timed calls returned in their last step as DIR/<name>.npy
+(float64; the reference arm: the oracle's final C2 pose); the inputs are seeded, so two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -40,7 +43,6 @@ C4_RADIUS = 0.05
 C4_ICP_ITERS = 10                # fixed iterations of the sharded 10 M-point corridor registration
 C5_TRIALS = 5000                 # perturbation Monte-Carlo (BASELINE.json configs[4]), split over the ranks
 ALG_BYTES_PER_SLOT = 32          # float4 point + float4 plane (SURVEY.md §8d)
-K1_NCU_TRAFFIC_BYTES = 320.07e6 + 3.54e6   # dram read + write of one 10 M-slot K1 launch (ncu --set full, profiles/k1_r2_ncu_summary.txt)
 
 
 def env_int(name, default):
@@ -56,11 +58,19 @@ def measured_peak_gbs():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (NVIDIA H100 SXM data sheet, 3.35 TB/s HBM3)"
+
+
+def _die_with_parent():
+    """In the sampler child before exec: SIGTERM it when bench.py ends, by an exception or a signal included
+    (prctl PR_SET_PDEATHSIG), so no nvidia-smi is left behind."""
+    import ctypes
+    import signal
+    ctypes.CDLL(None, use_errno=True).prctl(1, int(signal.SIGTERM), 0, 0, 0)
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -74,7 +84,7 @@ class ClockSampler:
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits",
                                           "-lms", "20", "-i", str(self.index)],
-                                         stdout=open(self.path, "w"), stderr=subprocess.DEVNULL)
+                                         stdout=open(self.path, "w"), stderr=subprocess.DEVNULL, preexec_fn=_die_with_parent)
         except Exception:
             self.proc = None
 
@@ -120,6 +130,27 @@ def c2_params(default_params):
                           handling="PRECONDITIONED_CG")
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def log_arrays(prefix, logs):
+    """The per-iteration records a caller of dcreg_icp_run receives, as arrays (one row per iteration)."""
+    return {f"{prefix}_log_n_effective": [r.n_effective for r in logs], f"{prefix}_log_n_corr_pt": [r.n_corr_pt for r in logs],
+            f"{prefix}_log_rmse": [r.rmse for r in logs], f"{prefix}_log_fitness": [r.fitness for r in logs],
+            f"{prefix}_log_objective": [r.objective for r in logs], f"{prefix}_log_dx": [list(r.dx) for r in logs],
+            f"{prefix}_log_T": [list(r.T) for r in logs], f"{prefix}_log_degenerate_mask": [list(r.analysis.degenerate_mask) for r in logs]}
+
+
+def write_dump(out_dir, dump):
+    arrays = {k: np.asarray(v, dtype=np.float64) for k, v in dump.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise SystemExit(f"bench.py: --dump-outputs would write {total} bytes (limit {DUMP_LIMIT_BYTES})")
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
+
+
 # ------------------------------------------------------------------------------------------------
 # reference arm / cpu baseline: the oracle port on host cores
 # ------------------------------------------------------------------------------------------------
@@ -128,7 +159,7 @@ def workload_config(world):
     return {"workload": f"C2 synthetic cylinder pair {C2_POINTS} pts x {C2_ITERS} fixed ICP iterations per step from the published "
                         "perturbation, method Ours (Schur detection + PCG), search_radius 1.0, weight derivative off (released default)",
             "parallelism": "replicas (one scan pair per GPU)" if world > 1 else "1 GPU",
-            "l2": "K1 roofline inputs 320 MB > 126 MB L2; no flush needed",
+            "l2": "K1 roofline inputs 320 MB > 50 MB L2; no flush needed",
             "roofline_workload": f"C4 synthetic corridor {C4_SLOTS} slots, frozen float4 planes"}
 
 
@@ -309,7 +340,7 @@ def run_reference(args, rank, world):
         return
     arm = CpuArm(seed=42)
     arm.calibrate()
-    times, _ = arm.steps(args.steps, args.warmup)
+    times, T = arm.steps(args.steps, args.warmup)
     cpu = arm.describe(times)
     cpu["reference_faithful_8_threads"] = arm.faithful()
     value = cpu["value"]
@@ -324,6 +355,8 @@ def run_reference(args, rank, world):
         "gpu_launches": 0,
     }
     print(json.dumps(line))
+    if args.dump_outputs:
+        write_dump(args.dump_outputs, {"c2_T": T, "c2_iterations": C2_ITERS})   # the pose the GPU arm dumps as c2_T
 
 
 # ------------------------------------------------------------------------------------------------
@@ -384,6 +417,7 @@ def run_ours(args, rank, local_rank, world):
     e1.synchronize()
     res = ctx.icp_fetch()
     assert res.iterations == C2_ITERS
+    dump = {"c2_T": res.T, "c2_iterations": res.iterations, "c2_converged": res.converged}
     barrier()
     dev_ms = max_over_ranks(e0.elapsed_time(e1))
     launches = ctx.launch_count - l0
@@ -413,6 +447,7 @@ def run_ours(args, rank, local_rank, world):
     barrier()
     e2e_ms = max_over_ranks(max(e2.elapsed_time(e3), wall * 1e3))
     clocks = sampler.stop() if rank == 0 else None
+    dump.update(e2e_T=res.T, e2e_iterations=res.iterations, e2e_converged=res.converged, **log_arrays("e2e", res.logs))
     e2e_value = world * args.steps * C2_ITERS / (e2e_ms * 1e-3)
     from dcreg_b200.api import IterLog
     import ctypes
@@ -445,9 +480,12 @@ def run_ours(args, rank, local_rank, world):
         max over ranks per batch): one batch right after an idle gap reads ~1 us high while the clocks ramp"""
         ts = [max_over_ranks(ctx.time_reduce(f64, Tc, wd, reps, False)) for _ in range(5)]
         return float(np.median(ts)), ts
-    k1_ms, k1_batches = k1_time(False, False)                                   # inputs (320 MB) > L2 (126 MB)
+    k1_ms, k1_batches = k1_time(False, False)                                   # inputs (320 MB) > L2 (50 MB)
     k1_ms_f64, _ = k1_time(True, False)
     k1_ms_wd, _ = k1_time(False, True)
+    # time_reduce returns only a time: one more launch of the same kernel on the same inputs recomputes what the timed
+    # launches computed (deterministic for a fixed grid)
+    dump["k1_sums"], dump["k1_stats"] = ctx.reduce_device(False, Tc, False)
     barrier()
     peak, peak_src = measured_peak_gbs()
     n_local = hi - lo
@@ -469,6 +507,7 @@ def run_ours(args, rank, local_rank, world):
     f1.synchronize()
     barrier()
     c4_ms = max_over_ranks(f0.elapsed_time(f1)) / c4_runs
+    dump.update(c4_T=res4.T, c4_iterations=res4.iterations, **log_arrays("c4", res4.logs))
     comm_mode = ctx.comm_mode
     sharded_ok, sharded_dT = None, None
     ctx2 = Context(local_rank)                                               # plain context: no communicator
@@ -520,6 +559,8 @@ def run_ours(args, rank, local_rank, world):
     g1.record(stream2)
     g1.synchronize()
     w5 = time.perf_counter() - w5
+    dump.update(c5_T=np.array([t.T for t in trials]), c5_iterations=[t.iterations for t in trials],
+                c5_converged=[t.converged for t in trials], c5_status=[t.status for t in trials])
     barrier()
     c5_ms = max_over_ranks(max(g0.elapsed_time(g1), w5 * 1e3))
     n_conv = torch.tensor([float(sum(t.converged for t in trials)), float(sum(t.iterations for t in trials))],
@@ -581,7 +622,7 @@ def run_ours(args, rank, local_rank, world):
                              "ordered list reuses its plane - results identical to searching and fitting every time (tests/test_gpu_parity.py)"},
             "roofline": {"kernel": "k1s::reduce_stream_kernel<float4, wd=false> (K1)", "bound": "hbm", "achieved": achieved, "peak": peak,
                          "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": K1_NCU_TRAFFIC_BYTES * n_local / C4_SLOTS, "traffic_source": "ncu --set full dram__bytes_read+write per 10 M-slot launch, profiles/k1_r2_ncu_summary.txt",
+                         "traffic": ALG_BYTES_PER_SLOT * n_local, "traffic_source": "algorithmic: one float4 point + one float4 plane read per slot",
                          "peak_source": peak_src,
                          "ms_per_launch": k1_ms, "slots_per_launch": n_local, "bytes_per_slot": ALG_BYTES_PER_SLOT,
                          "timing": f"median of 5 batches of {reps} back-to-back launches, CUDA events on the launching stream", "batch_ms": k1_batches},
@@ -600,6 +641,8 @@ def run_ours(args, rank, local_rank, world):
             "clocks": clocks,
         }
         print(json.dumps(line))
+        if args.dump_outputs:
+            write_dump(args.dump_outputs, dump)
     ctx.close()
     if world > 1:
         dist.destroy_process_group()
@@ -612,9 +655,13 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step of each timed call as DIR/<name>.npy (float64)")
     ap.add_argument("--cpu-worker", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--cpu-trials", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     rank, local_rank, world = env_int("RANK", 0), env_int("LOCAL_RANK", 0), env_int("WORLD_SIZE", 1)
     if args.cpu_worker:
         pin_openmp_env(host_cpu_budget()[0])

@@ -1,4 +1,4 @@
-"""Build the sm_100a shared library in-tree with nvcc (no JIT cache: the .so travels with the repo)."""
+"""Build the sm_90a (H100) shared library in-tree with nvcc (no JIT cache: the .so travels with the repo)."""
 from __future__ import annotations
 
 import os
@@ -14,7 +14,7 @@ HEADERS = ["corr.cuh", "k1_reduce.cuh", "k1_stream.cuh", "k2_solve.cuh", "k2_fas
            "../../include/dcreg_b200.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "--shared", "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",

@@ -299,7 +299,7 @@ __device__ __forceinline__ void knn_search(const Grid& g, float qx, float qy, fl
         // outwards.  A row / cell is skipped only when its box distance exceeds the current 5th-best distance
         // (strictly, with a 1e-5 relative margin for the float arithmetic of the bound), so the search stays exact.
         // Loops are deliberately NOT unrolled: one copy of the scan loop keeps the kernel inside the instruction
-        // cache (the fully unrolled version stalled on instruction fetch, profiles/icp_iteration_r1).
+        // cache (a fully unrolled version stalls on instruction fetch).
         const int K = g.rings;
         const float cell = (float)(1.0 / g.inv_cell);
         const int lx = cx - g.ox, ly = cy - g.oy, lz = cz - g.oz;
@@ -515,7 +515,7 @@ __device__ __forceinline__ void knn_search_lb(const Grid& g, float qx, float qy,
 
 // ---- one query, one warp (dense grid) -----------------------------------------------------------------------------
 // Same contract as knn_search_lb, executed by all 32 lanes for ONE query: used when only a few slots of a warp need a
-// search, where the sequential search of one lane would keep the other 31 waiting for ~15 us.  Lanes set up the cell
+// search, where the sequential search of one lane would keep the other 31 waiting for the whole search.  Lanes set up the cell
 // rows in parallel, walk every row with stride 32 (coalesced), compact the candidates with d2 <= B into a 64-entry
 // shared buffer and rank them ((d2, index) order): ranks 0..6 are the list, everything else feeds lb.
 // Returns false (nothing usable) when more than 64 candidates survive the bound; the caller then searches sequentially.
@@ -673,9 +673,9 @@ __device__ __forceinline__ bool knn_warp_search(const Grid& g, float qx, float q
     if (prof) tc2 = clock64();
     // Rank of every candidate inside the bound = number of candidates that precede it in (d2, index) order; ranks 0..6 are
     // the list.  All-pairs over the (few: ~20 of ~45 scanned) hits with broadcast shared-memory reads: the iterations
-    // are independent, so unrolled they pipeline (~500 cycles).  Measured alternatives on the C2 loop (clock64 per
-    // phase, tools/timeline.py): seven warp-wide minimum extractions with REDUX 2200-2900 cycles (a serial chain of
-    // collectives), this loop not unrolled ~2000.
+    // are independent, so unrolled they pipeline.  Slower during development (clock64 per phase, tools/timeline.py; not
+    // re-measured on H100): seven warp-wide minimum extractions with REDUX (a serial chain of collectives), this loop
+    // not unrolled.
 #pragma unroll 1
     for (int en = lane; en < cnt; en += 32) {
         const unsigned long long ke = S.key[en];
@@ -822,9 +822,9 @@ __device__ __forceinline__ bool fit_plane(const Grid& g, const int (&kpos)[5], d
 
 // The same fit with the register-resident QR (small_la.cuh: same operations in the same order, bit-identical results).  A
 // separate function with its own register allocation: it is called from the fit work list of the loop kernel, where
-// almost nothing is live across the call (inlined into a loop body full of live state it spills; measured 3.7x slower
-// there).  Measured and rejected (round 2): a variant of the QR with hardware reciprocal / rsqrt seeds instead of the
-// ~30 IEEE divisions and square roots on the fit's dependent chain) makes a fit 7 -> 6 us, but on exactly rank-deficient
+// almost nothing is live across the call (inlined into a loop body full of live state it spills and ran several times
+// slower during development; not re-measured on H100).  Rejected: a variant of the QR with hardware reciprocal / rsqrt
+// seeds instead of the ~30 IEEE divisions and square roots on the fit's dependent chain) shortens a fit, but on exactly rank-deficient
 // neighbourhoods (collinear lattice points) its 1-ulp differences flip the pivoted QR's rank decision, and the loop then
 // disagrees with the generic fit by one correspondence (tests/test_gpu_parity.py, lattice scene).
 __device__ __noinline__ bool fit_plane_reg(const Grid& g, const int (&kpos)[5], double min_norm, double thickness,

@@ -1,4 +1,4 @@
-// dcreg_b200.cu - kernels + C ABI of the B200-native ICP / degeneracy engine (see include/dcreg_b200.h).
+// dcreg_b200.cu - kernels + C ABI of the H100 (sm_90a) ICP / degeneracy engine (see include/dcreg_b200.h).
 //
 // Data layout in HBM (per context):
 //   src      float4[N]   body-frame source points (x,y,z,-), uploaded once per scan
@@ -43,8 +43,8 @@ constexpr int kBlock = 256;
 
 // Programmatic dependent launch (sm_90+): the loop's two kernels are launched with the programmatic-stream-
 // serialization attribute, so kernel k+1 is scheduled while kernel k still runs; pdl_wait() blocks until kernel k
-// has completed and its writes are visible, pdl_release() lets kernel k+2 be scheduled.  Hides ~2 us of launch
-// latency per kernel on the loop's critical path.  Without the attribute both are no-ops.
+// has completed and its writes are visible, pdl_release() lets kernel k+2 be scheduled.  Hides the launch
+// latency of every kernel on the loop's critical path.  Without the attribute both are no-ops.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_release() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
@@ -320,7 +320,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
             DCREG_STAMP(1);
             __syncthreads();
             // -- 2. searches: few -> one warp per listed slot (the other slots' threads are not held up by a
-            //       15 us sequential search); many -> every thread searches for its own slot
+            //       long sequential search); many -> every thread searches for its own slot
             const int nS = sm.nS;
             if (coherent && nS <= a.coop_max) {
                 corr::WarpKnnSmem& W = *reinterpret_cast<corr::WarpKnnSmem*>(sm.tbuf[warp]);
@@ -519,8 +519,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
 
 // K2 as its own kernel: baseline methods (their generic single-thread step), hash-grid runs, the host-plane loop and the
 // NCCL fallback of a sharded run.  One warp per trial (blockIdx.x).
-// K2 executes a few thousand warp instructions exactly once per launch (round 1 ncu: top stall no_instruction, 14 cycles
-// per instruction).  Thanks to the programmatic dependent launch it starts while the
+// K2 executes a few thousand warp instructions exactly once per launch, so it stalls on instruction fetch.  Thanks to the programmatic dependent launch it starts while the
 // iteration kernel is still running, so it first executes the SAME code on a scratch copy of the state with the
 // previous iteration's sums (same branches, harmless stores), which pulls the instructions into the SM's caches;
 // only then does it wait for the iteration kernel and do the real step.
@@ -719,7 +718,7 @@ constexpr int kNcclSum = 0;
 // ------------------------------------------------------------------------------------------------
 struct dcreg_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     cudaStream_t stream = nullptr;
     std::string err;
     long long launches = 0;
@@ -898,7 +897,7 @@ int launch_reduce_k(dcreg_ctx* ctx, k1s::Args& a, int g) {
 
 template <typename PlaneT, bool kUseWd>
 int launch_reduce_t(dcreg_ctx* ctx, k1s::Args& a) {
-    // persistent grid: every SM holds 2 CTAs (launch bounds; 2 x (32 KB / 48 KB ring) fits the 227 KB carveout)
+    // persistent grid: every SM holds 2 CTAs (launch bounds; 2 x (32 KB / 48 KB ring) fits H100's 227 KB carveout)
     const long long nchunks = (a.n + 31) / 32;
     long long g = (long long)ctx->sm_count * 2;
     const long long need = (nchunks + k1s::kWarpsPerBlock - 1) / k1s::kWarpsPerBlock;
@@ -907,7 +906,7 @@ int launch_reduce_t(dcreg_ctx* ctx, k1s::Args& a) {
     int rc = ensure_partials(ctx, (int)g);
     if (rc) return rc;
     a.partials = ctx->d_partials;
-    // team size (k1_stream.cuh): 1, 2, 4, 37 and 296 CTAs per contiguous range all measured 70-71 us on 10 M slots
+    // team size (k1_stream.cuh): 1 CTA per contiguous range; larger teams were no faster during development (not re-measured on H100)
     return launch_reduce_k<PlaneT, kUseWd, 1>(ctx, a, (int)g);
 }
 
@@ -1534,7 +1533,7 @@ int dcreg_time_reduce(dcreg_ctx* ctx, int plane_is_f64, const double pose_Rt[12]
     for (int i = 0; i < 9; ++i) P.R[i] = pose_Rt[i];
     for (int i = 0; i < 3; ++i) P.t[i] = pose_Rt[9 + i];
     if (flush_l2 && !ctx->d_flush) {
-        ctx->flush_n = (256ll << 20) / sizeof(float4);   // 256 MiB > 126 MB L2
+        ctx->flush_n = (256ll << 20) / sizeof(float4);   // 256 MiB > 50 MB L2
         CK(cudaMalloc(&ctx->d_flush, (size_t)ctx->flush_n * sizeof(float4)));
     }
     const void* plane = plane_is_f64 ? (const void*)ctx->d_planes64 : (const void*)ctx->d_planes32;
@@ -1704,8 +1703,7 @@ static void key_bytes(std::vector<unsigned char>& k, const void* p, size_t n) {
 
 // Enqueue `iters` loop bodies.  The bodies are identical launches (pose, mode flags and the done flag live on the
 // device), so a chunk is captured once into a CUDA graph and replayed: one host call per chunk instead of one or two
-// launches per iteration - what keeps 8 independent ranks from queueing behind the host (round 1: 0.887 weak scaling
-// at 8 GPUs with nothing shared between the ranks).  Falls back to plain launches if capture is unavailable.
+// launches per iteration - what keeps independent ranks from queueing behind the host.  Falls back to plain launches if capture is unavailable.
 static int enqueue_iterations(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_params* prm, dcreg_iter_log* dlog, int log_cap, int iters) {
     static int use_graph = -1;
     if (use_graph < 0) use_graph = getenv("DCREG_NO_GRAPH") ? 0 : 1;

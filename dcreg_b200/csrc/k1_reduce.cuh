@@ -60,9 +60,8 @@ __device__ __forceinline__ double round_f32(double x) {
 // (|x| < 1.2e-38) come out as +-2^-126-sized values instead of 0 (an absolute perturbation of 1e-38 m on a
 // coordinate - far below one FP64 ulp of any coordinate that is not itself ~1e-22 m), and Inf/NaN map to ~1e38-
 // sized finite values which - like NaN in the reference - fail the weight gate and drop the slot.
-// Why not F2F: on B200 the 64-bit conversions, DFMA/DMUL/DADD and DMMA all issue through one shared pipe whose
-// issue cost is additive (measured per warp instruction and sub-partition: F2F.F64.F32 6, F2F.F32.F64 9, DFMA 2,
-// DMMA 16.4 cycles; tools/microbench*.cu), and that pipe is the binding resource of K1.
+// Why not F2F: the 64-bit conversions issue through the same FP64 pipe as DFMA/DMUL/DADD and DMMA, and that pipe is
+// the binding resource of K1 (tools/microbench*.cu measure the per-instruction costs on the device at hand).
 __device__ __forceinline__ double f32_to_f64(float f) {
     const unsigned u = __float_as_uint(f);
     const unsigned hi = (((u >> 3) & 0x0FFFFFFFu) + 0x38000000u) | (u & 0x80000000u);   // re-bias exponent by +896
@@ -110,7 +109,7 @@ __device__ __forceinline__ void slot_front(const Pose& P, double px, double py, 
 // the register-hungry k-NN / plane-fit code.  The per-slot components are transposed into the fragment layout
 // through a 2.3 KB per-warp shared buffer (8 STS.64 + 8 LDS.64 per 32 slots, conflict-free with the padded stride).
 // (The streaming kernel uses plain DFMA chains instead: there the FP64 issue slots are the bottleneck and
-// 29 DFMA x 2 cycles beat 8 DMMA x 16.4 cycles.)  All 32 lanes must call this convergently.
+// 29 DFMA take fewer FP64 issue slots than 8 DMMA.)  All 32 lanes must call this convergently.
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
     asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
                  : "+d"(c0), "+d"(c1)

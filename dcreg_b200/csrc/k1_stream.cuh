@@ -1,15 +1,14 @@
 // k1_stream.cuh - K1, the streaming kernel: fused point-to-plane residual / LOAM weight / gate / 6-DoF Jacobian
-// row / 21 + 6 (+2) normal-equation sums over device-resident (point, plane) slots, for sm_100a.
+// row / 21 + 6 (+2) normal-equation sums over device-resident (point, plane) slots, for sm_90a.
 //
-// Shape of the kernel and why (every statement below was measured on B200; profiles/k1_*.md, tools/microbench*.cu):
-//   * Cost model.  On B200 the FP64 vector ops (DFMA/DMUL/DADD: 2 cycles per warp instruction per SM sub-
-//     partition), the FP64 tensor op (DMMA m8n8k4: 16.4 cycles) and the 64-bit conversions (F2F.F64.F32 6,
-//     F2F.F32.F64 9 cycles) all issue through one shared pipe, and their costs ADD to the 1 cycle every other
-//     instruction takes: the kernel time is (instructions + extra FP64 slots) / issue rate, independent of
-//     occupancy once latency is covered.  Six rewrites that moved work between those units without lowering that
-//     sum (LDG vs TMA bulk + mbarrier ring vs cp.async ring, 8..32 warps/SM, 1..4 slots per thread, vector vs
-//     DMMA accumulation, F2F vs integer conversions) all landed on the same ~110-130 us for 10 M slots.
-//   * So the kernel minimises issue slots per slot (133 instructions, 56 of them FP64, per 32 slots): float->double
+// Shape of the kernel and why (tools/microbench*.cu measure the pipe costs this rests on):
+//   * Cost model.  The FP64 vector ops (DFMA/DMUL/DADD), the FP64 tensor op (DMMA m8n8k4) and the 64-bit
+//     conversions (F2F) all issue through one shared pipe, and their costs ADD to the cycle every other instruction
+//     takes: the kernel time is (instructions + extra FP64 slots) / issue rate, independent of occupancy once latency
+//     is covered.  Rewrites that only move work between those units (LDG vs TMA bulk + mbarrier ring vs cp.async
+//     ring, 8..32 warps/SM, 1..4 slots per thread, vector vs DMMA accumulation, F2F vs integer conversions) did not
+//     lower that sum during development (not re-measured on H100).
+//   * So the kernel minimises issue slots per slot: float->double
 //     is 3-4 integer instructions (IMAD.WIDE shifts the float fields into place; for the point the exponent re-bias
 //     is folded into the rotation constants), the reference's float32 round trips are 4 (LEA carry trick), the 29
 //     sums are plain DFMA chains (29 x 2 slots, cheaper than 8 DMMA x 16.4 + the 16 LDS/STS of a fragment
@@ -18,15 +17,13 @@
 //   * Loads: each lane copies its own 16 B point and 16 B (32 B) plane with cp.async (LDGSTS, L1 bypass) into a
 //     lane-private 4-deep shared-memory ring, so the ring needs NO barrier (only cp.async.wait_group) and no
 //     registers; 16 warps x 4 KB are in flight per SM.  (TMA bulk copies were tried first: a single producer
-//     thread per CTA topped out at 3.2 TB/s in a copy-only experiment, below what per-lane LDGSTS/LDG reach.)
+//     thread per CTA streamed less than per-lane LDGSTS/LDG in a copy-only experiment during development; not
+//     re-measured on H100.)
 //     A CTA streams one contiguous range of each array; its warps interleave 512 B chunks inside it.
 //   * Reduction: 31-shuffle transpose-reduction per warp -> per-block partial (32 doubles) -> the last block (atomic
 //     ticket) sums the partials in a fixed order with all loads in flight at once, applies the world->body
 //     congruence with 42 threads and writes the 27 + stats.  Deterministic for a given grid size.
-//   * Result on B200 (10 M slots, 320 MB): 67 us without the weight derivative (4.8 TB/s, 74 % of the measured
-//     6.48 TB/s copy peak), 75 us with it; time = 5.76 us per million slots (5.55 TB/s, 86 %) + 8.3 us fixed
-//     (2.2 launch, 2.1 ramp-up, 0.6 warp reduction, 3.5 grid reduction; tools/sweep_k1.py).  The 48 B/slot FP64-
-//     plane variant is DRAM-bound at 6.1 TB/s (95 %).
+//   * Measured time on H100: bench.py's `roofline` and `reduction` entries (DESIGN.md §4).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,7 +1,7 @@
 // k2_fast.cuh - the 3x3 pieces of the solve step, written for ONE dependent chain per lane.
 //
-// Where the time of the solve step goes (profiles/k2_step_r1: 4.4 k warp instructions executed exactly once by one
-// warp, ~15-18 us of every ICP iteration): two 3x3 Jacobi eigen-decompositions (6 sweeps x 3 rotations, each with two
+// Where the time of the solve step goes (~4.4 k warp instructions executed exactly once by one warp in every ICP
+// iteration): two 3x3 Jacobi eigen-decompositions (6 sweeps x 3 rotations, each with two
 // IEEE divisions and a square root = ~120 dependent instructions), two 3x3 inverses through a generic full-pivot LU on
 // local-memory arrays, and a PCG with two more divisions and a square root per iteration.  Nothing here is throughput:
 // it is one long dependent chain, so the only way to make it faster is to make it SHORTER.  This file does that

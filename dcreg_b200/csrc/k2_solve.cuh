@@ -471,9 +471,8 @@ __device__ inline void icp_step(const double* acc, IcpState* st, const dcreg_icp
 
 // ------------------------------------------------------------------------------------------------------------------
 // Warp-cooperative K2 step for the "Ours" method (SCHUR_CONDITION_NUMBER + PRECONDITIONED_CG), the per-iteration
-// critical path of the loop.  Why: executed by a single thread the step is ~7 k dependent FP64 instructions; on B200 a
-// dependent DFMA issues every ~40 cycles and the straight-line code is fetched cold on every launch (profiles/
-// k2_step_r1: 101 k cycles, top stall = no_instruction).  Here the 32 lanes share the work: the two 3x3 inverses and
+// critical path of the loop.  Why: executed by a single thread the step is ~7 k dependent FP64 instructions, each
+// waiting for the previous one, and the straight-line code is fetched cold on every launch.  Here the 32 lanes share the work: the two 3x3 inverses and
 // the two 3x3 Jacobi EVDs run on lanes 0/1 side by side, Schur products and the preconditioner are one entry per
 // lane, and the PCG mat-vecs are row-per-lane with shuffle broadcasts and butterfly dot products.  The in-loop record
 // gets the non-analysis fields; the analysis block is (re)computed for every record by log_fill_kernel after the run

@@ -4,8 +4,8 @@
 // icp_test_runner.cpp:1714-1863, one slot per thread).  Every phase of the kernel is a latency chain per tile, so:
 //   * a single run keeps all its tiles resident at once (<= 3 blocks per SM; more slots: the blocks loop over tiles);
 //   * a single run of a SMALL cloud (fewer 256-slot tiles than SMs) is cut into >= 2 tiles per SM at 32-slot
-//     granularity instead of leaving most SMs idle - measured 47.3 -> 36.1 us per iteration on the shipped 7 562-point
-//     cloud (tools/tile_sweep.py); no effect once there is a tile per SM;
+//     granularity instead of leaving most SMs idle - measured 45.6 -> 36.0 us per iteration on the shipped 7 562-point
+//     cloud on an H100 (tools/tile_sweep.py); no effect once there is a tile per SM;
 //   * batched trials (grid y = trial) are throughput-bound: full tiles, at most 64 blocks per trial.
 // tests/test_host_la.py::test_loop_tile_plan checks the invariants on the CPU.
 #pragma once

@@ -3,11 +3,11 @@
 // SURVEY.md §8e: the path shards by contiguous source-point blocks and has exactly ONE exchange per ICP iteration -
 // the sum over ranks of the 27 + 5 accumulators (the OpenMP `reduction(+: ...)` of icp_test_runner.cpp:1714 and
 // SymmetricHessianComputer::join, hessian_computer.h:103-108).  256 B per rank: pure latency.  A separate
-// ncclAllReduce kernel behind the reduction costs ~25 us per iteration (round 1: 65.9 -> 40.5 us for 10 M slots on
-// 8 GPUs, i.e. 1.6x), so the exchange lives in the LAST BLOCK of the reducing kernel instead:
+// ncclAllReduce kernel behind the reduction adds a launch and a collective to every iteration, so the exchange lives
+// in the LAST BLOCK of the reducing kernel instead:
 //
 //   every rank owns an 8 KB mailbox in its own HBM, mapped into every peer's address space (cudaIpc handles
-//   exchanged once in dcreg_comm_init; NVLink 5 / NVSwitch P2P stores);
+//   exchanged once in dcreg_comm_init; NVLink / NVSwitch P2P stores);
 //   epoch e (same on all ranks: every rank runs the same sequence of reductions):
 //     post : warp q of the last block stores this rank's 32 packed totals into rank q's mailbox slot
 //            pkt[e & 1][my_rank][0..63] as 64 self-validating 8-byte packets {32 data bits, epoch}: an aligned 8-byte

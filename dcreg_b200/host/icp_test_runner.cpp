@@ -1,4 +1,4 @@
-// icp_test_runner.cpp - the reference's experiment harness on top of the B200 engine's C ABI.
+// icp_test_runner.cpp - the reference's experiment harness on top of the engine's C ABI.
 //
 // Same surface as DCReg's `icp_test_runner` executable (DCReg/src/icp_main.cpp:6-52, icp_test_runner.cpp:20-516,
 // 603-1510): YAML schema (SURVEY.md Appendix B.1), method table keyed by name, per-method runs, statistics and the

@@ -1,5 +1,5 @@
 /*
- * dcreg_b200.h - C ABI of the B200-native point-to-plane ICP + Schur-decoupled degeneracy engine.
+ * dcreg_b200.h - C ABI of the H100 (sm_90a) point-to-plane ICP + Schur-decoupled degeneracy engine.
  *
  * This is the drop-in boundary for ONE hot path of JokerJohn/DCReg (SURVEY.md §8b).  The
  * reference has no FFI layer; each entry point below names the C++ member / code block of the

@@ -1,7 +1,7 @@
 """CPU oracle (NumPy/SciPy twin) for the DCReg hot path.  TEST INFRASTRUCTURE ONLY.
 
 This file restates, in plain FP64 NumPy, the one path of JokerJohn/DCReg that the
-B200 engine accelerates.  It is a *checker*: only ``tests/``, ``__graft_entry__.smoke()``
+CUDA engine accelerates.  It is a *checker*: only ``tests/``, ``__graft_entry__.smoke()``
 and ``bench.py``'s cpu_baseline / ``--impl reference`` leg may import it.  The product
 (``dcreg_b200``) never imports anything from ``oracle/``.
 
@@ -12,7 +12,7 @@ tests/golden/make_golden.py).  The reference binary itself cannot be built here
 (Eigen/PCL/yaml-cpp/Ceres/TBB/Open3D absent; its "Ours" path is a stub in the released
 source), see DESIGN.md.
 
-Every function cites the reference file:line (relative to /root/reference) it follows.
+Every function cites the reference file:line (relative to a checkout of the reference) it follows.
 The stubbed "Ours" stages (Schur detection, preconditioner, PCG) follow the paper's
 Alg. 1/3, Eq. 18-21, 43-46 as summarised in SURVEY.md §3.4 and are pinned by the shipped
 per-iteration ``dx`` / ``T`` of the authors' own run (G2).

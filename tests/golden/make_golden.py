@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """Extract the reference's shipped golden vectors into tests/golden/golden.json.
 
-Run HERE (needs /root/reference, which does not exist on the GPU box):
-    python tests/golden/make_golden.py
+Needs a checkout of the reference (JokerJohn/DCReg @ 0519bdb); nothing else reads it:
+    python tests/golden/make_golden.py <reference checkout>
 
-Sources (SURVEY.md §8c), all relative to /root/reference:
+Sources (SURVEY.md §8c), all relative to that checkout:
   G1  DCReg/dataset/icp_results/            released code, init t=(0.01,0.01,0.01), WD off
   G2  results/simulation/table3_fig9_fig10/ full code incl. "Ours", init (0.2,0.8,0.5 m;
                                             0.1,0.1,2 deg), weight derivative ON
@@ -16,8 +16,9 @@ import csv
 import json
 import os
 import re
+import sys
 
-REF = "/root/reference"
+REF = None
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 DX = ["dx_wx", "dx_wy", "dx_wz", "dx_x", "dx_y", "dx_z"]
@@ -118,4 +119,7 @@ def main():
 
 
 if __name__ == "__main__":
+    if len(sys.argv) != 2 or not os.path.isdir(sys.argv[1]):
+        sys.exit("usage: python tests/golden/make_golden.py <reference checkout (JokerJohn/DCReg @ 0519bdb)>")
+    REF = sys.argv[1]
     main()

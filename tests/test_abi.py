@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 @pytest.fixture(scope="module")
 def lib():
     from dcreg_b200 import build, api
-    build.build()                      # cross-compiles sm_100a with nvcc if stale
+    build.build()                      # cross-compiles sm_90a with nvcc if stale
     return api.load_library()
 
 
@@ -68,8 +68,8 @@ def test_no_device_fails_loudly(lib):
     assert e.value.status == api.NO_DEVICE
 
 
-def test_sass_is_sm100a():
+def test_sass_is_sm90a():
     import subprocess
     from dcreg_b200 import api
     out = subprocess.run(["cuobjdump", "--list-elf", api.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out

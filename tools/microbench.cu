@@ -1,5 +1,5 @@
-// Pipe-rate microbenchmarks for sm_100a (B200): FP64 FMA, F2F conversions, INT ALU, mixed.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench tools/microbench.cu
+// Pipe-rate microbenchmarks for sm_90a (H100): FP64 FMA, F2F conversions, INT ALU, mixed.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench tools/microbench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define ITERS 2048
@@ -25,7 +25,7 @@ __global__ void kern(double* out, double a, double b, int n) {
 }
 template <int MODE>
 void run(const char* name, double ops_per_iter_per_thread, int blocks_per_sm, int threads) {
-    int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     int clk = 0; cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0);
     double* out; cudaMalloc(&out, sizeof(double) * sms * blocks_per_sm * threads);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);

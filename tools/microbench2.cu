@@ -1,4 +1,4 @@
-// FP64 tensor-core (mma.sync m8n8k4 f64) rate on sm_100a, alone and mixed with DFMA / F2F.
+// FP64 tensor-core (mma.sync m8n8k4 f64) rate on sm_90a, alone and mixed with DFMA / F2F.
 #include <cstdio>
 #include <cuda_runtime.h>
 #define ITERS 2048
@@ -26,7 +26,7 @@ __global__ void kern(double* out, double a, double b, int n) {
 }
 template <int MODE, int NACC>
 void run(const char* name, int blocks_per_sm, int threads) {
-    int sms = 148; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     int clk = 0; cudaDeviceGetAttribute(&clk, cudaDevAttrClockRate, 0);
     double* out; cudaMalloc(&out, sizeof(double) * sms * blocks_per_sm * threads);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);

@@ -1,4 +1,4 @@
-// Read-only streaming bandwidth on B200: how fast can a kernel READ two 160 MB arrays (no writes)?
+// Read-only streaming bandwidth on H100: how fast can a kernel READ two 160 MB arrays (no writes)?
 #include <cstdio>
 #include <cuda_runtime.h>
 template <int U>
@@ -24,6 +24,7 @@ __global__ void cp(const float4* __restrict__ a, float4* __restrict__ b, long lo
 }
 int main() {
     const long long n = 10'000'000;
+    int sms = 132; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     float4 *a, *b; float* out;
     cudaMalloc(&a, n * 16); cudaMalloc(&b, n * 16); cudaMalloc(&out, 4);
     cudaMemset(a, 1, n * 16); cudaMemset(b, 2, n * 16);
@@ -38,15 +39,15 @@ int main() {
     };
     for (int bps : {2, 4, 8, 16}) {
         char nm[64];
-        snprintf(nm, 64, "read 2x160MB U=1 blocks/SM=%d", bps); time([&] { rd<1><<<148 * bps, 256>>>(a, b, n, out); }, nm, 2.0 * n * 16);
-        snprintf(nm, 64, "read 2x160MB U=2 blocks/SM=%d", bps); time([&] { rd<2><<<148 * bps, 256>>>(a, b, n, out); }, nm, 2.0 * n * 16);
-        snprintf(nm, 64, "read 2x160MB U=4 blocks/SM=%d", bps); time([&] { rd<4><<<148 * bps, 256>>>(a, b, n, out); }, nm, 2.0 * n * 16);
+        snprintf(nm, 64, "read 2x160MB U=1 blocks/SM=%d", bps); time([&] { rd<1><<<sms * bps, 256>>>(a, b, n, out); }, nm, 2.0 * n * 16);
+        snprintf(nm, 64, "read 2x160MB U=2 blocks/SM=%d", bps); time([&] { rd<2><<<sms * bps, 256>>>(a, b, n, out); }, nm, 2.0 * n * 16);
+        snprintf(nm, 64, "read 2x160MB U=4 blocks/SM=%d", bps); time([&] { rd<4><<<sms * bps, 256>>>(a, b, n, out); }, nm, 2.0 * n * 16);
     }
-    time([&] { cp<<<148 * 8, 256>>>(a, b, n); }, "copy 160MB->160MB (r+w bytes)", 2.0 * n * 16);
+    time([&] { cp<<<sms * 8, 256>>>(a, b, n); }, "copy 160MB->160MB (r+w bytes)", 2.0 * n * 16);
     // bigger buffers
     float4 *c, *d; const long long m = 64'000'000;
     cudaMalloc(&c, m * 16); cudaMalloc(&d, m * 16); cudaMemset(c, 1, m * 16); cudaMemset(d, 2, m * 16);
-    time([&] { rd<4><<<148 * 8, 256>>>(c, d, m, out); }, "read 2x1GB U=4 blocks/SM=8", 2.0 * m * 16);
-    time([&] { cp<<<148 * 8, 256>>>(c, d, m); }, "copy 1GB->1GB (r+w bytes)", 2.0 * m * 16);
+    time([&] { rd<4><<<sms * 8, 256>>>(c, d, m, out); }, "read 2x1GB U=4 blocks/SM=8", 2.0 * m * 16);
+    time([&] { cp<<<sms * 8, 256>>>(c, d, m); }, "copy 1GB->1GB (r+w bytes)", 2.0 * m * 16);
     return 0;
 }

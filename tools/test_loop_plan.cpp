@@ -29,21 +29,23 @@ int main() {
             }
         }
     }
-    // the shipped cloud and C2 on a B200
-    loop_plan::Tiles a = loop_plan::plan_tiles(7562, 1, 148, 256);
+    // the shipped cloud and C2 on an H100 (132 SMs)
+    loop_plan::Tiles a = loop_plan::plan_tiles(7562, 1, 132, 256);
     CHECK(a.tile == 32 && a.grid_x == 237);
-    a = loop_plan::plan_tiles(100000, 1, 148, 256);
+    a = loop_plan::plan_tiles(100000, 1, 132, 256);
     CHECK(a.tile == 256 && a.grid_x == 391);
-    a = loop_plan::plan_tiles(10000000, 1, 148, 256);
-    CHECK(a.tile == 256 && a.grid_x == 444);
-    a = loop_plan::plan_tiles(7562, 5000, 148, 256);
+    a = loop_plan::plan_tiles(10000000, 1, 132, 256);
+    CHECK(a.tile == 256 && a.grid_x == 396);
+    a = loop_plan::plan_tiles(7562, 5000, 132, 256);
     CHECK(a.tile == 256 && a.grid_x == 30);
     // the measurement override: honoured when it fits, ignored when it does not
-    a = loop_plan::plan_tiles(100000, 1, 148, 256, 232);
-    CHECK(a.tile == 232 && a.grid_x == 432);
-    a = loop_plan::plan_tiles(100000, 1, 148, 256, 128);
+    a = loop_plan::plan_tiles(90000, 1, 132, 256, 232);
+    CHECK(a.tile == 232 && a.grid_x == 388);
+    a = loop_plan::plan_tiles(100000, 1, 132, 256, 232);
     CHECK(a.tile == 256 && a.grid_x == 391);
-    a = loop_plan::plan_tiles(100000, 1, 148, 256, 7);
+    a = loop_plan::plan_tiles(100000, 1, 132, 256, 128);
+    CHECK(a.tile == 256 && a.grid_x == 391);
+    a = loop_plan::plan_tiles(100000, 1, 132, 256, 7);
     CHECK(a.tile == 256);
     std::printf("%lld cases, %d failures\n", cases, fails);
     if (!fails) std::printf("LOOP_PLAN_OK\n");

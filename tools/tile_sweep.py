@@ -1,5 +1,6 @@
 """Loop time against the tile size (source slots per block) of the iteration kernel: DCREG_TILE sweep.
-C2 (100 k points, 50 fixed iterations) and the shipped 7 562-point cloud (30 fixed iterations)."""
+C2 (100 k points, 50 fixed iterations) and the shipped 7 562-point cloud (30 fixed iterations).  A tile that would need
+more blocks than a single run may keep resident (loop_plan.hpp: 3 per SM) is ignored by plan_tiles, so it is skipped."""
 import os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -18,7 +19,11 @@ def sweep(name, pts, iters, tiles, reps=20):
         ctx.set_source(pts)
         stream = torch.cuda.ExternalStream(ctx.stream)
         ref = None
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
         for t in tiles:
+            if t and -(-len(pts) // t) > 3 * sms:
+                print(f"{name}: tile {t:>7}  skipped: {-(-len(pts) // t)} blocks > 3 x {sms} SMs, plan_tiles would keep 256", flush=True)
+                continue
             if t:
                 os.environ["DCREG_TILE"] = str(t)
             else:
