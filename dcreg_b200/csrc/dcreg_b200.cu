@@ -219,12 +219,64 @@ struct Iter2Args {
     float look;               // squared-distance look-ahead beyond the seed bound (kNnLook)
     unsigned int* stats;      // optional [2]: slots that searched, slots that refitted (profiling)
     int tile;                 // source slots per block and pass (<= kBlock; plan_iteration: chosen so the blocks fill whole SM rounds)
+    // single-trial folded run with a solver block (row_flags != null): block 0 sums the rows and solves (solver_block),
+    // blocks 1.. work on the tiles; no ticket
+    unsigned long long* row_flags;   // [grid.x - 1] row b is published with the value row_epoch + 1 of its launch
+    unsigned long long* row_epoch;   // per-context launch counter (device memory: graph-captured arguments are frozen)
+    IcpState* warm_state;            // scratch state of the solver block's warm-up step, or null (DCREG_NO_SOLVER_WARMUP)
 };
 
 __device__ __forceinline__ void cswap5(unsigned long long& ka, int& pa, unsigned long long& kb, int& pb) {
     if (kb < ka) {                                    // one 64-bit compare = (distance, then index) order (corr::knn_key)
         const unsigned long long tk = ka; ka = kb; kb = tk;
         const int tp = pa; pa = pb; pb = tp;
+    }
+}
+
+// The solver block of a single-trial folded run (blockIdx.x == 0, so it is dispatched first).  Without it the iteration
+// ends in a serial chain that starts only when the last tile block wins the ticket: sum of all rows, then a solve step
+// of a few thousand warp instructions fetched cold on whichever SM finished last.  Here, while the tile blocks work,
+// warp 0 runs one step on a scratch copy of the state with the previous iteration's sums (everything it reads is stable
+// after pdl_wait; it writes only the scratch state), which pulls the step's instructions into this SM's caches; then all
+// warps sum the rows as they land (k1s::stream_rows_to_fin: the same additions as the ticket path, bit for bit), and
+// the real step follows at once.  A row that never lands ends the trial with DCREG_CUDA_ERROR instead of hanging.
+constexpr unsigned long long kRowTimeoutNs = 4000000000ull;
+__device__ __noinline__ void solver_block(const Iter2Args& a, IcpState* st, Iter2Smem& sm, unsigned long long row_epoch,
+                                          unsigned int peer_epoch) {
+    const IterArgs& A = a.it;
+    const int tid = threadIdx.x, warp = tid >> 5;
+    k2::WarpSmem* wsm = reinterpret_cast<k2::WarpSmem*>(sm.tbuf[0]);
+    if (a.warm_state && warp == 0) {
+        for (int e = tid; e < (int)(sizeof(IcpState) / sizeof(int)); e += 32)
+            reinterpret_cast<int*>(a.warm_state)[e] = reinterpret_cast<const int*>(st)[e];
+        __syncwarp();
+        solve_step_in_kernel(A.acc, a.warm_state, &A.prm, nullptr, 0, wsm, a.src_radius, a.coherent_step, nullptr, nullptr);
+        DCREG_STAMP(1);
+    }
+    const bool ok = k1s::stream_rows_to_fin(sm.tail, A.partials, a.row_flags, row_epoch + 1, (int)gridDim.x - 1,
+                                            kRowTimeoutNs);
+    if (tid == 0) *a.row_epoch = row_epoch + 1;     // the next launch reads it after pdl_wait
+    DCREG_STAMP(6);
+    if (!ok) {
+        if (tid == 0) {
+            st->done = 1; st->converged = 0; st->status = DCREG_CUDA_ERROR;
+            if (a.n_active) atomicSub(a.n_active, 1u);
+        }
+        return;
+    }
+    peer::all_reduce32(a.peer, sm.tail.fin, sm.tail.red, peer_epoch);
+    k1s::congruence(sm.tail.fin, st->R, sm.tail.acc);
+    __syncthreads();
+    DCREG_STAMP(7);
+    if (tid < kAcc) A.acc[tid] = sm.tail.acc[tid];
+    if (warp == 0) {
+        solve_step_in_kernel(sm.tail.acc, st, &A.prm, a.log, a.log_cap, wsm, a.src_radius, a.coherent_step, a.n_active,
+                             a.stamps ? a.stamps + (size_t)gridDim.x * kStampSlots : nullptr);
+        DCREG_STAMP(8);
+        if (a.stamps && tid == 0) {
+            a.stamps[(size_t)gridDim.x * kStampSlots + 14] = 1;     // timeline: block 0 is the solver block
+            a.stamps[(size_t)gridDim.x * kStampSlots + 15] = 0;
+        }
     }
 }
 
@@ -239,10 +291,17 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     IcpState* const st = A.state + trial;
     if (st->done) return;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const bool solver_path = a.row_flags != nullptr;
+    if (solver_path && blockIdx.x == 0) {
+        DCREG_STAMP(0);
+        solver_block(a, st, sm, *a.row_epoch, peer::load_epoch(a.peer));
+        return;
+    }
     const k1::Pose P = load_pose(st);
     const corr::Grid& g = A.grid;
     const unsigned int epoch0 = peer::load_epoch(a.peer);     // (after pdl_wait: the previous launch has advanced it)
     DCREG_STAMP(0);
+    const int tb = (int)blockIdx.x - (solver_path ? 1 : 0), ntb = (int)gridDim.x - (solver_path ? 1 : 0);   // tile block
     // this trial's slices of the per-slot records
     int4* const rec_nn = a.nn + (size_t)trial * kNnRec * A.n;
     double4* const rec_plane = a.plane_cache + (size_t)trial * A.n;
@@ -260,7 +319,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     {
         // ---- tiles of a.tile (<= 256) slots with per-tile work lists, so that searches and fits run densely packed.  Lean mode (the
         // pose still moves a lot) uses the same phases: every slot searches (plain 5-NN), every accepted slot fits.
-        for (long long base = (long long)blockIdx.x * a.tile; base < A.n; base += (long long)gridDim.x * a.tile) {
+        for (long long base = (long long)tb * a.tile; base < A.n; base += (long long)ntb * a.tile) {
             const long long i = base + tid;
             const bool valid = tid < a.tile && i < A.n;
             if (tid == 0) { sm.nS = 0; sm.nF = 0; }
@@ -471,6 +530,8 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
         }
     }
     DCREG_STAMP(5);
+    // (the solver block advances the counter only after it has seen this block's flag, which carries the value read here)
+    const unsigned long long row_want = solver_path ? *a.row_epoch + 1 : 0ull;
     if (a.stats) {
         n_search = __reduce_add_sync(0xffffffffu, n_search);
         n_fit = __reduce_add_sync(0xffffffffu, n_fit);
@@ -499,6 +560,11 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     else if (lane == k1s::kPkB2) mine = G[6 * 8 + 6];
     else if (lane == k1s::kPkNeff) mine = (double)neff;
     else if (lane == k1s::kPkNpt) mine = (double)npt;
+    if (solver_path) {
+        k1s::publish_row(mine, sm.tail, A.partials + (size_t)tb * k1s::kPk, a.row_flags + tb, row_want);
+        DCREG_STAMP(6);
+        return;
+    }
     // ---- grid reduction of this trial, [sum over ranks], congruence, solve + pose update: all in the last block
     if (!k1s::reduce_to_fin(mine, sm.tail, A.partials + (size_t)trial * gridDim.x * k1s::kPk, A.counter + trial,
                             (int)blockIdx.x, (int)gridDim.x)) return;
@@ -762,6 +828,11 @@ struct dcreg_ctx {
     void drop_graphs() { for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec); graphs.clear(); }
     double* d_small = nullptr;       // scratch for the seams (>= 512 doubles)
     K2Scratch* d_k2_scratch = nullptr;   // K2's rehearsal state (see k2_step_kernel)
+    // solver block of a single-trial folded run (solver_block): row flags, launch counter, warm-up state.  The counter
+    // and the flags are never reset, so no flag written by an earlier launch can match a later one
+    unsigned long long* d_row_flags = nullptr; int row_flags_cap = 0;
+    unsigned long long* d_row_epoch = nullptr;
+    IcpState* d_warm_state = nullptr;
     dcreg_analysis* d_analysis = nullptr;
     float4* d_flush = nullptr; long long flush_n = 0;
 
@@ -802,6 +873,22 @@ int ensure_partials(dcreg_ctx* ctx, int blocks) {
     return DCREG_OK;
 }
 
+int ensure_row_flags(dcreg_ctx* ctx, int rows) {
+    if (!ctx->d_row_epoch) {
+        CK(cudaMalloc(&ctx->d_row_epoch, sizeof(unsigned long long)));
+        CK(cudaMemsetAsync(ctx->d_row_epoch, 0, sizeof(unsigned long long), ctx->stream));
+        CK(cudaMalloc(&ctx->d_warm_state, sizeof(IcpState)));
+        CK(cudaMemsetAsync(ctx->d_warm_state, 0, sizeof(IcpState), ctx->stream));
+    }
+    if (ctx->row_flags_cap >= rows) return DCREG_OK;
+    if (ctx->d_row_flags) cudaFree(ctx->d_row_flags);
+    ctx->d_row_flags = nullptr; ctx->row_flags_cap = 0;
+    CK(cudaMalloc(&ctx->d_row_flags, (size_t)rows * sizeof(unsigned long long)));
+    CK(cudaMemsetAsync(ctx->d_row_flags, 0, (size_t)rows * sizeof(unsigned long long), ctx->stream));   // below every epoch + 1
+    ctx->row_flags_cap = rows;
+    return DCREG_OK;
+}
+
 int ensure_planes(dcreg_ctx* ctx, long long n) {
     if (ctx->planes_cap >= n) return DCREG_OK;
     if (ctx->d_planes64) cudaFree(ctx->d_planes64);
@@ -832,6 +919,7 @@ int ensure_trials(dcreg_ctx* ctx, int trials) {
     CK(cudaMalloc(&ctx->d_counter, (size_t)trials * sizeof(unsigned int)));
     CK(cudaMemsetAsync(ctx->d_counter, 0, (size_t)trials * sizeof(unsigned int), ctx->stream));
     CK(cudaMalloc(&ctx->d_acc, (size_t)trials * kAcc * sizeof(double)));
+    CK(cudaMemsetAsync(ctx->d_acc, 0, (size_t)trials * kAcc * sizeof(double), ctx->stream));   // the solver block's warm-up input
     CK(cudaMalloc(&ctx->d_state, (size_t)trials * sizeof(IcpState)));
     CK(cudaMemsetAsync(ctx->d_state, 0, (size_t)trials * sizeof(IcpState), ctx->stream));
     CK(cudaMalloc(&ctx->d_T_init, (size_t)trials * 16 * sizeof(double)));
@@ -958,6 +1046,7 @@ int read_results(dcreg_ctx* ctx, int trials, double* T_out, dcreg_iter_log* log,
         if (n_iterations) n_iterations[t] = hs[t].iter;
         if (converged) converged[t] = hs[t].converged;
         if (status_out) status_out[t] = hs[t].status;
+        if (hs[t].status == DCREG_CUDA_ERROR) ctx->err = "loop: the solver block timed out waiting for the block rows";
     }
     if (log && log_cap > 0) {
         if (trials == 1) {
@@ -1043,7 +1132,8 @@ int dcreg_destroy(dcreg_ctx* ctx) {
     void* ptrs[] = {ctx->d_n_active, ctx->d_T_init, ctx->d_sort_tmp, ctx->d_src, ctx->d_stage, ctx->d_tgt, ctx->grid.keys, ctx->grid.cell_start, ctx->grid.hstart,
                     ctx->grid.hcount, ctx->d_src_sorted, ctx->d_cell_tmp, ctx->d_pt_cell, ctx->d_tile_sums,
                     ctx->grid.pts, ctx->grid.pos_of, ctx->d_planes64, ctx->d_planes32, ctx->d_partials, ctx->d_counter, ctx->d_acc,
-                    ctx->d_state, ctx->d_log, ctx->d_small, ctx->d_analysis, ctx->d_flush, ctx->d_nn, ctx->d_plane_cache, ctx->d_fit_state, ctx->d_iter_stats, ctx->d_src_radius, ctx->d_plane_key, ctx->d_k2_scratch};
+                    ctx->d_state, ctx->d_log, ctx->d_small, ctx->d_analysis, ctx->d_flush, ctx->d_nn, ctx->d_plane_cache, ctx->d_fit_state, ctx->d_iter_stats, ctx->d_src_radius, ctx->d_plane_key, ctx->d_k2_scratch,
+                    ctx->d_row_flags, ctx->d_row_epoch, ctx->d_warm_state};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
@@ -1346,16 +1436,28 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
             ctx->nn_cap = slots; ctx->nn_trials = trials;
             ctx->nn_valid = false;
         }
+        // the solve step inside the kernel unless the sum over ranks has to go through NCCL
+        L.fold_k2 = want_fold && !(ctx->comm && !ctx->peer_ok) && !getenv("DCREG_NO_FOLD") &&
+                    prm->detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm->handling == DCREG_HAND_PRECONDITIONED_CG;
+        // a single folded run: block 0 is a dedicated solver block (solver_block); batches keep the ticket, since a
+        // solver block per trial in a multi-wave grid could fill every resident slot with waiting blocks
+        const bool solver = L.fold_k2 && trials == 1 && !getenv("DCREG_NO_SOLVER_BLOCK");
         // blocks per trial and slots per block: loop_plan.hpp
         const char* tile_env = trials == 1 ? getenv("DCREG_TILE") : nullptr;            // measurement switch
-        const loop_plan::Tiles tp = loop_plan::plan_tiles(slots, trials, ctx->sm_count, kBlock, tile_env ? atoi(tile_env) : 0);
-        L.grid_x = (int)tp.grid_x;
+        const loop_plan::Tiles tp = loop_plan::plan_tiles(slots, trials, ctx->sm_count, kBlock, tile_env ? atoi(tile_env) : 0,
+                                                          solver ? 1 : 0);
+        L.grid_x = (int)tp.grid_x + (solver ? 1 : 0);
         L.b.tile = tp.tile;
         int rc = ensure_partials(ctx, L.grid_x * trials);
         if (rc) return rc;
+        if (solver && (rc = ensure_row_flags(ctx, (int)tp.grid_x))) return rc;
         a.partials = ctx->d_partials;
         Iter2Args& b = L.b;
         b.it = a;
+        if (solver) {
+            b.row_flags = ctx->d_row_flags; b.row_epoch = ctx->d_row_epoch;
+            b.warm_state = getenv("DCREG_NO_SOLVER_WARMUP") ? nullptr : ctx->d_warm_state;   // measurement switch
+        }
         b.nn = ctx->d_nn; b.plane_cache = ctx->d_plane_cache; b.fit_state = ctx->d_fit_state; b.plane_key = ctx->d_plane_key;
         b.force = ctx->force_coherent ? 1 : 0;
         { static int cm = -1; if (cm < 0) { const char* e = getenv("DCREG_COOP_MAX"); cm = e ? atoi(e) : kSearchListMax; } b.coop_max = cm; }
@@ -1366,9 +1468,6 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         float r2f = (float)r2;
         if ((double)r2f < r2) r2f = nextafterf(r2f, INFINITY);
         b.r2_up = r2f;
-        // the solve step inside the kernel unless the sum over ranks has to go through NCCL
-        L.fold_k2 = want_fold && !(ctx->comm && !ctx->peer_ok) && !getenv("DCREG_NO_FOLD") &&
-                    prm->detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm->handling == DCREG_HAND_PRECONDITIONED_CG;
         b.fold_k2 = L.fold_k2 ? 1 : 0;
         b.log = dlog; b.log_cap = log_cap;
         b.src_radius = ctx->d_src_radius; b.coherent_step = coherent_step_setting();

@@ -220,6 +220,85 @@ __device__ __forceinline__ bool reduce_to_fin(double mine, TailSmem& ts, double*
     return true;
 }
 
+// Solver-block variant of the same reduction (the loop kernel's single-trial path, dcreg_b200.cu): no ticket; a block
+// that has written its row publishes it with a per-row flag, and one dedicated block sums the rows while they land.
+//
+// Order rule, shared with reduce_to_fin: fin[l] = ((0 + W_0[l]) + W_1[l]) + ... + W_7[l], where W_w[l] =
+// ((0 + row_w[l]) + row_{w+8}[l]) + row_{w+16}[l] + ... in increasing row order.  stream_rows_to_fin performs exactly
+// these additions, only earlier: a row is added once it and every earlier row of its warp's sequence have landed, so
+// the result is bit-identical to reduce_to_fin over the same rows.
+//
+// Flags carry `want` = epoch + 1 of the launch (a per-context counter that only grows): flags are never reset, and a
+// flag left by an earlier launch holds a smaller value, so it never matches.
+__device__ __forceinline__ void publish_row(double mine, TailSmem& ts, double* row, unsigned long long* flag,
+                                            unsigned long long want) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    ts.red[warp][lane] = mine;
+    __syncthreads();
+    if (warp == 0) {
+        double s = 0.0;
+#pragma unroll
+        for (int w = 0; w < kWarpsPerBlock; ++w) s += ts.red[w][lane];
+        row[lane] = s;
+        __syncwarp();                                             // the warp's 32 stores happen-before lane 0's release
+        if (lane == 0) asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(flag), "l"(want) : "memory");
+    }
+}
+
+// All threads of the solver block call this (a warp may arrive late: nothing waits for it before the final barrier).
+// Warp w polls the flags of its next 32 rows (one acquire load per lane), takes the ready prefix of its sequence and
+// issues all of that prefix's loads at once, so after the last row lands about one poll round and the 8-way sum remain.
+// Returns false in every thread if a warp still missed a row `timeout_ns` after it first found none ready (ts.fin is
+// then meaningless).
+__device__ __forceinline__ bool stream_rows_to_fin(TailSmem& ts, const double* partials, const unsigned long long* flags,
+                                                   unsigned long long want, int nrows, unsigned long long timeout_ns) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    double s = 0.0;
+    bool timed_out = false;
+    int k = 0;                                                    // rows warp + 8 j, j < k, are summed
+    unsigned long long t0 = 0;
+    while (warp + kWarpsPerBlock * k < nrows) {
+        const int r = warp + kWarpsPerBlock * (k + lane);
+        bool ready = true;                                        // rows past the end count as landed
+        if (r < nrows) {
+            unsigned long long f;
+            asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(f) : "l"(flags + r) : "memory");
+            ready = f == want;
+        }
+        const unsigned int bits = __ballot_sync(0xffffffffu, ready);
+        const int n = bits == 0xffffffffu ? 32 : __ffs(~bits) - 1;    // ready prefix of the warp's sequence
+        __syncwarp();                                             // the acquiring lanes' view reaches every lane
+        for (int j0 = 0; j0 < n; j0 += 8) {
+            double t[8];
+#pragma unroll
+            for (int u = 0; u < 8; ++u) {
+                const int b = warp + kWarpsPerBlock * (k + j0 + u);
+                t[u] = (j0 + u < n && b < nrows) ? __ldcg(partials + (size_t)b * kPk + lane) : 0.0;
+            }
+#pragma unroll
+            for (int u = 0; u < 8; ++u)
+                if (j0 + u < n && warp + kWarpsPerBlock * (k + j0 + u) < nrows) s += t[u];
+        }
+        k += n;
+        if (n == 0) {
+            unsigned long long now;
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+            if (t0 == 0) t0 = now;
+            else if (now - t0 > timeout_ns) { timed_out = true; break; }
+        }
+    }
+    ts.red[warp][lane] = s;
+    const bool ok = !__syncthreads_or(timed_out);
+    if (warp == 0) {
+        double f = 0.0;
+#pragma unroll
+        for (int w = 0; w < kWarpsPerBlock; ++w) f += ts.red[w][lane];
+        ts.fin[lane] = f;
+    }
+    __syncthreads();
+    return ok;
+}
+
 // world -> body: H_body = Q^T H Q, g_body = Q^T g with Q = blkdiag(R, R); one thread per output entry.  fin: packed
 // world-frame totals (shared memory), out: k2::kAcc doubles (shared or global).  Called by all threads of the block.
 __device__ __forceinline__ void congruence(const double* fin, const double* R, double* out) {

@@ -20,13 +20,14 @@ struct Tiles {
 
 // tile_override: 0 = rule above; otherwise a requested tile size for single runs (measurement switch DCREG_TILE),
 // ignored when it is out of range or would not fit the resident blocks.
-inline Tiles plan_tiles(long long slots, int trials, int sm_count, int block_threads, int tile_override = 0) {
+// reserved: resident slots a single run keeps for blocks without a tile (the solver block), not counted in grid_x.
+inline Tiles plan_tiles(long long slots, int trials, int sm_count, int block_threads, int tile_override = 0, int reserved = 0) {
     Tiles t{block_threads, std::max<long long>(1, (slots + block_threads - 1) / block_threads)};
     if (trials != 1) {
         t.grid_x = std::min<long long>(t.grid_x, 64);
         return t;
     }
-    const long long cap = (long long)sm_count * 3;
+    const long long cap = (long long)sm_count * 3 - reserved;
     if (t.grid_x > cap) { t.grid_x = cap; return t; }
     int tile = block_threads;
     if (t.grid_x < sm_count) tile = (int)std::max<long long>(32, (slots / (2LL * sm_count) + 31) / 32 * 32);
