@@ -87,7 +87,7 @@ EXPORTS = [
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -122,6 +122,8 @@ def load_library():
                                   C.POINTER(ci)]
     lib.dcreg_icp_run_batch.argtypes = [vp, C.POINTER(IcpParams), ci, dp, dp, C.POINTER(ci), C.POINTER(ci), C.POINTER(ci),
                                         C.POINTER(IterLog), ci]
+    lib.dcreg_icp_run_scans.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(C.c_float), C.POINTER(i64), ci, dp, dp,
+                                        C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(IterLog), ci]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -182,8 +184,9 @@ def pose_Rt(T):
 
 
 class IcpResult:
-    def __init__(self, status, converged, iterations, T, logs):
+    def __init__(self, status, converged, iterations, T, logs, cov=None):
         self.status, self.converged, self.iterations, self.T, self.logs = status, converged, iterations, T, logs
+        self.cov = cov
 
 
 class Context:
@@ -373,6 +376,42 @@ class Context:
                     nrec = n_it[b] + 1
                 recs = [logs[b * cap + i] for i in range(nrec)]
             out.append(IcpResult(int(st[b]), bool(conv[b]), int(n_it[b]), T_out[b], recs))
+        return out
+
+    def icp_run_scans(self, params: IcpParams, scans, T_init, want_log: bool = False, want_cov: bool = False):
+        """Different scans (a list of (N_b, >=3) point arrays) against the context's target, side by side, each from its
+        own initial pose (T_init (B, 4, 4)).  The context's own source is left as it was.  Returns a list of IcpResult,
+        one per scan (logs only when want_log, .cov the post-loop 6x6 covariance when want_cov)."""
+        pts = [_as_points(s)[:, :3] for s in scans]
+        B = len(pts)
+        if B == 0:                                      # BAD_ARG from the library, like every other malformed batch
+            self._check(self.lib.dcreg_icp_run_scans(self._h, C.byref(params), 0, None, None, 3, None, None, None, None,
+                                                     None, None, None, 0))
+        xyz = np.ascontiguousarray(np.concatenate(pts, axis=0))
+        stride = 3
+        offsets = np.zeros(B + 1, dtype=np.int64)
+        offsets[1:] = np.cumsum([p.shape[0] for p in pts])
+        T_init = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
+        if T_init.shape[0] != B:
+            raise ValueError(f"icp_run_scans: {B} scans but {T_init.shape[0]} initial poses")
+        T_out = np.empty((B, 4, 4))
+        n_it = (C.c_int * B)(); conv = (C.c_int * B)(); st = (C.c_int * B)()
+        cov = np.empty((B, 6, 6)) if want_cov else None
+        cap = int(params.max_iterations) if want_log else 0
+        logs = (IterLog * max(cap * B, 1))() if want_log else None
+        self._check(self.lib.dcreg_icp_run_scans(self._h, C.byref(params), B, xyz.ctypes.data_as(C.POINTER(C.c_float)),
+                                                 offsets.ctypes.data_as(C.POINTER(C.c_int64)), stride, _dptr(T_init),
+                                                 _dptr(T_out), n_it, conv, st, _dptr(cov) if want_cov else None, logs, cap))
+        out = []
+        for b in range(B):
+            recs = []
+            if want_log:
+                nrec = min(n_it[b], cap)
+                if st[b] == NONFINITE_UPDATE and n_it[b] < cap:
+                    nrec = n_it[b] + 1
+                recs = [logs[b * cap + i] for i in range(nrec)]
+            out.append(IcpResult(int(st[b]), bool(conv[b]), int(n_it[b]), T_out[b], recs,
+                                 cov[b] if want_cov else None))
         return out
 
     def icp_run_host_planes(self, params: IcpParams, T_init, plane_fn, want_log: bool = True) -> IcpResult:

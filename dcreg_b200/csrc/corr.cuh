@@ -209,11 +209,8 @@ __global__ void grid_rank_cells_kernel(const float4* __restrict__ in, int n, con
 }
 
 // cell of a (transformed) source point for the spatial sort of the source cloud, clamped into the target box
-__global__ void source_cell_kernel(const float4* __restrict__ src, int n, Grid g, const double* __restrict__ T,
-                                   int* __restrict__ pt_cell, int* __restrict__ counts) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float4 p = src[i];
+// (T: the first 12 entries of a row-major 4x4 pose)
+__device__ __forceinline__ int source_cell(const Grid& g, const double* __restrict__ T, float4 p) {
     const double px = p.x, py = p.y, pz = p.z;
     const float qx = (float)(T[0] * px + T[1] * py + T[2] * pz + T[3]);
     const float qy = (float)(T[4] * px + T[5] * py + T[6] * pz + T[7]);
@@ -221,7 +218,14 @@ __global__ void source_cell_kernel(const float4* __restrict__ src, int n, Grid g
     const int cx = min(max(cell_coord(qx, g.inv_cell) - g.ox, 0), g.nx - 1);
     const int cy = min(max(cell_coord(qy, g.inv_cell) - g.oy, 0), g.ny - 1);
     const int cz = min(max(cell_coord(qz, g.inv_cell) - g.oz, 0), g.nz - 1);
-    const int c = (cz * g.ny + cy) * g.nx + cx;
+    return (cz * g.ny + cy) * g.nx + cx;
+}
+
+__global__ void source_cell_kernel(const float4* __restrict__ src, int n, Grid g, const double* __restrict__ T,
+                                   int* __restrict__ pt_cell, int* __restrict__ counts) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int c = source_cell(g, T, src[i]);
     pt_cell[i] = c;
     atomicAdd(&counts[c], 1);
 }

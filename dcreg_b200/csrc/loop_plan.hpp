@@ -6,8 +6,9 @@
 //   * a single run of a SMALL cloud (fewer 256-slot tiles than SMs) is cut into >= 2 tiles per SM at 32-slot
 //     granularity instead of leaving most SMs idle - measured 45.6 -> 36.0 us per iteration on the shipped 7 562-point
 //     cloud on an H100 (tools/tile_sweep.py); no effect once there is a tile per SM;
-//   * batched trials (grid y = trial) are throughput-bound: full tiles, at most 64 blocks per trial.
-// tests/test_host_la.py::test_loop_tile_plan checks the invariants on the CPU.
+//   * batched trials (grid y = trial) are throughput-bound: full tiles, at most 64 blocks per trial;
+//   * a batch of different scans (ragged slot counts) follows its largest scan (plan_scan_tiles).
+// tests/test_host_la.py::test_loop_tile_plan and tests/test_scan_plan.py check the invariants on the CPU.
 #pragma once
 #include <algorithm>
 
@@ -36,6 +37,14 @@ inline Tiles plan_tiles(long long slots, int trials, int sm_count, int block_thr
     t.tile = tile;
     t.grid_x = std::max<long long>(1, (slots + tile - 1) / tile);
     return t;
+}
+
+// A batch of different scans (trial = one scan with its own slot count, dcreg_icp_run_scans): one grid for all of them,
+// sized by the largest scan with the batch rule above (full tiles, at most 64 blocks per trial), also for one scan.
+// Block tb of scan b takes the tiles tb, tb + grid_x, ... below n_b; a block with tb * tile >= n_b takes none and only
+// contributes a zero row to its scan's reduction.
+inline Tiles plan_scan_tiles(long long max_slots, int block_threads) {
+    return plan_tiles(max_slots, 2, 0, block_threads);
 }
 
 }  // namespace loop_plan

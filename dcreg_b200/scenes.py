@@ -2,6 +2,7 @@
 
 C2  make_cylinder : the shipped cylinder's geometry (wall R = 40 m, z in [0, 20] + floor disc z = 0) at any size
 C3  make_parking  : ground-dominated local map + sparse verticals, LiDAR-like frame (stand-in, pair not shipped)
+    make_parking_frames : the same map and a sequence of frames along a path through it (batched localisation)
 C4  make_corridor : two parallel walls + floor + ceiling, rank-deficient along x
 C5  trial_poses   : seeded perturbations t ~ U[-1, 1]^3 m, rpy ~ U[-3, 3]^3 deg for the Monte-Carlo (SURVEY.md §8d)
     load_pcd_xyz  : PCD v0.7 `DATA binary` with float32 fields (the shipped clouds, SURVEY.md Appendix B.3)
@@ -63,10 +64,7 @@ def make_corridor(n, seed=44, length=200.0, half_width=2.0, height=3.0, noise=0.
     return np.ascontiguousarray(pts, dtype=np.float32)
 
 
-def make_parking(n_map=500_000, n_scan=6_000, seed=43, extent=60.0, max_range=30.0):
-    """Ground plane (z = -1.8 + 1 cm noise) with a few pillars/walls; the scan is a range-limited subsample of
-    the map seen from the origin.  Planar degeneracy: x, y, yaw weakly constrained."""
-    rng = np.random.default_rng(seed)
+def _parking_map(rng, n_map, extent):
     ng = int(n_map * 0.9)
     g = np.stack([rng.uniform(-extent, extent, ng), rng.uniform(-extent, extent, ng),
                   -1.8 + rng.normal(0, 0.01, ng)], axis=1)
@@ -77,12 +75,51 @@ def make_parking(n_map=500_000, n_scan=6_000, seed=43, extent=60.0, max_range=30
     ang = rng.uniform(0, 2 * np.pi, nv)
     v = np.stack([centers[which, 0] + 0.4 * np.cos(ang), centers[which, 1] + 0.4 * np.sin(ang),
                   rng.uniform(-1.8, 1.5, nv)], axis=1)
-    tgt = np.concatenate([g, v], axis=0).astype(np.float32)
+    return np.concatenate([g, v], axis=0).astype(np.float32)
+
+
+def make_parking(n_map=500_000, n_scan=6_000, seed=43, extent=60.0, max_range=30.0):
+    """Ground plane (z = -1.8 + 1 cm noise) with a few pillars/walls; the scan is a range-limited subsample of
+    the map seen from the origin.  Planar degeneracy: x, y, yaw weakly constrained."""
+    rng = np.random.default_rng(seed)
+    tgt = _parking_map(rng, n_map, extent)
     rngs = np.linalg.norm(tgt[:, :2], axis=1)
     cand = np.nonzero(rngs < max_range)[0]
     pick = rng.choice(cand, size=min(n_scan, cand.size), replace=False)
     scan = (tgt[pick].astype(np.float64) + rng.normal(0, 0.005, (pick.size, 3))).astype(np.float32)
     return np.ascontiguousarray(scan), np.ascontiguousarray(tgt)
+
+
+def make_parking_frames(n_frames, seed=47, n_map=500_000, n_scan=6_000, map_seed=43, extent=60.0, max_range=30.0,
+                        path_half_length=20.0):
+    """C3-shaped frames for map-based localisation: one make_parking map (same map_seed -> same map) and n_frames sensor
+    poses along an S-shaped path through it (z = 0, heading along the path).  Frame k keeps every map point within
+    max_range (horizontal) of the sensor with one fixed probability, chosen so that a frame at the path's start has about
+    n_scan points (so the sizes are ragged), adds 5 mm noise and expresses the points in the sensor frame.
+    The initial guesses are the true poses offset by the magnitudes of icp_pk01.yaml:30-44 (0.15 / 0.12 / 0.13 m,
+    0.015 / 1.31 / 2.17 deg) with random signs.  Returns (frames: list of (N_k, 3) float32, T_true (n, 4, 4),
+    T_init (n, 4, 4), map (n_map, 3) float32)."""
+    tgt = _parking_map(np.random.default_rng(map_seed), n_map, extent)
+    rng = np.random.default_rng(seed)
+    s = np.linspace(-1.0, 1.0, n_frames) if n_frames > 1 else np.zeros(1)
+    xs = path_half_length * s
+    ys = 0.25 * path_half_length * np.sin(np.pi * s)
+    heading = np.arctan2(0.25 * path_half_length * np.pi * np.cos(np.pi * s), path_half_length)
+    T_true = np.array([pose6d_to_matrix(xs[k], ys[k], 0.0, 0.0, 0.0, heading[k]) for k in range(n_frames)])
+    near0 = np.count_nonzero(np.hypot(tgt[:, 0] - xs[0], tgt[:, 1] - ys[0]) < max_range)
+    keep_p = min(1.0, n_scan / max(near0, 1))
+    frames, T_init = [], []
+    d = math.pi / 180.0
+    mag = np.array([0.15, 0.12, 0.13, 0.015 * d, 1.31 * d, 2.17 * d])
+    for k in range(n_frames):
+        near = np.nonzero(np.hypot(tgt[:, 0] - xs[k], tgt[:, 1] - ys[k]) < max_range)[0]
+        pick = near[rng.random(near.size) < keep_p]
+        pm = tgt[pick].astype(np.float64) + rng.normal(0, 0.005, (pick.size, 3))
+        R, t = T_true[k][:3, :3], T_true[k][:3, 3]
+        frames.append(np.ascontiguousarray(((pm - t) @ R).astype(np.float32)))        # R^T (p - t), row by row
+        off = mag * rng.choice([-1.0, 1.0], 6)
+        T_init.append(T_true[k] @ pose6d_to_matrix(*off))
+    return frames, T_true, np.array(T_init), tgt
 
 
 def trial_poses(n, seed=45, max_trans=1.0, max_rot_deg=3.0):
