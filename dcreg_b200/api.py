@@ -87,7 +87,7 @@ EXPORTS = [
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -124,6 +124,9 @@ def load_library():
                                         C.POINTER(IterLog), ci]
     lib.dcreg_icp_run_scans.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(C.c_float), C.POINTER(i64), ci, dp, dp,
                                         C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(IterLog), ci]
+    lib.dcreg_icp_run_pairs.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(C.c_float), C.POINTER(i64),
+                                        C.POINTER(C.c_float), C.POINTER(i64), ci, C.c_double, dp, dp, C.POINTER(ci),
+                                        C.POINTER(ci), C.POINTER(ci), dp, C.c_double, dp, C.POINTER(IterLog), ci]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -187,6 +190,7 @@ class IcpResult:
     def __init__(self, status, converged, iterations, T, logs, cov=None):
         self.status, self.converged, self.iterations, self.T, self.logs = status, converged, iterations, T, logs
         self.cov = cov
+        self.metrics = None
 
 
 class Context:
@@ -412,6 +416,57 @@ class Context:
                 recs = [logs[b * cap + i] for i in range(nrec)]
             out.append(IcpResult(int(st[b]), bool(conv[b]), int(n_it[b]), T_out[b], recs,
                                  cov[b] if want_cov else None))
+        return out
+
+    def icp_run_pairs(self, params: IcpParams, sources, targets, T_init, cell_size=None, want_log: bool = False,
+                      want_cov: bool = False, metrics_threshold=None):
+        """Pairs of clouds, each source (a list of (N_b, >=3) arrays) against its own target (a list of (M_b, >=3) arrays),
+        side by side, each from its own initial pose (T_init (B, 4, 4)).  cell_size: the targets' grid cell (default
+        params.search_radius).  Needs no set_target / set_source and leaves the context's clouds as they were.  Returns a
+        list of IcpResult, one per pair (logs only when want_log, .cov the post-loop 6x6 covariance when want_cov,
+        .metrics the point_to_point_metrics dict at the pair's final pose when metrics_threshold is given)."""
+        src = [_as_points(s)[:, :3] for s in sources]
+        tgt = [_as_points(t)[:, :3] for t in targets]
+        B = len(src)
+        if len(tgt) != B:
+            raise ValueError(f"icp_run_pairs: {B} sources but {len(tgt)} targets")
+        cell = float(params.search_radius if cell_size is None else cell_size)
+        if B == 0:                                      # BAD_ARG from the library, like every other malformed batch
+            self._check(self.lib.dcreg_icp_run_pairs(self._h, C.byref(params), 0, None, None, None, None, 3, cell, None,
+                                                     None, None, None, None, None, 0.0, None, None, 0))
+        xyz_s = np.ascontiguousarray(np.concatenate(src, axis=0))
+        xyz_t = np.ascontiguousarray(np.concatenate(tgt, axis=0))
+        off_s = np.zeros(B + 1, dtype=np.int64)
+        off_s[1:] = np.cumsum([p.shape[0] for p in src])
+        off_t = np.zeros(B + 1, dtype=np.int64)
+        off_t[1:] = np.cumsum([p.shape[0] for p in tgt])
+        T_init = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
+        if T_init.shape[0] != B:
+            raise ValueError(f"icp_run_pairs: {B} pairs but {T_init.shape[0]} initial poses")
+        T_out = np.empty((B, 4, 4))
+        n_it = (C.c_int * B)(); conv = (C.c_int * B)(); st = (C.c_int * B)()
+        cov = np.empty((B, 6, 6)) if want_cov else None
+        met = np.empty((B, 4)) if metrics_threshold is not None else None
+        cap = int(params.max_iterations) if want_log else 0
+        logs = (IterLog * max(cap * B, 1))() if want_log else None
+        fp = C.POINTER(C.c_float)
+        self._check(self.lib.dcreg_icp_run_pairs(
+            self._h, C.byref(params), B, xyz_s.ctypes.data_as(fp), off_s.ctypes.data_as(C.POINTER(C.c_int64)),
+            xyz_t.ctypes.data_as(fp), off_t.ctypes.data_as(C.POINTER(C.c_int64)), 3, cell, _dptr(T_init), _dptr(T_out),
+            n_it, conv, st, _dptr(cov) if want_cov else None,
+            float(metrics_threshold) if met is not None else 0.0, _dptr(met) if met is not None else None, logs, cap))
+        out = []
+        for b in range(B):
+            recs = []
+            if want_log:
+                nrec = min(n_it[b], cap)
+                if st[b] == NONFINITE_UPDATE and n_it[b] < cap:
+                    nrec = n_it[b] + 1
+                recs = [logs[b * cap + i] for i in range(nrec)]
+            r = IcpResult(int(st[b]), bool(conv[b]), int(n_it[b]), T_out[b], recs, cov[b] if want_cov else None)
+            if met is not None:
+                r.metrics = {"rmse": met[b, 0], "fitness": met[b, 1], "chamfer": met[b, 2], "n_valid": int(met[b, 3])}
+            out.append(r)
         return out
 
     def icp_run_host_planes(self, params: IcpParams, T_init, plane_fn, want_log: bool = True) -> IcpResult:

@@ -80,6 +80,52 @@ __global__ void grid_bounds_kernel(const float4* __restrict__ pts, int n, double
     }
 }
 
+// ---- grid arena: the dense grids of many clouds in one set of buffers (arena_plan.hpp) ----------------------------
+// segment of point i of a concatenation: the largest b with seg[b] <= i
+__device__ __forceinline__ int segment_of(const long long* __restrict__ seg, int nseg, long long i) {
+    int lo = 0, hi = nseg;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (seg[mid] <= i) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// grid_bounds_kernel per segment: grid y = segment b (points [seg[b], seg[b+1])), bounds[6 b ..] as above
+__global__ void grid_bounds_seg_kernel(const float4* __restrict__ pts, const long long* __restrict__ seg, double inv_cell,
+                                       int* __restrict__ bounds) {
+    const int b = blockIdx.y;
+    const long long e = seg[b + 1];
+    int lo[3] = {1 << 30, 1 << 30, 1 << 30}, hi[3] = {-(1 << 30), -(1 << 30), -(1 << 30)};
+    for (long long i = seg[b] + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < e; i += (long long)gridDim.x * blockDim.x) {
+        const float4 p = pts[i];
+        const int c[3] = {cell_coord(p.x, inv_cell), cell_coord(p.y, inv_cell), cell_coord(p.z, inv_cell)};
+        for (int k = 0; k < 3; ++k) { lo[k] = min(lo[k], c[k]); hi[k] = max(hi[k], c[k]); }
+    }
+    for (int k = 0; k < 3; ++k) {
+        for (int off = 16; off > 0; off >>= 1) {
+            lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], off));
+            hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], off));
+        }
+        if ((threadIdx.x & 31) == 0) { atomicMin(&bounds[6 * b + k], lo[k]); atomicMax(&bounds[6 * b + 3 + k], hi[k]); }
+    }
+}
+
+// grid_count_dense_kernel over an arena: the global cell id of a point is its segment's first cell (cell_off) plus its
+// dense index in that segment's own box (grids[b])
+__global__ void grid_count_seg_kernel(const float4* __restrict__ pts, int n, const long long* __restrict__ seg, int nseg,
+                                      const Grid* __restrict__ grids, const int* __restrict__ cell_off,
+                                      int* __restrict__ pt_cell, int* __restrict__ counts) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int b = segment_of(seg, nseg, i);
+    const Grid& g = grids[b];
+    const float4 p = pts[i];
+    const int c = cell_off[b] + dense_index(g, cell_coord(p.x, g.inv_cell), cell_coord(p.y, g.inv_cell), cell_coord(p.z, g.inv_cell));
+    pt_cell[i] = c;
+    atomicAdd(&counts[c], 1);
+}
+
 // cell id of a point: dense linear index (clamped into the box when `clamp`), or hash slot (insert mode)
 __global__ void grid_count_dense_kernel(const float4* __restrict__ pts, int n, Grid g, int* __restrict__ pt_cell,
                                         int* __restrict__ counts) {
@@ -751,11 +797,18 @@ __device__ __forceinline__ float nn1_search(const Grid& g, float qx, float qy, f
 
 // per-block partial sums: [0] sum of distances, [1] sum of squared distances below the threshold, [2] count below it.
 // When T != nullptr the query is fl32(T p) (pcl::transformPointCloud: FP64 math, float32 store), else p itself.
+// seg / grids (many pairs, dcreg_icp_run_pairs): grid y = pair b, whose queries are q[seg[b], seg[b+1]), searched in
+// grids[b], with the pose T[16 b ..] (row-major 4x4); partials [b][gridDim.x][3].  Otherwise one cloud: q[0, n) in g.
 __global__ void nn1_metrics_kernel(const float4* __restrict__ q, long long n, const double* __restrict__ T, Grid g,
-                                   double threshold, double* __restrict__ partials) {
+                                   double threshold, double* __restrict__ partials, const long long* __restrict__ seg = nullptr,
+                                   const Grid* __restrict__ grids = nullptr) {
     __shared__ double sh[3][8];
     double sd = 0.0, ssq = 0.0, cnt = 0.0;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int b = blockIdx.y;
+    long long i0 = 0;
+    if (seg) { i0 = seg[b]; n = seg[b + 1]; if (T) T += 16 * (size_t)b; }
+    if (grids) g = grids[b];
+    for (long long i = i0 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const float4 p = __ldg(&q[i]);
         float x = p.x, y = p.y, z = p.z;
         if (T) {
@@ -780,15 +833,17 @@ __global__ void nn1_metrics_kernel(const float4* __restrict__ q, long long n, co
     if (threadIdx.x < 3) {
         double s = 0.0;
         for (int w = 0; w < (int)(blockDim.x >> 5); ++w) s += sh[threadIdx.x][w];
-        partials[blockIdx.x * 3 + threadIdx.x] = s;
+        partials[((size_t)b * gridDim.x + blockIdx.x) * 3 + threadIdx.x] = s;
     }
 }
 
-// transform + float32 store of a cloud (aligned copy for the backward Chamfer pass)
+// transform + float32 store of a cloud (aligned copy for the backward Chamfer pass).  seg (many pairs): point i of
+// segment b uses the pose T[16 b ..]
 __global__ void transform_points_kernel(const float4* __restrict__ in, long long n, const double* __restrict__ T,
-                                        float4* __restrict__ out) {
+                                        float4* __restrict__ out, const long long* __restrict__ seg = nullptr, int nseg = 0) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    if (seg) T += 16 * (size_t)segment_of(seg, nseg, i);
     const float4 p = in[i];
     const double px = p.x, py = p.y, pz = p.z;
     out[i] = make_float4((float)(T[0] * px + T[1] * py + T[2] * pz + T[3]), (float)(T[4] * px + T[5] * py + T[6] * pz + T[7]),

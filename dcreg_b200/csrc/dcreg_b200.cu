@@ -21,10 +21,13 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+#include <cstddef>
 #include <string>
 #include <vector>
 
 #include "../../include/dcreg_b200.h"
+#include "arena_plan.hpp"
 #include "corr.cuh"
 #include "k1_reduce.cuh"
 #include "k1_stream.cuh"
@@ -192,6 +195,7 @@ struct Iter2Smem {
     int listS[kBlock], listF[kBlock];
     corr::RowRange rowtab[kSearchListMax][9];   // cell rows of the tile's listed searches (cell = radius)
     int nS, nF;
+    corr::Grid grid;                            // this trial's own target grid (Iter2Args::grids)
 };
 
 // Grid = (blocks per trial, trials).  A trial is one registration (one initial pose) of the context's source against
@@ -229,6 +233,9 @@ struct Iter2Args {
     // record slices at the same offsets (sized by the total slot count), and its own lever arm src_radius[b].
     // null: every trial runs the it.n slots of it.src, with record slices [b][it.n] and the one src_radius
     const long long* seg;
+    // many scan/target pairs (dcreg_icp_run_pairs, with seg): trial b searches its own target grid grids[b] (device
+    // memory, rings set) instead of it.grid.  Only the icp_iter2_kernel<., true> instantiation reads it
+    const corr::Grid* grids;
 };
 
 __device__ __forceinline__ void cswap5(unsigned long long& ka, int& pa, unsigned long long& kb, int& pb) {
@@ -285,7 +292,9 @@ __device__ __noinline__ void solver_block(const Iter2Args& a, IcpState* st, Iter
     }
 }
 
-template <bool kUseWd>
+// kGrids: every trial has its own target grid (Iter2Args::grids), copied into shared memory once per block; the other
+// paths keep reading it.grid from the kernel parameters, untouched by the table
+template <bool kUseWd, bool kGrids>
 __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_constant__ Iter2Args a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     Iter2Smem& sm = *reinterpret_cast<Iter2Smem*>(smem_raw);
@@ -303,7 +312,13 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
         return;
     }
     const k1::Pose P = load_pose(st);
-    const corr::Grid& g = A.grid;
+    if constexpr (kGrids) {
+        static_assert(sizeof(corr::Grid) % sizeof(int) == 0 && sizeof(corr::Grid) / sizeof(int) <= kBlock, "grid copy");
+        if (tid < (int)(sizeof(corr::Grid) / sizeof(int)))
+            reinterpret_cast<int*>(&sm.grid)[tid] = reinterpret_cast<const int*>(a.grids + trial)[tid];
+        __syncthreads();
+    }
+    const corr::Grid& g = kGrids ? sm.grid : A.grid;
     const unsigned int epoch0 = peer::load_epoch(a.peer);     // (after pdl_wait: the previous launch has advanced it)
     DCREG_STAMP(0);
     const int tb = (int)blockIdx.x - (solver_path ? 1 : 0), ntb = (int)gridDim.x - (solver_path ? 1 : 0);   // tile block
@@ -592,6 +607,19 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     }
 }
 
+// dynamic shared memory of the loop kernel: the per-trial grid copy (Iter2Smem::grid, the last member) only where the
+// kernel reads it
+constexpr size_t kIter2SmemNoGrid = offsetof(Iter2Smem, grid);
+
+template <bool kUseWd, bool kGrids>
+cudaError_t loop_kernel_attributes(size_t smem) {
+    cudaError_t e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 cudaSharedmemCarveoutMaxShared);
+    return e;
+}
+
 // K2 as its own kernel: baseline methods (their generic single-thread step), hash-grid runs, the host-plane loop and the
 // NCCL fallback of a sharded run.  One warp per trial (blockIdx.x).
 // K2 executes a few thousand warp instructions exactly once per launch, so it stalls on instruction fetch.  Thanks to the programmatic dependent launch it starts while the
@@ -725,10 +753,14 @@ __global__ void pack_source_kernel(const float* __restrict__ in, long long n, in
 // pack_source_kernel does (w = index inside its scan), takes the per-scan max |p| (the lever arm of that scan) and writes
 // the key of the per-scan spatial sort: (scan, target cell of fl32(T_b p)) with the point's index as the value.  A
 // stable sort on that key orders each segment exactly as sort_source_by_cell orders the scan alone: by cell, then index.
+// grids (scan/target pairs, dcreg_icp_run_pairs): scan b's cell is taken in its own target's grid grids[b], and the key
+// is that cell's global id in the grid arena, cell_off[b] + cell (the pairs' cell ranges follow each other in pair
+// order, so the key still sorts by scan first); g and ncells are then unused.
 __global__ void pack_scans_kernel(const float* __restrict__ in, long long n, int stride, const long long* __restrict__ seg,
                                   int n_scans, const double* __restrict__ T, corr::Grid g, long long ncells,
                                   float4* __restrict__ out, float* __restrict__ radius, unsigned long long* __restrict__ keys,
-                                  int* __restrict__ vals) {
+                                  int* __restrict__ vals, const corr::Grid* __restrict__ grids = nullptr,
+                                  const int* __restrict__ cell_off = nullptr) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     int b = -1;
     float r = 0.0f;
@@ -744,7 +776,8 @@ __global__ void pack_scans_kernel(const float* __restrict__ in, long long n, int
         out[i] = p;
         r = sqrtf(x * x + y * y + z * z);
         if (!(r < 3.0e38f)) r = 0.0f;
-        keys[i] = (unsigned long long)b * (unsigned long long)ncells + (unsigned long long)corr::source_cell(g, T + (size_t)b * 16, p);
+        if (grids) keys[i] = (unsigned long long)cell_off[b] + (unsigned long long)corr::source_cell(grids[b], T + (size_t)b * 16, p);
+        else keys[i] = (unsigned long long)b * (unsigned long long)ncells + (unsigned long long)corr::source_cell(g, T + (size_t)b * 16, p);
         vals[i] = (int)i;
     }
     // max |p| per scan: the lanes of a warp that hold points of the same scan reduce together
@@ -892,6 +925,23 @@ struct dcreg_ctx {
     unsigned long long* d_scan_keys = nullptr; int* d_scan_vals = nullptr;                   // [2][scan_cap]: sort in / out
     void* d_scan_sort_tmp = nullptr; size_t scan_sort_tmp_bytes = 0;
     long long* d_scan_seg = nullptr; float* d_scan_radius = nullptr; double* d_scan_cov = nullptr; int scans_cap = 0;
+    // scan/target pairs (dcreg_icp_run_pairs): the pairs' targets and their dense grids in arenas of their own (the
+    // context's target and grid stay as they were), and the grids over the aligned sources of the metrics
+    struct GridArena {
+        float4* pts = nullptr; int* pos_of = nullptr; float4* tmp = nullptr; int* pt_cell = nullptr; long long pts_cap = 0;
+        int* cell_start = nullptr; int* counts = nullptr; int* fill = nullptr; long long cells_cap = 0;
+        corr::Grid* d_grids = nullptr; int* d_cell_off = nullptr; int* d_bounds = nullptr; int segs_cap = 0;
+        void free_all() {
+            void* p[] = {pts, pos_of, tmp, pt_cell, cell_start, counts, fill, d_grids, d_cell_off, d_bounds};
+            for (void* q : p)
+                if (q) cudaFree(q);
+            *this = GridArena{};
+        }
+    };
+    GridArena pair_tgt, pair_aligned;
+    float4* d_pair_tgt = nullptr; long long pair_tgt_cap = 0;                    // targets, packed (w = global index)
+    long long* d_pair_tgt_seg = nullptr; double* d_pair_T = nullptr; int pairs_cap = 0;   // [n + 1] / [n][16] final poses
+    float4* d_pair_aligned = nullptr; long long pair_aligned_cap = 0;            // sources under their final poses
     dcreg_analysis* d_analysis = nullptr;
     float4* d_flush = nullptr; long long flush_n = 0;
 
@@ -1199,9 +1249,12 @@ int dcreg_destroy(dcreg_ctx* ctx) {
                     ctx->grid.pts, ctx->grid.pos_of, ctx->d_planes64, ctx->d_planes32, ctx->d_partials, ctx->d_counter, ctx->d_acc,
                     ctx->d_state, ctx->d_log, ctx->d_small, ctx->d_analysis, ctx->d_flush, ctx->d_nn, ctx->d_plane_cache, ctx->d_fit_state, ctx->d_iter_stats, ctx->d_src_radius, ctx->d_plane_key, ctx->d_k2_scratch,
                     ctx->d_row_flags, ctx->d_row_epoch, ctx->d_warm_state, ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_keys,
-                    ctx->d_scan_vals, ctx->d_scan_sort_tmp, ctx->d_scan_seg, ctx->d_scan_radius, ctx->d_scan_cov};
+                    ctx->d_scan_vals, ctx->d_scan_sort_tmp, ctx->d_scan_seg, ctx->d_scan_radius, ctx->d_scan_cov,
+                    ctx->d_pair_tgt, ctx->d_pair_tgt_seg, ctx->d_pair_T, ctx->d_pair_aligned};
     for (void* p : ptrs)
         if (p) cudaFree(p);
+    ctx->pair_tgt.free_all();
+    ctx->pair_aligned.free_all();
     if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
@@ -1456,7 +1509,105 @@ struct ScanBatch {
     long long total, max_n;     // points over all scans, points of the largest scan
     const long long* seg;       // device [n + 1]: scan b = points [seg[b], seg[b+1])
     const float* radius;        // device [n]: max |p| of each scan
+    // scan/target pairs (dcreg_icp_run_pairs): scan b against its own target grid; null / 0 for scans against the
+    // context's target
+    const corr::Grid* grids = nullptr;      // device [n] (build_grid_arena)
+    const int* cell_off = nullptr;          // device [n + 1]: first global cell of each grid in the arena
+    long long cells = 0;                    // dense cells of all grids
+    double cell_size = 0.0;
 };
+
+// Dense grids of n clouds at once (dcreg_icp_run_pairs): cloud b is d_pts[h_seg[b], h_seg[b+1]) (d_seg: the same offsets
+// on the device), all of them in the arena A (arena_plan.hpp).  One segmented bounds pass and one copy of the n x 6
+// bounds to the host (the only host sync), then one count, one exclusive scan, one scatter and one in-cell rank over all
+// clouds: the number of launches and syncs does not grow with n.  On return A.d_grids[b] is cloud b's grid (rings set,
+// A.pts / A.pos_of shared, cell_start at the cloud's first cell).  Inside every cloud the order of the points is the one
+// build_grid gives that cloud alone (by cell, then by index), and positions and .w (the global index) are shifted by the
+// constant h_seg[b]: the (distance, then index) order of the neighbour search and the equality of position lists are
+// unchanged.  A cloud whose box needs more than corr::kMaxDenseCells cells is rejected (no hash grids here).
+static int build_grid_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_pts, const int64_t* h_seg,
+                            const long long* d_seg, int n, double cell_size, int rings, const char* what,
+                            long long* cells_out) {
+    const long long m = h_seg[n];
+    if (A.segs_cap < n) {
+        void* old[] = {A.d_grids, A.d_cell_off, A.d_bounds};
+        for (void* p : old)
+            if (p) cudaFree(p);
+        A.d_grids = nullptr; A.d_cell_off = nullptr; A.d_bounds = nullptr; A.segs_cap = 0;
+        CK(cudaMalloc(&A.d_grids, (size_t)n * sizeof(corr::Grid)));
+        CK(cudaMalloc(&A.d_cell_off, (size_t)(n + 1) * sizeof(int)));
+        CK(cudaMalloc(&A.d_bounds, (size_t)n * 6 * sizeof(int)));
+        A.segs_cap = n;
+    }
+    if (A.pts_cap < m) {
+        void* old[] = {A.pts, A.pos_of, A.tmp, A.pt_cell};
+        for (void* p : old)
+            if (p) cudaFree(p);
+        A.pts = nullptr; A.pos_of = nullptr; A.tmp = nullptr; A.pt_cell = nullptr; A.pts_cap = 0;
+        CK(cudaMalloc(&A.pts, (size_t)m * sizeof(float4)));
+        CK(cudaMalloc(&A.pos_of, (size_t)m * sizeof(int)));
+        CK(cudaMalloc(&A.tmp, (size_t)m * sizeof(float4)));
+        CK(cudaMalloc(&A.pt_cell, (size_t)m * sizeof(int)));
+        A.pts_cap = m;
+    }
+    int rc = ensure_pinned(ctx, (size_t)n * 6 * sizeof(int));
+    if (rc) return rc;
+    const double inv_cell = 1.0 / cell_size;
+    std::vector<int> hb((size_t)n * 6);
+    long long max_m = 0;
+    for (int b = 0; b < n; ++b) {
+        for (int k = 0; k < 3; ++k) { hb[6 * (size_t)b + k] = 1 << 30; hb[6 * (size_t)b + 3 + k] = -(1 << 30); }
+        max_m = std::max<long long>(max_m, h_seg[b + 1] - h_seg[b]);
+    }
+    CK(cudaMemcpyAsync(A.d_bounds, hb.data(), hb.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    const unsigned bx = (unsigned)std::min<long long>(64, (max_m + 2047) / 2048);      // blocks per cloud
+    corr::grid_bounds_seg_kernel<<<dim3(bx, (unsigned)n), 256, 0, ctx->stream>>>(d_pts, d_seg, inv_cell, A.d_bounds);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(ctx->h_pinned, A.d_bounds, hb.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    memcpy(hb.data(), ctx->h_pinned, hb.size() * sizeof(int));
+    std::vector<arena_plan::Box> boxes;
+    long long cells = 0;
+    const std::string why = arena_plan::plan(n, hb.data(), boxes, &cells, what);
+    if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
+    if (A.cells_cap < cells) {
+        void* old[] = {A.cell_start, A.counts, A.fill};
+        for (void* p : old)
+            if (p) cudaFree(p);
+        A.cell_start = nullptr; A.counts = nullptr; A.fill = nullptr; A.cells_cap = 0;
+        CK(cudaMalloc(&A.cell_start, (size_t)(cells + 1) * sizeof(int)));
+        CK(cudaMalloc(&A.counts, (size_t)(cells + 1) * sizeof(int)));
+        CK(cudaMalloc(&A.fill, (size_t)cells * sizeof(int)));
+        A.cells_cap = cells;
+    }
+    std::vector<corr::Grid> hg((size_t)n);
+    std::vector<int> off((size_t)n + 1);
+    for (int b = 0; b < n; ++b) {
+        const arena_plan::Box& x = boxes[(size_t)b];
+        corr::Grid& g = hg[(size_t)b];
+        g = corr::Grid{};
+        g.pts = A.pts; g.pos_of = A.pos_of; g.n = (int)m; g.dense = 1; g.rings = rings; g.inv_cell = inv_cell;
+        g.ox = x.ox; g.oy = x.oy; g.oz = x.oz; g.nx = x.nx; g.ny = x.ny; g.nz = x.nz;
+        g.cell_start = A.cell_start + x.cell_off;
+        off[(size_t)b] = (int)x.cell_off;
+    }
+    off[(size_t)n] = (int)cells;
+    *cells_out = cells;
+    CK(cudaMemcpyAsync(A.d_grids, hg.data(), hg.size() * sizeof(corr::Grid), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(A.d_cell_off, off.data(), off.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(A.counts, 0, (size_t)(cells + 1) * sizeof(int), ctx->stream));
+    CK(cudaMemsetAsync(A.fill, 0, (size_t)cells * sizeof(int), ctx->stream));
+    const unsigned nb = (unsigned)((m + 255) / 256);
+    corr::grid_count_seg_kernel<<<nb, 256, 0, ctx->stream>>>(d_pts, (int)m, d_seg, n, A.d_grids, A.d_cell_off, A.pt_cell, A.counts);
+    ctx->launches++;
+    if ((rc = device_exclusive_scan(ctx, A.counts, cells + 1, A.cell_start))) return rc;
+    corr::grid_scatter_kernel<<<nb, 256, 0, ctx->stream>>>(d_pts, (int)m, A.pt_cell, A.cell_start, A.fill, A.tmp, 0);
+    corr::grid_rank_cells_kernel<<<nb, 256, 0, ctx->stream>>>(A.tmp, (int)m, A.pt_cell, A.cell_start, nullptr, A.pts, A.pos_of);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    return DCREG_OK;
+}
 
 static int ensure_scans(dcreg_ctx* ctx, int n_scans, long long total) {
     if (ctx->scans_cap < n_scans) {
@@ -1498,11 +1649,14 @@ static int upload_scans_sorted(dcreg_ctx* ctx, const ScanBatch& S, const float4*
     int* vals = ctx->d_scan_vals;
     pack_scans_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_stage, n, S.stride, S.seg, S.n, ctx->d_T_init,
                                                                            ctx->grid, ctx->grid_cells, ctx->d_scan_src,
-                                                                           ctx->d_scan_radius, keys, vals);
+                                                                           ctx->d_scan_radius, keys, vals, S.grids, S.cell_off);
     ctx->launches++;
     CK(cudaGetLastError());
+    // keys below n_scans * cells of the context's grid, or below the arena's cell count (pairs)
+    const unsigned long long key_end = S.grids ? (unsigned long long)S.cells
+                                               : (unsigned long long)S.n * (unsigned long long)ctx->grid_cells;
     int end_bit = 1;
-    while (end_bit < 64 && ((unsigned long long)S.n * (unsigned long long)ctx->grid_cells - 1ull) >> end_bit) ++end_bit;
+    while (end_bit < 64 && (key_end - 1ull) >> end_bit) ++end_bit;
     size_t tmp = 0;
     CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, keys, keys + n, vals, vals + n, (int)n, 0, end_bit, ctx->stream));
     if (ctx->scan_sort_tmp_bytes < tmp) {
@@ -1519,6 +1673,11 @@ static int upload_scans_sorted(dcreg_ctx* ctx, const ScanBatch& S, const float4*
     CK(cudaGetLastError());
     *src_out = ctx->d_scan_sorted;
     return DCREG_OK;
+}
+
+// rings of cells that cover the search radius (exactness of the 5-NN-within-radius rule); valid in [1, 4]
+static int search_rings(double search_radius, double cell_size) {
+    return (int)ceil(search_radius / cell_size - 1e-9);
 }
 
 static double coherent_step_setting() {
@@ -1543,18 +1702,19 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
     LoopPlan& L = *plan;
     L.trials = trials; L.use_wd = prm->use_weight_derivative != 0;
     IterArgs& a = L.a;
-    a.src = src; a.n = scans ? scans->total : ctx->n_src; a.grid = ctx->grid; a.state = ctx->d_state;
+    const bool pairs = scans && scans->grids;          // every trial has its own target grid (no context target needed)
+    a.src = src; a.n = scans ? scans->total : ctx->n_src; a.grid = pairs ? corr::Grid{} : ctx->grid; a.state = ctx->d_state;
     a.counter = ctx->d_counter; a.acc = ctx->d_acc;
     a.planes_out = planes_out; a.prm = *prm;
     {   // rings of cells that cover the search radius (exactness of the 5-NN-within-radius rule)
-        const int rings = (int)ceil(prm->search_radius / ctx->cell_size - 1e-9);
+        const int rings = search_rings(prm->search_radius, pairs ? scans->cell_size : ctx->cell_size);
         if (rings < 1 || rings > 4) {
             ctx->err = "search_radius / target cell_size must be in (0, 4]: rebuild the target index with a larger cell";
             return DCREG_BAD_ARG;
         }
         a.grid.rings = rings;
     }
-    L.fused2 = ctx->grid.dense && !planes_out && a.n <= 0x1fffffffLL && (scans || !getenv("DCREG_FUSED_SEARCH"));
+    L.fused2 = (pairs || ctx->grid.dense) && !planes_out && a.n <= 0x1fffffffLL && (scans || !getenv("DCREG_FUSED_SEARCH"));
     if ((trials > 1 || scans) && !L.fused2) {
         ctx->err = "batched trials need the dense target grid (target bounding box / cell size too large for it)";
         return DCREG_BAD_ARG;
@@ -1615,13 +1775,16 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         b.log = dlog; b.log_cap = log_cap;
         b.src_radius = scans ? scans->radius : ctx->d_src_radius; b.coherent_step = coherent_step_setting();
         b.seg = scans ? scans->seg : nullptr;
+        // (a CUDA graph of the loop freezes this pointer, not the table: the entries are rewritten before every pairs call
+        // and read at every launch, and a regrown table has a new pointer and so a new graph key)
+        b.grids = pairs ? scans->grids : nullptr;
         b.n_active = ctx->d_n_active;
         if (ctx->peer_ok) b.peer = ctx->peer_view;
         if (!ctx->loop_attr_done) {          // per device (= per context), not per process
-            CK(cudaFuncSetAttribute(icp_iter2_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Iter2Smem)));
-            CK(cudaFuncSetAttribute(icp_iter2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Iter2Smem)));
-            CK(cudaFuncSetAttribute(icp_iter2_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-            CK(cudaFuncSetAttribute(icp_iter2_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+            CK((loop_kernel_attributes<true, false>)(kIter2SmemNoGrid));
+            CK((loop_kernel_attributes<false, false>)(kIter2SmemNoGrid));
+            CK((loop_kernel_attributes<true, true>)(sizeof(Iter2Smem)));
+            CK((loop_kernel_attributes<false, true>)(sizeof(Iter2Smem)));
             ctx->loop_attr_done = true;
         }
     } else {
@@ -1640,8 +1803,13 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
         L.b.use_seeds = ctx->nn_valid ? 1 : 0;
         ctx->nn_valid = true;
         const dim3 grid((unsigned)L.grid_x, (unsigned)L.trials);
-        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+        if (L.b.grids) {
+            if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+            else CK(launch_pdl(icp_iter2_kernel<false, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+        } else {
+            if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+            else CK(launch_pdl(icp_iter2_kernel<false, false>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+        }
     } else {
         if (L.use_wd) icp_iteration_kernel<true><<<L.grid_x, kBlock, 0, ctx->stream>>>(L.a);
         else icp_iteration_kernel<false><<<L.grid_x, kBlock, 0, ctx->stream>>>(L.a);
@@ -2047,10 +2215,11 @@ static int run_loop(dcreg_ctx* ctx, const dcreg_icp_params* params, int trials, 
     return read_results(ctx, trials, T_out, log, log_cap, n_iterations, converged, status);
 }
 
-// need_source = false: the run brings its own source points (dcreg_icp_run_scans)
-static int check_run_args(dcreg_ctx* ctx, const dcreg_icp_params* params, bool need_source = true) {
+// need_source = false: the run brings its own source points (dcreg_icp_run_scans); need_target = false: and its own
+// targets (dcreg_icp_run_pairs)
+static int check_run_args(dcreg_ctx* ctx, const dcreg_icp_params* params, bool need_source = true, bool need_target = true) {
     if (need_source && (!ctx->d_src || ctx->n_src <= 0)) { ctx->err = "[ICP Error] Input measure cloud is null or empty."; return DCREG_BAD_ARG; }
-    if (!ctx->has_grid) { ctx->err = "[ICP Error] Target index is not set up in context."; return DCREG_BAD_ARG; }
+    if (need_target && !ctx->has_grid) { ctx->err = "[ICP Error] Target index is not set up in context."; return DCREG_BAD_ARG; }
     if (params->max_iterations < 0) { ctx->err = "icp_run: max_iterations < 0"; return DCREG_BAD_ARG; }
     if (!(params->weight_slope > 0.0) || !(params->weight_gate >= 0.0) || !(params->weight_gate < 1.0)) {
         ctx->err = "icp_run: weight_slope must be > 0 and weight_gate in [0, 1)";
@@ -2141,6 +2310,143 @@ int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_sc
         CK(cudaMemcpyAsync(cov, ctx->d_scan_cov, (size_t)n_scans * 36 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
     }
+    return DCREG_OK;
+}
+
+// the pairs' own device buffers (dcreg_icp_run_pairs): packed targets, target offsets, final poses
+static int ensure_pairs(dcreg_ctx* ctx, int n_pairs, long long n_tgt) {
+    if (ctx->pairs_cap < n_pairs) {
+        if (ctx->d_pair_tgt_seg) cudaFree(ctx->d_pair_tgt_seg);
+        if (ctx->d_pair_T) cudaFree(ctx->d_pair_T);
+        ctx->d_pair_tgt_seg = nullptr; ctx->d_pair_T = nullptr; ctx->pairs_cap = 0;
+        CK(cudaMalloc(&ctx->d_pair_tgt_seg, (size_t)(n_pairs + 1) * sizeof(long long)));
+        CK(cudaMalloc(&ctx->d_pair_T, (size_t)n_pairs * 16 * sizeof(double)));
+        ctx->pairs_cap = n_pairs;
+    }
+    if (ctx->pair_tgt_cap < n_tgt) {
+        if (ctx->d_pair_tgt) cudaFree(ctx->d_pair_tgt);
+        ctx->d_pair_tgt = nullptr; ctx->pair_tgt_cap = 0;
+        CK(cudaMalloc(&ctx->d_pair_tgt, (size_t)n_tgt * sizeof(float4)));
+        ctx->pair_tgt_cap = n_tgt;
+    }
+    return DCREG_OK;
+}
+
+// dcreg_point_to_point_metrics of every pair at its final pose T_out[b]: forward 1-NN of the aligned source in its
+// target's grid, grids over the aligned sources (build_grid_arena, same cell size), backward 1-NN of every target in
+// its own aligned source's grid.  The per-pair partial sums are added in a fixed block order, so a call reproduces bit
+// for bit; against the single call only the grouping of the FP64 sums differs.  out: [n][4] = rmse, fitness, chamfer,
+// n_valid.
+static int pairs_metrics(dcreg_ctx* ctx, const ScanBatch& S, const int64_t* src_off, const int64_t* tgt_off,
+                         const double* T_out, double threshold, double* out) {
+    const int n = S.n;
+    const long long ns = S.total, nt = tgt_off[n];
+    long long max_t = 0;
+    for (int b = 0; b < n; ++b) max_t = std::max<long long>(max_t, tgt_off[b + 1] - tgt_off[b]);
+    // blocks per pair: what the largest cloud needs, at most about 8 per SM over the whole call
+    auto blocks = [&](long long mx) {
+        const long long cap = std::max<long long>(1, (long long)ctx->sm_count * 8 / n);
+        return (int)std::max<long long>(1, std::min<long long>((mx + kBlock - 1) / kBlock, cap));
+    };
+    const int gf = blocks(S.max_n), gb = blocks(max_t);
+    int rc = ensure_partials(ctx, n * (gf + gb));             // 3 doubles per block and pair, forward then backward
+    if (rc) return rc;
+    if (ctx->pair_aligned_cap < ns) {
+        if (ctx->d_pair_aligned) cudaFree(ctx->d_pair_aligned);
+        ctx->d_pair_aligned = nullptr; ctx->pair_aligned_cap = 0;
+        CK(cudaMalloc(&ctx->d_pair_aligned, (size_t)ns * sizeof(float4)));
+        ctx->pair_aligned_cap = ns;
+    }
+    CK(cudaMemcpyAsync(ctx->d_pair_T, T_out, (size_t)n * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    double* fwd = ctx->d_partials;
+    double* bwd = ctx->d_partials + (size_t)3 * n * gf;
+    corr::nn1_metrics_kernel<<<dim3((unsigned)gf, (unsigned)n), kBlock, 0, ctx->stream>>>(ctx->d_scan_src, ns, ctx->d_pair_T, corr::Grid{},
+                                                                                        threshold, fwd, S.seg, S.grids);
+    corr::transform_points_kernel<<<(unsigned)((ns + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_scan_src, ns, ctx->d_pair_T,
+                                                                                        ctx->d_pair_aligned, S.seg, n);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    long long cells = 0;
+    if ((rc = build_grid_arena(ctx, ctx->pair_aligned, ctx->d_pair_aligned, src_off, S.seg, n, S.cell_size, 1,
+                               "p2p metrics: the aligned source of pair", &cells)))
+        return rc;
+    corr::nn1_metrics_kernel<<<dim3((unsigned)gb, (unsigned)n), kBlock, 0, ctx->stream>>>(ctx->d_pair_tgt, nt, nullptr, corr::Grid{},
+                                                                                        threshold, bwd, ctx->d_pair_tgt_seg,
+                                                                                        ctx->pair_aligned.d_grids);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    std::vector<double> hp((size_t)3 * n * (gf + gb));
+    CK(cudaMemcpyAsync(hp.data(), ctx->d_partials, hp.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    const double* hf = hp.data();
+    const double* hb = hp.data() + (size_t)3 * n * gf;
+    for (int b = 0; b < n; ++b) {
+        double sum_fwd = 0, sum_sq = 0, valid = 0, sum_bwd = 0;
+        for (int k = 0; k < gf; ++k) {
+            const double* p = hf + 3 * ((size_t)b * gf + k);
+            sum_fwd += p[0]; sum_sq += p[1]; valid += p[2];
+        }
+        for (int k = 0; k < gb; ++k) sum_bwd += hb[3 * ((size_t)b * gb + k)];
+        const double ns_b = (double)(src_off[b + 1] - src_off[b]), nt_b = (double)(tgt_off[b + 1] - tgt_off[b]);
+        double* o = out + 4 * (size_t)b;
+        o[0] = sqrt(sum_sq / ns_b);
+        o[1] = valid / ns_b;
+        o[2] = 0.5 * (sum_fwd / ns_b + sum_bwd / nt_b);
+        o[3] = valid;
+    }
+    return DCREG_OK;
+}
+
+int dcreg_icp_run_pairs(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_pairs, const float* src_xyz,
+                        const int64_t* src_offsets, const float* tgt_xyz, const int64_t* tgt_offsets, int stride,
+                        double cell_size, const double* T_init, double* T_out, int* n_iterations, int* converged,
+                        int* status, double* cov, double error_threshold, double* metrics, dcreg_iter_log* log,
+                        int log_cap) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!params || n_pairs <= 0 || !src_xyz || !src_offsets || !tgt_xyz || !tgt_offsets || !T_init || !T_out) {
+        ctx->err = "icp_run_pairs: null pointer or n_pairs <= 0";
+        return DCREG_BAD_ARG;
+    }
+    if (n_pairs > arena_plan::kMaxPairs) {
+        ctx->err = "icp_run_pairs: more than " + std::to_string(arena_plan::kMaxPairs) + " pairs in one call";
+        return DCREG_BAD_ARG;
+    }
+    if (stride < 3) { ctx->err = "icp_run_pairs: stride < 3"; return DCREG_BAD_ARG; }
+    if (!(cell_size > 0.0)) { ctx->err = "icp_run_pairs: cell_size <= 0"; return DCREG_BAD_ARG; }
+    if (ctx->comm) { ctx->err = "icp_run_pairs: pairs are independent - give each rank its own, do not shard them"; return DCREG_BAD_ARG; }
+    int rc = check_run_args(ctx, params, false, false);
+    if (rc) return rc;
+    const int rings = search_rings(params->search_radius, cell_size);
+    if (rings < 1 || rings > 4) { ctx->err = "icp_run_pairs: search_radius / cell_size must be in (0, 4]"; return DCREG_BAD_ARG; }
+    std::string why = arena_plan::check_offsets(n_pairs, src_offsets, arena_plan::kMaxPoints, "icp_run_pairs: source");
+    if (why.empty()) why = arena_plan::check_offsets(n_pairs, tgt_offsets, arena_plan::kMaxPoints, "icp_run_pairs: target");
+    if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
+    long long max_n = 0;
+    for (int b = 0; b < n_pairs; ++b) max_n = std::max<long long>(max_n, src_offsets[b + 1] - src_offsets[b]);
+    const long long n_src = src_offsets[n_pairs], n_tgt = tgt_offsets[n_pairs];
+    CK(cudaSetDevice(ctx->device));
+    if ((rc = ensure_scans(ctx, n_pairs, n_src)) || (rc = ensure_pairs(ctx, n_pairs, n_tgt))) return rc;
+    CK(cudaMemcpyAsync(ctx->d_scan_seg, src_offsets, (size_t)(n_pairs + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_pair_tgt_seg, tgt_offsets, (size_t)(n_pairs + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+    // the targets: packed with w = index over all targets, then every pair's dense grid in the arena
+    if ((rc = upload_points(ctx, tgt_xyz, n_tgt, stride, ctx->d_pair_tgt, nullptr))) return rc;
+    long long cells = 0;
+    if ((rc = build_grid_arena(ctx, ctx->pair_tgt, ctx->d_pair_tgt, tgt_offsets, ctx->d_pair_tgt_seg, n_pairs, cell_size,
+                               rings, "icp_run_pairs: target", &cells)))
+        return rc;
+    ScanBatch S{n_pairs, src_xyz, stride, n_src, max_n, ctx->d_scan_seg, ctx->d_scan_radius};
+    S.grids = ctx->pair_tgt.d_grids; S.cell_off = ctx->pair_tgt.d_cell_off; S.cells = cells; S.cell_size = cell_size;
+    std::vector<int> st_local;
+    if (!status) { st_local.resize(n_pairs); status = st_local.data(); }
+    if ((rc = run_loop(ctx, params, n_pairs, T_init, T_out, log, log_cap, n_iterations, converged, status, true, &S))) return rc;
+    if (cov) {                                                  // covariance_kernel's rule per pair
+        covariance_kernel<<<n_pairs, 32, 0, ctx->stream>>>(ctx->d_state, ctx->d_scan_cov);
+        ctx->launches++;
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(cov, ctx->d_scan_cov, (size_t)n_pairs * 36 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    if (metrics) return pairs_metrics(ctx, S, src_offsets, tgt_offsets, T_out, error_threshold, metrics);
     return DCREG_OK;
 }
 

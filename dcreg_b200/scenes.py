@@ -3,6 +3,7 @@
 C2  make_cylinder : the shipped cylinder's geometry (wall R = 40 m, z in [0, 20] + floor disc z = 0) at any size
 C3  make_parking  : ground-dominated local map + sparse verticals, LiDAR-like frame (stand-in, pair not shipped)
     make_parking_frames : the same map and a sequence of frames along a path through it (batched localisation)
+    make_parking_pairs  : frame k+1 of that path against the local submap around pose k (scan/target pairs)
 C4  make_corridor : two parallel walls + floor + ceiling, rank-deficient along x
 C5  trial_poses   : seeded perturbations t ~ U[-1, 1]^3 m, rpy ~ U[-3, 3]^3 deg for the Monte-Carlo (SURVEY.md §8d)
     load_pcd_xyz  : PCD v0.7 `DATA binary` with float32 fields (the shipped clouds, SURVEY.md Appendix B.3)
@@ -120,6 +121,32 @@ def make_parking_frames(n_frames, seed=47, n_map=500_000, n_scan=6_000, map_seed
         off = mag * rng.choice([-1.0, 1.0], 6)
         T_init.append(T_true[k] @ pose6d_to_matrix(*off))
     return frames, T_true, np.array(T_init), tgt
+
+
+def make_parking_pairs(n_pairs, seed=53, n_map=500_000, n_scan=6_000, map_seed=43, extent=60.0, max_range=30.0,
+                       path_half_length=20.0):
+    """Scan-to-submap pairs (odometry along a recorded sequence, loop-closure checks): the n_pairs + 1 sensor poses and
+    frames of make_parking_frames(n_pairs + 1, seed, ...).  Pair k registers frame k + 1 (in its own sensor frame)
+    against the local submap around pose k: every map point within max_range (horizontal) of sensor k, plus 5 mm noise,
+    in sensor frame k (about 100 k points at the defaults, ragged from pair to pair).  T_true[k] = inv(T_k) T_{k+1} maps
+    the source onto its target; T_init[k] = T_true[k] times the icp_pk01.yaml offsets with random signs, as in
+    make_parking_frames.  Returns (sources: list of (N_k, 3) float32, targets: list of (M_k, 3) float32,
+    T_true (n, 4, 4), T_init (n, 4, 4))."""
+    frames, T_world, _, tgt = make_parking_frames(n_pairs + 1, seed=seed, n_map=n_map, n_scan=n_scan, map_seed=map_seed,
+                                                  extent=extent, max_range=max_range, path_half_length=path_half_length)
+    rng = np.random.default_rng([seed, 1])
+    d = math.pi / 180.0
+    mag = np.array([0.15, 0.12, 0.13, 0.015 * d, 1.31 * d, 2.17 * d])
+    targets, T_true, T_init = [], [], []
+    for k in range(n_pairs):
+        R, t = T_world[k][:3, :3], T_world[k][:3, 3]
+        near = np.nonzero(np.hypot(tgt[:, 0] - t[0], tgt[:, 1] - t[1]) < max_range)[0]
+        pm = tgt[near].astype(np.float64) + rng.normal(0, 0.005, (near.size, 3))
+        targets.append(np.ascontiguousarray(((pm - t) @ R).astype(np.float32)))
+        Tk = np.linalg.inv(T_world[k]) @ T_world[k + 1]
+        T_true.append(Tk)
+        T_init.append(Tk @ pose6d_to_matrix(*(mag * rng.choice([-1.0, 1.0], 6))))
+    return frames[1:], targets, np.array(T_true), np.array(T_init)
 
 
 def trial_poses(n, seed=45, max_trans=1.0, max_rot_deg=3.0):

@@ -236,6 +236,23 @@ int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_sc
                         const int64_t* scan_offsets, int stride, const double* T_init, double* T_out,
                         int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
                         int log_cap);
+/* Many scan/target pairs, EACH SOURCE AGAINST ITS OWN TARGET (scan-to-submap odometry, loop-closure candidates), side by
+ * side in one sequence of launches, with one set of parameters.  src_xyz / tgt_xyz: HOST memory, concatenated, `stride`
+ * floats per point; pair b is source points [src_offsets[b], src_offsets[b+1]) against target points
+ * [tgt_offsets[b], tgt_offsets[b+1]) (n_pairs + 1 entries each, ascending strictly from 0: no empty source or target;
+ * at most 2^29 - 1 points per side, at most 65535 pairs).  cell_size: as in dcreg_set_target (search_radius / cell_size
+ * in (0, 4]); every target needs a dense grid (at most 2^27 cells in its bounding box, 2^30 over the call).
+ * T_init / T_out / n_iterations / converged / status / cov / log: as in dcreg_icp_run_scans, one per pair.
+ * metrics: n_pairs x 4 doubles or NULL; pair b's dcreg_point_to_point_metrics(T_out[b], error_threshold) = rmse, fitness,
+ * chamfer, n_valid (an aligned source too large for a dense grid: DCREG_BAD_ARG after the poses are written).
+ * Pair b gives what dcreg_set_target(tgt_b, cell_size) + dcreg_set_source(src_b) + dcreg_icp_run(T_init[b]) gives up to
+ * the grouping of the FP64 partial sums; a call reproduces bit for bit.  Needs no dcreg_set_target / dcreg_set_source
+ * beforehand and leaves the context's source, target and grid as they were.  Not available on a sharded context. */
+int dcreg_icp_run_pairs(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_pairs, const float* src_xyz,
+                        const int64_t* src_offsets, const float* tgt_xyz, const int64_t* tgt_offsets, int stride,
+                        double cell_size, const double* T_init, double* T_out, int* n_iterations, int* converged,
+                        int* status, double* cov, double error_threshold, double* metrics, dcreg_iter_log* log,
+                        int log_cap);
 /* Same loop, but correspondences are supplied by the caller each iteration through a callback
  * (host kd-tree mode, "PR1"): planes are 4*n doubles (nx,ny,nz,d), all-zero = none. */
 typedef int (*dcreg_plane_callback)(void* user, const double T[16], double* planes4,
