@@ -1,10 +1,10 @@
-// arena_plan.hpp - host-side planning of a grid arena: the dense target grids of many scan/target pairs
-// (dcreg_icp_run_pairs) built side by side in one set of buffers.
+// arena_plan.hpp - host-side planning of a grid arena: the dense grids of one or many clouds built side by side in one
+// set of buffers (the context's target, the targets of dcreg_icp_run_pairs, the aligned sources of the metrics).
 //
-// Pair b's points get one global cell numbering: its cells are [cell_off[b], cell_off[b] + cells[b]), in the x-fastest
-// dense order of its own bounding box, and the pairs follow each other.  One count / scan / scatter / rank over all
-// points then groups every pair's points exactly as a build of that pair alone would (by cell, then by index), only
-// shifted by the points of the pairs before it.  Everything here is plain C++ so tests/test_arena_plan.py can check it
+// Cloud b's points get one global cell numbering: its cells are [cell_off[b], cell_off[b] + cells[b]), in the x-fastest
+// dense order of its own bounding box, and the clouds follow each other.  One count / scan / scatter / rank over all
+// points then groups every cloud's points exactly as a build of that cloud alone would (by cell, then by index), only
+// shifted by the points of the clouds before it.  Everything here is plain C++ so tests/test_arena_plan.py can check it
 // on the CPU (tools/test_arena_plan.cpp).
 #pragma once
 #include <cstdint>
@@ -13,7 +13,7 @@
 
 namespace arena_plan {
 
-constexpr long long kMaxDenseCells = 1ll << 27;      // per grid: corr::kMaxDenseCells
+constexpr long long kMaxDenseCells = 1ll << 27;      // per dense grid (above it the context's target uses a hash table)
 constexpr int kCoordLimit = 1 << 19;                 // cell coordinates outside +-2^19: NaN / huge coordinates
 constexpr long long kMaxCells = 1ll << 30;           // all grids of a call: cell ids and cell_start entries are int32
 constexpr long long kMaxPoints = 0x1fffffffLL;       // points per side and call: int32 positions, the loop kernel's 2^29
@@ -38,25 +38,40 @@ inline std::string check_offsets(int n, const int64_t* off, long long max_total,
     return std::string();
 }
 
-// bounds: n x 6 ints, per segment the min cell coordinates (x, y, z) then the max.  Fills boxes[n] and *total_cells.
+enum Fit { kDense, kTooManyCells, kOutOfRange };
+
+// The box of one cloud from its bounds hb[6] (min cell coordinates x, y, z, then the max): kOutOfRange when a
+// coordinate lies outside the +-2^19 cell range, else *x (cell_off 0) and kDense when it has at most kMaxDenseCells
+// cells, kTooManyCells when it has more.
+inline Fit box_of(const int* hb, Box* x) {
+    for (int k = 0; k < 3; ++k)
+        if (hb[k] < -kCoordLimit || hb[3 + k] > kCoordLimit || hb[k] > hb[3 + k]) return kOutOfRange;
+    const long long nx = (long long)hb[3] - hb[0] + 1, ny = (long long)hb[4] - hb[1] + 1, nz = (long long)hb[5] - hb[2] + 1;
+    x->cells = nx * ny * nz;
+    x->cell_off = 0;
+    if (x->cells > kMaxDenseCells) return kTooManyCells;
+    x->ox = hb[0]; x->oy = hb[1]; x->oz = hb[2];
+    x->nx = (int)nx; x->ny = (int)ny; x->nz = (int)nz;
+    return kDense;
+}
+
+inline std::string out_of_range(const char* what) {
+    return std::string(what) + ": coordinates / cell_size exceed the +-2^19 cell range (NaN or huge coordinates?)";
+}
+
+// bounds: n x 6 ints, per segment as box_of reads them.  Fills boxes[n] and *total_cells.
 // Returns an empty string when every segment gets a dense grid, else the reason (naming the segment).
 inline std::string plan(int n, const int* bounds, std::vector<Box>& boxes, long long* total_cells, const char* what) {
     boxes.assign((size_t)n, Box{});
     long long off = 0;
     for (int b = 0; b < n; ++b) {
-        const int* hb = bounds + 6 * (size_t)b;
-        for (int k = 0; k < 3; ++k)
-            if (hb[k] < -kCoordLimit || hb[3 + k] > kCoordLimit || hb[k] > hb[3 + k])
-                return std::string(what) + " " + std::to_string(b) +
-                       ": coordinates / cell_size exceed the +-2^19 cell range (NaN or huge coordinates?)";
         Box& x = boxes[(size_t)b];
-        const long long nx = (long long)hb[3] - hb[0] + 1, ny = (long long)hb[4] - hb[1] + 1, nz = (long long)hb[5] - hb[2] + 1;
-        x.cells = nx * ny * nz;
-        if (x.cells > kMaxDenseCells)
-            return std::string(what) + " " + std::to_string(b) + ": bounding box of " + std::to_string(x.cells) +
-                   " cells is too large for a dense grid at this cell size (pairs use dense grids only)";
-        x.ox = hb[0]; x.oy = hb[1]; x.oz = hb[2];
-        x.nx = (int)nx; x.ny = (int)ny; x.nz = (int)nz;
+        const std::string seg = std::string(what) + " " + std::to_string(b);
+        const Fit fit = box_of(bounds + 6 * (size_t)b, &x);
+        if (fit == kOutOfRange) return out_of_range(seg.c_str());
+        if (fit == kTooManyCells)
+            return seg + ": bounding box of " + std::to_string(x.cells) +
+                   " cells is too large for a dense grid at this cell size (only the context's target falls back to a hash table)";
         x.cell_off = off;
         off += x.cells;
         if (off > kMaxCells)

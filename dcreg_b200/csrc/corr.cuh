@@ -15,7 +15,7 @@
 //   dense mode : cells of the target's bounding box in x-fastest linear order + cell_start[ncells + 1];
 //                the 3 x-adjacent cells of a row are ONE contiguous point range, so a query scans 9 ranges.
 //   hash mode  : open-addressing table keyed by the packed cell coordinates (fallback when the bounding box
-//                has more than kMaxDenseCells cells); a query probes 27 cells.
+//                has more than arena_plan::kMaxDenseCells cells); a query probes 27 cells.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -24,7 +24,6 @@
 namespace corr {
 
 constexpr unsigned long long kEmptyKey = ~0ull;
-constexpr long long kMaxDenseCells = 1ll << 27;
 
 struct Grid {
     float4* pts;                // n target points grouped by cell
@@ -62,25 +61,7 @@ __device__ __forceinline__ int dense_index(const Grid& g, int cx, int cy, int cz
     return ((cz - g.oz) * g.ny + (cy - g.oy)) * g.nx + (cx - g.ox);
 }
 
-// ---- build -----------------------------------------------------------------------------------
-// bounds[0..2] = min cell coords, bounds[3..5] = max cell coords (initialised to +-2^30 by the host)
-__global__ void grid_bounds_kernel(const float4* __restrict__ pts, int n, double inv_cell, int* __restrict__ bounds) {
-    int lo[3] = {1 << 30, 1 << 30, 1 << 30}, hi[3] = {-(1 << 30), -(1 << 30), -(1 << 30)};
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const float4 p = pts[i];
-        const int c[3] = {cell_coord(p.x, inv_cell), cell_coord(p.y, inv_cell), cell_coord(p.z, inv_cell)};
-        for (int k = 0; k < 3; ++k) { lo[k] = min(lo[k], c[k]); hi[k] = max(hi[k], c[k]); }
-    }
-    for (int k = 0; k < 3; ++k) {
-        for (int off = 16; off > 0; off >>= 1) {
-            lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], off));
-            hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], off));
-        }
-        if ((threadIdx.x & 31) == 0) { atomicMin(&bounds[k], lo[k]); atomicMax(&bounds[3 + k], hi[k]); }
-    }
-}
-
-// ---- grid arena: the dense grids of many clouds in one set of buffers (arena_plan.hpp) ----------------------------
+// ---- build: the dense grids of one or many clouds in one set of buffers (arena_plan.hpp) --------------------------
 // segment of point i of a concatenation: the largest b with seg[b] <= i
 __device__ __forceinline__ int segment_of(const long long* __restrict__ seg, int nseg, long long i) {
     int lo = 0, hi = nseg;
@@ -91,7 +72,8 @@ __device__ __forceinline__ int segment_of(const long long* __restrict__ seg, int
     return lo;
 }
 
-// grid_bounds_kernel per segment: grid y = segment b (points [seg[b], seg[b+1])), bounds[6 b ..] as above
+// cell bounds per segment: grid y = segment b (points [seg[b], seg[b+1])); bounds[6 b ..] = min cell coords (x, y, z),
+// then max cell coords (initialised to +-2^30 by the host)
 __global__ void grid_bounds_seg_kernel(const float4* __restrict__ pts, const long long* __restrict__ seg, double inv_cell,
                                        int* __restrict__ bounds) {
     const int b = blockIdx.y;
@@ -111,8 +93,8 @@ __global__ void grid_bounds_seg_kernel(const float4* __restrict__ pts, const lon
     }
 }
 
-// grid_count_dense_kernel over an arena: the global cell id of a point is its segment's first cell (cell_off) plus its
-// dense index in that segment's own box (grids[b])
+// cell id of a point and the per-cell counts: the global cell id is the point's segment's first cell (cell_off) plus
+// its dense linear index in that segment's own box (grids[b])
 __global__ void grid_count_seg_kernel(const float4* __restrict__ pts, int n, const long long* __restrict__ seg, int nseg,
                                       const Grid* __restrict__ grids, const int* __restrict__ cell_off,
                                       int* __restrict__ pt_cell, int* __restrict__ counts) {
@@ -126,17 +108,7 @@ __global__ void grid_count_seg_kernel(const float4* __restrict__ pts, int n, con
     atomicAdd(&counts[c], 1);
 }
 
-// cell id of a point: dense linear index (clamped into the box when `clamp`), or hash slot (insert mode)
-__global__ void grid_count_dense_kernel(const float4* __restrict__ pts, int n, Grid g, int* __restrict__ pt_cell,
-                                        int* __restrict__ counts) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float4 p = pts[i];
-    const int c = dense_index(g, cell_coord(p.x, g.inv_cell), cell_coord(p.y, g.inv_cell), cell_coord(p.z, g.inv_cell));
-    pt_cell[i] = c;
-    atomicAdd(&counts[c], 1);
-}
-
+// hash slot of a point (inserting its cell's key) and the per-slot counts
 __global__ void grid_insert_hash_kernel(const float4* __restrict__ pts, int n, Grid g, int* __restrict__ pt_slot) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -796,19 +768,19 @@ __device__ __forceinline__ float nn1_search(const Grid& g, float qx, float qy, f
 }
 
 // per-block partial sums: [0] sum of distances, [1] sum of squared distances below the threshold, [2] count below it.
-// When T != nullptr the query is fl32(T p) (pcl::transformPointCloud: FP64 math, float32 store), else p itself.
-// seg / grids (many pairs, dcreg_icp_run_pairs): grid y = pair b, whose queries are q[seg[b], seg[b+1]), searched in
-// grids[b], with the pose T[16 b ..] (row-major 4x4); partials [b][gridDim.x][3].  Otherwise one cloud: q[0, n) in g.
-__global__ void nn1_metrics_kernel(const float4* __restrict__ q, long long n, const double* __restrict__ T, Grid g,
-                                   double threshold, double* __restrict__ partials, const long long* __restrict__ seg = nullptr,
-                                   const Grid* __restrict__ grids = nullptr) {
+// Grid y = pair b, whose queries are q[seg[b], seg[b+1]), searched in grids[b]; partials [b][gridDim.x][3].  When
+// T != nullptr the query is fl32(T_b p) with the pose T_b = T[16 b ..] (row-major 4x4; pcl::transformPointCloud: FP64
+// math, float32 store), else p itself.
+__global__ void nn1_metrics_kernel(const float4* __restrict__ q, const long long* __restrict__ seg,
+                                   const Grid* __restrict__ grids, const double* __restrict__ T, double threshold,
+                                   double* __restrict__ partials) {
     __shared__ double sh[3][8];
     double sd = 0.0, ssq = 0.0, cnt = 0.0;
     const int b = blockIdx.y;
-    long long i0 = 0;
-    if (seg) { i0 = seg[b]; n = seg[b + 1]; if (T) T += 16 * (size_t)b; }
-    if (grids) g = grids[b];
-    for (long long i = i0 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const long long n = seg[b + 1];
+    const Grid& g = grids[b];
+    if (T) T += 16 * (size_t)b;
+    for (long long i = seg[b] + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
         const float4 p = __ldg(&q[i]);
         float x = p.x, y = p.y, z = p.z;
         if (T) {
@@ -837,13 +809,13 @@ __global__ void nn1_metrics_kernel(const float4* __restrict__ q, long long n, co
     }
 }
 
-// transform + float32 store of a cloud (aligned copy for the backward Chamfer pass).  seg (many pairs): point i of
-// segment b uses the pose T[16 b ..]
+// transform + float32 store of clouds (aligned copies for the backward Chamfer pass): point i of segment b uses the
+// pose T[16 b ..]
 __global__ void transform_points_kernel(const float4* __restrict__ in, long long n, const double* __restrict__ T,
-                                        float4* __restrict__ out, const long long* __restrict__ seg = nullptr, int nseg = 0) {
+                                        float4* __restrict__ out, const long long* __restrict__ seg, int nseg) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    if (seg) T += 16 * (size_t)segment_of(seg, nseg, i);
+    T += 16 * (size_t)segment_of(seg, nseg, i);
     const float4 p = in[i];
     const double px = p.x, py = p.y, pz = p.z;
     out[i] = make_float4((float)(T[0] * px + T[1] * py + T[2] * pz + T[3]), (float)(T[4] * px + T[5] * py + T[6] * pz + T[7]),

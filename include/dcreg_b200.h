@@ -148,8 +148,9 @@ void* dcreg_stream(dcreg_ctx* ctx);
  * Point2PlaneICP_SO3_OpenMP (icp_test_runner.h:92-102). */
 int dcreg_set_source(dcreg_ctx* ctx, const float* xyz, int64_t n, int stride);
 /* Target cloud + its spatial index.  Replaces ICPContext::setTargetCloud's kd-tree build
- * (utils.hpp:393-424): a device hash grid with cell = `cell_size` (pass the search radius;
- * exact 5-NN-within-radius then only needs the 27 surrounding cells). */
+ * (utils.hpp:393-424): a device dense grid with cell = `cell_size` (pass the search radius;
+ * exact 5-NN-within-radius then only needs the 27 surrounding cells), with a hash-table fallback when the bounding box
+ * has more than 2^27 cells. */
 int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size);
 
 /* ---- seam 1: correspondence stage (icp_test_runner.cpp:1714-1813) -------------------------

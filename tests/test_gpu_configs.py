@@ -333,9 +333,11 @@ def test_host_planes_fitness_uses_the_callers_count(ctx, golden, cylinder):
 # ------------------------------------------------------------------------------------------------
 def test_hash_grid_path_matches_oracle(ctx, cylinder):
     """Two far outliers blow the target's bounding box up to ~1e11 cells: the index falls back to the hash table, the
-    loop to the one-thread-per-slot kernel + separate solve kernel.  Same trajectory as the oracle; a batch is refused."""
-    from dcreg_b200 import default_params
-    from dcreg_b200.api import DcregError
+    loop to the one-thread-per-slot kernel + separate solve kernel.  Same trajectory as the oracle; a batch and the
+    point-to-point metrics (dense grids only) are refused.  Back on a dense target, the context's reused grid arena
+    gives the bits of a fresh context."""
+    from dcreg_b200 import Context, default_params
+    from dcreg_b200.api import BAD_ARG, DcregError
     from dcreg_b200.scenes import g2_initial_pose
     tgt = np.concatenate([cylinder, np.array([[4000.0, 4500.0, 5000.0], [-4000.0, -3000.0, 2000.0]], np.float32)]).astype(np.float32)
     T0 = g2_initial_pose()
@@ -351,7 +353,20 @@ def test_hash_grid_path_matches_oracle(ctx, cylinder):
     assert o.se3_log_distance(T_ref, res.T) < 1e-6
     with pytest.raises(DcregError):
         ctx.icp_run_batch(gp, perturbations(2))
+    with pytest.raises(DcregError) as e:
+        ctx.point_to_point_metrics(res.T, 0.2)
+    assert e.value.status == BAD_ARG
     ctx.set_target(cylinder, 1.0)            # back to a dense grid for the tests that follow
+    dense = ctx.icp_run(gp, T0)
+    m = ctx.point_to_point_metrics(dense.T, 0.2)
+    with Context(0) as fresh:
+        fresh.set_target(cylinder, 1.0)
+        fresh.set_source(cylinder)
+        ref = fresh.icp_run(gp, T0)
+        assert m == fresh.point_to_point_metrics(ref.T, 0.2)
+    assert (dense.status, dense.iterations, dense.converged) == (ref.status, ref.iterations, ref.converged)
+    assert dense.T.tobytes() == ref.T.tobytes()
+    assert [np.array(L.H27).tobytes() for L in dense.logs] == [np.array(L.H27).tobytes() for L in ref.logs]
 
 
 def test_batch_with_aborting_trials(ctx, cylinder):

@@ -3,7 +3,7 @@
 Every pair of a batch must be the registration dcreg_set_target(target) + dcreg_set_source(source) + dcreg_icp_run would
 give: status, iteration counts, flags, per-iteration counts and masks identical, sums / steps / poses equal to the
 rounding of FP64 sums grouped differently.  With one shared map as every target it must be bit-identical to
-dcreg_icp_run_scans against that map (the grid arena orders every target as build_grid does).  A batch reproduces bit for
+dcreg_icp_run_scans against that map (dcreg_set_target builds its grid with the same arena code, as one cloud).  A batch reproduces bit for
 bit, leaves the context's own clouds alone, and its per-pair covariance and point-to-point metrics equal the single calls'.
 """
 import ctypes as C

@@ -1,7 +1,8 @@
 // Host check of arena_plan.hpp (tests/test_arena_plan.py): the planning of a grid arena, the dense grids of many
 // clouds in one set of buffers (dcreg_icp_run_pairs).  Per-cloud boxes and dims from the bounds, cell offsets that
-// follow each other, the +-2^19 cell range, the dense-cell limit per cloud and in total, the offset tables; and a
-// replay of the arena's grouping (one stable order by global cell id) against every cloud grouped alone.
+// follow each other, the +-2^19 cell range, the dense-cell limit per cloud and in total, the one-cloud decision of the
+// context's target (dense, hash table or error), the offset tables; and a replay of the arena's grouping (one stable
+// order by global cell id) against every cloud grouped alone.
 #include <algorithm>
 #include <cstdio>
 #include <numeric>
@@ -43,13 +44,18 @@ int main() {
     for (int k = 0; k < 3; ++k) {
         int hb[12] = {0, 0, 0, 1, 1, 1, -L, -L, -L, -L + 3, -L + 3, -L + 3};
         CHECK(arena_plan::plan(2, hb, boxes, &cells, "cloud").empty());
+        arena_plan::Box one;                                    // box_of: the context's target alone
+        CHECK(arena_plan::box_of(hb + 6, &one) == arena_plan::kDense && one.ox == -L && one.cells == 64);
         hb[6 + k] = -L - 1;
         const std::string why = arena_plan::plan(2, hb, boxes, &cells, "cloud");
         CHECK(why.find("cloud 1") != std::string::npos && why.find("2^19") != std::string::npos);
         int hi[6] = {L - 2, L - 2, L - 2, L, L, L};
         CHECK(arena_plan::plan(1, hi, boxes, &cells, "cloud").empty());
+        CHECK(arena_plan::box_of(hi, &one) == arena_plan::kDense && one.cells == 27 && one.cell_off == 0);
         hi[3 + k] = L + 1;
         CHECK(arena_plan::plan(1, hi, boxes, &cells, "cloud").find("2^19") != std::string::npos);
+        CHECK(arena_plan::box_of(hi, &one) == arena_plan::kOutOfRange);                // the context's target: an error
+        CHECK(arena_plan::box_of(hb + 6, &one) == arena_plan::kOutOfRange);
     }
     // NaN / infinite coordinates come back as INT_MIN cell coordinates
     {
@@ -63,6 +69,11 @@ int main() {
         int big[6] = {0, 0, 0, 1023, 1023, 128};
         const std::string why = arena_plan::plan(1, big, boxes, &cells, "cloud");
         CHECK(why.find("dense") != std::string::npos && why.find("cloud 0") != std::string::npos);
+        // the same limit for the context's target alone, where one row more means the hash table, not an error
+        arena_plan::Box one;
+        CHECK(arena_plan::box_of(ok, &one) == arena_plan::kDense && one.cells == (1ll << 27));
+        CHECK(one.ox == 0 && one.nx == 1024 && one.ny == 1024 && one.nz == 128 && one.cell_off == 0);
+        CHECK(arena_plan::box_of(big, &one) == arena_plan::kTooManyCells && one.cells == (1ll << 27) + (1ll << 20));
     }
     // all clouds of a call: 8 x 2^27 = 2^30 cells fit, a ninth does not
     {
