@@ -193,6 +193,22 @@ class IcpResult:
         self.metrics = None
 
 
+def _trial_results(st, conv, n_it, T_out, logs, cap, cov=None):
+    """One IcpResult per trial from a batched call's per-trial outputs.  logs: cap records per trial, or None.  A trial
+    holds min(iterations, cap) records, one more when it aborted with NONFINITE_UPDATE before the cap (that abort
+    writes the record of the failed iteration)."""
+    out = []
+    for b in range(len(st)):
+        recs = []
+        if logs is not None:
+            nrec = min(n_it[b], cap)
+            if st[b] == NONFINITE_UPDATE and n_it[b] < cap:
+                nrec = n_it[b] + 1
+            recs = [logs[b * cap + i] for i in range(nrec)]
+        out.append(IcpResult(int(st[b]), bool(conv[b]), int(n_it[b]), T_out[b], recs, None if cov is None else cov[b]))
+    return out
+
+
 class Context:
     """One engine context per GPU (owns the stream, device buffers and the optional NCCL comm)."""
 
@@ -371,16 +387,7 @@ class Context:
         logs = (IterLog * max(cap * B, 1))() if want_log else None
         self._check(self.lib.dcreg_icp_run_batch(self._h, C.byref(params), B, _dptr(T_init), _dptr(T_out), n_it, conv, st,
                                                  logs, cap))
-        out = []
-        for b in range(B):
-            recs = []
-            if want_log:
-                nrec = min(n_it[b], cap)
-                if st[b] == NONFINITE_UPDATE and n_it[b] < cap:
-                    nrec = n_it[b] + 1
-                recs = [logs[b * cap + i] for i in range(nrec)]
-            out.append(IcpResult(int(st[b]), bool(conv[b]), int(n_it[b]), T_out[b], recs))
-        return out
+        return _trial_results(st, conv, n_it, T_out, logs, cap)
 
     def icp_run_scans(self, params: IcpParams, scans, T_init, want_log: bool = False, want_cov: bool = False):
         """Different scans (a list of (N_b, >=3) point arrays) against the context's target, side by side, each from its
@@ -406,17 +413,7 @@ class Context:
         self._check(self.lib.dcreg_icp_run_scans(self._h, C.byref(params), B, xyz.ctypes.data_as(C.POINTER(C.c_float)),
                                                  offsets.ctypes.data_as(C.POINTER(C.c_int64)), stride, _dptr(T_init),
                                                  _dptr(T_out), n_it, conv, st, _dptr(cov) if want_cov else None, logs, cap))
-        out = []
-        for b in range(B):
-            recs = []
-            if want_log:
-                nrec = min(n_it[b], cap)
-                if st[b] == NONFINITE_UPDATE and n_it[b] < cap:
-                    nrec = n_it[b] + 1
-                recs = [logs[b * cap + i] for i in range(nrec)]
-            out.append(IcpResult(int(st[b]), bool(conv[b]), int(n_it[b]), T_out[b], recs,
-                                 cov[b] if want_cov else None))
-        return out
+        return _trial_results(st, conv, n_it, T_out, logs, cap, cov)
 
     def icp_run_pairs(self, params: IcpParams, sources, targets, T_init, cell_size=None, want_log: bool = False,
                       want_cov: bool = False, metrics_threshold=None):
@@ -455,18 +452,10 @@ class Context:
             xyz_t.ctypes.data_as(fp), off_t.ctypes.data_as(C.POINTER(C.c_int64)), 3, cell, _dptr(T_init), _dptr(T_out),
             n_it, conv, st, _dptr(cov) if want_cov else None,
             float(metrics_threshold) if met is not None else 0.0, _dptr(met) if met is not None else None, logs, cap))
-        out = []
-        for b in range(B):
-            recs = []
-            if want_log:
-                nrec = min(n_it[b], cap)
-                if st[b] == NONFINITE_UPDATE and n_it[b] < cap:
-                    nrec = n_it[b] + 1
-                recs = [logs[b * cap + i] for i in range(nrec)]
-            r = IcpResult(int(st[b]), bool(conv[b]), int(n_it[b]), T_out[b], recs, cov[b] if want_cov else None)
-            if met is not None:
-                r.metrics = {"rmse": met[b, 0], "fitness": met[b, 1], "chamfer": met[b, 2], "n_valid": int(met[b, 3])}
-            out.append(r)
+        out = _trial_results(st, conv, n_it, T_out, logs, cap, cov)
+        if met is not None:
+            for r, m in zip(out, met):
+                r.metrics = {"rmse": m[0], "fitness": m[1], "chamfer": m[2], "n_valid": int(m[3])}
         return out
 
     def icp_run_host_planes(self, params: IcpParams, T_init, plane_fn, want_log: bool = True) -> IcpResult:

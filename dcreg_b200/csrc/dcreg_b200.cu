@@ -732,59 +732,46 @@ __global__ void covariance_kernel(const IcpState* st, double* cov) {
         for (int i = 0; i < 36; ++i) cov[i] = (i % 7 == 0) ? 1e6 : 0.0;
 }
 
-__global__ void pack_source_kernel(const float* __restrict__ in, long long n, int stride, float4* __restrict__ out,
-                                   float* __restrict__ radius) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    float r = 0.0f;
-    if (i < n) {
-        const float x = in[i * stride], y = in[i * stride + 1], z = in[i * stride + 2];
-        out[i] = make_float4(x, y, z, __int_as_float((int)i));   // w = slot index
-        r = sqrtf(x * x + y * y + z * z);
-        if (!(r < 3.0e38f)) r = 0.0f;                            // NaN / Inf points do not define a lever arm
-    }
-    if (radius) {                                               // max |p|: lever arm that turns a rotation step into metres
-#pragma unroll
-        for (int off = 16; off > 0; off >>= 1) r = fmaxf(r, __shfl_xor_sync(0xffffffffu, r, off));
-        if ((threadIdx.x & 31) == 0 && r > 0.0f) atomicMax(reinterpret_cast<int*>(radius), __float_as_int(r));
-    }
-}
-
-// A batch of scans concatenated (dcreg_icp_run_scans): scan b owns the points [seg[b], seg[b+1]).  Packs every point as
-// pack_source_kernel does (w = index inside its scan), takes the per-scan max |p| (the lever arm of that scan) and writes
-// the key of the per-scan spatial sort: (scan, target cell of fl32(T_b p)) with the point's index as the value.  A
-// stable sort on that key orders each segment exactly as sort_source_by_cell orders the scan alone: by cell, then index.
-// grids (scan/target pairs, dcreg_icp_run_pairs): scan b's cell is taken in its own target's grid grids[b], and the key
-// is that cell's global id in the grid arena, cell_off[b] + cell (the pairs' cell ranges follow each other in pair
-// order, so the key still sorts by scan first); g and ncells are then unused.
-__global__ void pack_scans_kernel(const float* __restrict__ in, long long n, int stride, const long long* __restrict__ seg,
-                                  int n_scans, const double* __restrict__ T, corr::Grid g, long long ncells,
-                                  float4* __restrict__ out, float* __restrict__ radius, unsigned long long* __restrict__ keys,
-                                  int* __restrict__ vals, const corr::Grid* __restrict__ grids = nullptr,
-                                  const int* __restrict__ cell_off = nullptr) {
+// Pack host points (`stride` floats each) into float4 with w = the point's index inside its segment, and take each
+// segment's max |p| into radius[b] (the lever arm that turns a rotation step into metres; NaN / Inf points count as 0).
+// One segment (seg null, n_seg = 1): w is the global index and radius, when given, the max over all points.
+__global__ void pack_points_kernel(const float* __restrict__ in, long long n, int stride, const long long* __restrict__ seg,
+                                   int n_seg, float4* __restrict__ out, float* __restrict__ radius) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     int b = -1;
     float r = 0.0f;
     if (i < n) {
-        int lo = 0, hi = n_scans;                                // largest b with seg[b] <= i
-        while (hi - lo > 1) {
-            const int mid = (lo + hi) >> 1;
-            if (seg[mid] <= i) lo = mid; else hi = mid;
-        }
-        b = lo;
+        b = corr::segment_of(seg, n_seg, i);     // one segment reads no table: seg may be null
         const float x = in[i * stride], y = in[i * stride + 1], z = in[i * stride + 2];
-        const float4 p = make_float4(x, y, z, __int_as_float((int)(i - seg[b])));
-        out[i] = p;
+        out[i] = make_float4(x, y, z, __int_as_float((int)(i - (b > 0 ? seg[b] : 0))));
         r = sqrtf(x * x + y * y + z * z);
         if (!(r < 3.0e38f)) r = 0.0f;
-        if (grids) keys[i] = (unsigned long long)cell_off[b] + (unsigned long long)corr::source_cell(grids[b], T + (size_t)b * 16, p);
-        else keys[i] = (unsigned long long)b * (unsigned long long)ncells + (unsigned long long)corr::source_cell(g, T + (size_t)b * 16, p);
-        vals[i] = (int)i;
     }
-    // max |p| per scan: the lanes of a warp that hold points of the same scan reduce together
-    const unsigned peers = __match_any_sync(0xffffffffu, b);
-    const unsigned rmax = __reduce_max_sync(peers, __float_as_uint(r));      // r >= 0: the bits order like the values
-    if (b >= 0 && (int)(threadIdx.x & 31) == __ffs(peers) - 1 && rmax > 0u)
-        atomicMax(reinterpret_cast<unsigned int*>(radius + b), rmax);
+    if (radius) {                               // the lanes of a warp that hold points of the same segment reduce together
+        const unsigned peers = __match_any_sync(0xffffffffu, b);
+        const unsigned rmax = __reduce_max_sync(peers, __float_as_uint(r));  // r >= 0: the bits order like the values
+        if (b >= 0 && (int)(threadIdx.x & 31) == __ffs(peers) - 1 && rmax > 0u)
+            atomicMax(reinterpret_cast<unsigned int*>(radius + b), rmax);
+    }
+}
+
+// Key of the scans' spatial sort (upload_scans_sorted) of packed points: (scan b, target cell of fl32(T_b p)) with
+// T_b = T[16 b ..], and the point's index as the value.  A stable sort on that key orders each segment exactly as
+// sort_source_by_cell orders the scan alone: by cell, then index.  Against the context's grid g the key is
+// b * ncells + cell.  grids (scan/target pairs, dcreg_icp_run_pairs): scan b's cell is taken in its own target's grid
+// grids[b], and the key is that cell's global id in the grid arena, cell_off[b] + cell (the pairs' cell ranges follow
+// each other in pair order, so the key still sorts by scan first); g and ncells are then unused.
+__global__ void cell_key_kernel(const float4* __restrict__ pts, long long n, const long long* __restrict__ seg, int n_seg,
+                                const double* __restrict__ T, corr::Grid g, long long ncells,
+                                const corr::Grid* __restrict__ grids, const int* __restrict__ cell_off,
+                                unsigned long long* __restrict__ keys, int* __restrict__ vals) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int b = corr::segment_of(seg, n_seg, i);
+    const float4 p = pts[i];
+    if (grids) keys[i] = (unsigned long long)cell_off[b] + (unsigned long long)corr::source_cell(grids[b], T + (size_t)b * 16, p);
+    else keys[i] = (unsigned long long)b * (unsigned long long)ncells + (unsigned long long)corr::source_cell(g, T + (size_t)b * 16, p);
+    vals[i] = (int)i;
 }
 
 __global__ void gather_points_kernel(const float4* __restrict__ in, const int* __restrict__ idx, long long n,
@@ -1072,13 +1059,17 @@ int ensure_stage(dcreg_ctx* ctx, size_t bytes) {
     return DCREG_OK;
 }
 
-int upload_points(dcreg_ctx* ctx, const float* xyz, long long n, int stride, float4* d_out, float* d_radius) {
+// host points -> d_out, packed by pack_points_kernel (d_seg: device table of n_seg segments, or null for one; d_radius:
+// [n_seg] per-segment max |p|, or null)
+int upload_points(dcreg_ctx* ctx, const float* xyz, long long n, int stride, const long long* d_seg, int n_seg,
+                  float4* d_out, float* d_radius) {
     const size_t bytes = (size_t)n * stride * sizeof(float);
     const int rc = ensure_stage(ctx, bytes);
     if (rc) return rc;
     CK(cudaMemcpyAsync(ctx->d_stage, xyz, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    if (d_radius) CK(cudaMemsetAsync(d_radius, 0, sizeof(float), ctx->stream));
-    pack_source_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_stage, n, stride, d_out, d_radius);
+    if (d_radius) CK(cudaMemsetAsync(d_radius, 0, (size_t)n_seg * sizeof(float), ctx->stream));
+    pack_points_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_stage, n, stride, d_seg, n_seg, d_out,
+                                                                            d_radius);
     ctx->launches++;
     CK(cudaGetLastError());
     return DCREG_OK;
@@ -1285,7 +1276,7 @@ int dcreg_set_source(dcreg_ctx* ctx, const float* xyz, int64_t n, int stride) {
     ctx->n_src = n;
     if (ctx->nranks == 1) ctx->n_src_total = n;
     if (!ctx->d_src_radius) CK(cudaMalloc(&ctx->d_src_radius, sizeof(float)));
-    return upload_points(ctx, xyz, n, stride, ctx->d_src, ctx->d_src_radius);
+    return upload_points(ctx, xyz, n, stride, nullptr, 1, ctx->d_src, ctx->d_src_radius);
 }
 
 int dcreg_set_global_source_count(dcreg_ctx* ctx, int64_t n_total) {
@@ -1482,7 +1473,7 @@ int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, do
     ctx->has_grid = false;
     CK(cudaMalloc(&ctx->d_tgt, (size_t)m * sizeof(float4)));
     ctx->n_tgt = m;
-    int rc = upload_points(ctx, xyz, m, stride, ctx->d_tgt, nullptr);
+    int rc = upload_points(ctx, xyz, m, stride, nullptr, 1, ctx->d_tgt, nullptr);
     if (rc) return rc;
     ctx->cell_size = cell_size;
     // the target is the one cloud of tgt_arena
@@ -1680,16 +1671,13 @@ static int ensure_scans(dcreg_ctx* ctx, int n_scans, long long total) {
 // radix sort of the (scan, cell) keys keeps the segments contiguous and in scan order and needs no per-scan cell tables.
 static int upload_scans_sorted(dcreg_ctx* ctx, const ScanBatch& S, const float4** src_out) {
     const long long n = S.total;
-    const size_t bytes = (size_t)n * S.stride * sizeof(float);
-    int rc = ensure_stage(ctx, bytes);
+    int rc = upload_points(ctx, S.xyz, n, S.stride, S.seg, S.n, ctx->d_scan_src, ctx->d_scan_radius);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_stage, S.xyz, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemsetAsync(ctx->d_scan_radius, 0, (size_t)S.n * sizeof(float), ctx->stream));
     unsigned long long* keys = ctx->d_scan_keys;
     int* vals = ctx->d_scan_vals;
-    pack_scans_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_stage, n, S.stride, S.seg, S.n, ctx->d_T_init,
-                                                                           ctx->grid, ctx->grid_cells, ctx->d_scan_src,
-                                                                           ctx->d_scan_radius, keys, vals, S.grids, S.cell_off);
+    const unsigned nb = (unsigned)((n + 255) / 256);
+    cell_key_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_scan_src, n, S.seg, S.n, ctx->d_T_init, ctx->grid, ctx->grid_cells,
+                                                 S.grids, S.cell_off, keys, vals);
     ctx->launches++;
     CK(cudaGetLastError());
     // keys below n_scans * cells of the context's grid, or below the arena's cell count (pairs)
@@ -1708,7 +1696,7 @@ static int upload_scans_sorted(dcreg_ctx* ctx, const ScanBatch& S, const float4*
     tmp = ctx->scan_sort_tmp_bytes;
     CK(cub::DeviceRadixSort::SortPairs(ctx->d_scan_sort_tmp, tmp, keys, keys + n, vals, vals + n, (int)n, 0, end_bit,
                                        ctx->stream));
-    gather_points_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_scan_src, vals + n, n, ctx->d_scan_sorted);
+    gather_points_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_scan_src, vals + n, n, ctx->d_scan_sorted);
     ctx->launches++;                                             // (the radix sort's own kernels are not counted)
     CK(cudaGetLastError());
     *src_out = ctx->d_scan_sorted;
@@ -2298,17 +2286,54 @@ int dcreg_icp_fetch(dcreg_ctx* ctx, double T_out[16], int* n_iterations, int* co
     return rc ? rc : status;
 }
 
+// The trials of one call are the loop kernel's grid y: at most kMaxPairs.  offsets (scans, pairs): the sources' table
+static int check_batch(dcreg_ctx* ctx, int n, const int64_t* offsets, const char* what) {
+    std::string why;
+    if (n > arena_plan::kMaxPairs)
+        why = std::string(what) + ": more than " + std::to_string(arena_plan::kMaxPairs) + " trials in one call";
+    else if (offsets)
+        why = arena_plan::check_offsets(n, offsets, arena_plan::kMaxPoints, what);
+    if (why.empty()) return DCREG_OK;
+    ctx->err = why;
+    return DCREG_BAD_ARG;
+}
+
 int dcreg_icp_run_batch(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_trials, const double* T_init,
                         double* T_out, int* n_iterations, int* converged, int* status, dcreg_iter_log* log, int log_cap) {
     if (!ctx) return DCREG_BAD_ARG;
     if (!params || !T_init || !T_out || n_trials <= 0) { ctx->err = "icp_run_batch: null pointer or n_trials <= 0"; return DCREG_BAD_ARG; }
     if (ctx->comm) { ctx->err = "icp_run_batch: trials are independent - distribute them over ranks, do not shard them"; return DCREG_BAD_ARG; }
-    int rc = check_run_args(ctx, params);
-    if (rc) return rc;
+    int rc = check_batch(ctx, n_trials, nullptr, "icp_run_batch");
+    if (rc || (rc = check_run_args(ctx, params))) return rc;
     CK(cudaSetDevice(ctx->device));
     std::vector<int> st_local;
     if (!status) { st_local.resize(n_trials); status = st_local.data(); }
     return run_loop(ctx, params, n_trials, T_init, T_out, log, log_cap, n_iterations, converged, status);
+}
+
+// What dcreg_icp_run_scans and dcreg_icp_run_pairs share once check_batch has passed their sources' offsets: S.n
+// sources (S.xyz, S.stride; S.grids etc. for pairs) registered side by side, one trial each, then covariance_kernel's
+// rule per trial.  Leaves the packed sources in ctx->d_scan_src and their offsets in ctx->d_scan_seg.
+static int run_sources(dcreg_ctx* ctx, const dcreg_icp_params* params, ScanBatch S, const int64_t* offsets,
+                       const double* T_init, double* T_out, int* n_iterations, int* converged, int* status, double* cov,
+                       dcreg_iter_log* log, int log_cap) {
+    S.total = offsets[S.n];
+    for (int b = 0; b < S.n; ++b) S.max_n = std::max<long long>(S.max_n, offsets[b + 1] - offsets[b]);
+    int rc = ensure_scans(ctx, S.n, S.total);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(ctx->d_scan_seg, offsets, (size_t)(S.n + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+    S.seg = ctx->d_scan_seg; S.radius = ctx->d_scan_radius;
+    std::vector<int> st_local;
+    if (!status) { st_local.resize(S.n); status = st_local.data(); }
+    if ((rc = run_loop(ctx, params, S.n, T_init, T_out, log, log_cap, n_iterations, converged, status, true, &S))) return rc;
+    if (cov) {
+        covariance_kernel<<<S.n, 32, 0, ctx->stream>>>(ctx->d_state, ctx->d_scan_cov);
+        ctx->launches++;
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(cov, ctx->d_scan_cov, (size_t)S.n * 36 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    return DCREG_OK;
 }
 
 int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_scans, const float* xyz,
@@ -2327,30 +2352,10 @@ int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_sc
         ctx->err = "icp_run_scans: batches need the dense target grid (target bounding box / cell size too large for it)";
         return DCREG_BAD_ARG;
     }
-    if (scan_offsets[0] != 0) { ctx->err = "icp_run_scans: scan_offsets[0] must be 0"; return DCREG_BAD_ARG; }
-    long long max_n = 0;
-    for (int b = 0; b < n_scans; ++b) {
-        const long long nb = scan_offsets[b + 1] - scan_offsets[b];
-        if (nb <= 0) { ctx->err = "icp_run_scans: scan " + std::to_string(b) + " is empty (offsets must ascend strictly)"; return DCREG_BAD_ARG; }
-        if (nb > max_n) max_n = nb;
-    }
-    const long long total = scan_offsets[n_scans];
-    if (total > 0x1fffffffLL) { ctx->err = "icp_run_scans: more than 2^29 points in one batch"; return DCREG_BAD_ARG; }
+    if ((rc = check_batch(ctx, n_scans, scan_offsets, "icp_run_scans: scan"))) return rc;
     CK(cudaSetDevice(ctx->device));
-    if ((rc = ensure_scans(ctx, n_scans, total))) return rc;
-    CK(cudaMemcpyAsync(ctx->d_scan_seg, scan_offsets, (size_t)(n_scans + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
-    const ScanBatch S{n_scans, xyz, stride, total, max_n, ctx->d_scan_seg, ctx->d_scan_radius};
-    std::vector<int> st_local;
-    if (!status) { st_local.resize(n_scans); status = st_local.data(); }
-    if ((rc = run_loop(ctx, params, n_scans, T_init, T_out, log, log_cap, n_iterations, converged, status, true, &S))) return rc;
-    if (cov) {                                                  // covariance_kernel's rule per scan
-        covariance_kernel<<<n_scans, 32, 0, ctx->stream>>>(ctx->d_state, ctx->d_scan_cov);
-        ctx->launches++;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(cov, ctx->d_scan_cov, (size_t)n_scans * 36 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    return DCREG_OK;
+    return run_sources(ctx, params, ScanBatch{n_scans, xyz, stride}, scan_offsets, T_init, T_out, n_iterations, converged,
+                       status, cov, log, log_cap);
 }
 
 // the pairs' own device buffers (dcreg_icp_run_pairs): packed targets, target offsets, final poses
@@ -2382,10 +2387,6 @@ int dcreg_icp_run_pairs(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_pa
         ctx->err = "icp_run_pairs: null pointer or n_pairs <= 0";
         return DCREG_BAD_ARG;
     }
-    if (n_pairs > arena_plan::kMaxPairs) {
-        ctx->err = "icp_run_pairs: more than " + std::to_string(arena_plan::kMaxPairs) + " pairs in one call";
-        return DCREG_BAD_ARG;
-    }
     if (stride < 3) { ctx->err = "icp_run_pairs: stride < 3"; return DCREG_BAD_ARG; }
     if (!(cell_size > 0.0)) { ctx->err = "icp_run_pairs: cell_size <= 0"; return DCREG_BAD_ARG; }
     if (ctx->comm) { ctx->err = "icp_run_pairs: pairs are independent - give each rank its own, do not shard them"; return DCREG_BAD_ARG; }
@@ -2393,34 +2394,23 @@ int dcreg_icp_run_pairs(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_pa
     if (rc) return rc;
     const int rings = search_rings(params->search_radius, cell_size);
     if (rings < 1 || rings > 4) { ctx->err = "icp_run_pairs: search_radius / cell_size must be in (0, 4]"; return DCREG_BAD_ARG; }
-    std::string why = arena_plan::check_offsets(n_pairs, src_offsets, arena_plan::kMaxPoints, "icp_run_pairs: source");
-    if (why.empty()) why = arena_plan::check_offsets(n_pairs, tgt_offsets, arena_plan::kMaxPoints, "icp_run_pairs: target");
+    if ((rc = check_batch(ctx, n_pairs, src_offsets, "icp_run_pairs: source"))) return rc;
+    const std::string why = arena_plan::check_offsets(n_pairs, tgt_offsets, arena_plan::kMaxPoints, "icp_run_pairs: target");
     if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
-    long long max_n = 0;
-    for (int b = 0; b < n_pairs; ++b) max_n = std::max<long long>(max_n, src_offsets[b + 1] - src_offsets[b]);
-    const long long n_src = src_offsets[n_pairs], n_tgt = tgt_offsets[n_pairs];
+    const long long n_tgt = tgt_offsets[n_pairs];
     CK(cudaSetDevice(ctx->device));
-    if ((rc = ensure_scans(ctx, n_pairs, n_src)) || (rc = ensure_pairs(ctx, n_pairs, n_tgt))) return rc;
-    CK(cudaMemcpyAsync(ctx->d_scan_seg, src_offsets, (size_t)(n_pairs + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+    if ((rc = ensure_pairs(ctx, n_pairs, n_tgt))) return rc;
     CK(cudaMemcpyAsync(ctx->d_pair_tgt_seg, tgt_offsets, (size_t)(n_pairs + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
     // the targets: packed with w = index over all targets, then every pair's dense grid in the arena
-    if ((rc = upload_points(ctx, tgt_xyz, n_tgt, stride, ctx->d_pair_tgt, nullptr))) return rc;
+    if ((rc = upload_points(ctx, tgt_xyz, n_tgt, stride, nullptr, 1, ctx->d_pair_tgt, nullptr))) return rc;
     long long cells = 0;
     if ((rc = build_grid_arena(ctx, ctx->pair_tgt, ctx->d_pair_tgt, tgt_offsets, ctx->d_pair_tgt_seg, n_pairs, cell_size,
                                rings, "icp_run_pairs: target", &cells)))
         return rc;
-    ScanBatch S{n_pairs, src_xyz, stride, n_src, max_n, ctx->d_scan_seg, ctx->d_scan_radius};
+    ScanBatch S{n_pairs, src_xyz, stride};
     S.grids = ctx->pair_tgt.d_grids; S.cell_off = ctx->pair_tgt.d_cell_off; S.cells = cells; S.cell_size = cell_size;
-    std::vector<int> st_local;
-    if (!status) { st_local.resize(n_pairs); status = st_local.data(); }
-    if ((rc = run_loop(ctx, params, n_pairs, T_init, T_out, log, log_cap, n_iterations, converged, status, true, &S))) return rc;
-    if (cov) {                                                  // covariance_kernel's rule per pair
-        covariance_kernel<<<n_pairs, 32, 0, ctx->stream>>>(ctx->d_state, ctx->d_scan_cov);
-        ctx->launches++;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(cov, ctx->d_scan_cov, (size_t)n_pairs * 36 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
+    if ((rc = run_sources(ctx, params, S, src_offsets, T_init, T_out, n_iterations, converged, status, cov, log, log_cap)))
+        return rc;
     if (!metrics) return DCREG_OK;
     CK(cudaMemcpyAsync(ctx->d_pair_T, T_out, (size_t)n_pairs * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     return p2p_metrics(ctx, n_pairs, ctx->d_scan_src, ctx->d_scan_seg, src_offsets, ctx->d_pair_tgt, ctx->d_pair_tgt_seg,

@@ -215,24 +215,26 @@ int dcreg_icp_fetch(dcreg_ctx* ctx, double T_out[16], int* n_iterations, int* co
  * (BASELINE.json configs[4]) calls.  T_init / T_out: n_trials row-major 4x4 matrices; n_iterations / converged / status:
  * n_trials ints (status[t] = what dcreg_icp_run would have returned for trial t; any may be NULL except T_init, T_out);
  * log: n_trials x log_cap records (trial-major) or NULL.  Every trial runs the kernels a dcreg_icp_run from the same
- * T_init runs: counts, masks and iteration counts are identical, poses equal up to the order of the FP64 sums (the
- * source is sorted by target cell once, under trial 0's pose, and a single run of a small cloud uses smaller tiles;
- * 1e-8 on the poses in the tests; a batch itself is reproducible bit for bit).  Not
+ * T_init runs (at most 65535 trials: the grid's y-dimension): counts, masks and iteration counts are identical, poses
+ * equal up to the order of the FP64 sums (the source is sorted by target cell once, under trial 0's pose, and a single
+ * run of a small cloud uses smaller tiles; 1e-8 on the poses in the tests; a batch itself is reproducible bit for
+ * bit).  Not
  * available on a sharded context: trials are independent, distribute them over ranks instead.  Needs the dense grid. */
 int dcreg_icp_run_batch(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_trials, const double* T_init,
                         double* T_out, int* n_iterations, int* converged, int* status, dcreg_iter_log* log,
                         int log_cap);
 /* Many DIFFERENT source scans (e.g. the LiDAR frames of a sequence) against the context's target, side by side in one
- * sequence of launches, with one set of parameters.  xyz: HOST memory, all scans concatenated, `stride` floats per point
- * as in dcreg_set_source; scan b is points [scan_offsets[b], scan_offsets[b+1]) (n_scans + 1 entries, ascending from 0,
- * no empty scan).  T_init / T_out: n_scans row-major 4x4 matrices; n_iterations / converged / status: n_scans ints
- * (status[b] = what dcreg_icp_run would have returned for scan b alone; may be NULL); cov: n_scans x 36 doubles, scan b's
- * post-loop covariance as dcreg_last_covariance gives it after a single run, or NULL; log: n_scans x log_cap records
- * (scan-major) or NULL.  Each scan is sorted by target cell under its own initial pose and stops on its own convergence
- * test; it differs from dcreg_set_source(scan b) + dcreg_icp_run only in how the FP64 partial sums are grouped (counts,
- * masks and iteration counts identical, poses equal to rounding; a batch itself is reproducible bit for bit).  The scans
- * go to buffers of their own: the context's source and what dcreg_icp_run computes from it are left as they were.
- * Not available on a sharded context (distribute scans over ranks instead).  Needs the dense grid. */
+ * sequence of launches, with one set of parameters.  xyz: HOST memory, all scans concatenated, `stride` floats per
+ * point as in dcreg_set_source; scan b is points [scan_offsets[b], scan_offsets[b+1]) (n_scans + 1 entries, ascending
+ * from 0, no empty scan; at most 2^29 - 1 points and 65535 scans).  T_init / T_out: n_scans row-major 4x4 matrices;
+ * n_iterations / converged / status: n_scans ints (status[b] = what dcreg_icp_run would have returned for scan b alone;
+ * may be NULL); cov: n_scans x 36 doubles, scan b's post-loop covariance as dcreg_last_covariance gives it after a
+ * single run, or NULL; log: n_scans x log_cap records (scan-major) or NULL.  Each scan is sorted by target cell under
+ * its own initial pose and stops on its own convergence test; it differs from dcreg_set_source(scan b) + dcreg_icp_run
+ * only in how the FP64 partial sums are grouped (counts, masks and iteration counts identical, poses equal to rounding;
+ * a batch itself is reproducible bit for bit).  The scans go to buffers of their own: the context's source and what
+ * dcreg_icp_run computes from it are left as they were. Not available on a sharded context (distribute scans over ranks
+ * instead).  Needs the dense grid. */
 int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_scans, const float* xyz,
                         const int64_t* scan_offsets, int stride, const double* T_init, double* T_out,
                         int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,

@@ -197,11 +197,16 @@ def test_batched_trials_match_oracle(ctx, cylinder):
 
 def test_batch_bad_arguments(ctx, cylinder):
     from dcreg_b200 import default_params
-    from dcreg_b200.api import DcregError
+    from dcreg_b200.api import BAD_ARG, DcregError
     ctx.set_target(cylinder, 1.0)
     ctx.set_source(cylinder)
     with pytest.raises(DcregError):
         ctx.icp_run_batch(default_params(weight_gate=1.5), perturbations(2))
+    # more trials than the loop kernel's grid y holds (65535): rejected before anything is launched
+    launches = ctx.launch_count
+    with pytest.raises(DcregError) as e:
+        ctx.icp_run_batch(default_params(), np.broadcast_to(np.eye(4), (65536, 4, 4)))
+    assert e.value.status == BAD_ARG and ctx.launch_count == launches
     res = ctx.icp_run_batch(default_params(max_iterations=0), perturbations(3))
     assert all(r.iterations == 0 and not r.converged for r in res)
 

@@ -196,6 +196,13 @@ def test_scans_bad_arguments(ctx, scene, cylinder):
     for kw in bad:
         assert call(**kw) == api.BAD_ARG, kw
         assert lib.dcreg_last_error(h).decode(), kw
+    # more scans than the loop kernel's grid y holds (65535): rejected before anything is launched
+    n_big = 65536
+    big = dict(n=n_big, pts=np.zeros((n_big, 3), np.float32), offsets=np.arange(n_big + 1, dtype=np.int64),
+               T0=np.ascontiguousarray(np.broadcast_to(np.eye(4), (n_big, 4, 4))), Tout=np.empty((n_big, 4, 4)))
+    launches = ctx.launch_count
+    assert call(**big) == api.BAD_ARG
+    assert ctx.launch_count == launches
     with pytest.raises(api.DcregError) as e:
         ctx.icp_run_scans(prm, [], np.zeros((0, 4, 4)))
     assert e.value.status == api.BAD_ARG
