@@ -87,7 +87,7 @@ EXPORTS = [
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -127,6 +127,9 @@ def load_library():
     lib.dcreg_icp_run_pairs.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(C.c_float), C.POINTER(i64),
                                         C.POINTER(C.c_float), C.POINTER(i64), ci, C.c_double, dp, dp, C.POINTER(ci),
                                         C.POINTER(ci), C.POINTER(ci), dp, C.c_double, dp, C.POINTER(IterLog), ci]
+    lib.dcreg_icp_run_sequences.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
+                                            C.POINTER(i64), ci, dp, dp, dp, dp, C.POINTER(ci), C.POINTER(ci), C.POINTER(ci),
+                                            dp, C.POINTER(IterLog), ci]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -186,11 +189,29 @@ def pose_Rt(T):
     return np.ascontiguousarray(np.concatenate([T[:3, :3].reshape(-1), T[:3, 3]]))
 
 
+def compose_prior(T, D):
+    """The next frame's prior T D of dcreg_icp_run_sequences, bit for bit as the device composes it: R' = R R_D and
+    t' = R t_D + t, every entry ((a0 b0 + a1 b1) + a2 b2) [+ t] in FP64, one rounding per operation (elementwise NumPy
+    ops, no matmul, no FMA), no re-orthonormalisation.  T, D: (..., 4, 4); returns (..., 4, 4) with the row [0, 0, 0, 1]."""
+    T = np.asarray(T, dtype=np.float64)
+    D = np.asarray(D, dtype=np.float64)
+    shape = np.broadcast_shapes(T.shape, D.shape)
+    out = np.zeros(shape)
+    for c in range(4):
+        col = (T[..., :3, 0] * D[..., 0:1, c] + T[..., :3, 1] * D[..., 1:2, c]) + T[..., :3, 2] * D[..., 2:3, c]
+        if c == 3:
+            col = col + T[..., :3, 3]
+        out[..., :3, c] = col
+    out[..., 3, 3] = 1.0
+    return out
+
+
 class IcpResult:
     def __init__(self, status, converged, iterations, T, logs, cov=None):
         self.status, self.converged, self.iterations, self.T, self.logs = status, converged, iterations, T, logs
         self.cov = cov
         self.metrics = None
+        self.T_prior = None             # icp_run_sequences: the initial pose the frame started from
 
 
 def _trial_results(st, conv, n_it, T_out, logs, cap, cov=None):
@@ -414,6 +435,49 @@ class Context:
                                                  offsets.ctypes.data_as(C.POINTER(C.c_int64)), stride, _dptr(T_init),
                                                  _dptr(T_out), n_it, conv, st, _dptr(cov) if want_cov else None, logs, cap))
         return _trial_results(st, conv, n_it, T_out, logs, cap, cov)
+
+    def icp_run_sequences(self, params: IcpParams, sequences, T_init, deltas=None, want_log: bool = False,
+                          want_cov: bool = False):
+        """Sequences of frames against the context's target (`sequences`: a list of lists of (N, >=3) point arrays).
+        Inside a sequence the frames run one after another on the device, frame k+1 starting from
+        compose_prior(frame k's result, deltas[k]); the sequences run side by side.  T_init (S, 4, 4): the prior of each
+        sequence's first frame.  deltas: (n_frames, 4, 4) increments over all frames in order (a sequence's last entry is
+        unused), or None for identity.  Returns a list of IcpResult, one per frame in order, with .T_prior the pose the
+        frame started from (logs only when want_log, .cov when want_cov).  The context's own source is left as it was."""
+        lens = [len(s) for s in sequences]
+        S = len(lens)
+        pts = [_as_points(f)[:, :3] for s in sequences for f in s]
+        n = len(pts)
+        seq_off = np.zeros(S + 1, dtype=np.int32)
+        seq_off[1:] = np.cumsum(lens)
+        if S == 0 or n == 0:                            # BAD_ARG from the library, like every other malformed batch
+            self._check(self.lib.dcreg_icp_run_sequences(self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)),
+                                                         0, None, None, 3, None, None, None, None, None, None, None, None,
+                                                         None, 0))
+        xyz = np.ascontiguousarray(np.concatenate(pts, axis=0))
+        offsets = np.zeros(n + 1, dtype=np.int64)
+        offsets[1:] = np.cumsum([p.shape[0] for p in pts])
+        T_init = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
+        if T_init.shape[0] != S:
+            raise ValueError(f"icp_run_sequences: {S} sequences but {T_init.shape[0]} initial poses")
+        if deltas is not None:
+            deltas = np.ascontiguousarray(deltas, dtype=np.float64).reshape(-1, 4, 4)
+            if deltas.shape[0] != n:
+                raise ValueError(f"icp_run_sequences: {n} frames but {deltas.shape[0]} increments")
+        T_prior = np.empty((n, 4, 4)); T_out = np.empty((n, 4, 4))
+        n_it = (C.c_int * n)(); conv = (C.c_int * n)(); st = (C.c_int * n)()
+        cov = np.empty((n, 6, 6)) if want_cov else None
+        cap = int(params.max_iterations) if want_log else 0
+        logs = (IterLog * max(cap * n, 1))() if want_log else None
+        self._check(self.lib.dcreg_icp_run_sequences(
+            self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n,
+            xyz.ctypes.data_as(C.POINTER(C.c_float)), offsets.ctypes.data_as(C.POINTER(C.c_int64)), 3, _dptr(T_init),
+            _dptr(deltas) if deltas is not None else None, _dptr(T_prior), _dptr(T_out), n_it, conv, st,
+            _dptr(cov) if want_cov else None, logs, cap))
+        out = _trial_results(st, conv, n_it, T_out, logs, cap, cov)
+        for r, Tp in zip(out, T_prior):
+            r.T_prior = Tp
+        return out
 
     def icp_run_pairs(self, params: IcpParams, sources, targets, T_init, cell_size=None, want_log: bool = False,
                       want_cov: bool = False, metrics_threshold=None):

@@ -93,6 +93,81 @@ __device__ __noinline__ void solve_step_in_kernel(const double* acc, IcpState* s
     if (lane == 0 && n_active && st->done) atomicSub(n_active, 1u);
 }
 
+// ---- sequences of frames (dcreg_icp_run_sequences) --------------------------------------------------------------
+// Grid y is the sequence LANE s; it runs the frames [first[s], first[s+1]) one after another, frame cursor[s] now.  The
+// reduction's working set (partials, ticket, sums) belongs to the lane; everything a registration owns (loop state,
+// record slices, lever arm, log slice, covariance) to the frame.  The cursor lives in device memory like the pose and
+// the mode flags, since a captured chunk of the loop freezes its kernel arguments.
+struct SeqView {
+    int* cursor;              // [lanes] frame the lane runs now (>= first[s + 1]: the lane is finished); null: no sequences
+    const int* first;         // [lanes + 1] frame ranges
+    const double* delta;      // [frames][16] row-major increments (frame k's result -> frame k+1's prior), or null (identity)
+    double* T_prior;          // [frames][16] the prior each frame started from
+    const long long* seg;     // [frames + 1] point offsets of the frames
+    unsigned int* n_active;   // lanes still running
+};
+
+// A fresh loop state at pose T (row-major 4x4) over n_source points: a trial of a batch before its first iteration, or
+// a frame of a sequence when the frame before it stops.  Unseeded, lean mode: the records of the slot range are unused.
+__device__ __forceinline__ void init_loop_state(IcpState* st, const double* T, long long n_source) {
+    for (int r = 0; r < 3; ++r) {
+        for (int c = 0; c < 3; ++c) st->R[r * 3 + c] = T[r * 4 + c];
+        st->t[r] = T[r * 4 + 3];
+    }
+    st->iter = 0; st->done = 0; st->converged = 0; st->status = DCREG_OK;
+    for (int i = 0; i < 36; ++i) st->H_last[i] = (i % 7 == 0) ? 1.0 : 0.0;
+    st->n_source_total = n_source;
+    st->step_rot = 1.0e30; st->step_trans = 1.0e30; st->seeds = 0; st->coherent_used = 0; st->coherent = 0; st->warm = 0;
+    st->t_last = k2::globaltimer_ns();                      // tic of iteration 0 (icp_test_runner.cpp:1695)
+}
+
+// Prior of the next frame, T' = T D: R' = R R_D, t' = R t_D + t, every entry ((a0 b0 + a1 b1) + a2 b2) [+ t] rounded in
+// that order with no FMA contraction and no re-orthonormalisation (dcreg_b200.api.compose_prior gives the same bits).
+// The host uses it for the dead-reckoned priors (plain x86-64 double arithmetic, which has no FMA to contract to).
+__host__ __device__ __forceinline__ void compose_prior(const double* R, const double* t, const double* D, double* T) {
+#ifdef __CUDA_ARCH__
+#define DCREG_MUL(x, y) __dmul_rn(x, y)
+#define DCREG_ADD(x, y) __dadd_rn(x, y)
+#else
+#define DCREG_MUL(x, y) ((x) * (y))
+#define DCREG_ADD(x, y) ((x) + (y))
+#endif
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+            double s = DCREG_ADD(DCREG_ADD(DCREG_MUL(R[3 * r], D[c]), DCREG_MUL(R[3 * r + 1], D[4 + c])),
+                                 DCREG_MUL(R[3 * r + 2], D[8 + c]));
+            if (c == 3) s = DCREG_ADD(s, t[r]);
+            T[4 * r + c] = s;
+        }
+#undef DCREG_MUL
+#undef DCREG_ADD
+    T[12] = 0.0; T[13] = 0.0; T[14] = 0.0; T[15] = 1.0;
+}
+
+// Lane s's frame `frame` has stopped (converged, max_iterations or aborted): start the next frame of the lane from the
+// pose this one returned composed with its increment, or, after the lane's last frame, count the lane as finished.  One
+// thread, right after the solve step; the next launch reads the cursor after pdl_wait.  Own register allocation, like
+// solve_step_in_kernel: the tile code does not pay for it.
+__device__ __noinline__ void advance_frame(SeqView q, IcpState* states, int s, int frame) {
+    const int next = frame + 1;
+    if (next < q.first[s + 1]) {
+        const IcpState* st = states + frame;
+        double D[16] = {1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0};
+        if (q.delta)
+            for (int i = 0; i < 16; ++i) D[i] = q.delta[(size_t)frame * 16 + i];
+        double T[16];
+        compose_prior(st->R, st->t, D, T);
+        double* P = q.T_prior + (size_t)next * 16;
+        for (int i = 0; i < 16; ++i) P[i] = T[i];
+        init_loop_state(states + next, T, q.seg[next + 1] - q.seg[next]);
+    } else {
+        atomicSub(q.n_active, 1u);
+    }
+    q.cursor[s] = next;
+}
+
 struct IterArgs {
     const float4* src;        // source points, w = bit-cast original index (spatially sorted copy or the original)
     long long n;
@@ -234,8 +309,11 @@ struct Iter2Args {
     // null: every trial runs the it.n slots of it.src, with record slices [b][it.n] and the one src_radius
     const long long* seg;
     // many scan/target pairs (dcreg_icp_run_pairs, with seg): trial b searches its own target grid grids[b] (device
-    // memory, rings set) instead of it.grid.  Only the icp_iter2_kernel<., true> instantiation reads it
+    // memory, rings set) instead of it.grid.  Only the icp_iter2_kernel<., true, .> instantiation reads it
     const corr::Grid* grids;
+    // sequences of frames (dcreg_icp_run_sequences, with seg: the frames' slot ranges): grid y is the lane, the trial the
+    // frame seq.cursor[lane].  Only the icp_iter2_kernel<., ., true> instantiation reads it
+    SeqView seq;
 };
 
 __device__ __forceinline__ void cswap5(unsigned long long& ka, int& pa, unsigned long long& kb, int& pb) {
@@ -293,19 +371,25 @@ __device__ __noinline__ void solver_block(const Iter2Args& a, IcpState* st, Iter
 }
 
 // kGrids: every trial has its own target grid (Iter2Args::grids), copied into shared memory once per block; the other
-// paths keep reading it.grid from the kernel parameters, untouched by the table
-template <bool kUseWd, bool kGrids>
+// paths keep reading it.grid from the kernel parameters, untouched by the table.  kSeq: grid y is a sequence lane
+// (Iter2Args::seq) whose trial is the frame it runs now; the reduction's working set is the lane's
+template <bool kUseWd, bool kGrids, bool kSeq>
 __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_constant__ Iter2Args a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     Iter2Smem& sm = *reinterpret_cast<Iter2Smem*>(smem_raw);
     const IterArgs& A = a.it;
     pdl_wait();                                   // the pose / mode flags come from the previous iteration's solve step
     pdl_release();
-    const int trial = (int)blockIdx.y;
+    const int ys = (int)blockIdx.y;               // owner of partials / ticket / sums: the trial, or (kSeq) the lane
+    int trial = ys;
+    if constexpr (kSeq) {                         // (the cursor too: written by the previous launch's frame advance)
+        trial = a.seq.cursor[ys];
+        if (trial >= a.seq.first[ys + 1]) return;
+    }
     IcpState* const st = A.state + trial;
     if (st->done) return;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const bool solver_path = a.row_flags != nullptr;
+    const bool solver_path = !kSeq && a.row_flags != nullptr;
     if (solver_path && blockIdx.x == 0) {
         DCREG_STAMP(0);
         solver_block(a, st, sm, *a.row_epoch, peer::load_epoch(a.peer));
@@ -589,19 +673,23 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
         return;
     }
     // ---- grid reduction of this trial, [sum over ranks], congruence, solve + pose update: all in the last block
-    if (!k1s::reduce_to_fin(mine, sm.tail, A.partials + (size_t)trial * gridDim.x * k1s::kPk, A.counter + trial,
+    if (!k1s::reduce_to_fin(mine, sm.tail, A.partials + (size_t)ys * gridDim.x * k1s::kPk, A.counter + ys,
                             (int)blockIdx.x, (int)gridDim.x)) return;
     DCREG_STAMP(6);
     peer::all_reduce32(a.peer, sm.tail.fin, sm.tail.red, epoch0);
     k1s::congruence(sm.tail.fin, st->R, sm.tail.acc);
     __syncthreads();
     DCREG_STAMP(7);
-    if (tid < kAcc) A.acc[(size_t)trial * kAcc + tid] = sm.tail.acc[tid];
+    if (tid < kAcc) A.acc[(size_t)ys * kAcc + tid] = sm.tail.acc[tid];
     if (a.fold_k2 && warp == 0) {
         solve_step_in_kernel(sm.tail.acc, st, &A.prm, a.log ? a.log + (size_t)trial * a.log_cap : nullptr, a.log_cap,
                              reinterpret_cast<k2::WarpSmem*>(sm.tbuf[0]), a.seg ? a.src_radius + trial : a.src_radius,
                              a.coherent_step, a.n_active,
                              a.stamps ? a.stamps + (size_t)gridDim.x * kStampSlots : nullptr);
+        if constexpr (kSeq) {                     // (a.n_active is null here: the advance counts finished lanes)
+            __syncwarp();
+            if (lane == 0 && st->done) advance_frame(a.seq, A.state, ys, trial);
+        }
         DCREG_STAMP(8);
         if (a.stamps && tid == 0) a.stamps[(size_t)gridDim.x * kStampSlots + 15] = blockIdx.x;      // which block was last
     }
@@ -611,11 +699,12 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
 // kernel reads it
 constexpr size_t kIter2SmemNoGrid = offsetof(Iter2Smem, grid);
 
-template <bool kUseWd, bool kGrids>
+template <bool kUseWd, bool kGrids, bool kSeq>
 cudaError_t loop_kernel_attributes(size_t smem) {
-    cudaError_t e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids, kSeq>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)smem);
     if (e == cudaSuccess)
-        e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids>, cudaFuncAttributePreferredSharedMemoryCarveout,
+        e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids, kSeq>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                  cudaSharedmemCarveoutMaxShared);
     return e;
 }
@@ -634,17 +723,25 @@ struct K2Scratch {
 
 // One warp per trial (blockIdx.x): acc_all [B][kAcc], st_all [B], log_all [B][log_cap].  scratch (rehearsal) only for B = 1.
 // radius_per_trial: src_radius is [B] (a batch of different scans) instead of one value for every trial.
+// seq.cursor set (sequences of frames): blockIdx.x is a lane with acc_all [lanes][kAcc]; its trial is the frame it runs
+// now, and the step that stops a frame advances the lane (no rehearsal: scratch is null)
 __global__ void __launch_bounds__(32) k2_step_kernel(const double* acc_all, IcpState* st_all, dcreg_icp_params prm,
                                                      dcreg_iter_log* log_all, int log_cap, const float* src_radius,
                                                      double coherent_step, K2Scratch* scratch, unsigned int* n_active,
-                                                     int radius_per_trial) {
+                                                     int radius_per_trial, SeqView seq) {
     __shared__ k2::WarpSmem sm;
     pdl_release();
     const int lane = threadIdx.x;
     const double* acc = acc_all + (size_t)blockIdx.x * kAcc;
-    IcpState* st = st_all + blockIdx.x;
-    dcreg_iter_log* log = log_all ? log_all + (size_t)blockIdx.x * log_cap : nullptr;
-    if (src_radius && radius_per_trial) src_radius += blockIdx.x;
+    int trial = (int)blockIdx.x;
+    if (seq.cursor) {
+        pdl_wait();                                       // the cursor comes from the previous launch's advance
+        trial = seq.cursor[blockIdx.x];
+        if (trial >= seq.first[blockIdx.x + 1]) return;
+    }
+    IcpState* st = st_all + trial;
+    dcreg_iter_log* log = log_all ? log_all + (size_t)trial * log_cap : nullptr;
+    if (src_radius && radius_per_trial) src_radius += trial;
     const double max_step = coherent_step * prm.search_radius;
     const bool warp_path = prm.detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm.handling == DCREG_HAND_PRECONDITIONED_CG;
 #pragma unroll 1
@@ -671,6 +768,7 @@ __global__ void __launch_bounds__(32) k2_step_kernel(const double* acc_all, IcpS
         __syncwarp();
         if (pass == 1 && scratch) scratch->acc_prev[lane] = acc[lane];              // kAcc == 32: next launch's rehearsal input
         if (pass == 1 && lane == 0 && n_active && st->done) atomicSub(n_active, 1u);
+        if (pass == 1 && lane == 0 && seq.cursor && st->done) advance_frame(seq, st_all, (int)blockIdx.x, trial);
     }
 }
 
@@ -793,23 +891,13 @@ __global__ void flush_l2_kernel(float4* buf, long long n, float v) {
 }
 
 // one thread per trial: T = [n_trials][16] row-major 4x4 initial poses.  seg (a batch of scans, Iter2Args::seg): trial b
-// has seg[b+1] - seg[b] source points instead of n_total
+// has seg[b+1] - seg[b] source points instead of n_total.  running: the start value of n_active (trials, or lanes)
 __global__ void init_state_kernel(IcpState* states, const double* T, long long n_total, unsigned int* counters, int n_trials,
-                                  unsigned int* n_active, const long long* seg) {
+                                  unsigned int* n_active, const long long* seg, int running) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b == 0 && n_active) *n_active = (unsigned)n_trials;
+    if (b == 0 && n_active) *n_active = (unsigned)running;
     if (b >= n_trials) return;
-    IcpState* st = states + b;
-    const double* Tb = T + (size_t)b * 16;
-    for (int r = 0; r < 3; ++r) {
-        for (int c = 0; c < 3; ++c) st->R[r * 3 + c] = Tb[r * 4 + c];
-        st->t[r] = Tb[r * 4 + 3];
-    }
-    st->iter = 0; st->done = 0; st->converged = 0; st->status = DCREG_OK;
-    for (int i = 0; i < 36; ++i) st->H_last[i] = (i % 7 == 0) ? 1.0 : 0.0;
-    st->n_source_total = seg ? seg[b + 1] - seg[b] : n_total;
-    st->step_rot = 1.0e30; st->step_trans = 1.0e30; st->seeds = 0; st->coherent_used = 0; st->coherent = 0; st->warm = 0;
-    st->t_last = k2::globaltimer_ns();                      // tic of iteration 0 (icp_test_runner.cpp:1695)
+    init_loop_state(states + b, T + (size_t)b * 16, seg ? seg[b + 1] - seg[b] : n_total);
     counters[b] = 0u;
 }
 
@@ -912,6 +1000,10 @@ struct dcreg_ctx {
     unsigned long long* d_scan_keys = nullptr; int* d_scan_vals = nullptr;                   // [2][scan_cap]: sort in / out
     void* d_scan_sort_tmp = nullptr; size_t scan_sort_tmp_bytes = 0;
     long long* d_scan_seg = nullptr; float* d_scan_radius = nullptr; double* d_scan_cov = nullptr; int scans_cap = 0;
+    // sequences of frames (dcreg_icp_run_sequences; the frames use the scans' buffers): lane cursors and frame ranges
+    // [lanes] / [lanes + 1], increments and priors [frames][16]
+    int* d_seq_cursor = nullptr; int* d_seq_first = nullptr; int seq_lanes_cap = 0;
+    double* d_seq_delta = nullptr; double* d_seq_prior = nullptr; int seq_frames_cap = 0;
     // Grow-only arenas of dense grids (build_grid_arena): the context's target (one cloud; `grid` points into it), the
     // targets of dcreg_icp_run_pairs (the context's target and grid stay as they were), and the grids over the aligned
     // sources of the point-to-point metrics
@@ -1244,7 +1336,8 @@ int dcreg_destroy(dcreg_ctx* ctx) {
                     ctx->d_state, ctx->d_log, ctx->d_small, ctx->d_analysis, ctx->d_flush, ctx->d_nn, ctx->d_plane_cache, ctx->d_fit_state, ctx->d_iter_stats, ctx->d_src_radius, ctx->d_plane_key, ctx->d_k2_scratch,
                     ctx->d_row_flags, ctx->d_row_epoch, ctx->d_warm_state, ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_keys,
                     ctx->d_scan_vals, ctx->d_scan_sort_tmp, ctx->d_scan_seg, ctx->d_scan_radius, ctx->d_scan_cov,
-                    ctx->d_pair_tgt, ctx->d_pair_tgt_seg, ctx->d_pair_T, ctx->d_aligned};
+                    ctx->d_pair_tgt, ctx->d_pair_tgt_seg, ctx->d_pair_T, ctx->d_aligned, ctx->d_seq_cursor, ctx->d_seq_first,
+                    ctx->d_seq_delta, ctx->d_seq_prior};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     ctx->tgt_arena.free_all();
@@ -1638,6 +1731,11 @@ struct ScanBatch {
     const int* cell_off = nullptr;          // device [n + 1]: first global cell of each grid in the arena
     long long cells = 0;                    // dense cells of all grids
     double cell_size = 0.0;
+    // sequences of frames (dcreg_icp_run_sequences): the scans are frames, run one after another in `lanes` lanes
+    // (seq.cursor set; seq.seg = seg), at most max_bodies loop bodies in all
+    int lanes = 0;
+    long long max_bodies = 0;
+    SeqView seq{};
 };
 
 static int ensure_scans(dcreg_ctx* ctx, int n_scans, long long total) {
@@ -1806,13 +1904,17 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         // (a CUDA graph of the loop freezes this pointer, not the table: the entries are rewritten before every pairs call
         // and read at every launch, and a regrown table has a new pointer and so a new graph key)
         b.grids = pairs ? scans->grids : nullptr;
-        b.n_active = ctx->d_n_active;
+        // sequences: trials = lanes; the frame advance, not the solve step, counts the lanes still running
+        b.seq = scans ? scans->seq : SeqView{};
+        b.n_active = b.seq.cursor ? nullptr : ctx->d_n_active;
         if (ctx->peer_ok) b.peer = ctx->peer_view;
         if (!ctx->loop_attr_done) {          // per device (= per context), not per process
-            CK((loop_kernel_attributes<true, false>)(kIter2SmemNoGrid));
-            CK((loop_kernel_attributes<false, false>)(kIter2SmemNoGrid));
-            CK((loop_kernel_attributes<true, true>)(sizeof(Iter2Smem)));
-            CK((loop_kernel_attributes<false, true>)(sizeof(Iter2Smem)));
+            CK((loop_kernel_attributes<true, false, false>)(kIter2SmemNoGrid));
+            CK((loop_kernel_attributes<false, false, false>)(kIter2SmemNoGrid));
+            CK((loop_kernel_attributes<true, true, false>)(sizeof(Iter2Smem)));
+            CK((loop_kernel_attributes<false, true, false>)(sizeof(Iter2Smem)));
+            CK((loop_kernel_attributes<true, false, true>)(kIter2SmemNoGrid));
+            CK((loop_kernel_attributes<false, false, true>)(kIter2SmemNoGrid));
             ctx->loop_attr_done = true;
         }
     } else {
@@ -1832,11 +1934,14 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
         ctx->nn_valid = true;
         const dim3 grid((unsigned)L.grid_x, (unsigned)L.trials);
         if (L.b.grids) {
-            if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
-            else CK(launch_pdl(icp_iter2_kernel<false, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+            if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, false>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+            else CK(launch_pdl(icp_iter2_kernel<false, true, false>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+        } else if (L.b.seq.cursor) {
+            if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+            else CK(launch_pdl(icp_iter2_kernel<false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
         } else {
-            if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-            else CK(launch_pdl(icp_iter2_kernel<false, false>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+            if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, false>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+            else CK(launch_pdl(icp_iter2_kernel<false, false, false>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
         }
     } else {
         if (L.use_wd) icp_iteration_kernel<true><<<L.grid_x, kBlock, 0, ctx->stream>>>(L.a);
@@ -1848,12 +1953,14 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
 }
 
 // the separate solve kernel (one warp per trial): baseline methods, hash-grid / seam paths, NCCL fallback of a sharded run
-// scan_radius: the per-scan lever arms of a batch of scans (ScanBatch::radius), or null (the context's source)
+// scan_radius: the per-scan lever arms of a batch of scans (ScanBatch::radius), or null (the context's source).
+// seq: the sequences of a dcreg_icp_run_sequences call (trials = lanes), or null
 static int launch_k2(dcreg_ctx* ctx, const dcreg_icp_params* prm, dcreg_iter_log* dlog, int log_cap, int trials = 1,
-                     const float* scan_radius = nullptr) {
+                     const float* scan_radius = nullptr, const SeqView* seq = nullptr) {
     CK(launch_pdl(k2_step_kernel, dim3((unsigned)trials), dim3(32), 0, ctx->stream, (const double*)ctx->d_acc, ctx->d_state, *prm,
                   dlog, log_cap, scan_radius ? scan_radius : (const float*)ctx->d_src_radius, coherent_step_setting(),
-                  trials == 1 ? ctx->d_k2_scratch : (K2Scratch*)nullptr, ctx->d_n_active, scan_radius ? 1 : 0));
+                  trials == 1 && !seq ? ctx->d_k2_scratch : (K2Scratch*)nullptr, seq ? nullptr : ctx->d_n_active,
+                  scan_radius ? 1 : 0, seq ? *seq : SeqView{}));
     ctx->launches++;
     return DCREG_OK;
 }
@@ -1864,18 +1971,22 @@ static int launch_body(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_params* prm,
     if (rc) return rc;
     if (with_k2 && !L.fold_k2) {
         if ((rc = nccl_allreduce_acc(ctx))) return rc;          // no-op on one GPU / with peer mailboxes
-        if ((rc = launch_k2(ctx, prm, dlog, log_cap, L.trials, L.b.seg ? L.b.src_radius : nullptr))) return rc;
+        if ((rc = launch_k2(ctx, prm, dlog, log_cap, L.trials, L.b.seg ? L.b.src_radius : nullptr,
+                            L.b.seq.cursor ? &L.b.seq : nullptr)))
+            return rc;
     }
     return DCREG_OK;
 }
 
-static int init_state(dcreg_ctx* ctx, const double* T, int trials = 1, const long long* scan_seg = nullptr) {
+// running: the start value of the running-trials counter n_active (0: trials)
+static int init_state(dcreg_ctx* ctx, const double* T, int trials = 1, const long long* scan_seg = nullptr, int running = 0) {
     ctx->nn_valid = false;            // a new run: no neighbours of a previous iteration to seed the search with
     int rc = ensure_trials(ctx, trials);
     if (rc) return rc;
     CK(cudaMemcpyAsync(ctx->d_T_init, T, (size_t)trials * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     init_state_kernel<<<(trials + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_state, ctx->d_T_init, ctx->n_src_total, ctx->d_counter,
-                                                                   trials, ctx->d_n_active, scan_seg);
+                                                                   trials, ctx->d_n_active, scan_seg,
+                                                                   running > 0 ? running : trials);
     ctx->launches++;
     CK(cudaGetLastError());
     return DCREG_OK;
@@ -2209,26 +2320,36 @@ static int run_loop(dcreg_ctx* ctx, const dcreg_icp_params* params, int trials, 
     if (log && log_cap > 0 && (rc = ensure_log(ctx, (long long)trials * log_cap))) return rc;
     dcreg_iter_log* dlog = (log && log_cap > 0) ? ctx->d_log : nullptr;
     if (dlog) CK(cudaMemsetAsync(dlog, 0, (size_t)trials * log_cap * sizeof(dcreg_iter_log), ctx->stream));   // aborted iterations leave fields untouched
-    if ((rc = init_state(ctx, T_init, trials, scans ? scans->seg : nullptr))) return rc;
+    // sequences (scans->seq.cursor set): the trials are the frames, the launches' grid y the lanes
+    const bool chain = scans && scans->seq.cursor;
+    const int lanes = chain ? scans->lanes : trials;
+    if ((rc = init_state(ctx, T_init, trials, scans ? scans->seg : nullptr, lanes))) return rc;
+    if (chain)         // a lane's first prior is its T_init; the frame advance writes the others
+        CK(cudaMemcpyAsync(scans->seq.T_prior, ctx->d_T_init, (size_t)trials * 16 * sizeof(double), cudaMemcpyDeviceToDevice,
+                           ctx->stream));
     const float4* src_iter = ctx->d_src;
     if (scans) rc = upload_scans_sorted(ctx, *scans, &src_iter);              // each scan under its own initial pose
     else rc = sort_source_by_cell(ctx, T_init, &src_iter);                    // locality only: any pose of the batch will do
     if (rc) return rc;
     LoopPlan L;
-    if ((rc = plan_iteration(ctx, params, src_iter, nullptr, trials, dlog, dlog ? log_cap : 0, true, &L, scans))) return rc;
+    if ((rc = plan_iteration(ctx, params, src_iter, nullptr, lanes, dlog, dlog ? log_cap : 0, true, &L, scans))) return rc;
     if ((rc = ensure_pinned(ctx, (size_t)trials * sizeof(IcpState)))) return rc;
     // fixed iteration count: the whole run is one chunk; otherwise chunks of 16 with a peek at the number of running
-    // trials in between (the only host sync inside a run; iterations past convergence exit at once on the device)
-    const int chunk = params->fixed_iterations ? (params->max_iterations < 64 ? params->max_iterations : 64) : 16;
-    int issued = 0;
-    while (issued < params->max_iterations) {
-        int todo = params->max_iterations - issued;
+    // trials in between (the only host sync inside a run; iterations past convergence exit at once on the device).
+    // Sequences: chunks of 16 with a peek at the lanes still running, up to max_bodies (a frame never needs more than
+    // max_iterations bodies), whatever fixed_iterations says
+    const long long cap = chain ? scans->max_bodies : params->max_iterations;
+    const bool peek = fetch && (chain || !params->fixed_iterations);
+    const int chunk = params->fixed_iterations && !chain ? (params->max_iterations < 64 ? params->max_iterations : 64) : 16;
+    long long issued = 0;
+    while (issued < cap) {
+        long long todo = cap - issued;
         if (todo > chunk) todo = chunk;
         // a captured chunk is always `chunk` bodies long (one graph per run shape); bodies past max_iterations exit at once
-        const int bodies = (todo < chunk && issued > 0) ? chunk : todo;
+        const int bodies = (todo < chunk && issued > 0) ? chunk : (int)todo;
         if ((rc = enqueue_iterations(ctx, L, params, dlog, dlog ? log_cap : 0, bodies))) return rc;
         issued += bodies;
-        if (fetch && issued < params->max_iterations && !params->fixed_iterations) {
+        if (peek && issued < cap) {
             unsigned int* flag = (unsigned int*)ctx->h_pinned;       // trials still running (every solve step that finishes one decrements it)
             CK(cudaMemcpyAsync(flag, ctx->d_n_active, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
             CK(cudaStreamSynchronize(ctx->stream));
@@ -2323,6 +2444,7 @@ static int run_sources(dcreg_ctx* ctx, const dcreg_icp_params* params, ScanBatch
     if (rc) return rc;
     CK(cudaMemcpyAsync(ctx->d_scan_seg, offsets, (size_t)(S.n + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
     S.seg = ctx->d_scan_seg; S.radius = ctx->d_scan_radius;
+    S.seq.seg = S.seg;                                  // (read only by sequences)
     std::vector<int> st_local;
     if (!status) { st_local.resize(S.n); status = st_local.data(); }
     if ((rc = run_loop(ctx, params, S.n, T_init, T_out, log, log_cap, n_iterations, converged, status, true, &S))) return rc;
@@ -2356,6 +2478,95 @@ int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_sc
     CK(cudaSetDevice(ctx->device));
     return run_sources(ctx, params, ScanBatch{n_scans, xyz, stride}, scan_offsets, T_init, T_out, n_iterations, converged,
                        status, cov, log, log_cap);
+}
+
+// the sequences' own device buffers (dcreg_icp_run_sequences): lane cursors and frame ranges, increments, priors
+static int ensure_sequences(dcreg_ctx* ctx, int n_seqs, int n_frames) {
+    if (ctx->seq_lanes_cap < n_seqs) {
+        if (ctx->d_seq_cursor) cudaFree(ctx->d_seq_cursor);
+        if (ctx->d_seq_first) cudaFree(ctx->d_seq_first);
+        ctx->d_seq_cursor = nullptr; ctx->d_seq_first = nullptr; ctx->seq_lanes_cap = 0;
+        CK(cudaMalloc(&ctx->d_seq_cursor, (size_t)n_seqs * sizeof(int)));
+        CK(cudaMalloc(&ctx->d_seq_first, (size_t)(n_seqs + 1) * sizeof(int)));
+        ctx->seq_lanes_cap = n_seqs;
+    }
+    if (ctx->seq_frames_cap < n_frames) {
+        if (ctx->d_seq_delta) cudaFree(ctx->d_seq_delta);
+        if (ctx->d_seq_prior) cudaFree(ctx->d_seq_prior);
+        ctx->d_seq_delta = nullptr; ctx->d_seq_prior = nullptr; ctx->seq_frames_cap = 0;
+        CK(cudaMalloc(&ctx->d_seq_delta, (size_t)n_frames * 16 * sizeof(double)));
+        CK(cudaMalloc(&ctx->d_seq_prior, (size_t)n_frames * 16 * sizeof(double)));
+        ctx->seq_frames_cap = n_frames;
+    }
+    return DCREG_OK;
+}
+
+int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                            int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                            const double* T_init, const double* deltas, double* T_prior, double* T_out,
+                            int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
+                            int log_cap) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!params || n_seqs <= 0 || n_frames <= 0 || !seq_offsets || !xyz || !frame_offsets || !T_init || !T_out) {
+        ctx->err = "icp_run_sequences: null pointer, n_seqs <= 0 or n_frames <= 0";
+        return DCREG_BAD_ARG;
+    }
+    if (stride < 3) { ctx->err = "icp_run_sequences: stride < 3"; return DCREG_BAD_ARG; }
+    if (ctx->comm) { ctx->err = "icp_run_sequences: sequences are independent - give each rank its own, do not shard them"; return DCREG_BAD_ARG; }
+    int rc = check_run_args(ctx, params, false);
+    if (rc) return rc;
+    if (params->max_iterations < 1) { ctx->err = "icp_run_sequences: max_iterations must be >= 1"; return DCREG_BAD_ARG; }
+    if (!ctx->grid.dense) {
+        ctx->err = "icp_run_sequences: sequences need the dense target grid (target bounding box / cell size too large for it)";
+        return DCREG_BAD_ARG;
+    }
+    if ((rc = check_batch(ctx, n_frames, frame_offsets, "icp_run_sequences: frame"))) return rc;
+    {   // the sequence table: n_seqs + 1 entries from 0, ascending strictly (no empty sequence), up to n_frames
+        std::string why;
+        if (seq_offsets[0] != 0) why = "icp_run_sequences: seq_offsets must start at 0";
+        for (int s = 0; s < n_seqs && why.empty(); ++s)
+            if (seq_offsets[s + 1] <= seq_offsets[s])
+                why = "icp_run_sequences: sequence " + std::to_string(s) + " is empty (seq_offsets must ascend strictly)";
+        if (why.empty() && seq_offsets[n_seqs] != n_frames)
+            why = "icp_run_sequences: seq_offsets[n_seqs] = " + std::to_string(seq_offsets[n_seqs]) + " but n_frames = " +
+                  std::to_string(n_frames);
+        if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
+    }
+    CK(cudaSetDevice(ctx->device));
+    // every frame is sorted by target cell under its dead-reckoned prior (T_init composed with the increments alone):
+    // the sort only buys locality, and the chained prior is not known before the frame before it has run
+    static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    std::vector<double> T_dr((size_t)n_frames * 16);
+    long long max_bodies = 0;
+    for (int s = 0; s < n_seqs; ++s) {
+        const int f0 = seq_offsets[s], f1 = seq_offsets[s + 1];
+        memcpy(&T_dr[(size_t)f0 * 16], T_init + (size_t)s * 16, 16 * sizeof(double));
+        for (int f = f0 + 1; f < f1; ++f) {
+            const double* T = &T_dr[(size_t)(f - 1) * 16];
+            const double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]}, t[3] = {T[3], T[7], T[11]};
+            compose_prior(R, t, deltas ? deltas + (size_t)(f - 1) * 16 : kIdentity, &T_dr[(size_t)f * 16]);
+        }
+        max_bodies = std::max<long long>(max_bodies, (long long)(f1 - f0) * params->max_iterations);
+    }
+    if ((rc = ensure_sequences(ctx, n_seqs, n_frames))) return rc;
+    CK(cudaMemcpyAsync(ctx->d_seq_first, seq_offsets, (size_t)(n_seqs + 1) * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_seq_cursor, seq_offsets, (size_t)n_seqs * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    if (deltas)
+        CK(cudaMemcpyAsync(ctx->d_seq_delta, deltas, (size_t)n_frames * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    ScanBatch S{n_frames, xyz, stride};
+    S.lanes = n_seqs;
+    S.max_bodies = max_bodies;
+    S.seq.cursor = ctx->d_seq_cursor; S.seq.first = ctx->d_seq_first; S.seq.delta = deltas ? ctx->d_seq_delta : nullptr;
+    S.seq.T_prior = ctx->d_seq_prior; S.seq.n_active = ctx->d_n_active;
+    if ((rc = run_sources(ctx, params, S, frame_offsets, T_dr.data(), T_out, n_iterations, converged, status, cov, log,
+                          log_cap)))
+        return rc;
+    if (T_prior) {
+        CK(cudaMemcpyAsync(T_prior, ctx->d_seq_prior, (size_t)n_frames * 16 * sizeof(double), cudaMemcpyDeviceToHost,
+                           ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    return DCREG_OK;
 }
 
 // the pairs' own device buffers (dcreg_icp_run_pairs): packed targets, target offsets, final poses

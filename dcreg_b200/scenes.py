@@ -4,6 +4,7 @@ C2  make_cylinder : the shipped cylinder's geometry (wall R = 40 m, z in [0, 20]
 C3  make_parking  : ground-dominated local map + sparse verticals, LiDAR-like frame (stand-in, pair not shipped)
     make_parking_frames : the same map and a sequence of frames along a path through it (batched localisation)
     make_parking_pairs  : frame k+1 of that path against the local submap around pose k (scan/target pairs)
+    make_parking_sequence : those frames with drifting odometry increments (sequences with chained priors)
 C4  make_corridor : two parallel walls + floor + ceiling, rank-deficient along x
 C5  trial_poses   : seeded perturbations t ~ U[-1, 1]^3 m, rpy ~ U[-3, 3]^3 deg for the Monte-Carlo (SURVEY.md §8d)
     load_pcd_xyz  : PCD v0.7 `DATA binary` with float32 fields (the shipped clouds, SURVEY.md Appendix B.3)
@@ -147,6 +148,26 @@ def make_parking_pairs(n_pairs, seed=53, n_map=500_000, n_scan=6_000, map_seed=4
         T_true.append(Tk)
         T_init.append(Tk @ pose6d_to_matrix(*(mag * rng.choice([-1.0, 1.0], 6))))
     return frames[1:], targets, np.array(T_true), np.array(T_init)
+
+
+def make_parking_sequence(n_frames, seed=47, odo_sigma=(0.03, 0.3), n_map=500_000, n_scan=6_000, map_seed=43,
+                          extent=60.0, max_range=30.0, path_half_length=20.0):
+    """A localisation sequence: the frames and true poses of make_parking_frames(n_frames, seed, ...) with the odometry
+    a front end would feed dcreg_icp_run_sequences.  deltas[k] = inv(T_k) T_{k+1} times a seeded perturbation (each
+    translation axis ~ N(0, odo_sigma[0]) m, each roll / pitch / yaw ~ N(0, odo_sigma[1]) deg), so that composing the
+    increments alone (dead reckoning) drifts; the last entry is the identity (unused).  T_init0 = T_true[0] times the
+    icp_pk01.yaml offsets with random signs, as in make_parking_frames.  Returns (frames: list of (N_k, 3) float32,
+    T_true (n, 4, 4), T_init0 (4, 4), deltas (n, 4, 4), map (n_map, 3) float32)."""
+    frames, T_true, T_init, tgt = make_parking_frames(n_frames, seed=seed, n_map=n_map, n_scan=n_scan, map_seed=map_seed,
+                                                      extent=extent, max_range=max_range,
+                                                      path_half_length=path_half_length)
+    rng = np.random.default_rng([seed, 2])
+    d = math.pi / 180.0
+    deltas = np.tile(np.eye(4), (n_frames, 1, 1))
+    for k in range(n_frames - 1):
+        e = np.concatenate([rng.normal(0.0, odo_sigma[0], 3), rng.normal(0.0, odo_sigma[1] * d, 3)])
+        deltas[k] = np.linalg.inv(T_true[k]) @ T_true[k + 1] @ pose6d_to_matrix(*e)
+    return frames, T_true, T_init[0], deltas, tgt
 
 
 def trial_poses(n, seed=45, max_trans=1.0, max_rot_deg=3.0):

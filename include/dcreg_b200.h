@@ -256,6 +256,37 @@ int dcreg_icp_run_pairs(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_pa
                         double cell_size, const double* T_init, double* T_out, int* n_iterations, int* converged,
                         int* status, double* cov, double error_threshold, double* metrics, dcreg_iter_log* log,
                         int log_cap);
+/* S independent SEQUENCES OF FRAMES against the context's target (map-based localisation: frame k+1 starts from frame
+ * k's registered pose composed with the odometry increment between the two).  Inside a sequence the frames run strictly
+ * one after another, entirely on the device: frame k+1's initial pose is T_out[k] * delta[k], composed on the device when
+ * frame k stops (converged, max_iterations reached or aborted), with no host round trip in between.  Different sequences
+ * run side by side (the loop kernel's grid y).
+ * xyz / frame_offsets / stride: all frames concatenated in HOST memory, as in dcreg_icp_run_scans (n_frames + 1 entries,
+ * ascending strictly from 0: no empty frame; at most 2^29 - 1 points and 65535 frames in one call).
+ * seq_offsets: n_seqs + 1 ascending ints over the frames (0 .. n_frames); sequence s is frames
+ * [seq_offsets[s], seq_offsets[s+1]), and every sequence has at least one frame.
+ * T_init: n_seqs row-major 4x4 poses, the prior of each sequence's first frame.  deltas: n_frames row-major 4x4
+ * increments (entry k maps frame k's result to frame k+1's prior; the entry of a sequence's last frame is ignored), or
+ * NULL for identity (the constant-position model).  T_prior (out, may be NULL): n_frames x 16, the prior each frame
+ * actually started from.  T_out / n_iterations / converged / status / cov / log: one per frame, as in
+ * dcreg_icp_run_scans (status[k] = what dcreg_icp_run returns for frame k alone from T_prior[k]).
+ * - Abort and non-convergence do not stop a sequence: the next prior is composed from the pose the frame returned (on an
+ *   abort the last pose, as dcreg_icp_run leaves it); the caller sees it in status / converged.
+ * - Composition rule: R' = R R_delta, t' = R t_delta + t in FP64, every entry rounded as ((a0 b0 + a1 b1) + a2 b2), then
+ *   + t, with no FMA contraction and no re-orthonormalisation.  dcreg_b200.api.compose_prior reproduces the bits.
+ * - Each frame is sorted by target cell under its dead-reckoned prior (T_init composed with the increments alone), so a
+ *   frame differs from dcreg_set_source(frame k) + dcreg_icp_run(T_prior[k]) only in how the FP64 partial sums are
+ *   grouped (counts, masks and iteration counts identical, poses equal to rounding); a call reproduces bit for bit.
+ * - Device memory grows with the points of the call (about 100 B per point, as for scans): process a long recording in
+ *   calls of a few thousand frames, each call's T_init being the previous call's last T_out * delta.
+ * The frames go to buffers of their own: the context's source and what dcreg_icp_run, trial batches and scan batches
+ * compute are left as they were.  Needs max_iterations >= 1 and the dense grid; not available on a sharded context
+ * (give every rank its own sequences).  Errors: DCREG_BAD_ARG with dcreg_last_error, as dcreg_icp_run_scans. */
+int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                            int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                            const double* T_init, const double* deltas, double* T_prior, double* T_out,
+                            int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
+                            int log_cap);
 /* Same loop, but correspondences are supplied by the caller each iteration through a callback
  * (host kd-tree mode, "PR1"): planes are 4*n doubles (nx,ny,nz,d), all-zero = none. */
 typedef int (*dcreg_plane_callback)(void* user, const double T[16], double* planes4,
