@@ -4,7 +4,9 @@ The product is the sm_90a CUDA library ``libdcreg_b200.so`` behind the C ABI in 
 this package is its thin ctypes host binding.  There is no CPU fallback.
 """
 from .api import (Context, DcregError, IcpParams, Analysis, IterLog, default_params, load_library, DET, HAND, STATUS,
-                  LIB_PATH, EXPORTS, pose_Rt, compose_prior)
+                  LIB_PATH, EXPORTS, pose_Rt, compose_prior, map_points,
+                  constant_velocity_increment)
 
 __all__ = ["Context", "DcregError", "IcpParams", "Analysis", "IterLog", "default_params", "load_library", "DET",
-           "HAND", "STATUS", "LIB_PATH", "EXPORTS", "pose_Rt", "compose_prior"]
+           "HAND", "STATUS", "LIB_PATH", "EXPORTS", "pose_Rt", "compose_prior", "map_points",
+           "constant_velocity_increment"]

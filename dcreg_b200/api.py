@@ -87,7 +87,7 @@ EXPORTS = [
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -130,6 +130,9 @@ def load_library():
     lib.dcreg_icp_run_sequences.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
                                             C.POINTER(i64), ci, dp, dp, dp, dp, C.POINTER(ci), C.POINTER(ci), C.POINTER(ci),
                                             dp, C.POINTER(IterLog), ci]
+    lib.dcreg_icp_run_odometry.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
+                                           C.POINTER(i64), ci, C.c_double, ci, ci, dp, dp, dp, dp, C.POINTER(ci),
+                                           C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(IterLog), ci]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -203,6 +206,34 @@ def compose_prior(T, D):
             col = col + T[..., :3, 3]
         out[..., :3, c] = col
     out[..., 3, 3] = 1.0
+    return out
+
+
+def map_points(T, P):
+    """The local-map points of dcreg_icp_run_odometry, bit for bit as the device transforms them: frame points P (N, >=3)
+    float32 under the pose T (4, 4), each coordinate ((r0 x + r1 y) + r2 z) + t in FP64 with one rounding per operation
+    (elementwise NumPy ops, no matmul, no FMA), then one float32 rounding.  Returns (N, 3) float32."""
+    T = np.asarray(T, dtype=np.float64)
+    P = np.asarray(P, dtype=np.float32)[:, :3].astype(np.float64)
+    out = np.empty((P.shape[0], 3), dtype=np.float32)
+    for r in range(3):
+        out[:, r] = (((T[r, 0] * P[:, 0] + T[r, 1] * P[:, 1]) + T[r, 2] * P[:, 2]) + T[r, 3]).astype(np.float32)
+    return out
+
+
+def constant_velocity_increment(T_prev, T):
+    """The constant-velocity increment of dcreg_icp_run_odometry, inv(T_prev) T, bit for bit as the device forms it:
+    R_D = R_prev^T R, t_D = R_prev^T (t - t_prev), the differences rounded first, every entry ((a0 b0 + a1 b1) + a2 b2)
+    in FP64 with one rounding per operation.  T_prev, T: (4, 4); returns (4, 4) with the row [0, 0, 0, 1]."""
+    A = np.asarray(T_prev, dtype=np.float64)
+    B = np.asarray(T, dtype=np.float64)
+    dt = B[:3, 3] - A[:3, 3]
+    out = np.zeros((4, 4))
+    for r in range(3):
+        for c in range(3):
+            out[r, c] = (A[0, r] * B[0, c] + A[1, r] * B[1, c]) + A[2, r] * B[2, c]
+        out[r, 3] = (A[0, r] * dt[0] + A[1, r] * dt[1]) + A[2, r] * dt[2]
+    out[3, 3] = 1.0
     return out
 
 
@@ -474,6 +505,55 @@ class Context:
             xyz.ctypes.data_as(C.POINTER(C.c_float)), offsets.ctypes.data_as(C.POINTER(C.c_int64)), 3, _dptr(T_init),
             _dptr(deltas) if deltas is not None else None, _dptr(T_prior), _dptr(T_out), n_it, conv, st,
             _dptr(cov) if want_cov else None, logs, cap))
+        out = _trial_results(st, conv, n_it, T_out, logs, cap, cov)
+        for r, Tp in zip(out, T_prior):
+            r.T_prior = Tp
+        return out
+
+    def icp_run_odometry(self, params: IcpParams, sequences, T_init, deltas=None, motion: str = "increments",
+                         map_frames: int = 10, cell_size=None, want_log: bool = False, want_cov: bool = False):
+        """Scan-to-map odometry (`sequences`: a list of lists of (N, >=3) point arrays): frame k of a sequence registers
+        against the local map of the frames [k - map_frames, k) before it, each placed at its own registered pose
+        (map_points), starting from compose_prior(frame k-1's result, D).  motion "increments": D = deltas[k-1]
+        (deltas: (n_frames, 4, 4) over all frames in order, or None for identity); "constant_velocity": D =
+        constant_velocity_increment(T_out[k-2], T_out[k-1]) (identity after the anchor; deltas must be None).  The first
+        frame of each sequence is its anchor: not registered, T = T_prior = T_init[s].  cell_size: the maps' grid cell
+        (default search_radius).  Returns a list of IcpResult, one per frame in order, with .T_prior (logs only when
+        want_log, .cov when want_cov).  Needs no target; the context's source and target are left as they were."""
+        models = {"increments": 0, "constant_velocity": 1}
+        if motion not in models:
+            raise ValueError(f"icp_run_odometry: motion must be one of {sorted(models)}, not {motion!r}")
+        lens = [len(s) for s in sequences]
+        S = len(lens)
+        pts = [_as_points(f)[:, :3] for s in sequences for f in s]
+        n = len(pts)
+        seq_off = np.zeros(S + 1, dtype=np.int32)
+        seq_off[1:] = np.cumsum(lens)
+        cell = float(params.search_radius if cell_size is None else cell_size)
+        if S == 0 or n == 0:                            # BAD_ARG from the library, like every other malformed batch
+            self._check(self.lib.dcreg_icp_run_odometry(self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)),
+                                                        0, None, None, 3, cell, int(map_frames), models[motion], None, None,
+                                                        None, None, None, None, None, None, None, 0))
+        xyz = np.ascontiguousarray(np.concatenate(pts, axis=0))
+        offsets = np.zeros(n + 1, dtype=np.int64)
+        offsets[1:] = np.cumsum([p.shape[0] for p in pts])
+        T_init = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
+        if T_init.shape[0] != S:
+            raise ValueError(f"icp_run_odometry: {S} sequences but {T_init.shape[0]} initial poses")
+        if deltas is not None:
+            deltas = np.ascontiguousarray(deltas, dtype=np.float64).reshape(-1, 4, 4)
+            if deltas.shape[0] != n:
+                raise ValueError(f"icp_run_odometry: {n} frames but {deltas.shape[0]} increments")
+        T_prior = np.empty((n, 4, 4)); T_out = np.empty((n, 4, 4))
+        n_it = (C.c_int * n)(); conv = (C.c_int * n)(); st = (C.c_int * n)()
+        cov = np.empty((n, 6, 6)) if want_cov else None
+        cap = int(params.max_iterations) if want_log else 0
+        logs = (IterLog * max(cap * n, 1))() if want_log else None
+        self._check(self.lib.dcreg_icp_run_odometry(
+            self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n,
+            xyz.ctypes.data_as(C.POINTER(C.c_float)), offsets.ctypes.data_as(C.POINTER(C.c_int64)), 3, cell,
+            int(map_frames), models[motion], _dptr(T_init), _dptr(deltas) if deltas is not None else None, _dptr(T_prior),
+            _dptr(T_out), n_it, conv, st, _dptr(cov) if want_cov else None, logs, cap))
         out = _trial_results(st, conv, n_it, T_out, logs, cap, cov)
         for r, Tp in zip(out, T_prior):
             r.T_prior = Tp

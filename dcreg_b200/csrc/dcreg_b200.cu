@@ -33,6 +33,7 @@
 #include "k1_stream.cuh"
 #include "k2_solve.cuh"
 #include "loop_plan.hpp"
+#include "odom_plan.hpp"
 #include "peer_reduce.cuh"
 
 using k2::IcpState;
@@ -144,6 +145,35 @@ __host__ __device__ __forceinline__ void compose_prior(const double* R, const do
 #undef DCREG_MUL
 #undef DCREG_ADD
     T[12] = 0.0; T[13] = 0.0; T[14] = 0.0; T[15] = 1.0;
+}
+
+// The constant-velocity increment of dcreg_icp_run_odometry, D = inv(T_a) T_b for the poses (Ra, ta) of frame k-2 and
+// (Rb, tb) of frame k-1: R_D = Ra^T Rb, t_D = Ra^T (tb - ta), the differences rounded first, every entry
+// ((a0 b0 + a1 b1) + a2 b2) with no FMA contraction (dcreg_b200.api.constant_velocity_increment gives the same bits).
+__host__ __device__ __forceinline__ void constant_velocity_increment(const double* Ra, const double* ta, const double* Rb,
+                                                                     const double* tb, double* D) {
+#ifdef __CUDA_ARCH__
+#define DCREG_MUL(x, y) __dmul_rn(x, y)
+#define DCREG_ADD(x, y) __dadd_rn(x, y)
+#define DCREG_SUB(x, y) __dsub_rn(x, y)
+#else
+#define DCREG_MUL(x, y) ((x) * (y))
+#define DCREG_ADD(x, y) ((x) + (y))
+#define DCREG_SUB(x, y) ((x) - (y))
+#endif
+    const double dt[3] = {DCREG_SUB(tb[0], ta[0]), DCREG_SUB(tb[1], ta[1]), DCREG_SUB(tb[2], ta[2])};
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+            D[4 * r + c] = DCREG_ADD(DCREG_ADD(DCREG_MUL(Ra[r], Rb[c]), DCREG_MUL(Ra[3 + r], Rb[3 + c])),
+                                     DCREG_MUL(Ra[6 + r], Rb[6 + c]));
+        D[4 * r + 3] = DCREG_ADD(DCREG_ADD(DCREG_MUL(Ra[r], dt[0]), DCREG_MUL(Ra[3 + r], dt[1])), DCREG_MUL(Ra[6 + r], dt[2]));
+    }
+#undef DCREG_MUL
+#undef DCREG_ADD
+#undef DCREG_SUB
+    D[12] = 0.0; D[13] = 0.0; D[14] = 0.0; D[15] = 1.0;
 }
 
 // Lane s's frame `frame` has stopped (converged, max_iterations or aborted): start the next frame of the lane from the
@@ -372,7 +402,8 @@ __device__ __noinline__ void solver_block(const Iter2Args& a, IcpState* st, Iter
 
 // kGrids: every trial has its own target grid (Iter2Args::grids), copied into shared memory once per block; the other
 // paths keep reading it.grid from the kernel parameters, untouched by the table.  kSeq: grid y is a sequence lane
-// (Iter2Args::seq) whose trial is the frame it runs now; the reduction's working set is the lane's
+// (Iter2Args::seq) whose trial is the frame it runs now; the reduction's working set is the lane's.  Both (odometry,
+// dcreg_icp_run_odometry): the grid is the lane's, grids[lane], a local map rebuilt before every step
 template <bool kUseWd, bool kGrids, bool kSeq>
 __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_constant__ Iter2Args a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -399,7 +430,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     if constexpr (kGrids) {
         static_assert(sizeof(corr::Grid) % sizeof(int) == 0 && sizeof(corr::Grid) / sizeof(int) <= kBlock, "grid copy");
         if (tid < (int)(sizeof(corr::Grid) / sizeof(int)))
-            reinterpret_cast<int*>(&sm.grid)[tid] = reinterpret_cast<const int*>(a.grids + trial)[tid];
+            reinterpret_cast<int*>(&sm.grid)[tid] = reinterpret_cast<const int*>(a.grids + (kSeq ? ys : trial))[tid];
         __syncthreads();
     }
     const corr::Grid& g = kGrids ? sm.grid : A.grid;
@@ -901,6 +932,56 @@ __global__ void init_state_kernel(IcpState* states, const double* T, long long n
     counters[b] = 0u;
 }
 
+// ---- odometry (dcreg_icp_run_odometry; odom_plan.hpp) ------------------------------------------------------------
+// The local maps of one step: m points in all, piece p (a window frame) being map points [dst[p], dst[p+1]) = the points
+// src[src_at[p] ..] of the frame's packed input (input order) under the frame's final pose, states[frame[p]].  Every
+// coordinate is ((r0 x + r1 y) + r2 z) + t in FP64, one rounding per operation, then one float32 rounding
+// (dcreg_b200.api.map_points gives the same bits); w = the point's index over the step's maps, as a packed target.
+__global__ void map_points_kernel(const float4* __restrict__ src, const long long* __restrict__ dst, int pieces,
+                                  const long long* __restrict__ src_at, const int* __restrict__ frame, long long m,
+                                  const IcpState* __restrict__ states, float4* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const int p = corr::segment_of(dst, pieces, i);
+    const IcpState* st = states + frame[p];
+    const float4 q = src[src_at[p] + (i - dst[p])];
+    const double x = q.x, y = q.y, z = q.z;
+    float v[3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+        v[r] = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(st->R[3 * r], x), __dmul_rn(st->R[3 * r + 1], y)),
+                                          __dmul_rn(st->R[3 * r + 2], z)),
+                                st->t[r]);
+    out[i] = make_float4(v[0], v[1], v[2], __int_as_float((int)i));
+}
+
+// Start of step `step_first` (one thread per lane of `lanes`): lane j < active runs frame step_first + j and nothing
+// after it (its frame range is that one frame, so the frame advance ends the lane), the other lanes run nothing.  The
+// frame's prior is compose_prior(frame k-1's result, D) with D = delta[prev] (or identity), or (constant velocity) the
+// increment from frame k-2 to frame k-1 (identity after the anchor).
+__global__ void odom_start_kernel(IcpState* states, const long long* __restrict__ seg, double* T_prior, int* cursor,
+                                  int* first, unsigned int* n_active, int lanes, int step_first, int active,
+                                  const int* __restrict__ prev, const int* __restrict__ prev2, const double* __restrict__ delta,
+                                  int motion) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j == 0) { *n_active = (unsigned)active; first[lanes] = step_first + active; }
+    if (j >= lanes) return;
+    const int f = step_first + min(j, active);
+    first[j] = f; cursor[j] = f;
+    if (j >= active) return;
+    const IcpState* a = states + prev[j];
+    double D[16] = {1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0};
+    if (motion == DCREG_MOTION_CONSTANT_VELOCITY) {
+        if (prev2[j] >= 0) constant_velocity_increment(states[prev2[j]].R, states[prev2[j]].t, a->R, a->t, D);
+    } else if (delta) {
+        for (int i = 0; i < 16; ++i) D[i] = delta[(size_t)prev[j] * 16 + i];
+    }
+    double T[16];
+    compose_prior(a->R, a->t, D, T);
+    for (int i = 0; i < 16; ++i) T_prior[(size_t)f * 16 + i] = T[i];
+    init_loop_state(states + f, T, seg[f + 1] - seg[f]);
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1004,6 +1085,10 @@ struct dcreg_ctx {
     // [lanes] / [lanes + 1], increments and priors [frames][16]
     int* d_seq_cursor = nullptr; int* d_seq_first = nullptr; int seq_lanes_cap = 0;
     double* d_seq_delta = nullptr; double* d_seq_prior = nullptr; int seq_frames_cap = 0;
+    // odometry (dcreg_icp_run_odometry; the frames use the scans' and the sequences' buffers): every step's tables
+    // (odom_plan.hpp) in one upload, the step's local maps, and their grids in an arena of their own
+    long long* d_odom_ll = nullptr; long long odom_ll_cap = 0; int* d_odom_int = nullptr; long long odom_int_cap = 0;
+    float4* d_odom_map = nullptr; long long odom_map_cap = 0;
     // Grow-only arenas of dense grids (build_grid_arena): the context's target (one cloud; `grid` points into it), the
     // targets of dcreg_icp_run_pairs (the context's target and grid stay as they were), and the grids over the aligned
     // sources of the point-to-point metrics
@@ -1018,7 +1103,7 @@ struct dcreg_ctx {
             *this = GridArena{};
         }
     };
-    GridArena tgt_arena, pair_tgt, aligned;
+    GridArena tgt_arena, pair_tgt, aligned, odom_maps;
     // the hash tables of a target too large for a dense grid (build_hash_grid; points in tgt_arena)
     unsigned long long* d_hash_keys = nullptr; int* d_hash_start = nullptr; int* d_hash_count = nullptr; long long hash_cap = 0;
     float4* d_pair_tgt = nullptr; long long pair_tgt_cap = 0;                    // targets, packed (w = global index)
@@ -1153,12 +1238,27 @@ int ensure_stage(dcreg_ctx* ctx, size_t bytes) {
 
 // host points -> d_out, packed by pack_points_kernel (d_seg: device table of n_seg segments, or null for one; d_radius:
 // [n_seg] per-segment max |p|, or null)
+// order / in_off (odometry): segment b of the device copy is host segment order[b], points [in_off[order[b]], ..) of xyz;
+// null: xyz in order
 int upload_points(dcreg_ctx* ctx, const float* xyz, long long n, int stride, const long long* d_seg, int n_seg,
-                  float4* d_out, float* d_radius) {
+                  float4* d_out, float* d_radius, const int* order = nullptr, const int64_t* in_off = nullptr) {
     const size_t bytes = (size_t)n * stride * sizeof(float);
     const int rc = ensure_stage(ctx, bytes);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_stage, xyz, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (!order) {
+        CK(cudaMemcpyAsync(ctx->d_stage, xyz, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    } else {
+        long long at = 0;                              // one copy per run of segments that are also consecutive on the host
+        for (int b = 0; b < n_seg;) {
+            int e = b + 1;
+            while (e < n_seg && order[e] == order[e - 1] + 1) ++e;
+            const long long a0 = in_off[order[b]], a1 = in_off[order[e - 1] + 1];
+            CK(cudaMemcpyAsync(ctx->d_stage + (size_t)at * stride, xyz + (size_t)a0 * stride,
+                               (size_t)(a1 - a0) * stride * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+            at += a1 - a0;
+            b = e;
+        }
+    }
     if (d_radius) CK(cudaMemsetAsync(d_radius, 0, (size_t)n_seg * sizeof(float), ctx->stream));
     pack_points_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_stage, n, stride, d_seg, n_seg, d_out,
                                                                             d_radius);
@@ -1337,12 +1437,13 @@ int dcreg_destroy(dcreg_ctx* ctx) {
                     ctx->d_row_flags, ctx->d_row_epoch, ctx->d_warm_state, ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_keys,
                     ctx->d_scan_vals, ctx->d_scan_sort_tmp, ctx->d_scan_seg, ctx->d_scan_radius, ctx->d_scan_cov,
                     ctx->d_pair_tgt, ctx->d_pair_tgt_seg, ctx->d_pair_T, ctx->d_aligned, ctx->d_seq_cursor, ctx->d_seq_first,
-                    ctx->d_seq_delta, ctx->d_seq_prior};
+                    ctx->d_seq_delta, ctx->d_seq_prior, ctx->d_odom_ll, ctx->d_odom_int, ctx->d_odom_map};
     for (void* p : ptrs)
         if (p) cudaFree(p);
     ctx->tgt_arena.free_all();
     ctx->pair_tgt.free_all();
     ctx->aligned.free_all();
+    ctx->odom_maps.free_all();
     if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
@@ -1736,6 +1837,13 @@ struct ScanBatch {
     int lanes = 0;
     long long max_bodies = 0;
     SeqView seq{};
+    // odometry (dcreg_icp_run_odometry): scan b is host frame order[b] (points from in_off), and every scan is sorted by
+    // its own cell in the sensor frame: poses sort_T (device [n][16], identities) in the box sort_grid (sort_cells cells)
+    const int* order = nullptr;
+    const int64_t* in_off = nullptr;
+    const double* sort_T = nullptr;
+    corr::Grid sort_grid{};
+    long long sort_cells = 0;
 };
 
 static int ensure_scans(dcreg_ctx* ctx, int n_scans, long long total) {
@@ -1769,18 +1877,23 @@ static int ensure_scans(dcreg_ctx* ctx, int n_scans, long long total) {
 // radix sort of the (scan, cell) keys keeps the segments contiguous and in scan order and needs no per-scan cell tables.
 static int upload_scans_sorted(dcreg_ctx* ctx, const ScanBatch& S, const float4** src_out) {
     const long long n = S.total;
-    int rc = upload_points(ctx, S.xyz, n, S.stride, S.seg, S.n, ctx->d_scan_src, ctx->d_scan_radius);
+    int rc = upload_points(ctx, S.xyz, n, S.stride, S.seg, S.n, ctx->d_scan_src, ctx->d_scan_radius, S.order, S.in_off);
     if (rc) return rc;
     unsigned long long* keys = ctx->d_scan_keys;
     int* vals = ctx->d_scan_vals;
     const unsigned nb = (unsigned)((n + 255) / 256);
-    cell_key_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_scan_src, n, S.seg, S.n, ctx->d_T_init, ctx->grid, ctx->grid_cells,
-                                                 S.grids, S.cell_off, keys, vals);
+    if (S.sort_T)
+        cell_key_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_scan_src, n, S.seg, S.n, S.sort_T, S.sort_grid, S.sort_cells,
+                                                     nullptr, nullptr, keys, vals);
+    else
+        cell_key_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_scan_src, n, S.seg, S.n, ctx->d_T_init, ctx->grid,
+                                                     ctx->grid_cells, S.grids, S.cell_off, keys, vals);
     ctx->launches++;
     CK(cudaGetLastError());
-    // keys below n_scans * cells of the context's grid, or below the arena's cell count (pairs)
-    const unsigned long long key_end = S.grids ? (unsigned long long)S.cells
-                                               : (unsigned long long)S.n * (unsigned long long)ctx->grid_cells;
+    // keys below n_scans * cells of the context's grid (or of the sensor-frame box), or below the arena's cell count (pairs)
+    const unsigned long long key_end = S.sort_T ? (unsigned long long)S.n * (unsigned long long)S.sort_cells
+                                       : S.grids ? (unsigned long long)S.cells
+                                                 : (unsigned long long)S.n * (unsigned long long)ctx->grid_cells;
     int end_bit = 1;
     while (end_bit < 64 && (key_end - 1ull) >> end_bit) ++end_bit;
     size_t tmp = 0;
@@ -1915,6 +2028,8 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
             CK((loop_kernel_attributes<false, true, false>)(sizeof(Iter2Smem)));
             CK((loop_kernel_attributes<true, false, true>)(kIter2SmemNoGrid));
             CK((loop_kernel_attributes<false, false, true>)(kIter2SmemNoGrid));
+            CK((loop_kernel_attributes<true, true, true>)(sizeof(Iter2Smem)));
+            CK((loop_kernel_attributes<false, true, true>)(sizeof(Iter2Smem)));
             ctx->loop_attr_done = true;
         }
     } else {
@@ -1933,7 +2048,10 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
         L.b.use_seeds = ctx->nn_valid ? 1 : 0;
         ctx->nn_valid = true;
         const dim3 grid((unsigned)L.grid_x, (unsigned)L.trials);
-        if (L.b.grids) {
+        if (L.b.grids && L.b.seq.cursor) {
+            if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+            else CK(launch_pdl(icp_iter2_kernel<false, true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+        } else if (L.b.grids) {
             if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, false>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
             else CK(launch_pdl(icp_iter2_kernel<false, true, false>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
         } else if (L.b.seq.cursor) {
@@ -2501,6 +2619,21 @@ static int ensure_sequences(dcreg_ctx* ctx, int n_seqs, int n_frames) {
     return DCREG_OK;
 }
 
+// the sequence table: n_seqs + 1 entries from 0, ascending strictly (no empty sequence), up to n_frames
+static int check_seq_offsets(dcreg_ctx* ctx, int n_seqs, const int* seq_offsets, int n_frames, const char* what) {
+    std::string why;
+    const std::string w(what);
+    if (seq_offsets[0] != 0) why = w + ": seq_offsets must start at 0";
+    for (int s = 0; s < n_seqs && why.empty(); ++s)
+        if (seq_offsets[s + 1] <= seq_offsets[s])
+            why = w + ": sequence " + std::to_string(s) + " is empty (seq_offsets must ascend strictly)";
+    if (why.empty() && seq_offsets[n_seqs] != n_frames)
+        why = w + ": seq_offsets[n_seqs] = " + std::to_string(seq_offsets[n_seqs]) + " but n_frames = " + std::to_string(n_frames);
+    if (why.empty()) return DCREG_OK;
+    ctx->err = why;
+    return DCREG_BAD_ARG;
+}
+
 int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
                             int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
                             const double* T_init, const double* deltas, double* T_prior, double* T_out,
@@ -2521,17 +2654,7 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
         return DCREG_BAD_ARG;
     }
     if ((rc = check_batch(ctx, n_frames, frame_offsets, "icp_run_sequences: frame"))) return rc;
-    {   // the sequence table: n_seqs + 1 entries from 0, ascending strictly (no empty sequence), up to n_frames
-        std::string why;
-        if (seq_offsets[0] != 0) why = "icp_run_sequences: seq_offsets must start at 0";
-        for (int s = 0; s < n_seqs && why.empty(); ++s)
-            if (seq_offsets[s + 1] <= seq_offsets[s])
-                why = "icp_run_sequences: sequence " + std::to_string(s) + " is empty (seq_offsets must ascend strictly)";
-        if (why.empty() && seq_offsets[n_seqs] != n_frames)
-            why = "icp_run_sequences: seq_offsets[n_seqs] = " + std::to_string(seq_offsets[n_seqs]) + " but n_frames = " +
-                  std::to_string(n_frames);
-        if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
-    }
+    if ((rc = check_seq_offsets(ctx, n_seqs, seq_offsets, n_frames, "icp_run_sequences"))) return rc;
     CK(cudaSetDevice(ctx->device));
     // every frame is sorted by target cell under its dead-reckoned prior (T_init composed with the increments alone):
     // the sort only buys locality, and the chained prior is not known before the frame before it has run
@@ -2566,6 +2689,240 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
                            ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
     }
+    return DCREG_OK;
+}
+
+// the odometry's own device buffers (dcreg_icp_run_odometry): every step's tables, one step's local maps
+static int ensure_odometry(dcreg_ctx* ctx, long long n_ll, long long n_int, long long map_points) {
+    if (ctx->odom_ll_cap < n_ll) {
+        if (ctx->d_odom_ll) cudaFree(ctx->d_odom_ll);
+        ctx->d_odom_ll = nullptr; ctx->odom_ll_cap = 0;
+        CK(cudaMalloc(&ctx->d_odom_ll, (size_t)n_ll * sizeof(long long)));
+        ctx->odom_ll_cap = n_ll;
+    }
+    if (ctx->odom_int_cap < n_int) {
+        if (ctx->d_odom_int) cudaFree(ctx->d_odom_int);
+        ctx->d_odom_int = nullptr; ctx->odom_int_cap = 0;
+        CK(cudaMalloc(&ctx->d_odom_int, (size_t)n_int * sizeof(int)));
+        ctx->odom_int_cap = n_int;
+    }
+    if (ctx->odom_map_cap < map_points) {
+        if (ctx->d_odom_map) cudaFree(ctx->d_odom_map);
+        ctx->d_odom_map = nullptr; ctx->odom_map_cap = 0;
+        CK(cudaMalloc(&ctx->d_odom_map, (size_t)map_points * sizeof(float4)));
+        ctx->odom_map_cap = map_points;
+    }
+    return DCREG_OK;
+}
+
+int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                           int n_frames, const float* xyz, const int64_t* frame_offsets, int stride, double cell_size,
+                           int map_frames, int motion, const double* T_init, const double* deltas, double* T_prior,
+                           double* T_out, int* n_iterations, int* converged, int* status, double* cov,
+                           dcreg_iter_log* log, int log_cap) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!params || n_seqs <= 0 || n_frames <= 0 || !seq_offsets || !xyz || !frame_offsets || !T_init || !T_out) {
+        ctx->err = "icp_run_odometry: null pointer, n_seqs <= 0 or n_frames <= 0";
+        return DCREG_BAD_ARG;
+    }
+    if (stride < 3) { ctx->err = "icp_run_odometry: stride < 3"; return DCREG_BAD_ARG; }
+    if (!(cell_size > 0.0)) { ctx->err = "icp_run_odometry: cell_size <= 0"; return DCREG_BAD_ARG; }
+    if (map_frames < 1) { ctx->err = "icp_run_odometry: map_frames must be >= 1"; return DCREG_BAD_ARG; }
+    if (motion != DCREG_MOTION_INCREMENTS && motion != DCREG_MOTION_CONSTANT_VELOCITY) {
+        ctx->err = "icp_run_odometry: motion must be DCREG_MOTION_INCREMENTS or DCREG_MOTION_CONSTANT_VELOCITY";
+        return DCREG_BAD_ARG;
+    }
+    if (motion == DCREG_MOTION_CONSTANT_VELOCITY && deltas) {
+        ctx->err = "icp_run_odometry: the constant-velocity model takes no deltas (pass NULL)";
+        return DCREG_BAD_ARG;
+    }
+    if (ctx->comm) { ctx->err = "icp_run_odometry: sequences are independent - give each rank its own, do not shard them"; return DCREG_BAD_ARG; }
+    int rc = check_run_args(ctx, params, false, false);
+    if (rc) return rc;
+    if (params->max_iterations < 1) { ctx->err = "icp_run_odometry: max_iterations must be >= 1"; return DCREG_BAD_ARG; }
+    const int rings = search_rings(params->search_radius, cell_size);
+    if (rings < 1 || rings > 4) { ctx->err = "icp_run_odometry: search_radius / cell_size must be in (0, 4]"; return DCREG_BAD_ARG; }
+    if ((rc = check_batch(ctx, n_frames, frame_offsets, "icp_run_odometry: frame"))) return rc;
+    if ((rc = check_seq_offsets(ctx, n_seqs, seq_offsets, n_frames, "icp_run_odometry"))) return rc;
+    odom_plan::Plan P;
+    {
+        const std::string why = odom_plan::make(n_seqs, seq_offsets, n_frames, frame_offsets, map_frames,
+                                                arena_plan::kMaxPoints, &P);
+        if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
+    }
+    CK(cudaSetDevice(ctx->device));
+    const int n_steps = (int)P.steps.size();
+    // every step's tables in one upload: long long map_seg [A + 1], piece_dst [P + 1], piece_src [P]; int piece_frame
+    // [P], prev [A], prev2 [A] (A lanes, P window frames)
+    std::vector<long long> hll;
+    std::vector<int> hint;
+    std::vector<size_t> at_ll((size_t)n_steps, 0), at_int((size_t)n_steps, 0);
+    for (int i = 1; i < n_steps; ++i) {
+        const odom_plan::Step& st = P.steps[(size_t)i];
+        at_ll[(size_t)i] = hll.size(); at_int[(size_t)i] = hint.size();
+        hll.insert(hll.end(), st.map_seg.begin(), st.map_seg.end());
+        hll.insert(hll.end(), st.piece_dst.begin(), st.piece_dst.end());
+        hll.insert(hll.end(), st.piece_src.begin(), st.piece_src.end());
+        hint.insert(hint.end(), st.piece_frame.begin(), st.piece_frame.end());
+        hint.insert(hint.end(), st.prev.begin(), st.prev.end());
+        hint.insert(hint.end(), st.prev2.begin(), st.prev2.end());
+    }
+    const long long total = P.dev_off[(size_t)n_frames];
+    if ((rc = ensure_scans(ctx, n_frames, total)) || (rc = ensure_sequences(ctx, n_seqs, n_frames)) ||
+        (rc = ensure_odometry(ctx, std::max<long long>((long long)hll.size(), 1), std::max<long long>((long long)hint.size(), 1),
+                              std::max<long long>(P.max_map, 1))))
+        return rc;
+    if (!hll.empty()) {
+        CK(cudaMemcpyAsync(ctx->d_odom_ll, hll.data(), hll.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->d_odom_int, hint.data(), hint.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    CK(cudaMemcpyAsync(ctx->d_scan_seg, P.dev_off.data(), (size_t)(n_frames + 1) * sizeof(long long), cudaMemcpyHostToDevice,
+                       ctx->stream));
+    // device order: every frame's loop state starts at its sequence's T_init (an anchor keeps it: T_out = T_prior =
+    // T_init, no iteration, not converged), the increments follow the frames
+    std::vector<double> T_dev((size_t)n_frames * 16), ident((size_t)n_frames * 16, 0.0), D_dev;
+    for (int s = 0; s < n_seqs; ++s)
+        for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k)
+            memcpy(&T_dev[(size_t)P.dev[(size_t)k] * 16], T_init + (size_t)s * 16, 16 * sizeof(double));
+    for (int d = 0; d < n_frames; ++d)
+        for (int c = 0; c < 4; ++c) ident[(size_t)d * 16 + 5 * c] = 1.0;
+    if (deltas) {
+        D_dev.resize((size_t)n_frames * 16);
+        for (int k = 0; k < n_frames; ++k) memcpy(&D_dev[(size_t)P.dev[(size_t)k] * 16], deltas + (size_t)k * 16, 16 * sizeof(double));
+        CK(cudaMemcpyAsync(ctx->d_seq_delta, D_dev.data(), D_dev.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    if (log && log_cap > 0 && (rc = ensure_log(ctx, (long long)n_frames * log_cap))) return rc;
+    dcreg_iter_log* dlog = (log && log_cap > 0) ? ctx->d_log : nullptr;
+    if (dlog) CK(cudaMemsetAsync(dlog, 0, (size_t)n_frames * log_cap * sizeof(dcreg_iter_log), ctx->stream));
+    if ((rc = init_state(ctx, T_dev.data(), n_frames, ctx->d_scan_seg, n_seqs))) return rc;
+    // the frames are uploaded in device order and sorted once, each by its own cell in the sensor frame (identity poses,
+    // a box of 1024^3 cells around the sensor: locality only, the chained priors are not known yet)
+    CK(cudaMemcpyAsync(ctx->d_seq_prior, ident.data(), ident.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    ScanBatch S{n_frames, xyz, stride};
+    S.total = total;
+    for (int d = 0; d < n_frames; ++d) S.max_n = std::max<long long>(S.max_n, P.dev_off[(size_t)d + 1] - P.dev_off[(size_t)d]);
+    S.seg = ctx->d_scan_seg; S.radius = ctx->d_scan_radius;
+    S.order = P.input.data(); S.in_off = frame_offsets;
+    S.sort_T = ctx->d_seq_prior;
+    S.sort_grid.inv_cell = 1.0 / cell_size;
+    S.sort_grid.ox = S.sort_grid.oy = S.sort_grid.oz = -512;
+    S.sort_grid.nx = S.sort_grid.ny = S.sort_grid.nz = 1024;
+    S.sort_cells = 1ll << 30;
+    const float4* src_iter = nullptr;
+    if ((rc = upload_scans_sorted(ctx, S, &src_iter))) return rc;
+    S.sort_T = nullptr;
+    CK(cudaMemcpyAsync(ctx->d_seq_prior, ctx->d_T_init, (size_t)n_frames * 16 * sizeof(double), cudaMemcpyDeviceToDevice,
+                       ctx->stream));
+    // lanes: grid y of the loop kernel; a lane's frame range is set by odom_start_kernel at every step
+    S.lanes = n_seqs;
+    S.seq.cursor = ctx->d_seq_cursor; S.seq.first = ctx->d_seq_first; S.seq.delta = nullptr;
+    S.seq.T_prior = ctx->d_seq_prior; S.seq.seg = ctx->d_scan_seg; S.seq.n_active = ctx->d_n_active;
+    S.cell_size = cell_size;
+    if ((rc = ensure_pinned(ctx, (size_t)n_frames * sizeof(IcpState)))) return rc;
+    LoopPlan L;
+    bool planned = false;
+    int failed = n_steps;                       // the step whose map had no dense grid
+    const double inv_cell = 1.0 / cell_size;
+    for (int i = 1; i < n_steps; ++i) {
+        const odom_plan::Step& st = P.steps[(size_t)i];
+        const long long m = st.map_seg[(size_t)st.active];
+        const int pieces = (int)st.piece_frame.size();
+        const long long* d_map_seg = ctx->d_odom_ll + at_ll[(size_t)i];
+        const long long* d_dst = d_map_seg + st.active + 1;
+        const long long* d_src_at = d_dst + pieces + 1;
+        const int* d_frame = ctx->d_odom_int + at_int[(size_t)i];
+        const int* d_prev = d_frame + pieces;
+        const int* d_prev2 = d_prev + st.active;
+        // 1. the lanes' local maps from the window frames' device-resident results
+        map_points_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_scan_src, d_dst, pieces, d_src_at,
+                                                                                d_frame, m, ctx->d_state, ctx->d_odom_map);
+        ctx->launches++;
+        CK(cudaGetLastError());
+        // 2. their dense grids, one arena segment per lane (the bounds copy is the step's sync besides the loop's peeks)
+        std::vector<int> hb;
+        if ((rc = arena_bounds(ctx, ctx->odom_maps, ctx->d_odom_map, st.map_seg.data(), d_map_seg, st.active, inv_cell, hb)))
+            return rc;
+        std::vector<arena_plan::Box> boxes;
+        long long cells = 0;
+        const std::string why = arena_plan::plan(st.active, hb.data(), boxes, &cells, "local map of lane");
+        if (!why.empty()) {
+            int b = 0;
+            arena_plan::Box x;
+            while (b < st.active - 1 && arena_plan::box_of(hb.data() + 6 * (size_t)b, &x) == arena_plan::kDense) ++b;
+            const int s = st.seq[(size_t)b];
+            ctx->err = "icp_run_odometry: sequence " + std::to_string(s) + ", frame " + std::to_string(seq_offsets[s] + i) +
+                       " (frame " + std::to_string(i) + " of the sequence): " + why;
+            failed = i;
+            break;
+        }
+        if ((rc = arena_fill(ctx, ctx->odom_maps, ctx->d_odom_map, d_map_seg, st.active, m, boxes.data(), cells, inv_cell,
+                             rings)))
+            return rc;
+        // 3. every lane's frame of this step: its prior and a fresh loop state
+        odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
+            ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
+            st.first, st.active, d_prev, d_prev2, deltas ? ctx->d_seq_delta : nullptr, motion);
+        ctx->launches++;
+        CK(cudaGetLastError());
+        // 4. the loop: the same chunks (and CUDA graphs) at every step - the grid table keeps its pointer (the first step
+        // has the most lanes, so the arena's table never regrows after it), only its entries change
+        if (!planned) {
+            S.grids = ctx->odom_maps.d_grids; S.cell_off = ctx->odom_maps.d_cell_off;
+            if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? log_cap : 0, true, &L, &S))) return rc;
+            planned = true;
+        }
+        const long long cap = params->max_iterations;
+        long long issued = 0;
+        while (issued < cap) {
+            long long todo = cap - issued;
+            if (todo > 16) todo = 16;
+            const int bodies = (todo < 16 && issued > 0) ? 16 : (int)todo;
+            if ((rc = enqueue_iterations(ctx, L, params, dlog, dlog ? log_cap : 0, bodies))) return rc;
+            issued += bodies;
+            if (issued < cap) {
+                unsigned int* flag = (unsigned int*)ctx->h_pinned;      // lanes whose frame still runs
+                CK(cudaMemcpyAsync(flag, ctx->d_n_active, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
+                CK(cudaStreamSynchronize(ctx->stream));
+                if (*flag == 0u) break;
+            }
+        }
+    }
+    // results (device order), then back to the caller's frame order; after a failed step only the frames before it
+    if (dlog) {
+        log_fill_kernel<<<dim3((log_cap + 31) / 32, n_frames), 32, 0, ctx->stream>>>(dlog, log_cap, ctx->d_state, *params);
+        ctx->launches++;
+    }
+    std::vector<double> To((size_t)n_frames * 16), Tp, cv;
+    std::vector<int> it((size_t)n_frames), cg((size_t)n_frames), sts((size_t)n_frames);
+    std::vector<dcreg_iter_log> lg(dlog ? (size_t)n_frames * log_cap : 0);
+    const std::string err = ctx->err;
+    if ((rc = read_results(ctx, n_frames, To.data(), dlog ? lg.data() : nullptr, log_cap, it.data(), cg.data(), sts.data())))
+        return rc;
+    if (cov) {
+        cv.resize((size_t)n_frames * 36);
+        covariance_kernel<<<n_frames, 32, 0, ctx->stream>>>(ctx->d_state, ctx->d_scan_cov);
+        ctx->launches++;
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(cv.data(), ctx->d_scan_cov, cv.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    if (T_prior) {
+        Tp.resize((size_t)n_frames * 16);
+        CK(cudaMemcpyAsync(Tp.data(), ctx->d_seq_prior, Tp.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+    const int done = failed < n_steps ? P.steps[(size_t)failed].first : n_frames;
+    for (int k = 0; k < n_frames; ++k) {
+        const size_t d = (size_t)P.dev[(size_t)k];
+        if ((int)d >= done) continue;
+        memcpy(T_out + (size_t)k * 16, &To[d * 16], 16 * sizeof(double));
+        if (T_prior) memcpy(T_prior + (size_t)k * 16, &Tp[d * 16], 16 * sizeof(double));
+        if (n_iterations) n_iterations[k] = it[d];
+        if (converged) converged[k] = cg[d];
+        if (status) status[k] = sts[d];
+        if (cov) memcpy(cov + (size_t)k * 36, &cv[d * 36], 36 * sizeof(double));
+        if (dlog) memcpy(log + (size_t)k * log_cap, &lg[d * log_cap], (size_t)log_cap * sizeof(dcreg_iter_log));
+    }
+    if (failed < n_steps) { ctx->err = err; return DCREG_BAD_ARG; }
     return DCREG_OK;
 }
 

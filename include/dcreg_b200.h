@@ -57,6 +57,9 @@ typedef enum dcreg_handling {
     DCREG_HAND_TRUNCATED_SVD = 5
 } dcreg_handling;
 
+/* Motion model of dcreg_icp_run_odometry: how frame k's prior follows from frame k-1's result. */
+typedef enum dcreg_motion { DCREG_MOTION_INCREMENTS = 0, DCREG_MOTION_CONSTANT_VELOCITY = 1 } dcreg_motion;
+
 /* -------------------------------------------------------------------------------------------
  * Parameters: POD mirror of ICPRunner::Config + ICPParameters
  * (DCReg/include/utils.hpp:82-103, 132-171), passed by pointer, no global state
@@ -287,6 +290,43 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
                             const double* T_init, const double* deltas, double* T_prior, double* T_out,
                             int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
                             int log_cap);
+/* S independent sequences of SCAN-TO-MAP ODOMETRY (a LiDAR front end with no prebuilt map): frame k registers against a
+ * local map made from the results of the frames before it in its sequence, all on the device (no dcreg_set_target, no
+ * host round trip between frames).  Different sequences run side by side.
+ * xyz / frame_offsets / stride / seq_offsets / T_init and the outputs T_prior / T_out / n_iterations / converged /
+ * status / cov / log: as in dcreg_icp_run_sequences (one entry per frame, in the caller's frame order).
+ * cell_size: the dense-grid cell of the local maps; search_radius / cell_size must be in (0, 4].
+ * - Anchor: the first frame of sequence s is not registered.  T_out = T_prior = T_init[s], n_iterations = 0,
+ *   converged = 0, status = DCREG_OK, no log records, cov = 1e6 I (the rule for a run that did not converge).
+ * - Map of frame k: the frames j in [max(first frame of the sequence, k - map_frames), k), ascending j, each frame's
+ *   points in input order.  Point p of frame j becomes fl32(R_j p + t_j) with (R_j, t_j) = T_out[j]; each coordinate is
+ *   ((r0 x + r1 y) + r2 z) + t in FP64 with one rounding per operation and no FMA, then one float32 rounding
+ *   (dcreg_b200.api.map_points gives the same bits).  Every frame of the window goes in, aborted ones included, at the
+ *   pose it returned; no downsampling, cropping or keyframe selection.
+ * - Prior of frame k: compose_prior(T_out[k-1], D) with the rounding rule of dcreg_icp_run_sequences.
+ *   motion = DCREG_MOTION_INCREMENTS: D = deltas[k-1], or the identity when deltas is NULL.
+ *   motion = DCREG_MOTION_CONSTANT_VELOCITY (deltas must be NULL): D = identity when frame k-1 is the anchor, else
+ *   inv(T_out[k-2]) T_out[k-1], i.e. R_D = R_{k-2}^T R_{k-1}, t_D = R_{k-2}^T (t_{k-1} - t_{k-2}), the differences
+ *   rounded first, every entry ((a0 b0 + a1 b1) + a2 b2) with no FMA (dcreg_b200.api.constant_velocity_increment).
+ * - Frame k returns what dcreg_set_target(map_k, cell_size) + dcreg_set_source(frame k) + dcreg_icp_run(T_prior[k])
+ *   returns, up to how the FP64 partial sums are grouped (the frames are sorted once per call by their own cells in the
+ *   sensor frame): counts, masks, iteration counts and status identical, poses equal to rounding.  A call reproduces bit
+ *   for bit.
+ * - Execution: step i registers frame i of every sequence that has one; before it, the device assembles the step's maps
+ *   from the poses in device memory and builds their dense grids (one host sync for the grids' bounds per step).
+ * Limits (DCREG_BAD_ARG before anything is launched): map_frames >= 1, max_iterations >= 1, a valid motion (constant
+ * velocity with deltas == NULL), no sharded context, at most 65535 frames and 2^29 - 1 frame points, and at every step at
+ * most 2^29 - 1 map points over all sequences.  A map whose bounding box is too large for a dense grid at cell_size (over
+ * 2^27 cells, or coordinates outside +-2^19 cells) is only found at its step: the call then returns DCREG_BAD_ARG with
+ * dcreg_last_error naming the sequence and frame, the frames of the earlier steps have their outputs, and the context
+ * stays usable.  The context's source, target and grid, and what the other calls compute, are left as they were.
+ * A long recording goes in calls: each call starts with the previous call's last frame as its anchor, at the pose that
+ * call returned; the first frames of a call then see maps of fewer frames than map_frames. */
+int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                           int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                           double cell_size, int map_frames, int motion, const double* T_init, const double* deltas,
+                           double* T_prior, double* T_out, int* n_iterations, int* converged, int* status,
+                           double* cov, dcreg_iter_log* log, int log_cap);
 /* Same loop, but correspondences are supplied by the caller each iteration through a callback
  * (host kd-tree mode, "PR1"): planes are 4*n doubles (nx,ny,nz,d), all-zero = none. */
 typedef int (*dcreg_plane_callback)(void* user, const double T[16], double* planes4,
