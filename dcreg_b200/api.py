@@ -18,6 +18,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import types
 
 import numpy as np
 
@@ -185,6 +186,36 @@ def _as_points(xyz):
     if a.ndim != 2 or a.shape[1] < 3:
         raise ValueError("points must be (N, >=3)")
     return a
+
+
+def _fptr(a):
+    return a.ctypes.data_as(C.POINTER(C.c_float)) if a is not None else None
+
+
+def _iptr(a):
+    return a.ctypes.data_as(C.POINTER(C.c_int64)) if a is not None else None
+
+
+def _optr(a):
+    return _dptr(a) if a is not None else None
+
+
+def _pack(clouds):
+    """The clouds (a list of (N_b, >=3) arrays) as one contiguous (sum N_b, 3) float32 array and their int64 offsets
+    [len + 1]; (None, None) for no clouds."""
+    pts = [_as_points(c)[:, :3] for c in clouds]
+    if not pts:
+        return None, None
+    off = np.zeros(len(pts) + 1, dtype=np.int64)
+    off[1:] = np.cumsum([p.shape[0] for p in pts])
+    return np.ascontiguousarray(np.concatenate(pts, axis=0)), off
+
+
+def _pack_sequences(sequences):
+    """The int32 sequence table [len + 1] of a list of lists of frames, and _pack of all frames in order."""
+    seq_off = np.zeros(len(sequences) + 1, dtype=np.int32)
+    seq_off[1:] = np.cumsum([len(s) for s in sequences])
+    return (seq_off,) + _pack([f for s in sequences for f in s])
 
 
 def pose_Rt(T):
@@ -441,31 +472,47 @@ class Context:
                                                  logs, cap))
         return _trial_results(st, conv, n_it, T_out, logs, cap)
 
+    def _run_batched(self, name, call, params, n, n_poses, noun, T_init, want_log, want_cov, deltas=None,
+                     want_prior=False):
+        """The steps the batched calls share: check T_init (n_poses of them, one per `noun`) and deltas, allocate the
+        outputs of n trials, run call(o) (the library function with o's outputs) and build one IcpResult per trial.  An
+        empty batch goes to the library as it is and gets BAD_ARG, like every other malformed batch."""
+        o = types.SimpleNamespace(n=0, T_init=None, deltas=None, T_prior=None, T_out=None, n_it=None, conv=None, st=None,
+                                  cov=None, logs=None, cap=0)
+        if n == 0 or n_poses == 0:
+            self._check(call(o))
+        o.T_init = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
+        if o.T_init.shape[0] != n_poses:
+            raise ValueError(f"{name}: {n_poses} {noun} but {o.T_init.shape[0]} initial poses")
+        if deltas is not None:
+            o.deltas = np.ascontiguousarray(deltas, dtype=np.float64).reshape(-1, 4, 4)
+            if o.deltas.shape[0] != n:
+                raise ValueError(f"{name}: {n} frames but {o.deltas.shape[0]} increments")
+        o.n = n
+        o.T_prior = np.empty((n, 4, 4)) if want_prior else None
+        o.T_out = np.empty((n, 4, 4))
+        o.n_it = (C.c_int * n)(); o.conv = (C.c_int * n)(); o.st = (C.c_int * n)()
+        o.cov = np.empty((n, 6, 6)) if want_cov else None
+        o.cap = int(params.max_iterations) if want_log else 0
+        o.logs = (IterLog * max(o.cap * n, 1))() if want_log else None
+        self._check(call(o))
+        out = _trial_results(o.st, o.conv, o.n_it, o.T_out, o.logs, o.cap, o.cov)
+        if want_prior:
+            for r, Tp in zip(out, o.T_prior):
+                r.T_prior = Tp
+        return out
+
     def icp_run_scans(self, params: IcpParams, scans, T_init, want_log: bool = False, want_cov: bool = False):
         """Different scans (a list of (N_b, >=3) point arrays) against the context's target, side by side, each from its
         own initial pose (T_init (B, 4, 4)).  The context's own source is left as it was.  Returns a list of IcpResult,
         one per scan (logs only when want_log, .cov the post-loop 6x6 covariance when want_cov)."""
-        pts = [_as_points(s)[:, :3] for s in scans]
-        B = len(pts)
-        if B == 0:                                      # BAD_ARG from the library, like every other malformed batch
-            self._check(self.lib.dcreg_icp_run_scans(self._h, C.byref(params), 0, None, None, 3, None, None, None, None,
-                                                     None, None, None, 0))
-        xyz = np.ascontiguousarray(np.concatenate(pts, axis=0))
-        stride = 3
-        offsets = np.zeros(B + 1, dtype=np.int64)
-        offsets[1:] = np.cumsum([p.shape[0] for p in pts])
-        T_init = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
-        if T_init.shape[0] != B:
-            raise ValueError(f"icp_run_scans: {B} scans but {T_init.shape[0]} initial poses")
-        T_out = np.empty((B, 4, 4))
-        n_it = (C.c_int * B)(); conv = (C.c_int * B)(); st = (C.c_int * B)()
-        cov = np.empty((B, 6, 6)) if want_cov else None
-        cap = int(params.max_iterations) if want_log else 0
-        logs = (IterLog * max(cap * B, 1))() if want_log else None
-        self._check(self.lib.dcreg_icp_run_scans(self._h, C.byref(params), B, xyz.ctypes.data_as(C.POINTER(C.c_float)),
-                                                 offsets.ctypes.data_as(C.POINTER(C.c_int64)), stride, _dptr(T_init),
-                                                 _dptr(T_out), n_it, conv, st, _dptr(cov) if want_cov else None, logs, cap))
-        return _trial_results(st, conv, n_it, T_out, logs, cap, cov)
+        xyz, off = _pack(scans)
+        B = len(scans)
+
+        def call(o):
+            return self.lib.dcreg_icp_run_scans(self._h, C.byref(params), o.n, _fptr(xyz), _iptr(off), 3, _optr(o.T_init),
+                                                _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov), o.logs, o.cap)
+        return self._run_batched("icp_run_scans", call, params, B, B, "scans", T_init, want_log, want_cov)
 
     def icp_run_sequences(self, params: IcpParams, sequences, T_init, deltas=None, want_log: bool = False,
                           want_cov: bool = False):
@@ -475,40 +522,16 @@ class Context:
         sequence's first frame.  deltas: (n_frames, 4, 4) increments over all frames in order (a sequence's last entry is
         unused), or None for identity.  Returns a list of IcpResult, one per frame in order, with .T_prior the pose the
         frame started from (logs only when want_log, .cov when want_cov).  The context's own source is left as it was."""
-        lens = [len(s) for s in sequences]
-        S = len(lens)
-        pts = [_as_points(f)[:, :3] for s in sequences for f in s]
-        n = len(pts)
-        seq_off = np.zeros(S + 1, dtype=np.int32)
-        seq_off[1:] = np.cumsum(lens)
-        if S == 0 or n == 0:                            # BAD_ARG from the library, like every other malformed batch
-            self._check(self.lib.dcreg_icp_run_sequences(self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)),
-                                                         0, None, None, 3, None, None, None, None, None, None, None, None,
-                                                         None, 0))
-        xyz = np.ascontiguousarray(np.concatenate(pts, axis=0))
-        offsets = np.zeros(n + 1, dtype=np.int64)
-        offsets[1:] = np.cumsum([p.shape[0] for p in pts])
-        T_init = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
-        if T_init.shape[0] != S:
-            raise ValueError(f"icp_run_sequences: {S} sequences but {T_init.shape[0]} initial poses")
-        if deltas is not None:
-            deltas = np.ascontiguousarray(deltas, dtype=np.float64).reshape(-1, 4, 4)
-            if deltas.shape[0] != n:
-                raise ValueError(f"icp_run_sequences: {n} frames but {deltas.shape[0]} increments")
-        T_prior = np.empty((n, 4, 4)); T_out = np.empty((n, 4, 4))
-        n_it = (C.c_int * n)(); conv = (C.c_int * n)(); st = (C.c_int * n)()
-        cov = np.empty((n, 6, 6)) if want_cov else None
-        cap = int(params.max_iterations) if want_log else 0
-        logs = (IterLog * max(cap * n, 1))() if want_log else None
-        self._check(self.lib.dcreg_icp_run_sequences(
-            self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n,
-            xyz.ctypes.data_as(C.POINTER(C.c_float)), offsets.ctypes.data_as(C.POINTER(C.c_int64)), 3, _dptr(T_init),
-            _dptr(deltas) if deltas is not None else None, _dptr(T_prior), _dptr(T_out), n_it, conv, st,
-            _dptr(cov) if want_cov else None, logs, cap))
-        out = _trial_results(st, conv, n_it, T_out, logs, cap, cov)
-        for r, Tp in zip(out, T_prior):
-            r.T_prior = Tp
-        return out
+        seq_off, xyz, off = _pack_sequences(sequences)
+        S, n = len(sequences), int(seq_off[-1])
+
+        def call(o):
+            return self.lib.dcreg_icp_run_sequences(
+                self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off), 3,
+                _optr(o.T_init), _optr(o.deltas), _optr(o.T_prior), _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov),
+                o.logs, o.cap)
+        return self._run_batched("icp_run_sequences", call, params, n, S, "sequences", T_init, want_log, want_cov, deltas,
+                                 want_prior=True)
 
     def icp_run_odometry(self, params: IcpParams, sequences, T_init, deltas=None, motion: str = "increments",
                          map_frames: int = 10, cell_size=None, want_log: bool = False, want_cov: bool = False):
@@ -523,41 +546,17 @@ class Context:
         models = {"increments": 0, "constant_velocity": 1}
         if motion not in models:
             raise ValueError(f"icp_run_odometry: motion must be one of {sorted(models)}, not {motion!r}")
-        lens = [len(s) for s in sequences]
-        S = len(lens)
-        pts = [_as_points(f)[:, :3] for s in sequences for f in s]
-        n = len(pts)
-        seq_off = np.zeros(S + 1, dtype=np.int32)
-        seq_off[1:] = np.cumsum(lens)
+        seq_off, xyz, off = _pack_sequences(sequences)
+        S, n = len(sequences), int(seq_off[-1])
         cell = float(params.search_radius if cell_size is None else cell_size)
-        if S == 0 or n == 0:                            # BAD_ARG from the library, like every other malformed batch
-            self._check(self.lib.dcreg_icp_run_odometry(self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)),
-                                                        0, None, None, 3, cell, int(map_frames), models[motion], None, None,
-                                                        None, None, None, None, None, None, None, 0))
-        xyz = np.ascontiguousarray(np.concatenate(pts, axis=0))
-        offsets = np.zeros(n + 1, dtype=np.int64)
-        offsets[1:] = np.cumsum([p.shape[0] for p in pts])
-        T_init = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
-        if T_init.shape[0] != S:
-            raise ValueError(f"icp_run_odometry: {S} sequences but {T_init.shape[0]} initial poses")
-        if deltas is not None:
-            deltas = np.ascontiguousarray(deltas, dtype=np.float64).reshape(-1, 4, 4)
-            if deltas.shape[0] != n:
-                raise ValueError(f"icp_run_odometry: {n} frames but {deltas.shape[0]} increments")
-        T_prior = np.empty((n, 4, 4)); T_out = np.empty((n, 4, 4))
-        n_it = (C.c_int * n)(); conv = (C.c_int * n)(); st = (C.c_int * n)()
-        cov = np.empty((n, 6, 6)) if want_cov else None
-        cap = int(params.max_iterations) if want_log else 0
-        logs = (IterLog * max(cap * n, 1))() if want_log else None
-        self._check(self.lib.dcreg_icp_run_odometry(
-            self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n,
-            xyz.ctypes.data_as(C.POINTER(C.c_float)), offsets.ctypes.data_as(C.POINTER(C.c_int64)), 3, cell,
-            int(map_frames), models[motion], _dptr(T_init), _dptr(deltas) if deltas is not None else None, _dptr(T_prior),
-            _dptr(T_out), n_it, conv, st, _dptr(cov) if want_cov else None, logs, cap))
-        out = _trial_results(st, conv, n_it, T_out, logs, cap, cov)
-        for r, Tp in zip(out, T_prior):
-            r.T_prior = Tp
-        return out
+
+        def call(o):
+            return self.lib.dcreg_icp_run_odometry(
+                self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off), 3,
+                cell, int(map_frames), models[motion], _optr(o.T_init), _optr(o.deltas), _optr(o.T_prior),
+                _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov), o.logs, o.cap)
+        return self._run_batched("icp_run_odometry", call, params, n, S, "sequences", T_init, want_log, want_cov, deltas,
+                                 want_prior=True)
 
     def icp_run_pairs(self, params: IcpParams, sources, targets, T_init, cell_size=None, want_log: bool = False,
                       want_cov: bool = False, metrics_threshold=None):
@@ -566,37 +565,20 @@ class Context:
         params.search_radius).  Needs no set_target / set_source and leaves the context's clouds as they were.  Returns a
         list of IcpResult, one per pair (logs only when want_log, .cov the post-loop 6x6 covariance when want_cov,
         .metrics the point_to_point_metrics dict at the pair's final pose when metrics_threshold is given)."""
-        src = [_as_points(s)[:, :3] for s in sources]
-        tgt = [_as_points(t)[:, :3] for t in targets]
-        B = len(src)
-        if len(tgt) != B:
-            raise ValueError(f"icp_run_pairs: {B} sources but {len(tgt)} targets")
+        xyz_s, off_s = _pack(sources)
+        xyz_t, off_t = _pack(targets)
+        B = len(sources)
+        if len(targets) != B:
+            raise ValueError(f"icp_run_pairs: {B} sources but {len(targets)} targets")
         cell = float(params.search_radius if cell_size is None else cell_size)
-        if B == 0:                                      # BAD_ARG from the library, like every other malformed batch
-            self._check(self.lib.dcreg_icp_run_pairs(self._h, C.byref(params), 0, None, None, None, None, 3, cell, None,
-                                                     None, None, None, None, None, 0.0, None, None, 0))
-        xyz_s = np.ascontiguousarray(np.concatenate(src, axis=0))
-        xyz_t = np.ascontiguousarray(np.concatenate(tgt, axis=0))
-        off_s = np.zeros(B + 1, dtype=np.int64)
-        off_s[1:] = np.cumsum([p.shape[0] for p in src])
-        off_t = np.zeros(B + 1, dtype=np.int64)
-        off_t[1:] = np.cumsum([p.shape[0] for p in tgt])
-        T_init = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
-        if T_init.shape[0] != B:
-            raise ValueError(f"icp_run_pairs: {B} pairs but {T_init.shape[0]} initial poses")
-        T_out = np.empty((B, 4, 4))
-        n_it = (C.c_int * B)(); conv = (C.c_int * B)(); st = (C.c_int * B)()
-        cov = np.empty((B, 6, 6)) if want_cov else None
         met = np.empty((B, 4)) if metrics_threshold is not None else None
-        cap = int(params.max_iterations) if want_log else 0
-        logs = (IterLog * max(cap * B, 1))() if want_log else None
-        fp = C.POINTER(C.c_float)
-        self._check(self.lib.dcreg_icp_run_pairs(
-            self._h, C.byref(params), B, xyz_s.ctypes.data_as(fp), off_s.ctypes.data_as(C.POINTER(C.c_int64)),
-            xyz_t.ctypes.data_as(fp), off_t.ctypes.data_as(C.POINTER(C.c_int64)), 3, cell, _dptr(T_init), _dptr(T_out),
-            n_it, conv, st, _dptr(cov) if want_cov else None,
-            float(metrics_threshold) if met is not None else 0.0, _dptr(met) if met is not None else None, logs, cap))
-        out = _trial_results(st, conv, n_it, T_out, logs, cap, cov)
+
+        def call(o):
+            return self.lib.dcreg_icp_run_pairs(
+                self._h, C.byref(params), o.n, _fptr(xyz_s), _iptr(off_s), _fptr(xyz_t), _iptr(off_t), 3, cell,
+                _optr(o.T_init), _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov),
+                float(metrics_threshold) if met is not None and o.n else 0.0, _optr(met) if o.n else None, o.logs, o.cap)
+        out = self._run_batched("icp_run_pairs", call, params, B, B, "pairs", T_init, want_log, want_cov)
         if met is not None:
             for r, m in zip(out, met):
                 r.metrics = {"rmse": m[0], "fitness": m[1], "chamfer": m[2], "n_valid": int(m[3])}

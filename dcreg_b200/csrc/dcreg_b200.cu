@@ -884,7 +884,7 @@ __global__ void pack_points_kernel(const float* __restrict__ in, long long n, in
     }
 }
 
-// Key of the scans' spatial sort (upload_scans_sorted) of packed points: (scan b, target cell of fl32(T_b p)) with
+// Key of the scans' spatial sort (sort_sources) of packed points: (scan b, target cell of fl32(T_b p)) with
 // T_b = T[16 b ..], and the point's index as the value.  A stable sort on that key orders each segment exactly as
 // sort_source_by_cell orders the scan alone: by cell, then index.  Against the context's grid g the key is
 // b * ncells + cell.  grids (scan/target pairs, dcreg_icp_run_pairs): scan b's cell is taken in its own target's grid
@@ -1025,6 +1025,36 @@ constexpr int kNcclSum = 0;
 // ------------------------------------------------------------------------------------------------
 // context
 // ------------------------------------------------------------------------------------------------
+// A grow-only allocation with one owner: ensure(n) reallocates, at exactly n elements, only when the capacity is below
+// n (the old contents are lost), and the destructor frees it.  kPinned: page-locked host memory.
+template <typename T, bool kPinned = false>
+struct DevBuf {
+    T* p = nullptr;
+    long long cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
+    operator T*() const { return p; }
+    void release() {
+        if (p) {
+            if (kPinned) cudaFreeHost(p);
+            else cudaFree(p);
+        }
+        p = nullptr; cap = 0;
+    }
+    cudaError_t ensure(long long n) {
+        if (cap >= n) return cudaSuccess;
+        release();
+        void* q = nullptr;
+        const cudaError_t e = kPinned ? cudaMallocHost(&q, (size_t)n * sizeof(T)) : cudaMalloc(&q, (size_t)n * sizeof(T));
+        if (e == cudaSuccess) { p = (T*)q; cap = n; }
+        return e;
+    }
+};
+template <typename T>
+using PinnedBuf = DevBuf<T, true>;
+
 struct dcreg_ctx {
     int device = 0;
     int sm_count = 132;
@@ -1032,36 +1062,35 @@ struct dcreg_ctx {
     std::string err;
     long long launches = 0;
 
-    float4* d_src = nullptr; long long n_src = 0; long long n_src_cap = 0; long long n_src_total = 0;
-    float* d_stage = nullptr; size_t stage_bytes = 0;
+    DevBuf<float4> d_src; long long n_src = 0; long long n_src_total = 0;
+    DevBuf<float> d_stage;                                                 // host point uploads before packing
 
-    float4* d_tgt = nullptr; long long n_tgt = 0;
+    DevBuf<float4> d_tgt; long long n_tgt = 0;                             // exactly n_tgt: every set_target reallocates it
     corr::Grid grid{}; long long grid_cells = 0; bool has_grid = false;
-    double4* d_plane_cache = nullptr; signed char* d_fit_state = nullptr;   // plane of the slot's current five neighbours
-    int* d_plane_key = nullptr;                                             // ... and which five (ascending positions)
+    DevBuf<double4> d_plane_cache; DevBuf<signed char> d_fit_state;        // plane of the slot's current five neighbours
+    DevBuf<int> d_plane_key;                                               // ... and which five (ascending positions)
     bool force_coherent = false;                                           // profiling (dcreg_time_iteration what = 0)
-    float* d_src_radius = nullptr;                                         // max |p| over the source cloud (device)
-    unsigned int* d_iter_stats = nullptr;                                  // optional profiling counters of the iteration kernel
-    int4* d_nn = nullptr; long long nn_cap = 0; bool nn_valid = false;   // neighbours of the sorted source (seeds of the next iteration)
-    float4* d_src_sorted = nullptr; long long src_sorted_cap = 0;     // source in target-cell order (w = original index)
-    float4* d_sort_tmp = nullptr;                                     // ... before the in-cell ranking
-    int* d_cell_tmp = nullptr; long long cell_tmp_cap = 0;            // counts / fill cursors for the source sort
-    int* d_pt_cell = nullptr; long long pt_cell_cap = 0;
-    int* d_tile_sums = nullptr; long long tile_sums_cap = 0;
+    DevBuf<float> d_src_radius;                                            // max |p| over the source cloud (device)
+    DevBuf<unsigned int> d_iter_stats;                                     // profiling counters of the iteration kernel (while enabled)
+    DevBuf<int4> d_nn; bool nn_valid = false;                              // neighbours of the sorted source (seeds of the next iteration)
+    long long nn_slots = 0; int nn_trials = 0;                             // shape of the per-slot records (d_nn, d_plane_cache, ...)
+    DevBuf<float4> d_src_sorted;                                           // source in target-cell order (w = original index)
+    DevBuf<float4> d_sort_tmp;                                             // ... before the in-cell ranking
+    DevBuf<int> d_cell_tmp;                                                // counts / fill cursors for the source sort
+    DevBuf<int> d_pt_cell;
+    DevBuf<int> d_tile_sums;
     double cell_size = 0.0;
 
-    double4* d_planes64 = nullptr; float4* d_planes32 = nullptr; long long planes_cap = 0;
+    DevBuf<double4> d_planes64; DevBuf<float4> d_planes32;
 
-    // per-trial arrays (dcreg_icp_run = 1 trial, dcreg_icp_run_batch = many): [trials_cap] each
-    int trials_cap = 0;
-    double* d_partials = nullptr; int partials_blocks = 0;
-    unsigned int* d_counter = nullptr;
-    double* d_acc = nullptr;
-    IcpState* d_state = nullptr;
-    unsigned int* d_n_active = nullptr;   // trials still running
-    double* d_T_init = nullptr; int T_init_cap = 0;
-    int nn_trials = 0;                    // trials the per-slot record arrays (d_nn, d_plane_cache, ...) are sized for
-    dcreg_iter_log* d_log = nullptr; long long log_cap = 0;   // records, [trials][log_cap of the run]
+    // per-trial arrays (dcreg_icp_run = 1 trial, dcreg_icp_run_batch = many)
+    DevBuf<double> d_partials;            // [blocks][kPartialDoubles]
+    DevBuf<unsigned int> d_counter;
+    DevBuf<double> d_acc;
+    DevBuf<IcpState> d_state;
+    DevBuf<unsigned int> d_n_active;      // trials still running
+    DevBuf<double> d_T_init;
+    DevBuf<dcreg_iter_log> d_log;         // records, [trials][log_cap of the run]
     bool loop_attr_done = false, k1_attr_done[8] = {false, false, false, false, false, false, false, false};
     // CUDA graphs of one chunk of loop iterations, keyed on the kernel arguments (a few shapes alternate in practice:
     // with / without a log, one trial / a batch); most recently used first
@@ -1069,50 +1098,54 @@ struct dcreg_ctx {
     std::vector<LoopGraph> graphs; bool graph_off = false;
     long long graph_launches = 0;
     void drop_graphs() { for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec); graphs.clear(); }
-    double* d_small = nullptr;       // scratch for the seams (>= 512 doubles)
-    K2Scratch* d_k2_scratch = nullptr;   // K2's rehearsal state (see k2_step_kernel)
+    DevBuf<double> d_small;              // scratch for the seams (1024 doubles)
+    DevBuf<K2Scratch> d_k2_scratch;      // K2's rehearsal state (see k2_step_kernel)
     // solver block of a single-trial folded run (solver_block): row flags, launch counter, warm-up state.  The counter
     // and the flags are never reset, so no flag written by an earlier launch can match a later one
-    unsigned long long* d_row_flags = nullptr; int row_flags_cap = 0;
-    unsigned long long* d_row_epoch = nullptr;
-    IcpState* d_warm_state = nullptr;
-    // a batch of different scans (dcreg_icp_run_scans) in buffers of its own: the context's source stays as it was
-    float4* d_scan_src = nullptr; float4* d_scan_sorted = nullptr; long long scan_cap = 0;   // packed / in sort order
-    unsigned long long* d_scan_keys = nullptr; int* d_scan_vals = nullptr;                   // [2][scan_cap]: sort in / out
-    void* d_scan_sort_tmp = nullptr; size_t scan_sort_tmp_bytes = 0;
-    long long* d_scan_seg = nullptr; float* d_scan_radius = nullptr; double* d_scan_cov = nullptr; int scans_cap = 0;
-    // sequences of frames (dcreg_icp_run_sequences; the frames use the scans' buffers): lane cursors and frame ranges
-    // [lanes] / [lanes + 1], increments and priors [frames][16]
-    int* d_seq_cursor = nullptr; int* d_seq_first = nullptr; int seq_lanes_cap = 0;
-    double* d_seq_delta = nullptr; double* d_seq_prior = nullptr; int seq_frames_cap = 0;
-    // odometry (dcreg_icp_run_odometry; the frames use the scans' and the sequences' buffers): every step's tables
-    // (odom_plan.hpp) in one upload, the step's local maps, and their grids in an arena of their own
-    long long* d_odom_ll = nullptr; long long odom_ll_cap = 0; int* d_odom_int = nullptr; long long odom_int_cap = 0;
-    float4* d_odom_map = nullptr; long long odom_map_cap = 0;
+    DevBuf<unsigned long long> d_row_flags;
+    DevBuf<unsigned long long> d_row_epoch;
+    DevBuf<IcpState> d_warm_state;
+    // the sources of a batched call (dcreg_icp_run_scans, _pairs, _sequences, _odometry) in buffers of their own: the
+    // context's source stays as it was.  [points] packed / in sort order, [2][points] sort keys and values in / out,
+    // [sources + 1] offsets, [sources] lever arms and covariances
+    DevBuf<float4> d_scan_src, d_scan_sorted;
+    DevBuf<unsigned long long> d_scan_keys; DevBuf<int> d_scan_vals;
+    DevBuf<unsigned char> d_scan_sort_tmp;
+    DevBuf<long long> d_scan_seg; DevBuf<float> d_scan_radius; DevBuf<double> d_scan_cov;
+    // sequences of frames (dcreg_icp_run_sequences, _odometry; the frames are the batch's sources): lane cursors and
+    // frame ranges [lanes] / [lanes + 1], increments and priors [frames][16]
+    DevBuf<int> d_seq_cursor, d_seq_first;
+    DevBuf<double> d_seq_delta, d_seq_prior;
+    // odometry (dcreg_icp_run_odometry): every step's tables (odom_plan.hpp) in one upload, the step's local maps, and
+    // their grids in an arena of their own
+    DevBuf<long long> d_odom_ll; DevBuf<int> d_odom_int;
+    DevBuf<float4> d_odom_map;
     // Grow-only arenas of dense grids (build_grid_arena): the context's target (one cloud; `grid` points into it), the
-    // targets of dcreg_icp_run_pairs (the context's target and grid stay as they were), and the grids over the aligned
-    // sources of the point-to-point metrics
+    // targets of dcreg_icp_run_pairs (the context's target and grid stay as they were), the grids over the aligned
+    // sources of the point-to-point metrics, and odometry's local maps
     struct GridArena {
-        float4* pts = nullptr; int* pos_of = nullptr; float4* tmp = nullptr; int* pt_cell = nullptr; long long pts_cap = 0;
-        int* cell_start = nullptr; int* counts = nullptr; int* fill = nullptr; long long cells_cap = 0;
-        corr::Grid* d_grids = nullptr; int* d_cell_off = nullptr; int* d_bounds = nullptr; int segs_cap = 0;
-        void free_all() {
-            void* p[] = {pts, pos_of, tmp, pt_cell, cell_start, counts, fill, d_grids, d_cell_off, d_bounds};
-            for (void* q : p)
-                if (q) cudaFree(q);
-            *this = GridArena{};
+        DevBuf<float4> pts, tmp; DevBuf<int> pos_of, pt_cell;               // [points]
+        DevBuf<int> cell_start, counts, fill;                               // [cells + 1], [cells + 1], [cells]
+        DevBuf<corr::Grid> d_grids; DevBuf<int> d_cell_off, d_bounds;       // [clouds], [clouds + 1], [clouds][6]
+        // room for m points in `cells` cells
+        cudaError_t reserve(long long m, long long cells) {
+            cudaError_t e;
+            if ((e = pts.ensure(m)) || (e = pos_of.ensure(m)) || (e = tmp.ensure(m)) || (e = pt_cell.ensure(m)) ||
+                (e = cell_start.ensure(cells + 1)) || (e = counts.ensure(cells + 1)) || (e = fill.ensure(cells)))
+                return e;
+            return cudaSuccess;
         }
     };
     GridArena tgt_arena, pair_tgt, aligned, odom_maps;
     // the hash tables of a target too large for a dense grid (build_hash_grid; points in tgt_arena)
-    unsigned long long* d_hash_keys = nullptr; int* d_hash_start = nullptr; int* d_hash_count = nullptr; long long hash_cap = 0;
-    float4* d_pair_tgt = nullptr; long long pair_tgt_cap = 0;                    // targets, packed (w = global index)
-    long long* d_pair_tgt_seg = nullptr; double* d_pair_T = nullptr; int pairs_cap = 0;   // [n + 1] / [n][16] final poses
-    float4* d_aligned = nullptr; long long aligned_cap = 0;                      // sources under their final poses
-    dcreg_analysis* d_analysis = nullptr;
-    float4* d_flush = nullptr; long long flush_n = 0;
+    DevBuf<unsigned long long> d_hash_keys; DevBuf<int> d_hash_start, d_hash_count;
+    DevBuf<float4> d_pair_tgt;                                   // targets, packed (w = global index)
+    DevBuf<long long> d_pair_tgt_seg; DevBuf<double> d_pair_T;   // [n + 1] / [n][16] final poses
+    DevBuf<float4> d_aligned;                                    // sources under their final poses
+    DevBuf<dcreg_analysis> d_analysis;
+    DevBuf<float4> d_flush;
 
-    void* h_pinned = nullptr; size_t pinned_bytes = 0;
+    PinnedBuf<unsigned char> h_pinned;
 
     ncclComm_t comm = nullptr; int rank = 0, nranks = 1;
     // peer mailboxes for the in-kernel sum over ranks (peer_reduce.cuh); NCCL all-reduce is the fallback
@@ -1131,75 +1164,31 @@ namespace {
         }                                                                                          \
     } while (0)
 
-int ensure_pinned(dcreg_ctx* ctx, size_t bytes) {
-    if (ctx->pinned_bytes >= bytes) return DCREG_OK;
-    if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
-    ctx->h_pinned = nullptr; ctx->pinned_bytes = 0;
-    CK(cudaMallocHost(&ctx->h_pinned, bytes));
-    ctx->pinned_bytes = bytes;
-    return DCREG_OK;
-}
-
-int ensure_partials(dcreg_ctx* ctx, int blocks) {
-    if (ctx->partials_blocks >= blocks) return DCREG_OK;
-    if (ctx->d_partials) cudaFree(ctx->d_partials);
-    ctx->d_partials = nullptr;
-    CK(cudaMalloc(&ctx->d_partials, (size_t)blocks * 72 * sizeof(double)));   // >= k1s::kPart and kAcc
-    ctx->partials_blocks = blocks;
-    return DCREG_OK;
-}
+constexpr long long kPartialDoubles = 72;   // d_partials per block: >= k1s::kPart and kAcc
 
 int ensure_row_flags(dcreg_ctx* ctx, int rows) {
     if (!ctx->d_row_epoch) {
-        CK(cudaMalloc(&ctx->d_row_epoch, sizeof(unsigned long long)));
+        CK(ctx->d_row_epoch.ensure(1));
         CK(cudaMemsetAsync(ctx->d_row_epoch, 0, sizeof(unsigned long long), ctx->stream));
-        CK(cudaMalloc(&ctx->d_warm_state, sizeof(IcpState)));
+        CK(ctx->d_warm_state.ensure(1));
         CK(cudaMemsetAsync(ctx->d_warm_state, 0, sizeof(IcpState), ctx->stream));
     }
-    if (ctx->row_flags_cap >= rows) return DCREG_OK;
-    if (ctx->d_row_flags) cudaFree(ctx->d_row_flags);
-    ctx->d_row_flags = nullptr; ctx->row_flags_cap = 0;
-    CK(cudaMalloc(&ctx->d_row_flags, (size_t)rows * sizeof(unsigned long long)));
+    if (ctx->d_row_flags.cap >= rows) return DCREG_OK;
+    CK(ctx->d_row_flags.ensure(rows));
     CK(cudaMemsetAsync(ctx->d_row_flags, 0, (size_t)rows * sizeof(unsigned long long), ctx->stream));   // below every epoch + 1
-    ctx->row_flags_cap = rows;
-    return DCREG_OK;
-}
-
-int ensure_planes(dcreg_ctx* ctx, long long n) {
-    if (ctx->planes_cap >= n) return DCREG_OK;
-    if (ctx->d_planes64) cudaFree(ctx->d_planes64);
-    if (ctx->d_planes32) cudaFree(ctx->d_planes32);
-    ctx->d_planes64 = nullptr; ctx->d_planes32 = nullptr; ctx->planes_cap = 0;
-    CK(cudaMalloc(&ctx->d_planes64, (size_t)n * sizeof(double4)));
-    CK(cudaMalloc(&ctx->d_planes32, (size_t)n * sizeof(float4)));
-    ctx->planes_cap = n;
-    return DCREG_OK;
-}
-
-int ensure_log(dcreg_ctx* ctx, long long records) {
-    if (ctx->log_cap >= records) return DCREG_OK;
-    if (ctx->d_log) cudaFree(ctx->d_log);
-    ctx->d_log = nullptr; ctx->log_cap = 0;
-    CK(cudaMalloc(&ctx->d_log, (size_t)records * sizeof(dcreg_iter_log)));
-    ctx->log_cap = records;
     return DCREG_OK;
 }
 
 // per-trial loop state: IcpState, ticket, sums, initial poses
 int ensure_trials(dcreg_ctx* ctx, int trials) {
-    if (ctx->trials_cap >= trials) return DCREG_OK;
-    void* old[] = {ctx->d_counter, ctx->d_acc, ctx->d_state, ctx->d_T_init};
-    for (void* p : old)
-        if (p) cudaFree(p);
-    ctx->d_counter = nullptr; ctx->d_acc = nullptr; ctx->d_state = nullptr; ctx->d_T_init = nullptr; ctx->trials_cap = 0;
-    CK(cudaMalloc(&ctx->d_counter, (size_t)trials * sizeof(unsigned int)));
+    if (ctx->d_state.cap >= trials) return DCREG_OK;
+    CK(ctx->d_counter.ensure(trials));
     CK(cudaMemsetAsync(ctx->d_counter, 0, (size_t)trials * sizeof(unsigned int), ctx->stream));
-    CK(cudaMalloc(&ctx->d_acc, (size_t)trials * kAcc * sizeof(double)));
+    CK(ctx->d_acc.ensure((long long)trials * kAcc));
     CK(cudaMemsetAsync(ctx->d_acc, 0, (size_t)trials * kAcc * sizeof(double), ctx->stream));   // the solver block's warm-up input
-    CK(cudaMalloc(&ctx->d_state, (size_t)trials * sizeof(IcpState)));
+    CK(ctx->d_state.ensure(trials));
     CK(cudaMemsetAsync(ctx->d_state, 0, (size_t)trials * sizeof(IcpState), ctx->stream));
-    CK(cudaMalloc(&ctx->d_T_init, (size_t)trials * 16 * sizeof(double)));
-    ctx->trials_cap = trials;
+    CK(ctx->d_T_init.ensure((long long)trials * 16));
     ctx->drop_graphs();
     return DCREG_OK;
 }
@@ -1226,16 +1215,6 @@ int stream_grid(const dcreg_ctx* ctx, long long n, int per_sm) {
     return (int)(need < cap ? need : cap);
 }
 
-// device staging buffer of host point uploads
-int ensure_stage(dcreg_ctx* ctx, size_t bytes) {
-    if (ctx->stage_bytes >= bytes) return DCREG_OK;
-    if (ctx->d_stage) cudaFree(ctx->d_stage);
-    ctx->d_stage = nullptr; ctx->stage_bytes = 0;
-    CK(cudaMalloc(&ctx->d_stage, bytes));
-    ctx->stage_bytes = bytes;
-    return DCREG_OK;
-}
-
 // host points -> d_out, packed by pack_points_kernel (d_seg: device table of n_seg segments, or null for one; d_radius:
 // [n_seg] per-segment max |p|, or null)
 // order / in_off (odometry): segment b of the device copy is host segment order[b], points [in_off[order[b]], ..) of xyz;
@@ -1243,8 +1222,7 @@ int ensure_stage(dcreg_ctx* ctx, size_t bytes) {
 int upload_points(dcreg_ctx* ctx, const float* xyz, long long n, int stride, const long long* d_seg, int n_seg,
                   float4* d_out, float* d_radius, const int* order = nullptr, const int64_t* in_off = nullptr) {
     const size_t bytes = (size_t)n * stride * sizeof(float);
-    const int rc = ensure_stage(ctx, bytes);
-    if (rc) return rc;
+    CK(ctx->d_stage.ensure(n * stride));
     if (!order) {
         CK(cudaMemcpyAsync(ctx->d_stage, xyz, bytes, cudaMemcpyHostToDevice, ctx->stream));
     } else {
@@ -1292,8 +1270,7 @@ int launch_reduce_t(dcreg_ctx* ctx, k1s::Args& a) {
     const long long need = (nchunks + k1s::kWarpsPerBlock - 1) / k1s::kWarpsPerBlock;
     if (g > need) g = need;
     if (g < 1) g = 1;
-    int rc = ensure_partials(ctx, (int)g);
-    if (rc) return rc;
+    CK(ctx->d_partials.ensure(g * kPartialDoubles));
     a.partials = ctx->d_partials;
     // team size (k1_stream.cuh): 1 CTA per contiguous range; larger teams were no faster during development (not re-measured on H100)
     return launch_reduce_k<PlaneT, kUseWd, 1>(ctx, a, (int)g);
@@ -1330,9 +1307,8 @@ int nccl_allreduce_acc(dcreg_ctx* ctx) {
 // status_out[t] = dcreg_status of trial t.
 int read_results(dcreg_ctx* ctx, int trials, double* T_out, dcreg_iter_log* log, int log_cap, int* n_iterations,
                  int* converged, int* status_out) {
-    int rc = ensure_pinned(ctx, (size_t)trials * sizeof(IcpState));
-    if (rc) return rc;
-    IcpState* hs = (IcpState*)ctx->h_pinned;
+    CK(ctx->h_pinned.ensure((long long)trials * sizeof(IcpState)));
+    IcpState* hs = (IcpState*)ctx->h_pinned.p;
     CK(cudaMemcpyAsync(hs, ctx->d_state, (size_t)trials * sizeof(IcpState), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     for (int t = 0; t < trials; ++t) {
@@ -1412,39 +1388,26 @@ int dcreg_create(int device_id, dcreg_ctx** out) {
         const int rc = ensure_trials(ctx, 1);
         if (rc) return rc;
     }
-    CK(cudaMalloc(&ctx->d_n_active, sizeof(unsigned int)));
+    CK(ctx->d_n_active.ensure(1));
     CK(cudaMemsetAsync(ctx->d_n_active, 0, sizeof(unsigned int), ctx->stream));
-    CK(cudaMalloc(&ctx->d_small, 1024 * sizeof(double)));
+    CK(ctx->d_small.ensure(1024));
     if (!getenv("DCREG_NO_K2_REHEARSAL")) {
-        CK(cudaMalloc(&ctx->d_k2_scratch, sizeof(K2Scratch)));
+        CK(ctx->d_k2_scratch.ensure(1));
         CK(cudaMemsetAsync(ctx->d_k2_scratch, 0, sizeof(K2Scratch), ctx->stream));
     }
-    CK(cudaMalloc(&ctx->d_analysis, sizeof(dcreg_analysis)));
+    CK(ctx->d_analysis.ensure(1));
     CK(cudaStreamSynchronize(ctx->stream));
     return DCREG_OK;
 }
 
+// Nothing may be queued or captured when the buffers go: the stream is drained, the communicator and the CUDA graphs
+// released, and the buffers then freed by their owners as the context is deleted (the device is still current).
 int dcreg_destroy(dcreg_ctx* ctx) {
     if (!ctx) return DCREG_BAD_ARG;
     cudaSetDevice(ctx->device);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);
     dcreg_comm_destroy(ctx);
     ctx->drop_graphs();
-    void* ptrs[] = {ctx->d_n_active, ctx->d_T_init, ctx->d_sort_tmp, ctx->d_src, ctx->d_stage, ctx->d_tgt, ctx->d_hash_keys,
-                    ctx->d_hash_start, ctx->d_hash_count, ctx->d_src_sorted, ctx->d_cell_tmp, ctx->d_pt_cell, ctx->d_tile_sums,
-                    ctx->d_planes64, ctx->d_planes32, ctx->d_partials, ctx->d_counter, ctx->d_acc,
-                    ctx->d_state, ctx->d_log, ctx->d_small, ctx->d_analysis, ctx->d_flush, ctx->d_nn, ctx->d_plane_cache, ctx->d_fit_state, ctx->d_iter_stats, ctx->d_src_radius, ctx->d_plane_key, ctx->d_k2_scratch,
-                    ctx->d_row_flags, ctx->d_row_epoch, ctx->d_warm_state, ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_keys,
-                    ctx->d_scan_vals, ctx->d_scan_sort_tmp, ctx->d_scan_seg, ctx->d_scan_radius, ctx->d_scan_cov,
-                    ctx->d_pair_tgt, ctx->d_pair_tgt_seg, ctx->d_pair_T, ctx->d_aligned, ctx->d_seq_cursor, ctx->d_seq_first,
-                    ctx->d_seq_delta, ctx->d_seq_prior, ctx->d_odom_ll, ctx->d_odom_int, ctx->d_odom_map};
-    for (void* p : ptrs)
-        if (p) cudaFree(p);
-    ctx->tgt_arena.free_all();
-    ctx->pair_tgt.free_all();
-    ctx->aligned.free_all();
-    ctx->odom_maps.free_all();
-    if (ctx->h_pinned) cudaFreeHost(ctx->h_pinned);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
     return DCREG_OK;
@@ -1453,23 +1416,18 @@ int dcreg_destroy(dcreg_ctx* ctx) {
 const char* dcreg_last_error(const dcreg_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 void* dcreg_stream(dcreg_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
 int64_t dcreg_launch_count(const dcreg_ctx* ctx) { return ctx ? ctx->launches : 0; }
-void* dcreg_device_source(dcreg_ctx* ctx) { return ctx ? ctx->d_src : nullptr; }
-void* dcreg_device_planes_f64(dcreg_ctx* ctx) { return ctx ? ctx->d_planes64 : nullptr; }
-void* dcreg_device_planes_f32(dcreg_ctx* ctx) { return ctx ? ctx->d_planes32 : nullptr; }
+void* dcreg_device_source(dcreg_ctx* ctx) { return ctx ? ctx->d_src.p : nullptr; }
+void* dcreg_device_planes_f64(dcreg_ctx* ctx) { return ctx ? ctx->d_planes64.p : nullptr; }
+void* dcreg_device_planes_f32(dcreg_ctx* ctx) { return ctx ? ctx->d_planes32.p : nullptr; }
 
 int dcreg_set_source(dcreg_ctx* ctx, const float* xyz, int64_t n, int stride) {
     if (!ctx) return DCREG_BAD_ARG;
     if (!xyz || n <= 0 || stride < 3) { ctx->err = "dcreg_set_source: empty cloud or stride < 3"; return DCREG_BAD_ARG; }
     CK(cudaSetDevice(ctx->device));
-    if (ctx->n_src_cap < n) {
-        if (ctx->d_src) cudaFree(ctx->d_src);
-        ctx->d_src = nullptr; ctx->n_src_cap = 0;
-        CK(cudaMalloc(&ctx->d_src, (size_t)n * sizeof(float4)));
-        ctx->n_src_cap = n;
-    }
+    CK(ctx->d_src.ensure(n));
     ctx->n_src = n;
     if (ctx->nranks == 1) ctx->n_src_total = n;
-    if (!ctx->d_src_radius) CK(cudaMalloc(&ctx->d_src_radius, sizeof(float)));
+    CK(ctx->d_src_radius.ensure(1));
     return upload_points(ctx, xyz, n, stride, nullptr, 1, ctx->d_src, ctx->d_src_radius);
 }
 
@@ -1482,12 +1440,7 @@ int dcreg_set_global_source_count(dcreg_ctx* ctx, int64_t n_total) {
 // exclusive scan of `n` ints (in -> out) on ctx's stream; tile_sums is ctx-owned scratch
 static int device_exclusive_scan(dcreg_ctx* ctx, const int* in, long long n, int* out) {
     const int ntiles = (int)((n + corr::kScanTile - 1) / corr::kScanTile);
-    if (ctx->tile_sums_cap < ntiles) {
-        if (ctx->d_tile_sums) cudaFree(ctx->d_tile_sums);
-        ctx->d_tile_sums = nullptr; ctx->tile_sums_cap = 0;
-        CK(cudaMalloc(&ctx->d_tile_sums, (size_t)ntiles * sizeof(int)));
-        ctx->tile_sums_cap = ntiles;
-    }
+    CK(ctx->d_tile_sums.ensure(ntiles));
     corr::scan_tile_sums_kernel<<<ntiles, 256, 0, ctx->stream>>>(in, (int)n, ctx->d_tile_sums);
     corr::scan_tile_offsets_kernel<<<1, 1024, 0, ctx->stream>>>(ctx->d_tile_sums, ntiles);
     corr::scan_tile_apply_kernel<<<ntiles, 256, 0, ctx->stream>>>(in, (int)n, ctx->d_tile_sums, out);
@@ -1503,48 +1456,14 @@ static int device_exclusive_scan(dcreg_ctx* ctx, const int* in, long long n, int
 // the points are grouped by cell, then by index, and positions and .w (the global index) are shifted by the constant
 // h_seg[b]: the (distance, then index) order of the neighbour search and the equality of position lists are those of
 // the cloud built alone.  Replaces the kd-tree build of ICPContext::setTargetCloud (utils.hpp:393-424).
-static int ensure_arena_points(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, long long m) {
-    if (A.pts_cap >= m) return DCREG_OK;
-    void* old[] = {A.pts, A.pos_of, A.tmp, A.pt_cell};
-    for (void* p : old)
-        if (p) cudaFree(p);
-    A.pts = nullptr; A.pos_of = nullptr; A.tmp = nullptr; A.pt_cell = nullptr; A.pts_cap = 0;
-    CK(cudaMalloc(&A.pts, (size_t)m * sizeof(float4)));
-    CK(cudaMalloc(&A.pos_of, (size_t)m * sizeof(int)));
-    CK(cudaMalloc(&A.tmp, (size_t)m * sizeof(float4)));
-    CK(cudaMalloc(&A.pt_cell, (size_t)m * sizeof(int)));
-    A.pts_cap = m;
-    return DCREG_OK;
-}
-
-static int ensure_arena_cells(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, long long cells) {
-    if (A.cells_cap >= cells) return DCREG_OK;
-    void* old[] = {A.cell_start, A.counts, A.fill};
-    for (void* p : old)
-        if (p) cudaFree(p);
-    A.cell_start = nullptr; A.counts = nullptr; A.fill = nullptr; A.cells_cap = 0;
-    CK(cudaMalloc(&A.cell_start, (size_t)(cells + 1) * sizeof(int)));
-    CK(cudaMalloc(&A.counts, (size_t)(cells + 1) * sizeof(int)));
-    CK(cudaMalloc(&A.fill, (size_t)cells * sizeof(int)));
-    A.cells_cap = cells;
-    return DCREG_OK;
-}
 
 // hb[n * 6]: per cloud the min cell coordinates (x, y, z), then the max (arena_plan::box_of)
 static int arena_bounds(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_pts, const int64_t* h_seg,
                         const long long* d_seg, int n, double inv_cell, std::vector<int>& hb) {
-    if (A.segs_cap < n) {
-        void* old[] = {A.d_grids, A.d_cell_off, A.d_bounds};
-        for (void* p : old)
-            if (p) cudaFree(p);
-        A.d_grids = nullptr; A.d_cell_off = nullptr; A.d_bounds = nullptr; A.segs_cap = 0;
-        CK(cudaMalloc(&A.d_grids, (size_t)n * sizeof(corr::Grid)));
-        CK(cudaMalloc(&A.d_cell_off, (size_t)(n + 1) * sizeof(int)));
-        CK(cudaMalloc(&A.d_bounds, (size_t)n * 6 * sizeof(int)));
-        A.segs_cap = n;
-    }
-    int rc = ensure_pinned(ctx, (size_t)n * 6 * sizeof(int));
-    if (rc) return rc;
+    CK(A.d_grids.ensure(n));
+    CK(A.d_cell_off.ensure(n + 1));
+    CK(A.d_bounds.ensure((long long)n * 6));
+    CK(ctx->h_pinned.ensure((long long)n * 6 * sizeof(int)));
     hb.resize((size_t)n * 6);
     long long max_m = 0;
     for (int b = 0; b < n; ++b) {
@@ -1559,7 +1478,7 @@ static int arena_bounds(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(ctx->h_pinned, A.d_bounds, hb.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    memcpy(hb.data(), ctx->h_pinned, hb.size() * sizeof(int));
+    memcpy(hb.data(), ctx->h_pinned.p, hb.size() * sizeof(int));
     return DCREG_OK;
 }
 
@@ -1577,7 +1496,7 @@ static corr::Grid arena_grid(const dcreg_ctx::GridArena& A, const arena_plan::Bo
 static int arena_fill(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_pts, const long long* d_seg, int n,
                       long long m, const arena_plan::Box* boxes, long long cells, double inv_cell, int rings) {
     int rc;
-    if ((rc = ensure_arena_points(ctx, A, m)) || (rc = ensure_arena_cells(ctx, A, cells))) return rc;
+    CK(A.reserve(m, cells));
     std::vector<corr::Grid> hg((size_t)n);
     std::vector<int> off((size_t)n + 1);
     for (int b = 0; b < n; ++b) {
@@ -1626,17 +1545,10 @@ static int build_hash_grid(dcreg_ctx* ctx, long long m, double inv_cell) {
     long long cap = 1024;
     while (cap < 2 * m) cap <<= 1;
     int rc;
-    if ((rc = ensure_arena_points(ctx, A, m)) || (rc = ensure_arena_cells(ctx, A, cap))) return rc;   // A.fill: per slot
-    if (ctx->hash_cap < cap) {
-        void* old[] = {ctx->d_hash_keys, ctx->d_hash_start, ctx->d_hash_count};
-        for (void* p : old)
-            if (p) cudaFree(p);
-        ctx->d_hash_keys = nullptr; ctx->d_hash_start = nullptr; ctx->d_hash_count = nullptr; ctx->hash_cap = 0;
-        CK(cudaMalloc(&ctx->d_hash_keys, (size_t)cap * sizeof(unsigned long long)));
-        CK(cudaMalloc(&ctx->d_hash_start, (size_t)cap * sizeof(int)));
-        CK(cudaMalloc(&ctx->d_hash_count, (size_t)cap * sizeof(int)));
-        ctx->hash_cap = cap;
-    }
+    CK(A.reserve(m, cap));                                                  // A.fill: per slot
+    CK(ctx->d_hash_keys.ensure(cap));
+    CK(ctx->d_hash_start.ensure(cap));
+    CK(ctx->d_hash_count.ensure(cap));
     corr::Grid g{};
     g.pts = A.pts; g.pos_of = A.pos_of; g.n = (int)m; g.dense = 0; g.rings = 1; g.inv_cell = inv_cell;
     g.keys = ctx->d_hash_keys; g.hstart = ctx->d_hash_start; g.hcount = ctx->d_hash_count; g.mask = (unsigned)(cap - 1);
@@ -1661,11 +1573,10 @@ int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, do
         return DCREG_BAD_ARG;
     }
     CK(cudaSetDevice(ctx->device));
-    if (ctx->d_tgt) cudaFree(ctx->d_tgt);
-    ctx->d_tgt = nullptr;
+    ctx->d_tgt.release();                               // not grow-only: exactly m points
     ctx->grid = corr::Grid{}; ctx->grid_cells = 0;
     ctx->has_grid = false;
-    CK(cudaMalloc(&ctx->d_tgt, (size_t)m * sizeof(float4)));
+    CK(ctx->d_tgt.ensure(m));
     ctx->n_tgt = m;
     int rc = upload_points(ctx, xyz, m, stride, nullptr, 1, ctx->d_tgt, nullptr);
     if (rc) return rc;
@@ -1717,14 +1628,9 @@ static int p2p_metrics(dcreg_ctx* ctx, int n, const float4* d_src, const long lo
         return (int)std::max<long long>(1, std::min<long long>((mx + kBlock - 1) / kBlock, cap));
     };
     const int gf = blocks(max_s), gb = blocks(max_t);
-    int rc = ensure_partials(ctx, n * (gf + gb));             // 3 doubles per block and pair, forward then backward
-    if (rc) return rc;
-    if (ctx->aligned_cap < ns) {
-        if (ctx->d_aligned) cudaFree(ctx->d_aligned);
-        ctx->d_aligned = nullptr; ctx->aligned_cap = 0;
-        CK(cudaMalloc(&ctx->d_aligned, (size_t)ns * sizeof(float4)));
-        ctx->aligned_cap = ns;
-    }
+    CK(ctx->d_partials.ensure((long long)n * (gf + gb) * kPartialDoubles));   // 3 doubles per block and pair, forward then backward
+    CK(ctx->d_aligned.ensure(ns));
+    int rc;
     double* fwd = ctx->d_partials;
     double* bwd = ctx->d_partials + (size_t)3 * n * gf;
     corr::nn1_metrics_kernel<<<dim3((unsigned)gf, (unsigned)n), kBlock, 0, ctx->stream>>>(d_src, d_src_seg, fwd_grids, d_T,
@@ -1784,22 +1690,10 @@ static int sort_source_by_cell(dcreg_ctx* ctx, const double T[16], const float4*
     *src_out = ctx->d_src;
     if (!ctx->grid.dense || ctx->n_src > 0x7fffffffLL) return DCREG_OK;
     const long long n = ctx->n_src, ncells = ctx->grid_cells;
-    if (ctx->src_sorted_cap < n) {
-        if (ctx->d_src_sorted) cudaFree(ctx->d_src_sorted);
-        if (ctx->d_sort_tmp) cudaFree(ctx->d_sort_tmp);
-        if (ctx->d_pt_cell) cudaFree(ctx->d_pt_cell);
-        ctx->d_src_sorted = nullptr; ctx->d_sort_tmp = nullptr; ctx->d_pt_cell = nullptr; ctx->src_sorted_cap = 0;
-        CK(cudaMalloc(&ctx->d_src_sorted, (size_t)n * sizeof(float4)));
-        CK(cudaMalloc(&ctx->d_sort_tmp, (size_t)n * sizeof(float4)));
-        CK(cudaMalloc(&ctx->d_pt_cell, (size_t)n * sizeof(int)));
-        ctx->src_sorted_cap = n;
-    }
-    if (ctx->cell_tmp_cap < 3 * (ncells + 1)) {
-        if (ctx->d_cell_tmp) cudaFree(ctx->d_cell_tmp);
-        ctx->d_cell_tmp = nullptr; ctx->cell_tmp_cap = 0;
-        CK(cudaMalloc(&ctx->d_cell_tmp, (size_t)3 * (ncells + 1) * sizeof(int)));
-        ctx->cell_tmp_cap = 3 * (ncells + 1);
-    }
+    CK(ctx->d_src_sorted.ensure(n));
+    CK(ctx->d_sort_tmp.ensure(n));
+    CK(ctx->d_pt_cell.ensure(n));
+    CK(ctx->d_cell_tmp.ensure(3 * (ncells + 1)));
     int* counts = ctx->d_cell_tmp;
     int* start = counts + (ncells + 1);
     int* fill = start + (ncells + 1);
@@ -1819,93 +1713,108 @@ static int sort_source_by_cell(dcreg_ctx* ctx, const double T[16], const float4*
     return DCREG_OK;
 }
 
-// The scans of a dcreg_icp_run_scans call: host points (concatenated, `stride` floats per point) and the device copies.
-struct ScanBatch {
-    int n;                      // scans (= trials)
-    const float* xyz; int stride;
-    long long total, max_n;     // points over all scans, points of the largest scan
-    const long long* seg;       // device [n + 1]: scan b = points [seg[b], seg[b+1])
-    const float* radius;        // device [n]: max |p| of each scan
-    // scan/target pairs (dcreg_icp_run_pairs): scan b against its own target grid; null / 0 for scans against the
-    // context's target
-    const corr::Grid* grids = nullptr;      // device [n] (build_grid_arena)
-    const int* cell_off = nullptr;          // device [n + 1]: first global cell of each grid in the arena
-    long long cells = 0;                    // dense cells of all grids
-    double cell_size = 0.0;
-    // sequences of frames (dcreg_icp_run_sequences): the scans are frames, run one after another in `lanes` lanes
-    // (seq.cursor set; seq.seg = seg), at most max_bodies loop bodies in all
-    int lanes = 0;
-    long long max_bodies = 0;
-    SeqView seq{};
-    // odometry (dcreg_icp_run_odometry): scan b is host frame order[b] (points from in_off), and every scan is sorted by
-    // its own cell in the sensor frame: poses sort_T (device [n][16], identities) in the box sort_grid (sort_cells cells)
+// A batch of sources registered side by side, one trial each (dcreg_icp_run_scans, _pairs, _sequences, _odometry): what
+// the loop needs to know about it.  The sources live in buffers of their own (ctx->d_scan_*): the context's source stays.
+struct Batch {
+    // the sources: n clouds of host points (`stride` floats each); offsets (host, [n + 1]): source b is points
+    // [offsets[b], offsets[b+1]) of the device copy.  order / in_off (odometry): source b is host frame order[b], points
+    // [in_off[order[b]], ..) of xyz; null: xyz in order
+    int n;
+    const float* xyz;
+    int stride;
+    const int64_t* offsets;
     const int* order = nullptr;
     const int64_t* in_off = nullptr;
+    // the sort (locality only): every source by the cells of its points under ...
+    enum Sort {
+        kContextGrid,   // ... its trial's initial pose, in the context's grid
+        kGridTable,     // ... its trial's initial pose, in its own grid of the table (cell_off, `cells` in all)
+        kBox,           // ... the poses sort_T (device [n][16]), in the box sort_box of sort_cells cells
+    } sort = kContextGrid;
     const double* sort_T = nullptr;
-    corr::Grid sort_grid{};
+    corr::Grid sort_box{};
     long long sort_cells = 0;
+    // the grid each trial searches: the context's grid, or (grid_table) its own entry of the device table `grids`, built
+    // with cell_size from the arena whose first cells are cell_off [n + 1]
+    bool grid_table = false;
+    const corr::Grid* grids = nullptr;
+    const int* cell_off = nullptr;
+    long long cells = 0;
+    double cell_size = 0.0;
+    // lanes: none (0), or the sources are frames that run one after another in `lanes` lanes (grid y of the loop kernel),
+    // at most max_bodies loop bodies in all
+    int lanes = 0;
+    SeqView seq{};
+    long long max_bodies = 0;
+
+    long long total() const { return offsets[n]; }
+    long long max_n() const {
+        long long m = 0;
+        for (int b = 0; b < n; ++b) m = std::max<long long>(m, offsets[b + 1] - offsets[b]);
+        return m;
+    }
 };
 
-static int ensure_scans(dcreg_ctx* ctx, int n_scans, long long total) {
-    if (ctx->scans_cap < n_scans) {
-        void* old[] = {ctx->d_scan_seg, ctx->d_scan_radius, ctx->d_scan_cov};
-        for (void* p : old)
-            if (p) cudaFree(p);
-        ctx->d_scan_seg = nullptr; ctx->d_scan_radius = nullptr; ctx->d_scan_cov = nullptr; ctx->scans_cap = 0;
-        CK(cudaMalloc(&ctx->d_scan_seg, (size_t)(n_scans + 1) * sizeof(long long)));
-        CK(cudaMalloc(&ctx->d_scan_radius, (size_t)n_scans * sizeof(float)));
-        CK(cudaMalloc(&ctx->d_scan_cov, (size_t)n_scans * 36 * sizeof(double)));
-        ctx->scans_cap = n_scans;
-    }
-    if (ctx->scan_cap < total) {
-        void* old[] = {ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_keys, ctx->d_scan_vals};
-        for (void* p : old)
-            if (p) cudaFree(p);
-        ctx->d_scan_src = nullptr; ctx->d_scan_sorted = nullptr; ctx->d_scan_keys = nullptr; ctx->d_scan_vals = nullptr;
-        ctx->scan_cap = 0;
-        CK(cudaMalloc(&ctx->d_scan_src, (size_t)total * sizeof(float4)));
-        CK(cudaMalloc(&ctx->d_scan_sorted, (size_t)total * sizeof(float4)));
-        CK(cudaMalloc(&ctx->d_scan_keys, (size_t)2 * total * sizeof(unsigned long long)));
-        CK(cudaMalloc(&ctx->d_scan_vals, (size_t)2 * total * sizeof(int)));
-        ctx->scan_cap = total;
-    }
+// Room for a batch's sources on the device and its offsets in ctx->d_scan_seg (the trials' states read them)
+static int stage_sources(dcreg_ctx* ctx, const Batch& S) {
+    const long long total = S.total();
+    CK(ctx->d_scan_seg.ensure(S.n + 1));
+    CK(ctx->d_scan_radius.ensure(S.n));
+    CK(ctx->d_scan_cov.ensure((long long)S.n * 36));
+    CK(ctx->d_scan_src.ensure(total));
+    CK(ctx->d_scan_sorted.ensure(total));
+    CK(ctx->d_scan_keys.ensure(2 * total));
+    CK(ctx->d_scan_vals.ensure(2 * total));
+    CK(cudaMemcpyAsync(ctx->d_scan_seg, S.offsets, (size_t)(S.n + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
     return DCREG_OK;
 }
 
-// Upload the scans, pack them with their lever arms, and sort every scan by target cell under its own initial pose
-// (ctx->d_T_init, uploaded by init_state): the scans' counterpart of dcreg_set_source + sort_source_by_cell.  One stable
-// radix sort of the (scan, cell) keys keeps the segments contiguous and in scan order and needs no per-scan cell tables.
-static int upload_scans_sorted(dcreg_ctx* ctx, const ScanBatch& S, const float4** src_out) {
-    const long long n = S.total;
-    int rc = upload_points(ctx, S.xyz, n, S.stride, S.seg, S.n, ctx->d_scan_src, ctx->d_scan_radius, S.order, S.in_off);
+// The lanes' device tables (after stage_sources): cursors, frame ranges, increments (delta null: identity) and priors
+static int stage_lanes(dcreg_ctx* ctx, int lanes, int frames, SeqView* v) {
+    CK(ctx->d_seq_cursor.ensure(lanes));
+    CK(ctx->d_seq_first.ensure(lanes + 1));
+    CK(ctx->d_seq_delta.ensure((long long)frames * 16));
+    CK(ctx->d_seq_prior.ensure((long long)frames * 16));
+    *v = SeqView{ctx->d_seq_cursor, ctx->d_seq_first, nullptr, ctx->d_seq_prior, ctx->d_scan_seg, ctx->d_n_active};
+    return DCREG_OK;
+}
+
+// Upload the staged sources, pack them with their lever arms, and sort every source by cell (Batch::sort): the batch's
+// counterpart of dcreg_set_source + sort_source_by_cell.  One stable radix sort of the (source, cell) keys keeps the
+// segments contiguous and in order and needs no per-source cell tables.
+static int sort_sources(dcreg_ctx* ctx, const Batch& S, const float4** src_out) {
+    const long long n = S.total();
+    int rc = upload_points(ctx, S.xyz, n, S.stride, ctx->d_scan_seg, S.n, ctx->d_scan_src, ctx->d_scan_radius, S.order,
+                           S.in_off);
     if (rc) return rc;
     unsigned long long* keys = ctx->d_scan_keys;
     int* vals = ctx->d_scan_vals;
+    // keys below n * the cells of the context's grid or of the box, or below the table arena's cell count
+    const double* T = ctx->d_T_init;
+    corr::Grid g = ctx->grid;
+    long long ncells = ctx->grid_cells;
+    const corr::Grid* grids = nullptr;
+    const int* cell_off = nullptr;
+    unsigned long long key_end = (unsigned long long)S.n * (unsigned long long)ctx->grid_cells;
+    if (S.sort == Batch::kGridTable) {
+        grids = S.grids; cell_off = S.cell_off;
+        key_end = (unsigned long long)S.cells;
+    } else if (S.sort == Batch::kBox) {
+        T = S.sort_T; g = S.sort_box; ncells = S.sort_cells;
+        key_end = (unsigned long long)S.n * (unsigned long long)S.sort_cells;
+    }
     const unsigned nb = (unsigned)((n + 255) / 256);
-    if (S.sort_T)
-        cell_key_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_scan_src, n, S.seg, S.n, S.sort_T, S.sort_grid, S.sort_cells,
-                                                     nullptr, nullptr, keys, vals);
-    else
-        cell_key_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_scan_src, n, S.seg, S.n, ctx->d_T_init, ctx->grid,
-                                                     ctx->grid_cells, S.grids, S.cell_off, keys, vals);
+    cell_key_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_scan_src, n, ctx->d_scan_seg, S.n, T, g, ncells, grids, cell_off,
+                                                 keys, vals);
     ctx->launches++;
     CK(cudaGetLastError());
-    // keys below n_scans * cells of the context's grid (or of the sensor-frame box), or below the arena's cell count (pairs)
-    const unsigned long long key_end = S.sort_T ? (unsigned long long)S.n * (unsigned long long)S.sort_cells
-                                       : S.grids ? (unsigned long long)S.cells
-                                                 : (unsigned long long)S.n * (unsigned long long)ctx->grid_cells;
     int end_bit = 1;
     while (end_bit < 64 && (key_end - 1ull) >> end_bit) ++end_bit;
     size_t tmp = 0;
     CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, keys, keys + n, vals, vals + n, (int)n, 0, end_bit, ctx->stream));
-    if (ctx->scan_sort_tmp_bytes < tmp) {
-        if (ctx->d_scan_sort_tmp) cudaFree(ctx->d_scan_sort_tmp);
-        ctx->d_scan_sort_tmp = nullptr; ctx->scan_sort_tmp_bytes = 0;
-        CK(cudaMalloc(&ctx->d_scan_sort_tmp, tmp));
-        ctx->scan_sort_tmp_bytes = tmp;
-    }
-    tmp = ctx->scan_sort_tmp_bytes;
-    CK(cub::DeviceRadixSort::SortPairs(ctx->d_scan_sort_tmp, tmp, keys, keys + n, vals, vals + n, (int)n, 0, end_bit,
+    CK(ctx->d_scan_sort_tmp.ensure((long long)tmp));
+    tmp = (size_t)ctx->d_scan_sort_tmp.cap;
+    CK(cub::DeviceRadixSort::SortPairs(ctx->d_scan_sort_tmp.p, tmp, keys, keys + n, vals, vals + n, (int)n, 0, end_bit,
                                        ctx->stream));
     gather_points_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_scan_src, vals + n, n, ctx->d_scan_sorted);
     ctx->launches++;                                             // (the radix sort's own kernels are not counted)
@@ -1933,48 +1842,51 @@ struct LoopPlan {
     Iter2Args b{};            // arguments of the fused2 kernel
     IterArgs a{};             // arguments of the one-thread-per-slot kernel (hash grids, seam 1)
     bool use_wd = false;
+    bool grid_table = false;  // a batch whose trials search their own grids (Batch::grid_table)
+    bool lanes = false;       // a batch in sequence lanes (b.seq)
+    const float* scan_radius = nullptr;   // the lever arms of a batch's sources, or null (the context's source)
 };
 
-// scans: a batch of different scans (trial b = scan b, src = the scans in sort order), or null (the context's source)
+// batch: a batch of sources (trial b = source b, or lane b; src = the sources in sort order), or null (the context's source)
 static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const float4* src, double4* planes_out, int trials,
-                          dcreg_iter_log* dlog, int log_cap, bool want_fold, LoopPlan* plan, const ScanBatch* scans = nullptr) {
+                          dcreg_iter_log* dlog, int log_cap, bool want_fold, LoopPlan* plan, const Batch* batch = nullptr) {
     LoopPlan& L = *plan;
     L.trials = trials; L.use_wd = prm->use_weight_derivative != 0;
+    L.grid_table = batch && batch->grid_table;
+    L.lanes = batch && batch->lanes > 0;
+    L.scan_radius = batch ? ctx->d_scan_radius.p : nullptr;
     IterArgs& a = L.a;
-    const bool pairs = scans && scans->grids;          // every trial has its own target grid (no context target needed)
-    a.src = src; a.n = scans ? scans->total : ctx->n_src; a.grid = pairs ? corr::Grid{} : ctx->grid; a.state = ctx->d_state;
+    a.src = src; a.n = batch ? batch->total() : ctx->n_src; a.grid = L.grid_table ? corr::Grid{} : ctx->grid; a.state = ctx->d_state;
     a.counter = ctx->d_counter; a.acc = ctx->d_acc;
     a.planes_out = planes_out; a.prm = *prm;
     {   // rings of cells that cover the search radius (exactness of the 5-NN-within-radius rule)
-        const int rings = search_rings(prm->search_radius, pairs ? scans->cell_size : ctx->cell_size);
+        const int rings = search_rings(prm->search_radius, L.grid_table ? batch->cell_size : ctx->cell_size);
         if (rings < 1 || rings > 4) {
             ctx->err = "search_radius / target cell_size must be in (0, 4]: rebuild the target index with a larger cell";
             return DCREG_BAD_ARG;
         }
         a.grid.rings = rings;
     }
-    L.fused2 = (pairs || ctx->grid.dense) && !planes_out && a.n <= 0x1fffffffLL && (scans || !getenv("DCREG_FUSED_SEARCH"));
-    if ((trials > 1 || scans) && !L.fused2) {
+    L.fused2 = (L.grid_table || ctx->grid.dense) && !planes_out && a.n <= 0x1fffffffLL && (batch || !getenv("DCREG_FUSED_SEARCH"));
+    if ((trials > 1 || batch) && !L.fused2) {
         ctx->err = "batched trials need the dense target grid (target bounding box / cell size too large for it)";
         return DCREG_BAD_ARG;
     }
     if (L.fused2) {
         const long long slots = ctx->n_src;
-        // per-slot records: [trials][slots], or one slice per scan at its segment offset (total slots)
-        const long long rec_slots = scans ? scans->total : slots;
-        const int rec_trials = scans ? 1 : trials;
-        if (ctx->nn_cap < rec_slots || ctx->nn_trials < rec_trials) {
-            void* old[] = {ctx->d_nn, ctx->d_plane_cache, ctx->d_fit_state, ctx->d_plane_key};
-            for (void* p : old)
-                if (p) cudaFree(p);
-            ctx->d_nn = nullptr; ctx->d_plane_cache = nullptr; ctx->d_fit_state = nullptr; ctx->d_plane_key = nullptr;
-            ctx->nn_cap = 0; ctx->nn_trials = 0;
-            const size_t tot = (size_t)rec_slots * (size_t)rec_trials;
-            CK(cudaMalloc(&ctx->d_nn, tot * kNnRec * sizeof(int4)));
-            CK(cudaMalloc(&ctx->d_plane_cache, tot * sizeof(double4)));
-            CK(cudaMalloc(&ctx->d_fit_state, tot));
-            CK(cudaMalloc(&ctx->d_plane_key, tot * 5 * sizeof(int)));
-            ctx->nn_cap = rec_slots; ctx->nn_trials = rec_trials;
+        // per-slot records: [trials][slots], or one slice per source at its segment offset (total slots); reallocated
+        // at exactly this shape when either side of it grows
+        const long long rec_slots = batch ? a.n : slots;
+        const int rec_trials = batch ? 1 : trials;
+        if (ctx->nn_slots < rec_slots || ctx->nn_trials < rec_trials) {
+            const long long tot = rec_slots * rec_trials;
+            ctx->d_nn.release(); ctx->d_plane_cache.release(); ctx->d_fit_state.release(); ctx->d_plane_key.release();
+            ctx->nn_slots = 0; ctx->nn_trials = 0;
+            CK(ctx->d_nn.ensure(tot * kNnRec));
+            CK(ctx->d_plane_cache.ensure(tot));
+            CK(ctx->d_fit_state.ensure(tot));
+            CK(ctx->d_plane_key.ensure(tot * 5));
+            ctx->nn_slots = rec_slots; ctx->nn_trials = rec_trials;
             ctx->nn_valid = false;
         }
         // the solve step inside the kernel unless the sum over ranks has to go through NCCL
@@ -1982,23 +1894,23 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
                     prm->detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm->handling == DCREG_HAND_PRECONDITIONED_CG;
         // a single folded run: block 0 is a dedicated solver block (solver_block); batches keep the ticket, since a
         // solver block per trial in a multi-wave grid could fill every resident slot with waiting blocks
-        const bool solver = L.fold_k2 && trials == 1 && !scans && !getenv("DCREG_NO_SOLVER_BLOCK");
+        const bool solver = L.fold_k2 && trials == 1 && !batch && !getenv("DCREG_NO_SOLVER_BLOCK");
         // blocks per trial and slots per block: loop_plan.hpp
-        const char* tile_env = trials == 1 && !scans ? getenv("DCREG_TILE") : nullptr;  // measurement switch
-        const loop_plan::Tiles tp = scans ? loop_plan::plan_scan_tiles(scans->max_n, kBlock)
+        const char* tile_env = trials == 1 && !batch ? getenv("DCREG_TILE") : nullptr;  // measurement switch
+        const loop_plan::Tiles tp = batch ? loop_plan::plan_scan_tiles(batch->max_n(), kBlock)
                                           : loop_plan::plan_tiles(slots, trials, ctx->sm_count, kBlock, tile_env ? atoi(tile_env) : 0,
                                                                   solver ? 1 : 0);
         L.grid_x = (int)tp.grid_x + (solver ? 1 : 0);
         L.b.tile = tp.tile;
-        int rc = ensure_partials(ctx, L.grid_x * trials);
-        if (rc) return rc;
+        CK(ctx->d_partials.ensure((long long)L.grid_x * trials * kPartialDoubles));
+        int rc;
         if (solver && (rc = ensure_row_flags(ctx, (int)tp.grid_x))) return rc;
         a.partials = ctx->d_partials;
         Iter2Args& b = L.b;
         b.it = a;
         if (solver) {
             b.row_flags = ctx->d_row_flags; b.row_epoch = ctx->d_row_epoch;
-            b.warm_state = getenv("DCREG_NO_SOLVER_WARMUP") ? nullptr : ctx->d_warm_state;   // measurement switch
+            b.warm_state = getenv("DCREG_NO_SOLVER_WARMUP") ? nullptr : ctx->d_warm_state.p;   // measurement switch
         }
         b.nn = ctx->d_nn; b.plane_cache = ctx->d_plane_cache; b.fit_state = ctx->d_fit_state; b.plane_key = ctx->d_plane_key;
         b.force = ctx->force_coherent ? 1 : 0;
@@ -2012,14 +1924,14 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         b.r2_up = r2f;
         b.fold_k2 = L.fold_k2 ? 1 : 0;
         b.log = dlog; b.log_cap = log_cap;
-        b.src_radius = scans ? scans->radius : ctx->d_src_radius; b.coherent_step = coherent_step_setting();
-        b.seg = scans ? scans->seg : nullptr;
+        b.src_radius = batch ? ctx->d_scan_radius.p : ctx->d_src_radius.p; b.coherent_step = coherent_step_setting();
+        b.seg = batch ? ctx->d_scan_seg.p : nullptr;
         // (a CUDA graph of the loop freezes this pointer, not the table: the entries are rewritten before every pairs call
         // and read at every launch, and a regrown table has a new pointer and so a new graph key)
-        b.grids = pairs ? scans->grids : nullptr;
-        // sequences: trials = lanes; the frame advance, not the solve step, counts the lanes still running
-        b.seq = scans ? scans->seq : SeqView{};
-        b.n_active = b.seq.cursor ? nullptr : ctx->d_n_active;
+        b.grids = L.grid_table ? batch->grids : nullptr;
+        // lanes: trials = lanes; the frame advance, not the solve step, counts the lanes still running
+        b.seq = L.lanes ? batch->seq : SeqView{};
+        b.n_active = L.lanes ? nullptr : ctx->d_n_active.p;
         if (ctx->peer_ok) b.peer = ctx->peer_view;
         if (!ctx->loop_attr_done) {          // per device (= per context), not per process
             CK((loop_kernel_attributes<true, false, false>)(kIter2SmemNoGrid));
@@ -2034,8 +1946,7 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         }
     } else {
         L.grid_x = stream_grid(ctx, ctx->n_src, 16);
-        int rc = ensure_partials(ctx, L.grid_x);
-        if (rc) return rc;
+        CK(ctx->d_partials.ensure(L.grid_x * kPartialDoubles));
         a.partials = ctx->d_partials;
         L.fold_k2 = false;
     }
@@ -2048,13 +1959,13 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
         L.b.use_seeds = ctx->nn_valid ? 1 : 0;
         ctx->nn_valid = true;
         const dim3 grid((unsigned)L.grid_x, (unsigned)L.trials);
-        if (L.b.grids && L.b.seq.cursor) {
+        if (L.grid_table && L.lanes) {
             if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
             else CK(launch_pdl(icp_iter2_kernel<false, true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
-        } else if (L.b.grids) {
+        } else if (L.grid_table) {
             if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, false>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
             else CK(launch_pdl(icp_iter2_kernel<false, true, false>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
-        } else if (L.b.seq.cursor) {
+        } else if (L.lanes) {
             if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
             else CK(launch_pdl(icp_iter2_kernel<false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
         } else {
@@ -2071,13 +1982,13 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
 }
 
 // the separate solve kernel (one warp per trial): baseline methods, hash-grid / seam paths, NCCL fallback of a sharded run
-// scan_radius: the per-scan lever arms of a batch of scans (ScanBatch::radius), or null (the context's source).
-// seq: the sequences of a dcreg_icp_run_sequences call (trials = lanes), or null
+// scan_radius: the lever arms of a batch's sources, or null (the context's source).
+// seq: the lanes of a batch (trials = lanes), or null
 static int launch_k2(dcreg_ctx* ctx, const dcreg_icp_params* prm, dcreg_iter_log* dlog, int log_cap, int trials = 1,
                      const float* scan_radius = nullptr, const SeqView* seq = nullptr) {
-    CK(launch_pdl(k2_step_kernel, dim3((unsigned)trials), dim3(32), 0, ctx->stream, (const double*)ctx->d_acc, ctx->d_state, *prm,
-                  dlog, log_cap, scan_radius ? scan_radius : (const float*)ctx->d_src_radius, coherent_step_setting(),
-                  trials == 1 && !seq ? ctx->d_k2_scratch : (K2Scratch*)nullptr, seq ? nullptr : ctx->d_n_active,
+    CK(launch_pdl(k2_step_kernel, dim3((unsigned)trials), dim3(32), 0, ctx->stream, (const double*)ctx->d_acc.p, ctx->d_state.p, *prm,
+                  dlog, log_cap, scan_radius ? scan_radius : (const float*)ctx->d_src_radius.p, coherent_step_setting(),
+                  trials == 1 && !seq ? ctx->d_k2_scratch.p : (K2Scratch*)nullptr, seq ? nullptr : ctx->d_n_active.p,
                   scan_radius ? 1 : 0, seq ? *seq : SeqView{}));
     ctx->launches++;
     return DCREG_OK;
@@ -2089,9 +2000,7 @@ static int launch_body(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_params* prm,
     if (rc) return rc;
     if (with_k2 && !L.fold_k2) {
         if ((rc = nccl_allreduce_acc(ctx))) return rc;          // no-op on one GPU / with peer mailboxes
-        if ((rc = launch_k2(ctx, prm, dlog, log_cap, L.trials, L.b.seg ? L.b.src_radius : nullptr,
-                            L.b.seq.cursor ? &L.b.seq : nullptr)))
-            return rc;
+        if ((rc = launch_k2(ctx, prm, dlog, log_cap, L.trials, L.scan_radius, L.lanes ? &L.b.seq : nullptr))) return rc;
     }
     return DCREG_OK;
 }
@@ -2115,8 +2024,9 @@ int dcreg_find_planes(dcreg_ctx* ctx, const double T[16], double search_radius, 
     if (!ctx || !T) return DCREG_BAD_ARG;
     if (!ctx->d_src || !ctx->has_grid) { ctx->err = "dcreg_find_planes: set source and target first"; return DCREG_BAD_ARG; }
     CK(cudaSetDevice(ctx->device));
-    int rc = ensure_planes(ctx, ctx->n_src);
-    if (rc) return rc;
+    CK(ctx->d_planes64.ensure(ctx->n_src));
+    CK(ctx->d_planes32.ensure(ctx->n_src));
+    int rc;
     dcreg_icp_params prm;
     dcreg_default_params(&prm);
     prm.search_radius = search_radius;
@@ -2174,7 +2084,8 @@ int dcreg_reduce_normal_equations_host(dcreg_ctx* ctx, const float* src4, const 
     CK(cudaSetDevice(ctx->device));
     int rc = dcreg_set_source(ctx, src4, n, 4);
     if (rc) return rc;
-    if ((rc = ensure_planes(ctx, n))) return rc;
+    CK(ctx->d_planes64.ensure(n));
+    CK(ctx->d_planes32.ensure(n));
     if (plane_is_f64)
         CK(cudaMemcpyAsync(ctx->d_planes64, plane4, (size_t)n * sizeof(double4), cudaMemcpyHostToDevice, ctx->stream));
     else
@@ -2202,10 +2113,8 @@ int dcreg_time_reduce(dcreg_ctx* ctx, int plane_is_f64, const double pose_Rt[12]
     k1::Pose P;
     for (int i = 0; i < 9; ++i) P.R[i] = pose_Rt[i];
     for (int i = 0; i < 3; ++i) P.t[i] = pose_Rt[9 + i];
-    if (flush_l2 && !ctx->d_flush) {
-        ctx->flush_n = (256ll << 20) / sizeof(float4);   // 256 MiB > 50 MB L2
-        CK(cudaMalloc(&ctx->d_flush, (size_t)ctx->flush_n * sizeof(float4)));
-    }
+    const long long flush_n = (256ll << 20) / sizeof(float4);   // 256 MiB > 50 MB L2
+    if (flush_l2) CK(ctx->d_flush.ensure(flush_n));
     const void* plane = plane_is_f64 ? (const void*)ctx->d_planes64 : (const void*)ctx->d_planes32;
     int rc = DCREG_OK;
     double total = 0.0;
@@ -2228,7 +2137,7 @@ int dcreg_time_reduce(dcreg_ctx* ctx, int plane_is_f64, const double pose_Rt[12]
         std::vector<cudaEvent_t> e0(reps), e1(reps);
         for (int i = 0; i < reps; ++i) { CK(cudaEventCreate(&e0[i])); CK(cudaEventCreate(&e1[i])); }
         for (int i = 0; i < reps && rc == DCREG_OK; ++i) {
-            flush_l2_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(ctx->d_flush, ctx->flush_n, (float)i);
+            flush_l2_kernel<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(ctx->d_flush, flush_n, (float)i);
             ctx->launches++;
             CK(cudaEventRecord(e0[i], ctx->stream));
             rc = launch_reduce(ctx, ctx->d_src, plane, plane_is_f64 != 0, ctx->n_src, &P, use_weight_derivative);
@@ -2257,8 +2166,8 @@ int dcreg_iteration_counters(dcreg_ctx* ctx, int enable, uint64_t out[2]) {
         CK(cudaStreamSynchronize(ctx->stream));
         out[0] = h[0]; out[1] = h[1];
     }
-    if (enable && !ctx->d_iter_stats) CK(cudaMalloc(&ctx->d_iter_stats, 2 * sizeof(unsigned int)));
-    if (!enable && ctx->d_iter_stats) { cudaFree(ctx->d_iter_stats); ctx->d_iter_stats = nullptr; }
+    if (enable) CK(ctx->d_iter_stats.ensure(2));
+    else ctx->d_iter_stats.release();
     if (ctx->d_iter_stats) CK(cudaMemsetAsync(ctx->d_iter_stats, 0, 2 * sizeof(unsigned int), ctx->stream));
     return DCREG_OK;
 }
@@ -2429,57 +2338,141 @@ static int enqueue_iterations(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_param
     return DCREG_OK;
 }
 
-// The loop for `trials` registrations of the context's source against its target, side by side, or (scans) of one scan
-// each.  fetch = false: enqueue only (no host synchronisation at all: no peek between chunks, no read-back)
-static int run_loop(dcreg_ctx* ctx, const dcreg_icp_params* params, int trials, const double* T_init, double* T_out,
-                    dcreg_iter_log* log, int log_cap, int* n_iterations, int* converged, int* status, bool fetch = true,
-                    const ScanBatch* scans = nullptr) {
-    int rc;
-    if (log && log_cap > 0 && (rc = ensure_log(ctx, (long long)trials * log_cap))) return rc;
-    dcreg_iter_log* dlog = (log && log_cap > 0) ? ctx->d_log : nullptr;
-    if (dlog) CK(cudaMemsetAsync(dlog, 0, (size_t)trials * log_cap * sizeof(dcreg_iter_log), ctx->stream));   // aborted iterations leave fields untouched
-    // sequences (scans->seq.cursor set): the trials are the frames, the launches' grid y the lanes
-    const bool chain = scans && scans->seq.cursor;
-    const int lanes = chain ? scans->lanes : trials;
-    if ((rc = init_state(ctx, T_init, trials, scans ? scans->seg : nullptr, lanes))) return rc;
-    if (chain)         // a lane's first prior is its T_init; the frame advance writes the others
-        CK(cudaMemcpyAsync(scans->seq.T_prior, ctx->d_T_init, (size_t)trials * 16 * sizeof(double), cudaMemcpyDeviceToDevice,
-                           ctx->stream));
-    const float4* src_iter = ctx->d_src;
-    if (scans) rc = upload_scans_sorted(ctx, *scans, &src_iter);              // each scan under its own initial pose
-    else rc = sort_source_by_cell(ctx, T_init, &src_iter);                    // locality only: any pose of the batch will do
-    if (rc) return rc;
-    LoopPlan L;
-    if ((rc = plan_iteration(ctx, params, src_iter, nullptr, lanes, dlog, dlog ? log_cap : 0, true, &L, scans))) return rc;
-    if ((rc = ensure_pinned(ctx, (size_t)trials * sizeof(IcpState)))) return rc;
-    // fixed iteration count: the whole run is one chunk; otherwise chunks of 16 with a peek at the number of running
-    // trials in between (the only host sync inside a run; iterations past convergence exit at once on the device).
-    // Sequences: chunks of 16 with a peek at the lanes still running, up to max_bodies (a frame never needs more than
-    // max_iterations bodies), whatever fixed_iterations says
-    const long long cap = chain ? scans->max_bodies : params->max_iterations;
-    const bool peek = fetch && (chain || !params->fixed_iterations);
-    const int chunk = params->fixed_iterations && !chain ? (params->max_iterations < 64 ? params->max_iterations : 64) : 16;
-    long long issued = 0;
-    while (issued < cap) {
-        long long todo = cap - issued;
-        if (todo > chunk) todo = chunk;
-        // a captured chunk is always `chunk` bodies long (one graph per run shape); bodies past max_iterations exit at once
+// Enqueue up to `cap` loop bodies in chunks of `chunk`, with a peek at the number of running trials between chunks when
+// `peek` (the only host sync inside a run; bodies past a trial's end exit at once on the device).  After the first
+// chunk, a short last chunk is padded to `chunk` bodies, so each run shape has one graph.  The peek reads through
+// h_pinned (start_loop).
+static int run_chunks(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_params* prm, dcreg_iter_log* dlog, int log_cap,
+                      long long cap, int chunk, bool peek) {
+    for (long long issued = 0; issued < cap;) {
+        const long long todo = std::min<long long>(cap - issued, chunk);
         const int bodies = (todo < chunk && issued > 0) ? chunk : (int)todo;
-        if ((rc = enqueue_iterations(ctx, L, params, dlog, dlog ? log_cap : 0, bodies))) return rc;
+        const int rc = enqueue_iterations(ctx, L, prm, dlog, log_cap, bodies);
+        if (rc) return rc;
         issued += bodies;
         if (peek && issued < cap) {
-            unsigned int* flag = (unsigned int*)ctx->h_pinned;       // trials still running (every solve step that finishes one decrements it)
+            unsigned int* flag = (unsigned int*)ctx->h_pinned.p;       // every solve step that finishes a trial decrements it
             CK(cudaMemcpyAsync(flag, ctx->d_n_active, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
             CK(cudaStreamSynchronize(ctx->stream));
             if (*flag == 0u) break;
         }
     }
+    return DCREG_OK;
+}
+
+// Where a call's per-trial outputs go, in the caller's order (null: not wanted)
+struct Results {
+    double* T_out = nullptr;
+    int* n_iterations = nullptr;
+    int* converged = nullptr;
+    int* status = nullptr;
+    dcreg_iter_log* log = nullptr;
+    int log_cap = 0;                 // records per trial
+    double* cov = nullptr;           // [trials][36] by covariance_kernel's rule
+    double* T_prior = nullptr;       // [trials][16] the prior each frame started from (lanes)
+};
+
+// The device log of `trials` registrations when the call wants one (*dlog = null otherwise), zeroed: aborted iterations
+// leave fields untouched
+static int setup_log(dcreg_ctx* ctx, const Results& r, int trials, dcreg_iter_log** dlog) {
+    *dlog = nullptr;
+    if (!r.log || r.log_cap <= 0) return DCREG_OK;
+    const long long records = (long long)trials * r.log_cap;
+    CK(ctx->d_log.ensure(records));
+    CK(cudaMemsetAsync(ctx->d_log, 0, (size_t)records * sizeof(dcreg_iter_log), ctx->stream));
+    *dlog = ctx->d_log;
+    return DCREG_OK;
+}
+
+// Before a loop: the log, every trial's state, the sources in sort order (the context's source, or the staged sources of
+// a batch), the lanes' first priors, and the pinned buffer of the peeks and read_results
+static int start_loop(dcreg_ctx* ctx, int trials, const double* T_init, const Results& r, const Batch* batch,
+                      dcreg_iter_log** dlog, const float4** src) {
+    const bool lanes = batch && batch->lanes > 0;
+    int rc;
+    if ((rc = setup_log(ctx, r, trials, dlog))) return rc;
+    if ((rc = init_state(ctx, T_init, trials, batch ? ctx->d_scan_seg.p : nullptr, lanes ? batch->lanes : trials))) return rc;
+    if (batch) rc = sort_sources(ctx, *batch, src);
+    else rc = sort_source_by_cell(ctx, T_init, src);             // locality only: any pose of the batch will do
+    if (rc) return rc;
+    if (lanes)         // a lane's first prior is its T_init; the frame advance writes the others
+        CK(cudaMemcpyAsync(batch->seq.T_prior, ctx->d_T_init, (size_t)trials * 16 * sizeof(double), cudaMemcpyDeviceToDevice,
+                           ctx->stream));
+    CK(ctx->h_pinned.ensure((long long)trials * sizeof(IcpState)));
+    return DCREG_OK;
+}
+
+// The end of a call, after its loop: the log's fill-in, the results, then the covariances and the priors when asked for.
+// dev (odometry): the caller's trial k is device trial dev[k], and only the device trials below `done` are returned;
+// null: the same order, every trial.
+static int finish_call(dcreg_ctx* ctx, const dcreg_icp_params* prm, int trials, dcreg_iter_log* dlog, const Results& r,
+                       const int* dev = nullptr, int done = 0) {
     if (dlog) {
-        log_fill_kernel<<<dim3((log_cap + 31) / 32, trials), 32, 0, ctx->stream>>>(dlog, log_cap, ctx->d_state, *params);
+        log_fill_kernel<<<dim3((r.log_cap + 31) / 32, trials), 32, 0, ctx->stream>>>(dlog, r.log_cap, ctx->d_state, *prm);
         ctx->launches++;
     }
+    // device order: straight into the caller's arrays, or into host copies that are put in the caller's order below
+    Results d = r;
+    std::vector<double> To, cv, Tp;
+    std::vector<int> it, cg, st;
+    std::vector<dcreg_iter_log> lg;
+    if (dev) {
+        To.resize((size_t)trials * 16); it.resize(trials); cg.resize(trials); st.resize(trials);
+        d.T_out = To.data(); d.n_iterations = it.data(); d.converged = cg.data(); d.status = st.data();
+        if (dlog) { lg.resize((size_t)trials * r.log_cap); d.log = lg.data(); }
+        if (r.cov) { cv.resize((size_t)trials * 36); d.cov = cv.data(); }
+        if (r.T_prior) { Tp.resize((size_t)trials * 16); d.T_prior = Tp.data(); }
+    }
+    int rc = read_results(ctx, trials, d.T_out, dlog ? d.log : nullptr, r.log_cap, d.n_iterations, d.converged, d.status);
+    if (rc) return rc;
+    if (r.cov) {
+        covariance_kernel<<<trials, 32, 0, ctx->stream>>>(ctx->d_state, ctx->d_scan_cov);
+        ctx->launches++;
+        CK(cudaGetLastError());
+        CK(cudaMemcpyAsync(d.cov, ctx->d_scan_cov, (size_t)trials * 36 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    }
+    if (r.T_prior)
+        CK(cudaMemcpyAsync(d.T_prior, ctx->d_seq_prior, (size_t)trials * 16 * sizeof(double), cudaMemcpyDeviceToHost,
+                           ctx->stream));
+    if (r.cov || r.T_prior) CK(cudaStreamSynchronize(ctx->stream));
+    if (!dev) return DCREG_OK;
+    for (int k = 0; k < trials; ++k) {
+        const size_t t = (size_t)dev[k];
+        if ((int)t >= done) continue;
+        memcpy(r.T_out + (size_t)k * 16, &To[t * 16], 16 * sizeof(double));
+        if (r.n_iterations) r.n_iterations[k] = it[t];
+        if (r.converged) r.converged[k] = cg[t];
+        if (r.status) r.status[k] = st[t];
+        if (dlog) memcpy(r.log + (size_t)k * r.log_cap, &lg[t * r.log_cap], (size_t)r.log_cap * sizeof(dcreg_iter_log));
+        if (r.cov) memcpy(r.cov + (size_t)k * 36, &cv[t * 36], 36 * sizeof(double));
+        if (r.T_prior) memcpy(r.T_prior + (size_t)k * 16, &Tp[t * 16], 16 * sizeof(double));
+    }
+    return DCREG_OK;
+}
+
+// The loop for `trials` registrations side by side: of the context's source (batch null), or of the staged sources of a
+// batch (stage_sources), whose lanes, if any, run the trials as frames.  fetch = false: enqueue only (no host
+// synchronisation at all: no peek between chunks, no read-back)
+static int run_loop(dcreg_ctx* ctx, const dcreg_icp_params* params, int trials, const double* T_init, const Results& r,
+                    bool fetch = true, const Batch* batch = nullptr) {
+    dcreg_iter_log* dlog = nullptr;
+    const float4* src = nullptr;
+    int rc = start_loop(ctx, trials, T_init, r, batch, &dlog, &src);
+    if (rc) return rc;
+    const bool lanes = batch && batch->lanes > 0;
+    LoopPlan L;
+    if ((rc = plan_iteration(ctx, params, src, nullptr, lanes ? batch->lanes : trials, dlog, dlog ? r.log_cap : 0, true, &L,
+                             batch)))
+        return rc;
+    // fixed iteration count: the whole run is one chunk; otherwise chunks of 16 with a peek in between.  Lanes: chunks
+    // of 16 with a peek at the lanes still running, up to max_bodies (a frame never needs more than max_iterations
+    // bodies), whatever fixed_iterations says
+    const long long cap = lanes ? batch->max_bodies : params->max_iterations;
+    const int chunk = params->fixed_iterations && !lanes ? std::min(params->max_iterations, 64) : 16;
+    const bool peek = fetch && (lanes || !params->fixed_iterations);
+    if ((rc = run_chunks(ctx, L, params, dlog, dlog ? r.log_cap : 0, cap, chunk, peek))) return rc;
     if (!fetch) return DCREG_OK;
-    return read_results(ctx, trials, T_out, log, log_cap, n_iterations, converged, status);
+    return finish_call(ctx, params, trials, dlog, r);
 }
 
 // need_source = false: the run brings its own source points (dcreg_icp_run_scans); need_target = false: and its own
@@ -2503,7 +2496,7 @@ int dcreg_icp_run(dcreg_ctx* ctx, const dcreg_icp_params* params, const double T
     if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
     int status = DCREG_OK;
-    if ((rc = run_loop(ctx, params, 1, T_init, T_out, log, log_cap, n_iterations, converged, &status))) return rc;
+    if ((rc = run_loop(ctx, params, 1, T_init, Results{T_out, n_iterations, converged, &status, log, log_cap}))) return rc;
     return status;
 }
 
@@ -2513,7 +2506,7 @@ int dcreg_icp_enqueue(dcreg_ctx* ctx, const dcreg_icp_params* params, const doub
     int rc = check_run_args(ctx, params);
     if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
-    return run_loop(ctx, params, 1, T_init, nullptr, nullptr, 0, nullptr, nullptr, nullptr, false);
+    return run_loop(ctx, params, 1, T_init, Results{}, false);
 }
 
 int dcreg_icp_fetch(dcreg_ctx* ctx, double T_out[16], int* n_iterations, int* converged) {
@@ -2525,113 +2518,91 @@ int dcreg_icp_fetch(dcreg_ctx* ctx, double T_out[16], int* n_iterations, int* co
     return rc ? rc : status;
 }
 
-// The trials of one call are the loop kernel's grid y: at most kMaxPairs.  offsets (scans, pairs): the sources' table
-static int check_batch(dcreg_ctx* ctx, int n, const int64_t* offsets, const char* what) {
-    std::string why;
-    if (n > arena_plan::kMaxPairs)
-        why = std::string(what) + ": more than " + std::to_string(arena_plan::kMaxPairs) + " trials in one call";
-    else if (offsets)
-        why = arena_plan::check_offsets(n, offsets, arena_plan::kMaxPoints, what);
-    if (why.empty()) return DCREG_OK;
-    ctx->err = why;
-    return DCREG_BAD_ARG;
+// What a batched call (dcreg_icp_run_batch, _scans, _pairs, _sequences, _odometry) needs checked before anything is
+// launched.  Every message of its own starts with the call's name.
+struct BatchCheck {
+    const char* name;                   // "icp_run_scans"
+    bool args_ok;                       // no null pointer, positive counts ...
+    const char* args_msg;               // ... or what is wrong
+    const char* shard_msg;              // why a sharded context is refused
+    int n;                              // trials: at most kMaxPairs (the loop kernel's grid y)
+    const int64_t* offsets = nullptr;   // the sources' table (null: trials of the context's source) ...
+    const char* item = nullptr;         // ... and what a source is called in its messages
+    int stride = 3;
+    bool own_cell = false;              // the call builds its own grids with cell_size (search rings in [1, 4])
+    double cell_size = 0.0;
+    const char* own_msg = nullptr;      // a check of the call's own that failed, reported after the cell size
+    bool need_source = false, need_target = true;    // check_run_args
+    bool one_iteration = false;         // max_iterations >= 1
+    const char* dense = nullptr;        // the context's dense grid is needed by these ("batches")
+    int n_seqs = 0;                     // the sequence table [n_seqs + 1]: from 0, ascending strictly, up to n
+    const int* seq_offsets = nullptr;
+};
+
+static int check_batch_call(dcreg_ctx* ctx, const dcreg_icp_params* params, const BatchCheck& c) {
+    const std::string name(c.name);
+    auto bad = [ctx](const std::string& why) { ctx->err = why; return (int)DCREG_BAD_ARG; };
+    if (!c.args_ok) return bad(name + ": " + c.args_msg);
+    if (c.offsets && c.stride < 3) return bad(name + ": stride < 3");
+    if (c.own_cell && !(c.cell_size > 0.0)) return bad(name + ": cell_size <= 0");
+    if (c.own_msg) return bad(name + ": " + c.own_msg);
+    if (ctx->comm) return bad(name + ": " + c.shard_msg);
+    const std::string what = c.item ? name + ": " + c.item : name;
+    const std::string too_many = what + ": more than " + std::to_string(arena_plan::kMaxPairs) + " trials in one call";
+    if (!c.offsets && c.n > arena_plan::kMaxPairs) return bad(too_many);   // trials of the context's source: no table
+    const int rc = check_run_args(ctx, params, c.need_source, c.need_target);
+    if (rc) return rc;
+    if (c.one_iteration && params->max_iterations < 1) return bad(name + ": max_iterations must be >= 1");
+    if (c.dense && !ctx->grid.dense)
+        return bad(name + ": " + c.dense + " need the dense target grid (target bounding box / cell size too large for it)");
+    if (c.own_cell) {
+        const int rings = search_rings(params->search_radius, c.cell_size);
+        if (rings < 1 || rings > 4) return bad(name + ": search_radius / cell_size must be in (0, 4]");
+    }
+    if (c.offsets) {
+        if (c.n > arena_plan::kMaxPairs) return bad(too_many);
+        const std::string why = arena_plan::check_offsets(c.n, c.offsets, arena_plan::kMaxPoints, what.c_str());
+        if (!why.empty()) return bad(why);
+    }
+    if (c.seq_offsets) {
+        const int* so = c.seq_offsets;
+        if (so[0] != 0) return bad(name + ": seq_offsets must start at 0");
+        for (int s = 0; s < c.n_seqs; ++s)
+            if (so[s + 1] <= so[s])
+                return bad(name + ": sequence " + std::to_string(s) + " is empty (seq_offsets must ascend strictly)");
+        if (so[c.n_seqs] != c.n)
+            return bad(name + ": seq_offsets[n_seqs] = " + std::to_string(so[c.n_seqs]) + " but n_frames = " + std::to_string(c.n));
+    }
+    return DCREG_OK;
 }
 
 int dcreg_icp_run_batch(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_trials, const double* T_init,
                         double* T_out, int* n_iterations, int* converged, int* status, dcreg_iter_log* log, int log_cap) {
     if (!ctx) return DCREG_BAD_ARG;
-    if (!params || !T_init || !T_out || n_trials <= 0) { ctx->err = "icp_run_batch: null pointer or n_trials <= 0"; return DCREG_BAD_ARG; }
-    if (ctx->comm) { ctx->err = "icp_run_batch: trials are independent - distribute them over ranks, do not shard them"; return DCREG_BAD_ARG; }
-    int rc = check_batch(ctx, n_trials, nullptr, "icp_run_batch");
-    if (rc || (rc = check_run_args(ctx, params))) return rc;
-    CK(cudaSetDevice(ctx->device));
-    std::vector<int> st_local;
-    if (!status) { st_local.resize(n_trials); status = st_local.data(); }
-    return run_loop(ctx, params, n_trials, T_init, T_out, log, log_cap, n_iterations, converged, status);
-}
-
-// What dcreg_icp_run_scans and dcreg_icp_run_pairs share once check_batch has passed their sources' offsets: S.n
-// sources (S.xyz, S.stride; S.grids etc. for pairs) registered side by side, one trial each, then covariance_kernel's
-// rule per trial.  Leaves the packed sources in ctx->d_scan_src and their offsets in ctx->d_scan_seg.
-static int run_sources(dcreg_ctx* ctx, const dcreg_icp_params* params, ScanBatch S, const int64_t* offsets,
-                       const double* T_init, double* T_out, int* n_iterations, int* converged, int* status, double* cov,
-                       dcreg_iter_log* log, int log_cap) {
-    S.total = offsets[S.n];
-    for (int b = 0; b < S.n; ++b) S.max_n = std::max<long long>(S.max_n, offsets[b + 1] - offsets[b]);
-    int rc = ensure_scans(ctx, S.n, S.total);
+    BatchCheck c{"icp_run_batch", params && T_init && T_out && n_trials > 0, "null pointer or n_trials <= 0",
+                 "trials are independent - distribute them over ranks, do not shard them", n_trials};
+    c.need_source = true;
+    int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->d_scan_seg, offsets, (size_t)(S.n + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
-    S.seg = ctx->d_scan_seg; S.radius = ctx->d_scan_radius;
-    S.seq.seg = S.seg;                                  // (read only by sequences)
-    std::vector<int> st_local;
-    if (!status) { st_local.resize(S.n); status = st_local.data(); }
-    if ((rc = run_loop(ctx, params, S.n, T_init, T_out, log, log_cap, n_iterations, converged, status, true, &S))) return rc;
-    if (cov) {
-        covariance_kernel<<<S.n, 32, 0, ctx->stream>>>(ctx->d_state, ctx->d_scan_cov);
-        ctx->launches++;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(cov, ctx->d_scan_cov, (size_t)S.n * 36 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-    }
-    return DCREG_OK;
+    CK(cudaSetDevice(ctx->device));
+    return run_loop(ctx, params, n_trials, T_init, Results{T_out, n_iterations, converged, status, log, log_cap});
 }
 
 int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_scans, const float* xyz,
                         const int64_t* scan_offsets, int stride, const double* T_init, double* T_out, int* n_iterations,
                         int* converged, int* status, double* cov, dcreg_iter_log* log, int log_cap) {
     if (!ctx) return DCREG_BAD_ARG;
-    if (!params || n_scans <= 0 || !xyz || !scan_offsets || !T_init || !T_out) {
-        ctx->err = "icp_run_scans: null pointer or n_scans <= 0";
-        return DCREG_BAD_ARG;
-    }
-    if (stride < 3) { ctx->err = "icp_run_scans: stride < 3"; return DCREG_BAD_ARG; }
-    if (ctx->comm) { ctx->err = "icp_run_scans: scans are independent - distribute them over ranks, do not shard them"; return DCREG_BAD_ARG; }
-    int rc = check_run_args(ctx, params, false);
+    BatchCheck c{"icp_run_scans", params && n_scans > 0 && xyz && scan_offsets && T_init && T_out,
+                 "null pointer or n_scans <= 0", "scans are independent - distribute them over ranks, do not shard them",
+                 n_scans};
+    c.offsets = scan_offsets; c.item = "scan"; c.stride = stride; c.dense = "batches";
+    int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
-    if (!ctx->grid.dense) {
-        ctx->err = "icp_run_scans: batches need the dense target grid (target bounding box / cell size too large for it)";
-        return DCREG_BAD_ARG;
-    }
-    if ((rc = check_batch(ctx, n_scans, scan_offsets, "icp_run_scans: scan"))) return rc;
     CK(cudaSetDevice(ctx->device));
-    return run_sources(ctx, params, ScanBatch{n_scans, xyz, stride}, scan_offsets, T_init, T_out, n_iterations, converged,
-                       status, cov, log, log_cap);
-}
-
-// the sequences' own device buffers (dcreg_icp_run_sequences): lane cursors and frame ranges, increments, priors
-static int ensure_sequences(dcreg_ctx* ctx, int n_seqs, int n_frames) {
-    if (ctx->seq_lanes_cap < n_seqs) {
-        if (ctx->d_seq_cursor) cudaFree(ctx->d_seq_cursor);
-        if (ctx->d_seq_first) cudaFree(ctx->d_seq_first);
-        ctx->d_seq_cursor = nullptr; ctx->d_seq_first = nullptr; ctx->seq_lanes_cap = 0;
-        CK(cudaMalloc(&ctx->d_seq_cursor, (size_t)n_seqs * sizeof(int)));
-        CK(cudaMalloc(&ctx->d_seq_first, (size_t)(n_seqs + 1) * sizeof(int)));
-        ctx->seq_lanes_cap = n_seqs;
-    }
-    if (ctx->seq_frames_cap < n_frames) {
-        if (ctx->d_seq_delta) cudaFree(ctx->d_seq_delta);
-        if (ctx->d_seq_prior) cudaFree(ctx->d_seq_prior);
-        ctx->d_seq_delta = nullptr; ctx->d_seq_prior = nullptr; ctx->seq_frames_cap = 0;
-        CK(cudaMalloc(&ctx->d_seq_delta, (size_t)n_frames * 16 * sizeof(double)));
-        CK(cudaMalloc(&ctx->d_seq_prior, (size_t)n_frames * 16 * sizeof(double)));
-        ctx->seq_frames_cap = n_frames;
-    }
-    return DCREG_OK;
-}
-
-// the sequence table: n_seqs + 1 entries from 0, ascending strictly (no empty sequence), up to n_frames
-static int check_seq_offsets(dcreg_ctx* ctx, int n_seqs, const int* seq_offsets, int n_frames, const char* what) {
-    std::string why;
-    const std::string w(what);
-    if (seq_offsets[0] != 0) why = w + ": seq_offsets must start at 0";
-    for (int s = 0; s < n_seqs && why.empty(); ++s)
-        if (seq_offsets[s + 1] <= seq_offsets[s])
-            why = w + ": sequence " + std::to_string(s) + " is empty (seq_offsets must ascend strictly)";
-    if (why.empty() && seq_offsets[n_seqs] != n_frames)
-        why = w + ": seq_offsets[n_seqs] = " + std::to_string(seq_offsets[n_seqs]) + " but n_frames = " + std::to_string(n_frames);
-    if (why.empty()) return DCREG_OK;
-    ctx->err = why;
-    return DCREG_BAD_ARG;
+    const Batch S{n_scans, xyz, stride, scan_offsets};
+    if ((rc = stage_sources(ctx, S))) return rc;
+    return run_loop(ctx, params, n_scans, T_init, Results{T_out, n_iterations, converged, status, log, log_cap, cov}, true,
+                    &S);
 }
 
 int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
@@ -2640,27 +2611,20 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
                             int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
                             int log_cap) {
     if (!ctx) return DCREG_BAD_ARG;
-    if (!params || n_seqs <= 0 || n_frames <= 0 || !seq_offsets || !xyz || !frame_offsets || !T_init || !T_out) {
-        ctx->err = "icp_run_sequences: null pointer, n_seqs <= 0 or n_frames <= 0";
-        return DCREG_BAD_ARG;
-    }
-    if (stride < 3) { ctx->err = "icp_run_sequences: stride < 3"; return DCREG_BAD_ARG; }
-    if (ctx->comm) { ctx->err = "icp_run_sequences: sequences are independent - give each rank its own, do not shard them"; return DCREG_BAD_ARG; }
-    int rc = check_run_args(ctx, params, false);
+    BatchCheck c{"icp_run_sequences", params && n_seqs > 0 && n_frames > 0 && seq_offsets && xyz && frame_offsets && T_init && T_out,
+                 "null pointer, n_seqs <= 0 or n_frames <= 0",
+                 "sequences are independent - give each rank its own, do not shard them", n_frames};
+    c.offsets = frame_offsets; c.item = "frame"; c.stride = stride; c.one_iteration = true; c.dense = "sequences";
+    c.n_seqs = n_seqs; c.seq_offsets = seq_offsets;
+    int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
-    if (params->max_iterations < 1) { ctx->err = "icp_run_sequences: max_iterations must be >= 1"; return DCREG_BAD_ARG; }
-    if (!ctx->grid.dense) {
-        ctx->err = "icp_run_sequences: sequences need the dense target grid (target bounding box / cell size too large for it)";
-        return DCREG_BAD_ARG;
-    }
-    if ((rc = check_batch(ctx, n_frames, frame_offsets, "icp_run_sequences: frame"))) return rc;
-    if ((rc = check_seq_offsets(ctx, n_seqs, seq_offsets, n_frames, "icp_run_sequences"))) return rc;
     CK(cudaSetDevice(ctx->device));
     // every frame is sorted by target cell under its dead-reckoned prior (T_init composed with the increments alone):
     // the sort only buys locality, and the chained prior is not known before the frame before it has run
     static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
     std::vector<double> T_dr((size_t)n_frames * 16);
-    long long max_bodies = 0;
+    Batch S{n_frames, xyz, stride, frame_offsets};
+    S.lanes = n_seqs;
     for (int s = 0; s < n_seqs; ++s) {
         const int f0 = seq_offsets[s], f1 = seq_offsets[s + 1];
         memcpy(&T_dr[(size_t)f0 * 16], T_init + (size_t)s * 16, 16 * sizeof(double));
@@ -2669,50 +2633,17 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
             const double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]}, t[3] = {T[3], T[7], T[11]};
             compose_prior(R, t, deltas ? deltas + (size_t)(f - 1) * 16 : kIdentity, &T_dr[(size_t)f * 16]);
         }
-        max_bodies = std::max<long long>(max_bodies, (long long)(f1 - f0) * params->max_iterations);
+        S.max_bodies = std::max<long long>(S.max_bodies, (long long)(f1 - f0) * params->max_iterations);
     }
-    if ((rc = ensure_sequences(ctx, n_seqs, n_frames))) return rc;
+    if ((rc = stage_sources(ctx, S)) || (rc = stage_lanes(ctx, n_seqs, n_frames, &S.seq))) return rc;
     CK(cudaMemcpyAsync(ctx->d_seq_first, seq_offsets, (size_t)(n_seqs + 1) * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_seq_cursor, seq_offsets, (size_t)n_seqs * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-    if (deltas)
+    if (deltas) {
         CK(cudaMemcpyAsync(ctx->d_seq_delta, deltas, (size_t)n_frames * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    ScanBatch S{n_frames, xyz, stride};
-    S.lanes = n_seqs;
-    S.max_bodies = max_bodies;
-    S.seq.cursor = ctx->d_seq_cursor; S.seq.first = ctx->d_seq_first; S.seq.delta = deltas ? ctx->d_seq_delta : nullptr;
-    S.seq.T_prior = ctx->d_seq_prior; S.seq.n_active = ctx->d_n_active;
-    if ((rc = run_sources(ctx, params, S, frame_offsets, T_dr.data(), T_out, n_iterations, converged, status, cov, log,
-                          log_cap)))
-        return rc;
-    if (T_prior) {
-        CK(cudaMemcpyAsync(T_prior, ctx->d_seq_prior, (size_t)n_frames * 16 * sizeof(double), cudaMemcpyDeviceToHost,
-                           ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
+        S.seq.delta = ctx->d_seq_delta;
     }
-    return DCREG_OK;
-}
-
-// the odometry's own device buffers (dcreg_icp_run_odometry): every step's tables, one step's local maps
-static int ensure_odometry(dcreg_ctx* ctx, long long n_ll, long long n_int, long long map_points) {
-    if (ctx->odom_ll_cap < n_ll) {
-        if (ctx->d_odom_ll) cudaFree(ctx->d_odom_ll);
-        ctx->d_odom_ll = nullptr; ctx->odom_ll_cap = 0;
-        CK(cudaMalloc(&ctx->d_odom_ll, (size_t)n_ll * sizeof(long long)));
-        ctx->odom_ll_cap = n_ll;
-    }
-    if (ctx->odom_int_cap < n_int) {
-        if (ctx->d_odom_int) cudaFree(ctx->d_odom_int);
-        ctx->d_odom_int = nullptr; ctx->odom_int_cap = 0;
-        CK(cudaMalloc(&ctx->d_odom_int, (size_t)n_int * sizeof(int)));
-        ctx->odom_int_cap = n_int;
-    }
-    if (ctx->odom_map_cap < map_points) {
-        if (ctx->d_odom_map) cudaFree(ctx->d_odom_map);
-        ctx->d_odom_map = nullptr; ctx->odom_map_cap = 0;
-        CK(cudaMalloc(&ctx->d_odom_map, (size_t)map_points * sizeof(float4)));
-        ctx->odom_map_cap = map_points;
-    }
-    return DCREG_OK;
+    return run_loop(ctx, params, n_frames, T_dr.data(),
+                    Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, true, &S);
 }
 
 int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
@@ -2721,29 +2652,18 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
                            double* T_out, int* n_iterations, int* converged, int* status, double* cov,
                            dcreg_iter_log* log, int log_cap) {
     if (!ctx) return DCREG_BAD_ARG;
-    if (!params || n_seqs <= 0 || n_frames <= 0 || !seq_offsets || !xyz || !frame_offsets || !T_init || !T_out) {
-        ctx->err = "icp_run_odometry: null pointer, n_seqs <= 0 or n_frames <= 0";
-        return DCREG_BAD_ARG;
-    }
-    if (stride < 3) { ctx->err = "icp_run_odometry: stride < 3"; return DCREG_BAD_ARG; }
-    if (!(cell_size > 0.0)) { ctx->err = "icp_run_odometry: cell_size <= 0"; return DCREG_BAD_ARG; }
-    if (map_frames < 1) { ctx->err = "icp_run_odometry: map_frames must be >= 1"; return DCREG_BAD_ARG; }
-    if (motion != DCREG_MOTION_INCREMENTS && motion != DCREG_MOTION_CONSTANT_VELOCITY) {
-        ctx->err = "icp_run_odometry: motion must be DCREG_MOTION_INCREMENTS or DCREG_MOTION_CONSTANT_VELOCITY";
-        return DCREG_BAD_ARG;
-    }
-    if (motion == DCREG_MOTION_CONSTANT_VELOCITY && deltas) {
-        ctx->err = "icp_run_odometry: the constant-velocity model takes no deltas (pass NULL)";
-        return DCREG_BAD_ARG;
-    }
-    if (ctx->comm) { ctx->err = "icp_run_odometry: sequences are independent - give each rank its own, do not shard them"; return DCREG_BAD_ARG; }
-    int rc = check_run_args(ctx, params, false, false);
+    BatchCheck c{"icp_run_odometry", params && n_seqs > 0 && n_frames > 0 && seq_offsets && xyz && frame_offsets && T_init && T_out,
+                 "null pointer, n_seqs <= 0 or n_frames <= 0",
+                 "sequences are independent - give each rank its own, do not shard them", n_frames};
+    c.offsets = frame_offsets; c.item = "frame"; c.stride = stride; c.own_cell = true; c.cell_size = cell_size;
+    c.need_target = false; c.one_iteration = true; c.n_seqs = n_seqs; c.seq_offsets = seq_offsets;
+    if (map_frames < 1) c.own_msg = "map_frames must be >= 1";
+    else if (motion != DCREG_MOTION_INCREMENTS && motion != DCREG_MOTION_CONSTANT_VELOCITY)
+        c.own_msg = "motion must be DCREG_MOTION_INCREMENTS or DCREG_MOTION_CONSTANT_VELOCITY";
+    else if (motion == DCREG_MOTION_CONSTANT_VELOCITY && deltas)
+        c.own_msg = "the constant-velocity model takes no deltas (pass NULL)";
+    int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
-    if (params->max_iterations < 1) { ctx->err = "icp_run_odometry: max_iterations must be >= 1"; return DCREG_BAD_ARG; }
-    const int rings = search_rings(params->search_radius, cell_size);
-    if (rings < 1 || rings > 4) { ctx->err = "icp_run_odometry: search_radius / cell_size must be in (0, 4]"; return DCREG_BAD_ARG; }
-    if ((rc = check_batch(ctx, n_frames, frame_offsets, "icp_run_odometry: frame"))) return rc;
-    if ((rc = check_seq_offsets(ctx, n_seqs, seq_offsets, n_frames, "icp_run_odometry"))) return rc;
     odom_plan::Plan P;
     {
         const std::string why = odom_plan::make(n_seqs, seq_offsets, n_frames, frame_offsets, map_frames,
@@ -2767,17 +2687,27 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
         hint.insert(hint.end(), st.prev.begin(), st.prev.end());
         hint.insert(hint.end(), st.prev2.begin(), st.prev2.end());
     }
-    const long long total = P.dev_off[(size_t)n_frames];
-    if ((rc = ensure_scans(ctx, n_frames, total)) || (rc = ensure_sequences(ctx, n_seqs, n_frames)) ||
-        (rc = ensure_odometry(ctx, std::max<long long>((long long)hll.size(), 1), std::max<long long>((long long)hint.size(), 1),
-                              std::max<long long>(P.max_map, 1))))
-        return rc;
+    // the frames in device order, each sorted by its own cell in the sensor frame (identity poses, a box of 1024^3 cells
+    // around the sensor: locality only, the chained priors are not known yet); lanes: grid y of the loop kernel, a
+    // lane's frame range set by odom_start_kernel at every step; grids: the step's local maps
+    Batch S{n_frames, xyz, stride, P.dev_off.data()};
+    S.order = P.input.data(); S.in_off = frame_offsets;
+    S.sort = Batch::kBox;
+    S.sort_box.inv_cell = 1.0 / cell_size;
+    S.sort_box.ox = S.sort_box.oy = S.sort_box.oz = -512;
+    S.sort_box.nx = S.sort_box.ny = S.sort_box.nz = 1024;
+    S.sort_cells = 1ll << 30;
+    S.grid_table = true; S.cell_size = cell_size;
+    S.lanes = n_seqs;
+    if ((rc = stage_sources(ctx, S)) || (rc = stage_lanes(ctx, n_seqs, n_frames, &S.seq))) return rc;
+    S.sort_T = ctx->d_seq_prior;
+    CK(ctx->d_odom_ll.ensure(std::max<long long>((long long)hll.size(), 1)));
+    CK(ctx->d_odom_int.ensure(std::max<long long>((long long)hint.size(), 1)));
+    CK(ctx->d_odom_map.ensure(std::max<long long>(P.max_map, 1)));
     if (!hll.empty()) {
         CK(cudaMemcpyAsync(ctx->d_odom_ll, hll.data(), hll.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaMemcpyAsync(ctx->d_odom_int, hint.data(), hint.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     }
-    CK(cudaMemcpyAsync(ctx->d_scan_seg, P.dev_off.data(), (size_t)(n_frames + 1) * sizeof(long long), cudaMemcpyHostToDevice,
-                       ctx->stream));
     // device order: every frame's loop state starts at its sequence's T_init (an anchor keeps it: T_out = T_prior =
     // T_init, no iteration, not converged), the increments follow the frames
     std::vector<double> T_dev((size_t)n_frames * 16), ident((size_t)n_frames * 16, 0.0), D_dev;
@@ -2785,40 +2715,18 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
         for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k)
             memcpy(&T_dev[(size_t)P.dev[(size_t)k] * 16], T_init + (size_t)s * 16, 16 * sizeof(double));
     for (int d = 0; d < n_frames; ++d)
-        for (int c = 0; c < 4; ++c) ident[(size_t)d * 16 + 5 * c] = 1.0;
+        for (int c4 = 0; c4 < 4; ++c4) ident[(size_t)d * 16 + 5 * c4] = 1.0;
     if (deltas) {
         D_dev.resize((size_t)n_frames * 16);
         for (int k = 0; k < n_frames; ++k) memcpy(&D_dev[(size_t)P.dev[(size_t)k] * 16], deltas + (size_t)k * 16, 16 * sizeof(double));
         CK(cudaMemcpyAsync(ctx->d_seq_delta, D_dev.data(), D_dev.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     }
-    if (log && log_cap > 0 && (rc = ensure_log(ctx, (long long)n_frames * log_cap))) return rc;
-    dcreg_iter_log* dlog = (log && log_cap > 0) ? ctx->d_log : nullptr;
-    if (dlog) CK(cudaMemsetAsync(dlog, 0, (size_t)n_frames * log_cap * sizeof(dcreg_iter_log), ctx->stream));
-    if ((rc = init_state(ctx, T_dev.data(), n_frames, ctx->d_scan_seg, n_seqs))) return rc;
-    // the frames are uploaded in device order and sorted once, each by its own cell in the sensor frame (identity poses,
-    // a box of 1024^3 cells around the sensor: locality only, the chained priors are not known yet)
     CK(cudaMemcpyAsync(ctx->d_seq_prior, ident.data(), ident.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    ScanBatch S{n_frames, xyz, stride};
-    S.total = total;
-    for (int d = 0; d < n_frames; ++d) S.max_n = std::max<long long>(S.max_n, P.dev_off[(size_t)d + 1] - P.dev_off[(size_t)d]);
-    S.seg = ctx->d_scan_seg; S.radius = ctx->d_scan_radius;
-    S.order = P.input.data(); S.in_off = frame_offsets;
-    S.sort_T = ctx->d_seq_prior;
-    S.sort_grid.inv_cell = 1.0 / cell_size;
-    S.sort_grid.ox = S.sort_grid.oy = S.sort_grid.oz = -512;
-    S.sort_grid.nx = S.sort_grid.ny = S.sort_grid.nz = 1024;
-    S.sort_cells = 1ll << 30;
+    const Results R{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior};
+    dcreg_iter_log* dlog = nullptr;
     const float4* src_iter = nullptr;
-    if ((rc = upload_scans_sorted(ctx, S, &src_iter))) return rc;
-    S.sort_T = nullptr;
-    CK(cudaMemcpyAsync(ctx->d_seq_prior, ctx->d_T_init, (size_t)n_frames * 16 * sizeof(double), cudaMemcpyDeviceToDevice,
-                       ctx->stream));
-    // lanes: grid y of the loop kernel; a lane's frame range is set by odom_start_kernel at every step
-    S.lanes = n_seqs;
-    S.seq.cursor = ctx->d_seq_cursor; S.seq.first = ctx->d_seq_first; S.seq.delta = nullptr;
-    S.seq.T_prior = ctx->d_seq_prior; S.seq.seg = ctx->d_scan_seg; S.seq.n_active = ctx->d_n_active;
-    S.cell_size = cell_size;
-    if ((rc = ensure_pinned(ctx, (size_t)n_frames * sizeof(IcpState)))) return rc;
+    if ((rc = start_loop(ctx, n_frames, T_dev.data(), R, &S, &dlog, &src_iter))) return rc;
+    const int rings = search_rings(params->search_radius, cell_size);
     LoopPlan L;
     bool planned = false;
     int failed = n_steps;                       // the step whose map had no dense grid
@@ -2861,87 +2769,24 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
         // 3. every lane's frame of this step: its prior and a fresh loop state
         odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
             ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
-            st.first, st.active, d_prev, d_prev2, deltas ? ctx->d_seq_delta : nullptr, motion);
+            st.first, st.active, d_prev, d_prev2, deltas ? ctx->d_seq_delta.p : nullptr, motion);
         ctx->launches++;
         CK(cudaGetLastError());
         // 4. the loop: the same chunks (and CUDA graphs) at every step - the grid table keeps its pointer (the first step
         // has the most lanes, so the arena's table never regrows after it), only its entries change
         if (!planned) {
-            S.grids = ctx->odom_maps.d_grids; S.cell_off = ctx->odom_maps.d_cell_off;
+            S.grids = ctx->odom_maps.d_grids;
             if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? log_cap : 0, true, &L, &S))) return rc;
             planned = true;
         }
-        const long long cap = params->max_iterations;
-        long long issued = 0;
-        while (issued < cap) {
-            long long todo = cap - issued;
-            if (todo > 16) todo = 16;
-            const int bodies = (todo < 16 && issued > 0) ? 16 : (int)todo;
-            if ((rc = enqueue_iterations(ctx, L, params, dlog, dlog ? log_cap : 0, bodies))) return rc;
-            issued += bodies;
-            if (issued < cap) {
-                unsigned int* flag = (unsigned int*)ctx->h_pinned;      // lanes whose frame still runs
-                CK(cudaMemcpyAsync(flag, ctx->d_n_active, sizeof(unsigned int), cudaMemcpyDeviceToHost, ctx->stream));
-                CK(cudaStreamSynchronize(ctx->stream));
-                if (*flag == 0u) break;
-            }
-        }
+        if ((rc = run_chunks(ctx, L, params, dlog, dlog ? log_cap : 0, params->max_iterations, 16, true))) return rc;
     }
-    // results (device order), then back to the caller's frame order; after a failed step only the frames before it
-    if (dlog) {
-        log_fill_kernel<<<dim3((log_cap + 31) / 32, n_frames), 32, 0, ctx->stream>>>(dlog, log_cap, ctx->d_state, *params);
-        ctx->launches++;
-    }
-    std::vector<double> To((size_t)n_frames * 16), Tp, cv;
-    std::vector<int> it((size_t)n_frames), cg((size_t)n_frames), sts((size_t)n_frames);
-    std::vector<dcreg_iter_log> lg(dlog ? (size_t)n_frames * log_cap : 0);
+    // results in the caller's frame order; after a failed step only the frames before it, and that step's message
     const std::string err = ctx->err;
-    if ((rc = read_results(ctx, n_frames, To.data(), dlog ? lg.data() : nullptr, log_cap, it.data(), cg.data(), sts.data())))
+    if ((rc = finish_call(ctx, params, n_frames, dlog, R, P.dev.data(),
+                          failed < n_steps ? P.steps[(size_t)failed].first : n_frames)))
         return rc;
-    if (cov) {
-        cv.resize((size_t)n_frames * 36);
-        covariance_kernel<<<n_frames, 32, 0, ctx->stream>>>(ctx->d_state, ctx->d_scan_cov);
-        ctx->launches++;
-        CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(cv.data(), ctx->d_scan_cov, cv.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    if (T_prior) {
-        Tp.resize((size_t)n_frames * 16);
-        CK(cudaMemcpyAsync(Tp.data(), ctx->d_seq_prior, Tp.size() * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    CK(cudaStreamSynchronize(ctx->stream));
-    const int done = failed < n_steps ? P.steps[(size_t)failed].first : n_frames;
-    for (int k = 0; k < n_frames; ++k) {
-        const size_t d = (size_t)P.dev[(size_t)k];
-        if ((int)d >= done) continue;
-        memcpy(T_out + (size_t)k * 16, &To[d * 16], 16 * sizeof(double));
-        if (T_prior) memcpy(T_prior + (size_t)k * 16, &Tp[d * 16], 16 * sizeof(double));
-        if (n_iterations) n_iterations[k] = it[d];
-        if (converged) converged[k] = cg[d];
-        if (status) status[k] = sts[d];
-        if (cov) memcpy(cov + (size_t)k * 36, &cv[d * 36], 36 * sizeof(double));
-        if (dlog) memcpy(log + (size_t)k * log_cap, &lg[d * log_cap], (size_t)log_cap * sizeof(dcreg_iter_log));
-    }
     if (failed < n_steps) { ctx->err = err; return DCREG_BAD_ARG; }
-    return DCREG_OK;
-}
-
-// the pairs' own device buffers (dcreg_icp_run_pairs): packed targets, target offsets, final poses
-static int ensure_pairs(dcreg_ctx* ctx, int n_pairs, long long n_tgt) {
-    if (ctx->pairs_cap < n_pairs) {
-        if (ctx->d_pair_tgt_seg) cudaFree(ctx->d_pair_tgt_seg);
-        if (ctx->d_pair_T) cudaFree(ctx->d_pair_T);
-        ctx->d_pair_tgt_seg = nullptr; ctx->d_pair_T = nullptr; ctx->pairs_cap = 0;
-        CK(cudaMalloc(&ctx->d_pair_tgt_seg, (size_t)(n_pairs + 1) * sizeof(long long)));
-        CK(cudaMalloc(&ctx->d_pair_T, (size_t)n_pairs * 16 * sizeof(double)));
-        ctx->pairs_cap = n_pairs;
-    }
-    if (ctx->pair_tgt_cap < n_tgt) {
-        if (ctx->d_pair_tgt) cudaFree(ctx->d_pair_tgt);
-        ctx->d_pair_tgt = nullptr; ctx->pair_tgt_cap = 0;
-        CK(cudaMalloc(&ctx->d_pair_tgt, (size_t)n_tgt * sizeof(float4)));
-        ctx->pair_tgt_cap = n_tgt;
-    }
     return DCREG_OK;
 }
 
@@ -2951,33 +2796,31 @@ int dcreg_icp_run_pairs(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_pa
                         int* status, double* cov, double error_threshold, double* metrics, dcreg_iter_log* log,
                         int log_cap) {
     if (!ctx) return DCREG_BAD_ARG;
-    if (!params || n_pairs <= 0 || !src_xyz || !src_offsets || !tgt_xyz || !tgt_offsets || !T_init || !T_out) {
-        ctx->err = "icp_run_pairs: null pointer or n_pairs <= 0";
-        return DCREG_BAD_ARG;
-    }
-    if (stride < 3) { ctx->err = "icp_run_pairs: stride < 3"; return DCREG_BAD_ARG; }
-    if (!(cell_size > 0.0)) { ctx->err = "icp_run_pairs: cell_size <= 0"; return DCREG_BAD_ARG; }
-    if (ctx->comm) { ctx->err = "icp_run_pairs: pairs are independent - give each rank its own, do not shard them"; return DCREG_BAD_ARG; }
-    int rc = check_run_args(ctx, params, false, false);
+    BatchCheck c{"icp_run_pairs", params && n_pairs > 0 && src_xyz && src_offsets && tgt_xyz && tgt_offsets && T_init && T_out,
+                 "null pointer or n_pairs <= 0", "pairs are independent - give each rank its own, do not shard them", n_pairs};
+    c.offsets = src_offsets; c.item = "source"; c.stride = stride; c.own_cell = true; c.cell_size = cell_size;
+    c.need_target = false;
+    int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
-    const int rings = search_rings(params->search_radius, cell_size);
-    if (rings < 1 || rings > 4) { ctx->err = "icp_run_pairs: search_radius / cell_size must be in (0, 4]"; return DCREG_BAD_ARG; }
-    if ((rc = check_batch(ctx, n_pairs, src_offsets, "icp_run_pairs: source"))) return rc;
     const std::string why = arena_plan::check_offsets(n_pairs, tgt_offsets, arena_plan::kMaxPoints, "icp_run_pairs: target");
     if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
     const long long n_tgt = tgt_offsets[n_pairs];
     CK(cudaSetDevice(ctx->device));
-    if ((rc = ensure_pairs(ctx, n_pairs, n_tgt))) return rc;
+    CK(ctx->d_pair_tgt_seg.ensure(n_pairs + 1));
+    CK(ctx->d_pair_T.ensure((long long)n_pairs * 16));
+    CK(ctx->d_pair_tgt.ensure(n_tgt));
     CK(cudaMemcpyAsync(ctx->d_pair_tgt_seg, tgt_offsets, (size_t)(n_pairs + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
     // the targets: packed with w = index over all targets, then every pair's dense grid in the arena
     if ((rc = upload_points(ctx, tgt_xyz, n_tgt, stride, nullptr, 1, ctx->d_pair_tgt, nullptr))) return rc;
-    long long cells = 0;
+    Batch S{n_pairs, src_xyz, stride, src_offsets};
     if ((rc = build_grid_arena(ctx, ctx->pair_tgt, ctx->d_pair_tgt, tgt_offsets, ctx->d_pair_tgt_seg, n_pairs, cell_size,
-                               rings, "icp_run_pairs: target", &cells)))
+                               search_rings(params->search_radius, cell_size), "icp_run_pairs: target", &S.cells)))
         return rc;
-    ScanBatch S{n_pairs, src_xyz, stride};
-    S.grids = ctx->pair_tgt.d_grids; S.cell_off = ctx->pair_tgt.d_cell_off; S.cells = cells; S.cell_size = cell_size;
-    if ((rc = run_sources(ctx, params, S, src_offsets, T_init, T_out, n_iterations, converged, status, cov, log, log_cap)))
+    S.sort = Batch::kGridTable;
+    S.grid_table = true; S.grids = ctx->pair_tgt.d_grids; S.cell_off = ctx->pair_tgt.d_cell_off; S.cell_size = cell_size;
+    if ((rc = stage_sources(ctx, S)) ||
+        (rc = run_loop(ctx, params, n_pairs, T_init, Results{T_out, n_iterations, converged, status, log, log_cap, cov}, true,
+                       &S)))
         return rc;
     if (!metrics) return DCREG_OK;
     CK(cudaMemcpyAsync(ctx->d_pair_T, T_out, (size_t)n_pairs * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
@@ -2993,14 +2836,16 @@ int dcreg_icp_run_host_planes(dcreg_ctx* ctx, const dcreg_icp_params* params, co
     if (!params || !T_init || !T_out || !cb) { ctx->err = "icp_run_host_planes: null pointer"; return DCREG_BAD_ARG; }
     if (!ctx->d_src || ctx->n_src <= 0) { ctx->err = "[ICP Error] Input measure cloud is null or empty."; return DCREG_BAD_ARG; }
     CK(cudaSetDevice(ctx->device));
+    int status = DCREG_OK;
+    const Results R{T_out, n_iterations, converged, &status, log, log_cap};
+    dcreg_iter_log* dlog = nullptr;
     int rc;
-    if (log && log_cap > 0 && (rc = ensure_log(ctx, log_cap))) return rc;
-    dcreg_iter_log* dlog = (log && log_cap > 0) ? ctx->d_log : nullptr;
-    if (dlog) CK(cudaMemsetAsync(dlog, 0, (size_t)log_cap * sizeof(dcreg_iter_log), ctx->stream));
-    if ((rc = ensure_planes(ctx, ctx->n_src))) return rc;
-    if ((rc = ensure_pinned(ctx, sizeof(IcpState) + (size_t)ctx->n_src * sizeof(double4)))) return rc;
-    IcpState* hs = (IcpState*)ctx->h_pinned;
-    double* hplanes = (double*)((char*)ctx->h_pinned + sizeof(IcpState));
+    if ((rc = setup_log(ctx, R, 1, &dlog))) return rc;
+    CK(ctx->d_planes64.ensure(ctx->n_src));
+    CK(ctx->d_planes32.ensure(ctx->n_src));
+    CK(ctx->h_pinned.ensure((long long)(sizeof(IcpState) + (size_t)ctx->n_src * sizeof(double4))));
+    IcpState* hs = (IcpState*)ctx->h_pinned.p;
+    double* hplanes = (double*)(ctx->h_pinned.p + sizeof(IcpState));
     if ((rc = init_state(ctx, T_init))) return rc;
     double T[16];
     memcpy(T, T_init, sizeof(T));
@@ -3029,12 +2874,7 @@ int dcreg_icp_run_host_planes(dcreg_ctx* ctx, const dcreg_icp_params* params, co
         }
         if (hs->done) break;
     }
-    int status = DCREG_OK;
-    if (dlog) {
-        log_fill_kernel<<<dim3((log_cap + 31) / 32, 1), 32, 0, ctx->stream>>>(dlog, log_cap, ctx->d_state, *params);
-        ctx->launches++;
-    }
-    if ((rc = read_results(ctx, 1, T_out, log, log_cap, n_iterations, converged, &status))) return rc;
+    if ((rc = finish_call(ctx, params, 1, dlog, R))) return rc;
     return status;
 }
 
