@@ -825,39 +825,13 @@ __global__ void transform_points_kernel(const float4* __restrict__ in, long long
 // Plane through the 5 neighbours: least squares of [nb] x = -1, n = x/|x|, d = 1/|x|, gates
 // |x| >= min_norm and max_j (n.nb_j + d)^2 < thickness^2 (icp_test_runner.cpp:1727-1773).
 // Returns true and (n, d) when a valid plane exists.
-__device__ __forceinline__ bool fit_plane(const Grid& g, const int (&kpos)[5], double min_norm, double thickness,
-                                          double& nx, double& ny, double& nz, double& d) {
-    double A[15], b[5], x[3];
-#pragma unroll
-    for (int j = 0; j < 5; ++j) {
-        const float4 p = __ldg(&g.pts[kpos[j]]);
-        A[j * 3 + 0] = (double)p.x;
-        A[j * 3 + 1] = (double)p.y;
-        A[j * 3 + 2] = (double)p.z;
-        b[j] = -1.0;
-    }
-    dla::colpiv_qr_solve<5, 3>(A, b, x);
-    const double ps = sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
-    if (!(ps >= min_norm)) return false;                 // :1752 (also rejects NaN)
-    nx = x[0] / ps; ny = x[1] / ps; nz = x[2] / ps; d = 1.0 / ps;
-    double worst = 0.0;
-#pragma unroll
-    for (int j = 0; j < 5; ++j) {
-        const float4 p = __ldg(&g.pts[kpos[j]]);          // re-read (L1 hit) instead of holding 15 more doubles
-        double e = nx * (double)p.x + ny * (double)p.y + nz * (double)p.z + d;
-        e *= e;
-        worst = fmax(worst, e);
-    }
-    return worst < thickness * thickness;                // :1772-1773
-}
-
-// The same fit with the register-resident QR (small_la.cuh: same operations in the same order, bit-identical results).  A
-// separate function with its own register allocation: it is called from the fit work list of the loop kernel, where
-// almost nothing is live across the call (inlined into a loop body full of live state it spills and ran several times
-// slower during development; not re-measured on H100).  Rejected: a variant of the QR with hardware reciprocal / rsqrt
-// seeds instead of the ~30 IEEE divisions and square roots on the fit's dependent chain) shortens a fit, but on exactly rank-deficient
-// neighbourhoods (collinear lattice points) its 1-ulp differences flip the pivoted QR's rank decision, and the loop then
-// disagrees with the generic fit by one correspondence (tests/test_gpu_parity.py, lattice scene).
+// The QR is the register-resident one (small_la.cuh: the same operations in the same order as the generic
+// colpiv_qr_solve, bit-identical results; tools/test_qr_reg.cu).  A separate function with its own register allocation:
+// it is called from the fit work list of the loop kernel, where almost nothing is live across the call (inlined into a
+// loop body full of live state it spills and ran several times slower during development; not re-measured on H100).
+// Rejected: a variant of the QR with hardware reciprocal / rsqrt seeds instead of the ~30 IEEE divisions and square
+// roots on the fit's dependent chain shortens a fit, but on exactly rank-deficient neighbourhoods (collinear lattice
+// points) its 1-ulp differences flip the pivoted QR's rank decision and change a correspondence.
 __device__ __noinline__ bool fit_plane_reg(const Grid& g, const int (&kpos)[5], double min_norm, double thickness,
                                            double& nx, double& ny, double& nz, double& d) {
     double A[5][3], b[5], x[3];

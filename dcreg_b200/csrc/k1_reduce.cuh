@@ -1,6 +1,6 @@
-// k1_reduce.cuh - per-slot math and the Gram-matrix reduction shared by the two producers of the normal
-// equations: the streaming kernel K1 (k1_stream.cuh: frozen planes) and the fused ICP iteration kernel
-// (dcreg_b200.cu: planes come straight out of the correspondence stage).
+// k1_reduce.cuh - per-slot math of the normal equations and the loop kernel's DMMA Gram accumulation.  The loop kernel
+// (dcreg_b200.cu: planes come straight out of the correspondence stage) uses it as is; the streaming kernel K1
+// (k1_stream.cuh: frozen planes) has an issue-slot trimmed copy of the same arithmetic.  Both end in k1s's packed tail.
 //
 // Replaces, per source slot and per ICP iteration (reference file:line):
 //   pointBodyToGlobal (FP64 math, float32 store)         DCReg/include/utils.hpp:630-636
@@ -27,7 +27,6 @@ namespace k1 {
 
 using k2::kAcc;
 
-constexpr int kGramPart = 66;            // per-block partial: 64 Gram entries + N_eff + N_corr_pt
 constexpr int kTRow = 36;                // padded row stride (doubles) of a warp's DMMA transpose buffer
 
 struct Pose {            // R row-major, t
@@ -129,115 +128,6 @@ __device__ __forceinline__ void gram_accumulate_dmma(double* tb, int lane, const
         dmma884(e0, e1, f1, f1);                            // two accumulator pairs: halves the dependent chain
     }
     __syncwarp();
-}
-
-// ---- block / grid reduction of the Gram fragments ---------------------------------------------------------------
-struct GramSmem {
-    double red[8][kGramPart];
-    double fin[kGramPart + 6];
-    bool is_last;
-};
-
-// Every thread of a 256-thread block calls this with its two Gram entries (flat index 2*lane + {0,1} of its warp's
-// 8x8 Gram) and its counters.  Block partial -> global; the last block to arrive (atomic ticket) sums the partials
-// in a fixed order with its 8 warps in parallel, applies the world->body congruence with 42 threads and writes
-// acc_out[kAcc] = 21 upper-triangular entries (hessian_computer.h order) + 6 rhs + {sum r^2, N_eff, N_pt, sum b^2}.
-// Deterministic for a given grid size.
-__device__ __forceinline__ void finish_block(double c0, double c1, int neff, int npt, GramSmem& gs, double* partials,
-                                             unsigned int* counter, const double* R, double* acc_out) {
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-        neff += __shfl_down_sync(0xffffffffu, neff, off);
-        npt += __shfl_down_sync(0xffffffffu, npt, off);
-    }
-    gs.red[warp][2 * lane] = c0;
-    gs.red[warp][2 * lane + 1] = c1;
-    if (lane == 0) { gs.red[warp][64] = (double)neff; gs.red[warp][65] = (double)npt; }
-    __syncthreads();
-    if (tid < kGramPart) {
-        double s = 0.0;
-#pragma unroll
-        for (int w = 0; w < 8; ++w) s += gs.red[w][tid];
-        partials[(size_t)blockIdx.x * kGramPart + tid] = s;
-    }
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) {
-        const unsigned int tk = atomicAdd(counter, 1u);
-        gs.is_last = (tk == gridDim.x - 1);
-    }
-    __syncthreads();
-    if (!gs.is_last) return;
-    __threadfence();
-    {
-        const int nb = (int)gridDim.x;
-        double s0 = 0.0, s1 = 0.0, s2 = 0.0;                     // elements lane, lane + 32, lane + 64 (< kGramPart)
-        int b = warp;
-        for (; b + 24 < nb; b += 32) {                           // warp w sums blocks w, w+8, ...; 4 blocks per trip
-            double t0[4], t1[4], t2[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const double* row = partials + (size_t)(b + u * 8) * kGramPart;
-                t0[u] = __ldcg(row + lane);
-                t1[u] = __ldcg(row + 32 + lane);
-                t2[u] = (lane < kGramPart - 64) ? __ldcg(row + 64 + lane) : 0.0;
-            }
-#pragma unroll
-            for (int u = 0; u < 4; ++u) { s0 += t0[u]; s1 += t1[u]; s2 += t2[u]; }
-        }
-        for (; b < nb; b += 8) {
-            const double* row = partials + (size_t)b * kGramPart;
-            s0 += __ldcg(row + lane);
-            s1 += __ldcg(row + 32 + lane);
-            if (lane < kGramPart - 64) s2 += __ldcg(row + 64 + lane);
-        }
-        __syncthreads();                                          // red[][] is free again
-        gs.red[warp][lane] = s0;
-        gs.red[warp][32 + lane] = s1;
-        if (lane < kGramPart - 64) gs.red[warp][64 + lane] = s2;
-    }
-    __syncthreads();
-    double* fin = gs.fin;
-    if (tid < kGramPart) {
-        double s = 0.0;
-#pragma unroll
-        for (int w = 0; w < 8; ++w) s += gs.red[w][tid];
-        fin[tid] = s;
-    }
-    __syncthreads();
-    // Gram (world frame) -> H_body = Q^T H Q, g_body = Q^T g with Q = blkdiag(R, R): one thread per output entry
-    double* outv = &gs.red[0][0];
-    if (tid < 36) {
-        const int i = tid / 6, j = tid % 6;
-        if (j >= i) {
-            const int bi = (i / 3) * 3, bj = (j / 3) * 3, ii = i % 3, jj = j % 3;
-            double acc = 0.0;
-#pragma unroll
-            for (int k = 0; k < 3; ++k)
-#pragma unroll
-                for (int l = 0; l < 3; ++l) {
-                    const double h = 0.5 * (fin[(bi + k) * 8 + bj + l] + fin[(bj + l) * 8 + bi + k]);
-                    acc = fma(R[k * 3 + ii] * h, R[l * 3 + jj], acc);
-                }
-            outv[i * 6 - (i * (i - 1)) / 2 + (j - i)] = acc;      // packed upper-triangular index, row-major
-        }
-    } else if (tid < 42) {
-        const int i = tid - 36, bi = (i / 3) * 3, ii = i % 3;
-        double acc = 0.0;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) acc = fma(R[k * 3 + ii], 0.5 * (fin[(bi + k) * 8 + 6] + fin[6 * 8 + bi + k]), acc);
-        outv[21 + i] = acc;
-    } else if (tid == 42) {
-        outv[k2::kAccSumR2] = fin[7 * 8 + 7];
-        outv[k2::kAccNeff] = fin[64];
-        outv[k2::kAccNpt] = fin[65];
-        outv[k2::kAccSumB2] = fin[6 * 8 + 6];
-        outv[kAcc - 1] = 0.0;
-    }
-    __syncthreads();
-    if (tid < kAcc) acc_out[tid] = outv[tid];
-    if (tid == 0) *counter = 0u;
 }
 
 }  // namespace k1

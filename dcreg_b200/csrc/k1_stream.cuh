@@ -44,7 +44,7 @@ struct Args {
     k1::Pose pose;
     double Rs[9];                // R * 2^896: undoes the exponent bias the raw point conversion leaves out (f32_raw)
     double slope, gate;          // LOAM weight 1 - slope |r| (0.9) and its gate (0.1): constant-bank operands
-    double* partials;            // [grid][k1::kGramPart]
+    double* partials;            // [grid][kPk]
     unsigned int* counter;
     double* acc;                 // [k2::kAcc] final, body frame
     double npt_override;         // >= 0: N_corr_pt of this rank as counted by the caller's correspondence stage (host-kd-tree

@@ -337,8 +337,8 @@ def test_host_planes_fitness_uses_the_callers_count(ctx, golden, cylinder):
 # hash-grid fallback (bounding box too large for the dense cell table), aborting trials in a batch
 # ------------------------------------------------------------------------------------------------
 def test_hash_grid_path_matches_oracle(ctx, cylinder):
-    """Two far outliers blow the target's bounding box up to ~1e11 cells: the index falls back to the hash table, the
-    loop to the one-thread-per-slot kernel + separate solve kernel.  Same trajectory as the oracle; a batch and the
+    """Two far outliers blow the target's bounding box up to ~1e11 cells: the index falls back to the hash table and the
+    loop kernel stays in lean mode (a full search every iteration).  Same trajectory as the oracle; a batch and the
     point-to-point metrics (dense grids only) are refused.  Back on a dense target, the context's reused grid arena
     gives the bits of a fresh context."""
     from dcreg_b200 import Context, default_params
@@ -372,6 +372,41 @@ def test_hash_grid_path_matches_oracle(ctx, cylinder):
     assert (dense.status, dense.iterations, dense.converged) == (ref.status, ref.iterations, ref.converged)
     assert dense.T.tobytes() == ref.T.tobytes()
     assert [np.array(L.H27).tobytes() for L in dense.logs] == [np.array(L.H27).tobytes() for L in ref.logs]
+
+
+def test_hash_grid_target_equals_dense_target(ctx, cylinder):
+    """Target A is the cylinder plus two far outliers (a hash table), target B the cylinder alone (a dense grid); the
+    outliers come last, so the cylinder's point indices (the tie rule) agree and no query ever reaches them.  Seam 1
+    gives the same planes bit for bit; a fixed-iteration run on A, lean in every iteration, gives the counts of the run
+    on B, which reuses records once the pose settles, and its poses to rounding.  Timing coherent mode needs a dense grid."""
+    from dcreg_b200 import default_params
+    from dcreg_b200.api import BAD_ARG, DcregError
+    far = np.array([[4000.0, 4500.0, 5000.0], [-4000.0, -3000.0, 2000.0]], np.float32)
+    tgt_a = np.concatenate([cylinder, far]).astype(np.float32)
+    T0 = o.pose6d_to_matrix(0.1, 0.3, 0.2, math.radians(0.1), math.radians(-0.1), math.radians(1.0))
+    methods = [("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG"), ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")]
+    prms = [default_params(max_iterations=30, fixed_iterations=1, kappa_target=10.0, detection=d, handling=h)
+            for d, h in methods]
+    ctx.set_source(cylinder)
+    out = {}
+    for name, tgt in (("A", tgt_a), ("B", cylinder)):
+        ctx.set_target(tgt, 1.0)
+        out[name] = (ctx.find_planes(T0, 1.0), [ctx.icp_run(p, T0) for p in prms])
+        if name == "A":
+            with pytest.raises(DcregError) as e:
+                ctx.time_iteration(prms[0], T0, 0, 2)
+            assert e.value.status == BAD_ARG
+    (planes_a, npt_a), runs_a = out["A"]
+    (planes_b, npt_b), runs_b = out["B"]
+    assert npt_a == npt_b > 0
+    assert planes_a.tobytes() == planes_b.tobytes()
+    for a, b in zip(runs_a, runs_b):
+        assert (a.status, a.iterations, a.converged) == (b.status, b.iterations, b.converged) and a.iterations == 30
+        for la, lb in zip(a.logs, b.logs):
+            assert la.n_effective == lb.n_effective and la.n_corr_pt == lb.n_corr_pt
+            assert list(la.analysis.degenerate_mask) == list(lb.analysis.degenerate_mask)
+            assert o.se3_log_distance(np.array(la.T).reshape(4, 4), np.array(lb.T).reshape(4, 4)) < 1e-9
+        assert o.se3_log_distance(a.T, b.T) < 1e-9
 
 
 def test_batch_with_aborting_trials(ctx, cylinder):

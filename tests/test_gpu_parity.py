@@ -356,9 +356,9 @@ def test_icp_fixed_iterations_synthetic_cylinder(ctx):
 @pytest.mark.parametrize("method", ["Ours", "ME-TSVD"])
 def test_loop_with_reused_correspondences_equals_full_search_every_iteration(ctx, method):
     """The loop's iteration kernel reuses neighbour lists (gap certificate) and plane fits (same five points) once the
-    pose moves little.  Against the same loop with a full search and a fresh fit in EVERY iteration (the one-thread-per-
-    slot kernel, DCREG_FUSED_SEARCH=1) the per-iteration counts must be identical and the poses equal to rounding; the
-    counters show that the reuse paths were actually taken."""
+    pose moves little.  Against the same loop with a full search and a fresh fit in EVERY iteration (the loop kernel's
+    lean mode in every iteration, DCREG_FUSED_SEARCH=1) the per-iteration counts must be identical and the poses equal
+    to rounding; the counters show that the reuse paths were actually taken."""
     from dcreg_b200 import default_params
     from dcreg_b200.scenes import make_cylinder
     pts = make_cylinder(30_000, seed=7)
@@ -386,7 +386,8 @@ def test_loop_with_reused_correspondences_equals_full_search_every_iteration(ctx
 def test_loop_reuse_on_a_lattice_with_duplicates_and_ties(ctx):
     """Worst case for the neighbour bookkeeping: a regular lattice (many exactly equal distances -> index rule),
     duplicated target points, a dense patch (more than 64 candidates inside a loose bound -> the warp search gives up
-    and the slot searches sequentially) and a source that is not a multiple of the tile size."""
+    and the slot searches sequentially) and a source that is not a multiple of the tile size.  The reference is a full
+    search and a fresh fit in every iteration (lean mode throughout, DCREG_FUSED_SEARCH=1)."""
     from dcreg_b200 import default_params
     g = np.arange(-6, 6, 0.25, dtype=np.float32)
     X, Y = np.meshgrid(g, g)
