@@ -88,7 +88,7 @@ EXPORTS = [
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_voxel_downsample", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -134,6 +134,12 @@ def load_library():
     lib.dcreg_icp_run_odometry.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
                                            C.POINTER(i64), ci, C.c_double, ci, ci, dp, dp, dp, dp, C.POINTER(ci),
                                            C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(IterLog), ci]
+    lib.dcreg_icp_run_odometry_voxel.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
+                                                 C.POINTER(i64), ci, C.c_double, ci, ci, C.c_double, C.c_double, dp, dp,
+                                                 C.POINTER(i64), dp, dp, C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp,
+                                                 C.POINTER(IterLog), ci]
+    lib.dcreg_voxel_downsample.argtypes = [vp, ci, C.POINTER(C.c_float), C.POINTER(i64), ci, C.c_double,
+                                           C.POINTER(C.c_float), C.POINTER(i64), C.POINTER(i64)]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -268,12 +274,41 @@ def constant_velocity_increment(T_prev, T):
     return out
 
 
+VOXEL_LIMIT = 1 << 20      # voxel coordinates must lie in [-2^20, 2^20): 21 bits per axis in one 63-bit key
+
+
+def voxel_downsample(P, voxel):
+    """The voxel filter of dcreg_voxel_downsample, bit for bit: the voxel of a point is np.floor(p.astype(float64) *
+    (1.0 / voxel)) per axis, rows with a non-finite coordinate have none and are dropped, and each voxel keeps its first
+    point.  P: (N, >=3).  Returns (points (K, 3) float32, the kept rows' coordinates unchanged; index (K,) int64, their
+    rows in P, ascending).  Raises ValueError for a voxel that is not finite and > 0, or a voxel coordinate outside
+    [-2^20, 2^20)."""
+    P = np.asarray(P, dtype=np.float32)
+    if P.ndim != 2 or P.shape[1] < 3:
+        raise ValueError("points must be (N, >=3)")
+    voxel = float(voxel)
+    if not (voxel > 0.0 and np.isfinite(voxel)):
+        raise ValueError(f"voxel_downsample: voxel must be finite and > 0, not {voxel}")
+    xyz = P[:, :3]
+    rows = np.nonzero(np.isfinite(xyz).all(axis=1))[0]
+    with np.errstate(invalid="ignore", over="ignore"):
+        keys = np.floor(xyz[rows].astype(np.float64) * (1.0 / voxel))
+    if not ((keys >= -VOXEL_LIMIT) & (keys < VOXEL_LIMIT)).all():
+        raise ValueError("voxel_downsample: a voxel coordinate lies outside [-2^20, 2^20) (voxel too small for the "
+                         "cloud's coordinates)")
+    k = keys.astype(np.int64) + VOXEL_LIMIT
+    _, first = np.unique((k[:, 0] << 42) | (k[:, 1] << 21) | k[:, 2], return_index=True)
+    keep = rows[np.sort(first)].astype(np.int64)
+    return np.ascontiguousarray(xyz[keep]), keep
+
+
 class IcpResult:
     def __init__(self, status, converged, iterations, T, logs, cov=None):
         self.status, self.converged, self.iterations, self.T, self.logs = status, converged, iterations, T, logs
         self.cov = cov
         self.metrics = None
         self.T_prior = None             # icp_run_sequences: the initial pose the frame started from
+        self.n_points = None            # icp_run_odometry: the frame's points after the source filter
 
 
 def _trial_results(st, conv, n_it, T_out, logs, cap, cov=None):
@@ -533,15 +568,31 @@ class Context:
         return self._run_batched("icp_run_sequences", call, params, n, S, "sequences", T_init, want_log, want_cov, deltas,
                                  want_prior=True)
 
+    def voxel_downsample(self, clouds, voxel: float):
+        """dcreg_voxel_downsample of every cloud (a list of (N_b, >=3) arrays) in one call on the device: a list of
+        (points (K_b, 3) float32, index (K_b,) int64), as api.voxel_downsample gives for each cloud alone."""
+        xyz, off = _pack(clouds)
+        n = len(clouds)
+        total = int(off[-1]) if n else 0
+        pts = np.empty((max(total, 1), 3), dtype=np.float32)
+        idx = np.empty(max(total, 1), dtype=np.int64)
+        kept = np.zeros(n + 1, dtype=np.int64)
+        self._check(self.lib.dcreg_voxel_downsample(self._h, n, _fptr(xyz), _iptr(off), 3, float(voxel), _fptr(pts),
+                                                    _iptr(kept), _iptr(idx)))
+        return [(pts[a:b].copy(), idx[a:b].copy()) for a, b in zip(kept[:-1], kept[1:])]
+
     def icp_run_odometry(self, params: IcpParams, sequences, T_init, deltas=None, motion: str = "increments",
-                         map_frames: int = 10, cell_size=None, want_log: bool = False, want_cov: bool = False):
+                         map_frames: int = 10, cell_size=None, want_log: bool = False, want_cov: bool = False,
+                         source_voxel: float = 0.0, map_voxel: float = 0.0):
         """Scan-to-map odometry (`sequences`: a list of lists of (N, >=3) point arrays): frame k of a sequence registers
         against the local map of the frames [k - map_frames, k) before it, each placed at its own registered pose
         (map_points), starting from compose_prior(frame k-1's result, D).  motion "increments": D = deltas[k-1]
         (deltas: (n_frames, 4, 4) over all frames in order, or None for identity); "constant_velocity": D =
         constant_velocity_increment(T_out[k-2], T_out[k-1]) (identity after the anchor; deltas must be None).  The first
         frame of each sequence is its anchor: not registered, T = T_prior = T_init[s].  cell_size: the maps' grid cell
-        (default search_radius).  Returns a list of IcpResult, one per frame in order, with .T_prior (logs only when
+        (default search_radius).  source_voxel / map_voxel (0: no filter): voxel_downsample every frame in its sensor
+        frame, and every local map in world coordinates (dcreg_icp_run_odometry_voxel).  Returns a list of IcpResult,
+        one per frame in order, with .T_prior and .n_points, the frame's points after the source filter (logs only when
         want_log, .cov when want_cov).  Needs no target; the context's source and target are left as they were."""
         models = {"increments": 0, "constant_velocity": 1}
         if motion not in models:
@@ -549,14 +600,27 @@ class Context:
         seq_off, xyz, off = _pack_sequences(sequences)
         S, n = len(sequences), int(seq_off[-1])
         cell = float(params.search_radius if cell_size is None else cell_size)
+        filtered = source_voxel != 0.0 or map_voxel != 0.0
+        npts = np.diff(off) if off is not None else np.zeros(0, dtype=np.int64)
+        if filtered:
+            npts = np.zeros(max(n, 1), dtype=np.int64)
 
         def call(o):
+            if filtered:
+                return self.lib.dcreg_icp_run_odometry_voxel(
+                    self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
+                    3, cell, int(map_frames), models[motion], float(source_voxel), float(map_voxel), _optr(o.T_init),
+                    _optr(o.deltas), _iptr(npts), _optr(o.T_prior), _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov),
+                    o.logs, o.cap)
             return self.lib.dcreg_icp_run_odometry(
                 self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off), 3,
                 cell, int(map_frames), models[motion], _optr(o.T_init), _optr(o.deltas), _optr(o.T_prior),
                 _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov), o.logs, o.cap)
-        return self._run_batched("icp_run_odometry", call, params, n, S, "sequences", T_init, want_log, want_cov, deltas,
-                                 want_prior=True)
+        out = self._run_batched("icp_run_odometry", call, params, n, S, "sequences", T_init, want_log, want_cov, deltas,
+                                want_prior=True)
+        for r, c in zip(out, npts):
+            r.n_points = int(c)
+        return out
 
     def icp_run_pairs(self, params: IcpParams, sources, targets, T_init, cell_size=None, want_log: bool = False,
                       want_cov: bool = False, metrics_threshold=None):

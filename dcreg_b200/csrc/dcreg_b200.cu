@@ -924,6 +924,71 @@ __global__ void odom_start_kernel(IcpState* states, const long long* __restrict_
     init_loop_state(states + f, T, seg[f + 1] - seg[f]);
 }
 
+// ---- voxel filter (dcreg_voxel_downsample, dcreg_icp_run_odometry_voxel) -------------------------------------------
+// n points (`stride` floats each: host layout, or float4) in n_seg clouds, cloud b being points [seg[b], seg[b+1]).
+// Point i's voxel is floor((double)p * inv) per axis (corr::cell_coord before the integer conversion); the survivor of a
+// voxel is its point of smallest index, kept bit for bit, and the survivors keep their input order.  Four passes for all
+// clouds at once: hash, flag, exclusive scan, scatter.
+constexpr double kVoxelLimit = 1048576.0;   // voxel coordinates must lie in [-2^20, 2^20): the range of corr::pack_key
+
+// Pass 1: cloud b owns the slots [tab[b], tab[b+1]) (a power of two) of the open-addressing table keys / first; point i
+// claims its voxel's slot and atomicMin's its index into it (the minimum does not depend on the order threads arrive
+// in).  slot_of[i] = the slot, or -1 for a point with a non-finite coordinate (no voxel) or out of range (bad[b] = 1).
+__global__ void voxel_hash_kernel(const float* __restrict__ in, long long n, int stride, const long long* __restrict__ seg,
+                                  int n_seg, const long long* __restrict__ tab, double inv, unsigned long long* __restrict__ keys,
+                                  int* __restrict__ first, long long* __restrict__ slot_of, int* __restrict__ bad) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int b = corr::segment_of(seg, n_seg, i);
+    slot_of[i] = -1;
+    const float x = in[i * stride], y = in[i * stride + 1], z = in[i * stride + 2];
+    if (!isfinite(x) || !isfinite(y) || !isfinite(z)) return;
+    const double fx = floor(__dmul_rn((double)x, inv)), fy = floor(__dmul_rn((double)y, inv)),
+                 fz = floor(__dmul_rn((double)z, inv));
+    if (!(fx >= -kVoxelLimit && fx < kVoxelLimit && fy >= -kVoxelLimit && fy < kVoxelLimit && fz >= -kVoxelLimit &&
+          fz < kVoxelLimit)) {
+        bad[b] = 1;
+        return;
+    }
+    const unsigned long long key = corr::pack_key((int)fx, (int)fy, (int)fz);
+    const long long base = tab[b];
+    const unsigned int mask = (unsigned int)(tab[b + 1] - base - 1);
+    unsigned int s = corr::hash_key(key) & mask;
+    while (true) {
+        const unsigned long long prev = atomicCAS(&keys[base + s], corr::kEmptyKey, key);
+        if (prev == corr::kEmptyKey || prev == key) break;
+        s = (s + 1) & mask;
+    }
+    atomicMin(&first[base + s], (int)i);
+    slot_of[i] = base + s;
+}
+
+// Pass 2: keep[i] = 1 iff point i is the first of its voxel; keep[n] = 0 (the scan's total)
+__global__ void voxel_flag_kernel(const long long* __restrict__ slot_of, long long n, const int* __restrict__ first,
+                                  int* __restrict__ keep) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > n) return;
+    const long long s = i < n ? slot_of[i] : -1;
+    keep[i] = s >= 0 && first[s] == (int)i;
+}
+
+// Pass 4 (pos: the exclusive scan of keep): kept point i goes to out[pos[i]] (out_stride 3: x y z; 4: x y z and w = its
+// index over all kept points, as pack_points_kernel packs one cloud), index[pos[i]] = its index in its own cloud (index
+// may be null); out_seg[b] = pos[seg[b]] for b <= n_seg, the kept points' offsets.  n + 1 threads.
+__global__ void voxel_scatter_kernel(const float* __restrict__ in, long long n, int stride, const long long* __restrict__ seg,
+                                     int n_seg, const int* __restrict__ keep, const int* __restrict__ pos,
+                                     float* __restrict__ out, int out_stride, long long* __restrict__ index,
+                                     long long* __restrict__ out_seg) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i <= n_seg) out_seg[i] = pos[seg[i]];
+    if (i >= n || !keep[i]) return;
+    const long long p = pos[i];
+    float* o = out + p * out_stride;
+    o[0] = in[i * stride]; o[1] = in[i * stride + 1]; o[2] = in[i * stride + 2];
+    if (out_stride == 4) o[3] = __int_as_float((int)p);
+    if (index) index[p] = i - seg[corr::segment_of(seg, n_seg, i)];
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1061,7 +1126,13 @@ struct dcreg_ctx {
     // odometry (dcreg_icp_run_odometry): every step's tables (odom_plan.hpp) in one upload, the step's local maps, and
     // their grids in an arena of their own
     DevBuf<long long> d_odom_ll; DevBuf<int> d_odom_int;
-    DevBuf<float4> d_odom_map;
+    DevBuf<float4> d_odom_map, d_odom_map_vox;                         // ... and the maps after the voxel filter
+    // the voxel filter (voxel_filter): table [slots] keys / first indices, [points] slots, [points + 1] flags and their
+    // scan, [clouds + 1] table offsets, input and kept offsets, [clouds] range flags, [points][3] kept xyz and indices
+    DevBuf<unsigned long long> d_vox_keys; DevBuf<int> d_vox_first;
+    DevBuf<long long> d_vox_slot; DevBuf<int> d_vox_keep, d_vox_pos;
+    DevBuf<long long> d_vox_tab, d_vox_in_seg, d_vox_seg; DevBuf<int> d_vox_bad;
+    DevBuf<float> d_vox_xyz; DevBuf<long long> d_vox_index;
     // Grow-only arenas of dense grids (build_grid_arena): the context's target (one cloud; `grid` points into it), the
     // targets of dcreg_icp_run_pairs (the context's target and grid stay as they were), the grids over the aligned
     // sources of the point-to-point metrics, and odometry's local maps
@@ -1152,13 +1223,14 @@ static cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
 // host points -> d_out, packed by pack_points_kernel (d_seg: device table of n_seg segments, or null for one; d_radius:
 // [n_seg] per-segment max |p|, or null)
 // order / in_off (odometry): segment b of the device copy is host segment order[b], points [in_off[order[b]], ..) of xyz;
-// null: xyz in order
+// null: xyz in order.  kind: cudaMemcpyDeviceToDevice when xyz is device memory (the voxel filter's output)
 int upload_points(dcreg_ctx* ctx, const float* xyz, long long n, int stride, const long long* d_seg, int n_seg,
-                  float4* d_out, float* d_radius, const int* order = nullptr, const int64_t* in_off = nullptr) {
+                  float4* d_out, float* d_radius, const int* order = nullptr, const int64_t* in_off = nullptr,
+                  cudaMemcpyKind kind = cudaMemcpyHostToDevice) {
     const size_t bytes = (size_t)n * stride * sizeof(float);
     CK(ctx->d_stage.ensure(n * stride));
     if (!order) {
-        CK(cudaMemcpyAsync(ctx->d_stage, xyz, bytes, cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->d_stage, xyz, bytes, kind, ctx->stream));
     } else {
         long long at = 0;                              // one copy per run of segments that are also consecutive on the host
         for (int b = 0; b < n_seg;) {
@@ -1166,7 +1238,7 @@ int upload_points(dcreg_ctx* ctx, const float* xyz, long long n, int stride, con
             while (e < n_seg && order[e] == order[e - 1] + 1) ++e;
             const long long a0 = in_off[order[b]], a1 = in_off[order[e - 1] + 1];
             CK(cudaMemcpyAsync(ctx->d_stage + (size_t)at * stride, xyz + (size_t)a0 * stride,
-                               (size_t)(a1 - a0) * stride * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+                               (size_t)(a1 - a0) * stride * sizeof(float), kind, ctx->stream));
             at += a1 - a0;
             b = e;
         }
@@ -1383,6 +1455,94 @@ static int device_exclusive_scan(dcreg_ctx* ctx, const int* in, long long n, int
     return DCREG_OK;
 }
 
+// ---- the voxel filter on the device (voxel_hash_kernel .. voxel_scatter_kernel) ---------------------------------------
+// Cloud b's table region: the least power of two >= 2 n_b slots.  tab[n + 1] gets the regions' offsets; returns the total.
+static long long voxel_tables(int n, const int64_t* h_seg, std::vector<long long>& tab) {
+    tab.assign((size_t)n + 1, 0);
+    for (int b = 0; b < n; ++b) {
+        long long cap = 2;
+        while (cap < 2 * (h_seg[b + 1] - h_seg[b])) cap <<= 1;
+        tab[(size_t)b + 1] = tab[(size_t)b] + cap;
+    }
+    return tab[(size_t)n];
+}
+
+// Room for a filter of n points in n_seg clouds over `slots` table slots
+static int voxel_reserve(dcreg_ctx* ctx, long long n, int n_seg, long long slots) {
+    CK(ctx->d_vox_keys.ensure(slots));
+    CK(ctx->d_vox_first.ensure(slots));
+    CK(ctx->d_vox_slot.ensure(n));
+    CK(ctx->d_vox_keep.ensure(n + 1));
+    CK(ctx->d_vox_pos.ensure(n + 1));
+    CK(ctx->d_vox_tab.ensure(n_seg + 1));
+    CK(ctx->d_vox_seg.ensure(n_seg + 1));
+    CK(ctx->d_vox_bad.ensure(n_seg));
+    return DCREG_OK;
+}
+
+// The voxel filter of n_seg clouds, n points of `stride` floats at d_in, with offsets d_seg (device) and h_seg (host).
+// The kept points go to d_out (out_stride 3 or 4, see voxel_scatter_kernel) and their indices in their own cloud to
+// d_index (null: not wanted); the kept offsets to ctx->d_vox_seg [n_seg + 1], and bad[b] != 0 in ctx->d_vox_bad when
+// cloud b has a voxel coordinate outside [-2^20, 2^20).  Six launches whatever n_seg, no host sync.
+static int voxel_filter(dcreg_ctx* ctx, const float* d_in, long long n, int stride, const long long* d_seg,
+                        const int64_t* h_seg, int n_seg, double voxel, float* d_out, int out_stride, long long* d_index) {
+    std::vector<long long> tab;
+    const long long slots = voxel_tables(n_seg, h_seg, tab);
+    int rc = voxel_reserve(ctx, n, n_seg, slots);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(ctx->d_vox_tab, tab.data(), tab.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(ctx->d_vox_keys, 0xff, (size_t)slots * sizeof(unsigned long long), ctx->stream));   // kEmptyKey
+    CK(cudaMemsetAsync(ctx->d_vox_first, 0x7f, (size_t)slots * sizeof(int), ctx->stream));   // above every index
+    CK(cudaMemsetAsync(ctx->d_vox_bad, 0, (size_t)n_seg * sizeof(int), ctx->stream));
+    const unsigned nb = (unsigned)((n + 255) / 256), nb1 = (unsigned)((n + 256) / 256);
+    voxel_hash_kernel<<<nb, 256, 0, ctx->stream>>>(d_in, n, stride, d_seg, n_seg, ctx->d_vox_tab, 1.0 / voxel,
+                                                   ctx->d_vox_keys, ctx->d_vox_first, ctx->d_vox_slot, ctx->d_vox_bad);
+    voxel_flag_kernel<<<nb1, 256, 0, ctx->stream>>>(ctx->d_vox_slot, n, ctx->d_vox_first, ctx->d_vox_keep);
+    ctx->launches += 2;
+    CK(cudaGetLastError());
+    if ((rc = device_exclusive_scan(ctx, ctx->d_vox_keep, n + 1, ctx->d_vox_pos))) return rc;
+    voxel_scatter_kernel<<<nb1, 256, 0, ctx->stream>>>(d_in, n, stride, d_seg, n_seg, ctx->d_vox_keep, ctx->d_vox_pos, d_out,
+                                                       out_stride, d_index, ctx->d_vox_seg);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return DCREG_OK;
+}
+
+// The voxel filter of n clouds of host points (xyz / offsets / stride as in dcreg_icp_run_scans, validated): the kept
+// points' xyz go to ctx->d_vox_xyz (3 floats a point, input order), their indices to ctx->d_vox_index when `index`.
+// One host sync, after which kept[n + 1] holds the kept offsets and bad[n] the range flags; fetch: *h_xyz (and *h_index)
+// then point at host copies of the kept xyz (and indices) in ctx->h_pinned.
+static int voxel_filter_host(dcreg_ctx* ctx, int n, const float* xyz, const int64_t* offsets, int stride, double voxel,
+                             bool index, bool fetch, int64_t* kept, int* bad, const float** h_xyz = nullptr,
+                             const long long** h_index = nullptr) {
+    const long long total = offsets[n];
+    CK(ctx->d_stage.ensure(total * stride));
+    CK(ctx->d_vox_in_seg.ensure(n + 1));
+    CK(ctx->d_vox_xyz.ensure(total * 3));
+    if (index) CK(ctx->d_vox_index.ensure(total));
+    CK(cudaMemcpyAsync(ctx->d_stage, xyz, (size_t)total * stride * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_vox_in_seg, offsets, (size_t)(n + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+    int rc = voxel_filter(ctx, ctx->d_stage, total, stride, ctx->d_vox_in_seg, offsets, n, voxel, ctx->d_vox_xyz, 3,
+                          index ? ctx->d_vox_index.p : nullptr);
+    if (rc) return rc;
+    // pinned: [n + 1] kept offsets, [n] flags (padded to 8 B), then (fetch) xyz [total][3] and indices [total]
+    const size_t b_seg = (size_t)(n + 1) * sizeof(long long), b_bad = ((size_t)n * sizeof(int) + 7) / 8 * 8;
+    const size_t b_xyz = fetch ? ((size_t)total * 3 * sizeof(float) + 7) / 8 * 8 : 0;
+    const size_t b_idx = fetch && index ? (size_t)total * sizeof(long long) : 0;
+    CK(ctx->h_pinned.ensure((long long)(b_seg + b_bad + b_xyz + b_idx)));
+    unsigned char* h = ctx->h_pinned.p;
+    CK(cudaMemcpyAsync(h, ctx->d_vox_seg, b_seg, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(h + b_seg, ctx->d_vox_bad, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    if (b_xyz) CK(cudaMemcpyAsync(h + b_seg + b_bad, ctx->d_vox_xyz, (size_t)total * 3 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    if (b_idx) CK(cudaMemcpyAsync(h + b_seg + b_bad + b_xyz, ctx->d_vox_index, b_idx, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    memcpy(kept, h, b_seg);
+    memcpy(bad, h + b_seg, (size_t)n * sizeof(int));
+    if (h_xyz) *h_xyz = (const float*)(h + b_seg + b_bad);
+    if (h_index) *h_index = (const long long*)(h + b_seg + b_bad + b_xyz);
+    return DCREG_OK;
+}
+
 // Grid arenas (dcreg_ctx::GridArena, planned by arena_plan.hpp): the dense grids of n clouds at once, cloud b being
 // d_pts[h_seg[b], h_seg[b+1]) (d_seg: the same offsets on the device).  One segmented bounds pass and one copy of the
 // n x 6 bounds to the host (arena_bounds: the only host sync), then one count, one exclusive scan, one scatter and one
@@ -1391,13 +1551,20 @@ static int device_exclusive_scan(dcreg_ctx* ctx, const int* in, long long n, int
 // h_seg[b]: the (distance, then index) order of the neighbour search and the equality of position lists are those of
 // the cloud built alone.  Replaces the kd-tree build of ICPContext::setTargetCloud (utils.hpp:393-424).
 
-// hb[n * 6]: per cloud the min cell coordinates (x, y, z), then the max (arena_plan::box_of)
+// Device bytes a caller wants back in the same sync as the bounds
+struct Readback { const void* dev; size_t bytes; void* host; };
+
+// hb[n * 6]: per cloud the min cell coordinates (x, y, z), then the max (arena_plan::box_of).  h_seg sizes the pass:
+// the clouds' point counts or upper bounds of them (d_seg is what the pass reads).  more: copied back before the sync
 static int arena_bounds(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_pts, const int64_t* h_seg,
-                        const long long* d_seg, int n, double inv_cell, std::vector<int>& hb) {
+                        const long long* d_seg, int n, double inv_cell, std::vector<int>& hb,
+                        const std::vector<Readback>& more = {}) {
     CK(A.d_grids.ensure(n));
     CK(A.d_cell_off.ensure(n + 1));
     CK(A.d_bounds.ensure((long long)n * 6));
-    CK(ctx->h_pinned.ensure((long long)n * 6 * sizeof(int)));
+    size_t pinned = ((size_t)n * 6 * sizeof(int) + 7) / 8 * 8;
+    for (const Readback& r : more) pinned += (r.bytes + 7) / 8 * 8;
+    CK(ctx->h_pinned.ensure((long long)pinned));
     hb.resize((size_t)n * 6);
     long long max_m = 0;
     for (int b = 0; b < n; ++b) {
@@ -1411,8 +1578,18 @@ static int arena_bounds(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d
     ctx->launches++;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(ctx->h_pinned, A.d_bounds, hb.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    size_t at = ((size_t)n * 6 * sizeof(int) + 7) / 8 * 8;
+    for (const Readback& r : more) {
+        CK(cudaMemcpyAsync(ctx->h_pinned.p + at, r.dev, r.bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        at += (r.bytes + 7) / 8 * 8;
+    }
     CK(cudaStreamSynchronize(ctx->stream));
     memcpy(hb.data(), ctx->h_pinned.p, hb.size() * sizeof(int));
+    at = ((size_t)n * 6 * sizeof(int) + 7) / 8 * 8;
+    for (const Readback& r : more) {
+        memcpy(r.host, ctx->h_pinned.p + at, r.bytes);
+        at += (r.bytes + 7) / 8 * 8;
+    }
     return DCREG_OK;
 }
 
@@ -1659,6 +1836,7 @@ struct Batch {
     const int64_t* offsets;
     const int* order = nullptr;
     const int64_t* in_off = nullptr;
+    cudaMemcpyKind kind = cudaMemcpyHostToDevice;   // cudaMemcpyDeviceToDevice: xyz is device memory
     // the sort (locality only): every source by the cells of its points under ...
     enum Sort {
         kContextGrid,   // ... its trial's initial pose, in the context's grid
@@ -1719,7 +1897,7 @@ static int stage_lanes(dcreg_ctx* ctx, int lanes, int frames, SeqView* v) {
 static int sort_sources(dcreg_ctx* ctx, const Batch& S, const float4** src_out) {
     const long long n = S.total();
     int rc = upload_points(ctx, S.xyz, n, S.stride, ctx->d_scan_seg, S.n, ctx->d_scan_src, ctx->d_scan_radius, S.order,
-                           S.in_off);
+                           S.in_off, S.kind);
     if (rc) return rc;
     unsigned long long* keys = ctx->d_scan_keys;
     int* vals = ctx->d_scan_vals;
@@ -2582,13 +2760,15 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
                     Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, true, &S);
 }
 
-int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
-                           int n_frames, const float* xyz, const int64_t* frame_offsets, int stride, double cell_size,
-                           int map_frames, int motion, const double* T_init, const double* deltas, double* T_prior,
-                           double* T_out, int* n_iterations, int* converged, int* status, double* cov,
-                           dcreg_iter_log* log, int log_cap) {
+// dcreg_icp_run_odometry (source_voxel = map_voxel = 0, `name` "icp_run_odometry") and dcreg_icp_run_odometry_voxel:
+// one body.  A voxel size of 0 leaves its filter out entirely: no launch, no copy, no sync.
+static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params* params, int n_seqs,
+                        const int* seq_offsets, int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                        double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                        const double* T_init, const double* deltas, int64_t* frame_points, double* T_prior, double* T_out,
+                        int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log, int log_cap) {
     if (!ctx) return DCREG_BAD_ARG;
-    BatchCheck c{"icp_run_odometry", params && n_seqs > 0 && n_frames > 0 && seq_offsets && xyz && frame_offsets && T_init && T_out,
+    BatchCheck c{name, params && n_seqs > 0 && n_frames > 0 && seq_offsets && xyz && frame_offsets && T_init && T_out,
                  "null pointer, n_seqs <= 0 or n_frames <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_frames};
     c.offsets = frame_offsets; c.item = "frame"; c.stride = stride; c.own_cell = true; c.cell_size = cell_size;
@@ -2598,15 +2778,44 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
         c.own_msg = "motion must be DCREG_MOTION_INCREMENTS or DCREG_MOTION_CONSTANT_VELOCITY";
     else if (motion == DCREG_MOTION_CONSTANT_VELOCITY && deltas)
         c.own_msg = "the constant-velocity model takes no deltas (pass NULL)";
+    else if (!(source_voxel >= 0.0 && source_voxel < INFINITY) || !(map_voxel >= 0.0 && map_voxel < INFINITY))
+        c.own_msg = "source_voxel and map_voxel must be finite and >= 0 (0: no filter)";
     int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
+    CK(cudaSetDevice(ctx->device));
+    // the frames' voxel filter: once per call, on the staged points in input order, before the pack and the sort; one
+    // sync for the kept counts.  From here on a frame is its kept points, on the device
+    const float* src_xyz = xyz;
+    int src_stride = stride;
+    const int64_t* src_off = frame_offsets;
+    std::vector<int64_t> kept;
+    if (source_voxel > 0.0) {
+        kept.resize((size_t)n_frames + 1);
+        std::vector<int> bad((size_t)n_frames);
+        if ((rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, source_voxel, false, false, kept.data(),
+                                    bad.data())))
+            return rc;
+        for (int s = 0; s < n_seqs; ++s)
+            for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k) {
+                const char* why = bad[(size_t)k] ? "a voxel coordinate of the source filter lies outside [-2^20, 2^20)"
+                                  : kept[(size_t)k + 1] == kept[(size_t)k] ? "no point is left by the source filter (no finite point)"
+                                                                           : nullptr;
+                if (why) {
+                    ctx->err = std::string(name) + ": sequence " + std::to_string(s) + ", frame " + std::to_string(k) +
+                               " (frame " + std::to_string(k - seq_offsets[s]) + " of the sequence): " + why;
+                    return DCREG_BAD_ARG;
+                }
+            }
+        src_xyz = ctx->d_vox_xyz; src_stride = 3; src_off = kept.data();
+    }
+    if (frame_points)
+        for (int k = 0; k < n_frames; ++k) frame_points[k] = src_off[k + 1] - src_off[k];
     odom_plan::Plan P;
     {
-        const std::string why = odom_plan::make(n_seqs, seq_offsets, n_frames, frame_offsets, map_frames,
+        const std::string why = odom_plan::make(n_seqs, seq_offsets, n_frames, src_off, map_frames,
                                                 arena_plan::kMaxPoints, &P);
         if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
     }
-    CK(cudaSetDevice(ctx->device));
     const int n_steps = (int)P.steps.size();
     // every step's tables in one upload: long long map_seg [A + 1], piece_dst [P + 1], piece_src [P]; int piece_frame
     // [P], prev [A], prev2 [A] (A lanes, P window frames)
@@ -2626,8 +2835,9 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
     // the frames in device order, each sorted by its own cell in the sensor frame (identity poses, a box of 1024^3 cells
     // around the sensor: locality only, the chained priors are not known yet); lanes: grid y of the loop kernel, a
     // lane's frame range set by odom_start_kernel at every step; grids: the step's local maps
-    Batch S{n_frames, xyz, stride, P.dev_off.data()};
-    S.order = P.input.data(); S.in_off = frame_offsets;
+    Batch S{n_frames, src_xyz, src_stride, P.dev_off.data()};
+    S.order = P.input.data(); S.in_off = src_off;
+    if (source_voxel > 0.0) S.kind = cudaMemcpyDeviceToDevice;
     S.sort = Batch::kBox;
     S.sort_box.inv_cell = 1.0 / cell_size;
     S.sort_box.ox = S.sort_box.oy = S.sort_box.oz = -512;
@@ -2640,6 +2850,14 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
     CK(ctx->d_odom_ll.ensure(std::max<long long>((long long)hll.size(), 1)));
     CK(ctx->d_odom_int.ensure(std::max<long long>((long long)hint.size(), 1)));
     CK(ctx->d_odom_map.ensure(std::max<long long>(P.max_map, 1)));
+    if (map_voxel > 0.0) {        // the maps' filter at its largest step, so no buffer regrows inside the loop
+        CK(ctx->d_odom_map_vox.ensure(std::max<long long>(P.max_map, 1)));
+        long long slots = 0;
+        std::vector<long long> tab;
+        for (int i = 1; i < n_steps; ++i)
+            slots = std::max(slots, voxel_tables(P.steps[(size_t)i].active, P.steps[(size_t)i].map_seg.data(), tab));
+        if ((rc = voxel_reserve(ctx, P.max_map, n_seqs, slots))) return rc;
+    }
     if (!hll.empty()) {
         CK(cudaMemcpyAsync(ctx->d_odom_ll, hll.data(), hll.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaMemcpyAsync(ctx->d_odom_int, hint.data(), hint.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
@@ -2682,25 +2900,53 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
                                                                                 d_frame, m, ctx->d_state, ctx->d_odom_map);
         ctx->launches++;
         CK(cudaGetLastError());
-        // 2. their dense grids, one arena segment per lane (the bounds copy is the step's sync besides the loop's peeks)
+        // 1b. (map_voxel) every lane's map through the voxel filter, in world coordinates, .w re-indexed over the step's
+        // kept map points; the grids are built over those, whose offsets come back in the bounds' copy
+        const float4* map = ctx->d_odom_map;
+        const long long* d_mseg = d_map_seg;
+        long long mk = m;
+        std::vector<int64_t> kept_map;
+        std::vector<int> bad_map;
+        std::vector<Readback> more;
+        if (map_voxel > 0.0) {
+            if ((rc = voxel_filter(ctx, (const float*)ctx->d_odom_map.p, m, 4, d_map_seg, st.map_seg.data(), st.active,
+                                   map_voxel, (float*)ctx->d_odom_map_vox.p, 4, nullptr)))
+                return rc;
+            map = ctx->d_odom_map_vox;
+            d_mseg = ctx->d_vox_seg;
+            kept_map.resize((size_t)st.active + 1);
+            bad_map.resize((size_t)st.active);
+            more = {Readback{ctx->d_vox_seg.p, kept_map.size() * sizeof(int64_t), kept_map.data()},
+                    Readback{ctx->d_vox_bad.p, bad_map.size() * sizeof(int), bad_map.data()}};
+        }
+        // 2. their dense grids, one arena segment per lane (the bounds copy is the step's sync besides the loop's peeks;
+        // the unfiltered map sizes bound the kept ones)
         std::vector<int> hb;
-        if ((rc = arena_bounds(ctx, ctx->odom_maps, ctx->d_odom_map, st.map_seg.data(), d_map_seg, st.active, inv_cell, hb)))
+        if ((rc = arena_bounds(ctx, ctx->odom_maps, map, st.map_seg.data(), d_mseg, st.active, inv_cell, hb, more)))
             return rc;
         std::vector<arena_plan::Box> boxes;
         long long cells = 0;
-        const std::string why = arena_plan::plan(st.active, hb.data(), boxes, &cells, "local map of lane");
-        if (!why.empty()) {
-            int b = 0;
+        int b = 0;
+        std::string why;
+        if (map_voxel > 0.0) {
+            while (b < st.active && !bad_map[(size_t)b]) ++b;
+            if (b < st.active) why = "its local map has a voxel coordinate of the map filter outside [-2^20, 2^20)";
+            mk = kept_map[(size_t)st.active];
+        }
+        if (why.empty()) {
+            why = arena_plan::plan(st.active, hb.data(), boxes, &cells, "local map of lane");
+            b = 0;
             arena_plan::Box x;
-            while (b < st.active - 1 && arena_plan::box_of(hb.data() + 6 * (size_t)b, &x) == arena_plan::kDense) ++b;
+            while (!why.empty() && b < st.active - 1 && arena_plan::box_of(hb.data() + 6 * (size_t)b, &x) == arena_plan::kDense) ++b;
+        }
+        if (!why.empty()) {
             const int s = st.seq[(size_t)b];
-            ctx->err = "icp_run_odometry: sequence " + std::to_string(s) + ", frame " + std::to_string(seq_offsets[s] + i) +
+            ctx->err = std::string(name) + ": sequence " + std::to_string(s) + ", frame " + std::to_string(seq_offsets[s] + i) +
                        " (frame " + std::to_string(i) + " of the sequence): " + why;
             failed = i;
             break;
         }
-        if ((rc = arena_fill(ctx, ctx->odom_maps, ctx->d_odom_map, d_map_seg, st.active, m, boxes.data(), cells, inv_cell,
-                             rings)))
+        if ((rc = arena_fill(ctx, ctx->odom_maps, map, d_mseg, st.active, mk, boxes.data(), cells, inv_cell, rings)))
             return rc;
         // 3. every lane's frame of this step: its prior and a fresh loop state
         odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
@@ -2723,6 +2969,55 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
                           failed < n_steps ? P.steps[(size_t)failed].first : n_frames)))
         return rc;
     if (failed < n_steps) { ctx->err = err; return DCREG_BAD_ARG; }
+    return DCREG_OK;
+}
+
+int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                           int n_frames, const float* xyz, const int64_t* frame_offsets, int stride, double cell_size,
+                           int map_frames, int motion, const double* T_init, const double* deltas, double* T_prior,
+                           double* T_out, int* n_iterations, int* converged, int* status, double* cov,
+                           dcreg_iter_log* log, int log_cap) {
+    return run_odometry(ctx, "icp_run_odometry", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
+                        cell_size, map_frames, motion, 0.0, 0.0, T_init, deltas, nullptr, T_prior, T_out, n_iterations,
+                        converged, status, cov, log, log_cap);
+}
+
+int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                                 int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                                 double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                                 const double* T_init, const double* deltas, int64_t* frame_points, double* T_prior,
+                                 double* T_out, int* n_iterations, int* converged, int* status, double* cov,
+                                 dcreg_iter_log* log, int log_cap) {
+    return run_odometry(ctx, "icp_run_odometry_voxel", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
+                        cell_size, map_frames, motion, source_voxel, map_voxel, T_init, deltas, frame_points, T_prior,
+                        T_out, n_iterations, converged, status, cov, log, log_cap);
+}
+
+int dcreg_voxel_downsample(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,
+                           double voxel, float* out_xyz, int64_t* out_offsets, int64_t* out_index) {
+    if (!ctx) return DCREG_BAD_ARG;
+    auto bad = [ctx](const std::string& why) { ctx->err = "voxel_downsample: " + why; return (int)DCREG_BAD_ARG; };
+    if (n_clouds <= 0 || !xyz || !offsets || !out_xyz || !out_offsets) return bad("null pointer or n_clouds <= 0");
+    if (stride < 3) return bad("stride < 3");
+    if (!(voxel > 0.0 && voxel < INFINITY)) return bad("voxel must be finite and > 0");
+    const std::string why = arena_plan::check_offsets(n_clouds, offsets, arena_plan::kMaxPoints, "cloud");
+    if (!why.empty()) return bad(why);
+    CK(cudaSetDevice(ctx->device));
+    std::vector<int> out_of_range((size_t)n_clouds);
+    std::vector<int64_t> kept((size_t)n_clouds + 1);
+    const float* h_xyz = nullptr;
+    const long long* h_index = nullptr;
+    int rc = voxel_filter_host(ctx, n_clouds, xyz, offsets, stride, voxel, out_index != nullptr, true, kept.data(),
+                               out_of_range.data(), &h_xyz, &h_index);
+    if (rc) return rc;
+    for (int b = 0; b < n_clouds; ++b)
+        if (out_of_range[(size_t)b])
+            return bad("cloud " + std::to_string(b) + ": a voxel coordinate lies outside [-2^20, 2^20) (voxel too small for "
+                       "the cloud's coordinates)");
+    memcpy(out_offsets, kept.data(), kept.size() * sizeof(int64_t));
+    const long long k = kept[(size_t)n_clouds];
+    memcpy(out_xyz, h_xyz, (size_t)k * 3 * sizeof(float));
+    if (out_index) memcpy(out_index, h_index, (size_t)k * sizeof(int64_t));
     return DCREG_OK;
 }
 

@@ -302,7 +302,7 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
  *   points in input order.  Point p of frame j becomes fl32(R_j p + t_j) with (R_j, t_j) = T_out[j]; each coordinate is
  *   ((r0 x + r1 y) + r2 z) + t in FP64 with one rounding per operation and no FMA, then one float32 rounding
  *   (dcreg_b200.api.map_points gives the same bits).  Every frame of the window goes in, aborted ones included, at the
- *   pose it returned; no downsampling, cropping or keyframe selection.
+ *   pose it returned; no downsampling (dcreg_icp_run_odometry_voxel adds voxel filters), cropping or keyframe selection.
  * - Prior of frame k: compose_prior(T_out[k-1], D) with the rounding rule of dcreg_icp_run_sequences.
  *   motion = DCREG_MOTION_INCREMENTS: D = deltas[k-1], or the identity when deltas is NULL.
  *   motion = DCREG_MOTION_CONSTANT_VELOCITY (deltas must be NULL): D = identity when frame k-1 is the anchor, else
@@ -327,6 +327,40 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
                            double cell_size, int map_frames, int motion, const double* T_init, const double* deltas,
                            double* T_prior, double* T_out, int* n_iterations, int* converged, int* status,
                            double* cov, dcreg_iter_log* log, int log_cap);
+/* dcreg_icp_run_odometry with voxel-filtered frames and local maps.  F_s(P) = dcreg_voxel_downsample(P, source_voxel),
+ * F_m(P) = dcreg_voxel_downsample(P, map_voxel); a voxel size of 0 means no filter (P itself).
+ * - Frame k's source is F_s(frame k), filtered in its own sensor frame.  frame_points (out, may be NULL): n_frames
+ *   counts, the size of F_s(frame k), anchors included (their kept points enter the maps too).
+ * - Map of frame k: F_m(concatenation over the window frames j of map_points(T_out[j], F_s(frame j))), with the window,
+ *   order and transform of dcreg_icp_run_odometry, filtered per sequence in world coordinates.
+ * - Frame k returns what dcreg_set_target(map_k, cell_size) + dcreg_set_source(F_s(frame k)) + dcreg_icp_run(T_prior[k])
+ *   returns, up to how the FP64 partial sums are grouped; priors, anchors, aborts, reproducibility and the untouched
+ *   context as in dcreg_icp_run_odometry, which is this call with source_voxel = map_voxel = 0 (same launches, same bytes).
+ * - Cost: the frames are filtered once per call (one extra host sync for the kept counts); each step's maps are
+ *   filtered on the device (six more launches per step whatever the number of sequences) and their kept counts come
+ *   back in the copy of the grids' bounds, so a step keeps its one host sync.
+ * Errors (DCREG_BAD_ARG, dcreg_last_error naming the sequence and frame): a negative or non-finite voxel size (before
+ * anything is launched); a frame with no finite point, or a voxel coordinate of the source filter outside [-2^20, 2^20)
+ * (after the frames' filter, before any loop launch); a step's map with a voxel coordinate outside that range (at its
+ * step, like a map too large for a dense grid: the earlier steps keep their outputs, the context stays usable). */
+int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                                 int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                                 double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                                 const double* T_init, const double* deltas, int64_t* frame_points, double* T_prior,
+                                 double* T_out, int* n_iterations, int* converged, int* status, double* cov,
+                                 dcreg_iter_log* log, int log_cap);
+/* Voxel downsampling of many clouds in one call (KISS-ICP's VoxelDownsample rule: the first point of every voxel).
+ * xyz / offsets / stride: HOST memory as in dcreg_icp_run_scans (n_clouds + 1 offsets, ascending strictly from 0, at
+ * most 2^29 - 1 points).  With inv = 1.0 / voxel in FP64, point i's voxel is (floor((double)x inv), floor((double)y inv),
+ * floor((double)z inv)); a point with a non-finite coordinate has none and is dropped.  Each voxel keeps its point of
+ * smallest index, its coordinates copied bit for bit; the kept points stay in input order.  dcreg_b200.api.voxel_downsample
+ * gives the same selection.  Every voxel coordinate must lie in [-2^20, 2^20) (checked in FP64): a cloud outside it is
+ * DCREG_BAD_ARG naming the cloud.  out_xyz: room for offsets[n_clouds] x 3 floats, cloud b's kept points being
+ * [out_offsets[b], out_offsets[b+1]) (n_clouds + 1 entries); out_index (may be NULL): each kept point's index inside its
+ * own cloud.  One host sync; the launches do not depend on n_clouds.  The context's source, target and grid are left
+ * as they were. */
+int dcreg_voxel_downsample(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,
+                           double voxel, float* out_xyz, int64_t* out_offsets, int64_t* out_index);
 /* Same loop, but correspondences are supplied by the caller each iteration through a callback
  * (host kd-tree mode, "PR1"): planes are 4*n doubles (nx,ny,nz,d), all-zero = none. */
 typedef int (*dcreg_plane_callback)(void* user, const double T[16], double* planes4,
