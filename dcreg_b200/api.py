@@ -17,6 +17,7 @@ There is NO CPU fallback: if the CUDA library is missing or no GPU is visible th
 from __future__ import annotations
 
 import ctypes as C
+import operator
 import os
 import types
 
@@ -88,7 +89,7 @@ EXPORTS = [
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_voxel_downsample", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -140,6 +141,12 @@ def load_library():
                                                  C.POINTER(IterLog), ci]
     lib.dcreg_voxel_downsample.argtypes = [vp, ci, C.POINTER(C.c_float), C.POINTER(i64), ci, C.c_double,
                                            C.POINTER(C.c_float), C.POINTER(i64), C.POINTER(i64)]
+    lib.dcreg_icp_run_odometry_voxel_n.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
+                                                   C.POINTER(i64), ci, C.c_double, ci, ci, C.c_double, C.c_double, ci, ci,
+                                                   dp, dp, C.POINTER(i64), dp, dp, C.POINTER(ci), C.POINTER(ci),
+                                                   C.POINTER(ci), dp, C.POINTER(IterLog), ci]
+    lib.dcreg_voxel_downsample_n.argtypes = [vp, ci, C.POINTER(C.c_float), C.POINTER(i64), ci, C.c_double, ci,
+                                             C.POINTER(C.c_float), C.POINTER(i64), C.POINTER(i64)]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -277,15 +284,30 @@ def constant_velocity_increment(T_prev, T):
 VOXEL_LIMIT = 1 << 20      # voxel coordinates must lie in [-2^20, 2^20): 21 bits per axis in one 63-bit key
 
 
-def voxel_downsample(P, voxel):
-    """The voxel filter of dcreg_voxel_downsample, bit for bit: the voxel of a point is np.floor(p.astype(float64) *
-    (1.0 / voxel)) per axis, rows with a non-finite coordinate have none and are dropped, and each voxel keeps its first
-    point.  P: (N, >=3).  Returns (points (K, 3) float32, the kept rows' coordinates unchanged; index (K,) int64, their
-    rows in P, ascending).  Raises ValueError for a voxel that is not finite and > 0, or a voxel coordinate outside
-    [-2^20, 2^20)."""
+def _max_points(v, name="max_points"):
+    """A voxel filter's cap as a C int: an integer >= 1 (bools and floats are refused)"""
+    if isinstance(v, (bool, np.bool_)):
+        raise ValueError(f"{name} must be an integer >= 1, not {v!r}")
+    try:
+        n = operator.index(v)
+    except TypeError:
+        raise ValueError(f"{name} must be an integer >= 1, not {v!r}") from None
+    if not 1 <= n < 2 ** 31:
+        raise ValueError(f"{name} must be an integer in [1, 2^31), not {n}")
+    return n
+
+
+def voxel_downsample(P, voxel, max_points=1):
+    """The voxel filter of dcreg_voxel_downsample_n, bit for bit: the voxel of a point is np.floor(p.astype(float64) *
+    (1.0 / voxel)) per axis, rows with a non-finite coordinate have none and are dropped, and each voxel keeps its
+    max_points points of smallest index (1: its first point, dcreg_voxel_downsample).  P: (N, >=3).  Returns (points
+    (K, 3) float32, the kept rows' coordinates unchanged; index (K,) int64, their rows in P, ascending).  Raises
+    ValueError for a voxel that is not finite and > 0, a max_points that is not an integer >= 1, or a voxel coordinate
+    outside [-2^20, 2^20)."""
     P = np.asarray(P, dtype=np.float32)
     if P.ndim != 2 or P.shape[1] < 3:
         raise ValueError("points must be (N, >=3)")
+    max_points = _max_points(max_points)
     voxel = float(voxel)
     if not (voxel > 0.0 and np.isfinite(voxel)):
         raise ValueError(f"voxel_downsample: voxel must be finite and > 0, not {voxel}")
@@ -297,8 +319,16 @@ def voxel_downsample(P, voxel):
         raise ValueError("voxel_downsample: a voxel coordinate lies outside [-2^20, 2^20) (voxel too small for the "
                          "cloud's coordinates)")
     k = keys.astype(np.int64) + VOXEL_LIMIT
-    _, first = np.unique((k[:, 0] << 42) | (k[:, 1] << 21) | k[:, 2], return_index=True)
-    keep = rows[np.sort(first)].astype(np.int64)
+    ids = (k[:, 0] << 42) | (k[:, 1] << 21) | k[:, 2]
+    # a stable sort by voxel keeps each voxel's rows ascending: a row's rank in its voxel is its distance to the voxel's
+    # first sorted position
+    order = np.argsort(ids, kind="stable")
+    s = ids[order]
+    at = np.arange(len(s))
+    starts = np.ones(len(s), dtype=bool)
+    starts[1:] = s[1:] != s[:-1]
+    rank = at - np.maximum.accumulate(np.where(starts, at, 0))
+    keep = rows[np.sort(order[rank < max_points])].astype(np.int64)
     return np.ascontiguousarray(xyz[keep]), keep
 
 
@@ -568,22 +598,25 @@ class Context:
         return self._run_batched("icp_run_sequences", call, params, n, S, "sequences", T_init, want_log, want_cov, deltas,
                                  want_prior=True)
 
-    def voxel_downsample(self, clouds, voxel: float):
-        """dcreg_voxel_downsample of every cloud (a list of (N_b, >=3) arrays) in one call on the device: a list of
-        (points (K_b, 3) float32, index (K_b,) int64), as api.voxel_downsample gives for each cloud alone."""
+    def voxel_downsample(self, clouds, voxel: float, max_points: int = 1):
+        """dcreg_voxel_downsample_n of every cloud (a list of (N_b, >=3) arrays) in one call on the device, each voxel
+        keeping up to max_points points: a list of (points (K_b, 3) float32, index (K_b,) int64), as
+        api.voxel_downsample gives for each cloud alone."""
+        max_points = _max_points(max_points)
         xyz, off = _pack(clouds)
         n = len(clouds)
         total = int(off[-1]) if n else 0
         pts = np.empty((max(total, 1), 3), dtype=np.float32)
         idx = np.empty(max(total, 1), dtype=np.int64)
         kept = np.zeros(n + 1, dtype=np.int64)
-        self._check(self.lib.dcreg_voxel_downsample(self._h, n, _fptr(xyz), _iptr(off), 3, float(voxel), _fptr(pts),
-                                                    _iptr(kept), _iptr(idx)))
+        self._check(self.lib.dcreg_voxel_downsample_n(self._h, n, _fptr(xyz), _iptr(off), 3, float(voxel), max_points,
+                                                      _fptr(pts), _iptr(kept), _iptr(idx)))
         return [(pts[a:b].copy(), idx[a:b].copy()) for a, b in zip(kept[:-1], kept[1:])]
 
     def icp_run_odometry(self, params: IcpParams, sequences, T_init, deltas=None, motion: str = "increments",
                          map_frames: int = 10, cell_size=None, want_log: bool = False, want_cov: bool = False,
-                         source_voxel: float = 0.0, map_voxel: float = 0.0):
+                         source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
+                         map_max_points: int = 1):
         """Scan-to-map odometry (`sequences`: a list of lists of (N, >=3) point arrays): frame k of a sequence registers
         against the local map of the frames [k - map_frames, k) before it, each placed at its own registered pose
         (map_points), starting from compose_prior(frame k-1's result, D).  motion "increments": D = deltas[k-1]
@@ -591,21 +624,32 @@ class Context:
         constant_velocity_increment(T_out[k-2], T_out[k-1]) (identity after the anchor; deltas must be None).  The first
         frame of each sequence is its anchor: not registered, T = T_prior = T_init[s].  cell_size: the maps' grid cell
         (default search_radius).  source_voxel / map_voxel (0: no filter): voxel_downsample every frame in its sensor
-        frame, and every local map in world coordinates (dcreg_icp_run_odometry_voxel).  Returns a list of IcpResult,
-        one per frame in order, with .T_prior and .n_points, the frame's points after the source filter (logs only when
-        want_log, .cov when want_cov).  Needs no target; the context's source and target are left as they were."""
+        frame, and every local map in world coordinates (dcreg_icp_run_odometry_voxel); source_max_points /
+        map_max_points: the points each voxel of those filters keeps (dcreg_icp_run_odometry_voxel_n).  Returns a list of
+        IcpResult, one per frame in order, with .T_prior and .n_points, the frame's points after the source filter (logs
+        only when want_log, .cov when want_cov).  Needs no target; the context's source and target are left as they
+        were."""
         models = {"increments": 0, "constant_velocity": 1}
         if motion not in models:
             raise ValueError(f"icp_run_odometry: motion must be one of {sorted(models)}, not {motion!r}")
+        source_max_points = _max_points(source_max_points, "source_max_points")
+        map_max_points = _max_points(map_max_points, "map_max_points")
         seq_off, xyz, off = _pack_sequences(sequences)
         S, n = len(sequences), int(seq_off[-1])
         cell = float(params.search_radius if cell_size is None else cell_size)
-        filtered = source_voxel != 0.0 or map_voxel != 0.0
+        capped = source_max_points != 1 or map_max_points != 1
+        filtered = source_voxel != 0.0 or map_voxel != 0.0 or capped
         npts = np.diff(off) if off is not None else np.zeros(0, dtype=np.int64)
         if filtered:
             npts = np.zeros(max(n, 1), dtype=np.int64)
 
         def call(o):
+            if capped:
+                return self.lib.dcreg_icp_run_odometry_voxel_n(
+                    self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
+                    3, cell, int(map_frames), models[motion], float(source_voxel), float(map_voxel), source_max_points,
+                    map_max_points, _optr(o.T_init), _optr(o.deltas), _iptr(npts), _optr(o.T_prior), _optr(o.T_out),
+                    o.n_it, o.conv, o.st, _optr(o.cov), o.logs, o.cap)
             if filtered:
                 return self.lib.dcreg_icp_run_odometry_voxel(
                     self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),

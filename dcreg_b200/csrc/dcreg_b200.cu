@@ -927,8 +927,8 @@ __global__ void odom_start_kernel(IcpState* states, const long long* __restrict_
 // ---- voxel filter (dcreg_voxel_downsample, dcreg_icp_run_odometry_voxel) -------------------------------------------
 // n points (`stride` floats each: host layout, or float4) in n_seg clouds, cloud b being points [seg[b], seg[b+1]).
 // Point i's voxel is floor((double)p * inv) per axis (corr::cell_coord before the integer conversion); the survivor of a
-// voxel is its point of smallest index, kept bit for bit, and the survivors keep their input order.  Four passes for all
-// clouds at once: hash, flag, exclusive scan, scatter.
+// voxel is its point of smallest index (with a cap of max_points: its max_points points of smallest index), kept bit for
+// bit, and the survivors keep their input order.  Four passes for all clouds at once: hash, flag, exclusive scan, scatter.
 constexpr double kVoxelLimit = 1048576.0;   // voxel coordinates must lie in [-2^20, 2^20): the range of corr::pack_key
 
 // Pass 1: cloud b owns the slots [tab[b], tab[b+1]) (a power of two) of the open-addressing table keys / first; point i
@@ -970,6 +970,31 @@ __global__ void voxel_flag_kernel(const long long* __restrict__ slot_of, long lo
     if (i > n) return;
     const long long s = i < n ? slot_of[i] : -1;
     keep[i] = s >= 0 && first[s] == (int)i;
+}
+
+// A cap of max_points > 1 points per voxel (dcreg_voxel_downsample_n) replaces pass 2 by a stable radix sort of the
+// points by slot and a flag pass over the sorted order.  The sort's input: key[i] = point i's slot as a uint32, or
+// `dropped` (the table's slot count: it sorts last) for a point with none; val[i] = i
+__global__ void voxel_sort_keys_kernel(const long long* __restrict__ slot_of, long long n, unsigned int dropped,
+                                       unsigned int* __restrict__ key, int* __restrict__ val) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const long long s = slot_of[i];
+    key[i] = s >= 0 ? (unsigned int)s : dropped;
+    val[i] = (int)i;
+}
+
+// key / val sorted stably by key, so a voxel's points are one run with their indices ascending: the point at sorted
+// position p has rank p - (start of its run) in its voxel, which is below max_points iff p < max_points or the key
+// max_points positions back differs.  keep[val[p]] = that for a point with a slot; keep[n] = 0.  n + 1 threads, O(1)
+// each whatever a voxel's occupancy.
+__global__ void voxel_cap_flag_kernel(const unsigned int* __restrict__ key, const int* __restrict__ val, long long n,
+                                      unsigned int dropped, int max_points, int* __restrict__ keep) {
+    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p > n) return;
+    if (p == n) { keep[n] = 0; return; }
+    const unsigned int k = key[p];
+    keep[val[p]] = k != dropped && (p < max_points || key[p - max_points] != k);
 }
 
 // Pass 4 (pos: the exclusive scan of keep): kept point i goes to out[pos[i]] (out_stride 3: x y z; 4: x y z and w = its
@@ -1133,6 +1158,9 @@ struct dcreg_ctx {
     DevBuf<long long> d_vox_slot; DevBuf<int> d_vox_keep, d_vox_pos;
     DevBuf<long long> d_vox_tab, d_vox_in_seg, d_vox_seg; DevBuf<int> d_vox_bad;
     DevBuf<float> d_vox_xyz; DevBuf<long long> d_vox_index;
+    // ... and with a cap above one point per voxel: [2][points] sort keys (slots) and values (indices) in / out
+    DevBuf<unsigned int> d_vox_skey; DevBuf<int> d_vox_sval;
+    DevBuf<unsigned char> d_vox_sort_tmp;
     // Grow-only arenas of dense grids (build_grid_arena): the context's target (one cloud; `grid` points into it), the
     // targets of dcreg_icp_run_pairs (the context's target and grid stay as they were), the grids over the aligned
     // sources of the point-to-point metrics, and odometry's local maps
@@ -1467,8 +1495,17 @@ static long long voxel_tables(int n, const int64_t* h_seg, std::vector<long long
     return tab[(size_t)n];
 }
 
-// Room for a filter of n points in n_seg clouds over `slots` table slots
-static int voxel_reserve(dcreg_ctx* ctx, long long n, int n_seg, long long slots) {
+// The radix sort's end bit for a table of `slots` slots: the bit width of `slots`, the key of a point with no slot (below
+// 4 n + 2 n_seg < 2^32 for n <= 2^29 - 1 points)
+static int voxel_key_bits(long long slots) {
+    int bits = 1;
+    while (slots >> bits) ++bits;
+    return bits;
+}
+
+// Room for a filter of n points in n_seg clouds over `slots` table slots, keeping up to max_points points per voxel.
+// The sort's scratch only grows with n and slots, so room for the largest of several filters is room for each of them
+static int voxel_reserve(dcreg_ctx* ctx, long long n, int n_seg, long long slots, int max_points = 1) {
     CK(ctx->d_vox_keys.ensure(slots));
     CK(ctx->d_vox_first.ensure(slots));
     CK(ctx->d_vox_slot.ensure(n));
@@ -1477,18 +1514,29 @@ static int voxel_reserve(dcreg_ctx* ctx, long long n, int n_seg, long long slots
     CK(ctx->d_vox_tab.ensure(n_seg + 1));
     CK(ctx->d_vox_seg.ensure(n_seg + 1));
     CK(ctx->d_vox_bad.ensure(n_seg));
+    if (max_points > 1) {
+        CK(ctx->d_vox_skey.ensure(2 * n));
+        CK(ctx->d_vox_sval.ensure(2 * n));
+        size_t tmp = 0;
+        CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, (const unsigned int*)nullptr, (unsigned int*)nullptr,
+                                           (const int*)nullptr, (int*)nullptr, (int)n, 0, voxel_key_bits(slots),
+                                           ctx->stream));
+        CK(ctx->d_vox_sort_tmp.ensure(std::max<long long>((long long)tmp, 1)));
+    }
     return DCREG_OK;
 }
 
-// The voxel filter of n_seg clouds, n points of `stride` floats at d_in, with offsets d_seg (device) and h_seg (host).
-// The kept points go to d_out (out_stride 3 or 4, see voxel_scatter_kernel) and their indices in their own cloud to
-// d_index (null: not wanted); the kept offsets to ctx->d_vox_seg [n_seg + 1], and bad[b] != 0 in ctx->d_vox_bad when
-// cloud b has a voxel coordinate outside [-2^20, 2^20).  Six launches whatever n_seg, no host sync.
+// The voxel filter of n_seg clouds, n points of `stride` floats at d_in, with offsets d_seg (device) and h_seg (host),
+// keeping up to max_points points per voxel.  The kept points go to d_out (out_stride 3 or 4, see voxel_scatter_kernel)
+// and their indices in their own cloud to d_index (null: not wanted); the kept offsets to ctx->d_vox_seg [n_seg + 1], and
+// bad[b] != 0 in ctx->d_vox_bad when cloud b has a voxel coordinate outside [-2^20, 2^20).  No host sync; whatever
+// n_seg, six launches for max_points = 1, and for max_points > 1 seven and the radix sort's own.
 static int voxel_filter(dcreg_ctx* ctx, const float* d_in, long long n, int stride, const long long* d_seg,
-                        const int64_t* h_seg, int n_seg, double voxel, float* d_out, int out_stride, long long* d_index) {
+                        const int64_t* h_seg, int n_seg, double voxel, float* d_out, int out_stride, long long* d_index,
+                        int max_points = 1) {
     std::vector<long long> tab;
     const long long slots = voxel_tables(n_seg, h_seg, tab);
-    int rc = voxel_reserve(ctx, n, n_seg, slots);
+    int rc = voxel_reserve(ctx, n, n_seg, slots, max_points);
     if (rc) return rc;
     CK(cudaMemcpyAsync(ctx->d_vox_tab, tab.data(), tab.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemsetAsync(ctx->d_vox_keys, 0xff, (size_t)slots * sizeof(unsigned long long), ctx->stream));   // kEmptyKey
@@ -1497,9 +1545,24 @@ static int voxel_filter(dcreg_ctx* ctx, const float* d_in, long long n, int stri
     const unsigned nb = (unsigned)((n + 255) / 256), nb1 = (unsigned)((n + 256) / 256);
     voxel_hash_kernel<<<nb, 256, 0, ctx->stream>>>(d_in, n, stride, d_seg, n_seg, ctx->d_vox_tab, 1.0 / voxel,
                                                    ctx->d_vox_keys, ctx->d_vox_first, ctx->d_vox_slot, ctx->d_vox_bad);
-    voxel_flag_kernel<<<nb1, 256, 0, ctx->stream>>>(ctx->d_vox_slot, n, ctx->d_vox_first, ctx->d_vox_keep);
-    ctx->launches += 2;
-    CK(cudaGetLastError());
+    if (max_points == 1) {
+        voxel_flag_kernel<<<nb1, 256, 0, ctx->stream>>>(ctx->d_vox_slot, n, ctx->d_vox_first, ctx->d_vox_keep);
+        ctx->launches += 2;
+        CK(cudaGetLastError());
+    } else {
+        unsigned int* key = ctx->d_vox_skey;
+        int* val = ctx->d_vox_sval;
+        const unsigned int dropped = (unsigned int)slots;
+        voxel_sort_keys_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_vox_slot, n, dropped, key, val);
+        ctx->launches += 2;
+        CK(cudaGetLastError());
+        size_t tmp = (size_t)ctx->d_vox_sort_tmp.cap;
+        CK(cub::DeviceRadixSort::SortPairs(ctx->d_vox_sort_tmp.p, tmp, key, key + n, val, val + n, (int)n, 0,
+                                           voxel_key_bits(slots), ctx->stream));
+        voxel_cap_flag_kernel<<<nb1, 256, 0, ctx->stream>>>(key + n, val + n, n, dropped, max_points, ctx->d_vox_keep);
+        ctx->launches++;                                         // (the radix sort's own kernels are not counted)
+        CK(cudaGetLastError());
+    }
     if ((rc = device_exclusive_scan(ctx, ctx->d_vox_keep, n + 1, ctx->d_vox_pos))) return rc;
     voxel_scatter_kernel<<<nb1, 256, 0, ctx->stream>>>(d_in, n, stride, d_seg, n_seg, ctx->d_vox_keep, ctx->d_vox_pos, d_out,
                                                        out_stride, d_index, ctx->d_vox_seg);
@@ -1508,13 +1571,13 @@ static int voxel_filter(dcreg_ctx* ctx, const float* d_in, long long n, int stri
     return DCREG_OK;
 }
 
-// The voxel filter of n clouds of host points (xyz / offsets / stride as in dcreg_icp_run_scans, validated): the kept
-// points' xyz go to ctx->d_vox_xyz (3 floats a point, input order), their indices to ctx->d_vox_index when `index`.
-// One host sync, after which kept[n + 1] holds the kept offsets and bad[n] the range flags; fetch: *h_xyz (and *h_index)
-// then point at host copies of the kept xyz (and indices) in ctx->h_pinned.
+// The voxel filter of n clouds of host points (xyz / offsets / stride as in dcreg_icp_run_scans, validated), up to
+// max_points points per voxel: the kept points' xyz go to ctx->d_vox_xyz (3 floats a point, input order), their indices
+// to ctx->d_vox_index when `index`.  One host sync, after which kept[n + 1] holds the kept offsets and bad[n] the range
+// flags; fetch: *h_xyz (and *h_index) then point at host copies of the kept xyz (and indices) in ctx->h_pinned.
 static int voxel_filter_host(dcreg_ctx* ctx, int n, const float* xyz, const int64_t* offsets, int stride, double voxel,
-                             bool index, bool fetch, int64_t* kept, int* bad, const float** h_xyz = nullptr,
-                             const long long** h_index = nullptr) {
+                             int max_points, bool index, bool fetch, int64_t* kept, int* bad,
+                             const float** h_xyz = nullptr, const long long** h_index = nullptr) {
     const long long total = offsets[n];
     CK(ctx->d_stage.ensure(total * stride));
     CK(ctx->d_vox_in_seg.ensure(n + 1));
@@ -1523,7 +1586,7 @@ static int voxel_filter_host(dcreg_ctx* ctx, int n, const float* xyz, const int6
     CK(cudaMemcpyAsync(ctx->d_stage, xyz, (size_t)total * stride * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_vox_in_seg, offsets, (size_t)(n + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
     int rc = voxel_filter(ctx, ctx->d_stage, total, stride, ctx->d_vox_in_seg, offsets, n, voxel, ctx->d_vox_xyz, 3,
-                          index ? ctx->d_vox_index.p : nullptr);
+                          index ? ctx->d_vox_index.p : nullptr, max_points);
     if (rc) return rc;
     // pinned: [n + 1] kept offsets, [n] flags (padded to 8 B), then (fetch) xyz [total][3] and indices [total]
     const size_t b_seg = (size_t)(n + 1) * sizeof(long long), b_bad = ((size_t)n * sizeof(int) + 7) / 8 * 8;
@@ -2760,13 +2823,15 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
                     Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, true, &S);
 }
 
-// dcreg_icp_run_odometry (source_voxel = map_voxel = 0, `name` "icp_run_odometry") and dcreg_icp_run_odometry_voxel:
-// one body.  A voxel size of 0 leaves its filter out entirely: no launch, no copy, no sync.
+// dcreg_icp_run_odometry (source_voxel = map_voxel = 0, `name` "icp_run_odometry"), dcreg_icp_run_odometry_voxel (caps
+// of 1) and dcreg_icp_run_odometry_voxel_n: one body.  A voxel size of 0 leaves its filter out entirely: no launch, no
+// copy, no sync.
 static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params* params, int n_seqs,
                         const int* seq_offsets, int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
                         double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
-                        const double* T_init, const double* deltas, int64_t* frame_points, double* T_prior, double* T_out,
-                        int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log, int log_cap) {
+                        int source_max_points, int map_max_points, const double* T_init, const double* deltas,
+                        int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                        int* status, double* cov, dcreg_iter_log* log, int log_cap) {
     if (!ctx) return DCREG_BAD_ARG;
     BatchCheck c{name, params && n_seqs > 0 && n_frames > 0 && seq_offsets && xyz && frame_offsets && T_init && T_out,
                  "null pointer, n_seqs <= 0 or n_frames <= 0",
@@ -2780,6 +2845,8 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         c.own_msg = "the constant-velocity model takes no deltas (pass NULL)";
     else if (!(source_voxel >= 0.0 && source_voxel < INFINITY) || !(map_voxel >= 0.0 && map_voxel < INFINITY))
         c.own_msg = "source_voxel and map_voxel must be finite and >= 0 (0: no filter)";
+    else if (source_max_points < 1 || map_max_points < 1)
+        c.own_msg = "source_max_points and map_max_points must be >= 1";
     int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
@@ -2792,8 +2859,8 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
     if (source_voxel > 0.0) {
         kept.resize((size_t)n_frames + 1);
         std::vector<int> bad((size_t)n_frames);
-        if ((rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, source_voxel, false, false, kept.data(),
-                                    bad.data())))
+        if ((rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, source_voxel, source_max_points, false,
+                                    false, kept.data(), bad.data())))
             return rc;
         for (int s = 0; s < n_seqs; ++s)
             for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k) {
@@ -2856,7 +2923,7 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         std::vector<long long> tab;
         for (int i = 1; i < n_steps; ++i)
             slots = std::max(slots, voxel_tables(P.steps[(size_t)i].active, P.steps[(size_t)i].map_seg.data(), tab));
-        if ((rc = voxel_reserve(ctx, P.max_map, n_seqs, slots))) return rc;
+        if ((rc = voxel_reserve(ctx, P.max_map, n_seqs, slots, map_max_points))) return rc;
     }
     if (!hll.empty()) {
         CK(cudaMemcpyAsync(ctx->d_odom_ll, hll.data(), hll.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
@@ -2910,7 +2977,7 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         std::vector<Readback> more;
         if (map_voxel > 0.0) {
             if ((rc = voxel_filter(ctx, (const float*)ctx->d_odom_map.p, m, 4, d_map_seg, st.map_seg.data(), st.active,
-                                   map_voxel, (float*)ctx->d_odom_map_vox.p, 4, nullptr)))
+                                   map_voxel, (float*)ctx->d_odom_map_vox.p, 4, nullptr, map_max_points)))
                 return rc;
             map = ctx->d_odom_map_vox;
             d_mseg = ctx->d_vox_seg;
@@ -2978,8 +3045,8 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
                            double* T_out, int* n_iterations, int* converged, int* status, double* cov,
                            dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
-                        cell_size, map_frames, motion, 0.0, 0.0, T_init, deltas, nullptr, T_prior, T_out, n_iterations,
-                        converged, status, cov, log, log_cap);
+                        cell_size, map_frames, motion, 0.0, 0.0, 1, 1, T_init, deltas, nullptr, T_prior, T_out,
+                        n_iterations, converged, status, cov, log, log_cap);
 }
 
 int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
@@ -2989,14 +3056,33 @@ int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params,
                                  double* T_out, int* n_iterations, int* converged, int* status, double* cov,
                                  dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_voxel", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
-                        cell_size, map_frames, motion, source_voxel, map_voxel, T_init, deltas, frame_points, T_prior,
-                        T_out, n_iterations, converged, status, cov, log, log_cap);
+                        cell_size, map_frames, motion, source_voxel, map_voxel, 1, 1, T_init, deltas, frame_points,
+                        T_prior, T_out, n_iterations, converged, status, cov, log, log_cap);
+}
+
+int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                                   int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                                   double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                                   int source_max_points, int map_max_points, const double* T_init,
+                                   const double* deltas, int64_t* frame_points, double* T_prior, double* T_out,
+                                   int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
+                                   int log_cap) {
+    return run_odometry(ctx, "icp_run_odometry_voxel_n", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets,
+                        stride, cell_size, map_frames, motion, source_voxel, map_voxel, source_max_points,
+                        map_max_points, T_init, deltas, frame_points, T_prior, T_out, n_iterations, converged, status,
+                        cov, log, log_cap);
 }
 
 int dcreg_voxel_downsample(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,
                            double voxel, float* out_xyz, int64_t* out_offsets, int64_t* out_index) {
+    return dcreg_voxel_downsample_n(ctx, n_clouds, xyz, offsets, stride, voxel, 1, out_xyz, out_offsets, out_index);
+}
+
+int dcreg_voxel_downsample_n(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,
+                             double voxel, int max_points, float* out_xyz, int64_t* out_offsets, int64_t* out_index) {
     if (!ctx) return DCREG_BAD_ARG;
     auto bad = [ctx](const std::string& why) { ctx->err = "voxel_downsample: " + why; return (int)DCREG_BAD_ARG; };
+    if (max_points < 1) return bad("max_points must be >= 1");
     if (n_clouds <= 0 || !xyz || !offsets || !out_xyz || !out_offsets) return bad("null pointer or n_clouds <= 0");
     if (stride < 3) return bad("stride < 3");
     if (!(voxel > 0.0 && voxel < INFINITY)) return bad("voxel must be finite and > 0");
@@ -3007,8 +3093,8 @@ int dcreg_voxel_downsample(dcreg_ctx* ctx, int n_clouds, const float* xyz, const
     std::vector<int64_t> kept((size_t)n_clouds + 1);
     const float* h_xyz = nullptr;
     const long long* h_index = nullptr;
-    int rc = voxel_filter_host(ctx, n_clouds, xyz, offsets, stride, voxel, out_index != nullptr, true, kept.data(),
-                               out_of_range.data(), &h_xyz, &h_index);
+    int rc = voxel_filter_host(ctx, n_clouds, xyz, offsets, stride, voxel, max_points, out_index != nullptr, true,
+                               kept.data(), out_of_range.data(), &h_xyz, &h_index);
     if (rc) return rc;
     for (int b = 0; b < n_clouds; ++b)
         if (out_of_range[(size_t)b])

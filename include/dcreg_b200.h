@@ -349,6 +349,22 @@ int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params,
                                  const double* T_init, const double* deltas, int64_t* frame_points, double* T_prior,
                                  double* T_out, int* n_iterations, int* converged, int* status, double* cov,
                                  dcreg_iter_log* log, int log_cap);
+/* dcreg_icp_run_odometry_voxel with a cap on the points each voxel keeps: F_s(P) = dcreg_voxel_downsample_n(P,
+ * source_voxel, source_max_points), F_m(P) = dcreg_voxel_downsample_n(P, map_voxel, map_max_points); everything else
+ * as in dcreg_icp_run_odometry_voxel, which is this call with source_max_points = map_max_points = 1 (same launches,
+ * same bytes).  A map cap of KISS-ICP's default 20 keeps a map's density where a cap of 1 thins it to about one frame's
+ * worth of points.  The map window is built in frame order and each frame's points in input order, so a voxel of the
+ * map keeps the points of its oldest window frames.  Cost of a cap above 1: the filter's radix sort and one more launch
+ * (see dcreg_voxel_downsample_n), once per call for the frames and once per step for the maps; the sort's scratch is
+ * sized once per call for the largest step, so a step keeps its one host sync and the chunk graphs are captured once.
+ * A cap below 1 is DCREG_BAD_ARG before anything is launched, whatever the voxel sizes. */
+int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                                   int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                                   double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                                   int source_max_points, int map_max_points, const double* T_init,
+                                   const double* deltas, int64_t* frame_points, double* T_prior, double* T_out,
+                                   int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
+                                   int log_cap);
 /* Voxel downsampling of many clouds in one call (KISS-ICP's VoxelDownsample rule: the first point of every voxel).
  * xyz / offsets / stride: HOST memory as in dcreg_icp_run_scans (n_clouds + 1 offsets, ascending strictly from 0, at
  * most 2^29 - 1 points).  With inv = 1.0 / voxel in FP64, point i's voxel is (floor((double)x inv), floor((double)y inv),
@@ -361,6 +377,17 @@ int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params,
  * as they were. */
 int dcreg_voxel_downsample(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,
                            double voxel, float* out_xyz, int64_t* out_offsets, int64_t* out_index);
+/* dcreg_voxel_downsample keeping up to max_points points per voxel (KISS-ICP's VoxelHashMap::AddPoints rule with
+ * max_points_per_voxel, points inserted in index order): within each cloud, each voxel keeps its max_points points of
+ * smallest index; voxels, dropped points, bit-for-bit copies, input order, out_index and errors as in
+ * dcreg_voxel_downsample, which is this call with max_points = 1 (same launches, same bytes).
+ * dcreg_b200.api.voxel_downsample(P, voxel, max_points) gives the same selection.  max_points < 1 is DCREG_BAD_ARG before
+ * anything is launched.
+ * Cost: max_points = 1 takes the cheaper path of one atomicMin per point.  max_points > 1 replaces it by a stable radix
+ * sort of the points by their voxel's table slot (32-bit keys, as many radix passes as the slot count has bits) and one
+ * O(1) pass per point whatever a voxel's occupancy: seven launches besides the sort's, whatever n_clouds. */
+int dcreg_voxel_downsample_n(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,
+                             double voxel, int max_points, float* out_xyz, int64_t* out_offsets, int64_t* out_index);
 /* Same loop, but correspondences are supplied by the caller each iteration through a callback
  * (host kd-tree mode, "PR1"): planes are 4*n doubles (nx,ny,nz,d), all-zero = none. */
 typedef int (*dcreg_plane_callback)(void* user, const double T[16], double* planes4,
