@@ -750,9 +750,12 @@ __global__ void k2_analyze_kernel(const double* v27, dcreg_icp_params prm, dcreg
     k2::analyze_and_solve<true>(v27, prm, out, dx);
 }
 
-// Post-run log fill: one thread per iteration record recomputes the FULL analysis from the record's H27
-// (same code, same inputs => identical mask / P / PCG counts as the in-loop critical path wrote) and thereby adds the
-// log-only quantities without putting them on the loop's critical path.
+// Post-run log fill: one thread per iteration record recomputes the FULL analysis from the record's H27 with the seam's
+// code and thereby adds the log-only quantities without putting them on the loop's critical path.  The baseline
+// methods' step (k2::icp_step) runs that same code on the same inputs, so its record is rewritten with identical
+// values.  The "Ours" step (k2::icp_step_warp_ours) has its own arithmetic: the decisions it wrote (mask, is_degenerate,
+// schur_singular, PCG iterations and residual) are kept, so the record describes the step that moved the pose even
+// where a decision sits within rounding of its threshold and the seam's code would have gone the other way.
 __global__ void log_fill_kernel(dcreg_iter_log* logs, int log_cap, const IcpState* states, dcreg_icp_params prm) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const IcpState* st = states + blockIdx.y;
@@ -760,8 +763,19 @@ __global__ void log_fill_kernel(dcreg_iter_log* logs, int log_cap, const IcpStat
     const int n = st->iter < log_cap ? st->iter : log_cap;
     if (i >= n) return;
     if (log[i].status != DCREG_OK) return;
+    dcreg_analysis* a = &log[i].analysis;
+    const bool ours = prm.detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm.handling == DCREG_HAND_PRECONDITIONED_CG;
+    int mask[6];
+    for (int k = 0; k < 6; ++k) mask[k] = a->degenerate_mask[k];
+    const int is_deg = a->is_degenerate, singular = a->schur_singular, pcg_it = a->pcg_iterations;
+    const double pcg_res = a->pcg_residual;
     double dx[6];
-    k2::analyze_and_solve<true>(log[i].H27, prm, &log[i].analysis, dx);
+    k2::analyze_and_solve<true>(log[i].H27, prm, a, dx);
+    if (ours) {
+        for (int k = 0; k < 6; ++k) a->degenerate_mask[k] = mask[k];
+        a->is_degenerate = is_deg; a->schur_singular = singular;
+        a->pcg_iterations = pcg_it; a->pcg_residual = pcg_res;
+    }
 }
 
 __global__ void pcg_kernel(const double* A, const double* b, const double* P, int max_it, double tol, double* x,

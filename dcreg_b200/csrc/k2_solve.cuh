@@ -474,9 +474,12 @@ __device__ inline void icp_step(const double* acc, IcpState* st, const dcreg_icp
 // critical path of the loop.  Why: executed by a single thread the step is ~7 k dependent FP64 instructions, each
 // waiting for the previous one, and the straight-line code is fetched cold on every launch.  Here the 32 lanes share the work: the two 3x3 inverses and
 // the two 3x3 Jacobi EVDs run on lanes 0/1 side by side, Schur products and the preconditioner are one entry per
-// lane, and the PCG mat-vecs are row-per-lane with shuffle broadcasts and butterfly dot products.  The in-loop record
-// gets the non-analysis fields; the analysis block is (re)computed for every record by log_fill_kernel after the run
-// with the same single-thread code the host seam uses, so mask / P / PCG counts in the log stay oracle-identical.
+// lane, and the PCG mat-vecs are row-per-lane with shuffle broadcasts and butterfly dot products.  Its arithmetic is
+// not the seam's (MUFU-seeded reciprocals, warm Jacobi, L D L^T pivots, FMAs, the squared stop rule), so a decision
+// whose margin is within rounding can go the other way here.  The in-loop record therefore gets, besides the
+// non-analysis fields, the decisions of the step that moved the pose: is_degenerate, degenerate_mask, schur_singular,
+// pcg_iterations and pcg_residual.  log_fill_kernel keeps those and fills the rest of the analysis block (eigenvalues,
+// eigenvectors, P, conditions) from the record's H27 with the host seam's single-thread code.
 // ------------------------------------------------------------------------------------------------------------------
 struct WarpSmem {
     double H[36], g[6];
@@ -505,8 +508,10 @@ __device__ __forceinline__ double row_dot_bcast(const double (&row)[6], double v
     return s;
 }
 
-// PCG on H x = g (paper Alg. 3): lanes 0..5 own rows/components, lanes 0..7 execute.  Returns iterations used.
-__device__ __forceinline__ int pcg6_warp(const WarpSmem& sm, int lane, int max_iter, double tol, double& x_out) {
+// PCG on H x = g (paper Alg. 3): lanes 0..5 own rows/components, lanes 0..7 execute.  Returns iterations used;
+// rn2_out = ||r||^2 at exit.
+__device__ __forceinline__ int pcg6_warp(const WarpSmem& sm, int lane, int max_iter, double tol, double& x_out,
+                                         double& rn2_out) {
     double Hrow[6], Prow[6];
 #pragma unroll
     for (int j = 0; j < 6; ++j) { Hrow[j] = lane < 6 ? sm.H[lane * 6 + j] : 0.0; Prow[j] = lane < 6 ? sm.P[lane * 6 + j] : 0.0; }
@@ -515,13 +520,16 @@ __device__ __forceinline__ int pcg6_warp(const WarpSmem& sm, int lane, int max_i
     double p = z;
     double rz = warp_sum(r * z);
     int it;
-    const double tol2 = tol * tol;                           // ||r|| < tol  <=>  ||r||^2 < tol^2: no square root on the chain
+    // ||r|| < tol  <=>  ||r||^2 < tol^2: no square root on the chain.  Exact only while tol^2 is a normal number: below
+    // tol ~1.5e-154 the square rounds (to 0 under ~1e-162) and the two rules part; the documented tolerances are far above.
+    const double tol2 = tol * tol;
+    double rn2 = max_iter < 1 ? warp_sum(r * r) : 0.0;
     for (it = 1; it <= max_iter; ++it) {
         const double Hp = row_dot_bcast(Hrow, p);
         const double alpha = k2f::fast_div(rz, warp_sum(p * Hp));
         x = fma(alpha, p, x);
         r = fma(-alpha, Hp, r);
-        const double rn2 = warp_sum(r * r);
+        rn2 = warp_sum(r * r);
         if (rn2 < tol2) break;                               // identical in every lane: uniform branch
         z = row_dot_bcast(Prow, r);
         const double rz_new = warp_sum(r * z);
@@ -529,6 +537,7 @@ __device__ __forceinline__ int pcg6_warp(const WarpSmem& sm, int lane, int max_i
         rz = rz_new;
     }
     x_out = x;
+    rn2_out = rn2;
     return it > max_iter ? max_iter : it;
 }
 
@@ -599,6 +608,7 @@ __device__ inline void icp_step_warp_ours(const double* acc, IcpState* st, const
     K2_STAMP(1);
     const bool schur_ok = sm.ok[0] && sm.ok[1];
     int degenerate = 0;
+    bool deg = false;                                        // lanes 0..5: this eigenvalue's flag of the mask
     if (schur_ok) {
         // ---- Schur complements (icp_test_runner.cpp:2443-2447, paper Eq. 18): one entry per lane ----
         double sval = 0.0;
@@ -640,7 +650,6 @@ __device__ inline void icp_step_warp_ours(const double* acc, IcpState* st, const
         __syncwarp();
         K2_STAMP(2);
         // ---- detection (Eq. 20-21) and preconditioner (Eq. 43-46) ----
-        bool deg = false;
         if (lane < 6) {
             const double* l = sm.lam[lane / 3];
             deg = l[2] / fmax(l[lane % 3], 1e-12) > prm.cond_thresh;
@@ -667,10 +676,12 @@ __device__ inline void icp_step_warp_ours(const double* acc, IcpState* st, const
     }
     K2_STAMP(3);
     // ---- solve ----
+    int pcg_it = 0;
+    double pcg_rn2 = 0.0;
     if (degenerate) {
         if (lane < 8) {
             double xi;
-            pcg6_warp(sm, lane, prm.pcg_max_iter, prm.pcg_tol, xi);
+            pcg_it = pcg6_warp(sm, lane, prm.pcg_max_iter, prm.pcg_tol, xi, pcg_rn2);
             if (lane < 6) sm.dx[lane] = xi;
         }
     } else if (lane == 0) {
@@ -678,6 +689,14 @@ __device__ inline void icp_step_warp_ours(const double* acc, IcpState* st, const
     }
     __syncwarp();
     K2_STAMP(4);
+    if (rec) {                                               // the decisions this step took (log_fill_kernel keeps them)
+        dcreg_analysis* an = &rec->analysis;
+        if (lane < 6) an->degenerate_mask[lane] = deg ? 1 : 0;
+        if (lane == 0) {
+            an->is_degenerate = degenerate; an->schur_singular = schur_ok ? 0 : 1;
+            an->pcg_iterations = pcg_it; an->pcg_residual = degenerate ? sqrt(pcg_rn2) : 0.0;
+        }
+    }
     const double dxi = lane < 6 ? sm.dx[lane] : 0.0;
     const bool finite = __ballot_sync(0xffffffffu, !isfinite(dxi)) == 0u;
     if (rec) {                                               // log only: off the pose's dependent chain

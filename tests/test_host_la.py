@@ -36,6 +36,42 @@ def test_fast_solve_step_pieces_on_the_host(tmp_path):
     assert "K2_FAST_OK" in res.stdout
 
 
+@pytest.mark.gpu
+def test_fast_solve_step_pieces_on_the_device(tmp_path):
+    """The same k2_fast.cuh checks built for sm_90a with the library's flags and run in a kernel, so the MUFU-seeded
+    reciprocals are the ones the solve step uses; plus fast_rcp / fast_div against __drcp_rn / __ddiv_rn over
+    [1e-300, 1e300] and fast_rsqrt against mpmath on a sample: at most the documented 2 ulp."""
+    import mpmath
+    import numpy as np
+    from dcreg_b200.build import NVCC_FLAGS, _nvcc
+    flags, skip = [], False                                # the library's flags without the shared-library and
+    for f in NVCC_FLAGS:                                   # ptxas-report options, each dropped with its argument
+        if skip:
+            skip = False
+        elif f in ("-Xcompiler", "-Xptxas"):
+            skip = True
+        elif f != "--shared":
+            flags.append(f)
+    assert "arch=compute_90a,code=sm_90a" in flags and "--fmad=true" in flags
+    exe = tmp_path / "test_k2_fast_dev"
+    subprocess.run([_nvcc()] + flags + ["-DK2F_DEVICE_TEST", "-o", str(exe), os.path.join(ROOT, "tools", "test_k2_fast.cu")],
+                   check=True, capture_output=True, text=True)
+    out = tmp_path / "rsqrt.bin"
+    res = subprocess.run([str(exe), str(out)], capture_output=True, text=True)
+    print(res.stdout)
+    assert res.returncode == 0, res.stdout + res.stderr
+    assert "K2_FAST_OK" in res.stdout
+    xy = np.fromfile(out, dtype=np.float64).reshape(-1, 2)
+    assert len(xy) > 20_000 and xy[:, 0].min() <= 1e-300 and xy[:, 0].max() >= 1e300
+    worst = 0
+    with mpmath.workdps(40):
+        for x, y in xy:
+            ref = float(1 / mpmath.sqrt(mpmath.mpf(x)))
+            worst = max(worst, abs(int(np.float64(y).view(np.int64)) - int(np.float64(ref).view(np.int64))))
+    print(f"fast_rsqrt: max {worst} ulp from the correctly rounded 1/sqrt(x) on {len(xy)} points")
+    assert worst <= 2
+
+
 def test_loop_tile_plan(tmp_path):
     """loop_plan.hpp (how a run's source slots are cut into blocks of the iteration kernel) as plain host C++: coverage,
     tile bounds, resident-block cap, the small-cloud rule and the values used for the shipped cloud / C2 / C4 / C5."""
