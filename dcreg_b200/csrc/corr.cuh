@@ -331,13 +331,11 @@ __device__ __forceinline__ void knn_search(const Grid& g, float qx, float qy, fl
         const float eps = 2e-6f * (fabsf(qx) + fabsf(qy) + fabsf(qz) + cell);
         const float fx = qx - (float)cx * cell, fy = qy - (float)cy * cell, fz = qz - (float)cz * cell;
         if (K == 1) {
-            // cell = search radius (the usual set-up): 9 rows of 3 cells.  Same rows, same pruning tests and the same
-            // own / left / right order as the general loop below, but a row's FOUR cell boundaries are fetched together
-            // (one memory round trip per visited row instead of up to six dependent ones: the lanes of a warp prune
-            // differently, so a warp walks nearly all 27 cells and every dependent load is on its critical path).
-            const float gl = fmaxf(fx - eps, 0.0f), gr = fmaxf((cell - fx) - eps, 0.0f);
-            const float gl2 = gl * gl * 0.99999f, gr2 = gr * gr * 0.99999f;
-            const int xa = min(max(lx - 1, 0), g.nx), xb = min(max(lx, 0), g.nx), xc = min(max(lx + 1, 0), g.nx), xd = min(max(lx + 2, 0), g.nx);
+            // cell = search radius (the usual set-up): 9 rows of 3 cells, own row first, rows pruned by the same test
+            // as the general loop below; a visited row costs one fetch of its two outer cell boundaries and one scan
+            // (the lanes of a warp prune differently, so a warp walks nearly all 27 cells and every dependent load is
+            // on its critical path).
+            const int xa = min(max(lx - 1, 0), g.nx), xd = min(max(lx + 2, 0), g.nx);
 #pragma unroll 1
             for (int r = 0; r < 9; ++r) {
                 // own row first, then the ring: (dz, dy) = (-1,-1) (-1,0) (-1,1) (0,-1) (0,1) (1,-1) (1,0) (1,1)
@@ -350,10 +348,12 @@ __device__ __forceinline__ void knn_search(const Grid& g, float qx, float qy, fl
                 const float row_lb = (gy * gy + gz * gz) * 0.99999f;
                 if (row_lb > knn_d2(k, 4)) continue;
                 const int* rowp = g.cell_start + (size_t)(zz * g.ny + yy) * g.nx;
-                const int b0 = __ldg(rowp + xa), b1 = __ldg(rowp + xb), b2 = __ldg(rowp + xc), b3 = __ldg(rowp + xd);
-                knn_scan_range(g.pts, b1, b2, qx, qy, qz, k);
-                if (row_lb + gl2 <= knn_d2(k, 4)) knn_scan_range(g.pts, b0, b1, qx, qy, qz, k);
-                if (row_lb + gr2 <= knn_d2(k, 4)) knn_scan_range(g.pts, b2, b3, qx, qy, qz, k);
+                // A row's three cells are one contiguous range: scanned in one pass, four loads in flight across the
+                // cell boundaries (~3 points per cell on a surface at cell = radius, so three separate passes spent
+                // most of their time in single-candidate trips, one memory round trip each).  The left / right cells
+                // are no longer pruned: their box-distance test only ever skips cells holding nothing below the
+                // current 5th key, so scanning them too leaves the list unchanged, bit for bit.
+                knn_scan_range(g.pts, __ldg(rowp + xa), __ldg(rowp + xd), qx, qy, qz, k);
             }
             return;
         }
