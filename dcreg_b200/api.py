@@ -89,7 +89,7 @@ EXPORTS = [
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_odometry_open", "dcreg_odometry_push", "dcreg_odometry_close", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -147,6 +147,12 @@ def load_library():
                                                    C.POINTER(ci), dp, C.POINTER(IterLog), ci]
     lib.dcreg_voxel_downsample_n.argtypes = [vp, ci, C.POINTER(C.c_float), C.POINTER(i64), ci, C.c_double, ci,
                                              C.POINTER(C.c_float), C.POINTER(i64), C.POINTER(i64)]
+    lib.dcreg_odometry_open.argtypes = [vp, C.POINTER(IcpParams), ci, C.c_double, ci, ci, C.c_double, C.c_double, ci, ci,
+                                        dp]
+    lib.dcreg_odometry_push.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(C.c_float), C.POINTER(i64), ci, dp,
+                                        C.POINTER(i64), dp, dp, C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp,
+                                        C.POINTER(IterLog), ci]
+    lib.dcreg_odometry_close.argtypes = [vp]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -666,6 +672,27 @@ class Context:
             r.n_points = int(c)
         return out
 
+    def odometry_session(self, params: IcpParams, n_seqs: int, T_init, motion: str = "increments", map_frames: int = 10,
+                         cell_size=None, source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
+                         map_max_points: int = 1):
+        """Open the context's odometry session (dcreg_odometry_open): icp_run_odometry's settings for n_seqs sequences
+        whose frames come in pushes (OdometrySession.push).  T_init (n_seqs, 4, 4): the pose of each sequence's first
+        frame.  Pushing a recording in any chunks gives byte for byte what one icp_run_odometry call over it gives.
+        One session per context; use it as a context manager, or close() it."""
+        models = {"increments": 0, "constant_velocity": 1}
+        if motion not in models:
+            raise ValueError(f"odometry_session: motion must be one of {sorted(models)}, not {motion!r}")
+        source_max_points = _max_points(source_max_points, "source_max_points")
+        map_max_points = _max_points(map_max_points, "map_max_points")
+        T0 = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
+        if T0.shape[0] != n_seqs:
+            raise ValueError(f"odometry_session: {n_seqs} sequences but {T0.shape[0]} initial poses")
+        cell = float(params.search_radius if cell_size is None else cell_size)
+        self._check(self.lib.dcreg_odometry_open(self._h, C.byref(params), int(n_seqs), cell, int(map_frames),
+                                                 models[motion], float(source_voxel), float(map_voxel), source_max_points,
+                                                 map_max_points, _dptr(T0)))
+        return OdometrySession(self, params, int(n_seqs))
+
     def icp_run_pairs(self, params: IcpParams, sources, targets, T_init, cell_size=None, want_log: bool = False,
                       want_cov: bool = False, metrics_threshold=None):
         """Pairs of clouds, each source (a list of (N_b, >=3) arrays) against its own target (a list of (M_b, >=3) arrays),
@@ -755,3 +782,54 @@ class Context:
 
     def set_global_source_count(self, n_total: int):
         self._check(self.lib.dcreg_set_global_source_count(self._h, int(n_total)))
+
+
+class OdometrySession:
+    """The context's odometry session (Context.odometry_session): frames pushed as they arrive, each sequence's local-map
+    window and motion-model state kept on the device from one push to the next."""
+
+    def __init__(self, ctx: Context, params: IcpParams, n_seqs: int):
+        self.ctx, self.params, self.n_seqs = ctx, params, n_seqs
+        self.open = True
+
+    def push(self, frames_per_seq, deltas=None, want_log: bool = False, want_cov: bool = False):
+        """The next frames of every sequence (dcreg_odometry_push): frames_per_seq, a list of n_seqs lists, possibly
+        empty, of (N, >=3) point arrays.  deltas: (frames, 4, 4) increments over the pushed frames in order (entry k maps
+        frame k's result to the next frame's prior in its sequence, which may come in a later push), or None for
+        identity.  Returns one list of IcpResult per sequence, as icp_run_odometry gives them (.T_prior, .n_points; logs
+        only when want_log, .cov when want_cov).  A push that fails raises DcregError and leaves the session as it was."""
+        ctx, lib = self.ctx, self.ctx.lib
+        if len(frames_per_seq) != self.n_seqs:
+            raise ValueError(f"odometry push: {self.n_seqs} sequences but {len(frames_per_seq)} frame lists")
+        seq_off, xyz, off = _pack_sequences(frames_per_seq)
+        n = int(seq_off[-1])
+        D = None
+        if deltas is not None:
+            D = np.ascontiguousarray(deltas, dtype=np.float64).reshape(-1, 4, 4)
+            if D.shape[0] != n:
+                raise ValueError(f"odometry push: {n} frames but {D.shape[0]} increments")
+        m = max(n, 1)
+        T_prior = np.empty((m, 4, 4)); T_out = np.empty((m, 4, 4))
+        npts = np.zeros(m, dtype=np.int64)
+        n_it = (C.c_int * m)(); conv = (C.c_int * m)(); st = (C.c_int * m)()
+        cov = np.empty((m, 6, 6)) if want_cov else None
+        cap = int(self.params.max_iterations) if want_log else 0
+        logs = (IterLog * max(cap * n, 1))() if want_log else None
+        ctx._check(lib.dcreg_odometry_push(ctx._h, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n, _fptr(xyz), _iptr(off),
+                                           3, _optr(D), _iptr(npts), _dptr(T_prior), _dptr(T_out), n_it, conv, st,
+                                           _optr(cov), logs, cap))
+        res = _trial_results(st[:n], conv[:n], n_it[:n], T_out, logs, cap, cov)
+        for r, Tp, c in zip(res, T_prior, npts):
+            r.T_prior, r.n_points = Tp, int(c)
+        return [res[a:b] for a, b in zip(seq_off[:-1], seq_off[1:])]
+
+    def close(self):
+        if self.open and self.ctx._h:
+            self.ctx._check(self.ctx.lib.dcreg_odometry_close(self.ctx._h))
+        self.open = False
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()

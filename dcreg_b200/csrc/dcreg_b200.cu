@@ -23,6 +23,7 @@
 
 #include <algorithm>
 #include <cstddef>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -1028,6 +1029,95 @@ __global__ void voxel_scatter_kernel(const float* __restrict__ in, long long n, 
     if (index) index[p] = i - seg[corr::segment_of(seg, n_seg, i)];
 }
 
+// ---- odometry sessions (dcreg_odometry_push; odom_plan::make_push) ---------------------------------------------------
+// Frame reference r of a push: r < n_frames is a pushed frame (device index d = r: points in the push's packed frames,
+// pose in states[d]); otherwise retained frame r - n_frames of the session (points in the window buffer, pose the
+// row-major 4x4 T_out the call that registered it returned, hist_T[16 (r - n_frames) ..], whose R and t are the bytes
+// of that frame's final loop state).
+__device__ __forceinline__ void ref_pose(int r, int n_frames, const IcpState* __restrict__ states,
+                                         const double* __restrict__ hist_T, double* R, double* t) {
+    if (r < n_frames) {
+        const IcpState* st = states + r;
+#pragma unroll
+        for (int i = 0; i < 9; ++i) R[i] = st->R[i];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) t[i] = st->t[i];
+    } else {
+        const double* T = hist_T + (size_t)(r - n_frames) * 16;
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+#pragma unroll
+            for (int b = 0; b < 3; ++b) R[3 * a + b] = T[4 * a + b];
+            t[a] = T[4 * a + 3];
+        }
+    }
+}
+
+// map_points_kernel for a push: piece p's points come from the push's packed frames (src) or from the window buffer
+// (win) by its frame reference frame[p], and so does its pose.  The same arithmetic and the same .w.
+__global__ void map_points_hist_kernel(const float4* __restrict__ src, const float4* __restrict__ win, int n_frames,
+                                       const long long* __restrict__ dst, int pieces, const long long* __restrict__ src_at,
+                                       const int* __restrict__ frame, long long m, const IcpState* __restrict__ states,
+                                       const double* __restrict__ hist_T, float4* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const int p = corr::segment_of(dst, pieces, i);
+    const int r = frame[p];
+    double R[9], t[3];
+    ref_pose(r, n_frames, states, hist_T, R, t);
+    const float4 q = (r < n_frames ? src : win)[src_at[p] + (i - dst[p])];
+    const double x = q.x, y = q.y, z = q.z;
+    float v[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+        v[c] = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(R[3 * c], x), __dmul_rn(R[3 * c + 1], y)),
+                                          __dmul_rn(R[3 * c + 2], z)),
+                                t[c]);
+    out[i] = make_float4(v[0], v[1], v[2], __int_as_float((int)i));
+}
+
+// odom_start_kernel for a push: prev / prev2 are frame references, and delta holds one entry per reference (pushed
+// frames, then retained frames), or is null
+__global__ void odom_start_hist_kernel(IcpState* states, const long long* __restrict__ seg, double* T_prior, int* cursor,
+                                       int* first, unsigned int* n_active, int lanes, int step_first, int active,
+                                       const int* __restrict__ prev, const int* __restrict__ prev2,
+                                       const double* __restrict__ delta, int motion, int n_frames,
+                                       const double* __restrict__ hist_T) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j == 0) { *n_active = (unsigned)active; first[lanes] = step_first + active; }
+    if (j >= lanes) return;
+    const int f = step_first + min(j, active);
+    first[j] = f; cursor[j] = f;
+    if (j >= active) return;
+    double Ra[9], ta[3];
+    ref_pose(prev[j], n_frames, states, hist_T, Ra, ta);
+    double D[16] = {1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0};
+    if (motion == DCREG_MOTION_CONSTANT_VELOCITY) {
+        if (prev2[j] >= 0) {
+            double Rb[9], tb[3];
+            ref_pose(prev2[j], n_frames, states, hist_T, Rb, tb);
+            constant_velocity_increment(Rb, tb, Ra, ta, D);
+        }
+    } else if (delta) {
+        for (int i = 0; i < 16; ++i) D[i] = delta[(size_t)prev[j] * 16 + i];
+    }
+    double T[16];
+    compose_prior(Ra, ta, D, T);
+    for (int i = 0; i < 16; ++i) T_prior[(size_t)f * 16 + i] = T[i];
+    init_loop_state(states + f, T, seg[f + 1] - seg[f]);
+}
+
+// The session's window after a push: m points in `pieces` retained frames, piece p being out[dst[p], dst[p+1]) = the
+// packed points (src_at[p] ..) of the push (ref[p] < n_frames) or of the old window.  One launch for every sequence.
+__global__ void retain_points_kernel(const float4* __restrict__ src, const float4* __restrict__ win, int n_frames,
+                                     const long long* __restrict__ dst, int pieces, const long long* __restrict__ src_at,
+                                     const int* __restrict__ ref, long long m, float4* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const int p = corr::segment_of(dst, pieces, i);
+    out[i] = (ref[p] < n_frames ? src : win)[src_at[p] + (i - dst[p])];
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1166,6 +1256,22 @@ struct dcreg_ctx {
     // their grids in an arena of their own
     DevBuf<long long> d_odom_ll; DevBuf<int> d_odom_int;
     DevBuf<float4> d_odom_map, d_odom_map_vox;                         // ... and the maps after the voxel filter
+    // the odometry session (dcreg_odometry_open .. _close), if one is open: the settings of its pushes, and what every
+    // sequence carries from one push to the next (odom_plan::History): the retained frames' kept points, packed and in
+    // input order as d_scan_src holds them, in win[cur] (the other buffer receives the next push's window), their poses
+    // (the T_out the host returned) and the last increment of every sequence
+    struct OdomSession {
+        dcreg_icp_params params{};
+        int n_seqs = 0, map_frames = 1, motion = 0, source_max_points = 1, map_max_points = 1;
+        double cell_size = 0.0, source_voxel = 0.0, map_voxel = 0.0;
+        std::vector<double> T_init;                                    // [n_seqs][16]
+        odom_plan::History hist;
+        std::vector<double> hist_T;                                    // [retained][16]
+        std::vector<double> last_delta;                                // [n_seqs][16]
+        DevBuf<float4> win[2]; int cur = 0;
+        DevBuf<double> d_hist_T;                                       // hist_T on the device
+    };
+    std::unique_ptr<OdomSession> odom;
     // the voxel filter (voxel_filter): table [slots] keys / first indices, [points] slots, [points + 1] flags and their
     // scan, [clouds + 1] table offsets, input and kept offsets, [clouds] range flags, [points][3] kept xyz and indices
     DevBuf<unsigned long long> d_vox_keys; DevBuf<int> d_vox_first;
@@ -2728,6 +2834,7 @@ struct BatchCheck {
     const char* dense = nullptr;        // the context's dense grid is needed by these ("batches")
     int n_seqs = 0;                     // the sequence table [n_seqs + 1]: from 0, ascending strictly, up to n
     const int* seq_offsets = nullptr;
+    bool empty_seqs = false;            // ... or only non-decreasing (dcreg_odometry_push: a sequence may have no frame)
 };
 
 static int check_batch_call(dcreg_ctx* ctx, const dcreg_icp_params* params, const BatchCheck& c) {
@@ -2759,8 +2866,10 @@ static int check_batch_call(dcreg_ctx* ctx, const dcreg_icp_params* params, cons
         const int* so = c.seq_offsets;
         if (so[0] != 0) return bad(name + ": seq_offsets must start at 0");
         for (int s = 0; s < c.n_seqs; ++s)
-            if (so[s + 1] <= so[s])
-                return bad(name + ": sequence " + std::to_string(s) + " is empty (seq_offsets must ascend strictly)");
+            if (c.empty_seqs ? so[s + 1] < so[s] : so[s + 1] <= so[s])
+                return bad(name + ": sequence " + std::to_string(s) +
+                           (c.empty_seqs ? " has a negative frame count (seq_offsets must not decrease)"
+                                         : " is empty (seq_offsets must ascend strictly)"));
         if (so[c.n_seqs] != c.n)
             return bad(name + ": seq_offsets[n_seqs] = " + std::to_string(so[c.n_seqs]) + " but n_frames = " + std::to_string(c.n));
     }
@@ -2840,30 +2949,74 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
 // dcreg_icp_run_odometry (source_voxel = map_voxel = 0, `name` "icp_run_odometry"), dcreg_icp_run_odometry_voxel (caps
 // of 1) and dcreg_icp_run_odometry_voxel_n: one body.  A voxel size of 0 leaves its filter out entirely: no launch, no
 // copy, no sync.
+// What is wrong with the settings of an odometry call or session, or null
+static const char* odometry_settings_error(int map_frames, int motion, bool deltas, double source_voxel, double map_voxel,
+                                           int source_max_points, int map_max_points) {
+    if (map_frames < 1) return "map_frames must be >= 1";
+    if (motion != DCREG_MOTION_INCREMENTS && motion != DCREG_MOTION_CONSTANT_VELOCITY)
+        return "motion must be DCREG_MOTION_INCREMENTS or DCREG_MOTION_CONSTANT_VELOCITY";
+    if (motion == DCREG_MOTION_CONSTANT_VELOCITY && deltas) return "the constant-velocity model takes no deltas (pass NULL)";
+    if (!(source_voxel >= 0.0 && source_voxel < INFINITY) || !(map_voxel >= 0.0 && map_voxel < INFINITY))
+        return "source_voxel and map_voxel must be finite and >= 0 (0: no filter)";
+    if (source_max_points < 1 || map_max_points < 1) return "source_max_points and map_max_points must be >= 1";
+    return nullptr;
+}
+
+// A push that succeeded becomes the session's state: the history after it, the retained frames' poses (the T_out bytes
+// just returned for this push's frames), every sequence's last increment (deltas' entry of its last pushed frame, or
+// the identity without deltas; a sequence with no frame keeps its own), and the window the retain step gathered.
+static void commit_push(dcreg_ctx::OdomSession& ss, const odom_plan::Push& u, int n_frames, const int* seq_offsets,
+                        const double* T_out, const double* deltas) {
+    std::vector<double> T((size_t)u.next_ref.size() * 16);
+    for (size_t e = 0; e < u.next_ref.size(); ++e) {
+        const int r = u.next_ref[e];
+        const double* from = r < n_frames ? T_out + (size_t)u.plan.input[(size_t)r] * 16 : &ss.hist_T[(size_t)(r - n_frames) * 16];
+        memcpy(&T[e * 16], from, 16 * sizeof(double));
+    }
+    static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    for (int s = 0; s < ss.n_seqs; ++s)
+        if (seq_offsets[s + 1] > seq_offsets[s])
+            memcpy(&ss.last_delta[(size_t)s * 16], deltas ? deltas + (size_t)(seq_offsets[s + 1] - 1) * 16 : kIdentity,
+                   16 * sizeof(double));
+    ss.hist_T.swap(T);
+    ss.hist = u.next;
+    ss.cur = 1 - ss.cur;
+}
+
+// sess (dcreg_odometry_push): the frames continue the session's sequences, whose retained frames (odom_plan::History)
+// act as anchors outside the call: they are not registered and return nothing, their points come from the window
+// buffer and their poses from the session, and their last increments continue the deltas.  A sequence may have no
+// frame.  The frames are named by their number in the sequence since the session opened.  Only a push that succeeds
+// changes the session (commit_push); null: a one-shot call, which launches and copies exactly as without sessions.
 static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params* params, int n_seqs,
                         const int* seq_offsets, int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
                         double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
                         int source_max_points, int map_max_points, const double* T_init, const double* deltas,
                         int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
-                        int* status, double* cov, dcreg_iter_log* log, int log_cap) {
+                        int* status, double* cov, dcreg_iter_log* log, int log_cap,
+                        dcreg_ctx::OdomSession* sess = nullptr) {
     if (!ctx) return DCREG_BAD_ARG;
     BatchCheck c{name, params && n_seqs > 0 && n_frames > 0 && seq_offsets && xyz && frame_offsets && T_init && T_out,
                  "null pointer, n_seqs <= 0 or n_frames <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_frames};
     c.offsets = frame_offsets; c.item = "frame"; c.stride = stride; c.own_cell = true; c.cell_size = cell_size;
     c.need_target = false; c.one_iteration = true; c.n_seqs = n_seqs; c.seq_offsets = seq_offsets;
-    if (map_frames < 1) c.own_msg = "map_frames must be >= 1";
-    else if (motion != DCREG_MOTION_INCREMENTS && motion != DCREG_MOTION_CONSTANT_VELOCITY)
-        c.own_msg = "motion must be DCREG_MOTION_INCREMENTS or DCREG_MOTION_CONSTANT_VELOCITY";
-    else if (motion == DCREG_MOTION_CONSTANT_VELOCITY && deltas)
-        c.own_msg = "the constant-velocity model takes no deltas (pass NULL)";
-    else if (!(source_voxel >= 0.0 && source_voxel < INFINITY) || !(map_voxel >= 0.0 && map_voxel < INFINITY))
-        c.own_msg = "source_voxel and map_voxel must be finite and >= 0 (0: no filter)";
-    else if (source_max_points < 1 || map_max_points < 1)
-        c.own_msg = "source_max_points and map_max_points must be >= 1";
+    c.empty_seqs = sess != nullptr;
+    c.own_msg = odometry_settings_error(map_frames, motion, deltas != nullptr, source_voxel, map_voxel, source_max_points,
+                                        map_max_points);
     int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
+    // "sequence s, frame k (frame j of the sequence)": the caller's frame k, j-th of sequence s in the call, or its
+    // number since the session opened
+    auto frame_name = [&](int s, int k) {
+        const int j = k - seq_offsets[s];
+        if (!sess)
+            return "sequence " + std::to_string(s) + ", frame " + std::to_string(k) + " (frame " + std::to_string(j) +
+                   " of the sequence)";
+        return "sequence " + std::to_string(s) + ", frame " + std::to_string(k) + " of the push (frame " +
+               std::to_string(sess->hist.seen[(size_t)s] + j) + " of the sequence since open)";
+    };
     // the frames' voxel filter: once per call, on the staged points in input order, before the pack and the sort; one
     // sync for the kept counts.  From here on a frame is its kept points, on the device
     const float* src_xyz = xyz;
@@ -2882,8 +3035,7 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
                                   : kept[(size_t)k + 1] == kept[(size_t)k] ? "no point is left by the source filter (no finite point)"
                                                                            : nullptr;
                 if (why) {
-                    ctx->err = std::string(name) + ": sequence " + std::to_string(s) + ", frame " + std::to_string(k) +
-                               " (frame " + std::to_string(k - seq_offsets[s]) + " of the sequence): " + why;
+                    ctx->err = std::string(name) + ": " + frame_name(s, k) + ": " + why;
                     return DCREG_BAD_ARG;
                 }
             }
@@ -2891,13 +3043,17 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
     }
     if (frame_points)
         for (int k = 0; k < n_frames; ++k) frame_points[k] = src_off[k + 1] - src_off[k];
-    odom_plan::Plan P;
+    odom_plan::Push U;
+    odom_plan::Plan& P = U.plan;
     {
-        const std::string why = odom_plan::make(n_seqs, seq_offsets, n_frames, src_off, map_frames,
-                                                arena_plan::kMaxPoints, &P);
+        const std::string why = sess ? odom_plan::make_push(n_seqs, seq_offsets, n_frames, src_off, map_frames,
+                                                            arena_plan::kMaxPoints, sess->hist, &U)
+                                     : odom_plan::make(n_seqs, seq_offsets, n_frames, src_off, map_frames,
+                                                       arena_plan::kMaxPoints, &P);
         if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
     }
     const int n_steps = (int)P.steps.size();
+    const int n_hist = sess ? (int)sess->hist.n.size() : 0;
     // every step's tables in one upload: long long map_seg [A + 1], piece_dst [P + 1], piece_src [P]; int piece_frame
     // [P], prev [A], prev2 [A] (A lanes, P window frames)
     std::vector<long long> hll;
@@ -2912,6 +3068,14 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         hint.insert(hint.end(), st.piece_frame.begin(), st.piece_frame.end());
         hint.insert(hint.end(), st.prev.begin(), st.prev.end());
         hint.insert(hint.end(), st.prev2.begin(), st.prev2.end());
+    }
+    // (sess) then the retain step's: long long keep_dst [K + 1], keep_src [K]; int keep_ref [K]
+    const size_t keep_ll = hll.size(), keep_int = hint.size();
+    const int keep = sess ? (int)U.keep_ref.size() : 0;
+    if (sess) {
+        hll.insert(hll.end(), U.keep_dst.begin(), U.keep_dst.end());
+        hll.insert(hll.end(), U.keep_src.begin(), U.keep_src.end());
+        hint.insert(hint.end(), U.keep_ref.begin(), U.keep_ref.end());
     }
     // the frames in device order, each sorted by its own cell in the sensor frame (identity poses, a box of 1024^3 cells
     // around the sensor: locality only, the chained priors are not known yet); lanes: grid y of the loop kernel, a
@@ -2951,10 +3115,41 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
             memcpy(&T_dev[(size_t)P.dev[(size_t)k] * 16], T_init + (size_t)s * 16, 16 * sizeof(double));
     for (int d = 0; d < n_frames; ++d)
         for (int c4 = 0; c4 < 4; ++c4) ident[(size_t)d * 16 + 5 * c4] = 1.0;
-    if (deltas) {
+    if (deltas && !sess) {
         D_dev.resize((size_t)n_frames * 16);
         for (int k = 0; k < n_frames; ++k) memcpy(&D_dev[(size_t)P.dev[(size_t)k] * 16], deltas + (size_t)k * 16, 16 * sizeof(double));
         CK(cudaMemcpyAsync(ctx->d_seq_delta, D_dev.data(), D_dev.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    }
+    // (sess) one increment per frame reference (the pushed frames, identity without deltas, then the retained frames: a
+    // sequence's last one carries the increment its push left), the retained poses, and room for the next window
+    const double* d_delta = deltas ? ctx->d_seq_delta.p : nullptr;
+    if (sess) {
+        d_delta = motion == DCREG_MOTION_INCREMENTS ? ctx->d_seq_delta.p : nullptr;
+        if (d_delta) {
+            D_dev.assign((size_t)(n_frames + n_hist) * 16, 0.0);
+            for (int e = 0; e < n_frames + n_hist; ++e)
+                for (int c4 = 0; c4 < 4; ++c4) D_dev[(size_t)e * 16 + 5 * c4] = 1.0;
+            if (deltas)
+                for (int k = 0; k < n_frames; ++k)
+                    memcpy(&D_dev[(size_t)P.dev[(size_t)k] * 16], deltas + (size_t)k * 16, 16 * sizeof(double));
+            const odom_plan::History& h = sess->hist;
+            for (int s = 0; s < n_seqs; ++s)
+                if (h.off[(size_t)s + 1] > h.off[(size_t)s])
+                    memcpy(&D_dev[(size_t)(n_frames + h.off[(size_t)s + 1] - 1) * 16], &sess->last_delta[(size_t)s * 16],
+                           16 * sizeof(double));
+            CK(ctx->d_seq_delta.ensure((long long)D_dev.size()));
+            CK(cudaMemcpyAsync(ctx->d_seq_delta, D_dev.data(), D_dev.size() * sizeof(double), cudaMemcpyHostToDevice,
+                               ctx->stream));
+            d_delta = ctx->d_seq_delta.p;       // (ensure may have moved it)
+        }
+        CK(sess->d_hist_T.ensure(std::max(n_hist, 1) * 16));
+        if (n_hist)
+            CK(cudaMemcpyAsync(sess->d_hist_T, sess->hist_T.data(), (size_t)n_hist * 16 * sizeof(double),
+                               cudaMemcpyHostToDevice, ctx->stream));
+        // grown with headroom: a window whose frames vary in size does not reallocate (and synchronise) at every push
+        DevBuf<float4>& nxt = sess->win[1 - sess->cur];
+        const long long need = std::max<long long>(U.keep_dst.back(), 1);
+        if (nxt.cap < need) CK(nxt.ensure(need + need / 4));
     }
     CK(cudaMemcpyAsync(ctx->d_seq_prior, ident.data(), ident.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     const Results R{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior};
@@ -2976,9 +3171,14 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         const int* d_frame = ctx->d_odom_int + at_int[(size_t)i];
         const int* d_prev = d_frame + pieces;
         const int* d_prev2 = d_prev + st.active;
-        // 1. the lanes' local maps from the window frames' device-resident results
-        map_points_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_scan_src, d_dst, pieces, d_src_at,
-                                                                                d_frame, m, ctx->d_state, ctx->d_odom_map);
+        // 1. the lanes' local maps from the window frames' device-resident results (sess: and from the retained frames)
+        if (sess)
+            map_points_hist_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(
+                ctx->d_scan_src, sess->win[sess->cur], n_frames, d_dst, pieces, d_src_at, d_frame, m, ctx->d_state,
+                sess->d_hist_T, ctx->d_odom_map);
+        else
+            map_points_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_scan_src, d_dst, pieces, d_src_at,
+                                                                                    d_frame, m, ctx->d_state, ctx->d_odom_map);
         ctx->launches++;
         CK(cudaGetLastError());
         // 1b. (map_voxel) every lane's map through the voxel filter, in world coordinates, .w re-indexed over the step's
@@ -3021,18 +3221,21 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
             while (!why.empty() && b < st.active - 1 && arena_plan::box_of(hb.data() + 6 * (size_t)b, &x) == arena_plan::kDense) ++b;
         }
         if (!why.empty()) {
-            const int s = st.seq[(size_t)b];
-            ctx->err = std::string(name) + ": sequence " + std::to_string(s) + ", frame " + std::to_string(seq_offsets[s] + i) +
-                       " (frame " + std::to_string(i) + " of the sequence): " + why;
+            ctx->err = std::string(name) + ": " + frame_name(st.seq[(size_t)b], P.input[(size_t)(st.first + b)]) + ": " + why;
             failed = i;
             break;
         }
         if ((rc = arena_fill(ctx, ctx->odom_maps, map, d_mseg, st.active, mk, boxes.data(), cells, inv_cell, rings)))
             return rc;
         // 3. every lane's frame of this step: its prior and a fresh loop state
-        odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
-            ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
-            st.first, st.active, d_prev, d_prev2, deltas ? ctx->d_seq_delta.p : nullptr, motion);
+        if (sess)
+            odom_start_hist_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
+                ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active,
+                n_seqs, st.first, st.active, d_prev, d_prev2, d_delta, motion, n_frames, sess->d_hist_T);
+        else
+            odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
+                ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
+                st.first, st.active, d_prev, d_prev2, d_delta, motion);
         ctx->launches++;
         CK(cudaGetLastError());
         // 4. the loop: the same chunks (and CUDA graphs) at every step - the grid table keeps its pointer (the first step
@@ -3044,12 +3247,24 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         }
         if ((rc = run_chunks(ctx, L, params, dlog, dlog ? log_cap : 0, params->max_iterations, 16, true))) return rc;
     }
+    // (sess) the next window: the retained frames' packed points, gathered from this push's frames and the old window
+    // into the other buffer, so the session's own window stays as it was until the push commits
+    const long long kept_points = sess ? U.keep_dst.back() : 0;
+    if (sess && failed == n_steps && kept_points > 0) {
+        const long long* d_keep_dst = ctx->d_odom_ll + keep_ll;
+        retain_points_kernel<<<(unsigned)((kept_points + 255) / 256), 256, 0, ctx->stream>>>(
+            ctx->d_scan_src, sess->win[sess->cur], n_frames, d_keep_dst, keep, d_keep_dst + keep + 1,
+            ctx->d_odom_int + keep_int, kept_points, sess->win[1 - sess->cur]);
+        ctx->launches++;
+        CK(cudaGetLastError());
+    }
     // results in the caller's frame order; after a failed step only the frames before it, and that step's message
     const std::string err = ctx->err;
     if ((rc = finish_call(ctx, params, n_frames, dlog, R, P.dev.data(),
                           failed < n_steps ? P.steps[(size_t)failed].first : n_frames)))
         return rc;
     if (failed < n_steps) { ctx->err = err; return DCREG_BAD_ARG; }
+    if (sess) commit_push(*sess, U, n_frames, seq_offsets, T_out, deltas);
     return DCREG_OK;
 }
 
@@ -3085,6 +3300,56 @@ int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* param
                         stride, cell_size, map_frames, motion, source_voxel, map_voxel, source_max_points,
                         map_max_points, T_init, deltas, frame_points, T_prior, T_out, n_iterations, converged, status,
                         cov, log, log_cap);
+}
+
+int dcreg_odometry_open(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
+                        int motion, double source_voxel, double map_voxel, int source_max_points, int map_max_points,
+                        const double* T_init) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (ctx->odom) { ctx->err = "odometry_open: a session is open already (dcreg_odometry_close it first)"; return DCREG_BAD_ARG; }
+    BatchCheck c{"odometry_open", params && n_seqs > 0 && T_init, "null pointer or n_seqs <= 0",
+                 "sequences are independent - give each rank its own, do not shard them", n_seqs};
+    c.own_cell = true; c.cell_size = cell_size; c.need_target = false; c.one_iteration = true;
+    c.own_msg = odometry_settings_error(map_frames, motion, false, source_voxel, map_voxel, source_max_points,
+                                        map_max_points);
+    const int rc = check_batch_call(ctx, params, c);
+    if (rc) return rc;
+    std::unique_ptr<dcreg_ctx::OdomSession> ss(new dcreg_ctx::OdomSession());
+    ss->params = *params;
+    ss->n_seqs = n_seqs; ss->map_frames = map_frames; ss->motion = motion;
+    ss->source_max_points = source_max_points; ss->map_max_points = map_max_points;
+    ss->cell_size = cell_size; ss->source_voxel = source_voxel; ss->map_voxel = map_voxel;
+    ss->T_init.assign(T_init, T_init + (size_t)n_seqs * 16);
+    ss->hist.seen.assign((size_t)n_seqs, 0);
+    ss->hist.off.assign((size_t)n_seqs + 1, 0);
+    ss->last_delta.assign((size_t)n_seqs * 16, 0.0);
+    for (int s = 0; s < n_seqs; ++s)
+        for (int c4 = 0; c4 < 4; ++c4) ss->last_delta[(size_t)s * 16 + 5 * c4] = 1.0;
+    ctx->odom = std::move(ss);
+    return DCREG_OK;
+}
+
+int dcreg_odometry_push(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
+                        const int64_t* frame_offsets, int stride, const double* deltas, int64_t* frame_points,
+                        double* T_prior, double* T_out, int* n_iterations, int* converged, int* status, double* cov,
+                        dcreg_iter_log* log, int log_cap) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!ctx->odom) { ctx->err = "odometry_push: no session is open (dcreg_odometry_open)"; return DCREG_BAD_ARG; }
+    dcreg_ctx::OdomSession& ss = *ctx->odom;
+    return run_odometry(ctx, "odometry_push", &ss.params, ss.n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
+                        ss.cell_size, ss.map_frames, ss.motion, ss.source_voxel, ss.map_voxel, ss.source_max_points,
+                        ss.map_max_points, ss.T_init.data(), deltas, frame_points, T_prior, T_out, n_iterations,
+                        converged, status, cov, log, log_cap, &ss);
+}
+
+// The session's buffers go with it; nothing queued may still read them
+int dcreg_odometry_close(dcreg_ctx* ctx) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!ctx->odom) { ctx->err = "odometry_close: no session is open (dcreg_odometry_open)"; return DCREG_BAD_ARG; }
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaStreamSynchronize(ctx->stream));
+    ctx->odom.reset();
+    return DCREG_OK;
 }
 
 int dcreg_voxel_downsample(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,

@@ -6,8 +6,9 @@
 // Step::active), one per lane, the lanes in ascending sequence order.  So a step's frames are one contiguous lane table,
 // and the loop's frame cursor stops at the end of a lane's only frame.  The map of lane j is the window frames
 // [max(first of the sequence, k - map_frames), k) of its sequence in ascending order, each frame's points in their input
-// order; the lanes' maps follow each other in one buffer.  Everything here is plain C++ so tests/test_odom_plan.py can
-// check it on the CPU (tools/test_odom_plan.cpp).
+// order; the lanes' maps follow each other in one buffer.  make_push plans a push to an odometry session the same way.
+// Everything here is plain C++ so tests/test_odom_plan.py and tests/test_odom_session_plan.py can check it on the CPU
+// (tools/test_odom_plan.cpp, tools/test_odom_session_plan.cpp).
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -89,6 +90,130 @@ inline std::string make(int n_seqs, const int* seq_off, int n_frames, const int6
                    " points, more than " + std::to_string(max_points) + " (int32 indexing)";
         p.max_map = std::max(p.max_map, m);
         p.max_pieces = std::max(p.max_pieces, (int)st.piece_frame.size());
+    }
+    return std::string();
+}
+
+// ---- a push to an odometry session (dcreg_odometry_push) -----------------------------------------------------------
+// A session carries, per sequence, the frames pushed so far and the last of them: the window frames the next frames'
+// maps need, with their points, and the frames the constant-velocity model needs, by pose alone.  Sequence s retains
+// its last min(seen, max(map_frames, 2)) frames; the last min(seen, map_frames) of them carry points (map_frames = 1
+// keeps the frame before the last as a pose alone).
+struct History {
+    std::vector<long long> seen;        // [n_seqs] frames of the sequence since the session opened
+    std::vector<int> off;               // [n_seqs + 1] retained frames of sequence s: [off[s], off[s + 1]), oldest first
+    std::vector<long long> at, n;       // [retained] first point in the window buffer, and points (0: a pose alone)
+};
+
+// A push numbers its frames like make(), with the retained frames acting as anchors that are not in the push: fixed
+// poses, not registered, no outputs.  Step 0 holds the anchors of the sequences that start in this push (their first
+// frame ever); step i >= 1 registers the i-th registrable pushed frame of every sequence that has one, lanes in
+// ascending sequence order.  A frame reference r (Step::prev, prev2, piece_frame, and keep_ref below) is the device
+// index of a pushed frame when r < n_frames, else retained frame r - n_frames of the history; piece_src is then a point
+// of the push's packed frames or of the window buffer.
+struct Push {
+    Plan plan;
+    History next;                       // the history after the push, its window packed sequence by sequence
+    std::vector<int> next_ref;          // [next retained] the frame each retained frame is
+    std::vector<long long> keep_dst;    // [keep + 1] the retained frames with points: where each goes in the new window
+    std::vector<long long> keep_src;    // [keep] its first point (push or window buffer, by keep_ref)
+    std::vector<int> keep_ref;          // [keep] its frame reference
+};
+
+inline int retained_frames(long long seen, int map_frames) {
+    return (int)std::min<long long>(seen, std::max(map_frames, 2));
+}
+
+// seq_off: n_seqs + 1 non-decreasing frame offsets of the pushed frames (a sequence may have none), frame_off: n_frames
+// + 1 point offsets, both validated; h: the history before the push.  Fails (returns the reason) when the maps of one
+// step hold more than max_points points.
+inline std::string make_push(int n_seqs, const int* seq_off, int n_frames, const int64_t* frame_off, int map_frames,
+                             long long max_points, const History& h, Push* out) {
+    Push& u = *out;
+    u = Push{};
+    Plan& p = u.plan;
+    // sequence s's pushed frame j is its frame seen[s] + j, at step j (a new sequence: j = 0 is its anchor) or j + 1
+    auto step_of = [&](int s, int j) { return h.seen[(size_t)s] > 0 ? j + 1 : j; };
+    int n_steps = 0;
+    for (int s = 0; s < n_seqs; ++s)
+        if (seq_off[s + 1] > seq_off[s]) n_steps = std::max(n_steps, step_of(s, seq_off[s + 1] - seq_off[s] - 1) + 1);
+    p.dev.assign((size_t)n_frames, -1);
+    p.input.assign((size_t)n_frames, -1);
+    p.steps.resize((size_t)n_steps);
+    int d = 0;
+    for (int i = 0; i < n_steps; ++i) {
+        Step& st = p.steps[(size_t)i];
+        st.first = d;
+        for (int s = 0; s < n_seqs; ++s) {
+            const int j = i - step_of(s, 0);
+            if (j >= 0 && j < seq_off[s + 1] - seq_off[s]) {
+                const int k = seq_off[s] + j;
+                p.dev[(size_t)k] = d;
+                p.input[(size_t)d] = k;
+                st.seq.push_back(s);
+                ++d;
+            }
+        }
+        st.active = (int)st.seq.size();
+    }
+    p.dev_off.assign((size_t)n_frames + 1, 0);
+    for (int e = 0; e < n_frames; ++e) {
+        const int k = p.input[(size_t)e];
+        p.dev_off[(size_t)e + 1] = p.dev_off[(size_t)e] + (frame_off[k + 1] - frame_off[k]);
+    }
+    // frame w (since open) of sequence s: a pushed frame, or one the history retains
+    auto ref = [&](int s, long long w) {
+        const long long seen = h.seen[(size_t)s];
+        return w >= seen ? p.dev[(size_t)(seq_off[s] + (w - seen))] : n_frames + h.off[(size_t)s + 1] - (int)(seen - w);
+    };
+    auto points = [&](int r) { return r < n_frames ? p.dev_off[(size_t)r + 1] - p.dev_off[(size_t)r] : h.n[(size_t)(r - n_frames)]; };
+    auto first_point = [&](int r) { return r < n_frames ? p.dev_off[(size_t)r] : h.at[(size_t)(r - n_frames)]; };
+    for (int i = 1; i < n_steps; ++i) {
+        Step& st = p.steps[(size_t)i];
+        st.map_seg.push_back(0);
+        st.piece_dst.push_back(0);
+        long long m = 0;
+        for (int j = 0; j < st.active; ++j) {
+            const int s = st.seq[(size_t)j];
+            const long long k = h.seen[(size_t)s] + (i - step_of(s, 0));
+            st.prev.push_back(ref(s, k - 1));
+            st.prev2.push_back(k - 1 > 0 ? ref(s, k - 2) : -1);
+            for (long long w = std::max<long long>(0, k - map_frames); w < k; ++w) {
+                const int r = ref(s, w);
+                st.piece_src.push_back(first_point(r));
+                st.piece_frame.push_back(r);
+                m += points(r);
+                st.piece_dst.push_back(m);
+            }
+            st.map_seg.push_back(m);
+        }
+        if (m > max_points)
+            return "odometry_push: the maps of step " + std::to_string(i) + " hold " + std::to_string(m) +
+                   " points, more than " + std::to_string(max_points) + " (int32 indexing)";
+        p.max_map = std::max(p.max_map, m);
+        p.max_pieces = std::max(p.max_pieces, (int)st.piece_frame.size());
+    }
+    // the history after the push
+    History& x = u.next;
+    x.seen.resize((size_t)n_seqs);
+    x.off.assign(1, 0);
+    u.keep_dst.assign(1, 0);
+    for (int s = 0; s < n_seqs; ++s) {
+        const long long c = h.seen[(size_t)s] + (seq_off[s + 1] - seq_off[s]);
+        x.seen[(size_t)s] = c;
+        const long long with_points = c - std::min<long long>(c, map_frames);
+        for (long long w = c - retained_frames(c, map_frames); w < c; ++w) {
+            const int r = ref(s, w);
+            u.next_ref.push_back(r);
+            x.at.push_back(u.keep_dst.back());
+            x.n.push_back(w >= with_points ? points(r) : 0);
+            if (w >= with_points) {
+                u.keep_ref.push_back(r);
+                u.keep_src.push_back(first_point(r));
+                u.keep_dst.push_back(u.keep_dst.back() + points(r));
+            }
+        }
+        x.off.push_back((int)x.n.size());
     }
     return std::string();
 }

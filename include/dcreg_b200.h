@@ -320,8 +320,9 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
  * 2^27 cells, or coordinates outside +-2^19 cells) is only found at its step: the call then returns DCREG_BAD_ARG with
  * dcreg_last_error naming the sequence and frame, the frames of the earlier steps have their outputs, and the context
  * stays usable.  The context's source, target and grid, and what the other calls compute, are left as they were.
- * A long recording goes in calls: each call starts with the previous call's last frame as its anchor, at the pose that
- * call returned; the first frames of a call then see maps of fewer frames than map_frames. */
+ * A recording that arrives frame by frame, or is too long for one call (about 100 B of device memory per point of the
+ * call), goes through an odometry session (dcreg_odometry_open / _push / _close): pushed in any chunks, it returns
+ * exactly what one call over the whole recording returns. */
 int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
                            int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
                            double cell_size, int map_frames, int motion, const double* T_init, const double* deltas,
@@ -365,6 +366,43 @@ int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* param
                                    const double* deltas, int64_t* frame_points, double* T_prior, double* T_out,
                                    int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
                                    int log_cap);
+/* ODOMETRY SESSION: scan-to-map odometry of S sequences fed as the frames arrive.  The session keeps each sequence's
+ * last map_frames registered frames (their filtered points in sensor coordinates and their poses) on the device
+ * between pushes, with the motion model's state, so no frame is uploaded or filtered twice.
+ * Contract: pushing a recording's frames in any chunking (one frame at a time, ragged pushes, sequences advancing at
+ * different rates) gives byte for byte the outputs of one dcreg_icp_run_odometry_voxel_n call over the whole recording
+ * with the session's settings: T_prior, T_out, n_iterations, converged, status, cov, frame_points and the log records
+ * (all but iter_time_ms).
+ * dcreg_odometry_open: the settings of that call (params is copied; cell_size, map_frames, motion, voxel sizes and caps,
+ *   T_init: n_seqs x 16), checked as that call checks them.  One session per context: open while one is open is
+ *   DCREG_BAD_ARG, as is a sharded context.  dcreg_destroy frees an open session.
+ * dcreg_odometry_push: the next frames of the sequences.  seq_offsets: n_seqs + 1 NON-DECREASING ints from 0 to
+ *   n_frames (n_frames >= 1; a sequence may get no frame, and then keeps its window untouched); xyz / frame_offsets /
+ *   stride and the outputs as in dcreg_icp_run_odometry_voxel_n, for the pushed frames in the caller's order.  Frame
+ *   numbers count from open: the first frame ever pushed to sequence s is its anchor (T_out = T_prior = T_init[s], cov
+ *   = 1e6 I, its points enter the maps).  deltas (n_frames x 16, or NULL for identity) has the one call's meaning: entry
+ *   k maps pushed frame k's result to the prior of the next frame of its sequence, which may come in a later push (the
+ *   session keeps each sequence's last entry), so the pushes' deltas concatenated are the one call's deltas.  With
+ *   DCREG_MOTION_CONSTANT_VELOCITY deltas must be NULL; the increment comes from the two previous results, wherever
+ *   they were pushed.
+ *   A push that fails returns DCREG_BAD_ARG with dcreg_last_error naming the sequence and its frame number since open
+ *   (bad tables, a frame the source filter leaves empty, a voxel coordinate out of range, a step's map with no dense
+ *   grid) and leaves the session exactly as it was: outputs of completed steps may have been written, but nothing is
+ *   committed, so the caller may split the push and retry.
+ *   Cost: a push costs what its frames cost in a one-shot call (the source filter's sync, one bounds copy per step, the
+ *   read-back) plus one launch that gathers the next windows; equal-shaped pushes reuse the buffers and the loop's CUDA
+ *   graphs.  Other calls may run between pushes without changing the session's results, and a push leaves the
+ *   context's source, target and grid as they were.
+ * dcreg_odometry_close: ends the session and frees its buffers; push or close without an open session is
+ *   DCREG_BAD_ARG. */
+int dcreg_odometry_open(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
+                        int motion, double source_voxel, double map_voxel, int source_max_points, int map_max_points,
+                        const double* T_init);
+int dcreg_odometry_push(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
+                        const int64_t* frame_offsets, int stride, const double* deltas, int64_t* frame_points,
+                        double* T_prior, double* T_out, int* n_iterations, int* converged, int* status, double* cov,
+                        dcreg_iter_log* log, int log_cap);
+int dcreg_odometry_close(dcreg_ctx* ctx);
 /* Voxel downsampling of many clouds in one call (KISS-ICP's VoxelDownsample rule: the first point of every voxel).
  * xyz / offsets / stride: HOST memory as in dcreg_icp_run_scans (n_clouds + 1 offsets, ascending strictly from 0, at
  * most 2^29 - 1 points).  With inv = 1.0 / voxel in FP64, point i's voxel is (floor((double)x inv), floor((double)y inv),
