@@ -17,6 +17,7 @@ There is NO CPU fallback: if the CUDA library is missing or no GPU is visible th
 from __future__ import annotations
 
 import ctypes as C
+import math
 import operator
 import os
 import types
@@ -89,7 +90,7 @@ EXPORTS = [
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_odometry_open", "dcreg_odometry_push", "dcreg_odometry_close", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_odometry_open", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_close", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -152,6 +153,14 @@ def load_library():
     lib.dcreg_odometry_push.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(C.c_float), C.POINTER(i64), ci, dp,
                                         C.POINTER(i64), dp, dp, C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp,
                                         C.POINTER(IterLog), ci]
+    lib.dcreg_icp_run_odometry_deskew.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
+                                                  C.POINTER(i64), ci, C.c_double, ci, ci, C.c_double, C.c_double, ci, ci,
+                                                  dp, dp, C.POINTER(C.c_float), C.POINTER(i64), dp, dp, C.POINTER(ci),
+                                                  C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(C.c_float), C.POINTER(IterLog),
+                                                  ci]
+    lib.dcreg_odometry_push_deskew.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(C.c_float), C.POINTER(i64), ci, dp,
+                                               C.POINTER(C.c_float), C.POINTER(i64), dp, dp, C.POINTER(ci), C.POINTER(ci),
+                                               C.POINTER(ci), dp, C.POINTER(C.c_float), C.POINTER(IterLog), ci]
     lib.dcreg_odometry_close.argtypes = [vp]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
@@ -237,6 +246,23 @@ def _pack_sequences(sequences):
     return (seq_off,) + _pack([f for s in sequences for f in s])
 
 
+def _pack_timestamps(timestamps, off, name):
+    """Per-frame timestamp arrays (nested like the frames) as one contiguous float32 array matching the packed points
+    with offsets off, or None"""
+    if timestamps is None:
+        return None
+    ts = [np.asarray(t, dtype=np.float32).reshape(-1) for t in timestamps]
+    if len(ts) != len(off) - 1 or any(t.shape[0] != b - a for t, a, b in zip(ts, off[:-1], off[1:])):
+        raise ValueError(f"{name}: timestamps must hold one value per point of every frame")
+    return np.ascontiguousarray(np.concatenate(ts) if ts else np.zeros(0, np.float32))
+
+
+def _split_deskewed(out, npts):
+    """(total, 3) deskewed points cut into one array per frame"""
+    at = np.concatenate([[0], np.cumsum(npts)])
+    return [out[a:b].copy() for a, b in zip(at[:-1], at[1:])]
+
+
 def pose_Rt(T):
     T = np.asarray(T, dtype=np.float64)
     return np.ascontiguousarray(np.concatenate([T[:3, :3].reshape(-1), T[:3, 3]]))
@@ -287,7 +313,136 @@ def constant_velocity_increment(T_prev, T):
     return out
 
 
-VOXEL_LIMIT = 1 << 20      # voxel coordinates must lie in [-2^20, 2^20): 21 bits per axis in one 63-bit key
+# The motion compensation of dcreg_icp_run_odometry_deskew (dcreg_b200/csrc/se3.cuh): the same formulas, operation order
+# and branch thresholds in FP64 NumPy.  A twist is xi = (rho, phi), Sophus's order.
+SE3_LOG_SMALL = 1e-10       # |quaternion vector| below which 2 atan(n / w) / n takes its series
+SE3_SMALL_ANGLE = 1e-3      # rotation angle below which A, B, C and the V^-1 factor take their series
+
+
+def _cross(a, b):
+    """a x b over the last axis, each entry a_i b_j - a_k b_l in FP64 (the device's order)"""
+    return np.stack([a[..., 1] * b[..., 2] - a[..., 2] * b[..., 1], a[..., 2] * b[..., 0] - a[..., 0] * b[..., 2],
+                     a[..., 0] * b[..., 1] - a[..., 1] * b[..., 0]], axis=-1)
+
+
+def se3_log(D):
+    """xi = Log(D) (6,) of a rigid motion D (4, 4), as se3.cuh forms it: the rotation's quaternion by Shepperd's rule
+    (w >= 0), theta = 2 atan2(|v|, w) for every angle in [0, pi], rho = V^-1 t.  The exact identity gives exactly 0; a
+    D with an entry that is not finite gives NaN."""
+    D = np.asarray(D, dtype=np.float64)
+    if not np.isfinite(D[:3]).all():
+        return np.full(6, np.nan)
+    R = [float(x) for x in D[:3, :3].reshape(-1)]
+    t = np.array(D[:3, 3], dtype=np.float64)
+    tr = (R[0] + R[4]) + R[8]
+    v = [0.0, 0.0, 0.0]
+    if tr > 0.0:
+        r = math.sqrt(tr + 1.0)
+        w = 0.5 * r
+        r = 0.5 / r
+        v = [(R[7] - R[5]) * r, (R[2] - R[6]) * r, (R[3] - R[1]) * r]
+    else:
+        i = 0
+        if R[4] > R[0]:
+            i = 1
+        if R[8] > R[4 * i]:
+            i = 2
+        j = (i + 1) % 3
+        k = (j + 1) % 3
+        r = math.sqrt(((R[4 * i] - R[4 * j]) - R[4 * k]) + 1.0)
+        v[i] = 0.5 * r
+        r = 0.5 / r
+        w = (R[3 * k + j] - R[3 * j + k]) * r
+        v[j] = (R[3 * j + i] + R[3 * i + j]) * r
+        v[k] = (R[3 * k + i] + R[3 * i + k]) * r
+    if w < 0.0:
+        w, v = -w, [-x for x in v]
+    n2 = (v[0] * v[0] + v[1] * v[1]) + v[2] * v[2]
+    if n2 < SE3_LOG_SMALL * SE3_LOG_SMALL:
+        f = 2.0 / w - (2.0 / 3.0) * n2 / ((w * w) * w)
+    else:
+        n = math.sqrt(n2)
+        f = 2.0 * math.atan2(n, w) / n
+    theta = f * math.sqrt(n2)
+    phi = np.array([f * v[0], f * v[1], f * v[2]])
+    if theta < SE3_SMALL_ANGLE:
+        c = 1.0 / 12.0 + (theta * theta) / 720.0
+    else:
+        h = 0.5 * theta
+        c = (1.0 - theta * math.cos(h) / (2.0 * math.sin(h))) / (theta * theta)
+    a = _cross(phi, t)
+    b = _cross(phi, a)
+    return np.concatenate([(t - 0.5 * a) + c * b, phi])
+
+
+def _exp_coeffs(t2):
+    """A = sin(theta) / theta, B = (1 - cos(theta)) / theta^2, C = (theta - sin(theta)) / theta^3 for theta^2 = t2
+    (array), with se3.cuh's series below SE3_SMALL_ANGLE"""
+    theta = np.sqrt(t2)
+    small = theta < SE3_SMALL_ANGLE
+    with np.errstate(invalid="ignore", divide="ignore"):
+        sn, cs = np.sin(theta), np.cos(theta)
+        A = np.where(small, 1.0 - t2 / 6.0 * (1.0 - t2 / 20.0), sn / theta)
+        B = np.where(small, 0.5 - t2 / 24.0 * (1.0 - t2 / 30.0), (1.0 - cs) / t2)
+        C = np.where(small, 1.0 / 6.0 - t2 / 120.0 * (1.0 - t2 / 42.0), (theta - sn) / (t2 * theta))
+    return A, B, C
+
+
+def se3_exp(xi):
+    """Exp(xi) (4, 4) of a twist xi (6,) = (rho, phi): Rodrigues for the rotation and t = V rho, with se3.cuh's
+    coefficients"""
+    xi = np.asarray(xi, dtype=np.float64)
+    rho, phi = xi[:3], xi[3:]
+    t2 = np.float64((phi[0] * phi[0] + phi[1] * phi[1]) + phi[2] * phi[2])
+    A, B, C = (float(x) for x in _exp_coeffs(np.array(t2)))
+    T = np.eye(4)
+    E = np.eye(3)
+    for c in range(3):                                      # column c = R e_c, formed as se3.cuh applies R to a point
+        a = _cross(phi, E[c])
+        T[:3, c] = (E[c] + A * a) + B * _cross(phi, a)
+    c1 = _cross(phi, rho)
+    T[:3, 3] = (rho + B * c1) + C * _cross(phi, c1)
+    return T
+
+
+def se3_exp_apply(xi, s, p):
+    """Exp(s_i xi) p_i for every row (s (N,), p (N, 3) FP64), as se3.cuh applies it: R p + V rho' in FP64, no rounding
+    to float32.  Returns (N, 3) float64."""
+    s = np.asarray(s, dtype=np.float64)[:, None]
+    rho, phi = s * xi[:3], s * xi[3:]
+    t2 = (phi[:, 0] * phi[:, 0] + phi[:, 1] * phi[:, 1]) + phi[:, 2] * phi[:, 2]
+    A, B, C = (x[:, None] for x in _exp_coeffs(t2))
+    a = _cross(phi, p)
+    c = _cross(phi, rho)
+    return ((p + A * a) + B * _cross(phi, a)) + ((rho + B * c) + C * _cross(phi, c))
+
+
+def deskew_points(P, timestamps, D):
+    """Points of one frame deskewed to mid-sweep as dcreg_icp_run_odometry_deskew does it: p' = fl32(Exp((tau - 0.5)
+    Log(D)) p) in FP64 with one float32 rounding, D (4, 4) the frame's increment, timestamps (N,) float32 in [0, 1].  A
+    row is copied bit for bit (no arithmetic) when tau = 0.5, when Log(D) is zero or not finite, when the row has a
+    non-finite coordinate, or when the result would have one.  P: (N, >=3).  Returns (N, 3) float32."""
+    P = np.asarray(P, dtype=np.float32)
+    if P.ndim != 2 or P.shape[1] < 3:
+        raise ValueError("points must be (N, >=3)")
+    xyz = np.array(P[:, :3])
+    tau = np.asarray(timestamps, dtype=np.float32).reshape(-1)
+    if tau.shape[0] != xyz.shape[0]:
+        raise ValueError(f"deskew_points: {xyz.shape[0]} points but {tau.shape[0]} timestamps")
+    xi = se3_log(D)
+    if not np.isfinite(xi).all() or (xi == 0.0).all():
+        return xyz
+    s = tau.astype(np.float64) - 0.5
+    move = (s != 0.0) & np.isfinite(xyz).all(axis=1)
+    with np.errstate(over="ignore", invalid="ignore"):
+        q = se3_exp_apply(xi, s[move], xyz[move].astype(np.float64)).astype(np.float32)
+    ok = np.isfinite(q).all(axis=1)
+    rows = np.nonzero(move)[0][ok]
+    xyz[rows] = q[ok]
+    return xyz
+
+
+VOXEL_LIMIT = 1 << 20     # voxel coordinates must lie in [-2^20, 2^20): 21 bits per axis in one 63-bit key
 
 
 def _max_points(v, name="max_points"):
@@ -345,6 +500,7 @@ class IcpResult:
         self.metrics = None
         self.T_prior = None             # icp_run_sequences: the initial pose the frame started from
         self.n_points = None            # icp_run_odometry: the frame's points after the source filter
+        self.deskewed = None            # icp_run_odometry (want_deskewed): those points after deskewing
 
 
 def _trial_results(st, conv, n_it, T_out, logs, cap, cov=None):
@@ -622,7 +778,7 @@ class Context:
     def icp_run_odometry(self, params: IcpParams, sequences, T_init, deltas=None, motion: str = "increments",
                          map_frames: int = 10, cell_size=None, want_log: bool = False, want_cov: bool = False,
                          source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
-                         map_max_points: int = 1):
+                         map_max_points: int = 1, timestamps=None, want_deskewed: bool = False):
         """Scan-to-map odometry (`sequences`: a list of lists of (N, >=3) point arrays): frame k of a sequence registers
         against the local map of the frames [k - map_frames, k) before it, each placed at its own registered pose
         (map_points), starting from compose_prior(frame k-1's result, D).  motion "increments": D = deltas[k-1]
@@ -634,7 +790,9 @@ class Context:
         map_max_points: the points each voxel of those filters keeps (dcreg_icp_run_odometry_voxel_n).  Returns a list of
         IcpResult, one per frame in order, with .T_prior and .n_points, the frame's points after the source filter (logs
         only when want_log, .cov when want_cov).  Needs no target; the context's source and target are left as they
-        were."""
+        were.  timestamps (nested like `sequences`: one float32 array per frame, each point's fraction of its sweep in
+        [0, 1]): deskew every registered frame with the increment its prior used (dcreg_icp_run_odometry_deskew);
+        want_deskewed: .deskewed holds each frame's kept points after deskewing ((n_points, 3) float32)."""
         models = {"increments": 0, "constant_velocity": 1}
         if motion not in models:
             raise ValueError(f"icp_run_odometry: motion must be one of {sorted(models)}, not {motion!r}")
@@ -645,11 +803,21 @@ class Context:
         cell = float(params.search_radius if cell_size is None else cell_size)
         capped = source_max_points != 1 or map_max_points != 1
         filtered = source_voxel != 0.0 or map_voxel != 0.0 or capped
+        deskew = timestamps is not None or want_deskewed
+        ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
+                              off if off is not None else np.zeros(1, np.int64), "icp_run_odometry")
         npts = np.diff(off) if off is not None else np.zeros(0, dtype=np.int64)
-        if filtered:
+        if filtered or deskew:
             npts = np.zeros(max(n, 1), dtype=np.int64)
+        desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
 
         def call(o):
+            if deskew:
+                return self.lib.dcreg_icp_run_odometry_deskew(
+                    self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
+                    3, cell, int(map_frames), models[motion], float(source_voxel), float(map_voxel), source_max_points,
+                    map_max_points, _optr(o.T_init), _optr(o.deltas), _fptr(ts), _iptr(npts), _optr(o.T_prior),
+                    _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov), _fptr(desk), o.logs, o.cap)
             if capped:
                 return self.lib.dcreg_icp_run_odometry_voxel_n(
                     self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
@@ -670,6 +838,9 @@ class Context:
                                 want_prior=True)
         for r, c in zip(out, npts):
             r.n_points = int(c)
+        if want_deskewed:
+            for r, d in zip(out, _split_deskewed(desk, npts[:n])):
+                r.deskewed = d
         return out
 
     def odometry_session(self, params: IcpParams, n_seqs: int, T_init, motion: str = "increments", map_frames: int = 10,
@@ -792,12 +963,15 @@ class OdometrySession:
         self.ctx, self.params, self.n_seqs = ctx, params, n_seqs
         self.open = True
 
-    def push(self, frames_per_seq, deltas=None, want_log: bool = False, want_cov: bool = False):
+    def push(self, frames_per_seq, deltas=None, want_log: bool = False, want_cov: bool = False, timestamps=None,
+             want_deskewed: bool = False):
         """The next frames of every sequence (dcreg_odometry_push): frames_per_seq, a list of n_seqs lists, possibly
         empty, of (N, >=3) point arrays.  deltas: (frames, 4, 4) increments over the pushed frames in order (entry k maps
         frame k's result to the next frame's prior in its sequence, which may come in a later push), or None for
         identity.  Returns one list of IcpResult per sequence, as icp_run_odometry gives them (.T_prior, .n_points; logs
-        only when want_log, .cov when want_cov).  A push that fails raises DcregError and leaves the session as it was."""
+        only when want_log, .cov when want_cov).  timestamps / want_deskewed: as in icp_run_odometry, nested like
+        frames_per_seq (dcreg_odometry_push_deskew).  A push that fails raises DcregError and leaves the session as it
+        was."""
         ctx, lib = self.ctx, self.ctx.lib
         if len(frames_per_seq) != self.n_seqs:
             raise ValueError(f"odometry push: {self.n_seqs} sequences but {len(frames_per_seq)} frame lists")
@@ -815,12 +989,24 @@ class OdometrySession:
         cov = np.empty((m, 6, 6)) if want_cov else None
         cap = int(self.params.max_iterations) if want_log else 0
         logs = (IterLog * max(cap * n, 1))() if want_log else None
-        ctx._check(lib.dcreg_odometry_push(ctx._h, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n, _fptr(xyz), _iptr(off),
-                                           3, _optr(D), _iptr(npts), _dptr(T_prior), _dptr(T_out), n_it, conv, st,
-                                           _optr(cov), logs, cap))
+        if timestamps is not None or want_deskewed:
+            ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
+                                  off if off is not None else np.zeros(1, np.int64), "odometry push")
+            desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
+            ctx._check(lib.dcreg_odometry_push_deskew(
+                ctx._h, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n, _fptr(xyz), _iptr(off), 3, _optr(D), _fptr(ts),
+                _iptr(npts), _dptr(T_prior), _dptr(T_out), n_it, conv, st, _optr(cov), _fptr(desk), logs, cap))
+        else:
+            desk = None
+            ctx._check(lib.dcreg_odometry_push(ctx._h, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n, _fptr(xyz),
+                                               _iptr(off), 3, _optr(D), _iptr(npts), _dptr(T_prior), _dptr(T_out), n_it,
+                                               conv, st, _optr(cov), logs, cap))
         res = _trial_results(st[:n], conv[:n], n_it[:n], T_out, logs, cap, cov)
         for r, Tp, c in zip(res, T_prior, npts):
             r.T_prior, r.n_points = Tp, int(c)
+        if want_deskewed:
+            for r, d in zip(res, _split_deskewed(desk, npts[:n])):
+                r.deskewed = d
         return [res[a:b] for a, b in zip(seq_off[:-1], seq_off[1:])]
 
     def close(self):

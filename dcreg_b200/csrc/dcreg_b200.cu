@@ -35,6 +35,7 @@
 #include "k2_solve.cuh"
 #include "loop_plan.hpp"
 #include "odom_plan.hpp"
+#include "se3.cuh"
 #include "peer_reduce.cuh"
 
 using k2::IcpState;
@@ -1118,6 +1119,91 @@ __global__ void retain_points_kernel(const float4* __restrict__ src, const float
     out[i] = (ref[p] < n_frames ? src : win)[src_at[p] + (i - dst[p])];
 }
 
+// ---- motion compensation (dcreg_icp_run_odometry_deskew, dcreg_odometry_push_deskew; se3.cuh) ---------------------
+// Once per call: ts[i] = the timestamp of packed point i (device order, segments seg[n_seg + 1]) from the caller's
+// timestamps ts_in.  Device frame b is the caller's frame whose input points start at in_at[b]; its point j is input
+// point j of that frame, or, after the source filter (index: d_vox_index), the input point index[kept_at[b] + j].
+__global__ void odom_ts_gather_kernel(const float* __restrict__ ts_in, long long n, const long long* __restrict__ seg,
+                                      int n_seg, const long long* __restrict__ in_at, const long long* __restrict__ kept_at,
+                                      const long long* __restrict__ index, float* __restrict__ ts) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int b = corr::segment_of(seg, n_seg, i);
+    const long long j = i - seg[b];
+    ts[i] = ts_in[in_at[b] + (index ? index[kept_at[b] + j] : j)];
+}
+
+// The increment D lane j's prior is composed with: the inputs odom_start_kernel / odom_start_hist_kernel read, formed
+// the same way, so D is bit for bit the one the prior used.  Frame references as in ref_pose (a one-shot call's are all
+// pushed frames, so hist_T is not read).
+__device__ __forceinline__ void odom_increment(int j, const IcpState* __restrict__ states, const int* __restrict__ prev,
+                                               const int* __restrict__ prev2, const double* __restrict__ delta, int motion,
+                                               int n_frames, const double* __restrict__ hist_T, double* D) {
+    for (int i = 0; i < 16; ++i) D[i] = (i % 5 == 0) ? 1.0 : 0.0;
+    if (motion == DCREG_MOTION_CONSTANT_VELOCITY) {
+        if (prev2[j] >= 0) {
+            double Ra[9], ta[3], Rb[9], tb[3];
+            ref_pose(prev[j], n_frames, states, hist_T, Ra, ta);
+            ref_pose(prev2[j], n_frames, states, hist_T, Rb, tb);
+            constant_velocity_increment(Rb, tb, Ra, ta, D);
+        }
+    } else if (delta) {
+        for (int i = 0; i < 16; ++i) D[i] = delta[(size_t)prev[j] * 16 + i];
+    }
+}
+
+// Per step, after the start kernel (one thread per lane j < active): xi[6 j ..] = Log(D) of the lane's increment, and
+// the lever arm of its frame step_first + j zeroed for odom_deskew_kernel to take again
+__global__ void odom_twist_kernel(const IcpState* __restrict__ states, int step_first, int active,
+                                  const int* __restrict__ prev, const int* __restrict__ prev2,
+                                  const double* __restrict__ delta, int motion, int n_frames,
+                                  const double* __restrict__ hist_T, double* __restrict__ xi, float* __restrict__ radius) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= active) return;
+    double D[16];
+    odom_increment(j, states, prev, prev2, delta, motion, n_frames, hist_T, D);
+    const double R[9] = {D[0], D[1], D[2], D[4], D[5], D[6], D[8], D[9], D[10]}, t[3] = {D[3], D[7], D[11]};
+    se3::se3_log(R, t, xi + 6 * (size_t)j);
+    radius[step_first + j] = 0.0f;
+}
+
+// Per step: the step's frames [step_first, step_first + active), points [base, base + n) of the packed (src) and the
+// sorted copy, deskewed in place by se3::deskew_point with their lane's twist.  A packed point's timestamp is ts[i]; a
+// sorted point's is that of its index in the frame (.w).  A point that does not move is not written.  The frame's lever
+// arm is taken again from the deskewed packed points with pack_points_kernel's rule.
+__global__ void odom_deskew_kernel(float4* __restrict__ src, float4* __restrict__ sorted, const long long* __restrict__ seg,
+                                   int step_first, int active, long long base, long long n, const float* __restrict__ ts,
+                                   const double* __restrict__ xi, float* __restrict__ radius) {
+    const long long i = base + (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    int b = -1;
+    float r = 0.0f;
+    if (i < base + n) {
+        const int j = corr::segment_of(seg + step_first, active, i);
+        b = step_first + j;
+        const double* x = xi + 6 * (size_t)j;
+        float o[3];
+        float4 p = src[i];
+        const float pi[3] = {p.x, p.y, p.z};
+        if (se3::deskew_point(x, ts[i], pi, o)) {
+            p.x = o[0]; p.y = o[1]; p.z = o[2];
+            src[i] = p;
+        }
+        float4 q = sorted[i];
+        const float qi[3] = {q.x, q.y, q.z};
+        if (se3::deskew_point(x, ts[seg[b] + __float_as_int(q.w)], qi, o)) {
+            q.x = o[0]; q.y = o[1]; q.z = o[2];
+            sorted[i] = q;
+        }
+        const float px = p.x, py = p.y, pz = p.z;
+        r = sqrtf(px * px + py * py + pz * pz);
+        if (!(r < 3.0e38f)) r = 0.0f;
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, b);
+    const unsigned rmax = __reduce_max_sync(peers, __float_as_uint(r));
+    if (b >= 0 && (int)(threadIdx.x & 31) == __ffs(peers) - 1 && rmax > 0u)
+        atomicMax(reinterpret_cast<unsigned int*>(radius + b), rmax);
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1256,6 +1342,10 @@ struct dcreg_ctx {
     // their grids in an arena of their own
     DevBuf<long long> d_odom_ll; DevBuf<int> d_odom_int;
     DevBuf<float4> d_odom_map, d_odom_map_vox;                         // ... and the maps after the voxel filter
+    // motion compensation (dcreg_icp_run_odometry_deskew): the caller's timestamps [input points], the packed points'
+    // [points], and the step's twists [lanes][6]
+    DevBuf<float> d_odom_ts_in, d_odom_ts;
+    DevBuf<double> d_odom_xi;
     // the odometry session (dcreg_odometry_open .. _close), if one is open: the settings of its pushes, and what every
     // sequence carries from one push to the next (odom_plan::History): the retained frames' kept points, packed and in
     // input order as d_scan_src holds them, in win[cur] (the other buffer receives the next push's window), their poses
@@ -2993,8 +3083,8 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
                         double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
                         int source_max_points, int map_max_points, const double* T_init, const double* deltas,
                         int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
-                        int* status, double* cov, dcreg_iter_log* log, int log_cap,
-                        dcreg_ctx::OdomSession* sess = nullptr) {
+                        int* status, double* cov, dcreg_iter_log* log, int log_cap, const float* timestamps,
+                        float* deskewed_xyz, dcreg_ctx::OdomSession* sess = nullptr) {
     if (!ctx) return DCREG_BAD_ARG;
     BatchCheck c{name, params && n_seqs > 0 && n_frames > 0 && seq_offsets && xyz && frame_offsets && T_init && T_out,
                  "null pointer, n_seqs <= 0 or n_frames <= 0",
@@ -3017,6 +3107,17 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         return "sequence " + std::to_string(s) + ", frame " + std::to_string(k) + " of the push (frame " +
                std::to_string(sess->hist.seen[(size_t)s] + j) + " of the sequence since open)";
     };
+    if (timestamps)             // every point's fraction of its sweep, before anything is launched
+        for (int s = 0; s < n_seqs; ++s)
+            for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k)
+                for (int64_t i = frame_offsets[k]; i < frame_offsets[k + 1]; ++i) {
+                    const float tau = timestamps[i];
+                    if (tau >= 0.0f && tau <= 1.0f) continue;
+                    ctx->err = std::string(name) + ": " + frame_name(s, k) + ": the timestamp of point " +
+                               std::to_string(i - frame_offsets[k]) + " is " +
+                               (std::isfinite(tau) ? std::to_string(tau) + ", outside [0, 1]" : std::string("not finite"));
+                    return DCREG_BAD_ARG;
+                }
     // the frames' voxel filter: once per call, on the staged points in input order, before the pack and the sort; one
     // sync for the kept counts.  From here on a frame is its kept points, on the device
     const float* src_xyz = xyz;
@@ -3026,8 +3127,8 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
     if (source_voxel > 0.0) {
         kept.resize((size_t)n_frames + 1);
         std::vector<int> bad((size_t)n_frames);
-        if ((rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, source_voxel, source_max_points, false,
-                                    false, kept.data(), bad.data())))
+        if ((rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, source_voxel, source_max_points,
+                                    timestamps != nullptr, false, kept.data(), bad.data())))
             return rc;
         for (int s = 0; s < n_seqs; ++s)
             for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k) {
@@ -3076,6 +3177,12 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         hll.insert(hll.end(), U.keep_dst.begin(), U.keep_dst.end());
         hll.insert(hll.end(), U.keep_src.begin(), U.keep_src.end());
         hint.insert(hint.end(), U.keep_ref.begin(), U.keep_ref.end());
+    }
+    // (timestamps) then the timestamp gather's: long long in_at [n_frames], kept_at [n_frames] (odom_ts_gather_kernel)
+    const size_t ts_ll = hll.size();
+    if (timestamps) {
+        for (int d = 0; d < n_frames; ++d) hll.push_back(frame_offsets[P.input[(size_t)d]]);
+        for (int d = 0; d < n_frames; ++d) hll.push_back(src_off[P.input[(size_t)d]]);
     }
     // the frames in device order, each sorted by its own cell in the sensor frame (identity poses, a box of 1024^3 cells
     // around the sensor: locality only, the chained priors are not known yet); lanes: grid y of the loop kernel, a
@@ -3156,6 +3263,21 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
     dcreg_iter_log* dlog = nullptr;
     const float4* src_iter = nullptr;
     if ((rc = start_loop(ctx, n_frames, T_dev.data(), R, &S, &dlog, &src_iter))) return rc;
+    // (timestamps) the caller's timestamps beside the packed points, once per call; the twists of a step's lanes
+    const long long n_points = P.dev_off[(size_t)n_frames];
+    if (timestamps) {
+        CK(ctx->d_odom_ts_in.ensure(std::max<long long>(frame_offsets[n_frames], 1)));
+        CK(ctx->d_odom_ts.ensure(std::max<long long>(n_points, 1)));
+        CK(ctx->d_odom_xi.ensure((long long)n_seqs * 6));
+        CK(cudaMemcpyAsync(ctx->d_odom_ts_in, timestamps, (size_t)frame_offsets[n_frames] * sizeof(float),
+                           cudaMemcpyHostToDevice, ctx->stream));
+        const long long* d_in_at = ctx->d_odom_ll + ts_ll;
+        odom_ts_gather_kernel<<<(unsigned)((n_points + 255) / 256), 256, 0, ctx->stream>>>(
+            ctx->d_odom_ts_in, n_points, ctx->d_scan_seg, n_frames, d_in_at, d_in_at + n_frames,
+            source_voxel > 0.0 ? ctx->d_vox_index.p : nullptr, ctx->d_odom_ts);
+        ctx->launches++;
+        CK(cudaGetLastError());
+    }
     const int rings = search_rings(params->search_radius, cell_size);
     LoopPlan L;
     bool planned = false;
@@ -3238,6 +3360,18 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
                 st.first, st.active, d_prev, d_prev2, d_delta, motion);
         ctx->launches++;
         CK(cudaGetLastError());
+        // 3b. (timestamps) the step's frames deskewed with the increments their priors used, outside the loop's graphs
+        if (timestamps) {
+            odom_twist_kernel<<<(unsigned)((st.active + 127) / 128), 128, 0, ctx->stream>>>(
+                ctx->d_state, st.first, st.active, d_prev, d_prev2, d_delta, motion, n_frames,
+                sess ? sess->d_hist_T.p : nullptr, ctx->d_odom_xi, ctx->d_scan_radius);
+            const long long a = P.dev_off[(size_t)st.first], np = P.dev_off[(size_t)(st.first + st.active)] - a;
+            odom_deskew_kernel<<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
+                ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_seg, st.first, st.active, a, np, ctx->d_odom_ts,
+                ctx->d_odom_xi, ctx->d_scan_radius);
+            ctx->launches += 2;
+            CK(cudaGetLastError());
+        }
         // 4. the loop: the same chunks (and CUDA graphs) at every step - the grid table keeps its pointer (the first step
         // has the most lanes, so the arena's table never regrows after it), only its entries change
         if (!planned) {
@@ -3264,6 +3398,20 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
                           failed < n_steps ? P.steps[(size_t)failed].first : n_frames)))
         return rc;
     if (failed < n_steps) { ctx->err = err; return DCREG_BAD_ARG; }
+    if (deskewed_xyz) {         // the frames' kept (deskewed) points, put in the caller's frame order
+        std::vector<float4> h((size_t)std::max<long long>(n_points, 1));
+        CK(cudaMemcpyAsync(h.data(), ctx->d_scan_src, (size_t)n_points * sizeof(float4), cudaMemcpyDeviceToHost,
+                           ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        for (int k = 0; k < n_frames; ++k) {
+            const long long d0 = P.dev_off[(size_t)P.dev[(size_t)k]];
+            float* o = deskewed_xyz + (size_t)src_off[k] * 3;
+            for (long long i = 0; i < src_off[k + 1] - src_off[k]; ++i) {
+                const float4 p = h[(size_t)(d0 + i)];
+                o[3 * i] = p.x; o[3 * i + 1] = p.y; o[3 * i + 2] = p.z;
+            }
+        }
+    }
     if (sess) commit_push(*sess, U, n_frames, seq_offsets, T_out, deltas);
     return DCREG_OK;
 }
@@ -3275,7 +3423,7 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
                            dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
                         cell_size, map_frames, motion, 0.0, 0.0, 1, 1, T_init, deltas, nullptr, T_prior, T_out,
-                        n_iterations, converged, status, cov, log, log_cap);
+                        n_iterations, converged, status, cov, log, log_cap, nullptr, nullptr);
 }
 
 int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
@@ -3286,7 +3434,7 @@ int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params,
                                  dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_voxel", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
                         cell_size, map_frames, motion, source_voxel, map_voxel, 1, 1, T_init, deltas, frame_points,
-                        T_prior, T_out, n_iterations, converged, status, cov, log, log_cap);
+                        T_prior, T_out, n_iterations, converged, status, cov, log, log_cap, nullptr, nullptr);
 }
 
 int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
@@ -3299,7 +3447,20 @@ int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* param
     return run_odometry(ctx, "icp_run_odometry_voxel_n", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets,
                         stride, cell_size, map_frames, motion, source_voxel, map_voxel, source_max_points,
                         map_max_points, T_init, deltas, frame_points, T_prior, T_out, n_iterations, converged, status,
-                        cov, log, log_cap);
+                        cov, log, log_cap, nullptr, nullptr);
+}
+
+int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                                  int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                                  double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                                  int source_max_points, int map_max_points, const double* T_init, const double* deltas,
+                                  const float* timestamps, int64_t* frame_points, double* T_prior, double* T_out,
+                                  int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
+                                  dcreg_iter_log* log, int log_cap) {
+    return run_odometry(ctx, "icp_run_odometry_deskew", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets,
+                        stride, cell_size, map_frames, motion, source_voxel, map_voxel, source_max_points,
+                        map_max_points, T_init, deltas, frame_points, T_prior, T_out, n_iterations, converged, status,
+                        cov, log, log_cap, timestamps, deskewed_xyz);
 }
 
 int dcreg_odometry_open(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
@@ -3339,7 +3500,20 @@ int dcreg_odometry_push(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, co
     return run_odometry(ctx, "odometry_push", &ss.params, ss.n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
                         ss.cell_size, ss.map_frames, ss.motion, ss.source_voxel, ss.map_voxel, ss.source_max_points,
                         ss.map_max_points, ss.T_init.data(), deltas, frame_points, T_prior, T_out, n_iterations,
-                        converged, status, cov, log, log_cap, &ss);
+                        converged, status, cov, log, log_cap, nullptr, nullptr, &ss);
+}
+
+int dcreg_odometry_push_deskew(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
+                               const int64_t* frame_offsets, int stride, const double* deltas, const float* timestamps,
+                               int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                               int* status, double* cov, float* deskewed_xyz, dcreg_iter_log* log, int log_cap) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!ctx->odom) { ctx->err = "odometry_push_deskew: no session is open (dcreg_odometry_open)"; return DCREG_BAD_ARG; }
+    dcreg_ctx::OdomSession& ss = *ctx->odom;
+    return run_odometry(ctx, "odometry_push_deskew", &ss.params, ss.n_seqs, seq_offsets, n_frames, xyz, frame_offsets,
+                        stride, ss.cell_size, ss.map_frames, ss.motion, ss.source_voxel, ss.map_voxel,
+                        ss.source_max_points, ss.map_max_points, ss.T_init.data(), deltas, frame_points, T_prior, T_out,
+                        n_iterations, converged, status, cov, log, log_cap, timestamps, deskewed_xyz, &ss);
 }
 
 // The session's buffers go with it; nothing queued may still read them

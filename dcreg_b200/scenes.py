@@ -5,6 +5,7 @@ C3  make_parking  : ground-dominated local map + sparse verticals, LiDAR-like fr
     make_parking_frames : the same map and a sequence of frames along a path through it (batched localisation)
     make_parking_pairs  : frame k+1 of that path against the local submap around pose k (scan/target pairs)
     make_parking_sequence : those frames with drifting odometry increments (sequences with chained priors)
+    make_parking_sweeps : those frames skewed by the sensor's motion during each sweep, with per-point timestamps
 C4  make_corridor : two parallel walls + floor + ceiling, rank-deficient along x
 C5  trial_poses   : seeded perturbations t ~ U[-1, 1]^3 m, rpy ~ U[-3, 3]^3 deg for the Monte-Carlo (SURVEY.md §8d)
     load_pcd_xyz  : PCD v0.7 `DATA binary` with float32 fields (the shipped clouds, SURVEY.md Appendix B.3)
@@ -168,6 +169,35 @@ def make_parking_sequence(n_frames, seed=47, odo_sigma=(0.03, 0.3), n_map=500_00
         e = np.concatenate([rng.normal(0.0, odo_sigma[0], 3), rng.normal(0.0, odo_sigma[1] * d, 3)])
         deltas[k] = np.linalg.inv(T_true[k]) @ T_true[k + 1] @ pose6d_to_matrix(*e)
     return frames, T_true, T_init[0], deltas, tgt
+
+
+def make_parking_sweeps(n_frames, seed=47, n_map=500_000, n_scan=6_000, map_seed=43, extent=60.0, max_range=30.0,
+                        path_half_length=20.0):
+    """make_parking_frames' path captured by a spinning LiDAR: each frame is a sweep during which the sensor moves.
+    The frames of make_parking_frames(n_frames, seed, ...) are the unskewed frames, in the mid-sweep sensor frame of
+    T_true[k].  Point i of frame k gets tau = (azimuth + pi) / (2 pi) in [0, 1] from its azimuth in that frame, and is
+    measured from the sensor pose T_k Exp((tau - 0.5) xi_k) with xi_k = Log(inv(T_{k-1}) T_k) (frame 0 takes frame 1's):
+    the skewed point is fl32(Exp(-(tau - 0.5) xi_k) p) (api.se3_exp_apply).  So the sweep motion is exactly the backward
+    increment, and deskewing frame k with D = inv(T_{k-1}) T_k (api.deskew_points) gives the unskewed frame back up to
+    float rounding.  Returns (skewed frames: list of (N_k, 3) float32, timestamps: list of (N_k,) float32, T_true
+    (n, 4, 4) mid-sweep poses, deltas (n, 4, 4) with deltas[k] = inv(T_k) T_{k+1} (the last the identity), the
+    unskewed frames)."""
+    from dcreg_b200 import api
+    frames, T_true, _, _ = make_parking_frames(n_frames, seed=seed, n_map=n_map, n_scan=n_scan, map_seed=map_seed,
+                                               extent=extent, max_range=max_range, path_half_length=path_half_length)
+    deltas = np.tile(np.eye(4), (n_frames, 1, 1))
+    for k in range(n_frames - 1):
+        deltas[k] = np.linalg.inv(T_true[k]) @ T_true[k + 1]
+    skewed, stamps = [], []
+    for k in range(n_frames):
+        xi = api.se3_log(deltas[k - 1] if k > 0 else deltas[0]) if n_frames > 1 else np.zeros(6)
+        p = frames[k].astype(np.float64)
+        tau = ((np.arctan2(p[:, 1], p[:, 0]) + np.pi) / (2.0 * np.pi)).astype(np.float32)
+        tau = np.clip(tau, np.float32(0.0), np.float32(1.0))
+        s = tau.astype(np.float64) - 0.5
+        skewed.append(np.ascontiguousarray(api.se3_exp_apply(xi, -s, p).astype(np.float32)))
+        stamps.append(tau)
+    return skewed, stamps, T_true, deltas, frames
 
 
 def trial_poses(n, seed=45, max_trans=1.0, max_rot_deg=3.0):

@@ -366,6 +366,37 @@ int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* param
                                    const double* deltas, int64_t* frame_points, double* T_prior, double* T_out,
                                    int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
                                    int log_cap);
+/* dcreg_icp_run_odometry_voxel_n with motion compensation (deskewing) of every registered frame, KISS-ICP's DeSkewScan.
+ * timestamps (HOST, one float per input point, indexed like xyz; NULL: this call is dcreg_icp_run_odometry_voxel_n
+ * itself, same launches, same bytes): tau, the point's fraction of its sweep in [0, 1], normalised by the caller; the
+ * reference time is mid-sweep, tau = 0.5, so T_out[k] is the sensor pose at the middle of frame k's sweep.
+ * - Motion: D_k, the increment frame k's prior is composed with (T_prior[k] = compose_prior(T_out[k-1], D_k)): deltas[k-1]
+ *   (or the identity) with DCREG_MOTION_INCREMENTS, constant_velocity_increment(T_out[k-2], T_out[k-1]) (identity right
+ *   after the anchor) with DCREG_MOTION_CONSTANT_VELOCITY - the same bytes.  xi_k = Log(D_k) (SE(3), Sophus's
+ *   convention: the rotation through its quaternion and atan2, exact on [0, pi]).
+ * - Deskew: every kept point p of frame k becomes fl32(Exp((tau - 0.5) xi_k) p), in FP64 with one float32 rounding
+ *   (Rodrigues and the V matrix; dcreg_b200/csrc/se3.cuh, and dcreg_b200.api.deskew_points for the NumPy twin).  A point
+ *   is copied bit for bit, with no arithmetic, when tau = 0.5, when xi_k is exactly zero or not finite, when it has a
+ *   non-finite coordinate, or when the result would have one: deskewing adds no non-finite coordinate.  Anchors are
+ *   never deskewed (nothing is known of their motion).  Accuracy: within one float32 ulp of the exact value or 1e-12 m,
+ *   whichever is larger (the device's sincos and libm's differ in the last FP64 bit).
+ * - Order: the source filter runs first, on the raw points (the plan needs every frame's kept count before the loop);
+ *   each kept point is then deskewed at its frame's step with its own timestamp.  KISS-ICP deskews, then filters; this
+ *   call filters, then deskews.
+ * - The deskewed frame is what frame k registers with, what enters the later maps (at T_out[k]) and what a session
+ *   retains.  deskewed_xyz (out, may be NULL): every frame's kept points after deskewing, 3 floats each, frame_points[k]
+ *   rows per frame in the caller's frame order, anchors included.
+ * - Cost: one timestamp upload and one gather launch per call, two launches per step (the lanes' twists, then every point
+ *   of the step's frames), outside the loop's CUDA graphs; deskewed_xyz costs one copy of the kept points.
+ * Errors (DCREG_BAD_ARG before anything is launched, dcreg_last_error naming the sequence, frame and point): a
+ * timestamp that is not finite, or outside [0, 1]; everything else as in dcreg_icp_run_odometry_voxel_n. */
+int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                                  int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                                  double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                                  int source_max_points, int map_max_points, const double* T_init, const double* deltas,
+                                  const float* timestamps, int64_t* frame_points, double* T_prior, double* T_out,
+                                  int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
+                                  dcreg_iter_log* log, int log_cap);
 /* ODOMETRY SESSION: scan-to-map odometry of S sequences fed as the frames arrive.  The session keeps each sequence's
  * last map_frames registered frames (their filtered points in sensor coordinates and their poses) on the device
  * between pushes, with the motion model's state, so no frame is uploaded or filtered twice.
@@ -402,6 +433,18 @@ int dcreg_odometry_push(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, co
                         const int64_t* frame_offsets, int stride, const double* deltas, int64_t* frame_points,
                         double* T_prior, double* T_out, int* n_iterations, int* converged, int* status, double* cov,
                         dcreg_iter_log* log, int log_cap);
+/* dcreg_odometry_push with motion compensation: timestamps and deskewed_xyz as in dcreg_icp_run_odometry_deskew, for the
+ * pushed frames (NULL timestamps: dcreg_odometry_push itself).  The session contract extends to it: any chunking gives
+ * byte for byte what one dcreg_icp_run_odometry_deskew call over the recording gives, deskewed_xyz included.  The
+ * increments are the one call's, so a pushed frame whose previous frames came in earlier pushes is deskewed with the
+ * retained poses or the sequence's last delta.  Pushes may mix: the frames of a push without timestamps are those of a
+ * call with every tau = 0.5 (copied), and the frames a session retains are the deskewed ones.  A timestamp that is not
+ * finite or outside [0, 1] is DCREG_BAD_ARG naming the sequence, its frame number since open and the point, before
+ * anything is launched, and leaves the session unchanged. */
+int dcreg_odometry_push_deskew(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
+                               const int64_t* frame_offsets, int stride, const double* deltas, const float* timestamps,
+                               int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                               int* status, double* cov, float* deskewed_xyz, dcreg_iter_log* log, int log_cap);
 int dcreg_odometry_close(dcreg_ctx* ctx);
 /* Voxel downsampling of many clouds in one call (KISS-ICP's VoxelDownsample rule: the first point of every voxel).
  * xyz / offsets / stride: HOST memory as in dcreg_icp_run_scans (n_clouds + 1 offsets, ascending strictly from 0, at
