@@ -678,9 +678,18 @@ template <bool kUseWd, bool kGrids, bool kSeq, bool kPlanes = false>
 cudaError_t loop_kernel_attributes(size_t smem) {
     cudaError_t e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids, kSeq, kPlanes>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess)
+    // the smallest shared-memory carveout that keeps 3 blocks resident (each also reserves 1 KB), so that the rest of the
+    // SM's unified data cache is L1 for the searches' and certificates' target reads.  The percentage is of the largest
+    // carveout and is rounded up to the next capacity the SM supports.
+    int dev = 0, max_smem = 0;
+    if (e == cudaSuccess) e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+    if (e == cudaSuccess) {
+        const size_t need = 3 * (smem + 1024);
+        const int pct = (int)std::min<size_t>(100, (need * 100 + (size_t)max_smem - 1) / (size_t)max_smem);
         e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids, kSeq, kPlanes>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                 cudaSharedmemCarveoutMaxShared);
+                                 pct);
+    }
     return e;
 }
 
