@@ -899,56 +899,6 @@ __global__ void init_state_kernel(IcpState* states, const double* T, long long n
     counters[b] = 0u;
 }
 
-// ---- odometry (dcreg_icp_run_odometry; odom_plan.hpp) ------------------------------------------------------------
-// The local maps of one step: m points in all, piece p (a window frame) being map points [dst[p], dst[p+1]) = the points
-// src[src_at[p] ..] of the frame's packed input (input order) under the frame's final pose, states[frame[p]].  Every
-// coordinate is ((r0 x + r1 y) + r2 z) + t in FP64, one rounding per operation, then one float32 rounding
-// (dcreg_b200.api.map_points gives the same bits); w = the point's index over the step's maps, as a packed target.
-__global__ void map_points_kernel(const float4* __restrict__ src, const long long* __restrict__ dst, int pieces,
-                                  const long long* __restrict__ src_at, const int* __restrict__ frame, long long m,
-                                  const IcpState* __restrict__ states, float4* __restrict__ out) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    const int p = corr::segment_of(dst, pieces, i);
-    const IcpState* st = states + frame[p];
-    const float4 q = src[src_at[p] + (i - dst[p])];
-    const double x = q.x, y = q.y, z = q.z;
-    float v[3];
-#pragma unroll
-    for (int r = 0; r < 3; ++r)
-        v[r] = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(st->R[3 * r], x), __dmul_rn(st->R[3 * r + 1], y)),
-                                          __dmul_rn(st->R[3 * r + 2], z)),
-                                st->t[r]);
-    out[i] = make_float4(v[0], v[1], v[2], __int_as_float((int)i));
-}
-
-// Start of step `step_first` (one thread per lane of `lanes`): lane j < active runs frame step_first + j and nothing
-// after it (its frame range is that one frame, so the frame advance ends the lane), the other lanes run nothing.  The
-// frame's prior is compose_prior(frame k-1's result, D) with D = delta[prev] (or identity), or (constant velocity) the
-// increment from frame k-2 to frame k-1 (identity after the anchor).
-__global__ void odom_start_kernel(IcpState* states, const long long* __restrict__ seg, double* T_prior, int* cursor,
-                                  int* first, unsigned int* n_active, int lanes, int step_first, int active,
-                                  const int* __restrict__ prev, const int* __restrict__ prev2, const double* __restrict__ delta,
-                                  int motion) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j == 0) { *n_active = (unsigned)active; first[lanes] = step_first + active; }
-    if (j >= lanes) return;
-    const int f = step_first + min(j, active);
-    first[j] = f; cursor[j] = f;
-    if (j >= active) return;
-    const IcpState* a = states + prev[j];
-    double D[16] = {1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0};
-    if (motion == DCREG_MOTION_CONSTANT_VELOCITY) {
-        if (prev2[j] >= 0) constant_velocity_increment(states[prev2[j]].R, states[prev2[j]].t, a->R, a->t, D);
-    } else if (delta) {
-        for (int i = 0; i < 16; ++i) D[i] = delta[(size_t)prev[j] * 16 + i];
-    }
-    double T[16];
-    compose_prior(a->R, a->t, D, T);
-    for (int i = 0; i < 16; ++i) T_prior[(size_t)f * 16 + i] = T[i];
-    init_loop_state(states + f, T, seg[f + 1] - seg[f]);
-}
-
 // ---- voxel filter (dcreg_voxel_downsample, dcreg_icp_run_odometry_voxel) -------------------------------------------
 // n points (`stride` floats each: host layout, or float4) in n_seg clouds, cloud b being points [seg[b], seg[b+1]).
 // Point i's voxel is floor((double)p * inv) per axis (corr::cell_coord before the integer conversion); the survivor of a
@@ -1039,11 +989,11 @@ __global__ void voxel_scatter_kernel(const float* __restrict__ in, long long n, 
     if (index) index[p] = i - seg[corr::segment_of(seg, n_seg, i)];
 }
 
-// ---- odometry sessions (dcreg_odometry_push; odom_plan::make_push) ---------------------------------------------------
-// Frame reference r of a push: r < n_frames is a pushed frame (device index d = r: points in the push's packed frames,
-// pose in states[d]); otherwise retained frame r - n_frames of the session (points in the window buffer, pose the
+// ---- odometry (dcreg_icp_run_odometry, dcreg_odometry_push; odom_plan.hpp) ------------------------------------------
+// Frame reference r (odom_plan::Push): r < n_frames is a frame of the call (device index d = r: points in its packed
+// frames, pose in states[d]); otherwise retained frame r - n_frames of a session (points in the window buffer, pose the
 // row-major 4x4 T_out the call that registered it returned, hist_T[16 (r - n_frames) ..], whose R and t are the bytes
-// of that frame's final loop state).
+// of that frame's final loop state).  A one-shot call has no retained frame: its hist_T and window are null.
 __device__ __forceinline__ void ref_pose(int r, int n_frames, const IcpState* __restrict__ states,
                                          const double* __restrict__ hist_T, double* R, double* t) {
     if (r < n_frames) {
@@ -1063,12 +1013,15 @@ __device__ __forceinline__ void ref_pose(int r, int n_frames, const IcpState* __
     }
 }
 
-// map_points_kernel for a push: piece p's points come from the push's packed frames (src) or from the window buffer
-// (win) by its frame reference frame[p], and so does its pose.  The same arithmetic and the same .w.
-__global__ void map_points_hist_kernel(const float4* __restrict__ src, const float4* __restrict__ win, int n_frames,
-                                       const long long* __restrict__ dst, int pieces, const long long* __restrict__ src_at,
-                                       const int* __restrict__ frame, long long m, const IcpState* __restrict__ states,
-                                       const double* __restrict__ hist_T, float4* __restrict__ out) {
+// The local maps of one step: m points in all, piece p (a window frame) being map points [dst[p], dst[p+1]) = the points
+// src_at[p] .. of the frame's packed input (input order) under the frame's final pose, both by its frame reference
+// frame[p].  Every coordinate is ((r0 x + r1 y) + r2 z) + t in FP64, one rounding per operation, then one float32
+// rounding (dcreg_b200.api.map_points gives the same bits); w = the point's index over the step's maps, as a packed
+// target.
+__global__ void map_points_kernel(const float4* __restrict__ src, const float4* __restrict__ win, int n_frames,
+                                  const long long* __restrict__ dst, int pieces, const long long* __restrict__ src_at,
+                                  const int* __restrict__ frame, long long m, const IcpState* __restrict__ states,
+                                  const double* __restrict__ hist_T, float4* __restrict__ out) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
     const int p = corr::segment_of(dst, pieces, i);
@@ -1086,31 +1039,43 @@ __global__ void map_points_hist_kernel(const float4* __restrict__ src, const flo
     out[i] = make_float4(v[0], v[1], v[2], __int_as_float((int)i));
 }
 
-// odom_start_kernel for a push: prev / prev2 are frame references, and delta holds one entry per reference (pushed
-// frames, then retained frames), or is null
-__global__ void odom_start_hist_kernel(IcpState* states, const long long* __restrict__ seg, double* T_prior, int* cursor,
-                                       int* first, unsigned int* n_active, int lanes, int step_first, int active,
-                                       const int* __restrict__ prev, const int* __restrict__ prev2,
-                                       const double* __restrict__ delta, int motion, int n_frames,
-                                       const double* __restrict__ hist_T) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j == 0) { *n_active = (unsigned)active; first[lanes] = step_first + active; }
-    if (j >= lanes) return;
-    const int f = step_first + min(j, active);
-    first[j] = f; cursor[j] = f;
-    if (j >= active) return;
-    double Ra[9], ta[3];
-    ref_pose(prev[j], n_frames, states, hist_T, Ra, ta);
-    double D[16] = {1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 0.0, 1.0};
+// The increment D lane j's prior is composed with: delta[prev[j]] (null: identity), or with constant velocity the
+// increment from frame k-2 to frame k-1 (identity after the anchor).  The start kernel and odom_twist_kernel both take
+// it from here, so the deskew twist is the increment the prior used, bit for bit.
+__device__ __forceinline__ void odom_increment(int j, const IcpState* __restrict__ states, const int* __restrict__ prev,
+                                               const int* __restrict__ prev2, const double* __restrict__ delta, int motion,
+                                               int n_frames, const double* __restrict__ hist_T, double* D) {
+    for (int i = 0; i < 16; ++i) D[i] = (i % 5 == 0) ? 1.0 : 0.0;
     if (motion == DCREG_MOTION_CONSTANT_VELOCITY) {
         if (prev2[j] >= 0) {
-            double Rb[9], tb[3];
+            double Ra[9], ta[3], Rb[9], tb[3];
+            ref_pose(prev[j], n_frames, states, hist_T, Ra, ta);
             ref_pose(prev2[j], n_frames, states, hist_T, Rb, tb);
             constant_velocity_increment(Rb, tb, Ra, ta, D);
         }
     } else if (delta) {
         for (int i = 0; i < 16; ++i) D[i] = delta[(size_t)prev[j] * 16 + i];
     }
+}
+
+// Start of step `step_first` (one thread per lane of `lanes`): lane j < active runs frame step_first + j and nothing
+// after it (its frame range is that one frame, so the frame advance ends the lane), the other lanes run nothing.  The
+// frame's prior is compose_prior(frame prev[j]'s pose, odom_increment); delta holds one entry per frame reference, or is
+// null.
+__global__ void odom_start_kernel(IcpState* states, const long long* __restrict__ seg, double* T_prior, int* cursor,
+                                  int* first, unsigned int* n_active, int lanes, int step_first, int active,
+                                  const int* __restrict__ prev, const int* __restrict__ prev2,
+                                  const double* __restrict__ delta, int motion, int n_frames,
+                                  const double* __restrict__ hist_T) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j == 0) { *n_active = (unsigned)active; first[lanes] = step_first + active; }
+    if (j >= lanes) return;
+    const int f = step_first + min(j, active);
+    first[j] = f; cursor[j] = f;
+    if (j >= active) return;
+    double D[16], Ra[9], ta[3];
+    odom_increment(j, states, prev, prev2, delta, motion, n_frames, hist_T, D);
+    ref_pose(prev[j], n_frames, states, hist_T, Ra, ta);
     double T[16];
     compose_prior(Ra, ta, D, T);
     for (int i = 0; i < 16; ++i) T_prior[(size_t)f * 16 + i] = T[i];
@@ -1140,25 +1105,6 @@ __global__ void odom_ts_gather_kernel(const float* __restrict__ ts_in, long long
     const int b = corr::segment_of(seg, n_seg, i);
     const long long j = i - seg[b];
     ts[i] = ts_in[in_at[b] + (index ? index[kept_at[b] + j] : j)];
-}
-
-// The increment D lane j's prior is composed with: the inputs odom_start_kernel / odom_start_hist_kernel read, formed
-// the same way, so D is bit for bit the one the prior used.  Frame references as in ref_pose (a one-shot call's are all
-// pushed frames, so hist_T is not read).
-__device__ __forceinline__ void odom_increment(int j, const IcpState* __restrict__ states, const int* __restrict__ prev,
-                                               const int* __restrict__ prev2, const double* __restrict__ delta, int motion,
-                                               int n_frames, const double* __restrict__ hist_T, double* D) {
-    for (int i = 0; i < 16; ++i) D[i] = (i % 5 == 0) ? 1.0 : 0.0;
-    if (motion == DCREG_MOTION_CONSTANT_VELOCITY) {
-        if (prev2[j] >= 0) {
-            double Ra[9], ta[3], Rb[9], tb[3];
-            ref_pose(prev[j], n_frames, states, hist_T, Ra, ta);
-            ref_pose(prev2[j], n_frames, states, hist_T, Rb, tb);
-            constant_velocity_increment(Rb, tb, Ra, ta, D);
-        }
-    } else if (delta) {
-        for (int i = 0; i < 16; ++i) D[i] = delta[(size_t)prev[j] * 16 + i];
-    }
 }
 
 // Per step, after the start kernel (one thread per lane j < active): xi[6 j ..] = Log(D) of the lane's increment, and
@@ -1286,6 +1232,14 @@ struct DevBuf {
 template <typename T>
 using PinnedBuf = DevBuf<T, true>;
 
+// The settings of scan-to-map odometry: a one-shot call's, or those dcreg_odometry_open gives every push of a session
+struct OdomSettings {
+    dcreg_icp_params params{};
+    int n_seqs = 0, map_frames = 1, motion = 0, source_max_points = 1, map_max_points = 1;
+    double cell_size = 0.0, source_voxel = 0.0, map_voxel = 0.0;
+    std::vector<double> T_init;                                        // [n_seqs][16]
+};
+
 struct dcreg_ctx {
     int device = 0;
     int sm_count = 132;
@@ -1360,10 +1314,7 @@ struct dcreg_ctx {
     // input order as d_scan_src holds them, in win[cur] (the other buffer receives the next push's window), their poses
     // (the T_out the host returned) and the last increment of every sequence
     struct OdomSession {
-        dcreg_icp_params params{};
-        int n_seqs = 0, map_frames = 1, motion = 0, source_max_points = 1, map_max_points = 1;
-        double cell_size = 0.0, source_voxel = 0.0, map_voxel = 0.0;
-        std::vector<double> T_init;                                    // [n_seqs][16]
+        OdomSettings set;
         odom_plan::History hist;
         std::vector<double> hist_T;                                    // [retained][16]
         std::vector<double> last_delta;                                // [n_seqs][16]
@@ -3045,19 +2996,29 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
                     Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, true, &S);
 }
 
-// dcreg_icp_run_odometry (source_voxel = map_voxel = 0, `name` "icp_run_odometry"), dcreg_icp_run_odometry_voxel (caps
-// of 1) and dcreg_icp_run_odometry_voxel_n: one body.  A voxel size of 0 leaves its filter out entirely: no launch, no
-// copy, no sync.
+// The settings of a one-shot call (dcreg_icp_run_odometry: source_voxel = map_voxel = 0, caps of 1; _voxel: caps of 1)
+// or of a session (dcreg_odometry_open).  A voxel size of 0 leaves its filter out entirely: no launch, no copy, no sync.
+// T_init stays empty when params or T_init is null or n_seqs <= 0, which the checks report as a null pointer; no valid
+// call has more than kMaxPairs sequences, so no more are read before the checks reject it.
+static OdomSettings odom_settings(const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
+                                  int motion, double source_voxel, double map_voxel, int source_max_points,
+                                  int map_max_points, const double* T_init) {
+    OdomSettings set{params ? *params : dcreg_icp_params{}, n_seqs, map_frames, motion, source_max_points, map_max_points,
+                     cell_size, source_voxel, map_voxel};
+    if (params && T_init && n_seqs > 0)
+        set.T_init.assign(T_init, T_init + (size_t)std::min(n_seqs, arena_plan::kMaxPairs) * 16);
+    return set;
+}
+
 // What is wrong with the settings of an odometry call or session, or null
-static const char* odometry_settings_error(int map_frames, int motion, bool deltas, double source_voxel, double map_voxel,
-                                           int source_max_points, int map_max_points) {
-    if (map_frames < 1) return "map_frames must be >= 1";
-    if (motion != DCREG_MOTION_INCREMENTS && motion != DCREG_MOTION_CONSTANT_VELOCITY)
+static const char* odometry_settings_error(const OdomSettings& set, bool deltas) {
+    if (set.map_frames < 1) return "map_frames must be >= 1";
+    if (set.motion != DCREG_MOTION_INCREMENTS && set.motion != DCREG_MOTION_CONSTANT_VELOCITY)
         return "motion must be DCREG_MOTION_INCREMENTS or DCREG_MOTION_CONSTANT_VELOCITY";
-    if (motion == DCREG_MOTION_CONSTANT_VELOCITY && deltas) return "the constant-velocity model takes no deltas (pass NULL)";
-    if (!(source_voxel >= 0.0 && source_voxel < INFINITY) || !(map_voxel >= 0.0 && map_voxel < INFINITY))
+    if (set.motion == DCREG_MOTION_CONSTANT_VELOCITY && deltas) return "the constant-velocity model takes no deltas (pass NULL)";
+    if (!(set.source_voxel >= 0.0 && set.source_voxel < INFINITY) || !(set.map_voxel >= 0.0 && set.map_voxel < INFINITY))
         return "source_voxel and map_voxel must be finite and >= 0 (0: no filter)";
-    if (source_max_points < 1 || map_max_points < 1) return "source_max_points and map_max_points must be >= 1";
+    if (set.source_max_points < 1 || set.map_max_points < 1) return "source_max_points and map_max_points must be >= 1";
     return nullptr;
 }
 
@@ -3073,7 +3034,7 @@ static void commit_push(dcreg_ctx::OdomSession& ss, const odom_plan::Push& u, in
         memcpy(&T[e * 16], from, 16 * sizeof(double));
     }
     static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    for (int s = 0; s < ss.n_seqs; ++s)
+    for (int s = 0; s < ss.set.n_seqs; ++s)
         if (seq_offsets[s + 1] > seq_offsets[s])
             memcpy(&ss.last_delta[(size_t)s * 16], deltas ? deltas + (size_t)(seq_offsets[s + 1] - 1) * 16 : kIdentity,
                    16 * sizeof(double));
@@ -3082,30 +3043,31 @@ static void commit_push(dcreg_ctx::OdomSession& ss, const odom_plan::Push& u, in
     ss.cur = 1 - ss.cur;
 }
 
-// sess (dcreg_odometry_push): the frames continue the session's sequences, whose retained frames (odom_plan::History)
-// act as anchors outside the call: they are not registered and return nothing, their points come from the window
-// buffer and their poses from the session, and their last increments continue the deltas.  A sequence may have no
-// frame.  The frames are named by their number in the sequence since the session opened.  Only a push that succeeds
-// changes the session (commit_push); null: a one-shot call, which launches and copies exactly as without sessions.
-static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params* params, int n_seqs,
+// Every odometry entry point: the frames continue the sequences of a history (odom_plan::History), whose retained
+// frames act as anchors outside the call: they are not registered and return nothing, their points come from the
+// window buffer and their poses from the session, and their last increments continue the deltas.  A one-shot call
+// (sess null) runs on the empty history, where every sequence starts.  A push (sess) runs on the session's: a sequence
+// may have no frame, frames are named by their number in the sequence since the session opened, the retain step
+// gathers the next window, and only a push that succeeds changes the session (commit_push).
+static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& set, dcreg_ctx::OdomSession* sess,
                         const int* seq_offsets, int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
-                        double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
-                        int source_max_points, int map_max_points, const double* T_init, const double* deltas,
-                        int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
-                        int* status, double* cov, dcreg_iter_log* log, int log_cap, const float* timestamps,
-                        float* deskewed_xyz, dcreg_ctx::OdomSession* sess = nullptr) {
+                        const double* deltas, const float* timestamps, const Results& R, int64_t* frame_points,
+                        float* deskewed_xyz) {
     if (!ctx) return DCREG_BAD_ARG;
-    BatchCheck c{name, params && n_seqs > 0 && n_frames > 0 && seq_offsets && xyz && frame_offsets && T_init && T_out,
+    const int n_seqs = set.n_seqs;
+    BatchCheck c{name, !set.T_init.empty() && n_frames > 0 && seq_offsets && xyz && frame_offsets && R.T_out,
                  "null pointer, n_seqs <= 0 or n_frames <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_frames};
-    c.offsets = frame_offsets; c.item = "frame"; c.stride = stride; c.own_cell = true; c.cell_size = cell_size;
+    c.offsets = frame_offsets; c.item = "frame"; c.stride = stride; c.own_cell = true; c.cell_size = set.cell_size;
     c.need_target = false; c.one_iteration = true; c.n_seqs = n_seqs; c.seq_offsets = seq_offsets;
     c.empty_seqs = sess != nullptr;
-    c.own_msg = odometry_settings_error(map_frames, motion, deltas != nullptr, source_voxel, map_voxel, source_max_points,
-                                        map_max_points);
+    c.own_msg = odometry_settings_error(set, deltas != nullptr);
+    const dcreg_icp_params* params = &set.params;
     int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
+    const odom_plan::History none(sess ? 0 : n_seqs);
+    const odom_plan::History& hist = sess ? sess->hist : none;
     // "sequence s, frame k (frame j of the sequence)": the caller's frame k, j-th of sequence s in the call, or its
     // number since the session opened
     auto frame_name = [&](int s, int k) {
@@ -3114,7 +3076,7 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
             return "sequence " + std::to_string(s) + ", frame " + std::to_string(k) + " (frame " + std::to_string(j) +
                    " of the sequence)";
         return "sequence " + std::to_string(s) + ", frame " + std::to_string(k) + " of the push (frame " +
-               std::to_string(sess->hist.seen[(size_t)s] + j) + " of the sequence since open)";
+               std::to_string(hist.seen[(size_t)s] + j) + " of the sequence since open)";
     };
     if (timestamps)             // every point's fraction of its sweep, before anything is launched
         for (int s = 0; s < n_seqs; ++s)
@@ -3133,10 +3095,10 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
     int src_stride = stride;
     const int64_t* src_off = frame_offsets;
     std::vector<int64_t> kept;
-    if (source_voxel > 0.0) {
+    if (set.source_voxel > 0.0) {
         kept.resize((size_t)n_frames + 1);
         std::vector<int> bad((size_t)n_frames);
-        if ((rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, source_voxel, source_max_points,
+        if ((rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, set.source_voxel, set.source_max_points,
                                     timestamps != nullptr, false, kept.data(), bad.data())))
             return rc;
         for (int s = 0; s < n_seqs; ++s)
@@ -3156,14 +3118,12 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
     odom_plan::Push U;
     odom_plan::Plan& P = U.plan;
     {
-        const std::string why = sess ? odom_plan::make_push(n_seqs, seq_offsets, n_frames, src_off, map_frames,
-                                                            arena_plan::kMaxPoints, sess->hist, &U)
-                                     : odom_plan::make(n_seqs, seq_offsets, n_frames, src_off, map_frames,
-                                                       arena_plan::kMaxPoints, &P);
-        if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
+        const std::string why = odom_plan::make_push(n_seqs, seq_offsets, n_frames, src_off, set.map_frames,
+                                                     arena_plan::kMaxPoints, hist, &U);
+        if (!why.empty()) { ctx->err = std::string(name) + ": " + why; return DCREG_BAD_ARG; }
     }
     const int n_steps = (int)P.steps.size();
-    const int n_hist = sess ? (int)sess->hist.n.size() : 0;
+    const int n_hist = (int)hist.n.size();
     // every step's tables in one upload: long long map_seg [A + 1], piece_dst [P + 1], piece_src [P]; int piece_frame
     // [P], prev [A], prev2 [A] (A lanes, P window frames)
     std::vector<long long> hll;
@@ -3198,77 +3158,76 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
     // lane's frame range set by odom_start_kernel at every step; grids: the step's local maps
     Batch S{n_frames, src_xyz, src_stride, P.dev_off.data()};
     S.order = P.input.data(); S.in_off = src_off;
-    if (source_voxel > 0.0) S.kind = cudaMemcpyDeviceToDevice;
+    if (set.source_voxel > 0.0) S.kind = cudaMemcpyDeviceToDevice;
     S.sort = Batch::kBox;
-    S.sort_box.inv_cell = 1.0 / cell_size;
+    S.sort_box.inv_cell = 1.0 / set.cell_size;
     S.sort_box.ox = S.sort_box.oy = S.sort_box.oz = -512;
     S.sort_box.nx = S.sort_box.ny = S.sort_box.nz = 1024;
     S.sort_cells = 1ll << 30;
-    S.grid_table = true; S.cell_size = cell_size;
+    S.grid_table = true; S.cell_size = set.cell_size;
     S.lanes = n_seqs;
     if ((rc = stage_sources(ctx, S)) || (rc = stage_lanes(ctx, n_seqs, n_frames, &S.seq))) return rc;
     S.sort_T = ctx->d_seq_prior;
     CK(ctx->d_odom_ll.ensure(std::max<long long>((long long)hll.size(), 1)));
     CK(ctx->d_odom_int.ensure(std::max<long long>((long long)hint.size(), 1)));
     CK(ctx->d_odom_map.ensure(std::max<long long>(P.max_map, 1)));
-    if (map_voxel > 0.0) {        // the maps' filter at its largest step, so no buffer regrows inside the loop
+    if (set.map_voxel > 0.0) {    // the maps' filter at its largest step, so no buffer regrows inside the loop
         CK(ctx->d_odom_map_vox.ensure(std::max<long long>(P.max_map, 1)));
         long long slots = 0;
         std::vector<long long> tab;
         for (int i = 1; i < n_steps; ++i)
             slots = std::max(slots, voxel_tables(P.steps[(size_t)i].active, P.steps[(size_t)i].map_seg.data(), tab));
-        if ((rc = voxel_reserve(ctx, P.max_map, n_seqs, slots, map_max_points))) return rc;
+        if ((rc = voxel_reserve(ctx, P.max_map, n_seqs, slots, set.map_max_points))) return rc;
     }
     if (!hll.empty()) {
         CK(cudaMemcpyAsync(ctx->d_odom_ll, hll.data(), hll.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaMemcpyAsync(ctx->d_odom_int, hint.data(), hint.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     }
     // device order: every frame's loop state starts at its sequence's T_init (an anchor keeps it: T_out = T_prior =
-    // T_init, no iteration, not converged), the increments follow the frames
-    std::vector<double> T_dev((size_t)n_frames * 16), ident((size_t)n_frames * 16, 0.0), D_dev;
+    // T_init, no iteration, not converged)
+    std::vector<double> T_dev((size_t)n_frames * 16), ident((size_t)n_frames * 16, 0.0);
     for (int s = 0; s < n_seqs; ++s)
         for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k)
-            memcpy(&T_dev[(size_t)P.dev[(size_t)k] * 16], T_init + (size_t)s * 16, 16 * sizeof(double));
+            memcpy(&T_dev[(size_t)P.dev[(size_t)k] * 16], &set.T_init[(size_t)s * 16], 16 * sizeof(double));
     for (int d = 0; d < n_frames; ++d)
         for (int c4 = 0; c4 < 4; ++c4) ident[(size_t)d * 16 + 5 * c4] = 1.0;
-    if (deltas && !sess) {
-        D_dev.resize((size_t)n_frames * 16);
-        for (int k = 0; k < n_frames; ++k) memcpy(&D_dev[(size_t)P.dev[(size_t)k] * 16], deltas + (size_t)k * 16, 16 * sizeof(double));
-        CK(cudaMemcpyAsync(ctx->d_seq_delta, D_dev.data(), D_dev.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    // one increment per frame reference: the frames' (identity without deltas), then the retained frames' (a sequence's
+    // last one carries the increment its push left; only a session retains frames); null: every increment is the identity
+    const double* d_delta = nullptr;
+    if (set.motion == DCREG_MOTION_INCREMENTS && (deltas || n_hist > 0)) {
+        std::vector<double> D_dev((size_t)(n_frames + n_hist) * 16, 0.0);
+        for (int e = 0; e < n_frames + n_hist; ++e)
+            for (int c4 = 0; c4 < 4; ++c4) D_dev[(size_t)e * 16 + 5 * c4] = 1.0;
+        if (deltas)
+            for (int k = 0; k < n_frames; ++k)
+                memcpy(&D_dev[(size_t)P.dev[(size_t)k] * 16], deltas + (size_t)k * 16, 16 * sizeof(double));
+        for (int s = 0; s < n_seqs; ++s)
+            if (hist.off[(size_t)s + 1] > hist.off[(size_t)s])
+                memcpy(&D_dev[(size_t)(n_frames + hist.off[(size_t)s + 1] - 1) * 16], &sess->last_delta[(size_t)s * 16],
+                       16 * sizeof(double));
+        CK(ctx->d_seq_delta.ensure((long long)D_dev.size()));
+        CK(cudaMemcpyAsync(ctx->d_seq_delta, D_dev.data(), D_dev.size() * sizeof(double), cudaMemcpyHostToDevice,
+                           ctx->stream));
+        d_delta = ctx->d_seq_delta;
     }
-    // (sess) one increment per frame reference (the pushed frames, identity without deltas, then the retained frames: a
-    // sequence's last one carries the increment its push left), the retained poses, and room for the next window
-    const double* d_delta = deltas ? ctx->d_seq_delta.p : nullptr;
+    // the retained frames' poses and points (none on the empty history: nothing reads them), and (sess) room for the
+    // next window, grown with headroom: a window whose frames vary in size does not reallocate (and synchronise) at
+    // every push
+    const double* d_hist_T = nullptr;
+    const float4* d_win = nullptr;
+    if (n_hist) {
+        CK(sess->d_hist_T.ensure((long long)n_hist * 16));
+        CK(cudaMemcpyAsync(sess->d_hist_T, sess->hist_T.data(), (size_t)n_hist * 16 * sizeof(double),
+                           cudaMemcpyHostToDevice, ctx->stream));
+        d_hist_T = sess->d_hist_T;
+        d_win = sess->win[sess->cur];
+    }
     if (sess) {
-        d_delta = motion == DCREG_MOTION_INCREMENTS ? ctx->d_seq_delta.p : nullptr;
-        if (d_delta) {
-            D_dev.assign((size_t)(n_frames + n_hist) * 16, 0.0);
-            for (int e = 0; e < n_frames + n_hist; ++e)
-                for (int c4 = 0; c4 < 4; ++c4) D_dev[(size_t)e * 16 + 5 * c4] = 1.0;
-            if (deltas)
-                for (int k = 0; k < n_frames; ++k)
-                    memcpy(&D_dev[(size_t)P.dev[(size_t)k] * 16], deltas + (size_t)k * 16, 16 * sizeof(double));
-            const odom_plan::History& h = sess->hist;
-            for (int s = 0; s < n_seqs; ++s)
-                if (h.off[(size_t)s + 1] > h.off[(size_t)s])
-                    memcpy(&D_dev[(size_t)(n_frames + h.off[(size_t)s + 1] - 1) * 16], &sess->last_delta[(size_t)s * 16],
-                           16 * sizeof(double));
-            CK(ctx->d_seq_delta.ensure((long long)D_dev.size()));
-            CK(cudaMemcpyAsync(ctx->d_seq_delta, D_dev.data(), D_dev.size() * sizeof(double), cudaMemcpyHostToDevice,
-                               ctx->stream));
-            d_delta = ctx->d_seq_delta.p;       // (ensure may have moved it)
-        }
-        CK(sess->d_hist_T.ensure(std::max(n_hist, 1) * 16));
-        if (n_hist)
-            CK(cudaMemcpyAsync(sess->d_hist_T, sess->hist_T.data(), (size_t)n_hist * 16 * sizeof(double),
-                               cudaMemcpyHostToDevice, ctx->stream));
-        // grown with headroom: a window whose frames vary in size does not reallocate (and synchronise) at every push
         DevBuf<float4>& nxt = sess->win[1 - sess->cur];
         const long long need = std::max<long long>(U.keep_dst.back(), 1);
         if (nxt.cap < need) CK(nxt.ensure(need + need / 4));
     }
     CK(cudaMemcpyAsync(ctx->d_seq_prior, ident.data(), ident.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    const Results R{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior};
     dcreg_iter_log* dlog = nullptr;
     const float4* src_iter = nullptr;
     if ((rc = start_loop(ctx, n_frames, T_dev.data(), R, &S, &dlog, &src_iter))) return rc;
@@ -3283,15 +3242,15 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         const long long* d_in_at = ctx->d_odom_ll + ts_ll;
         odom_ts_gather_kernel<<<(unsigned)((n_points + 255) / 256), 256, 0, ctx->stream>>>(
             ctx->d_odom_ts_in, n_points, ctx->d_scan_seg, n_frames, d_in_at, d_in_at + n_frames,
-            source_voxel > 0.0 ? ctx->d_vox_index.p : nullptr, ctx->d_odom_ts);
+            set.source_voxel > 0.0 ? ctx->d_vox_index.p : nullptr, ctx->d_odom_ts);
         ctx->launches++;
         CK(cudaGetLastError());
     }
-    const int rings = search_rings(params->search_radius, cell_size);
+    const int rings = search_rings(params->search_radius, set.cell_size);
     LoopPlan L;
     bool planned = false;
     int failed = n_steps;                       // the step whose map had no dense grid
-    const double inv_cell = 1.0 / cell_size;
+    const double inv_cell = 1.0 / set.cell_size;
     for (int i = 1; i < n_steps; ++i) {
         const odom_plan::Step& st = P.steps[(size_t)i];
         const long long m = st.map_seg[(size_t)st.active];
@@ -3302,14 +3261,10 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         const int* d_frame = ctx->d_odom_int + at_int[(size_t)i];
         const int* d_prev = d_frame + pieces;
         const int* d_prev2 = d_prev + st.active;
-        // 1. the lanes' local maps from the window frames' device-resident results (sess: and from the retained frames)
-        if (sess)
-            map_points_hist_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(
-                ctx->d_scan_src, sess->win[sess->cur], n_frames, d_dst, pieces, d_src_at, d_frame, m, ctx->d_state,
-                sess->d_hist_T, ctx->d_odom_map);
-        else
-            map_points_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(ctx->d_scan_src, d_dst, pieces, d_src_at,
-                                                                                    d_frame, m, ctx->d_state, ctx->d_odom_map);
+        // 1. the lanes' local maps from the window frames' device-resident results and the retained frames
+        map_points_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(
+            ctx->d_scan_src, d_win, n_frames, d_dst, pieces, d_src_at, d_frame, m, ctx->d_state, d_hist_T,
+            ctx->d_odom_map);
         ctx->launches++;
         CK(cudaGetLastError());
         // 1b. (map_voxel) every lane's map through the voxel filter, in world coordinates, .w re-indexed over the step's
@@ -3320,9 +3275,9 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         std::vector<int64_t> kept_map;
         std::vector<int> bad_map;
         std::vector<Readback> more;
-        if (map_voxel > 0.0) {
+        if (set.map_voxel > 0.0) {
             if ((rc = voxel_filter(ctx, (const float*)ctx->d_odom_map.p, m, 4, d_map_seg, st.map_seg.data(), st.active,
-                                   map_voxel, (float*)ctx->d_odom_map_vox.p, 4, nullptr, map_max_points)))
+                                   set.map_voxel, (float*)ctx->d_odom_map_vox.p, 4, nullptr, set.map_max_points)))
                 return rc;
             map = ctx->d_odom_map_vox;
             d_mseg = ctx->d_vox_seg;
@@ -3340,7 +3295,7 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         long long cells = 0;
         int b = 0;
         std::string why;
-        if (map_voxel > 0.0) {
+        if (set.map_voxel > 0.0) {
             while (b < st.active && !bad_map[(size_t)b]) ++b;
             if (b < st.active) why = "its local map has a voxel coordinate of the map filter outside [-2^20, 2^20)";
             mk = kept_map[(size_t)st.active];
@@ -3359,21 +3314,16 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         if ((rc = arena_fill(ctx, ctx->odom_maps, map, d_mseg, st.active, mk, boxes.data(), cells, inv_cell, rings)))
             return rc;
         // 3. every lane's frame of this step: its prior and a fresh loop state
-        if (sess)
-            odom_start_hist_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
-                ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active,
-                n_seqs, st.first, st.active, d_prev, d_prev2, d_delta, motion, n_frames, sess->d_hist_T);
-        else
-            odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
-                ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
-                st.first, st.active, d_prev, d_prev2, d_delta, motion);
+        odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
+            ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
+            st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T);
         ctx->launches++;
         CK(cudaGetLastError());
         // 3b. (timestamps) the step's frames deskewed with the increments their priors used, outside the loop's graphs
         if (timestamps) {
             odom_twist_kernel<<<(unsigned)((st.active + 127) / 128), 128, 0, ctx->stream>>>(
-                ctx->d_state, st.first, st.active, d_prev, d_prev2, d_delta, motion, n_frames,
-                sess ? sess->d_hist_T.p : nullptr, ctx->d_odom_xi, ctx->d_scan_radius);
+                ctx->d_state, st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T,
+                ctx->d_odom_xi, ctx->d_scan_radius);
             const long long a = P.dev_off[(size_t)st.first], np = P.dev_off[(size_t)(st.first + st.active)] - a;
             odom_deskew_kernel<<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
                 ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_seg, st.first, st.active, a, np, ctx->d_odom_ts,
@@ -3385,10 +3335,10 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
         // has the most lanes, so the arena's table never regrows after it), only its entries change
         if (!planned) {
             S.grids = ctx->odom_maps.d_grids;
-            if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? log_cap : 0, true, &L, &S))) return rc;
+            if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? R.log_cap : 0, true, &L, &S))) return rc;
             planned = true;
         }
-        if ((rc = run_chunks(ctx, L, params, dlog, dlog ? log_cap : 0, params->max_iterations, 16, true))) return rc;
+        if ((rc = run_chunks(ctx, L, params, dlog, dlog ? R.log_cap : 0, params->max_iterations, 16, true))) return rc;
     }
     // (sess) the next window: the retained frames' packed points, gathered from this push's frames and the old window
     // into the other buffer, so the session's own window stays as it was until the push commits
@@ -3421,7 +3371,7 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const dcreg_icp_params
             }
         }
     }
-    if (sess) commit_push(*sess, U, n_frames, seq_offsets, T_out, deltas);
+    if (sess) commit_push(*sess, U, n_frames, seq_offsets, R.T_out, deltas);
     return DCREG_OK;
 }
 
@@ -3430,9 +3380,10 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
                            int map_frames, int motion, const double* T_init, const double* deltas, double* T_prior,
                            double* T_out, int* n_iterations, int* converged, int* status, double* cov,
                            dcreg_iter_log* log, int log_cap) {
-    return run_odometry(ctx, "icp_run_odometry", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
-                        cell_size, map_frames, motion, 0.0, 0.0, 1, 1, T_init, deltas, nullptr, T_prior, T_out,
-                        n_iterations, converged, status, cov, log, log_cap, nullptr, nullptr);
+    return run_odometry(ctx, "icp_run_odometry",
+                        odom_settings(params, n_seqs, cell_size, map_frames, motion, 0.0, 0.0, 1, 1, T_init), nullptr,
+                        seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, nullptr,
+                        Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, nullptr, nullptr);
 }
 
 int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
@@ -3441,9 +3392,10 @@ int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params,
                                  const double* T_init, const double* deltas, int64_t* frame_points, double* T_prior,
                                  double* T_out, int* n_iterations, int* converged, int* status, double* cov,
                                  dcreg_iter_log* log, int log_cap) {
-    return run_odometry(ctx, "icp_run_odometry_voxel", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
-                        cell_size, map_frames, motion, source_voxel, map_voxel, 1, 1, T_init, deltas, frame_points,
-                        T_prior, T_out, n_iterations, converged, status, cov, log, log_cap, nullptr, nullptr);
+    return run_odometry(ctx, "icp_run_odometry_voxel",
+                        odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel, 1, 1, T_init),
+                        nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, nullptr,
+                        Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points, nullptr);
 }
 
 int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
@@ -3453,10 +3405,11 @@ int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* param
                                    const double* deltas, int64_t* frame_points, double* T_prior, double* T_out,
                                    int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
                                    int log_cap) {
-    return run_odometry(ctx, "icp_run_odometry_voxel_n", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets,
-                        stride, cell_size, map_frames, motion, source_voxel, map_voxel, source_max_points,
-                        map_max_points, T_init, deltas, frame_points, T_prior, T_out, n_iterations, converged, status,
-                        cov, log, log_cap, nullptr, nullptr);
+    return run_odometry(ctx, "icp_run_odometry_voxel_n",
+                        odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
+                                      source_max_points, map_max_points, T_init),
+                        nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, nullptr,
+                        Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points, nullptr);
 }
 
 int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
@@ -3466,10 +3419,12 @@ int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params
                                   const float* timestamps, int64_t* frame_points, double* T_prior, double* T_out,
                                   int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
                                   dcreg_iter_log* log, int log_cap) {
-    return run_odometry(ctx, "icp_run_odometry_deskew", params, n_seqs, seq_offsets, n_frames, xyz, frame_offsets,
-                        stride, cell_size, map_frames, motion, source_voxel, map_voxel, source_max_points,
-                        map_max_points, T_init, deltas, frame_points, T_prior, T_out, n_iterations, converged, status,
-                        cov, log, log_cap, timestamps, deskewed_xyz);
+    return run_odometry(ctx, "icp_run_odometry_deskew",
+                        odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
+                                      source_max_points, map_max_points, T_init),
+                        nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
+                        Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
+                        deskewed_xyz);
 }
 
 int dcreg_odometry_open(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
@@ -3477,21 +3432,16 @@ int dcreg_odometry_open(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_se
                         const double* T_init) {
     if (!ctx) return DCREG_BAD_ARG;
     if (ctx->odom) { ctx->err = "odometry_open: a session is open already (dcreg_odometry_close it first)"; return DCREG_BAD_ARG; }
-    BatchCheck c{"odometry_open", params && n_seqs > 0 && T_init, "null pointer or n_seqs <= 0",
+    std::unique_ptr<dcreg_ctx::OdomSession> ss(new dcreg_ctx::OdomSession());
+    ss->set = odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel, source_max_points,
+                            map_max_points, T_init);
+    BatchCheck c{"odometry_open", !ss->set.T_init.empty(), "null pointer or n_seqs <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_seqs};
     c.own_cell = true; c.cell_size = cell_size; c.need_target = false; c.one_iteration = true;
-    c.own_msg = odometry_settings_error(map_frames, motion, false, source_voxel, map_voxel, source_max_points,
-                                        map_max_points);
-    const int rc = check_batch_call(ctx, params, c);
+    c.own_msg = odometry_settings_error(ss->set, false);
+    const int rc = check_batch_call(ctx, &ss->set.params, c);
     if (rc) return rc;
-    std::unique_ptr<dcreg_ctx::OdomSession> ss(new dcreg_ctx::OdomSession());
-    ss->params = *params;
-    ss->n_seqs = n_seqs; ss->map_frames = map_frames; ss->motion = motion;
-    ss->source_max_points = source_max_points; ss->map_max_points = map_max_points;
-    ss->cell_size = cell_size; ss->source_voxel = source_voxel; ss->map_voxel = map_voxel;
-    ss->T_init.assign(T_init, T_init + (size_t)n_seqs * 16);
-    ss->hist.seen.assign((size_t)n_seqs, 0);
-    ss->hist.off.assign((size_t)n_seqs + 1, 0);
+    ss->hist = odom_plan::History(n_seqs);
     ss->last_delta.assign((size_t)n_seqs * 16, 0.0);
     for (int s = 0; s < n_seqs; ++s)
         for (int c4 = 0; c4 < 4; ++c4) ss->last_delta[(size_t)s * 16 + 5 * c4] = 1.0;
@@ -3506,10 +3456,9 @@ int dcreg_odometry_push(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, co
     if (!ctx) return DCREG_BAD_ARG;
     if (!ctx->odom) { ctx->err = "odometry_push: no session is open (dcreg_odometry_open)"; return DCREG_BAD_ARG; }
     dcreg_ctx::OdomSession& ss = *ctx->odom;
-    return run_odometry(ctx, "odometry_push", &ss.params, ss.n_seqs, seq_offsets, n_frames, xyz, frame_offsets, stride,
-                        ss.cell_size, ss.map_frames, ss.motion, ss.source_voxel, ss.map_voxel, ss.source_max_points,
-                        ss.map_max_points, ss.T_init.data(), deltas, frame_points, T_prior, T_out, n_iterations,
-                        converged, status, cov, log, log_cap, nullptr, nullptr, &ss);
+    return run_odometry(ctx, "odometry_push", ss.set, &ss, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas,
+                        nullptr, Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior},
+                        frame_points, nullptr);
 }
 
 int dcreg_odometry_push_deskew(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
@@ -3519,10 +3468,9 @@ int dcreg_odometry_push_deskew(dcreg_ctx* ctx, const int* seq_offsets, int n_fra
     if (!ctx) return DCREG_BAD_ARG;
     if (!ctx->odom) { ctx->err = "odometry_push_deskew: no session is open (dcreg_odometry_open)"; return DCREG_BAD_ARG; }
     dcreg_ctx::OdomSession& ss = *ctx->odom;
-    return run_odometry(ctx, "odometry_push_deskew", &ss.params, ss.n_seqs, seq_offsets, n_frames, xyz, frame_offsets,
-                        stride, ss.cell_size, ss.map_frames, ss.motion, ss.source_voxel, ss.map_voxel,
-                        ss.source_max_points, ss.map_max_points, ss.T_init.data(), deltas, frame_points, T_prior, T_out,
-                        n_iterations, converged, status, cov, log, log_cap, timestamps, deskewed_xyz, &ss);
+    return run_odometry(ctx, "odometry_push_deskew", ss.set, &ss, seq_offsets, n_frames, xyz, frame_offsets, stride,
+                        deltas, timestamps, Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior},
+                        frame_points, deskewed_xyz);
 }
 
 // The session's buffers go with it; nothing queued may still read them

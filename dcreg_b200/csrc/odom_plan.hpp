@@ -1,12 +1,13 @@
-// odom_plan.hpp - host-side planning of scan-to-map odometry (dcreg_icp_run_odometry): which frames run side by side,
-// where every frame lives on the device, and which points make each frame's local map.
+// odom_plan.hpp - host-side planning of scan-to-map odometry (dcreg_icp_run_odometry, dcreg_odometry_push): which
+// frames run side by side, where every frame lives on the device, and which points make each frame's local map.
 //
-// Step i registers frame i of every sequence that has more than i frames (step 0: the anchors, which are not
-// registered).  On the device the frames are numbered step by step: the frames of step i are [Step::first, Step::first +
-// Step::active), one per lane, the lanes in ascending sequence order.  So a step's frames are one contiguous lane table,
-// and the loop's frame cursor stops at the end of a lane's only frame.  The map of lane j is the window frames
-// [max(first of the sequence, k - map_frames), k) of its sequence in ascending order, each frame's points in their input
-// order; the lanes' maps follow each other in one buffer.  make_push plans a push to an odometry session the same way.
+// One plan serves both: a one-shot call is a push onto the empty history (History(n_seqs): no sequence has a frame yet).
+// Step i registers the i-th registrable frame of every sequence that has one (step 0: the anchors, the first frames of
+// sequences that start in the push, which are not registered).  On the device the frames are numbered step by step: the
+// frames of step i are [Step::first, Step::first + Step::active), one per lane, the lanes in ascending sequence order.
+// So a step's frames are one contiguous lane table, and the loop's frame cursor stops at the end of a lane's only frame.
+// The map of frame k (since its sequence started) is the window frames [max(0, k - map_frames), k) of its sequence in
+// ascending order, each frame's points in their input order; the lanes' maps follow each other in one buffer.
 // Everything here is plain C++ so tests/test_odom_plan.py and tests/test_odom_session_plan.py can check it on the CPU
 // (tools/test_odom_plan.cpp, tools/test_odom_session_plan.cpp).
 #pragma once
@@ -37,80 +38,22 @@ struct Plan {
     int max_pieces = 0;                 // the most window frames of one step
 };
 
-// seq_off: n_seqs + 1 frame offsets, frame_off: n_frames + 1 point offsets, both already validated (ascending strictly
-// from 0).  Fails (returns the reason) when the maps of one step hold more than max_points points.
-inline std::string make(int n_seqs, const int* seq_off, int n_frames, const int64_t* frame_off, int map_frames,
-                        long long max_points, Plan* out) {
-    Plan& p = *out;
-    p = Plan{};
-    int n_steps = 0;
-    for (int s = 0; s < n_seqs; ++s) n_steps = std::max(n_steps, seq_off[s + 1] - seq_off[s]);
-    p.dev.assign((size_t)n_frames, -1);
-    p.input.assign((size_t)n_frames, -1);
-    p.steps.resize((size_t)n_steps);
-    int d = 0;
-    for (int i = 0; i < n_steps; ++i) {
-        Step& st = p.steps[(size_t)i];
-        st.first = d;
-        for (int s = 0; s < n_seqs; ++s)
-            if (seq_off[s + 1] - seq_off[s] > i) {
-                const int k = seq_off[s] + i;
-                p.dev[(size_t)k] = d;
-                p.input[(size_t)d] = k;
-                st.seq.push_back(s);
-                ++d;
-            }
-        st.active = (int)st.seq.size();
-    }
-    p.dev_off.assign((size_t)n_frames + 1, 0);
-    for (int e = 0; e < n_frames; ++e) {
-        const int k = p.input[(size_t)e];
-        p.dev_off[(size_t)e + 1] = p.dev_off[(size_t)e] + (frame_off[k + 1] - frame_off[k]);
-    }
-    for (int i = 1; i < n_steps; ++i) {
-        Step& st = p.steps[(size_t)i];
-        st.map_seg.push_back(0);
-        st.piece_dst.push_back(0);
-        long long m = 0;
-        for (int j = 0; j < st.active; ++j) {
-            const int s = st.seq[(size_t)j], f0 = seq_off[s], k = f0 + i;
-            st.prev.push_back(p.dev[(size_t)k - 1]);
-            st.prev2.push_back(k - 1 > f0 ? p.dev[(size_t)k - 2] : -1);
-            for (int w = std::max(f0, k - map_frames); w < k; ++w) {
-                const int dw = p.dev[(size_t)w];
-                st.piece_src.push_back(p.dev_off[(size_t)dw]);
-                st.piece_frame.push_back(dw);
-                m += frame_off[w + 1] - frame_off[w];
-                st.piece_dst.push_back(m);
-            }
-            st.map_seg.push_back(m);
-        }
-        if (m > max_points)
-            return "icp_run_odometry: the maps of step " + std::to_string(i) + " hold " + std::to_string(m) +
-                   " points, more than " + std::to_string(max_points) + " (int32 indexing)";
-        p.max_map = std::max(p.max_map, m);
-        p.max_pieces = std::max(p.max_pieces, (int)st.piece_frame.size());
-    }
-    return std::string();
-}
-
-// ---- a push to an odometry session (dcreg_odometry_push) -----------------------------------------------------------
-// A session carries, per sequence, the frames pushed so far and the last of them: the window frames the next frames'
-// maps need, with their points, and the frames the constant-velocity model needs, by pose alone.  Sequence s retains
-// its last min(seen, max(map_frames, 2)) frames; the last min(seen, map_frames) of them carry points (map_frames = 1
-// keeps the frame before the last as a pose alone).
+// What a session carries, per sequence, from one push to the next: the frames pushed so far and the last of them: the
+// window frames the next frames' maps need, with their points, and the frames the constant-velocity model needs, by
+// pose alone.  Sequence s retains its last min(seen, max(map_frames, 2)) frames; the last min(seen, map_frames) of them
+// carry points (map_frames = 1 keeps the frame before the last as a pose alone).
 struct History {
     std::vector<long long> seen;        // [n_seqs] frames of the sequence since the session opened
     std::vector<int> off;               // [n_seqs + 1] retained frames of sequence s: [off[s], off[s + 1]), oldest first
     std::vector<long long> at, n;       // [retained] first point in the window buffer, and points (0: a pose alone)
+    History() = default;
+    explicit History(int n_seqs) : seen((size_t)n_seqs, 0), off((size_t)n_seqs + 1, 0) {}   // no frame yet
 };
 
-// A push numbers its frames like make(), with the retained frames acting as anchors that are not in the push: fixed
-// poses, not registered, no outputs.  Step 0 holds the anchors of the sequences that start in this push (their first
-// frame ever); step i >= 1 registers the i-th registrable pushed frame of every sequence that has one, lanes in
-// ascending sequence order.  A frame reference r (Step::prev, prev2, piece_frame, and keep_ref below) is the device
-// index of a pushed frame when r < n_frames, else retained frame r - n_frames of the history; piece_src is then a point
-// of the push's packed frames or of the window buffer.
+// The retained frames act as anchors that are not in the push: fixed poses, not registered, no outputs.  A frame
+// reference r (Step::prev, prev2, piece_frame, and keep_ref below) is the device index of a pushed frame when
+// r < n_frames, else retained frame r - n_frames of the history; piece_src is then a point of the push's packed frames
+// or of the window buffer.  On the empty history every reference is a pushed frame.
 struct Push {
     Plan plan;
     History next;                       // the history after the push, its window packed sequence by sequence
@@ -188,7 +131,7 @@ inline std::string make_push(int n_seqs, const int* seq_off, int n_frames, const
             st.map_seg.push_back(m);
         }
         if (m > max_points)
-            return "odometry_push: the maps of step " + std::to_string(i) + " hold " + std::to_string(m) +
+            return "the maps of step " + std::to_string(i) + " hold " + std::to_string(m) +
                    " points, more than " + std::to_string(max_points) + " (int32 indexing)";
         p.max_map = std::max(p.max_map, m);
         p.max_pieces = std::max(p.max_pieces, (int)st.piece_frame.size());

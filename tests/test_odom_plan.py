@@ -10,8 +10,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def test_odom_plan(tmp_path):
-    """odom_plan::make: frames numbered step by step with the lanes in sequence order, every window frame of every lane's
-    map in ascending order with its points contiguous, map offsets, previous-frame indices, and the point limit."""
+    """odom_plan::make_push onto the empty history (a one-shot call): frames numbered step by step with the lanes in
+    sequence order, every window frame of every lane's map in ascending order with its points contiguous, map offsets,
+    previous-frame indices, and the point limit."""
     gxx = shutil.which("g++")
     if not gxx:
         pytest.skip("g++ not available")

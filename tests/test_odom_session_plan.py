@@ -1,5 +1,5 @@
-"""Host side of the odometry session (dcreg_odometry_push): odom_plan::make_push against odom_plan::make over the whole
-recording, for random recordings pushed in random chunks, compiled as plain host C++."""
+"""Host side of the odometry session (dcreg_odometry_push): odom_plan::make_push against one push of the whole
+recording onto the empty history, for random recordings pushed in random chunks, compiled as plain host C++."""
 import os
 import shutil
 import subprocess

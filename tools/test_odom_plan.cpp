@@ -1,5 +1,6 @@
 // Host test of odom_plan.hpp (tests/test_odom_plan.py compiles and runs it): device numbering, lanes, windows, map
-// offsets and the per-step point limit of dcreg_icp_run_odometry, against a direct reading of the window rule.
+// offsets and the per-step point limit of dcreg_icp_run_odometry, a push onto the empty history, against a direct
+// reading of the window rule.
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -12,6 +13,15 @@ static int fails = 0;
         if (!(c)) { std::printf("FAIL %s:%d %s\n", __FILE__, __LINE__, #c); ++fails; } \
     } while (0)
 
+// The plan of a one-shot call: one push of the whole recording onto the empty history
+static std::string plan(int S, const int* so, int n, const int64_t* fo, int map_frames, long long max_points,
+                        odom_plan::Plan* p) {
+    odom_plan::Push u;
+    const std::string why = odom_plan::make_push(S, so, n, fo, map_frames, max_points, odom_plan::History(S), &u);
+    *p = u.plan;
+    return why;
+}
+
 static void check_case(const std::vector<int>& lens, int map_frames, unsigned seed) {
     const int S = (int)lens.size();
     std::vector<int> so(1, 0);
@@ -21,7 +31,7 @@ static void check_case(const std::vector<int>& lens, int map_frames, unsigned se
     srand(seed);
     for (int k = 0; k < n; ++k) fo.push_back(fo.back() + 1 + rand() % 50);
     odom_plan::Plan p;
-    CHECK(odom_plan::make(S, so.data(), n, fo.data(), map_frames, 1ll << 40, &p).empty());
+    CHECK(plan(S, so.data(), n, fo.data(), map_frames, 1ll << 40, &p).empty());
     int longest = 0;
     for (int l : lens) longest = l > longest ? l : longest;
     CHECK((int)p.steps.size() == longest);
@@ -73,8 +83,8 @@ static void check_case(const std::vector<int>& lens, int map_frames, unsigned se
     // the point limit: exactly the largest step's map points pass, one less fails naming a step
     if (longest > 1) {
         odom_plan::Plan p2;
-        CHECK(odom_plan::make(S, so.data(), n, fo.data(), map_frames, max_map, &p2).empty());
-        const std::string why = odom_plan::make(S, so.data(), n, fo.data(), map_frames, max_map - 1, &p2);
+        CHECK(plan(S, so.data(), n, fo.data(), map_frames, max_map, &p2).empty());
+        const std::string why = plan(S, so.data(), n, fo.data(), map_frames, max_map - 1, &p2);
         CHECK(!why.empty() && why.find("step") != std::string::npos);
     }
 }
@@ -92,7 +102,7 @@ int main() {
         std::vector<int64_t> fo;
         for (int k = 0; k <= 8; ++k) fo.push_back(10 * k);
         odom_plan::Plan p;
-        CHECK(odom_plan::make(1, so, 8, fo.data(), 3, 1000, &p).empty());
+        CHECK(plan(1, so, 8, fo.data(), 3, 1000, &p).empty());
         const odom_plan::Step& st = p.steps[7];
         CHECK(st.piece_frame.size() == 3 && st.piece_frame[0] == 4 && st.piece_frame[2] == 6);
         CHECK(st.map_seg[1] == 30 && p.max_map == 30);

@@ -1,9 +1,9 @@
 // Host test of odom_plan::make_push (tests/test_odom_session_plan.py compiles and runs it): random recordings pushed to
-// a session in random chunks, against odom_plan::make over the whole recording.  Every frame is named by (sequence,
-// frame of the sequence) and every point by its global index in the recording, so a push's window pieces, previous
-// frames and retained window can be compared with the one-call plan whatever the chunking.  The device buffers are
-// simulated as arrays of point ids: the push's packed frames in device order, and the window buffer the retain step
-// gathers.
+// a session in random chunks, against one push of the whole recording onto the empty history (the one-call plan, which
+// tools/test_odom_plan.cpp checks against the window rule).  Every frame is named by (sequence, frame of the sequence)
+// and every point by its global index in the recording, so a push's window pieces, previous frames and retained window
+// can be compared with the one-call plan whatever the chunking.  The device buffers are simulated as arrays of point
+// ids: the push's packed frames in device order, and the window buffer the retain step gathers.
 #include <cstdio>
 #include <cstdlib>
 #include <utility>
@@ -33,8 +33,9 @@ static void check_case(const std::vector<int>& lens, int map_frames, unsigned se
     const int n = so.back();
     std::vector<int64_t> fo(1, 0);
     for (int k = 0; k < n; ++k) fo.push_back(fo.back() + 1 + rnd(state) % 40);
-    odom_plan::Plan full;
-    CHECK(odom_plan::make(S, so.data(), n, fo.data(), map_frames, 1ll << 40, &full).empty());
+    odom_plan::Push one;
+    CHECK(odom_plan::make_push(S, so.data(), n, fo.data(), map_frames, 1ll << 40, odom_plan::History(S), &one).empty());
+    const odom_plan::Plan& full = one.plan;
     auto full_name = [&](int d) {
         const int k = full.input[(size_t)d];
         int s = 0;
@@ -43,9 +44,7 @@ static void check_case(const std::vector<int>& lens, int map_frames, unsigned se
     };
     auto global = [&](int s, long long w) { return so[s] + (int)w; };
     // the session
-    odom_plan::History h;
-    h.seen.assign((size_t)S, 0);
-    h.off.assign((size_t)S + 1, 0);
+    odom_plan::History h(S);
     std::vector<Name> h_name;                // the retained frames' names
     std::vector<long long> window;           // the window buffer: point ids
     std::vector<long long> done((size_t)S, 0);
