@@ -262,18 +262,16 @@ struct Iter2Args {
     unsigned int* n_active;   // trials still running (decremented by the step that finishes one); host polls it
     peer::View peer;          // multi-GPU: the sum over ranks, inside the last block (peer_reduce.cuh)
     unsigned long long* stamps;   // profiling only (dcreg_iteration_timeline): [grid.x][kStampSlots] globaltimer values, or null
-    int coop_max;             // more searching slots than this in a tile: every thread searches for itself (kSearchListMax)
     int force;                // 0: mode and seeds from the loop state (written by K2); 1: coherent mode, seeds = use_seeds
     int use_seeds;            // (force) records of the previous launch are valid
     float r2_up;              // search radius^2 rounded up to float
-    float look;               // squared-distance look-ahead beyond the seed bound (kNnLook)
     unsigned int* stats;      // optional [2]: slots that searched, slots that refitted (profiling)
     int tile;                 // source slots per block and pass (<= kBlock; plan_iteration: chosen so the blocks fill whole SM rounds)
     // single-trial folded run with a solver block (row_flags != null): block 0 sums the rows and solves (solver_block),
     // blocks 1.. work on the tiles; no ticket
     unsigned long long* row_flags;   // [grid.x - 1] row b is published with the value row_epoch + 1 of its launch
     unsigned long long* row_epoch;   // per-context launch counter (device memory: graph-captured arguments are frozen)
-    IcpState* warm_state;            // scratch state of the solver block's warm-up step, or null (DCREG_NO_SOLVER_WARMUP)
+    IcpState* warm_state;            // scratch state of the solver block's warm-up step
     // a batch of different scans (dcreg_icp_run_scans): trial b owns the source slots [seg[b], seg[b+1]) of it.src and the
     // record slices at the same offsets (sized by the total slot count), and its own lever arm src_radius[b].
     // null: every trial runs the it.n slots of it.src, with record slices [b][it.n] and the one src_radius
@@ -306,7 +304,7 @@ __device__ __noinline__ void solver_block(const Iter2Args& a, IcpState* st, Iter
     const IterArgs& A = a.it;
     const int tid = threadIdx.x, warp = tid >> 5;
     k2::WarpSmem* wsm = reinterpret_cast<k2::WarpSmem*>(sm.tbuf[0]);
-    if (a.warm_state && warp == 0) {
+    if (warp == 0) {
         for (int e = tid; e < (int)(sizeof(IcpState) / sizeof(int)); e += 32)
             reinterpret_cast<int*>(a.warm_state)[e] = reinterpret_cast<const int*>(st)[e];
         __syncwarp();
@@ -434,7 +432,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                         DCREG_CS(0, 1); DCREG_CS(2, 5); DCREG_CS(3, 4); DCREG_CS(1, 2); DCREG_CS(4, 6); DCREG_CS(2, 3);
                         DCREG_CS(4, 5); DCREG_CS(1, 2); DCREG_CS(3, 4); DCREG_CS(5, 6);
 #undef DCREG_CS
-                        B = fminf(B, corr::knn_d2(nn, 6) * a.look);
+                        B = fminf(B, corr::knn_d2(nn, 6) * kNnLook);
                         const float ex = qx - __int_as_float(s2.x), ey = qy - __int_as_float(s2.y), ez = qz - __int_as_float(s2.z);
                         const float delta = sqrtf(ex * ex + ey * ey + ez * ez);
                         const float lb = __int_as_float(s1.w);
@@ -462,11 +460,11 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
             // -- 2. searches: few -> one warp per listed slot (the other slots' threads are not held up by a
             //       long sequential search); many -> every thread searches for its own slot
             const int nS = sm.nS;
-            if (coherent && nS <= a.coop_max) {
+            if (coherent && nS <= kSearchListMax) {
                 corr::WarpKnnSmem& W = *reinterpret_cast<corr::WarpKnnSmem*>(sm.tbuf[warp]);
                 // cell = radius: the 9 cell rows of EVERY listed search are set up by all threads first (one memory round
                 // trip for the tile instead of one at the head of each of a warp's searches)
-                const bool pre_rows = g.rings == 1 && nS <= kSearchListMax;
+                const bool pre_rows = g.rings == 1;
                 if (pre_rows) {
                     for (int e = tid; e < nS * 9; e += kBlock) {
                         const int sidx = e / 9, r = e - sidx * 9;
@@ -1407,14 +1405,12 @@ int ensure_trials(dcreg_ctx* ctx, int trials) {
 // launch with the programmatic-stream-serialization attribute (see pdl_wait)
 template <typename... KArgs, typename... Args>
 static cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args... args) {
-    static int use = -1;
-    if (use < 0) use = getenv("DCREG_NO_PDL") ? 0 : 1;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = use ? 1 : 0;
+    cfg.attrs = attr; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
@@ -1490,7 +1486,6 @@ int launch_reduce(dcreg_ctx* ctx, const float4* d_src, const void* d_plane, bool
     a.slope = slope; a.gate = gate;
     a.npt_override = npt_override;
     if (ctx->peer_ok) a.peer = ctx->peer_view;                          // the sum over ranks happens inside the kernel
-    { static int dbg = -1; if (dbg < 0) { const char* e = getenv("DCREG_K1_DEBUG"); dbg = e ? atoi(e) : 0; } a.debug = dbg; }
     a.counter = ctx->d_counter; a.acc = ctx->d_acc;
     if (use_wd) return f64 ? launch_reduce_t<double4, true>(ctx, a) : launch_reduce_t<float4, true>(ctx, a);
     return f64 ? launch_reduce_t<double4, false>(ctx, a) : launch_reduce_t<float4, false>(ctx, a);
@@ -1595,10 +1590,8 @@ int dcreg_create(int device_id, dcreg_ctx** out) {
     CK(ctx->d_n_active.ensure(1));
     CK(cudaMemsetAsync(ctx->d_n_active, 0, sizeof(unsigned int), ctx->stream));
     CK(ctx->d_small.ensure(1024));
-    if (!getenv("DCREG_NO_K2_REHEARSAL")) {
-        CK(ctx->d_k2_scratch.ensure(1));
-        CK(cudaMemsetAsync(ctx->d_k2_scratch, 0, sizeof(K2Scratch), ctx->stream));
-    }
+    CK(ctx->d_k2_scratch.ensure(1));
+    CK(cudaMemsetAsync(ctx->d_k2_scratch, 0, sizeof(K2Scratch), ctx->stream));
     CK(ctx->d_analysis.ensure(1));
     CK(cudaStreamSynchronize(ctx->stream));
     return DCREG_OK;
@@ -2173,12 +2166,6 @@ static int search_rings(double search_radius, double cell_size) {
     return (int)ceil(search_radius / cell_size - 1e-9);
 }
 
-static double coherent_step_setting() {
-    static double v = -1.0;
-    if (v < 0.0) { const char* e = getenv("DCREG_COHERENT_STEP"); v = e ? atof(e) : kCoherentStep; }
-    return v;
-}
-
 // What one loop body looks like for this context: the loop kernel's arguments and grid, and whether the solve step is
 // inside it.
 struct LoopPlan {
@@ -2243,16 +2230,14 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         b.nn = ctx->d_nn; b.plane_cache = ctx->d_plane_cache; b.fit_state = ctx->d_fit_state; b.plane_key = ctx->d_plane_key;
     }
     // the solve step inside the kernel unless the sum over ranks has to go through NCCL
-    L.fold_k2 = want_fold && !(ctx->comm && !ctx->peer_ok) && !getenv("DCREG_NO_FOLD") &&
+    L.fold_k2 = want_fold && !(ctx->comm && !ctx->peer_ok) &&
                 prm->detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm->handling == DCREG_HAND_PRECONDITIONED_CG;
     // a single folded run: block 0 is a dedicated solver block (solver_block); batches keep the ticket, since a
     // solver block per trial in a multi-wave grid could fill every resident slot with waiting blocks
     const bool solver = L.fold_k2 && trials == 1 && !batch && !getenv("DCREG_NO_SOLVER_BLOCK");
     // blocks per trial and slots per block: loop_plan.hpp
-    const char* tile_env = trials == 1 && !batch ? getenv("DCREG_TILE") : nullptr;  // measurement switch
     const loop_plan::Tiles tp = batch ? loop_plan::plan_scan_tiles(batch->max_n(), kBlock)
-                                      : loop_plan::plan_tiles(slots, trials, ctx->sm_count, kBlock, tile_env ? atoi(tile_env) : 0,
-                                                              solver ? 1 : 0);
+                                      : loop_plan::plan_tiles(slots, trials, ctx->sm_count, kBlock, solver ? 1 : 0);
     L.grid_x = (int)tp.grid_x + (solver ? 1 : 0);
     b.tile = tp.tile;
     CK(ctx->d_partials.ensure((long long)L.grid_x * trials * kPartialDoubles));
@@ -2261,12 +2246,10 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
     a.partials = ctx->d_partials;
     if (solver) {
         b.row_flags = ctx->d_row_flags; b.row_epoch = ctx->d_row_epoch;
-        b.warm_state = getenv("DCREG_NO_SOLVER_WARMUP") ? nullptr : ctx->d_warm_state.p;   // measurement switch
+        b.warm_state = ctx->d_warm_state;
     }
     b.force = ctx->force_coherent && !lean_only ? 1 : 0;
-    { static int cm = -1; if (cm < 0) { const char* e = getenv("DCREG_COOP_MAX"); cm = e ? atoi(e) : kSearchListMax; } b.coop_max = cm; }
     b.use_seeds = ctx->nn_valid ? 1 : 0;
-    { static float lk = -1.f; if (lk < 0.f) { const char* e = getenv("DCREG_LOOK"); lk = e ? (float)atof(e) : kNnLook; } b.look = lk; }
     b.stats = ctx->d_iter_stats;
     const double r2 = prm->search_radius * prm->search_radius;
     float r2f = (float)r2;
@@ -2275,7 +2258,7 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
     b.fold_k2 = L.fold_k2 ? 1 : 0;
     b.log = dlog; b.log_cap = log_cap;
     b.src_radius = batch ? ctx->d_scan_radius.p : ctx->d_src_radius.p;
-    b.coherent_step = lean_only ? 0.0 : coherent_step_setting();
+    b.coherent_step = lean_only ? 0.0 : kCoherentStep;
     b.seg = batch ? ctx->d_scan_seg.p : nullptr;
     // (a CUDA graph of the loop freezes this pointer, not the table: the entries are rewritten before every pairs call
     // and read at every launch, and a regrown table has a new pointer and so a new graph key)
@@ -2631,9 +2614,7 @@ static void key_bytes(std::vector<unsigned char>& k, const void* p, size_t n) {
 // device), so a chunk is captured once into a CUDA graph and replayed: one host call per chunk instead of one or two
 // launches per iteration - what keeps independent ranks from queueing behind the host.  Falls back to plain launches if capture is unavailable.
 static int enqueue_iterations(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_params* prm, dcreg_iter_log* dlog, int log_cap, int iters) {
-    static int use_graph = -1;
-    if (use_graph < 0) use_graph = getenv("DCREG_NO_GRAPH") ? 0 : 1;
-    const bool graphable = use_graph && !ctx->graph_off && !L.b.force && iters > 1 &&
+    const bool graphable = !ctx->graph_off && !L.b.force && iters > 1 &&
                            (L.fold_k2 || !(ctx->comm && !ctx->peer_ok));          // no NCCL call inside a capture
     if (graphable) {
         std::vector<unsigned char> key;
@@ -3592,7 +3573,7 @@ int dcreg_icp_run_host_planes(dcreg_ctx* ctx, const dcreg_icp_params* params, co
                                 params->weight_slope, params->weight_gate, npt >= 0 ? (double)npt : -1.0)))
             return rc;
         if ((rc = nccl_allreduce_acc(ctx))) return rc;
-        if ((rc = launch_k2(ctx, params, dlog, log_cap, coherent_step_setting()))) return rc;
+        if ((rc = launch_k2(ctx, params, dlog, log_cap, kCoherentStep))) return rc;
         CK(cudaMemcpyAsync(hs, ctx->d_state, sizeof(IcpState), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
         for (int r = 0; r < 3; ++r) {

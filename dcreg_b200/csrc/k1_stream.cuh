@@ -50,7 +50,6 @@ struct Args {
     double npt_override;         // >= 0: N_corr_pt of this rank as counted by the caller's correspondence stage (host-kd-tree
                                  // mode: the reference counts BEFORE the plane gates, icp_test_runner.cpp:1726-1731, 1856)
     peer::View peer;             // multi-GPU: sum over ranks inside the last block (nranks <= 1: none)
-    int debug;                   // profiling only (tools/sweep_k1.py): 4 = exit at once, 3 = after the stream loop, 2 = before the grid reduction
 };
 
 // 16-byte asynchronous global -> shared copy (LDGSTS), L1 bypassed: the data is streamed exactly once
@@ -342,7 +341,6 @@ __global__ void __launch_bounds__(kThreads, 2) reduce_stream_kernel(const __grid
     Smem<PlaneT>& sm = *reinterpret_cast<Smem<PlaneT>*>(smem_raw);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const PlaneT* gplane = reinterpret_cast<const PlaneT*>(a.plane);
-    if (a.debug == 4) return;
     const unsigned int epoch0 = peer::load_epoch(a.peer);
 
     double vh[21], vg[6], vr2 = 0.0, vb2 = 0.0;          // the 29 running sums of this lane's slots
@@ -452,7 +450,6 @@ __global__ void __launch_bounds__(kThreads, 2) reduce_stream_kernel(const __grid
     }
     cp_async_wait<0>();
     int neff = (int)(counts >> 16), npt = (int)(counts & 0xffffu);
-    if (a.debug == 3) { if (vh[0] + vg[0] + vr2 + vb2 == 1.2345 && neff == 77) a.acc[0] = vh[1]; return; }
 
     // ---- reduction tail -------------------------------------------------------------------------------------
     // warp: 5-round transpose-reduction of the 32 per-lane values (29 sums, N_eff, N_pt, pad): every round halves
@@ -478,7 +475,6 @@ __global__ void __launch_bounds__(kThreads, 2) reduce_stream_kernel(const __grid
             v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
         }
     }
-    if (a.debug == 2) { if (v[0] == 1.2345) a.acc[0] = v[0]; return; }
     if (!reduce_to_fin(v[0], sm.tail, a.partials, a.counter, (int)blockIdx.x, (int)gridDim.x)) return;
     if (a.peer.nranks > 1 || a.npt_override >= 0.0) {             // (uniform) host-kd-tree count, sum over ranks
         if (a.npt_override >= 0.0 && tid == 0) sm.tail.fin[kPkNpt] = a.npt_override;

@@ -5,7 +5,7 @@
 //   * a single run keeps all its tiles resident at once (<= 3 blocks per SM; more slots: the blocks loop over tiles);
 //   * a single run of a SMALL cloud (fewer 256-slot tiles than SMs) is cut into >= 2 tiles per SM at 32-slot
 //     granularity instead of leaving most SMs idle - measured 45.6 -> 36.0 us per iteration on the shipped 7 562-point
-//     cloud on an H100 (tools/tile_sweep.py); no effect once there is a tile per SM;
+//     cloud on an H100 (with an earlier build that could force the tile size); no effect once there is a tile per SM;
 //   * batched trials (grid y = trial) are throughput-bound: full tiles, at most 64 blocks per trial;
 //   * a batch of different scans (ragged slot counts) follows its largest scan (plan_scan_tiles).
 // tests/test_host_la.py::test_loop_tile_plan and tests/test_scan_plan.py check the invariants on the CPU.
@@ -19,10 +19,8 @@ struct Tiles {
     long long grid_x;    // blocks per trial
 };
 
-// tile_override: 0 = rule above; otherwise a requested tile size for single runs (measurement switch DCREG_TILE),
-// ignored when it is out of range or would not fit the resident blocks.
 // reserved: resident slots a single run keeps for blocks without a tile (the solver block), not counted in grid_x.
-inline Tiles plan_tiles(long long slots, int trials, int sm_count, int block_threads, int tile_override = 0, int reserved = 0) {
+inline Tiles plan_tiles(long long slots, int trials, int sm_count, int block_threads, int reserved = 0) {
     Tiles t{block_threads, std::max<long long>(1, (slots + block_threads - 1) / block_threads)};
     if (trials != 1) {
         t.grid_x = std::min<long long>(t.grid_x, 64);
@@ -32,7 +30,6 @@ inline Tiles plan_tiles(long long slots, int trials, int sm_count, int block_thr
     if (t.grid_x > cap) { t.grid_x = cap; return t; }
     int tile = block_threads;
     if (t.grid_x < sm_count) tile = (int)std::max<long long>(32, (slots / (2LL * sm_count) + 31) / 32 * 32);
-    if (tile_override) tile = tile_override;
     if (tile < 32 || tile > block_threads || (slots + tile - 1) / tile > cap) tile = block_threads;
     t.tile = tile;
     t.grid_x = std::max<long long>(1, (slots + tile - 1) / tile);

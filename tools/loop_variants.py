@@ -1,5 +1,4 @@
-"""C2 step time (100 k points x 50 fixed iterations) and the per-iteration device times the log records,
-for the loop plumbing variants selected by the environment (DCREG_NO_GRAPH, DCREG_NO_FOLD, DCREG_NO_PDL)."""
+"""C2 step time (100 k points x 50 fixed iterations) and the per-iteration device times the log records."""
 import os, sys, time
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -26,22 +25,21 @@ with Context(0) as ctx:
     e1.synchronize()
     wall = time.perf_counter() - t0
     ms = e0.elapsed_time(e1) / 20
-    print(f"variant {os.environ.get('VARIANT', 'default')}: {ms * 1e3 / 50:7.2f} us/iteration device, {wall / 20 * 1e6 / 50:7.2f} us/iteration wall, "
+    print(f"{ms * 1e3 / 50:7.2f} us/iteration device, {wall / 20 * 1e6 / 50:7.2f} us/iteration wall, "
           f"launches/step {(ctx.launch_count - l0) / 20:.0f}")
     res = ctx.icp_run(prm, T0, want_log=True)
     t = np.array([L.iter_time_ms for L in res.logs]) * 1e3
     print("  iter_time_us:", " ".join(f"{x:.0f}" for x in t), f"| sum {t.sum():.0f}")
-    if os.environ.get("VARIANT", "default") == "default":
-        ctx.iteration_counters(True)
-        prev = (0, 0)
-        rows = []
-        for k in range(1, 51):
-            ctx.icp_run(default_params(search_radius=1.0, max_iterations=k, fixed_iterations=1, kappa_target=10.0), T0, want_log=False)
-            s_, f_ = ctx.iteration_counters(True)
-            rows.append((s_ - prev[0], f_ - prev[1]))
-            prev = (s_, f_)
-        ctx.iteration_counters(False)
-        print("  searched per iteration:", " ".join(str(r[0]) for r in rows))
-        print("  refitted per iteration:", " ".join(str(r[1]) for r in rows))
-        dx = [max(abs(x) for x in L.dx[3:]) for L in res.logs]
-        print("  max |dx_t| per iteration (m):", " ".join(f"{x:.1e}" for x in dx))
+    ctx.iteration_counters(True)
+    prev = (0, 0)
+    rows = []
+    for k in range(1, 51):
+        ctx.icp_run(default_params(search_radius=1.0, max_iterations=k, fixed_iterations=1, kappa_target=10.0), T0, want_log=False)
+        s_, f_ = ctx.iteration_counters(True)
+        rows.append((s_ - prev[0], f_ - prev[1]))
+        prev = (s_, f_)
+    ctx.iteration_counters(False)
+    print("  searched per iteration:", " ".join(str(r[0]) for r in rows))
+    print("  refitted per iteration:", " ".join(str(r[1]) for r in rows))
+    dx = [max(abs(x) for x in L.dx[3:]) for L in res.logs]
+    print("  max |dx_t| per iteration (m):", " ".join(f"{x:.1e}" for x in dx))

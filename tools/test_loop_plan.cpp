@@ -38,30 +38,21 @@ int main() {
     CHECK(a.tile == 256 && a.grid_x == 396);
     a = loop_plan::plan_tiles(7562, 5000, 132, 256);
     CHECK(a.tile == 256 && a.grid_x == 30);
-    // the measurement override: honoured when it fits, ignored when it does not
-    a = loop_plan::plan_tiles(90000, 1, 132, 256, 232);
-    CHECK(a.tile == 232 && a.grid_x == 388);
-    a = loop_plan::plan_tiles(100000, 1, 132, 256, 232);
-    CHECK(a.tile == 256 && a.grid_x == 391);
-    a = loop_plan::plan_tiles(100000, 1, 132, 256, 128);
-    CHECK(a.tile == 256 && a.grid_x == 391);
-    a = loop_plan::plan_tiles(100000, 1, 132, 256, 7);
-    CHECK(a.tile == 256);
     // a single folded run keeps one resident slot for the solver block: at most 3 SMs - 1 tile blocks
     for (int sm : sms)
         for (long long n = 1; n <= 400000; n += (n < 3000 ? 1 : 997)) {
-            const loop_plan::Tiles t = loop_plan::plan_tiles(n, 1, sm, 256, 0, 1);
+            const loop_plan::Tiles t = loop_plan::plan_tiles(n, 1, sm, 256, 1);
             ++cases;
             CHECK(t.tile >= 32 && t.tile <= 256 && t.tile % 32 == 0);
             CHECK(t.grid_x >= 1 && t.grid_x <= 3LL * sm - 1);
             if (t.grid_x < 3LL * sm - 1) CHECK(t.grid_x * t.tile >= n);
             if (t.grid_x * (long long)t.tile >= n) CHECK((t.grid_x - 1) * t.tile < n);
         }
-    a = loop_plan::plan_tiles(100000, 1, 132, 256, 0, 1);
+    a = loop_plan::plan_tiles(100000, 1, 132, 256, 1);
     CHECK(a.tile == 256 && a.grid_x == 391);                                  // C2: 391 tiles + the solver = 392 blocks
-    a = loop_plan::plan_tiles(10000000, 1, 132, 256, 0, 1);
+    a = loop_plan::plan_tiles(10000000, 1, 132, 256, 1);
     CHECK(a.tile == 256 && a.grid_x == 395);                                  // C4: 395 looping tile blocks
-    a = loop_plan::plan_tiles(7562, 1, 132, 256, 0, 1);
+    a = loop_plan::plan_tiles(7562, 1, 132, 256, 1);
     CHECK(a.tile == 32 && a.grid_x == 237);
     std::printf("%lld cases, %d failures\n", cases, fails);
     if (!fails) std::printf("LOOP_PLAN_OK\n");
