@@ -66,8 +66,8 @@ def local_map(seq, res_seq, k, map_frames):
     return np.concatenate([map_points(res_seq[j].T, seq[j]) for j in range(max(0, k - map_frames), k)])
 
 
-def reconstruct(ctx, prm, seq, res_seq, k, map_frames):
-    ctx.set_target(local_map(seq, res_seq, k, map_frames), CELL)
+def reconstruct(ctx, prm, seq, res_seq, k, map_frames, cell=CELL):
+    ctx.set_target(local_map(seq, res_seq, k, map_frames), cell)
     ctx.set_source(seq[k])
     return ctx.icp_run(prm, res_seq[k].T_prior)
 
@@ -109,18 +109,20 @@ def assert_priors(res, seqs, T_init, deltas, motion="increments"):
         k += len(rs)
 
 
-@pytest.mark.parametrize("method", ["Ours", "ME-TSVD"])
-def test_frames_equal_their_reconstruction(ctx, odo, method):
-    """Ours runs the frame's last step in the loop kernel's folded step; ME-TSVD in the separate solve kernel."""
+@pytest.mark.parametrize("method,cell", [pytest.param(m, c, id=m if c == CELL else f"{m}-cell{c}")
+                                         for c in (CELL, CELL / 2) for m in ("Ours", "ME-TSVD")])
+def test_frames_equal_their_reconstruction(ctx, odo, method, cell):
+    """Ours runs the frame's last step in the loop kernel's folded step; ME-TSVD in the separate solve kernel.
+    cell = CELL / 2: the local maps searched over 2 rings of cells."""
     seqs, frames, T_init, deltas, T_true = odo
     prm = params(method)
-    res = ctx.icp_run_odometry(prm, seqs, T_init, deltas, map_frames=3, cell_size=CELL, want_log=True, want_cov=True)
+    res = ctx.icp_run_odometry(prm, seqs, T_init, deltas, map_frames=3, cell_size=cell, want_log=True, want_cov=True)
     assert len(res) == len(frames) == 20
     assert_priors(res, seqs, T_init, deltas)
     for s, (seq, rs) in enumerate(zip(seqs, split(res, seqs))):
         assert_anchor(rs[0], T_init[s])
         for k in range(1, len(seq)):
-            assert_same_run(rs[k], reconstruct(ctx, prm, seq, rs, k, 3))
+            assert_same_run(rs[k], reconstruct(ctx, prm, seq, rs, k, 3, cell))
     assert sum(r.converged for r in res) >= 15
     assert max(o.se3_log_distance(r.T, T) for r, T in zip(res, T_true)) < 0.05
 

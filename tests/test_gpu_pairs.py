@@ -73,8 +73,8 @@ def assert_same_run(b, single, logs=True):
             assert np.max(np.abs(np.array(x.dx) - np.array(y.dx))) < 1e-8
 
 
-def single_run(ctx, prm, s, t, T, **kw):
-    ctx.set_target(t, RADIUS)
+def single_run(ctx, prm, s, t, T, cell=RADIUS, **kw):
+    ctx.set_target(t, cell)
     ctx.set_source(s)
     return ctx.icp_run(prm, T, **kw)
 
@@ -84,17 +84,19 @@ def same_bits(x, y):
             and [np.array(L.H27).tobytes() for L in x.logs] == [np.array(L.H27).tobytes() for L in y.logs])
 
 
-@pytest.mark.parametrize("method", ["Ours", "ME-TSVD"])
-def test_pairs_equal_single_runs(ctx, scene, method):
-    """Ours folds the solve step into the loop kernel; ME-TSVD takes the separate solve kernel (k2_step_kernel)."""
+@pytest.mark.parametrize("method,cell", [pytest.param(m, c, id=m if c == RADIUS else f"{m}-cell{c}")
+                                         for c in (RADIUS, RADIUS / 2) for m in ("Ours", "ME-TSVD")])
+def test_pairs_equal_single_runs(ctx, scene, method, cell):
+    """Ours folds the solve step into the loop kernel; ME-TSVD takes the separate solve kernel (k2_step_kernel).
+    cell = RADIUS / 2: the targets' grids searched over 2 rings of cells."""
     src, tgt, _, T_init = scene
     assert min(len(t) for t in tgt) < 5_000 and max(len(t) for t in tgt) > 80_000
     prm = c3_params(method)
-    batch = ctx.icp_run_pairs(prm, src, tgt, T_init, want_log=True)
+    batch = ctx.icp_run_pairs(prm, src, tgt, T_init, cell_size=cell, want_log=True)
     assert len(batch) == len(src)
     n_conv = 0
     for k, b in enumerate(batch):
-        assert_same_run(b, single_run(ctx, prm, src[k], tgt[k], T_init[k]))
+        assert_same_run(b, single_run(ctx, prm, src[k], tgt[k], T_init[k], cell=cell))
         n_conv += int(b.converged)
     assert n_conv >= 10                                     # the pairs stop on their own convergence tests
 

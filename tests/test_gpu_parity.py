@@ -353,19 +353,35 @@ def test_icp_fixed_iterations_synthetic_cylinder(ctx):
     check_against_oracle(res, conv, T, logs, status)
 
 
-@pytest.mark.parametrize("method", ["Ours", "ME-TSVD"])
-def test_loop_with_reused_correspondences_equals_full_search_every_iteration(ctx, method):
+def loop_reuse_cases():
+    """(method, target cell, shift of the scene): cell = radius (rings 1, the usual set-up; ids as before), finer cells
+    (rings 2, 3 with a non-integer radius / cell, 4) and the cylinder far from the origin"""
+    far = (4096.3, -2047.7, 130.1)
+    cases = [pytest.param(m, 1.0, None, id=m) for m in ("Ours", "ME-TSVD")]
+    cases += [pytest.param(m, c, None, id=f"{m}-cell{c}") for m in ("Ours", "ME-TSVD") for c in (0.5, 0.4, 0.25)]
+    cases += [pytest.param("Ours", 1.0, far, id="Ours-far")]
+    return cases
+
+
+@pytest.mark.parametrize("method,cell,shift", loop_reuse_cases())
+def test_loop_with_reused_correspondences_equals_full_search_every_iteration(ctx, method, cell, shift):
     """The loop's iteration kernel reuses neighbour lists (gap certificate) and plane fits (same five points) once the
     pose moves little.  Against the same loop with a full search and a fresh fit in EVERY iteration (the loop kernel's
     lean mode in every iteration, DCREG_FUSED_SEARCH=1) the per-iteration counts must be identical and the poses equal
-    to rounding; the counters show that the reuse paths were actually taken."""
+    to rounding; the counters show that the reuse paths were actually taken.  Target cells finer than the search
+    radius (1.0) run the warp and bounded searches over 2-4 rings of cells."""
     from dcreg_b200 import default_params
     from dcreg_b200.scenes import make_cylinder
     pts = make_cylinder(30_000, seed=7)
     T0 = o.pose6d_to_matrix(0.1, 0.3, 0.2, math.radians(0.1), math.radians(-0.1), math.radians(1.0))
+    if shift is not None:                                   # the same motion, about the moved cylinder
+        S = np.eye(4)
+        S[:3, 3] = shift
+        pts = (pts.astype(np.float64) + shift).astype(np.float32)
+        T0 = S @ T0 @ np.linalg.inv(S)
     det, hand = METHODS[method]
     prm = default_params(max_iterations=40, fixed_iterations=1, kappa_target=10.0, detection=det, handling=hand)
-    ctx.set_source(pts); ctx.set_target(pts, 1.0)
+    ctx.set_source(pts); ctx.set_target(pts, cell)
     ctx.iteration_counters(True)
     res = ctx.icp_run(prm, T0)
     searched, fitted = ctx.iteration_counters(False)
@@ -388,6 +404,17 @@ def test_loop_reuse_on_a_lattice_with_duplicates_and_ties(ctx):
     duplicated target points, a dense patch (more than 64 candidates inside a loose bound -> the warp search gives up
     and the slot searches sequentially) and a source that is not a multiple of the tile size.  The reference is a full
     search and a fresh fit in every iteration (lean mode throughout, DCREG_FUSED_SEARCH=1)."""
+    check_lattice_reuse(ctx, 1.0)
+
+
+@pytest.mark.parametrize("cell", [0.5, 0.25])
+def test_loop_reuse_on_a_lattice_at_finer_cells(ctx, cell):
+    """The lattice scene above with target cells of half and a quarter of the search radius: the warp and bounded
+    searches over 2 and 4 rings of cells; at 0.25 the lattice points lie on cell faces."""
+    check_lattice_reuse(ctx, cell)
+
+
+def check_lattice_reuse(ctx, cell):
     from dcreg_b200 import default_params
     g = np.arange(-6, 6, 0.25, dtype=np.float32)
     X, Y = np.meshgrid(g, g)
@@ -402,7 +429,7 @@ def test_loop_reuse_on_a_lattice_with_duplicates_and_ties(ctx):
     src = tgt[rng.permutation(len(tgt))[:7001]].copy()
     T0 = o.pose6d_to_matrix(0.06, -0.05, 0.04, math.radians(0.2), math.radians(-0.1), math.radians(0.4))
     prm = default_params(max_iterations=25, fixed_iterations=1, kappa_target=10.0)
-    ctx.set_source(src); ctx.set_target(tgt, 1.0)
+    ctx.set_source(src); ctx.set_target(tgt, cell)
     res = ctx.icp_run(prm, T0)
     os.environ["DCREG_FUSED_SEARCH"] = "1"
     try:

@@ -10,6 +10,22 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
+def device_program_flags():
+    """The library's nvcc flags for a standalone sm_90a program: without the shared-library and ptxas-report options,
+    each dropped with its argument."""
+    from dcreg_b200.build import NVCC_FLAGS
+    flags, skip = [], False
+    for f in NVCC_FLAGS:
+        if skip:
+            skip = False
+        elif f in ("-Xcompiler", "-Xptxas"):
+            skip = True
+        elif f != "--shared":
+            flags.append(f)
+    assert "arch=compute_90a,code=sm_90a" in flags and "--fmad=true" in flags
+    return flags
+
+
 def test_register_qr_is_bit_identical_to_the_generic_qr(tmp_path):
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     if not os.path.exists(nvcc):
@@ -43,18 +59,9 @@ def test_fast_solve_step_pieces_on_the_device(tmp_path):
     [1e-300, 1e300] and fast_rsqrt against mpmath on a sample: at most the documented 2 ulp."""
     import mpmath
     import numpy as np
-    from dcreg_b200.build import NVCC_FLAGS, _nvcc
-    flags, skip = [], False                                # the library's flags without the shared-library and
-    for f in NVCC_FLAGS:                                   # ptxas-report options, each dropped with its argument
-        if skip:
-            skip = False
-        elif f in ("-Xcompiler", "-Xptxas"):
-            skip = True
-        elif f != "--shared":
-            flags.append(f)
-    assert "arch=compute_90a,code=sm_90a" in flags and "--fmad=true" in flags
+    from dcreg_b200.build import _nvcc
     exe = tmp_path / "test_k2_fast_dev"
-    subprocess.run([_nvcc()] + flags + ["-DK2F_DEVICE_TEST", "-o", str(exe), os.path.join(ROOT, "tools", "test_k2_fast.cu")],
+    subprocess.run([_nvcc()] + device_program_flags() + ["-DK2F_DEVICE_TEST", "-o", str(exe), os.path.join(ROOT, "tools", "test_k2_fast.cu")],
                    check=True, capture_output=True, text=True)
     out = tmp_path / "rsqrt.bin"
     res = subprocess.run([str(exe), str(out)], capture_output=True, text=True)
