@@ -90,7 +90,7 @@ EXPORTS = [
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_odometry_open", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_close", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -162,6 +162,14 @@ def load_library():
                                                C.POINTER(C.c_float), C.POINTER(i64), dp, dp, C.POINTER(ci), C.POINTER(ci),
                                                C.POINTER(ci), dp, C.POINTER(C.c_float), C.POINTER(IterLog), ci]
     lib.dcreg_odometry_close.argtypes = [vp]
+    lib.dcreg_icp_run_odometry_map.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
+                                               C.POINTER(i64), ci, C.c_double, ci, C.c_double, C.c_double, ci, ci,
+                                               C.c_double, dp, dp, C.POINTER(C.c_float), C.POINTER(i64), dp, dp,
+                                               C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(C.c_float),
+                                               C.POINTER(IterLog), ci]
+    lib.dcreg_odometry_open_map.argtypes = [vp, C.POINTER(IcpParams), ci, C.c_double, ci, C.c_double, C.c_double, ci, ci,
+                                            C.c_double, dp]
+    lib.dcreg_odometry_local_map.argtypes = [vp, ci, C.POINTER(C.c_float), i64, C.POINTER(i64)]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -491,6 +499,60 @@ def voxel_downsample(P, voxel, max_points=1):
     rank = at - np.maximum.accumulate(np.where(starts, at, 0))
     keep = rows[np.sort(order[rank < max_points])].astype(np.int64)
     return np.ascontiguousarray(xyz[keep]), keep
+
+
+def _voxel_ids(xyz, voxel, name):
+    """Packed voxel keys of the rows of xyz (K, 3) float32, all finite, as voxel_downsample forms them"""
+    with np.errstate(invalid="ignore", over="ignore"):
+        keys = np.floor(xyz.astype(np.float64) * (1.0 / voxel))
+    if not ((keys >= -VOXEL_LIMIT) & (keys < VOXEL_LIMIT)).all():
+        raise ValueError(f"{name}: a voxel coordinate lies outside [-2^20, 2^20) (voxel too small for the cloud's "
+                         "coordinates)")
+    k = keys.astype(np.int64) + VOXEL_LIMIT
+    return (k[:, 0] << 42) | (k[:, 1] << 21) | k[:, 2]
+
+
+def voxel_map_prune(X, voxel, max_distance, t):
+    """The prune of the voxel map (dcreg_icp_run_odometry_map), bit for bit: every point of every voxel whose first point
+    q (its row of smallest index in X) has ((qx - tx)^2 + (qy - ty)^2) + (qz - tz)^2 >= max_distance^2 is dropped, in
+    FP64 from the float32 coordinates with one rounding per operation, max_distance^2 = max_distance * max_distance
+    (KISS-ICP's RemovePointsFarFromLocation).  Voxels as in voxel_downsample; rows with a non-finite coordinate have no
+    voxel and are dropped.  X: (N, >=3); t: the translation (3,).  Returns (points (K, 3) float32, the survivors' rows
+    unchanged and in order; index (K,) int64, their rows in X)."""
+    X = np.asarray(X, dtype=np.float32)
+    if X.ndim != 2 or X.shape[1] < 3:
+        raise ValueError("points must be (N, >=3)")
+    voxel, max_distance = float(voxel), float(max_distance)
+    if not (voxel > 0.0 and np.isfinite(voxel)):
+        raise ValueError(f"voxel_map_prune: voxel must be finite and > 0, not {voxel}")
+    if not max_distance > 0.0:
+        raise ValueError(f"voxel_map_prune: max_distance must be > 0 (+inf: no pruning), not {max_distance}")
+    xyz = X[:, :3]
+    rows = np.nonzero(np.isfinite(xyz).all(axis=1))[0]
+    ids = _voxel_ids(xyz[rows], voxel, "voxel_map_prune")
+    order = np.argsort(ids, kind="stable")
+    s = ids[order]
+    starts = np.ones(len(s), dtype=bool)
+    starts[1:] = s[1:] != s[:-1]
+    at = np.arange(len(s))
+    first = np.empty(len(s), dtype=np.int64)
+    first[order] = order[np.maximum.accumulate(np.where(starts, at, 0))]     # each row's voxel's first row (of rows)
+    q = xyz[rows[first]].astype(np.float64)
+    d = q - np.asarray(t, dtype=np.float64).reshape(3)
+    d2 = (d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2]
+    keep = rows[~(d2 >= max_distance * max_distance)].astype(np.int64)
+    return np.ascontiguousarray(xyz[keep]), keep
+
+
+def voxel_map_update(M, P, T, voxel, max_points, max_distance):
+    """One update of the voxel map of dcreg_icp_run_odometry_map, bit for bit: prune(cap(M ++ map_points(T, P)), t_T)
+    with cap = voxel_downsample(., voxel, max_points) (M first: older points win, KISS-ICP's AddPoints) and prune =
+    voxel_map_prune at T's translation.  M: the map (K, 3) float32 (may be empty); P: the frame's points (N, >=3) in its
+    sensor frame; T: its pose (4, 4).  Returns the new map (K', 3) float32."""
+    M = np.asarray(M, dtype=np.float32).reshape(-1, 3)
+    X = np.concatenate([M, map_points(T, P)])
+    capped, _ = voxel_downsample(X, voxel, max_points)
+    return voxel_map_prune(capped, voxel, max_distance, np.asarray(T, dtype=np.float64)[:3, 3])[0]
 
 
 class IcpResult:
@@ -843,6 +905,65 @@ class Context:
                 r.deskewed = d
         return out
 
+    def icp_run_odometry_map(self, params: IcpParams, sequences, T_init, deltas=None, motion: str = "increments", *,
+                             map_voxel: float, max_distance: float, cell_size=None, want_log: bool = False,
+                             want_cov: bool = False, source_voxel: float = 0.0, source_max_points: int = 1,
+                             map_max_points: int = 1, timestamps=None, want_deskewed: bool = False):
+        """icp_run_odometry with a persistent voxel map per sequence instead of the window (dcreg_icp_run_odometry_map,
+        KISS-ICP's VoxelHashMap): frame k registers against M_k, where M_1 = voxel_map_update(empty, F_s(anchor),
+        T_init[s]) and M_{k+1} = voxel_map_update(M_k, F_s(frame k), T_out[k], map_voxel, map_max_points,
+        max_distance).  map_voxel must be > 0; max_distance > 0 (inf: nothing is pruned, and the outputs are those of
+        icp_run_odometry with map_frames >= the longest sequence).  The arguments are icp_run_odometry's in the same
+        positions, without map_frames; map_voxel and max_distance are keyword-only."""
+        models = {"increments": 0, "constant_velocity": 1}
+        if motion not in models:
+            raise ValueError(f"icp_run_odometry_map: motion must be one of {sorted(models)}, not {motion!r}")
+        source_max_points = _max_points(source_max_points, "source_max_points")
+        map_max_points = _max_points(map_max_points, "map_max_points")
+        seq_off, xyz, off = _pack_sequences(sequences)
+        S, n = len(sequences), int(seq_off[-1])
+        cell = float(params.search_radius if cell_size is None else cell_size)
+        ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
+                              off if off is not None else np.zeros(1, np.int64), "icp_run_odometry_map")
+        npts = np.zeros(max(n, 1), dtype=np.int64)
+        desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
+
+        def call(o):
+            return self.lib.dcreg_icp_run_odometry_map(
+                self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off), 3,
+                cell, models[motion], float(source_voxel), float(map_voxel), source_max_points, map_max_points,
+                float(max_distance), _optr(o.T_init), _optr(o.deltas), _fptr(ts), _iptr(npts), _optr(o.T_prior),
+                _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov), _fptr(desk), o.logs, o.cap)
+        out = self._run_batched("icp_run_odometry_map", call, params, n, S, "sequences", T_init, want_log, want_cov,
+                                deltas, want_prior=True)
+        for r, c in zip(out, npts):
+            r.n_points = int(c)
+        if want_deskewed:
+            for r, d in zip(out, _split_deskewed(desk, npts[:n])):
+                r.deskewed = d
+        return out
+
+    def odometry_map_session(self, params: IcpParams, n_seqs: int, T_init, motion: str = "increments", *,
+                             map_voxel: float, max_distance: float, cell_size=None, source_voxel: float = 0.0,
+                             source_max_points: int = 1, map_max_points: int = 1):
+        """Open the context's odometry session with icp_run_odometry_map's voxel map (dcreg_odometry_open_map): the
+        OdometrySession of odometry_session, whose pushes give byte for byte what one icp_run_odometry_map call over the
+        recording gives, and whose local_map(s) returns sequence s's current map.  The arguments are odometry_session's
+        in the same positions, without map_frames; map_voxel and max_distance are keyword-only."""
+        models = {"increments": 0, "constant_velocity": 1}
+        if motion not in models:
+            raise ValueError(f"odometry_map_session: motion must be one of {sorted(models)}, not {motion!r}")
+        source_max_points = _max_points(source_max_points, "source_max_points")
+        map_max_points = _max_points(map_max_points, "map_max_points")
+        T0 = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
+        if T0.shape[0] != n_seqs:
+            raise ValueError(f"odometry_map_session: {n_seqs} sequences but {T0.shape[0]} initial poses")
+        cell = float(params.search_radius if cell_size is None else cell_size)
+        self._check(self.lib.dcreg_odometry_open_map(self._h, C.byref(params), int(n_seqs), cell, models[motion],
+                                                     float(source_voxel), float(map_voxel), source_max_points,
+                                                     map_max_points, float(max_distance), _dptr(T0)))
+        return OdometrySession(self, params, int(n_seqs))
+
     def odometry_session(self, params: IcpParams, n_seqs: int, T_init, motion: str = "increments", map_frames: int = 10,
                          cell_size=None, source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
                          map_max_points: int = 1):
@@ -1008,6 +1129,19 @@ class OdometrySession:
             for r, d in zip(res, _split_deskewed(desk, npts[:n])):
                 r.deskewed = d
         return [res[a:b] for a, b in zip(seq_off[:-1], seq_off[1:])]
+
+    def local_map(self, s: int):
+        """Sequence s's current voxel map (a session of Context.odometry_map_session, dcreg_odometry_local_map): M after
+        its last committed frame, (K, 3) float32 in map order (empty before its first frame)."""
+        ctx, lib = self.ctx, self.ctx.lib
+        n = C.c_int64(0)
+        rc = lib.dcreg_odometry_local_map(ctx._h, int(s), None, 0, C.byref(n))
+        if n.value == 0:
+            ctx._check(rc)
+            return np.zeros((0, 3), np.float32)
+        out = np.empty((n.value, 3), np.float32)
+        ctx._check(lib.dcreg_odometry_local_map(ctx._h, int(s), _fptr(out), n.value, C.byref(n)))
+        return out
 
     def close(self):
         if self.open and self.ctx._h:

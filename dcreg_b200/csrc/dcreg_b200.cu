@@ -972,7 +972,7 @@ __global__ void voxel_cap_flag_kernel(const unsigned int* __restrict__ key, cons
 
 // Pass 4 (pos: the exclusive scan of keep): kept point i goes to out[pos[i]] (out_stride 3: x y z; 4: x y z and w = its
 // index over all kept points, as pack_points_kernel packs one cloud), index[pos[i]] = its index in its own cloud (index
-// may be null); out_seg[b] = pos[seg[b]] for b <= n_seg, the kept points' offsets.  n + 1 threads.
+// may be null); out_seg[b] = pos[seg[b]] for b <= n_seg, the kept points' offsets.  max(n, n_seg) + 1 threads.
 __global__ void voxel_scatter_kernel(const float* __restrict__ in, long long n, int stride, const long long* __restrict__ seg,
                                      int n_seg, const int* __restrict__ keep, const int* __restrict__ pos,
                                      float* __restrict__ out, int out_stride, long long* __restrict__ index,
@@ -1089,6 +1089,60 @@ __global__ void retain_points_kernel(const float4* __restrict__ src, const float
     if (i >= m) return;
     const int p = corr::segment_of(dst, pieces, i);
     out[i] = (ref[p] < n_frames ? src : win)[src_at[p] + (i - dst[p])];
+}
+
+// ---- the voxel map (dcreg_icp_run_odometry_map, dcreg_odometry_open_map; odom_plan::map_step) ----------------------
+// The input of one map update: m points in `pieces` pieces, piece p being out[dst[p], dst[p+1]): an old map copied from
+// `old` (frame[p] < 0), or the packed points src_at[p] .. of pushed frame frame[p] under its final pose, with the
+// arithmetic of map_points_kernel (the same bits).  w = the point's index in the input.
+__global__ void map_update_input_kernel(const float4* __restrict__ src, const float4* __restrict__ old,
+                                        const long long* __restrict__ dst, int pieces, const long long* __restrict__ src_at,
+                                        const int* __restrict__ frame, long long m, const IcpState* __restrict__ states,
+                                        float4* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const int p = corr::segment_of(dst, pieces, i);
+    const int r = frame[p];
+    const long long at = src_at[p] + (i - dst[p]);
+    if (r < 0) {
+        const float4 q = old[at];
+        out[i] = make_float4(q.x, q.y, q.z, __int_as_float((int)i));
+        return;
+    }
+    const IcpState* st = states + r;
+    const float4 q = src[at];
+    const double x = q.x, y = q.y, z = q.z;
+    float v[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+        v[c] = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(st->R[3 * c], x), __dmul_rn(st->R[3 * c + 1], y)),
+                                          __dmul_rn(st->R[3 * c + 2], z)),
+                                st->t[c]);
+    out[i] = make_float4(v[0], v[1], v[2], __int_as_float((int)i));
+}
+
+// The voxel map's prune, between the voxel filter's flag pass and its scan (KISS-ICP's RemovePointsFarFromLocation): a
+// kept point i whose voxel's first point q (first[slot_of[i]], the voxel's smallest index) has ((qx - tx)^2 + (qy -
+// ty)^2) + (qz - tz)^2 >= max_d2 is dropped, in FP64 from the float32 coordinates with one rounding per operation.  t:
+// the translation of frame reference center[b] (ref_pose's rule) for segment b.  O(1) per point: every point of a
+// voxel reads the same first point, so a voxel goes or stays whole.
+__global__ void voxel_prune_kernel(const float* __restrict__ in, long long n, int stride, const long long* __restrict__ seg,
+                                   int n_seg, const long long* __restrict__ slot_of, const int* __restrict__ first,
+                                   const int* __restrict__ center, int n_frames, const IcpState* __restrict__ states,
+                                   const double* __restrict__ hist_T, double max_d2, int* __restrict__ keep) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || !keep[i]) return;
+    const int r = center[corr::segment_of(seg, n_seg, i)];
+    double t[3];
+    if (r < n_frames) {
+        for (int c = 0; c < 3; ++c) t[c] = states[r].t[c];
+    } else {
+        for (int c = 0; c < 3; ++c) t[c] = hist_T[(size_t)(r - n_frames) * 16 + 4 * c + 3];
+    }
+    const long long q = first[slot_of[i]];
+    const double dx = __dsub_rn((double)in[q * stride], t[0]), dy = __dsub_rn((double)in[q * stride + 1], t[1]),
+                 dz = __dsub_rn((double)in[q * stride + 2], t[2]);
+    if (__dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) >= max_d2) keep[i] = 0;
 }
 
 // ---- motion compensation (dcreg_icp_run_odometry_deskew, dcreg_odometry_push_deskew; se3.cuh) ---------------------
@@ -1236,6 +1290,10 @@ struct OdomSettings {
     int n_seqs = 0, map_frames = 1, motion = 0, source_max_points = 1, map_max_points = 1;
     double cell_size = 0.0, source_voxel = 0.0, map_voxel = 0.0;
     std::vector<double> T_init;                                        // [n_seqs][16]
+    // the voxel map (dcreg_icp_run_odometry_map, dcreg_odometry_open_map) instead of the window (map_frames unused):
+    // every sequence's map carried from frame to frame, pruned at max_distance (+inf: never)
+    bool voxel_map = false;
+    double max_distance = 0.0;
 };
 
 struct dcreg_ctx {
@@ -1303,6 +1361,10 @@ struct dcreg_ctx {
     // their grids in an arena of their own
     DevBuf<long long> d_odom_ll; DevBuf<int> d_odom_int;
     DevBuf<float4> d_odom_map, d_odom_map_vox;                         // ... and the maps after the voxel filter
+    // the voxel map: one update's tables (odom_plan::MapStep; its input goes to d_odom_map), and the updates' outputs,
+    // step after step in turns (an update reads the previous one's)
+    DevBuf<long long> d_vmap_ll; DevBuf<int> d_vmap_int;
+    DevBuf<float4> d_vmap[2];
     // motion compensation (dcreg_icp_run_odometry_deskew): the caller's timestamps [input points], the packed points'
     // [points], and the step's twists [lanes][6]
     DevBuf<float> d_odom_ts_in, d_odom_ts;
@@ -1318,6 +1380,9 @@ struct dcreg_ctx {
         std::vector<double> last_delta;                                // [n_seqs][16]
         DevBuf<float4> win[2]; int cur = 0;
         DevBuf<double> d_hist_T;                                       // hist_T on the device
+        // the voxel map (set.voxel_map): win[cur] holds every sequence's map instead of a window, sequence s's being
+        // points [map_off[s], map_off[s + 1]), its last frame in it (the push's final update gathers them in win[1 - cur])
+        std::vector<long long> map_off;                                // [n_seqs + 1]
     };
     std::unique_ptr<OdomSession> odom;
     // the voxel filter (voxel_filter): table [slots] keys / first indices, [points] slots, [points + 1] flags and their
@@ -1693,10 +1758,18 @@ static int voxel_reserve(dcreg_ctx* ctx, long long n, int n_seg, long long slots
 // keeping up to max_points points per voxel.  The kept points go to d_out (out_stride 3 or 4, see voxel_scatter_kernel)
 // and their indices in their own cloud to d_index (null: not wanted); the kept offsets to ctx->d_vox_seg [n_seg + 1], and
 // bad[b] != 0 in ctx->d_vox_bad when cloud b has a voxel coordinate outside [-2^20, 2^20).  No host sync; whatever
-// n_seg, six launches for max_points = 1, and for max_points > 1 seven and the radix sort's own.
+// n_seg, six launches for max_points = 1, and for max_points > 1 seven and the radix sort's own.  prune (the voxel map):
+// voxel_prune_kernel between the flags and the scan, one launch more.
+struct VoxelPrune {
+    const int* center;                  // [n_seg] the frame reference whose translation prunes each cloud
+    int n_frames;                       // ... read as ref_pose reads it
+    const IcpState* states;
+    const double* hist_T;
+    double max_d2;                      // max_distance * max_distance
+};
 static int voxel_filter(dcreg_ctx* ctx, const float* d_in, long long n, int stride, const long long* d_seg,
                         const int64_t* h_seg, int n_seg, double voxel, float* d_out, int out_stride, long long* d_index,
-                        int max_points = 1) {
+                        int max_points = 1, const VoxelPrune* prune = nullptr) {
     std::vector<long long> tab;
     const long long slots = voxel_tables(n_seg, h_seg, tab);
     int rc = voxel_reserve(ctx, n, n_seg, slots, max_points);
@@ -1726,8 +1799,18 @@ static int voxel_filter(dcreg_ctx* ctx, const float* d_in, long long n, int stri
         ctx->launches++;                                         // (the radix sort's own kernels are not counted)
         CK(cudaGetLastError());
     }
+    if (prune) {
+        voxel_prune_kernel<<<nb, 256, 0, ctx->stream>>>(d_in, n, stride, d_seg, n_seg, ctx->d_vox_slot, ctx->d_vox_first,
+                                                        prune->center, prune->n_frames, prune->states, prune->hist_T,
+                                                        prune->max_d2, ctx->d_vox_keep);
+        ctx->launches++;
+        CK(cudaGetLastError());
+    }
     if ((rc = device_exclusive_scan(ctx, ctx->d_vox_keep, n + 1, ctx->d_vox_pos))) return rc;
-    voxel_scatter_kernel<<<nb1, 256, 0, ctx->stream>>>(d_in, n, stride, d_seg, n_seg, ctx->d_vox_keep, ctx->d_vox_pos, d_out,
+    // the scatter's threads also write the n_seg + 1 kept offsets: with empty clouds (the voxel map's updates) there may
+    // be more of those than points
+    const unsigned nbs = (unsigned)((std::max<long long>(n, n_seg) + 256) / 256);
+    voxel_scatter_kernel<<<nbs, 256, 0, ctx->stream>>>(d_in, n, stride, d_seg, n_seg, ctx->d_vox_keep, ctx->d_vox_pos, d_out,
                                                        out_stride, d_index, ctx->d_vox_seg);
     ctx->launches++;
     CK(cudaGetLastError());
@@ -2993,14 +3076,63 @@ static OdomSettings odom_settings(const dcreg_icp_params* params, int n_seqs, do
 
 // What is wrong with the settings of an odometry call or session, or null
 static const char* odometry_settings_error(const OdomSettings& set, bool deltas) {
-    if (set.map_frames < 1) return "map_frames must be >= 1";
+    if (!set.voxel_map && set.map_frames < 1) return "map_frames must be >= 1";
     if (set.motion != DCREG_MOTION_INCREMENTS && set.motion != DCREG_MOTION_CONSTANT_VELOCITY)
         return "motion must be DCREG_MOTION_INCREMENTS or DCREG_MOTION_CONSTANT_VELOCITY";
     if (set.motion == DCREG_MOTION_CONSTANT_VELOCITY && deltas) return "the constant-velocity model takes no deltas (pass NULL)";
     if (!(set.source_voxel >= 0.0 && set.source_voxel < INFINITY) || !(set.map_voxel >= 0.0 && set.map_voxel < INFINITY))
         return "source_voxel and map_voxel must be finite and >= 0 (0: no filter)";
     if (set.source_max_points < 1 || set.map_max_points < 1) return "source_max_points and map_max_points must be >= 1";
+    if (set.voxel_map && !(set.map_voxel > 0.0)) return "the voxel map needs a map_voxel > 0";
+    if (set.voxel_map && !(set.max_distance > 0.0)) return "max_distance must be > 0 (+inf: no pruning), not NaN";
     return nullptr;
+}
+
+// One update of the voxel maps (odom_plan::map_step): its input, [old map | new frame] per segment, in d_odom_map, then
+// the capped voxel filter with the prune into `out`, the kept offsets in ctx->d_vox_seg and the range flags in
+// ctx->d_vox_bad.  The buffers grow with headroom, since the maps' sizes follow the results.  No host sync; the input
+// launch and the filter's, one more for the prune, whatever the number of sequences.
+static int map_update(dcreg_ctx* ctx, const OdomSettings& set, const odom_plan::MapStep& ms, int n_frames,
+                      const double* d_hist_T, const float4* d_old, DevBuf<float4>& out) {
+    const int segs = (int)ms.seq.size(), pieces = (int)ms.piece_frame.size();
+    const long long m = ms.seg[(size_t)segs];
+    // long long seg [segs + 1], piece_dst [pieces + 1], piece_src [pieces]; int piece_frame [pieces], center [segs]
+    std::vector<long long> hll(ms.seg.begin(), ms.seg.end());
+    hll.insert(hll.end(), ms.piece_dst.begin(), ms.piece_dst.end());
+    hll.insert(hll.end(), ms.piece_src.begin(), ms.piece_src.end());
+    std::vector<int> hint(ms.piece_frame.begin(), ms.piece_frame.end());
+    hint.insert(hint.end(), ms.center.begin(), ms.center.end());
+    auto grow = [](auto& b, long long need) { return b.cap >= need ? cudaSuccess : b.ensure(need + need / 4); };
+    CK(grow(ctx->d_vmap_ll, (long long)hll.size()));
+    CK(grow(ctx->d_vmap_int, std::max<long long>((long long)hint.size(), 1)));
+    CK(grow(ctx->d_odom_map, std::max<long long>(m, 1)));
+    CK(grow(out, std::max<long long>(m, 1)));
+    CK(cudaMemcpyAsync(ctx->d_vmap_ll, hll.data(), hll.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+    if (!hint.empty())
+        CK(cudaMemcpyAsync(ctx->d_vmap_int, hint.data(), hint.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+    const long long* d_seg = ctx->d_vmap_ll;
+    const long long* d_dst = d_seg + segs + 1;
+    const int* d_frame = ctx->d_vmap_int;
+    if (m == 0) {           // no map and no frame to insert anywhere
+        CK(ctx->d_vox_seg.ensure(segs + 1));
+        CK(ctx->d_vox_bad.ensure(std::max(segs, 1)));
+        CK(cudaMemsetAsync(ctx->d_vox_seg, 0, (size_t)(segs + 1) * sizeof(long long), ctx->stream));
+        CK(cudaMemsetAsync(ctx->d_vox_bad, 0, (size_t)segs * sizeof(int), ctx->stream));
+        return DCREG_OK;
+    }
+    std::vector<long long> tab;
+    const long long slots = voxel_tables(segs, ms.seg.data(), tab);
+    if (ctx->d_vox_slot.cap < m || ctx->d_vox_keys.cap < slots || (set.map_max_points > 1 && ctx->d_vox_skey.cap < 2 * m)) {
+        const int rc = voxel_reserve(ctx, m + m / 4, set.n_seqs, slots + slots / 4, set.map_max_points);
+        if (rc) return rc;
+    }
+    map_update_input_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(
+        ctx->d_scan_src, d_old, d_dst, pieces, d_dst + pieces + 1, d_frame, m, ctx->d_state, ctx->d_odom_map);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    const VoxelPrune prune{d_frame + pieces, n_frames, ctx->d_state, d_hist_T, set.max_distance * set.max_distance};
+    return voxel_filter(ctx, (const float*)ctx->d_odom_map.p, m, 4, d_seg, ms.seg.data(), segs, set.map_voxel,
+                        (float*)out.p, 4, nullptr, set.map_max_points, &prune);
 }
 
 // A push that succeeded becomes the session's state: the history after it, the retained frames' poses (the T_out bytes
@@ -3099,8 +3231,8 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     odom_plan::Push U;
     odom_plan::Plan& P = U.plan;
     {
-        const std::string why = odom_plan::make_push(n_seqs, seq_offsets, n_frames, src_off, set.map_frames,
-                                                     arena_plan::kMaxPoints, hist, &U);
+        const std::string why = odom_plan::make_push(n_seqs, seq_offsets, n_frames, src_off,
+                                                     set.voxel_map ? 0 : set.map_frames, arena_plan::kMaxPoints, hist, &U);
         if (!why.empty()) { ctx->err = std::string(name) + ": " + why; return DCREG_BAD_ARG; }
     }
     const int n_steps = (int)P.steps.size();
@@ -3152,7 +3284,7 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     CK(ctx->d_odom_ll.ensure(std::max<long long>((long long)hll.size(), 1)));
     CK(ctx->d_odom_int.ensure(std::max<long long>((long long)hint.size(), 1)));
     CK(ctx->d_odom_map.ensure(std::max<long long>(P.max_map, 1)));
-    if (set.map_voxel > 0.0) {    // the maps' filter at its largest step, so no buffer regrows inside the loop
+    if (set.map_voxel > 0.0 && !set.voxel_map) {   // the maps' filter at its largest step: no regrowth inside the loop
         CK(ctx->d_odom_map_vox.ensure(std::max<long long>(P.max_map, 1)));
         long long slots = 0;
         std::vector<long long> tab;
@@ -3232,6 +3364,13 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     bool planned = false;
     int failed = n_steps;                       // the step whose map had no dense grid
     const double inv_cell = 1.0 / set.cell_size;
+    // (voxel map) where every sequence's map is: the session's maps before the first update, then each update's output
+    odom_plan::MapState MS;
+    const float4* d_old = nullptr;
+    if (set.voxel_map) {
+        MS = odom_plan::map_start(n_seqs, n_frames, hist, sess ? sess->map_off.data() : nullptr);
+        if (sess) d_old = sess->win[sess->cur];
+    }
     for (int i = 1; i < n_steps; ++i) {
         const odom_plan::Step& st = P.steps[(size_t)i];
         const long long m = st.map_seg[(size_t)st.active];
@@ -3242,43 +3381,76 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
         const int* d_frame = ctx->d_odom_int + at_int[(size_t)i];
         const int* d_prev = d_frame + pieces;
         const int* d_prev2 = d_prev + st.active;
-        // 1. the lanes' local maps from the window frames' device-resident results and the retained frames
-        map_points_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(
-            ctx->d_scan_src, d_win, n_frames, d_dst, pieces, d_src_at, d_frame, m, ctx->d_state, d_hist_T,
-            ctx->d_odom_map);
-        ctx->launches++;
-        CK(cudaGetLastError());
-        // 1b. (map_voxel) every lane's map through the voxel filter, in world coordinates, .w re-indexed over the step's
-        // kept map points; the grids are built over those, whose offsets come back in the bounds' copy
         const float4* map = ctx->d_odom_map;
         const long long* d_mseg = d_map_seg;
+        const int64_t* h_mseg = st.map_seg.data();
         long long mk = m;
         std::vector<int64_t> kept_map;
         std::vector<int> bad_map;
         std::vector<Readback> more;
-        if (set.map_voxel > 0.0) {
-            if ((rc = voxel_filter(ctx, (const float*)ctx->d_odom_map.p, m, 4, d_map_seg, st.map_seg.data(), st.active,
-                                   set.map_voxel, (float*)ctx->d_odom_map_vox.p, 4, nullptr, set.map_max_points)))
-                return rc;
-            map = ctx->d_odom_map_vox;
-            d_mseg = ctx->d_vox_seg;
-            kept_map.resize((size_t)st.active + 1);
-            bad_map.resize((size_t)st.active);
-            more = {Readback{ctx->d_vox_seg.p, kept_map.size() * sizeof(int64_t), kept_map.data()},
-                    Readback{ctx->d_vox_bad.p, bad_map.size() * sizeof(int), bad_map.data()}};
+        odom_plan::MapStep ms;
+        std::string why, who = frame_name(st.seq[0], P.input[(size_t)st.first]);
+        if (set.voxel_map) {
+            // 1. (voxel map) one update: every lane's map becomes its previous one with frame k-1 inserted at its pose,
+            // capped and pruned (with a session, every other sequence's map is carried along); the grids are built over
+            // the lanes' part of the output, whose offsets come back in the bounds' copy
+            odom_plan::map_step(P, i, sess != nullptr, MS, &ms);
+            if (ms.seg.back() > arena_plan::kMaxPoints) {
+                why = "the maps of its step and their new frames hold " + std::to_string(ms.seg.back()) +
+                      " points, more than " + std::to_string(arena_plan::kMaxPoints) + " (int32 indexing)";
+            } else {
+                DevBuf<float4>& out = ctx->d_vmap[i % 2];
+                if ((rc = map_update(ctx, set, ms, n_frames, d_hist_T, d_old, out))) return rc;
+                map = out;
+                d_mseg = ctx->d_vox_seg;
+                h_mseg = ms.seg.data();
+                kept_map.resize(ms.seq.size() + 1);
+                bad_map.resize(ms.seq.size());
+                more = {Readback{ctx->d_vox_seg.p, kept_map.size() * sizeof(int64_t), kept_map.data()},
+                        Readback{ctx->d_vox_bad.p, bad_map.size() * sizeof(int), bad_map.data()}};
+            }
+        } else {
+            // 1. the lanes' local maps from the window frames' device-resident results and the retained frames
+            map_points_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(
+                ctx->d_scan_src, d_win, n_frames, d_dst, pieces, d_src_at, d_frame, m, ctx->d_state, d_hist_T,
+                ctx->d_odom_map);
+            ctx->launches++;
+            CK(cudaGetLastError());
+            // 1b. (map_voxel) every lane's map through the voxel filter, in world coordinates, .w re-indexed over the
+            // step's kept map points; the grids are built over those, whose offsets come back in the bounds' copy
+            if (set.map_voxel > 0.0) {
+                if ((rc = voxel_filter(ctx, (const float*)ctx->d_odom_map.p, m, 4, d_map_seg, st.map_seg.data(), st.active,
+                                       set.map_voxel, (float*)ctx->d_odom_map_vox.p, 4, nullptr, set.map_max_points)))
+                    return rc;
+                map = ctx->d_odom_map_vox;
+                d_mseg = ctx->d_vox_seg;
+                kept_map.resize((size_t)st.active + 1);
+                bad_map.resize((size_t)st.active);
+                more = {Readback{ctx->d_vox_seg.p, kept_map.size() * sizeof(int64_t), kept_map.data()},
+                        Readback{ctx->d_vox_bad.p, bad_map.size() * sizeof(int), bad_map.data()}};
+            }
         }
         // 2. their dense grids, one arena segment per lane (the bounds copy is the step's sync besides the loop's peeks;
         // the unfiltered map sizes bound the kept ones)
         std::vector<int> hb;
-        if ((rc = arena_bounds(ctx, ctx->odom_maps, map, st.map_seg.data(), d_mseg, st.active, inv_cell, hb, more)))
+        if (why.empty() && (rc = arena_bounds(ctx, ctx->odom_maps, map, h_mseg, d_mseg, st.active, inv_cell, hb, more)))
             return rc;
         std::vector<arena_plan::Box> boxes;
         long long cells = 0;
         int b = 0;
-        std::string why;
-        if (set.map_voxel > 0.0) {
-            while (b < st.active && !bad_map[(size_t)b]) ++b;
-            if (b < st.active) why = "its local map has a voxel coordinate of the map filter outside [-2^20, 2^20)";
+        if (why.empty() && set.map_voxel > 0.0) {
+            const int segs = (int)bad_map.size();
+            while (b < segs && !bad_map[(size_t)b]) ++b;
+            if (b < st.active) {
+                why = "its local map has a voxel coordinate of the map filter outside [-2^20, 2^20)";
+            } else if (b < segs) {        // a carried sequence's last frame (voxel map)
+                who = frame_name(ms.seq[(size_t)b], P.input[(size_t)ms.center[(size_t)b]]);
+                why = "its points at its pose have a voxel coordinate of the map filter outside [-2^20, 2^20)";
+            } else if (set.voxel_map) {
+                b = 0;
+                while (b < st.active && kept_map[(size_t)b + 1] > kept_map[(size_t)b]) ++b;
+                if (b < st.active) why = "its local map is empty: every voxel lies max_distance or more from the last pose";
+            }
             mk = kept_map[(size_t)st.active];
         }
         if (why.empty()) {
@@ -3288,9 +3460,14 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
             while (!why.empty() && b < st.active - 1 && arena_plan::box_of(hb.data() + 6 * (size_t)b, &x) == arena_plan::kDense) ++b;
         }
         if (!why.empty()) {
-            ctx->err = std::string(name) + ": " + frame_name(st.seq[(size_t)b], P.input[(size_t)(st.first + b)]) + ": " + why;
+            if (b < st.active) who = frame_name(st.seq[(size_t)b], P.input[(size_t)(st.first + b)]);
+            ctx->err = std::string(name) + ": " + who + ": " + why;
             failed = i;
             break;
+        }
+        if (set.voxel_map) {
+            odom_plan::map_commit(ms, kept_map.data(), MS);
+            d_old = map;
         }
         if ((rc = arena_fill(ctx, ctx->odom_maps, map, d_mseg, st.active, mk, boxes.data(), cells, inv_cell, rings)))
             return rc;
@@ -3332,12 +3509,46 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
         ctx->launches++;
         CK(cudaGetLastError());
     }
+    // (voxel map, sess) the final update: every sequence's map with its last frame in it, packed by sequence into the
+    // session's other buffer, so the session's own maps stay as they were until the push commits; one more sync
+    std::vector<long long> map_off;
+    bool map_failed = false;
+    if (sess && set.voxel_map && failed == n_steps) {
+        odom_plan::MapStep ms;
+        odom_plan::map_step(P, n_steps, true, MS, &ms);
+        int b = 0;
+        while (ms.center[(size_t)b] < 0 || ms.center[(size_t)b] >= n_frames) ++b;    // a sequence with a pushed frame
+        std::string why;
+        if (ms.seg.back() > arena_plan::kMaxPoints) {
+            why = "the maps after the push and their new frames hold " + std::to_string(ms.seg.back()) +
+                  " points, more than " + std::to_string(arena_plan::kMaxPoints) + " (int32 indexing)";
+        } else {
+            if ((rc = map_update(ctx, set, ms, n_frames, d_hist_T, d_old, sess->win[1 - sess->cur]))) return rc;
+            map_off.resize((size_t)n_seqs + 1);
+            std::vector<int> bad((size_t)n_seqs);
+            CK(cudaMemcpyAsync(map_off.data(), ctx->d_vox_seg, map_off.size() * sizeof(long long), cudaMemcpyDeviceToHost,
+                               ctx->stream));
+            CK(cudaMemcpyAsync(bad.data(), ctx->d_vox_bad, bad.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+            CK(cudaStreamSynchronize(ctx->stream));
+            int e = 0;
+            while (e < n_seqs && !bad[(size_t)e]) ++e;
+            if (e < n_seqs) {
+                b = e;
+                why = "its points at its pose have a voxel coordinate of the map filter outside [-2^20, 2^20)";
+            }
+        }
+        if (!why.empty()) {
+            ctx->err = std::string(name) + ": " + frame_name(ms.seq[(size_t)b], P.input[(size_t)ms.center[(size_t)b]]) +
+                       ": " + why;
+            map_failed = true;
+        }
+    }
     // results in the caller's frame order; after a failed step only the frames before it, and that step's message
     const std::string err = ctx->err;
     if ((rc = finish_call(ctx, params, n_frames, dlog, R, P.dev.data(),
                           failed < n_steps ? P.steps[(size_t)failed].first : n_frames)))
         return rc;
-    if (failed < n_steps) { ctx->err = err; return DCREG_BAD_ARG; }
+    if (failed < n_steps || map_failed) { ctx->err = err; return DCREG_BAD_ARG; }
     if (deskewed_xyz) {         // the frames' kept (deskewed) points, put in the caller's frame order
         std::vector<float4> h((size_t)std::max<long long>(n_points, 1));
         CK(cudaMemcpyAsync(h.data(), ctx->d_scan_src, (size_t)n_points * sizeof(float4), cudaMemcpyDeviceToHost,
@@ -3352,7 +3563,10 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
             }
         }
     }
-    if (sess) commit_push(*sess, U, n_frames, seq_offsets, R.T_out, deltas);
+    if (sess) {
+        commit_push(*sess, U, n_frames, seq_offsets, R.T_out, deltas);
+        if (set.voxel_map) sess->map_off.swap(map_off);
+    }
     return DCREG_OK;
 }
 
@@ -3408,25 +3622,101 @@ int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params
                         deskewed_xyz);
 }
 
-int dcreg_odometry_open(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
-                        int motion, double source_voxel, double map_voxel, int source_max_points, int map_max_points,
-                        const double* T_init) {
-    if (!ctx) return DCREG_BAD_ARG;
-    if (ctx->odom) { ctx->err = "odometry_open: a session is open already (dcreg_odometry_close it first)"; return DCREG_BAD_ARG; }
+// the settings of the voxel map (dcreg_icp_run_odometry_map, dcreg_odometry_open_map): no window
+static OdomSettings odom_map_settings(const dcreg_icp_params* params, int n_seqs, double cell_size, int motion,
+                                      double source_voxel, double map_voxel, int source_max_points, int map_max_points,
+                                      double max_distance, const double* T_init) {
+    OdomSettings set = odom_settings(params, n_seqs, cell_size, 0, motion, source_voxel, map_voxel, source_max_points,
+                                     map_max_points, T_init);
+    set.voxel_map = true;
+    set.max_distance = max_distance;
+    return set;
+}
+
+int dcreg_icp_run_odometry_map(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                               int n_frames, const float* xyz, const int64_t* frame_offsets, int stride, double cell_size,
+                               int motion, double source_voxel, double map_voxel, int source_max_points,
+                               int map_max_points, double max_distance, const double* T_init, const double* deltas,
+                               const float* timestamps, int64_t* frame_points, double* T_prior, double* T_out,
+                               int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
+                               dcreg_iter_log* log, int log_cap) {
+    return run_odometry(ctx, "icp_run_odometry_map",
+                        odom_map_settings(params, n_seqs, cell_size, motion, source_voxel, map_voxel, source_max_points,
+                                          map_max_points, max_distance, T_init),
+                        nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
+                        Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
+                        deskewed_xyz);
+}
+
+// Opens the context's one session with the settings `set` (dcreg_odometry_open, _open_map)
+static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& set) {
+    if (ctx->odom) {
+        ctx->err = std::string(name) + ": a session is open already (dcreg_odometry_close it first)";
+        return DCREG_BAD_ARG;
+    }
     std::unique_ptr<dcreg_ctx::OdomSession> ss(new dcreg_ctx::OdomSession());
-    ss->set = odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel, source_max_points,
-                            map_max_points, T_init);
-    BatchCheck c{"odometry_open", !ss->set.T_init.empty(), "null pointer or n_seqs <= 0",
+    ss->set = set;
+    const int n_seqs = set.n_seqs;
+    BatchCheck c{name, !ss->set.T_init.empty(), "null pointer or n_seqs <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_seqs};
-    c.own_cell = true; c.cell_size = cell_size; c.need_target = false; c.one_iteration = true;
+    c.own_cell = true; c.cell_size = set.cell_size; c.need_target = false; c.one_iteration = true;
     c.own_msg = odometry_settings_error(ss->set, false);
     const int rc = check_batch_call(ctx, &ss->set.params, c);
     if (rc) return rc;
     ss->hist = odom_plan::History(n_seqs);
+    ss->map_off.assign((size_t)n_seqs + 1, 0);
     ss->last_delta.assign((size_t)n_seqs * 16, 0.0);
     for (int s = 0; s < n_seqs; ++s)
         for (int c4 = 0; c4 < 4; ++c4) ss->last_delta[(size_t)s * 16 + 5 * c4] = 1.0;
     ctx->odom = std::move(ss);
+    return DCREG_OK;
+}
+
+int dcreg_odometry_open(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
+                        int motion, double source_voxel, double map_voxel, int source_max_points, int map_max_points,
+                        const double* T_init) {
+    if (!ctx) return DCREG_BAD_ARG;
+    return open_session(ctx, "odometry_open",
+                        odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
+                                      source_max_points, map_max_points, T_init));
+}
+
+int dcreg_odometry_open_map(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int motion,
+                            double source_voxel, double map_voxel, int source_max_points, int map_max_points,
+                            double max_distance, const double* T_init) {
+    if (!ctx) return DCREG_BAD_ARG;
+    return open_session(ctx, "odometry_open_map",
+                        odom_map_settings(params, n_seqs, cell_size, motion, source_voxel, map_voxel, source_max_points,
+                                          map_max_points, max_distance, T_init));
+}
+
+int dcreg_odometry_local_map(dcreg_ctx* ctx, int seq, float* xyz, int64_t cap, int64_t* n) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!ctx->odom) { ctx->err = "odometry_local_map: no session is open (dcreg_odometry_open_map)"; return DCREG_BAD_ARG; }
+    const dcreg_ctx::OdomSession& ss = *ctx->odom;
+    if (!ss.set.voxel_map) {
+        ctx->err = "odometry_local_map: the session keeps a window of frames, not a voxel map (dcreg_odometry_open_map)";
+        return DCREG_BAD_ARG;
+    }
+    if (!n || seq < 0 || seq >= ss.set.n_seqs) {
+        ctx->err = "odometry_local_map: null n, or seq outside [0, n_seqs)";
+        return DCREG_BAD_ARG;
+    }
+    const long long a = ss.map_off[(size_t)seq], m = ss.map_off[(size_t)seq + 1] - a;
+    *n = m;
+    if (cap < m || (m > 0 && !xyz)) {
+        ctx->err = "odometry_local_map: sequence " + std::to_string(seq) + "'s map has " + std::to_string(m) +
+                   " points, more than cap = " + std::to_string(cap) + " (or xyz is null)";
+        return DCREG_BAD_ARG;
+    }
+    if (m == 0) return DCREG_OK;
+    CK(cudaSetDevice(ctx->device));
+    std::vector<float4> h((size_t)m);
+    CK(cudaMemcpyAsync(h.data(), ss.win[ss.cur].p + a, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (long long i = 0; i < m; ++i) {
+        xyz[3 * i] = h[(size_t)i].x; xyz[3 * i + 1] = h[(size_t)i].y; xyz[3 * i + 2] = h[(size_t)i].z;
+    }
     return DCREG_OK;
 }
 

@@ -161,4 +161,99 @@ inline std::string make_push(int n_seqs, const int* seq_off, int n_frames, const
     return std::string();
 }
 
+// ---- the voxel map (dcreg_icp_run_odometry_map, dcreg_odometry_open_map) -------------------------------------------
+// Instead of a window, every sequence carries one map from frame to frame, KISS-ICP's VoxelHashMap: after frame k is
+// registered, M_{k+1} = prune(cap(M_k ++ map_points(T_out[k], frame k)), t_k).  make_push then runs with map_frames = 0:
+// the history keeps the motion model's two poses and no points, and the steps have no window pieces.  Instead, before
+// its registrations, step i >= 1 runs one map update over segments: segment b is [the current map of its sequence | the
+// sequence's last frame, when that frame is not in the map yet], capped and pruned at the pose of that last frame.  The
+// segments are the step's lanes in lane order (so the first `active` segments of the update's output are the lanes'
+// maps, as the grids need them), then, with `carry`, every other sequence with a map or a frame to insert, ascending, so
+// that the update's output holds every map and the previous one can be overwritten.  The final update (i = n_steps,
+// after the last registration) has one segment per sequence in sequence order: a session's maps after the push.  The
+// sizes come back from the device after every update (map_commit), so the layout of a step is only known at that step.
+struct MapState {
+    std::vector<long long> at, n;       // [n_seqs] sequence s's map: points [at[s], at[s] + n[s]) of the last update's output
+    std::vector<int> last;              // [n_seqs] frame reference of its last frame so far (-1: none)
+    std::vector<char> pending;          // [n_seqs] that frame is not in the map yet
+};
+
+struct MapStep {
+    std::vector<int> seq;               // [segs] sequence of segment b (the lanes first)
+    std::vector<int> center;            // [segs] the frame reference whose pose prunes segment b (-1: an empty segment)
+    std::vector<int64_t> seg;           // [segs + 1] segment b is points [seg[b], seg[b + 1]) of the update's input
+    std::vector<long long> piece_dst;   // [pieces + 1] where each piece goes in the update's input
+    std::vector<long long> piece_src;   // [pieces] its first point: in the old maps, or in the push's packed frames
+    std::vector<int> piece_frame;       // [pieces] -1: an old map, copied; else the pushed frame, under its pose
+};
+
+// The maps before a push: map_off[n_seqs + 1], the session's maps packed by sequence (null: every map empty); h: the
+// history before the push (a sequence's last frame is its last retained frame, already in its map)
+inline MapState map_start(int n_seqs, int n_frames, const History& h, const long long* map_off) {
+    MapState ms;
+    ms.at.assign((size_t)n_seqs, 0);
+    ms.n.assign((size_t)n_seqs, 0);
+    ms.last.assign((size_t)n_seqs, -1);
+    ms.pending.assign((size_t)n_seqs, 0);
+    for (int s = 0; s < n_seqs; ++s) {
+        if (map_off) { ms.at[(size_t)s] = map_off[s]; ms.n[(size_t)s] = map_off[s + 1] - map_off[s]; }
+        if (h.off[(size_t)s + 1] > h.off[(size_t)s]) ms.last[(size_t)s] = n_frames + h.off[(size_t)s + 1] - 1;
+    }
+    return ms;
+}
+
+// The update before step i of plan p (1 <= i < steps), or the final update (i = steps)
+inline void map_step(const Plan& p, int i, bool carry, MapState& ms, MapStep* out) {
+    MapStep& m = *out;
+    m = MapStep{};
+    const int n_seqs = (int)ms.at.size(), n_steps = (int)p.steps.size();
+    const Step& pv = p.steps[(size_t)i - 1];        // its frames are now their sequences' last frames, not in the maps
+    for (int j = 0; j < pv.active; ++j) {
+        ms.last[(size_t)pv.seq[(size_t)j]] = pv.first + j;
+        ms.pending[(size_t)pv.seq[(size_t)j]] = 1;
+    }
+    if (i < n_steps) {
+        m.seq = p.steps[(size_t)i].seq;
+        if (carry) {
+            std::vector<char> lane((size_t)n_seqs, 0);
+            for (int s : m.seq) lane[(size_t)s] = 1;
+            for (int s = 0; s < n_seqs; ++s)
+                if (!lane[(size_t)s] && (ms.n[(size_t)s] > 0 || ms.pending[(size_t)s])) m.seq.push_back(s);
+        }
+    } else {
+        for (int s = 0; s < n_seqs; ++s) m.seq.push_back(s);
+    }
+    m.seg.push_back(0);
+    m.piece_dst.push_back(0);
+    long long at = 0;
+    for (int s : m.seq) {
+        const int r = ms.last[(size_t)s];
+        if (ms.n[(size_t)s] > 0) {
+            m.piece_src.push_back(ms.at[(size_t)s]);
+            m.piece_frame.push_back(-1);
+            at += ms.n[(size_t)s];
+            m.piece_dst.push_back(at);
+        }
+        if (ms.pending[(size_t)s]) {
+            m.piece_src.push_back(p.dev_off[(size_t)r]);
+            m.piece_frame.push_back(r);
+            at += p.dev_off[(size_t)r + 1] - p.dev_off[(size_t)r];
+            m.piece_dst.push_back(at);
+        }
+        m.center.push_back(at > m.seg.back() ? r : -1);
+        m.seg.push_back(at);
+    }
+}
+
+// After the update m ran: kept[segs + 1], its output's offsets; every sequence of m has its map there, its last frame in
+// it.  A sequence that is not in m keeps its state (a one-shot call without carry never reads it again).
+inline void map_commit(const MapStep& m, const int64_t* kept, MapState& ms) {
+    for (size_t b = 0; b < m.seq.size(); ++b) {
+        const int s = m.seq[b];
+        ms.at[(size_t)s] = kept[b];
+        ms.n[(size_t)s] = kept[b + 1] - kept[b];
+        ms.pending[(size_t)s] = 0;
+    }
+}
+
 }  // namespace odom_plan

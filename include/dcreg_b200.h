@@ -397,6 +397,38 @@ int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params
                                   const float* timestamps, int64_t* frame_points, double* T_prior, double* T_out,
                                   int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
                                   dcreg_iter_log* log, int log_cap);
+/* dcreg_icp_run_odometry_deskew with a PERSISTENT VOXEL MAP per sequence instead of the window of map_frames frames
+ * (KISS-ICP's VoxelHashMap): the map is carried from frame to frame, so it covers the space around the sensor rather than
+ * the last W frames.  Same arguments, without map_frames, plus max_distance; timestamps and deskewed_xyz may be NULL
+ * (NULL timestamps: no deskewing, as in dcreg_icp_run_odometry_voxel_n).
+ * - Update: U(M, P, T) = prune(cap(M ++ map_points(T, P)), t_T), with cap(X) = dcreg_voxel_downsample_n(X, map_voxel,
+ *   map_max_points) (each voxel keeps its map_max_points points of smallest index, bit for bit, in order: M comes first,
+ *   so older points win, KISS-ICP's AddPoints) and prune(X, t) dropping every point of every voxel whose first point q
+ *   has ((qx - tx)^2 + (qy - ty)^2) + (qz - tz)^2 >= max_distance^2 (KISS-ICP's RemovePointsFarFromLocation), in FP64
+ *   from the float32 coordinates, one rounding per operation, no FMA, max_distance^2 = max_distance * max_distance in
+ *   FP64.  Survivors keep their order.  dcreg_b200.api.voxel_map_update gives the same bits.
+ * - Maps: M_1 = U(empty, F_s(anchor), T_init[s]), M_{k+1} = U(M_k, F_s(frame k), T_out[k]): every frame goes in at the
+ *   pose it returned, aborted ones included, deskewed when timestamps are given.  Frame k registers against M_k and
+ *   returns what dcreg_set_target(M_k, cell_size) + dcreg_set_source(F_s(frame k)) + dcreg_icp_run(T_prior[k]) returns,
+ *   up to how the FP64 partial sums are grouped; priors, anchors, deskewing, covariances and logs as in
+ *   dcreg_icp_run_odometry_deskew.
+ * - max_distance = +inf prunes nothing; then, since cap(cap(A) ++ B) = cap(A ++ B), M_k is the window map of
+ *   dcreg_icp_run_odometry_deskew with map_frames >= the longest sequence, and every output is the same bytes.
+ * - Cost per step: one launch that lays out [old map | new frame] for every sequence, the capped filter and one prune
+ *   launch, whatever the number of sequences; the new maps' sizes come back in the copy of the grids' bounds, so a step
+ *   keeps its one host sync.  Buffers are sized from the sizes read back so far and grow with headroom.
+ * Errors (DCREG_BAD_ARG before anything is launched): map_voxel not finite and > 0, map_max_points < 1, max_distance NaN
+ * or <= 0 (+inf is allowed); everything else as in dcreg_icp_run_odometry_deskew.  At its step (dcreg_last_error naming
+ * the sequence and frame; the earlier steps keep their outputs, the context stays usable): a map with no dense grid, an
+ * empty map (every voxel pruned), a map voxel coordinate outside [-2^20, 2^20), more than 2^29 - 1 map points over a
+ * step's sequences. */
+int dcreg_icp_run_odometry_map(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                               int n_frames, const float* xyz, const int64_t* frame_offsets, int stride, double cell_size,
+                               int motion, double source_voxel, double map_voxel, int source_max_points,
+                               int map_max_points, double max_distance, const double* T_init, const double* deltas,
+                               const float* timestamps, int64_t* frame_points, double* T_prior, double* T_out,
+                               int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
+                               dcreg_iter_log* log, int log_cap);
 /* ODOMETRY SESSION: scan-to-map odometry of S sequences fed as the frames arrive.  The session keeps each sequence's
  * last map_frames registered frames (their filtered points in sensor coordinates and their poses) on the device
  * between pushes, with the motion model's state, so no frame is uploaded or filtered twice.
@@ -445,6 +477,23 @@ int dcreg_odometry_push_deskew(dcreg_ctx* ctx, const int* seq_offsets, int n_fra
                                const int64_t* frame_offsets, int stride, const double* deltas, const float* timestamps,
                                int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
                                int* status, double* cov, float* deskewed_xyz, dcreg_iter_log* log, int log_cap);
+/* dcreg_odometry_open for the voxel map of dcreg_icp_run_odometry_map: the settings of that call (no map_frames; the
+ * same checks), and dcreg_odometry_push / _push_deskew push onto it unchanged.  The session keeps every sequence's map
+ * (its last frame already in it) and the motion model's two last poses on the device; the contract carries over: any
+ * chunking gives byte for byte the outputs of one dcreg_icp_run_odometry_map call over the recording, and a push that
+ * fails (also at its step: a map with no dense grid, an empty map, a voxel coordinate out of range, too many points)
+ * commits nothing.  One exception to the contract: the 2^29 - 1 point limit counts an update's whole input, which in a
+ * session also holds the maps carried along (in the push's final update, every sequence's map), so near that limit a
+ * session can fail a push that the one call over the same recording accepts.  Cost: a push's steps as in the one call, with the maps of the sequences without a frame at a step
+ * carried through its update, plus one final update that puts the push's last frames in their maps (one more sync). */
+int dcreg_odometry_open_map(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int motion,
+                            double source_voxel, double map_voxel, int source_max_points, int map_max_points,
+                            double max_distance, const double* T_init);
+/* The current voxel map of sequence seq of the session dcreg_odometry_open_map opened: M after the sequence's last
+ * committed frame (empty before its first), copied to the HOST as 3 floats per point in map order.  *n always receives
+ * its size; a cap below it (or a null xyz for a non-empty map) is DCREG_BAD_ARG and writes nothing else.  DCREG_BAD_ARG
+ * also without a session, for a window session, a null n or a seq outside [0, n_seqs). */
+int dcreg_odometry_local_map(dcreg_ctx* ctx, int seq, float* xyz, int64_t cap, int64_t* n);
 int dcreg_odometry_close(dcreg_ctx* ctx);
 /* Voxel downsampling of many clouds in one call (KISS-ICP's VoxelDownsample rule: the first point of every voxel).
  * xyz / offsets / stride: HOST memory as in dcreg_icp_run_scans (n_clouds + 1 offsets, ascending strictly from 0, at
