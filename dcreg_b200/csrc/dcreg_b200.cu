@@ -1011,22 +1011,29 @@ __device__ __forceinline__ void ref_pose(int r, int n_frames, const IcpState* __
     }
 }
 
-// The local maps of one step: m points in all, piece p (a window frame) being map points [dst[p], dst[p+1]) = the points
-// src_at[p] .. of the frame's packed input (input order) under the frame's final pose, both by its frame reference
-// frame[p].  Every coordinate is ((r0 x + r1 y) + r2 z) + t in FP64, one rounding per operation, then one float32
-// rounding (dcreg_b200.api.map_points gives the same bits); w = the point's index over the step's maps, as a packed
-// target.
-__global__ void map_points_kernel(const float4* __restrict__ src, const float4* __restrict__ win, int n_frames,
-                                  const long long* __restrict__ dst, int pieces, const long long* __restrict__ src_at,
-                                  const int* __restrict__ frame, long long m, const IcpState* __restrict__ states,
-                                  const double* __restrict__ hist_T, float4* __restrict__ out) {
+// The maps of one step, or the input of one voxel-map update (odom_plan::MapInput): m points in all, piece p being map
+// points [dst[p], dst[p+1]) = the points src_at[p] .. of frame reference r = frame[p]: an old voxel map copied from `old`
+// (r < 0), or a frame's packed input (input order) under its final pose (ref_pose).  Every transformed coordinate is
+// ((r0 x + r1 y) + r2 z) + t in FP64, one rounding per operation, then one float32 rounding (dcreg_b200.api.map_points
+// gives the same bits); w = the point's index over the maps, as a packed target.
+__global__ void map_points_kernel(const float4* __restrict__ src, const float4* __restrict__ win,
+                                  const float4* __restrict__ old, int n_frames, const long long* __restrict__ dst,
+                                  int pieces, const long long* __restrict__ src_at, const int* __restrict__ frame,
+                                  long long m, const IcpState* __restrict__ states, const double* __restrict__ hist_T,
+                                  float4* __restrict__ out) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
     const int p = corr::segment_of(dst, pieces, i);
     const int r = frame[p];
+    const long long at = src_at[p] + (i - dst[p]);
+    if (r < 0) {
+        const float4 q = old[at];
+        out[i] = make_float4(q.x, q.y, q.z, __int_as_float((int)i));
+        return;
+    }
     double R[9], t[3];
     ref_pose(r, n_frames, states, hist_T, R, t);
-    const float4 q = (r < n_frames ? src : win)[src_at[p] + (i - dst[p])];
+    const float4 q = (r < n_frames ? src : win)[at];
     const double x = q.x, y = q.y, z = q.z;
     float v[3];
 #pragma unroll
@@ -1092,35 +1099,6 @@ __global__ void retain_points_kernel(const float4* __restrict__ src, const float
 }
 
 // ---- the voxel map (dcreg_icp_run_odometry_map, dcreg_odometry_open_map; odom_plan::map_step) ----------------------
-// The input of one map update: m points in `pieces` pieces, piece p being out[dst[p], dst[p+1]): an old map copied from
-// `old` (frame[p] < 0), or the packed points src_at[p] .. of pushed frame frame[p] under its final pose, with the
-// arithmetic of map_points_kernel (the same bits).  w = the point's index in the input.
-__global__ void map_update_input_kernel(const float4* __restrict__ src, const float4* __restrict__ old,
-                                        const long long* __restrict__ dst, int pieces, const long long* __restrict__ src_at,
-                                        const int* __restrict__ frame, long long m, const IcpState* __restrict__ states,
-                                        float4* __restrict__ out) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    const int p = corr::segment_of(dst, pieces, i);
-    const int r = frame[p];
-    const long long at = src_at[p] + (i - dst[p]);
-    if (r < 0) {
-        const float4 q = old[at];
-        out[i] = make_float4(q.x, q.y, q.z, __int_as_float((int)i));
-        return;
-    }
-    const IcpState* st = states + r;
-    const float4 q = src[at];
-    const double x = q.x, y = q.y, z = q.z;
-    float v[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c)
-        v[c] = (float)__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(st->R[3 * c], x), __dmul_rn(st->R[3 * c + 1], y)),
-                                          __dmul_rn(st->R[3 * c + 2], z)),
-                                st->t[c]);
-    out[i] = make_float4(v[0], v[1], v[2], __int_as_float((int)i));
-}
-
 // The voxel map's prune, between the voxel filter's flag pass and its scan (KISS-ICP's RemovePointsFarFromLocation): a
 // kept point i whose voxel's first point q (first[slot_of[i]], the voxel's smallest index) has ((qx - tx)^2 + (qy -
 // ty)^2) + (qz - tz)^2 >= max_d2 is dropped, in FP64 from the float32 coordinates with one rounding per operation.  t:
@@ -1255,7 +1233,8 @@ constexpr int kNcclSum = 0;
 // context
 // ------------------------------------------------------------------------------------------------
 // A grow-only allocation with one owner: ensure(n) reallocates, at exactly n elements, only when the capacity is below
-// n (the old contents are lost), and the destructor frees it.  kPinned: page-locked host memory.
+// n (the old contents are lost), and the destructor frees it; grow(n) reallocates with a quarter of headroom, for sizes
+// that follow results.  kPinned: page-locked host memory.
 template <typename T, bool kPinned = false>
 struct DevBuf {
     T* p = nullptr;
@@ -1280,6 +1259,7 @@ struct DevBuf {
         if (e == cudaSuccess) { p = (T*)q; cap = n; }
         return e;
     }
+    cudaError_t grow(long long n) { return cap >= n ? cudaSuccess : ensure(n + n / 4); }
 };
 template <typename T>
 using PinnedBuf = DevBuf<T, true>;
@@ -1357,12 +1337,12 @@ struct dcreg_ctx {
     // frame ranges [lanes] / [lanes + 1], increments and priors [frames][16]
     DevBuf<int> d_seq_cursor, d_seq_first;
     DevBuf<double> d_seq_delta, d_seq_prior;
-    // odometry (dcreg_icp_run_odometry): every step's tables (odom_plan.hpp) in one upload, the step's local maps, and
-    // their grids in an arena of their own
+    // odometry (dcreg_icp_run_odometry): every step's tables (odom_plan.hpp) in one upload, the step's local maps (or a
+    // voxel-map update's input), and their grids in an arena of their own
     DevBuf<long long> d_odom_ll; DevBuf<int> d_odom_int;
-    DevBuf<float4> d_odom_map, d_odom_map_vox;                         // ... and the maps after the voxel filter
-    // the voxel map: one update's tables (odom_plan::MapStep; its input goes to d_odom_map), and the updates' outputs,
-    // step after step in turns (an update reads the previous one's)
+    DevBuf<float4> d_odom_map;
+    // the voxel map: one update's tables (odom_plan::MapInput), uploaded per update.  The maps after the voxel filter:
+    // a window's in d_vmap[0], the voxel map's updates in turns (an update reads the previous one's output)
     DevBuf<long long> d_vmap_ll; DevBuf<int> d_vmap_int;
     DevBuf<float4> d_vmap[2];
     // motion compensation (dcreg_icp_run_odometry_deskew): the caller's timestamps [input points], the packed points'
@@ -3088,51 +3068,126 @@ static const char* odometry_settings_error(const OdomSettings& set, bool deltas)
     return nullptr;
 }
 
-// One update of the voxel maps (odom_plan::map_step): its input, [old map | new frame] per segment, in d_odom_map, then
-// the capped voxel filter with the prune into `out`, the kept offsets in ctx->d_vox_seg and the range flags in
-// ctx->d_vox_bad.  The buffers grow with headroom, since the maps' sizes follow the results.  No host sync; the input
-// launch and the filter's, one more for the prune, whatever the number of sequences.
-static int map_update(dcreg_ctx* ctx, const OdomSettings& set, const odom_plan::MapStep& ms, int n_frames,
-                      const double* d_hist_T, const float4* d_old, DevBuf<float4>& out) {
-    const int segs = (int)ms.seq.size(), pieces = (int)ms.piece_frame.size();
-    const long long m = ms.seg[(size_t)segs];
-    // long long seg [segs + 1], piece_dst [pieces + 1], piece_src [pieces]; int piece_frame [pieces], center [segs]
-    std::vector<long long> hll(ms.seg.begin(), ms.seg.end());
-    hll.insert(hll.end(), ms.piece_dst.begin(), ms.piece_dst.end());
-    hll.insert(hll.end(), ms.piece_src.begin(), ms.piece_src.end());
-    std::vector<int> hint(ms.piece_frame.begin(), ms.piece_frame.end());
-    hint.insert(hint.end(), ms.center.begin(), ms.center.end());
-    auto grow = [](auto& b, long long need) { return b.cap >= need ? cudaSuccess : b.ensure(need + need / 4); };
-    CK(grow(ctx->d_vmap_ll, (long long)hll.size()));
-    CK(grow(ctx->d_vmap_int, std::max<long long>((long long)hint.size(), 1)));
-    CK(grow(ctx->d_odom_map, std::max<long long>(m, 1)));
-    CK(grow(out, std::max<long long>(m, 1)));
-    CK(cudaMemcpyAsync(ctx->d_vmap_ll, hll.data(), hll.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
-    if (!hint.empty())
-        CK(cudaMemcpyAsync(ctx->d_vmap_int, hint.data(), hint.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-    const long long* d_seg = ctx->d_vmap_ll;
-    const long long* d_dst = d_seg + segs + 1;
-    const int* d_frame = ctx->d_vmap_int;
+// A step's maps (or a session's final voxel-map update): segment b is points [d_seg[b], d_seg[b + 1]) of `map` (null:
+// not built); with a map filter its kept offsets and range flags come back with the next copy of `more`
+struct StepMap {
+    const float4* map = nullptr;
+    const long long* d_seg = nullptr;
+    std::vector<int64_t> kept;          // (map filter) [segs + 1]
+    std::vector<int> bad;               // (map filter) [segs]
+    std::vector<Readback> more;
+};
+
+// One odometry call or push (run_odometry): its arguments, what its phases share, and the phases, in the order they run
+struct OdomCall {
+    dcreg_ctx* ctx; const char* name; const OdomSettings& set; dcreg_ctx::OdomSession* sess;
+    const int* seq_offsets; int n_frames; const float* xyz; const int64_t* frame_offsets; int stride;
+    const double* deltas; const float* timestamps; const Results& R; int64_t* frame_points; float* deskewed_xyz;
+    const int n_seqs = set.n_seqs;
+    const dcreg_icp_params* params = &set.params;
+    odom_plan::History none;                        // a one-shot call's history, once check() has validated n_seqs
+    const odom_plan::History& hist = sess ? sess->hist : none;
+    // the frames as the device gets them: the caller's, or the source filter's kept points (src_off: kept offsets)
+    const float* src_xyz = xyz; int src_stride = stride; const int64_t* src_off = frame_offsets;
+    std::vector<int64_t> kept;
+    odom_plan::Push U;
+    const odom_plan::Plan& P = U.plan;
+    // where the tables are in d_odom_ll / d_odom_int: step i's map's (odom_plan::pack), then its int prev, prev2; the
+    // retain step's and the timestamp gather's
+    std::vector<size_t> at_ll, at_int;
+    size_t keep_ll = 0, keep_int = 0, ts_ll = 0;
+    Batch S{};
+    const double* d_delta = nullptr;                // one increment per frame reference (null: every one the identity)
+    const double* d_hist_T = nullptr;               // the retained frames' poses and points (null: none)
+    const float4* d_win = nullptr;
+    dcreg_iter_log* dlog = nullptr; const float4* src_iter = nullptr;
+    LoopPlan L; bool planned = false;
+    int failed = -1;                                // the step whose maps failed (-1: none)
+    // (voxel map) where every sequence's map is: the session's maps before the first update, then each update's output
+    odom_plan::MapState MS;
+    const float4* d_old = nullptr;
+
+    int check(), upload(), start(), step(int i), finish();
+    int build_map(const odom_plan::MapInput& in, const long long* ll, const int* ints, DevBuf<float4>& out, StepMap* sm);
+
+    // "sequence s, frame k (frame j of the sequence)": the caller's frame k, j-th of sequence s in the call, or its
+    // number since the session opened
+    std::string frame_name(int s, int k) const {
+        const int j = k - seq_offsets[s];
+        if (!sess)
+            return "sequence " + std::to_string(s) + ", frame " + std::to_string(k) + " (frame " + std::to_string(j) +
+                   " of the sequence)";
+        return "sequence " + std::to_string(s) + ", frame " + std::to_string(k) + " of the push (frame " +
+               std::to_string(hist.seen[(size_t)s] + j) + " of the sequence since open)";
+    }
+    // odom_plan::map_failure's reason, if any, into ctx->err: segment `b` of `in`, a lane of step st or (st null) a
+    // session's final update
+    bool map_failed(const odom_plan::MapInput& in, const odom_plan::Step* st, const std::string& why, int b) {
+        if (why.empty()) return false;
+        const int d = st && b < st->active ? st->first + b : in.center[(size_t)b];
+        ctx->err = std::string(name) + ": " + frame_name(in.seq[(size_t)b], P.input[(size_t)d]) + ": " + why;
+        return true;
+    }
+};
+
+// The maps of `in`, its tables on the device at ll / ints (null: a voxel-map update's, whose sizes follow the last
+// update's results, packed and uploaded here): map_points_kernel into d_odom_map, then with a map filter the capped
+// voxel filter into `out`, pruned in the voxel map.  The buffers grow with headroom (a window reserved them for its
+// largest step).  An input over arena_plan::kMaxPoints is not built (odom_plan::map_failure names it).  No sync.
+int OdomCall::build_map(const odom_plan::MapInput& in, const long long* ll, const int* ints, DevBuf<float4>& out,
+                        StepMap* sm) {
+    const int segs = (int)in.seq.size(), pieces = (int)in.piece_frame.size();
+    const long long m = in.seg.back();
+    const bool filter = set.map_voxel > 0.0;
+    int rc;
+    if (m > arena_plan::kMaxPoints) return DCREG_OK;
+    if (!ll) {
+        std::vector<long long> hll;
+        std::vector<int> hint;
+        odom_plan::pack(in, hll, hint);
+        CK(ctx->d_vmap_ll.grow((long long)hll.size()));
+        CK(ctx->d_vmap_int.grow(std::max<long long>((long long)hint.size(), 1)));
+        CK(cudaMemcpyAsync(ctx->d_vmap_ll, hll.data(), hll.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
+        if (!hint.empty())
+            CK(cudaMemcpyAsync(ctx->d_vmap_int, hint.data(), hint.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
+        ll = ctx->d_vmap_ll;
+        ints = ctx->d_vmap_int;
+    }
+    CK(ctx->d_odom_map.grow(std::max<long long>(m, 1)));
+    if (filter) CK(out.grow(std::max<long long>(m, 1)));
     if (m == 0) {           // no map and no frame to insert anywhere
         CK(ctx->d_vox_seg.ensure(segs + 1));
         CK(ctx->d_vox_bad.ensure(std::max(segs, 1)));
         CK(cudaMemsetAsync(ctx->d_vox_seg, 0, (size_t)(segs + 1) * sizeof(long long), ctx->stream));
         CK(cudaMemsetAsync(ctx->d_vox_bad, 0, (size_t)segs * sizeof(int), ctx->stream));
-        return DCREG_OK;
+    } else {
+        std::vector<long long> tab;
+        const long long slots = filter ? voxel_tables(segs, in.seg.data(), tab) : 0;
+        if (filter && (ctx->d_vox_slot.cap < m || ctx->d_vox_keys.cap < slots ||
+                       (set.map_max_points > 1 && ctx->d_vox_skey.cap < 2 * m)) &&
+            (rc = voxel_reserve(ctx, m + m / 4, n_seqs, slots + slots / 4, set.map_max_points)))
+            return rc;
+        const long long* d_dst = ll + segs + 1;
+        map_points_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(
+            ctx->d_scan_src, d_win, d_old, n_frames, d_dst, pieces, d_dst + pieces + 1, ints, m, ctx->d_state, d_hist_T,
+            ctx->d_odom_map);
+        ctx->launches++;
+        CK(cudaGetLastError());
+        const VoxelPrune prune{ints + pieces, n_frames, ctx->d_state, d_hist_T, set.max_distance * set.max_distance};
+        if (filter && (rc = voxel_filter(ctx, (const float*)ctx->d_odom_map.p, m, 4, ll, in.seg.data(), segs,
+                                         set.map_voxel, (float*)out.p, 4, nullptr, set.map_max_points,
+                                         in.center.empty() ? nullptr : &prune)))
+            return rc;
     }
-    std::vector<long long> tab;
-    const long long slots = voxel_tables(segs, ms.seg.data(), tab);
-    if (ctx->d_vox_slot.cap < m || ctx->d_vox_keys.cap < slots || (set.map_max_points > 1 && ctx->d_vox_skey.cap < 2 * m)) {
-        const int rc = voxel_reserve(ctx, m + m / 4, set.n_seqs, slots + slots / 4, set.map_max_points);
-        if (rc) return rc;
+    sm->map = filter ? out.p : ctx->d_odom_map.p;
+    sm->d_seg = filter ? ctx->d_vox_seg.p : ll;
+    if (filter) {
+        sm->kept.resize((size_t)segs + 1);
+        sm->bad.resize((size_t)segs);
+        sm->more = {Readback{ctx->d_vox_seg.p, sm->kept.size() * sizeof(int64_t), sm->kept.data()},
+                    Readback{ctx->d_vox_bad.p, sm->bad.size() * sizeof(int), sm->bad.data()}};
     }
-    map_update_input_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(
-        ctx->d_scan_src, d_old, d_dst, pieces, d_dst + pieces + 1, d_frame, m, ctx->d_state, ctx->d_odom_map);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    const VoxelPrune prune{d_frame + pieces, n_frames, ctx->d_state, d_hist_T, set.max_distance * set.max_distance};
-    return voxel_filter(ctx, (const float*)ctx->d_odom_map.p, m, 4, d_seg, ms.seg.data(), segs, set.map_voxel,
-                        (float*)out.p, 4, nullptr, set.map_max_points, &prune);
+    return DCREG_OK;
 }
 
 // A push that succeeded becomes the session's state: the history after it, the retained frames' poses (the T_out bytes
@@ -3156,18 +3211,9 @@ static void commit_push(dcreg_ctx::OdomSession& ss, const odom_plan::Push& u, in
     ss.cur = 1 - ss.cur;
 }
 
-// Every odometry entry point: the frames continue the sequences of a history (odom_plan::History), whose retained
-// frames act as anchors outside the call: they are not registered and return nothing, their points come from the
-// window buffer and their poses from the session, and their last increments continue the deltas.  A one-shot call
-// (sess null) runs on the empty history, where every sequence starts.  A push (sess) runs on the session's: a sequence
-// may have no frame, frames are named by their number in the sequence since the session opened, the retain step
-// gathers the next window, and only a push that succeeds changes the session (commit_push).
-static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& set, dcreg_ctx::OdomSession* sess,
-                        const int* seq_offsets, int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
-                        const double* deltas, const float* timestamps, const Results& R, int64_t* frame_points,
-                        float* deskewed_xyz) {
-    if (!ctx) return DCREG_BAD_ARG;
-    const int n_seqs = set.n_seqs;
+// The call and its frames: the timestamps, and the frames' voxel filter (once per call, on the staged points in input
+// order, before the pack and the sort; one sync for the kept counts).  From here on a frame is its kept points
+int OdomCall::check() {
     BatchCheck c{name, !set.T_init.empty() && n_frames > 0 && seq_offsets && xyz && frame_offsets && R.T_out,
                  "null pointer, n_seqs <= 0 or n_frames <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_frames};
@@ -3175,22 +3221,10 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     c.need_target = false; c.one_iteration = true; c.n_seqs = n_seqs; c.seq_offsets = seq_offsets;
     c.empty_seqs = sess != nullptr;
     c.own_msg = odometry_settings_error(set, deltas != nullptr);
-    const dcreg_icp_params* params = &set.params;
     int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
+    if (!sess) none = odom_plan::History(n_seqs);
     CK(cudaSetDevice(ctx->device));
-    const odom_plan::History none(sess ? 0 : n_seqs);
-    const odom_plan::History& hist = sess ? sess->hist : none;
-    // "sequence s, frame k (frame j of the sequence)": the caller's frame k, j-th of sequence s in the call, or its
-    // number since the session opened
-    auto frame_name = [&](int s, int k) {
-        const int j = k - seq_offsets[s];
-        if (!sess)
-            return "sequence " + std::to_string(s) + ", frame " + std::to_string(k) + " (frame " + std::to_string(j) +
-                   " of the sequence)";
-        return "sequence " + std::to_string(s) + ", frame " + std::to_string(k) + " of the push (frame " +
-               std::to_string(hist.seen[(size_t)s] + j) + " of the sequence since open)";
-    };
     if (timestamps)             // every point's fraction of its sweep, before anything is launched
         for (int s = 0; s < n_seqs; ++s)
             for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k)
@@ -3202,12 +3236,6 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
                                (std::isfinite(tau) ? std::to_string(tau) + ", outside [0, 1]" : std::string("not finite"));
                     return DCREG_BAD_ARG;
                 }
-    // the frames' voxel filter: once per call, on the staged points in input order, before the pack and the sort; one
-    // sync for the kept counts.  From here on a frame is its kept points, on the device
-    const float* src_xyz = xyz;
-    int src_stride = stride;
-    const int64_t* src_off = frame_offsets;
-    std::vector<int64_t> kept;
     if (set.source_voxel > 0.0) {
         kept.resize((size_t)n_frames + 1);
         std::vector<int> bad((size_t)n_frames);
@@ -3228,8 +3256,13 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     }
     if (frame_points)
         for (int k = 0; k < n_frames; ++k) frame_points[k] = src_off[k + 1] - src_off[k];
-    odom_plan::Push U;
-    odom_plan::Plan& P = U.plan;
+    return DCREG_OK;
+}
+
+// The plan, and what the steps read that is known before them: every step's tables in one upload, the frames, the
+// increments, the retained frames' poses, and room for the largest step's maps and (sess) the next window
+int OdomCall::upload() {
+    int rc;
     {
         const std::string why = odom_plan::make_push(n_seqs, seq_offsets, n_frames, src_off,
                                                      set.voxel_map ? 0 : set.map_frames, arena_plan::kMaxPoints, hist, &U);
@@ -3237,31 +3270,25 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     }
     const int n_steps = (int)P.steps.size();
     const int n_hist = (int)hist.n.size();
-    // every step's tables in one upload: long long map_seg [A + 1], piece_dst [P + 1], piece_src [P]; int piece_frame
-    // [P], prev [A], prev2 [A] (A lanes, P window frames)
     std::vector<long long> hll;
     std::vector<int> hint;
-    std::vector<size_t> at_ll((size_t)n_steps, 0), at_int((size_t)n_steps, 0);
+    at_ll.assign((size_t)n_steps, 0); at_int.assign((size_t)n_steps, 0);
     for (int i = 1; i < n_steps; ++i) {
         const odom_plan::Step& st = P.steps[(size_t)i];
         at_ll[(size_t)i] = hll.size(); at_int[(size_t)i] = hint.size();
-        hll.insert(hll.end(), st.map_seg.begin(), st.map_seg.end());
-        hll.insert(hll.end(), st.piece_dst.begin(), st.piece_dst.end());
-        hll.insert(hll.end(), st.piece_src.begin(), st.piece_src.end());
-        hint.insert(hint.end(), st.piece_frame.begin(), st.piece_frame.end());
+        odom_plan::pack(st.map, hll, hint);
         hint.insert(hint.end(), st.prev.begin(), st.prev.end());
         hint.insert(hint.end(), st.prev2.begin(), st.prev2.end());
     }
     // (sess) then the retain step's: long long keep_dst [K + 1], keep_src [K]; int keep_ref [K]
-    const size_t keep_ll = hll.size(), keep_int = hint.size();
-    const int keep = sess ? (int)U.keep_ref.size() : 0;
+    keep_ll = hll.size(); keep_int = hint.size();
     if (sess) {
         hll.insert(hll.end(), U.keep_dst.begin(), U.keep_dst.end());
         hll.insert(hll.end(), U.keep_src.begin(), U.keep_src.end());
         hint.insert(hint.end(), U.keep_ref.begin(), U.keep_ref.end());
     }
     // (timestamps) then the timestamp gather's: long long in_at [n_frames], kept_at [n_frames] (odom_ts_gather_kernel)
-    const size_t ts_ll = hll.size();
+    ts_ll = hll.size();
     if (timestamps) {
         for (int d = 0; d < n_frames; ++d) hll.push_back(frame_offsets[P.input[(size_t)d]]);
         for (int d = 0; d < n_frames; ++d) hll.push_back(src_off[P.input[(size_t)d]]);
@@ -3269,7 +3296,7 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     // the frames in device order, each sorted by its own cell in the sensor frame (identity poses, a box of 1024^3 cells
     // around the sensor: locality only, the chained priors are not known yet); lanes: grid y of the loop kernel, a
     // lane's frame range set by odom_start_kernel at every step; grids: the step's local maps
-    Batch S{n_frames, src_xyz, src_stride, P.dev_off.data()};
+    S = Batch{n_frames, src_xyz, src_stride, P.dev_off.data()};
     S.order = P.input.data(); S.in_off = src_off;
     if (set.source_voxel > 0.0) S.kind = cudaMemcpyDeviceToDevice;
     S.sort = Batch::kBox;
@@ -3285,28 +3312,19 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     CK(ctx->d_odom_int.ensure(std::max<long long>((long long)hint.size(), 1)));
     CK(ctx->d_odom_map.ensure(std::max<long long>(P.max_map, 1)));
     if (set.map_voxel > 0.0 && !set.voxel_map) {   // the maps' filter at its largest step: no regrowth inside the loop
-        CK(ctx->d_odom_map_vox.ensure(std::max<long long>(P.max_map, 1)));
+        CK(ctx->d_vmap[0].ensure(std::max<long long>(P.max_map, 1)));
         long long slots = 0;
         std::vector<long long> tab;
         for (int i = 1; i < n_steps; ++i)
-            slots = std::max(slots, voxel_tables(P.steps[(size_t)i].active, P.steps[(size_t)i].map_seg.data(), tab));
+            slots = std::max(slots, voxel_tables(P.steps[(size_t)i].active, P.steps[(size_t)i].map.seg.data(), tab));
         if ((rc = voxel_reserve(ctx, P.max_map, n_seqs, slots, set.map_max_points))) return rc;
     }
     if (!hll.empty()) {
         CK(cudaMemcpyAsync(ctx->d_odom_ll, hll.data(), hll.size() * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaMemcpyAsync(ctx->d_odom_int, hint.data(), hint.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     }
-    // device order: every frame's loop state starts at its sequence's T_init (an anchor keeps it: T_out = T_prior =
-    // T_init, no iteration, not converged)
-    std::vector<double> T_dev((size_t)n_frames * 16), ident((size_t)n_frames * 16, 0.0);
-    for (int s = 0; s < n_seqs; ++s)
-        for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k)
-            memcpy(&T_dev[(size_t)P.dev[(size_t)k] * 16], &set.T_init[(size_t)s * 16], 16 * sizeof(double));
-    for (int d = 0; d < n_frames; ++d)
-        for (int c4 = 0; c4 < 4; ++c4) ident[(size_t)d * 16 + 5 * c4] = 1.0;
     // one increment per frame reference: the frames' (identity without deltas), then the retained frames' (a sequence's
     // last one carries the increment its push left; only a session retains frames); null: every increment is the identity
-    const double* d_delta = nullptr;
     if (set.motion == DCREG_MOTION_INCREMENTS && (deltas || n_hist > 0)) {
         std::vector<double> D_dev((size_t)(n_frames + n_hist) * 16, 0.0);
         for (int e = 0; e < n_frames + n_hist; ++e)
@@ -3326,8 +3344,6 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     // the retained frames' poses and points (none on the empty history: nothing reads them), and (sess) room for the
     // next window, grown with headroom: a window whose frames vary in size does not reallocate (and synchronise) at
     // every push
-    const double* d_hist_T = nullptr;
-    const float4* d_win = nullptr;
     if (n_hist) {
         CK(sess->d_hist_T.ensure((long long)n_hist * 16));
         CK(cudaMemcpyAsync(sess->d_hist_T, sess->hist_T.data(), (size_t)n_hist * 16 * sizeof(double),
@@ -3335,16 +3351,22 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
         d_hist_T = sess->d_hist_T;
         d_win = sess->win[sess->cur];
     }
-    if (sess) {
-        DevBuf<float4>& nxt = sess->win[1 - sess->cur];
-        const long long need = std::max<long long>(U.keep_dst.back(), 1);
-        if (nxt.cap < need) CK(nxt.ensure(need + need / 4));
-    }
+    if (sess) CK(sess->win[1 - sess->cur].grow(std::max<long long>(U.keep_dst.back(), 1)));
+    return DCREG_OK;
+}
+
+// The loop's start: every frame's loop state at its sequence's T_init (device order; an anchor keeps it: T_out = T_prior
+// = T_init, no iteration, not converged), and (timestamps) the caller's timestamps beside the packed points
+int OdomCall::start() {
+    int rc;
+    std::vector<double> T_dev((size_t)n_frames * 16), ident((size_t)n_frames * 16, 0.0);
+    for (int s = 0; s < n_seqs; ++s)
+        for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k)
+            memcpy(&T_dev[(size_t)P.dev[(size_t)k] * 16], &set.T_init[(size_t)s * 16], 16 * sizeof(double));
+    for (int d = 0; d < n_frames; ++d)
+        for (int c4 = 0; c4 < 4; ++c4) ident[(size_t)d * 16 + 5 * c4] = 1.0;
     CK(cudaMemcpyAsync(ctx->d_seq_prior, ident.data(), ident.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-    dcreg_iter_log* dlog = nullptr;
-    const float4* src_iter = nullptr;
     if ((rc = start_loop(ctx, n_frames, T_dev.data(), R, &S, &dlog, &src_iter))) return rc;
-    // (timestamps) the caller's timestamps beside the packed points, once per call; the twists of a step's lanes
     const long long n_points = P.dev_off[(size_t)n_frames];
     if (timestamps) {
         CK(ctx->d_odom_ts_in.ensure(std::max<long long>(frame_offsets[n_frames], 1)));
@@ -3359,197 +3381,120 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
         ctx->launches++;
         CK(cudaGetLastError());
     }
-    const int rings = search_rings(params->search_radius, set.cell_size);
-    LoopPlan L;
-    bool planned = false;
-    int failed = n_steps;                       // the step whose map had no dense grid
-    const double inv_cell = 1.0 / set.cell_size;
-    // (voxel map) where every sequence's map is: the session's maps before the first update, then each update's output
-    odom_plan::MapState MS;
-    const float4* d_old = nullptr;
     if (set.voxel_map) {
         MS = odom_plan::map_start(n_seqs, n_frames, hist, sess ? sess->map_off.data() : nullptr);
         if (sess) d_old = sess->win[sess->cur];
     }
-    for (int i = 1; i < n_steps; ++i) {
-        const odom_plan::Step& st = P.steps[(size_t)i];
-        const long long m = st.map_seg[(size_t)st.active];
-        const int pieces = (int)st.piece_frame.size();
-        const long long* d_map_seg = ctx->d_odom_ll + at_ll[(size_t)i];
-        const long long* d_dst = d_map_seg + st.active + 1;
-        const long long* d_src_at = d_dst + pieces + 1;
-        const int* d_frame = ctx->d_odom_int + at_int[(size_t)i];
-        const int* d_prev = d_frame + pieces;
-        const int* d_prev2 = d_prev + st.active;
-        const float4* map = ctx->d_odom_map;
-        const long long* d_mseg = d_map_seg;
-        const int64_t* h_mseg = st.map_seg.data();
-        long long mk = m;
-        std::vector<int64_t> kept_map;
-        std::vector<int> bad_map;
-        std::vector<Readback> more;
-        odom_plan::MapStep ms;
-        std::string why, who = frame_name(st.seq[0], P.input[(size_t)st.first]);
-        if (set.voxel_map) {
-            // 1. (voxel map) one update: every lane's map becomes its previous one with frame k-1 inserted at its pose,
-            // capped and pruned (with a session, every other sequence's map is carried along); the grids are built over
-            // the lanes' part of the output, whose offsets come back in the bounds' copy
-            odom_plan::map_step(P, i, sess != nullptr, MS, &ms);
-            if (ms.seg.back() > arena_plan::kMaxPoints) {
-                why = "the maps of its step and their new frames hold " + std::to_string(ms.seg.back()) +
-                      " points, more than " + std::to_string(arena_plan::kMaxPoints) + " (int32 indexing)";
-            } else {
-                DevBuf<float4>& out = ctx->d_vmap[i % 2];
-                if ((rc = map_update(ctx, set, ms, n_frames, d_hist_T, d_old, out))) return rc;
-                map = out;
-                d_mseg = ctx->d_vox_seg;
-                h_mseg = ms.seg.data();
-                kept_map.resize(ms.seq.size() + 1);
-                bad_map.resize(ms.seq.size());
-                more = {Readback{ctx->d_vox_seg.p, kept_map.size() * sizeof(int64_t), kept_map.data()},
-                        Readback{ctx->d_vox_bad.p, bad_map.size() * sizeof(int), bad_map.data()}};
-            }
-        } else {
-            // 1. the lanes' local maps from the window frames' device-resident results and the retained frames
-            map_points_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(
-                ctx->d_scan_src, d_win, n_frames, d_dst, pieces, d_src_at, d_frame, m, ctx->d_state, d_hist_T,
-                ctx->d_odom_map);
-            ctx->launches++;
-            CK(cudaGetLastError());
-            // 1b. (map_voxel) every lane's map through the voxel filter, in world coordinates, .w re-indexed over the
-            // step's kept map points; the grids are built over those, whose offsets come back in the bounds' copy
-            if (set.map_voxel > 0.0) {
-                if ((rc = voxel_filter(ctx, (const float*)ctx->d_odom_map.p, m, 4, d_map_seg, st.map_seg.data(), st.active,
-                                       set.map_voxel, (float*)ctx->d_odom_map_vox.p, 4, nullptr, set.map_max_points)))
-                    return rc;
-                map = ctx->d_odom_map_vox;
-                d_mseg = ctx->d_vox_seg;
-                kept_map.resize((size_t)st.active + 1);
-                bad_map.resize((size_t)st.active);
-                more = {Readback{ctx->d_vox_seg.p, kept_map.size() * sizeof(int64_t), kept_map.data()},
-                        Readback{ctx->d_vox_bad.p, bad_map.size() * sizeof(int), bad_map.data()}};
-            }
-        }
-        // 2. their dense grids, one arena segment per lane (the bounds copy is the step's sync besides the loop's peeks;
-        // the unfiltered map sizes bound the kept ones)
-        std::vector<int> hb;
-        if (why.empty() && (rc = arena_bounds(ctx, ctx->odom_maps, map, h_mseg, d_mseg, st.active, inv_cell, hb, more)))
+    return DCREG_OK;
+}
+
+// Step i >= 1; when its maps fail, ctx->err names the frame, `failed` the step, and nothing of it runs
+int OdomCall::step(int i) {
+    const odom_plan::Step& st = P.steps[(size_t)i];
+    int rc;
+    // 1. the lanes' local maps from the window frames' device-resident results and the retained frames, or (voxel map)
+    // one update: every lane's map becomes its previous one with frame k-1 inserted at its pose, capped and pruned (with
+    // a session, every other sequence's map is carried along); then the map filter, if any
+    odom_plan::MapInput update;
+    const odom_plan::MapInput& in = set.voxel_map ? update : st.map;
+    if (set.voxel_map) odom_plan::map_step(P, i, sess != nullptr, MS, &update);
+    StepMap sm;
+    if ((rc = set.voxel_map ? build_map(update, nullptr, nullptr, ctx->d_vmap[i % 2], &sm)
+                            : build_map(st.map, ctx->d_odom_ll + at_ll[(size_t)i], ctx->d_odom_int + at_int[(size_t)i],
+                                        ctx->d_vmap[0], &sm)))
+        return rc;
+    // 2. their dense grids, one arena segment per lane (the bounds copy is the step's sync besides the loop's peeks, and
+    // brings the filter's kept offsets back; the unfiltered map sizes bound the kept ones)
+    const double inv_cell = 1.0 / set.cell_size;
+    std::vector<int> hb;
+    std::vector<arena_plan::Box> boxes;
+    long long cells = 0;
+    std::string plan_why;
+    if (sm.map) {
+        if ((rc = arena_bounds(ctx, ctx->odom_maps, sm.map, in.seg.data(), sm.d_seg, st.active, inv_cell, hb, sm.more)))
             return rc;
-        std::vector<arena_plan::Box> boxes;
-        long long cells = 0;
-        int b = 0;
-        if (why.empty() && set.map_voxel > 0.0) {
-            const int segs = (int)bad_map.size();
-            while (b < segs && !bad_map[(size_t)b]) ++b;
-            if (b < st.active) {
-                why = "its local map has a voxel coordinate of the map filter outside [-2^20, 2^20)";
-            } else if (b < segs) {        // a carried sequence's last frame (voxel map)
-                who = frame_name(ms.seq[(size_t)b], P.input[(size_t)ms.center[(size_t)b]]);
-                why = "its points at its pose have a voxel coordinate of the map filter outside [-2^20, 2^20)";
-            } else if (set.voxel_map) {
-                b = 0;
-                while (b < st.active && kept_map[(size_t)b + 1] > kept_map[(size_t)b]) ++b;
-                if (b < st.active) why = "its local map is empty: every voxel lies max_distance or more from the last pose";
-            }
-            mk = kept_map[(size_t)st.active];
-        }
-        if (why.empty()) {
-            why = arena_plan::plan(st.active, hb.data(), boxes, &cells, "local map of lane");
-            b = 0;
-            arena_plan::Box x;
-            while (!why.empty() && b < st.active - 1 && arena_plan::box_of(hb.data() + 6 * (size_t)b, &x) == arena_plan::kDense) ++b;
-        }
-        if (!why.empty()) {
-            if (b < st.active) who = frame_name(st.seq[(size_t)b], P.input[(size_t)(st.first + b)]);
-            ctx->err = std::string(name) + ": " + who + ": " + why;
-            failed = i;
-            break;
-        }
-        if (set.voxel_map) {
-            odom_plan::map_commit(ms, kept_map.data(), MS);
-            d_old = map;
-        }
-        if ((rc = arena_fill(ctx, ctx->odom_maps, map, d_mseg, st.active, mk, boxes.data(), cells, inv_cell, rings)))
-            return rc;
-        // 3. every lane's frame of this step: its prior and a fresh loop state
-        odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
-            ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
-            st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T);
-        ctx->launches++;
-        CK(cudaGetLastError());
-        // 3b. (timestamps) the step's frames deskewed with the increments their priors used, outside the loop's graphs
-        if (timestamps) {
-            odom_twist_kernel<<<(unsigned)((st.active + 127) / 128), 128, 0, ctx->stream>>>(
-                ctx->d_state, st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T,
-                ctx->d_odom_xi, ctx->d_scan_radius);
-            const long long a = P.dev_off[(size_t)st.first], np = P.dev_off[(size_t)(st.first + st.active)] - a;
-            odom_deskew_kernel<<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
-                ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_seg, st.first, st.active, a, np, ctx->d_odom_ts,
-                ctx->d_odom_xi, ctx->d_scan_radius);
-            ctx->launches += 2;
-            CK(cudaGetLastError());
-        }
-        // 4. the loop: the same chunks (and CUDA graphs) at every step - the grid table keeps its pointer (the first step
-        // has the most lanes, so the arena's table never regrows after it), only its entries change
-        if (!planned) {
-            S.grids = ctx->odom_maps.d_grids;
-            if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? R.log_cap : 0, true, &L, &S))) return rc;
-            planned = true;
-        }
-        if ((rc = run_chunks(ctx, L, params, dlog, dlog ? R.log_cap : 0, params->max_iterations, 16, true))) return rc;
+        plan_why = arena_plan::plan(st.active, hb.data(), boxes, &cells, "local map of lane");
     }
-    // (sess) the next window: the retained frames' packed points, gathered from this push's frames and the old window
-    // into the other buffer, so the session's own window stays as it was until the push commits
+    int b = 0;
+    const std::string why = odom_plan::map_failure(in, st.active, n_frames, arena_plan::kMaxPoints, sm.bad, sm.kept, hb,
+                                                   plan_why, &b);
+    if (map_failed(in, &st, why, b)) {
+        failed = i;
+        return DCREG_OK;
+    }
+    if (set.voxel_map) {
+        odom_plan::map_commit(update, sm.kept.data(), MS);
+        d_old = sm.map;
+    }
+    const long long m = sm.kept.empty() ? in.seg[(size_t)st.active] : sm.kept[(size_t)st.active];
+    if ((rc = arena_fill(ctx, ctx->odom_maps, sm.map, sm.d_seg, st.active, m, boxes.data(), cells, inv_cell,
+                         search_rings(params->search_radius, set.cell_size))))
+        return rc;
+    // 3. every lane's frame of this step: its prior and a fresh loop state
+    const int* d_prev = ctx->d_odom_int + at_int[(size_t)i] + st.map.piece_frame.size() + st.map.center.size();
+    const int* d_prev2 = d_prev + st.active;
+    odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
+        ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
+        st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    // 3b. (timestamps) the step's frames deskewed with the increments their priors used, outside the loop's graphs
+    if (timestamps) {
+        odom_twist_kernel<<<(unsigned)((st.active + 127) / 128), 128, 0, ctx->stream>>>(
+            ctx->d_state, st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T,
+            ctx->d_odom_xi, ctx->d_scan_radius);
+        const long long a = P.dev_off[(size_t)st.first], np = P.dev_off[(size_t)(st.first + st.active)] - a;
+        odom_deskew_kernel<<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
+            ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_seg, st.first, st.active, a, np, ctx->d_odom_ts,
+            ctx->d_odom_xi, ctx->d_scan_radius);
+        ctx->launches += 2;
+        CK(cudaGetLastError());
+    }
+    // 4. the loop: the same chunks (and CUDA graphs) at every step - the grid table keeps its pointer (the first step
+    // has the most lanes, so the arena's table never regrows after it), only its entries change
+    if (!planned) {
+        S.grids = ctx->odom_maps.d_grids;
+        if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? R.log_cap : 0, true, &L, &S))) return rc;
+        planned = true;
+    }
+    return run_chunks(ctx, L, params, dlog, dlog ? R.log_cap : 0, params->max_iterations, 16, true);
+}
+
+// After the steps: (sess) the next window, and (voxel map) the final update, every sequence's map with its last frame
+// in it, packed by sequence (one more sync), both into the session's other buffer, so its own stays as it was until
+// the push commits; then the results in the caller's frame order (after a failed step only the frames before it, and
+// that step's message), the deskewed points, the commit
+int OdomCall::finish() {
+    int rc;
     const long long kept_points = sess ? U.keep_dst.back() : 0;
-    if (sess && failed == n_steps && kept_points > 0) {
+    if (sess && failed < 0 && kept_points > 0) {
         const long long* d_keep_dst = ctx->d_odom_ll + keep_ll;
+        const int keep = (int)U.keep_ref.size();
         retain_points_kernel<<<(unsigned)((kept_points + 255) / 256), 256, 0, ctx->stream>>>(
             ctx->d_scan_src, sess->win[sess->cur], n_frames, d_keep_dst, keep, d_keep_dst + keep + 1,
             ctx->d_odom_int + keep_int, kept_points, sess->win[1 - sess->cur]);
         ctx->launches++;
         CK(cudaGetLastError());
     }
-    // (voxel map, sess) the final update: every sequence's map with its last frame in it, packed by sequence into the
-    // session's other buffer, so the session's own maps stay as they were until the push commits; one more sync
-    std::vector<long long> map_off;
-    bool map_failed = false;
-    if (sess && set.voxel_map && failed == n_steps) {
-        odom_plan::MapStep ms;
-        odom_plan::map_step(P, n_steps, true, MS, &ms);
+    StepMap sm;
+    bool update_failed = false;
+    if (sess && set.voxel_map && failed < 0) {
+        odom_plan::MapInput in;
+        odom_plan::map_step(P, (int)P.steps.size(), true, MS, &in);
+        if ((rc = build_map(in, nullptr, nullptr, sess->win[1 - sess->cur], &sm))) return rc;
+        for (const Readback& r : sm.more) CK(cudaMemcpyAsync(r.host, r.dev, r.bytes, cudaMemcpyDeviceToHost, ctx->stream));
+        if (sm.map) CK(cudaStreamSynchronize(ctx->stream));
         int b = 0;
-        while (ms.center[(size_t)b] < 0 || ms.center[(size_t)b] >= n_frames) ++b;    // a sequence with a pushed frame
-        std::string why;
-        if (ms.seg.back() > arena_plan::kMaxPoints) {
-            why = "the maps after the push and their new frames hold " + std::to_string(ms.seg.back()) +
-                  " points, more than " + std::to_string(arena_plan::kMaxPoints) + " (int32 indexing)";
-        } else {
-            if ((rc = map_update(ctx, set, ms, n_frames, d_hist_T, d_old, sess->win[1 - sess->cur]))) return rc;
-            map_off.resize((size_t)n_seqs + 1);
-            std::vector<int> bad((size_t)n_seqs);
-            CK(cudaMemcpyAsync(map_off.data(), ctx->d_vox_seg, map_off.size() * sizeof(long long), cudaMemcpyDeviceToHost,
-                               ctx->stream));
-            CK(cudaMemcpyAsync(bad.data(), ctx->d_vox_bad, bad.size() * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-            CK(cudaStreamSynchronize(ctx->stream));
-            int e = 0;
-            while (e < n_seqs && !bad[(size_t)e]) ++e;
-            if (e < n_seqs) {
-                b = e;
-                why = "its points at its pose have a voxel coordinate of the map filter outside [-2^20, 2^20)";
-            }
-        }
-        if (!why.empty()) {
-            ctx->err = std::string(name) + ": " + frame_name(ms.seq[(size_t)b], P.input[(size_t)ms.center[(size_t)b]]) +
-                       ": " + why;
-            map_failed = true;
-        }
+        const std::string why = odom_plan::map_failure(in, 0, n_frames, arena_plan::kMaxPoints, sm.bad, sm.kept, {}, "", &b);
+        update_failed = map_failed(in, nullptr, why, b);
     }
-    // results in the caller's frame order; after a failed step only the frames before it, and that step's message
     const std::string err = ctx->err;
     if ((rc = finish_call(ctx, params, n_frames, dlog, R, P.dev.data(),
-                          failed < n_steps ? P.steps[(size_t)failed].first : n_frames)))
+                          failed >= 0 ? P.steps[(size_t)failed].first : n_frames)))
         return rc;
-    if (failed < n_steps || map_failed) { ctx->err = err; return DCREG_BAD_ARG; }
+    if (failed >= 0 || update_failed) { ctx->err = err; return DCREG_BAD_ARG; }
     if (deskewed_xyz) {         // the frames' kept (deskewed) points, put in the caller's frame order
+        const long long n_points = P.dev_off[(size_t)n_frames];
         std::vector<float4> h((size_t)std::max<long long>(n_points, 1));
         CK(cudaMemcpyAsync(h.data(), ctx->d_scan_src, (size_t)n_points * sizeof(float4), cudaMemcpyDeviceToHost,
                            ctx->stream));
@@ -3565,9 +3510,29 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     }
     if (sess) {
         commit_push(*sess, U, n_frames, seq_offsets, R.T_out, deltas);
-        if (set.voxel_map) sess->map_off.swap(map_off);
+        if (set.voxel_map) sess->map_off.assign(sm.kept.begin(), sm.kept.end());
     }
     return DCREG_OK;
+}
+
+// Every odometry entry point: the frames continue the sequences of a history (odom_plan::History), whose retained
+// frames act as anchors outside the call: they are not registered and return nothing, their points come from the
+// window buffer and their poses from the session, and their last increments continue the deltas.  A one-shot call
+// (sess null) runs on the empty history, where every sequence starts.  A push (sess) runs on the session's: a sequence
+// may have no frame, frames are named by their number in the sequence since the session opened, the retain step
+// gathers the next window, and only a push that succeeds changes the session (commit_push).
+static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& set, dcreg_ctx::OdomSession* sess,
+                        const int* seq_offsets, int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                        const double* deltas, const float* timestamps, const Results& R, int64_t* frame_points,
+                        float* deskewed_xyz) {
+    if (!ctx) return DCREG_BAD_ARG;
+    OdomCall o{ctx, name, set, sess, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps, R,
+               frame_points, deskewed_xyz};
+    int rc;
+    if ((rc = o.check()) || (rc = o.upload()) || (rc = o.start())) return rc;
+    for (int i = 1; i < (int)o.P.steps.size() && o.failed < 0; ++i)
+        if ((rc = o.step(i))) return rc;
+    return o.finish();
 }
 
 int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,

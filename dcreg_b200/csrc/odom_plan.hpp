@@ -7,33 +7,58 @@
 // frames of step i are [Step::first, Step::first + Step::active), one per lane, the lanes in ascending sequence order.
 // So a step's frames are one contiguous lane table, and the loop's frame cursor stops at the end of a lane's only frame.
 // The map of frame k (since its sequence started) is the window frames [max(0, k - map_frames), k) of its sequence in
-// ascending order, each frame's points in their input order; the lanes' maps follow each other in one buffer.
-// Everything here is plain C++ so tests/test_odom_plan.py and tests/test_odom_session_plan.py can check it on the CPU
-// (tools/test_odom_plan.cpp, tools/test_odom_session_plan.cpp).
+// ascending order, each frame's points in their input order; the lanes' maps follow each other in one buffer.  Every
+// map input, a step's windows or a voxel-map update's, is one piece table (MapInput), which map_points_kernel lays out.
+// Everything here is plain C++ so tests/test_odom_plan.py, tests/test_odom_session_plan.py and
+// tests/test_odom_map_plan.py can check it on the CPU (tools/test_odom_*plan.cpp).
 #pragma once
 #include <algorithm>
 #include <cstdint>
 #include <string>
 #include <vector>
 
+#include "arena_plan.hpp"
+
 namespace odom_plan {
+
+// A piece table: segment b (one map) is points [seg[b], seg[b + 1]) of the input, piece p (a run of points) is points
+// [piece_dst[p], piece_dst[p + 1]) = points piece_src[p] .. of frame reference r = piece_frame[p] (see Push) under its
+// final pose, or, for r = -1, of the last voxel-map update's output, copied.
+struct MapInput {
+    std::vector<int> seq;               // [segs] sequence of segment b (a step's lanes first, in lane order)
+    std::vector<int> center;            // [segs] (voxel map) the frame reference whose pose prunes segment b (-1: empty)
+    std::vector<int64_t> seg = {0};     // [segs + 1]
+    std::vector<long long> piece_dst = {0};     // [pieces + 1]
+    std::vector<long long> piece_src;   // [pieces]
+    std::vector<int> piece_frame;       // [pieces]
+    void add_piece(long long src, int r, long long n) {
+        piece_src.push_back(src); piece_frame.push_back(r); piece_dst.push_back(piece_dst.back() + n);
+    }
+    void end_segment(int s) { seq.push_back(s); seg.push_back(piece_dst.back()); }
+};
+
+// A piece table's device layout, appended: long long seg, piece_dst, piece_src; int piece_frame, center
+inline void pack(const MapInput& in, std::vector<long long>& ll, std::vector<int>& ints) {
+    ll.insert(ll.end(), in.seg.begin(), in.seg.end());
+    ll.insert(ll.end(), in.piece_dst.begin(), in.piece_dst.end());
+    ll.insert(ll.end(), in.piece_src.begin(), in.piece_src.end());
+    ints.insert(ints.end(), in.piece_frame.begin(), in.piece_frame.end());
+    ints.insert(ints.end(), in.center.begin(), in.center.end());
+}
 
 struct Step {
     int first = 0;                      // device index of the step's first frame; lane j runs first + j
     int active = 0;                     // lanes: the sequences with a frame at this step
     std::vector<int> seq;               // [active] sequence of lane j
     std::vector<int> prev, prev2;       // [active] device index of frame k - 1, and of k - 2 (-1: k - 1 is the anchor)
-    std::vector<int64_t> map_seg;       // [active + 1] lane j's map is points [map_seg[j], map_seg[j + 1]) of the step
-    std::vector<long long> piece_dst;   // [pieces + 1] where each window frame's points go in the step's maps
-    std::vector<long long> piece_src;   // [pieces] first point of the window frame (device order)
-    std::vector<int> piece_frame;       // [pieces] device index of the window frame (its pose)
+    MapInput map;                       // the lanes' window maps, one segment per lane (the voxel map: none)
 };
 
 struct Plan {
     std::vector<int> dev;               // [n_frames] device index of input frame k
     std::vector<int> input;             // [n_frames] input frame of device index d
     std::vector<int64_t> dev_off;       // [n_frames + 1] point offsets of the frames in device order
-    std::vector<Step> steps;            // steps[0]: the anchors (no map, no pieces)
+    std::vector<Step> steps;            // steps[0]: the anchors (no map)
     long long max_map = 0;              // the most map points of one step
     int max_pieces = 0;                 // the most window frames of one step
 };
@@ -51,7 +76,7 @@ struct History {
 };
 
 // The retained frames act as anchors that are not in the push: fixed poses, not registered, no outputs.  A frame
-// reference r (Step::prev, prev2, piece_frame, and keep_ref below) is the device index of a pushed frame when
+// reference r (Step::prev, prev2, MapInput::piece_frame, and keep_ref below) is the device index of a pushed frame when
 // r < n_frames, else retained frame r - n_frames of the history; piece_src is then a point of the push's packed frames
 // or of the window buffer.  On the empty history every reference is a pushed frame.
 struct Push {
@@ -113,9 +138,6 @@ inline std::string make_push(int n_seqs, const int* seq_off, int n_frames, const
     auto first_point = [&](int r) { return r < n_frames ? p.dev_off[(size_t)r] : h.at[(size_t)(r - n_frames)]; };
     for (int i = 1; i < n_steps; ++i) {
         Step& st = p.steps[(size_t)i];
-        st.map_seg.push_back(0);
-        st.piece_dst.push_back(0);
-        long long m = 0;
         for (int j = 0; j < st.active; ++j) {
             const int s = st.seq[(size_t)j];
             const long long k = h.seen[(size_t)s] + (i - step_of(s, 0));
@@ -123,18 +145,16 @@ inline std::string make_push(int n_seqs, const int* seq_off, int n_frames, const
             st.prev2.push_back(k - 1 > 0 ? ref(s, k - 2) : -1);
             for (long long w = std::max<long long>(0, k - map_frames); w < k; ++w) {
                 const int r = ref(s, w);
-                st.piece_src.push_back(first_point(r));
-                st.piece_frame.push_back(r);
-                m += points(r);
-                st.piece_dst.push_back(m);
+                st.map.add_piece(first_point(r), r, points(r));
             }
-            st.map_seg.push_back(m);
+            st.map.end_segment(s);
         }
+        const long long m = st.map.seg.back();
         if (m > max_points)
             return "the maps of step " + std::to_string(i) + " hold " + std::to_string(m) +
                    " points, more than " + std::to_string(max_points) + " (int32 indexing)";
         p.max_map = std::max(p.max_map, m);
-        p.max_pieces = std::max(p.max_pieces, (int)st.piece_frame.size());
+        p.max_pieces = std::max(p.max_pieces, (int)st.map.piece_frame.size());
     }
     // the history after the push
     History& x = u.next;
@@ -178,15 +198,6 @@ struct MapState {
     std::vector<char> pending;          // [n_seqs] that frame is not in the map yet
 };
 
-struct MapStep {
-    std::vector<int> seq;               // [segs] sequence of segment b (the lanes first)
-    std::vector<int> center;            // [segs] the frame reference whose pose prunes segment b (-1: an empty segment)
-    std::vector<int64_t> seg;           // [segs + 1] segment b is points [seg[b], seg[b + 1]) of the update's input
-    std::vector<long long> piece_dst;   // [pieces + 1] where each piece goes in the update's input
-    std::vector<long long> piece_src;   // [pieces] its first point: in the old maps, or in the push's packed frames
-    std::vector<int> piece_frame;       // [pieces] -1: an old map, copied; else the pushed frame, under its pose
-};
-
 // The maps before a push: map_off[n_seqs + 1], the session's maps packed by sequence (null: every map empty); h: the
 // history before the push (a sequence's last frame is its last retained frame, already in its map)
 inline MapState map_start(int n_seqs, int n_frames, const History& h, const long long* map_off) {
@@ -203,57 +214,73 @@ inline MapState map_start(int n_seqs, int n_frames, const History& h, const long
 }
 
 // The update before step i of plan p (1 <= i < steps), or the final update (i = steps)
-inline void map_step(const Plan& p, int i, bool carry, MapState& ms, MapStep* out) {
-    MapStep& m = *out;
-    m = MapStep{};
+inline void map_step(const Plan& p, int i, bool carry, MapState& ms, MapInput* out) {
+    MapInput& m = *out;
+    m = MapInput{};
     const int n_seqs = (int)ms.at.size(), n_steps = (int)p.steps.size();
     const Step& pv = p.steps[(size_t)i - 1];        // its frames are now their sequences' last frames, not in the maps
     for (int j = 0; j < pv.active; ++j) {
         ms.last[(size_t)pv.seq[(size_t)j]] = pv.first + j;
         ms.pending[(size_t)pv.seq[(size_t)j]] = 1;
     }
+    std::vector<int> seq;
     if (i < n_steps) {
-        m.seq = p.steps[(size_t)i].seq;
+        seq = p.steps[(size_t)i].seq;
         if (carry) {
             std::vector<char> lane((size_t)n_seqs, 0);
-            for (int s : m.seq) lane[(size_t)s] = 1;
+            for (int s : seq) lane[(size_t)s] = 1;
             for (int s = 0; s < n_seqs; ++s)
-                if (!lane[(size_t)s] && (ms.n[(size_t)s] > 0 || ms.pending[(size_t)s])) m.seq.push_back(s);
+                if (!lane[(size_t)s] && (ms.n[(size_t)s] > 0 || ms.pending[(size_t)s])) seq.push_back(s);
         }
     } else {
-        for (int s = 0; s < n_seqs; ++s) m.seq.push_back(s);
+        for (int s = 0; s < n_seqs; ++s) seq.push_back(s);
     }
-    m.seg.push_back(0);
-    m.piece_dst.push_back(0);
-    long long at = 0;
-    for (int s : m.seq) {
+    for (int s : seq) {
         const int r = ms.last[(size_t)s];
-        if (ms.n[(size_t)s] > 0) {
-            m.piece_src.push_back(ms.at[(size_t)s]);
-            m.piece_frame.push_back(-1);
-            at += ms.n[(size_t)s];
-            m.piece_dst.push_back(at);
-        }
-        if (ms.pending[(size_t)s]) {
-            m.piece_src.push_back(p.dev_off[(size_t)r]);
-            m.piece_frame.push_back(r);
-            at += p.dev_off[(size_t)r + 1] - p.dev_off[(size_t)r];
-            m.piece_dst.push_back(at);
-        }
-        m.center.push_back(at > m.seg.back() ? r : -1);
-        m.seg.push_back(at);
+        if (ms.n[(size_t)s] > 0) m.add_piece(ms.at[(size_t)s], -1, ms.n[(size_t)s]);
+        if (ms.pending[(size_t)s]) m.add_piece(p.dev_off[(size_t)r], r, p.dev_off[(size_t)r + 1] - p.dev_off[(size_t)r]);
+        m.center.push_back(m.piece_dst.back() > m.seg.back() ? r : -1);
+        m.end_segment(s);
     }
 }
 
 // After the update m ran: kept[segs + 1], its output's offsets; every sequence of m has its map there, its last frame in
 // it.  A sequence that is not in m keeps its state (a one-shot call without carry never reads it again).
-inline void map_commit(const MapStep& m, const int64_t* kept, MapState& ms) {
+inline void map_commit(const MapInput& m, const int64_t* kept, MapState& ms) {
     for (size_t b = 0; b < m.seq.size(); ++b) {
         const int s = m.seq[b];
         ms.at[(size_t)s] = kept[b];
         ms.n[(size_t)s] = kept[b + 1] - kept[b];
         ms.pending[(size_t)s] = 0;
     }
+}
+
+// Why the maps of `in` (a step's, its first `lanes` segments the lanes', or a session's final voxel-map update, lanes =
+// 0) cannot be searched ("": they can), and the segment the message names (*at; a lane by its frame of the step, else by
+// center[b]).  From the host data, each empty when the call has none (bad[segs], kept[segs + 1]: the map filter's range
+// flags and kept offsets; hb[lanes * 6], plan_why: the grids' bounds, arena_plan::plan's result), in order: more than
+// max_points points (not built); a voxel coordinate out of range; a lane's map the prune left empty; the grids' plan.
+inline std::string map_failure(const MapInput& in, int lanes, int n_frames, long long max_points,
+                               const std::vector<int>& bad, const std::vector<int64_t>& kept, const std::vector<int>& hb,
+                               const std::string& plan_why, int* at) {
+    int& b = *at;
+    b = 0;
+    if (in.seg.back() > max_points) {
+        while (lanes == 0 && (in.center[(size_t)b] < 0 || in.center[(size_t)b] >= n_frames)) ++b;
+        return std::string(lanes > 0 ? "the maps of its step" : "the maps after the push") + " and their new frames hold " +
+               std::to_string(in.seg.back()) + " points, more than " + std::to_string(max_points) + " (int32 indexing)";
+    }
+    for (b = 0; b < (int)bad.size(); ++b)
+        if (bad[(size_t)b])
+            return b < lanes ? "its local map has a voxel coordinate of the map filter outside [-2^20, 2^20)"
+                             : "its points at its pose have a voxel coordinate of the map filter outside [-2^20, 2^20)";
+    for (b = 0; !in.center.empty() && !kept.empty() && b < lanes; ++b)
+        if (kept[(size_t)b + 1] == kept[(size_t)b])
+            return "its local map is empty: every voxel lies max_distance or more from the last pose";
+    arena_plan::Box x;
+    for (b = 0; !plan_why.empty() && b < lanes - 1 && arena_plan::box_of(hb.data() + 6 * (size_t)b, &x) == arena_plan::kDense;)
+        ++b;
+    return plan_why;
 }
 
 }  // namespace odom_plan

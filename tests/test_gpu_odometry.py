@@ -260,7 +260,7 @@ def test_odometry_bad_arguments(ctx, odo):
 
     assert call() == api.OK
     assert call(motion=1, Dd=None) == api.OK
-    bad = [dict(n_seqs=0), dict(seq_off=np.array([0, 3, 2], np.int32)), dict(seq_off=np.array([0, 0, 4], np.int32)),
+    bad = [dict(n_seqs=0), dict(n_seqs=-1), dict(seq_off=np.array([0, 3, 2], np.int32)), dict(seq_off=np.array([0, 0, 4], np.int32)),
            dict(seq_off=np.array([0, 1, 3], np.int32)),
            dict(offsets=np.array([0, off[1], off[1], off[3], off[4]], np.int64)),
            dict(map_frames=0), dict(map_frames=-2), dict(motion=2), dict(motion=-1), dict(motion=1),   # cv with deltas

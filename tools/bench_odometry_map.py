@@ -17,7 +17,8 @@ sequences: the window's from the twin, the voxel maps' from the twin's M_k), and
 poses.  Parity (exits non-zero on a mismatch): the inf arm is the window call with map_frames >= the longest sequence,
 byte for byte in T_out, T_prior, status, iterations, converged and points; every registered frame of the two finite
 voxel-map arms equals its reconstruction set_target(twin M_k) + set_source + icp_run(T_prior) (status, iterations and
-converged identical, pose <= 1e-8 on the SE(3) log).  Prints one JSON line with the card name and power limit."""
+converged identical, pose <= 1e-8 on the SE(3) log).  Prints one JSON line with the card name and power limit;
+--dump-outputs DIR writes every arm's poses, priors, flags and kept points per frame as float64 .npy files."""
 import argparse
 import json
 import math
@@ -33,6 +34,7 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 from bench_scans import card  # noqa: E402
+from bench_odometry_voxel import dump_results  # noqa: E402
 from bench_sequences import pose_errors  # noqa: E402
 
 MAP_FRAMES = 10
@@ -45,6 +47,7 @@ def main():
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--source-voxel", type=float, default=0.25)
     ap.add_argument("--small", action="store_true", help="a quick rehearsal: 2 small workloads")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     import torch
     import dcreg_oracle as o
@@ -68,6 +71,7 @@ def main():
                                                  for a, (v, c, d) in vmaps.items()},
             "n_scan": n_scan, "n_map": n_map, "workloads": {}, "card": card()}
     ok_all = True
+    dumps = {}
     with Context(0) as ctx:
         stream = torch.cuda.ExternalStream(ctx.stream)
 
@@ -156,7 +160,10 @@ def main():
                         "map_points_per_step": {"mean": float(np.mean(per_step)), "max": int(max(per_step))},
                         "max_err_vs_truth": {"trans_m": drift[0], "rot_deg": drift[1]}}
             line["workloads"][name] = w
+            dumps.update({f"{name}_{a}": res[a] for a in arms})
     print(json.dumps(line))
+    if args.dump_outputs:
+        dump_results(args.dump_outputs, "odometry_map", dumps)
     if not ok_all:
         raise SystemExit("bench_odometry_map.py: parity FAILED")
 

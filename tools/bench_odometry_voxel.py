@@ -19,7 +19,8 @@ clouds of 100 000 points in one call (host arrays in and out) against the twin o
 Parity (asserted; exits non-zero on a mismatch): every registered frame of the device arm against its reconstruction
 with the twin (set_target(filtered map, cell) + set_source(filtered frame) + icp_run(T_prior)): status, iterations and
 converged identical, pose <= 1e-8 on the SE(3) log; and the device filter's output equal to the twin's bit for bit.
-Prints one JSON line with the card name and power limit."""
+Prints one JSON line with the card name and power limit; --dump-outputs DIR writes every arm's poses, priors, flags and
+kept points per frame, and the filter's kept points and indices, as float64 .npy files."""
 import argparse
 import json
 import os
@@ -48,12 +49,21 @@ def map_sizes(seqs_sizes):
     return out
 
 
+def dump_results(path, prefix, runs):
+    """runs: {name: [OdometryResult]} -> PATH/PREFIX_NAME_{T,T_prior,iterations,converged,status,n_points}.npy"""
+    os.makedirs(path, exist_ok=True)
+    for name, res in runs.items():
+        for k in ("T", "T_prior", "iterations", "converged", "status", "n_points"):
+            np.save(os.path.join(path, f"{prefix}_{name}_{k}.npy"), np.asarray([getattr(r, k) for r in res], np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--source-voxel", type=float, default=0.25)
     ap.add_argument("--map-voxel", type=float, default=0.25)
     ap.add_argument("--small", action="store_true", help="a quick rehearsal: 2 small workloads")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     import torch
     import dcreg_oracle as o
@@ -74,6 +84,7 @@ def main():
     line = {"metric": "frames_per_s", "map_frames": MAP_FRAMES, "source_voxel": sv, "map_voxel": mv,
             "n_scan": n_scan, "n_map": n_map, "workloads": {}, "card": card()}
     ok_all = True
+    dumps = {}
     with Context(0) as ctx:
         stream = torch.cuda.ExternalStream(ctx.stream)
 
@@ -159,6 +170,7 @@ def main():
                         "map_points_per_step": {"mean": float(np.mean(maps[a])), "max": int(max(maps[a]))},
                         "max_err_vs_truth": {"trans_m": drift[0], "rot_deg": drift[1]}}
             line["workloads"][name] = w
+            dumps.update({f"{name}_{a}": res[a] for a in arms})
         # the standalone filter: one device call over n_clouds clouds against the twin on each
         frames, _, _, _, _ = make_parking_sequence(n_clouds, seed=90, n_map=n_map, n_scan=n_scan, max_range=20.0)
         clouds = [f[:n_scan] for f in frames]
@@ -179,6 +191,11 @@ def main():
                           "twin_ms": tm, "twin_points_per_s": n_pts / (tm * 1e-3), "twin_runs_ms": twin_ms,
                           "equal_to_twin": equal}
     print(json.dumps(line))
+    if args.dump_outputs:
+        dump_results(args.dump_outputs, "odometry_voxel", dumps)
+        for c, (p, i) in enumerate(got):
+            np.save(os.path.join(args.dump_outputs, f"voxel_filter_{c}_xyz.npy"), np.asarray(p, np.float64))
+            np.save(os.path.join(args.dump_outputs, f"voxel_filter_{c}_index.npy"), np.asarray(i, np.float64))
     if not ok_all:
         raise SystemExit("bench_odometry_voxel.py: parity FAILED")
 

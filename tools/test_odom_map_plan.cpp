@@ -71,7 +71,7 @@ static void run_push(const Recording& rec, const std::vector<int>& cnt, std::vec
     const int n_steps = (int)p.steps.size();
     for (int i = 1; i <= n_steps; ++i) {
         if (i == n_steps && !carry) break;
-        odom_plan::MapStep m;
+        odom_plan::MapInput m;
         odom_plan::map_step(p, i, carry, ms, &m);
         const int segs = (int)m.seq.size();
         CHECK((int)m.seg.size() == segs + 1 && (int)m.center.size() == segs && m.seg[0] == 0);
@@ -175,7 +175,65 @@ static void check_case(const std::vector<int>& lens, unsigned seed, int max_push
     CHECK(pushes >= 1);
 }
 
+// odom_plan::pack and odom_plan::map_failure on hand-made layouts: 3 segments (segs 0, 1: the lanes of a step; 2: a
+// carried sequence) over a push of 6 frames
+static void check_failures() {
+    const std::string range = "a voxel coordinate of the map filter outside [-2^20, 2^20)";
+    odom_plan::MapInput in;
+    in.add_piece(0, -1, 4); in.add_piece(40, 2, 3); in.end_segment(1);       // sequence 1: its old map and frame 2
+    in.add_piece(4, -1, 2); in.add_piece(50, 5, 2); in.end_segment(3);       // sequence 3: its old map and frame 5
+    in.add_piece(6, -1, 3); in.end_segment(4);                               // sequence 4: its old map alone
+    in.center = {2, 5, 7};                                                   // 7: a retained frame
+    std::vector<long long> ll;
+    std::vector<int> ints;
+    odom_plan::pack(in, ll, ints);
+    CHECK(ll == std::vector<long long>({0, 7, 11, 14, 0, 4, 7, 9, 11, 14, 0, 40, 4, 50, 6}));
+    CHECK(ints == std::vector<int>({-1, 2, -1, 5, -1, 2, 5, 7}));
+    const std::vector<int> none, ok3 = {0, 0, 0};
+    const std::vector<int64_t> kept = {0, 5, 9, 11};
+    int at = -1;
+    CHECK(odom_plan::map_failure(in, 2, 6, 14, ok3, kept, none, "", &at).empty() && at == 0);
+    CHECK(odom_plan::map_failure(in, 0, 6, 14, ok3, kept, none, "", &at).empty());
+    // the point limit: a step names its first lane, the final update its first sequence with a pushed frame
+    odom_plan::MapInput fin = in;
+    fin.center = {-1, 7, 5};
+    CHECK(odom_plan::map_failure(in, 2, 6, 13, none, {}, none, "", &at) ==
+              "the maps of its step and their new frames hold 14 points, more than 13 (int32 indexing)" && at == 0);
+    CHECK(odom_plan::map_failure(fin, 0, 6, 13, none, {}, none, "", &at) ==
+              "the maps after the push and their new frames hold 14 points, more than 13 (int32 indexing)" && at == 2);
+    // the map filter's range: a lane's map, or a carried sequence's last frame at its pose; before an empty map
+    CHECK(odom_plan::map_failure(in, 2, 6, 14, {0, 1, 1}, {0, 5, 5, 9}, none, "", &at) == "its local map has " + range &&
+          at == 1);
+    CHECK(odom_plan::map_failure(in, 2, 6, 14, {0, 0, 1}, {0, 0, 5, 9}, none, "", &at) ==
+              "its points at its pose have " + range && at == 2);
+    CHECK(odom_plan::map_failure(in, 0, 6, 14, {0, 1, 0}, kept, none, "", &at) == "its points at its pose have " + range &&
+          at == 1);
+    // a lane's map that the prune left empty (the voxel map only; a carried sequence's may be empty)
+    const std::string empty = "its local map is empty: every voxel lies max_distance or more from the last pose";
+    CHECK(odom_plan::map_failure(in, 2, 6, 14, ok3, {0, 5, 5, 5}, none, "x", &at) == empty && at == 1);
+    CHECK(odom_plan::map_failure(in, 2, 6, 14, ok3, {0, 5, 9, 9}, none, "", &at).empty());
+    CHECK(odom_plan::map_failure(in, 0, 6, 14, ok3, {0, 0, 0, 0}, none, "", &at).empty());
+    odom_plan::MapInput win = in;
+    win.center.clear();
+    CHECK(odom_plan::map_failure(win, 2, 6, 14, ok3, {0, 0, 5, 9}, none, "", &at).empty());
+    // the grids' plan: named at the first lane whose box is not dense, else the last lane
+    std::vector<int> hb = {0, 0, 0, 3, 3, 3, 0, 0, 0, 1 << 20, 1, 1, 5, 5, 5, 6, 6, 6};
+    std::vector<arena_plan::Box> boxes;
+    long long cells = 0;
+    const std::string why = arena_plan::plan(3, hb.data(), boxes, &cells, "local map of lane");
+    CHECK(!why.empty() && why.find("local map of lane 1") != std::string::npos);
+    CHECK(odom_plan::map_failure(win, 3, 6, 14, none, {}, hb, why, &at) == why && at == 1);
+    CHECK(odom_plan::map_failure(in, 3, 6, 14, ok3, {0, 5, 9, 11}, hb, why, &at) == why && at == 1);
+    hb[9] = 1;
+    CHECK(arena_plan::plan(3, hb.data(), boxes, &cells, "local map of lane").empty());
+    CHECK(odom_plan::map_failure(win, 3, 6, 14, none, {}, hb, "all grids too large", &at) == "all grids too large" &&
+          at == 2);
+    CHECK(odom_plan::map_failure(win, 2, 6, 14, none, {}, hb, "all grids too large", &at) == "all grids too large" &&
+          at == 1);
+}
+
 int main() {
+    check_failures();
     unsigned state = 4242u;
     for (int c = 0; c < 60; ++c) {
         const int S = 1 + (int)(rnd(state) % 4);

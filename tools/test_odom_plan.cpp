@@ -57,26 +57,27 @@ static void check_case(const std::vector<int>& lens, int map_frames, unsigned se
             ++j;
         }
         CHECK(st.active == j);
-        if (i == 0) { CHECK(st.piece_frame.empty() && st.map_seg.empty()); continue; }
+        if (i == 0) { CHECK(st.map.piece_frame.empty() && st.map.seg.size() == 1 && st.map.seq.empty()); continue; }
+        CHECK(st.map.seq == st.seq && st.map.center.empty());     // one segment per lane, nothing pruned
         // every lane's map: the window frames in ascending order, each frame's points contiguous
         size_t q = 0;
         long long m = 0;
-        CHECK(st.map_seg[0] == 0 && st.piece_dst[0] == 0);
+        CHECK(st.map.seg[0] == 0 && st.map.piece_dst[0] == 0);
         for (int l = 0; l < st.active; ++l) {
             const int s = st.seq[l], k = so[s] + i;
             const int w0 = k - map_frames > so[s] ? k - map_frames : so[s];
-            CHECK(st.map_seg[l] == m);
+            CHECK(st.map.seg[l] == m);
             for (int w = w0; w < k; ++w, ++q) {
-                CHECK(q < st.piece_frame.size());
-                CHECK(st.piece_frame[q] == p.dev[w]);
-                CHECK(st.piece_src[q] == p.dev_off[p.dev[w]]);
-                CHECK(st.piece_dst[q] == m);
+                CHECK(q < st.map.piece_frame.size());
+                CHECK(st.map.piece_frame[q] == p.dev[w]);
+                CHECK(st.map.piece_src[q] == p.dev_off[p.dev[w]]);
+                CHECK(st.map.piece_dst[q] == m);
                 m += fo[w + 1] - fo[w];
-                CHECK(st.piece_dst[q + 1] == m);
+                CHECK(st.map.piece_dst[q + 1] == m);
             }
-            CHECK(st.map_seg[l + 1] == m);
+            CHECK(st.map.seg[l + 1] == m);
         }
-        CHECK(q == st.piece_frame.size() && st.piece_dst.size() == q + 1);
+        CHECK(q == st.map.piece_frame.size() && st.map.piece_dst.size() == q + 1);
         max_map = m > max_map ? m : max_map;
     }
     CHECK(p.max_map == max_map);
@@ -104,8 +105,8 @@ int main() {
         odom_plan::Plan p;
         CHECK(plan(1, so, 8, fo.data(), 3, 1000, &p).empty());
         const odom_plan::Step& st = p.steps[7];
-        CHECK(st.piece_frame.size() == 3 && st.piece_frame[0] == 4 && st.piece_frame[2] == 6);
-        CHECK(st.map_seg[1] == 30 && p.max_map == 30);
+        CHECK(st.map.piece_frame.size() == 3 && st.map.piece_frame[0] == 4 && st.map.piece_frame[2] == 6);
+        CHECK(st.map.seg[1] == 30 && p.max_map == 30);
     }
     if (fails) { std::printf("%d failures\n", fails); return 1; }
     std::printf("ODOM_PLAN_OK\n");

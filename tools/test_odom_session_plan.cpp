@@ -109,21 +109,21 @@ static void check_case(const std::vector<int>& lens, int map_frames, unsigned se
                 CHECK((st.prev2[(size_t)j] < 0) == (fs.prev2[(size_t)fj] < 0));
                 if (st.prev2[(size_t)j] >= 0) CHECK(name_of(st.prev2[(size_t)j]) == full_name(fs.prev2[(size_t)fj]));
                 // window pieces: the same frames in the same order, and the points they read are those frames' points
-                CHECK(st.map_seg[(size_t)j + 1] - st.map_seg[(size_t)j] == fs.map_seg[(size_t)fj + 1] - fs.map_seg[(size_t)fj]);
+                CHECK(st.map.seg[(size_t)j + 1] - st.map.seg[(size_t)j] == fs.map.seg[(size_t)fj + 1] - fs.map.seg[(size_t)fj]);
                 size_t q0 = 0, f0 = 0;
-                while (q0 < st.piece_dst.size() && st.piece_dst[q0] < st.map_seg[(size_t)j]) ++q0;
-                while (f0 < fs.piece_dst.size() && fs.piece_dst[f0] < fs.map_seg[(size_t)fj]) ++f0;
-                for (; f0 + 1 < fs.piece_dst.size() && fs.piece_dst[f0] < fs.map_seg[(size_t)fj + 1]; ++f0, ++q0) {
-                    CHECK(q0 + 1 < st.piece_dst.size());
-                    if (q0 + 1 >= st.piece_dst.size()) break;
-                    const int r = st.piece_frame[q0];
+                while (q0 < st.map.piece_dst.size() && st.map.piece_dst[q0] < st.map.seg[(size_t)j]) ++q0;
+                while (f0 < fs.map.piece_dst.size() && fs.map.piece_dst[f0] < fs.map.seg[(size_t)fj]) ++f0;
+                for (; f0 + 1 < fs.map.piece_dst.size() && fs.map.piece_dst[f0] < fs.map.seg[(size_t)fj + 1]; ++f0, ++q0) {
+                    CHECK(q0 + 1 < st.map.piece_dst.size());
+                    if (q0 + 1 >= st.map.piece_dst.size()) break;
+                    const int r = st.map.piece_frame[q0];
                     const Name w = name_of(r);
-                    CHECK(w == full_name(fs.piece_frame[f0]));
-                    const long long len = st.piece_dst[q0 + 1] - st.piece_dst[q0];
-                    CHECK(len == fs.piece_dst[f0 + 1] - fs.piece_dst[f0]);
+                    CHECK(w == full_name(fs.map.piece_frame[f0]));
+                    const long long len = st.map.piece_dst[q0 + 1] - st.map.piece_dst[q0];
+                    CHECK(len == fs.map.piece_dst[f0 + 1] - fs.map.piece_dst[f0]);
                     const int g = global(w.first, w.second);
                     CHECK(len == fo[g + 1] - fo[g]);
-                    for (long long t = 0; t < len; ++t) CHECK(point_at(r, st.piece_src[q0] + t) == fo[g] + t);
+                    for (long long t = 0; t < len; ++t) CHECK(point_at(r, st.map.piece_src[q0] + t) == fo[g] + t);
                 }
             }
         }
