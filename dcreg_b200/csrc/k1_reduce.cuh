@@ -55,20 +55,10 @@ __device__ __forceinline__ double round_f32(double x) {
     return __longlong_as_double((long long)b);
 }
 
-// float -> double on the integer ALU, 5 instructions.  Exact for every normal float; +-0 and float denormals
-// (|x| < 1.2e-38) come out as +-2^-126-sized values instead of 0 (an absolute perturbation of 1e-38 m on a
-// coordinate - far below one FP64 ulp of any coordinate that is not itself ~1e-22 m), and Inf/NaN map to ~1e38-
-// sized finite values which - like NaN in the reference - fail the weight gate and drop the slot.
-// Why not F2F: the 64-bit conversions issue through the same FP64 pipe as DFMA/DMUL/DADD and DMMA, and that pipe is
-// the binding resource of K1 (tools/microbench*.cu measure the per-instruction costs on the device at hand).
-__device__ __forceinline__ double f32_to_f64(float f) {
-    const unsigned u = __float_as_uint(f);
-    const unsigned hi = (((u >> 3) & 0x0FFFFFFFu) + 0x38000000u) | (u & 0x80000000u);   // re-bias exponent by +896
-    return __hiloint2double((int)hi, (int)(u << 29));
-}
-
 // Per-slot front: residual, weight, gate, float32 round trips, Jacobian row in the world frame.
-// Output c[8] = [k (Rp x u'), k u', b, r], all zeros for an invalid slot (no plane or gated out).
+// Output c[8] = [k (Rp x u'), k u', b, r], all zeros for an invalid slot (no plane or gated out).  A non-finite point
+// gives a NaN or infinite r (the point arrives through an exact conversion), so it fails the gate as in the reference;
+// the row is built from Rp only when the slot is valid, since 0 x NaN would otherwise put NaN into every sum.
 // slope / gate: dcreg_icp_params::weight_slope / weight_gate (0.9 / 0.1 in the reference, icp_test_runner.cpp:1776, 1785)
 template <bool kUseWd>
 __device__ __forceinline__ void slot_front(const Pose& P, double px, double py, double pz, double nx, double ny,
@@ -95,9 +85,10 @@ __device__ __forceinline__ void slot_front(const Pose& P, double px, double py, 
         const double k = 2.0 - rcp_newton(sw);
         ux *= k; uy *= k; uz *= k;
     }
-    c[0] = wy * uz - wz * uy;                                     // Rp x (k u')
-    c[1] = wz * ux - wx * uz;
-    c[2] = wx * uy - wy * ux;
+    const double vx = valid ? wx : 0.0, vy = valid ? wy : 0.0, vz = valid ? wz : 0.0;
+    c[0] = vy * uz - vz * uy;                                     // Rp x (k u')
+    c[1] = vz * ux - vx * uz;
+    c[2] = vx * uy - vy * ux;
     c[3] = ux; c[4] = uy; c[5] = uz;
     neff += valid ? 1 : 0;
 }

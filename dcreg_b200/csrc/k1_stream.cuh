@@ -71,7 +71,9 @@ __device__ __forceinline__ double f32_raw(float f) {
     asm("mul.wide.u32 %0, %1, 0x20000000;" : "=l"(w) : "r"(u & 0x7fffffffu));
     return __hiloint2double((int)((unsigned)(w >> 32) | (u & 0x80000000u)), (int)(unsigned)w);
 }
-// float -> double in 4 instructions (same value as k1::f32_to_f64)
+// float -> double in 4 instructions.  Exact for every normal float; +-0 and float denormals (|x| < 1.2e-38) come out
+// as +-2^-127-sized values instead of 0 (an absolute perturbation of 1e-38 on a plane component), and Inf / NaN map to
+// finite values (plane_to_f64 drops such a slot).
 __device__ __forceinline__ double f32_f64(float f) {
     const unsigned u = __float_as_uint(f);
     unsigned long long w;
@@ -92,25 +94,42 @@ __device__ __forceinline__ double rnd_f32(double x) {
     return __hiloint2double((int)hi2, (int)(lo2 & 0xE0000000u));
 }
 
+// Non-finite inputs.  The integer conversions above map NaN and +-Inf to finite values, so a NaN would not reach r by
+// itself: with an exactly zero plane component (0 x huge = 0) r can stay small and the slot pass the gate, adding
+// ~1e77 to H.  In the reference such a slot has a NaN or infinite r, hence s = max(0, .) = 0 (icp_test_runner.cpp:1776),
+// and is dropped.  So `has` also requires every input of the slot to be finite: the integer max of the magnitude bits
+// (the same `& 0x7fffffff` the conversions use) below the all-ones exponent, on the integer pipe.
+__device__ __forceinline__ unsigned f32_mag(float f) { return __float_as_uint(f) & 0x7fffffffu; }
+
 template <typename PlaneT>
 __device__ __forceinline__ void plane_to_f64(const PlaneT& v, double& nx, double& ny, double& nz, double& d, bool& has);
 template <>
 __device__ __forceinline__ void plane_to_f64<float4>(const float4& v, double& nx, double& ny, double& nz, double& d,
                                                      bool& has) {
-    has = ((__float_as_uint(v.x) | __float_as_uint(v.y) | __float_as_uint(v.z)) & 0x7fffffffu) != 0u;
+    const unsigned mn = max(max(f32_mag(v.x), f32_mag(v.y)), f32_mag(v.z));
+    has = (mn - 1u) < 0x7f7fffffu && f32_mag(v.w) < 0x7f800000u;  // a non-zero, finite normal and a finite offset
     nx = f32_f64(v.x); ny = f32_f64(v.y); nz = f32_f64(v.z); d = f32_f64(v.w);
 }
 template <>
 __device__ __forceinline__ void plane_to_f64<double4>(const double4& v, double& nx, double& ny, double& nz, double& d,
                                                       bool& has) {
-    has = (v.x != 0.0) || (v.y != 0.0) || (v.z != 0.0);
-    nx = v.x; ny = v.y; nz = v.z; d = v.w;
+    const unsigned hx = (unsigned)__double2hiint(v.x) & 0x7fffffffu, hy = (unsigned)__double2hiint(v.y) & 0x7fffffffu;
+    const unsigned hz = (unsigned)__double2hiint(v.z) & 0x7fffffffu, hd = (unsigned)__double2hiint(v.w) & 0x7fffffffu;
+    const unsigned lo = (unsigned)__double2loint(v.x) | (unsigned)__double2loint(v.y) | (unsigned)__double2loint(v.z);
+    has = ((hx | hy | hz | lo) != 0u) && max(max(hx, hy), max(hz, hd)) < 0x7ff00000u;
+    // a dropped slot's s is +0, and 0 x NaN or 0 x Inf in s n would still reach the sums: keep only the low words of
+    // such a normal (a finite value below 2^-1022, like the leftovers of s and r in front)
+    nx = __hiloint2double(has ? __double2hiint(v.x) : 0, __double2loint(v.x));
+    ny = __hiloint2double(has ? __double2hiint(v.y) : 0, __double2loint(v.y));
+    nz = __hiloint2double(has ? __double2hiint(v.z) : 0, __double2loint(v.z));
+    d = v.w;
 }
 
 // Per-slot front of the streaming kernel: same arithmetic as k1::slot_front (k1_reduce.cuh), issue-slot trimmed:
 // raw-scaled point conversion, 4-instruction rounding, gate constants from the constant bank, and an invalid slot is
 // dropped by zeroing only the HIGH words of s and r (the leftovers are < 2^-1022, so every product that reaches an
-// accumulator underflows to exactly 0).  counts: bit 0.. = slots with a plane, bit 16.. = slots that pass the gate.
+// accumulator underflows to exactly 0).  counts: bit 0.. = slots with a plane (non-zero, finite), bit 16.. = slots
+// that pass the gate (and whose point is finite).
 template <bool kUseWd>
 __device__ __forceinline__ void front(const Args& a, float4 p, double nx, double ny, double nz, double d, bool has,
                                       double (&c)[8], unsigned& counts) {
@@ -123,7 +142,8 @@ __device__ __forceinline__ void front(const Args& a, float4 p, double nx, double
     const double qz = rnd_f32(wz + a.pose.t[2]);
     const double rr = fma(nx, qx, fma(ny, qy, fma(nz, qz, d)));   // icp_test_runner.cpp:1774
     const double ss = fma(fabs(rr), -a.slope, 1.0);               // :1776 (max(0, .) is implied by the gate)
-    const bool valid = has && (ss > a.gate);                      // :1785
+    const bool finite = max(max(f32_mag(p.x), f32_mag(p.y)), f32_mag(p.z)) < 0x7f800000u;   // (plane: in `has`)
+    const bool valid = has && finite && (ss > a.gate);            // :1785
     const double s = __hiloint2double(valid ? __double2hiint(ss) : 0, __double2loint(ss));
     const double r = __hiloint2double(valid ? __double2hiint(rr) : 0, __double2loint(rr));
     double ux = rnd_f32(s * nx);                                  // coeff.x/y/z (:1787-1789)

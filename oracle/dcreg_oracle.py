@@ -172,7 +172,11 @@ def fit_planes(nb):
 
     Least-squares solve of nb @ x = -1 (reference: 5x3 colPivHouseholderQr).  Here: batched
     pseudo-inverse (agrees with the QR solution to rounding for full-rank systems and yields a
-    zero component for an all-zero column, like Eigen's pivoted solve).
+    zero component for an all-zero column, like Eigen's pivoted solve).  On other rank-deficient
+    neighbourhoods (collinear or duplicated points) the minimum-norm solution differs from the
+    pivoted QR's basic one; those are pinned by dcreg_oracle_rows.qr53, the operation-for-operation
+    restatement of the kernel's QR.  This whole-loop oracle keeps pinv: it is a fast, independent
+    route to the shipped golden runs, whose neighbourhoods are full rank or have zero columns.
     Returns n (K,3), d (K,), ok (K,) [norm >= 1e-6 and thickness gate passed].
     """
     K = nb.shape[0]
