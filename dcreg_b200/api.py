@@ -82,6 +82,14 @@ class IterLog(C.Structure):
 PLANE_CALLBACK = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double),
                              C.POINTER(C.c_int64))
 
+class AdaptiveThreshold(C.Structure):
+    """dcreg_adaptive_threshold: the settings of odometry's adaptive search radius (KISS-ICP's defaults)"""
+    _fields_ = [("initial_threshold", C.c_double), ("min_motion", C.c_double), ("max_range", C.c_double)]
+
+    def __init__(self, initial_threshold=2.0, min_motion=0.1, max_range=100.0):
+        super().__init__(float(initial_threshold), float(min_motion), float(max_range))
+
+
 _lib = None
 
 # every symbol include/dcreg_b200.h declares (checked by tests/test_abi.py)
@@ -90,7 +98,7 @@ EXPORTS = [
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_icp_run_odometry_adaptive", "dcreg_odometry_open_adaptive", "dcreg_odometry_push_adaptive", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -170,6 +178,16 @@ def load_library():
     lib.dcreg_odometry_open_map.argtypes = [vp, C.POINTER(IcpParams), ci, C.c_double, ci, C.c_double, C.c_double, ci, ci,
                                             C.c_double, dp]
     lib.dcreg_odometry_local_map.argtypes = [vp, ci, C.POINTER(C.c_float), i64, C.POINTER(i64)]
+    lib.dcreg_icp_run_odometry_adaptive.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
+                                                    C.POINTER(i64), ci, C.c_double, ci, ci, C.c_double, C.c_double, ci, ci,
+                                                    C.c_double, C.POINTER(AdaptiveThreshold), dp, dp, C.POINTER(C.c_float),
+                                                    C.POINTER(i64), dp, dp, C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp,
+                                                    C.POINTER(C.c_float), dp, C.POINTER(IterLog), ci]
+    lib.dcreg_odometry_open_adaptive.argtypes = [vp, C.POINTER(IcpParams), ci, C.c_double, ci, ci, C.c_double, C.c_double,
+                                                 ci, ci, C.c_double, C.POINTER(AdaptiveThreshold), dp]
+    lib.dcreg_odometry_push_adaptive.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(C.c_float), C.POINTER(i64), ci, dp,
+                                                 C.POINTER(C.c_float), C.POINTER(i64), dp, dp, C.POINTER(ci), C.POINTER(ci),
+                                                 C.POINTER(ci), dp, C.POINTER(C.c_float), dp, C.POINTER(IterLog), ci]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -319,6 +337,71 @@ def constant_velocity_increment(T_prev, T):
         out[r, 3] = (A[0, r] * dt[0] + A[1, r] * dt[1]) + A[2, r] * dt[2]
     out[3, 3] = 1.0
     return out
+
+
+# The adaptive threshold of dcreg_icp_run_odometry_adaptive (dcreg_b200/csrc/adaptive_threshold.cuh): the same formulas
+# and operation order in Python floats (FP64, one rounding per operation).  A state is (sse, n), (0.0, 0) at the anchor.
+def adaptive_threshold_radius(state, initial_threshold, ceiling):
+    """The search radius a sequence in `state` registers its next frame with, min(3 sigma, ceiling), bit for bit"""
+    sse, n = state
+    sigma = float(initial_threshold) if n == 0 else math.sqrt(float(sse) / float(n))
+    r = 3.0 * sigma
+    return r if r < float(ceiling) else float(ceiling)
+
+
+def _rotation_angle(R):
+    """The rotation angle of R (9 row-major floats) by se3_log's route: Shepperd's quaternion, 2 atan2(|v|, w)"""
+    if not all(math.isfinite(x) for x in R):
+        return math.nan
+    tr = (R[0] + R[4]) + R[8]
+    v = [0.0, 0.0, 0.0]
+    if tr > 0.0:
+        r = math.sqrt(tr + 1.0)
+        w = 0.5 * r
+        r = 0.5 / r
+        v = [(R[7] - R[5]) * r, (R[2] - R[6]) * r, (R[3] - R[1]) * r]
+    else:
+        i = 0
+        if R[4] > R[0]:
+            i = 1
+        if R[8] > R[4 * i]:
+            i = 2
+        j = (i + 1) % 3
+        k = (j + 1) % 3
+        r = math.sqrt(((R[4 * i] - R[4 * j]) - R[4 * k]) + 1.0)
+        v[i] = 0.5 * r
+        r = 0.5 / r
+        w = (R[3 * k + j] - R[3 * j + k]) * r
+        v[j] = (R[3 * j + i] + R[3 * i + j]) * r
+        v[k] = (R[3 * k + i] + R[3 * i + k]) * r
+    w = abs(w)
+    n2 = (v[0] * v[0] + v[1] * v[1]) + v[2] * v[2]
+    n = math.sqrt(n2)
+    if n2 < SE3_LOG_SMALL * SE3_LOG_SMALL:
+        return (2.0 / w - (2.0 / 3.0) * n2 / ((w * w) * w)) * n
+    return 2.0 * math.atan2(n, w)
+
+
+def adaptive_threshold_error(T_prior, T_out, max_range):
+    """e of one frame: with D = constant_velocity_increment(T_prior, T_out) (how far registration corrected the
+    prediction), 2 max_range sin(theta / 2) + |t_D|.  NaN when a pose is not finite."""
+    with np.errstate(invalid="ignore", over="ignore"):
+        D = constant_velocity_increment(T_prior, T_out)
+    theta = _rotation_angle([float(x) for x in D[:3, :3].reshape(-1)])
+    t = [float(x) for x in D[:3, 3]]
+    t2 = (t[0] * t[0] + t[1] * t[1]) + t[2] * t[2]
+    if not (math.isfinite(theta) and math.isfinite(t2)):
+        return math.nan
+    return (2.0 * float(max_range)) * math.sin(0.5 * theta) + math.sqrt(t2)
+
+
+def adaptive_threshold_update(state, T_prior, T_out, min_motion, max_range):
+    """The state after a frame that started from T_prior and returned T_out: e is a sample when finite and > min_motion"""
+    sse, n = state
+    e = adaptive_threshold_error(T_prior, T_out, max_range)
+    if math.isfinite(e) and e > float(min_motion):
+        return (float(sse) + e * e, int(n) + 1)
+    return (float(sse), int(n))
 
 
 # The motion compensation of dcreg_icp_run_odometry_deskew (dcreg_b200/csrc/se3.cuh): the same formulas, operation order
@@ -563,6 +646,7 @@ class IcpResult:
         self.T_prior = None             # icp_run_sequences: the initial pose the frame started from
         self.n_points = None            # icp_run_odometry: the frame's points after the source filter
         self.deskewed = None            # icp_run_odometry (want_deskewed): those points after deskewing
+        self.search_radius = None       # icp_run_odometry (adaptive / want_radius): the radius the frame registered with
 
 
 def _trial_results(st, conv, n_it, T_out, logs, cap, cov=None):
@@ -840,7 +924,8 @@ class Context:
     def icp_run_odometry(self, params: IcpParams, sequences, T_init, deltas=None, motion: str = "increments",
                          map_frames: int = 10, cell_size=None, want_log: bool = False, want_cov: bool = False,
                          source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
-                         map_max_points: int = 1, timestamps=None, want_deskewed: bool = False):
+                         map_max_points: int = 1, timestamps=None, want_deskewed: bool = False, adaptive=None,
+                         want_radius: bool = False):
         """Scan-to-map odometry (`sequences`: a list of lists of (N, >=3) point arrays): frame k of a sequence registers
         against the local map of the frames [k - map_frames, k) before it, each placed at its own registered pose
         (map_points), starting from compose_prior(frame k-1's result, D).  motion "increments": D = deltas[k-1]
@@ -854,10 +939,16 @@ class Context:
         only when want_log, .cov when want_cov).  Needs no target; the context's source and target are left as they
         were.  timestamps (nested like `sequences`: one float32 array per frame, each point's fraction of its sweep in
         [0, 1]): deskew every registered frame with the increment its prior used (dcreg_icp_run_odometry_deskew);
-        want_deskewed: .deskewed holds each frame's kept points after deskewing ((n_points, 3) float32)."""
+        want_deskewed: .deskewed holds each frame's kept points after deskewing ((n_points, 3) float32).
+        adaptive (an AdaptiveThreshold): every frame's search radius follows its sequence's motion-model error under
+        the ceiling params.search_radius (dcreg_icp_run_odometry_adaptive; the twin is adaptive_threshold_*), and
+        .search_radius holds the radius each frame registered with (0 for anchors); want_radius: .search_radius also
+        without the threshold (that entry point with adaptive = NULL)."""
         models = {"increments": 0, "constant_velocity": 1}
         if motion not in models:
             raise ValueError(f"icp_run_odometry: motion must be one of {sorted(models)}, not {motion!r}")
+        with_radius = adaptive is not None or want_radius
+        radius = np.zeros(max(sum(len(s) for s in sequences), 1)) if with_radius else None
         source_max_points = _max_points(source_max_points, "source_max_points")
         map_max_points = _max_points(map_max_points, "map_max_points")
         seq_off, xyz, off = _pack_sequences(sequences)
@@ -869,11 +960,18 @@ class Context:
         ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
                               off if off is not None else np.zeros(1, np.int64), "icp_run_odometry")
         npts = np.diff(off) if off is not None else np.zeros(0, dtype=np.int64)
-        if filtered or deskew:
+        if filtered or deskew or with_radius:
             npts = np.zeros(max(n, 1), dtype=np.int64)
         desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
 
         def call(o):
+            if with_radius:
+                return self.lib.dcreg_icp_run_odometry_adaptive(
+                    self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
+                    3, cell, int(map_frames), models[motion], float(source_voxel), float(map_voxel), source_max_points,
+                    map_max_points, 0.0, None if adaptive is None else C.byref(adaptive), _optr(o.T_init),
+                    _optr(o.deltas), _fptr(ts), _iptr(npts), _optr(o.T_prior), _optr(o.T_out), o.n_it, o.conv, o.st,
+                    _optr(o.cov), _fptr(desk), _dptr(radius), o.logs, o.cap)
             if deskew:
                 return self.lib.dcreg_icp_run_odometry_deskew(
                     self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
@@ -900,6 +998,9 @@ class Context:
                                 want_prior=True)
         for r, c in zip(out, npts):
             r.n_points = int(c)
+        if with_radius:
+            for r, x in zip(out, radius):
+                r.search_radius = float(x)
         if want_deskewed:
             for r, d in zip(out, _split_deskewed(desk, npts[:n])):
                 r.deskewed = d
@@ -908,7 +1009,8 @@ class Context:
     def icp_run_odometry_map(self, params: IcpParams, sequences, T_init, deltas=None, motion: str = "increments", *,
                              map_voxel: float, max_distance: float, cell_size=None, want_log: bool = False,
                              want_cov: bool = False, source_voxel: float = 0.0, source_max_points: int = 1,
-                             map_max_points: int = 1, timestamps=None, want_deskewed: bool = False):
+                             map_max_points: int = 1, timestamps=None, want_deskewed: bool = False, adaptive=None,
+                             want_radius: bool = False):
         """icp_run_odometry with a persistent voxel map per sequence instead of the window (dcreg_icp_run_odometry_map,
         KISS-ICP's VoxelHashMap): frame k registers against M_k, where M_1 = voxel_map_update(empty, F_s(anchor),
         T_init[s]) and M_{k+1} = voxel_map_update(M_k, F_s(frame k), T_out[k], map_voxel, map_max_points,
@@ -928,7 +1030,17 @@ class Context:
         npts = np.zeros(max(n, 1), dtype=np.int64)
         desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
 
+        with_radius = adaptive is not None or want_radius
+        radius = np.zeros(max(n, 1)) if with_radius else None
+
         def call(o):
+            if with_radius:
+                return self.lib.dcreg_icp_run_odometry_adaptive(
+                    self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
+                    3, cell, 0, models[motion], float(source_voxel), float(map_voxel), source_max_points,
+                    map_max_points, float(max_distance), None if adaptive is None else C.byref(adaptive),
+                    _optr(o.T_init), _optr(o.deltas), _fptr(ts), _iptr(npts), _optr(o.T_prior), _optr(o.T_out), o.n_it,
+                    o.conv, o.st, _optr(o.cov), _fptr(desk), _dptr(radius), o.logs, o.cap)
             return self.lib.dcreg_icp_run_odometry_map(
                 self._h, C.byref(params), S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off), 3,
                 cell, models[motion], float(source_voxel), float(map_voxel), source_max_points, map_max_points,
@@ -938,6 +1050,9 @@ class Context:
                                 deltas, want_prior=True)
         for r, c in zip(out, npts):
             r.n_points = int(c)
+        if with_radius:
+            for r, x in zip(out, radius):
+                r.search_radius = float(x)
         if want_deskewed:
             for r, d in zip(out, _split_deskewed(desk, npts[:n])):
                 r.deskewed = d
@@ -945,7 +1060,7 @@ class Context:
 
     def odometry_map_session(self, params: IcpParams, n_seqs: int, T_init, motion: str = "increments", *,
                              map_voxel: float, max_distance: float, cell_size=None, source_voxel: float = 0.0,
-                             source_max_points: int = 1, map_max_points: int = 1):
+                             source_max_points: int = 1, map_max_points: int = 1, adaptive=None):
         """Open the context's odometry session with icp_run_odometry_map's voxel map (dcreg_odometry_open_map): the
         OdometrySession of odometry_session, whose pushes give byte for byte what one icp_run_odometry_map call over the
         recording gives, and whose local_map(s) returns sequence s's current map.  The arguments are odometry_session's
@@ -959,6 +1074,11 @@ class Context:
         if T0.shape[0] != n_seqs:
             raise ValueError(f"odometry_map_session: {n_seqs} sequences but {T0.shape[0]} initial poses")
         cell = float(params.search_radius if cell_size is None else cell_size)
+        if adaptive is not None:        # dcreg_odometry_open_adaptive: its pushes return .search_radius
+            self._check(self.lib.dcreg_odometry_open_adaptive(
+                self._h, C.byref(params), int(n_seqs), cell, 0, models[motion], float(source_voxel), float(map_voxel),
+                source_max_points, map_max_points, float(max_distance), C.byref(adaptive), _dptr(T0)))
+            return OdometrySession(self, params, int(n_seqs), adaptive=True)
         self._check(self.lib.dcreg_odometry_open_map(self._h, C.byref(params), int(n_seqs), cell, models[motion],
                                                      float(source_voxel), float(map_voxel), source_max_points,
                                                      map_max_points, float(max_distance), _dptr(T0)))
@@ -966,7 +1086,7 @@ class Context:
 
     def odometry_session(self, params: IcpParams, n_seqs: int, T_init, motion: str = "increments", map_frames: int = 10,
                          cell_size=None, source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
-                         map_max_points: int = 1):
+                         map_max_points: int = 1, adaptive=None):
         """Open the context's odometry session (dcreg_odometry_open): icp_run_odometry's settings for n_seqs sequences
         whose frames come in pushes (OdometrySession.push).  T_init (n_seqs, 4, 4): the pose of each sequence's first
         frame.  Pushing a recording in any chunks gives byte for byte what one icp_run_odometry call over it gives.
@@ -980,6 +1100,11 @@ class Context:
         if T0.shape[0] != n_seqs:
             raise ValueError(f"odometry_session: {n_seqs} sequences but {T0.shape[0]} initial poses")
         cell = float(params.search_radius if cell_size is None else cell_size)
+        if adaptive is not None:        # dcreg_odometry_open_adaptive: its pushes return .search_radius
+            self._check(self.lib.dcreg_odometry_open_adaptive(
+                self._h, C.byref(params), int(n_seqs), cell, int(map_frames), models[motion], float(source_voxel),
+                float(map_voxel), source_max_points, map_max_points, 0.0, C.byref(adaptive), _dptr(T0)))
+            return OdometrySession(self, params, int(n_seqs), adaptive=True)
         self._check(self.lib.dcreg_odometry_open(self._h, C.byref(params), int(n_seqs), cell, int(map_frames),
                                                  models[motion], float(source_voxel), float(map_voxel), source_max_points,
                                                  map_max_points, _dptr(T0)))
@@ -1080,8 +1205,9 @@ class OdometrySession:
     """The context's odometry session (Context.odometry_session): frames pushed as they arrive, each sequence's local-map
     window and motion-model state kept on the device from one push to the next."""
 
-    def __init__(self, ctx: Context, params: IcpParams, n_seqs: int):
+    def __init__(self, ctx: Context, params: IcpParams, n_seqs: int, adaptive: bool = False):
         self.ctx, self.params, self.n_seqs = ctx, params, n_seqs
+        self.adaptive = adaptive        # opened with an AdaptiveThreshold: every push returns .search_radius
         self.open = True
 
     def push(self, frames_per_seq, deltas=None, want_log: bool = False, want_cov: bool = False, timestamps=None,
@@ -1110,7 +1236,16 @@ class OdometrySession:
         cov = np.empty((m, 6, 6)) if want_cov else None
         cap = int(self.params.max_iterations) if want_log else 0
         logs = (IterLog * max(cap * n, 1))() if want_log else None
-        if timestamps is not None or want_deskewed:
+        radius = np.zeros(m) if self.adaptive else None
+        if self.adaptive:
+            ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
+                                  off if off is not None else np.zeros(1, np.int64), "odometry push")
+            desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
+            ctx._check(lib.dcreg_odometry_push_adaptive(
+                ctx._h, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n, _fptr(xyz), _iptr(off), 3, _optr(D), _fptr(ts),
+                _iptr(npts), _dptr(T_prior), _dptr(T_out), n_it, conv, st, _optr(cov), _fptr(desk), _dptr(radius), logs,
+                cap))
+        elif timestamps is not None or want_deskewed:
             ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
                                   off if off is not None else np.zeros(1, np.int64), "odometry push")
             desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
@@ -1125,6 +1260,9 @@ class OdometrySession:
         res = _trial_results(st[:n], conv[:n], n_it[:n], T_out, logs, cap, cov)
         for r, Tp, c in zip(res, T_prior, npts):
             r.T_prior, r.n_points = Tp, int(c)
+        if self.adaptive:
+            for r, x in zip(res, radius):
+                r.search_radius = float(x)
         if want_deskewed:
             for r, d in zip(res, _split_deskewed(desk, npts[:n])):
                 r.deskewed = d

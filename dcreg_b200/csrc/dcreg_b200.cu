@@ -28,6 +28,7 @@
 #include <vector>
 
 #include "../../include/dcreg_b200.h"
+#include "adaptive_threshold.cuh"
 #include "arena_plan.hpp"
 #include "corr.cuh"
 #include "k1_reduce.cuh"
@@ -241,6 +242,11 @@ struct Iter2Smem {
     corr::RowRange rowtab[kSearchListMax][9];   // cell rows of the tile's listed searches (cell = radius)
     int nS, nF;
     corr::Grid grid;                            // this trial's own target grid (Iter2Args::grids)
+    // odometry (kGrids and kSeq): the search radius of the lane's frame (Iter2Args::lane_radius, or the parameters'), its
+    // square rounded up to float, and for the solve step the parameters with that radius
+    double radius;
+    float r2_up;
+    dcreg_icp_params prm;
 };
 
 // Grid = (blocks per trial, trials).  A trial is one registration (one initial pose) of the context's source against
@@ -282,6 +288,10 @@ struct Iter2Args {
     // sequences of frames (dcreg_icp_run_sequences, with seg: the frames' slot ranges): grid y is the lane, the trial the
     // frame seq.cursor[lane].  Only the icp_iter2_kernel<., ., true> instantiation reads it
     SeqView seq;
+    // odometry with the adaptive threshold (dcreg_icp_run_odometry_adaptive): [lanes] the search radius of the frame each
+    // lane runs at this step, in device memory (a captured chunk freezes its arguments), or null: prm.search_radius.
+    // Only the icp_iter2_kernel<., true, true> instantiation reads it
+    const double* lane_radius;
 };
 
 __device__ __forceinline__ void cswap5(unsigned long long& ka, int& pa, unsigned long long& kb, int& pb) {
@@ -371,6 +381,13 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
         static_assert(sizeof(corr::Grid) % sizeof(int) == 0 && sizeof(corr::Grid) / sizeof(int) <= kBlock, "grid copy");
         if (tid < (int)(sizeof(corr::Grid) / sizeof(int)))
             reinterpret_cast<int*>(&sm.grid)[tid] = reinterpret_cast<const int*>(a.grids + (kSeq ? ys : trial))[tid];
+        if constexpr (kSeq) {
+            if (tid == kBlock - 1) {              // r2_up: plan_iteration's round-up of the squared radius
+                const double r = a.lane_radius ? a.lane_radius[ys] : A.prm.search_radius;
+                sm.radius = r;
+                sm.r2_up = a.lane_radius ? __double2float_ru(__dmul_rn(r, r)) : a.r2_up;
+            }
+        }
         __syncthreads();
     }
     const corr::Grid& g = kGrids ? sm.grid : A.grid;
@@ -394,7 +411,9 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     double c0 = 0.0, c1 = 0.0, e0 = 0.0, e1 = 0.0;
     int neff = 0, npt = 0;
     unsigned n_search = 0, n_fit = 0;
-    const double r2max = A.prm.search_radius * A.prm.search_radius;
+    double radius = A.prm.search_radius;
+    if constexpr (kGrids && kSeq) radius = sm.radius;
+    const double r2max = radius * radius;
     {
         // ---- tiles of a.tile (<= 256) slots with per-tile work lists, so that searches and fits run densely packed.  Lean mode (the
         // pose still moves a lot) uses the same phases: every slot searches (plain 5-NN), every accepted slot fits.
@@ -413,7 +432,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                 const float qx = (float)(P.R[0] * px + P.R[1] * py + P.R[2] * pz + P.t[0]);
                 const float qy = (float)(P.R[3] * px + P.R[4] * py + P.R[5] * pz + P.t[1]);
                 const float qz = (float)(P.R[6] * px + P.R[7] * py + P.R[8] * pz + P.t[2]);
-                float B = a.r2_up;
+                float B = (kGrids && kSeq) ? sm.r2_up : a.r2_up;
                 need = true;
                 if (use_seeds) {
                     const int4 s0 = rec_nn[kNnRec * i], s1 = rec_nn[kNnRec * i + 1], s2 = rec_nn[kNnRec * i + 2];   // one round trip
@@ -477,7 +496,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                     const int t = sm.listS[w];
                     const float4 q = sm.q[t];
                     corr::KnnM r;
-                    float lbq = a.r2_up * 0.9999f;    // nothing beyond the rings of cells is closer than the radius
+                    float lbq = ((kGrids && kSeq) ? sm.r2_up : a.r2_up) * 0.9999f;    // nothing beyond the rings of cells is closer than the radius
                     const bool got = corr::knn_warp_search(g, q.x, q.y, q.z, q.w, W, r, lbq,
                                                            (a.stamps && warp == 0) ? reinterpret_cast<long long*>(a.stamps + (size_t)blockIdx.x * kStampSlots + 9) : nullptr,
                                                            pre_rows ? sm.rowtab[w] : nullptr);
@@ -496,7 +515,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                 const float4 q = sm.q[tid];
                 if (coherent) {
                     corr::KnnM r;
-                    float lbq = a.r2_up * 0.9999f;
+                    float lbq = ((kGrids && kSeq) ? sm.r2_up : a.r2_up) * 0.9999f;
                     corr::knn_search_lb(g, q.x, q.y, q.z, q.w, r, lbq);
 #pragma unroll
                     for (int k = 0; k < corr::kSeeds; ++k) sm.res[tid][k] = r.pos[k];
@@ -655,7 +674,19 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     DCREG_STAMP(7);
     if (tid < kAcc) A.acc[(size_t)ys * kAcc + tid] = sm.tail.acc[tid];
     if (a.fold_k2 && warp == 0) {
-        solve_step_in_kernel(sm.tail.acc, st, &A.prm, a.log ? a.log + (size_t)trial * a.log_cap : nullptr, a.log_cap,
+        const dcreg_icp_params* prm = &A.prm;
+        if constexpr (kGrids && kSeq) {           // the step limit of coherent mode follows the frame's own radius
+            if (a.lane_radius) {
+                static_assert(sizeof(dcreg_icp_params) % sizeof(int) == 0, "parameter copy");
+                for (int e = lane; e < (int)(sizeof(dcreg_icp_params) / sizeof(int)); e += 32)
+                    reinterpret_cast<int*>(&sm.prm)[e] = reinterpret_cast<const int*>(&A.prm)[e];
+                __syncwarp();
+                if (lane == 0) sm.prm.search_radius = sm.radius;
+                __syncwarp();
+                prm = &sm.prm;
+            }
+        }
+        solve_step_in_kernel(sm.tail.acc, st, prm, a.log ? a.log + (size_t)trial * a.log_cap : nullptr, a.log_cap,
                              reinterpret_cast<k2::WarpSmem*>(sm.tbuf[0]), a.seg ? a.src_radius + trial : a.src_radius,
                              a.coherent_step, a.n_active,
                              a.stamps ? a.stamps + (size_t)gridDim.x * kStampSlots : nullptr);
@@ -671,6 +702,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
 // dynamic shared memory of the loop kernel: the per-trial grid copy (Iter2Smem::grid, the last member) only where the
 // kernel reads it
 constexpr size_t kIter2SmemNoGrid = offsetof(Iter2Smem, grid);
+constexpr size_t kIter2SmemGrid = offsetof(Iter2Smem, radius);      // ... and odometry's radius fields only there
 
 template <bool kUseWd, bool kGrids, bool kSeq, bool kPlanes = false>
 cudaError_t loop_kernel_attributes(size_t smem) {
@@ -706,11 +738,11 @@ struct K2Scratch {
 // One warp per trial (blockIdx.x): acc_all [B][kAcc], st_all [B], log_all [B][log_cap].  scratch (rehearsal) only for B = 1.
 // radius_per_trial: src_radius is [B] (a batch of different scans) instead of one value for every trial.
 // seq.cursor set (sequences of frames): blockIdx.x is a lane with acc_all [lanes][kAcc]; its trial is the frame it runs
-// now, and the step that stops a frame advances the lane (no rehearsal: scratch is null)
+// now, and the step that stops a frame advances the lane (no rehearsal: scratch is null).  lane_radius: Iter2Args's, or null
 __global__ void __launch_bounds__(32) k2_step_kernel(const double* acc_all, IcpState* st_all, dcreg_icp_params prm,
                                                      dcreg_iter_log* log_all, int log_cap, const float* src_radius,
                                                      double coherent_step, K2Scratch* scratch, unsigned int* n_active,
-                                                     int radius_per_trial, SeqView seq) {
+                                                     int radius_per_trial, SeqView seq, const double* lane_radius) {
     __shared__ k2::WarpSmem sm;
     pdl_release();
     const int lane = threadIdx.x;
@@ -724,7 +756,8 @@ __global__ void __launch_bounds__(32) k2_step_kernel(const double* acc_all, IcpS
     IcpState* st = st_all + trial;
     dcreg_iter_log* log = log_all ? log_all + (size_t)trial * log_cap : nullptr;
     if (src_radius && radius_per_trial) src_radius += trial;
-    const double max_step = coherent_step * prm.search_radius;
+    // (odometry's adaptive threshold: the lane's own search radius, Iter2Args::lane_radius)
+    const double max_step = coherent_step * (lane_radius ? lane_radius[blockIdx.x] : prm.search_radius);
     const bool warp_path = prm.detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm.handling == DCREG_HAND_PRECONDITIONED_CG;
 #pragma unroll 1
     for (int pass = scratch ? 0 : 1; pass < 2; ++pass) {
@@ -1189,6 +1222,29 @@ __global__ void odom_deskew_kernel(float4* __restrict__ src, float4* __restrict_
         atomicMax(reinterpret_cast<unsigned int*>(radius + b), rmax);
 }
 
+// ---- the adaptive threshold (dcreg_icp_run_odometry_adaptive; adaptive_threshold.cuh) -----------------------------
+// Per step, after its loop has ended (one thread per lane j < active): the lane's frame step_first + j, which has
+// stopped, is folded into its sequence's state, state[seq[j]], with the correction inv(T_prior) T_out, and the
+// sequence's next radius goes to lane_radius[next_lane[j]], the lane that runs the sequence at the next step (-1: none).
+// The lanes of a step keep their order into the next one, so next_lane[j] <= j is written by one thread and read by
+// none here.
+__global__ void odom_threshold_kernel(const IcpState* __restrict__ states, const double* __restrict__ T_prior,
+                                      int step_first, int active, const int* __restrict__ seq,
+                                      const int* __restrict__ next_lane, adaptive::Settings set, double ceiling,
+                                      adaptive::State* __restrict__ state, double* lane_radius) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= active) return;
+    const IcpState* st = states + step_first + j;
+    const double* P = T_prior + (size_t)(step_first + j) * 16;
+    const double Ra[9] = {P[0], P[1], P[2], P[4], P[5], P[6], P[8], P[9], P[10]}, ta[3] = {P[3], P[7], P[11]};
+    double D[16];
+    constant_velocity_increment(Ra, ta, st->R, st->t, D);
+    adaptive::State x = state[seq[j]];
+    adaptive::fold(&x, adaptive::model_error(D, set.max_range), set.min_motion);
+    state[seq[j]] = x;
+    if (next_lane[j] >= 0) lane_radius[next_lane[j]] = adaptive::radius(x, set.initial_threshold, ceiling);
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------
@@ -1274,6 +1330,10 @@ struct OdomSettings {
     // every sequence's map carried from frame to frame, pruned at max_distance (+inf: never)
     bool voxel_map = false;
     double max_distance = 0.0;
+    // the adaptive threshold (dcreg_icp_run_odometry_adaptive, dcreg_odometry_open_adaptive): every frame's search radius
+    // follows its sequence's motion-model error, under the ceiling params.search_radius
+    bool adaptive = false;
+    adaptive::Settings threshold{};
 };
 
 struct dcreg_ctx {
@@ -1349,6 +1409,9 @@ struct dcreg_ctx {
     // [points], and the step's twists [lanes][6]
     DevBuf<float> d_odom_ts_in, d_odom_ts;
     DevBuf<double> d_odom_xi;
+    // the adaptive threshold: every sequence's (sse, n) [n_seqs], and the radii of the coming step's lanes [lanes]
+    DevBuf<adaptive::State> d_thr_state;
+    DevBuf<double> d_lane_radius;
     // the odometry session (dcreg_odometry_open .. _close), if one is open: the settings of its pushes, and what every
     // sequence carries from one push to the next (odom_plan::History): the retained frames' kept points, packed and in
     // input order as d_scan_src holds them, in win[cur] (the other buffer receives the next push's window), their poses
@@ -1363,6 +1426,8 @@ struct dcreg_ctx {
         // the voxel map (set.voxel_map): win[cur] holds every sequence's map instead of a window, sequence s's being
         // points [map_off[s], map_off[s + 1]), its last frame in it (the push's final update gathers them in win[1 - cur])
         std::vector<long long> map_off;                                // [n_seqs + 1]
+        // (set.adaptive) every sequence's threshold state after its last committed frame; a push uploads it
+        std::vector<adaptive::State> thr_state;                        // [n_seqs]
     };
     std::unique_ptr<OdomSession> odom;
     // the voxel filter (voxel_filter): table [slots] keys / first indices, [points] slots, [points + 1] flags and their
@@ -1892,15 +1957,17 @@ static corr::Grid arena_grid(const dcreg_ctx::GridArena& A, const arena_plan::Bo
     return g;
 }
 
-// groups the m points of the n clouds with boxes[n] (`cells` in all); on return A.d_grids[b] is cloud b's grid
+// groups the m points of the n clouds with boxes[n] (`cells` in all); on return A.d_grids[b] is cloud b's grid.
+// cloud_rings: [n] every cloud's own ring count instead of `rings`, or null
 static int arena_fill(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_pts, const long long* d_seg, int n,
-                      long long m, const arena_plan::Box* boxes, long long cells, double inv_cell, int rings) {
+                      long long m, const arena_plan::Box* boxes, long long cells, double inv_cell, int rings,
+                      const int* cloud_rings = nullptr) {
     int rc;
     CK(A.reserve(m, cells));
     std::vector<corr::Grid> hg((size_t)n);
     std::vector<int> off((size_t)n + 1);
     for (int b = 0; b < n; ++b) {
-        hg[(size_t)b] = arena_grid(A, boxes[b], m, inv_cell, rings);
+        hg[(size_t)b] = arena_grid(A, boxes[b], m, inv_cell, cloud_rings ? cloud_rings[b] : rings);
         off[(size_t)b] = (int)boxes[b].cell_off;
     }
     off[(size_t)n] = (int)cells;
@@ -2333,8 +2400,8 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
     if (!ctx->loop_attr_done) {          // per device (= per context), not per process
         CK((loop_kernel_attributes<true, false, false>)(kIter2SmemNoGrid));
         CK((loop_kernel_attributes<false, false, false>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<true, true, false>)(sizeof(Iter2Smem)));
-        CK((loop_kernel_attributes<false, true, false>)(sizeof(Iter2Smem)));
+        CK((loop_kernel_attributes<true, true, false>)(kIter2SmemGrid));
+        CK((loop_kernel_attributes<false, true, false>)(kIter2SmemGrid));
         CK((loop_kernel_attributes<true, false, true>)(kIter2SmemNoGrid));
         CK((loop_kernel_attributes<false, false, true>)(kIter2SmemNoGrid));
         CK((loop_kernel_attributes<true, true, true>)(sizeof(Iter2Smem)));
@@ -2356,8 +2423,8 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
         if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
         else CK(launch_pdl(icp_iter2_kernel<false, true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
     } else if (L.grid_table) {
-        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, false>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false, true, false>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, false>, grid, dim3(kBlock), kIter2SmemGrid, ctx->stream, L.b));
+        else CK(launch_pdl(icp_iter2_kernel<false, true, false>, grid, dim3(kBlock), kIter2SmemGrid, ctx->stream, L.b));
     } else if (L.lanes) {
         if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
         else CK(launch_pdl(icp_iter2_kernel<false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
@@ -2372,13 +2439,14 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
 
 // the separate solve kernel (one warp per trial): baseline methods, the host-plane loop, NCCL fallback of a sharded run
 // coherent_step: the plan's (Iter2Args::coherent_step).  scan_radius: the lever arms of a batch's sources, or null (the
-// context's source).  seq: the lanes of a batch (trials = lanes), or null
+// context's source).  seq: the lanes of a batch (trials = lanes), or null; lane_radius: Iter2Args's
 static int launch_k2(dcreg_ctx* ctx, const dcreg_icp_params* prm, dcreg_iter_log* dlog, int log_cap, double coherent_step,
-                     int trials = 1, const float* scan_radius = nullptr, const SeqView* seq = nullptr) {
+                     int trials = 1, const float* scan_radius = nullptr, const SeqView* seq = nullptr,
+                     const double* lane_radius = nullptr) {
     CK(launch_pdl(k2_step_kernel, dim3((unsigned)trials), dim3(32), 0, ctx->stream, (const double*)ctx->d_acc.p, ctx->d_state.p, *prm,
                   dlog, log_cap, scan_radius ? scan_radius : (const float*)ctx->d_src_radius.p, coherent_step,
                   trials == 1 && !seq ? ctx->d_k2_scratch.p : (K2Scratch*)nullptr, seq ? nullptr : ctx->d_n_active.p,
-                  scan_radius ? 1 : 0, seq ? *seq : SeqView{}));
+                  scan_radius ? 1 : 0, seq ? *seq : SeqView{}, lane_radius));
     ctx->launches++;
     return DCREG_OK;
 }
@@ -2389,7 +2457,8 @@ static int launch_body(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_params* prm,
     if (rc) return rc;
     if (with_k2 && !L.fold_k2) {
         if ((rc = nccl_allreduce_acc(ctx))) return rc;          // no-op on one GPU / with peer mailboxes
-        if ((rc = launch_k2(ctx, prm, dlog, log_cap, L.b.coherent_step, L.trials, L.scan_radius, L.lanes ? &L.b.seq : nullptr)))
+        if ((rc = launch_k2(ctx, prm, dlog, log_cap, L.b.coherent_step, L.trials, L.scan_radius, L.lanes ? &L.b.seq : nullptr,
+                            L.b.lane_radius)))
             return rc;
     }
     return DCREG_OK;
@@ -3065,6 +3134,10 @@ static const char* odometry_settings_error(const OdomSettings& set, bool deltas)
     if (set.source_max_points < 1 || set.map_max_points < 1) return "source_max_points and map_max_points must be >= 1";
     if (set.voxel_map && !(set.map_voxel > 0.0)) return "the voxel map needs a map_voxel > 0";
     if (set.voxel_map && !(set.max_distance > 0.0)) return "max_distance must be > 0 (+inf: no pruning), not NaN";
+    const adaptive::Settings& a = set.threshold;
+    if (set.adaptive && !(a.initial_threshold > 0.0 && a.initial_threshold < INFINITY && a.min_motion >= 0.0 &&
+                          a.min_motion < INFINITY && a.max_range > 0.0 && a.max_range < INFINITY))
+        return "adaptive: initial_threshold and max_range must be finite and > 0, min_motion finite and >= 0";
     return nullptr;
 }
 
@@ -3083,6 +3156,7 @@ struct OdomCall {
     dcreg_ctx* ctx; const char* name; const OdomSettings& set; dcreg_ctx::OdomSession* sess;
     const int* seq_offsets; int n_frames; const float* xyz; const int64_t* frame_offsets; int stride;
     const double* deltas; const float* timestamps; const Results& R; int64_t* frame_points; float* deskewed_xyz;
+    double* search_radius;                          // (out, may be null) the radius every frame registered with; anchors 0
     const int n_seqs = set.n_seqs;
     const dcreg_icp_params* params = &set.params;
     odom_plan::History none;                        // a one-shot call's history, once check() has validated n_seqs
@@ -3092,8 +3166,8 @@ struct OdomCall {
     std::vector<int64_t> kept;
     odom_plan::Push U;
     const odom_plan::Plan& P = U.plan;
-    // where the tables are in d_odom_ll / d_odom_int: step i's map's (odom_plan::pack), then its int prev, prev2; the
-    // retain step's and the timestamp gather's
+    // where the tables are in d_odom_ll / d_odom_int: step i's map's (odom_plan::pack), then its int prev, prev2 and
+    // (adaptive) the threshold kernel's seq, next_lane; the retain step's and the timestamp gather's
     std::vector<size_t> at_ll, at_int;
     size_t keep_ll = 0, keep_int = 0, ts_ll = 0;
     Batch S{};
@@ -3106,6 +3180,7 @@ struct OdomCall {
     // (voxel map) where every sequence's map is: the session's maps before the first update, then each update's output
     odom_plan::MapState MS;
     const float4* d_old = nullptr;
+    std::vector<double> frame_radius;               // [n_frames] the caller's frames' radii, as their steps run
 
     int check(), upload(), start(), step(int i), finish();
     int build_map(const odom_plan::MapInput& in, const long long* ll, const int* ints, DevBuf<float4>& out, StepMap* sm);
@@ -3279,6 +3354,18 @@ int OdomCall::upload() {
         odom_plan::pack(st.map, hll, hint);
         hint.insert(hint.end(), st.prev.begin(), st.prev.end());
         hint.insert(hint.end(), st.prev2.begin(), st.prev2.end());
+        if (set.adaptive) {     // lane j's sequence, and the lane that runs it at the next step
+            hint.insert(hint.end(), st.seq.begin(), st.seq.end());
+            for (int s : st.seq) {
+                int next = -1;
+                if (i + 1 < n_steps) {
+                    const std::vector<int>& ns = P.steps[(size_t)i + 1].seq;
+                    const auto it = std::lower_bound(ns.begin(), ns.end(), s);
+                    if (it != ns.end() && *it == s) next = (int)(it - ns.begin());
+                }
+                hint.push_back(next);
+            }
+        }
     }
     // (sess) then the retain step's: long long keep_dst [K + 1], keep_src [K]; int keep_ref [K]
     keep_ll = hll.size(); keep_int = hint.size();
@@ -3385,6 +3472,20 @@ int OdomCall::start() {
         MS = odom_plan::map_start(n_seqs, n_frames, hist, sess ? sess->map_off.data() : nullptr);
         if (sess) d_old = sess->win[sess->cur];
     }
+    frame_radius.assign((size_t)n_frames, 0.0);
+    if (set.adaptive) {         // the sequences' committed states, and the radii step 1's lanes register with
+        const std::vector<adaptive::State> h =
+            sess ? sess->thr_state : std::vector<adaptive::State>((size_t)n_seqs, adaptive::State{0.0, 0});
+        std::vector<double> r;
+        if (P.steps.size() > 1)
+            for (int s : P.steps[1].seq)
+                r.push_back(adaptive::radius(h[(size_t)s], set.threshold.initial_threshold, params->search_radius));
+        CK(ctx->d_thr_state.ensure(n_seqs));
+        CK(ctx->d_lane_radius.ensure(n_seqs));
+        CK(cudaMemcpyAsync(ctx->d_thr_state, h.data(), h.size() * sizeof(adaptive::State), cudaMemcpyHostToDevice, ctx->stream));
+        if (!r.empty())
+            CK(cudaMemcpyAsync(ctx->d_lane_radius, r.data(), r.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    }
     return DCREG_OK;
 }
 
@@ -3404,8 +3505,12 @@ int OdomCall::step(int i) {
                                         ctx->d_vmap[0], &sm)))
         return rc;
     // 2. their dense grids, one arena segment per lane (the bounds copy is the step's sync besides the loop's peeks, and
-    // brings the filter's kept offsets back; the unfiltered map sizes bound the kept ones)
+    // brings the filter's kept offsets back; the unfiltered map sizes bound the kept ones).  (adaptive) the lanes' radii,
+    // which the last step's threshold kernel left, ride the same copy; each lane's grid gets its own ring count
     const double inv_cell = 1.0 / set.cell_size;
+    std::vector<double> lane_r((size_t)st.active, params->search_radius);
+    std::vector<int> lane_rings;
+    if (set.adaptive) sm.more.push_back(Readback{ctx->d_lane_radius.p, lane_r.size() * sizeof(double), lane_r.data()});
     std::vector<int> hb;
     std::vector<arena_plan::Box> boxes;
     long long cells = 0;
@@ -3427,8 +3532,12 @@ int OdomCall::step(int i) {
         d_old = sm.map;
     }
     const long long m = sm.kept.empty() ? in.seg[(size_t)st.active] : sm.kept[(size_t)st.active];
+    for (int j = 0; j < st.active; ++j) {
+        frame_radius[(size_t)P.input[(size_t)(st.first + j)]] = lane_r[(size_t)j];
+        if (set.adaptive) lane_rings.push_back(std::max(1, search_rings(lane_r[(size_t)j], set.cell_size)));
+    }
     if ((rc = arena_fill(ctx, ctx->odom_maps, sm.map, sm.d_seg, st.active, m, boxes.data(), cells, inv_cell,
-                         search_rings(params->search_radius, set.cell_size))))
+                         search_rings(params->search_radius, set.cell_size), set.adaptive ? lane_rings.data() : nullptr)))
         return rc;
     // 3. every lane's frame of this step: its prior and a fresh loop state
     const int* d_prev = ctx->d_odom_int + at_int[(size_t)i] + st.map.piece_frame.size() + st.map.center.size();
@@ -3455,9 +3564,20 @@ int OdomCall::step(int i) {
     if (!planned) {
         S.grids = ctx->odom_maps.d_grids;
         if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? R.log_cap : 0, true, &L, &S))) return rc;
+        L.b.lane_radius = set.adaptive ? ctx->d_lane_radius.p : nullptr;
         planned = true;
     }
-    return run_chunks(ctx, L, params, dlog, dlog ? R.log_cap : 0, params->max_iterations, 16, true);
+    if ((rc = run_chunks(ctx, L, params, dlog, dlog ? R.log_cap : 0, params->max_iterations, 16, true))) return rc;
+    // 5. (adaptive) the step's frames into their sequences' threshold states, and the next step's radii
+    if (set.adaptive) {
+        const int* d_seq = d_prev2 + st.active;
+        odom_threshold_kernel<<<(unsigned)((st.active + 127) / 128), 128, 0, ctx->stream>>>(
+            ctx->d_state, ctx->d_seq_prior, st.first, st.active, d_seq, d_seq + st.active, set.threshold,
+            params->search_radius, ctx->d_thr_state, ctx->d_lane_radius);
+        ctx->launches++;
+        CK(cudaGetLastError());
+    }
+    return DCREG_OK;
 }
 
 // After the steps: (sess) the next window, and (voxel map) the final update, every sequence's map with its last frame
@@ -3489,9 +3609,16 @@ int OdomCall::finish() {
         update_failed = map_failed(in, nullptr, why, b);
     }
     const std::string err = ctx->err;
+    std::vector<adaptive::State> thr;               // (sess, adaptive) the states after the push, read back with the results
+    if (sess && set.adaptive && failed < 0 && !update_failed) {
+        thr.resize((size_t)n_seqs);
+        CK(cudaMemcpyAsync(thr.data(), ctx->d_thr_state, thr.size() * sizeof(adaptive::State), cudaMemcpyDeviceToHost,
+                           ctx->stream));
+    }
     if ((rc = finish_call(ctx, params, n_frames, dlog, R, P.dev.data(),
                           failed >= 0 ? P.steps[(size_t)failed].first : n_frames)))
         return rc;
+    if (search_radius) memcpy(search_radius, frame_radius.data(), frame_radius.size() * sizeof(double));
     if (failed >= 0 || update_failed) { ctx->err = err; return DCREG_BAD_ARG; }
     if (deskewed_xyz) {         // the frames' kept (deskewed) points, put in the caller's frame order
         const long long n_points = P.dev_off[(size_t)n_frames];
@@ -3511,6 +3638,7 @@ int OdomCall::finish() {
     if (sess) {
         commit_push(*sess, U, n_frames, seq_offsets, R.T_out, deltas);
         if (set.voxel_map) sess->map_off.assign(sm.kept.begin(), sm.kept.end());
+        if (set.adaptive) sess->thr_state.swap(thr);
     }
     return DCREG_OK;
 }
@@ -3524,10 +3652,10 @@ int OdomCall::finish() {
 static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& set, dcreg_ctx::OdomSession* sess,
                         const int* seq_offsets, int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
                         const double* deltas, const float* timestamps, const Results& R, int64_t* frame_points,
-                        float* deskewed_xyz) {
+                        float* deskewed_xyz, double* search_radius = nullptr) {
     if (!ctx) return DCREG_BAD_ARG;
     OdomCall o{ctx, name, set, sess, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps, R,
-               frame_points, deskewed_xyz};
+               frame_points, deskewed_xyz, search_radius};
     int rc;
     if ((rc = o.check()) || (rc = o.upload()) || (rc = o.start())) return rc;
     for (int i = 1; i < (int)o.P.steps.size() && o.failed < 0; ++i)
@@ -3613,7 +3741,40 @@ int dcreg_icp_run_odometry_map(dcreg_ctx* ctx, const dcreg_icp_params* params, i
                         deskewed_xyz);
 }
 
-// Opens the context's one session with the settings `set` (dcreg_odometry_open, _open_map)
+// the settings of dcreg_icp_run_odometry_adaptive / dcreg_odometry_open_adaptive: the window (map_frames >= 1) or the
+// voxel map (map_frames = 0), with the adaptive threshold when `adaptive` is given
+static OdomSettings odom_adaptive_settings(const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
+                                           int motion, double source_voxel, double map_voxel, int source_max_points,
+                                           int map_max_points, double max_distance,
+                                           const dcreg_adaptive_threshold* adaptive, const double* T_init) {
+    OdomSettings set = map_frames == 0 ? odom_map_settings(params, n_seqs, cell_size, motion, source_voxel, map_voxel,
+                                                           source_max_points, map_max_points, max_distance, T_init)
+                                       : odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel,
+                                                       map_voxel, source_max_points, map_max_points, T_init);
+    if (adaptive) {
+        set.adaptive = true;
+        set.threshold = adaptive::Settings{adaptive->initial_threshold, adaptive->min_motion, adaptive->max_range};
+    }
+    return set;
+}
+
+int dcreg_icp_run_odometry_adaptive(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                                    int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                                    double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                                    int source_max_points, int map_max_points, double max_distance,
+                                    const dcreg_adaptive_threshold* adaptive, const double* T_init, const double* deltas,
+                                    const float* timestamps, int64_t* frame_points, double* T_prior, double* T_out,
+                                    int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
+                                    double* search_radius, dcreg_iter_log* log, int log_cap) {
+    return run_odometry(ctx, "icp_run_odometry_adaptive",
+                        odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
+                                               source_max_points, map_max_points, max_distance, adaptive, T_init),
+                        nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
+                        Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
+                        deskewed_xyz, search_radius);
+}
+
+// Opens the context's one session with the settings `set` (dcreg_odometry_open, _open_map, _open_adaptive)
 static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& set) {
     if (ctx->odom) {
         ctx->err = std::string(name) + ": a session is open already (dcreg_odometry_close it first)";
@@ -3630,6 +3791,7 @@ static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     if (rc) return rc;
     ss->hist = odom_plan::History(n_seqs);
     ss->map_off.assign((size_t)n_seqs + 1, 0);
+    ss->thr_state.assign((size_t)n_seqs, adaptive::State{0.0, 0});
     ss->last_delta.assign((size_t)n_seqs * 16, 0.0);
     for (int s = 0; s < n_seqs; ++s)
         for (int c4 = 0; c4 < 4; ++c4) ss->last_delta[(size_t)s * 16 + 5 * c4] = 1.0;
@@ -3653,6 +3815,16 @@ int dcreg_odometry_open_map(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
     return open_session(ctx, "odometry_open_map",
                         odom_map_settings(params, n_seqs, cell_size, motion, source_voxel, map_voxel, source_max_points,
                                           map_max_points, max_distance, T_init));
+}
+
+int dcreg_odometry_open_adaptive(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size,
+                                 int map_frames, int motion, double source_voxel, double map_voxel, int source_max_points,
+                                 int map_max_points, double max_distance, const dcreg_adaptive_threshold* adaptive,
+                                 const double* T_init) {
+    if (!ctx) return DCREG_BAD_ARG;
+    return open_session(ctx, "odometry_open_adaptive",
+                        odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
+                                               source_max_points, map_max_points, max_distance, adaptive, T_init));
 }
 
 int dcreg_odometry_local_map(dcreg_ctx* ctx, int seq, float* xyz, int64_t cap, int64_t* n) {
@@ -3707,6 +3879,19 @@ int dcreg_odometry_push_deskew(dcreg_ctx* ctx, const int* seq_offsets, int n_fra
     return run_odometry(ctx, "odometry_push_deskew", ss.set, &ss, seq_offsets, n_frames, xyz, frame_offsets, stride,
                         deltas, timestamps, Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior},
                         frame_points, deskewed_xyz);
+}
+
+int dcreg_odometry_push_adaptive(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
+                                 const int64_t* frame_offsets, int stride, const double* deltas, const float* timestamps,
+                                 int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                                 int* status, double* cov, float* deskewed_xyz, double* search_radius, dcreg_iter_log* log,
+                                 int log_cap) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!ctx->odom) { ctx->err = "odometry_push_adaptive: no session is open (dcreg_odometry_open)"; return DCREG_BAD_ARG; }
+    dcreg_ctx::OdomSession& ss = *ctx->odom;
+    return run_odometry(ctx, "odometry_push_adaptive", ss.set, &ss, seq_offsets, n_frames, xyz, frame_offsets, stride,
+                        deltas, timestamps, Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior},
+                        frame_points, deskewed_xyz, search_radius);
 }
 
 // The session's buffers go with it; nothing queued may still read them

@@ -495,6 +495,63 @@ int dcreg_odometry_open_map(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
  * also without a session, for a window session, a null n or a seq outside [0, n_seqs). */
 int dcreg_odometry_local_map(dcreg_ctx* ctx, int seq, float* xyz, int64_t cap, int64_t* n);
 int dcreg_odometry_close(dcreg_ctx* ctx);
+/* THE ADAPTIVE THRESHOLD (KISS-ICP's AdaptiveThreshold): every frame's search radius follows how far registration has had
+ * to correct its sequence's motion model so far, so a model that is sometimes wrong (constant velocity through a turn)
+ * widens the basin only while it is wrong.  The radius of frame k+1 depends on T_prior[k] and T_out[k], which exist only
+ * on the device until the call returns: it cannot be done from outside without one call per frame.
+ * initial_threshold: sigma before a sequence has a sample; min_motion: errors at or below it are not samples;
+ * max_range: the lever arm that turns the rotation error into metres.  KISS-ICP's defaults are 2.0, 0.1 and 100.0. */
+typedef struct dcreg_adaptive_threshold {
+    double initial_threshold, min_motion, max_range;
+} dcreg_adaptive_threshold;
+/* Scan-to-map odometry with every setting of dcreg_icp_run_odometry_deskew and dcreg_icp_run_odometry_map, plus the
+ * adaptive threshold.  map_frames >= 1: the window of dcreg_icp_run_odometry_deskew (max_distance is not read);
+ * map_frames = 0: the voxel map of dcreg_icp_run_odometry_map, pruned at max_distance.  adaptive == NULL is that call
+ * itself: same launches, same bytes, search_radius filled with params->search_radius.
+ * - State, per sequence: (sse, n), FP64 and integer, (0, 0) at the sequence's anchor.  sigma = initial_threshold when
+ *   n = 0, else sqrt(sse / n).  Frame k registers with radius_k = min(3 sigma, params->search_radius): the parameter
+ *   becomes the ceiling, and search_radius / cell_size in (0, 4] is still what is checked.  sqrt, the division, 3 sigma
+ *   and the min are single IEEE operations: radius_k is a bit-exact function of (sse, n).
+ * - Update, after frame k has stopped (converged, not converged or aborted; anchors never): D =
+ *   constant_velocity_increment(T_prior[k], T_out[k]) = inv(T_prior[k]) T_out[k] with that function's rounding rule;
+ *   theta = the rotation angle of R_D through its quaternion, 2 atan2(|v|, w) (the route of the deskew's Log);
+ *   e = 2 max_range sin(theta / 2) + |t_D| in FP64.  If e is finite and e > min_motion: sse += e e, n += 1; otherwise
+ *   the state stays (a frame that returns its prior contributes nothing).  dcreg_b200.api.adaptive_threshold_error /
+ *   _update / _radius are the NumPy twin: the radius bit for bit from (sse, n); e to a few FP64 ulp (the device's sin
+ *   and atan2 and libm's differ in the last bit), so compare a frame with the radius the call returned.
+ * - Everything that follows the radius follows the frame's own: the 5-NN-within-radius rule, the rings of grid cells a
+ *   search visits (ceil(radius_k / cell_size), at least 1; lanes of one step may differ), the step limit of coherent
+ *   mode, the fitness count.  Frame k returns what dcreg_set_target(map_k, cell_size) + dcreg_set_source(frame k) +
+ *   dcreg_icp_run(T_prior[k]) returns with params.search_radius = radius_k, up to how the FP64 sums are grouped.
+ * - search_radius (out, may be NULL): n_frames doubles in the caller's frame order, radius_k; anchors get 0.
+ * - Cost: one launch per step whatever the number of sequences (one thread per lane, after the step's loop, outside
+ *   the loop's CUDA graphs); the next step's radii come back in the copy of the grids' bounds, so a step keeps its one
+ *   host sync, and the chunk graphs are still captured once per call.
+ * Errors (DCREG_BAD_ARG before anything is launched): initial_threshold or max_range not finite or <= 0, min_motion not
+ * finite or < 0; everything else as in the call the map selects. */
+int dcreg_icp_run_odometry_adaptive(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                                    int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                                    double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                                    int source_max_points, int map_max_points, double max_distance,
+                                    const dcreg_adaptive_threshold* adaptive, const double* T_init, const double* deltas,
+                                    const float* timestamps, int64_t* frame_points, double* T_prior, double* T_out,
+                                    int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
+                                    double* search_radius, dcreg_iter_log* log, int log_cap);
+/* dcreg_odometry_open (map_frames >= 1) or dcreg_odometry_open_map (map_frames = 0) with the adaptive threshold
+ * (adaptive == NULL: that call itself).  Every sequence's (sse, n) is session state: a push starts from the committed
+ * state, a push that fails commits nothing, and any chunking of a recording gives byte for byte what one
+ * dcreg_icp_run_odometry_adaptive call over it gives, search_radius included.  dcreg_odometry_push and _push_deskew push
+ * onto it unchanged; dcreg_odometry_push_adaptive is dcreg_odometry_push_deskew that also returns search_radius (on a
+ * session without the threshold: params->search_radius). */
+int dcreg_odometry_open_adaptive(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size,
+                                 int map_frames, int motion, double source_voxel, double map_voxel, int source_max_points,
+                                 int map_max_points, double max_distance, const dcreg_adaptive_threshold* adaptive,
+                                 const double* T_init);
+int dcreg_odometry_push_adaptive(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
+                                 const int64_t* frame_offsets, int stride, const double* deltas, const float* timestamps,
+                                 int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                                 int* status, double* cov, float* deskewed_xyz, double* search_radius, dcreg_iter_log* log,
+                                 int log_cap);
 /* Voxel downsampling of many clouds in one call (KISS-ICP's VoxelDownsample rule: the first point of every voxel).
  * xyz / offsets / stride: HOST memory as in dcreg_icp_run_scans (n_clouds + 1 offsets, ascending strictly from 0, at
  * most 2^29 - 1 points).  With inv = 1.0 / voxel in FP64, point i's voxel is (floor((double)x inv), floor((double)y inv),
