@@ -95,7 +95,7 @@ _lib = None
 # every symbol include/dcreg_b200.h declares (checked by tests/test_abi.py)
 EXPORTS = [
     "dcreg_abi_version", "dcreg_create", "dcreg_destroy", "dcreg_last_error", "dcreg_default_params",
-    "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_find_planes",
+    "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_set_target_sparse", "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
     "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_icp_run_odometry_adaptive", "dcreg_odometry_open_adaptive", "dcreg_odometry_push_adaptive", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
@@ -123,6 +123,7 @@ def load_library():
     lib.dcreg_stream.argtypes = [vp]; lib.dcreg_stream.restype = vp
     lib.dcreg_set_source.argtypes = [vp, C.POINTER(C.c_float), i64, ci]
     lib.dcreg_set_target.argtypes = [vp, C.POINTER(C.c_float), i64, ci, C.c_double]
+    lib.dcreg_set_target_sparse.argtypes = [vp, C.POINTER(C.c_float), i64, ci, C.c_double]
     lib.dcreg_find_planes.argtypes = [vp, dp, C.c_double, dp, C.POINTER(i64)]
     lib.dcreg_reduce_normal_equations.argtypes = [vp, vp, vp, i64, dp, ci, dp, dp]
     lib.dcreg_reduce_normal_equations_f64plane.argtypes = [vp, vp, vp, i64, dp, ci, dp, dp]
@@ -721,6 +722,13 @@ class Context:
         a = _as_points(xyz)
         self._check(self.lib.dcreg_set_target(self._h, a.ctypes.data_as(C.POINTER(C.c_float)), a.shape[0], a.shape[1],
                                               float(cell_size)))
+
+    def set_target_sparse(self, xyz, cell_size: float):
+        """set_target for maps too large for a dense grid: past 2^27 cells of the bounding box, a sparse row index on
+        which the batched calls and find_planes run as on a dense grid (include/dcreg_b200.h); below, set_target."""
+        a = _as_points(xyz)
+        self._check(self.lib.dcreg_set_target_sparse(self._h, a.ctypes.data_as(C.POINTER(C.c_float)), a.shape[0],
+                                                     a.shape[1], float(cell_size)))
 
     # -- seams --
     def find_planes(self, T, search_radius: float, want_planes: bool = True):

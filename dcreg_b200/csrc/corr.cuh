@@ -16,10 +16,14 @@
 //                the 3 x-adjacent cells of a row are ONE contiguous point range, so a query scans 9 ranges.
 //   hash mode  : open-addressing table keyed by the packed cell coordinates (fallback when the bounding box
 //                has more than arena_plan::kMaxDenseCells cells); a query probes 27 cells.
+//   sparse mode: the dense order of the points, and cell_start only where a search can read it: a table of row starts
+//                (sparse_index.hpp) replaces the box's table, so the searches run the dense traversal with one table
+//                lookup per range end (dcreg_set_target_sparse).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "small_la.cuh"
+#include "sparse_index.hpp"
 
 namespace corr {
 
@@ -29,19 +33,21 @@ struct Grid {
     float4* pts;                // n target points grouped by cell
     int* pos_of;                // [n] position in pts of the point with original index i (inverse of pts[j].w)
     int n;
-    int dense;                  // 1: dense mode, 0: hash mode
+    int dense;                  // 1: dense mode, 0: hash mode, kSparseGrid: sparse mode
     int rings;                  // ceil(search radius / cell edge): cells per direction a query must look at
     double inv_cell;            // 1 / cell edge
     // dense mode
     int ox, oy, oz;             // cell coordinates of the bounding box's minimum corner
     int nx, ny, nz;
     int* cell_start;            // [nx*ny*nz + 1]
-    // hash mode
+    // hash mode (sparse mode: keys = sparse_index::key of (x, y, z) box-local, hstart = cs, no hcount)
     unsigned long long* keys;   // capacity entries, kEmptyKey = free
     int* hstart;                // capacity
     int* hcount;                // capacity
     unsigned int mask;          // capacity - 1 (capacity is a power of two)
 };
+
+constexpr int kSparseGrid = 2;  // Grid::dense of the sparse row index
 
 __host__ __device__ __forceinline__ int cell_coord(float v, double inv_cell) {
     return (int)floor((double)v * inv_cell);
@@ -248,6 +254,79 @@ __global__ void source_cell_kernel(const float4* __restrict__ src, int n, Grid g
     atomicAdd(&counts[c], 1);
 }
 
+// ---- build of the sparse row index (sparse_index.hpp; g: the grid being built, box fields set) -----------------------
+// sort key of every point (its box-local cell) and its index as the value
+__global__ void sparse_key_kernel(const float4* __restrict__ pts, int n, Grid g, unsigned long long* __restrict__ keys,
+                                  int* __restrict__ vals) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 p = pts[i];
+    keys[i] = sparse_index::key(cell_coord(p.x, g.inv_cell) - g.ox, cell_coord(p.y, g.inv_cell) - g.oy,
+                                cell_coord(p.z, g.inv_cell) - g.oz);
+    vals[i] = i;
+}
+
+// the points in sort order (w = original index) and the inverse permutation
+__global__ void sparse_gather_kernel(const float4* __restrict__ pts, const int* __restrict__ order, int n,
+                                     float4* __restrict__ out, int* __restrict__ pos_of) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const int i = order[j];
+    float4 p = pts[i];
+    p.w = __int_as_float(i);
+    out[j] = p;
+    pos_of[i] = j;
+}
+
+// table entries the occupied cell starting at sorted position j adds (sparse_index::new_entries), summed into *count
+__global__ void sparse_count_kernel(const unsigned long long* __restrict__ sorted, int n, int nx,
+                                    unsigned long long* __restrict__ count) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long c = 0;
+    if (j < n && (j == 0 || sorted[j - 1] != sorted[j])) {
+        int lo, hi;
+        sparse_index::new_entries(sorted[j], j > 0 ? sorted[j - 1] : sparse_index::kEmpty, nx, &lo, &hi);
+        if (hi >= lo) c = (unsigned long long)(hi - lo + 1);
+    }
+    c = __reduce_add_sync(0xffffffffu, (unsigned)c);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, c);
+}
+
+// ... and their cs, each (row, x) inserted by the one cell that adds it
+__global__ void sparse_insert_kernel(const unsigned long long* __restrict__ sorted, int n, int nx, Grid g) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n || (j > 0 && sorted[j - 1] == sorted[j])) return;
+    int lo, hi;
+    sparse_index::new_entries(sorted[j], j > 0 ? sorted[j - 1] : sparse_index::kEmpty, nx, &lo, &hi);
+    const unsigned long long row = sparse_index::row_of(sorted[j]) << sparse_index::kBits;
+    for (int x = lo; x <= hi; ++x) {
+        const unsigned long long k = row | (unsigned long long)x;
+        unsigned int s = sparse_index::slot(k, g.mask);
+        while (atomicCAS(&g.keys[s], sparse_index::kEmpty, k) != sparse_index::kEmpty) s = (s + 1) & g.mask;
+        g.hstart[s] = (int)sparse_index::cs(sorted, n, k);
+    }
+}
+
+// cs of box-local cell (x, yy, zz) of a sparse grid, or -1 when the table has no entry for it
+__device__ __forceinline__ int sparse_cs(const Grid& g, int zz, int yy, int x) {
+    const unsigned long long k = sparse_index::key(x, yy, zz);
+    unsigned int s = sparse_index::slot(k, g.mask);
+    while (true) {
+        const unsigned long long kk = __ldg(&g.keys[s]);
+        if (kk == k) return __ldg(&g.hstart[s]);
+        if (kk == sparse_index::kEmpty) return -1;
+        s = (s + 1) & g.mask;
+    }
+}
+
+// point range of the cells [x0, x1) of row (yy, zz) of a sparse grid (x1 - x0 <= sparse_index::kReach): a range that
+// holds a point has both ends in the table
+__device__ __forceinline__ void sparse_span(const Grid& g, int zz, int yy, int x0, int x1, int& s, int& e) {
+    s = sparse_cs(g, zz, yy, x0);
+    e = sparse_cs(g, zz, yy, x1);
+    if (s < 0 || e < 0) { s = 0; e = 0; }
+}
+
 // ---- query -----------------------------------------------------------------------------------
 // The five best so far, ascending.  key = (bits of the squared distance) << 32 | original index: squared distances are
 // non-negative floats, whose bit patterns order like unsigned integers, so ONE 64-bit unsigned compare is the (distance,
@@ -312,9 +391,11 @@ __device__ __forceinline__ void knn_scan_range(const float4* __restrict__ pts, i
     }
 }
 
+// kSparse: g is a sparse row index (Grid::dense == kSparseGrid): the dense traversal, each range read from its table
+template <bool kSparse = false>
 __device__ __forceinline__ void knn_search(const Grid& g, float qx, float qy, float qz, Knn5& k) {
     const int cx = cell_coord(qx, g.inv_cell), cy = cell_coord(qy, g.inv_cell), cz = cell_coord(qz, g.inv_cell);
-    if (g.dense) {
+    if (kSparse || g.dense) {
         // K = ceil(radius / cell) rings of cells cover the search radius (K = 1 when cell = radius; a finer grid,
         // cell = radius / 2, K = 2, scans ~3x fewer candidates because most cells are pruned by their box distance).
         // Rows (dy, dz) are visited in rings of growing max(|dy|, |dz|); inside a row the own column first, then
@@ -353,7 +434,13 @@ __device__ __forceinline__ void knn_search(const Grid& g, float qx, float qy, fl
                 // most of their time in single-candidate trips, one memory round trip each).  The left / right cells
                 // are no longer pruned: their box-distance test only ever skips cells holding nothing below the
                 // current 5th key, so scanning them too leaves the list unchanged, bit for bit.
-                knn_scan_range(g.pts, __ldg(rowp + xa), __ldg(rowp + xd), qx, qy, qz, k);
+                if constexpr (kSparse) {
+                    int s, e;
+                    sparse_span(g, zz, yy, xa, xd, s, e);
+                    knn_scan_range(g.pts, s, e, qx, qy, qz, k);
+                } else {
+                    knn_scan_range(g.pts, __ldg(rowp + xa), __ldg(rowp + xd), qx, qy, qz, k);
+                }
             }
             return;
         }
@@ -381,7 +468,13 @@ __device__ __forceinline__ void knn_search(const Grid& g, float qx, float qy, fl
                     // own column, then +-1, +-2, ... : stop a side once its gap bound exceeds the 5th-best distance
                     {
                         const int x0 = min(max(lx, 0), g.nx), x1 = min(max(lx + 1, 0), g.nx);
-                        knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
+                        if constexpr (kSparse) {
+                            int s, e;
+                            sparse_span(g, zz, yy, x0, x1, s, e);
+                            knn_scan_range(g.pts, s, e, qx, qy, qz, k);
+                        } else {
+                            knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
+                        }
                     }
 #pragma unroll 1
                     for (int dx = 1; dx <= K; ++dx) {
@@ -390,12 +483,24 @@ __device__ __forceinline__ void knn_search(const Grid& g, float qx, float qy, fl
                         const bool left = (row_lb + gl * gl * 0.99999f) <= knn_d2(k, 4);
                         if (left) {
                             const int x0 = min(max(lx - dx, 0), g.nx), x1 = min(max(lx - dx + 1, 0), g.nx);
-                            knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
+                            if constexpr (kSparse) {
+                                int s, e;
+                                sparse_span(g, zz, yy, x0, x1, s, e);
+                                knn_scan_range(g.pts, s, e, qx, qy, qz, k);
+                            } else {
+                                knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
+                            }
                         }
                         const bool right = (row_lb + gr * gr * 0.99999f) <= knn_d2(k, 4);
                         if (right) {
                             const int x0 = min(max(lx + dx, 0), g.nx), x1 = min(max(lx + dx + 1, 0), g.nx);
-                            knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
+                            if constexpr (kSparse) {
+                                int s, e;
+                                sparse_span(g, zz, yy, x0, x1, s, e);
+                                knn_scan_range(g.pts, s, e, qx, qy, qz, k);
+                            } else {
+                                knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
+                            }
                         }
                         if (!left && !right) break;
                     }
@@ -473,6 +578,7 @@ __device__ __forceinline__ void knn_scan_range_lb(const float4* __restrict__ pts
     }
 }
 
+template <bool kSparse = false>
 __device__ __forceinline__ void knn_search_lb(const Grid& g, float qx, float qy, float qz, float B, KnnM& k, float& lb) {
     constexpr int L = kSeeds - 1;
 #pragma unroll
@@ -506,7 +612,13 @@ __device__ __forceinline__ void knn_search_lb(const Grid& g, float qx, float qy,
                 const int* rowp = g.cell_start + (size_t)(zz * g.ny + yy) * g.nx;
                 {
                     const int x0 = min(max(lx, 0), g.nx), x1 = min(max(lx + 1, 0), g.nx);
-                    knn_scan_range_lb(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k, lb);
+                    if constexpr (kSparse) {
+                        int s, e;
+                        sparse_span(g, zz, yy, x0, x1, s, e);
+                        knn_scan_range_lb(g.pts, s, e, qx, qy, qz, k, lb);
+                    } else {
+                        knn_scan_range_lb(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k, lb);
+                    }
                 }
                 bool left = true, right = true;
 #pragma unroll 1
@@ -516,7 +628,13 @@ __device__ __forceinline__ void knn_search_lb(const Grid& g, float qx, float qy,
                         const float b = row_lb + gl * gl * 0.99999f;
                         if (b <= knn_d2(k, L)) {
                             const int x0 = min(max(lx - dx, 0), g.nx), x1 = min(max(lx - dx + 1, 0), g.nx);
-                            knn_scan_range_lb(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k, lb);
+                            if constexpr (kSparse) {
+                                int s, e;
+                                sparse_span(g, zz, yy, x0, x1, s, e);
+                                knn_scan_range_lb(g.pts, s, e, qx, qy, qz, k, lb);
+                            } else {
+                                knn_scan_range_lb(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k, lb);
+                            }
                         } else { lb = fminf(lb, b); left = false; }
                     }
                     if (right) {
@@ -524,7 +642,13 @@ __device__ __forceinline__ void knn_search_lb(const Grid& g, float qx, float qy,
                         const float b = row_lb + gr * gr * 0.99999f;
                         if (b <= knn_d2(k, L)) {
                             const int x0 = min(max(lx + dx, 0), g.nx), x1 = min(max(lx + dx + 1, 0), g.nx);
-                            knn_scan_range_lb(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k, lb);
+                            if constexpr (kSparse) {
+                                int s, e;
+                                sparse_span(g, zz, yy, x0, x1, s, e);
+                                knn_scan_range_lb(g.pts, s, e, qx, qy, qz, k, lb);
+                            } else {
+                                knn_scan_range_lb(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k, lb);
+                            }
                         } else { lb = fminf(lb, b); right = false; }
                     }
                     if (!left && !right) break;
@@ -558,6 +682,7 @@ struct WarpKnnSmem {
 // (icp_iter2_kernel): one memory round trip for the whole tile instead of one at the head of every search.
 struct RowRange { int s, e; float lb; };
 
+template <bool kSparse = false>
 __device__ __forceinline__ RowRange knn_row_range(const Grid& g, float qx, float qy, float qz, float B, int r) {
     const int K = g.rings, W = 2 * K + 1;
     const float cell = (float)(1.0 / g.inv_cell);
@@ -591,8 +716,12 @@ __device__ __forceinline__ RowRange knn_row_range(const Grid& g, float qx, float
             }
             xa = max(xa, 0); xb = min(xb, g.nx - 1);
             if (xa <= xb) {
-                const int* rowp = g.cell_start + (size_t)(zz * g.ny + yy) * g.nx;
-                out.s = __ldg(rowp + xa); out.e = __ldg(rowp + xb + 1);
+                if constexpr (kSparse) {
+                    sparse_span(g, zz, yy, xa, xb + 1, out.s, out.e);
+                } else {
+                    const int* rowp = g.cell_start + (size_t)(zz * g.ny + yy) * g.nx;
+                    out.s = __ldg(rowp + xa); out.e = __ldg(rowp + xb + 1);
+                }
             }
         } else {
             out.lb = row_lb;
@@ -603,6 +732,7 @@ __device__ __forceinline__ RowRange knn_row_range(const Grid& g, float qx, float
 
 // prof (profiling only, may be null): [0] += cycles of the row set-up, [1] += prefix + candidate scan, [2] += selection,
 // [3] += searches, [4] += candidates scanned
+template <bool kSparse = false>
 __device__ __forceinline__ bool knn_warp_search(const Grid& g, float qx, float qy, float qz, float B, WarpKnnSmem& S,
                                                 KnnM& out, float& lb, long long* prof = nullptr, const RowRange* pre = nullptr) {
     const unsigned full = 0xffffffffu;
@@ -614,7 +744,7 @@ __device__ __forceinline__ bool knn_warp_search(const Grid& g, float qx, float q
     if (lane < kSeeds) { S.okey[lane] = knn_key(B, 0x7fffffff); S.opos[lane] = -1; }
 #pragma unroll 1
     for (int r = lane; r < nrows; r += 32) {
-        const RowRange rr = pre ? pre[r] : knn_row_range(g, qx, qy, qz, B, r);
+        const RowRange rr = pre ? pre[r] : knn_row_range<kSparse>(g, qx, qy, qz, B, r);
         lbl = fminf(lbl, rr.lb);
         S.rs[r] = rr.s; S.re[r] = rr.e;
     }

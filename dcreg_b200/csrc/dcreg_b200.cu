@@ -353,8 +353,9 @@ __device__ __noinline__ void solver_block(const Iter2Args& a, IcpState* st, Iter
 // (Iter2Args::seq) whose trial is the frame it runs now; the reduction's working set is the lane's.  Both (odometry,
 // dcreg_icp_run_odometry): the grid is the lane's, grids[lane], a local map rebuilt before every step.  kPlanes (seam 1,
 // dcreg_find_planes): every slot's plane goes to it.planes_out; a flag of its own, since the store costs the other
-// instantiations spills
-template <bool kUseWd, bool kGrids, bool kSeq, bool kPlanes = false>
+// instantiations spills.  kSparse: it.grid is the context's sparse row index (dcreg_set_target_sparse), whose searches
+// read their ranges from its table (corr::sparse_span)
+template <bool kUseWd, bool kGrids, bool kSeq, bool kPlanes = false, bool kSparse = false>
 __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_constant__ Iter2Args a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     Iter2Smem& sm = *reinterpret_cast<Iter2Smem*>(smem_raw);
@@ -488,7 +489,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                     for (int e = tid; e < nS * 9; e += kBlock) {
                         const int sidx = e / 9, r = e - sidx * 9;
                         const float4 q = sm.q[sm.listS[sidx]];
-                        sm.rowtab[sidx][r] = corr::knn_row_range(g, q.x, q.y, q.z, q.w, r);
+                        sm.rowtab[sidx][r] = corr::knn_row_range<kSparse>(g, q.x, q.y, q.z, q.w, r);
                     }
                     __syncthreads();
                 }
@@ -497,7 +498,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                     const float4 q = sm.q[t];
                     corr::KnnM r;
                     float lbq = ((kGrids && kSeq) ? sm.r2_up : a.r2_up) * 0.9999f;    // nothing beyond the rings of cells is closer than the radius
-                    const bool got = corr::knn_warp_search(g, q.x, q.y, q.z, q.w, W, r, lbq,
+                    const bool got = corr::knn_warp_search<kSparse>(g, q.x, q.y, q.z, q.w, W, r, lbq,
                                                            (a.stamps && warp == 0) ? reinterpret_cast<long long*>(a.stamps + (size_t)blockIdx.x * kStampSlots + 9) : nullptr,
                                                            pre_rows ? sm.rowtab[w] : nullptr);
                     if (got) {
@@ -516,14 +517,14 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                 if (coherent) {
                     corr::KnnM r;
                     float lbq = ((kGrids && kSeq) ? sm.r2_up : a.r2_up) * 0.9999f;
-                    corr::knn_search_lb(g, q.x, q.y, q.z, q.w, r, lbq);
+                    corr::knn_search_lb<kSparse>(g, q.x, q.y, q.z, q.w, r, lbq);
 #pragma unroll
                     for (int k = 0; k < corr::kSeeds; ++k) sm.res[tid][k] = r.pos[k];
                     sm.res[tid][7] = __float_as_int(lbq); sm.res[tid][8] = __float_as_int(corr::knn_d2(r, 4));
                 } else {                              // lean: plain exact 5-NN, nothing kept for the next iteration
                     corr::Knn5 r;
                     corr::knn_init(r);
-                    corr::knn_search(g, q.x, q.y, q.z, r);
+                    corr::knn_search<kSparse>(g, q.x, q.y, q.z, r);
                     int rpos[5];
                     corr::knn_positions(g, r, rpos);
 #pragma unroll
@@ -704,9 +705,9 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
 constexpr size_t kIter2SmemNoGrid = offsetof(Iter2Smem, grid);
 constexpr size_t kIter2SmemGrid = offsetof(Iter2Smem, radius);      // ... and odometry's radius fields only there
 
-template <bool kUseWd, bool kGrids, bool kSeq, bool kPlanes = false>
+template <bool kUseWd, bool kGrids, bool kSeq, bool kPlanes = false, bool kSparse = false>
 cudaError_t loop_kernel_attributes(size_t smem) {
-    cudaError_t e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids, kSeq, kPlanes>,
+    cudaError_t e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids, kSeq, kPlanes, kSparse>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     // the smallest shared-memory carveout that keeps 3 blocks resident (each also reserves 1 KB), so that the rest of the
     // SM's unified data cache is L1 for the searches' and certificates' target reads.  The percentage is of the largest
@@ -717,7 +718,7 @@ cudaError_t loop_kernel_attributes(size_t smem) {
     if (e == cudaSuccess) {
         const size_t need = 3 * (smem + 1024);
         const int pct = (int)std::min<size_t>(100, (need * 100 + (size_t)max_smem - 1) / (size_t)max_smem);
-        e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids, kSeq, kPlanes>, cudaFuncAttributePreferredSharedMemoryCarveout,
+        e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids, kSeq, kPlanes, kSparse>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                  pct);
     }
     return e;
@@ -899,6 +900,32 @@ __global__ void cell_key_kernel(const float4* __restrict__ pts, long long n, con
     if (grids) keys[i] = (unsigned long long)cell_off[b] + (unsigned long long)corr::source_cell(grids[b], T + (size_t)b * 16, p);
     else keys[i] = (unsigned long long)b * (unsigned long long)ncells + (unsigned long long)corr::source_cell(g, T + (size_t)b * 16, p);
     vals[i] = (int)i;
+}
+
+// Keys of the spatial sort against a sparse row index (sort_by_sparse_cell), whose box is too large for one cell id:
+// the cell (x, y, z) of fl32(T_b p) unclamped, in two stable passes.  Pass 0: key (y, x) of point i = j.  Pass 1: key
+// (segment b, z) of point i = order[j], the order pass 0 left.  Signed coordinates are flipped into unsigned order.
+__global__ void sparse_source_key_kernel(const float4* __restrict__ pts, long long n, const long long* __restrict__ seg,
+                                         int n_seg, const double* __restrict__ T, double inv_cell, int pass,
+                                         const int* __restrict__ order, unsigned long long* __restrict__ keys,
+                                         int* __restrict__ vals) {
+    const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const long long i = pass ? order[j] : j;
+    const int b = corr::segment_of(seg, n_seg, i);
+    const double* Tb = T + (size_t)b * 16;
+    const float4 p = pts[i];
+    const double px = p.x, py = p.y, pz = p.z;
+    if (pass == 0) {
+        const float qx = (float)(Tb[0] * px + Tb[1] * py + Tb[2] * pz + Tb[3]);
+        const float qy = (float)(Tb[4] * px + Tb[5] * py + Tb[6] * pz + Tb[7]);
+        keys[j] = ((unsigned long long)((unsigned)corr::cell_coord(qy, inv_cell) ^ 0x80000000u) << 32) |
+                  (unsigned long long)((unsigned)corr::cell_coord(qx, inv_cell) ^ 0x80000000u);
+    } else {
+        const float qz = (float)(Tb[8] * px + Tb[9] * py + Tb[10] * pz + Tb[11]);
+        keys[j] = ((unsigned long long)b << 32) | (unsigned long long)((unsigned)corr::cell_coord(qz, inv_cell) ^ 0x80000000u);
+    }
+    vals[j] = (int)i;
 }
 
 __global__ void gather_points_kernel(const float4* __restrict__ in, const int* __restrict__ idx, long long n,
@@ -2033,10 +2060,62 @@ static int build_hash_grid(dcreg_ctx* ctx, long long m, double inv_cell) {
     return DCREG_OK;
 }
 
-int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size) {
+// The context's target when its box has more than arena_plan::kMaxDenseCells cells and the caller asked for the sparse
+// row index (dcreg_set_target_sparse; sparse_index.hpp), from the bounds hb[6] of its m points.  One stable radix sort
+// of the box-local cell keys gives the dense grid's point order; the table holds cs of every cell a search can read.
+// One sync, for the entry count that sizes the table.  Points in tgt_arena, the table in the hash table's buffers.
+static int build_sparse_index(dcreg_ctx* ctx, long long m, double inv_cell, const int* hb) {
+    dcreg_ctx::GridArena& A = ctx->tgt_arena;
+    CK(A.pts.ensure(m));
+    CK(A.pos_of.ensure(m));
+    CK(ctx->d_scan_keys.ensure(2 * m));
+    CK(ctx->d_scan_vals.ensure(2 * m));
+    corr::Grid g{};
+    g.pts = A.pts; g.pos_of = A.pos_of; g.n = (int)m; g.dense = corr::kSparseGrid; g.rings = 1; g.inv_cell = inv_cell;
+    g.ox = hb[0]; g.oy = hb[1]; g.oz = hb[2];
+    g.nx = hb[3] - hb[0] + 1; g.ny = hb[4] - hb[1] + 1; g.nz = hb[5] - hb[2] + 1;
+    unsigned long long* keys = ctx->d_scan_keys;
+    int* vals = ctx->d_scan_vals;
+    const unsigned long long key_max = sparse_index::key(g.nx - 1, g.ny - 1, g.nz - 1);
+    int end_bit = 1;
+    while (end_bit < 64 && key_max >> end_bit) ++end_bit;
+    size_t tmp = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, keys, keys + m, vals, vals + m, (int)m, 0, end_bit, ctx->stream));
+    CK(ctx->d_scan_sort_tmp.ensure((long long)tmp));
+    tmp = (size_t)ctx->d_scan_sort_tmp.cap;
+    const unsigned nb = (unsigned)((m + 255) / 256);
+    corr::sparse_key_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_tgt, (int)m, g, keys, vals);
+    CK(cudaGetLastError());
+    CK(cub::DeviceRadixSort::SortPairs(ctx->d_scan_sort_tmp.p, tmp, keys, keys + m, vals, vals + m, (int)m, 0, end_bit,
+                                       ctx->stream));
+    const unsigned long long* sorted = keys + m;
+    corr::sparse_gather_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_tgt, vals + m, (int)m, A.pts, A.pos_of);
+    unsigned long long* d_entries = reinterpret_cast<unsigned long long*>(vals);      // (the sort's input values are spent)
+    CK(cudaMemsetAsync(d_entries, 0, sizeof(unsigned long long), ctx->stream));
+    corr::sparse_count_kernel<<<nb, 256, 0, ctx->stream>>>(sorted, (int)m, g.nx, d_entries);
+    CK(cudaGetLastError());
+    unsigned long long* h_entries = reinterpret_cast<unsigned long long*>(ctx->h_pinned.p);
+    CK(cudaMemcpyAsync(h_entries, d_entries, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    const long long cap = sparse_index::capacity((long long)*h_entries);
+    if (cap > (1ll << 32)) { ctx->err = "dcreg_set_target_sparse: the sparse index needs more than 2^32 table slots"; return DCREG_BAD_ARG; }
+    CK(ctx->d_hash_keys.ensure(cap));
+    CK(ctx->d_hash_start.ensure(cap));
+    g.keys = ctx->d_hash_keys; g.hstart = ctx->d_hash_start; g.hcount = nullptr; g.mask = (unsigned)(cap - 1);
+    CK(cudaMemsetAsync(g.keys, 0xff, (size_t)cap * sizeof(unsigned long long), ctx->stream));
+    corr::sparse_insert_kernel<<<nb, 256, 0, ctx->stream>>>(sorted, (int)m, g.nx, g);
+    ctx->launches += 4;                                          // (the radix sort's own kernels are not counted)
+    CK(cudaGetLastError());
+    ctx->grid = g;
+    return DCREG_OK;
+}
+
+// dcreg_set_target, and with `sparse` dcreg_set_target_sparse: the same up to the choice past the dense-cell limit
+static int set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size, bool sparse) {
     if (!ctx) return DCREG_BAD_ARG;
     if (!xyz || m <= 0 || stride < 3 || !(cell_size > 0.0) || m > 0x7fffffffLL) {
-        ctx->err = "dcreg_set_target: empty cloud, stride < 3, cell_size <= 0 or too many points";
+        ctx->err = std::string(sparse ? "dcreg_set_target_sparse" : "dcreg_set_target") +
+                   ": empty cloud, stride < 3, cell_size <= 0 or too many points";
         return DCREG_BAD_ARG;
     }
     CK(cudaSetDevice(ctx->device));
@@ -2062,13 +2141,21 @@ int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, do
         if ((rc = arena_fill(ctx, ctx->tgt_arena, ctx->d_tgt, d_seg, 1, m, &box, box.cells, inv_cell, 1))) return rc;
         ctx->grid = arena_grid(ctx->tgt_arena, box, m, inv_cell, 1);
         ctx->grid_cells = box.cells;
-    } else if ((rc = build_hash_grid(ctx, m, inv_cell))) {
+    } else if ((rc = sparse ? build_sparse_index(ctx, m, inv_cell, hb.data()) : build_hash_grid(ctx, m, inv_cell))) {
         return rc;
     }
     const cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) { ctx->err = std::string("grid build: ") + cudaGetErrorString(e); return DCREG_CUDA_ERROR; }
     ctx->has_grid = true;
     return DCREG_OK;
+}
+
+int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size) {
+    return set_target(ctx, xyz, m, stride, cell_size, false);
+}
+
+int dcreg_set_target_sparse(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size) {
+    return set_target(ctx, xyz, m, stride, cell_size, true);
 }
 
 // Post-run point-to-point metrics of n pairs, replaces calculatePointToPointError (DCReg/include/utils.hpp:538-589;
@@ -2140,6 +2227,10 @@ int dcreg_point_to_point_metrics(dcreg_ctx* ctx, const double T[16], double erro
     if (!T || !out) { ctx->err = "p2p metrics: null pointer"; return DCREG_BAD_ARG; }
     if (!ctx->d_src || !ctx->has_grid || !ctx->d_tgt) { ctx->err = "p2p metrics: set source and target first"; return DCREG_BAD_ARG; }
     if (!ctx->grid.dense) { ctx->err = "p2p metrics need the dense grid (target bounding box too large for this cell size)"; return DCREG_BAD_ARG; }
+    if (ctx->grid.dense == corr::kSparseGrid) {          // nn1_search expands rings over the whole box
+        ctx->err = "p2p metrics need the dense grid (the target is a sparse row index: dcreg_set_target_sparse)";
+        return DCREG_BAD_ARG;
+    }
     CK(cudaSetDevice(ctx->device));
     const int64_t seg[4] = {0, ctx->n_tgt, 0, ctx->n_src};
     long long* d_seg = own_segs(ctx);
@@ -2150,11 +2241,51 @@ int dcreg_point_to_point_metrics(dcreg_ctx* ctx, const double T[16], double erro
                        ctx->cell_size, error_threshold, "p2p metrics: the aligned source", out);
 }
 
-// Spatial sort of the source by the target cell of T*p (dense grids only): consecutive threads of the iteration
-// kernel then query neighbouring cells, so their candidate loads hit the same lines and their trip counts agree.
-// The sorted copy carries the original index in .w; the pose moves little during ICP, so one sort per run suffices.
+// Spatial sort against the context's sparse row index, whose box is too large for one cell id: the n points of every
+// segment b (d_seg, n_seg; null and 1: one cloud) by the cell of fl32(T_b p) (d_T [n_seg][16]), z, then y, then x, then
+// by index, unclamped - the order a dense grid's sort gives whenever those cells lie inside its box.  Two stable radix
+// passes, (y, x) then (segment, z), through the batch's key buffers; into out, w kept.
+static int sort_by_sparse_cell(dcreg_ctx* ctx, const float4* pts, long long n, const long long* d_seg, int n_seg,
+                               const double* d_T, float4* out) {
+    CK(ctx->d_scan_keys.ensure(2 * n));
+    CK(ctx->d_scan_vals.ensure(2 * n));
+    unsigned long long* keys = ctx->d_scan_keys;
+    int* vals = ctx->d_scan_vals;
+    int end_bit = 33;                                            // pass 1: segment above the 32 bits of z
+    while (end_bit < 64 && ((unsigned long long)(n_seg - 1) >> (end_bit - 32))) ++end_bit;
+    size_t tmp0 = 0, tmp1 = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp0, keys, keys + n, vals, vals + n, (int)n, 0, 64, ctx->stream));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp1, keys, keys + n, vals, vals + n, (int)n, 0, end_bit, ctx->stream));
+    CK(ctx->d_scan_sort_tmp.ensure((long long)std::max(tmp0, tmp1)));
+    const unsigned nb = (unsigned)((n + 255) / 256);
+    for (int pass = 0; pass < 2; ++pass) {
+        sparse_source_key_kernel<<<nb, 256, 0, ctx->stream>>>(pts, n, d_seg, n_seg, d_T, ctx->grid.inv_cell, pass, vals + n,
+                                                               keys, vals);
+        CK(cudaGetLastError());
+        size_t tmp = (size_t)ctx->d_scan_sort_tmp.cap;
+        CK(cub::DeviceRadixSort::SortPairs(ctx->d_scan_sort_tmp.p, tmp, keys, keys + n, vals, vals + n, (int)n, 0,
+                                           pass ? end_bit : 64, ctx->stream));
+    }
+    gather_points_kernel<<<nb, 256, 0, ctx->stream>>>(pts, vals + n, n, out);
+    ctx->launches += 3;                                          // (the radix sorts' own kernels are not counted)
+    CK(cudaGetLastError());
+    return DCREG_OK;
+}
+
+// Spatial sort of the source by the target cell of T*p (dense grids and sparse row indexes): consecutive threads of the
+// iteration kernel then query neighbouring cells, so their candidate loads hit the same lines and their trip counts
+// agree.  The sorted copy carries the original index in .w; the pose moves little during ICP, so one sort per run suffices.
 static int sort_source_by_cell(dcreg_ctx* ctx, const double T[16], const float4** src_out) {
     *src_out = ctx->d_src;
+    if (ctx->grid.dense == corr::kSparseGrid && ctx->n_src <= 0x7fffffffLL) {
+        CK(ctx->d_src_sorted.ensure(ctx->n_src));
+        double* dT = ctx->d_small + 640;
+        CK(cudaMemcpyAsync(dT, T, 12 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        const int rc = sort_by_sparse_cell(ctx, ctx->d_src, ctx->n_src, nullptr, 1, dT, ctx->d_src_sorted);
+        if (rc) return rc;
+        *src_out = ctx->d_src_sorted;
+        return DCREG_OK;
+    }
     if (!ctx->grid.dense || ctx->n_src > 0x7fffffffLL) return DCREG_OK;
     const long long n = ctx->n_src, ncells = ctx->grid_cells;
     CK(ctx->d_src_sorted.ensure(n));
@@ -2255,6 +2386,12 @@ static int sort_sources(dcreg_ctx* ctx, const Batch& S, const float4** src_out) 
     int rc = upload_points(ctx, S.xyz, n, S.stride, ctx->d_scan_seg, S.n, ctx->d_scan_src, ctx->d_scan_radius, S.order,
                            S.in_off, S.kind);
     if (rc) return rc;
+    if (S.sort == Batch::kContextGrid && ctx->grid.dense == corr::kSparseGrid) {
+        if ((rc = sort_by_sparse_cell(ctx, ctx->d_scan_src, n, ctx->d_scan_seg, S.n, ctx->d_T_init, ctx->d_scan_sorted)))
+            return rc;
+        *src_out = ctx->d_scan_sorted;
+        return DCREG_OK;
+    }
     unsigned long long* keys = ctx->d_scan_keys;
     int* vals = ctx->d_scan_vals;
     // keys below n * the cells of the context's grid or of the box, or below the table arena's cell count
@@ -2305,6 +2442,7 @@ struct LoopPlan {
     bool use_wd = false;
     bool grid_table = false;  // a batch whose trials search their own grids (Batch::grid_table)
     bool lanes = false;       // a batch in sequence lanes (b.seq)
+    bool sparse = false;      // it.grid is the context's sparse row index (the kSparse instantiations)
     const float* scan_radius = nullptr;   // the lever arms of a batch's sources, or null (the context's source)
 };
 
@@ -2315,6 +2453,7 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
     L.trials = trials; L.use_wd = prm->use_weight_derivative != 0;
     L.grid_table = batch && batch->grid_table;
     L.lanes = batch && batch->lanes > 0;
+    L.sparse = !L.grid_table && ctx->grid.dense == corr::kSparseGrid;
     L.scan_radius = batch ? ctx->d_scan_radius.p : nullptr;
     Iter2Args& b = L.b;
     IterArgs& a = b.it;
@@ -2407,6 +2546,11 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         CK((loop_kernel_attributes<true, true, true>)(sizeof(Iter2Smem)));
         CK((loop_kernel_attributes<false, true, true>)(sizeof(Iter2Smem)));
         CK((loop_kernel_attributes<false, false, false, true>)(kIter2SmemNoGrid));
+        CK((loop_kernel_attributes<true, false, false, false, true>)(kIter2SmemNoGrid));
+        CK((loop_kernel_attributes<false, false, false, false, true>)(kIter2SmemNoGrid));
+        CK((loop_kernel_attributes<true, false, true, false, true>)(kIter2SmemNoGrid));
+        CK((loop_kernel_attributes<false, false, true, false, true>)(kIter2SmemNoGrid));
+        CK((loop_kernel_attributes<false, false, false, true, true>)(kIter2SmemNoGrid));
         ctx->loop_attr_done = true;
     }
     return DCREG_OK;
@@ -2418,7 +2562,14 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
     ctx->nn_valid = true;
     const dim3 grid((unsigned)L.grid_x, (unsigned)L.trials);
     if (L.b.it.planes_out) {             // seam 1: dcreg_find_planes runs the context's grid with the default parameters
-        CK(launch_pdl(icp_iter2_kernel<false, false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+        if (L.sparse) CK(launch_pdl(icp_iter2_kernel<false, false, false, true, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+        else CK(launch_pdl(icp_iter2_kernel<false, false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+    } else if (L.sparse && L.lanes) {
+        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, true, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+        else CK(launch_pdl(icp_iter2_kernel<false, false, true, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+    } else if (L.sparse) {
+        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+        else CK(launch_pdl(icp_iter2_kernel<false, false, false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
     } else if (L.grid_table && L.lanes) {
         if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
         else CK(launch_pdl(icp_iter2_kernel<false, true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));

@@ -6,6 +6,7 @@ C3  make_parking  : ground-dominated local map + sparse verticals, LiDAR-like fr
     make_parking_pairs  : frame k+1 of that path against the local submap around pose k (scan/target pairs)
     make_parking_sequence : those frames with drifting odometry increments (sequences with chained priors)
     make_parking_sweeps : those frames skewed by the sensor's motion during each sweep, with per-point timestamps
+    make_large_map / make_large_map_frames : 4 x 4 parking maps 1 km apart (too large for a dense grid) and frames in them
 C4  make_corridor : two parallel walls + floor + ceiling, rank-deficient along x
 C5  trial_poses   : seeded perturbations t ~ U[-1, 1]^3 m, rpy ~ U[-3, 3]^3 deg for the Monte-Carlo (SURVEY.md §8d)
     load_pcd_xyz  : PCD v0.7 `DATA binary` with float32 fields (the shipped clouds, SURVEY.md Appendix B.3)
@@ -198,6 +199,44 @@ def make_parking_sweeps(n_frames, seed=47, n_map=500_000, n_scan=6_000, map_seed
         skewed.append(np.ascontiguousarray(api.se3_exp_apply(xi, -s, p).astype(np.float32)))
         stamps.append(tau)
     return skewed, stamps, T_true, deltas, frames
+
+
+def make_large_map(n_side=4, spacing=1000.0, n_map=500_000, map_seed=43, extent=60.0):
+    """A prior map too large for a dense grid: n_side x n_side parking maps (_parking_map, tile t from seed map_seed + t),
+    their centres spacing metres apart on a square lattice starting at the origin.  At 0.5 m cells the 4 x 4 default
+    spans about 6 240 x 6 240 x 7 = 2.7e8 cells (dcreg_set_target_sparse).  Returns (map (n_side^2 n_map, 3) float32,
+    tile centres (n_side^2, 3))."""
+    tiles, centres = [], []
+    for t in range(n_side * n_side):
+        c = np.array([spacing * (t % n_side), spacing * (t // n_side), 0.0])
+        tiles.append(_parking_map(np.random.default_rng(map_seed + t), n_map, extent).astype(np.float64) + c)
+        centres.append(c)
+    return np.ascontiguousarray(np.concatenate(tiles).astype(np.float32)), np.array(centres)
+
+
+def make_large_map_frames(n_frames, seed=61, n_side=4, spacing=1000.0, n_map=500_000, n_scan=6_000, map_seed=43,
+                          extent=60.0, max_range=30.0, path_half_length=20.0):
+    """Frames for localisation against make_large_map(n_side, spacing, n_map, map_seed, extent): frame k lies in tile
+    k % n_side^2, on that tile's make_parking_frames path (seed + t, map_seed + t), its poses shifted to the tile's centre,
+    so that the frames of one tile form one sequence.  Returns (frames: list of (N_k, 3) float32, T_true (n, 4, 4),
+    T_init (n, 4, 4), tile of every frame (n,))."""
+    n_tiles = n_side * n_side
+    tile = np.arange(n_frames) % n_tiles
+    frames = [None] * n_frames
+    T_true, T_init = np.zeros((n_frames, 4, 4)), np.zeros((n_frames, 4, 4))
+    for t in range(n_tiles):
+        ks = np.nonzero(tile == t)[0]
+        if ks.size == 0:
+            continue
+        f, Tt, Ti, _ = make_parking_frames(ks.size, seed=seed + t, n_map=n_map, n_scan=n_scan, map_seed=map_seed + t,
+                                           extent=extent, max_range=max_range, path_half_length=path_half_length)
+        c = np.array([spacing * (t % n_side), spacing * (t // n_side), 0.0])
+        for j, k in enumerate(ks):
+            frames[k] = f[j]
+            T_true[k], T_init[k] = Tt[j], Ti[j]
+            T_true[k][:3, 3] += c
+            T_init[k][:3, 3] += c
+    return frames, T_true, T_init, tile
 
 
 def trial_poses(n, seed=45, max_trans=1.0, max_rot_deg=3.0):

@@ -155,6 +155,17 @@ int dcreg_set_source(dcreg_ctx* ctx, const float* xyz, int64_t n, int stride);
  * exact 5-NN-within-radius then only needs the 27 surrounding cells), with a hash-table fallback when the bounding box
  * has more than 2^27 cells. */
 int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size);
+/* Target cloud for maps too large for a dense grid (city-scale prior maps).  Same arguments and checks as
+ * dcreg_set_target, and while the bounding box has at most 2^27 cells it IS dcreg_set_target (same launches, same
+ * bytes).  Past that the index is a sparse row index instead of the hash table: the points in the dense grid's order
+ * (by cell z, y, x, then index) and an open-addressing table of the row starts the searches read, about 12 B per table
+ * slot with at most 18 entries per occupied cell (2 slots per entry, rounded up to a power of two), instead of 12 B per
+ * cell of the box.  On it dcreg_icp_run, _enqueue / _fetch (records and coherent mode as on a dense grid),
+ * dcreg_icp_run_batch, _scans, _sequences and dcreg_find_planes work as on a dense grid: for sources whose query cells
+ * stay inside a dense grid's box, a target whose extra points lie outside every search returns that grid's results bit
+ * for bit.  dcreg_point_to_point_metrics refuses it (DCREG_BAD_ARG).  A cell coordinate outside +-2^19 gives
+ * DCREG_BAD_ARG. */
+int dcreg_set_target_sparse(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size);
 
 /* ---- seam 1: correspondence stage (icp_test_runner.cpp:1714-1813) -------------------------
  * For every source slot: q = fl32(R p + t), exact 5-NN in the target, 5th d^2 < radius^2,

@@ -266,6 +266,7 @@ static void write(FILE* f, const std::vector<T>& v) {
     if (v.size() && fwrite(v.data(), sizeof(T), v.size(), f) != v.size()) { fprintf(stderr, "short write\n"); exit(2); }
 }
 
+#ifndef CORR_SEARCH_NO_MAIN      // tools/test_sparse_search.cu reuses the input format and helpers above
 int main(int argc, char** argv) {
     if (argc != 3) { fprintf(stderr, "usage: %s <input> <output>\n", argv[0]); return 2; }
     const Input in = read_input(argv[1]);
@@ -337,3 +338,4 @@ int main(int argc, char** argv) {
     printf("CORR_SEARCH_DONE %d queries, %d row pairs\n", nq, in.nrr);
     return 0;
 }
+#endif
