@@ -95,7 +95,8 @@ _lib = None
 # every symbol include/dcreg_b200.h declares (checked by tests/test_abi.py)
 EXPORTS = [
     "dcreg_abi_version", "dcreg_create", "dcreg_destroy", "dcreg_last_error", "dcreg_default_params",
-    "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_set_target_sparse", "dcreg_find_planes",
+    "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_set_target_sparse", "dcreg_set_sparse_maps",
+    "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
     "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_icp_run_odometry_adaptive", "dcreg_odometry_open_adaptive", "dcreg_odometry_push_adaptive", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
@@ -124,6 +125,7 @@ def load_library():
     lib.dcreg_set_source.argtypes = [vp, C.POINTER(C.c_float), i64, ci]
     lib.dcreg_set_target.argtypes = [vp, C.POINTER(C.c_float), i64, ci, C.c_double]
     lib.dcreg_set_target_sparse.argtypes = [vp, C.POINTER(C.c_float), i64, ci, C.c_double]
+    lib.dcreg_set_sparse_maps.argtypes = [vp, ci]
     lib.dcreg_find_planes.argtypes = [vp, dp, C.c_double, dp, C.POINTER(i64)]
     lib.dcreg_reduce_normal_equations.argtypes = [vp, vp, vp, i64, dp, ci, dp, dp]
     lib.dcreg_reduce_normal_equations_f64plane.argtypes = [vp, vp, vp, i64, dp, ci, dp, dp]
@@ -729,6 +731,11 @@ class Context:
         a = _as_points(xyz)
         self._check(self.lib.dcreg_set_target_sparse(self._h, a.ctypes.data_as(C.POINTER(C.c_float)), a.shape[0],
                                                      a.shape[1], float(cell_size)))
+
+    def set_sparse_maps(self, enable: bool):
+        """Sparse row indexes, instead of a refusal, for odometry's local maps and icp_run_pairs' targets too large for
+        dense grids (include/dcreg_b200.h, dcreg_set_sparse_maps).  A session keeps the value it had when it opened."""
+        self._check(self.lib.dcreg_set_sparse_maps(self._h, 1 if enable else 0))
 
     # -- seams --
     def find_planes(self, T, search_radius: float, want_planes: bool = True):

@@ -81,4 +81,22 @@ inline std::string plan(int n, const int* bounds, std::vector<Box>& boxes, long 
     return std::string();
 }
 
+// plan for a caller that may build sparse row indexes instead (dcreg_set_sparse_maps): when plan rejects the clouds only
+// for their cell counts (a box over kMaxDenseCells, or over kMaxCells in all), *sparse is set and the reason is empty;
+// a coordinate outside the +-2^19 cell range is still refused, naming the first such cloud.  The boxes are then unset:
+// a sparse index takes its box from the bounds.
+inline std::string plan_or_sparse(int n, const int* bounds, std::vector<Box>& boxes, long long* total_cells,
+                                  const char* what, bool* sparse) {
+    *sparse = false;
+    const std::string why = plan(n, bounds, boxes, total_cells, what);
+    if (why.empty()) return why;
+    Box x;
+    for (int b = 0; b < n; ++b)
+        if (box_of(bounds + 6 * (size_t)b, &x) == kOutOfRange)
+            return out_of_range((std::string(what) + " " + std::to_string(b)).c_str());
+    *sparse = true;
+    *total_cells = 0;
+    return std::string();
+}
+
 }  // namespace arena_plan

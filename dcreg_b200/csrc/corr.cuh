@@ -307,6 +307,85 @@ __global__ void sparse_insert_kernel(const unsigned long long* __restrict__ sort
     }
 }
 
+// ---- the sparse row indexes of many clouds in one arena (segment b: points [seg[b], seg[b+1]), its index grids[b],
+// box fields set).  A cloud's box-local key takes 63 bits, so the cloud id does not fit beside it: the order (cloud,
+// z, y, x, index) comes from two stable passes.  Pass 0: key (y, x) of point i = j; pass 1: key (cloud, z) of point
+// i = order[j], the order pass 0 left.
+__global__ void sparse_seg_key_kernel(const float4* __restrict__ pts, int n, const long long* __restrict__ seg, int nseg,
+                                      const Grid* __restrict__ grids, int pass, const int* __restrict__ order,
+                                      unsigned long long* __restrict__ keys, int* __restrict__ vals) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const int i = pass ? order[j] : j;
+    const int b = segment_of(seg, nseg, i);
+    const Grid& g = grids[b];
+    const float4 p = pts[i];
+    if (pass == 0)
+        keys[j] = sparse_index::key(cell_coord(p.x, g.inv_cell) - g.ox, cell_coord(p.y, g.inv_cell) - g.oy, 0);
+    else
+        keys[j] = ((unsigned long long)b << sparse_index::kBits) | (unsigned long long)(cell_coord(p.z, g.inv_cell) - g.oz);
+    vals[j] = i;
+}
+
+// the points in sort order (w = index over all clouds, as arena_fill leaves it), the inverse permutation, and the
+// box-local key of every sorted position in its cloud's box (sorted positions keep the clouds' segments)
+__global__ void sparse_seg_gather_kernel(const float4* __restrict__ pts, const int* __restrict__ order, int n,
+                                         const long long* __restrict__ seg, int nseg, const Grid* __restrict__ grids,
+                                         float4* __restrict__ out, int* __restrict__ pos_of,
+                                         unsigned long long* __restrict__ sorted) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const int i = order[j];
+    const Grid& g = grids[segment_of(seg, nseg, j)];
+    float4 p = pts[i];
+    sorted[j] = sparse_index::key(cell_coord(p.x, g.inv_cell) - g.ox, cell_coord(p.y, g.inv_cell) - g.oy,
+                                  cell_coord(p.z, g.inv_cell) - g.oz);
+    p.w = __int_as_float(i);
+    out[j] = p;
+    pos_of[i] = j;
+}
+
+// every cloud's table entries (sparse_index::new_entries within its segment), summed into count[b]
+__global__ void sparse_seg_count_kernel(const unsigned long long* __restrict__ sorted, int n,
+                                        const long long* __restrict__ seg, int nseg, const Grid* __restrict__ grids,
+                                        unsigned long long* __restrict__ count) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    int b = nseg - 1;
+    unsigned c = 0;
+    if (j < n) {
+        b = segment_of(seg, nseg, j);
+        const long long first = seg[b];
+        if (j == first || sorted[j - 1] != sorted[j]) {
+            int lo, hi;
+            sparse_index::new_entries(sorted[j], j > first ? sorted[j - 1] : sparse_index::kEmpty, grids[b].nx, &lo, &hi);
+            if (hi >= lo) c = (unsigned)(hi - lo + 1);
+        }
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, b);
+    c = __reduce_add_sync(peers, c);
+    if ((int)(threadIdx.x & 31) == __ffs(peers) - 1 && c) atomicAdd(&count[b], (unsigned long long)c);
+}
+
+// ... and their cs in every cloud's own table, shifted by the cloud's first position
+__global__ void sparse_seg_insert_kernel(const unsigned long long* __restrict__ sorted, int n,
+                                         const long long* __restrict__ seg, int nseg, const Grid* __restrict__ grids) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const int b = segment_of(seg, nseg, j);
+    const long long first = seg[b];
+    if (j > first && sorted[j - 1] == sorted[j]) return;
+    const Grid& g = grids[b];
+    int lo, hi;
+    sparse_index::new_entries(sorted[j], j > first ? sorted[j - 1] : sparse_index::kEmpty, g.nx, &lo, &hi);
+    const unsigned long long row = sparse_index::row_of(sorted[j]) << sparse_index::kBits;
+    for (int x = lo; x <= hi; ++x) {
+        const unsigned long long k = row | (unsigned long long)x;
+        unsigned int s = sparse_index::slot(k, g.mask);
+        while (atomicCAS(&g.keys[s], sparse_index::kEmpty, k) != sparse_index::kEmpty) s = (s + 1) & g.mask;
+        g.hstart[s] = (int)(first + sparse_index::cs(sorted + first, seg[b + 1] - first, k));
+    }
+}
+
 // cs of box-local cell (x, yy, zz) of a sparse grid, or -1 when the table has no entry for it
 __device__ __forceinline__ int sparse_cs(const Grid& g, int zz, int yy, int x) {
     const unsigned long long k = sparse_index::key(x, yy, zz);

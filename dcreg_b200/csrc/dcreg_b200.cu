@@ -1361,6 +1361,8 @@ struct OdomSettings {
     // follows its sequence's motion-model error, under the ceiling params.search_radius
     bool adaptive = false;
     adaptive::Settings threshold{};
+    // (a session) dcreg_set_sparse_maps as it was at open; a one-shot call reads the context's
+    bool sparse_maps = false;
 };
 
 struct dcreg_ctx {
@@ -1473,6 +1475,10 @@ struct dcreg_ctx {
         DevBuf<float4> pts, tmp; DevBuf<int> pos_of, pt_cell;               // [points]
         DevBuf<int> cell_start, counts, fill;                               // [cells + 1], [cells + 1], [cells]
         DevBuf<corr::Grid> d_grids; DevBuf<int> d_cell_off, d_bounds;       // [clouds], [clouds + 1], [clouds][6]
+        // sparse row indexes instead (build_sparse_arena): [2][points] sort keys and values, the sort's scratch,
+        // [clouds] entry counts, and every cloud's table side by side
+        DevBuf<unsigned long long> skeys, entries, tab_keys; DevBuf<int> svals, tab_start;
+        DevBuf<unsigned char> sort_tmp;
         // room for m points in `cells` cells
         cudaError_t reserve(long long m, long long cells) {
             cudaError_t e;
@@ -1483,6 +1489,9 @@ struct dcreg_ctx {
         }
     };
     GridArena tgt_arena, pair_tgt, aligned, odom_maps;
+    // dcreg_set_sparse_maps: odometry's local maps and the pairs' targets past the dense-grid limits get sparse row
+    // indexes instead of a refusal (a session keeps the value it had at open)
+    bool sparse_maps = false;
     // the hash tables of a target too large for a dense grid (build_hash_grid; points in tgt_arena)
     DevBuf<unsigned long long> d_hash_keys; DevBuf<int> d_hash_start, d_hash_count;
     DevBuf<float4> d_pair_tgt;                                   // targets, packed (w = global index)
@@ -2013,20 +2022,115 @@ static int arena_fill(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_p
     return DCREG_OK;
 }
 
-// Both steps; a cloud whose box needs more than arena_plan::kMaxDenseCells cells is rejected (no hash grids here).
+// The arena's clouds as sparse row indexes (sparse_index.hpp) instead of dense grids, for a step or call whose boxes are
+// too large for them (arena_plan::plan_or_sparse): the m points of the n clouds with the bounds hb[n * 6] (host offsets
+// h_seg[n + 1]).  The points end in the order arena_fill gives them (by cloud, then cell z, y, x, then index; positions
+// and .w over all clouds) from two stable radix passes, (y, x) then (cloud, z); one count of every cloud's table entries
+// comes back in one sync (the only one); the tables lie side by side (sparse_index::layout), and on return A.d_grids[b]
+// is cloud b's index.  Five launches and one sync, whatever n.  *bad: the first cloud whose table would need more than
+// sparse_index::kMaxSlots slots (nothing is inserted), else -1.  cloud_rings: as in arena_fill.
+static int build_sparse_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_pts, const long long* d_seg,
+                              const std::vector<long long>& h_seg, int n, const int* hb, double inv_cell, int rings,
+                              const int* cloud_rings, int* bad) {
+    *bad = -1;
+    const long long m = h_seg[(size_t)n];
+    CK(A.pts.ensure(m));
+    CK(A.pos_of.ensure(m));
+    CK(A.skeys.ensure(2 * m));
+    CK(A.svals.ensure(2 * m));
+    CK(A.entries.ensure(n));
+    std::vector<corr::Grid> hg((size_t)n);
+    for (int b = 0; b < n; ++b) {
+        const int* x = hb + 6 * (size_t)b;
+        corr::Grid& g = hg[(size_t)b];
+        g.pts = A.pts; g.pos_of = A.pos_of; g.n = (int)m; g.dense = corr::kSparseGrid;
+        g.rings = cloud_rings ? cloud_rings[b] : rings; g.inv_cell = inv_cell;
+        g.ox = x[0]; g.oy = x[1]; g.oz = x[2];
+        g.nx = x[3] - x[0] + 1; g.ny = x[4] - x[1] + 1; g.nz = x[5] - x[2] + 1;
+    }
+    CK(cudaMemcpyAsync(A.d_grids, hg.data(), hg.size() * sizeof(corr::Grid), cudaMemcpyHostToDevice, ctx->stream));
+    unsigned long long* keys = A.skeys;
+    int* vals = A.svals;
+    int end_bit = sparse_index::kBits + 1;                       // pass 1: the cloud above the kBits of z
+    while (end_bit < 64 && ((unsigned long long)(n - 1) >> (end_bit - sparse_index::kBits))) ++end_bit;
+    size_t tmp0 = 0, tmp1 = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp0, keys, keys + m, vals, vals + m, (int)m, 0, 2 * sparse_index::kBits,
+                                       ctx->stream));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp1, keys, keys + m, vals, vals + m, (int)m, 0, end_bit, ctx->stream));
+    CK(A.sort_tmp.ensure((long long)std::max(tmp0, tmp1)));
+    const unsigned nb = (unsigned)((m + 255) / 256);
+    for (int pass = 0; pass < 2; ++pass) {
+        corr::sparse_seg_key_kernel<<<nb, 256, 0, ctx->stream>>>(d_pts, (int)m, d_seg, n, A.d_grids, pass, vals + m, keys,
+                                                                  vals);
+        CK(cudaGetLastError());
+        size_t tmp = (size_t)A.sort_tmp.cap;
+        CK(cub::DeviceRadixSort::SortPairs(A.sort_tmp.p, tmp, keys, keys + m, vals, vals + m, (int)m, 0,
+                                           pass ? end_bit : 2 * sparse_index::kBits, ctx->stream));
+    }
+    unsigned long long* sorted = keys;                           // (the passes' input keys are spent)
+    corr::sparse_seg_gather_kernel<<<nb, 256, 0, ctx->stream>>>(d_pts, vals + m, (int)m, d_seg, n, A.d_grids, A.pts,
+                                                                 A.pos_of, sorted);
+    CK(cudaMemsetAsync(A.entries, 0, (size_t)n * sizeof(unsigned long long), ctx->stream));
+    corr::sparse_seg_count_kernel<<<nb, 256, 0, ctx->stream>>>(sorted, (int)m, d_seg, n, A.d_grids, A.entries);
+    CK(cudaGetLastError());
+    CK(ctx->h_pinned.ensure((long long)n * (long long)sizeof(unsigned long long)));
+    std::vector<unsigned long long> entries((size_t)n);
+    CK(cudaMemcpyAsync(ctx->h_pinned.p, A.entries, entries.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                       ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    memcpy(entries.data(), ctx->h_pinned.p, entries.size() * sizeof(unsigned long long));
+    std::vector<long long> cap((size_t)n), off((size_t)n + 1);
+    ctx->launches += 4;                                          // (the radix sorts' own kernels are not counted)
+    if ((*bad = sparse_index::layout(n, entries.data(), cap.data(), off.data())) >= 0) return DCREG_OK;
+    CK(A.tab_keys.ensure(off[(size_t)n]));
+    CK(A.tab_start.ensure(off[(size_t)n]));
+    for (int b = 0; b < n; ++b) {
+        corr::Grid& g = hg[(size_t)b];
+        g.keys = A.tab_keys.p + off[(size_t)b]; g.hstart = A.tab_start.p + off[(size_t)b]; g.hcount = nullptr;
+        g.mask = (unsigned)(cap[(size_t)b] - 1);
+    }
+    CK(cudaMemcpyAsync(A.d_grids, hg.data(), hg.size() * sizeof(corr::Grid), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(A.tab_keys, 0xff, (size_t)off[(size_t)n] * sizeof(unsigned long long), ctx->stream));
+    corr::sparse_seg_insert_kernel<<<nb, 256, 0, ctx->stream>>>(sorted, (int)m, d_seg, n, A.d_grids);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return DCREG_OK;
+}
+
+// Both steps; a cloud whose box needs more than arena_plan::kMaxDenseCells cells is rejected (no hash grids here),
+// unless sparse_at is given: then such clouds (or more than kMaxCells in all) make every cloud a sparse row index
+// (build_sparse_arena), and *sparse_at is the first cloud over kMaxDenseCells (n: none, only the total is over), or -1
+// when the grids are dense.
 static int build_grid_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_pts, const int64_t* h_seg,
                             const long long* d_seg, int n, double cell_size, int rings, const char* what,
-                            long long* cells_out) {
+                            long long* cells_out, int* sparse_at = nullptr) {
     const double inv_cell = 1.0 / cell_size;
     std::vector<int> hb;
     int rc = arena_bounds(ctx, A, d_pts, h_seg, d_seg, n, inv_cell, hb);
     if (rc) return rc;
     std::vector<arena_plan::Box> boxes;
     long long cells = 0;
-    const std::string why = arena_plan::plan(n, hb.data(), boxes, &cells, what);
+    bool sparse = false;
+    const std::string why = sparse_at ? arena_plan::plan_or_sparse(n, hb.data(), boxes, &cells, what, &sparse)
+                                      : arena_plan::plan(n, hb.data(), boxes, &cells, what);
     if (!why.empty()) { ctx->err = why; return DCREG_BAD_ARG; }
     if (cells_out) *cells_out = cells;
-    return arena_fill(ctx, A, d_pts, d_seg, n, h_seg[n], boxes.data(), cells, inv_cell, rings);
+    if (!sparse) {
+        if (sparse_at) *sparse_at = -1;
+        return arena_fill(ctx, A, d_pts, d_seg, n, h_seg[n], boxes.data(), cells, inv_cell, rings);
+    }
+    arena_plan::Box x;
+    for (*sparse_at = 0; *sparse_at < n && arena_plan::box_of(hb.data() + 6 * (size_t)*sparse_at, &x) == arena_plan::kDense;)
+        ++*sparse_at;
+    int bad = -1;
+    if ((rc = build_sparse_arena(ctx, A, d_pts, d_seg, std::vector<long long>(h_seg, h_seg + n + 1), n, hb.data(),
+                                 inv_cell, rings, nullptr, &bad)))
+        return rc;
+    if (bad >= 0) {
+        ctx->err = std::string(what) + " " + std::to_string(bad) + ": its sparse index would need more than 2^32 table slots";
+        return DCREG_BAD_ARG;
+    }
+    return DCREG_OK;
 }
 
 // one-segment offset tables of the context's own clouds (device, in d_small): [0, 1] = {0, n_tgt}, [2, 3] = {0, n_src}
@@ -2158,6 +2262,13 @@ int dcreg_set_target_sparse(dcreg_ctx* ctx, const float* xyz, int64_t m, int str
     return set_target(ctx, xyz, m, stride, cell_size, true);
 }
 
+int dcreg_set_sparse_maps(dcreg_ctx* ctx, int enable) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (enable != 0 && enable != 1) { ctx->err = "set_sparse_maps: enable must be 0 or 1"; return DCREG_BAD_ARG; }
+    ctx->sparse_maps = enable == 1;
+    return DCREG_OK;
+}
+
 // Post-run point-to-point metrics of n pairs, replaces calculatePointToPointError (DCReg/include/utils.hpp:538-589;
 // called at icp_test_runner.cpp:506-510 and once per CSV row at :1463-1470).  Pair b: source d_src[src_off[b],
 // src_off[b+1]) under the pose d_T[16 b ..], target d_tgt[tgt_off[b], tgt_off[b+1]) with the dense grid fwd_grids[b]
@@ -2246,7 +2357,7 @@ int dcreg_point_to_point_metrics(dcreg_ctx* ctx, const double T[16], double erro
 // by index, unclamped - the order a dense grid's sort gives whenever those cells lie inside its box.  Two stable radix
 // passes, (y, x) then (segment, z), through the batch's key buffers; into out, w kept.
 static int sort_by_sparse_cell(dcreg_ctx* ctx, const float4* pts, long long n, const long long* d_seg, int n_seg,
-                               const double* d_T, float4* out) {
+                               const double* d_T, double inv_cell, float4* out) {
     CK(ctx->d_scan_keys.ensure(2 * n));
     CK(ctx->d_scan_vals.ensure(2 * n));
     unsigned long long* keys = ctx->d_scan_keys;
@@ -2259,7 +2370,7 @@ static int sort_by_sparse_cell(dcreg_ctx* ctx, const float4* pts, long long n, c
     CK(ctx->d_scan_sort_tmp.ensure((long long)std::max(tmp0, tmp1)));
     const unsigned nb = (unsigned)((n + 255) / 256);
     for (int pass = 0; pass < 2; ++pass) {
-        sparse_source_key_kernel<<<nb, 256, 0, ctx->stream>>>(pts, n, d_seg, n_seg, d_T, ctx->grid.inv_cell, pass, vals + n,
+        sparse_source_key_kernel<<<nb, 256, 0, ctx->stream>>>(pts, n, d_seg, n_seg, d_T, inv_cell, pass, vals + n,
                                                                keys, vals);
         CK(cudaGetLastError());
         size_t tmp = (size_t)ctx->d_scan_sort_tmp.cap;
@@ -2281,7 +2392,7 @@ static int sort_source_by_cell(dcreg_ctx* ctx, const double T[16], const float4*
         CK(ctx->d_src_sorted.ensure(ctx->n_src));
         double* dT = ctx->d_small + 640;
         CK(cudaMemcpyAsync(dT, T, 12 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-        const int rc = sort_by_sparse_cell(ctx, ctx->d_src, ctx->n_src, nullptr, 1, dT, ctx->d_src_sorted);
+        const int rc = sort_by_sparse_cell(ctx, ctx->d_src, ctx->n_src, nullptr, 1, dT, ctx->grid.inv_cell, ctx->d_src_sorted);
         if (rc) return rc;
         *src_out = ctx->d_src_sorted;
         return DCREG_OK;
@@ -2340,6 +2451,9 @@ struct Batch {
     const int* cell_off = nullptr;
     long long cells = 0;
     double cell_size = 0.0;
+    // the table's grids are sparse row indexes (build_sparse_arena): the kSparse instantiations, and kGridTable sorts
+    // by the unclamped cell (sort_by_sparse_cell)
+    bool sparse = false;
     // lanes: none (0), or the sources are frames that run one after another in `lanes` lanes (grid y of the loop kernel),
     // at most max_bodies loop bodies in all
     int lanes = 0;
@@ -2386,8 +2500,10 @@ static int sort_sources(dcreg_ctx* ctx, const Batch& S, const float4** src_out) 
     int rc = upload_points(ctx, S.xyz, n, S.stride, ctx->d_scan_seg, S.n, ctx->d_scan_src, ctx->d_scan_radius, S.order,
                            S.in_off, S.kind);
     if (rc) return rc;
-    if (S.sort == Batch::kContextGrid && ctx->grid.dense == corr::kSparseGrid) {
-        if ((rc = sort_by_sparse_cell(ctx, ctx->d_scan_src, n, ctx->d_scan_seg, S.n, ctx->d_T_init, ctx->d_scan_sorted)))
+    const bool sparse_ctx = S.sort == Batch::kContextGrid && ctx->grid.dense == corr::kSparseGrid;
+    if (sparse_ctx || (S.sort == Batch::kGridTable && S.sparse)) {
+        if ((rc = sort_by_sparse_cell(ctx, ctx->d_scan_src, n, ctx->d_scan_seg, S.n, ctx->d_T_init,
+                                      sparse_ctx ? ctx->grid.inv_cell : 1.0 / S.cell_size, ctx->d_scan_sorted)))
             return rc;
         *src_out = ctx->d_scan_sorted;
         return DCREG_OK;
@@ -2442,7 +2558,7 @@ struct LoopPlan {
     bool use_wd = false;
     bool grid_table = false;  // a batch whose trials search their own grids (Batch::grid_table)
     bool lanes = false;       // a batch in sequence lanes (b.seq)
-    bool sparse = false;      // it.grid is the context's sparse row index (the kSparse instantiations)
+    bool sparse = false;      // it.grid, or (grid_table) every grid of the table, is a sparse row index (kSparse)
     const float* scan_radius = nullptr;   // the lever arms of a batch's sources, or null (the context's source)
 };
 
@@ -2453,7 +2569,7 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
     L.trials = trials; L.use_wd = prm->use_weight_derivative != 0;
     L.grid_table = batch && batch->grid_table;
     L.lanes = batch && batch->lanes > 0;
-    L.sparse = !L.grid_table && ctx->grid.dense == corr::kSparseGrid;
+    L.sparse = L.grid_table ? batch->sparse : ctx->grid.dense == corr::kSparseGrid;
     L.scan_radius = batch ? ctx->d_scan_radius.p : nullptr;
     Iter2Args& b = L.b;
     IterArgs& a = b.it;
@@ -2551,6 +2667,10 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         CK((loop_kernel_attributes<true, false, true, false, true>)(kIter2SmemNoGrid));
         CK((loop_kernel_attributes<false, false, true, false, true>)(kIter2SmemNoGrid));
         CK((loop_kernel_attributes<false, false, false, true, true>)(kIter2SmemNoGrid));
+        CK((loop_kernel_attributes<true, true, false, false, true>)(kIter2SmemGrid));
+        CK((loop_kernel_attributes<false, true, false, false, true>)(kIter2SmemGrid));
+        CK((loop_kernel_attributes<true, true, true, false, true>)(sizeof(Iter2Smem)));
+        CK((loop_kernel_attributes<false, true, true, false, true>)(sizeof(Iter2Smem)));
         ctx->loop_attr_done = true;
     }
     return DCREG_OK;
@@ -2564,6 +2684,12 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
     if (L.b.it.planes_out) {             // seam 1: dcreg_find_planes runs the context's grid with the default parameters
         if (L.sparse) CK(launch_pdl(icp_iter2_kernel<false, false, false, true, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
         else CK(launch_pdl(icp_iter2_kernel<false, false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
+    } else if (L.sparse && L.grid_table && L.lanes) {
+        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, true, false, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+        else CK(launch_pdl(icp_iter2_kernel<false, true, true, false, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
+    } else if (L.sparse && L.grid_table) {
+        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, false, false, true>, grid, dim3(kBlock), kIter2SmemGrid, ctx->stream, L.b));
+        else CK(launch_pdl(icp_iter2_kernel<false, true, false, false, true>, grid, dim3(kBlock), kIter2SmemGrid, ctx->stream, L.b));
     } else if (L.sparse && L.lanes) {
         if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, true, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
         else CK(launch_pdl(icp_iter2_kernel<false, false, true, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
@@ -2904,7 +3030,7 @@ static int enqueue_iterations(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_param
         Iter2Args kb = L.b;
         kb.use_seeds = 0;
         key_bytes(key, &kb, sizeof(kb));
-        const int meta[4] = {L.grid_x, L.trials, L.use_wd ? 1 : 0, iters};
+        const int meta[5] = {L.grid_x, L.trials, L.use_wd ? 1 : 0, iters, L.sparse ? 1 : 0};   // (kSparse: another kernel)
         key_bytes(key, meta, sizeof(meta));
         key_bytes(key, prm, sizeof(*prm));
         cudaGraphExec_t exec = nullptr;
@@ -3327,6 +3453,9 @@ struct OdomCall {
     const float4* d_win = nullptr;
     dcreg_iter_log* dlog = nullptr; const float4* src_iter = nullptr;
     LoopPlan L; bool planned = false;
+    // (sparse_maps) the plan of the steps whose maps are sparse row indexes, made at the first such step
+    const bool sparse_maps = sess ? set.sparse_maps : ctx->sparse_maps;
+    LoopPlan L_sparse; bool planned_sparse = false;
     int failed = -1;                                // the step whose maps failed (-1: none)
     // (voxel map) where every sequence's map is: the session's maps before the first update, then each update's output
     odom_plan::MapState MS;
@@ -3666,10 +3795,12 @@ int OdomCall::step(int i) {
     std::vector<arena_plan::Box> boxes;
     long long cells = 0;
     std::string plan_why;
+    bool sparse = false;            // (sparse_maps) a lane's box, or the step's boxes in all, too large for dense grids
     if (sm.map) {
         if ((rc = arena_bounds(ctx, ctx->odom_maps, sm.map, in.seg.data(), sm.d_seg, st.active, inv_cell, hb, sm.more)))
             return rc;
-        plan_why = arena_plan::plan(st.active, hb.data(), boxes, &cells, "local map of lane");
+        plan_why = sparse_maps ? arena_plan::plan_or_sparse(st.active, hb.data(), boxes, &cells, "local map of lane", &sparse)
+                               : arena_plan::plan(st.active, hb.data(), boxes, &cells, "local map of lane");
     }
     int b = 0;
     const std::string why = odom_plan::map_failure(in, st.active, n_frames, arena_plan::kMaxPoints, sm.bad, sm.kept, hb,
@@ -3687,9 +3818,22 @@ int OdomCall::step(int i) {
         frame_radius[(size_t)P.input[(size_t)(st.first + j)]] = lane_r[(size_t)j];
         if (set.adaptive) lane_rings.push_back(std::max(1, search_rings(lane_r[(size_t)j], set.cell_size)));
     }
-    if ((rc = arena_fill(ctx, ctx->odom_maps, sm.map, sm.d_seg, st.active, m, boxes.data(), cells, inv_cell,
-                         search_rings(params->search_radius, set.cell_size), set.adaptive ? lane_rings.data() : nullptr)))
+    const int rings = search_rings(params->search_radius, set.cell_size);
+    if (sparse) {           // every lane a sparse row index (one more sync, for the tables' sizes)
+        std::vector<long long> seg((size_t)st.active + 1);
+        for (int j = 0; j <= st.active; ++j) seg[(size_t)j] = sm.kept.empty() ? in.seg[(size_t)j] : sm.kept[(size_t)j];
+        int bad = -1;
+        if ((rc = build_sparse_arena(ctx, ctx->odom_maps, sm.map, sm.d_seg, seg, st.active, hb.data(), inv_cell, rings,
+                                     set.adaptive ? lane_rings.data() : nullptr, &bad)))
+            return rc;
+        if (map_failed(in, &st, bad < 0 ? "" : "its local map's sparse index would need more than 2^32 table slots", bad)) {
+            failed = i;
+            return DCREG_OK;
+        }
+    } else if ((rc = arena_fill(ctx, ctx->odom_maps, sm.map, sm.d_seg, st.active, m, boxes.data(), cells, inv_cell, rings,
+                                set.adaptive ? lane_rings.data() : nullptr))) {
         return rc;
+    }
     // 3. every lane's frame of this step: its prior and a fresh loop state
     const int* d_prev = ctx->d_odom_int + at_int[(size_t)i] + st.map.piece_frame.size() + st.map.center.size();
     const int* d_prev2 = d_prev + st.active;
@@ -3712,13 +3856,17 @@ int OdomCall::step(int i) {
     }
     // 4. the loop: the same chunks (and CUDA graphs) at every step - the grid table keeps its pointer (the first step
     // has the most lanes, so the arena's table never regrows after it), only its entries change
-    if (!planned) {
+    // (a step of sparse maps runs the kSparse instantiation: a plan and chunk graphs of its own)
+    LoopPlan& LP = sparse ? L_sparse : L;
+    bool& have_plan = sparse ? planned_sparse : planned;
+    if (!have_plan) {
         S.grids = ctx->odom_maps.d_grids;
-        if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? R.log_cap : 0, true, &L, &S))) return rc;
-        L.b.lane_radius = set.adaptive ? ctx->d_lane_radius.p : nullptr;
-        planned = true;
+        S.sparse = sparse;
+        if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? R.log_cap : 0, true, &LP, &S))) return rc;
+        LP.b.lane_radius = set.adaptive ? ctx->d_lane_radius.p : nullptr;
+        have_plan = true;
     }
-    if ((rc = run_chunks(ctx, L, params, dlog, dlog ? R.log_cap : 0, params->max_iterations, 16, true))) return rc;
+    if ((rc = run_chunks(ctx, LP, params, dlog, dlog ? R.log_cap : 0, params->max_iterations, 16, true))) return rc;
     // 5. (adaptive) the step's frames into their sequences' threshold states, and the next step's radii
     if (set.adaptive) {
         const int* d_seq = d_prev2 + st.active;
@@ -3933,6 +4081,7 @@ static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     }
     std::unique_ptr<dcreg_ctx::OdomSession> ss(new dcreg_ctx::OdomSession());
     ss->set = set;
+    ss->set.sparse_maps = ctx->sparse_maps;
     const int n_seqs = set.n_seqs;
     BatchCheck c{name, !ss->set.T_init.empty(), "null pointer or n_seqs <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_seqs};
@@ -4112,16 +4261,27 @@ int dcreg_icp_run_pairs(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_pa
     // the targets: packed with w = index over all targets, then every pair's dense grid in the arena
     if ((rc = upload_points(ctx, tgt_xyz, n_tgt, stride, nullptr, 1, ctx->d_pair_tgt, nullptr))) return rc;
     Batch S{n_pairs, src_xyz, stride, src_offsets};
+    int sparse_at = -1;             // (sparse_maps) the targets are sparse row indexes: the first too large for a grid
     if ((rc = build_grid_arena(ctx, ctx->pair_tgt, ctx->d_pair_tgt, tgt_offsets, ctx->d_pair_tgt_seg, n_pairs, cell_size,
-                               search_rings(params->search_radius, cell_size), "icp_run_pairs: target", &S.cells)))
+                               search_rings(params->search_radius, cell_size), "icp_run_pairs: target", &S.cells,
+                               ctx->sparse_maps ? &sparse_at : nullptr)))
         return rc;
     S.sort = Batch::kGridTable;
     S.grid_table = true; S.grids = ctx->pair_tgt.d_grids; S.cell_off = ctx->pair_tgt.d_cell_off; S.cell_size = cell_size;
+    S.sparse = sparse_at >= 0;
     if ((rc = stage_sources(ctx, S)) ||
         (rc = run_loop(ctx, params, n_pairs, T_init, Results{T_out, n_iterations, converged, status, log, log_cap, cov}, true,
                        &S)))
         return rc;
     if (!metrics) return DCREG_OK;
+    if (S.sparse) {                 // nn1_search expands rings over the whole box
+        ctx->err = sparse_at < n_pairs
+                       ? "p2p metrics: the target of pair " + std::to_string(sparse_at) +
+                             " is too large for a dense grid (a sparse row index: the metrics need the dense grid)"
+                       : std::string("p2p metrics: the targets of the call exceed 2^30 dense cells in total (sparse row "
+                                     "indexes: the metrics need dense grids), from pair 0");
+        return DCREG_BAD_ARG;
+    }
     CK(cudaMemcpyAsync(ctx->d_pair_T, T_out, (size_t)n_pairs * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     return p2p_metrics(ctx, n_pairs, ctx->d_scan_src, ctx->d_scan_seg, src_offsets, ctx->d_pair_tgt, ctx->d_pair_tgt_seg,
                        tgt_offsets, ctx->pair_tgt.d_grids, ctx->d_pair_T, cell_size, error_threshold,

@@ -76,4 +76,20 @@ inline long long capacity(long long entries) {
     return cap;
 }
 
+constexpr long long kMaxSlots = 1ll << 32;           // Grid::mask is 32 bits
+
+// The tables of n clouds side by side in one buffer (the sparse arenas of odometry's local maps and of
+// dcreg_icp_run_pairs' targets): cloud b's table is slots [off[b], off[b] + cap[b]), cap[b] = capacity(entries[b]);
+// off has n + 1 entries, off[n] the total.  Returns the first cloud whose table would need more than kMaxSlots slots
+// (cap and off then hold the clouds before it), or -1.
+inline int layout(int n, const unsigned long long* entries, long long* cap, long long* off) {
+    off[0] = 0;
+    for (int b = 0; b < n; ++b) {
+        cap[b] = capacity((long long)entries[b]);
+        if (cap[b] > kMaxSlots) return b;
+        off[b + 1] = off[b] + cap[b];
+    }
+    return -1;
+}
+
 }  // namespace sparse_index

@@ -264,3 +264,35 @@ def load_pcd_xyz(path):
     a = np.frombuffer(raw, dtype="<f4", count=npts * nf, offset=head_end).reshape(npts, nf)
     cols = [hdr["FIELDS"].index(c) for c in ("x", "y", "z")]
     return np.ascontiguousarray(a[:, cols], dtype=np.float32)
+
+
+def make_long_range_sequence(n_frames, seed=47, n_far=2_000, far_range=(150.0, 200.0), far_height=20.0, n_facades=8,
+                             n_map=500_000, n_scan=6_000, map_seed=43, extent=60.0, max_range=30.0,
+                             path_half_length=20.0):
+    """A long-range sensor's recording: the frames of make_parking_frames(n_frames, seed, ...) plus sparse far
+    structure, n_facades world-fixed vertical facades (30 m wide, far_height tall from the ground at z = -1.8) at
+    horizontal distances in far_range from the origin, at evenly spaced azimuths.  Every frame sees n_far of their points
+    (5 mm noise), in its sensor frame.  With the defaults a window map spans about 400 x 400 x 20 m: at 0.25 m cells about
+    1 600 x 1 600 x 81 = 2.1e8 cells, past the dense grid's 2^27 (dcreg_set_sparse_maps).  Returns (frames: list of
+    (N_k, 3) float32, T_true (n, 4, 4), deltas (n, 4, 4) with deltas[k] = inv(T_k) T_{k+1} (the last the identity))."""
+    frames, T_true, _, _ = make_parking_frames(n_frames, seed=seed, n_map=n_map, n_scan=n_scan, map_seed=map_seed,
+                                               extent=extent, max_range=max_range, path_half_length=path_half_length)
+    rng = np.random.default_rng([seed, 3])
+    walls = []
+    for f in range(n_facades):
+        az = 2.0 * np.pi * f / n_facades
+        dist = rng.uniform(far_range[0], far_range[1])
+        c, u = dist * np.array([np.cos(az), np.sin(az)]), np.array([-np.sin(az), np.cos(az)])
+        m = 4 * n_far
+        w = rng.uniform(-15.0, 15.0, m)
+        walls.append(np.stack([c[0] + w * u[0], c[1] + w * u[1], -1.8 + rng.uniform(0.0, far_height, m)], axis=1))
+    far = np.concatenate(walls)
+    deltas = np.tile(np.eye(4), (n_frames, 1, 1))
+    for k in range(n_frames - 1):
+        deltas[k] = np.linalg.inv(T_true[k]) @ T_true[k + 1]
+    out = []
+    for k in range(n_frames):
+        pm = far[rng.choice(far.shape[0], n_far, replace=False)] + rng.normal(0, 0.005, (n_far, 3))
+        R, t = T_true[k][:3, :3], T_true[k][:3, 3]
+        out.append(np.ascontiguousarray(np.concatenate([frames[k], ((pm - t) @ R).astype(np.float32)])))
+    return out, T_true, deltas

@@ -166,6 +166,19 @@ int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, do
  * for bit.  dcreg_point_to_point_metrics refuses it (DCREG_BAD_ARG).  A cell coordinate outside +-2^19 gives
  * DCREG_BAD_ARG. */
 int dcreg_set_target_sparse(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size);
+/* Sparse row indexes for the grids the library builds itself: the local maps of dcreg_icp_run_odometry* and of the
+ * odometry sessions, and the targets of dcreg_icp_run_pairs.  enable = 0 (the default): such a map or target whose
+ * bounding box has more than 2^27 cells at cell_size, or a step's or call's grids with more than 2^30 cells in all, is
+ * DCREG_BAD_ARG, as documented at those calls.  enable = 1: that step (every lane of it) or that call (every pair of
+ * it) builds sparse row indexes instead (those of dcreg_set_target_sparse, one per map or target, in one set of buffers;
+ * one more host sync), and returns what the dense grids would return on the same points: a search of a sparse index
+ * gives the dense grid's results bit for bit.  A step or call that fits dense grids runs exactly as with enable = 0;
+ * there is no other choice between the two.  Still DCREG_BAD_ARG with enable = 1: a cell coordinate outside +-2^19, a
+ * map or target whose index would need more than 2^32 table slots, and, for dcreg_icp_run_pairs with metrics, a call
+ * whose targets are sparse (after the poses are written, naming the pair).  An odometry session keeps the value it had
+ * at dcreg_odometry_open*: changing it later does not change that session's pushes.  enable other than 0 or 1:
+ * DCREG_BAD_ARG. */
+int dcreg_set_sparse_maps(dcreg_ctx* ctx, int enable);
 
 /* ---- seam 1: correspondence stage (icp_test_runner.cpp:1714-1813) -------------------------
  * For every source slot: q = fl32(R p + t), exact 5-NN in the target, 5th d^2 < radius^2,
@@ -258,10 +271,13 @@ int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_sc
  * floats per point; pair b is source points [src_offsets[b], src_offsets[b+1]) against target points
  * [tgt_offsets[b], tgt_offsets[b+1]) (n_pairs + 1 entries each, ascending strictly from 0: no empty source or target;
  * at most 2^29 - 1 points per side, at most 65535 pairs).  cell_size: as in dcreg_set_target (search_radius / cell_size
- * in (0, 4]); every target needs a dense grid (at most 2^27 cells in its bounding box, 2^30 over the call).
+ * in (0, 4]); every target needs a dense grid (at most 2^27 cells in its bounding box, 2^30 over the call), unless
+ * dcreg_set_sparse_maps(1): then a call past those limits gives every target a sparse row index, and pair b equals
+ * dcreg_set_target_sparse(tgt_b) + dcreg_set_source(src_b) + dcreg_icp_run(T_init[b]) up to the FP64 grouping.
  * T_init / T_out / n_iterations / converged / status / cov / log: as in dcreg_icp_run_scans, one per pair.
  * metrics: n_pairs x 4 doubles or NULL; pair b's dcreg_point_to_point_metrics(T_out[b], error_threshold) = rmse, fitness,
- * chamfer, n_valid (an aligned source too large for a dense grid: DCREG_BAD_ARG after the poses are written).
+ * chamfer, n_valid (an aligned source too large for a dense grid, or a call whose targets are sparse row indexes:
+ * DCREG_BAD_ARG after the poses are written, naming the pair).
  * Pair b gives what dcreg_set_target(tgt_b, cell_size) + dcreg_set_source(src_b) + dcreg_icp_run(T_init[b]) gives up to
  * the grouping of the FP64 partial sums; a call reproduces bit for bit.  Needs no dcreg_set_target / dcreg_set_source
  * beforehand and leaves the context's source, target and grid as they were.  Not available on a sharded context. */
@@ -330,7 +346,9 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
  * most 2^29 - 1 map points over all sequences.  A map whose bounding box is too large for a dense grid at cell_size (over
  * 2^27 cells, or coordinates outside +-2^19 cells) is only found at its step: the call then returns DCREG_BAD_ARG with
  * dcreg_last_error naming the sequence and frame, the frames of the earlier steps have their outputs, and the context
- * stays usable.  The context's source, target and grid, and what the other calls compute, are left as they were.
+ * stays usable.  With dcreg_set_sparse_maps(1) a step whose maps are over 2^27 cells each, or 2^30 in all, gives every
+ * lane a sparse row index instead (one more host sync at that step) and returns the same results as dense grids would;
+ * coordinates outside +-2^19 cells are still refused.  The context's source, target and grid, and what the other calls compute, are left as they were.
  * A recording that arrives frame by frame, or is too long for one call (about 100 B of device memory per point of the
  * call), goes through an odometry session (dcreg_odometry_open / _push / _close): pushed in any chunks, it returns
  * exactly what one call over the whole recording returns. */
@@ -354,7 +372,8 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
  * Errors (DCREG_BAD_ARG, dcreg_last_error naming the sequence and frame): a negative or non-finite voxel size (before
  * anything is launched); a frame with no finite point, or a voxel coordinate of the source filter outside [-2^20, 2^20)
  * (after the frames' filter, before any loop launch); a step's map with a voxel coordinate outside that range (at its
- * step, like a map too large for a dense grid: the earlier steps keep their outputs, the context stays usable). */
+ * step, like a map too large for a dense grid: the earlier steps keep their outputs, the context stays usable).
+ * dcreg_set_sparse_maps applies as in dcreg_icp_run_odometry. */
 int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
                                  int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
                                  double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
@@ -430,9 +449,10 @@ int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params
  *   keeps its one host sync.  Buffers are sized from the sizes read back so far and grow with headroom.
  * Errors (DCREG_BAD_ARG before anything is launched): map_voxel not finite and > 0, map_max_points < 1, max_distance NaN
  * or <= 0 (+inf is allowed); everything else as in dcreg_icp_run_odometry_deskew.  At its step (dcreg_last_error naming
- * the sequence and frame; the earlier steps keep their outputs, the context stays usable): a map with no dense grid, an
- * empty map (every voxel pruned), a map voxel coordinate outside [-2^20, 2^20), more than 2^29 - 1 map points over a
- * step's sequences. */
+ * the sequence and frame; the earlier steps keep their outputs, the context stays usable): a map with no dense grid
+ * (without dcreg_set_sparse_maps(1), as in dcreg_icp_run_odometry), an empty map (every voxel pruned), a map voxel
+ * coordinate outside [-2^20, 2^20), more than 2^29 - 1 map points over a step's sequences.  An unpruned map
+ * (max_distance = +inf) of a long drive outgrows the dense grid: dcreg_set_sparse_maps(1) keeps it running. */
 int dcreg_icp_run_odometry_map(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
                                int n_frames, const float* xyz, const int64_t* frame_offsets, int stride, double cell_size,
                                int motion, double source_voxel, double map_voxel, int source_max_points,
@@ -448,7 +468,8 @@ int dcreg_icp_run_odometry_map(dcreg_ctx* ctx, const dcreg_icp_params* params, i
  * with the session's settings: T_prior, T_out, n_iterations, converged, status, cov, frame_points and the log records
  * (all but iter_time_ms).
  * dcreg_odometry_open: the settings of that call (params is copied; cell_size, map_frames, motion, voxel sizes and caps,
- *   T_init: n_seqs x 16), checked as that call checks them.  One session per context: open while one is open is
+ *   T_init: n_seqs x 16), checked as that call checks them, and dcreg_set_sparse_maps as it is at open (every push
+ *   uses that value, so any chunking still gives the one call's bytes; _open_map and _open_adaptive record it too).  One session per context: open while one is open is
  *   DCREG_BAD_ARG, as is a sharded context.  dcreg_destroy frees an open session.
  * dcreg_odometry_push: the next frames of the sequences.  seq_offsets: n_seqs + 1 NON-DECREASING ints from 0 to
  *   n_frames (n_frames >= 1; a sequence may get no frame, and then keeps its window untouched); xyz / frame_offsets /
