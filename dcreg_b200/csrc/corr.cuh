@@ -18,7 +18,8 @@
 //                has more than arena_plan::kMaxDenseCells cells); a query probes 27 cells.
 //   sparse mode: the dense order of the points, and cell_start only where a search can read it: a table of row starts
 //                (sparse_index.hpp) replaces the box's table, so the searches run the dense traversal with one table
-//                lookup per range end (dcreg_set_target_sparse).
+//                lookup per range end.  One build, the sparse_seg_* kernels below, serves dcreg_set_target_sparse (one
+//                cloud), odometry's local maps and dcreg_icp_run_pairs' targets (one cloud each).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -254,63 +255,10 @@ __global__ void source_cell_kernel(const float4* __restrict__ src, int n, Grid g
     atomicAdd(&counts[c], 1);
 }
 
-// ---- build of the sparse row index (sparse_index.hpp; g: the grid being built, box fields set) -----------------------
-// sort key of every point (its box-local cell) and its index as the value
-__global__ void sparse_key_kernel(const float4* __restrict__ pts, int n, Grid g, unsigned long long* __restrict__ keys,
-                                  int* __restrict__ vals) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float4 p = pts[i];
-    keys[i] = sparse_index::key(cell_coord(p.x, g.inv_cell) - g.ox, cell_coord(p.y, g.inv_cell) - g.oy,
-                                cell_coord(p.z, g.inv_cell) - g.oz);
-    vals[i] = i;
-}
-
-// the points in sort order (w = original index) and the inverse permutation
-__global__ void sparse_gather_kernel(const float4* __restrict__ pts, const int* __restrict__ order, int n,
-                                     float4* __restrict__ out, int* __restrict__ pos_of) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n) return;
-    const int i = order[j];
-    float4 p = pts[i];
-    p.w = __int_as_float(i);
-    out[j] = p;
-    pos_of[i] = j;
-}
-
-// table entries the occupied cell starting at sorted position j adds (sparse_index::new_entries), summed into *count
-__global__ void sparse_count_kernel(const unsigned long long* __restrict__ sorted, int n, int nx,
-                                    unsigned long long* __restrict__ count) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    unsigned long long c = 0;
-    if (j < n && (j == 0 || sorted[j - 1] != sorted[j])) {
-        int lo, hi;
-        sparse_index::new_entries(sorted[j], j > 0 ? sorted[j - 1] : sparse_index::kEmpty, nx, &lo, &hi);
-        if (hi >= lo) c = (unsigned long long)(hi - lo + 1);
-    }
-    c = __reduce_add_sync(0xffffffffu, (unsigned)c);
-    if ((threadIdx.x & 31) == 0 && c) atomicAdd(count, c);
-}
-
-// ... and their cs, each (row, x) inserted by the one cell that adds it
-__global__ void sparse_insert_kernel(const unsigned long long* __restrict__ sorted, int n, int nx, Grid g) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= n || (j > 0 && sorted[j - 1] == sorted[j])) return;
-    int lo, hi;
-    sparse_index::new_entries(sorted[j], j > 0 ? sorted[j - 1] : sparse_index::kEmpty, nx, &lo, &hi);
-    const unsigned long long row = sparse_index::row_of(sorted[j]) << sparse_index::kBits;
-    for (int x = lo; x <= hi; ++x) {
-        const unsigned long long k = row | (unsigned long long)x;
-        unsigned int s = sparse_index::slot(k, g.mask);
-        while (atomicCAS(&g.keys[s], sparse_index::kEmpty, k) != sparse_index::kEmpty) s = (s + 1) & g.mask;
-        g.hstart[s] = (int)sparse_index::cs(sorted, n, k);
-    }
-}
-
-// ---- the sparse row indexes of many clouds in one arena (segment b: points [seg[b], seg[b+1]), its index grids[b],
-// box fields set).  A cloud's box-local key takes 63 bits, so the cloud id does not fit beside it: the order (cloud,
-// z, y, x, index) comes from two stable passes.  Pass 0: key (y, x) of point i = j; pass 1: key (cloud, z) of point
-// i = order[j], the order pass 0 left.
+// ---- build: the sparse row indexes (sparse_index.hpp) of one or many clouds in one arena (segment b: points [seg[b],
+// seg[b+1]), its index grids[b], box fields set).  A cloud's box-local key takes 63 bits, so the cloud id does not fit
+// beside it: the order (cloud, z, y, x, index) comes from two stable passes.  Pass 0: key (y, x) of point i = j; pass
+// 1: key (cloud, z) of point i = order[j], the order pass 0 left.
 __global__ void sparse_seg_key_kernel(const float4* __restrict__ pts, int n, const long long* __restrict__ seg, int nseg,
                                       const Grid* __restrict__ grids, int pass, const int* __restrict__ order,
                                       unsigned long long* __restrict__ keys, int* __restrict__ vals) {

@@ -1468,9 +1468,9 @@ struct dcreg_ctx {
     // ... and with a cap above one point per voxel: [2][points] sort keys (slots) and values (indices) in / out
     DevBuf<unsigned int> d_vox_skey; DevBuf<int> d_vox_sval;
     DevBuf<unsigned char> d_vox_sort_tmp;
-    // Grow-only arenas of dense grids (build_grid_arena): the context's target (one cloud; `grid` points into it), the
-    // targets of dcreg_icp_run_pairs (the context's target and grid stay as they were), the grids over the aligned
-    // sources of the point-to-point metrics, and odometry's local maps
+    // Grow-only arenas of dense grids (build_grid_arena) or sparse row indexes (build_sparse_arena): the context's
+    // target (one cloud; `grid` points into it), the targets of dcreg_icp_run_pairs (the context's target and grid stay
+    // as they were), the grids over the aligned sources of the point-to-point metrics, and odometry's local maps
     struct GridArena {
         DevBuf<float4> pts, tmp; DevBuf<int> pos_of, pt_cell;               // [points]
         DevBuf<int> cell_start, counts, fill;                               // [cells + 1], [cells + 1], [cells]
@@ -1492,7 +1492,7 @@ struct dcreg_ctx {
     // dcreg_set_sparse_maps: odometry's local maps and the pairs' targets past the dense-grid limits get sparse row
     // indexes instead of a refusal (a session keeps the value it had at open)
     bool sparse_maps = false;
-    // the hash tables of a target too large for a dense grid (build_hash_grid; points in tgt_arena)
+    // the hash table of a dcreg_set_target target too large for a dense grid (build_hash_grid; points in tgt_arena)
     DevBuf<unsigned long long> d_hash_keys; DevBuf<int> d_hash_start, d_hash_count;
     DevBuf<float4> d_pair_tgt;                                   // targets, packed (w = global index)
     DevBuf<long long> d_pair_tgt_seg; DevBuf<double> d_pair_T;   // [n + 1] / [n][16] final poses
@@ -2028,10 +2028,11 @@ static int arena_fill(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_p
 // and .w over all clouds) from two stable radix passes, (y, x) then (cloud, z); one count of every cloud's table entries
 // comes back in one sync (the only one); the tables lie side by side (sparse_index::layout), and on return A.d_grids[b]
 // is cloud b's index.  Five launches and one sync, whatever n.  *bad: the first cloud whose table would need more than
-// sparse_index::kMaxSlots slots (nothing is inserted), else -1.  cloud_rings: as in arena_fill.
+// sparse_index::kMaxSlots slots (nothing is inserted), else -1.  cloud_rings: as in arena_fill.  grid0: if given, gets
+// cloud 0's index (the host copy of A.d_grids[0]).
 static int build_sparse_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_pts, const long long* d_seg,
                               const std::vector<long long>& h_seg, int n, const int* hb, double inv_cell, int rings,
-                              const int* cloud_rings, int* bad) {
+                              const int* cloud_rings, int* bad, corr::Grid* grid0 = nullptr) {
     *bad = -1;
     const long long m = h_seg[(size_t)n];
     CK(A.pts.ensure(m));
@@ -2051,12 +2052,19 @@ static int build_sparse_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const flo
     CK(cudaMemcpyAsync(A.d_grids, hg.data(), hg.size() * sizeof(corr::Grid), cudaMemcpyHostToDevice, ctx->stream));
     unsigned long long* keys = A.skeys;
     int* vals = A.svals;
-    int end_bit = sparse_index::kBits + 1;                       // pass 1: the cloud above the kBits of z
-    while (end_bit < 64 && ((unsigned long long)(n - 1) >> (end_bit - sparse_index::kBits))) ++end_bit;
+    // each pass sorts only the bits its keys use: up to the largest (y, x) of any box, and (last cloud, its top z)
+    unsigned long long top[2] = {0, 0};
+    for (int b = 0; b < n; ++b) {
+        const corr::Grid& g = hg[(size_t)b];
+        top[0] = std::max(top[0], sparse_index::key(g.nx - 1, g.ny - 1, 0));
+        top[1] = std::max(top[1], ((unsigned long long)b << sparse_index::kBits) | (unsigned long long)(g.nz - 1));
+    }
+    int end_bit[2] = {1, 1};
+    for (int p = 0; p < 2; ++p)
+        while (end_bit[p] < 64 && top[p] >> end_bit[p]) ++end_bit[p];
     size_t tmp0 = 0, tmp1 = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp0, keys, keys + m, vals, vals + m, (int)m, 0, 2 * sparse_index::kBits,
-                                       ctx->stream));
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp1, keys, keys + m, vals, vals + m, (int)m, 0, end_bit, ctx->stream));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp0, keys, keys + m, vals, vals + m, (int)m, 0, end_bit[0], ctx->stream));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp1, keys, keys + m, vals, vals + m, (int)m, 0, end_bit[1], ctx->stream));
     CK(A.sort_tmp.ensure((long long)std::max(tmp0, tmp1)));
     const unsigned nb = (unsigned)((m + 255) / 256);
     for (int pass = 0; pass < 2; ++pass) {
@@ -2064,8 +2072,8 @@ static int build_sparse_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const flo
                                                                   vals);
         CK(cudaGetLastError());
         size_t tmp = (size_t)A.sort_tmp.cap;
-        CK(cub::DeviceRadixSort::SortPairs(A.sort_tmp.p, tmp, keys, keys + m, vals, vals + m, (int)m, 0,
-                                           pass ? end_bit : 2 * sparse_index::kBits, ctx->stream));
+        CK(cub::DeviceRadixSort::SortPairs(A.sort_tmp.p, tmp, keys, keys + m, vals, vals + m, (int)m, 0, end_bit[pass],
+                                           ctx->stream));
     }
     unsigned long long* sorted = keys;                           // (the passes' input keys are spent)
     corr::sparse_seg_gather_kernel<<<nb, 256, 0, ctx->stream>>>(d_pts, vals + m, (int)m, d_seg, n, A.d_grids, A.pts,
@@ -2094,6 +2102,7 @@ static int build_sparse_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const flo
     corr::sparse_seg_insert_kernel<<<nb, 256, 0, ctx->stream>>>(sorted, (int)m, d_seg, n, A.d_grids);
     ctx->launches++;
     CK(cudaGetLastError());
+    if (grid0) *grid0 = hg[0];
     return DCREG_OK;
 }
 
@@ -2164,56 +2173,6 @@ static int build_hash_grid(dcreg_ctx* ctx, long long m, double inv_cell) {
     return DCREG_OK;
 }
 
-// The context's target when its box has more than arena_plan::kMaxDenseCells cells and the caller asked for the sparse
-// row index (dcreg_set_target_sparse; sparse_index.hpp), from the bounds hb[6] of its m points.  One stable radix sort
-// of the box-local cell keys gives the dense grid's point order; the table holds cs of every cell a search can read.
-// One sync, for the entry count that sizes the table.  Points in tgt_arena, the table in the hash table's buffers.
-static int build_sparse_index(dcreg_ctx* ctx, long long m, double inv_cell, const int* hb) {
-    dcreg_ctx::GridArena& A = ctx->tgt_arena;
-    CK(A.pts.ensure(m));
-    CK(A.pos_of.ensure(m));
-    CK(ctx->d_scan_keys.ensure(2 * m));
-    CK(ctx->d_scan_vals.ensure(2 * m));
-    corr::Grid g{};
-    g.pts = A.pts; g.pos_of = A.pos_of; g.n = (int)m; g.dense = corr::kSparseGrid; g.rings = 1; g.inv_cell = inv_cell;
-    g.ox = hb[0]; g.oy = hb[1]; g.oz = hb[2];
-    g.nx = hb[3] - hb[0] + 1; g.ny = hb[4] - hb[1] + 1; g.nz = hb[5] - hb[2] + 1;
-    unsigned long long* keys = ctx->d_scan_keys;
-    int* vals = ctx->d_scan_vals;
-    const unsigned long long key_max = sparse_index::key(g.nx - 1, g.ny - 1, g.nz - 1);
-    int end_bit = 1;
-    while (end_bit < 64 && key_max >> end_bit) ++end_bit;
-    size_t tmp = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp, keys, keys + m, vals, vals + m, (int)m, 0, end_bit, ctx->stream));
-    CK(ctx->d_scan_sort_tmp.ensure((long long)tmp));
-    tmp = (size_t)ctx->d_scan_sort_tmp.cap;
-    const unsigned nb = (unsigned)((m + 255) / 256);
-    corr::sparse_key_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_tgt, (int)m, g, keys, vals);
-    CK(cudaGetLastError());
-    CK(cub::DeviceRadixSort::SortPairs(ctx->d_scan_sort_tmp.p, tmp, keys, keys + m, vals, vals + m, (int)m, 0, end_bit,
-                                       ctx->stream));
-    const unsigned long long* sorted = keys + m;
-    corr::sparse_gather_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_tgt, vals + m, (int)m, A.pts, A.pos_of);
-    unsigned long long* d_entries = reinterpret_cast<unsigned long long*>(vals);      // (the sort's input values are spent)
-    CK(cudaMemsetAsync(d_entries, 0, sizeof(unsigned long long), ctx->stream));
-    corr::sparse_count_kernel<<<nb, 256, 0, ctx->stream>>>(sorted, (int)m, g.nx, d_entries);
-    CK(cudaGetLastError());
-    unsigned long long* h_entries = reinterpret_cast<unsigned long long*>(ctx->h_pinned.p);
-    CK(cudaMemcpyAsync(h_entries, d_entries, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    const long long cap = sparse_index::capacity((long long)*h_entries);
-    if (cap > (1ll << 32)) { ctx->err = "dcreg_set_target_sparse: the sparse index needs more than 2^32 table slots"; return DCREG_BAD_ARG; }
-    CK(ctx->d_hash_keys.ensure(cap));
-    CK(ctx->d_hash_start.ensure(cap));
-    g.keys = ctx->d_hash_keys; g.hstart = ctx->d_hash_start; g.hcount = nullptr; g.mask = (unsigned)(cap - 1);
-    CK(cudaMemsetAsync(g.keys, 0xff, (size_t)cap * sizeof(unsigned long long), ctx->stream));
-    corr::sparse_insert_kernel<<<nb, 256, 0, ctx->stream>>>(sorted, (int)m, g.nx, g);
-    ctx->launches += 4;                                          // (the radix sort's own kernels are not counted)
-    CK(cudaGetLastError());
-    ctx->grid = g;
-    return DCREG_OK;
-}
-
 // dcreg_set_target, and with `sparse` dcreg_set_target_sparse: the same up to the choice past the dense-cell limit
 static int set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size, bool sparse) {
     if (!ctx) return DCREG_BAD_ARG;
@@ -2245,7 +2204,13 @@ static int set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, d
         if ((rc = arena_fill(ctx, ctx->tgt_arena, ctx->d_tgt, d_seg, 1, m, &box, box.cells, inv_cell, 1))) return rc;
         ctx->grid = arena_grid(ctx->tgt_arena, box, m, inv_cell, 1);
         ctx->grid_cells = box.cells;
-    } else if ((rc = sparse ? build_sparse_index(ctx, m, inv_cell, hb.data()) : build_hash_grid(ctx, m, inv_cell))) {
+    } else if (sparse) {
+        int bad = -1;
+        if ((rc = build_sparse_arena(ctx, ctx->tgt_arena, ctx->d_tgt, d_seg, {0, m}, 1, hb.data(), inv_cell, 1, nullptr,
+                                     &bad, &ctx->grid)))
+            return rc;
+        if (bad >= 0) { ctx->err = "dcreg_set_target_sparse: the sparse index needs more than 2^32 table slots"; return DCREG_BAD_ARG; }
+    } else if ((rc = build_hash_grid(ctx, m, inv_cell))) {
         return rc;
     }
     const cudaError_t e = cudaStreamSynchronize(ctx->stream);

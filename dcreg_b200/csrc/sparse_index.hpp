@@ -1,5 +1,6 @@
-// sparse_index.hpp - the sparse row index of a target whose cell bounding box is too large for a dense grid
-// (dcreg_set_target_sparse).
+// sparse_index.hpp - the sparse row index of a cloud whose cell bounding box is too large for a dense grid: the
+// context's target (dcreg_set_target_sparse), odometry's local maps and dcreg_icp_run_pairs' targets
+// (dcreg_set_sparse_maps), each a cloud of a grid arena built by build_sparse_arena.
 //
 // The loop's searches never read a cell's own table entry: they read cell_start of a row (z, y) at two x positions and
 // scan the contiguous point range between them, [x0, x1) with x1 - x0 <= 2K + 1 <= kReach (K = rings <= 4).  The index
@@ -12,7 +13,7 @@
 //     occupied cell has both ends in the table, so a range is [cs(x0), cs(x1)) when both lookups hit and empty
 //     otherwise.
 // Coordinates are box-local (cell minus the box's minimum corner): every one lies in [0, 2^21), so a cell packs into
-// 63 bits with z in the high bits and its key is also the radix-sort key of the point order.  Plain C++ (host and
+// 63 bits with z in the high bits and the keys' order is the point order.  Plain C++ (host and
 // device): tests/test_sparse_index_twin.py builds it with tools/test_sparse_index.cpp.
 #pragma once
 #include <cstdint>
@@ -78,8 +79,8 @@ inline long long capacity(long long entries) {
 
 constexpr long long kMaxSlots = 1ll << 32;           // Grid::mask is 32 bits
 
-// The tables of n clouds side by side in one buffer (the sparse arenas of odometry's local maps and of
-// dcreg_icp_run_pairs' targets): cloud b's table is slots [off[b], off[b] + cap[b]), cap[b] = capacity(entries[b]);
+// The tables of n clouds side by side in one buffer (a sparse arena: the context's target is n = 1, and its one
+// table is capacity(entries[0]) slots at offset 0): cloud b's table is slots [off[b], off[b] + cap[b]), cap[b] = capacity(entries[b]);
 // off has n + 1 entries, off[n] the total.  Returns the first cloud whose table would need more than kMaxSlots slots
 // (cap and off then hold the clouds before it), or -1.
 inline int layout(int n, const unsigned long long* entries, long long* cap, long long* off) {

@@ -3,8 +3,9 @@ of the same points, and against the float32 brute force.
 
 tools/test_sparse_search.cu takes tools/test_corr_search.cu's input (the points, their dense layout and the queries of
 tests/test_gpu_corr_search.py, inside and outside the box, at ring counts 1-4), builds the sparse index with the
-production build kernels and runs knn_search, knn_search_lb, knn_warp_search (with and, at one ring, without the loop's
-row table) and knn_row_range on both.  Contracts:
+production build (build_sparse_arena's kernels on a one-cloud arena, the builder of every sparse index) and runs
+knn_search, knn_search_lb, knn_warp_search (with and, at one ring, without the loop's row table) and knn_row_range on
+both.  Contracts:
   * the sparse build's points and positions are byte-identical to the dense layout;
   * every search returns bit-identical keys, positions and lb on both (row pairs: lb, and [s, e) unless it is empty,
     which the sparse index reports as [0, 0) where the dense grid has [cs, cs));
