@@ -34,6 +34,7 @@
 #include "k1_reduce.cuh"
 #include "k1_stream.cuh"
 #include "k2_solve.cuh"
+#include "lane_plan.hpp"
 #include "loop_plan.hpp"
 #include "odom_plan.hpp"
 #include "se3.cuh"
@@ -292,6 +293,11 @@ struct Iter2Args {
     // lane runs at this step, in device memory (a captured chunk freezes its arguments), or null: prm.search_radius.
     // Only the icp_iter2_kernel<., true, true> instantiation reads it
     const double* lane_radius;
+    // per-lane solver settings (dcreg_set_lane_params): [lanes] in device memory, grid y's entry lane_prm[ys], or with
+    // lane_seq (odometry, whose steps compact the lanes) lane_prm[lane_seq[ys]]; null: it.prm for every lane.  Only a
+    // lane whose settings run "Ours" folds its solve step; k2_step_kernel runs the others'
+    const dcreg_icp_params* lane_prm;
+    const int* lane_seq;
 };
 
 __device__ __forceinline__ void cswap5(unsigned long long& ka, int& pa, unsigned long long& kb, int& pb) {
@@ -676,11 +682,16 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     if (tid < kAcc) A.acc[(size_t)ys * kAcc + tid] = sm.tail.acc[tid];
     if (a.fold_k2 && warp == 0) {
         const dcreg_icp_params* prm = &A.prm;
+        if (a.lane_prm) {                         // per-lane settings: this lane's, and k2_step_kernel steps a baseline lane
+            prm = a.lane_prm + (a.lane_seq ? a.lane_seq[ys] : ys);
+            if (!(prm->detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm->handling == DCREG_HAND_PRECONDITIONED_CG))
+                return;
+        }
         if constexpr (kGrids && kSeq) {           // the step limit of coherent mode follows the frame's own radius
             if (a.lane_radius) {
                 static_assert(sizeof(dcreg_icp_params) % sizeof(int) == 0, "parameter copy");
                 for (int e = lane; e < (int)(sizeof(dcreg_icp_params) / sizeof(int)); e += 32)
-                    reinterpret_cast<int*>(&sm.prm)[e] = reinterpret_cast<const int*>(&A.prm)[e];
+                    reinterpret_cast<int*>(&sm.prm)[e] = reinterpret_cast<const int*>(prm)[e];
                 __syncwarp();
                 if (lane == 0) sm.prm.search_radius = sm.radius;
                 __syncwarp();
@@ -740,10 +751,13 @@ struct K2Scratch {
 // radius_per_trial: src_radius is [B] (a batch of different scans) instead of one value for every trial.
 // seq.cursor set (sequences of frames): blockIdx.x is a lane with acc_all [lanes][kAcc]; its trial is the frame it runs
 // now, and the step that stops a frame advances the lane (no rehearsal: scratch is null).  lane_radius: Iter2Args's, or null
+// lane_prm, lane_seq: Iter2Args's (per-lane settings; prm is entry 0); folded: the iteration kernel has run the step of
+// every lane whose settings run "Ours", so their blocks return at once
 __global__ void __launch_bounds__(32) k2_step_kernel(const double* acc_all, IcpState* st_all, dcreg_icp_params prm,
                                                      dcreg_iter_log* log_all, int log_cap, const float* src_radius,
                                                      double coherent_step, K2Scratch* scratch, unsigned int* n_active,
-                                                     int radius_per_trial, SeqView seq, const double* lane_radius) {
+                                                     int radius_per_trial, SeqView seq, const double* lane_radius,
+                                                     const dcreg_icp_params* lane_prm, const int* lane_seq, int folded) {
     __shared__ k2::WarpSmem sm;
     pdl_release();
     const int lane = threadIdx.x;
@@ -754,12 +768,23 @@ __global__ void __launch_bounds__(32) k2_step_kernel(const double* acc_all, IcpS
         trial = seq.cursor[blockIdx.x];
         if (trial >= seq.first[blockIdx.x + 1]) return;
     }
+    // the lane's settings in shared memory: its entry (read after the cursor, since a lane past its last frame may be
+    // past the step's lanes of lane_seq too), or prm.  The step reads them there in both cases
+    __shared__ dcreg_icp_params P;
+    if (lane_prm) {
+        const int* from = reinterpret_cast<const int*>(lane_prm + (lane_seq ? lane_seq[blockIdx.x] : blockIdx.x));
+        for (int e = lane; e < (int)(sizeof(dcreg_icp_params) / sizeof(int)); e += 32) reinterpret_cast<int*>(&P)[e] = from[e];
+    } else if (lane == 0) {
+        P = prm;
+    }
+    __syncwarp();
+    const bool warp_path = P.detection == DCREG_DET_SCHUR_CONDITION_NUMBER && P.handling == DCREG_HAND_PRECONDITIONED_CG;
+    if (folded && warp_path) return;
     IcpState* st = st_all + trial;
     dcreg_iter_log* log = log_all ? log_all + (size_t)trial * log_cap : nullptr;
     if (src_radius && radius_per_trial) src_radius += trial;
     // (odometry's adaptive threshold: the lane's own search radius, Iter2Args::lane_radius)
     const double max_step = coherent_step * (lane_radius ? lane_radius[blockIdx.x] : prm.search_radius);
-    const bool warp_path = prm.detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm.handling == DCREG_HAND_PRECONDITIONED_CG;
 #pragma unroll 1
     for (int pass = scratch ? 0 : 1; pass < 2; ++pass) {
         const double* acc_use = acc;
@@ -777,9 +802,9 @@ __global__ void __launch_bounds__(32) k2_step_kernel(const double* acc_all, IcpS
         // mode of the next iteration kernel: records pay off once no source point moves more than ~5 % of the search radius
         const double lever = src_radius ? (double)*src_radius : 1.0e30;
         if (warp_path) {
-            k2::icp_step_warp_ours(acc_use, st_use, prm, log_use, log_cap, sm, lever, max_step);   // all 32 lanes cooperate
+            k2::icp_step_warp_ours(acc_use, st_use, P, log_use, log_cap, sm, lever, max_step);   // all 32 lanes cooperate
         } else if (lane == 0) {
-            k2::icp_step(acc_use, st_use, prm, log_use, log_cap, lever, max_step);    // baseline methods: generic single-thread path
+            k2::icp_step(acc_use, st_use, P, log_use, log_cap, lever, max_step);    // baseline methods: generic single-thread path
         }
         __syncwarp();
         if (pass == 1 && scratch) scratch->acc_prev[lane] = acc[lane];              // kAcc == 32: next launch's rehearsal input
@@ -799,7 +824,20 @@ __global__ void k2_analyze_kernel(const double* v27, dcreg_icp_params prm, dcreg
 // values.  The "Ours" step (k2::icp_step_warp_ours) has its own arithmetic: the decisions it wrote (mask, is_degenerate,
 // schur_singular, PCG iterations and residual) are kept, so the record describes the step that moved the pose even
 // where a decision sits within rounding of its threshold and the seam's code would have gone the other way.
-__global__ void log_fill_kernel(dcreg_iter_log* logs, int log_cap, const IcpState* states, dcreg_icp_params prm) {
+// lane_prm (per-lane settings, prm is entry 0): trial y's record uses lane_prm[trial_lane[y]], or without trial_lane
+// lane_prm[y]; null: prm.
+__global__ void log_fill_kernel(dcreg_iter_log* logs, int log_cap, const IcpState* states, dcreg_icp_params prm,
+                                const dcreg_icp_params* lane_prm, const int* trial_lane) {
+    // the trial's settings in shared memory (every thread of the block fills the same trial's records)
+    __shared__ dcreg_icp_params P;
+    if (lane_prm) {
+        const int* from = reinterpret_cast<const int*>(lane_prm + (trial_lane ? trial_lane[blockIdx.y] : blockIdx.y));
+        for (int e = threadIdx.x; e < (int)(sizeof(dcreg_icp_params) / sizeof(int)); e += blockDim.x)
+            reinterpret_cast<int*>(&P)[e] = from[e];
+    } else if (threadIdx.x == 0) {
+        P = prm;
+    }
+    __syncthreads();
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const IcpState* st = states + blockIdx.y;
     dcreg_iter_log* log = logs + (size_t)blockIdx.y * log_cap;
@@ -807,13 +845,13 @@ __global__ void log_fill_kernel(dcreg_iter_log* logs, int log_cap, const IcpStat
     if (i >= n) return;
     if (log[i].status != DCREG_OK) return;
     dcreg_analysis* a = &log[i].analysis;
-    const bool ours = prm.detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm.handling == DCREG_HAND_PRECONDITIONED_CG;
+    const bool ours = P.detection == DCREG_DET_SCHUR_CONDITION_NUMBER && P.handling == DCREG_HAND_PRECONDITIONED_CG;
     int mask[6];
     for (int k = 0; k < 6; ++k) mask[k] = a->degenerate_mask[k];
     const int is_deg = a->is_degenerate, singular = a->schur_singular, pcg_it = a->pcg_iterations;
     const double pcg_res = a->pcg_residual;
     double dx[6];
-    k2::analyze_and_solve<true>(log[i].H27, prm, a, dx);
+    k2::analyze_and_solve<true>(log[i].H27, P, a, dx);
     if (ours) {
         for (int k = 0; k < 6; ++k) a->degenerate_mask[k] = mask[k];
         a->is_degenerate = is_deg; a->schur_singular = singular;
@@ -1363,6 +1401,9 @@ struct OdomSettings {
     adaptive::Settings threshold{};
     // (a session) dcreg_set_sparse_maps as it was at open; a one-shot call reads the context's
     bool sparse_maps = false;
+    // dcreg_set_lane_params on (at open, for a session): every sequence's settings [n_seqs], params being entry 0; off:
+    // empty
+    std::vector<dcreg_icp_params> lanes;
 };
 
 struct dcreg_ctx {
@@ -1492,6 +1533,12 @@ struct dcreg_ctx {
     // dcreg_set_sparse_maps: odometry's local maps and the pairs' targets past the dense-grid limits get sparse row
     // indexes instead of a refusal (a session keeps the value it had at open)
     bool sparse_maps = false;
+    // dcreg_set_lane_params: the batched calls' params point to one entry per lane (a session keeps the value it had at
+    // open).  A call's entries [lanes] (plan_iteration), an odometry step's device lane -> sequence [lanes], and the log
+    // fill's device trial -> lane [trials]
+    bool lane_params = false;
+    DevBuf<dcreg_icp_params> d_lane_prm;
+    DevBuf<int> d_lane_seq, d_trial_lane;
     // the hash table of a dcreg_set_target target too large for a dense grid (build_hash_grid; points in tgt_arena)
     DevBuf<unsigned long long> d_hash_keys; DevBuf<int> d_hash_start, d_hash_count;
     DevBuf<float4> d_pair_tgt;                                   // targets, packed (w = global index)
@@ -2234,6 +2281,13 @@ int dcreg_set_sparse_maps(dcreg_ctx* ctx, int enable) {
     return DCREG_OK;
 }
 
+int dcreg_set_lane_params(dcreg_ctx* ctx, int enable) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (enable != 0 && enable != 1) { ctx->err = "set_lane_params: enable must be 0 or 1"; return DCREG_BAD_ARG; }
+    ctx->lane_params = enable == 1;
+    return DCREG_OK;
+}
+
 // Post-run point-to-point metrics of n pairs, replaces calculatePointToPointError (DCReg/include/utils.hpp:538-589;
 // called at icp_test_runner.cpp:506-510 and once per CSV row at :1463-1470).  Pair b: source d_src[src_off[b],
 // src_off[b+1]) under the pose d_T[16 b ..], target d_tgt[tgt_off[b], tgt_off[b+1]) with the dense grid fwd_grids[b]
@@ -2517,7 +2571,8 @@ static int search_rings(double search_radius, double cell_size) {
 // What one loop body looks like for this context: the loop kernel's arguments and grid, and whether the solve step is
 // inside it.
 struct LoopPlan {
-    bool fold_k2 = false;     // the solve / update step runs in the iteration kernel's last block
+    bool fold_k2 = false;     // the solve / update step runs in the iteration kernel's last block (of some lanes)
+    bool k2 = true;           // k2_step_kernel follows the iteration kernel (the step of some lanes is not folded)
     int grid_x = 1, trials = 1;
     Iter2Args b{};            // arguments of icp_iter2_kernel
     bool use_wd = false;
@@ -2527,9 +2582,25 @@ struct LoopPlan {
     const float* scan_radius = nullptr;   // the lever arms of a batch's sources, or null (the context's source)
 };
 
-// batch: a batch of sources (trial b = source b, or lane b; src = the sources in sort order), or null (the context's source)
+// The per-lane settings of a batched call (dcreg_set_lane_params): its n entries, one per lane, or none (n = 0: every
+// lane runs the call's params)
+struct Lanes {
+    const dcreg_icp_params* p = nullptr;
+    int n = 0;
+};
+
+// params' lanes when the setting is on: none when every entry has entry 0's settings, so that such a call is the call
+// with one params (the same launches, graphs and bytes)
+static Lanes call_lanes(const dcreg_icp_params* params, int n, bool on) {
+    if (!on || n < 2 || lane_plan::uniform(params, n)) return Lanes{};
+    return Lanes{params, n};
+}
+
+// batch: a batch of sources (trial b = source b, or lane b; src = the sources in sort order), or null (the context's
+// source).  lanes: the call's per-lane settings (prm is entry 0), written to the context's lane table
 static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const float4* src, double4* planes_out, int trials,
-                          dcreg_iter_log* dlog, int log_cap, bool want_fold, LoopPlan* plan, const Batch* batch = nullptr) {
+                          dcreg_iter_log* dlog, int log_cap, bool want_fold, LoopPlan* plan, const Batch* batch = nullptr,
+                          const Lanes& lanes = Lanes{}) {
     LoopPlan& L = *plan;
     L.trials = trials; L.use_wd = prm->use_weight_derivative != 0;
     L.grid_table = batch && batch->grid_table;
@@ -2579,12 +2650,20 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         }
         b.nn = ctx->d_nn; b.plane_cache = ctx->d_plane_cache; b.fit_state = ctx->d_fit_state; b.plane_key = ctx->d_plane_key;
     }
-    // the solve step inside the kernel unless the sum over ranks has to go through NCCL
-    L.fold_k2 = want_fold && !(ctx->comm && !ctx->peer_ok) &&
-                prm->detection == DCREG_DET_SCHUR_CONDITION_NUMBER && prm->handling == DCREG_HAND_PRECONDITIONED_CG;
+    // the solve step inside the kernel unless the sum over ranks has to go through NCCL, for the lanes that run "Ours"
+    // (lane_plan.hpp): all of them, none, or a mix, which runs K2 after the iteration kernel as well
+    const bool can_fold = want_fold && !(ctx->comm && !ctx->peer_ok);
+    const lane_plan::Mix mix = lanes.n ? lane_plan::mix(lanes.p, lanes.n, can_fold) : lane_plan::mix(prm, 1, can_fold);
+    L.fold_k2 = mix.fold; L.k2 = mix.k2;
+    if (lanes.n) {
+        CK(ctx->d_lane_prm.ensure(lanes.n));
+        CK(cudaMemcpyAsync(ctx->d_lane_prm, lanes.p, (size_t)lanes.n * sizeof(dcreg_icp_params), cudaMemcpyHostToDevice,
+                           ctx->stream));
+        b.lane_prm = ctx->d_lane_prm;
+    }
     // a single folded run: block 0 is a dedicated solver block (solver_block); batches keep the ticket, since a
     // solver block per trial in a multi-wave grid could fill every resident slot with waiting blocks
-    const bool solver = L.fold_k2 && trials == 1 && !batch && !getenv("DCREG_NO_SOLVER_BLOCK");
+    const bool solver = L.fold_k2 && trials == 1 && !batch && !lanes.n && !getenv("DCREG_NO_SOLVER_BLOCK");
     // blocks per trial and slots per block: loop_plan.hpp
     const loop_plan::Tiles tp = batch ? loop_plan::plan_scan_tiles(batch->max_n(), kBlock)
                                       : loop_plan::plan_tiles(slots, trials, ctx->sm_count, kBlock, solver ? 1 : 0);
@@ -2684,11 +2763,12 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
 // context's source).  seq: the lanes of a batch (trials = lanes), or null; lane_radius: Iter2Args's
 static int launch_k2(dcreg_ctx* ctx, const dcreg_icp_params* prm, dcreg_iter_log* dlog, int log_cap, double coherent_step,
                      int trials = 1, const float* scan_radius = nullptr, const SeqView* seq = nullptr,
-                     const double* lane_radius = nullptr) {
+                     const double* lane_radius = nullptr, const LoopPlan* L = nullptr) {
     CK(launch_pdl(k2_step_kernel, dim3((unsigned)trials), dim3(32), 0, ctx->stream, (const double*)ctx->d_acc.p, ctx->d_state.p, *prm,
                   dlog, log_cap, scan_radius ? scan_radius : (const float*)ctx->d_src_radius.p, coherent_step,
                   trials == 1 && !seq ? ctx->d_k2_scratch.p : (K2Scratch*)nullptr, seq ? nullptr : ctx->d_n_active.p,
-                  scan_radius ? 1 : 0, seq ? *seq : SeqView{}, lane_radius));
+                  scan_radius ? 1 : 0, seq ? *seq : SeqView{}, lane_radius, L ? L->b.lane_prm : nullptr,
+                  L ? L->b.lane_seq : nullptr, L && L->fold_k2 ? 1 : 0));
     ctx->launches++;
     return DCREG_OK;
 }
@@ -2697,10 +2777,10 @@ static int launch_k2(dcreg_ctx* ctx, const dcreg_icp_params* prm, dcreg_iter_log
 static int launch_body(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_params* prm, dcreg_iter_log* dlog, int log_cap, bool with_k2) {
     int rc = launch_plan(ctx, L);
     if (rc) return rc;
-    if (with_k2 && !L.fold_k2) {
+    if (with_k2 && L.k2) {
         if ((rc = nccl_allreduce_acc(ctx))) return rc;          // no-op on one GPU / with peer mailboxes
         if ((rc = launch_k2(ctx, prm, dlog, log_cap, L.b.coherent_step, L.trials, L.scan_radius, L.lanes ? &L.b.seq : nullptr,
-                            L.b.lane_radius)))
+                            L.b.lane_radius, &L)))
             return rc;
     }
     return DCREG_OK;
@@ -2989,13 +3069,15 @@ static void key_bytes(std::vector<unsigned char>& k, const void* p, size_t n) {
 // launches per iteration - what keeps independent ranks from queueing behind the host.  Falls back to plain launches if capture is unavailable.
 static int enqueue_iterations(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_params* prm, dcreg_iter_log* dlog, int log_cap, int iters) {
     const bool graphable = !ctx->graph_off && !L.b.force && iters > 1 &&
-                           (L.fold_k2 || !(ctx->comm && !ctx->peer_ok));          // no NCCL call inside a capture
+                           (!L.k2 || !(ctx->comm && !ctx->peer_ok));              // no NCCL call inside a capture
     if (graphable) {
         std::vector<unsigned char> key;
         Iter2Args kb = L.b;
         kb.use_seeds = 0;
         key_bytes(key, &kb, sizeof(kb));
-        const int meta[5] = {L.grid_x, L.trials, L.use_wd ? 1 : 0, iters, L.sparse ? 1 : 0};   // (kSparse: another kernel)
+        // (kSparse: another kernel; k2: whether a K2 launch follows every iteration kernel, which a mix of per-lane
+        // settings decides at the same Iter2Args)
+        const int meta[6] = {L.grid_x, L.trials, L.use_wd ? 1 : 0, iters, L.sparse ? 1 : 0, L.k2 ? 1 : 0};
         key_bytes(key, meta, sizeof(meta));
         key_bytes(key, prm, sizeof(*prm));
         cudaGraphExec_t exec = nullptr;
@@ -3029,7 +3111,7 @@ static int enqueue_iterations(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_param
         if (exec) {
             CK(cudaGraphLaunch(exec, ctx->stream));
             ctx->nn_valid = true;
-            ctx->launches += (long long)iters * (L.fold_k2 ? 1 : 2); ctx->graph_launches++;
+            ctx->launches += (long long)iters * (L.k2 ? 2 : 1); ctx->graph_launches++;
             return DCREG_OK;
         }
     }
@@ -3106,11 +3188,21 @@ static int start_loop(dcreg_ctx* ctx, int trials, const double* T_init, const Re
 
 // The end of a call, after its loop: the log's fill-in, the results, then the covariances and the priors when asked for.
 // dev (odometry): the caller's trial k is device trial dev[k], and only the device trials below `done` are returned;
-// null: the same order, every trial.
+// null: the same order, every trial.  lanes (per-lane settings, in the context's lane table): device trial t's record
+// takes lane trial_lane[t]'s, or lane t's without trial_lane.
 static int finish_call(dcreg_ctx* ctx, const dcreg_icp_params* prm, int trials, dcreg_iter_log* dlog, const Results& r,
-                       const int* dev = nullptr, int done = 0) {
+                       const int* dev = nullptr, int done = 0, const Lanes& lanes = Lanes{},
+                       const int* trial_lane = nullptr) {
     if (dlog) {
-        log_fill_kernel<<<dim3((r.log_cap + 31) / 32, trials), 32, 0, ctx->stream>>>(dlog, r.log_cap, ctx->d_state, *prm);
+        const int* d_trial_lane = nullptr;
+        if (lanes.n && trial_lane) {
+            CK(ctx->d_trial_lane.ensure(trials));
+            CK(cudaMemcpyAsync(ctx->d_trial_lane, trial_lane, (size_t)trials * sizeof(int), cudaMemcpyHostToDevice,
+                               ctx->stream));
+            d_trial_lane = ctx->d_trial_lane;
+        }
+        log_fill_kernel<<<dim3((r.log_cap + 31) / 32, trials), 32, 0, ctx->stream>>>(
+            dlog, r.log_cap, ctx->d_state, *prm, lanes.n ? ctx->d_lane_prm.p : nullptr, d_trial_lane);
         ctx->launches++;
     }
     // device order: straight into the caller's arrays, or into host copies that are put in the caller's order below
@@ -3154,9 +3246,11 @@ static int finish_call(dcreg_ctx* ctx, const dcreg_icp_params* prm, int trials, 
 
 // The loop for `trials` registrations side by side: of the context's source (batch null), or of the staged sources of a
 // batch (stage_sources), whose lanes, if any, run the trials as frames.  fetch = false: enqueue only (no host
-// synchronisation at all: no peek between chunks, no read-back)
+// synchronisation at all: no peek between chunks, no read-back).  lane_set: per-lane settings (params is entry 0), one per
+// trial, or (batch lanes) one per lane with trial_lane the lane of every trial
 static int run_loop(dcreg_ctx* ctx, const dcreg_icp_params* params, int trials, const double* T_init, const Results& r,
-                    bool fetch = true, const Batch* batch = nullptr) {
+                    bool fetch = true, const Batch* batch = nullptr, const Lanes& lane_set = Lanes{},
+                    const int* trial_lane = nullptr) {
     dcreg_iter_log* dlog = nullptr;
     const float4* src = nullptr;
     int rc = start_loop(ctx, trials, T_init, r, batch, &dlog, &src);
@@ -3164,7 +3258,7 @@ static int run_loop(dcreg_ctx* ctx, const dcreg_icp_params* params, int trials, 
     const bool lanes = batch && batch->lanes > 0;
     LoopPlan L;
     if ((rc = plan_iteration(ctx, params, src, nullptr, lanes ? batch->lanes : trials, dlog, dlog ? r.log_cap : 0, true, &L,
-                             batch)))
+                             batch, lane_set)))
         return rc;
     // fixed iteration count: the whole run is one chunk; otherwise chunks of 16 with a peek in between.  Lanes: chunks
     // of 16 with a peek at the lanes still running, up to max_bodies (a frame never needs more than max_iterations
@@ -3174,7 +3268,7 @@ static int run_loop(dcreg_ctx* ctx, const dcreg_icp_params* params, int trials, 
     const bool peek = fetch && (lanes || !params->fixed_iterations);
     if ((rc = run_chunks(ctx, L, params, dlog, dlog ? r.log_cap : 0, cap, chunk, peek))) return rc;
     if (!fetch) return DCREG_OK;
-    return finish_call(ctx, params, trials, dlog, r);
+    return finish_call(ctx, params, trials, dlog, r, nullptr, 0, lane_set, trial_lane);
 }
 
 // need_source = false: the run brings its own source points (dcreg_icp_run_scans); need_target = false: and its own
@@ -3240,6 +3334,7 @@ struct BatchCheck {
     int n_seqs = 0;                     // the sequence table [n_seqs + 1]: from 0, ascending strictly, up to n
     const int* seq_offsets = nullptr;
     bool empty_seqs = false;            // ... or only non-decreasing (dcreg_odometry_push: a sequence may have no frame)
+    int lanes = 0;                      // dcreg_set_lane_params: params holds this many entries (0: one)
 };
 
 static int check_batch_call(dcreg_ctx* ctx, const dcreg_icp_params* params, const BatchCheck& c) {
@@ -3278,6 +3373,9 @@ static int check_batch_call(dcreg_ctx* ctx, const dcreg_icp_params* params, cons
         if (so[c.n_seqs] != c.n)
             return bad(name + ": seq_offsets[n_seqs] = " + std::to_string(so[c.n_seqs]) + " but n_frames = " + std::to_string(c.n));
     }
+    // the fields every lane shares equal entry 0's, whose checks above are then every entry's
+    const std::string why = lane_plan::check_common(params, c.lanes, c.name);
+    if (!why.empty()) return bad(why);
     return DCREG_OK;
 }
 
@@ -3287,10 +3385,12 @@ int dcreg_icp_run_batch(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_tr
     BatchCheck c{"icp_run_batch", params && T_init && T_out && n_trials > 0, "null pointer or n_trials <= 0",
                  "trials are independent - distribute them over ranks, do not shard them", n_trials};
     c.need_source = true;
+    c.lanes = ctx->lane_params ? n_trials : 0;
     int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
-    return run_loop(ctx, params, n_trials, T_init, Results{T_out, n_iterations, converged, status, log, log_cap});
+    return run_loop(ctx, params, n_trials, T_init, Results{T_out, n_iterations, converged, status, log, log_cap}, true,
+                    nullptr, call_lanes(params, n_trials, ctx->lane_params));
 }
 
 int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_scans, const float* xyz,
@@ -3301,13 +3401,14 @@ int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_sc
                  "null pointer or n_scans <= 0", "scans are independent - distribute them over ranks, do not shard them",
                  n_scans};
     c.offsets = scan_offsets; c.item = "scan"; c.stride = stride; c.dense = "batches";
+    c.lanes = ctx->lane_params ? n_scans : 0;
     int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
     const Batch S{n_scans, xyz, stride, scan_offsets};
     if ((rc = stage_sources(ctx, S))) return rc;
     return run_loop(ctx, params, n_scans, T_init, Results{T_out, n_iterations, converged, status, log, log_cap, cov}, true,
-                    &S);
+                    &S, call_lanes(params, n_scans, ctx->lane_params));
 }
 
 int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
@@ -3321,6 +3422,7 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
                  "sequences are independent - give each rank its own, do not shard them", n_frames};
     c.offsets = frame_offsets; c.item = "frame"; c.stride = stride; c.one_iteration = true; c.dense = "sequences";
     c.n_seqs = n_seqs; c.seq_offsets = seq_offsets;
+    c.lanes = ctx->lane_params ? n_seqs : 0;
     int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
     CK(cudaSetDevice(ctx->device));
@@ -3347,21 +3449,29 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
         CK(cudaMemcpyAsync(ctx->d_seq_delta, deltas, (size_t)n_frames * 16 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
         S.seq.delta = ctx->d_seq_delta;
     }
+    // (per-lane settings) every frame's record takes its sequence's
+    std::vector<int> frame_seq((size_t)n_frames);
+    for (int s = 0; s < n_seqs; ++s)
+        for (int f = seq_offsets[s]; f < seq_offsets[s + 1]; ++f) frame_seq[(size_t)f] = s;
     return run_loop(ctx, params, n_frames, T_dr.data(),
-                    Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, true, &S);
+                    Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, true, &S,
+                    call_lanes(params, n_seqs, ctx->lane_params), frame_seq.data());
 }
 
 // The settings of a one-shot call (dcreg_icp_run_odometry: source_voxel = map_voxel = 0, caps of 1; _voxel: caps of 1)
 // or of a session (dcreg_odometry_open).  A voxel size of 0 leaves its filter out entirely: no launch, no copy, no sync.
 // T_init stays empty when params or T_init is null or n_seqs <= 0, which the checks report as a null pointer; no valid
-// call has more than kMaxPairs sequences, so no more are read before the checks reject it.
+// call has more than kMaxPairs sequences, so no more are read before the checks reject it.  lanes: params holds one
+// entry per sequence (dcreg_set_lane_params), read the same way.
 static OdomSettings odom_settings(const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
                                   int motion, double source_voxel, double map_voxel, int source_max_points,
-                                  int map_max_points, const double* T_init) {
+                                  int map_max_points, const double* T_init, bool lanes) {
     OdomSettings set{params ? *params : dcreg_icp_params{}, n_seqs, map_frames, motion, source_max_points, map_max_points,
                      cell_size, source_voxel, map_voxel};
-    if (params && T_init && n_seqs > 0)
+    if (params && T_init && n_seqs > 0) {
         set.T_init.assign(T_init, T_init + (size_t)std::min(n_seqs, arena_plan::kMaxPairs) * 16);
+        if (lanes) set.lanes.assign(params, params + std::min(n_seqs, arena_plan::kMaxPairs));
+    }
     return set;
 }
 
@@ -3401,6 +3511,8 @@ struct OdomCall {
     double* search_radius;                          // (out, may be null) the radius every frame registered with; anchors 0
     const int n_seqs = set.n_seqs;
     const dcreg_icp_params* params = &set.params;
+    // (dcreg_set_lane_params) every sequence's settings, indexed through the step's lane -> sequence table d_lane_seq
+    const Lanes lanes = call_lanes(set.lanes.data(), (int)set.lanes.size(), true);
     odom_plan::History none;                        // a one-shot call's history, once check() has validated n_seqs
     const odom_plan::History& hist = sess ? sess->hist : none;
     // the frames as the device gets them: the caller's, or the source filter's kept points (src_off: kept offsets)
@@ -3541,7 +3653,8 @@ int OdomCall::check() {
     c.need_target = false; c.one_iteration = true; c.n_seqs = n_seqs; c.seq_offsets = seq_offsets;
     c.empty_seqs = sess != nullptr;
     c.own_msg = odometry_settings_error(set, deltas != nullptr);
-    int rc = check_batch_call(ctx, params, c);
+    c.lanes = (int)set.lanes.size();
+    int rc = check_batch_call(ctx, set.lanes.empty() ? params : set.lanes.data(), c);
     if (rc) return rc;
     if (!sess) none = odom_plan::History(n_seqs);
     CK(cudaSetDevice(ctx->device));
@@ -3827,10 +3940,15 @@ int OdomCall::step(int i) {
     if (!have_plan) {
         S.grids = ctx->odom_maps.d_grids;
         S.sparse = sparse;
-        if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? R.log_cap : 0, true, &LP, &S))) return rc;
+        if (lanes.n) CK(ctx->d_lane_seq.ensure(n_seqs));
+        if ((rc = plan_iteration(ctx, params, src_iter, nullptr, n_seqs, dlog, dlog ? R.log_cap : 0, true, &LP, &S, lanes)))
+            return rc;
         LP.b.lane_radius = set.adaptive ? ctx->d_lane_radius.p : nullptr;
+        LP.b.lane_seq = lanes.n ? ctx->d_lane_seq.p : nullptr;
         have_plan = true;
     }
+    if (lanes.n)            // the sequence each lane of this step runs (the lanes' settings are the sequences')
+        CK(cudaMemcpyAsync(ctx->d_lane_seq, st.seq.data(), st.seq.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = run_chunks(ctx, LP, params, dlog, dlog ? R.log_cap : 0, params->max_iterations, 16, true))) return rc;
     // 5. (adaptive) the step's frames into their sequences' threshold states, and the next step's radii
     if (set.adaptive) {
@@ -3879,8 +3997,14 @@ int OdomCall::finish() {
         CK(cudaMemcpyAsync(thr.data(), ctx->d_thr_state, thr.size() * sizeof(adaptive::State), cudaMemcpyDeviceToHost,
                            ctx->stream));
     }
+    std::vector<int> dev_seq;                       // (lanes) every device trial's sequence, for its log records
+    if (lanes.n) {
+        dev_seq.resize((size_t)n_frames);
+        for (int s = 0; s < n_seqs; ++s)
+            for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k) dev_seq[(size_t)P.dev[(size_t)k]] = s;
+    }
     if ((rc = finish_call(ctx, params, n_frames, dlog, R, P.dev.data(),
-                          failed >= 0 ? P.steps[(size_t)failed].first : n_frames)))
+                          failed >= 0 ? P.steps[(size_t)failed].first : n_frames, lanes, dev_seq.data())))
         return rc;
     if (search_radius) memcpy(search_radius, frame_radius.data(), frame_radius.size() * sizeof(double));
     if (failed >= 0 || update_failed) { ctx->err = err; return DCREG_BAD_ARG; }
@@ -3933,7 +4057,9 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
                            double* T_out, int* n_iterations, int* converged, int* status, double* cov,
                            dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry",
-                        odom_settings(params, n_seqs, cell_size, map_frames, motion, 0.0, 0.0, 1, 1, T_init), nullptr,
+                        odom_settings(params, n_seqs, cell_size, map_frames, motion, 0.0, 0.0, 1, 1, T_init,
+                                      ctx && ctx->lane_params),
+                        nullptr,
                         seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, nullptr,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, nullptr, nullptr);
 }
@@ -3945,7 +4071,8 @@ int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params,
                                  double* T_out, int* n_iterations, int* converged, int* status, double* cov,
                                  dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_voxel",
-                        odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel, 1, 1, T_init),
+                        odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel, 1, 1, T_init,
+                                      ctx && ctx->lane_params),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, nullptr,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points, nullptr);
 }
@@ -3959,7 +4086,7 @@ int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* param
                                    int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_voxel_n",
                         odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
-                                      source_max_points, map_max_points, T_init),
+                                      source_max_points, map_max_points, T_init, ctx && ctx->lane_params),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, nullptr,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points, nullptr);
 }
@@ -3973,7 +4100,7 @@ int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params
                                   dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_deskew",
                         odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
-                                      source_max_points, map_max_points, T_init),
+                                      source_max_points, map_max_points, T_init, ctx && ctx->lane_params),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
                         deskewed_xyz);
@@ -3982,9 +4109,9 @@ int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params
 // the settings of the voxel map (dcreg_icp_run_odometry_map, dcreg_odometry_open_map): no window
 static OdomSettings odom_map_settings(const dcreg_icp_params* params, int n_seqs, double cell_size, int motion,
                                       double source_voxel, double map_voxel, int source_max_points, int map_max_points,
-                                      double max_distance, const double* T_init) {
+                                      double max_distance, const double* T_init, bool lanes) {
     OdomSettings set = odom_settings(params, n_seqs, cell_size, 0, motion, source_voxel, map_voxel, source_max_points,
-                                     map_max_points, T_init);
+                                     map_max_points, T_init, lanes);
     set.voxel_map = true;
     set.max_distance = max_distance;
     return set;
@@ -3999,7 +4126,7 @@ int dcreg_icp_run_odometry_map(dcreg_ctx* ctx, const dcreg_icp_params* params, i
                                dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_map",
                         odom_map_settings(params, n_seqs, cell_size, motion, source_voxel, map_voxel, source_max_points,
-                                          map_max_points, max_distance, T_init),
+                                          map_max_points, max_distance, T_init, ctx && ctx->lane_params),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
                         deskewed_xyz);
@@ -4010,11 +4137,11 @@ int dcreg_icp_run_odometry_map(dcreg_ctx* ctx, const dcreg_icp_params* params, i
 static OdomSettings odom_adaptive_settings(const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
                                            int motion, double source_voxel, double map_voxel, int source_max_points,
                                            int map_max_points, double max_distance,
-                                           const dcreg_adaptive_threshold* adaptive, const double* T_init) {
+                                           const dcreg_adaptive_threshold* adaptive, const double* T_init, bool lanes) {
     OdomSettings set = map_frames == 0 ? odom_map_settings(params, n_seqs, cell_size, motion, source_voxel, map_voxel,
-                                                           source_max_points, map_max_points, max_distance, T_init)
+                                                           source_max_points, map_max_points, max_distance, T_init, lanes)
                                        : odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel,
-                                                       map_voxel, source_max_points, map_max_points, T_init);
+                                                       map_voxel, source_max_points, map_max_points, T_init, lanes);
     if (adaptive) {
         set.adaptive = true;
         set.threshold = adaptive::Settings{adaptive->initial_threshold, adaptive->min_motion, adaptive->max_range};
@@ -4032,7 +4159,8 @@ int dcreg_icp_run_odometry_adaptive(dcreg_ctx* ctx, const dcreg_icp_params* para
                                     double* search_radius, dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_adaptive",
                         odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
-                                               source_max_points, map_max_points, max_distance, adaptive, T_init),
+                                               source_max_points, map_max_points, max_distance, adaptive, T_init,
+                                               ctx && ctx->lane_params),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
                         deskewed_xyz, search_radius);
@@ -4052,7 +4180,8 @@ static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& se
                  "sequences are independent - give each rank its own, do not shard them", n_seqs};
     c.own_cell = true; c.cell_size = set.cell_size; c.need_target = false; c.one_iteration = true;
     c.own_msg = odometry_settings_error(ss->set, false);
-    const int rc = check_batch_call(ctx, &ss->set.params, c);
+    c.lanes = (int)ss->set.lanes.size();
+    const int rc = check_batch_call(ctx, ss->set.lanes.empty() ? &ss->set.params : ss->set.lanes.data(), c);
     if (rc) return rc;
     ss->hist = odom_plan::History(n_seqs);
     ss->map_off.assign((size_t)n_seqs + 1, 0);
@@ -4070,7 +4199,7 @@ int dcreg_odometry_open(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_se
     if (!ctx) return DCREG_BAD_ARG;
     return open_session(ctx, "odometry_open",
                         odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
-                                      source_max_points, map_max_points, T_init));
+                                      source_max_points, map_max_points, T_init, ctx && ctx->lane_params));
 }
 
 int dcreg_odometry_open_map(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int motion,
@@ -4079,7 +4208,7 @@ int dcreg_odometry_open_map(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
     if (!ctx) return DCREG_BAD_ARG;
     return open_session(ctx, "odometry_open_map",
                         odom_map_settings(params, n_seqs, cell_size, motion, source_voxel, map_voxel, source_max_points,
-                                          map_max_points, max_distance, T_init));
+                                          map_max_points, max_distance, T_init, ctx && ctx->lane_params));
 }
 
 int dcreg_odometry_open_adaptive(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size,
@@ -4089,7 +4218,8 @@ int dcreg_odometry_open_adaptive(dcreg_ctx* ctx, const dcreg_icp_params* params,
     if (!ctx) return DCREG_BAD_ARG;
     return open_session(ctx, "odometry_open_adaptive",
                         odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
-                                               source_max_points, map_max_points, max_distance, adaptive, T_init));
+                                               source_max_points, map_max_points, max_distance, adaptive, T_init,
+                                               ctx && ctx->lane_params));
 }
 
 int dcreg_odometry_local_map(dcreg_ctx* ctx, int seq, float* xyz, int64_t cap, int64_t* n) {
@@ -4213,6 +4343,7 @@ int dcreg_icp_run_pairs(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_pa
                  "null pointer or n_pairs <= 0", "pairs are independent - give each rank its own, do not shard them", n_pairs};
     c.offsets = src_offsets; c.item = "source"; c.stride = stride; c.own_cell = true; c.cell_size = cell_size;
     c.need_target = false;
+    c.lanes = ctx->lane_params ? n_pairs : 0;
     int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
     const std::string why = arena_plan::check_offsets(n_pairs, tgt_offsets, arena_plan::kMaxPoints, "icp_run_pairs: target");
@@ -4236,7 +4367,7 @@ int dcreg_icp_run_pairs(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_pa
     S.sparse = sparse_at >= 0;
     if ((rc = stage_sources(ctx, S)) ||
         (rc = run_loop(ctx, params, n_pairs, T_init, Results{T_out, n_iterations, converged, status, log, log_cap, cov}, true,
-                       &S)))
+                       &S, call_lanes(params, n_pairs, ctx->lane_params))))
         return rc;
     if (!metrics) return DCREG_OK;
     if (S.sparse) {                 // nn1_search expands rings over the whole box

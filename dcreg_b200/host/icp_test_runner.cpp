@@ -17,7 +17,9 @@
 //
 // Extension (not in the reference, which has no RNG - SURVEY.md §6 C5): an optional `monte_carlo:` block runs a seeded
 // perturbation study of every listed method through dcreg_icp_run_batch (all trials advance side by side on the GPU) and
-// writes monte_carlo_<method>.csv + monte_carlo_summary.txt.  Absent block = the reference's behaviour, unchanged.
+// writes monte_carlo_<method>.csv + monte_carlo_summary.txt.  Absent block = the reference's behaviour, unchanged.  With
+// `one_call: true` every method x trials runs as the lanes of ONE dcreg_icp_run_batch call (dcreg_set_lane_params: a
+// block of `trials` lanes per method, each with that method's settings and the same drawn poses), same files.
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -84,7 +86,14 @@ struct Config {                    // DCReg/include/utils.hpp:132-171
     int mc_trials = 0;
     unsigned long long mc_seed = 45;
     double mc_max_trans = 1.0, mc_max_rot_deg = 3.0;
+    bool mc_one_call = false;               // monte_carlo.one_call: all methods x trials in one batched call
 };
+
+// The methods the SO(3) path recognises by name (icp_test_runner.cpp's dispatch); the others are reported and skipped
+static bool is_so3_method(const std::string& name) {
+    static const char* so3_names[] = {"Ours", "NONE", "ME-SR", "FCN-SR", "ME-TSVD", "ME-TReg"};
+    return std::find_if(std::begin(so3_names), std::end(so3_names), [&](const char* s) { return name == s; }) != std::end(so3_names);
+}
 
 bool loadConfig(const std::string& filename, Config& c) {      // icp_test_runner.cpp:20-153
     try {
@@ -142,6 +151,7 @@ bool loadConfig(const std::string& filename, Config& c) {      // icp_test_runne
             if (mc["max_trans_m"]) c.mc_max_trans = mc["max_trans_m"].as<double>();
             if (mc["max_rot_deg"]) c.mc_max_rot_deg = mc["max_rot_deg"].as<double>();
             if (c.mc_trials < 0 || c.mc_trials > 65535) throw yaml_lite::ParseError("monte_carlo.trials must be in [0, 65535]");
+            if (mc["one_call"]) c.mc_one_call = mc["one_call"].as<bool>();
         }
         // icp_params.XICP_*: parsed by the reference for the (out-of-scope) XICP baseline; accepted and ignored here
         if (y["test_methods"])
@@ -150,6 +160,13 @@ bool loadConfig(const std::string& filename, Config& c) {      // icp_test_runne
                 if (v.size() < 2) throw yaml_lite::ParseError("test_methods." + kv.first + " needs [detection, handling]");
                 c.test_methods[kv.first] = {v[0], v[1]};
             }
+        if (c.mc_one_call) {            // the lanes of the one call: at most 65535 (the loop kernel's grid y)
+            long long lanes = 0;
+            for (const auto& kv : c.test_methods) lanes += is_so3_method(kv.first) ? c.mc_trials : 0;
+            if (lanes > 65535)
+                throw yaml_lite::ParseError("monte_carlo.one_call: methods x trials = " + std::to_string(lanes) +
+                                            " lanes, more than 65535 in one call");
+        }
         std::cout << "\n=== Loaded Configuration ===" << std::endl;
         std::cout << "STD_REG_GAMMA: " << c.icp_params.STD_REG_GAMMA << std::endl;
         std::cout << "ADAPTIVE_REG_ALPHA: " << c.icp_params.ADAPTIVE_REG_ALPHA << std::endl;
@@ -291,10 +308,7 @@ private:
         }
     }
 
-    static bool isSo3Method(const std::string& name) {
-        static const char* so3_names[] = {"Ours", "NONE", "ME-SR", "FCN-SR", "ME-TSVD", "ME-TReg"};
-        return std::find_if(std::begin(so3_names), std::end(so3_names), [&](const char* s) { return name == s; }) != std::end(so3_names);
-    }
+    static bool isSo3Method(const std::string& name) { return is_so3_method(name); }
 
     dcreg_icp_params engineParams(int det, int hand) const {
         dcreg_icp_params p;
@@ -308,13 +322,14 @@ private:
         return p;
     }
 
-    // The perturbation study (extension, see the file header): one dcreg_icp_run_batch call per method.
+    // The perturbation study (extension, see the file header): one dcreg_icp_run_batch call per method, or (one_call) one
+    // call whose lanes hold every method's block of trials.
     bool runMonteCarlo() {
         const int n = config_.mc_trials;
         std::mt19937_64 gen(config_.mc_seed);
         auto uni = [&](double a) { return ((double)(gen() >> 11) * (1.0 / 9007199254740992.0) * 2.0 - 1.0) * a; };   // [-a, a)
         std::vector<Pose6D> init((size_t)n);
-        std::vector<double> T0((size_t)n * 16), T1((size_t)n * 16);
+        std::vector<double> T0((size_t)n * 16);
         for (int i = 0; i < n; ++i) {
             Pose6D& q = init[i];
             q.x = uni(config_.mc_max_trans); q.y = uni(config_.mc_max_trans); q.z = uni(config_.mc_max_trans);
@@ -328,14 +343,48 @@ private:
         summary << std::setw(15) << "Method" << std::setw(12) << "Converged%" << std::setw(12) << "Failed" << std::setw(14) << "MeanTrans(m)"
                 << std::setw(14) << "MedTrans(m)" << std::setw(14) << "MeanRot(deg)" << std::setw(14) << "MedRot(deg)" << std::setw(12) << "Avg_Iters"
                 << std::setw(12) << "Time(ms)" << std::setw(12) << "Trials/s\n";
-        for (const auto& kv : config_.test_methods) {
-            if (!isSo3Method(kv.first)) continue;
-            const dcreg_icp_params p = engineParams(detection_from_string(kv.second.first), handling_from_string(kv.second.second));
-            std::vector<int> iters((size_t)n), conv((size_t)n), status((size_t)n);
-            const auto t0 = std::chrono::high_resolution_clock::now();
-            if (!check(dcreg_icp_run_batch(ctx_, &p, n, T0.data(), T1.data(), iters.data(), conv.data(), status.data(), nullptr, 0), "icp_run_batch")) return false;
-            const double ms = std::chrono::duration<double, std::milli>(std::chrono::high_resolution_clock::now() - t0).count();
-            std::ofstream f(config_.output_folder + "monte_carlo_" + kv.first + ".csv");
+        std::vector<std::string> names;
+        std::vector<dcreg_icp_params> prm;
+        for (const auto& kv : config_.test_methods)
+            if (isSo3Method(kv.first)) {
+                names.push_back(kv.first);
+                prm.push_back(engineParams(detection_from_string(kv.second.first), handling_from_string(kv.second.second)));
+            }
+        const int m = (int)names.size();
+        const bool one = config_.mc_one_call && m > 0;
+        std::vector<int> iters_all((size_t)m * n), conv_all((size_t)m * n), status_all((size_t)m * n);
+        std::vector<double> T1_all((size_t)m * n * 16), ms_all((size_t)m);
+        auto now = [] { return std::chrono::high_resolution_clock::now(); };
+        if (one) {                  // method k: lanes [k n, (k + 1) n), its settings in each, the same drawn poses
+            std::vector<dcreg_icp_params> lanes;
+            std::vector<double> T0_all;
+            for (int k = 0; k < m; ++k) {
+                lanes.insert(lanes.end(), (size_t)n, prm[(size_t)k]);
+                T0_all.insert(T0_all.end(), T0.begin(), T0.end());
+            }
+            if (!check(dcreg_set_lane_params(ctx_, 1), "set_lane_params")) return false;
+            const auto t0 = now();
+            const bool ok = check(dcreg_icp_run_batch(ctx_, lanes.data(), m * n, T0_all.data(), T1_all.data(), iters_all.data(),
+                                                      conv_all.data(), status_all.data(), nullptr, 0), "icp_run_batch");
+            const double ms = std::chrono::duration<double, std::milli>(now() - t0).count();
+            dcreg_set_lane_params(ctx_, 0);
+            if (!ok) return false;
+            std::fill(ms_all.begin(), ms_all.end(), ms);
+        }
+        for (int mi = 0; mi < m; ++mi) {
+            const std::string& name = names[(size_t)mi];
+            int* iters = iters_all.data() + (size_t)mi * n;
+            int* conv = conv_all.data() + (size_t)mi * n;
+            int* status = status_all.data() + (size_t)mi * n;
+            double* T1 = T1_all.data() + (size_t)mi * n * 16;
+            if (!one) {
+                const auto t0 = now();
+                if (!check(dcreg_icp_run_batch(ctx_, &prm[(size_t)mi], n, T0.data(), T1, iters, conv, status, nullptr, 0), "icp_run_batch")) return false;
+                ms_all[(size_t)mi] = std::chrono::duration<double, std::milli>(now() - t0).count();
+            }
+            const double ms = ms_all[(size_t)mi];
+            const int timed_trials = one ? m * n : n;       // (one_call) Time(ms) is the one call's, over every lane
+            std::ofstream f(config_.output_folder + "monte_carlo_" + name + ".csv");
             f << "Trial,Init_x,Init_y,Init_z,Init_roll_deg,Init_pitch_deg,Init_yaw_deg,Converged,Iterations,Status,Trans_Error_m,Rot_Error_deg";
             for (int k = 0; k < 12; ++k) f << ",T" << k / 4 << k % 4;
             f << "\n" << std::setprecision(17);
@@ -355,11 +404,11 @@ private:
             auto mean = [](const std::vector<double>& v) { double s = 0; for (double x : v) s += x; return v.empty() ? 0.0 : s / (double)v.size(); };
             auto median = [](std::vector<double> v) { if (v.empty()) return 0.0; std::sort(v.begin(), v.end()); return v[v.size() / 2]; };
             const double ok = (double)std::max<size_t>(1, te.size());
-            summary << std::setw(15) << kv.first << std::fixed << std::setw(12) << std::setprecision(1) << 100.0 * n_conv / (double)n << std::setw(12) << n_fail
+            summary << std::setw(15) << name << std::fixed << std::setw(12) << std::setprecision(1) << 100.0 * n_conv / (double)n << std::setw(12) << n_fail
                     << std::setw(14) << std::setprecision(6) << mean(te) << std::setw(14) << median(te) << std::setw(14) << mean(re) << std::setw(14) << median(re)
                     << std::setw(12) << std::setprecision(1) << (double)it_sum / ok << std::setw(12) << std::setprecision(2) << ms
-                    << std::setw(12) << std::setprecision(0) << 1000.0 * n / ms << "\n";
-            std::cout << "Monte-Carlo " << kv.first << ": " << n << " trials in " << ms << " ms, " << n_conv << " converged, " << n_fail << " aborted" << std::endl;
+                    << std::setw(12) << std::setprecision(0) << 1000.0 * timed_trials / ms << "\n";
+            std::cout << "Monte-Carlo " << name << ": " << n << " trials in " << ms << " ms, " << n_conv << " converged, " << n_fail << " aborted" << std::endl;
         }
         std::cout << "Monte-Carlo results saved to " << config_.output_folder << "monte_carlo_summary.txt" << std::endl;
         return true;
@@ -758,7 +807,7 @@ int dumpConfig(const std::string& config_file) {
               << "\nSTD_REG_GAMMA=" << c.icp_params.STD_REG_GAMMA << "\nKAPPA_TARGET=" << c.icp_params.KAPPA_TARGET << "\nPCG_TOLERANCE="
               << c.icp_params.PCG_TOLERANCE << "\nPCG_MAX_ITER=" << c.icp_params.PCG_MAX_ITER << "\nTSVD_SINGULAR_THRESH="
               << c.icp_params.TSVD_SINGULAR_THRESH << "\nLOAM_EIGEN_THRESH=" << c.icp_params.LOAM_EIGEN_THRESH << "\nmc_trials=" << c.mc_trials
-              << "\nmc_seed=" << c.mc_seed << "\nmc_max_trans=" << c.mc_max_trans << "\nmc_max_rot_deg=" << c.mc_max_rot_deg << "\n";
+              << "\nmc_seed=" << c.mc_seed << "\nmc_max_trans=" << c.mc_max_trans << "\nmc_max_rot_deg=" << c.mc_max_rot_deg << "\nmc_one_call=" << c.mc_one_call << "\n";
     std::cout << "initial_matrix=";
     for (int i = 0; i < 16; ++i) std::cout << c.initial_matrix.m[i] << (i < 15 ? "," : "\n");
     std::cout << "gt_matrix=";

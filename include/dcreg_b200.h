@@ -179,6 +179,23 @@ int dcreg_set_target_sparse(dcreg_ctx* ctx, const float* xyz, int64_t m, int str
  * at dcreg_odometry_open*: changing it later does not change that session's pushes.  enable other than 0 or 1:
  * DCREG_BAD_ARG. */
 int dcreg_set_sparse_maps(dcreg_ctx* ctx, int enable);
+/* Per-lane solver settings: compare methods or sweep a threshold across the lanes of one batched call.  enable = 0 (the
+ * default): every call takes one dcreg_icp_params.  enable = 1: the params argument of the batched calls points to one
+ * dcreg_icp_params per lane: n_trials for dcreg_icp_run_batch, n_scans for _scans, n_pairs for _pairs, and n_seqs for
+ * _sequences, every dcreg_icp_run_odometry* and dcreg_odometry_open, _open_map and _open_adaptive (every frame of
+ * sequence s uses entry s).  Single-run calls (dcreg_icp_run, _enqueue, _host_planes, dcreg_find_planes,
+ * dcreg_analyze_and_solve, dcreg_time_* and the timeline) read entry 0 only.
+ *   Per lane: detection, handling, conv_thresh_rot, conv_thresh_trans, cond_thresh, eig_thresh, kappa_target, pcg_tol,
+ *   pcg_max_iter, std_reg_gamma, min_effective_points (the fields only the solve step and the log read).
+ *   Common: search_radius, max_iterations, fixed_iterations, use_weight_derivative, plane_thickness, weight_slope,
+ *   weight_gate and min_normal_norm must equal entry 0's byte for byte; otherwise the call is DCREG_BAD_ARG before
+ *   anything runs, and dcreg_last_error names the call, the first differing entry and the field.  reserved0 is ignored.
+ * Lane b of a call returns byte for byte what the same call returns for lane b when every entry is a copy of entry b
+ * (every output but iter_time_ms), and a call whose entries are all alike is the call with one params (same bytes, same
+ * launches).  In one call the lanes running "Ours" (Schur detection + PCG) solve inside the iteration kernel and the
+ * others in a second kernel after it.  An odometry session copies the entries at open and keeps the setting it had
+ * then; changing the setting later does not change its pushes.  enable other than 0 or 1: DCREG_BAD_ARG. */
+int dcreg_set_lane_params(dcreg_ctx* ctx, int enable);
 
 /* ---- seam 1: correspondence stage (icp_test_runner.cpp:1714-1813) -------------------------
  * For every source slot: q = fl32(R p + t), exact 5-NN in the target, 5th d^2 < radius^2,
