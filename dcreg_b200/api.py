@@ -97,11 +97,11 @@ _lib = None
 EXPORTS = [
     "dcreg_abi_version", "dcreg_create", "dcreg_destroy", "dcreg_last_error", "dcreg_default_params",
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_set_target_sparse", "dcreg_set_sparse_maps",
-    "dcreg_set_lane_params",
+    "dcreg_set_lane_params", "dcreg_set_map_spacing",
     "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_icp_run_odometry_adaptive", "dcreg_odometry_open_adaptive", "dcreg_odometry_push_adaptive", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_icp_run_odometry_adaptive", "dcreg_odometry_open_adaptive", "dcreg_odometry_push_adaptive", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_voxel_downsample_spaced", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -129,6 +129,7 @@ def load_library():
     lib.dcreg_set_target_sparse.argtypes = [vp, C.POINTER(C.c_float), i64, ci, C.c_double]
     lib.dcreg_set_sparse_maps.argtypes = [vp, ci]
     lib.dcreg_set_lane_params.argtypes = [vp, ci]
+    lib.dcreg_set_map_spacing.argtypes = [vp, C.c_double]
     lib.dcreg_find_planes.argtypes = [vp, dp, C.c_double, dp, C.POINTER(i64)]
     lib.dcreg_reduce_normal_equations.argtypes = [vp, vp, vp, i64, dp, ci, dp, dp]
     lib.dcreg_reduce_normal_equations_f64plane.argtypes = [vp, vp, vp, i64, dp, ci, dp, dp]
@@ -162,6 +163,8 @@ def load_library():
                                                    C.POINTER(ci), dp, C.POINTER(IterLog), ci]
     lib.dcreg_voxel_downsample_n.argtypes = [vp, ci, C.POINTER(C.c_float), C.POINTER(i64), ci, C.c_double, ci,
                                              C.POINTER(C.c_float), C.POINTER(i64), C.POINTER(i64)]
+    lib.dcreg_voxel_downsample_spaced.argtypes = [vp, ci, C.POINTER(C.c_float), C.POINTER(i64), ci, C.c_double, ci,
+                                                  C.c_double, C.POINTER(C.c_float), C.POINTER(i64), C.POINTER(i64)]
     lib.dcreg_odometry_open.argtypes = [vp, C.POINTER(IcpParams), ci, C.c_double, ci, ci, C.c_double, C.c_double, ci, ci,
                                         dp]
     lib.dcreg_odometry_push.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(C.c_float), C.POINTER(i64), ci, dp,
@@ -555,18 +558,21 @@ def _max_points(v, name="max_points"):
     return n
 
 
-def voxel_downsample(P, voxel, max_points=1):
-    """The voxel filter of dcreg_voxel_downsample_n, bit for bit: the voxel of a point is np.floor(p.astype(float64) *
-    (1.0 / voxel)) per axis, rows with a non-finite coordinate have none and are dropped, and each voxel keeps its
-    max_points points of smallest index (1: its first point, dcreg_voxel_downsample).  P: (N, >=3).  Returns (points
-    (K, 3) float32, the kept rows' coordinates unchanged; index (K,) int64, their rows in P, ascending).  Raises
-    ValueError for a voxel that is not finite and > 0, a max_points that is not an integer >= 1, or a voxel coordinate
-    outside [-2^20, 2^20)."""
+def voxel_downsample(P, voxel, max_points=1, min_spacing=0.0):
+    """The voxel filter of dcreg_voxel_downsample_n (min_spacing = 0) and dcreg_voxel_downsample_spaced, bit for bit:
+    the voxel of a point is np.floor(p.astype(float64) * (1.0 / voxel)) per axis, rows with a non-finite coordinate have
+    none and are dropped, and each voxel keeps its max_points points of smallest index (1: its first point,
+    dcreg_voxel_downsample).  min_spacing > 0: going through a voxel's rows in ascending index, a row is kept iff fewer
+    than max_points rows of its voxel are kept before it and each kept row q before it has ((px - qx)^2 + (py - qy)^2) +
+    (pz - qz)^2 >= min_spacing * min_spacing in FP64 (KISS-ICP's AddPoints).  P: (N, >=3).  Returns (points (K, 3)
+    float32, the kept rows' coordinates unchanged; index (K,) int64, their rows in P, ascending).  Raises ValueError for
+    a voxel that is not finite and > 0, a max_points that is not an integer >= 1, a min_spacing that is not finite and
+    >= 0, or a voxel coordinate outside [-2^20, 2^20)."""
     P = np.asarray(P, dtype=np.float32)
     if P.ndim != 2 or P.shape[1] < 3:
         raise ValueError("points must be (N, >=3)")
     max_points = _max_points(max_points)
-    voxel = float(voxel)
+    voxel, min_spacing = float(voxel), _min_spacing(min_spacing)
     if not (voxel > 0.0 and np.isfinite(voxel)):
         raise ValueError(f"voxel_downsample: voxel must be finite and > 0, not {voxel}")
     xyz = P[:, :3]
@@ -586,8 +592,50 @@ def voxel_downsample(P, voxel, max_points=1):
     starts = np.ones(len(s), dtype=bool)
     starts[1:] = s[1:] != s[:-1]
     rank = at - np.maximum.accumulate(np.where(starts, at, 0))
-    keep = rows[np.sort(order[rank < max_points])].astype(np.int64)
+    if min_spacing > 0.0 and max_points > 1:
+        sel = order[_spaced_ranks(xyz[rows[order]], np.nonzero(starts)[0], max_points, min_spacing)]
+    else:
+        sel = order[rank < max_points]
+    keep = rows[np.sort(sel)].astype(np.int64)
     return np.ascontiguousarray(xyz[keep]), keep
+
+
+def _min_spacing(s):
+    s = float(s)
+    if not (s >= 0.0 and np.isfinite(s)):
+        raise ValueError(f"min_spacing must be finite and >= 0 (0: no spacing), not {s}")
+    return s
+
+
+def _spaced_ranks(X, starts, max_points, min_spacing):
+    """The spacing rule over voxels sorted into runs: X (N, 3) float32 rows, each voxel one run beginning at `starts`
+    with its rows in ascending index.  Round r settles the rank-r row of every run still open, against that run's kept
+    rows.  Returns the sorted positions kept, ascending."""
+    n = len(X)
+    length = np.append(starts[1:], n) - starts
+    room = np.minimum(length, max_points)
+    base = np.cumsum(room) - room                           # run g's kept rows: kept[base[g] : base[g] + count[g]]
+    kept = np.empty((int(room.sum()), 3))                   # in FP64 (exact)
+    count = np.zeros(len(starts), dtype=np.int64)
+    flag = np.zeros(n, dtype=bool)
+    s2 = min_spacing * min_spacing
+    open_ = np.arange(len(starts))
+    r = 0
+    while len(open_):
+        at = starts[open_] + r
+        c = X[at].astype(np.float64)
+        held = count[open_]
+        ok = np.ones(len(open_), dtype=bool)
+        row = np.repeat(np.arange(len(open_)), held)        # every (candidate, kept row of its run) pair at once
+        d = c[row] - kept[np.repeat(base[open_], held) + np.arange(len(row)) - np.repeat(np.cumsum(held) - held, held)]
+        ok[row[~((d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2] >= s2)]] = False
+        g = open_[ok]
+        flag[at[ok]] = True
+        kept[base[g] + count[g]] = c[ok]
+        count[g] += 1
+        r += 1
+        open_ = open_[(length[open_] > r) & (count[open_] < max_points)]
+    return np.nonzero(flag)[0]
 
 
 def _voxel_ids(xyz, voxel, name):
@@ -633,14 +681,15 @@ def voxel_map_prune(X, voxel, max_distance, t):
     return np.ascontiguousarray(xyz[keep]), keep
 
 
-def voxel_map_update(M, P, T, voxel, max_points, max_distance):
+def voxel_map_update(M, P, T, voxel, max_points, max_distance, min_spacing=0.0):
     """One update of the voxel map of dcreg_icp_run_odometry_map, bit for bit: prune(cap(M ++ map_points(T, P)), t_T)
-    with cap = voxel_downsample(., voxel, max_points) (M first: older points win, KISS-ICP's AddPoints) and prune =
-    voxel_map_prune at T's translation.  M: the map (K, 3) float32 (may be empty); P: the frame's points (N, >=3) in its
-    sensor frame; T: its pose (4, 4).  Returns the new map (K', 3) float32."""
+    with cap = voxel_downsample(., voxel, max_points, min_spacing) (M first: older points win, KISS-ICP's AddPoints;
+    min_spacing: dcreg_set_map_spacing) and prune = voxel_map_prune at T's translation.  M: the map (K, 3) float32 (may
+    be empty); P: the frame's points (N, >=3) in its sensor frame; T: its pose (4, 4).  Returns the new map (K', 3)
+    float32."""
     M = np.asarray(M, dtype=np.float32).reshape(-1, 3)
     X = np.concatenate([M, map_points(T, P)])
-    capped, _ = voxel_downsample(X, voxel, max_points)
+    capped, _ = voxel_downsample(X, voxel, max_points, min_spacing)
     return voxel_map_prune(capped, voxel, max_distance, np.asarray(T, dtype=np.float64)[:3, 3])[0]
 
 
@@ -740,6 +789,13 @@ class Context:
         """Sparse row indexes, instead of a refusal, for odometry's local maps and icp_run_pairs' targets too large for
         dense grids (include/dcreg_b200.h, dcreg_set_sparse_maps).  A session keeps the value it had when it opened."""
         self._check(self.lib.dcreg_set_sparse_maps(self._h, 1 if enable else 0))
+
+    def set_map_spacing(self, min_spacing: float):
+        """Minimum point spacing of odometry's map filter (include/dcreg_b200.h, dcreg_set_map_spacing): every local
+        map's voxels keep points at least min_spacing apart, as api.voxel_downsample(..., min_spacing) keeps them (0, the
+        default: the cap rule; KISS-ICP uses map_voxel / sqrt(map_max_points)).  A session keeps the value it had when it
+        opened."""
+        self._check(self.lib.dcreg_set_map_spacing(self._h, float(min_spacing)))
 
     def set_lane_params(self, enable: bool):
         """Per-lane solver settings (include/dcreg_b200.h, dcreg_set_lane_params): the batched calls' params point to one
@@ -962,10 +1018,10 @@ class Context:
             return self._run_batched("icp_run_sequences", call, p0, n, S, "sequences", T_init, want_log, want_cov,
                                      deltas, want_prior=True)
 
-    def voxel_downsample(self, clouds, voxel: float, max_points: int = 1):
+    def voxel_downsample(self, clouds, voxel: float, max_points: int = 1, min_spacing: float = 0.0):
         """dcreg_voxel_downsample_n of every cloud (a list of (N_b, >=3) arrays) in one call on the device, each voxel
-        keeping up to max_points points: a list of (points (K_b, 3) float32, index (K_b,) int64), as
-        api.voxel_downsample gives for each cloud alone."""
+        keeping up to max_points points (min_spacing > 0: dcreg_voxel_downsample_spaced, at least min_spacing apart): a
+        list of (points (K_b, 3) float32, index (K_b,) int64), as api.voxel_downsample gives for each cloud alone."""
         max_points = _max_points(max_points)
         xyz, off = _pack(clouds)
         n = len(clouds)
@@ -973,8 +1029,13 @@ class Context:
         pts = np.empty((max(total, 1), 3), dtype=np.float32)
         idx = np.empty(max(total, 1), dtype=np.int64)
         kept = np.zeros(n + 1, dtype=np.int64)
-        self._check(self.lib.dcreg_voxel_downsample_n(self._h, n, _fptr(xyz), _iptr(off), 3, float(voxel), max_points,
-                                                      _fptr(pts), _iptr(kept), _iptr(idx)))
+        if min_spacing == 0.0:
+            rc = self.lib.dcreg_voxel_downsample_n(self._h, n, _fptr(xyz), _iptr(off), 3, float(voxel), max_points,
+                                                   _fptr(pts), _iptr(kept), _iptr(idx))
+        else:
+            rc = self.lib.dcreg_voxel_downsample_spaced(self._h, n, _fptr(xyz), _iptr(off), 3, float(voxel), max_points,
+                                                        float(min_spacing), _fptr(pts), _iptr(kept), _iptr(idx))
+        self._check(rc)
         return [(pts[a:b].copy(), idx[a:b].copy()) for a, b in zip(kept[:-1], kept[1:])]
 
     def icp_run_odometry(self, params, sequences, T_init, deltas=None, motion: str = "increments",

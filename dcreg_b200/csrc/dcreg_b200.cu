@@ -1068,6 +1068,67 @@ __global__ void voxel_cap_flag_kernel(const unsigned int* __restrict__ key, cons
     keep[val[p]] = k != dropped && (p < max_points || key[p - max_points] != k);
 }
 
+// The capped filter with a minimum point spacing (dcreg_voxel_downsample_spaced, dcreg_set_map_spacing; KISS-ICP's
+// AddPoints): over the same sorted key / val, a voxel's point is kept iff fewer than max_points of its voxel are kept
+// before it and every kept point q before it has ((px - qx)^2 + (py - qy)^2) + (pz - qz)^2 >= s2, in FP64 from the
+// float32 coordinates with one rounding per operation (the prune's arithmetic).  Warp w owns every run that starts in
+// sorted positions [32 w, 32 w + 32) and walks it in batches of 32: each lane tests its candidate against the run's
+// kept points so far, then the batch settles one kept point per round (ballot, ffs, shuffle of its coordinates to the
+// lanes after it), at most max_points rounds per run.  Each run is settled in index order by one warp, so the flags
+// are a function of the points alone.  kept_at: scratch of n ints (the sort's consumed input values), run [a, b)
+// listing its kept points' input indices at [a, a + kept); keep[n] = 0.  O(run length x max_points) per run.
+__global__ void voxel_space_flag_kernel(const float* __restrict__ in, int stride, const unsigned int* __restrict__ key,
+                                        const int* __restrict__ val, long long n, unsigned int dropped, int max_points,
+                                        double s2, int* __restrict__ kept_at, int* __restrict__ keep) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t == 0) keep[n] = 0;
+    const int lane = threadIdx.x & 31;
+    const long long w0 = t - lane;
+    if (w0 >= n) return;                                         // whole warps: n is the same for every lane
+    const long long q0 = w0 + lane;
+    unsigned int starts = __ballot_sync(~0u, q0 < n && (q0 == 0 || key[q0 - 1] != key[q0]));
+    while (starts) {
+        const long long a = w0 + __ffs(starts) - 1;
+        starts &= starts - 1;
+        const unsigned int k = key[a];
+        int n_kept = 0;
+        for (long long b = a;; b += 32) {
+            const long long p = b + lane;
+            const bool in_run = p < n && key[p] == k;
+            const unsigned int run = __ballot_sync(~0u, in_run);
+            const int i = in_run ? val[p] : 0;
+            bool ok = in_run && k != dropped && n_kept < max_points;
+            double px = 0.0, py = 0.0, pz = 0.0;
+            if (ok) {
+                px = (double)in[(long long)i * stride]; py = (double)in[(long long)i * stride + 1];
+                pz = (double)in[(long long)i * stride + 2];
+                for (int j = 0; j < n_kept && ok; ++j) {
+                    const long long q = (long long)kept_at[a + j] * stride;
+                    const double dx = __dsub_rn(px, (double)in[q]), dy = __dsub_rn(py, (double)in[q + 1]),
+                                 dz = __dsub_rn(pz, (double)in[q + 2]);
+                    ok = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) >= s2;
+                }
+            }
+            unsigned int cand = __ballot_sync(~0u, ok), kept = 0u;
+            while (cand && n_kept < max_points) {
+                const int l = __ffs(cand) - 1;
+                kept |= 1u << l;
+                const double lx = __shfl_sync(~0u, px, l), ly = __shfl_sync(~0u, py, l), lz = __shfl_sync(~0u, pz, l);
+                if (lane == l) kept_at[a + n_kept] = i;
+                ++n_kept;
+                if (ok && lane > l) {
+                    const double dx = __dsub_rn(px, lx), dy = __dsub_rn(py, ly), dz = __dsub_rn(pz, lz);
+                    ok = __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz)) >= s2;
+                }
+                cand = __ballot_sync(~0u, ok && lane > l);
+            }
+            if (in_run) keep[i] = (int)((kept >> lane) & 1u);
+            if (run != ~0u) break;                               // the run ends in this batch
+            __syncwarp();                                        // this batch's kept_at entries, for the next
+        }
+    }
+}
+
 // Pass 4 (pos: the exclusive scan of keep): kept point i goes to out[pos[i]] (out_stride 3: x y z; 4: x y z and w = its
 // index over all kept points, as pack_points_kernel packs one cloud), index[pos[i]] = its index in its own cloud (index
 // may be null); out_seg[b] = pos[seg[b]] for b <= n_seg, the kept points' offsets.  max(n, n_seg) + 1 threads.
@@ -1399,8 +1460,10 @@ struct OdomSettings {
     // follows its sequence's motion-model error, under the ceiling params.search_radius
     bool adaptive = false;
     adaptive::Settings threshold{};
-    // (a session) dcreg_set_sparse_maps as it was at open; a one-shot call reads the context's
+    // (a session) dcreg_set_sparse_maps and dcreg_set_map_spacing as they were at open; a one-shot call reads the
+    // context's
     bool sparse_maps = false;
+    double map_spacing = 0.0;
     // dcreg_set_lane_params on (at open, for a session): every sequence's settings [n_seqs], params being entry 0; off:
     // empty
     std::vector<dcreg_icp_params> lanes;
@@ -1533,6 +1596,9 @@ struct dcreg_ctx {
     // dcreg_set_sparse_maps: odometry's local maps and the pairs' targets past the dense-grid limits get sparse row
     // indexes instead of a refusal (a session keeps the value it had at open)
     bool sparse_maps = false;
+    // dcreg_set_map_spacing: the minimum point spacing of odometry's map filter (0: the cap rule; a session keeps the
+    // value it had at open)
+    double map_spacing = 0.0;
     // dcreg_set_lane_params: the batched calls' params point to one entry per lane (a session keeps the value it had at
     // open).  A call's entries [lanes] (plan_iteration), an odometry step's device lane -> sequence [lanes], and the log
     // fill's device trial -> lane [trials]
@@ -1886,8 +1952,9 @@ static int voxel_reserve(dcreg_ctx* ctx, long long n, int n_seg, long long slots
 // keeping up to max_points points per voxel.  The kept points go to d_out (out_stride 3 or 4, see voxel_scatter_kernel)
 // and their indices in their own cloud to d_index (null: not wanted); the kept offsets to ctx->d_vox_seg [n_seg + 1], and
 // bad[b] != 0 in ctx->d_vox_bad when cloud b has a voxel coordinate outside [-2^20, 2^20).  No host sync; whatever
-// n_seg, six launches for max_points = 1, and for max_points > 1 seven and the radix sort's own.  prune (the voxel map):
-// voxel_prune_kernel between the flags and the scan, one launch more.
+// n_seg, six launches for max_points = 1, and for max_points > 1 seven and the radix sort's own.  min_spacing > 0 with
+// max_points > 1: voxel_space_flag_kernel instead of voxel_cap_flag_kernel, same launches; 0 is the cap rule.  prune
+// (the voxel map): voxel_prune_kernel between the flags and the scan, one launch more.
 struct VoxelPrune {
     const int* center;                  // [n_seg] the frame reference whose translation prunes each cloud
     int n_frames;                       // ... read as ref_pose reads it
@@ -1897,7 +1964,7 @@ struct VoxelPrune {
 };
 static int voxel_filter(dcreg_ctx* ctx, const float* d_in, long long n, int stride, const long long* d_seg,
                         const int64_t* h_seg, int n_seg, double voxel, float* d_out, int out_stride, long long* d_index,
-                        int max_points = 1, const VoxelPrune* prune = nullptr) {
+                        int max_points = 1, double min_spacing = 0.0, const VoxelPrune* prune = nullptr) {
     std::vector<long long> tab;
     const long long slots = voxel_tables(n_seg, h_seg, tab);
     int rc = voxel_reserve(ctx, n, n_seg, slots, max_points);
@@ -1923,7 +1990,11 @@ static int voxel_filter(dcreg_ctx* ctx, const float* d_in, long long n, int stri
         size_t tmp = (size_t)ctx->d_vox_sort_tmp.cap;
         CK(cub::DeviceRadixSort::SortPairs(ctx->d_vox_sort_tmp.p, tmp, key, key + n, val, val + n, (int)n, 0,
                                            voxel_key_bits(slots), ctx->stream));
-        voxel_cap_flag_kernel<<<nb1, 256, 0, ctx->stream>>>(key + n, val + n, n, dropped, max_points, ctx->d_vox_keep);
+        if (min_spacing > 0.0)      // val [0, n), the sort's consumed input, lists each run's kept points
+            voxel_space_flag_kernel<<<nb1, 256, 0, ctx->stream>>>(d_in, stride, key + n, val + n, n, dropped, max_points,
+                                                                  min_spacing * min_spacing, val, ctx->d_vox_keep);
+        else
+            voxel_cap_flag_kernel<<<nb1, 256, 0, ctx->stream>>>(key + n, val + n, n, dropped, max_points, ctx->d_vox_keep);
         ctx->launches++;                                         // (the radix sort's own kernels are not counted)
         CK(cudaGetLastError());
     }
@@ -1946,11 +2017,11 @@ static int voxel_filter(dcreg_ctx* ctx, const float* d_in, long long n, int stri
 }
 
 // The voxel filter of n clouds of host points (xyz / offsets / stride as in dcreg_icp_run_scans, validated), up to
-// max_points points per voxel: the kept points' xyz go to ctx->d_vox_xyz (3 floats a point, input order), their indices
+// max_points points per voxel at least min_spacing apart (0: no spacing): the kept points' xyz go to ctx->d_vox_xyz (3 floats a point, input order), their indices
 // to ctx->d_vox_index when `index`.  One host sync, after which kept[n + 1] holds the kept offsets and bad[n] the range
 // flags; fetch: *h_xyz (and *h_index) then point at host copies of the kept xyz (and indices) in ctx->h_pinned.
 static int voxel_filter_host(dcreg_ctx* ctx, int n, const float* xyz, const int64_t* offsets, int stride, double voxel,
-                             int max_points, bool index, bool fetch, int64_t* kept, int* bad,
+                             int max_points, double min_spacing, bool index, bool fetch, int64_t* kept, int* bad,
                              const float** h_xyz = nullptr, const long long** h_index = nullptr) {
     const long long total = offsets[n];
     CK(ctx->d_stage.ensure(total * stride));
@@ -1960,7 +2031,7 @@ static int voxel_filter_host(dcreg_ctx* ctx, int n, const float* xyz, const int6
     CK(cudaMemcpyAsync(ctx->d_stage, xyz, (size_t)total * stride * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_vox_in_seg, offsets, (size_t)(n + 1) * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream));
     int rc = voxel_filter(ctx, ctx->d_stage, total, stride, ctx->d_vox_in_seg, offsets, n, voxel, ctx->d_vox_xyz, 3,
-                          index ? ctx->d_vox_index.p : nullptr, max_points);
+                          index ? ctx->d_vox_index.p : nullptr, max_points, min_spacing);
     if (rc) return rc;
     // pinned: [n + 1] kept offsets, [n] flags (padded to 8 B), then (fetch) xyz [total][3] and indices [total]
     const size_t b_seg = (size_t)(n + 1) * sizeof(long long), b_bad = ((size_t)n * sizeof(int) + 7) / 8 * 8;
@@ -2278,6 +2349,16 @@ int dcreg_set_sparse_maps(dcreg_ctx* ctx, int enable) {
     if (!ctx) return DCREG_BAD_ARG;
     if (enable != 0 && enable != 1) { ctx->err = "set_sparse_maps: enable must be 0 or 1"; return DCREG_BAD_ARG; }
     ctx->sparse_maps = enable == 1;
+    return DCREG_OK;
+}
+
+int dcreg_set_map_spacing(dcreg_ctx* ctx, double min_spacing) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!(min_spacing >= 0.0 && min_spacing < INFINITY)) {
+        ctx->err = "set_map_spacing: min_spacing must be finite and >= 0 (0: no spacing)";
+        return DCREG_BAD_ARG;
+    }
+    ctx->map_spacing = min_spacing;
     return DCREG_OK;
 }
 
@@ -3533,6 +3614,7 @@ struct OdomCall {
     // (sparse_maps) the plan of the steps whose maps are sparse row indexes, made at the first such step
     const bool sparse_maps = sess ? set.sparse_maps : ctx->sparse_maps;
     LoopPlan L_sparse; bool planned_sparse = false;
+    const double map_spacing = sess ? set.map_spacing : ctx->map_spacing;   // the map filter's minimum spacing
     int failed = -1;                                // the step whose maps failed (-1: none)
     // (voxel map) where every sequence's map is: the session's maps before the first update, then each update's output
     odom_plan::MapState MS;
@@ -3607,7 +3689,7 @@ int OdomCall::build_map(const odom_plan::MapInput& in, const long long* ll, cons
         CK(cudaGetLastError());
         const VoxelPrune prune{ints + pieces, n_frames, ctx->d_state, d_hist_T, set.max_distance * set.max_distance};
         if (filter && (rc = voxel_filter(ctx, (const float*)ctx->d_odom_map.p, m, 4, ll, in.seg.data(), segs,
-                                         set.map_voxel, (float*)out.p, 4, nullptr, set.map_max_points,
+                                         set.map_voxel, (float*)out.p, 4, nullptr, set.map_max_points, map_spacing,
                                          in.center.empty() ? nullptr : &prune)))
             return rc;
     }
@@ -3673,7 +3755,7 @@ int OdomCall::check() {
         kept.resize((size_t)n_frames + 1);
         std::vector<int> bad((size_t)n_frames);
         if ((rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, set.source_voxel, set.source_max_points,
-                                    timestamps != nullptr, false, kept.data(), bad.data())))
+                                    0.0, timestamps != nullptr, false, kept.data(), bad.data())))
             return rc;
         for (int s = 0; s < n_seqs; ++s)
             for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k) {
@@ -4175,6 +4257,7 @@ static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     std::unique_ptr<dcreg_ctx::OdomSession> ss(new dcreg_ctx::OdomSession());
     ss->set = set;
     ss->set.sparse_maps = ctx->sparse_maps;
+    ss->set.map_spacing = ctx->map_spacing;
     const int n_seqs = set.n_seqs;
     BatchCheck c{name, !ss->set.T_init.empty(), "null pointer or n_seqs <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_seqs};
@@ -4306,9 +4389,17 @@ int dcreg_voxel_downsample(dcreg_ctx* ctx, int n_clouds, const float* xyz, const
 
 int dcreg_voxel_downsample_n(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,
                              double voxel, int max_points, float* out_xyz, int64_t* out_offsets, int64_t* out_index) {
+    return dcreg_voxel_downsample_spaced(ctx, n_clouds, xyz, offsets, stride, voxel, max_points, 0.0, out_xyz,
+                                         out_offsets, out_index);
+}
+
+int dcreg_voxel_downsample_spaced(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,
+                                  double voxel, int max_points, double min_spacing, float* out_xyz, int64_t* out_offsets,
+                                  int64_t* out_index) {
     if (!ctx) return DCREG_BAD_ARG;
     auto bad = [ctx](const std::string& why) { ctx->err = "voxel_downsample: " + why; return (int)DCREG_BAD_ARG; };
     if (max_points < 1) return bad("max_points must be >= 1");
+    if (!(min_spacing >= 0.0 && min_spacing < INFINITY)) return bad("min_spacing must be finite and >= 0 (0: no spacing)");
     if (n_clouds <= 0 || !xyz || !offsets || !out_xyz || !out_offsets) return bad("null pointer or n_clouds <= 0");
     if (stride < 3) return bad("stride < 3");
     if (!(voxel > 0.0 && voxel < INFINITY)) return bad("voxel must be finite and > 0");
@@ -4319,8 +4410,8 @@ int dcreg_voxel_downsample_n(dcreg_ctx* ctx, int n_clouds, const float* xyz, con
     std::vector<int64_t> kept((size_t)n_clouds + 1);
     const float* h_xyz = nullptr;
     const long long* h_index = nullptr;
-    int rc = voxel_filter_host(ctx, n_clouds, xyz, offsets, stride, voxel, max_points, out_index != nullptr, true,
-                               kept.data(), out_of_range.data(), &h_xyz, &h_index);
+    int rc = voxel_filter_host(ctx, n_clouds, xyz, offsets, stride, voxel, max_points, min_spacing, out_index != nullptr,
+                               true, kept.data(), out_of_range.data(), &h_xyz, &h_index);
     if (rc) return rc;
     for (int b = 0; b < n_clouds; ++b)
         if (out_of_range[(size_t)b])

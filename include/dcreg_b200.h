@@ -196,6 +196,15 @@ int dcreg_set_sparse_maps(dcreg_ctx* ctx, int enable);
  * others in a second kernel after it.  An odometry session copies the entries at open and keeps the setting it had
  * then; changing the setting later does not change its pushes.  enable other than 0 or 1: DCREG_BAD_ARG. */
 int dcreg_set_lane_params(dcreg_ctx* ctx, int enable);
+/* Minimum point spacing of scan-to-map odometry's map filter (KISS-ICP's VoxelHashMap::AddPoints): with min_spacing > 0,
+ * F_m(P) = dcreg_voxel_downsample_spaced(P, map_voxel, map_max_points, min_spacing) instead of dcreg_voxel_downsample_n,
+ * for the window and the voxel map of every dcreg_icp_run_odometry_voxel, _voxel_n, _deskew, _map and _adaptive call and
+ * of sessions.  KISS-ICP's value is map_voxel / sqrt(map_max_points).  It leaves the source filter F_s,
+ * dcreg_icp_run_odometry and _sequences, and maps with map_voxel = 0 or map_max_points = 1 unchanged (same launches,
+ * same bytes), and so does 0, the default.  A step keeps its launches and its one host sync.  An odometry session keeps
+ * the value it had at dcreg_odometry_open*: changing it later does not change that session's pushes, and
+ * dcreg_odometry_local_map returns the spaced map.  min_spacing NaN, negative or infinite: DCREG_BAD_ARG. */
+int dcreg_set_map_spacing(dcreg_ctx* ctx, double min_spacing);
 
 /* ---- seam 1: correspondence stage (icp_test_runner.cpp:1714-1813) -------------------------
  * For every source slot: q = fl32(R p + t), exact 5-NN in the target, 5th d^2 < radius^2,
@@ -624,6 +633,21 @@ int dcreg_voxel_downsample(dcreg_ctx* ctx, int n_clouds, const float* xyz, const
  * O(1) pass per point whatever a voxel's occupancy: seven launches besides the sort's, whatever n_clouds. */
 int dcreg_voxel_downsample_n(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,
                              double voxel, int max_points, float* out_xyz, int64_t* out_offsets, int64_t* out_index);
+/* dcreg_voxel_downsample_n with a minimum point spacing (KISS-ICP's AddPoints, which skips a point closer than
+ * voxel / sqrt(max_points_per_voxel) to a point already in its voxel).  Within each cloud and voxel, in ascending index,
+ * point p is kept iff fewer than max_points points of its voxel are kept before it and every kept point q before it has
+ * ((px - qx)^2 + (py - qy)^2) + (pz - qz)^2 >= min_spacing^2, in FP64 from the float32 coordinates with one rounding
+ * per operation and min_spacing^2 = min_spacing * min_spacing (a point exactly min_spacing away is kept).  A voxel's
+ * first point is always kept; the result is idempotent, and filtering filter(A) ++ B gives filter(A ++ B).  Voxels,
+ * dropped points, bit-for-bit copies, input order, out_index and errors as in dcreg_voxel_downsample_n, which is this
+ * call with min_spacing = 0; max_points = 1 or min_spacing = 0 runs it (same launches, same bytes), and min_spacing
+ * above twice the voxel size keeps what max_points = 1 keeps.  dcreg_b200.api.voxel_downsample(P, voxel, max_points,
+ * min_spacing) gives the same selection.  min_spacing NaN, negative or infinite is DCREG_BAD_ARG before anything is
+ * launched.  Cost: the radix sort of dcreg_voxel_downsample_n and the same launches, whatever n_clouds; its O(1) flag
+ * pass becomes one in which a warp settles each voxel's points in order, O(points x max_points) per voxel. */
+int dcreg_voxel_downsample_spaced(dcreg_ctx* ctx, int n_clouds, const float* xyz, const int64_t* offsets, int stride,
+                                  double voxel, int max_points, double min_spacing, float* out_xyz, int64_t* out_offsets,
+                                  int64_t* out_index);
 /* Same loop, but correspondences are supplied by the caller each iteration through a callback
  * (host kd-tree mode, "PR1"): planes are 4*n doubles (nx,ny,nz,d), all-zero = none. */
 typedef int (*dcreg_plane_callback)(void* user, const double T[16], double* planes4,
