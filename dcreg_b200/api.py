@@ -774,13 +774,14 @@ class Context:
         self.n_source = a.shape[0]
 
     def set_target(self, xyz, cell_size: float):
+        """A dense grid, or past 2^27 cells of the bounding box a sparse row index on which the batched calls and
+        find_planes run as on a dense grid (include/dcreg_b200.h, dcreg_set_target)."""
         a = _as_points(xyz)
         self._check(self.lib.dcreg_set_target(self._h, a.ctypes.data_as(C.POINTER(C.c_float)), a.shape[0], a.shape[1],
                                               float(cell_size)))
 
     def set_target_sparse(self, xyz, cell_size: float):
-        """set_target for maps too large for a dense grid: past 2^27 cells of the bounding box, a sparse row index on
-        which the batched calls and find_planes run as on a dense grid (include/dcreg_b200.h); below, set_target."""
+        """Identical to set_target (dcreg_set_target_sparse, kept for compatibility: include/dcreg_b200.h)."""
         a = _as_points(xyz)
         self._check(self.lib.dcreg_set_target_sparse(self._h, a.ctypes.data_as(C.POINTER(C.c_float)), a.shape[0],
                                                      a.shape[1], float(cell_size)))

@@ -13,7 +13,7 @@
 
 namespace arena_plan {
 
-constexpr long long kMaxDenseCells = 1ll << 27;      // per dense grid (above it the context's target uses a hash table)
+constexpr long long kMaxDenseCells = 1ll << 27;      // per dense grid (above it: a sparse row index, or an error)
 constexpr int kCoordLimit = 1 << 19;                 // cell coordinates outside +-2^19: NaN / huge coordinates
 constexpr long long kMaxCells = 1ll << 30;           // all grids of a call: cell ids and cell_start entries are int32
 constexpr long long kMaxPoints = 0x1fffffffLL;       // points per side and call: int32 positions, the loop kernel's 2^29
@@ -71,7 +71,7 @@ inline std::string plan(int n, const int* bounds, std::vector<Box>& boxes, long 
         if (fit == kOutOfRange) return out_of_range(seg.c_str());
         if (fit == kTooManyCells)
             return seg + ": bounding box of " + std::to_string(x.cells) +
-                   " cells is too large for a dense grid at this cell size (only the context's target falls back to a hash table)";
+                   " cells is too large for a dense grid at this cell size (dcreg_set_sparse_maps(1) builds a sparse row index instead)";
         x.cell_off = off;
         off += x.cells;
         if (off > kMaxCells)

@@ -14,12 +14,11 @@
 // Layout in HBM: target points grouped by cell (float4: x, y, z, bit-cast original index).
 //   dense mode : cells of the target's bounding box in x-fastest linear order + cell_start[ncells + 1];
 //                the 3 x-adjacent cells of a row are ONE contiguous point range, so a query scans 9 ranges.
-//   hash mode  : open-addressing table keyed by the packed cell coordinates (fallback when the bounding box
-//                has more than arena_plan::kMaxDenseCells cells); a query probes 27 cells.
-//   sparse mode: the dense order of the points, and cell_start only where a search can read it: a table of row starts
-//                (sparse_index.hpp) replaces the box's table, so the searches run the dense traversal with one table
-//                lookup per range end.  One build, the sparse_seg_* kernels below, serves dcreg_set_target_sparse (one
-//                cloud), odometry's local maps and dcreg_icp_run_pairs' targets (one cloud each).
+//   sparse mode: (a bounding box of more than arena_plan::kMaxDenseCells cells) the dense order of the points, and
+//                cell_start only where a search can read it: a table of row starts (sparse_index.hpp) replaces the
+//                box's table, so the searches run the dense traversal with one table lookup per range end.  One build,
+//                the sparse_seg_* kernels below, serves dcreg_set_target (one cloud), odometry's local maps and
+//                dcreg_icp_run_pairs' targets (one cloud each).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -34,17 +33,16 @@ struct Grid {
     float4* pts;                // n target points grouped by cell
     int* pos_of;                // [n] position in pts of the point with original index i (inverse of pts[j].w)
     int n;
-    int dense;                  // 1: dense mode, 0: hash mode, kSparseGrid: sparse mode
+    int dense;                  // 1: dense mode, kSparseGrid: sparse mode
     int rings;                  // ceil(search radius / cell edge): cells per direction a query must look at
     double inv_cell;            // 1 / cell edge
-    // dense mode
+    // dense mode (sparse mode: the box, no cell_start)
     int ox, oy, oz;             // cell coordinates of the bounding box's minimum corner
     int nx, ny, nz;
     int* cell_start;            // [nx*ny*nz + 1]
-    // hash mode (sparse mode: keys = sparse_index::key of (x, y, z) box-local, hstart = cs, no hcount)
-    unsigned long long* keys;   // capacity entries, kEmptyKey = free
-    int* hstart;                // capacity
-    int* hcount;                // capacity
+    // sparse mode: the row-start table
+    unsigned long long* keys;   // capacity entries: sparse_index::key of (x, y, z) box-local, sparse_index::kEmpty = free
+    int* hstart;                // capacity: cs of the key's cell
     unsigned int mask;          // capacity - 1 (capacity is a power of two)
 };
 
@@ -113,23 +111,6 @@ __global__ void grid_count_seg_kernel(const float4* __restrict__ pts, int n, con
     const int c = cell_off[b] + dense_index(g, cell_coord(p.x, g.inv_cell), cell_coord(p.y, g.inv_cell), cell_coord(p.z, g.inv_cell));
     pt_cell[i] = c;
     atomicAdd(&counts[c], 1);
-}
-
-// hash slot of a point (inserting its cell's key) and the per-slot counts
-__global__ void grid_insert_hash_kernel(const float4* __restrict__ pts, int n, Grid g, int* __restrict__ pt_slot) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const float4 p = pts[i];
-    const unsigned long long key = pack_key(cell_coord(p.x, g.inv_cell), cell_coord(p.y, g.inv_cell),
-                                            cell_coord(p.z, g.inv_cell));
-    unsigned int slot = hash_key(key) & g.mask;
-    while (true) {
-        const unsigned long long prev = atomicCAS(&g.keys[slot], kEmptyKey, key);
-        if (prev == kEmptyKey || prev == key) break;
-        slot = (slot + 1) & g.mask;
-    }
-    pt_slot[i] = (int)slot;
-    atomicAdd(&g.hcount[slot], 1);
 }
 
 // exclusive scan of an int array, three phases (tile sums, scan of tile sums, tile rescan)
@@ -216,17 +197,16 @@ __global__ void grid_scatter_kernel(const float4* __restrict__ pts, int n, const
 // order; this pass moves every point to (cell start + number of points of its cell with a smaller index).  One thread
 // per point, O(points in its cell) reads of a range its neighbours read too - parallel over POINTS, so a cell with
 // thousands of points (dense map, cell = search radius) no longer serialises on one thread the way a per-cell insertion
-// sort does.  `cell_of` is indexed by the original point index (p.w): dense cell id or hash slot.
+// sort does.  `cell_of` is indexed by the original point index (p.w).
 __global__ void grid_rank_cells_kernel(const float4* __restrict__ in, int n, const int* __restrict__ cell_of,
-                                       const int* __restrict__ start, const int* __restrict__ count,
-                                       float4* __restrict__ out, int* __restrict__ pos_of) {
+                                       const int* __restrict__ start, float4* __restrict__ out, int* __restrict__ pos_of) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n) return;
     const float4 p = in[j];
     const int me = __float_as_int(p.w);
     const int c = cell_of[me];
     const int s = start[c];
-    const int e = count ? s + count[c] : start[c + 1];
+    const int e = start[c + 1];
     int rank = 0;
     for (int k = s; k < e; ++k) rank += (__float_as_int(__ldg(&in[k].w)) < me) ? 1 : 0;
     out[s + rank] = p;
@@ -422,79 +402,93 @@ __device__ __forceinline__ void knn_scan_range(const float4* __restrict__ pts, i
 template <bool kSparse = false>
 __device__ __forceinline__ void knn_search(const Grid& g, float qx, float qy, float qz, Knn5& k) {
     const int cx = cell_coord(qx, g.inv_cell), cy = cell_coord(qy, g.inv_cell), cz = cell_coord(qz, g.inv_cell);
-    if (kSparse || g.dense) {
-        // K = ceil(radius / cell) rings of cells cover the search radius (K = 1 when cell = radius; a finer grid,
-        // cell = radius / 2, K = 2, scans ~3x fewer candidates because most cells are pruned by their box distance).
-        // Rows (dy, dz) are visited in rings of growing max(|dy|, |dz|); inside a row the own column first, then
-        // outwards.  A row / cell is skipped only when its box distance exceeds the current 5th-best distance
-        // (strictly, with a 1e-5 relative margin for the float arithmetic of the bound), so the search stays exact.
-        // Loops are deliberately NOT unrolled: one copy of the scan loop keeps the kernel inside the instruction
-        // cache (a fully unrolled version stalls on instruction fetch).
-        const int K = g.rings;
-        const float cell = (float)(1.0 / g.inv_cell);
-        const int lx = cx - g.ox, ly = cy - g.oy, lz = cz - g.oz;
-        if (lx + K < 0 || lx - K >= g.nx) return;
-        // position inside the own cell, in [0, cell) up to float rounding of cx * cell: every gap below is shrunk
-        // by an absolute eps that covers that rounding, so a bound can only be too small (never prunes a hit)
-        const float eps = 2e-6f * (fabsf(qx) + fabsf(qy) + fabsf(qz) + cell);
-        const float fx = qx - (float)cx * cell, fy = qy - (float)cy * cell, fz = qz - (float)cz * cell;
-        if (K == 1) {
-            // cell = search radius (the usual set-up): 9 rows of 3 cells, own row first, rows pruned by the same test
-            // as the general loop below; a visited row costs one fetch of its two outer cell boundaries and one scan
-            // (the lanes of a warp prune differently, so a warp walks nearly all 27 cells and every dependent load is
-            // on its critical path).
-            const int xa = min(max(lx - 1, 0), g.nx), xd = min(max(lx + 2, 0), g.nx);
+    // K = ceil(radius / cell) rings of cells cover the search radius (K = 1 when cell = radius; a finer grid,
+    // cell = radius / 2, K = 2, scans ~3x fewer candidates because most cells are pruned by their box distance).
+    // Rows (dy, dz) are visited in rings of growing max(|dy|, |dz|); inside a row the own column first, then
+    // outwards.  A row / cell is skipped only when its box distance exceeds the current 5th-best distance
+    // (strictly, with a 1e-5 relative margin for the float arithmetic of the bound), so the search stays exact.
+    // Loops are deliberately NOT unrolled: one copy of the scan loop keeps the kernel inside the instruction
+    // cache (a fully unrolled version stalls on instruction fetch).
+    const int K = g.rings;
+    const float cell = (float)(1.0 / g.inv_cell);
+    const int lx = cx - g.ox, ly = cy - g.oy, lz = cz - g.oz;
+    if (lx + K < 0 || lx - K >= g.nx) return;
+    // position inside the own cell, in [0, cell) up to float rounding of cx * cell: every gap below is shrunk
+    // by an absolute eps that covers that rounding, so a bound can only be too small (never prunes a hit)
+    const float eps = 2e-6f * (fabsf(qx) + fabsf(qy) + fabsf(qz) + cell);
+    const float fx = qx - (float)cx * cell, fy = qy - (float)cy * cell, fz = qz - (float)cz * cell;
+    if (K == 1) {
+        // cell = search radius (the usual set-up): 9 rows of 3 cells, own row first, rows pruned by the same test
+        // as the general loop below; a visited row costs one fetch of its two outer cell boundaries and one scan
+        // (the lanes of a warp prune differently, so a warp walks nearly all 27 cells and every dependent load is
+        // on its critical path).
+        const int xa = min(max(lx - 1, 0), g.nx), xd = min(max(lx + 2, 0), g.nx);
 #pragma unroll 1
-            for (int r = 0; r < 9; ++r) {
-                // own row first, then the ring: (dz, dy) = (-1,-1) (-1,0) (-1,1) (0,-1) (0,1) (1,-1) (1,0) (1,1)
-                const int q = r == 0 ? 4 : (r <= 4 ? r - 1 : r);
-                const int dz = q / 3 - 1, dy = q % 3 - 1;
-                const int zz = lz + dz, yy = ly + dy;
-                if (zz < 0 || zz >= g.nz || yy < 0 || yy >= g.ny) continue;
-                const float gz = dz == 0 ? 0.0f : fmaxf((dz < 0 ? fz : cell - fz) - eps, 0.0f);
-                const float gy = dy == 0 ? 0.0f : fmaxf((dy < 0 ? fy : cell - fy) - eps, 0.0f);
+        for (int r = 0; r < 9; ++r) {
+            // own row first, then the ring: (dz, dy) = (-1,-1) (-1,0) (-1,1) (0,-1) (0,1) (1,-1) (1,0) (1,1)
+            const int q = r == 0 ? 4 : (r <= 4 ? r - 1 : r);
+            const int dz = q / 3 - 1, dy = q % 3 - 1;
+            const int zz = lz + dz, yy = ly + dy;
+            if (zz < 0 || zz >= g.nz || yy < 0 || yy >= g.ny) continue;
+            const float gz = dz == 0 ? 0.0f : fmaxf((dz < 0 ? fz : cell - fz) - eps, 0.0f);
+            const float gy = dy == 0 ? 0.0f : fmaxf((dy < 0 ? fy : cell - fy) - eps, 0.0f);
+            const float row_lb = (gy * gy + gz * gz) * 0.99999f;
+            if (row_lb > knn_d2(k, 4)) continue;
+            const int* rowp = g.cell_start + (size_t)(zz * g.ny + yy) * g.nx;
+            // A row's three cells are one contiguous range: scanned in one pass, four loads in flight across the
+            // cell boundaries (~3 points per cell on a surface at cell = radius, so three separate passes spent
+            // most of their time in single-candidate trips, one memory round trip each).  The left / right cells
+            // are no longer pruned: their box-distance test only ever skips cells holding nothing below the
+            // current 5th key, so scanning them too leaves the list unchanged, bit for bit.
+            if constexpr (kSparse) {
+                int s, e;
+                sparse_span(g, zz, yy, xa, xd, s, e);
+                knn_scan_range(g.pts, s, e, qx, qy, qz, k);
+            } else {
+                knn_scan_range(g.pts, __ldg(rowp + xa), __ldg(rowp + xd), qx, qy, qz, k);
+            }
+        }
+        return;
+    }
+#pragma unroll 1
+    for (int ring = 0; ring <= K; ++ring) {
+        // a whole ring is at least (ring - 1) * cell + (distance to the own cell's nearest face) away
+        if (ring > 1) {
+            const float m = fmaxf(fminf(fminf(fy, cell - fy), fminf(fz, cell - fz)) + (float)(ring - 1) * cell - eps, 0.0f);
+            if (m * m * 0.99999f > knn_d2(k, 4)) break;
+        }
+#pragma unroll 1
+        for (int dz = -ring; dz <= ring; ++dz) {
+            const int zz = lz + dz;
+            if (zz < 0 || zz >= g.nz) continue;
+            const float gz = dz == 0 ? 0.0f : fmaxf((dz < 0 ? fz + (float)(-dz - 1) * cell : (cell - fz) + (float)(dz - 1) * cell) - eps, 0.0f);
+            const int stepy = (dz == -ring || dz == ring) ? 1 : 2 * ring;     // only the ring's boundary rows
+#pragma unroll 1
+            for (int dy = -ring; dy <= ring; dy += (stepy > 0 ? stepy : 1)) {
+                const int yy = ly + dy;
+                if (yy < 0 || yy >= g.ny) continue;
+                const float gy = dy == 0 ? 0.0f : fmaxf((dy < 0 ? fy + (float)(-dy - 1) * cell : (cell - fy) + (float)(dy - 1) * cell) - eps, 0.0f);
                 const float row_lb = (gy * gy + gz * gz) * 0.99999f;
                 if (row_lb > knn_d2(k, 4)) continue;
                 const int* rowp = g.cell_start + (size_t)(zz * g.ny + yy) * g.nx;
-                // A row's three cells are one contiguous range: scanned in one pass, four loads in flight across the
-                // cell boundaries (~3 points per cell on a surface at cell = radius, so three separate passes spent
-                // most of their time in single-candidate trips, one memory round trip each).  The left / right cells
-                // are no longer pruned: their box-distance test only ever skips cells holding nothing below the
-                // current 5th key, so scanning them too leaves the list unchanged, bit for bit.
-                if constexpr (kSparse) {
-                    int s, e;
-                    sparse_span(g, zz, yy, xa, xd, s, e);
-                    knn_scan_range(g.pts, s, e, qx, qy, qz, k);
-                } else {
-                    knn_scan_range(g.pts, __ldg(rowp + xa), __ldg(rowp + xd), qx, qy, qz, k);
+                // own column, then +-1, +-2, ... : stop a side once its gap bound exceeds the 5th-best distance
+                {
+                    const int x0 = min(max(lx, 0), g.nx), x1 = min(max(lx + 1, 0), g.nx);
+                    if constexpr (kSparse) {
+                        int s, e;
+                        sparse_span(g, zz, yy, x0, x1, s, e);
+                        knn_scan_range(g.pts, s, e, qx, qy, qz, k);
+                    } else {
+                        knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
+                    }
                 }
-            }
-            return;
-        }
 #pragma unroll 1
-        for (int ring = 0; ring <= K; ++ring) {
-            // a whole ring is at least (ring - 1) * cell + (distance to the own cell's nearest face) away
-            if (ring > 1) {
-                const float m = fmaxf(fminf(fminf(fy, cell - fy), fminf(fz, cell - fz)) + (float)(ring - 1) * cell - eps, 0.0f);
-                if (m * m * 0.99999f > knn_d2(k, 4)) break;
-            }
-#pragma unroll 1
-            for (int dz = -ring; dz <= ring; ++dz) {
-                const int zz = lz + dz;
-                if (zz < 0 || zz >= g.nz) continue;
-                const float gz = dz == 0 ? 0.0f : fmaxf((dz < 0 ? fz + (float)(-dz - 1) * cell : (cell - fz) + (float)(dz - 1) * cell) - eps, 0.0f);
-                const int stepy = (dz == -ring || dz == ring) ? 1 : 2 * ring;     // only the ring's boundary rows
-#pragma unroll 1
-                for (int dy = -ring; dy <= ring; dy += (stepy > 0 ? stepy : 1)) {
-                    const int yy = ly + dy;
-                    if (yy < 0 || yy >= g.ny) continue;
-                    const float gy = dy == 0 ? 0.0f : fmaxf((dy < 0 ? fy + (float)(-dy - 1) * cell : (cell - fy) + (float)(dy - 1) * cell) - eps, 0.0f);
-                    const float row_lb = (gy * gy + gz * gz) * 0.99999f;
-                    if (row_lb > knn_d2(k, 4)) continue;
-                    const int* rowp = g.cell_start + (size_t)(zz * g.ny + yy) * g.nx;
-                    // own column, then +-1, +-2, ... : stop a side once its gap bound exceeds the 5th-best distance
-                    {
-                        const int x0 = min(max(lx, 0), g.nx), x1 = min(max(lx + 1, 0), g.nx);
+                for (int dx = 1; dx <= K; ++dx) {
+                    const float gl = fmaxf(fx + (float)(dx - 1) * cell - eps, 0.0f);
+                    const float gr = fmaxf((cell - fx) + (float)(dx - 1) * cell - eps, 0.0f);
+                    const bool left = (row_lb + gl * gl * 0.99999f) <= knn_d2(k, 4);
+                    if (left) {
+                        const int x0 = min(max(lx - dx, 0), g.nx), x1 = min(max(lx - dx + 1, 0), g.nx);
                         if constexpr (kSparse) {
                             int s, e;
                             sparse_span(g, zz, yy, x0, x1, s, e);
@@ -503,53 +497,21 @@ __device__ __forceinline__ void knn_search(const Grid& g, float qx, float qy, fl
                             knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
                         }
                     }
-#pragma unroll 1
-                    for (int dx = 1; dx <= K; ++dx) {
-                        const float gl = fmaxf(fx + (float)(dx - 1) * cell - eps, 0.0f);
-                        const float gr = fmaxf((cell - fx) + (float)(dx - 1) * cell - eps, 0.0f);
-                        const bool left = (row_lb + gl * gl * 0.99999f) <= knn_d2(k, 4);
-                        if (left) {
-                            const int x0 = min(max(lx - dx, 0), g.nx), x1 = min(max(lx - dx + 1, 0), g.nx);
-                            if constexpr (kSparse) {
-                                int s, e;
-                                sparse_span(g, zz, yy, x0, x1, s, e);
-                                knn_scan_range(g.pts, s, e, qx, qy, qz, k);
-                            } else {
-                                knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
-                            }
+                    const bool right = (row_lb + gr * gr * 0.99999f) <= knn_d2(k, 4);
+                    if (right) {
+                        const int x0 = min(max(lx + dx, 0), g.nx), x1 = min(max(lx + dx + 1, 0), g.nx);
+                        if constexpr (kSparse) {
+                            int s, e;
+                            sparse_span(g, zz, yy, x0, x1, s, e);
+                            knn_scan_range(g.pts, s, e, qx, qy, qz, k);
+                        } else {
+                            knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
                         }
-                        const bool right = (row_lb + gr * gr * 0.99999f) <= knn_d2(k, 4);
-                        if (right) {
-                            const int x0 = min(max(lx + dx, 0), g.nx), x1 = min(max(lx + dx + 1, 0), g.nx);
-                            if constexpr (kSparse) {
-                                int s, e;
-                                sparse_span(g, zz, yy, x0, x1, s, e);
-                                knn_scan_range(g.pts, s, e, qx, qy, qz, k);
-                            } else {
-                                knn_scan_range(g.pts, __ldg(rowp + x0), __ldg(rowp + x1), qx, qy, qz, k);
-                            }
-                        }
-                        if (!left && !right) break;
                     }
+                    if (!left && !right) break;
                 }
             }
         }
-    } else {
-        const int K = g.rings;
-        for (int dz = -K; dz <= K; ++dz)
-            for (int dy = -K; dy <= K; ++dy)
-                for (int dx = -K; dx <= K; ++dx) {
-                    const unsigned long long key = pack_key(cx + dx, cy + dy, cz + dz);
-                    unsigned int slot = hash_key(key) & g.mask;
-                    int start = 0, cnt = 0;
-                    while (true) {
-                        const unsigned long long kk = __ldg(&g.keys[slot]);
-                        if (kk == key) { start = __ldg(&g.hstart[slot]); cnt = __ldg(&g.hcount[slot]); break; }
-                        if (kk == kEmptyKey) break;
-                        slot = (slot + 1) & g.mask;
-                    }
-                    knn_scan_range(g.pts, start, start + cnt, qx, qy, qz, k);
-                }
     }
 }
 

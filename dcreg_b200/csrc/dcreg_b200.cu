@@ -2,7 +2,7 @@
 //
 // Data layout in HBM (per context):
 //   src      float4[N]   body-frame source points (x,y,z,-), uploaded once per scan
-//   tgt grid float4[M]   target points grouped by hash-grid cell + keys/start/count tables
+//   tgt grid float4[M]   target points grouped by grid cell + cell_start table (dense grid) or row-start table (sparse)
 //   planes64 double4[N]  (nx,ny,nz,d) per source slot, only materialised for the seams / host-plane mode
 //   planes32 float4[N]   the 32 B/slot frozen-plane layout of the K1 benchmark
 //   per trial (dcreg_icp_run: one, dcreg_icp_run_batch: many): neighbour records / plane cache (100 B per slot),
@@ -1605,8 +1605,6 @@ struct dcreg_ctx {
     bool lane_params = false;
     DevBuf<dcreg_icp_params> d_lane_prm;
     DevBuf<int> d_lane_seq, d_trial_lane;
-    // the hash table of a dcreg_set_target target too large for a dense grid (build_hash_grid; points in tgt_arena)
-    DevBuf<unsigned long long> d_hash_keys; DevBuf<int> d_hash_start, d_hash_count;
     DevBuf<float4> d_pair_tgt;                                   // targets, packed (w = global index)
     DevBuf<long long> d_pair_tgt_seg; DevBuf<double> d_pair_T;   // [n + 1] / [n][16] final poses
     DevBuf<float4> d_aligned;                                    // sources under their final poses
@@ -2134,7 +2132,7 @@ static int arena_fill(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_p
     ctx->launches++;
     if ((rc = device_exclusive_scan(ctx, A.counts, cells + 1, A.cell_start))) return rc;
     corr::grid_scatter_kernel<<<nb, 256, 0, ctx->stream>>>(d_pts, (int)m, A.pt_cell, A.cell_start, A.fill, A.tmp, 0);
-    corr::grid_rank_cells_kernel<<<nb, 256, 0, ctx->stream>>>(A.tmp, (int)m, A.pt_cell, A.cell_start, nullptr, A.pts, A.pos_of);
+    corr::grid_rank_cells_kernel<<<nb, 256, 0, ctx->stream>>>(A.tmp, (int)m, A.pt_cell, A.cell_start, A.pts, A.pos_of);
     ctx->launches += 2;
     CK(cudaGetLastError());
     return DCREG_OK;
@@ -2212,7 +2210,7 @@ static int build_sparse_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const flo
     CK(A.tab_start.ensure(off[(size_t)n]));
     for (int b = 0; b < n; ++b) {
         corr::Grid& g = hg[(size_t)b];
-        g.keys = A.tab_keys.p + off[(size_t)b]; g.hstart = A.tab_start.p + off[(size_t)b]; g.hcount = nullptr;
+        g.keys = A.tab_keys.p + off[(size_t)b]; g.hstart = A.tab_start.p + off[(size_t)b];
         g.mask = (unsigned)(cap[(size_t)b] - 1);
     }
     CK(cudaMemcpyAsync(A.d_grids, hg.data(), hg.size() * sizeof(corr::Grid), cudaMemcpyHostToDevice, ctx->stream));
@@ -2224,10 +2222,9 @@ static int build_sparse_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const flo
     return DCREG_OK;
 }
 
-// Both steps; a cloud whose box needs more than arena_plan::kMaxDenseCells cells is rejected (no hash grids here),
-// unless sparse_at is given: then such clouds (or more than kMaxCells in all) make every cloud a sparse row index
-// (build_sparse_arena), and *sparse_at is the first cloud over kMaxDenseCells (n: none, only the total is over), or -1
-// when the grids are dense.
+// Both steps; a cloud whose box needs more than arena_plan::kMaxDenseCells cells is rejected, unless sparse_at is
+// given: then such clouds (or more than kMaxCells in all) make every cloud a sparse row index (build_sparse_arena), and
+// *sparse_at is the first cloud over kMaxDenseCells (n: none, only the total is over), or -1 when the grids are dense.
 static int build_grid_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float4* d_pts, const int64_t* h_seg,
                             const long long* d_seg, int n, double cell_size, int rings, const char* what,
                             long long* cells_out, int* sparse_at = nullptr) {
@@ -2263,40 +2260,12 @@ static int build_grid_arena(dcreg_ctx* ctx, dcreg_ctx::GridArena& A, const float
 // one-segment offset tables of the context's own clouds (device, in d_small): [0, 1] = {0, n_tgt}, [2, 3] = {0, n_src}
 static long long* own_segs(dcreg_ctx* ctx) { return (long long*)(ctx->d_small + 512); }
 
-// The context's target when its box has more than arena_plan::kMaxDenseCells cells: its m points grouped by the slots
-// of an open-addressing hash table.  The points and the scratch are tgt_arena's; the tables are the context's own.
-static int build_hash_grid(dcreg_ctx* ctx, long long m, double inv_cell) {
-    dcreg_ctx::GridArena& A = ctx->tgt_arena;
-    long long cap = 1024;
-    while (cap < 2 * m) cap <<= 1;
-    int rc;
-    CK(A.reserve(m, cap));                                                  // A.fill: per slot
-    CK(ctx->d_hash_keys.ensure(cap));
-    CK(ctx->d_hash_start.ensure(cap));
-    CK(ctx->d_hash_count.ensure(cap));
-    corr::Grid g{};
-    g.pts = A.pts; g.pos_of = A.pos_of; g.n = (int)m; g.dense = 0; g.rings = 1; g.inv_cell = inv_cell;
-    g.keys = ctx->d_hash_keys; g.hstart = ctx->d_hash_start; g.hcount = ctx->d_hash_count; g.mask = (unsigned)(cap - 1);
-    CK(cudaMemsetAsync(g.keys, 0xff, (size_t)cap * sizeof(unsigned long long), ctx->stream));
-    CK(cudaMemsetAsync(g.hcount, 0, (size_t)cap * sizeof(int), ctx->stream));
-    CK(cudaMemsetAsync(A.fill, 0, (size_t)cap * sizeof(int), ctx->stream));
-    const unsigned nb = (unsigned)((m + 255) / 256);
-    corr::grid_insert_hash_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_tgt, (int)m, g, A.pt_cell);
-    if ((rc = device_exclusive_scan(ctx, g.hcount, cap, g.hstart))) return rc;
-    corr::grid_scatter_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_tgt, (int)m, A.pt_cell, g.hstart, A.fill, A.tmp, 0);
-    corr::grid_rank_cells_kernel<<<nb, 256, 0, ctx->stream>>>(A.tmp, (int)m, A.pt_cell, g.hstart, g.hcount, A.pts, A.pos_of);
-    ctx->launches += 3;
-    CK(cudaGetLastError());
-    ctx->grid = g;
-    return DCREG_OK;
-}
-
-// dcreg_set_target, and with `sparse` dcreg_set_target_sparse: the same up to the choice past the dense-cell limit
-static int set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size, bool sparse) {
+// dcreg_set_target and its alias dcreg_set_target_sparse (`name`, for the error texts): a dense grid, or past
+// arena_plan::kMaxDenseCells cells a sparse row index
+static int set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size, const char* name) {
     if (!ctx) return DCREG_BAD_ARG;
     if (!xyz || m <= 0 || stride < 3 || !(cell_size > 0.0) || m > 0x7fffffffLL) {
-        ctx->err = std::string(sparse ? "dcreg_set_target_sparse" : "dcreg_set_target") +
-                   ": empty cloud, stride < 3, cell_size <= 0 or too many points";
+        ctx->err = std::string(name) + ": empty cloud, stride < 3, cell_size <= 0 or too many points";
         return DCREG_BAD_ARG;
     }
     CK(cudaSetDevice(ctx->device));
@@ -2322,14 +2291,12 @@ static int set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, d
         if ((rc = arena_fill(ctx, ctx->tgt_arena, ctx->d_tgt, d_seg, 1, m, &box, box.cells, inv_cell, 1))) return rc;
         ctx->grid = arena_grid(ctx->tgt_arena, box, m, inv_cell, 1);
         ctx->grid_cells = box.cells;
-    } else if (sparse) {
+    } else {
         int bad = -1;
         if ((rc = build_sparse_arena(ctx, ctx->tgt_arena, ctx->d_tgt, d_seg, {0, m}, 1, hb.data(), inv_cell, 1, nullptr,
                                      &bad, &ctx->grid)))
             return rc;
-        if (bad >= 0) { ctx->err = "dcreg_set_target_sparse: the sparse index needs more than 2^32 table slots"; return DCREG_BAD_ARG; }
-    } else if ((rc = build_hash_grid(ctx, m, inv_cell))) {
-        return rc;
+        if (bad >= 0) { ctx->err = std::string(name) + ": the sparse index needs more than 2^32 table slots"; return DCREG_BAD_ARG; }
     }
     const cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) { ctx->err = std::string("grid build: ") + cudaGetErrorString(e); return DCREG_CUDA_ERROR; }
@@ -2338,11 +2305,11 @@ static int set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, d
 }
 
 int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size) {
-    return set_target(ctx, xyz, m, stride, cell_size, false);
+    return set_target(ctx, xyz, m, stride, cell_size, "dcreg_set_target");
 }
 
 int dcreg_set_target_sparse(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size) {
-    return set_target(ctx, xyz, m, stride, cell_size, true);
+    return set_target(ctx, xyz, m, stride, cell_size, "dcreg_set_target_sparse");
 }
 
 int dcreg_set_sparse_maps(dcreg_ctx* ctx, int enable) {
@@ -2437,9 +2404,9 @@ int dcreg_point_to_point_metrics(dcreg_ctx* ctx, const double T[16], double erro
     if (!ctx) return DCREG_BAD_ARG;
     if (!T || !out) { ctx->err = "p2p metrics: null pointer"; return DCREG_BAD_ARG; }
     if (!ctx->d_src || !ctx->has_grid || !ctx->d_tgt) { ctx->err = "p2p metrics: set source and target first"; return DCREG_BAD_ARG; }
-    if (!ctx->grid.dense) { ctx->err = "p2p metrics need the dense grid (target bounding box too large for this cell size)"; return DCREG_BAD_ARG; }
     if (ctx->grid.dense == corr::kSparseGrid) {          // nn1_search expands rings over the whole box
-        ctx->err = "p2p metrics need the dense grid (the target is a sparse row index: dcreg_set_target_sparse)";
+        ctx->err = "p2p metrics need the dense grid (the target is a sparse row index: its bounding box is too large for "
+                   "this cell size)";
         return DCREG_BAD_ARG;
     }
     CK(cudaSetDevice(ctx->device));
@@ -2488,7 +2455,8 @@ static int sort_by_sparse_cell(dcreg_ctx* ctx, const float4* pts, long long n, c
 // agree.  The sorted copy carries the original index in .w; the pose moves little during ICP, so one sort per run suffices.
 static int sort_source_by_cell(dcreg_ctx* ctx, const double T[16], const float4** src_out) {
     *src_out = ctx->d_src;
-    if (ctx->grid.dense == corr::kSparseGrid && ctx->n_src <= 0x7fffffffLL) {
+    if (ctx->n_src > 0x7fffffffLL) return DCREG_OK;
+    if (ctx->grid.dense == corr::kSparseGrid) {
         CK(ctx->d_src_sorted.ensure(ctx->n_src));
         double* dT = ctx->d_small + 640;
         CK(cudaMemcpyAsync(dT, T, 12 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
@@ -2497,7 +2465,6 @@ static int sort_source_by_cell(dcreg_ctx* ctx, const double T[16], const float4*
         *src_out = ctx->d_src_sorted;
         return DCREG_OK;
     }
-    if (!ctx->grid.dense || ctx->n_src > 0x7fffffffLL) return DCREG_OK;
     const long long n = ctx->n_src, ncells = ctx->grid_cells;
     CK(ctx->d_src_sorted.ensure(n));
     CK(ctx->d_sort_tmp.ensure(n));
@@ -2515,7 +2482,7 @@ static int sort_source_by_cell(dcreg_ctx* ctx, const double T[16], const float4*
     int rc = device_exclusive_scan(ctx, counts, ncells + 1, start);
     if (rc) return rc;
     corr::grid_scatter_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_src, (int)n, ctx->d_pt_cell, start, fill, ctx->d_sort_tmp, 0);
-    corr::grid_rank_cells_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_sort_tmp, (int)n, ctx->d_pt_cell, start, nullptr, ctx->d_src_sorted, nullptr);
+    corr::grid_rank_cells_kernel<<<nb, 256, 0, ctx->stream>>>(ctx->d_sort_tmp, (int)n, ctx->d_pt_cell, start, ctx->d_src_sorted, nullptr);
     ctx->launches += 3;
     CK(cudaGetLastError());
     *src_out = ctx->d_src_sorted;
@@ -2702,14 +2669,12 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         a.grid.rings = rings;
     }
     // Lean only: a plain 5-NN search and a fresh fit for every slot in every iteration, no records (coherent_step 0:
-    // the solve step never switches to coherent mode).  A hash-grid target has no cell_start table for coherent mode's
-    // bounded and warp searches; seam 1 (planes_out) fits every slot once; more than 2^29 - 1 slots would need more than
-    // 54 GB of records (101 B per slot); DCREG_FUSED_SEARCH (a single run of the context's source) is the reference the
-    // record-reusing loop is tested against.
-    const bool lean_only = (!L.grid_table && !ctx->grid.dense) || planes_out || a.n > arena_plan::kMaxPoints ||
-                           (!batch && getenv("DCREG_FUSED_SEARCH"));
-    if ((trials > 1 || batch) && lean_only) {
-        ctx->err = "batched trials need the dense target grid (target bounding box / cell size too large for it)";
+    // the solve step never switches to coherent mode).  Seam 1 (planes_out) fits every slot once; more than 2^29 - 1
+    // slots would need more than 54 GB of records (101 B per slot); DCREG_FUSED_SEARCH (a single run of the context's
+    // source) is the reference the record-reusing loop is tested against.
+    const bool lean_only = planes_out || a.n > arena_plan::kMaxPoints || (!batch && getenv("DCREG_FUSED_SEARCH"));
+    if ((trials > 1 || batch) && lean_only) {   // only dcreg_icp_run_batch: a batch's sources total at most kMaxPoints
+        ctx->err = "batched trials need per-slot records (more than 2^29 - 1 source points, or DCREG_FUSED_SEARCH set)";
         return DCREG_BAD_ARG;
     }
     const long long slots = ctx->n_src;
@@ -3038,10 +3003,6 @@ int dcreg_time_iteration(dcreg_ctx* ctx, const dcreg_icp_params* params, const d
                          float* ms_per_body) {
     if (!ctx || !params || !T || reps <= 0 || !ms_per_body) return DCREG_BAD_ARG;
     if (!ctx->d_src || !ctx->has_grid) { ctx->err = "time_iteration: set source and target first"; return DCREG_BAD_ARG; }
-    if (what == 0 && !ctx->grid.dense) {
-        ctx->err = "time_iteration: what = 0 (coherent mode) needs a dense target grid; a hash-grid target always searches in full";
-        return DCREG_BAD_ARG;
-    }
     CK(cudaSetDevice(ctx->device));
     dcreg_icp_params prm = *params;
     prm.fixed_iterations = 1;
@@ -3411,7 +3372,6 @@ struct BatchCheck {
     const char* own_msg = nullptr;      // a check of the call's own that failed, reported after the cell size
     bool need_source = false, need_target = true;    // check_run_args
     bool one_iteration = false;         // max_iterations >= 1
-    const char* dense = nullptr;        // the context's dense grid is needed by these ("batches")
     int n_seqs = 0;                     // the sequence table [n_seqs + 1]: from 0, ascending strictly, up to n
     const int* seq_offsets = nullptr;
     bool empty_seqs = false;            // ... or only non-decreasing (dcreg_odometry_push: a sequence may have no frame)
@@ -3432,8 +3392,6 @@ static int check_batch_call(dcreg_ctx* ctx, const dcreg_icp_params* params, cons
     const int rc = check_run_args(ctx, params, c.need_source, c.need_target);
     if (rc) return rc;
     if (c.one_iteration && params->max_iterations < 1) return bad(name + ": max_iterations must be >= 1");
-    if (c.dense && !ctx->grid.dense)
-        return bad(name + ": " + c.dense + " need the dense target grid (target bounding box / cell size too large for it)");
     if (c.own_cell) {
         const int rings = search_rings(params->search_radius, c.cell_size);
         if (rings < 1 || rings > 4) return bad(name + ": search_radius / cell_size must be in (0, 4]");
@@ -3481,7 +3439,7 @@ int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_sc
     BatchCheck c{"icp_run_scans", params && n_scans > 0 && xyz && scan_offsets && T_init && T_out,
                  "null pointer or n_scans <= 0", "scans are independent - distribute them over ranks, do not shard them",
                  n_scans};
-    c.offsets = scan_offsets; c.item = "scan"; c.stride = stride; c.dense = "batches";
+    c.offsets = scan_offsets; c.item = "scan"; c.stride = stride;
     c.lanes = ctx->lane_params ? n_scans : 0;
     int rc = check_batch_call(ctx, params, c);
     if (rc) return rc;
@@ -3501,7 +3459,7 @@ int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int 
     BatchCheck c{"icp_run_sequences", params && n_seqs > 0 && n_frames > 0 && seq_offsets && xyz && frame_offsets && T_init && T_out,
                  "null pointer, n_seqs <= 0 or n_frames <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_frames};
-    c.offsets = frame_offsets; c.item = "frame"; c.stride = stride; c.one_iteration = true; c.dense = "sequences";
+    c.offsets = frame_offsets; c.item = "frame"; c.stride = stride; c.one_iteration = true;
     c.n_seqs = n_seqs; c.seq_offsets = seq_offsets;
     c.lanes = ctx->lane_params ? n_seqs : 0;
     int rc = check_batch_call(ctx, params, c);

@@ -152,25 +152,23 @@ void* dcreg_stream(dcreg_ctx* ctx);
 int dcreg_set_source(dcreg_ctx* ctx, const float* xyz, int64_t n, int stride);
 /* Target cloud + its spatial index.  Replaces ICPContext::setTargetCloud's kd-tree build
  * (utils.hpp:393-424): a device dense grid with cell = `cell_size` (pass the search radius;
- * exact 5-NN-within-radius then only needs the 27 surrounding cells), with a hash-table fallback when the bounding box
- * has more than 2^27 cells. */
-int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size);
-/* Target cloud for maps too large for a dense grid (city-scale prior maps).  Same arguments and checks as
- * dcreg_set_target, and while the bounding box has at most 2^27 cells it IS dcreg_set_target (same launches, same
- * bytes).  Past that the index is a sparse row index instead of the hash table: the points in the dense grid's order
+ * exact 5-NN-within-radius then only needs the 27 surrounding cells).  A map too large for a dense grid (a bounding box
+ * of more than 2^27 cells: city-scale prior maps) gets a sparse row index instead: the points in the dense grid's order
  * (by cell z, y, x, then index) and an open-addressing table of the row starts the searches read, about 12 B per table
  * slot with at most 18 entries per occupied cell (2 slots per entry, rounded up to a power of two), instead of 12 B per
  * cell of the box.  On it dcreg_icp_run, _enqueue / _fetch (records and coherent mode as on a dense grid),
- * dcreg_icp_run_batch, _scans, _sequences and dcreg_find_planes work as on a dense grid: for sources whose query cells
- * stay inside a dense grid's box, a target whose extra points lie outside every search returns that grid's results bit
- * for bit.  dcreg_point_to_point_metrics refuses it (DCREG_BAD_ARG).  A cell coordinate outside +-2^19 gives
- * DCREG_BAD_ARG. */
+ * dcreg_icp_run_batch, _scans, _sequences, dcreg_find_planes and dcreg_time_iteration work as on a dense grid: for
+ * sources whose query cells stay inside a dense grid's box, a target whose extra points lie outside every search returns
+ * that grid's results bit for bit.  dcreg_point_to_point_metrics refuses it (DCREG_BAD_ARG).  A cell coordinate outside
+ * +-2^19, or a sparse index that would need more than 2^32 table slots, gives DCREG_BAD_ARG. */
+int dcreg_set_target(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size);
+/* Identical to dcreg_set_target (kept for compatibility; its error texts name dcreg_set_target_sparse). */
 int dcreg_set_target_sparse(dcreg_ctx* ctx, const float* xyz, int64_t m, int stride, double cell_size);
 /* Sparse row indexes for the grids the library builds itself: the local maps of dcreg_icp_run_odometry* and of the
  * odometry sessions, and the targets of dcreg_icp_run_pairs.  enable = 0 (the default): such a map or target whose
  * bounding box has more than 2^27 cells at cell_size, or a step's or call's grids with more than 2^30 cells in all, is
  * DCREG_BAD_ARG, as documented at those calls.  enable = 1: that step (every lane of it) or that call (every pair of
- * it) builds sparse row indexes instead (those of dcreg_set_target_sparse, one per map or target, in one set of buffers;
+ * it) builds sparse row indexes instead (those of dcreg_set_target, one per map or target, in one set of buffers;
  * one more host sync), and returns what the dense grids would return on the same points: a search of a sparse index
  * gives the dense grid's results bit for bit.  A step or call that fits dense grids runs exactly as with enable = 0;
  * there is no other choice between the two.  Still DCREG_BAD_ARG with enable = 1: a cell coordinate outside +-2^19, a
@@ -272,7 +270,7 @@ int dcreg_icp_fetch(dcreg_ctx* ctx, double T_out[16], int* n_iterations, int* co
  * equal up to the order of the FP64 sums (the source is sorted by target cell once, under trial 0's pose, and a single
  * run of a small cloud uses smaller tiles; 1e-8 on the poses in the tests; a batch itself is reproducible bit for
  * bit).  Not
- * available on a sharded context: trials are independent, distribute them over ranks instead.  Needs the dense grid. */
+ * available on a sharded context: trials are independent, distribute them over ranks instead. */
 int dcreg_icp_run_batch(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_trials, const double* T_init,
                         double* T_out, int* n_iterations, int* converged, int* status, dcreg_iter_log* log,
                         int log_cap);
@@ -287,7 +285,7 @@ int dcreg_icp_run_batch(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_tr
  * only in how the FP64 partial sums are grouped (counts, masks and iteration counts identical, poses equal to rounding;
  * a batch itself is reproducible bit for bit).  The scans go to buffers of their own: the context's source and what
  * dcreg_icp_run computes from it are left as they were. Not available on a sharded context (distribute scans over ranks
- * instead).  Needs the dense grid. */
+ * instead). */
 int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_scans, const float* xyz,
                         const int64_t* scan_offsets, int stride, const double* T_init, double* T_out,
                         int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
@@ -299,7 +297,7 @@ int dcreg_icp_run_scans(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_sc
  * at most 2^29 - 1 points per side, at most 65535 pairs).  cell_size: as in dcreg_set_target (search_radius / cell_size
  * in (0, 4]); every target needs a dense grid (at most 2^27 cells in its bounding box, 2^30 over the call), unless
  * dcreg_set_sparse_maps(1): then a call past those limits gives every target a sparse row index, and pair b equals
- * dcreg_set_target_sparse(tgt_b) + dcreg_set_source(src_b) + dcreg_icp_run(T_init[b]) up to the FP64 grouping.
+ * dcreg_set_target(tgt_b) + dcreg_set_source(src_b) + dcreg_icp_run(T_init[b]) up to the FP64 grouping.
  * T_init / T_out / n_iterations / converged / status / cov / log: as in dcreg_icp_run_scans, one per pair.
  * metrics: n_pairs x 4 doubles or NULL; pair b's dcreg_point_to_point_metrics(T_out[b], error_threshold) = rmse, fitness,
  * chamfer, n_valid (an aligned source too large for a dense grid, or a call whose targets are sparse row indexes:
@@ -336,7 +334,7 @@ int dcreg_icp_run_pairs(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_pa
  * - Device memory grows with the points of the call (about 100 B per point, as for scans): process a long recording in
  *   calls of a few thousand frames, each call's T_init being the previous call's last T_out * delta.
  * The frames go to buffers of their own: the context's source and what dcreg_icp_run, trial batches and scan batches
- * compute are left as they were.  Needs max_iterations >= 1 and the dense grid; not available on a sharded context
+ * compute are left as they were.  Needs max_iterations >= 1; not available on a sharded context
  * (give every rank its own sequences).  Errors: DCREG_BAD_ARG with dcreg_last_error, as dcreg_icp_run_scans. */
 int dcreg_icp_run_sequences(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
                             int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,

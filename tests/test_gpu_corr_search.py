@@ -1,8 +1,8 @@
 """The neighbour searches of corr.cuh, query by query, against a float32 brute force.
 
-tools/test_corr_search.cu runs the production device functions (knn_search on the dense and on a hash grid,
-knn_search_lb, knn_warp_search with and without the loop kernel's row table, knn_row_range, nn1_search) and corr.cuh's
-grid build kernels on a grid and queries written by this file; the reference here is NumPy:
+tools/test_corr_search.cu runs the production device functions (knn_search on the dense grid and on the sparse row
+index of the same points, knn_search_lb, knn_warp_search with and without the loop kernel's row table, knn_row_range,
+nn1_search) and corr.cuh's grid build kernels on a grid and queries written by this file; the reference here is NumPy:
 
   * the layout twin (grid_layout): cell coordinates floor(float64(v) * (1 / cell)), the points' min / max cell as the
     box, x-fastest cells, ascending original index inside a cell, .w = the index bit-cast to float32, cell_start the
@@ -13,7 +13,7 @@ grid build kernels on a grid and queries written by this file; the reference her
 
 Contracts, bit for bit on keys and positions:
   knn_search (dense)  the 5 smallest keys of the cube, padded with knn_key(3e38, 0x7fffffff)
-  knn_search (hash)   the dense result
+  knn_search (sparse) the dense result
   knn_search_lb       the 7 smallest keys of the cube below knn_key(B, 0x7fffffff) (d2 == B with a real index is kept),
                       padded with that sentinel at position -1; positions are pos_of[index]
   knn_warp_search     got == (cube points with d2 <= B) <= 64; when got, knn_search_lb's list; with the row table
@@ -307,7 +307,7 @@ def read_output(path, nq, nrr):
         at += a.nbytes
         return a.reshape(shape) if shape else a
 
-    out = {"knn5": take(np.uint64, nq * 5, (nq, 5)), "knn5h": take(np.uint64, nq * 5, (nq, 5)),
+    out = {"knn5": take(np.uint64, nq * 5, (nq, 5)), "knn5s": take(np.uint64, nq * 5, (nq, 5)),
            "lb_keys": take(np.uint64, nq * 7, (nq, 7)), "lb_pos": take(np.int32, nq * 7, (nq, 7)), "lb": take(F, nq)}
     for w in ("warp", "pre"):
         out[w] = {"got": take(np.int32, nq), "keys": take(np.uint64, nq * 7, (nq, 7)),
@@ -372,12 +372,12 @@ def test_searches_match_brute_force(harness, tmp_path, name, cell):
     assert o["bounds"].tolist() == [*L.o, *(L.o + L.n3 - 1)]
     assert o["same"].tolist() == [1, 1, 1], "grid build: pts / pos_of / cell_start differ from the layout twin"
 
-    # knn_search: the cube's five smallest keys, on the dense and on the hash grid
+    # knn_search: the cube's five smallest keys, on the dense grid and on the sparse row index
     bad = (o["knn5"] != ref.knn5).any(axis=1)
     assert not bad.any(), f"knn_search: {int(bad.sum())} lists differ, first {where(bad)}: {o['knn5'][first_bad(bad)]} " \
                           f"!= {ref.knn5[first_bad(bad)]}"
-    bad = (o["knn5h"] != o["knn5"]).any(axis=1)
-    assert not bad.any(), f"knn_search on the hash grid: {int(bad.sum())} lists differ, first {where(bad)}"
+    bad = (o["knn5s"] != o["knn5"]).any(axis=1)
+    assert not bad.any(), f"knn_search on the sparse row index: {int(bad.sum())} lists differ, first {where(bad)}"
 
     # knn_search_lb: the cube's seven smallest keys inside the bound, positions, and lb
     bad = (o["lb_keys"] != ref.lb_keys).any(axis=1) | (o["lb_pos"] != ref.lb_pos).any(axis=1)

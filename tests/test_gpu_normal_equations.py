@@ -270,9 +270,9 @@ def test_shipped_cylinder_g1_g2(ctx, golden, cylinder):
 
 
 @pytest.mark.gpu
-def test_ragged_sizes_cells_and_hash_grid(ctx, cylinder):
-    """tile tails (1 tile - 1, 32 k + 1, a last block with one slot), cells of radius / 2, 3, 4 (rings 2-4) and the
-    hash-grid target"""
+def test_ragged_sizes_cells_and_sparse_index(ctx, cylinder):
+    """tile tails (1 tile - 1, 32 k + 1, a last block with one slot), cells of radius / 2, 3, 4 (rings 2-4) and a
+    sparse-row-index target"""
     from dcreg_b200.scenes import g2_initial_pose
     T0 = g2_initial_pose()
     tree = cKDTree(cylinder.astype(np.float64))
@@ -290,8 +290,8 @@ def test_ragged_sizes_cells_and_hash_grid(ctx, cylinder):
     report("cells r/2..r/4")
     tgt = np.concatenate([cylinder, np.array([[4000.0, 4500.0, 5000.0], [-4000.0, -3000.0, 2000.0]], F)]).astype(F)
     ctx.set_target(tgt, 1.0)
-    check_run("hash grid", ctx.icp_run(prm, T0), cylinder, tgt, T0, prm)
-    report("hash grid")
+    check_run("sparse index", ctx.icp_run(prm, T0), cylinder, tgt, T0, prm)
+    report("sparse index")
 
 
 @pytest.mark.gpu

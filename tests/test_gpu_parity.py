@@ -225,7 +225,7 @@ def test_k1_linearity_at_scale(ctx):
 
 
 # ------------------------------------------------------------------------------------------------
-# seam 1: correspondences (hash-grid exact 5-NN + plane fit)
+# seam 1: correspondences (grid exact 5-NN + plane fit)
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("setup", ["G1", "G2"])
 def test_find_planes_matches_oracle(ctx, golden, cylinder, tree, setup):

@@ -206,11 +206,10 @@ def test_scans_bad_arguments(ctx, scene, cylinder):
     with pytest.raises(api.DcregError) as e:
         ctx.icp_run_scans(prm, [], np.zeros((0, 4, 4)))
     assert e.value.status == api.BAD_ARG
-    # a hash-grid target (bounding box too large for a dense grid at this cell size)
+    # a target too large for a dense grid at this cell size: a sparse row index, which the call runs on
     far = np.concatenate([cylinder, cylinder + np.float32(4.0e4)])
     ctx.set_target(far, RADIUS)
-    assert call() == api.BAD_ARG
-    assert "dense" in lib.dcreg_last_error(h).decode()
+    assert call() == api.OK
     # no target at all; a sharded context (a one-rank communicator)
     from dcreg_b200 import Context
     with Context(0) as fresh:

@@ -1,12 +1,14 @@
-"""dcreg_set_target_sparse: the sparse row index for maps too large for a dense grid (sparse_index.hpp).
+"""dcreg_set_target past the dense-grid limit, and its alias dcreg_set_target_sparse: the sparse row index for maps too
+large for a dense grid (sparse_index.hpp).
 
 Target B is a parking map (plus four points at its far corners that stretch its box in z over every query): a dense grid.
 Target A is B plus two far points that sort after every map cell and come last in index, which lifts A's box past 2^27
 cells: a sparse row index whose points and positions are B's, followed by the two.  For sources whose query cells stay
 inside B's box, every call on A must equal the same call on B bit for bit - T, T_prior, status, iterations, converged,
-cov and every log record but its iter_time_ms - and find_planes must too.  On the 4 x 4 tile map (make_large_map) every
-scan and sequence frame equals its own single run on the same sparse target, as the batched calls' contracts state, and
-a call reproduces bit for bit.
+cov and every log record but its iter_time_ms - and find_planes must too; A built by dcreg_set_target and by
+dcreg_set_target_sparse is the same build (launches) and gives the same bits.  On the 4 x 4 tile map (make_large_map)
+every scan and sequence frame equals its own single run on the same sparse target, as the batched calls' contracts
+state, and a call reproduces bit for bit.
 """
 import ctypes as C
 
@@ -125,16 +127,19 @@ def test_find_planes_sparse_equals_dense(ctx, scene):
 
 @pytest.mark.parametrize("method", ["Ours", "ME-TSVD"])
 def test_every_call_sparse_equals_dense(ctx, scene, method):
-    """icp_run (with its log), enqueue / fetch, _batch, _scans and _sequences on A equal the same calls on B bit for bit."""
+    """icp_run (with its log), enqueue / fetch, _batch, _scans and _sequences on A equal the same calls on B bit for bit;
+    on A from set_target they equal those on A from set_target_sparse, after a build of the same launches."""
     from dcreg_b200.scenes import trial_poses
     frames, _, T_init, A, B = scene
     prm = params(method)
     trials = T_init[3] @ trial_poses(6, seed=73, max_trans=0.2, max_rot_deg=1.0)
     seqs = [frames[0:4], frames[4:8], frames[8:12]]
     deltas = np.array([np.linalg.inv(T_init[k]) @ T_init[min(k + 1, 11)] for k in range(12)])
-    out = {}
-    for name, tgt in (("B", B), ("A", A)):
-        ctx.set_target(tgt, RADIUS) if name == "B" else ctx.set_target_sparse(tgt, RADIUS)
+    out, builds = {}, {}
+    for name, tgt, build in (("B", B, ctx.set_target), ("A", A, ctx.set_target_sparse), ("A2", A, ctx.set_target)):
+        n0 = ctx.launch_count
+        build(tgt, RADIUS)
+        builds[name] = ctx.launch_count - n0
         ctx.set_source(frames[3])
         r = dict(single=ctx.icp_run(prm, T_init[3]))
         ctx.icp_enqueue(prm, T_init[3])
@@ -153,6 +158,15 @@ def test_every_call_sparse_equals_dense(ctx, scene, method):
             assert_identical(x, y)
     assert sum(int(x.converged) for x in b["scans"]) >= 8     # the runs do real work
     assert b["single"].iterations > 2
+    a2 = out["A2"]
+    assert builds["A2"] == builds["A"]
+    assert_identical(a2["single"], a["single"])
+    assert a2["fetch"].T.tobytes() == a["fetch"].T.tobytes()
+    assert (a2["fetch"].iterations, a2["fetch"].converged) == (a["fetch"].iterations, a["fetch"].converged)
+    for k in ("batch", "scans", "seqs"):
+        assert len(a2[k]) == len(a[k])
+        for x, y in zip(a2[k], a[k]):
+            assert_identical(x, y)
 
 
 def test_bad_arguments(ctx, scene):

@@ -1,5 +1,5 @@
-"""Frames/s of localisation against maps too large for a dense grid (dcreg_set_target_sparse), against the dense grid
-and against the only route such maps had before: dcreg_set_target's hash table and the per-frame loop.
+"""Frames/s of localisation against maps too large for a dense grid (their sparse row index), in the batched calls against
+the dense grid, and against the per-frame loop.
 
 Arms (radius = cell = 0.5, 30 iterations, ROT 1e-5 / TRANS 1e-3 (icp_pk01.yaml), method Ours):
   (a) dense : the 0.5 M-point parking map, dense grid; --frames frames of make_parking_frames as one dcreg_icp_run_scans
@@ -10,8 +10,8 @@ Arms (radius = cell = 0.5, 30 iterations, ROT 1e-5 / TRANS 1e-3 (icp_pk01.yaml),
   (c) large : make_large_map (4 x 4 parking maps 1 km apart, --tile-points each, 2.7e8 cells of box) on the sparse index,
               --frames frames of make_large_map_frames as one _scans call and as one _sequences call (a sequence per
               tile, its increments from the true poses);
-  (d) hash  : the large map through dcreg_set_target (its hash table) and the per-frame dcreg_set_source +
-              dcreg_icp_run loop over (c)'s frames.
+  (d) loop  : the large map through dcreg_set_target (the same sparse index as (c)) and the per-frame dcreg_set_source
+              + dcreg_icp_run loop over (c)'s frames.
 Calls are timed as tools/bench_scans.py times them (the max of CUDA events on the context's stream and the host wall
 clock, host arrays in, results out, after a warm-up), --runs times, medians reported.  The sparse index's device bytes
 (points, positions and table, computed from the build rule) are reported against the dense tables' 12 B per cell of the
@@ -146,11 +146,11 @@ def main():
                 ctx.set_source(f)
                 res.append(ctx.icp_run(prm, T, want_log=False))
             return res
-        arm("d_hash_frame_loop", n, frame_loop)
+        arm("d_frame_loop", n, frame_loop)
     out["index_parking_sparse"] = index_bytes(park_far, RADIUS)
     out["index_large"] = index_bytes(big, RADIUS)
-    out["speedup_c_scans_vs_d"] = out["c_sparse_scans"]["frames_per_s"] / out["d_hash_frame_loop"]["frames_per_s"]
-    out["speedup_c_sequences_vs_d"] = out["c_sparse_sequences"]["frames_per_s"] / out["d_hash_frame_loop"]["frames_per_s"]
+    out["speedup_c_scans_vs_d"] = out["c_sparse_scans"]["frames_per_s"] / out["d_frame_loop"]["frames_per_s"]
+    out["speedup_c_sequences_vs_d"] = out["c_sparse_sequences"]["frames_per_s"] / out["d_frame_loop"]["frames_per_s"]
     line = {"metric": "frames_per_s", "frames": n, "lanes": L, "tile_points": args.tile_points, **out, "card": card()}
     print(json.dumps(line))
     if args.dump_outputs:

@@ -1,7 +1,7 @@
 // Host check of arena_plan.hpp (tests/test_arena_plan.py): the planning of a grid arena, the dense grids of many
 // clouds in one set of buffers (dcreg_icp_run_pairs).  Per-cloud boxes and dims from the bounds, cell offsets that
 // follow each other, the +-2^19 cell range, the dense-cell limit per cloud and in total, the one-cloud decision of the
-// context's target (dense, hash table or error), the offset tables; and a replay of the arena's grouping (one stable
+// context's target (dense, sparse row index or error), the offset tables; and a replay of the arena's grouping (one stable
 // order by global cell id) against every cloud grouped alone.
 #include <algorithm>
 #include <cstdio>
@@ -69,7 +69,7 @@ int main() {
         int big[6] = {0, 0, 0, 1023, 1023, 128};
         const std::string why = arena_plan::plan(1, big, boxes, &cells, "cloud");
         CHECK(why.find("dense") != std::string::npos && why.find("cloud 0") != std::string::npos);
-        // the same limit for the context's target alone, where one row more means the hash table, not an error
+        // the same limit for the context's target alone, where one row more means a sparse row index, not an error
         arena_plan::Box one;
         CHECK(arena_plan::box_of(ok, &one) == arena_plan::kDense && one.cells == (1ll << 27));
         CHECK(one.ox == 0 && one.nx == 1024 && one.ny == 1024 && one.nz == 128 && one.cell_off == 0);

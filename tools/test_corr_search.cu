@@ -5,8 +5,8 @@
 // The input is one grid and a list of queries: the target points in their original order, the dense grid layout the
 // test computed for them (points grouped by cell, x-fastest cells, ascending index inside a cell), and per query its
 // position and squared bound B.  The harness runs the production device functions on it, unchanged:
-//   knn_search      one thread per query, on the dense grid and on a hash grid of the same points (built here on the
-//                   host with corr::pack_key / corr::hash_key);
+//   knn_search      one thread per query, on the dense grid and on the sparse row index of the same points (built
+//                   here with the production build, build_sparse);
 //   knn_search_lb   one thread per query, bound B, starting lb = r2_up * 0.9999 (as icp_iter2_kernel);
 //   knn_warp_search one warp per query, rows set up by the search itself and, when rings == 1, also from a table of
 //                   rows every thread set up beforehand with knn_row_range (the loop kernel's `pre` path);
@@ -15,10 +15,12 @@
 // and builds the dense grid again from the raw points with corr.cuh's build kernels (bounds, count, three-phase scan,
 // scatter, rank; the order of arena_fill for one cloud), reporting whether the result is byte-identical to the input
 // layout.  Binary formats: see read_input / the writes at the end of main (little-endian, no padding).
+#include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
+#include <cub/device/device_radix_sort.cuh>
 #include "../dcreg_b200/csrc/corr.cuh"
 
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { fprintf(stderr, "CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); exit(2); } } while (0)
@@ -92,14 +94,14 @@ static std::vector<T> download(const T* d, size_t count) {
 
 struct ThreadOut {
     unsigned long long* knn5;     // [nq][5] dense knn_search
-    unsigned long long* knn5h;    // [nq][5] hash knn_search
+    unsigned long long* knn5s;    // [nq][5] sparse knn_search
     unsigned long long* lbk;      // [nq][7] knn_search_lb
     int* lbp;                     // [nq][7]
     float* lbv;                   // [nq]
     float* nn1;                   // [nq]
 };
 
-__global__ void thread_searches_kernel(corr::Grid g, corr::Grid h, const float* __restrict__ q, const float* __restrict__ B,
+__global__ void thread_searches_kernel(corr::Grid g, corr::Grid s, const float* __restrict__ q, const float* __restrict__ B,
                                        int nq, float lb0, ThreadOut o) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= nq) return;
@@ -109,8 +111,8 @@ __global__ void thread_searches_kernel(corr::Grid g, corr::Grid h, const float* 
     corr::knn_search(g, qx, qy, qz, k);
     for (int j = 0; j < 5; ++j) o.knn5[5 * (size_t)i + j] = k.key[j];
     corr::knn_init(k);
-    corr::knn_search(h, qx, qy, qz, k);
-    for (int j = 0; j < 5; ++j) o.knn5h[5 * (size_t)i + j] = k.key[j];
+    corr::knn_search<true>(s, qx, qy, qz, k);
+    for (int j = 0; j < 5; ++j) o.knn5s[5 * (size_t)i + j] = k.key[j];
     corr::KnnM m;
     float lb = lb0;
     corr::knn_search_lb(g, qx, qy, qz, B[i], m, lb);
@@ -165,47 +167,6 @@ __global__ void warp_searches_kernel(corr::Grid g, const float* __restrict__ q, 
     }
 }
 
-// hash grid of the same points, built on the host (the layout build_hash_grid makes: points grouped by slot, ascending
-// index inside a slot)
-struct HostHash {
-    std::vector<unsigned long long> keys;
-    std::vector<int> start, count;
-    std::vector<float4> pts;
-    unsigned mask;
-};
-static HostHash build_hash(const Input& in) {
-    HostHash H;
-    long long cap = 1024;
-    while (cap < 2ll * in.n) cap <<= 1;
-    H.mask = (unsigned)(cap - 1);
-    H.keys.assign((size_t)cap, corr::kEmptyKey);
-    H.start.assign((size_t)cap, 0);
-    H.count.assign((size_t)cap, 0);
-    std::vector<int> slot_of((size_t)in.n);
-    for (int i = 0; i < in.n; ++i) {
-        const float* p = &in.xyz[3 * (size_t)i];
-        const unsigned long long key = corr::pack_key(corr::cell_coord(p[0], in.inv_cell), corr::cell_coord(p[1], in.inv_cell),
-                                                      corr::cell_coord(p[2], in.inv_cell));
-        unsigned slot = corr::hash_key(key) & H.mask;
-        while (H.keys[slot] != corr::kEmptyKey && H.keys[slot] != key) slot = (slot + 1) & H.mask;
-        H.keys[slot] = key;
-        slot_of[(size_t)i] = (int)slot;
-        H.count[slot]++;
-    }
-    int run = 0;
-    for (long long s = 0; s < cap; ++s) { H.start[(size_t)s] = run; run += H.count[(size_t)s]; }
-    std::vector<int> fill((size_t)cap, 0);
-    H.pts.resize((size_t)in.n);
-    for (int i = 0; i < in.n; ++i) {
-        const int s = slot_of[(size_t)i];
-        float4 p;
-        p.x = in.xyz[3 * (size_t)i]; p.y = in.xyz[3 * (size_t)i + 1]; p.z = in.xyz[3 * (size_t)i + 2];
-        memcpy(&p.w, &i, sizeof(int));
-        H.pts[(size_t)(H.start[(size_t)s] + fill[(size_t)s]++)] = p;
-    }
-    return H;
-}
-
 // corr.cuh's build kernels on the raw points, in arena_fill's order for one cloud; flags: pts, pos_of, cell_start
 // byte-identical to the input layout
 static void grid_build_check(const Input& in, int (&bounds)[6], int (&same)[3]) {
@@ -248,7 +209,7 @@ static void grid_build_check(const Input& in, int (&bounds)[6], int (&same)[3]) 
     corr::scan_tile_offsets_kernel<<<1, 1024>>>(tile_sums, ntiles);
     corr::scan_tile_apply_kernel<<<ntiles, 256>>>(counts, (int)ns, tile_sums, start);
     corr::grid_scatter_kernel<<<nb, 256>>>(d_raw, in.n, pt_cell, start, fill, tmp, 0);
-    corr::grid_rank_cells_kernel<<<nb, 256>>>(tmp, in.n, pt_cell, start, nullptr, out, pos_of);
+    corr::grid_rank_cells_kernel<<<nb, 256>>>(tmp, in.n, pt_cell, start, out, pos_of);
     CK(cudaGetLastError());
     CK(cudaDeviceSynchronize());
     const std::vector<float4> hp = download(out, (size_t)in.n);
@@ -259,6 +220,60 @@ static void grid_build_check(const Input& in, int (&bounds)[6], int (&same)[3]) 
     for (void* p : {(void*)d_raw, (void*)d_seg, (void*)d_bounds, (void*)d_grids, (void*)d_cell_off, (void*)counts, (void*)fill,
                     (void*)start, (void*)pt_cell, (void*)tmp, (void*)out, (void*)pos_of, (void*)tile_sums})
         cudaFree(p);
+}
+
+// The sparse row index of the same points (box: the dense layout's g), built with the production build as
+// build_sparse_arena runs it on a one-cloud arena: corr::sparse_seg_key_kernel and a stable radix sort over (y, x), then
+// over (cloud, z); sparse_seg_gather_kernel, sparse_seg_count_kernel, sparse_index::layout, sparse_seg_insert_kernel.
+// check: pts identical and pos_of identical to the dense layout, table entries.
+static corr::Grid build_sparse(const Input& in, const corr::Grid& g, int (&check)[3]) {
+    const int n = in.n;
+    std::vector<float4> raw((size_t)n);
+    for (int i = 0; i < n; ++i) raw[(size_t)i] = make_float4(in.xyz[3 * (size_t)i], in.xyz[3 * (size_t)i + 1], in.xyz[3 * (size_t)i + 2], 0.0f);
+    float4* d_raw = upload(raw);
+    corr::Grid s = g;
+    s.dense = corr::kSparseGrid; s.cell_start = nullptr;
+    s.pts = alloc<float4>((size_t)n); s.pos_of = alloc<int>((size_t)n);
+    const long long* d_seg = upload(std::vector<long long>{0, n});
+    corr::Grid* d_grids = upload(std::vector<corr::Grid>{s});
+    unsigned long long* keys = alloc<unsigned long long>(2 * (size_t)n);
+    int* vals = alloc<int>(2 * (size_t)n);
+    // each pass sorts the bits of its largest key: (y, x) of the box's far corner, (cloud 0, z) of its top
+    const unsigned long long top[2] = {sparse_index::key(s.nx - 1, s.ny - 1, 0), (unsigned long long)(s.nz - 1)};
+    int end_bit[2] = {1, 1};
+    for (int p = 0; p < 2; ++p)
+        while (end_bit[p] < 64 && top[p] >> end_bit[p]) ++end_bit[p];
+    size_t tmp0 = 0, tmp1 = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp0, keys, keys + n, vals, vals + n, n, 0, end_bit[0]));
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp1, keys, keys + n, vals, vals + n, n, 0, end_bit[1]));
+    size_t tmp = std::max(tmp0, tmp1);
+    unsigned char* d_tmp = alloc<unsigned char>(tmp);
+    const unsigned nb = (unsigned)((n + 255) / 256);
+    for (int pass = 0; pass < 2; ++pass) {
+        corr::sparse_seg_key_kernel<<<nb, 256>>>(d_raw, n, d_seg, 1, d_grids, pass, vals + n, keys, vals);
+        CK(cub::DeviceRadixSort::SortPairs(d_tmp, tmp, keys, keys + n, vals, vals + n, n, 0, end_bit[pass]));
+    }
+    unsigned long long* sorted = keys;                           // (the passes' input keys are spent)
+    corr::sparse_seg_gather_kernel<<<nb, 256>>>(d_raw, vals + n, n, d_seg, 1, d_grids, s.pts, s.pos_of, sorted);
+    unsigned long long* d_entries = alloc<unsigned long long>(1);
+    corr::sparse_seg_count_kernel<<<nb, 256>>>(sorted, n, d_seg, 1, d_grids, d_entries);
+    CK(cudaGetLastError());
+    const unsigned long long entries = download(d_entries, 1)[0];
+    long long cap, off[2];
+    if (sparse_index::layout(1, &entries, &cap, off) >= 0) { fprintf(stderr, "sparse index over 2^32 slots\n"); exit(2); }
+    s.keys = alloc<unsigned long long>((size_t)cap);
+    CK(cudaMemset(s.keys, 0xff, (size_t)cap * sizeof(unsigned long long)));
+    s.hstart = alloc<int>((size_t)cap); s.mask = (unsigned)(cap - 1);
+    CK(cudaMemcpy(d_grids, &s, sizeof(s), cudaMemcpyHostToDevice));
+    corr::sparse_seg_insert_kernel<<<nb, 256>>>(sorted, n, d_seg, 1, d_grids);
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    const std::vector<float4> sp = download(s.pts, (size_t)n);
+    const std::vector<int> spos = download(s.pos_of, (size_t)n);
+    check[0] = memcmp(sp.data(), in.pts.data(), sp.size() * sizeof(float4)) == 0;
+    check[1] = memcmp(spos.data(), in.pos_of.data(), spos.size() * sizeof(int)) == 0;
+    check[2] = (int)entries;
+    return s;
 }
 
 template <class T>
@@ -279,11 +294,8 @@ int main(int argc, char** argv) {
     g.pts = upload(in.pts); g.pos_of = upload(in.pos_of); g.n = in.n; g.dense = 1; g.rings = in.rings;
     g.inv_cell = in.inv_cell; g.ox = in.ox; g.oy = in.oy; g.oz = in.oz; g.nx = in.nx; g.ny = in.ny; g.nz = in.nz;
     g.cell_start = upload(in.cell_start);
-
-    const HostHash H = build_hash(in);
-    corr::Grid h{};
-    h.pts = upload(H.pts); h.pos_of = nullptr; h.n = in.n; h.dense = 0; h.rings = in.rings; h.inv_cell = in.inv_cell;
-    h.keys = upload(H.keys); h.hstart = upload(H.start); h.hcount = upload(H.count); h.mask = H.mask;
+    int sparse_check[3];
+    const corr::Grid s = build_sparse(in, g, sparse_check);
 
     float* d_q = upload(in.q);
     float* d_B = upload(in.B);
@@ -291,7 +303,7 @@ int main(int argc, char** argv) {
 
     ThreadOut to{alloc<unsigned long long>(nq_ * 5), alloc<unsigned long long>(nq_ * 5), alloc<unsigned long long>(nq_ * 7),
                  alloc<int>(nq_ * 7), alloc<float>(nq_), alloc<float>(nq_)};
-    thread_searches_kernel<<<(nq + 127) / 128, 128>>>(g, h, d_q, d_B, nq, lb0, to);
+    thread_searches_kernel<<<(nq + 127) / 128, 128>>>(g, s, d_q, d_B, nq, lb0, to);
     CK(cudaGetLastError());
 
     const unsigned wblocks = (unsigned)((nq + kWarpsPerBlock - 1) / kWarpsPerBlock);
@@ -313,14 +325,14 @@ int main(int argc, char** argv) {
     int bounds[6], same[3];
     grid_build_check(in, bounds, same);
 
-    // output: knn5, knn5h (uint64 [nq][5]); lb search keys (uint64 [nq][7]), positions (int32 [nq][7]), lb (float32
+    // output: knn5, knn5s (uint64 [nq][5]); lb search keys (uint64 [nq][7]), positions (int32 [nq][7]), lb (float32
     // [nq]); warp search got (int32 [nq]), keys, positions, lb; the same four with the row table (zeros unless
     // rings == 1); nn1 (float32 [nq]); row pairs (int32 [nrr][3]: s, e, bits of lb); grid build: bounds (int32 [6]),
     // identical pts / pos_of / cell_start (int32 [3])
     FILE* f = fopen(argv[2], "wb");
     if (!f) { fprintf(stderr, "cannot write %s\n", argv[2]); return 2; }
     write(f, download(to.knn5, nq_ * 5));
-    write(f, download(to.knn5h, nq_ * 5));
+    write(f, download(to.knn5s, nq_ * 5));
     write(f, download(to.lbk, nq_ * 7));
     write(f, download(to.lbp, nq_ * 7));
     write(f, download(to.lbv, nq_));

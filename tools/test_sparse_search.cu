@@ -3,11 +3,9 @@
 //   test_sparse_search <input> <output>
 //
 // The input is tools/test_corr_search.cu's: the target points, their dense grid layout and the queries.  The harness
-// builds the sparse row index of the same points with the production build, as build_sparse_arena runs it on a one-cloud
-// arena (corr::sparse_seg_key_kernel and a stable radix sort over (y, x), then over (cloud, z); sparse_seg_gather_kernel,
-// sparse_seg_count_kernel, sparse_index::layout, sparse_seg_insert_kernel) and reports whether its points and positions
-// are byte-identical to the dense layout.  Then it runs the searches of corr.cuh on the
-// dense grid and on the sparse index (their kSparse instantiations), unchanged: knn_search, knn_search_lb,
+// builds the sparse row index of the same points with the production build (test_corr_search.cu's build_sparse) and
+// reports whether its points and positions are byte-identical to the dense layout.  Then it runs the searches of
+// corr.cuh on the dense grid and on the sparse index (their kSparse instantiations), unchanged: knn_search, knn_search_lb,
 // knn_warp_search without and (rings == 1) with the loop kernel's row table, and knn_row_range on the listed pairs.
 // Output: the sparse build check (int32 [3]: pts identical, pos_of identical, table entries), then for the dense grid
 // and then the sparse index: knn5 (uint64 [nq][5]), the bounded list keys (uint64 [nq][7]), positions (int32 [nq][7]),
@@ -15,7 +13,6 @@
 // and the row pairs (int32 [nrr][3]: s, e, bits of lb).
 #define CORR_SEARCH_NO_MAIN
 #include "test_corr_search.cu"
-#include <cub/device/device_radix_sort.cuh>
 
 struct Out {
     unsigned long long* knn5;     // [nq][5]
@@ -131,52 +128,9 @@ int main(int argc, char** argv) {
     g.inv_cell = in.inv_cell; g.ox = in.ox; g.oy = in.oy; g.oz = in.oz; g.nx = in.nx; g.ny = in.ny; g.nz = in.nz;
     g.cell_start = upload(in.cell_start);
 
-    // the sparse row index of the same points, built as build_sparse_arena builds a one-cloud arena (box: the dense
-    // layout's)
-    std::vector<float4> raw((size_t)n);
-    for (int i = 0; i < n; ++i) raw[(size_t)i] = make_float4(in.xyz[3 * (size_t)i], in.xyz[3 * (size_t)i + 1], in.xyz[3 * (size_t)i + 2], 0.0f);
-    float4* d_raw = upload(raw);
-    corr::Grid s = g;
-    s.dense = corr::kSparseGrid; s.cell_start = nullptr;
-    s.pts = alloc<float4>((size_t)n); s.pos_of = alloc<int>((size_t)n);
-    const long long* d_seg = upload(std::vector<long long>{0, n});
-    corr::Grid* d_grids = upload(std::vector<corr::Grid>{s});
-    unsigned long long* keys = alloc<unsigned long long>(2 * (size_t)n);
-    int* vals = alloc<int>(2 * (size_t)n);
-    // each pass sorts the bits of its largest key: (y, x) of the box's far corner, (cloud 0, z) of its top
-    const unsigned long long top[2] = {sparse_index::key(s.nx - 1, s.ny - 1, 0), (unsigned long long)(s.nz - 1)};
-    int end_bit[2] = {1, 1};
-    for (int p = 0; p < 2; ++p)
-        while (end_bit[p] < 64 && top[p] >> end_bit[p]) ++end_bit[p];
-    size_t tmp0 = 0, tmp1 = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp0, keys, keys + n, vals, vals + n, n, 0, end_bit[0]));
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp1, keys, keys + n, vals, vals + n, n, 0, end_bit[1]));
-    size_t tmp = std::max(tmp0, tmp1);
-    unsigned char* d_tmp = alloc<unsigned char>(tmp);
-    const unsigned nb = (unsigned)((n + 255) / 256);
-    for (int pass = 0; pass < 2; ++pass) {
-        corr::sparse_seg_key_kernel<<<nb, 256>>>(d_raw, n, d_seg, 1, d_grids, pass, vals + n, keys, vals);
-        CK(cub::DeviceRadixSort::SortPairs(d_tmp, tmp, keys, keys + n, vals, vals + n, n, 0, end_bit[pass]));
-    }
-    unsigned long long* sorted = keys;                           // (the passes' input keys are spent)
-    corr::sparse_seg_gather_kernel<<<nb, 256>>>(d_raw, vals + n, n, d_seg, 1, d_grids, s.pts, s.pos_of, sorted);
-    unsigned long long* d_entries = alloc<unsigned long long>(1);
-    corr::sparse_seg_count_kernel<<<nb, 256>>>(sorted, n, d_seg, 1, d_grids, d_entries);
-    CK(cudaGetLastError());
-    const unsigned long long entries = download(d_entries, 1)[0];
-    long long cap, off[2];
-    if (sparse_index::layout(1, &entries, &cap, off) >= 0) { fprintf(stderr, "sparse index over 2^32 slots\n"); return 2; }
-    s.keys = alloc<unsigned long long>((size_t)cap);
-    CK(cudaMemset(s.keys, 0xff, (size_t)cap * sizeof(unsigned long long)));
-    s.hstart = alloc<int>((size_t)cap); s.hcount = nullptr; s.mask = (unsigned)(cap - 1);
-    CK(cudaMemcpy(d_grids, &s, sizeof(s), cudaMemcpyHostToDevice));
-    corr::sparse_seg_insert_kernel<<<nb, 256>>>(sorted, n, d_seg, 1, d_grids);
-    CK(cudaGetLastError());
-    CK(cudaDeviceSynchronize());
-    const std::vector<float4> sp = download(s.pts, (size_t)n);
-    const std::vector<int> spos = download(s.pos_of, (size_t)n);
-    const int check[3] = {memcmp(sp.data(), in.pts.data(), sp.size() * sizeof(float4)) == 0,
-                          memcmp(spos.data(), in.pos_of.data(), spos.size() * sizeof(int)) == 0, (int)entries};
+    // the sparse row index of the same points
+    int check[3];
+    const corr::Grid s = build_sparse(in, g, check);
 
     float* d_q = upload(in.q);
     float* d_B = upload(in.B);
@@ -190,6 +144,6 @@ int main(int argc, char** argv) {
     write_out(f, od, in);
     write_out(f, os, in);
     fclose(f);
-    printf("SPARSE_SEARCH_DONE %d queries, %d row pairs, %llu entries\n", in.nq, in.nrr, entries);
+    printf("SPARSE_SEARCH_DONE %d queries, %d row pairs, %d entries\n", in.nq, in.nrr, check[2]);
     return 0;
 }
