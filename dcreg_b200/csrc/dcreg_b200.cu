@@ -22,9 +22,11 @@
 #include <string.h>
 
 #include <algorithm>
+#include <array>
 #include <cstddef>
 #include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/dcreg_b200.h"
@@ -284,14 +286,14 @@ struct Iter2Args {
     // null: every trial runs the it.n slots of it.src, with record slices [b][it.n] and the one src_radius
     const long long* seg;
     // many scan/target pairs (dcreg_icp_run_pairs, with seg): trial b searches its own target grid grids[b] (device
-    // memory, rings set) instead of it.grid.  Only the icp_iter2_kernel<., true, .> instantiation reads it
+    // memory, rings set) instead of it.grid.  Only the kGrids instantiations read it
     const corr::Grid* grids;
     // sequences of frames (dcreg_icp_run_sequences, with seg: the frames' slot ranges): grid y is the lane, the trial the
-    // frame seq.cursor[lane].  Only the icp_iter2_kernel<., ., true> instantiation reads it
+    // frame seq.cursor[lane].  Only the kSeq instantiations read it
     SeqView seq;
     // odometry with the adaptive threshold (dcreg_icp_run_odometry_adaptive): [lanes] the search radius of the frame each
     // lane runs at this step, in device memory (a captured chunk freezes its arguments), or null: prm.search_radius.
-    // Only the icp_iter2_kernel<., true, true> instantiation reads it
+    // Only the kGrids && kSeq instantiations read it
     const double* lane_radius;
     // per-lane solver settings (dcreg_set_lane_params): [lanes] in device memory, grid y's entry lane_prm[ys], or with
     // lane_seq (odometry, whose steps compact the lanes) lane_prm[lane_seq[ys]]; null: it.prm for every lane.  Only a
@@ -711,15 +713,13 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     }
 }
 
-// dynamic shared memory of the loop kernel: the per-trial grid copy (Iter2Smem::grid, the last member) only where the
-// kernel reads it
-constexpr size_t kIter2SmemNoGrid = offsetof(Iter2Smem, grid);
-constexpr size_t kIter2SmemGrid = offsetof(Iter2Smem, radius);      // ... and odometry's radius fields only there
+// A kernel instantiation and the dynamic shared memory it is launched with
+template <typename Args>
+struct KernelEntry { void (*kernel)(Args); size_t smem; };
+using LoopKernel = KernelEntry<Iter2Args>;
 
-template <bool kUseWd, bool kGrids, bool kSeq, bool kPlanes = false, bool kSparse = false>
-cudaError_t loop_kernel_attributes(size_t smem) {
-    cudaError_t e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids, kSeq, kPlanes, kSparse>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+static cudaError_t loop_kernel_attributes(const LoopKernel& k) {
+    cudaError_t e = cudaFuncSetAttribute(k.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem);
     // the smallest shared-memory carveout that keeps 3 blocks resident (each also reserves 1 KB), so that the rest of the
     // SM's unified data cache is L1 for the searches' and certificates' target reads.  The percentage is of the largest
     // carveout and is rounded up to the next capacity the SM supports.
@@ -727,10 +727,9 @@ cudaError_t loop_kernel_attributes(size_t smem) {
     if (e == cudaSuccess) e = cudaGetDevice(&dev);
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
     if (e == cudaSuccess) {
-        const size_t need = 3 * (smem + 1024);
+        const size_t need = 3 * (k.smem + 1024);
         const int pct = (int)std::min<size_t>(100, (need * 100 + (size_t)max_smem - 1) / (size_t)max_smem);
-        e = cudaFuncSetAttribute(icp_iter2_kernel<kUseWd, kGrids, kSeq, kPlanes, kSparse>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                 pct);
+        e = cudaFuncSetAttribute(k.kernel, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
     }
     return e;
 }
@@ -1505,7 +1504,7 @@ struct dcreg_ctx {
     DevBuf<unsigned int> d_n_active;      // trials still running
     DevBuf<double> d_T_init;
     DevBuf<dcreg_iter_log> d_log;         // records, [trials][log_cap of the run]
-    bool loop_attr_done = false, k1_attr_done[8] = {false, false, false, false, false, false, false, false};
+    bool loop_attr_done = false, k1_attr_done[4] = {};     // k1: one per kReduceKernels entry
     // CUDA graphs of one chunk of loop iterations, keyed on the kernel arguments (a few shapes alternate in practice:
     // with / without a log, one trial / a batch); most recently used first
     struct LoopGraph { std::vector<unsigned char> key; cudaGraphExec_t exec; };
@@ -1702,36 +1701,34 @@ int upload_points(dcreg_ctx* ctx, const float* xyz, long long n, int stride, con
     return DCREG_OK;
 }
 
-template <typename PlaneT, bool kUseWd, int kTeamCtas>
-int launch_reduce_k(dcreg_ctx* ctx, k1s::Args& a, int g) {
-    auto kern = k1s::reduce_stream_kernel<PlaneT, kUseWd, kTeamCtas>;
-    const size_t smem = sizeof(k1s::Smem<PlaneT>);
-    // function attributes are per device: one flag per context (= per device) and kernel variant, not per process
-    bool& configured = ctx->k1_attr_done[(sizeof(PlaneT) == 32 ? 2 : 0) + (kUseWd ? 1 : 0)];
-    if (!configured) {
-        CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CK(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-        configured = true;
-    }
-    kern<<<g, k1s::kThreads, smem, ctx->stream>>>(a);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    return DCREG_OK;
-}
+// The K1 streaming reduction's instantiations, entry (f64 planes ? 2 : 0) + (weight derivative ? 1 : 0).  Team size
+// (k1_stream.cuh): 1 CTA per contiguous range; larger teams were no faster during development (not re-measured on H100)
+using ReduceKernel = KernelEntry<k1s::Args>;
+static constexpr ReduceKernel kReduceKernels[] = {
+    {k1s::reduce_stream_kernel<float4, false, 1>, sizeof(k1s::Smem<float4>)},
+    {k1s::reduce_stream_kernel<float4, true, 1>, sizeof(k1s::Smem<float4>)},
+    {k1s::reduce_stream_kernel<double4, false, 1>, sizeof(k1s::Smem<double4>)},
+    {k1s::reduce_stream_kernel<double4, true, 1>, sizeof(k1s::Smem<double4>)},
+};
+static_assert(std::size(kReduceKernels) == sizeof(dcreg_ctx::k1_attr_done), "one attribute flag per K1 kernel");
 
-template <typename PlaneT, bool kUseWd>
-int launch_reduce_t(dcreg_ctx* ctx, k1s::Args& a) {
-    // persistent grid: every SM holds 2 CTAs (launch bounds; 2 x (32 KB / 48 KB ring) fits H100's 227 KB carveout)
-    const long long nchunks = (a.n + 31) / 32;
-    long long g = (long long)ctx->sm_count * 2;
-    const long long need = (nchunks + k1s::kWarpsPerBlock - 1) / k1s::kWarpsPerBlock;
-    if (g > need) g = need;
-    if (g < 1) g = 1;
-    CK(ctx->d_partials.ensure(g * kPartialDoubles));
-    a.partials = ctx->d_partials;
-    // team size (k1_stream.cuh): 1 CTA per contiguous range; larger teams were no faster during development (not re-measured on H100)
-    return launch_reduce_k<PlaneT, kUseWd, 1>(ctx, a, (int)g);
+// The loop kernel's instantiations, entry v = loop_plan variant v, with the bytes of its loop_plan::smem_class.  Defined
+// after every kernel: where a template kernel is instantiated sets the order of the module's functions, and with the
+// loop kernels ahead of k2_step_kernel ptxas scheduled k2_step_kernel differently
+template <int v>
+constexpr LoopKernel loop_kernel() {
+    constexpr loop_plan::Variant f = loop_plan::variant_flags(v);
+    constexpr size_t smem[] = {offsetof(Iter2Smem, grid), offsetof(Iter2Smem, radius), sizeof(Iter2Smem)};
+    static_assert(loop_plan::kSmemNoGrid == 0 && loop_plan::kSmemGrid == 1 && loop_plan::kSmemFull == 2,
+                  "smem[] is indexed by loop_plan::SmemClass");
+    return LoopKernel{icp_iter2_kernel<f.use_wd, f.grids, f.seq, f.planes, f.sparse>, smem[loop_plan::smem_class(v)]};
 }
+template <int... v>
+constexpr std::array<LoopKernel, sizeof...(v)> loop_kernel_table(std::integer_sequence<int, v...>) {
+    return {loop_kernel<v>()...};
+}
+static constexpr auto kLoopKernels = loop_kernel_table(std::make_integer_sequence<int, loop_plan::kVariants>{});
+static_assert(kLoopKernels.size() == loop_plan::kVariants, "one loop kernel per loop_plan variant");
 
 // slope / gate: dcreg_icp_params::weight_slope / weight_gate (0.9 / 0.1 in the reference, icp_test_runner.cpp:1776, 1785)
 int launch_reduce(dcreg_ctx* ctx, const float4* d_src, const void* d_plane, bool f64, long long n,
@@ -1744,8 +1741,25 @@ int launch_reduce(dcreg_ctx* ctx, const float4* d_src, const void* d_plane, bool
     a.npt_override = npt_override;
     if (ctx->peer_ok) a.peer = ctx->peer_view;                          // the sum over ranks happens inside the kernel
     a.counter = ctx->d_counter; a.acc = ctx->d_acc;
-    if (use_wd) return f64 ? launch_reduce_t<double4, true>(ctx, a) : launch_reduce_t<float4, true>(ctx, a);
-    return f64 ? launch_reduce_t<double4, false>(ctx, a) : launch_reduce_t<float4, false>(ctx, a);
+    // persistent grid: every SM holds 2 CTAs (launch bounds; 2 x (32 KB / 48 KB ring) fits H100's 227 KB carveout)
+    const long long nchunks = (a.n + 31) / 32;
+    long long g = (long long)ctx->sm_count * 2;
+    const long long need = (nchunks + k1s::kWarpsPerBlock - 1) / k1s::kWarpsPerBlock;
+    if (g > need) g = need;
+    if (g < 1) g = 1;
+    CK(ctx->d_partials.ensure(g * kPartialDoubles));
+    a.partials = ctx->d_partials;
+    const int v = (f64 ? 2 : 0) + (use_wd ? 1 : 0);
+    const ReduceKernel& k = kReduceKernels[v];
+    if (!ctx->k1_attr_done[v]) {        // function attributes are per device: per context (= per device), not per process
+        CK(cudaFuncSetAttribute(k.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem));
+        CK(cudaFuncSetAttribute(k.kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+        ctx->k1_attr_done[v] = true;
+    }
+    k.kernel<<<(int)g, k1s::kThreads, k.smem, ctx->stream>>>(a);
+    ctx->launches++;
+    CK(cudaGetLastError());
+    return DCREG_OK;
 }
 
 // Fallback exchange (no peer mapping): one ncclAllReduce of the 32 sums behind the reducing kernel.
@@ -2623,10 +2637,8 @@ struct LoopPlan {
     bool k2 = true;           // k2_step_kernel follows the iteration kernel (the step of some lanes is not folded)
     int grid_x = 1, trials = 1;
     Iter2Args b{};            // arguments of icp_iter2_kernel
-    bool use_wd = false;
-    bool grid_table = false;  // a batch whose trials search their own grids (Batch::grid_table)
+    int variant = 0;          // its instantiation (loop_plan::variant), an index into kLoopKernels
     bool lanes = false;       // a batch in sequence lanes (b.seq)
-    bool sparse = false;      // it.grid, or (grid_table) every grid of the table, is a sparse row index (kSparse)
     const float* scan_radius = nullptr;   // the lever arms of a batch's sources, or null (the context's source)
 };
 
@@ -2650,18 +2662,17 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
                           dcreg_iter_log* dlog, int log_cap, bool want_fold, LoopPlan* plan, const Batch* batch = nullptr,
                           const Lanes& lanes = Lanes{}) {
     LoopPlan& L = *plan;
-    L.trials = trials; L.use_wd = prm->use_weight_derivative != 0;
-    L.grid_table = batch && batch->grid_table;
+    L.trials = trials;
+    const bool grid_table = batch && batch->grid_table;       // the trials search their own grids
     L.lanes = batch && batch->lanes > 0;
-    L.sparse = L.grid_table ? batch->sparse : ctx->grid.dense == corr::kSparseGrid;
     L.scan_radius = batch ? ctx->d_scan_radius.p : nullptr;
     Iter2Args& b = L.b;
     IterArgs& a = b.it;
-    a.src = src; a.n = batch ? batch->total() : ctx->n_src; a.grid = L.grid_table ? corr::Grid{} : ctx->grid; a.state = ctx->d_state;
+    a.src = src; a.n = batch ? batch->total() : ctx->n_src; a.grid = grid_table ? corr::Grid{} : ctx->grid; a.state = ctx->d_state;
     a.counter = ctx->d_counter; a.acc = ctx->d_acc;
     a.planes_out = planes_out; a.prm = *prm;
     {   // rings of cells that cover the search radius (exactness of the 5-NN-within-radius rule)
-        const int rings = search_rings(prm->search_radius, L.grid_table ? batch->cell_size : ctx->cell_size);
+        const int rings = search_rings(prm->search_radius, grid_table ? batch->cell_size : ctx->cell_size);
         if (rings < 1 || rings > 4) {
             ctx->err = "search_radius / target cell_size must be in (0, 4]: rebuild the target index with a larger cell";
             return DCREG_BAD_ARG;
@@ -2677,6 +2688,9 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
         ctx->err = "batched trials need per-slot records (more than 2^29 - 1 source points, or DCREG_FUSED_SEARCH set)";
         return DCREG_BAD_ARG;
     }
+    // (seam 1 has no batch here, so the variant is one of kLoopKernels)
+    const bool sparse = grid_table ? batch->sparse : ctx->grid.dense == corr::kSparseGrid;
+    L.variant = loop_plan::variant(planes_out != nullptr, sparse, grid_table, L.lanes, prm->use_weight_derivative != 0);
     const long long slots = ctx->n_src;
     if (!lean_only) {
         // per-slot records: [trials][slots], or one slice per source at its segment offset (total slots); reallocated
@@ -2737,30 +2751,13 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
     b.seg = batch ? ctx->d_scan_seg.p : nullptr;
     // (a CUDA graph of the loop freezes this pointer, not the table: the entries are rewritten before every pairs call
     // and read at every launch, and a regrown table has a new pointer and so a new graph key)
-    b.grids = L.grid_table ? batch->grids : nullptr;
+    b.grids = grid_table ? batch->grids : nullptr;
     // lanes: trials = lanes; the frame advance, not the solve step, counts the lanes still running
     b.seq = L.lanes ? batch->seq : SeqView{};
     b.n_active = L.lanes ? nullptr : ctx->d_n_active.p;
     if (ctx->peer_ok && !planes_out) b.peer = ctx->peer_view;       // seam 1 counts this rank's slots only
     if (!ctx->loop_attr_done) {          // per device (= per context), not per process
-        CK((loop_kernel_attributes<true, false, false>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<false, false, false>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<true, true, false>)(kIter2SmemGrid));
-        CK((loop_kernel_attributes<false, true, false>)(kIter2SmemGrid));
-        CK((loop_kernel_attributes<true, false, true>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<false, false, true>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<true, true, true>)(sizeof(Iter2Smem)));
-        CK((loop_kernel_attributes<false, true, true>)(sizeof(Iter2Smem)));
-        CK((loop_kernel_attributes<false, false, false, true>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<true, false, false, false, true>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<false, false, false, false, true>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<true, false, true, false, true>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<false, false, true, false, true>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<false, false, false, true, true>)(kIter2SmemNoGrid));
-        CK((loop_kernel_attributes<true, true, false, false, true>)(kIter2SmemGrid));
-        CK((loop_kernel_attributes<false, true, false, false, true>)(kIter2SmemGrid));
-        CK((loop_kernel_attributes<true, true, true, false, true>)(sizeof(Iter2Smem)));
-        CK((loop_kernel_attributes<false, true, true, false, true>)(sizeof(Iter2Smem)));
+        for (const LoopKernel& k : kLoopKernels) CK(loop_kernel_attributes(k));
         ctx->loop_attr_done = true;
     }
     return DCREG_OK;
@@ -2770,35 +2767,8 @@ static int plan_iteration(dcreg_ctx* ctx, const dcreg_icp_params* prm, const flo
 static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
     L.b.use_seeds = ctx->nn_valid ? 1 : 0;
     ctx->nn_valid = true;
-    const dim3 grid((unsigned)L.grid_x, (unsigned)L.trials);
-    if (L.b.it.planes_out) {             // seam 1: dcreg_find_planes runs the context's grid with the default parameters
-        if (L.sparse) CK(launch_pdl(icp_iter2_kernel<false, false, false, true, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false, false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-    } else if (L.sparse && L.grid_table && L.lanes) {
-        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, true, false, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false, true, true, false, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
-    } else if (L.sparse && L.grid_table) {
-        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, false, false, true>, grid, dim3(kBlock), kIter2SmemGrid, ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false, true, false, false, true>, grid, dim3(kBlock), kIter2SmemGrid, ctx->stream, L.b));
-    } else if (L.sparse && L.lanes) {
-        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, true, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false, false, true, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-    } else if (L.sparse) {
-        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false, false, false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-    } else if (L.grid_table && L.lanes) {
-        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false, true, true>, grid, dim3(kBlock), sizeof(Iter2Smem), ctx->stream, L.b));
-    } else if (L.grid_table) {
-        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, true, false>, grid, dim3(kBlock), kIter2SmemGrid, ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false, true, false>, grid, dim3(kBlock), kIter2SmemGrid, ctx->stream, L.b));
-    } else if (L.lanes) {
-        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false, false, true>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-    } else {
-        if (L.use_wd) CK(launch_pdl(icp_iter2_kernel<true, false, false>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-        else CK(launch_pdl(icp_iter2_kernel<false, false, false>, grid, dim3(kBlock), kIter2SmemNoGrid, ctx->stream, L.b));
-    }
+    const LoopKernel& k = kLoopKernels[L.variant];
+    CK(launch_pdl(k.kernel, dim3((unsigned)L.grid_x, (unsigned)L.trials), dim3(kBlock), k.smem, ctx->stream, L.b));
     ctx->launches++;
     CK(cudaGetLastError());
     return DCREG_OK;
@@ -3117,9 +3087,9 @@ static int enqueue_iterations(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_param
         Iter2Args kb = L.b;
         kb.use_seeds = 0;
         key_bytes(key, &kb, sizeof(kb));
-        // (kSparse: another kernel; k2: whether a K2 launch follows every iteration kernel, which a mix of per-lane
-        // settings decides at the same Iter2Args)
-        const int meta[6] = {L.grid_x, L.trials, L.use_wd ? 1 : 0, iters, L.sparse ? 1 : 0, L.k2 ? 1 : 0};
+        // (the variant: the kernel, e.g. kSparse at the same Iter2Args; k2: whether a K2 launch follows every iteration
+        // kernel, which a mix of per-lane settings decides at the same Iter2Args)
+        const int meta[5] = {L.grid_x, L.trials, L.variant, iters, L.k2 ? 1 : 0};
         key_bytes(key, meta, sizeof(meta));
         key_bytes(key, prm, sizeof(*prm));
         cudaGraphExec_t exec = nullptr;

@@ -8,6 +8,7 @@
 //     cloud on an H100 (with an earlier build that could force the tile size); no effect once there is a tile per SM;
 //   * batched trials (grid y = trial) are throughput-bound: full tiles, at most 64 blocks per trial;
 //   * a batch of different scans (ragged slot counts) follows its largest scan (plan_scan_tiles).
+// Also which instantiation of the iteration kernel a plan runs (variant), with how much shared memory (smem_class).
 // tests/test_host_la.py::test_loop_tile_plan and tests/test_scan_plan.py check the invariants on the CPU.
 #pragma once
 #include <algorithm>
@@ -42,6 +43,30 @@ inline Tiles plan_tiles(long long slots, int trials, int sm_count, int block_thr
 // contributes a zero row to its scan's reduction.
 inline Tiles plan_scan_tiles(long long max_slots, int block_threads) {
     return plan_tiles(max_slots, 2, 0, block_threads);
+}
+
+// The instantiations icp_iter2_kernel<kUseWd, kGrids, kSeq, kPlanes, kSparse> a plan can run.  Variants 0-15 are the
+// loop bodies: bit 0 kUseWd, bit 1 kGrids, bit 2 kSeq, bit 3 kSparse.  16 and 17 are seam 1 (kPlanes, dcreg_find_planes)
+// on a dense grid and on a sparse index, with no grid table, no lanes and no weight derivative.
+struct Variant { bool use_wd, grids, seq, planes, sparse; };
+constexpr int kVariants = 18;
+constexpr Variant variant_flags(int v) {
+    return v < 16 ? Variant{(v & 1) != 0, (v & 2) != 0, (v & 4) != 0, false, (v & 8) != 0}
+                  : Variant{false, false, false, true, v == 17};
+}
+
+// The variant of a plan: planes_out set (seam 1), sparse row indexes, every trial its own grid (grid_table), sequence
+// lanes, the weight derivative.  -1: seam 1 of a batch, which has none (plan_iteration refuses it before it asks).
+constexpr int variant(bool planes, bool sparse, bool grid_table, bool lanes, bool use_wd) {
+    if (planes) return grid_table || lanes ? -1 : 16 + (sparse ? 1 : 0);
+    return (use_wd ? 1 : 0) + (grid_table ? 2 : 0) + (lanes ? 4 : 0) + (sparse ? 8 : 0);
+}
+
+// A variant's dynamic shared memory: Iter2Smem up to its per-trial grid copy, which only kGrids reads, up to odometry's
+// radius fields, which only kGrids && kSeq reads, or all of it
+enum SmemClass { kSmemNoGrid, kSmemGrid, kSmemFull };
+constexpr SmemClass smem_class(int v) {
+    return !variant_flags(v).grids ? kSmemNoGrid : variant_flags(v).seq ? kSmemFull : kSmemGrid;
 }
 
 }  // namespace loop_plan

@@ -571,7 +571,7 @@ def random_slots(n, T, seed):
 
 
 def cta_ranges(n, sm_count):
-    """k1_stream.cuh with launch_reduce_t's grid: each CTA's contiguous chunk range [c_lo, c_hi)"""
+    """k1_stream.cuh with launch_reduce's grid: each CTA's contiguous chunk range [c_lo, c_hi)"""
     nchunks = (n + 31) // 32
     g = max(1, min(2 * sm_count, (nchunks + WARPS - 1) // WARPS))
     per, rem = divmod(nchunks, g)

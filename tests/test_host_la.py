@@ -81,7 +81,8 @@ def test_fast_solve_step_pieces_on_the_device(tmp_path):
 
 def test_loop_tile_plan(tmp_path):
     """loop_plan.hpp (how a run's source slots are cut into blocks of the iteration kernel) as plain host C++: coverage,
-    tile bounds, resident-block cap, the small-cloud rule and the values used for the shipped cloud / C2 / C4 / C5."""
+    tile bounds, resident-block cap, the small-cloud rule and the values used for the shipped cloud / C2 / C4 / C5; and
+    which iteration-kernel instantiation and shared memory a plan runs, against launch_plan's former if-ladder."""
     gxx = shutil.which("g++")
     if not gxx:
         pytest.skip("g++ not available")
