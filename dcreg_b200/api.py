@@ -298,6 +298,76 @@ def _split_deskewed(out, npts):
     return [out[a:b].copy() for a, b in zip(at[:-1], at[1:])]
 
 
+_MOTIONS = {"increments": 0, "constant_velocity": 1}
+
+
+def _motion(motion, name):
+    if motion not in _MOTIONS:
+        raise ValueError(f"{name}: motion must be one of {sorted(_MOTIONS)}, not {motion!r}")
+    return _MOTIONS[motion]
+
+
+# The arguments after the context of every odometry and voxel-downsample entry point, in C order with the names of
+# include/dcreg_b200.h: the one place the binding and the tests know these signatures.
+_RUN = "params n_seqs seq_offsets n_frames xyz frame_offsets stride cell_size"
+_FILTERS = "source_voxel map_voxel source_max_points map_max_points"
+_OUTPUTS = "T_prior T_out n_iterations converged status cov"
+_PUSH = "seq_offsets n_frames xyz frame_offsets stride deltas"
+_DOWNSAMPLE = "n_clouds xyz offsets stride voxel"
+_ODOMETRY_ARGS = {name: " ".join(args).split() for name, args in {
+    "dcreg_icp_run_odometry": (_RUN, "map_frames motion T_init deltas", _OUTPUTS, "log log_cap"),
+    "dcreg_icp_run_odometry_voxel": (_RUN, "map_frames motion source_voxel map_voxel T_init deltas frame_points",
+                                     _OUTPUTS, "log log_cap"),
+    "dcreg_icp_run_odometry_voxel_n": (_RUN, "map_frames motion", _FILTERS, "T_init deltas frame_points", _OUTPUTS,
+                                       "log log_cap"),
+    "dcreg_icp_run_odometry_deskew": (_RUN, "map_frames motion", _FILTERS, "T_init deltas timestamps frame_points",
+                                      _OUTPUTS, "deskewed_xyz log log_cap"),
+    "dcreg_icp_run_odometry_map": (_RUN, "motion", _FILTERS, "max_distance T_init deltas timestamps frame_points",
+                                   _OUTPUTS, "deskewed_xyz log log_cap"),
+    "dcreg_icp_run_odometry_adaptive": (_RUN, "map_frames motion", _FILTERS,
+                                        "max_distance adaptive T_init deltas timestamps frame_points", _OUTPUTS,
+                                        "deskewed_xyz search_radius log log_cap"),
+    "dcreg_odometry_open": ("params n_seqs cell_size map_frames motion", _FILTERS, "T_init"),
+    "dcreg_odometry_open_map": ("params n_seqs cell_size motion", _FILTERS, "max_distance T_init"),
+    "dcreg_odometry_open_adaptive": ("params n_seqs cell_size map_frames motion", _FILTERS,
+                                     "max_distance adaptive T_init"),
+    "dcreg_odometry_push": (_PUSH, "frame_points", _OUTPUTS, "log log_cap"),
+    "dcreg_odometry_push_deskew": (_PUSH, "timestamps frame_points", _OUTPUTS, "deskewed_xyz log log_cap"),
+    "dcreg_odometry_push_adaptive": (_PUSH, "timestamps frame_points", _OUTPUTS,
+                                     "deskewed_xyz search_radius log log_cap"),
+    "dcreg_voxel_downsample": (_DOWNSAMPLE, "out_xyz out_offsets out_index"),
+    "dcreg_voxel_downsample_n": (_DOWNSAMPLE, "max_points out_xyz out_offsets out_index"),
+    "dcreg_voxel_downsample_spaced": (_DOWNSAMPLE, "max_points min_spacing out_xyz out_offsets out_index"),
+}.items()}
+_ODOMETRY_NAMES = {a for args in _ODOMETRY_ARGS.values() for a in args}
+
+
+def _odometry_call(lib, h, entry, **values):
+    """lib.<entry>(h, ...) with values laid out in the entry's order (_ODOMETRY_ARGS).  A pointer argument not given is
+    NULL, a scalar not given is a ctypes error, and a value the entry does not take is left out: one set of values serves
+    every entry point a call may pick."""
+    unknown = values.keys() - _ODOMETRY_NAMES
+    if unknown:
+        raise TypeError(f"{entry}: no argument named {sorted(unknown)}")
+    return getattr(lib, entry)(h, *(values.get(k) for k in _ODOMETRY_ARGS[entry]))
+
+
+def _odometry_entry(op, radius=False, voxel_map=False, deskew=False, capped=False, filtered=False):
+    """The entry point of op ("icp_run_odometry", "odometry_open" or "odometry_push") for a call with these settings: the
+    narrowest that takes them all.  Each entry point names itself in dcreg_last_error."""
+    if radius:
+        return f"dcreg_{op}_adaptive"
+    if voxel_map:
+        return f"dcreg_{op}_map"
+    if deskew:
+        return f"dcreg_{op}_deskew"
+    if capped:
+        return f"dcreg_{op}_voxel_n"
+    if filtered:
+        return f"dcreg_{op}_voxel"
+    return f"dcreg_{op}"
+
+
 def pose_Rt(T):
     T = np.asarray(T, dtype=np.float64)
     return np.ascontiguousarray(np.concatenate([T[:3, :3].reshape(-1), T[:3, 3]]))
@@ -1030,13 +1100,10 @@ class Context:
         pts = np.empty((max(total, 1), 3), dtype=np.float32)
         idx = np.empty(max(total, 1), dtype=np.int64)
         kept = np.zeros(n + 1, dtype=np.int64)
-        if min_spacing == 0.0:
-            rc = self.lib.dcreg_voxel_downsample_n(self._h, n, _fptr(xyz), _iptr(off), 3, float(voxel), max_points,
-                                                   _fptr(pts), _iptr(kept), _iptr(idx))
-        else:
-            rc = self.lib.dcreg_voxel_downsample_spaced(self._h, n, _fptr(xyz), _iptr(off), 3, float(voxel), max_points,
-                                                        float(min_spacing), _fptr(pts), _iptr(kept), _iptr(idx))
-        self._check(rc)
+        entry = "dcreg_voxel_downsample_n" if min_spacing == 0.0 else "dcreg_voxel_downsample_spaced"
+        self._check(_odometry_call(self.lib, self._h, entry, n_clouds=n, xyz=_fptr(xyz), offsets=_iptr(off), stride=3,
+                                   voxel=float(voxel), max_points=max_points, min_spacing=float(min_spacing),
+                                   out_xyz=_fptr(pts), out_offsets=_iptr(kept), out_index=_iptr(idx)))
         return [(pts[a:b].copy(), idx[a:b].copy()) for a, b in zip(kept[:-1], kept[1:])]
 
     def icp_run_odometry(self, params, sequences, T_init, deltas=None, motion: str = "increments",
@@ -1062,69 +1129,9 @@ class Context:
         the ceiling params.search_radius (dcreg_icp_run_odometry_adaptive; the twin is adaptive_threshold_*), and
         .search_radius holds the radius each frame registered with (0 for anchors); want_radius: .search_radius also
         without the threshold (that entry point with adaptive = NULL)."""
-        models = {"increments": 0, "constant_velocity": 1}
-        if motion not in models:
-            raise ValueError(f"icp_run_odometry: motion must be one of {sorted(models)}, not {motion!r}")
-        with_radius = adaptive is not None or want_radius
-        radius = np.zeros(max(sum(len(s) for s in sequences), 1)) if with_radius else None
-        source_max_points = _max_points(source_max_points, "source_max_points")
-        map_max_points = _max_points(map_max_points, "map_max_points")
-        seq_off, xyz, off = _pack_sequences(sequences)
-        S, n = len(sequences), int(seq_off[-1])
-        params, parg, per_lane = self._lanes("icp_run_odometry", params, S)
-        cell = float(params.search_radius if cell_size is None else cell_size)
-        capped = source_max_points != 1 or map_max_points != 1
-        filtered = source_voxel != 0.0 or map_voxel != 0.0 or capped
-        deskew = timestamps is not None or want_deskewed
-        ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
-                              off if off is not None else np.zeros(1, np.int64), "icp_run_odometry")
-        npts = np.diff(off) if off is not None else np.zeros(0, dtype=np.int64)
-        if filtered or deskew or with_radius:
-            npts = np.zeros(max(n, 1), dtype=np.int64)
-        desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
-
-        def call(o):
-            if with_radius:
-                return self.lib.dcreg_icp_run_odometry_adaptive(
-                    self._h, parg, S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
-                    3, cell, int(map_frames), models[motion], float(source_voxel), float(map_voxel), source_max_points,
-                    map_max_points, 0.0, None if adaptive is None else C.byref(adaptive), _optr(o.T_init),
-                    _optr(o.deltas), _fptr(ts), _iptr(npts), _optr(o.T_prior), _optr(o.T_out), o.n_it, o.conv, o.st,
-                    _optr(o.cov), _fptr(desk), _dptr(radius), o.logs, o.cap)
-            if deskew:
-                return self.lib.dcreg_icp_run_odometry_deskew(
-                    self._h, parg, S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
-                    3, cell, int(map_frames), models[motion], float(source_voxel), float(map_voxel), source_max_points,
-                    map_max_points, _optr(o.T_init), _optr(o.deltas), _fptr(ts), _iptr(npts), _optr(o.T_prior),
-                    _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov), _fptr(desk), o.logs, o.cap)
-            if capped:
-                return self.lib.dcreg_icp_run_odometry_voxel_n(
-                    self._h, parg, S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
-                    3, cell, int(map_frames), models[motion], float(source_voxel), float(map_voxel), source_max_points,
-                    map_max_points, _optr(o.T_init), _optr(o.deltas), _iptr(npts), _optr(o.T_prior), _optr(o.T_out),
-                    o.n_it, o.conv, o.st, _optr(o.cov), o.logs, o.cap)
-            if filtered:
-                return self.lib.dcreg_icp_run_odometry_voxel(
-                    self._h, parg, S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
-                    3, cell, int(map_frames), models[motion], float(source_voxel), float(map_voxel), _optr(o.T_init),
-                    _optr(o.deltas), _iptr(npts), _optr(o.T_prior), _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov),
-                    o.logs, o.cap)
-            return self.lib.dcreg_icp_run_odometry(
-                self._h, parg, S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off), 3,
-                cell, int(map_frames), models[motion], _optr(o.T_init), _optr(o.deltas), _optr(o.T_prior),
-                _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov), o.logs, o.cap)
-        with self._lane_setting(per_lane):
-            out = self._run_batched("icp_run_odometry", call, params, n, S, "sequences", T_init, want_log, want_cov,
-                                    deltas, want_prior=True)
-        for r, c in zip(out, npts):
-            r.n_points = int(c)
-        if with_radius:
-            for r, x in zip(out, radius):
-                r.search_radius = float(x)
-        if want_deskewed:
-            for r, d in zip(out, _split_deskewed(desk, npts[:n])):
-                r.deskewed = d
-        return out
+        return self._odometry("icp_run_odometry", params, sequences, T_init, deltas, motion, map_frames, None, cell_size,
+                              want_log, want_cov, source_voxel, map_voxel, source_max_points, map_max_points, timestamps,
+                              want_deskewed, adaptive, want_radius)
 
     def icp_run_odometry_map(self, params, sequences, T_init, deltas=None, motion: str = "increments", *,
                              map_voxel: float, max_distance: float, cell_size=None, want_log: bool = False,
@@ -1137,39 +1144,49 @@ class Context:
         max_distance).  map_voxel must be > 0; max_distance > 0 (inf: nothing is pruned, and the outputs are those of
         icp_run_odometry with map_frames >= the longest sequence).  The arguments are icp_run_odometry's in the same
         positions, without map_frames; map_voxel and max_distance are keyword-only."""
-        models = {"increments": 0, "constant_velocity": 1}
-        if motion not in models:
-            raise ValueError(f"icp_run_odometry_map: motion must be one of {sorted(models)}, not {motion!r}")
+        return self._odometry("icp_run_odometry_map", params, sequences, T_init, deltas, motion, 0,
+                              float(max_distance), cell_size, want_log, want_cov, source_voxel, map_voxel,
+                              source_max_points, map_max_points, timestamps, want_deskewed, adaptive, want_radius)
+
+    def _odometry(self, name, params, sequences, T_init, deltas, motion, map_frames, max_distance, cell_size, want_log,
+                  want_cov, source_voxel, map_voxel, source_max_points, map_max_points, timestamps, want_deskewed,
+                  adaptive, want_radius):
+        """icp_run_odometry (max_distance None: the window of map_frames frames) and icp_run_odometry_map (map_frames
+        0: the voxel map pruned at max_distance)"""
+        motion = _motion(motion, name)
         source_max_points = _max_points(source_max_points, "source_max_points")
         map_max_points = _max_points(map_max_points, "map_max_points")
         seq_off, xyz, off = _pack_sequences(sequences)
         S, n = len(sequences), int(seq_off[-1])
-        params, parg, per_lane = self._lanes("icp_run_odometry_map", params, S)
+        params, parg, per_lane = self._lanes(name, params, S)
         cell = float(params.search_radius if cell_size is None else cell_size)
-        ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
-                              off if off is not None else np.zeros(1, np.int64), "icp_run_odometry_map")
-        npts = np.zeros(max(n, 1), dtype=np.int64)
-        desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
-
         with_radius = adaptive is not None or want_radius
+        entry = _odometry_entry("icp_run_odometry", radius=with_radius, voxel_map=max_distance is not None,
+                                deskew=timestamps is not None or want_deskewed,
+                                capped=source_max_points != 1 or map_max_points != 1,
+                                filtered=source_voxel != 0.0 or map_voxel != 0.0)
+        ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
+                              off if off is not None else np.zeros(1, np.int64), name)
+        npts = np.diff(off) if off is not None else np.zeros(0, dtype=np.int64)
+        if entry != "dcreg_icp_run_odometry":       # the others return each frame's points after the source filter
+            npts = np.zeros(max(n, 1), dtype=np.int64)
+        desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
         radius = np.zeros(max(n, 1)) if with_radius else None
 
         def call(o):
-            if with_radius:
-                return self.lib.dcreg_icp_run_odometry_adaptive(
-                    self._h, parg, S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off),
-                    3, cell, 0, models[motion], float(source_voxel), float(map_voxel), source_max_points,
-                    map_max_points, float(max_distance), None if adaptive is None else C.byref(adaptive),
-                    _optr(o.T_init), _optr(o.deltas), _fptr(ts), _iptr(npts), _optr(o.T_prior), _optr(o.T_out), o.n_it,
-                    o.conv, o.st, _optr(o.cov), _fptr(desk), _dptr(radius), o.logs, o.cap)
-            return self.lib.dcreg_icp_run_odometry_map(
-                self._h, parg, S, seq_off.ctypes.data_as(C.POINTER(C.c_int)), o.n, _fptr(xyz), _iptr(off), 3,
-                cell, models[motion], float(source_voxel), float(map_voxel), source_max_points, map_max_points,
-                float(max_distance), _optr(o.T_init), _optr(o.deltas), _fptr(ts), _iptr(npts), _optr(o.T_prior),
-                _optr(o.T_out), o.n_it, o.conv, o.st, _optr(o.cov), _fptr(desk), o.logs, o.cap)
+            return _odometry_call(
+                self.lib, self._h, entry, params=parg, n_seqs=S, seq_offsets=seq_off.ctypes.data_as(C.POINTER(C.c_int)),
+                n_frames=o.n, xyz=_fptr(xyz), frame_offsets=_iptr(off), stride=3, cell_size=cell,
+                map_frames=int(map_frames), motion=motion, source_voxel=float(source_voxel), map_voxel=float(map_voxel),
+                source_max_points=source_max_points, map_max_points=map_max_points,
+                max_distance=0.0 if max_distance is None else float(max_distance),
+                adaptive=None if adaptive is None else C.byref(adaptive), T_init=_optr(o.T_init), deltas=_optr(o.deltas),
+                timestamps=_fptr(ts), frame_points=_iptr(npts), T_prior=_optr(o.T_prior), T_out=_optr(o.T_out),
+                n_iterations=o.n_it, converged=o.conv, status=o.st, cov=_optr(o.cov), deskewed_xyz=_fptr(desk),
+                search_radius=_optr(radius), log=o.logs, log_cap=o.cap)
         with self._lane_setting(per_lane):
-            out = self._run_batched("icp_run_odometry_map", call, params, n, S, "sequences", T_init, want_log, want_cov,
-                                    deltas, want_prior=True)
+            out = self._run_batched(name, call, params, n, S, "sequences", T_init, want_log, want_cov, deltas,
+                                    want_prior=True)
         for r, c in zip(out, npts):
             r.n_points = int(c)
         if with_radius:
@@ -1187,26 +1204,8 @@ class Context:
         OdometrySession of odometry_session, whose pushes give byte for byte what one icp_run_odometry_map call over the
         recording gives, and whose local_map(s) returns sequence s's current map.  The arguments are odometry_session's
         in the same positions, without map_frames; map_voxel and max_distance are keyword-only."""
-        models = {"increments": 0, "constant_velocity": 1}
-        if motion not in models:
-            raise ValueError(f"odometry_map_session: motion must be one of {sorted(models)}, not {motion!r}")
-        source_max_points = _max_points(source_max_points, "source_max_points")
-        map_max_points = _max_points(map_max_points, "map_max_points")
-        T0 = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
-        if T0.shape[0] != n_seqs:
-            raise ValueError(f"odometry_map_session: {n_seqs} sequences but {T0.shape[0]} initial poses")
-        params, parg, per_lane = self._lanes("odometry_map_session", params, int(n_seqs))
-        cell = float(params.search_radius if cell_size is None else cell_size)
-        with self._lane_setting(per_lane):
-            if adaptive is not None:        # dcreg_odometry_open_adaptive: its pushes return .search_radius
-                self._check(self.lib.dcreg_odometry_open_adaptive(
-                    self._h, parg, int(n_seqs), cell, 0, models[motion], float(source_voxel), float(map_voxel),
-                    source_max_points, map_max_points, float(max_distance), C.byref(adaptive), _dptr(T0)))
-                return OdometrySession(self, params, int(n_seqs), adaptive=True)
-            self._check(self.lib.dcreg_odometry_open_map(self._h, parg, int(n_seqs), cell, models[motion],
-                                                         float(source_voxel), float(map_voxel), source_max_points,
-                                                         map_max_points, float(max_distance), _dptr(T0)))
-        return OdometrySession(self, params, int(n_seqs))
+        return self._open_session("odometry_map_session", params, n_seqs, T_init, motion, 0, float(max_distance),
+                                  cell_size, source_voxel, map_voxel, source_max_points, map_max_points, adaptive)
 
     def odometry_session(self, params, n_seqs: int, T_init, motion: str = "increments", map_frames: int = 10,
                          cell_size=None, source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
@@ -1215,26 +1214,30 @@ class Context:
         whose frames come in pushes (OdometrySession.push).  T_init (n_seqs, 4, 4): the pose of each sequence's first
         frame.  Pushing a recording in any chunks gives byte for byte what one icp_run_odometry call over it gives.
         One session per context; use it as a context manager, or close() it."""
-        models = {"increments": 0, "constant_velocity": 1}
-        if motion not in models:
-            raise ValueError(f"odometry_session: motion must be one of {sorted(models)}, not {motion!r}")
+        return self._open_session("odometry_session", params, n_seqs, T_init, motion, map_frames, None, cell_size,
+                                  source_voxel, map_voxel, source_max_points, map_max_points, adaptive)
+
+    def _open_session(self, name, params, n_seqs, T_init, motion, map_frames, max_distance, cell_size, source_voxel,
+                      map_voxel, source_max_points, map_max_points, adaptive):
+        """odometry_session (max_distance None) and odometry_map_session (map_frames 0), as in _odometry"""
+        motion = _motion(motion, name)
         source_max_points = _max_points(source_max_points, "source_max_points")
         map_max_points = _max_points(map_max_points, "map_max_points")
         T0 = np.ascontiguousarray(T_init, dtype=np.float64).reshape(-1, 4, 4)
         if T0.shape[0] != n_seqs:
-            raise ValueError(f"odometry_session: {n_seqs} sequences but {T0.shape[0]} initial poses")
-        params, parg, per_lane = self._lanes("odometry_session", params, int(n_seqs))
+            raise ValueError(f"{name}: {n_seqs} sequences but {T0.shape[0]} initial poses")
+        params, parg, per_lane = self._lanes(name, params, int(n_seqs))
         cell = float(params.search_radius if cell_size is None else cell_size)
+        # dcreg_odometry_open_adaptive's pushes return .search_radius
+        entry = _odometry_entry("odometry_open", radius=adaptive is not None, voxel_map=max_distance is not None)
         with self._lane_setting(per_lane):
-            if adaptive is not None:        # dcreg_odometry_open_adaptive: its pushes return .search_radius
-                self._check(self.lib.dcreg_odometry_open_adaptive(
-                    self._h, parg, int(n_seqs), cell, int(map_frames), models[motion], float(source_voxel),
-                    float(map_voxel), source_max_points, map_max_points, 0.0, C.byref(adaptive), _dptr(T0)))
-                return OdometrySession(self, params, int(n_seqs), adaptive=True)
-            self._check(self.lib.dcreg_odometry_open(self._h, parg, int(n_seqs), cell, int(map_frames), models[motion],
-                                                     float(source_voxel), float(map_voxel), source_max_points,
-                                                     map_max_points, _dptr(T0)))
-        return OdometrySession(self, params, int(n_seqs))
+            self._check(_odometry_call(
+                self.lib, self._h, entry, params=parg, n_seqs=int(n_seqs), cell_size=cell, map_frames=int(map_frames),
+                motion=motion, source_voxel=float(source_voxel), map_voxel=float(map_voxel),
+                source_max_points=source_max_points, map_max_points=map_max_points,
+                max_distance=0.0 if max_distance is None else float(max_distance),
+                adaptive=None if adaptive is None else C.byref(adaptive), T_init=_dptr(T0)))
+        return OdometrySession(self, params, int(n_seqs), adaptive=adaptive is not None)
 
     def icp_run_pairs(self, params, sources, targets, T_init, cell_size=None, want_log: bool = False,
                       want_cov: bool = False, metrics_threshold=None):
@@ -1347,7 +1350,7 @@ class OdometrySession:
         only when want_log, .cov when want_cov).  timestamps / want_deskewed: as in icp_run_odometry, nested like
         frames_per_seq (dcreg_odometry_push_deskew).  A push that fails raises DcregError and leaves the session as it
         was."""
-        ctx, lib = self.ctx, self.ctx.lib
+        ctx = self.ctx
         if len(frames_per_seq) != self.n_seqs:
             raise ValueError(f"odometry push: {self.n_seqs} sequences but {len(frames_per_seq)} frame lists")
         seq_off, xyz, off = _pack_sequences(frames_per_seq)
@@ -1365,26 +1368,15 @@ class OdometrySession:
         cap = int(self.params.max_iterations) if want_log else 0
         logs = (IterLog * max(cap * n, 1))() if want_log else None
         radius = np.zeros(m) if self.adaptive else None
-        if self.adaptive:
-            ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
-                                  off if off is not None else np.zeros(1, np.int64), "odometry push")
-            desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
-            ctx._check(lib.dcreg_odometry_push_adaptive(
-                ctx._h, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n, _fptr(xyz), _iptr(off), 3, _optr(D), _fptr(ts),
-                _iptr(npts), _dptr(T_prior), _dptr(T_out), n_it, conv, st, _optr(cov), _fptr(desk), _dptr(radius), logs,
-                cap))
-        elif timestamps is not None or want_deskewed:
-            ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
-                                  off if off is not None else np.zeros(1, np.int64), "odometry push")
-            desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
-            ctx._check(lib.dcreg_odometry_push_deskew(
-                ctx._h, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n, _fptr(xyz), _iptr(off), 3, _optr(D), _fptr(ts),
-                _iptr(npts), _dptr(T_prior), _dptr(T_out), n_it, conv, st, _optr(cov), _fptr(desk), logs, cap))
-        else:
-            desk = None
-            ctx._check(lib.dcreg_odometry_push(ctx._h, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n, _fptr(xyz),
-                                               _iptr(off), 3, _optr(D), _iptr(npts), _dptr(T_prior), _dptr(T_out), n_it,
-                                               conv, st, _optr(cov), logs, cap))
+        ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
+                              off if off is not None else np.zeros(1, np.int64), "odometry push")
+        desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
+        entry = _odometry_entry("odometry_push", radius=self.adaptive, deskew=timestamps is not None or want_deskewed)
+        ctx._check(_odometry_call(
+            ctx.lib, ctx._h, entry, seq_offsets=seq_off.ctypes.data_as(C.POINTER(C.c_int)), n_frames=n, xyz=_fptr(xyz),
+            frame_offsets=_iptr(off), stride=3, deltas=_optr(D), timestamps=_fptr(ts), frame_points=_iptr(npts),
+            T_prior=_dptr(T_prior), T_out=_dptr(T_out), n_iterations=n_it, converged=conv, status=st, cov=_optr(cov),
+            deskewed_xyz=_fptr(desk), search_radius=_optr(radius), log=logs, log_cap=cap))
         res = _trial_results(st[:n], conv[:n], n_it[:n], T_out, logs, cap, cov)
         for r, Tp, c in zip(res, T_prior, npts):
             r.T_prior, r.n_points = Tp, int(c)

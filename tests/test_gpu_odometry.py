@@ -14,99 +14,18 @@ import pytest
 
 import dcreg_oracle as o
 
+from odom_harness import (CELL, RADIUS, assert_anchor, assert_priors, assert_same_run, ctx, parking,  # noqa: F401
+                          params, raw_odometry, reconstruct, split, window_map)
+
 pytestmark = pytest.mark.gpu
-
-RADIUS = 0.5
-CELL = 0.5
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
 
 
 @pytest.fixture(scope="module")
 def odo():
     """20 dense frames (about 20 k points, 16 points / m^2 of ground) of one path with drifting odometry, split into
     sequences of 1, 7 and 12 frames; T_init = the true pose of each sequence's first frame."""
-    from dcreg_b200.scenes import make_parking_sequence
-    frames, T_true, _, deltas, _ = make_parking_sequence(20, seed=71, n_scan=20_000, max_range=20.0)
-    bounds = [0, 1, 8, 20]
-    seqs = [frames[a:b] for a, b in zip(bounds[:-1], bounds[1:])]
-    return seqs, frames, T_true[bounds[:-1]], deltas, T_true
-
-
-def params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
-
-
-def rel_err(a, b):
-    a = np.asarray(a, dtype=np.float64); b = np.asarray(b, dtype=np.float64)
-    return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-300))
-
-
-def split(res, seqs):
-    out, k = [], 0
-    for s in seqs:
-        out.append(res[k:k + len(s)])
-        k += len(s)
-    return out
-
-
-def local_map(seq, res_seq, k, map_frames):
-    from dcreg_b200.api import map_points
-    return np.concatenate([map_points(res_seq[j].T, seq[j]) for j in range(max(0, k - map_frames), k)])
-
-
-def reconstruct(ctx, prm, seq, res_seq, k, map_frames, cell=CELL):
-    ctx.set_target(local_map(seq, res_seq, k, map_frames), cell)
-    ctx.set_source(seq[k])
-    return ctx.icp_run(prm, res_seq[k].T_prior)
-
-
-def assert_same_run(b, single, logs=True):
-    assert (b.status, b.iterations, b.converged) == (single.status, single.iterations, single.converged)
-    assert o.se3_log_distance(single.T, b.T) < 1e-8
-    if not logs:
-        return
-    assert len(b.logs) == len(single.logs)
-    for x, y in zip(b.logs, single.logs):
-        assert x.n_effective == y.n_effective and x.n_corr_pt == y.n_corr_pt
-        assert list(x.analysis.degenerate_mask) == list(y.analysis.degenerate_mask)
-        if x.status == 0:
-            assert rel_err(np.array(x.H27), np.array(y.H27)) < 1e-8
-            assert np.max(np.abs(np.array(x.dx) - np.array(y.dx))) < 1e-8
-
-
-def assert_anchor(r, T0):
-    T0 = np.ascontiguousarray(T0, dtype=np.float64)
-    assert r.T.tobytes() == T0.tobytes() and r.T_prior.tobytes() == T0.tobytes()
-    assert (r.iterations, r.converged, r.status) == (0, 0, 0)
-    assert len(r.logs) == 0
-    if r.cov is not None:
-        assert r.cov.tobytes() == (np.eye(6) * 1e6).tobytes()
-
-
-def assert_priors(res, seqs, T_init, deltas, motion="increments"):
-    from dcreg_b200.api import compose_prior, constant_velocity_increment
-    k = 0
-    for s, rs in enumerate(split(res, seqs)):
-        assert rs[0].T_prior.tobytes() == np.ascontiguousarray(T_init[s]).tobytes()
-        for j in range(1, len(rs)):
-            if motion == "constant_velocity":
-                D = np.eye(4) if j == 1 else constant_velocity_increment(rs[j - 2].T, rs[j - 1].T)
-            else:
-                D = np.eye(4) if deltas is None else deltas[k + j - 1]
-            assert rs[j].T_prior.tobytes() == compose_prior(rs[j - 1].T, D).tobytes(), (s, j)
-        k += len(rs)
+    seqs, T_init, deltas, frames, T_true = parking()
+    return seqs, frames, T_init, deltas, T_true
 
 
 @pytest.mark.parametrize("method,cell", [pytest.param(m, c, id=m if c == CELL else f"{m}-cell{c}")
@@ -122,7 +41,7 @@ def test_frames_equal_their_reconstruction(ctx, odo, method, cell):
     for s, (seq, rs) in enumerate(zip(seqs, split(res, seqs))):
         assert_anchor(rs[0], T_init[s])
         for k in range(1, len(seq)):
-            assert_same_run(rs[k], reconstruct(ctx, prm, seq, rs, k, 3, cell))
+            assert_same_run(rs[k], reconstruct(ctx, prm, seq, rs, k, 3, cell=cell))
     assert sum(r.converged for r in res) >= 15
     assert max(o.se3_log_distance(r.T, T) for r, T in zip(res, T_true)) < 0.05
 
@@ -225,7 +144,7 @@ def test_first_frames_match_oracle(ctx, odo):
     cp = oc.make_params(search_radius=RADIUS, max_iterations=30, conv_rot=1e-5, conv_trans=1e-3, kappa_target=10.0)
     for k in (1, 2, 3):
         b = res[k]
-        sc = oc.Scene(seq[k], local_map(seq, res, k, 3))
+        sc = oc.Scene(seq[k], window_map(seq, res, k, 3))
         st, conv, n_it, Tc, clogs = sc.icp_run(cp, b.T_prior)
         sc.close()
         assert (b.status, b.converged, b.iterations) == (st, conv, n_it), k
@@ -252,11 +171,13 @@ def test_odometry_bad_arguments(ctx, odo):
     def call(n_seqs=2, seq_off=so, n_frames=4, pts=xyz, offsets=off, p=prm, handle=h, T0=T, cell=CELL, map_frames=3,
              motion=0, Dd=D, stride=3):
         Tout = np.empty((max(n_frames, 1), 4, 4))
-        return lib.dcreg_icp_run_odometry(handle, C.byref(p), n_seqs, seq_off.ctypes.data_as(C.POINTER(C.c_int)), n_frames,
-                                          pts.ctypes.data_as(C.POINTER(C.c_float)), offsets.ctypes.data_as(C.POINTER(C.c_int64)),
-                                          stride, cell, map_frames, motion, T0.ctypes.data_as(dp),
-                                          Dd.ctypes.data_as(dp) if Dd is not None else None, None, Tout.ctypes.data_as(dp),
-                                          None, None, None, None, None, 0)
+        return api._odometry_call(lib, handle, "dcreg_icp_run_odometry", params=C.byref(p), n_seqs=n_seqs,
+                                  seq_offsets=seq_off.ctypes.data_as(C.POINTER(C.c_int)), n_frames=n_frames,
+                                  xyz=pts.ctypes.data_as(C.POINTER(C.c_float)),
+                                  frame_offsets=offsets.ctypes.data_as(C.POINTER(C.c_int64)), stride=stride,
+                                  cell_size=cell, map_frames=map_frames, motion=motion, T_init=T0.ctypes.data_as(dp),
+                                  deltas=Dd.ctypes.data_as(dp) if Dd is not None else None,
+                                  T_out=Tout.ctypes.data_as(dp), log_cap=0)
 
     assert call() == api.OK
     assert call(motion=1, Dd=None) == api.OK
@@ -287,18 +208,11 @@ def test_odometry_bad_arguments(ctx, odo):
     assert e.value.status == api.BAD_ARG
     msg = lib.dcreg_last_error(h).decode()
     assert "sequence 0" in msg and "frame 3" in msg, msg
-    pts = np.ascontiguousarray(np.concatenate(seq), dtype=np.float32)
-    offs = np.zeros(6, np.int64); offs[1:] = np.cumsum([len(f) for f in seq])
-    Tout = np.full((5, 4, 4), -7.0)
-    n_it = (C.c_int * 5)(*([-1] * 5))
-    rc = lib.dcreg_icp_run_odometry(h, C.byref(prm), 1, np.array([0, 5], np.int32).ctypes.data_as(C.POINTER(C.c_int)), 5,
-                                    pts.ctypes.data_as(C.POINTER(C.c_float)), offs.ctypes.data_as(C.POINTER(C.c_int64)), 3,
-                                    CELL, 3, 0, np.ascontiguousarray(T_init[2:3]).ctypes.data_as(dp),
-                                    np.ascontiguousarray(deltas[8:13]).ctypes.data_as(dp), None, Tout.ctypes.data_as(dp),
-                                    n_it, None, None, None, None, 0)
+    rc, out = raw_odometry(ctx, "dcreg_icp_run_odometry", prm, [seq], T_init[2:3], deltas[8:13])
+    n_it, Tout = out["n_it"], out["T_out"]
     assert rc == api.BAD_ARG
     assert all(n_it[k] >= 0 for k in range(3)) and n_it[1] > 0 and n_it[3] == -1 and n_it[4] == -1
-    assert np.all(Tout[3:] == -7.0) and Tout[2, 3, 3] == 1.0
+    assert np.all(Tout[3:] == -1.0) and Tout[2, 3, 3] == 1.0
     good = ctx.icp_run_odometry(prm, seqs, T_init, deltas, map_frames=3, cell_size=CELL, want_log=True)
     with Context(0) as fresh:
         ref = fresh.icp_run_odometry(prm, seqs, T_init, deltas, map_frames=3, cell_size=CELL, want_log=True)

@@ -11,48 +11,30 @@ import math
 import numpy as np
 import pytest
 
-from test_gpu_odometry import assert_anchor, assert_priors, assert_same_run, local_map, split
-from test_gpu_odometry_map import twin_maps
-from test_gpu_odometry_stream import LENS, RAGGED, assert_same, one_per_push
+from odom_harness import (CELL, RADIUS, RAGGED, assert_anchor, assert_priors, assert_same_flat,  # noqa: F401
+                          assert_same_run, ctx, one_per_push, params, parking, parking_sweeps, pushed, rel_err, split,
+                          twin_maps, window_map)
 
 pytestmark = pytest.mark.gpu
 
-RADIUS = 0.5
-CELL = 0.5
-MV, DIST = 0.25, 10.0          # the voxel map's voxel (test_gpu_odometry_map.MV) and prune distance
+LENS = (1, 7, 12)
+MV, DIST = 0.25, 10.0          # the voxel map's voxel and prune distance
 CEILING = 2.0                  # four rings of cells: the ceiling of the tests whose radii move
 MAPS = ["window", "voxel_map"]
 METHODS = ["Ours", "ME-TSVD"]
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
+MAP_KW = {"window": dict(map_frames=3), "voxel_map": dict(map_voxel=MV, max_distance=DIST)}
 
 
 @pytest.fixture(scope="module")
 def odo():
     """20 frames of one path (about 8 k points each, 20 m range) with drifting odometry, in sequences of 1, 7 and 12"""
-    from dcreg_b200.scenes import make_parking_sequence
-    frames, T_true, _, deltas, _ = make_parking_sequence(20, seed=71, n_scan=8_000, max_range=20.0)
-    bounds = np.concatenate([[0], np.cumsum(LENS)])
-    seqs = [list(frames[a:b]) for a, b in zip(bounds[:-1], bounds[1:])]
-    return seqs, np.ascontiguousarray(T_true[bounds[:-1]]), deltas
+    return parking(LENS, n_scan=8_000)[:3]
 
 
 @pytest.fixture(scope="module")
 def sweeps():
     """12 skewed sweeps with per-point timestamps in sequences of 5 and 7 frames (unskewed anchors)"""
-    from dcreg_b200.scenes import make_parking_sweeps
-    skewed, stamps, T_true, deltas, frames = make_parking_sweeps(12, seed=71, n_scan=8_000, max_range=20.0)
-    b = [0, 5, 12]
-    for a in b[:-1]:
-        skewed[a] = frames[a]
-    cut = lambda x: [list(x[p:q]) for p, q in zip(b[:-1], b[1:])]        # noqa: E731
-    return dict(skewed=cut(skewed), stamps=cut(stamps), T_init=np.ascontiguousarray(T_true[b[:-1]]), deltas=deltas)
+    return parking_sweeps((5, 7), n_scan=8_000)
 
 
 @pytest.fixture(scope="module")
@@ -73,15 +55,6 @@ def noisy():
     return seqs, np.ascontiguousarray(T_true[0:20:5]), deltas
 
 
-def params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
-
-
 def threshold(*a):
     from dcreg_b200.api import AdaptiveThreshold
     return AdaptiveThreshold(*a)
@@ -96,19 +69,8 @@ def run(ctx, which, prm, seqs, T_init, deltas, **kw):
 
 
 def open_session(ctx, which, prm, n_seqs, T_init, **kw):
-    if which == "voxel_map":
-        return ctx.odometry_map_session(prm, n_seqs, T_init, map_voxel=MV, max_distance=DIST, cell_size=CELL, **kw)
-    return ctx.odometry_session(prm, n_seqs, T_init, map_frames=3, cell_size=CELL, **kw)
-
-
-def assert_same_flat(a, b, radius=True):
-    assert_same([a], [b])
-    for x, y in zip(a, b):
-        assert (x.deskewed is None) == (y.deskewed is None)
-        if x.deskewed is not None:
-            assert x.deskewed.tobytes() == y.deskewed.tobytes()
-        if radius:
-            assert x.search_radius == y.search_radius
+    open_ = ctx.odometry_map_session if which == "voxel_map" else ctx.odometry_session
+    return open_(prm, n_seqs, T_init, cell_size=CELL, **MAP_KW[which], **kw)
 
 
 def counted(ctx, f):
@@ -134,7 +96,7 @@ def test_null_is_the_existing_call(ctx, odo, sweeps, method, which):
         D = None if kw.get("motion") == "constant_velocity" else dl
         ref, n_ref = counted(ctx, lambda: run(ctx, which, prm, sq, T0, D, **kw))
         got, n_got = counted(ctx, lambda: run(ctx, which, prm, sq, T0, D, want_radius=True, **kw))
-        assert_same_flat(got, ref, radius=False)
+        assert_same_flat(got, ref)
         assert n_got == n_ref
         for rs in split(got, sq):
             assert [r.search_radius for r in rs] == [0.0] + [RADIUS] * (len(rs) - 1)
@@ -155,7 +117,7 @@ def test_radius_at_the_ceiling_gives_the_existing_bytes(ctx, odo, sweeps, method
         D = None if kw.get("motion") == "constant_velocity" else dl
         ref, n_ref = counted(ctx, lambda: run(ctx, which, prm, sq, T0, D, **kw))
         got, n_got = counted(ctx, lambda: run(ctx, which, prm, sq, T0, D, adaptive=thr, **kw))
-        assert_same_flat(got, ref, radius=False)
+        assert_same_flat(got, ref)
         assert n_got == n_ref + max(len(s) for s in sq) - 1
         for rs in split(got, sq):
             assert [r.search_radius for r in rs] == [0.0] + [RADIUS] * (len(rs) - 1)
@@ -194,7 +156,7 @@ def reconstruct(ctx, which, method, seq, rs, k, frames=None, sv=0.0, cap=1, maps
         ctx.set_target(maps[k], CELL)
     else:
         fs = frames if frames is not None else [voxel_downsample(f, sv, 1)[0] if sv else f for f in seq]
-        ctx.set_target(local_map(fs, rs, k, 3), CELL)
+        ctx.set_target(window_map(fs, rs, k, 3), CELL)
     ctx.set_source(src)
     return ctx.icp_run(prm, rs[k].T_prior)
 
@@ -204,7 +166,6 @@ def assert_same_run_wide_steps(b, single):
     priors at 0.5 m, and the solve passes the rounding of sums that agree to 1e-8 on in proportion (measured: 3e-7 of
     the update); everything counted stays identical and the poses agree to 1e-8"""
     import dcreg_oracle as o
-    from test_gpu_odometry import rel_err
     assert (b.status, b.iterations, b.converged) == (single.status, single.iterations, single.converged)
     assert o.se3_log_distance(single.T, b.T) < 1e-8
     assert len(b.logs) == len(single.logs)
@@ -220,7 +181,7 @@ def assert_reconstructions(ctx, which, method, res, seqs, T_init, sv=0.0, cap=1,
     for s, (seq, rs) in enumerate(zip(seqs, split(res, seqs))):
         assert_anchor(rs[0], T_init[s])
         frames = [r.deskewed for r in rs] if deskewed else None
-        maps = twin_maps(seq, rs, sv, cap, DIST, frames=frames) if which == "voxel_map" else None
+        maps = twin_maps(seq, rs, sv, MV, cap, DIST, frames=frames) if which == "voxel_map" else None
         for k in range(1, len(seq)):
             same(rs[k], reconstruct(ctx, which, method, seq, rs, k, frames, sv, cap, maps))
 
@@ -282,24 +243,12 @@ def test_lanes_of_one_step_search_different_ring_counts(ctx, noisy, method, whic
     assert_reconstructions(ctx, which, method, res, seqs, T_init, cap=4, same=assert_same_run_wide_steps)
 
 
-def pushed(ctx, which, prm, seqs, T_init, chunks, deltas, thr, stamps=None, ts_push=None, **kw):
-    first = np.concatenate([[0], np.cumsum([len(s) for s in seqs])])
-    done = [0] * len(seqs)
-    out = [[] for _ in seqs]
-    with open_session(ctx, which, prm, len(seqs), T_init, adaptive=thr, **kw) as sess:
-        for i, cnt in enumerate(chunks):
-            part = [seqs[s][done[s]:done[s] + c] for s, c in enumerate(cnt)]
-            D = None
-            if deltas is not None:
-                D = np.concatenate([deltas[first[s] + done[s]:first[s] + done[s] + c] for s, c in enumerate(cnt)])
-            ts = None
-            if stamps is not None and (ts_push is None or ts_push(i)):
-                ts = [stamps[s][done[s]:done[s] + c] for s, c in enumerate(cnt)]
-            for s, r in enumerate(sess.push(part, D, want_log=True, want_cov=True, timestamps=ts,
-                                            want_deskewed=stamps is not None)):
-                out[s].extend(r)
-            done = [d + c for d, c in zip(done, cnt)]
-    return [r for rs in out for r in rs]
+def pushed_flat(ctx, which, prm, seqs, T_init, chunks, deltas, thr, stamps=None, **kw):
+    """The recording pushed in chunks into a session with the threshold thr, with logs and covariances (deskewed points
+    with stamps): one flat list of results"""
+    res = pushed(ctx, prm, seqs, T_init, chunks, deltas, voxel_map=which == "voxel_map", stamps=stamps, want_log=True,
+                 want_cov=True, want_deskewed=stamps is not None, adaptive=thr, **MAP_KW[which], **kw)
+    return [r for rs in res for r in rs]
 
 
 @pytest.mark.parametrize("which", MAPS)
@@ -314,8 +263,8 @@ def test_chunkings_equal_one_call(ctx, odo, which, motion):
         ref = run(ctx, which, prm, seqs, T_init, D, motion=motion, adaptive=thr, map_max_points=4)
         assert len({r.search_radius for r in ref}) >= 4
         for chunks in ([list(LENS)], one_per_push(LENS), RAGGED):
-            got = pushed(ctx, which, prm, seqs, T_init, chunks, D, thr, motion=motion, map_max_points=4)
-            assert_same_flat(got, ref)
+            got = pushed_flat(ctx, which, prm, seqs, T_init, chunks, D, thr, motion=motion, map_max_points=4)
+            assert_same_flat(got, ref, radius=True)
 
 
 @pytest.mark.parametrize("which", MAPS)
@@ -329,9 +278,9 @@ def test_mixed_deskew_and_plain_pushes(ctx, sweeps, which):
     stamps = [[t if not 1 <= k < 3 else np.full_like(t, 0.5) for k, t in enumerate(ts)] for ts in sw["stamps"]]
     ref = run(ctx, which, prm, sw["skewed"], sw["T_init"], sw["deltas"], adaptive=thr, source_voxel=0.3,
               map_max_points=4, timestamps=stamps, want_deskewed=True)
-    got = pushed(ctx, which, prm, sw["skewed"], sw["T_init"], chunks, sw["deltas"], thr, stamps=sw["stamps"],
-                 ts_push=with_ts, source_voxel=0.3, map_max_points=4)
-    assert_same_flat(got, ref)
+    got = pushed_flat(ctx, which, prm, sw["skewed"], sw["T_init"], chunks, sw["deltas"], thr, stamps=sw["stamps"],
+                      ts_push=with_ts, source_voxel=0.3, map_max_points=4)
+    assert_same_flat(got, ref, radius=True)
 
 
 @pytest.mark.parametrize("which", MAPS)
@@ -353,7 +302,7 @@ def test_failed_push_leaves_the_threshold_state(ctx, odo, which):
             sess.push([[far, seq[3]]], deltas[10:12])
         assert e.value.status == api.BAD_ARG
         got += sess.push([seq[2:]], deltas[10:14], want_log=True, want_cov=True)[0]
-    assert_same_flat(got, ref)
+    assert_same_flat(got, ref, radius=True)
     assert len({r.search_radius for r in ref}) > 3
 
 
@@ -370,8 +319,8 @@ def test_reproducible_and_context_untouched(ctx, odo):
     a2 = run(ctx, "window", wide, seqs, T_init, deltas, adaptive=thr)
     b2 = run(ctx, "voxel_map", wide, seqs, T_init, deltas, adaptive=thr)
     after = ctx.icp_run(prm, T_init[2])
-    assert_same_flat(a2, a)
-    assert_same_flat(b2, b)
+    assert_same_flat(a2, a, radius=True)
+    assert_same_flat(b2, b, radius=True)
     for r in (mid, after):
         assert (r.status, r.iterations, r.converged) == (before.status, before.iterations, before.converged)
         assert r.T.tobytes() == before.T.tobytes()

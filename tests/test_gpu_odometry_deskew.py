@@ -7,42 +7,11 @@ import pytest
 
 import dcreg_oracle as o
 
+from odom_harness import CELL, RADIUS, ctx, params, pushed, result_bytes, sweeps  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
-RADIUS = 0.5
-CELL = 0.5
 LENS = (5, 7)
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
-
-
-@pytest.fixture(scope="module")
-def sweeps():
-    """12 sweeps of one path (about 20 k points each) in sequences of 5 and 7 frames; the anchors are unskewed (an
-    anchor is never deskewed), T_init the true pose of each sequence's first frame"""
-    from dcreg_b200.scenes import make_parking_sweeps
-    skewed, stamps, T_true, deltas, frames = make_parking_sweeps(12, seed=71, n_scan=20_000, max_range=20.0)
-    b = np.concatenate([[0], np.cumsum(LENS)])
-    for a in b[:-1]:
-        skewed[a] = frames[a]
-    cut = lambda x: [list(x[p:q]) for p, q in zip(b[:-1], b[1:])]
-    return dict(skewed=cut(skewed), stamps=cut(stamps), unskewed=cut(frames), T_init=np.ascontiguousarray(T_true[b[:-1]]),
-                deltas=deltas, T_true=T_true)
-
-
-def params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
 
 
 def flat(x):
@@ -54,19 +23,6 @@ def run(ctx, prm, sw, frames="skewed", stamps="stamps", **kw):
     kw.setdefault("deltas", sw["deltas"] if kw.get("motion", "increments") == "increments" else None)
     ts = None if stamps is None else (sw[stamps] if isinstance(stamps, str) else stamps)
     return ctx.icp_run_odometry(prm, sw[frames], sw["T_init"], cell_size=CELL, timestamps=ts, **kw)
-
-
-def result_bytes(res):
-    out = []
-    for r in res:
-        logs = []
-        for x in r.logs:
-            y = type(x).from_buffer_copy(bytes(x))
-            y.iter_time_ms = 0.0
-            logs.append(bytes(y))
-        out.append((r.status, r.iterations, r.converged, r.n_points, r.T.tobytes(), r.T_prior.tobytes(),
-                    None if r.cov is None else r.cov.tobytes(), logs))
-    return out
 
 
 def increments(res, sw, motion):
@@ -181,29 +137,13 @@ def test_deskewing_recovers_the_unskewed_result(ctx, sweeps):
         assert np.degrees(np.arccos(np.clip((np.trace(dT[:3, :3]) - 1) / 2, -1, 1))) < 0.05
 
 
-def streamed(ctx, prm, sw, chunks, stamps_of=None, **kw):
-    """The recording pushed in chunks; stamps_of(i): whether push i carries timestamps"""
-    first = np.concatenate([[0], np.cumsum(LENS)])
-    done = [0] * len(LENS)
-    out = [[] for _ in LENS]
-    with ctx.odometry_session(prm, len(LENS), sw["T_init"], cell_size=CELL, map_frames=3, **kw) as sess:
-        for i, cnt in enumerate(chunks):
-            part = [sw["skewed"][s][done[s]:done[s] + c] for s, c in enumerate(cnt)]
-            ts = [sw["stamps"][s][done[s]:done[s] + c] for s, c in enumerate(cnt)]
-            D = np.concatenate([sw["deltas"][first[s] + done[s]:first[s] + done[s] + c] for s, c in enumerate(cnt)])
-            use = stamps_of(i) if stamps_of else True
-            for s, r in enumerate(sess.push(part, D, want_log=True, timestamps=ts if use else None, want_deskewed=True)):
-                out[s].extend(r)
-            done = [d + c for d, c in zip(done, cnt)]
-    return flat(out)
-
-
 @pytest.mark.parametrize("filters", [dict(), dict(source_voxel=0.25, map_voxel=0.25, map_max_points=4)])
 def test_sessions_equal_one_call(ctx, sweeps, filters):
     prm = params()
     ref = run(ctx, prm, sweeps, want_log=True, want_deskewed=True, **filters)
     for chunks in ([list(LENS)], [[1, 1]] * 5 + [[0, 1], [0, 1]], [[2, 3], [0, 1], [3, 3]]):
-        got = streamed(ctx, prm, sweeps, chunks, **filters)
+        got = flat(pushed(ctx, prm, sweeps["skewed"], sweeps["T_init"], chunks, sweeps["deltas"],
+                          stamps=sweeps["stamps"], want_log=True, want_deskewed=True, map_frames=3, **filters))
         assert result_bytes(got) == result_bytes(ref)
         assert all(a.deskewed.tobytes() == b.deskewed.tobytes() for a, b in zip(got, ref))
     # pushes without timestamps are frames with tau = 0.5
@@ -217,7 +157,8 @@ def test_sessions_equal_one_call(ctx, sweeps, filters):
                     mixed[s][j] = np.full(len(mixed[s][j]), 0.5, np.float32)
             first[s] += c
     ref = run(ctx, prm, sweeps, stamps=mixed, want_log=True, want_deskewed=True, **filters)
-    got = streamed(ctx, prm, sweeps, chunks, stamps_of=lambda i: i != 1, **filters)
+    got = flat(pushed(ctx, prm, sweeps["skewed"], sweeps["T_init"], chunks, sweeps["deltas"], stamps=sweeps["stamps"],
+                      ts_push=lambda i: i != 1, want_log=True, want_deskewed=True, map_frames=3, **filters))
     assert result_bytes(got) == result_bytes(ref)
     assert all(a.deskewed.tobytes() == b.deskewed.tobytes() for a, b in zip(got, ref))
 

@@ -10,97 +10,25 @@ import math
 import numpy as np
 import pytest
 
-from test_gpu_odometry import assert_anchor, assert_priors, assert_same_run, split
-from test_gpu_odometry_stream import LENS, RAGGED, assert_same, log_bytes, one_per_push, raw_push
+from odom_harness import (CELL, RADIUS, RAGGED, assert_anchor, assert_priors, assert_same, assert_same_flat,  # noqa: F401
+                          assert_same_run, ctx, log_bytes, map_call, odo, one_per_push, params, pushed, raw_odometry,
+                          raw_push, seq_results, split, sweeps, twin_maps, window_call)
 
 pytestmark = pytest.mark.gpu
 
-RADIUS = 0.5
-CELL = 0.5
+LENS = (1, 7, 12)
 SV, MV = 0.3, 0.25            # source and map voxel sizes
 DIST = 10.0                   # a prune distance well inside the scenes' 20 m sensor range
 dp = C.POINTER(C.c_double)
+MAP = "dcreg_icp_run_odometry_map"
+RAW_MAP = dict(source_voxel=SV, map_voxel=MV, source_max_points=1, map_max_points=4, max_distance=DIST)
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
-
-
-@pytest.fixture(scope="module")
-def odo():
-    """20 frames of one path (about 20 k points each, 20 m range) with drifting odometry, in sequences of 1, 7 and 12"""
-    from dcreg_b200.scenes import make_parking_sequence
-    frames, T_true, _, deltas, _ = make_parking_sequence(20, seed=71, n_scan=20_000, max_range=20.0)
-    bounds = np.concatenate([[0], np.cumsum(LENS)])
-    seqs = [list(frames[a:b]) for a, b in zip(bounds[:-1], bounds[1:])]
-    return seqs, np.ascontiguousarray(T_true[bounds[:-1]]), deltas
-
-
-@pytest.fixture(scope="module")
-def sweeps():
-    """12 skewed sweeps with per-point timestamps in sequences of 5 and 7 frames (unskewed anchors)"""
-    from dcreg_b200.scenes import make_parking_sweeps
-    skewed, stamps, T_true, deltas, frames = make_parking_sweeps(12, seed=71, n_scan=20_000, max_range=20.0)
-    b = [0, 5, 12]
-    for a in b[:-1]:
-        skewed[a] = frames[a]
-    cut = lambda x: [list(x[p:q]) for p, q in zip(b[:-1], b[1:])]        # noqa: E731
-    return dict(skewed=cut(skewed), stamps=cut(stamps), T_init=np.ascontiguousarray(T_true[b[:-1]]), deltas=deltas)
-
-
-def params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
-
-
-def seq_results(res, seqs):
-    return [list(r) for r in split(res, seqs)]
-
-
-def twin_maps(seq, rs, sv, cap, dist, frames=None):
-    """The twin's maps M_1 .. M_n of one sequence from its results: M_{k+1} = voxel_map_update(M_k, F_s(frame k), T_out[k])
-    (frames: the frames as inserted, e.g. deskewed; default F_s(seq[k]))"""
-    from dcreg_b200.api import voxel_downsample, voxel_map_update
-    M = np.zeros((0, 3), np.float32)
-    out = [None]
-    for k in range(len(rs)):
-        P = frames[k] if frames is not None else (voxel_downsample(seq[k], sv, 1)[0] if sv else seq[k])
-        M = voxel_map_update(M, P, rs[k].T, MV, cap, dist)
-        out.append(M)
-    return out
-
-
-def map_session(ctx, prm, seqs, T_init, chunks, deltas=None, stamps=None, ts_push=None, between=None, **kw):
-    """The recording pushed in `chunks`; returns (results per sequence, [local maps of every sequence after each push]).
-    stamps: per-frame timestamps nested like seqs, sent with the pushes where ts_push(i) (default: all)."""
-    first = np.concatenate([[0], np.cumsum([len(s) for s in seqs])])
-    done = [0] * len(seqs)
-    out = [[] for _ in seqs]
+def map_session(ctx, prm, seqs, T_init, chunks, deltas=None, **kw):
+    """The recording pushed in `chunks` into a voxel-map session, with logs and covariances: (results per sequence,
+    [local maps of every sequence after each push])"""
     maps = []
-    with ctx.odometry_map_session(prm, len(seqs), T_init, cell_size=CELL, **kw) as sess:
-        for i, cnt in enumerate(chunks):
-            part = [seqs[s][done[s]:done[s] + c] for s, c in enumerate(cnt)]
-            D = None
-            if deltas is not None:
-                D = np.concatenate([deltas[first[s] + done[s]:first[s] + done[s] + c] for s, c in enumerate(cnt)])
-            ts = None
-            if stamps is not None and (ts_push is None or ts_push(i)):
-                ts = [stamps[s][done[s]:done[s] + c] for s, c in enumerate(cnt)]
-            for s, r in enumerate(sess.push(part, D, want_log=True, want_cov=True, timestamps=ts)):
-                assert len(r) == cnt[s]
-                out[s].extend(r)
-            done = [d + c for d, c in zip(done, cnt)]
-            maps.append([sess.local_map(s) for s in range(len(seqs))])
-            if between:
-                between(i)
+    out = pushed(ctx, prm, seqs, T_init, chunks, deltas, voxel_map=True, maps=maps, want_log=True, want_cov=True, **kw)
     return out, maps
 
 
@@ -114,31 +42,13 @@ def test_local_map_equals_twin_after_every_push(ctx, odo, cap, sv):
                             map_max_points=cap, max_distance=DIST)
     pruned = 0
     for s, (seq, rs) in enumerate(zip(seqs, res)):
-        twin = twin_maps(seq, rs, sv, cap, DIST)
+        twin = twin_maps(seq, rs, sv, MV, cap, DIST)
         for i in range(len(maps)):
             k = min(i + 1, len(seq))                    # frames of sequence s pushed after push i
             assert maps[i][s].tobytes() == twin[k].tobytes(), (s, i)
         every = np.concatenate([map_points(r.T, voxel_downsample(f, sv, 1)[0] if sv else f) for f, r in zip(seq, rs)])
         pruned += len(voxel_downsample(every, MV, cap)[0]) - len(twin[-1])
     assert pruned > 0
-
-
-def window_call(ctx, prm, seqs, T_init, deltas, **kw):
-    return ctx.icp_run_odometry(prm, seqs, T_init, deltas, map_frames=max(len(s) for s in seqs) + 3, cell_size=CELL,
-                                want_log=True, want_cov=True, **kw)
-
-
-def map_call(ctx, prm, seqs, T_init, deltas, dist, **kw):
-    return ctx.icp_run_odometry_map(prm, seqs, T_init, deltas, max_distance=dist, cell_size=CELL,
-                                    want_log=True, want_cov=True, **kw)
-
-
-def assert_same_flat(a, b):
-    assert_same([a], [b])
-    for x, y in zip(a, b):
-        assert (x.deskewed is None) == (y.deskewed is None)
-        if x.deskewed is not None:
-            assert x.deskewed.tobytes() == y.deskewed.tobytes()
 
 
 @pytest.mark.parametrize("motion", ["increments", "constant_velocity"])
@@ -179,7 +89,7 @@ def test_frames_equal_their_reconstruction(ctx, odo, method):
     assert_priors(res, seqs, T_init, deltas)
     for s, (seq, rs) in enumerate(zip(seqs, split(res, seqs))):
         assert_anchor(rs[0], T_init[s])
-        twin = twin_maps(seq, rs, SV, 4, DIST)
+        twin = twin_maps(seq, rs, SV, MV, 4, DIST)
         for k in range(1, len(seq)):
             ctx.set_target(twin[k], CELL)
             ctx.set_source(voxel_downsample(seq[k], SV, 1)[0])
@@ -194,7 +104,7 @@ def test_deskewed_frames_enter_the_map(ctx, sweeps):
     res = map_call(ctx, prm, sw["skewed"], sw["T_init"], sw["deltas"], DIST, source_voxel=SV, map_voxel=MV,
                    map_max_points=4, timestamps=sw["stamps"], want_deskewed=True)
     for seq, rs in zip(sw["skewed"], split(res, sw["skewed"])):
-        twin = twin_maps(seq, rs, SV, 4, DIST, frames=[r.deskewed for r in rs])
+        twin = twin_maps(seq, rs, SV, MV, 4, DIST, frames=[r.deskewed for r in rs])
         for k in range(1, len(seq)):
             ctx.set_target(twin[k], CELL)
             ctx.set_source(rs[k].deskewed)
@@ -214,7 +124,7 @@ def test_session_chunkings_equal_one_call(ctx, odo, chunking):
     got, maps = map_session(ctx, prm, seqs, T_init, CHUNKS[chunking], deltas, max_distance=DIST, **kw)
     assert_same(got, seq_results(ref, seqs))
     for s, (seq, rs) in enumerate(zip(seqs, got)):                 # the last maps hold every frame
-        assert maps[-1][s].tobytes() == twin_maps(seq, rs, SV, 4, DIST)[-1].tobytes()
+        assert maps[-1][s].tobytes() == twin_maps(seq, rs, SV, MV, 4, DIST)[-1].tobytes()
 
 
 def test_session_constant_velocity_across_pushes(ctx, odo):
@@ -310,7 +220,7 @@ def test_failed_pushes_change_nothing(ctx, odo):
         got += sess.push([seq[3:]], D[3:], want_log=True, want_cov=True)[0]
         final = sess.local_map(0)
     assert_same([got], ref)
-    assert final.tobytes() == twin_maps(seq, got, 0.0, 4, DIST)[-1].tobytes()
+    assert final.tobytes() == twin_maps(seq, got, 0.0, MV, 4, DIST)[-1].tobytes()
 
 
 def test_empty_map_fails_at_its_step(ctx, odo):
@@ -356,32 +266,6 @@ def test_more_sequences_than_map_points(ctx, odo):
         assert [sess.local_map(s).tobytes() for s in range(S)] == [w.tobytes() for w in want]
 
 
-def raw_map_call(ctx, prm, seqs, T_init, deltas, map_voxel=MV, cap=4, dist=DIST, log_cap=30):
-    """dcreg_icp_run_odometry_map with every output, log times zeroed: (rc, dict of arrays)"""
-    from dcreg_b200 import api
-    frames = [f for s in seqs for f in s]
-    n = len(frames)
-    xyz = np.ascontiguousarray(np.concatenate(frames), dtype=np.float32)
-    off = np.zeros(n + 1, np.int64); off[1:] = np.cumsum([len(f) for f in frames])
-    so = np.zeros(len(seqs) + 1, np.int32); so[1:] = np.cumsum([len(s) for s in seqs])
-    out = dict(T_prior=np.full((n, 4, 4), -1.0), T_out=np.full((n, 4, 4), -1.0), n_it=np.full(n, -1, np.int32),
-               conv=np.full(n, -1, np.int32), st=np.full(n, -1, np.int32), cov=np.full((n, 36), -1.0),
-               npts=np.full(n, -1, np.int64), log=np.zeros(max(n * log_cap, 1) * C.sizeof(api.IterLog), np.uint8))
-    T0 = np.ascontiguousarray(T_init, dtype=np.float64)
-    D = None if deltas is None else np.ascontiguousarray(deltas, dtype=np.float64)
-    ip = lambda a: a.ctypes.data_as(C.POINTER(C.c_int))                       # noqa: E731
-    rc = ctx.lib.dcreg_icp_run_odometry_map(
-        ctx._h, C.byref(prm), len(seqs), ip(so), n, xyz.ctypes.data_as(C.POINTER(C.c_float)),
-        off.ctypes.data_as(C.POINTER(C.c_int64)), 3, CELL, 0, SV, float(map_voxel), 1, int(cap), float(dist),
-        T0.ctypes.data_as(dp), D.ctypes.data_as(dp) if D is not None else None, None,
-        out["npts"].ctypes.data_as(C.POINTER(C.c_int64)), out["T_prior"].ctypes.data_as(dp),
-        out["T_out"].ctypes.data_as(dp), ip(out["n_it"]), ip(out["conv"]), ip(out["st"]), out["cov"].ctypes.data_as(dp),
-        None, C.cast(out["log"].ctypes.data, C.POINTER(api.IterLog)) if log_cap else None, log_cap)
-    for rec in (api.IterLog * (n * log_cap)).from_buffer(out["log"]):
-        rec.iter_time_ms = 0.0
-    return rc, out
-
-
 def test_reproducible_and_context_intact(ctx, odo):
     seqs, T_init, deltas = odo
     prm = params()
@@ -389,8 +273,8 @@ def test_reproducible_and_context_intact(ctx, odo):
     ctx.set_target(np.concatenate(frames[:3]), CELL)
     ctx.set_source(frames[1])
     one = ctx.icp_run(prm, T_init[1])
-    rc_a, a = raw_map_call(ctx, prm, seqs, T_init, deltas)
-    rc_b, b = raw_map_call(ctx, prm, seqs, T_init, deltas)
+    rc_a, a = raw_odometry(ctx, MAP, prm, seqs, T_init, deltas, log_cap=30, **RAW_MAP)
+    rc_b, b = raw_odometry(ctx, MAP, prm, seqs, T_init, deltas, log_cap=30, **RAW_MAP)
     assert rc_a == rc_b == 0
     for k in a:
         assert a[k].tobytes() == b[k].tobytes(), k
@@ -399,7 +283,7 @@ def test_reproducible_and_context_intact(ctx, odo):
     assert [log_bytes(x) for x in again.logs] == [log_bytes(y) for y in one.logs]
     from dcreg_b200 import Context
     with Context(0) as fresh:
-        rc, c = raw_map_call(fresh, prm, seqs, T_init, deltas)
+        rc, c = raw_odometry(fresh, MAP, prm, seqs, T_init, deltas, log_cap=30, **RAW_MAP)
         assert rc == 0
         for k in a:
             assert a[k].tobytes() == c[k].tobytes(), k
@@ -415,7 +299,7 @@ def test_launches_per_step_do_not_depend_on_sequences(ctx, odo):
     counts = []
     for ss, T0 in ((one, T_init[2:3]), (three, np.stack([T_init[1], T_init[2], T_init[2]]))):
         a = ctx.launch_count
-        rc, _ = raw_map_call(ctx, prm, ss, T0, None, log_cap=0)
+        rc, _ = raw_odometry(ctx, MAP, prm, ss, T0, None, **RAW_MAP)
         assert rc == 0
         counts.append(ctx.launch_count - a)
     assert counts[0] == counts[1], counts
@@ -442,7 +326,8 @@ def test_bad_arguments(ctx, odo):
                                 (math.nan, 4, DIST, "map_voxel"), (MV, 0, DIST, "max_points"),
                                 (MV, 4, 0.0, "max_distance"), (MV, 4, -1.0, "max_distance"),
                                 (MV, 4, math.nan, "max_distance")):
-        rc, out = raw_map_call(ctx, prm, [seq], T_init[2:3], deltas[8:12], mv, cap, dist)
+        rc, out = raw_odometry(ctx, MAP, prm, [seq], T_init[2:3], deltas[8:12], log_cap=30,
+                               **(RAW_MAP | dict(map_voxel=mv, map_max_points=cap, max_distance=dist)))
         assert rc == api.BAD_ARG, (mv, cap, dist)
         assert what in lib.dcreg_last_error(h).decode(), (mv, cap, dist)
         assert np.all(out["n_it"] == -1)

@@ -3,52 +3,15 @@
 Every comparison is byte for byte against one icp_run_odometry call over the same frames with the session's settings:
 T_out, T_prior, status, iterations, converged, n_points, cov, and every log record with iter_time_ms zeroed.
 """
-import ctypes as C
-
 import numpy as np
 import pytest
 
+from odom_harness import (CELL, RADIUS, RAGGED, assert_same, ctx, log_bytes, odo, one_per_push, params,  # noqa: F401
+                          pushed, raw_push, split)
+
 pytestmark = pytest.mark.gpu
 
-RADIUS = 0.5
-CELL = 0.5
 LENS = (1, 7, 12)
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
-
-
-@pytest.fixture(scope="module")
-def odo():
-    """The scene of tests/test_gpu_odometry.py: 20 frames of one path (about 20 k points each), sequences of 1, 7 and 12
-    frames, T_init the true pose of each sequence's first frame."""
-    from dcreg_b200.scenes import make_parking_sequence
-    frames, T_true, _, deltas, _ = make_parking_sequence(20, seed=71, n_scan=20_000, max_range=20.0)
-    bounds = np.concatenate([[0], np.cumsum(LENS)])
-    seqs = [list(frames[a:b]) for a, b in zip(bounds[:-1], bounds[1:])]
-    return seqs, np.ascontiguousarray(T_true[bounds[:-1]]), deltas
-
-
-def params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
-
-
-def one_per_push(lens):
-    """Pushes of one frame per sequence while it has frames"""
-    return [[1 if k < n else 0 for n in lens] for k in range(max(lens))]
-
-
-RAGGED = [[1, 2, 0], [0, 0, 5], [0, 3, 1], [0, 2, 6]]     # sequences at different rates, with empty entries
 
 
 def chunkings(lens):
@@ -56,55 +19,7 @@ def chunkings(lens):
 
 
 def one_call(ctx, prm, seqs, T_init, deltas=None, **kw):
-    res = ctx.icp_run_odometry(prm, seqs, T_init, deltas, cell_size=CELL, **kw)
-    out, k = [], 0
-    for s in seqs:
-        out.append(res[k:k + len(s)])
-        k += len(s)
-    return out
-
-
-def streamed(ctx, prm, seqs, T_init, chunks, deltas=None, want_log=False, want_cov=False, between=None, **kw):
-    """The recording pushed in `chunks` (per push, the frames of every sequence); deltas: the one call's deltas, cut
-    into the pushes' entries.  between(i): run after push i.  Returns one list of results per sequence."""
-    first = np.concatenate([[0], np.cumsum([len(s) for s in seqs])])
-    done = [0] * len(seqs)
-    out = [[] for _ in seqs]
-    with ctx.odometry_session(prm, len(seqs), T_init, cell_size=CELL, **kw) as sess:
-        for i, cnt in enumerate(chunks):
-            part = [seqs[s][done[s]:done[s] + c] for s, c in enumerate(cnt)]
-            D = None
-            if deltas is not None:
-                D = np.concatenate([deltas[first[s] + done[s]:first[s] + done[s] + c] for s, c in enumerate(cnt)])
-            for s, r in enumerate(sess.push(part, D, want_log=want_log, want_cov=want_cov)):
-                assert len(r) == cnt[s]
-                out[s].extend(r)
-            done = [d + c for d, c in zip(done, cnt)]
-            if between:
-                between(i)
-    assert done == [len(s) for s in seqs]
-    return out
-
-
-def log_bytes(rec):
-    r = type(rec).from_buffer_copy(bytes(rec))
-    r.iter_time_ms = 0.0
-    return bytes(r)
-
-
-def assert_same(a_seqs, b_seqs):
-    assert [len(x) for x in a_seqs] == [len(x) for x in b_seqs]
-    for s, (xa, xb) in enumerate(zip(a_seqs, b_seqs)):
-        for k, (a, b) in enumerate(zip(xa, xb)):
-            where = (s, k)
-            assert (a.status, a.iterations, a.converged, a.n_points) == (b.status, b.iterations, b.converged, b.n_points), where
-            assert a.T.tobytes() == b.T.tobytes(), where
-            assert a.T_prior.tobytes() == b.T_prior.tobytes(), where
-            assert (a.cov is None) == (b.cov is None), where
-            if a.cov is not None:
-                assert a.cov.tobytes() == b.cov.tobytes(), where
-            assert len(a.logs) == len(b.logs), where
-            assert [log_bytes(x) for x in a.logs] == [log_bytes(y) for y in b.logs], where
+    return split(ctx.icp_run_odometry(prm, seqs, T_init, deltas, cell_size=CELL, **kw), seqs)
 
 
 @pytest.mark.parametrize("method", ["Ours", "ME-TSVD"])
@@ -115,7 +30,7 @@ def test_chunkings_equal_one_call(ctx, odo, method, chunking):
     prm = params(method)
     for extra in (dict(), dict(want_log=True, want_cov=True)):
         ref = one_call(ctx, prm, seqs, T_init, deltas, map_frames=3, **extra)
-        got = streamed(ctx, prm, seqs, T_init, chunkings(LENS)[chunking], deltas, map_frames=3, **extra)
+        got = pushed(ctx, prm, seqs, T_init, chunkings(LENS)[chunking], deltas, map_frames=3, **extra)
         assert_same(got, ref)
 
 
@@ -127,9 +42,9 @@ def test_constant_velocity_across_pushes(ctx, odo, map_frames):
     prm = params()
     chunks = [[1, 1, 1]] + one_per_push([0, 6, 11])
     ref = one_call(ctx, prm, seqs, T_init, None, motion="constant_velocity", map_frames=map_frames, want_log=True)
-    got = streamed(ctx, prm, seqs, T_init, chunks, None, motion="constant_velocity", map_frames=map_frames, want_log=True)
+    got = pushed(ctx, prm, seqs, T_init, chunks, None, motion="constant_velocity", map_frames=map_frames, want_log=True)
     assert_same(got, ref)
-    ragged = streamed(ctx, prm, seqs, T_init, RAGGED, None, motion="constant_velocity", map_frames=map_frames)
+    ragged = pushed(ctx, prm, seqs, T_init, RAGGED, None, motion="constant_velocity", map_frames=map_frames)
     assert_same(ragged, one_call(ctx, prm, seqs, T_init, None, motion="constant_velocity", map_frames=map_frames))
 
 
@@ -140,7 +55,7 @@ def test_filters(ctx, odo, filters):
     prm = params()
     ref = one_call(ctx, prm, seqs, T_init, deltas, map_frames=3, want_cov=True, **filters)
     for chunks in (one_per_push(LENS), RAGGED):
-        got = streamed(ctx, prm, seqs, T_init, chunks, deltas, map_frames=3, want_cov=True, **filters)
+        got = pushed(ctx, prm, seqs, T_init, chunks, deltas, map_frames=3, want_cov=True, **filters)
         assert_same(got, ref)
     if "source_voxel" in filters:
         assert all(r.n_points < 20_000 for rs in ref for r in rs)
@@ -155,7 +70,7 @@ def test_aborted_frame_enters_later_maps(ctx, odo):
     prm = params()
     ref = one_call(ctx, prm, [seq], T_init[2:3], deltas[8:15], map_frames=3, want_log=True)
     assert ref[0][2].status == api.NOT_ENOUGH_POINTS
-    got = streamed(ctx, prm, [seq], T_init[2:3], [[2], [1], [1], [3]], deltas[8:15], map_frames=3, want_log=True)
+    got = pushed(ctx, prm, [seq], T_init[2:3], [[2], [1], [1], [3]], deltas[8:15], map_frames=3, want_log=True)
     assert_same(got, ref)
 
 
@@ -165,7 +80,7 @@ def test_fixed_iterations(ctx, odo, method):
     prm = params(method, fixed_iterations=1, max_iterations=5)
     ref = one_call(ctx, prm, seqs, T_init, deltas, map_frames=3)
     assert all(r.iterations == 5 for rs in ref for r in rs[1:])
-    assert_same(streamed(ctx, prm, seqs, T_init, one_per_push(LENS), deltas, map_frames=3), ref)
+    assert_same(pushed(ctx, prm, seqs, T_init, one_per_push(LENS), deltas, map_frames=3), ref)
 
 
 def test_other_calls_between_pushes(ctx, odo):
@@ -193,30 +108,13 @@ def test_other_calls_between_pushes(ctx, odo):
         else:
             ctx.voxel_downsample([seqs[2][3], seqs[1][2]], 0.3, 2)
 
-    got = streamed(ctx, prm, seqs, T_init, one_per_push(LENS), deltas, map_frames=3, want_log=True, between=between)
+    got = pushed(ctx, prm, seqs, T_init, one_per_push(LENS), deltas, map_frames=3, want_log=True, between=between)
     assert_same(got, ref)
     after = ctx.icp_run(prm, T_init[2])
     for r in seen + [after]:
         assert (r.status, r.iterations, r.converged) == (before.status, before.iterations, before.converged)
         assert r.T.tobytes() == before.T.tobytes()
         assert [log_bytes(x) for x in r.logs] == [log_bytes(y) for y in before.logs]
-
-
-def raw_push(ctx, seq_off, frames, deltas=None, stride=3, offsets=None, n=None):
-    """dcreg_odometry_push through ctypes, for tables the Python binding would not build"""
-    dp = C.POINTER(C.c_double)
-    so = np.ascontiguousarray(seq_off, dtype=np.int32)
-    n = int(so[-1]) if n is None else n
-    xyz = np.ascontiguousarray(np.concatenate(frames) if frames else np.zeros((1, 3)), dtype=np.float32)
-    if offsets is None:
-        offsets = np.concatenate([[0], np.cumsum([len(f) for f in frames])]).astype(np.int64)
-    T_out = np.empty((max(n, 1), 4, 4))
-    D = None if deltas is None else np.ascontiguousarray(deltas, dtype=np.float64)
-    return ctx.lib.dcreg_odometry_push(ctx._h, so.ctypes.data_as(C.POINTER(C.c_int)), n,
-                                       xyz.ctypes.data_as(C.POINTER(C.c_float)),
-                                       np.ascontiguousarray(offsets, np.int64).ctypes.data_as(C.POINTER(C.c_int64)), stride,
-                                       D.ctypes.data_as(dp) if D is not None else None, None, None, T_out.ctypes.data_as(dp),
-                                       None, None, None, None, None, 0)
 
 
 def test_failed_map_push_changes_nothing(ctx, odo):
@@ -249,7 +147,7 @@ def test_pre_launch_errors_change_nothing(ctx, odo):
     short = [s[:4] for s in seqs]
     dl = np.concatenate([deltas[0:1], deltas[1:5], deltas[8:12]])
     ref = one_call(ctx, prm, short, T_init, dl, map_frames=3, source_voxel=0.25, want_log=True)
-    assert lib.dcreg_odometry_push(h, None, 1, None, None, 3, None, None, None, None, None, None, None, None, None, 0) == api.BAD_ARG
+    assert api._odometry_call(lib, h, "dcreg_odometry_push", n_frames=1, stride=3, log_cap=0) == api.BAD_ARG
     assert "no session" in lib.dcreg_last_error(h).decode()
     assert lib.dcreg_odometry_close(h) == api.BAD_ARG
     nan = np.full((50, 3), np.nan, np.float32)

@@ -5,64 +5,24 @@ Every registered frame of a filtered call is checked against its reconstruction 
 voxel_downsample(frame k, source_voxel), its map voxel_downsample(concatenation of map_points(T_out[j], filtered frame
 j) over the window, map_voxel), then set_target + set_source + icp_run(T_prior[k]) with the tolerances of
 tests/test_gpu_odometry.py."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
-from test_gpu_odometry import CELL, assert_anchor, assert_priors, assert_same_run, params, split
+from odom_harness import (CELL, assert_anchor, assert_priors, assert_same_run, clouds_of_every_case, ctx,  # noqa: F401
+                          parking, params, raw_downsample, raw_odometry, reconstruct, split)
 
 pytestmark = pytest.mark.gpu
 
 SV, MV = 0.3, 0.25            # source and map voxel sizes of the tests
-dp = C.POINTER(C.c_double)
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
+VOXEL = "dcreg_icp_run_odometry_voxel"
+FIRST = "dcreg_voxel_downsample"
 
 
 @pytest.fixture(scope="module")
 def odo():
     """20 frames of about 20 k points of one path with drifting odometry, in sequences of 1, 7 and 12 frames."""
-    from dcreg_b200.scenes import make_parking_sequence
-    frames, T_true, _, deltas, _ = make_parking_sequence(20, seed=71, n_scan=20_000, max_range=20.0)
-    bounds = [0, 1, 8, 20]
-    seqs = [frames[a:b] for a, b in zip(bounds[:-1], bounds[1:])]
-    return seqs, frames, T_true[bounds[:-1]], deltas, T_true
-
-
-def clouds_of_every_case():
-    rng = np.random.default_rng(11)
-    g = np.arange(-5, 5, dtype=np.float64) * 0.25
-    lattice = np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3).astype(np.float32)
-    lattice = np.concatenate([lattice, np.nextafter(lattice, np.float32(-np.inf))])
-    dup = rng.uniform(-3, 3, (300, 3)).astype(np.float32)
-    holes = rng.uniform(-3, 3, (700, 3)).astype(np.float32)
-    holes[::5, 0] = np.nan
-    holes[2::9, 1] = np.inf
-    holes[4::13, 2] = -np.inf
-    return [rng.standard_normal((5000, 3)).astype(np.float32) * 4, lattice, np.concatenate([dup, dup, dup[::-1]]), holes,
-            np.array([[-0.1, 0.2, -0.3]], np.float32), (rng.standard_normal((20000, 3)) * 30).astype(np.float32)]
-
-
-def raw_downsample(ctx, clouds, voxel, stride=3, want_index=True):
-    """dcreg_voxel_downsample on (N_b, stride) clouds: (rc, points, offsets, index)"""
-    xyz = np.ascontiguousarray(np.concatenate([np.asarray(c, np.float32)[:, :stride] for c in clouds]), dtype=np.float32)
-    off = np.zeros(len(clouds) + 1, np.int64)
-    off[1:] = np.cumsum([len(c) for c in clouds])
-    pts = np.empty((max(len(xyz), 1), 3), np.float32)
-    kept = np.zeros(len(clouds) + 1, np.int64)
-    idx = np.empty(max(len(xyz), 1), np.int64)
-    rc = ctx.lib.dcreg_voxel_downsample(ctx._h, len(clouds), xyz.ctypes.data_as(C.POINTER(C.c_float)),
-                                        off.ctypes.data_as(C.POINTER(C.c_int64)), stride, float(voxel),
-                                        pts.ctypes.data_as(C.POINTER(C.c_float)), kept.ctypes.data_as(C.POINTER(C.c_int64)),
-                                        idx.ctypes.data_as(C.POINTER(C.c_int64)) if want_index else None)
-    return rc, pts, kept, idx
+    seqs, T_init, deltas, frames, T_true = parking()
+    return seqs, frames, T_init, deltas, T_true
 
 
 @pytest.mark.parametrize("voxel", [0.1, 0.25, 1.0])
@@ -77,12 +37,12 @@ def test_downsample_equals_twin(ctx, voxel):
     # stride 4 (xyzi), the same selection; without the index output
     rng = np.random.default_rng(12)
     c4 = [np.concatenate([c, rng.uniform(0, 1, (len(c), 1)).astype(np.float32)], axis=1) for c in clouds]
-    rc, pts, kept, idx = raw_downsample(ctx, c4, voxel, stride=4)
+    rc, pts, kept, idx = raw_downsample(ctx, FIRST, c4, voxel, stride=4)
     assert rc == 0
     for b, c in enumerate(clouds):
         tp, ti = voxel_downsample(c, voxel)
         assert pts[kept[b]:kept[b + 1]].tobytes() == tp.tobytes() and np.array_equal(idx[kept[b]:kept[b + 1]], ti)
-    rc, pts2, kept2, _ = raw_downsample(ctx, c4, voxel, stride=4, want_index=False)
+    rc, pts2, kept2, _ = raw_downsample(ctx, FIRST, c4, voxel, stride=4, want_index=False)
     assert rc == 0 and np.array_equal(kept2, kept) and pts2[:kept[-1]].tobytes() == pts[:kept[-1]].tobytes()
 
 
@@ -99,16 +59,16 @@ def test_downsample_bad_arguments(ctx):
     from dcreg_b200 import api
     good = [np.zeros((3, 3), np.float32), np.ones((2, 3), np.float32)]
     far = [good[0], np.array([[0.0, 0.0, 0.0], [3.0e5, 0.0, 0.0]], np.float32)]
-    rc, _, _, _ = raw_downsample(ctx, far, 0.25)                             # 1.2e6 voxels > 2^20
+    rc, _, _, _ = raw_downsample(ctx, FIRST, far, 0.25)                      # 1.2e6 voxels > 2^20
     assert rc == api.BAD_ARG and "cloud 1" in ctx.lib.dcreg_last_error(ctx._h).decode()
     with pytest.raises(ValueError):
         api.voxel_downsample(far[1], 0.25)
-    assert raw_downsample(ctx, far, 1.0)[0] == api.OK
+    assert raw_downsample(ctx, FIRST, far, 1.0)[0] == api.OK
     launches = ctx.launch_count
     for v in (0.0, -0.5, np.nan, np.inf):
-        assert raw_downsample(ctx, good, v)[0] == api.BAD_ARG, v
-    assert raw_downsample(ctx, good, 0.5, stride=2)[0] == api.BAD_ARG
-    assert raw_downsample(ctx, [good[0], good[0][:0], good[1]], 0.5)[0] == api.BAD_ARG       # an empty cloud
+        assert raw_downsample(ctx, FIRST, good, v)[0] == api.BAD_ARG, v
+    assert raw_downsample(ctx, FIRST, good, 0.5, stride=2)[0] == api.BAD_ARG
+    assert raw_downsample(ctx, FIRST, [good[0], good[0][:0], good[1]], 0.5)[0] == api.BAD_ARG      # an empty cloud
     with pytest.raises(api.DcregError) as e:
         ctx.voxel_downsample([], 0.5)
     assert e.value.status == api.BAD_ARG
@@ -116,46 +76,14 @@ def test_downsample_bad_arguments(ctx):
     assert ctx.voxel_downsample(good, 0.5)[1][1].tolist() == [0]             # the context stays usable
 
 
-def raw_odometry(ctx, prm, seqs, T_init, deltas, map_frames=3, voxel=None, motion=0, log_cap=0):
-    """dcreg_icp_run_odometry (voxel None) or dcreg_icp_run_odometry_voxel (voxel = (source, map)) with every output:
-    (rc, dict of output arrays)"""
-    from dcreg_b200 import api
-    frames = [f for s in seqs for f in s]
-    n = len(frames)
-    xyz = np.ascontiguousarray(np.concatenate(frames), dtype=np.float32)
-    off = np.zeros(n + 1, np.int64); off[1:] = np.cumsum([len(f) for f in frames])
-    so = np.zeros(len(seqs) + 1, np.int32); so[1:] = np.cumsum([len(s) for s in seqs])
-    out = dict(T_prior=np.full((n, 4, 4), -1.0), T_out=np.full((n, 4, 4), -1.0), n_it=np.full(n, -1, np.int32),
-               conv=np.full(n, -1, np.int32), st=np.full(n, -1, np.int32), cov=np.full((n, 36), -1.0),
-               npts=np.full(n, -1, np.int64), log=np.zeros(max(n * log_cap, 1) * C.sizeof(api.IterLog), np.uint8))
-    T0 = np.ascontiguousarray(T_init, dtype=np.float64)
-    D = None if deltas is None else np.ascontiguousarray(deltas, dtype=np.float64)
-    ip = lambda a: a.ctypes.data_as(C.POINTER(C.c_int))                       # noqa: E731
-    head = (ctx._h, C.byref(prm), len(seqs), ip(so), n, xyz.ctypes.data_as(C.POINTER(C.c_float)),
-            off.ctypes.data_as(C.POINTER(C.c_int64)), 3, CELL, map_frames, motion)
-    tail = (out["T_prior"].ctypes.data_as(dp), out["T_out"].ctypes.data_as(dp), ip(out["n_it"]), ip(out["conv"]),
-            ip(out["st"]), out["cov"].ctypes.data_as(dp),
-            C.cast(out["log"].ctypes.data, C.POINTER(api.IterLog)) if log_cap else None,
-            log_cap)
-    Dp = D.ctypes.data_as(dp) if D is not None else None
-    if voxel is None:
-        rc = ctx.lib.dcreg_icp_run_odometry(*head, T0.ctypes.data_as(dp), Dp, *tail)
-    else:
-        rc = ctx.lib.dcreg_icp_run_odometry_voxel(*head, float(voxel[0]), float(voxel[1]), T0.ctypes.data_as(dp), Dp,
-                                                  out["npts"].ctypes.data_as(C.POINTER(C.c_int64)), *tail)
-    for rec in (api.IterLog * (n * log_cap)).from_buffer(out["log"]):
-        rec.iter_time_ms = 0.0                                                 # a device clock reading: differs per run
-    return rc, out
-
-
 def test_zero_voxels_are_the_existing_call(ctx, odo):
     """(0, 0): the same launches and the same bytes in every output as dcreg_icp_run_odometry."""
     seqs, _, T_init, deltas, _ = odo
     prm = params()
     a0 = ctx.launch_count
-    rc_a, a = raw_odometry(ctx, prm, seqs, T_init, deltas, log_cap=30)
+    rc_a, a = raw_odometry(ctx, "dcreg_icp_run_odometry", prm, seqs, T_init, deltas, log_cap=30)
     a1 = ctx.launch_count
-    rc_b, b = raw_odometry(ctx, prm, seqs, T_init, deltas, voxel=(0.0, 0.0), log_cap=30)
+    rc_b, b = raw_odometry(ctx, VOXEL, prm, seqs, T_init, deltas, source_voxel=0.0, map_voxel=0.0, log_cap=30)
     assert ctx.launch_count - a1 == a1 - a0
     assert rc_a == rc_b == 0
     for k in ("T_prior", "T_out", "n_it", "conv", "st", "cov", "log"):
@@ -164,20 +92,6 @@ def test_zero_voxels_are_the_existing_call(ctx, odo):
     res = ctx.icp_run_odometry(prm, seqs, T_init, deltas, map_frames=3, cell_size=CELL)
     assert [r.n_points for r in res] == b["npts"].tolist()
     assert all(r.T.tobytes() == T.tobytes() for r, T in zip(res, a["T_out"]))
-
-
-def filtered_map(seq, res_seq, k, map_frames, sv, mv):
-    from dcreg_b200.api import map_points, voxel_downsample
-    fs = (lambda P: voxel_downsample(P, sv)[0]) if sv else (lambda P: P)
-    M = np.concatenate([map_points(res_seq[j].T, fs(seq[j])) for j in range(max(0, k - map_frames), k)])
-    return voxel_downsample(M, mv)[0] if mv else M
-
-
-def reconstruct(ctx, prm, seq, res_seq, k, map_frames, sv, mv):
-    from dcreg_b200.api import voxel_downsample
-    ctx.set_target(filtered_map(seq, res_seq, k, map_frames, sv, mv), CELL)
-    ctx.set_source(voxel_downsample(seq[k], sv)[0] if sv else seq[k])
-    return ctx.icp_run(prm, res_seq[k].T_prior)
 
 
 @pytest.mark.parametrize("voxels", [(SV, 0.0), (0.0, MV), (SV, MV)], ids=["source", "map", "both"])
@@ -216,8 +130,8 @@ def test_filtered_reproducible_and_context_intact(ctx, odo):
     ctx.set_target(np.concatenate(frames[:3]), CELL)
     ctx.set_source(frames[1])
     one = ctx.icp_run(prm, T_true[1])
-    rc_a, a = raw_odometry(ctx, prm, seqs, T_init, deltas, voxel=(SV, MV), log_cap=30)
-    rc_b, b = raw_odometry(ctx, prm, seqs, T_init, deltas, voxel=(SV, MV), log_cap=30)
+    rc_a, a = raw_odometry(ctx, VOXEL, prm, seqs, T_init, deltas, source_voxel=SV, map_voxel=MV, log_cap=30)
+    rc_b, b = raw_odometry(ctx, VOXEL, prm, seqs, T_init, deltas, source_voxel=SV, map_voxel=MV, log_cap=30)
     assert rc_a == rc_b == 0
     for k in a:
         assert a[k].tobytes() == b[k].tobytes(), k
@@ -238,7 +152,8 @@ def test_launches_per_step_do_not_depend_on_sequences(ctx, odo):
     for name, ss, T0 in (("one", one, T_init[2:3]), ("three", three, T3)):
         for vox in (None, (SV, MV)):
             a = ctx.launch_count
-            rc, _ = raw_odometry(ctx, prm, ss, T0, None, voxel=vox)
+            entry, sizes = (VOXEL, dict(source_voxel=SV, map_voxel=MV)) if vox else ("dcreg_icp_run_odometry", {})
+            rc, _ = raw_odometry(ctx, entry, prm, ss, T0, None, **sizes)
             assert rc == 0
             counts[name, vox] = ctx.launch_count - a
     assert counts["one", None] == counts["three", None] and counts["one", (SV, MV)] == counts["three", (SV, MV)]
@@ -256,7 +171,7 @@ def test_filtered_odometry_bad_arguments(ctx, odo):
     D = deltas[8:14]
     launches = ctx.launch_count
     for vox in ((-0.1, 0.0), (0.0, -1.0), (np.nan, 0.0), (0.0, np.inf)):
-        rc, _ = raw_odometry(ctx, prm, [seq], T0, D, voxel=vox)
+        rc, _ = raw_odometry(ctx, VOXEL, prm, [seq], T0, D, source_voxel=vox[0], map_voxel=vox[1])
         assert rc == api.BAD_ARG, vox
         assert "voxel" in ctx.lib.dcreg_last_error(ctx._h).decode()
     assert ctx.launch_count == launches                                        # nothing launched
@@ -274,17 +189,17 @@ def test_filtered_odometry_bad_arguments(ctx, odo):
     # and the map of frame 4 holds its points; frames 0 - 3 keep their outputs, the context stays usable
     D_far = D.copy()
     D_far[2, 0, 3] += 1.0e6
-    rc, out = raw_odometry(ctx, prm, [seq], T0, D_far, voxel=(0.0, MV))
+    rc, out = raw_odometry(ctx, VOXEL, prm, [seq], T0, D_far, source_voxel=0.0, map_voxel=MV)
     msg = ctx.lib.dcreg_last_error(ctx._h).decode()
     assert rc == api.BAD_ARG and "sequence 0" in msg and "frame 4" in msg and "voxel" in msg, msg
     assert all(out["n_it"][k] >= 0 for k in range(4)) and out["n_it"][1] > 0
     assert out["n_it"][4] == -1 and out["n_it"][5] == -1 and np.all(out["T_out"][4:] == -1.0)
     assert out["st"][3] == api.NOT_ENOUGH_POINTS and out["T_out"][3, 0, 3] > 5e5
-    rc, good = raw_odometry(ctx, prm, [seq], T0, D, voxel=(SV, MV))
+    rc, good = raw_odometry(ctx, VOXEL, prm, [seq], T0, D, source_voxel=SV, map_voxel=MV)
     assert rc == api.OK
     from dcreg_b200 import Context
     with Context(0) as fresh:
-        rc, ref = raw_odometry(fresh, prm, [seq], T0, D, voxel=(SV, MV))
+        rc, ref = raw_odometry(fresh, VOXEL, prm, [seq], T0, D, source_voxel=SV, map_voxel=MV)
         assert rc == api.OK
         for k in good:
             assert good[k].tobytes() == ref[k].tobytes(), k

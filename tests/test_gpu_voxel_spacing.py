@@ -5,52 +5,26 @@ Every registered frame of a spaced call is checked against its reconstruction wi
 voxel_downsample(window, map_voxel, map_max_points, s) for the window, and the chain of voxel_map_update(..., s) for the
 voxel map."""
 import contextlib
-import ctypes as C
 import math
 
 import numpy as np
 import pytest
 
-from test_gpu_odometry import assert_anchor, assert_priors, assert_same_run, split
-from test_gpu_odometry_map import (CELL, DIST, MV, SV, assert_same_flat, map_call, map_session, params, raw_map_call,
-                                   seq_results, window_call)
-from test_gpu_odometry_stream import LENS, RAGGED, assert_same, one_per_push
-from test_gpu_voxel_cap import crowded_clouds, raw_downsample_n
+from odom_harness import (CELL, RAGGED, assert_anchor, assert_priors, assert_same, assert_same_flat,  # noqa: F401
+                          assert_same_run, crowded_clouds, ctx, map_call, odo, one_per_push, params, pushed,
+                          raw_downsample, raw_odometry, seq_results, source_points, split, sweeps, twin_maps,
+                          window_call, window_map)
 
 pytestmark = pytest.mark.gpu
 
+LENS = (1, 7, 12)
+SV, MV = 0.3, 0.25            # source and map voxel sizes
+DIST = 10.0                   # the voxel map's prune distance
 CAP = 4
 S = MV / math.sqrt(CAP)          # KISS-ICP's spacing for the map filter of the tests
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
-
-
-@pytest.fixture(scope="module")
-def odo():
-    """20 frames of one path (about 20 k points each, 20 m range) with drifting odometry, in sequences of 1, 7 and 12"""
-    from dcreg_b200.scenes import make_parking_sequence
-    frames, T_true, _, deltas, _ = make_parking_sequence(20, seed=71, n_scan=20_000, max_range=20.0)
-    bounds = np.concatenate([[0], np.cumsum(LENS)])
-    seqs = [list(frames[a:b]) for a, b in zip(bounds[:-1], bounds[1:])]
-    return seqs, np.ascontiguousarray(T_true[bounds[:-1]]), deltas
-
-
-@pytest.fixture(scope="module")
-def sweeps():
-    """12 skewed sweeps with per-point timestamps in sequences of 5 and 7 frames (unskewed anchors)"""
-    from dcreg_b200.scenes import make_parking_sweeps
-    skewed, stamps, T_true, deltas, frames = make_parking_sweeps(12, seed=71, n_scan=20_000, max_range=20.0)
-    b = [0, 5, 12]
-    for a in b[:-1]:
-        skewed[a] = frames[a]
-    cut = lambda x: [list(x[p:q]) for p, q in zip(b[:-1], b[1:])]        # noqa: E731
-    return dict(skewed=cut(skewed), stamps=cut(stamps), T_init=np.ascontiguousarray(T_true[b[:-1]]), deltas=deltas)
+SPACED = "dcreg_voxel_downsample_spaced"
+MAP = "dcreg_icp_run_odometry_map"
+RAW_MAP = dict(source_voxel=SV, map_voxel=MV, source_max_points=1, map_max_points=4, max_distance=DIST)
 
 
 @contextlib.contextmanager
@@ -60,22 +34,6 @@ def spacing(ctx, s):
         yield
     finally:
         ctx.set_map_spacing(0.0)
-
-
-def raw_spaced(ctx, clouds, voxel, max_points, s, stride=3, want_index=True):
-    """dcreg_voxel_downsample_spaced on (N_b, stride) clouds: (rc, points, offsets, index)"""
-    xyz = np.ascontiguousarray(np.concatenate([np.asarray(c, np.float32)[:, :stride] for c in clouds]), dtype=np.float32)
-    off = np.zeros(len(clouds) + 1, np.int64)
-    off[1:] = np.cumsum([len(c) for c in clouds])
-    pts = np.empty((max(len(xyz), 1), 3), np.float32)
-    kept = np.zeros(len(clouds) + 1, np.int64)
-    idx = np.empty(max(len(xyz), 1), np.int64)
-    rc = ctx.lib.dcreg_voxel_downsample_spaced(ctx._h, len(clouds), xyz.ctypes.data_as(C.POINTER(C.c_float)),
-                                               off.ctypes.data_as(C.POINTER(C.c_int64)), stride, float(voxel),
-                                               int(max_points), float(s), pts.ctypes.data_as(C.POINTER(C.c_float)),
-                                               kept.ctypes.data_as(C.POINTER(C.c_int64)),
-                                               idx.ctypes.data_as(C.POINTER(C.c_int64)) if want_index else None)
-    return rc, pts, kept, idx
 
 
 def assert_equals_twin(pts, kept, idx, clouds, voxel, max_points, s):
@@ -105,13 +63,15 @@ def test_spaced_downsample_equals_twin(ctx, voxel, max_points):
     c4 = [np.concatenate([c, rng.uniform(0, 1, (len(c), 1)).astype(np.float32)], axis=1) for c in clouds]
     for s in (voxel / math.sqrt(max_points), 0.2 * voxel, 0.01 * voxel):
         for stride in (3, 4):
-            rc, pts, kept, idx = raw_spaced(ctx, c4, voxel, max_points, s, stride=stride)
+            rc, pts, kept, idx = raw_downsample(ctx, SPACED, c4, voxel, stride=stride, max_points=max_points,
+                                                min_spacing=s)
             assert rc == 0
             assert_equals_twin(pts, kept, idx, clouds, voxel, max_points, s)
         got = ctx.voxel_downsample(clouds, voxel, max_points, s)
         assert [p.tobytes() for p, _ in got] == [pts[a:b].tobytes() for a, b in zip(kept[:-1], kept[1:])]
-    rc, pts2, kept2, _ = raw_spaced(ctx, c4, voxel, max_points, S, stride=4, want_index=False)
-    rc3, pts3, kept3, _ = raw_spaced(ctx, c4, voxel, max_points, S, stride=4)
+    rc, pts2, kept2, _ = raw_downsample(ctx, SPACED, c4, voxel, stride=4, want_index=False, max_points=max_points,
+                                        min_spacing=S)
+    rc3, pts3, kept3, _ = raw_downsample(ctx, SPACED, c4, voxel, stride=4, max_points=max_points, min_spacing=S)
     assert rc == rc3 == 0 and np.array_equal(kept2, kept3) and pts2[:kept3[-1]].tobytes() == pts3[:kept3[-1]].tobytes()
 
 
@@ -121,12 +81,12 @@ def test_crowded_voxel_and_raw_frames(ctx, raw_frames, max_points):
     from dcreg_b200.api import voxel_downsample
     clouds = crowded_clouds()[-1:]
     for s in (0.25 / math.sqrt(min(max_points, 20)), 0.004):
-        rc, pts, kept, idx = raw_spaced(ctx, clouds, 0.25, max_points, s)
+        rc, pts, kept, idx = raw_downsample(ctx, SPACED, clouds, 0.25, max_points=max_points, min_spacing=s)
         assert rc == 0
         assert_equals_twin(pts, kept, idx, clouds, 0.25, max_points, s)
     for voxel in (0.5, 0.25):
         s = voxel / math.sqrt(min(max_points, 20))
-        rc, pts, kept, idx = raw_spaced(ctx, raw_frames, voxel, max_points, s)
+        rc, pts, kept, idx = raw_downsample(ctx, SPACED, raw_frames, voxel, max_points=max_points, min_spacing=s)
         assert rc == 0
         assert_equals_twin(pts, kept, idx, raw_frames, voxel, max_points, s)
         assert kept[-1] < sum(len(voxel_downsample(f, voxel, max_points)[1]) for f in raw_frames)
@@ -136,9 +96,9 @@ def test_zero_spacing_and_one_point_caps_are_the_n_call(ctx, raw_frames):
     clouds = crowded_clouds() + raw_frames[:1]
     for voxel, cap, s in ((0.25, 4, 0.0), (0.5, 20, 0.0), (0.25, 1, 0.1), (0.5, 1, 10.0)):
         a0 = ctx.launch_count
-        a = raw_downsample_n(ctx, clouds, voxel, cap)
+        a = raw_downsample(ctx, "dcreg_voxel_downsample_n", clouds, voxel, max_points=cap)
         a1 = ctx.launch_count
-        b = raw_spaced(ctx, clouds, voxel, cap, s)
+        b = raw_downsample(ctx, SPACED, clouds, voxel, max_points=cap, min_spacing=s)
         assert ctx.launch_count - a1 == a1 - a0
         assert a[0] == b[0] == 0
         kept = a[2]
@@ -156,12 +116,6 @@ def test_spaced_launches_do_not_grow_with_clouds(ctx):
     c = ctx.launch_count
     ctx.voxel_downsample(clouds * 8, 0.5, 4)
     assert ctx.launch_count - c == c - b == b - a == 7
-
-
-def window_map(seq, rs, k, map_frames, s):
-    from dcreg_b200.api import map_points, voxel_downsample
-    M = np.concatenate([map_points(rs[j].T, voxel_downsample(seq[j], SV, 1)[0]) for j in range(max(0, k - map_frames), k)])
-    return voxel_downsample(M, MV, CAP, s)[0]
 
 
 @pytest.mark.parametrize("motion", ["increments", "constant_velocity"])
@@ -183,24 +137,12 @@ def test_window_frames_equal_their_reconstruction(ctx, odo, method, motion):
     for s, (seq, rs) in enumerate(zip(seqs, split(res, seqs))):
         assert_anchor(rs[0], T_init[s])
         for k in range(1, len(seq)):
-            M = window_map(seq, rs, k, 3, S)
-            thinner += len(window_map(seq, rs, k, 3, 0.0)) - len(M)
+            M = window_map(seq, rs, k, 3, SV, MV, (1, CAP), S)
+            thinner += len(window_map(seq, rs, k, 3, SV, MV, (1, CAP), 0.0)) - len(M)
             ctx.set_target(M, CELL)
-            ctx.set_source(voxel_downsample(seq[k], SV, 1)[0])
+            ctx.set_source(source_points(seq[k], SV))
             assert_same_run(rs[k], ctx.icp_run(prm, rs[k].T_prior))
     assert thinner > 0
-
-
-def twin_maps(seq, rs, s, frames=None):
-    """The twin's voxel maps M_1 .. M_n of one sequence, spaced at s"""
-    from dcreg_b200.api import voxel_downsample, voxel_map_update
-    M = np.zeros((0, 3), np.float32)
-    out = [None]
-    for k in range(len(rs)):
-        P = frames[k] if frames is not None else voxel_downsample(seq[k], SV, 1)[0]
-        M = voxel_map_update(M, P, rs[k].T, MV, CAP, DIST, s)
-        out.append(M)
-    return out
 
 
 @pytest.mark.parametrize("motion", ["increments", "constant_velocity"])
@@ -215,10 +157,10 @@ def test_voxel_map_frames_equal_their_reconstruction(ctx, odo, method, motion):
                        map_max_points=CAP)
     for s, (seq, rs) in enumerate(zip(seqs, split(res, seqs))):
         assert_anchor(rs[0], T_init[s])
-        twin = twin_maps(seq, rs, S)
+        twin = twin_maps(seq, rs, SV, MV, CAP, DIST, S)
         for k in range(1, len(seq)):
             ctx.set_target(twin[k], CELL)
-            ctx.set_source(voxel_downsample(seq[k], SV, 1)[0])
+            ctx.set_source(source_points(seq[k], SV))
             assert_same_run(rs[k], ctx.icp_run(prm, rs[k].T_prior))
 
 
@@ -234,7 +176,7 @@ def test_deskewed_frames_with_spacing(ctx, sweeps, method):
                                      want_log=True, want_cov=True, **kw)
         res_m = map_call(ctx, prm, sw["skewed"], sw["T_init"], sw["deltas"], DIST, **kw)
     for seq, rw, rm in zip(sw["skewed"], split(res_w, sw["skewed"]), split(res_m, sw["skewed"])):
-        twin = twin_maps(seq, rm, S, frames=[r.deskewed for r in rm])
+        twin = twin_maps(seq, rm, SV, MV, CAP, DIST, S, frames=[r.deskewed for r in rm])
         for k in range(1, len(seq)):
             M = np.concatenate([map_points(rw[j].T, rw[j].deskewed) for j in range(max(0, k - 3), k)])
             ctx.set_target(voxel_downsample(M, MV, CAP, S)[0], CELL)
@@ -264,10 +206,11 @@ def test_local_map_equals_twin_after_every_push(ctx, odo):
     seqs, T_init, deltas = odo
     prm = params()
     with spacing(ctx, S):
-        res, maps = map_session(ctx, prm, seqs, T_init, one_per_push(LENS), deltas, source_voxel=SV, map_voxel=MV,
-                                map_max_points=CAP, max_distance=DIST)
+        maps = []
+        res = pushed(ctx, prm, seqs, T_init, one_per_push(LENS), deltas, voxel_map=True, maps=maps, want_log=True,
+                     want_cov=True, source_voxel=SV, map_voxel=MV, map_max_points=CAP, max_distance=DIST)
     for s, (seq, rs) in enumerate(zip(seqs, res)):
-        twin = twin_maps(seq, rs, S)
+        twin = twin_maps(seq, rs, SV, MV, CAP, DIST, S)
         for i in range(len(maps)):
             assert maps[i][s].tobytes() == twin[min(i + 1, len(seq))].tobytes(), (s, i)
 
@@ -286,31 +229,18 @@ def test_session_chunkings_equal_one_call(ctx, odo, chunking):
         wref = ctx.icp_run_odometry(prm, seqs, T_init, deltas, map_frames=3, cell_size=CELL, want_log=True,
                                     want_cov=True, **kw)
         toggle = lambda i: ctx.set_map_spacing([0.0, 0.3, S][i % 3])           # noqa: E731
-        got, maps = map_session(ctx, prm, seqs, T_init, CHUNKS[chunking], deltas, max_distance=DIST, between=toggle,
-                                **kw)
+        maps = []
+        got = pushed(ctx, prm, seqs, T_init, CHUNKS[chunking], deltas, voxel_map=True, maps=maps, between=toggle,
+                     want_log=True, want_cov=True, max_distance=DIST, **kw)
         ctx.set_map_spacing(S)
         assert_same(got, seq_results(ref, seqs))
         for s, (seq, rs) in enumerate(zip(seqs, got)):
-            assert maps[-1][s].tobytes() == twin_maps(seq, rs, S)[-1].tobytes()
+            assert maps[-1][s].tobytes() == twin_maps(seq, rs, SV, MV, CAP, DIST, S)[-1].tobytes()
         # the window session too
-        first = np.concatenate([[0], np.cumsum(LENS)])
-        done = [0] * len(seqs)
-        out = [[] for _ in seqs]
-        with ctx.odometry_session(prm, len(seqs), T_init, map_frames=3, cell_size=CELL, **kw) as sess:
-            for i, cnt in enumerate(CHUNKS[chunking]):
-                part = [seqs[s][done[s]:done[s] + c] for s, c in enumerate(cnt)]
-                D = np.concatenate([deltas[first[s] + done[s]:first[s] + done[s] + c] for s, c in enumerate(cnt)])
-                for s, r in enumerate(sess.push(part, D, want_log=True, want_cov=True)):
-                    out[s].extend(r)
-                done = [d + c for d, c in zip(done, cnt)]
-                toggle(i)
+        out = pushed(ctx, prm, seqs, T_init, CHUNKS[chunking], deltas, between=toggle, want_log=True, want_cov=True,
+                     map_frames=3, **kw)
         ctx.set_map_spacing(S)
         assert_same(out, seq_results(wref, seqs))
-
-
-def raw_spaced_map_call(ctx, *a, **kw):
-    with spacing(ctx, S):
-        return raw_map_call(ctx, *a, **kw)
 
 
 def test_reproducible_and_context_intact(ctx, odo):
@@ -320,9 +250,10 @@ def test_reproducible_and_context_intact(ctx, odo):
     ctx.set_target(np.concatenate(frames[:3]), CELL)
     ctx.set_source(frames[1])
     one = ctx.icp_run(prm, T_init[1])
-    rc_a, a = raw_spaced_map_call(ctx, prm, seqs, T_init, deltas)
-    rc_b, b = raw_spaced_map_call(ctx, prm, seqs, T_init, deltas)
-    rc_0, z = raw_map_call(ctx, prm, seqs, T_init, deltas)                    # the setting is back at 0
+    with spacing(ctx, S):
+        rc_a, a = raw_odometry(ctx, MAP, prm, seqs, T_init, deltas, log_cap=30, **RAW_MAP)
+        rc_b, b = raw_odometry(ctx, MAP, prm, seqs, T_init, deltas, log_cap=30, **RAW_MAP)
+    rc_0, z = raw_odometry(ctx, MAP, prm, seqs, T_init, deltas, log_cap=30, **RAW_MAP)     # the setting is back at 0
     assert rc_a == rc_b == rc_0 == 0
     for k in a:
         assert a[k].tobytes() == b[k].tobytes(), k
@@ -330,8 +261,8 @@ def test_reproducible_and_context_intact(ctx, odo):
     again = ctx.icp_run(prm, T_init[1])
     assert again.T.tobytes() == one.T.tobytes() and again.iterations == one.iterations
     from dcreg_b200 import Context
-    with Context(0) as fresh:
-        rc, c = raw_spaced_map_call(fresh, prm, seqs, T_init, deltas)
+    with Context(0) as fresh, spacing(fresh, S):
+        rc, c = raw_odometry(fresh, MAP, prm, seqs, T_init, deltas, log_cap=30, **RAW_MAP)
         assert rc == 0
         for k in a:
             assert a[k].tobytes() == c[k].tobytes(), k
@@ -349,7 +280,7 @@ def test_launches_per_step_do_not_depend_on_sequences(ctx, odo):
         for s in (0.0, S):
             with spacing(ctx, s):
                 a = ctx.launch_count
-                rc, _ = raw_map_call(ctx, prm, ss, T0, None, log_cap=0)
+                rc, _ = raw_odometry(ctx, MAP, prm, ss, T0, None, **RAW_MAP)
                 b = ctx.launch_count
                 ctx.icp_run_odometry(prm, ss, T0, None, map_frames=3, cell_size=CELL, source_voxel=SV, map_voxel=MV,
                                      map_max_points=CAP)
@@ -381,7 +312,7 @@ def test_bad_arguments(ctx, odo):
     good = [np.zeros((3, 3), np.float32), np.ones((2, 3), np.float32)]
     launches = ctx.launch_count
     for bad in (math.nan, -1e-9, -1.0, math.inf, -math.inf):
-        assert raw_spaced(ctx, good, 0.5, 4, bad)[0] == api.BAD_ARG, bad
+        assert raw_downsample(ctx, SPACED, good, 0.5, max_points=4, min_spacing=bad)[0] == api.BAD_ARG, bad
         assert "min_spacing" in ctx.lib.dcreg_last_error(ctx._h).decode()
         assert ctx.lib.dcreg_set_map_spacing(ctx._h, bad) == api.BAD_ARG, bad
         assert "min_spacing" in ctx.lib.dcreg_last_error(ctx._h).decode()
