@@ -21,21 +21,9 @@ against the true mid-sweep poses.  Parity (asserted; the tool exits non-zero if 
 for byte, and deskew_true's deskewed points of every frame lie within one float32 ulp (or 1e-12 m) of
 api.deskew_points with the true increment.  Prints one JSON line with the card name and power limit; --dump-outputs DIR
 writes every arm's poses as float64 .npy files."""
-import argparse
-import json
-import os
-import sys
-import time
-
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from bench_scans import card  # noqa: E402
-from bench_sequences import pose_errors  # noqa: E402
+import bench_harness as h
 
 MAP_FRAMES = 10
 CELL = 0.5
@@ -48,40 +36,19 @@ WORKLOADS = {
 ARMS = ["skewed", "deskew_cv", "deskew_true", "unskewed", "mid"]
 
 
-def same_bytes(a, b):
-    return ((a.status, a.iterations, a.converged, a.n_points) == (b.status, b.iterations, b.converged, b.n_points)
-            and a.T.tobytes() == b.T.tobytes() and a.T_prior.tobytes() == b.T_prior.tobytes())
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--runs", type=int, default=3)
+    ap = h.parser()
     ap.add_argument("--workloads", default=",".join(WORKLOADS), help="comma-separated subset of " + ",".join(WORKLOADS))
-    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
-    import torch
-    from dcreg_b200 import Context, default_params
+    h.require_gpu()
+    from dcreg_b200 import Context
     from dcreg_b200.api import DcregError, deskew_points, voxel_downsample
     from dcreg_b200.scenes import make_parking_sweeps
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_odometry_deskew.py: no CUDA device - dcreg_b200 has no CPU fallback")
-    prm = default_params(max_iterations=30, search_radius=0.5, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3,
-                         kappa_target=10.0, detection="SCHUR_CONDITION_NUMBER", handling="PRECONDITIONED_CG")
-    line = {"metric": "frames_per_s", "map_frames": MAP_FRAMES, "workloads": {}, "card": card()}
+    prm = h.c3_params()
+    line = {"metric": "frames_per_s", "map_frames": MAP_FRAMES, "workloads": {}, "card": h.card()}
     ok_all = True
     dumps = {}
     with Context(0) as ctx:
-        stream = torch.cuda.ExternalStream(ctx.stream)
-
-        def timed(fn):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            w = time.perf_counter()
-            e0.record(stream)
-            out = fn()
-            e1.record(stream)
-            e1.synchronize()
-            return out, max(e0.elapsed_time(e1) / 1e3, time.perf_counter() - w)
-
         for name in args.workloads.split(","):
             wl = WORKLOADS[name]
             seqs = {"skewed": [], "unskewed": [], "stamps": [], "mid": []}
@@ -112,23 +79,21 @@ def main():
                 "mid": lambda: ctx.icp_run_odometry(prm, seqs["unskewed"], T_init, deltas, map_frames=MAP_FRAMES,
                                                     cell_size=CELL, timestamps=seqs["mid"], **f),
             }
-            res = {}                                               # warm-up, and the outputs checked below
-            for a in ARMS:
-                try:
-                    res[a] = arms[a]()
-                except DcregError as e:                            # an arm whose odometry diverged: its message
-                    res[a] = str(e)
-            live = [a for a in ARMS if not isinstance(res[a], str)]
-            times = {a: [] for a in live}
-            for _ in range(args.runs):
-                for a in live:
-                    r, dt = timed(arms[a])
-                    times[a].append(dt)
-                    ok_all &= all(same_bytes(x, y) for x, y in zip(r, res[a]))
+            warm, repeats = {}, []
+
+            def check(a, out):                          # the warm-up's outputs are checked below; every round repeats them
+                if a in warm:
+                    repeats.append(all(h.same_bytes(x, y) for x, y in zip(out, warm[a])))
+                else:
+                    warm[a] = out
+            # an arm whose odometry diverged keeps its message
+            outs, _, med = h.run_arms(ctx, arms, args.runs, DcregError, check)
+            res = {a: warm.get(a, o) for a, o in outs.items()}
+            ok_all &= all(repeats)
             for a in ("deskew_true", "unskewed", "mid"):
                 if isinstance(res[a], str):
                     raise SystemExit(f"bench_odometry_deskew.py: {name}: {a} failed: {res[a]}")
-            parity = all(same_bytes(x, y) for x, y in zip(res["mid"], res["unskewed"]))
+            parity = all(h.same_bytes(x, y) for x, y in zip(res["mid"], res["unskewed"]))
             k = 0
             for s, (sk, ts) in enumerate(zip(seqs["skewed"], seqs["stamps"])):
                 for j in range(len(sk)):
@@ -147,22 +112,16 @@ def main():
                 if isinstance(res[a], str):
                     out["arms"][a] = {"error": res[a]}
                     continue
-                dt, dr = pose_errors(T_true, [r.T for r in res[a]])
-                out["arms"][a] = {"frames_per_s": round(n_frames / float(np.median(times[a])), 1),
+                dt, dr = h.pose_errors(T_true, [r.T for r in res[a]])
+                out["arms"][a] = {"frames_per_s": round(n_frames / (med[a] * 1e-3), 1),
                                   "iterations": int(sum(r.iterations for r in res[a])),
                                   "converged": int(sum(r.converged for r in res[a])),
                                   "max_trans_err_m": round(dt, 4), "max_rot_err_deg": round(dr, 4)}
-                dumps[f"{name}_{a}_T"] = np.array([r.T for r in res[a]])
-            out["mid_overhead_pct"] = round(100.0 * (np.median(times["mid"]) / np.median(times["unskewed"]) - 1.0), 2)
+                dumps.update(h.result_dumps(f"{name}_{a}", res[a], ("T",)))
+            out["mid_overhead_pct"] = round(100.0 * (med["mid"] / med["unskewed"] - 1.0), 2)
             line["workloads"][name] = out
-    if args.dump_outputs:
-        os.makedirs(args.dump_outputs, exist_ok=True)
-        for k, v in dumps.items():
-            np.save(os.path.join(args.dump_outputs, k + ".npy"), v)
     line["parity"] = bool(ok_all)
-    print(json.dumps(line))
-    if not ok_all:
-        sys.exit(1)
+    h.finish(args, line, dumps, ok_all, 1)
 
 
 if __name__ == "__main__":

@@ -24,21 +24,11 @@ Parity (asserted; the tool exits non-zero if it fails): every frame of (a) equal
 status, iterations, converged, n_points).  Reported: frames/s per arm, and the drift against the true poses of (a) and
 (d).  Prints one JSON line with the card name and power limit; --dump-outputs DIR writes (a)'s outputs as float64
 .npy files."""
-import argparse
-import json
-import os
-import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from bench_scans import card  # noqa: E402
-from bench_sequences import pose_errors  # noqa: E402
+import bench_harness as h
 
 MAP_FRAMES = 10
 CELL = 0.5
@@ -50,67 +40,42 @@ WORKLOADS = {
 }
 
 
-def same_bytes(a, b):
-    return ((a.status, a.iterations, a.converged, a.n_points) == (b.status, b.iterations, b.converged, b.n_points)
-            and a.T.tobytes() == b.T.tobytes() and a.T_prior.tobytes() == b.T_prior.tobytes())
-
-
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--runs", type=int, default=3)
+    ap = h.parser()
     ap.add_argument("--workloads", default=",".join(WORKLOADS), help="comma-separated subset of " + ",".join(WORKLOADS))
-    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
-    import torch
-    from dcreg_b200 import Context, default_params
-    from dcreg_b200.api import compose_prior, map_points
-    from dcreg_b200.scenes import make_parking_sequence
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_odometry_stream.py: no CUDA device - dcreg_b200 has no CPU fallback")
-    prm = default_params(max_iterations=30, search_radius=0.5, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3,
-                         kappa_target=10.0, detection="SCHUR_CONDITION_NUMBER", handling="PRECONDITIONED_CG")
-    line = {"metric": "frames_per_s", "map_frames": MAP_FRAMES, "workloads": {}, "card": card()}
+    h.require_gpu()
+    from dcreg_b200 import Context
+    from dcreg_b200.api import compose_prior
+    prm = h.c3_params()
+    line = {"metric": "frames_per_s", "map_frames": MAP_FRAMES, "workloads": {}, "card": h.card()}
     ok_all = True
     dumps = {}
     with Context(0) as ctx:
-        stream = torch.cuda.ExternalStream(ctx.stream)
-
-        def timed(fn):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            w = time.perf_counter()
-            e0.record(stream)
-            out = fn()
-            e1.record(stream)
-            e1.synchronize()
-            w = time.perf_counter() - w
-            return out, max(e0.elapsed_time(e1), w * 1e3)
-
         for name in args.workloads.split(","):
             wl = WORKLOADS[name]
             filt = wl["filters"]
-            seqs, T0, deltas, T_true = [], [], [], []
-            for n, seed in wl["spec"]:
-                frames, Tt, _, D, _ = make_parking_sequence(n, seed=seed, n_map=wl["n_map"], n_scan=wl["n_scan"],
-                                                            max_range=20.0)
-                seqs.append(frames); T0.append(Tt[0]); deltas.append(D); T_true.append(Tt)
-            T0, T_true = np.array(T0), np.concatenate(T_true)
+            seqs, T0, D_all, T_true = h.parking_sequences(wl["spec"], n_map=wl["n_map"], n_scan=wl["n_scan"],
+                                                          max_range=20.0)
+            deltas = h.per_sequence(seqs, D_all)
             first = np.concatenate([[0], np.cumsum([len(f) for f in seqs])])
-            D_all = np.concatenate(deltas)
             n_frames, S, L = len(D_all), len(seqs), max(len(f) for f in seqs)
 
             def one_call():
                 return ctx.icp_run_odometry(prm, seqs, T0, D_all, map_frames=MAP_FRAMES, cell_size=CELL, **filt)
 
-            def session(lat=None):
+            lats = []                                                           # every session's push latencies
+
+            def session():
                 out = [[] for _ in seqs]
+                lats.append([])
                 with ctx.odometry_session(prm, S, T0, map_frames=MAP_FRAMES, cell_size=CELL, **filt) as sess:
                     for k in range(L):
                         part = [[f[k]] if k < len(f) else [] for f in seqs]
                         D = np.stack([deltas[s][k] for s in range(S) if k < len(seqs[s])])
                         w = time.perf_counter()
                         res = sess.push(part, D)
-                        if lat is not None:
-                            lat.append((time.perf_counter() - w) * 1e3)
+                        lats[-1].append((time.perf_counter() - w) * 1e3)
                         for s, r in enumerate(res):
                             out[s].extend(r)
                 return [r for rs in out for r in rs]
@@ -122,7 +87,7 @@ def main():
                     Ts = [T0[s]]
                     for j in range(1, len(frames)):
                         T = compose_prior(Ts[j - 1], deltas[s][j - 1])
-                        m = np.concatenate([map_points(Ts[i], src[i]) for i in range(max(0, j - MAP_FRAMES), j)])
+                        m = h.window_map(src, Ts, j, MAP_FRAMES)
                         if filt:
                             m = ctx.voxel_downsample([m], filt["map_voxel"], filt["map_max_points"])[0][0]
                         ctx.set_target(m, CELL)
@@ -145,15 +110,8 @@ def main():
                 return [T for s in range(S) for T in Ts[s]]
 
             arms = {"session": session, "call": one_call, "loop": host_loop, "per_frame": per_frame_calls}
-            for fn in arms.values():                                            # warm-up of every arm
-                fn()
-            ms = {a: [] for a in arms}
-            lat = []
-            outs = {}
-            for _ in range(max(1, args.runs)):
-                for a, fn in arms.items():
-                    outs[a], t = timed((lambda: session(lat)) if a == "session" else fn)
-                    ms[a].append(t)
+            outs, ms, med = h.run_arms(ctx, arms, args.runs)
+            lat = [t for x in lats[1:] for t in x]                              # the timed rounds' pushes
             # parity: the session against the call, byte for byte
             sess_res, call_res = outs["session"], outs["call"]
             by_frame = [None] * n_frames                                        # the session's results in call order
@@ -162,7 +120,7 @@ def main():
                 for j in range(len(seqs[s])):
                     by_frame[first[s] + j] = sess_res[k]
                     k += 1
-            ok = len(sess_res) == n_frames and all(same_bytes(a, b) for a, b in zip(by_frame, call_res))
+            ok = len(sess_res) == n_frames and all(h.same_bytes(a, b) for a, b in zip(by_frame, call_res))
             ok_all = ok_all and ok
             reg = [r for r in call_res if r.iterations > 0]
             w = {"sequences": S, "frames": n_frames, "filters": filt,
@@ -170,27 +128,17 @@ def main():
                  "mean_iterations": float(np.mean([r.iterations for r in reg])),
                  "parity": {"session_equals_call_bytes": ok}}
             for a in arms:
-                m = float(np.median(ms[a]))
-                w[a] = {"frames_per_s": n_frames / (m * 1e-3), "ms": m, "runs_ms": ms[a]}
+                w[a] = h.rate(n_frames, med[a], ms[a])
             w["session"]["push_latency_ms"] = {"p50": float(np.percentile(lat, 50)), "p90": float(np.percentile(lat, 90)),
                                                "max": float(np.max(lat)), "pushes": len(lat)}
-            drift_a = pose_errors(T_true, [r.T for r in by_frame])
-            drift_d = pose_errors(T_true, outs["per_frame"])
+            drift_a = h.pose_errors(T_true, [r.T for r in by_frame])
+            drift_d = h.pose_errors(T_true, outs["per_frame"])
             w["session"]["max_err_vs_truth"] = {"trans_m": drift_a[0], "rot_deg": drift_a[1]}
             w["per_frame"]["max_err_vs_truth"] = {"trans_m": drift_d[0], "rot_deg": drift_d[1]}
             line["workloads"][name] = w
-            dumps[name] = by_frame
-    print(json.dumps(line))
-    if args.dump_outputs:
-        os.makedirs(args.dump_outputs, exist_ok=True)
-        for name, res in dumps.items():
-            for k, v in {"T": [r.T for r in res], "T_prior": [r.T_prior for r in res],
-                         "iterations": [r.iterations for r in res], "converged": [r.converged for r in res],
-                         "status": [r.status for r in res], "n_points": [r.n_points for r in res]}.items():
-                np.save(os.path.join(args.dump_outputs, f"odometry_stream_{name}_{k}.npy"), np.asarray(v, dtype=np.float64))
-    if not ok_all:
-        bad = [n for n, w in line["workloads"].items() if not w["parity"]["session_equals_call_bytes"]]
-        raise SystemExit(f"bench_odometry_stream.py: the session's outputs differ from the call's in {bad}")
+            dumps.update(h.result_dumps(f"odometry_stream_{name}", by_frame, h.FIELDS + ("n_points",)))
+    bad = [n for n, w in line["workloads"].items() if not w["parity"]["session_equals_call_bytes"]]
+    h.finish(args, line, dumps, ok_all, f"bench_odometry_stream.py: the session's outputs differ from the call's in {bad}")
 
 
 if __name__ == "__main__":

@@ -11,55 +11,26 @@ converged identical, pose <= 1e-8 on the SE(3) log); the tool exits non-zero if 
 the largest translation / rotation error against the true poses of the chained results and of the dead-reckoned priors
 (T_init composed with the increments alone).  Prints one JSON line with the card name and power limit; --dump-outputs
 DIR writes the chained poses, priors and flags as float64 .npy files."""
-import argparse
-import json
-import os
-import sys
-import time
-
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from bench_scans import card  # noqa: E402
-
-
-def pose_errors(T_true, T):
-    """Largest translation (m) and rotation (deg) error of the poses T against T_true."""
-    import dcreg_oracle as o
-    dt, dr = 0.0, 0.0
-    for A, B in zip(T_true, T):
-        E = np.linalg.inv(A) @ B
-        dt = max(dt, float(np.linalg.norm(E[:3, 3])))
-        dr = max(dr, float(np.degrees(np.linalg.norm(o.so3_log(E[:3, :3])))))
-    return dt, dr
+import bench_harness as h
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--runs", type=int, default=3)
-    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
-    args = ap.parse_args()
-    import torch
+    args = h.parser().parse_args()
+    h.require_gpu()
     import dcreg_oracle as o                                                   # se3 log distance (NumPy), checker only
-    from dcreg_b200 import Context, default_params
+    from dcreg_b200 import Context
     from dcreg_b200.api import compose_prior
     from dcreg_b200.scenes import make_parking_sequence
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_sequences.py: no CUDA device - dcreg_b200 has no CPU fallback")
-    prm = default_params(search_radius=0.5, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3,
-                         kappa_target=10.0, detection="SCHUR_CONDITION_NUMBER", handling="PRECONDITIONED_CG")
+    prm = h.c3_params()
     workloads = {"1x256": [(256, 47)], "8x64": [(64, 71 + i) for i in range(8)]}
-    line = {"metric": "frames_per_s", "workloads": {}, "card": card()}
+    line = {"metric": "frames_per_s", "workloads": {}, "card": h.card()}
     ok_all = True
     dumps = {}
     with Context(0) as ctx:
-        stream = torch.cuda.ExternalStream(ctx.stream)
-        park_map = None
         for name, spec in workloads.items():
+            # localisation starts from the scene's perturbed initial pose, against the scene's map
             seqs, T0, deltas, T_true = [], [], [], []
             for n, seed in spec:
                 frames, Tt, Ti0, D, park_map = make_parking_sequence(n, seed=seed)
@@ -67,9 +38,6 @@ def main():
             T0, deltas, T_true = np.array(T0), np.concatenate(deltas), np.concatenate(T_true)
             ctx.set_target(park_map, 0.5)
             n_frames = len(deltas)
-
-            def call():
-                return ctx.icp_run_sequences(prm, seqs, T0, deltas)
 
             def frame_loop():
                 out, k = [], 0
@@ -84,24 +52,9 @@ def main():
                         k += 1
                 return out
 
-            def timed(fn):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                w = time.perf_counter()
-                e0.record(stream)
-                out = fn()
-                e1.record(stream)
-                e1.synchronize()
-                w = time.perf_counter() - w
-                return out, max(e0.elapsed_time(e1), w * 1e3)
-
-            call()                                                             # warm-up of both shapes
-            frame_loop()
-            call_ms, loop_ms = [], []
-            for _ in range(max(1, args.runs)):
-                res, ms = timed(call)
-                call_ms.append(ms)
-                loop, ms = timed(frame_loop)
-                loop_ms.append(ms)
+            outs, ms, med = h.run_arms(ctx, {"call": lambda: ctx.icp_run_sequences(prm, seqs, T0, deltas),
+                                             "loop": frame_loop}, args.runs)
+            res, loop = outs["call"], outs["loop"]
             same, worst = True, 0.0
             for b, s in zip(res, loop):
                 same = same and (b.status, b.iterations, b.converged) == (s.status, s.iterations, s.converged)
@@ -115,32 +68,21 @@ def main():
                     T_dr.append(T)
                     T = compose_prior(T, deltas[k])
                     k += 1
-            chained = pose_errors(T_true, [r.T for r in res])
-            dead = pose_errors(T_true, T_dr)
-            cm, lm = float(np.median(call_ms)), float(np.median(loop_ms))
-            sizes = [len(f) for frames in seqs for f in frames]
+            chained = h.pose_errors(T_true, [r.T for r in res])
+            dead = h.pose_errors(T_true, T_dr)
             line["workloads"][name] = {
-                "sequences": len(seqs), "frames": n_frames, "frames_per_s": n_frames / (cm * 1e-3), "ms": cm,
-                "runs_ms": call_ms, "loop_frames_per_s": n_frames / (lm * 1e-3), "loop_ms": lm, "loop_runs_ms": loop_ms,
-                "speedup_vs_loop": lm / cm, "mean_iterations": float(np.mean([r.iterations for r in res])),
+                "sequences": len(seqs), "frames": n_frames, **h.rate(n_frames, med["call"], ms["call"]),
+                **h.rate(n_frames, med["loop"], ms["loop"], "loop_"), "speedup_vs_loop": med["loop"] / med["call"],
+                "mean_iterations": float(np.mean([r.iterations for r in res])),
                 "converged": int(sum(r.converged for r in res)),
-                "points_per_frame": {"min": int(min(sizes)), "max": int(max(sizes)), "total": int(sum(sizes))},
+                "points_per_frame": h.spread([len(f) for frames in seqs for f in frames]),
                 "parity": {"ok": ok, "identical_status_iterations_converged": same, "max_pose_err": worst,
                            "tolerance": 1e-8},
                 "max_err_vs_truth": {"chained": {"trans_m": chained[0], "rot_deg": chained[1]},
                                      "dead_reckoned_prior": {"trans_m": dead[0], "rot_deg": dead[1]}}}
-            dumps[name] = res
-    print(json.dumps(line))
-    if args.dump_outputs:
-        os.makedirs(args.dump_outputs, exist_ok=True)
-        for name, res in dumps.items():
-            for k, v in {"T": [r.T for r in res], "T_prior": [r.T_prior for r in res],
-                         "iterations": [r.iterations for r in res], "converged": [r.converged for r in res],
-                         "status": [r.status for r in res]}.items():
-                np.save(os.path.join(args.dump_outputs, f"sequences_{name}_{k}.npy"), np.asarray(v, dtype=np.float64))
-    if not ok_all:
-        bad = {n: w["parity"] for n, w in line["workloads"].items() if not w["parity"]["ok"]}
-        raise SystemExit(f"bench_sequences.py: parity FAILED {bad}")
+            dumps.update(h.result_dumps(f"sequences_{name}", res))
+    bad = {n: w["parity"] for n, w in line["workloads"].items() if not w["parity"]["ok"]}
+    h.finish(args, line, dumps, ok_all, f"bench_sequences.py: parity FAILED {bad}")
 
 
 if __name__ == "__main__":

@@ -15,23 +15,13 @@ every arm runs the whole recording):
       1 x --frames and --lanes x (--frames / --lanes).  forced_sparse_equals_dense_bit_for_bit reports whether their
       poses and iteration counts agree (the extra point changes the largest frame, and with it the tile size, so they
       need not).
-Each call is timed with a host clock around it (it ends in a sync), after one warm-up call of the same shape; the arms
-alternate, --runs rounds, medians reported.  Prints one JSON line with the card name and power limit read in the same
-run; --dump-outputs DIR writes every odometry arm's poses, iterations, converged flags and statuses as .npy."""
-import argparse
-import json
-import os
-import sys
-import time
-
+Each call is timed as tools/bench_scans.py times its calls (the max of CUDA events on the context's stream and the host
+wall clock), after one warm-up call of the same shape; the arms alternate, --runs rounds, medians reported.  Prints one
+JSON line with the card name and power limit read in the same run; --dump-outputs DIR writes every odometry arm's poses,
+iterations, converged flags and statuses as .npy."""
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-
-from bench_scans import card  # noqa: E402
+import bench_harness as h
 
 RADIUS = 0.5
 CELL = 0.25
@@ -43,17 +33,15 @@ def split(frames, lanes):
 
 
 def main():
-    ap = argparse.ArgumentParser()
+    ap = h.parser()
     ap.add_argument("--frames", type=int, default=128)
     ap.add_argument("--lanes", type=int, default=8)
-    ap.add_argument("--runs", type=int, default=3)
-    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
-    from dcreg_b200 import Context, default_params, api
+    h.require_gpu()
+    from dcreg_b200 import Context
     from dcreg_b200.scenes import make_long_range_sequence
 
-    prm = default_params(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3,
-                         kappa_target=10.0)
+    prm = h.c3_params(search_radius=RADIUS)
     far_frames, T_true, deltas = make_long_range_sequence(args.frames, seed=91)
     near_frames = [f[:len(f) - 2_000] for f in far_frames]              # the same recording without the facades
     one_far = np.array([[3.0e4, 3.0e4, 60.0]], np.float32)
@@ -82,38 +70,24 @@ def main():
         return ctx.icp_run_odometry_map(prm, seqs, T0, deltas, map_voxel=CELL,
                                         map_max_points=20, max_distance=float("inf"), cell_size=CELL)
 
-    def timed(fn):
-        t0 = time.perf_counter()
-        out = fn()
-        return time.perf_counter() - t0, out
-
-    outs, times = {}, {k: [] for k in arms}
-    for name in arms:                                               # warm-up: buffers, graphs
-        outs[name] = run(name)
+    host = "host_loop_window_1x%d" % args.frames
     seqs_w, _ = arms["window_1x%d" % args.frames][0]
-    res_w = outs["window_1x%d" % args.frames]
-    host_times = []
+    res_w = run("window_1x%d" % args.frames)                        # the priors the host loop starts from
 
     def host_loop():
         seq = seqs_w[0]
         for k in range(1, len(seq)):
-            m = np.concatenate([api.map_points(res_w[j].T, seq[j]) for j in range(max(0, k - 10), k)])
-            ctx.set_target_sparse(m, CELL)
+            ctx.set_target_sparse(h.window_map(seq, [r.T for r in res_w], k, 10), CELL)
             ctx.set_source(seq[k])
             ctx.icp_run(prm, res_w[k].T_prior, want_log=False)
-    for r in range(args.runs):
-        for name in arms:
-            dt, outs[name] = timed(lambda: run(name))
-            times[name].append(dt)
-        dt, _ = timed(host_loop)
-        host_times.append(dt)
-    result = {"bench": "sparse_maps", "card": card(), "frames": args.frames, "lanes": args.lanes, "cell": CELL,
+    outs, _, med = h.run_arms(ctx, {**{name: lambda name=name: run(name) for name in arms}, host: host_loop}, args.runs)
+    result = {"bench": "sparse_maps", "card": h.card(), "frames": args.frames, "lanes": args.lanes, "cell": CELL,
               "runs": args.runs, "frames_per_s": {}}
     for name in arms:
         nf = sum(len(s) for s in arms[name][0][0])
-        result["frames_per_s"][name] = nf / float(np.median(times[name]))
-    result["frames_per_s"]["host_loop_window_1x%d" % args.frames] = (args.frames - 1) / float(np.median(host_times))
-    m9 = np.concatenate([api.map_points(res_w[j].T, seqs_w[0][j]) for j in range(0, 10)])
+        result["frames_per_s"][name] = nf / (med[name] * 1e-3)
+    result["frames_per_s"][host] = (args.frames - 1) / (med[host] * 1e-3)
+    m9 = h.window_map(seqs_w[0], [r.T for r in res_w], 10, 10)
     c = np.floor(m9.astype(np.float64) / CELL)
     result["window_map_box_cells"] = float(np.prod(c.max(0) - c.min(0) + 1))
     same = []
@@ -121,14 +95,12 @@ def main():
         a, b = outs["dense_%s" % tag], outs["forced_sparse_%s" % tag]
         same.append(all(x.T.tobytes() == y.T.tobytes() and x.iterations == y.iterations for x, y in zip(a, b)))
     result["forced_sparse_equals_dense_bit_for_bit"] = same
-    if args.dump_outputs:
-        os.makedirs(args.dump_outputs, exist_ok=True)
-        for name, out in outs.items():
-            np.save(os.path.join(args.dump_outputs, name + "_T.npy"), np.stack([x.T for x in out]))
-            np.save(os.path.join(args.dump_outputs, name + "_iters.npy"),
-                    np.array([[x.iterations, x.converged, x.status] for x in out], np.float64))
+    dumps = {}
+    for name in arms:
+        dumps[name + "_T"] = [x.T for x in outs[name]]
+        dumps[name + "_iters"] = [[x.iterations, x.converged, x.status] for x in outs[name]]
     ctx.close()
-    print(json.dumps(result))
+    h.finish(args, result, dumps)
 
 
 if __name__ == "__main__":

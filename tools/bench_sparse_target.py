@@ -15,22 +15,11 @@ Arms (radius = cell = 0.5, 30 iterations, ROT 1e-5 / TRANS 1e-3 (icp_pk01.yaml),
 Calls are timed as tools/bench_scans.py times them (the max of CUDA events on the context's stream and the host wall
 clock, host arrays in, results out, after a warm-up), --runs times, medians reported.  The sparse index's device bytes
 (points, positions and table, computed from the build rule) are reported against the dense tables' 12 B per cell of the
-box, with its build time (host clock around the call, which ends in a sync).  Prints one JSON line with the card name and
+box, with its build time (timed as the calls, the median of three).  Prints one JSON line with the card name and
 power limit; --dump-outputs DIR writes every arm's poses, iterations, converged flags and statuses as float64 .npy."""
-import argparse
-import json
-import os
-import sys
-import time
-
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-
-from bench_scans import card  # noqa: E402
+import bench_harness as h
 
 RADIUS = 0.5
 FAR = np.array([[2000.0, 1500.0, 400.0], [3000.0, 3000.0, 500.0]], dtype=np.float32)
@@ -58,20 +47,15 @@ def index_bytes(xyz, cell):
 
 
 def main():
-    ap = argparse.ArgumentParser()
+    ap = h.parser()
     ap.add_argument("--frames", type=int, default=64)
     ap.add_argument("--lanes", type=int, default=8)
     ap.add_argument("--tile-points", type=int, default=500_000)
-    ap.add_argument("--runs", type=int, default=3)
-    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
-    import torch
-    from dcreg_b200 import Context, default_params
+    h.require_gpu()
+    from dcreg_b200 import Context
     from dcreg_b200.scenes import make_large_map, make_large_map_frames, make_parking_frames, make_parking_sequence
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_sparse_target.py: no CUDA device - dcreg_b200 has no CPU fallback")
-    prm = default_params(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3,
-                         kappa_target=10.0, detection="SCHUR_CONDITION_NUMBER", handling="PRECONDITIONED_CG")
+    prm = h.c3_params(search_radius=RADIUS)
     n, L = args.frames, args.lanes
     frames, _, T_init, park = make_parking_frames(n, seed=47)
     sq_frames, _, sq_T0, sq_deltas, _ = make_parking_sequence(n, seed=47)
@@ -92,38 +76,19 @@ def main():
     l_deltas = np.concatenate([[np.linalg.inv(lT_true[g[i]]) @ lT_true[g[min(i + 1, g.size - 1)]] for i in range(g.size)]
                                for g in groups])
     l_T0 = np.array([lT_init[g[0]] for g in groups])
-    out, dump = {}, {}
+    out, dumps = {}, {}
     with Context(0) as ctx:
-        stream = torch.cuda.ExternalStream(ctx.stream)
-
-        def timed(fn):
-            fn()                                                   # warm-up of the shape
-            ms, res = [], None
-            for _ in range(max(1, args.runs)):
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                w = time.perf_counter()
-                e0.record(stream)
-                res = fn()
-                e1.record(stream)
-                e1.synchronize()
-                ms.append(max(e0.elapsed_time(e1), (time.perf_counter() - w) * 1e3))
-            return res, float(np.median(ms)), ms
 
         def arm(name, n_frames, fn):
-            res, ms, runs = timed(fn)
-            out[name] = {"frames_per_s": n_frames / (ms * 1e-3), "ms": ms, "runs_ms": runs,
-                         "converged": int(sum(r.converged for r in res)),
+            outs, ms, med = h.run_arms(ctx, {name: fn}, args.runs)
+            res = outs[name]
+            out[name] = {**h.rate(n_frames, med[name], ms[name]), "converged": int(sum(r.converged for r in res)),
                          "mean_iterations": float(np.mean([r.iterations for r in res]))}
-            dump[name] = res
+            dumps.update(h.result_dumps(name, res, ("T", "iterations", "converged", "status")))
             return res
 
         def build_time(fn):
-            t = []
-            for _ in range(3):
-                w = time.perf_counter()
-                fn()
-                t.append((time.perf_counter() - w) * 1e3)
-            return float(np.median(t))
+            return float(np.median([h.timed(ctx, fn)[1] for _ in range(3)]))
 
         ctx.set_target(park, RADIUS)
         a_scans = arm("a_dense_scans", n, lambda: ctx.icp_run_scans(prm, frames, T_init))
@@ -151,14 +116,8 @@ def main():
     out["index_large"] = index_bytes(big, RADIUS)
     out["speedup_c_scans_vs_d"] = out["c_sparse_scans"]["frames_per_s"] / out["d_frame_loop"]["frames_per_s"]
     out["speedup_c_sequences_vs_d"] = out["c_sparse_sequences"]["frames_per_s"] / out["d_frame_loop"]["frames_per_s"]
-    line = {"metric": "frames_per_s", "frames": n, "lanes": L, "tile_points": args.tile_points, **out, "card": card()}
-    print(json.dumps(line))
-    if args.dump_outputs:
-        os.makedirs(args.dump_outputs, exist_ok=True)
-        for name, res in dump.items():
-            for k, v in {"T": [r.T for r in res], "iterations": [r.iterations for r in res],
-                         "converged": [r.converged for r in res], "status": [r.status for r in res]}.items():
-                np.save(os.path.join(args.dump_outputs, f"{name}_{k}.npy"), np.asarray(v, dtype=np.float64))
+    line = {"metric": "frames_per_s", "frames": n, "lanes": L, "tile_points": args.tile_points, **out, "card": h.card()}
+    h.finish(args, line, dumps)
 
 
 if __name__ == "__main__":

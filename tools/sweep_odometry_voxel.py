@@ -20,23 +20,12 @@ call at max_points 1 and 20, against the twin on each cloud.
 Parity (asserted; exits non-zero on a mismatch): every registered frame of every filtered arm against its
 reconstruction with the twin (set_target(filtered map, cell) + set_source(filtered frame) + icp_run(T_prior)): status,
 iterations and converged identical, pose <= 1e-8 on the SE(3) log, n_points the twin's; and the standalone filter's
-output equal to the twin's bit for bit.  Prints one JSON line with the card name and power limit."""
-import argparse
-import json
-import os
-import sys
-import time
-
+output equal to the twin's bit for bit.  Prints one JSON line with the card name and power limit; --dump-outputs DIR
+writes every arm's poses, priors, flags and kept points per frame, and the filter's kept points and indices, as float64
+.npy files."""
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-
-from bench_odometry_voxel import map_sizes  # noqa: E402
-from bench_scans import card  # noqa: E402
-from bench_sequences import pose_errors  # noqa: E402
+import bench_harness as h
 
 MAP_FRAMES = 10
 CELL = 0.5
@@ -45,21 +34,16 @@ ARMS = [("raw", None, None), ("m0.25x1", 0.25, 1), ("m0.25x2", 0.25, 2), ("m0.25
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--runs", type=int, default=3)
+    ap = h.parser()
     ap.add_argument("--source-voxel", type=float, default=0.25)
     ap.add_argument("--small", action="store_true", help="a quick rehearsal: 2 small workloads")
     args = ap.parse_args()
-    import torch
-    import dcreg_oracle as o
-    from dcreg_b200 import Context, default_params
-    from dcreg_b200.api import map_points, voxel_downsample
+    h.require_gpu()
+    from dcreg_b200 import Context
+    from dcreg_b200.api import voxel_downsample
     from dcreg_b200.scenes import make_parking_sequence
-    if not torch.cuda.is_available():
-        raise SystemExit("sweep_odometry_voxel.py: no CUDA device - dcreg_b200 has no CPU fallback")
     sv = args.source_voxel
-    prm = default_params(max_iterations=30, search_radius=0.5, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3,
-                         kappa_target=10.0, detection="SCHUR_CONDITION_NUMBER", handling="PRECONDITIONED_CG")
+    prm = h.c3_params()
     if args.small:
         workloads = {"1x8": [(8, 47)], "2x4": [(4, 71), (4, 72)]}
         n_map, n_scan, n_clouds = 200_000, 10_000, 4
@@ -67,27 +51,12 @@ def main():
         workloads = {"1x128": [(128, 47)], "8x32": [(32, 71 + i) for i in range(8)]}
         n_map, n_scan, n_clouds = 2_000_000, 100_000, 64
     line = {"metric": "frames_per_s", "map_frames": MAP_FRAMES, "source_voxel": sv, "n_scan": n_scan, "n_map": n_map,
-            "workloads": {}, "card": card()}
+            "workloads": {}, "card": h.card()}
     ok_all = True
+    dumps = {}
     with Context(0) as ctx:
-        stream = torch.cuda.ExternalStream(ctx.stream)
-
-        def timed(fn):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            w = time.perf_counter()
-            e0.record(stream)
-            out = fn()
-            e1.record(stream)
-            e1.synchronize()
-            w = time.perf_counter() - w
-            return out, max(e0.elapsed_time(e1), w * 1e3)
-
         for name, spec in workloads.items():
-            seqs, T0, deltas, T_true = [], [], [], []
-            for n, seed in spec:
-                frames, Tt, _, D, _ = make_parking_sequence(n, seed=seed, n_map=n_map, n_scan=n_scan, max_range=20.0)
-                seqs.append(frames); T0.append(Tt[0]); deltas.append(D); T_true.append(Tt)
-            T0, deltas, T_true = np.array(T0), np.concatenate(deltas), np.concatenate(T_true)
+            seqs, T0, deltas, T_true = h.parking_sequences(spec, n_map=n_map, n_scan=n_scan, max_range=20.0)
             n_frames = len(deltas)
 
             def arm(mv, cap):
@@ -95,51 +64,25 @@ def main():
                     return lambda: ctx.icp_run_odometry(prm, seqs, T0, deltas, map_frames=MAP_FRAMES, cell_size=CELL)
                 return lambda: ctx.icp_run_odometry(prm, seqs, T0, deltas, map_frames=MAP_FRAMES, cell_size=CELL,
                                                     source_voxel=sv, map_voxel=mv, map_max_points=cap)
-            arms = {a: arm(mv, cap) for a, mv, cap in ARMS}
-            for fn in arms.values():                                           # warm-up
-                fn()
-            ms = {a: [] for a in arms}
-            res = {}
-            for _ in range(max(1, args.runs)):
-                for a, fn in arms.items():
-                    res[a], t = timed(fn)
-                    ms[a].append(t)
+            outs, ms, med = h.run_arms(ctx, {a: arm(mv, cap) for a, mv, cap in ARMS}, args.runs)
             filt = [[voxel_downsample(f, sv)[0] for f in frames] for frames in seqs]
             w = {"sequences": len(seqs), "frames": n_frames, "tolerance": 1e-8}
             for a, mv, cap in ARMS:
+                res = outs[a]
                 # parity of a filtered arm, and its kept map sizes
-                same, worst, k, maps = True, 0.0, 0, {}
                 if mv is not None:
-                    for s, frames in enumerate(seqs):
-                        rs = res[a][k:k + len(frames)]
-                        placed = [map_points(rs[j].T, filt[s][j]) for j in range(len(frames))]
-                        for j in range(1, len(frames)):
-                            M = voxel_downsample(np.concatenate(placed[max(0, j - MAP_FRAMES):j]), mv, cap)[0]
-                            maps[j] = maps.get(j, 0) + len(M)
-                            ctx.set_target(M, CELL)
-                            ctx.set_source(filt[s][j])
-                            single = ctx.icp_run(prm, rs[j].T_prior, want_log=False)
-                            b = rs[j]
-                            same = same and (b.status, b.iterations, b.converged) == (single.status, single.iterations,
-                                                                                       single.converged)
-                            same = same and b.n_points == len(filt[s][j])
-                            worst = max(worst, float(o.se3_log_distance(single.T, b.T)))
-                        k += len(frames)
+                    same, worst, step_maps = h.replay(ctx, prm, filt, res, lambda s, j, rs, M: voxel_downsample(
+                        h.window_map(filt[s], [r.T for r in rs], j, MAP_FRAMES), mv, cap)[0], CELL, points=True)
                     ok = same and worst <= 1e-8
                     ok_all = ok_all and ok
-                    step_maps = [maps[j] for j in sorted(maps)]
                     parity = {"ok": ok, "identical_status_iterations_converged_points": same, "max_pose_err": worst}
                 else:
-                    step_maps = map_sizes([[len(f) for f in frames] for frames in seqs])
+                    step_maps = h.map_sizes([[len(f) for f in frames] for frames in seqs], MAP_FRAMES)
                     parity = None
-                m = float(np.median(ms[a]))
-                reg = [r for r in res[a] if r.iterations > 0]
-                drift = pose_errors(T_true, [r.T for r in res[a]])
-                w[a] = {"map_voxel": mv, "map_max_points": cap, "frames_per_s": n_frames / (m * 1e-3), "ms": m,
-                        "runs_ms": ms[a], "mean_iterations": float(np.mean([r.iterations for r in reg])),
-                        "converged": int(sum(r.converged for r in reg)), "registered": len(reg),
+                w[a] = {"map_voxel": mv, "map_max_points": cap, **h.arm_block(n_frames, med[a], ms[a], res, T_true),
                         "map_points_per_step": {"mean": float(np.mean(step_maps)), "max": int(max(step_maps))},
-                        "max_err_vs_truth": {"trans_m": drift[0], "rot_deg": drift[1]}, "parity": parity}
+                        "parity": parity}
+                dumps.update(h.result_dumps(f"sweep_{name}_{a}", res, h.FIELDS + ("n_points",)))
             line["workloads"][name] = w
         # the standalone filter: one device call over n_clouds clouds against the twin on each, at 1 and 20 points a voxel
         frames, _, _, _, _ = make_parking_sequence(n_clouds, seed=90, n_map=n_map, n_scan=n_scan, max_range=20.0)
@@ -147,24 +90,17 @@ def main():
         n_pts = sum(len(c) for c in clouds)
         line["filter"] = {"clouds": len(clouds), "points": n_pts, "voxel": sv}
         for cap in (1, 20):
-            ctx.voxel_downsample(clouds, sv, cap)
-            dev_ms, twin_ms = [], []
-            for _ in range(max(1, args.runs)):
-                got, t = timed(lambda: ctx.voxel_downsample(clouds, sv, cap))
-                dev_ms.append(t)
-                t0 = time.perf_counter()
-                twin = [voxel_downsample(c, sv, cap) for c in clouds]
-                twin_ms.append((time.perf_counter() - t0) * 1e3)
+            outs, ms, med = h.run_arms(ctx, {"device": lambda: ctx.voxel_downsample(clouds, sv, cap),
+                                             "twin": lambda: [voxel_downsample(c, sv, cap) for c in clouds]}, args.runs)
+            got, twin = outs["device"], outs["twin"]
             equal = all(p.tobytes() == tp.tobytes() and np.array_equal(i, ti) for (p, i), (tp, ti) in zip(got, twin))
             ok_all = ok_all and equal
-            dm, tm = float(np.median(dev_ms)), float(np.median(twin_ms))
             line["filter"][f"max_points_{cap}"] = {
-                "kept": int(sum(len(i) for _, i in got)), "device_ms": dm, "device_points_per_s": n_pts / (dm * 1e-3),
-                "device_runs_ms": dev_ms, "twin_ms": tm, "twin_points_per_s": n_pts / (tm * 1e-3), "twin_runs_ms": twin_ms,
-                "equal_to_twin": equal}
-    print(json.dumps(line))
-    if not ok_all:
-        raise SystemExit("sweep_odometry_voxel.py: parity FAILED")
+                "kept": int(sum(len(i) for _, i in got)), **h.rate(n_pts, med["device"], ms["device"], "device_", "points"),
+                **h.rate(n_pts, med["twin"], ms["twin"], "twin_", "points"), "equal_to_twin": equal}
+            for c, (p, i) in enumerate(got):
+                dumps[f"sweep_filter_{cap}_{c}_xyz"], dumps[f"sweep_filter_{cap}_{c}_index"] = p, i
+    h.finish(args, line, dumps, ok_all, "sweep_odometry_voxel.py: parity FAILED")
 
 
 if __name__ == "__main__":
