@@ -16,6 +16,7 @@ There is NO CPU fallback: if the CUDA library is missing or no GPU is visible th
 """
 from __future__ import annotations
 
+import bisect
 import contextlib
 import ctypes as C
 import math
@@ -91,6 +92,25 @@ class AdaptiveThreshold(C.Structure):
         super().__init__(float(initial_threshold), float(min_motion), float(max_range))
 
 
+class Gyro(C.Structure):
+    """dcreg_gyro: R_sensor_imu (3, 3) maps IMU-frame rates into the LiDAR frame, bias (3,) rad/s is subtracted first"""
+    _fields_ = [("R_sensor_imu", C.c_double * 9), ("bias", C.c_double * 3)]
+
+    def __init__(self, R_sensor_imu=None, bias=(0.0, 0.0, 0.0)):
+        super().__init__()
+        R = np.eye(3) if R_sensor_imu is None else np.asarray(R_sensor_imu, dtype=np.float64).reshape(3, 3)
+        self.R_sensor_imu[:] = [float(x) for x in R.reshape(-1)]
+        self.bias[:] = [float(x) for x in np.asarray(bias, dtype=np.float64).reshape(3)]
+
+    @property
+    def R(self):
+        return np.array(self.R_sensor_imu[:]).reshape(3, 3)
+
+    @property
+    def b(self):
+        return np.array(self.bias[:])
+
+
 _lib = None
 
 # every symbol include/dcreg_b200.h declares (checked by tests/test_abi.py)
@@ -101,7 +121,7 @@ EXPORTS = [
     "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_icp_run_odometry_adaptive", "dcreg_odometry_open_adaptive", "dcreg_odometry_push_adaptive", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_voxel_downsample_spaced", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_icp_run_odometry_adaptive", "dcreg_odometry_open_adaptive", "dcreg_odometry_push_adaptive", "dcreg_icp_run_odometry_gyro", "dcreg_odometry_open_gyro", "dcreg_odometry_push_gyro", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_voxel_downsample_spaced", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -197,6 +217,18 @@ def load_library():
     lib.dcreg_odometry_push_adaptive.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(C.c_float), C.POINTER(i64), ci, dp,
                                                  C.POINTER(C.c_float), C.POINTER(i64), dp, dp, C.POINTER(ci), C.POINTER(ci),
                                                  C.POINTER(ci), dp, C.POINTER(C.c_float), dp, C.POINTER(IterLog), ci]
+    lib.dcreg_icp_run_odometry_gyro.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
+                                                C.POINTER(i64), ci, C.c_double, ci, ci, C.c_double, C.c_double, ci, ci,
+                                                C.c_double, C.POINTER(AdaptiveThreshold), C.POINTER(Gyro), dp, dp,
+                                                C.POINTER(C.c_float), dp, dp, C.POINTER(i64), C.POINTER(i64), dp, dp,
+                                                C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(C.c_float), dp,
+                                                C.POINTER(IterLog), ci]
+    lib.dcreg_odometry_open_gyro.argtypes = [vp, C.POINTER(IcpParams), ci, C.c_double, ci, ci, C.c_double, C.c_double,
+                                             ci, ci, C.c_double, C.POINTER(AdaptiveThreshold), C.POINTER(Gyro), dp]
+    lib.dcreg_odometry_push_gyro.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(C.c_float), C.POINTER(i64), ci, dp,
+                                             C.POINTER(C.c_float), dp, dp, C.POINTER(i64), C.POINTER(i64), dp, dp,
+                                             C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(C.c_float), dp,
+                                             C.POINTER(IterLog), ci]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -292,6 +324,28 @@ def _pack_timestamps(timestamps, off, name):
     return np.ascontiguousarray(np.concatenate(ts) if ts else np.zeros(0, np.float32))
 
 
+def _pack_gyro(name, gyro, frame_times, gyro_samples, n_frames, n_seqs):
+    """(frame_times (n_frames, 2), samples (rows, 4), sample_offsets int64 [n_seqs + 1]) as contiguous arrays, or Nones
+    without gyro input (a gyro session's push may leave both out; one without the other is refused)"""
+    if gyro is None:
+        if frame_times is not None or gyro_samples is not None:
+            raise ValueError(f"{name}: frame_times and gyro_samples need gyro input")
+        return None, None, None
+    if (frame_times is None) != (gyro_samples is None):
+        raise ValueError(f"{name}: frame_times and gyro_samples go together")
+    if frame_times is None:
+        return None, None, None
+    ft = np.ascontiguousarray(frame_times, dtype=np.float64).reshape(-1, 2)
+    if ft.shape[0] != n_frames:
+        raise ValueError(f"{name}: {n_frames} frames but {ft.shape[0]} frame times")
+    if len(gyro_samples) != n_seqs:
+        raise ValueError(f"{name}: {n_seqs} sequences but {len(gyro_samples)} sample arrays")
+    smp = [np.asarray(x, dtype=np.float64).reshape(-1, 4) for x in gyro_samples]
+    off = np.zeros(n_seqs + 1, dtype=np.int64)
+    off[1:] = np.cumsum([x.shape[0] for x in smp])
+    return ft, np.ascontiguousarray(np.concatenate(smp) if smp else np.zeros((0, 4))), off
+
+
 def _split_deskewed(out, npts):
     """(total, 3) deskewed points cut into one array per frame"""
     at = np.concatenate([[0], np.cumsum(npts)])
@@ -327,6 +381,9 @@ _ODOMETRY_ARGS = {name: " ".join(args).split() for name, args in {
     "dcreg_icp_run_odometry_adaptive": (_RUN, "map_frames motion", _FILTERS,
                                         "max_distance adaptive T_init deltas timestamps frame_points", _OUTPUTS,
                                         "deskewed_xyz search_radius log log_cap"),
+    "dcreg_icp_run_odometry_gyro": (_RUN, "map_frames motion", _FILTERS,
+                                    "max_distance adaptive gyro T_init deltas timestamps frame_times samples",
+                                    "sample_offsets frame_points", _OUTPUTS, "deskewed_xyz search_radius log log_cap"),
     "dcreg_odometry_open": ("params n_seqs cell_size map_frames motion", _FILTERS, "T_init"),
     "dcreg_odometry_open_map": ("params n_seqs cell_size motion", _FILTERS, "max_distance T_init"),
     "dcreg_odometry_open_adaptive": ("params n_seqs cell_size map_frames motion", _FILTERS,
@@ -335,6 +392,10 @@ _ODOMETRY_ARGS = {name: " ".join(args).split() for name, args in {
     "dcreg_odometry_push_deskew": (_PUSH, "timestamps frame_points", _OUTPUTS, "deskewed_xyz log log_cap"),
     "dcreg_odometry_push_adaptive": (_PUSH, "timestamps frame_points", _OUTPUTS,
                                      "deskewed_xyz search_radius log log_cap"),
+    "dcreg_odometry_open_gyro": ("params n_seqs cell_size map_frames motion", _FILTERS,
+                                 "max_distance adaptive gyro T_init"),
+    "dcreg_odometry_push_gyro": (_PUSH, "timestamps frame_times samples sample_offsets frame_points", _OUTPUTS,
+                                 "deskewed_xyz search_radius log log_cap"),
     "dcreg_voxel_downsample": (_DOWNSAMPLE, "out_xyz out_offsets out_index"),
     "dcreg_voxel_downsample_n": (_DOWNSAMPLE, "max_points out_xyz out_offsets out_index"),
     "dcreg_voxel_downsample_spaced": (_DOWNSAMPLE, "max_points min_spacing out_xyz out_offsets out_index"),
@@ -352,9 +413,11 @@ def _odometry_call(lib, h, entry, **values):
     return getattr(lib, entry)(h, *(values.get(k) for k in _ODOMETRY_ARGS[entry]))
 
 
-def _odometry_entry(op, radius=False, voxel_map=False, deskew=False, capped=False, filtered=False):
+def _odometry_entry(op, radius=False, voxel_map=False, deskew=False, capped=False, filtered=False, gyro=False):
     """The entry point of op ("icp_run_odometry", "odometry_open" or "odometry_push") for a call with these settings: the
     narrowest that takes them all.  Each entry point names itself in dcreg_last_error."""
+    if gyro:
+        return f"dcreg_{op}_gyro"
     if radius:
         return f"dcreg_{op}_adaptive"
     if voxel_map:
@@ -609,6 +672,164 @@ def deskew_points(P, timestamps, D):
     ok = np.isfinite(q).all(axis=1)
     rows = np.nonzero(move)[0][ok]
     xyz[rows] = q[ok]
+    return xyz
+
+
+# The gyroscope rotation of dcreg_icp_run_odometry_gyro (dcreg_b200/csrc/se3.cuh): the same formulas and operation order
+# in Python floats and elementwise NumPy (FP64, one rounding per operation, no FMA; sin and cos from libm).  samples:
+# (n, 4) rows (t, wx, wy, wz) in the IMU frame, t strictly ascending.
+GYRO_ORTHO_TOL = 1e-6       # the largest |R^T R - I| entry R_sensor_imu may have
+
+
+def _so3_exp(phi):
+    """Exp(phi) as 9 row-major floats: R_rr = 1 + B (phi_r^2 - t2), R_rc = A K_rc + B phi_r phi_c (se3::so3_exp)"""
+    t2 = (phi[0] * phi[0] + phi[1] * phi[1]) + phi[2] * phi[2]
+    theta = math.sqrt(t2)
+    if theta < SE3_SMALL_ANGLE:
+        A = 1.0 - (t2 / 6.0) * (1.0 - t2 / 20.0)
+        B = 0.5 - (t2 / 24.0) * (1.0 - t2 / 30.0)
+    else:
+        A = math.sin(theta) / theta
+        B = (1.0 - math.cos(theta)) / t2
+    K = [0.0, -phi[2], phi[1], phi[2], 0.0, -phi[0], -phi[1], phi[0], 0.0]
+    return [1.0 + B * (phi[r] * phi[r] - t2) if r == c else A * K[3 * r + c] + B * (phi[r] * phi[c])
+            for r in range(3) for c in range(3)]
+
+
+def _mat3_mul(M, E):
+    """M E as 9 row-major floats, every entry ((m0 e0 + m1 e1) + m2 e2)"""
+    return [(M[3 * r] * E[c] + M[3 * r + 1] * E[3 + c]) + M[3 * r + 2] * E[6 + c] for r in range(3) for c in range(3)]
+
+
+def _gyro_rate(R, bias, row):
+    """R (omega - bias) of one sample row, each entry ((r0 d0 + r1 d1) + r2 d2)"""
+    d = [float(row[1]) - bias[0], float(row[2]) - bias[1], float(row[3]) - bias[2]]
+    return [(R[3 * r] * d[0] + R[3 * r + 1] * d[1]) + R[3 * r + 2] * d[2] for r in range(3)]
+
+
+def _gyro_piece(M, w, d):
+    """M Exp(w d)"""
+    return _mat3_mul(M, _so3_exp([w[0] * d, w[1] * d, w[2] * d]))
+
+
+def _gyro_setup(samples, R_sensor_imu, bias):
+    S = np.asarray(samples, dtype=np.float64).reshape(-1, 4)
+    R = [float(x) for x in np.asarray(R_sensor_imu, dtype=np.float64).reshape(9)]
+    b = [float(x) for x in np.asarray(bias, dtype=np.float64).reshape(3)]
+    return S, [float(t) for t in S[:, 0]], R, b
+
+
+def gyro_rotation(samples, a, b, R_sensor_imu=np.eye(3), bias=(0.0, 0.0, 0.0)):
+    """G(a -> b) (3, 3) as the device forms a prior's rotation: for a <= b the walk from a to b in time order, M = I then M
+    = M Exp(w_j d_j) over the sample intervals [t_j, t_{j+1}) clipped to [a, b] (d_j > 0), w_j = R_sensor_imu (omega_j -
+    bias) (zero-order hold).  It reads only the samples that bracket [a, b]: one at or before a and one at or after b
+    must exist (ValueError otherwise).  a > b: G(b -> a)^T."""
+    a, b = float(a), float(b)
+    if a > b:
+        return gyro_rotation(samples, b, a, R_sensor_imu, bias).T
+    S, t, R, bs = _gyro_setup(samples, R_sensor_imu, bias)
+    j = bisect.bisect_right(t, a) - 1
+    if j < 0 or not t or t[-1] < b:
+        raise ValueError(f"gyro_rotation: the samples do not bracket [{a!r}, {b!r}]")
+    M = [1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0]
+    cur = a
+    while cur < b:
+        nxt = min(t[j + 1], b)
+        M = _gyro_piece(M, _gyro_rate(R, bs, S[j]), nxt - cur)
+        cur = nxt
+        j += 1
+    return np.array(M).reshape(3, 3)
+
+
+def gyro_knots(samples, start, span, R_sensor_imu=np.eye(3), bias=(0.0, 0.0, 0.0)):
+    """The knot table of the sweep [start, start + span] (se3::gyro_knots): knots at its mid-sweep time tm = start + 0.5
+    span and at every sample time strictly inside the sweep other than tm, ascending, each a row of 16: the time, Q =
+    G(tm -> time) as the walk from tm forms it (backwards, with negative durations, for knots before tm), the rate after
+    the knot (of the last sample at or before it) and the rate before it (of the last sample strictly before it).  Needs a
+    sample at or before start and one at or after the end.  Returns (K, 16) float64."""
+    start, span = float(start), float(span)
+    tm, end = start + 0.5 * span, start + span
+    S, t, R, bs = _gyro_setup(samples, R_sensor_imu, bias)
+    lo = bisect.bisect_right(t, start) - 1
+    if lo < 0 or not t or t[-1] < end:
+        raise ValueError(f"gyro_knots: the samples do not bracket the sweep [{start!r}, {end!r}]")
+    jb, ja = bisect.bisect_left(t, tm) - 1, bisect.bisect_right(t, tm) - 1
+    I = [1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0]
+    mid = [tm] + I + _gyro_rate(R, bs, S[ja]) + _gyro_rate(R, bs, S[jb])
+    before, Q, cur, w = [], I, tm, mid[13:16]
+    while jb > lo:                                      # the samples in (start, tm), newest first
+        Q = _gyro_piece(Q, w, t[jb] - cur)
+        cur = t[jb]
+        k = [cur] + Q + _gyro_rate(R, bs, S[jb]) + _gyro_rate(R, bs, S[jb - 1])
+        before.append(k)
+        w = k[13:16]
+        jb -= 1
+    after, Q, cur, w = [], I, tm, mid[10:13]
+    while ja + 1 < len(t) and t[ja + 1] < end:          # the samples in (tm, end)
+        Q = _gyro_piece(Q, w, t[ja + 1] - cur)
+        cur = t[ja + 1]
+        ja += 1
+        k = [cur] + Q + _gyro_rate(R, bs, S[ja]) + _gyro_rate(R, bs, S[ja - 1])
+        after.append(k)
+        w = k[10:13]
+    return np.array(before[::-1] + [mid] + after)
+
+
+def gyro_increment(samples, tm_prev, tm, T_prev2=None, T_prev=None, R_sensor_imu=np.eye(3), bias=(0.0, 0.0, 0.0)):
+    """The increment D a non-anchor frame's prior is composed with (dcreg_icp_run_odometry_gyro): rotation G(tm_prev ->
+    tm), translation that of constant_velocity_increment(T_prev2, T_prev) (zero right after the anchor: T_prev2 None)"""
+    D = np.eye(4) if T_prev2 is None else constant_velocity_increment(T_prev2, T_prev)
+    D[:3, :3] = gyro_rotation(samples, tm_prev, tm, R_sensor_imu, bias)
+    return D
+
+
+def deskew_points_gyro(P, timestamps, frame_time, tm_prev, samples, t_D=(0.0, 0.0, 0.0), R_sensor_imu=np.eye(3),
+                       bias=(0.0, 0.0, 0.0)):
+    """Points of one frame deskewed to mid-sweep as dcreg_icp_run_odometry_gyro does it (se3::deskew_point_gyro).
+    frame_time = (start, span); point i's time is t = start + tau_i span, tm = start + 0.5 span.  G = G(tm -> t) from
+    the sweep's knot table (gyro_knots): for t >= tm the last knot k at or before t, G = Q_k Exp(w_after (t - t_k)); for
+    t < tm the first knot at or after t, G = Q_k Exp(w_before (t - t_k)).  p' = fl32(G p + s t_D), s = (t - tm) / (tm -
+    tm_prev), every entry (((g0 x + g1 y) + g2 z) + s t_D).  A row is copied bit for bit when t = tm, when it has a
+    non-finite coordinate, or when the result would have one or equal it.  P: (N, >=3).  Returns (N, 3) float32."""
+    P = np.asarray(P, dtype=np.float32)
+    if P.ndim != 2 or P.shape[1] < 3:
+        raise ValueError("points must be (N, >=3)")
+    xyz = np.array(P[:, :3])
+    tau = np.asarray(timestamps, dtype=np.float32).reshape(-1)
+    if tau.shape[0] != xyz.shape[0]:
+        raise ValueError(f"deskew_points_gyro: {xyz.shape[0]} points but {tau.shape[0]} timestamps")
+    start, span = float(frame_time[0]), float(frame_time[1])
+    tm = start + 0.5 * span
+    K = gyro_knots(samples, start, span, R_sensor_imu, bias)
+    t = start + tau.astype(np.float64) * span
+    rows = np.nonzero((t != tm) & np.isfinite(xyz).all(axis=1))[0]
+    t = t[rows]
+    fwd = t >= tm
+    k = np.where(fwd, np.searchsorted(K[:, 0], t, side="right") - 1, np.searchsorted(K[:, 0], t, side="left"))
+    w = np.where(fwd[:, None], K[k, 10:13], K[k, 13:16])
+    phi = w * (t - K[k, 0])[:, None]
+    t2 = (phi[:, 0] * phi[:, 0] + phi[:, 1] * phi[:, 1]) + phi[:, 2] * phi[:, 2]
+    theta = np.sqrt(t2)
+    small = theta < SE3_SMALL_ANGLE
+    sn = np.array([math.sin(x) for x in theta]) if len(theta) else theta
+    cs = np.array([math.cos(x) for x in theta]) if len(theta) else theta
+    with np.errstate(invalid="ignore", divide="ignore"):
+        A = np.where(small, 1.0 - (t2 / 6.0) * (1.0 - t2 / 20.0), sn / theta)
+        B = np.where(small, 0.5 - (t2 / 24.0) * (1.0 - t2 / 30.0), (1.0 - cs) / t2)
+    Kx = [np.zeros_like(t2), -phi[:, 2], phi[:, 1], phi[:, 2], np.zeros_like(t2), -phi[:, 0], -phi[:, 1], phi[:, 0],
+          np.zeros_like(t2)]
+    E = [1.0 + B * (phi[:, r] * phi[:, r] - t2) if r == c else A * Kx[3 * r + c] + B * (phi[:, r] * phi[:, c])
+         for r in range(3) for c in range(3)]
+    Q = K[k, 1:10]
+    G = [(Q[:, 3 * r] * E[c] + Q[:, 3 * r + 1] * E[3 + c]) + Q[:, 3 * r + 2] * E[6 + c] for r in range(3) for c in range(3)]
+    s = (t - tm) / (tm - float(tm_prev))
+    tD = [float(x) for x in np.asarray(t_D, dtype=np.float64).reshape(3)]
+    p = xyz[rows].astype(np.float64)
+    with np.errstate(over="ignore", invalid="ignore"):
+        q = np.stack([(((G[3 * r] * p[:, 0] + G[3 * r + 1] * p[:, 1]) + G[3 * r + 2] * p[:, 2]) + s * tD[r])
+                      for r in range(3)], axis=1).astype(np.float32)
+    ok = np.isfinite(q).all(axis=1) & ~(q == xyz[rows]).all(axis=1)
+    xyz[rows[ok]] = q[ok]
     return xyz
 
 
@@ -1110,7 +1331,7 @@ class Context:
                          map_frames: int = 10, cell_size=None, want_log: bool = False, want_cov: bool = False,
                          source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
                          map_max_points: int = 1, timestamps=None, want_deskewed: bool = False, adaptive=None,
-                         want_radius: bool = False):
+                         want_radius: bool = False, gyro=None, frame_times=None, gyro_samples=None):
         """Scan-to-map odometry (`sequences`: a list of lists of (N, >=3) point arrays): frame k of a sequence registers
         against the local map of the frames [k - map_frames, k) before it, each placed at its own registered pose
         (map_points), starting from compose_prior(frame k-1's result, D).  motion "increments": D = deltas[k-1]
@@ -1128,16 +1349,20 @@ class Context:
         adaptive (an AdaptiveThreshold): every frame's search radius follows its sequence's motion-model error under
         the ceiling params.search_radius (dcreg_icp_run_odometry_adaptive; the twin is adaptive_threshold_*), and
         .search_radius holds the radius each frame registered with (0 for anchors); want_radius: .search_radius also
-        without the threshold (that entry point with adaptive = NULL)."""
+        without the threshold (that entry point with adaptive = NULL).
+        gyro (a Gyro), frame_times ((n_frames, 2) (start, span) in seconds over all frames in order) and gyro_samples (one
+        (n_s, 4) array (t, wx, wy, wz) per sequence): every non-anchor frame's prior rotation, and with timestamps its
+        deskew rotation, come from the integrated rates (dcreg_icp_run_odometry_gyro; the twin is gyro_rotation,
+        gyro_increment and deskew_points_gyro); motion must be "constant_velocity".  .search_radius as with adaptive."""
         return self._odometry("icp_run_odometry", params, sequences, T_init, deltas, motion, map_frames, None, cell_size,
                               want_log, want_cov, source_voxel, map_voxel, source_max_points, map_max_points, timestamps,
-                              want_deskewed, adaptive, want_radius)
+                              want_deskewed, adaptive, want_radius, gyro, frame_times, gyro_samples)
 
     def icp_run_odometry_map(self, params, sequences, T_init, deltas=None, motion: str = "increments", *,
                              map_voxel: float, max_distance: float, cell_size=None, want_log: bool = False,
                              want_cov: bool = False, source_voxel: float = 0.0, source_max_points: int = 1,
                              map_max_points: int = 1, timestamps=None, want_deskewed: bool = False, adaptive=None,
-                             want_radius: bool = False):
+                             want_radius: bool = False, gyro=None, frame_times=None, gyro_samples=None):
         """icp_run_odometry with a persistent voxel map per sequence instead of the window (dcreg_icp_run_odometry_map,
         KISS-ICP's VoxelHashMap): frame k registers against M_k, where M_1 = voxel_map_update(empty, F_s(anchor),
         T_init[s]) and M_{k+1} = voxel_map_update(M_k, F_s(frame k), T_out[k], map_voxel, map_max_points,
@@ -1146,11 +1371,12 @@ class Context:
         positions, without map_frames; map_voxel and max_distance are keyword-only."""
         return self._odometry("icp_run_odometry_map", params, sequences, T_init, deltas, motion, 0,
                               float(max_distance), cell_size, want_log, want_cov, source_voxel, map_voxel,
-                              source_max_points, map_max_points, timestamps, want_deskewed, adaptive, want_radius)
+                              source_max_points, map_max_points, timestamps, want_deskewed, adaptive, want_radius, gyro,
+                              frame_times, gyro_samples)
 
     def _odometry(self, name, params, sequences, T_init, deltas, motion, map_frames, max_distance, cell_size, want_log,
                   want_cov, source_voxel, map_voxel, source_max_points, map_max_points, timestamps, want_deskewed,
-                  adaptive, want_radius):
+                  adaptive, want_radius, gyro=None, frame_times=None, gyro_samples=None):
         """icp_run_odometry (max_distance None: the window of map_frames frames) and icp_run_odometry_map (map_frames
         0: the voxel map pruned at max_distance)"""
         motion = _motion(motion, name)
@@ -1160,11 +1386,12 @@ class Context:
         S, n = len(sequences), int(seq_off[-1])
         params, parg, per_lane = self._lanes(name, params, S)
         cell = float(params.search_radius if cell_size is None else cell_size)
-        with_radius = adaptive is not None or want_radius
+        with_radius = adaptive is not None or want_radius or gyro is not None
         entry = _odometry_entry("icp_run_odometry", radius=with_radius, voxel_map=max_distance is not None,
                                 deskew=timestamps is not None or want_deskewed,
                                 capped=source_max_points != 1 or map_max_points != 1,
-                                filtered=source_voxel != 0.0 or map_voxel != 0.0)
+                                filtered=source_voxel != 0.0 or map_voxel != 0.0, gyro=gyro is not None)
+        ft, smp, smp_off = _pack_gyro(name, gyro, frame_times, gyro_samples, n, S)
         ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
                               off if off is not None else np.zeros(1, np.int64), name)
         npts = np.diff(off) if off is not None else np.zeros(0, dtype=np.int64)
@@ -1183,7 +1410,9 @@ class Context:
                 adaptive=None if adaptive is None else C.byref(adaptive), T_init=_optr(o.T_init), deltas=_optr(o.deltas),
                 timestamps=_fptr(ts), frame_points=_iptr(npts), T_prior=_optr(o.T_prior), T_out=_optr(o.T_out),
                 n_iterations=o.n_it, converged=o.conv, status=o.st, cov=_optr(o.cov), deskewed_xyz=_fptr(desk),
-                search_radius=_optr(radius), log=o.logs, log_cap=o.cap)
+                search_radius=_optr(radius), log=o.logs, log_cap=o.cap,
+                gyro=None if gyro is None else C.byref(gyro), frame_times=_optr(ft), samples=_optr(smp),
+                sample_offsets=_iptr(smp_off))
         with self._lane_setting(per_lane):
             out = self._run_batched(name, call, params, n, S, "sequences", T_init, want_log, want_cov, deltas,
                                     want_prior=True)
@@ -1199,26 +1428,27 @@ class Context:
 
     def odometry_map_session(self, params, n_seqs: int, T_init, motion: str = "increments", *,
                              map_voxel: float, max_distance: float, cell_size=None, source_voxel: float = 0.0,
-                             source_max_points: int = 1, map_max_points: int = 1, adaptive=None):
+                             source_max_points: int = 1, map_max_points: int = 1, adaptive=None, gyro=None):
         """Open the context's odometry session with icp_run_odometry_map's voxel map (dcreg_odometry_open_map): the
         OdometrySession of odometry_session, whose pushes give byte for byte what one icp_run_odometry_map call over the
         recording gives, and whose local_map(s) returns sequence s's current map.  The arguments are odometry_session's
         in the same positions, without map_frames; map_voxel and max_distance are keyword-only."""
         return self._open_session("odometry_map_session", params, n_seqs, T_init, motion, 0, float(max_distance),
-                                  cell_size, source_voxel, map_voxel, source_max_points, map_max_points, adaptive)
+                                  cell_size, source_voxel, map_voxel, source_max_points, map_max_points, adaptive, gyro)
 
     def odometry_session(self, params, n_seqs: int, T_init, motion: str = "increments", map_frames: int = 10,
                          cell_size=None, source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
-                         map_max_points: int = 1, adaptive=None):
+                         map_max_points: int = 1, adaptive=None, gyro=None):
         """Open the context's odometry session (dcreg_odometry_open): icp_run_odometry's settings for n_seqs sequences
         whose frames come in pushes (OdometrySession.push).  T_init (n_seqs, 4, 4): the pose of each sequence's first
         frame.  Pushing a recording in any chunks gives byte for byte what one icp_run_odometry call over it gives.
-        One session per context; use it as a context manager, or close() it."""
+        One session per context; use it as a context manager, or close() it.  gyro (a Gyro): dcreg_odometry_open_gyro,
+        whose pushes take frame_times and gyro_samples and return .search_radius."""
         return self._open_session("odometry_session", params, n_seqs, T_init, motion, map_frames, None, cell_size,
-                                  source_voxel, map_voxel, source_max_points, map_max_points, adaptive)
+                                  source_voxel, map_voxel, source_max_points, map_max_points, adaptive, gyro)
 
     def _open_session(self, name, params, n_seqs, T_init, motion, map_frames, max_distance, cell_size, source_voxel,
-                      map_voxel, source_max_points, map_max_points, adaptive):
+                      map_voxel, source_max_points, map_max_points, adaptive, gyro=None):
         """odometry_session (max_distance None) and odometry_map_session (map_frames 0), as in _odometry"""
         motion = _motion(motion, name)
         source_max_points = _max_points(source_max_points, "source_max_points")
@@ -1229,15 +1459,17 @@ class Context:
         params, parg, per_lane = self._lanes(name, params, int(n_seqs))
         cell = float(params.search_radius if cell_size is None else cell_size)
         # dcreg_odometry_open_adaptive's pushes return .search_radius
-        entry = _odometry_entry("odometry_open", radius=adaptive is not None, voxel_map=max_distance is not None)
+        entry = _odometry_entry("odometry_open", radius=adaptive is not None, voxel_map=max_distance is not None,
+                                gyro=gyro is not None)
         with self._lane_setting(per_lane):
             self._check(_odometry_call(
                 self.lib, self._h, entry, params=parg, n_seqs=int(n_seqs), cell_size=cell, map_frames=int(map_frames),
                 motion=motion, source_voxel=float(source_voxel), map_voxel=float(map_voxel),
                 source_max_points=source_max_points, map_max_points=map_max_points,
                 max_distance=0.0 if max_distance is None else float(max_distance),
-                adaptive=None if adaptive is None else C.byref(adaptive), T_init=_dptr(T0)))
-        return OdometrySession(self, params, int(n_seqs), adaptive=adaptive is not None)
+                adaptive=None if adaptive is None else C.byref(adaptive), gyro=None if gyro is None else C.byref(gyro),
+                T_init=_dptr(T0)))
+        return OdometrySession(self, params, int(n_seqs), adaptive=adaptive is not None, gyro=gyro is not None)
 
     def icp_run_pairs(self, params, sources, targets, T_init, cell_size=None, want_log: bool = False,
                       want_cov: bool = False, metrics_threshold=None):
@@ -1336,20 +1568,23 @@ class OdometrySession:
     """The context's odometry session (Context.odometry_session): frames pushed as they arrive, each sequence's local-map
     window and motion-model state kept on the device from one push to the next."""
 
-    def __init__(self, ctx: Context, params: IcpParams, n_seqs: int, adaptive: bool = False):
+    def __init__(self, ctx: Context, params: IcpParams, n_seqs: int, adaptive: bool = False, gyro: bool = False):
         self.ctx, self.params, self.n_seqs = ctx, params, n_seqs
         self.adaptive = adaptive        # opened with an AdaptiveThreshold: every push returns .search_radius
+        self.gyro = gyro                # opened with a Gyro: pushes take frame_times and gyro_samples
         self.open = True
 
     def push(self, frames_per_seq, deltas=None, want_log: bool = False, want_cov: bool = False, timestamps=None,
-             want_deskewed: bool = False):
+             want_deskewed: bool = False, frame_times=None, gyro_samples=None):
         """The next frames of every sequence (dcreg_odometry_push): frames_per_seq, a list of n_seqs lists, possibly
         empty, of (N, >=3) point arrays.  deltas: (frames, 4, 4) increments over the pushed frames in order (entry k maps
         frame k's result to the next frame's prior in its sequence, which may come in a later push), or None for
         identity.  Returns one list of IcpResult per sequence, as icp_run_odometry gives them (.T_prior, .n_points; logs
         only when want_log, .cov when want_cov).  timestamps / want_deskewed: as in icp_run_odometry, nested like
-        frames_per_seq (dcreg_odometry_push_deskew).  A push that fails raises DcregError and leaves the session as it
-        was."""
+        frames_per_seq (dcreg_odometry_push_deskew).  frame_times ((frames, 2) over the pushed frames in order) and
+        gyro_samples (one (n_s, 4) array per sequence, holding the samples that bracket every pushed frame's interval
+        from the previous mid-sweep to its sweep's end): a gyro session's input (dcreg_odometry_push_gyro).  A push that
+        fails raises DcregError and leaves the session as it was."""
         ctx = self.ctx
         if len(frames_per_seq) != self.n_seqs:
             raise ValueError(f"odometry push: {self.n_seqs} sequences but {len(frames_per_seq)} frame lists")
@@ -1367,20 +1602,23 @@ class OdometrySession:
         cov = np.empty((m, 6, 6)) if want_cov else None
         cap = int(self.params.max_iterations) if want_log else 0
         logs = (IterLog * max(cap * n, 1))() if want_log else None
-        radius = np.zeros(m) if self.adaptive else None
+        radius = np.zeros(m) if self.adaptive or self.gyro else None
+        ft, smp, smp_off = _pack_gyro("odometry push", self.gyro or None, frame_times, gyro_samples, n, self.n_seqs)
         ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
                               off if off is not None else np.zeros(1, np.int64), "odometry push")
         desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
-        entry = _odometry_entry("odometry_push", radius=self.adaptive, deskew=timestamps is not None or want_deskewed)
+        entry = _odometry_entry("odometry_push", radius=self.adaptive, deskew=timestamps is not None or want_deskewed,
+                                gyro=self.gyro)
         ctx._check(_odometry_call(
             ctx.lib, ctx._h, entry, seq_offsets=seq_off.ctypes.data_as(C.POINTER(C.c_int)), n_frames=n, xyz=_fptr(xyz),
             frame_offsets=_iptr(off), stride=3, deltas=_optr(D), timestamps=_fptr(ts), frame_points=_iptr(npts),
             T_prior=_dptr(T_prior), T_out=_dptr(T_out), n_iterations=n_it, converged=conv, status=st, cov=_optr(cov),
-            deskewed_xyz=_fptr(desk), search_radius=_optr(radius), log=logs, log_cap=cap))
+            deskewed_xyz=_fptr(desk), search_radius=_optr(radius), log=logs, log_cap=cap, frame_times=_optr(ft),
+            samples=_optr(smp), sample_offsets=_iptr(smp_off)))
         res = _trial_results(st[:n], conv[:n], n_it[:n], T_out, logs, cap, cov)
         for r, Tp, c in zip(res, T_prior, npts):
             r.T_prior, r.n_points = Tp, int(c)
-        if self.adaptive:
+        if radius is not None:
             for r, x in zip(res, radius):
                 r.search_radius = float(x)
         if want_deskewed:

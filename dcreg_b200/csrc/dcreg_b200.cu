@@ -1224,12 +1224,16 @@ __device__ __forceinline__ void odom_increment(int j, const IcpState* __restrict
 // Start of step `step_first` (one thread per lane of `lanes`): lane j < active runs frame step_first + j and nothing
 // after it (its frame range is that one frame, so the frame advance ends the lane), the other lanes run nothing.  The
 // frame's prior is compose_prior(frame prev[j]'s pose, odom_increment); delta holds one entry per frame reference, or is
-// null.
-__global__ void odom_start_kernel(IcpState* states, const long long* __restrict__ seg, double* T_prior, int* cursor,
-                                  int* first, unsigned int* n_active, int lanes, int step_first, int active,
-                                  const int* __restrict__ prev, const int* __restrict__ prev2,
-                                  const double* __restrict__ delta, int motion, int n_frames,
-                                  const double* __restrict__ hist_T) {
+// null.  kGyro (odom_start_gyro_kernel): the increment's rotation is the frame's gyro rotation G[9 f ..] instead, and
+// with tD the increment's translation goes to tD[3 j ..] and the frame's lever arm is zeroed, for
+// odom_deskew_gyro_kernel.
+template <bool kGyro>
+__device__ __forceinline__ void odom_start(IcpState* states, const long long* __restrict__ seg, double* T_prior,
+                                           int* cursor, int* first, unsigned int* n_active, int lanes, int step_first,
+                                           int active, const int* __restrict__ prev, const int* __restrict__ prev2,
+                                           const double* __restrict__ delta, int motion, int n_frames,
+                                           const double* __restrict__ hist_T, const double* __restrict__ G,
+                                           double* __restrict__ tD, float* __restrict__ radius) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j == 0) { *n_active = (unsigned)active; first[lanes] = step_first + active; }
     if (j >= lanes) return;
@@ -1238,11 +1242,37 @@ __global__ void odom_start_kernel(IcpState* states, const long long* __restrict_
     if (j >= active) return;
     double D[16], Ra[9], ta[3];
     odom_increment(j, states, prev, prev2, delta, motion, n_frames, hist_T, D);
+    if (kGyro) {
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) D[4 * r + c] = G[(size_t)f * 9 + 3 * r + c];
+        if (tD) {
+            for (int r = 0; r < 3; ++r) tD[3 * (size_t)j + r] = D[4 * r + 3];
+            radius[f] = 0.0f;
+        }
+    }
     ref_pose(prev[j], n_frames, states, hist_T, Ra, ta);
     double T[16];
     compose_prior(Ra, ta, D, T);
     for (int i = 0; i < 16; ++i) T_prior[(size_t)f * 16 + i] = T[i];
     init_loop_state(states + f, T, seg[f + 1] - seg[f]);
+}
+
+__global__ void odom_start_kernel(IcpState* states, const long long* __restrict__ seg, double* T_prior, int* cursor,
+                                  int* first, unsigned int* n_active, int lanes, int step_first, int active,
+                                  const int* __restrict__ prev, const int* __restrict__ prev2,
+                                  const double* __restrict__ delta, int motion, int n_frames,
+                                  const double* __restrict__ hist_T) {
+    odom_start<false>(states, seg, T_prior, cursor, first, n_active, lanes, step_first, active, prev, prev2, delta,
+                      motion, n_frames, hist_T, nullptr, nullptr, nullptr);
+}
+
+__global__ void odom_start_gyro_kernel(IcpState* states, const long long* __restrict__ seg, double* T_prior, int* cursor,
+                                       int* first, unsigned int* n_active, int lanes, int step_first, int active,
+                                       const int* __restrict__ prev, const int* __restrict__ prev2, int n_frames,
+                                       const double* __restrict__ hist_T, const double* __restrict__ G,
+                                       double* __restrict__ tD, float* __restrict__ radius) {
+    odom_start<true>(states, seg, T_prior, cursor, first, n_active, lanes, step_first, active, prev, prev2, nullptr,
+                     DCREG_MOTION_CONSTANT_VELOCITY, n_frames, hist_T, G, tD, radius);
 }
 
 // The session's window after a push: m points in `pieces` retained frames, piece p being out[dst[p], dst[p+1]) = the
@@ -1334,6 +1364,65 @@ __global__ void odom_deskew_kernel(float4* __restrict__ src, float4* __restrict_
         float4 q = sorted[i];
         const float qi[3] = {q.x, q.y, q.z};
         if (se3::deskew_point(x, ts[seg[b] + __float_as_int(q.w)], qi, o)) {
+            q.x = o[0]; q.y = o[1]; q.z = o[2];
+            sorted[i] = q;
+        }
+        const float px = p.x, py = p.y, pz = p.z;
+        r = sqrtf(px * px + py * py + pz * pz);
+        if (!(r < 3.0e38f)) r = 0.0f;
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, b);
+    const unsigned rmax = __reduce_max_sync(peers, __float_as_uint(r));
+    if (b >= 0 && (int)(threadIdx.x & 31) == __ffs(peers) - 1 && rmax > 0u)
+        atomicMax(reinterpret_cast<unsigned int*>(radius + b), rmax);
+}
+
+// ---- gyroscope input (dcreg_icp_run_odometry_gyro, dcreg_odometry_push_gyro; se3.cuh) -----------------------------
+// Device frame d's sweep: ft[4 d ..] = (start, span, tm, tm_prev), tm = start + 0.5 span its mid-sweep time and tm_prev
+// the previous frame's; its sequence's samples are rows [range[2 d], range[2 d + 1]) of smp; its knot table is knots
+// [kKnotStride knot_off[d] ..], empty for an anchor.
+//
+// Once per call, before the steps (one thread per device frame; the poses play no part): every non-anchor frame's
+// G(tm_prev -> tm), the rotation of its prior's increment, into G[9 d ..], and its sweep's knot table.
+__global__ void odom_gyro_kernel(se3::Gyro g, const double* __restrict__ smp, const double* __restrict__ ft,
+                                 const long long* __restrict__ range, const long long* __restrict__ knot_off,
+                                 int n_frames, double* __restrict__ G, double* __restrict__ knots) {
+    const int d = blockIdx.x * blockDim.x + threadIdx.x;
+    if (d >= n_frames || knot_off[d + 1] == knot_off[d]) return;
+    const double* s = smp + (size_t)range[2 * d] * se3::kSampleStride;
+    const long long n = range[2 * d + 1] - range[2 * d];
+    const double* f = ft + 4 * (size_t)d;
+    se3::gyro_rotation(g, s, n, f[3], f[2], G + 9 * (size_t)d);
+    se3::gyro_knots(g, s, n, f[0], f[2], __dadd_rn(f[0], f[1]), knots + (size_t)knot_off[d] * se3::kKnotStride);
+}
+
+// Per step, after odom_start_gyro_kernel: odom_deskew_kernel with se3::deskew_point_gyro, the lane's increment
+// translation tD[3 j ..] and its frame's knot table; the lever arm is taken again the same way.
+__global__ void odom_deskew_gyro_kernel(float4* __restrict__ src, float4* __restrict__ sorted,
+                                        const long long* __restrict__ seg, int step_first, int active, long long base,
+                                        long long n, const float* __restrict__ ts, const double* __restrict__ ft,
+                                        const long long* __restrict__ knot_off, const double* __restrict__ knots,
+                                        const double* __restrict__ tD, float* __restrict__ radius) {
+    const long long i = base + (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    int b = -1;
+    float r = 0.0f;
+    if (i < base + n) {
+        const int j = corr::segment_of(seg + step_first, active, i);
+        b = step_first + j;
+        const double* f = ft + 4 * (size_t)b;
+        const double* K = knots + (size_t)knot_off[b] * se3::kKnotStride;
+        const int nk = (int)(knot_off[b + 1] - knot_off[b]);
+        const double* t = tD + 3 * (size_t)j;
+        float o[3];
+        float4 p = src[i];
+        const float pi[3] = {p.x, p.y, p.z};
+        if (se3::deskew_point_gyro(K, nk, f[0], f[1], f[2], f[3], t, ts[i], pi, o)) {
+            p.x = o[0]; p.y = o[1]; p.z = o[2];
+            src[i] = p;
+        }
+        float4 q = sorted[i];
+        const float qi[3] = {q.x, q.y, q.z};
+        if (se3::deskew_point_gyro(K, nk, f[0], f[1], f[2], f[3], t, ts[seg[b] + __float_as_int(q.w)], qi, o)) {
             q.x = o[0]; q.y = o[1]; q.z = o[2];
             sorted[i] = q;
         }
@@ -1459,6 +1548,10 @@ struct OdomSettings {
     // follows its sequence's motion-model error, under the ceiling params.search_radius
     bool adaptive = false;
     adaptive::Settings threshold{};
+    // gyroscope input (dcreg_icp_run_odometry_gyro, dcreg_odometry_open_gyro): every non-anchor frame's prior rotation
+    // and deskew rotation come from integrated gyro rates
+    bool gyro = false;
+    se3::Gyro gyro_set{};
     // (a session) dcreg_set_sparse_maps and dcreg_set_map_spacing as they were at open; a one-shot call reads the
     // context's
     bool sparse_maps = false;
@@ -1541,6 +1634,9 @@ struct dcreg_ctx {
     // [points], and the step's twists [lanes][6]
     DevBuf<float> d_odom_ts_in, d_odom_ts;
     DevBuf<double> d_odom_xi;
+    // gyroscope input: the call's samples [rows][4], every device frame's (start, span, tm, tm_prev) [n_frames][4], its
+    // prior's rotation [n_frames][9] and the knot tables [knots][16] (odom_gyro_kernel)
+    DevBuf<double> d_gyro_smp, d_gyro_ft, d_gyro_G, d_gyro_knots;
     // the adaptive threshold: every sequence's (sse, n) [n_seqs], and the radii of the coming step's lanes [lanes]
     DevBuf<adaptive::State> d_thr_state;
     DevBuf<double> d_lane_radius;
@@ -1560,6 +1656,8 @@ struct dcreg_ctx {
         std::vector<long long> map_off;                                // [n_seqs + 1]
         // (set.adaptive) every sequence's threshold state after its last committed frame; a push uploads it
         std::vector<adaptive::State> thr_state;                        // [n_seqs]
+        // (set.gyro) every sequence's last committed mid-sweep time (NaN: none yet, or pushed without frame times)
+        std::vector<double> last_mid;                                  // [n_seqs]
     };
     std::unique_ptr<OdomSession> odom;
     // the voxel filter (voxel_filter): table [slots] keys / first indices, [points] slots, [points + 1] flags and their
@@ -3484,6 +3582,9 @@ static OdomSettings odom_settings(const dcreg_icp_params* params, int n_seqs, do
     return set;
 }
 
+// How far R_sensor_imu^T R_sensor_imu may be from I, entry by entry
+constexpr double kGyroOrthoTol = 1e-6;
+
 // What is wrong with the settings of an odometry call or session, or null
 static const char* odometry_settings_error(const OdomSettings& set, bool deltas) {
     if (!set.voxel_map && set.map_frames < 1) return "map_frames must be >= 1";
@@ -3499,6 +3600,22 @@ static const char* odometry_settings_error(const OdomSettings& set, bool deltas)
     if (set.adaptive && !(a.initial_threshold > 0.0 && a.initial_threshold < INFINITY && a.min_motion >= 0.0 &&
                           a.min_motion < INFINITY && a.max_range > 0.0 && a.max_range < INFINITY))
         return "adaptive: initial_threshold and max_range must be finite and > 0, min_motion finite and >= 0";
+    if (set.gyro) {
+        if (set.motion != DCREG_MOTION_CONSTANT_VELOCITY || deltas)
+            return "gyro input needs DCREG_MOTION_CONSTANT_VELOCITY and deltas == NULL (the gyro gives the rotation)";
+        const se3::Gyro& g = set.gyro_set;
+        bool finite = true;
+        for (int i = 0; i < 9; ++i) finite = finite && std::isfinite(g.R_si[i]);
+        if (!finite) return "gyro: R_sensor_imu has an entry that is not finite";
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) {
+                const double e = (g.R_si[r] * g.R_si[c] + g.R_si[3 + r] * g.R_si[3 + c]) + g.R_si[6 + r] * g.R_si[6 + c];
+                if (!(std::fabs(e - (r == c ? 1.0 : 0.0)) <= kGyroOrthoTol))
+                    return "gyro: R_sensor_imu is not a rotation (an entry of R^T R - I exceeds 1e-6)";
+            }
+        if (!(std::isfinite(g.bias[0]) && std::isfinite(g.bias[1]) && std::isfinite(g.bias[2])))
+            return "gyro: bias has an entry that is not finite";
+    }
     return nullptr;
 }
 
@@ -3512,12 +3629,21 @@ struct StepMap {
     std::vector<Readback> more;
 };
 
+// The gyro input of a call or push (dcreg_icp_run_odometry_gyro, dcreg_odometry_push_gyro): frame_times [n_frames][2]
+// (start, span), samples [rows][4] (t, wx, wy, wz), sequence s's rows [sample_offsets[s], sample_offsets[s + 1])
+struct GyroInput {
+    const double* frame_times = nullptr;
+    const double* samples = nullptr;
+    const int64_t* sample_offsets = nullptr;
+};
+
 // One odometry call or push (run_odometry): its arguments, what its phases share, and the phases, in the order they run
 struct OdomCall {
     dcreg_ctx* ctx; const char* name; const OdomSettings& set; dcreg_ctx::OdomSession* sess;
     const int* seq_offsets; int n_frames; const float* xyz; const int64_t* frame_offsets; int stride;
     const double* deltas; const float* timestamps; const Results& R; int64_t* frame_points; float* deskewed_xyz;
     double* search_radius;                          // (out, may be null) the radius every frame registered with; anchors 0
+    GyroInput gi;                                   // (set.gyro) the frames' times and the samples, or all null
     const int n_seqs = set.n_seqs;
     const dcreg_icp_params* params = &set.params;
     // (dcreg_set_lane_params) every sequence's settings, indexed through the step's lane -> sequence table d_lane_seq
@@ -3548,10 +3674,21 @@ struct OdomCall {
     odom_plan::MapState MS;
     const float4* d_old = nullptr;
     std::vector<double> frame_radius;               // [n_frames] the caller's frames' radii, as their steps run
+    // (set.gyro) every frame's (start, span, tm, tm_prev) and whether it is an anchor, in the caller's order; every
+    // sequence's last mid-sweep time after the push; where the knot offsets and sample ranges are in d_odom_ll
+    std::vector<double> gyro_ft;
+    std::vector<char> gyro_anchor;
+    std::vector<double> next_mid;
+    size_t gyro_ll = 0;
+    long long gyro_knots = 0;
 
-    int check(), upload(), start(), step(int i), finish();
+    int check(), check_gyro(), upload(), start(), step(int i), finish();
     int build_map(const odom_plan::MapInput& in, const long long* ll, const int* ints, DevBuf<float4>& out, StepMap* sm);
 
+    // the sequence of the caller's frame k
+    int frame_seq_of(int k) const {
+        return (int)(std::upper_bound(seq_offsets, seq_offsets + n_seqs + 1, k) - seq_offsets) - 1;
+    }
     // "sequence s, frame k (frame j of the sequence)": the caller's frame k, j-th of sequence s in the call, or its
     // number since the session opened
     std::string frame_name(int s, int k) const {
@@ -3679,6 +3816,7 @@ int OdomCall::check() {
                                (std::isfinite(tau) ? std::to_string(tau) + ", outside [0, 1]" : std::string("not finite"));
                     return DCREG_BAD_ARG;
                 }
+    if ((set.gyro || gi.frame_times || gi.samples || gi.sample_offsets) && (rc = check_gyro())) return rc;
     if (set.source_voxel > 0.0) {
         kept.resize((size_t)n_frames + 1);
         std::vector<int> bad((size_t)n_frames);
@@ -3699,6 +3837,78 @@ int OdomCall::check() {
     }
     if (frame_points)
         for (int k = 0; k < n_frames; ++k) frame_points[k] = src_off[k + 1] - src_off[k];
+    return DCREG_OK;
+}
+
+// (gyro) The frame times and samples, before anything is launched: the samples finite and strictly ascending in time
+// within each sequence; every frame's span finite and > 0, its start, mid-sweep tm = start + 0.5 span and end = start +
+// span distinct; and every non-anchor frame's tm after the previous frame's, with a sample at or before min(tm_prev,
+// start) and one at or after its end.  A push without gyro input (all null) on a gyro session may hold anchors only.
+int OdomCall::check_gyro() {
+    auto bad = [&](const std::string& why) { ctx->err = std::string(name) + ": " + why; return DCREG_BAD_ARG; };
+    const bool given = gi.frame_times && gi.samples && gi.sample_offsets;
+    if (!set.gyro) return bad("frame_times, samples and sample_offsets need a session opened with gyro input");
+    if (!given && (gi.frame_times || gi.samples || gi.sample_offsets))
+        return bad("frame_times, samples and sample_offsets are given together or not at all");
+    if (!given && !sess) return bad("gyro input needs frame_times, samples and sample_offsets");
+    const int64_t* so = gi.sample_offsets;
+    if (given) {
+        if (so[0] != 0) return bad("sample_offsets[0] must be 0");
+        for (int s = 0; s < n_seqs; ++s) {
+            if (so[s + 1] < so[s]) return bad("sample_offsets must be non-decreasing");
+            for (int64_t i = so[s]; i < so[s + 1]; ++i) {
+                const double* r = gi.samples + (size_t)i * se3::kSampleStride;
+                const std::string at = "sequence " + std::to_string(s) + ", sample " + std::to_string(i - so[s]) +
+                                       " (row " + std::to_string(i) + ")";
+                if (!(std::isfinite(r[0]) && std::isfinite(r[1]) && std::isfinite(r[2]) && std::isfinite(r[3])))
+                    return bad(at + ": a value that is not finite");
+                if (i > so[s] && !(r[0] > r[-se3::kSampleStride]))
+                    return bad(at + ": its time is not after the previous sample's (times must be strictly ascending)");
+            }
+        }
+    }
+    gyro_ft.assign((size_t)n_frames * 4, NAN);
+    gyro_anchor.assign((size_t)n_frames, 1);
+    next_mid.assign((size_t)n_seqs, NAN);
+    for (int s = 0; s < n_seqs; ++s) {
+        const bool started = sess && hist.seen[(size_t)s] > 0;
+        double prev = sess ? sess->last_mid[(size_t)s] : NAN;
+        const double* sm = given ? gi.samples + (size_t)so[s] * se3::kSampleStride : nullptr;
+        const long long ns = given ? so[s + 1] - so[s] : 0;
+        for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k) {
+            const bool anchor = !started && k == seq_offsets[s];
+            gyro_anchor[(size_t)k] = anchor;
+            if (!given) {
+                if (!anchor)
+                    return bad(frame_name(s, k) + ": its prior needs gyro samples (dcreg_odometry_push_gyro)");
+                continue;
+            }
+            const double start = gi.frame_times[2 * (size_t)k], span = gi.frame_times[2 * (size_t)k + 1];
+            const double tm = start + 0.5 * span, end = start + span;
+            if (!(std::isfinite(start) && std::isfinite(span) && span > 0.0))
+                return bad(frame_name(s, k) + ": its start and span must be finite and its span > 0");
+            if (!(start < tm && tm < end && std::isfinite(end)))
+                return bad(frame_name(s, k) + ": its span is too small to separate start, mid-sweep and end in FP64");
+            if (!anchor) {
+                if (std::isnan(prev))
+                    return bad(frame_name(s, k) + ": the previous frame's mid-sweep time is unknown (it was pushed "
+                                                  "without frame times)");
+                if (!(tm > prev))
+                    return bad(frame_name(s, k) + ": its mid-sweep time " + std::to_string(tm) +
+                               " is not after the previous frame's, " + std::to_string(prev));
+                const double lo = std::min(prev, start);
+                if (se3::gyro_last(sm, ns, lo, false) < 0)
+                    return bad(frame_name(s, k) + ": no gyro sample at or before " + std::to_string(lo) +
+                               " (the previous mid-sweep time or the sweep's start)");
+                if (ns == 0 || sm[(size_t)(ns - 1) * se3::kSampleStride] < end)
+                    return bad(frame_name(s, k) + ": no gyro sample at or after the sweep's end, " + std::to_string(end));
+            }
+            const double f[4] = {start, span, tm, prev};
+            std::copy(f, f + 4, &gyro_ft[(size_t)k * 4]);
+            prev = tm;
+        }
+        next_mid[(size_t)s] = prev;
+    }
     return DCREG_OK;
 }
 
@@ -3747,6 +3957,27 @@ int OdomCall::upload() {
     if (timestamps) {
         for (int d = 0; d < n_frames; ++d) hll.push_back(frame_offsets[P.input[(size_t)d]]);
         for (int d = 0; d < n_frames; ++d) hll.push_back(src_off[P.input[(size_t)d]]);
+    }
+    // (gyro input) then odom_gyro_kernel's: long long knot_off [n_frames + 1], range [n_frames][2] (device order)
+    gyro_ll = hll.size();
+    if (set.gyro && gi.samples) {
+        hll.push_back(0);
+        for (int d = 0; d < n_frames; ++d) {
+            const int k = P.input[(size_t)d];
+            int nb = 0;
+            const double* f = &gyro_ft[(size_t)k * 4];
+            const int64_t* so = gi.sample_offsets;
+            const int s = frame_seq_of(k);
+            hll.push_back(hll.back() + (gyro_anchor[(size_t)k] ? 0
+                                        : se3::gyro_knot_count(gi.samples + (size_t)so[s] * se3::kSampleStride,
+                                                               so[s + 1] - so[s], f[0], f[2], f[0] + f[1], &nb)));
+        }
+        gyro_knots = hll.back();
+        for (int d = 0; d < n_frames; ++d) {
+            const int s = frame_seq_of(P.input[(size_t)d]);
+            hll.push_back(gi.sample_offsets[s]);
+            hll.push_back(gi.sample_offsets[s + 1]);
+        }
     }
     // the frames in device order, each sorted by its own cell in the sensor frame (identity poses, a box of 1024^3 cells
     // around the sensor: locality only, the chained priors are not known yet); lanes: grid y of the loop kernel, a
@@ -3833,6 +4064,26 @@ int OdomCall::start() {
         odom_ts_gather_kernel<<<(unsigned)((n_points + 255) / 256), 256, 0, ctx->stream>>>(
             ctx->d_odom_ts_in, n_points, ctx->d_scan_seg, n_frames, d_in_at, d_in_at + n_frames,
             set.source_voxel > 0.0 ? ctx->d_vox_index.p : nullptr, ctx->d_odom_ts);
+        ctx->launches++;
+        CK(cudaGetLastError());
+    }
+    if (set.gyro && gi.samples) {   // every non-anchor frame's prior rotation and knot table, from one upload
+        const int64_t rows = gi.sample_offsets[n_seqs];
+        std::vector<double> ft((size_t)n_frames * 4);
+        for (int d = 0; d < n_frames; ++d)
+            std::copy(&gyro_ft[(size_t)P.input[(size_t)d] * 4], &gyro_ft[(size_t)P.input[(size_t)d] * 4] + 4, &ft[(size_t)d * 4]);
+        CK(ctx->d_gyro_smp.ensure(std::max<long long>(rows * se3::kSampleStride, 1)));
+        CK(ctx->d_gyro_ft.ensure((long long)ft.size()));
+        CK(ctx->d_gyro_G.ensure((long long)n_frames * 9));
+        CK(ctx->d_gyro_knots.ensure(std::max<long long>(gyro_knots * se3::kKnotStride, 1)));
+        if (rows)
+            CK(cudaMemcpyAsync(ctx->d_gyro_smp, gi.samples, (size_t)rows * se3::kSampleStride * sizeof(double),
+                               cudaMemcpyHostToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->d_gyro_ft, ft.data(), ft.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        const long long* d_knot_off = ctx->d_odom_ll + gyro_ll;
+        odom_gyro_kernel<<<(unsigned)((n_frames + 127) / 128), 128, 0, ctx->stream>>>(
+            set.gyro_set, ctx->d_gyro_smp, ctx->d_gyro_ft, d_knot_off + n_frames + 1, d_knot_off, n_frames,
+            ctx->d_gyro_G, ctx->d_gyro_knots);
         ctx->launches++;
         CK(cudaGetLastError());
     }
@@ -3925,13 +4176,27 @@ int OdomCall::step(int i) {
     // 3. every lane's frame of this step: its prior and a fresh loop state
     const int* d_prev = ctx->d_odom_int + at_int[(size_t)i] + st.map.piece_frame.size() + st.map.center.size();
     const int* d_prev2 = d_prev + st.active;
-    odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
-        ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
-        st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T);
+    if (set.gyro)       // (gyro) the increment's rotation from the gyro, its translation kept for the deskew
+        odom_start_gyro_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
+            ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active,
+            n_seqs, st.first, st.active, d_prev, d_prev2, n_frames, d_hist_T, ctx->d_gyro_G,
+            timestamps ? ctx->d_odom_xi.p : nullptr, ctx->d_scan_radius);
+    else
+        odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
+            ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
+            st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T);
     ctx->launches++;
     CK(cudaGetLastError());
     // 3b. (timestamps) the step's frames deskewed with the increments their priors used, outside the loop's graphs
-    if (timestamps) {
+    if (timestamps && set.gyro) {
+        const long long a = P.dev_off[(size_t)st.first], np = P.dev_off[(size_t)(st.first + st.active)] - a;
+        const long long* d_knot_off = ctx->d_odom_ll + gyro_ll;
+        odom_deskew_gyro_kernel<<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
+            ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_seg, st.first, st.active, a, np, ctx->d_odom_ts,
+            ctx->d_gyro_ft, d_knot_off, ctx->d_gyro_knots, ctx->d_odom_xi, ctx->d_scan_radius);
+        ctx->launches++;
+        CK(cudaGetLastError());
+    } else if (timestamps) {
         odom_twist_kernel<<<(unsigned)((st.active + 127) / 128), 128, 0, ctx->stream>>>(
             ctx->d_state, st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T,
             ctx->d_odom_xi, ctx->d_scan_radius);
@@ -4037,6 +4302,9 @@ int OdomCall::finish() {
         commit_push(*sess, U, n_frames, seq_offsets, R.T_out, deltas);
         if (set.voxel_map) sess->map_off.assign(sm.kept.begin(), sm.kept.end());
         if (set.adaptive) sess->thr_state.swap(thr);
+        if (set.gyro)
+            for (int s = 0; s < n_seqs; ++s)
+                if (seq_offsets[s + 1] > seq_offsets[s]) sess->last_mid[(size_t)s] = next_mid[(size_t)s];
     }
     return DCREG_OK;
 }
@@ -4050,10 +4318,10 @@ int OdomCall::finish() {
 static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& set, dcreg_ctx::OdomSession* sess,
                         const int* seq_offsets, int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
                         const double* deltas, const float* timestamps, const Results& R, int64_t* frame_points,
-                        float* deskewed_xyz, double* search_radius = nullptr) {
+                        float* deskewed_xyz, double* search_radius = nullptr, GyroInput gi = {}) {
     if (!ctx) return DCREG_BAD_ARG;
     OdomCall o{ctx, name, set, sess, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps, R,
-               frame_points, deskewed_xyz, search_radius};
+               frame_points, deskewed_xyz, search_radius, gi};
     int rc;
     if ((rc = o.check()) || (rc = o.upload()) || (rc = o.start())) return rc;
     for (int i = 1; i < (int)o.P.steps.size() && o.failed < 0; ++i)
@@ -4176,7 +4444,39 @@ int dcreg_icp_run_odometry_adaptive(dcreg_ctx* ctx, const dcreg_icp_params* para
                         deskewed_xyz, search_radius);
 }
 
-// Opens the context's one session with the settings `set` (dcreg_odometry_open, _open_map, _open_adaptive)
+// the settings of dcreg_icp_run_odometry_gyro / dcreg_odometry_open_gyro: the adaptive call's, with the gyro when given
+static OdomSettings odom_gyro_settings(OdomSettings set, const dcreg_gyro* gyro) {
+    if (gyro) {
+        set.gyro = true;
+        std::copy(gyro->R_sensor_imu, gyro->R_sensor_imu + 9, set.gyro_set.R_si);
+        std::copy(gyro->bias, gyro->bias + 3, set.gyro_set.bias);
+    }
+    return set;
+}
+
+int dcreg_icp_run_odometry_gyro(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                                int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                                double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                                int source_max_points, int map_max_points, double max_distance,
+                                const dcreg_adaptive_threshold* adaptive, const dcreg_gyro* gyro, const double* T_init,
+                                const double* deltas, const float* timestamps, const double* frame_times,
+                                const double* samples, const int64_t* sample_offsets, int64_t* frame_points,
+                                double* T_prior, double* T_out, int* n_iterations, int* converged, int* status,
+                                double* cov, float* deskewed_xyz, double* search_radius, dcreg_iter_log* log,
+                                int log_cap) {
+    return run_odometry(ctx, "icp_run_odometry_gyro",
+                        odom_gyro_settings(odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion,
+                                                                  source_voxel, map_voxel, source_max_points,
+                                                                  map_max_points, max_distance, adaptive, T_init,
+                                                                  ctx && ctx->lane_params),
+                                           gyro),
+                        nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
+                        Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
+                        deskewed_xyz, search_radius,
+                        gyro ? GyroInput{frame_times, samples, sample_offsets} : GyroInput{});
+}
+
+// Opens the context's one session with the settings `set` (dcreg_odometry_open, _open_map, _open_adaptive, _open_gyro)
 static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& set) {
     if (ctx->odom) {
         ctx->err = std::string(name) + ": a session is open already (dcreg_odometry_close it first)";
@@ -4197,6 +4497,7 @@ static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     ss->hist = odom_plan::History(n_seqs);
     ss->map_off.assign((size_t)n_seqs + 1, 0);
     ss->thr_state.assign((size_t)n_seqs, adaptive::State{0.0, 0});
+    ss->last_mid.assign((size_t)n_seqs, NAN);
     ss->last_delta.assign((size_t)n_seqs * 16, 0.0);
     for (int s = 0; s < n_seqs; ++s)
         for (int c4 = 0; c4 < 4; ++c4) ss->last_delta[(size_t)s * 16 + 5 * c4] = 1.0;
@@ -4231,6 +4532,19 @@ int dcreg_odometry_open_adaptive(dcreg_ctx* ctx, const dcreg_icp_params* params,
                         odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
                                                source_max_points, map_max_points, max_distance, adaptive, T_init,
                                                ctx && ctx->lane_params));
+}
+
+int dcreg_odometry_open_gyro(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
+                             int motion, double source_voxel, double map_voxel, int source_max_points,
+                             int map_max_points, double max_distance, const dcreg_adaptive_threshold* adaptive,
+                             const dcreg_gyro* gyro, const double* T_init) {
+    if (!ctx) return DCREG_BAD_ARG;
+    return open_session(ctx, "odometry_open_gyro",
+                        odom_gyro_settings(odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion,
+                                                                  source_voxel, map_voxel, source_max_points,
+                                                                  map_max_points, max_distance, adaptive, T_init,
+                                                                  ctx && ctx->lane_params),
+                                           gyro));
 }
 
 int dcreg_odometry_local_map(dcreg_ctx* ctx, int seq, float* xyz, int64_t cap, int64_t* n) {
@@ -4298,6 +4612,20 @@ int dcreg_odometry_push_adaptive(dcreg_ctx* ctx, const int* seq_offsets, int n_f
     return run_odometry(ctx, "odometry_push_adaptive", ss.set, &ss, seq_offsets, n_frames, xyz, frame_offsets, stride,
                         deltas, timestamps, Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior},
                         frame_points, deskewed_xyz, search_radius);
+}
+
+int dcreg_odometry_push_gyro(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
+                             const int64_t* frame_offsets, int stride, const double* deltas, const float* timestamps,
+                             const double* frame_times, const double* samples, const int64_t* sample_offsets,
+                             int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                             int* status, double* cov, float* deskewed_xyz, double* search_radius, dcreg_iter_log* log,
+                             int log_cap) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!ctx->odom) { ctx->err = "odometry_push_gyro: no session is open (dcreg_odometry_open_gyro)"; return DCREG_BAD_ARG; }
+    dcreg_ctx::OdomSession& ss = *ctx->odom;
+    return run_odometry(ctx, "odometry_push_gyro", ss.set, &ss, seq_offsets, n_frames, xyz, frame_offsets, stride,
+                        deltas, timestamps, Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior},
+                        frame_points, deskewed_xyz, search_radius, GyroInput{frame_times, samples, sample_offsets});
 }
 
 // The session's buffers go with it; nothing queued may still read them

@@ -128,6 +128,202 @@ SE3_HD bool deskew_point(const double* xi, float tau, const float* p, float* out
     return move;
 }
 
+// ---- gyroscope rotation (dcreg_icp_run_odometry_gyro) ------------------------------------------------------------
+// Every product, sum and difference below is one IEEE operation (no FMA contraction on the device), so the host build
+// and dcreg_b200.api.gyro_rotation / gyro_knots / deskew_points_gyro give the same bits; on the device only sin and cos
+// (CUDA's sincos) may differ from libm in the last bit.
+#ifdef __CUDA_ARCH__
+#define SE3_MUL(x, y) __dmul_rn(x, y)
+#define SE3_ADD(x, y) __dadd_rn(x, y)
+#define SE3_SUB(x, y) __dsub_rn(x, y)
+#else
+#define SE3_MUL(x, y) ((x) * (y))
+#define SE3_ADD(x, y) ((x) + (y))
+#define SE3_SUB(x, y) ((x) - (y))
+#endif
+
+// The gyro's settings: R_si maps IMU-frame rates into the LiDAR frame (row-major), bias is subtracted first (rad/s)
+struct Gyro {
+    double R_si[9];
+    double bias[3];
+};
+
+// Rows of a sample array: (t, wx, wy, wz), t strictly ascending
+constexpr int kSampleStride = 4;
+// One knot of a sweep's table: time, Q = G(t_m -> time) row-major, the rate after the knot, the rate before it
+constexpr int kKnotStride = 16;
+
+// R = Exp(phi), row-major, by Rodrigues: R = I + A K + B K^2 with K = [phi]x and K^2 = phi phi^T - theta^2 I, so
+// R_rr = 1 + B (phi_r^2 - t2) and R_rc = A K_rc + B phi_r phi_c, with se3_exp_apply's A, B and series threshold
+SE3_HD void so3_exp(const double* phi, double* R) {
+    const double t2 = SE3_ADD(SE3_ADD(SE3_MUL(phi[0], phi[0]), SE3_MUL(phi[1], phi[1])), SE3_MUL(phi[2], phi[2]));
+    const double theta = sqrt(t2);
+    double A, B;
+    if (theta < kSmallAngle) {
+        A = SE3_SUB(1.0, SE3_MUL(t2 / 6.0, SE3_SUB(1.0, t2 / 20.0)));
+        B = SE3_SUB(0.5, SE3_MUL(t2 / 24.0, SE3_SUB(1.0, t2 / 30.0)));
+    } else {
+        double sn, cs;
+#ifdef __CUDA_ARCH__
+        sincos(theta, &sn, &cs);
+#else
+        sn = sin(theta); cs = cos(theta);
+#endif
+        A = sn / theta;
+        B = SE3_SUB(1.0, cs) / t2;
+    }
+    const double K[9] = {0.0, -phi[2], phi[1], phi[2], 0.0, -phi[0], -phi[1], phi[0], 0.0};
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c)
+            R[3 * r + c] = r == c ? SE3_ADD(1.0, SE3_MUL(B, SE3_SUB(SE3_MUL(phi[r], phi[r]), t2)))
+                                  : SE3_ADD(SE3_MUL(A, K[3 * r + c]), SE3_MUL(B, SE3_MUL(phi[r], phi[c])));
+}
+
+// M = M E, every entry ((m0 e0 + m1 e1) + m2 e2)
+SE3_HD void mat3_mul_right(double* M, const double* E) {
+    double o[9];
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c)
+            o[3 * r + c] = SE3_ADD(SE3_ADD(SE3_MUL(M[3 * r], E[c]), SE3_MUL(M[3 * r + 1], E[3 + c])),
+                                   SE3_MUL(M[3 * r + 2], E[6 + c]));
+    for (int i = 0; i < 9; ++i) M[i] = o[i];
+}
+
+// The rate of sample j in the LiDAR frame: R_si (omega_j - bias), each entry ((r0 d0 + r1 d1) + r2 d2)
+SE3_HD void gyro_rate(const Gyro& g, const double* smp, long long j, double* w) {
+    const double* s = smp + (size_t)j * kSampleStride;
+    const double d[3] = {SE3_SUB(s[1], g.bias[0]), SE3_SUB(s[2], g.bias[1]), SE3_SUB(s[3], g.bias[2])};
+    for (int r = 0; r < 3; ++r)
+        w[r] = SE3_ADD(SE3_ADD(SE3_MUL(g.R_si[3 * r], d[0]), SE3_MUL(g.R_si[3 * r + 1], d[1])), SE3_MUL(g.R_si[3 * r + 2], d[2]));
+}
+
+// M = M Exp(w d): one zero-order-hold piece of d seconds (d < 0: walked backwards)
+SE3_HD void gyro_piece(double* M, const double* w, double d) {
+    const double phi[3] = {SE3_MUL(w[0], d), SE3_MUL(w[1], d), SE3_MUL(w[2], d)};
+    double E[9];
+    so3_exp(phi, E);
+    mat3_mul_right(M, E);
+}
+
+// The last sample j in [0, n) with t_j <= t (strict: t_j < t), or -1
+SE3_HD long long gyro_last(const double* smp, long long n, double t, bool strict) {
+    long long lo = 0, hi = n;           // the first sample past t is in [lo, hi]
+    while (lo < hi) {
+        const long long mid = lo + (hi - lo) / 2;
+        const double tm = smp[(size_t)mid * kSampleStride];
+        if (strict ? tm < t : tm <= t) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo - 1;
+}
+
+// G(a -> b), a <= b, over n samples: the walk from a to b in time order, M = I then M = M Exp(w_j d_j) for every sample
+// interval [t_j, t_{j+1}) clipped to [a, b] with d_j > 0, w_j the rate of sample j (zero-order hold).  Needs a sample at
+// or before a and one at or after b (the caller checks); it reads no sample outside them.
+SE3_HD void gyro_rotation(const Gyro& g, const double* smp, long long n, double a, double b, double* G) {
+    for (int i = 0; i < 9; ++i) G[i] = (i % 4 == 0) ? 1.0 : 0.0;
+    long long j = gyro_last(smp, n, a, false);
+    double cur = a;
+    while (cur < b) {
+        const double t1 = smp[(size_t)(j + 1) * kSampleStride];
+        const double nxt = t1 < b ? t1 : b;
+        double w[3];
+        gyro_rate(g, smp, j, w);
+        gyro_piece(G, w, SE3_SUB(nxt, cur));
+        cur = nxt;
+        ++j;
+    }
+}
+
+// The knots of a sweep [start, end] with mid-sweep tm: tm, and every sample time strictly inside (start, end) other
+// than tm.  Returns how many lie before tm (*before) and in all.
+SE3_HD int gyro_knot_count(const double* smp, long long n, double start, double tm, double end, int* before) {
+    const long long lo = gyro_last(smp, n, start, false), m0 = gyro_last(smp, n, tm, true),
+                    m1 = gyro_last(smp, n, tm, false), hi = gyro_last(smp, n, end, true);
+    *before = (int)(m0 - lo);
+    return 1 + (int)(m0 - lo) + (int)(hi - m1);
+}
+
+// The knot table of that sweep, ascending in time, kKnotStride doubles per knot: the time, Q = G(tm -> time) as the walk
+// from tm to the knot forms it (forwards: M = M Exp(w d); backwards: the same with d < 0, which is G(time -> tm)^T up
+// to rounding), the rate after the knot (of the last sample at or before it) and the rate before it (of the last sample
+// strictly before it).  Needs a sample at or before start and one at or after end.
+SE3_HD void gyro_knots(const Gyro& g, const double* smp, long long n, double start, double tm, double end, double* K) {
+    int nb = 0;
+    gyro_knot_count(smp, n, start, tm, end, &nb);
+    double Q[9];
+    double* k = K + (size_t)nb * kKnotStride;           // tm's knot
+    for (int i = 0; i < 9; ++i) Q[i] = (i % 4 == 0) ? 1.0 : 0.0;
+    long long ja = gyro_last(smp, n, tm, false), jb = gyro_last(smp, n, tm, true);
+    k[0] = tm;
+    for (int i = 0; i < 9; ++i) k[1 + i] = Q[i];
+    gyro_rate(g, smp, ja, k + 10);
+    gyro_rate(g, smp, jb, k + 13);
+    double cur = tm;                                    // backwards: the samples in (start, tm), newest first
+    for (int i = nb - 1; i >= 0; --i) {
+        const double t = smp[(size_t)jb * kSampleStride];
+        double* o = K + (size_t)i * kKnotStride;
+        gyro_piece(Q, K + (size_t)(i + 1) * kKnotStride + 13, SE3_SUB(t, cur));
+        cur = t;
+        o[0] = t;
+        for (int c = 0; c < 9; ++c) o[1 + c] = Q[c];
+        gyro_rate(g, smp, jb, o + 10);
+        gyro_rate(g, smp, jb - 1, o + 13);
+        --jb;
+    }
+    for (int i = 0; i < 9; ++i) Q[i] = (i % 4 == 0) ? 1.0 : 0.0;
+    cur = tm;                                           // forwards: the samples in (tm, end)
+    for (double* o = k + kKnotStride; ja + 1 < n && smp[(size_t)(ja + 1) * kSampleStride] < end; o += kKnotStride) {
+        const double t = smp[(size_t)(ja + 1) * kSampleStride];
+        gyro_piece(Q, o - kKnotStride + 10, SE3_SUB(t, cur));
+        cur = t;
+        ++ja;
+        o[0] = t;
+        for (int c = 0; c < 9; ++c) o[1 + c] = Q[c];
+        gyro_rate(g, smp, ja, o + 10);
+        gyro_rate(g, smp, ja - 1, o + 13);
+    }
+}
+
+// One point of a sweep deskewed to mid-sweep with the gyro: the point's time t = start + tau span; G = G(tm -> t) from
+// the sweep's knot table K (nk knots): for t >= tm the last knot k at or before t, G = Q_k Exp(w_after (t - t_k)); for
+// t < tm the first knot at or after t, G = Q_k Exp(w_before (t - t_k)) (the walk from tm to t, continued from the knot);
+// out = fl32(G p + s tD), s = (t - tm) / (tm - tm_prev), every entry (((g0 x + g1 y) + g2 z) + s tD_r).  p itself, bit
+// for bit, when t = tm, when p has a non-finite coordinate, or when the result would have one or equal p.  Returns
+// whether it moved the point.
+SE3_HD bool deskew_point_gyro(const double* K, int nk, double start, double span, double tm, double tm_prev,
+                              const double* tD, float tau, const float* p, float* out) {
+    const double t = SE3_ADD(start, SE3_MUL((double)tau, span));
+    bool move = t != tm && isfinite(p[0]) && isfinite(p[1]) && isfinite(p[2]);
+    float o[3] = {p[0], p[1], p[2]};
+    if (move) {
+        int lo = 0, hi = nk;            // the first knot past t (t >= tm), or at or past t (t < tm), is in [lo, hi]
+        const bool fwd = t >= tm;
+        while (lo < hi) {
+            const int mid = (lo + hi) / 2;
+            const double tk = K[(size_t)mid * kKnotStride];
+            if (fwd ? tk <= t : tk < t) lo = mid + 1;
+            else hi = mid;
+        }
+        const double* k = K + (size_t)(fwd ? lo - 1 : lo) * kKnotStride;
+        double G[9];
+        for (int i = 0; i < 9; ++i) G[i] = k[1 + i];
+        gyro_piece(G, k + (fwd ? 10 : 13), SE3_SUB(t, k[0]));
+        const double s = SE3_SUB(t, tm) / SE3_SUB(tm, tm_prev);
+        const double x = p[0], y = p[1], z = p[2];
+        for (int r = 0; r < 3; ++r)
+            o[r] = (float)SE3_ADD(SE3_ADD(SE3_ADD(SE3_MUL(G[3 * r], x), SE3_MUL(G[3 * r + 1], y)), SE3_MUL(G[3 * r + 2], z)),
+                                  SE3_MUL(s, tD[r]));
+        move = isfinite(o[0]) && isfinite(o[1]) && isfinite(o[2]) && !(o[0] == p[0] && o[1] == p[1] && o[2] == p[2]);
+    }
+    for (int r = 0; r < 3; ++r) out[r] = move ? o[r] : p[r];
+    return move;
+}
+
+#undef SE3_MUL
+#undef SE3_ADD
+#undef SE3_SUB
+
 }  // namespace se3
 
 #undef SE3_HD

@@ -201,6 +201,62 @@ def make_parking_sweeps(n_frames, seed=47, n_map=500_000, n_scan=6_000, map_seed
     return skewed, stamps, T_true, deltas, frames
 
 
+def make_parking_imu(n_frames, rate_hz=200, noise=0.0, bias=(0.0, 0.0, 0.0), seed=71, period=0.1, pure_rotation=False,
+                     R_sensor_imu=None, n_scan=6_000, map_seed=43, n_map=500_000, extent=60.0, max_range=30.0,
+                     path_half_length=20.0):
+    """make_parking_frames' path as a continuous trajectory seen by a spinning LiDAR with a gyroscope.  Frame k's sweep is
+    [start_k, start_k + period) with start_k = (k - 0.5) period, mid-sweep tm_k = start_k + 0.5 period, and T(tm_k) =
+    T_true[k].  Between consecutive mid-sweeps the twist is constant: T(t) = T_{k-1} Exp(((t - tm_{k-1}) / (tm_k -
+    tm_{k-1})) xi_k), xi_k = Log(inv(T_{k-1}) T_k) (before tm_0 the first interval's twist, after the last mid-sweep the
+    last one's).  Point i of frame k gets tau = (azimuth + pi) / (2 pi) from the unskewed frame and is measured from
+    T(start_k + tau period): the skewed point is fl32(Exp(-sigma xi) p), sigma = (t - tm_k) / interval.  The gyro
+    samples are the exact body rates phi_k / interval, in the IMU frame (R_sensor_imu^T, default identity), at rate_hz
+    between consecutive mid-sweeps and at every mid-sweep, so the zero-order hold is exact for rotation; plus seeded
+    white noise (rad/s) and a constant bias when given.  pure_rotation: the path's headings about a fixed position.
+    Returns (skewed frames, timestamps, frame_times (n, 2) (start, span), samples (m, 4) (t, wx, wy, wz), T_true (n, 4,
+    4), unskewed frames)."""
+    from dcreg_b200 import api
+    frames, T_true, _, _ = make_parking_frames(n_frames, seed=seed, n_map=n_map, n_scan=n_scan, map_seed=map_seed,
+                                               extent=extent, max_range=max_range, path_half_length=path_half_length)
+    if pure_rotation:
+        T_true = T_true.copy()
+        T_true[:, :3, 3] = 0.0
+    frame_times = np.stack([(np.arange(n_frames) - 0.5) * period, np.full(n_frames, float(period))], axis=1)
+    tm = frame_times[:, 0] + 0.5 * frame_times[:, 1]
+    xi = [api.se3_log(np.linalg.inv(T_true[k - 1]) @ T_true[k]) for k in range(1, n_frames)] or [np.zeros(6)]
+    dt = np.diff(tm) if n_frames > 1 else np.array([float(period)])
+    seg = lambda k: min(max(k, 1), max(n_frames - 1, 1)) - 1              # the interval [tm_{j-1}, tm_j] of index j
+    sub = max(1, int(round(rate_hz * period)))
+    times, rates = [], []
+    for j in range(-1, n_frames):                    # every interval, plus one before the first and one after the last
+        a = tm[0] - dt[0] if j < 0 else tm[j]
+        step = dt[0] if j < 0 else dt[min(j, len(dt) - 1)]
+        x = xi[seg(j + 1)]
+        for i in range(sub):
+            times.append(a + i * (step / sub))
+            rates.append(x[3:] / dt[seg(j + 1)])
+    times.append(tm[-1] + dt[-1])
+    rates.append(rates[-1])
+    Rsi = np.eye(3) if R_sensor_imu is None else np.asarray(R_sensor_imu, dtype=np.float64)
+    rng = np.random.default_rng([seed, 3])
+    w = np.array(rates) @ Rsi + np.asarray(bias, dtype=np.float64) + rng.normal(0.0, noise, (len(rates), 3))
+    samples = np.concatenate([np.array(times)[:, None], w], axis=1)
+    skewed, stamps = [], []
+    for k in range(n_frames):
+        p = frames[k].astype(np.float64)
+        tau = np.clip(((np.arctan2(p[:, 1], p[:, 0]) + np.pi) / (2.0 * np.pi)).astype(np.float32), np.float32(0.0),
+                      np.float32(1.0))
+        t = frame_times[k, 0] + tau.astype(np.float64) * frame_times[k, 1]
+        before = t < tm[k]
+        sig = np.where(before, (t - tm[k]) / dt[seg(k)], (t - tm[k]) / dt[seg(k + 1)])
+        q = np.empty_like(p)
+        for side, x in ((before, xi[seg(k)]), (~before, xi[seg(k + 1)])):
+            q[side] = api.se3_exp_apply(x, -sig[side], p[side])
+        skewed.append(np.ascontiguousarray(q.astype(np.float32)))
+        stamps.append(tau)
+    return skewed, stamps, frame_times, samples, T_true, frames
+
+
 def make_large_map(n_side=4, spacing=1000.0, n_map=500_000, map_seed=43, extent=60.0):
     """A prior map too large for a dense grid: n_side x n_side parking maps (_parking_map, tile t from seed map_seed + t),
     their centres spacing metres apart on a square lattice starting at the origin.  At 0.5 m cells the 4 x 4 default

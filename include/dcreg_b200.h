@@ -608,6 +608,69 @@ int dcreg_odometry_push_adaptive(dcreg_ctx* ctx, const int* seq_offsets, int n_f
                                  int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
                                  int* status, double* cov, float* deskewed_xyz, double* search_radius, dcreg_iter_log* log,
                                  int log_cap);
+/* GYROSCOPE INPUT: the rotation over a sweep, and between two sweeps, from integrated angular rates instead of the
+ * constant-velocity guess.  R_sensor_imu: the rotation from the IMU frame to the LiDAR frame (row-major); bias: a
+ * constant gyro bias (rad/s).  Nothing is estimated. */
+typedef struct dcreg_gyro {
+    double R_sensor_imu[9];
+    double bias[3];
+} dcreg_gyro;
+/* dcreg_icp_run_odometry_adaptive with gyro input.  gyro == NULL is that call itself (frame_times, samples and
+ * sample_offsets are not read): the same launches and the same bytes.
+ * - Inputs (HOST memory): frame_times, n_frames x 2 doubles (start, span) in seconds; point i of frame k was measured at
+ *   t = start_k + tau_i span_k (tau: timestamps), and the mid-sweep time tm_k = start_k + 0.5 span_k is the time of
+ *   T_out[k].  samples: rows of 4 doubles (t, wx, wy, wz) in the IMU frame, sequence s's rows [sample_offsets[s],
+ *   sample_offsets[s + 1]) (n_seqs + 1 int64, from 0).
+ * - Rate: w_j = R_sensor_imu (omega_j - bias) in FP64, held on [t_j, t_{j+1}) (zero-order hold).
+ * - Rotation G(a -> b), a <= b: the walk from a to b in time order, M = I then M = M Exp(w_j d_j) over the sample
+ *   intervals clipped to [a, b] (Exp: Rodrigues with the deskew's small-angle series).  It reads only the samples that
+ *   bracket [a, b], which is what makes a session's chunking exact.
+ * - Prior of a non-anchor frame k: D = [G(tm_{k-1} -> tm_k) | t_D], t_D the translation of the constant-velocity
+ *   increment (zero right after the anchor), T_prior[k] = compose_prior(T_out[k-1], D).  motion must be
+ *   DCREG_MOTION_CONSTANT_VELOCITY and deltas NULL.
+ * - Deskew of a non-anchor frame (timestamps given): p' = fl32(G(tm_k -> t) p + s t_D), s = (t - tm_k) / (tm_k -
+ *   tm_{k-1}); G(tm -> t) for t < tm walks backwards (= G(t -> tm)^T up to rounding).  A point is copied bit for bit
+ *   when t = tm, when it has a non-finite coordinate, or when the result would have one or equal it.  timestamps ==
+ *   NULL: every tau = 0.5, the points are untouched and only the priors use the gyro.
+ * - dcreg_b200.api.gyro_rotation, gyro_knots, gyro_increment and deskew_points_gyro are the NumPy twin (bit for bit on
+ *   the host; the device's sin and cos may differ in the last bit).  Everything else (source filter, then the deskew at
+ *   the frame's step; maps; adaptive threshold; anchors; aborts; covariances) is dcreg_icp_run_odometry_adaptive's.
+ * - Cost: one upload of the samples and one launch per call (one thread per frame: its prior's rotation and its sweep's
+ *   knot table, the rotation at every sample time inside the sweep relative to mid-sweep); per step the start kernel
+ *   takes the rotation from there and one deskew launch replaces the twist and deskew launches (per point: a binary
+ *   search over the knots, one Exp, a 3x3 product).  No host sync is added; the launches do not depend on n_seqs.
+ * Errors (DCREG_BAD_ARG before anything is launched, naming the sequence, frame or sample): R_sensor_imu not finite or
+ * with an entry of R^T R - I above 1e-6; a bias that is not finite; sample times not strictly ascending within a
+ * sequence or a sample value that is not finite; a span that is not finite and > 0 (or too small to separate start,
+ * tm and end); mid-sweep times not strictly ascending within a sequence; a non-anchor frame with no sample at or before
+ * min(tm_{k-1}, start_k) or none at or after start_k + span_k; another motion model, or deltas. */
+int dcreg_icp_run_odometry_gyro(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                                int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                                double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                                int source_max_points, int map_max_points, double max_distance,
+                                const dcreg_adaptive_threshold* adaptive, const dcreg_gyro* gyro, const double* T_init,
+                                const double* deltas, const float* timestamps, const double* frame_times,
+                                const double* samples, const int64_t* sample_offsets, int64_t* frame_points,
+                                double* T_prior, double* T_out, int* n_iterations, int* converged, int* status,
+                                double* cov, float* deskewed_xyz, double* search_radius, dcreg_iter_log* log,
+                                int log_cap);
+/* dcreg_odometry_open_adaptive with gyro input (gyro == NULL: that call itself), and its push.  The session keeps every
+ * sequence's last mid-sweep time.  Contract: any chunking gives byte for byte the one dcreg_icp_run_odometry_gyro call's
+ * outputs; a push whose first frame's previous mid-sweep time lies in an earlier push must include the samples that
+ * bracket it.  A push that fails commits nothing.  dcreg_odometry_push, _push_deskew and _push_adaptive on a gyro
+ * session (and _push_gyro with frame_times, samples and sample_offsets all NULL) push frames with no samples: they are
+ * DCREG_BAD_ARG when a frame is not an anchor, and an anchor pushed that way leaves its mid-sweep time unknown, so the
+ * sequence's next frame is refused too.  Gyro input on a session opened without it is DCREG_BAD_ARG. */
+int dcreg_odometry_open_gyro(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
+                             int motion, double source_voxel, double map_voxel, int source_max_points,
+                             int map_max_points, double max_distance, const dcreg_adaptive_threshold* adaptive,
+                             const dcreg_gyro* gyro, const double* T_init);
+int dcreg_odometry_push_gyro(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
+                             const int64_t* frame_offsets, int stride, const double* deltas, const float* timestamps,
+                             const double* frame_times, const double* samples, const int64_t* sample_offsets,
+                             int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                             int* status, double* cov, float* deskewed_xyz, double* search_radius, dcreg_iter_log* log,
+                             int log_cap);
 /* Voxel downsampling of many clouds in one call (KISS-ICP's VoxelDownsample rule: the first point of every voxel).
  * xyz / offsets / stride: HOST memory as in dcreg_icp_run_scans (n_clouds + 1 offsets, ascending strictly from 0, at
  * most 2^29 - 1 points).  With inv = 1.0 / voxel in FP64, point i's voxel is (floor((double)x inv), floor((double)y inv),
