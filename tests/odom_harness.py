@@ -1,5 +1,6 @@
-"""What the odometry and voxel GPU tests share: the scenes, the solver settings, the asserts, the twins of the window and
-voxel maps, one driver that pushes a recording into a session in chunks, and the raw callers of the C entry points.
+"""What the odometry and voxel GPU tests share: the scenes, the asserts, the twins of the window and voxel maps, one
+driver that pushes a recording into a session in chunks, and the raw callers of the C entry points.  The context, the
+solver settings and the comparison of two runs come from harness.py.
 
 Each test module keeps its own scenario (sequence lengths, points per frame, voxel sizes, caps, distances) and passes
 it in; module-scoped fixtures imported from here are still set up once per module."""
@@ -8,19 +9,10 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import dcreg_oracle as o
+from harness import log_bytes
 
-RADIUS = 0.5
 CELL = 0.5
 RAGGED = [[1, 2, 0], [0, 0, 5], [0, 3, 1], [0, 2, 6]]     # sequences of 1, 7 and 12 frames at different rates
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
 
 
 def parking(lens=(1, 7, 12), n_scan=20_000):
@@ -82,26 +74,12 @@ def crowded_clouds():
     return clouds_of_every_case() + [crowded]
 
 
-def params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
-
-
 def one_per_push(lens):
     """Pushes of one frame per sequence while it has frames"""
     return [[1 if k < n else 0 for n in lens] for k in range(max(lens))]
 
 
 # -- asserts --
-def rel_err(a, b):
-    a = np.asarray(a, dtype=np.float64); b = np.asarray(b, dtype=np.float64)
-    return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-300))
-
-
 def split(res, seqs):
     out, k = [], 0
     for s in seqs:
@@ -112,20 +90,6 @@ def split(res, seqs):
 
 def seq_results(res, seqs):
     return [list(r) for r in split(res, seqs)]
-
-
-def assert_same_run(b, single, logs=True):
-    assert (b.status, b.iterations, b.converged) == (single.status, single.iterations, single.converged)
-    assert o.se3_log_distance(single.T, b.T) < 1e-8
-    if not logs:
-        return
-    assert len(b.logs) == len(single.logs)
-    for x, y in zip(b.logs, single.logs):
-        assert x.n_effective == y.n_effective and x.n_corr_pt == y.n_corr_pt
-        assert list(x.analysis.degenerate_mask) == list(y.analysis.degenerate_mask)
-        if x.status == 0:
-            assert rel_err(np.array(x.H27), np.array(y.H27)) < 1e-8
-            assert np.max(np.abs(np.array(x.dx) - np.array(y.dx))) < 1e-8
 
 
 def assert_anchor(r, T0):
@@ -149,12 +113,6 @@ def assert_priors(res, seqs, T_init, deltas, motion="increments"):
                 D = np.eye(4) if deltas is None else deltas[k + j - 1]
             assert rs[j].T_prior.tobytes() == compose_prior(rs[j - 1].T, D).tobytes(), (s, j)
         k += len(rs)
-
-
-def log_bytes(rec):
-    r = type(rec).from_buffer_copy(bytes(rec))
-    r.iter_time_ms = 0.0
-    return bytes(r)
 
 
 def result_bytes(res):

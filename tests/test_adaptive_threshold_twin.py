@@ -3,16 +3,14 @@
 50-digit evaluation, the sample rule at min_motion, poses that are not finite, the radius rule, and
 dcreg_b200/csrc/adaptive_threshold.cuh built as host C++ against the twin."""
 import math
-import os
-import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
 from dcreg_b200 import api
+from harness import tool_program
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INIT, MIN_MOTION, MAX_RANGE, CEILING = 2.0, 0.1, 100.0, 2.0
 
 
@@ -165,12 +163,7 @@ def test_chunked_replay_equals_the_straight_one():
 
 
 def test_host_build_matches_the_twin(tmp_path):
-    cxx = shutil.which("g++") or shutil.which("c++")
-    if not cxx:
-        pytest.skip("no host C++ compiler")
-    exe = tmp_path / "test_adaptive_threshold"
-    subprocess.run([cxx, "-O2", "-std=c++17", "-o", str(exe), os.path.join(ROOT, "tools", "test_adaptive_threshold.cpp")],
-                   check=True, capture_output=True, text=True)
+    exe = tool_program(tmp_path, "test_adaptive_threshold.cpp", compiler="c++")
     rng = np.random.default_rng(29)
     frames = corrections(rng, 400)
     for ang in (0.0, 1e-12, 1e-6, 0.1, 1.0, math.pi - 1e-6, math.pi - 1e-3):      # large corrections too

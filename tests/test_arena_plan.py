@@ -1,25 +1,18 @@
 """Host side of dcreg_icp_run_pairs (many scan/target pairs, each against its own target): the grid-arena planning of
 arena_plan.hpp compiled as plain host C++, and the seeded scan-to-submap pair generator the benchmark and the GPU tests
 use."""
-import os
-import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from harness import tool_program
 
 
 def test_arena_plan(tmp_path):
     """arena_plan: per-cloud dims and cell offsets, the +-2^19 cell range, the dense-cell limits per cloud and per call,
     the offset tables, and the arena's grouping of every cloud equal to the cloud grouped alone."""
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    exe = tmp_path / "test_arena_plan"
-    subprocess.run([gxx, "-O2", "-std=c++17", "-o", str(exe), os.path.join(ROOT, "tools", "test_arena_plan.cpp")],
-                   check=True, capture_output=True, text=True)
+    exe = tool_program(tmp_path, "test_arena_plan.cpp")
     res = subprocess.run([str(exe)], capture_output=True, text=True)
     assert res.returncode == 0, res.stdout + res.stderr
     assert "ARENA_PLAN_OK" in res.stdout

@@ -11,18 +11,7 @@ duplicated points, that whenever the rule says "skip" the re-ranked first five o
 import numpy as np
 import pytest
 
-F = np.float32
-
-
-def dist2(q, pts, pairwise=False):
-    """corr::dist2: float32 differences, products and sums, x then y then z, no fused operations.  Every query against
-    every point ((m, n) result), or with pairwise=True query i against point i."""
-    if not pairwise:
-        q, pts = q[:, None, :], pts[None, :, :]
-    ex = (q[..., 0] - pts[..., 0]).astype(F)
-    ey = (q[..., 1] - pts[..., 1]).astype(F)
-    ez = (q[..., 2] - pts[..., 2]).astype(F)
-    return ((ex * ex).astype(F) + (ey * ey).astype(F)).astype(F) + (ez * ez).astype(F)
+from harness import F, dist2
 
 
 def order(d2):

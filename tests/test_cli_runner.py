@@ -5,7 +5,6 @@ sequences), PCD reader/writer round trip, pose-error metric against the oracle, 
 GPU test: the binary reproduces the reference's shipped per-iteration CSV rows (tests/golden/golden.json) on the shipped
 cylinder cloud for every method of the SO(3) path.
 """
-import csv
 import math
 import os
 import subprocess
@@ -15,112 +14,12 @@ import pytest
 
 import dcreg_oracle as o
 from dcreg_b200 import build as b
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden")
-
-METHODS = {
-    "ME-SR": ("FULL_EVD_MIN_EIGENVALUE", "SOLUTION_REMAPPING"),
-    "ME-TSVD": ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD"),
-    "ME-TReg": ("FULL_EVD_MIN_EIGENVALUE", "STANDARD_REGULARIZATION"),
-    "FCN-SR": ("FULL_SVD_CONDITION", "SOLUTION_REMAPPING"),
-    "Ours": ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG"),
-}
+from harness import GOLD, METHODS, dump, read_csv, write_config
 
 
 @pytest.fixture(scope="module")
 def runner():
     return b.build_runner()
-
-
-def write_config(path, out_dir, setup, methods, extra_methods="", extra=""):
-    x, y, z = setup["init_xyz"]
-    r, p, w = setup["init_rpy_deg"]
-    lines = "\n".join(f'  "{m}": [ "{METHODS[m][0]}", "{METHODS[m][1]}" ]' for m in methods)
-    with open(path, "w") as f:
-        f.write(f"""
-test:
-  num_runs: 1     # Number of test runs (set to 1 for single run)
-  save_pcd: true  # Save aligned point clouds
-  save_error_pcd: false
-  visualize: false  # Enable visualization
-
-# Output Options
-output:
-  save_csv: true
-
-paths:
-  folder_path: "{GOLD}/"
-  output_folder: "{out_dir}/"
-  source_pcd: "cylinder_7562.pcd"
-  target_pcd: "cylinder_7562.pcd"
-
-icp:
-  search_radius: {setup['search_radius']}
-  max_iterations: {setup['max_iterations']}
-  error_threshold: 0.2  # Error threshold (m)
-
-  CONVERGENCE_THRESH_TRANS: {setup['conv_trans']}
-  CONVERGENCE_THRESH_ROT: {setup['conv_rot']}
-
-  normal_nn: 5
-  use_weight_derivative: {'true' if setup['use_weight_derivative'] else 'false'}
-
-initial_noise:
-  # x: 9.0
-  x: {x}
-  y: {y}
-  z: {z}
-  roll_deg: {r}
-  pitch_deg: {p}
-  yaw_deg: {w}
-
-gt_pose:
-  x: 0.0
-  y: 0.0
-  z: 0.0
-  roll_deg: 0.0
-  pitch_deg: 0.0
-  yaw_deg: 0.
-
-degeneracy:
-  condition_threshold: {setup['cond_thresh']}  # DEGENERACY_THRES_COND
-  eigenvalue_threshold: {setup['eig_thresh']}
-
-method_params:
-
-  standard_reg:
-    gamma: {setup['std_reg_gamma']}  # STD_REG_GAMMA
-
-  pcg:
-    kappa_target: {setup['kappa_target']}
-    tolerance: 1e-6
-    max_iter: 10
-
-  tsvd:
-    singular_threshold: 120.0
-
-icp_params:
-  XICP_ENOUGH_INFO_THRESHOLD: 300.0      # ignored
-
-test_methods:
-#  "None": [ "NONE_DETE", "NONE_HAND" ]
-{lines}
-{extra_methods}
-{extra}
-""")
-
-
-def dump(runner, cfg):
-    out = subprocess.run([runner, "--dump-config", cfg], capture_output=True, text=True, check=True).stdout
-    kv, methods = {}, []
-    for line in out.splitlines():
-        if line.startswith("method="):
-            methods.append(line[len("method="):].split("|"))
-        elif "=" in line and not line.startswith("="):
-            k, v = line.split("=", 1)
-            kv[k] = v
-    return kv, methods
 
 
 def test_yaml_config_parses_like_the_reference(runner, golden, tmp_path):
@@ -205,11 +104,6 @@ def test_runner_fails_loudly_without_a_device(runner, golden, tmp_path):
     res = subprocess.run([runner, str(cfg)], capture_output=True, text=True)
     assert res.returncode != 0
     assert "no CUDA device" in res.stderr and "Test run failed!" in res.stderr
-
-
-def read_csv(path):
-    with open(path) as f:
-        return list(csv.DictReader(f))
 
 
 @pytest.mark.gpu

@@ -15,25 +15,13 @@ import pytest
 
 import dcreg_oracle as o
 import dcreg_oracle_c as oc
+from harness import ctx, rel_err  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
-
-
 def host_threads():
     return max(1, min(32, len(os.sched_getaffinity(0))))
-
-
-def rel_err(a, b):
-    a = np.asarray(a, dtype=np.float64); b = np.asarray(b, dtype=np.float64)
-    return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-300))
 
 
 # ------------------------------------------------------------------------------------------------

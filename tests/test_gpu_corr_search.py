@@ -7,7 +7,7 @@ nn1_search) and corr.cuh's grid build kernels on a grid and queries written by t
   * the layout twin (grid_layout): cell coordinates floor(float64(v) * (1 / cell)), the points' min / max cell as the
     box, x-fastest cells, ascending original index inside a cell, .w = the index bit-cast to float32, cell_start the
     exclusive scan of the cell counts and pos_of its inverse;
-  * distances: corr::dist2 (FLANN L2_Simple in float32, test_certificate_logic.dist2), ordered by the key
+  * distances: corr::dist2 (FLANN L2_Simple in float32, harness.dist2), ordered by the key
     (bits(d2) << 32) | index: the (distance, then index) rule of the kd-tree the searches replace;
   * the cube of a query: the points whose cell differs from the query's cell by at most K = rings on each axis.
 
@@ -26,131 +26,14 @@ also checks that nothing beyond the rings is nearer than the starting bound r2_u
 (lb >= min(r2_up * 0.9999, d2 of the 7th entry): every contribution to lb comes from a candidate, cell or row rejected
 against the current 7th entry, which only decreases).
 """
-import functools
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-from test_certificate_logic import dist2
-
-F = np.float32
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HARNESS = os.path.join(ROOT, "tools", "test_corr_search.cu")
-MAGIC = 0x43525331
-RADIUS = 0.5
-CELLS = [0.5, 0.3, 0.25, 0.2, 0.125]                 # rings 1, 2, 2, 3, 4
-SENT = 0x7FFFFFFF
-LOOK = F(1.21)                                       # kNnLook: the seeded bound is 1.21 x the 7th squared distance
-WARP_CAP = 64                                        # kWarpKnnCap
-
-
-def rings_of(radius, cell):
-    """search_rings in dcreg_b200.cu"""
-    return int(np.ceil(radius / cell - 1e-9))
-
-
-def r2_up(radius):
-    r2 = radius * radius
-    f = F(r2)
-    return np.nextafter(f, F(np.inf)) if float(f) < r2 else f
-
-
-def keys_of(d2, idx):
-    d2 = np.asarray(d2, F)
-    return (d2.view(np.uint32).astype(np.uint64) << np.uint64(32)) | np.asarray(idx, np.int64).astype(np.uint64)
-
-
-def key_d2(keys):
-    return (np.asarray(keys, np.uint64) >> np.uint64(32)).astype(np.uint32).view(F)
-
-
-def key_idx(keys):
-    return (np.asarray(keys, np.uint64) & np.uint64(0xFFFFFFFF)).astype(np.int64)
-
-
-# ---- the layout twin ----------------------------------------------------------------------------------------------
-class Layout:
-    def __init__(self, pts, cell):
-        self.inv = 1.0 / cell
-        c = np.floor(pts.astype(np.float64) * self.inv).astype(np.int64)
-        self.o = c.min(axis=0)
-        self.n3 = c.max(axis=0) - self.o + 1
-        nx, ny, _ = self.n3
-        lin = ((c[:, 2] - self.o[2]) * ny + (c[:, 1] - self.o[1])) * nx + (c[:, 0] - self.o[0])
-        self.ncells = int(np.prod(self.n3))
-        self.lin = lin
-        self.order = np.argsort(lin, kind="stable")          # by cell, then by index
-        self.cell_start = np.zeros(self.ncells + 1, np.int32)
-        self.cell_start[1:] = np.cumsum(np.bincount(lin, minlength=self.ncells))
-        self.pts4 = np.empty((len(pts), 4), F)
-        self.pts4[:, :3] = pts[self.order]
-        self.pts4[:, 3] = self.order.astype(np.int32).view(F)
-        self.pos_of = np.empty(len(pts), np.int32)
-        self.pos_of[self.order] = np.arange(len(pts), dtype=np.int32)
-
-    def local_cell(self, q):
-        return np.floor(np.asarray(q, F).astype(np.float64) * self.inv).astype(np.int64) - self.o
-
-    def row_ranges(self, q, K):
-        """position range [s, e) in pts4 of the cube cells of every (query, row), rows r = (dz + K) W + (dy + K),
-        W = 2K + 1, as knn_row_range numbers them; (nq, W^2) each, s == e where the row holds nothing"""
-        c = self.local_cell(q)
-        W = 2 * K + 1
-        r = np.arange(W * W)
-        dz, dy = r // W - K, r % W - K
-        nx, ny, nz = self.n3
-        yy, zz = c[:, 1:2] + dy[None], c[:, 2:3] + dz[None]
-        valid = (yy >= 0) & (yy < ny) & (zz >= 0) & (zz < nz)
-        base = np.where(valid, (zz * ny + yy) * nx, 0)
-        xa = np.clip(c[:, 0:1] - K, 0, nx)
-        xb = np.clip(c[:, 0:1] + K + 1, 0, nx)
-        s = np.where(valid, self.cell_start[base + xa], 0)
-        e = np.where(valid, self.cell_start[base + xb], 0)
-        return s, np.maximum(e, s)
-
-
-def expand(s, e):
-    """the ranges [s, e) as flat (range number, position) pairs"""
-    s, e = s.ravel().astype(np.int64), e.ravel().astype(np.int64)
-    ln = e - s
-    owner = np.repeat(np.arange(len(s)), ln)
-    pos = np.arange(int(ln.sum())) - np.repeat(np.cumsum(ln) - ln, ln) + np.repeat(s, ln)
-    return owner, pos
-
-
-def smallest(group, keys, ngroups, k, fill_keys, payload=None, fill_payload=-1):
-    """per group the k smallest keys, ascending, padded with fill_keys[group] (and the payload of each key)"""
-    order = np.lexsort((keys, group))
-    g, ks = group[order], keys[order]
-    rank = np.arange(len(g)) - np.searchsorted(g, np.arange(ngroups))[g]
-    keep = rank < k
-    out = np.repeat(np.asarray(fill_keys, np.uint64).reshape(-1, 1), k, axis=1) if np.ndim(fill_keys) else \
-        np.full((ngroups, k), fill_keys, np.uint64)
-    out[g[keep], rank[keep]] = ks[keep]
-    if payload is None:
-        return out
-    pay = np.full((ngroups, k), fill_payload, np.int64)
-    pay[g[keep], rank[keep]] = payload[order][keep]
-    return out, pay
-
-
-class Reference:
-    """The brute force over every query's cube (exact: the cube's points are gathered from the layout twin)."""
-
-    def __init__(self, pts, L, K, q, B):
-        nq = len(q)
-        self.W2 = (2 * K + 1) ** 2
-        self.rs, self.re = L.row_ranges(q, K)
-        owner, pos = expand(self.rs, self.re)
-        qi = owner // self.W2
-        d2 = dist2(q[qi], L.pts4[pos, :3], pairwise=True)
-        keys = keys_of(d2, L.order[pos])
-        self.knn5 = smallest(qi, keys, nq, 5, keys_of(F(3.0e38), SENT))
-        inb = keys < keys_of(B, SENT)[qi]
-        self.lb_keys, self.lb_pos = smallest(qi[inb], keys[inb], nq, 7, keys_of(B, SENT), pos[inb])
-        self.n_in = np.bincount(qi[d2 <= B[qi]], minlength=nq)       # cube points inside the bound
+from harness import dist2, tool_program
+from search_harness import (CELLS, CLOUDS, RADIUS, SENT, WARP_CAP, F, Layout, Reference, bounds_for, cloud, expand,
+                            first_bad, key_d2, key_idx, make_queries, on_face, r2_up, rings_of, write_input)
 
 
 class Ball:
@@ -185,118 +68,7 @@ def nn1_reference(tree, pts, q):
     return np.array([dist2(q[i:i + 1], pts[np.asarray(x, np.int64)]).min() for i, x in enumerate(lists)], F)
 
 
-# ---- scenes -------------------------------------------------------------------------------------------------------
-def surface(seed=21, n=16_000):
-    rng = np.random.default_rng(seed)
-    xy = rng.uniform(-4.0, 4.0, (n, 2))
-    z = 0.15 * np.sin(1.3 * xy[:, 0]) * np.cos(0.9 * xy[:, 1]) + rng.normal(0, 0.005, n)
-    return np.column_stack([xy, z]).astype(F)
-
-
-def lattice():
-    """the target of test_gpu_parity.py::test_loop_reuse_on_a_lattice_with_duplicates_and_ties: 0.25 m lattices,
-    exact duplicates (floor[::5]) and a 0.05 m patch with ~300 points within 0.5 m of its inside"""
-    g = np.arange(-6, 6, 0.25, dtype=F)
-    X, Y = np.meshgrid(g, g)
-    floor = np.stack([X.ravel(), Y.ravel(), np.zeros(X.size, F)], axis=1)
-    wall = np.stack([X.ravel(), np.full(X.size, 6.0, F), (Y.ravel() + 6.0) * 0.5], axis=1)
-    wall2 = np.stack([np.full(X.size, -6.0, F), X.ravel(), (Y.ravel() + 6.0) * 0.5], axis=1)
-    d = np.arange(-1, 1, 0.05, dtype=F)
-    DX, DY = np.meshgrid(d, d)
-    dense = np.stack([DX.ravel(), DY.ravel(), np.zeros(DX.size, F)], axis=1)
-    return np.concatenate([floor, wall, wall2, dense, floor[::5]]).astype(F)
-
-
-@functools.lru_cache(maxsize=None)
-def cloud(name):
-    if name == "surface":
-        return surface()
-    if name == "lattice":
-        return lattice()
-    if name == "sparse":                 # ~2.5 points within 0.5 m of a point: many lists shorter than 5 or 7
-        return np.random.default_rng(23).uniform(-4.0, 4.0, (2_500, 3)).astype(F)
-    if name == "surface+4096":
-        return (surface().astype(np.float64) + [4096.3, -2047.7, 130.1]).astype(F)
-    if name == "surface+30000":          # inside arena_plan::kCoordLimit at cell 0.125; eps = 2e-6 |q| ~ 0.08 m
-        return (surface().astype(np.float64) + [30000.3, -12000.7, 50.1]).astype(F)
-    raise KeyError(name)
-
-
-CLOUDS = ["surface", "lattice", "sparse", "surface+4096", "surface+30000"]
-PATCH = {"lattice": ((-1.0, -1.0, -0.02), (0.95, 0.95, 0.02))}
-
-
-def on_face(v, inv):
-    """the smallest float32 of the cell that contains v, on each coordinate: a point exactly on the cell's lower faces"""
-    v = np.asarray(v, F)
-    k = np.floor(v.astype(np.float64) * inv)
-    x = (k / inv).astype(F)
-    for _ in range(8):                   # walk to the first float whose cell is k (float cells need not start at k * cell)
-        x = np.where(np.floor(x.astype(np.float64) * inv) < k, np.nextafter(x, F(np.inf)), x)
-        x = np.where(np.floor(np.nextafter(x, F(-np.inf)).astype(np.float64) * inv) >= k, np.nextafter(x, F(-np.inf)), x)
-    return x
-
-
-def make_queries(name, pts, L, K, cell, seed):
-    rng = np.random.default_rng(seed)
-    n = len(pts)
-    pick = lambda m: pts[rng.integers(0, n, m)].astype(np.float64)
-    kinds = []
-
-    def add(kind, q):
-        kinds.append((kind, np.asarray(q, np.float64).astype(F)))
-
-    for s in (0.0, 1e-4, 3e-3, 0.03, 0.15, 0.4):                     # target points plus noise
-        add("noise", pick(50) + rng.normal(0, s, (50, 3)))
-    for naxes in (1, 2, 3):                                           # on faces, edges, corners
-        q = (pick(60) + rng.normal(0, 0.05, (60, 3))).astype(F)
-        snapped = on_face(q, L.inv)
-        for i in range(len(q)):
-            ax = rng.choice(3, naxes, replace=False)
-            q[i, ax] = snapped[i, ax]
-        add("face", q)
-    lo, hi = L.o * cell, (L.o + L.n3) * cell                         # box faces (up to the rounding of the cells)
-    for axis in range(3):                                             # outside the box on each side
-        srt = np.argsort(pts[:, axis])
-        for side, base in ((-1, lo[axis]), (1, hi[axis])):
-            near = srt[:max(20, n // 50)] if side < 0 else srt[-max(20, n // 50):]
-            for off in (0.5 * cell, K * cell - 0.02 * cell, K * cell + 0.02 * cell):
-                q = pts[rng.choice(near, 8)].astype(np.float64)
-                q[:, axis] = base + side * off
-                add("outside", q)
-    ctr = 0.5 * (pts.min(axis=0).astype(np.float64) + pts.max(axis=0))
-    d = rng.normal(0, 1, (30, 3))
-    add("far", ctr + d / np.linalg.norm(d, axis=1, keepdims=True) * rng.uniform(3.0, 30.0, (30, 1)))
-    if name in PATCH:
-        a, b = PATCH[name]
-        add("patch", rng.uniform(a, b, (80, 3)))
-    kind = np.concatenate([[k] * len(q) for k, q in kinds])
-    q = np.concatenate([q for _, q in kinds]).astype(F)
-    return kind, q
-
-
-def bounds_for(tree, pts, q, r2):
-    """the four bounds B of every query: r2_up (first iteration), min(1.21 d7, r2_up) (seeded), d7 exactly (d2 == B),
-    just below d3 (sentinels); d3 / d7 the 3rd / 7th smallest float32 d2 (r2_up where that is farther)"""
-    _, nb = tree.query(q.astype(np.float64), k=24)
-    d = np.sort(dist2(q[:, None, :], pts[nb], pairwise=True), axis=1)
-    d3, d7 = d[:, 2], d[:, 6]
-    b_seed = np.minimum(r2, (d7 * LOOK).astype(F))
-    b_exact = np.where(d7 <= r2, d7, r2)
-    b_below = np.minimum(r2, np.nextafter(d3, F(0)))
-    return [np.full(len(q), r2, F), b_seed.astype(F), b_exact.astype(F), b_below.astype(F)]
-
-
 # ---- the harness --------------------------------------------------------------------------------------------------
-def write_input(path, pts, L, K, r2, q, B, rr):
-    hdr = np.array([MAGIC, len(pts), len(q), len(rr), K, *L.o, *L.n3, 0], np.int64).astype(np.int32)
-    hdr[11] = np.array([r2], F).view(np.int32)[0]
-    with open(path, "wb") as f:
-        for a in (hdr, np.float64(L.inv), np.ascontiguousarray(pts, F), L.pts4, L.pos_of, L.cell_start,
-                  np.ascontiguousarray(q, F), np.ascontiguousarray(B, F), np.ascontiguousarray(rr, np.int32)):
-            f.write(np.asarray(a).tobytes())
-
-
 def read_output(path, nq, nrr):
     buf = open(path, "rb").read()
     at = 0
@@ -323,15 +95,8 @@ def read_output(path, nq, nrr):
 
 @pytest.fixture(scope="module")
 def harness(tmp_path_factory):
-    from dcreg_b200.build import _nvcc
-    from test_host_la import device_program_flags
-    exe = tmp_path_factory.mktemp("corr_search") / "test_corr_search"
-    subprocess.run([_nvcc()] + device_program_flags() + ["-o", str(exe), HARNESS], check=True, capture_output=True, text=True)
-    return exe
-
-
-def first_bad(mask):
-    return int(np.flatnonzero(mask)[0]) if mask.any() else -1
+    return tool_program(tmp_path_factory.mktemp("corr_search"), "test_corr_search.cu", compiler="device",
+                        skip_missing=False)
 
 
 @pytest.mark.gpu
@@ -463,14 +228,7 @@ def test_searches_match_brute_force(harness, tmp_path, name, cell):
 # ---- CPU checks of the reference itself ----------------------------------------------------------------------------
 def test_harness_compiles_for_sm90a(tmp_path):
     """tools/test_corr_search.cu builds with the library's flags (no GPU needed to compile)."""
-    from dcreg_b200.build import _nvcc
-    from test_host_la import device_program_flags
-    try:
-        nvcc = _nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc not available")
-    res = subprocess.run([nvcc] + device_program_flags() + ["-o", str(tmp_path / "h"), HARNESS], capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
+    tool_program(tmp_path, "test_corr_search.cu", compiler="device")
 
 
 @pytest.mark.parametrize("cell", CELLS)

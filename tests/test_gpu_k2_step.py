@@ -18,8 +18,8 @@ import math
 import numpy as np
 import pytest
 
-import dcreg_oracle as o
 import dcreg_oracle_mp as m
+from harness import METHODS, ctx, designed, run_designed  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -27,17 +27,10 @@ DX_TOL = 64.0          # rec.dx vs the reference: |dx - dx_ref|_max <= DX_TOL * 
 WORST = {}             # label -> [records, clear, checked against mp, worst dx error in units of cond(H) eps]
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
-
-
 def ours(**over):
     from dcreg_b200 import default_params
-    kw = dict(detection="SCHUR_CONDITION_NUMBER", handling="PRECONDITIONED_CG", kappa_target=10.0)
+    det, hand = METHODS["Ours"]
+    kw = dict(detection=det, handling=hand, kappa_target=10.0)
     kw.update(over)
     return default_params(**kw)
 
@@ -211,64 +204,6 @@ def test_odometry(ctx):
 # ------------------------------------------------------------------------------------------------------------------
 # designed systems through the host-plane loop (K1 + k2_step_kernel)
 # ------------------------------------------------------------------------------------------------------------------
-def designed(kind, rng_seed=5, n=900, tilt=0.0):
-    """Source points and world planes whose normal equations do not depend on the pose (to rounding): each point keeps
-    its normal (rotated with the pose) and its residual rho.  Returns (points f32, normals, rho)."""
-    rng = np.random.default_rng(rng_seed)
-    if kind == "generic":                       # anisotropic translation and rotation blocks, all ratios distinct
-        p = rng.uniform(-5.0, 5.0, (n, 3)) * np.array([1.0, 0.6, 0.3])
-        u = rng.standard_normal((n, 3)) * np.array([1.0, 0.35, 0.12])
-        nrm = u / np.linalg.norm(u, axis=1, keepdims=True)
-        rho = rng.uniform(-2e-3, 2e-3, n)
-    elif kind in ("box2", "box3"):              # axis-aligned faces of a symmetric box: equal Schur eigenvalues
-        # every face point comes with its reflections in the face's two other coordinates, so the coupling H_Rt and
-        # the off-diagonal entries vanish; box3: the same count per axis (H_tt = c I), box2: fewer on the z faces
-        per = n // 24
-        ext = np.array([4.0, 4.0, 0.5])
-        p, nrm = [], []
-        for ax in range(3):
-            cnt = per if kind == "box3" or ax < 2 else max(1, per // 20)
-            for sgn in (-1.0, 1.0):
-                q = rng.uniform(-1.0, 1.0, (cnt, 3)) * ext
-                q[:, ax] = sgn * ext[ax]
-                for f in ((1, 1), (1, -1), (-1, 1), (-1, -1)):
-                    s = np.ones(3); s[[a for a in range(3) if a != ax]] = f
-                    p.append(q * s); nrm.append(np.tile(np.eye(3)[ax] * sgn, (cnt, 1)))
-        p, nrm = np.concatenate(p), np.concatenate(nrm)
-        rho = 1e-3 * rng.choice([-1.0, 1.0], len(p))                    # |rho| equal: every point has the same weight
-    elif kind in ("rank2", "rank2_rot", "tilt"):   # translation block of rank 2 (+ tilt out of the plane)
-        p = rng.uniform(-5.0, 5.0, (n, 3))
-        ang = rng.uniform(0.0, 2.0 * math.pi, n)
-        nrm = np.stack([np.cos(ang), np.sin(ang), np.zeros(n)], axis=1)
-        if kind == "tilt":
-            nrm[:, 2] = tilt * np.where(np.arange(n) % 2 == 0, 1.0, -1.0)
-            nrm /= np.linalg.norm(nrm, axis=1, keepdims=True)
-        if kind == "rank2_rot":
-            Rg = o.pose6d_to_matrix(0, 0, 0, 0.7, -0.4, 1.1)[:3, :3]
-            nrm = nrm @ Rg.T
-        rho = rng.uniform(-2e-3, 2e-3, n)
-    else:
-        raise ValueError(kind)
-    return p.astype(np.float32), nrm, rho
-
-
-def run_designed(ctx, sysd, prm, T0=None):
-    p, nrm, rho = sysd
-    p64 = p.astype(np.float64)
-
-    def plane_fn(T):
-        R, t = T[:3, :3], T[:3, 3]
-        q = (p64 @ R.T + t).astype(np.float32).astype(np.float64)          # fl32(R p + t), as K1 forms it
-        nw = nrm @ R.T
-        planes = np.empty((len(p), 4))
-        planes[:, :3] = nw
-        planes[:, 3] = rho - np.einsum("kj,kj->k", nw, q)
-        return planes, len(p)
-
-    ctx.set_source(p)
-    return ctx.icp_run_host_planes(prm, np.eye(4) if T0 is None else T0, plane_fn)
-
-
 def sweep(ctx, sysd, label, prms, iters, mp_at):
     out = []
     for prm in prms:

@@ -4,52 +4,19 @@ Contract 1: lane b returns byte for byte what the same call returns for lane b w
 (T_out, T_prior, iterations, converged, status, cov, n_points, metrics, search_radius and every log record with
 iter_time_ms zeroed).  Contract 2: identical entries are the call with one params, launches included.
 """
-import os
-
 import numpy as np
 import pytest
 
+from harness import METHODS, RADIUS, ctx, log_bytes, params, read_csv, write_config  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-RADIUS = 0.5
 CELL = 0.5
 LENS = (1, 7, 12)
-METHODS = {                       # the six methods the CLI's SO(3) path recognises (icp_test_runner's test_methods)
-    "Ours": ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG"),
-    "NONE": ("NONE_DETE", "NONE_HAND"),
-    "ME-SR": ("FULL_EVD_MIN_EIGENVALUE", "SOLUTION_REMAPPING"),
-    "FCN-SR": ("FULL_SVD_CONDITION", "SOLUTION_REMAPPING"),
-    "ME-TSVD": ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD"),
-    "ME-TReg": ("FULL_EVD_MIN_EIGENVALUE", "STANDARD_REGULARIZATION"),
-}
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
-
-
-def prm(method="Ours", radius=RADIUS, **over):
-    from dcreg_b200 import default_params
-    det, hand = METHODS[method]
-    kw = dict(search_radius=radius, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
 
 
 def kappa(k, method="Ours", radius=RADIUS):
-    return prm(method, radius, cond_thresh=k, kappa_target=k)
-
-
-def log_bytes(rec):
-    r = type(rec).from_buffer_copy(bytes(rec))
-    r.iter_time_ms = 0.0
-    return bytes(r)
+    return params(method, radius, cond_thresh=k, kappa_target=k)
 
 
 def assert_same(a, b, where):
@@ -81,19 +48,18 @@ def lanes_vs_uniform(run, entries, lane_of=None):
 
 # ---- the cylinder of the G2 setup: batches of trials and scans ----------------------------------------------------
 @pytest.fixture(scope="module")
-def cylinder():
-    from dcreg_b200.scenes import g2_initial_pose, load_pcd_xyz, trial_poses
-    pts = load_pcd_xyz(os.path.join(ROOT, "tests", "golden", "cylinder_7562.pcd"))
-    T = g2_initial_pose() @ trial_poses(12, seed=5, max_trans=0.3, max_rot_deg=2.0)
-    return pts, T
+def g2_trials(cylinder):
+    """the shipped cylinder and 12 trial poses about the G2 setup's initial pose"""
+    from dcreg_b200.scenes import g2_initial_pose, trial_poses
+    return cylinder, g2_initial_pose() @ trial_poses(12, seed=5, max_trans=0.3, max_rot_deg=2.0)
 
 
 def g2(method, **over):
-    return prm(method, radius=1.0, use_weight_derivative=1, **over)
+    return params(method, radius=1.0, use_weight_derivative=1, **over)
 
 
-def test_batch_mixes_all_six_methods(ctx, cylinder):
-    pts, T = cylinder
+def test_batch_mixes_all_six_methods(ctx, g2_trials):
+    pts, T = g2_trials
     ctx.set_source(pts)
     ctx.set_target(pts, 1.0)
     names = list(METHODS)
@@ -101,9 +67,9 @@ def test_batch_mixes_all_six_methods(ctx, cylinder):
     lanes_vs_uniform(lambda p: ctx.icp_run_batch(p, T, want_log=True), entries)
 
 
-def test_identical_entries_are_the_uniform_call(ctx, cylinder):
+def test_identical_entries_are_the_uniform_call(ctx, g2_trials):
     """Contract 2: the same bytes and the same launch count, for "Ours" (folded) and a baseline (K2)"""
-    pts, T = cylinder
+    pts, T = g2_trials
     ctx.set_source(pts)
     ctx.set_target(pts, 1.0)
     for method in ("Ours", "ME-SR"):
@@ -118,11 +84,11 @@ def test_identical_entries_are_the_uniform_call(ctx, cylinder):
             assert_same(a, b, (method, k))
 
 
-def test_swapped_mixes_at_one_shape(ctx, cylinder):
+def test_swapped_mixes_at_one_shape(ctx, g2_trials):
     """Calls of one shape whose lanes are all "Ours" (no K2 launch) and then mixed (a K2 launch after every iteration
     kernel, at the same kernel arguments), with swapped mixes: each equals its uniform references (the loop's graph key
     covers whether a K2 launch follows, so a mixed call never replays the all-"Ours" call's graph)"""
-    pts, T = cylinder
+    pts, T = g2_trials
     ctx.set_source(pts)
     ctx.set_target(pts, 1.0)
     a = [g2("Ours" if k % 2 else "ME-TSVD") for k in range(len(T))]
@@ -139,7 +105,7 @@ def test_scans(ctx):
     from dcreg_b200.scenes import make_parking_frames
     scans, _, T_init, tgt = make_parking_frames(6, n_map=200_000, n_scan=4_000)
     ctx.set_target(tgt, RADIUS)
-    entries = [prm(m) for m in ("Ours", "ME-TSVD", "Ours", "FCN-SR", "NONE", "ME-TReg")]
+    entries = [params(m) for m in ("Ours", "ME-TSVD", "Ours", "FCN-SR", "NONE", "ME-TReg")]
     entries[2] = kappa(100.0)
     lanes_vs_uniform(lambda p: ctx.icp_run_scans(p, scans, T_init, want_log=True, want_cov=True), entries)
 
@@ -147,7 +113,7 @@ def test_scans(ctx):
 def test_pairs_with_metrics(ctx):
     from dcreg_b200.scenes import make_parking_pairs
     src, tgt, _, T_init = make_parking_pairs(5, n_map=200_000, n_scan=3_000)
-    entries = [prm("Ours"), prm("ME-SR"), kappa(3.0), prm("ME-TSVD"), kappa(300.0)]
+    entries = [params("Ours"), params("ME-SR"), kappa(3.0), params("ME-TSVD"), kappa(300.0)]
     lanes_vs_uniform(lambda p: ctx.icp_run_pairs(p, src, tgt, T_init, want_log=True, want_cov=True,
                                                  metrics_threshold=0.1), entries)
 
@@ -166,24 +132,27 @@ def frame_seq(seqs):
     return [s for s, q in enumerate(seqs) for _ in q]
 
 
-MIXES = {"kappa": [kappa(2.0), kappa(30.0), kappa(1000.0)],
-         "methods": [prm("ME-TSVD"), kappa(50.0), prm("FCN-SR")]}
+@pytest.fixture(scope="module")
+def mixes():
+    """per-lane entries of the sequence, odometry and session tests"""
+    return {"kappa": [kappa(2.0), kappa(30.0), kappa(1000.0)],
+            "methods": [params("ME-TSVD"), kappa(50.0), params("FCN-SR")]}
 
 
-def test_sequences(ctx, odo):
+def test_sequences(ctx, odo, mixes):
     seqs, T_init, deltas, tgt = odo
     ctx.set_target(tgt, RADIUS)
-    for entries in MIXES.values():
+    for entries in mixes.values():
         lanes_vs_uniform(lambda p: ctx.icp_run_sequences(p, seqs, T_init, deltas, want_log=True, want_cov=True), entries,
                          frame_seq(seqs))
 
 
-@pytest.mark.parametrize("mix", list(MIXES))
+@pytest.mark.parametrize("mix", ["kappa", "methods"])
 @pytest.mark.parametrize("kind", ["window", "voxel_map", "adaptive"])
-def test_odometry(ctx, odo, kind, mix):
+def test_odometry(ctx, odo, mixes, kind, mix):
     from dcreg_b200.api import AdaptiveThreshold
     seqs, T_init, deltas, _ = odo
-    entries = MIXES[mix]
+    entries = mixes[mix]
     if kind == "window":
         def run(p):
             return ctx.icp_run_odometry(p, seqs, T_init, deltas, map_frames=3, cell_size=CELL, want_log=True,
@@ -219,9 +188,9 @@ def pushed(ctx, sess, seqs, deltas, between=None):
     return [r for q in got for r in q]
 
 
-def test_session_ragged_pushes_equal_one_call(ctx, odo):
+def test_session_ragged_pushes_equal_one_call(ctx, odo, mixes):
     seqs, T_init, deltas, _ = odo
-    entries = MIXES["methods"]
+    entries = mixes["methods"]
     ref = ctx.icp_run_odometry(entries, seqs, T_init, deltas, map_frames=3, cell_size=CELL, want_log=True)
     with ctx.odometry_session(entries, 3, T_init, map_frames=3, cell_size=CELL) as sess:
         flat = pushed(ctx, sess, seqs, deltas)
@@ -229,11 +198,11 @@ def test_session_ragged_pushes_equal_one_call(ctx, odo):
         assert_same(a, b, k)
 
 
-def test_session_keeps_its_setting(ctx, odo):
+def test_session_keeps_its_setting(ctx, odo, mixes):
     """A session opened with the setting on keeps its per-lane entries when the setting goes off and on again between
     pushes, and one opened with it off keeps its one params when it goes on (the library reads no array at a push)"""
     seqs, T_init, deltas, _ = odo
-    entries = MIXES["kappa"]
+    entries = mixes["kappa"]
     ref = ctx.icp_run_odometry(entries, seqs, T_init, deltas, map_frames=3, cell_size=CELL, want_log=True)
     ctx.set_lane_params(True)
     try:
@@ -259,9 +228,9 @@ COMMON = {"search_radius": 0.6, "max_iterations": 29, "fixed_iterations": 1, "us
           "plane_thickness": 0.3, "weight_slope": 0.8, "weight_gate": 0.2, "min_normal_norm": 1e-5}
 
 
-def test_common_fields_refused(ctx, cylinder, odo):
+def test_common_fields_refused(ctx, g2_trials, odo):
     from dcreg_b200 import DcregError
-    pts, T = cylinder
+    pts, T = g2_trials
     seqs, T_init, deltas, _ = odo
     ctx.set_source(pts)
     ctx.set_target(pts, 1.0)
@@ -273,13 +242,13 @@ def test_common_fields_refused(ctx, cylinder, odo):
             ctx.icp_run_batch(entries, T[:3])
         assert "icp_run_batch: entry 2: " + field in str(e.value)
         with pytest.raises(DcregError) as e:
-            ctx.odometry_session([prm(), prm(), prm(**{field: value})], 3, T_init, map_frames=3, cell_size=CELL)
+            ctx.odometry_session([params(), params(), params(**{field: value})], 3, T_init, map_frames=3, cell_size=CELL)
         assert "entry 2: " + field in str(e.value)
     assert not ctx._lane_params
     for a, b in zip(ctx.icp_run_batch(g2("Ours"), T[:3]), ref):              # the context is still usable
         assert_same(a, b, "after")
-    with ctx.odometry_session([prm(), kappa(3.0), prm()], 3, T_init, map_frames=3, cell_size=CELL) as sess:
-        bad = [prm(), prm(), prm(weight_gate=0.3)]
+    with ctx.odometry_session([params(), kappa(3.0), params()], 3, T_init, map_frames=3, cell_size=CELL) as sess:
+        bad = [params(), params(), params(weight_gate=0.3)]
         with pytest.raises(DcregError):
             ctx.icp_run_odometry(bad, seqs, T_init, deltas, map_frames=3, cell_size=CELL)
         assert len(sess.push([[seqs[0][0]], [], []])[0]) == 1                  # the session too
@@ -290,12 +259,12 @@ def test_common_fields_refused(ctx, cylinder, odo):
     assert "enable must be 0 or 1" in ctx.lib.dcreg_last_error(h).decode()
 
 
-def test_single_runs_read_entry_zero(ctx, cylinder):
+def test_single_runs_read_entry_zero(ctx, g2_trials):
     """With the setting on, dcreg_icp_run, _enqueue and dcreg_analyze_and_solve given an array whose later entries
     differ (another method, an invalid iteration count) return what they return for entry 0 alone"""
     import ctypes as C
     from dcreg_b200.api import Analysis, IcpParams, IterLog
-    pts, T = cylinder
+    pts, T = g2_trials
     ctx.set_source(pts)
     ctx.set_target(pts, 1.0)
     lib, h = ctx.lib, ctx._h
@@ -338,7 +307,6 @@ def test_cli_one_call_csvs(golden, tmp_path):
     so its FP64 grouping does), and a summary whose Trials/s counts every lane of the one call"""
     import subprocess
     from dcreg_b200 import build as b
-    from test_cli_runner import read_csv, write_config
     runner = b.build_runner()
     names = ["Ours", "ME-SR", "FCN-SR", "ME-TSVD", "ME-TReg"]
     mc = "monte_carlo:\n  trials: 40\n  seed: 13\n  max_trans_m: 0.6\n  max_rot_deg: 2.0\n"

@@ -16,8 +16,6 @@ reference against the plain oracle (find_correspondences + build_rows) on tie-fr
 sensitivity to a dropped, doubled, stale or foreign slot row.
 """
 import math
-import os
-import shutil
 import subprocess
 
 import numpy as np
@@ -26,8 +24,8 @@ from scipy.spatial import cKDTree
 
 import dcreg_oracle as o
 import dcreg_oracle_rows as rows
+from harness import METHODS, ctx, init_T, ties_lattice, tool_program  # noqa: F401
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F = np.float32
 STATS = {}             # label -> [records, slots, band counts {reason: n}, worst error / allowance]
 
@@ -109,12 +107,7 @@ def qr_systems(n=48_000, seed=3):
 
 
 def test_qr_restatement_is_bit_identical_to_the_host_build(tmp_path):
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        pytest.skip("nvcc not available")
-    exe = tmp_path / "qr53_host"
-    subprocess.run([nvcc, "-O2", "-o", str(exe), os.path.join(ROOT, "tools", "qr53_host.cu")], check=True,
-                   capture_output=True, text=True)
+    exe = tool_program(tmp_path, "qr53_host.cu", compiler="nvcc")
     P = qr_systems()
     P.astype(np.float64).tofile(tmp_path / "a.bin")
     res = subprocess.run([str(exe), str(tmp_path / "a.bin"), str(tmp_path / "x.bin")], capture_output=True, text=True)
@@ -223,17 +216,10 @@ def test_allowance_catches_a_wrong_slot_row(cylinder):
 # ------------------------------------------------------------------------------------------------------------------
 # GPU: the loop's records at every entry point
 # ------------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
-
-
 def ours(**over):
     from dcreg_b200 import default_params
-    kw = dict(detection="SCHUR_CONDITION_NUMBER", handling="PRECONDITIONED_CG", kappa_target=10.0)
+    det, hand = METHODS["Ours"]
+    kw = dict(detection=det, handling=hand, kappa_target=10.0)
     kw.update(over)
     return default_params(**kw)
 
@@ -257,7 +243,6 @@ def test_c2_records(ctx, use_wd):
 
 @pytest.mark.gpu
 def test_shipped_cylinder_g1_g2(ctx, golden, cylinder):
-    from test_oracle_golden import init_T
     tree = cKDTree(cylinder.astype(np.float64))
     ctx.set_target(cylinder, 1.0)
     ctx.set_source(cylinder)
@@ -296,8 +281,7 @@ def test_ragged_sizes_cells_and_sparse_index(ctx, cylinder):
 
 @pytest.mark.gpu
 def test_lattice_with_duplicates_and_ties(ctx):
-    from test_gpu_corr_search import lattice
-    tgt = lattice()
+    tgt = ties_lattice()
     rng = np.random.default_rng(5)
     src = tgt[rng.permutation(len(tgt))[:7001]].copy()
     T0 = o.pose6d_to_matrix(0.06, -0.05, 0.04, math.radians(0.2), math.radians(-0.1), math.radians(0.4))

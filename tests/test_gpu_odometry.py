@@ -14,8 +14,9 @@ import pytest
 
 import dcreg_oracle as o
 
-from odom_harness import (CELL, RADIUS, assert_anchor, assert_priors, assert_same_run, ctx, parking,  # noqa: F401
-                          params, raw_odometry, reconstruct, split, window_map)
+from harness import RADIUS, assert_same_run, ctx, params  # noqa: F401
+from odom_harness import (CELL, assert_anchor, assert_priors, parking, raw_odometry, reconstruct, split,  # noqa: F401
+                          window_map)
 
 pytestmark = pytest.mark.gpu
 

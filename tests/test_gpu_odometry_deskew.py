@@ -7,7 +7,8 @@ import pytest
 
 import dcreg_oracle as o
 
-from odom_harness import CELL, RADIUS, ctx, params, pushed, result_bytes, sweeps  # noqa: F401
+from harness import RADIUS, ctx, params  # noqa: F401
+from odom_harness import CELL, pushed, result_bytes, sweeps  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 

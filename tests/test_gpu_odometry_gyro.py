@@ -11,8 +11,8 @@ import math
 import numpy as np
 import pytest
 
-from odom_harness import (CELL, assert_anchor, assert_same_flat, assert_same_run, ctx, params, raw_odometry,  # noqa: F401
-                          split, window_map)
+from harness import assert_same_run, ctx, params  # noqa: F401
+from odom_harness import CELL, assert_anchor, assert_same_flat, raw_odometry, split, window_map  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 

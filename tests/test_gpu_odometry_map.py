@@ -10,9 +10,10 @@ import math
 import numpy as np
 import pytest
 
-from odom_harness import (CELL, RADIUS, RAGGED, assert_anchor, assert_priors, assert_same, assert_same_flat,  # noqa: F401
-                          assert_same_run, ctx, log_bytes, map_call, odo, one_per_push, params, pushed, raw_odometry,
-                          raw_push, seq_results, split, sweeps, twin_maps, window_call)
+from harness import RADIUS, assert_same_run, ctx, log_bytes, params  # noqa: F401
+from odom_harness import (CELL, RAGGED, assert_anchor, assert_priors, assert_same, assert_same_flat,  # noqa: F401
+                          map_call, odo, one_per_push, pushed, raw_odometry, raw_push, seq_results, split, sweeps,
+                          twin_maps, window_call)
 
 pytestmark = pytest.mark.gpu
 

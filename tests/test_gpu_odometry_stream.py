@@ -6,8 +6,8 @@ T_out, T_prior, status, iterations, converged, n_points, cov, and every log reco
 import numpy as np
 import pytest
 
-from odom_harness import (CELL, RADIUS, RAGGED, assert_same, ctx, log_bytes, odo, one_per_push, params,  # noqa: F401
-                          pushed, raw_push, split)
+from harness import RADIUS, ctx, log_bytes, params  # noqa: F401
+from odom_harness import CELL, RAGGED, assert_same, odo, one_per_push, pushed, raw_push, split  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 

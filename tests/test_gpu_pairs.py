@@ -12,18 +12,9 @@ import numpy as np
 import pytest
 
 import dcreg_oracle as o
+from harness import RADIUS, assert_same_run, ctx, params, rel_err  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-RADIUS = 0.5
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
 
 
 @pytest.fixture(scope="module")
@@ -45,34 +36,6 @@ def scene():
     return src, cut, T_true, T_init
 
 
-def c3_params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
-
-
-def rel_err(a, b):
-    a = np.asarray(a, dtype=np.float64); b = np.asarray(b, dtype=np.float64)
-    return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-300))
-
-
-def assert_same_run(b, single, logs=True):
-    assert (b.status, b.iterations, b.converged) == (single.status, single.iterations, single.converged)
-    assert o.se3_log_distance(single.T, b.T) < 1e-8
-    if not logs:
-        return
-    assert len(b.logs) == len(single.logs)
-    for x, y in zip(b.logs, single.logs):
-        assert x.n_effective == y.n_effective and x.n_corr_pt == y.n_corr_pt
-        assert list(x.analysis.degenerate_mask) == list(y.analysis.degenerate_mask)
-        if x.status == 0:
-            assert rel_err(np.array(x.H27), np.array(y.H27)) < 1e-8
-            assert np.max(np.abs(np.array(x.dx) - np.array(y.dx))) < 1e-8
-
-
 def single_run(ctx, prm, s, t, T, cell=RADIUS, **kw):
     ctx.set_target(t, cell)
     ctx.set_source(s)
@@ -91,7 +54,7 @@ def test_pairs_equal_single_runs(ctx, scene, method, cell):
     cell = RADIUS / 2: the targets' grids searched over 2 rings of cells."""
     src, tgt, _, T_init = scene
     assert min(len(t) for t in tgt) < 5_000 and max(len(t) for t in tgt) > 80_000
-    prm = c3_params(method)
+    prm = params(method)
     batch = ctx.icp_run_pairs(prm, src, tgt, T_init, cell_size=cell, want_log=True)
     assert len(batch) == len(src)
     n_conv = 0
@@ -105,7 +68,7 @@ def test_pairs_shared_map_bit_identical_to_scans(ctx):
     """Every target is the same map: bit for bit what icp_run_scans gives after set_target(map)."""
     from dcreg_b200.scenes import make_parking_frames
     frames, _, T_init, park_map = make_parking_frames(6, seed=57, n_map=200_000, n_scan=3_000)
-    prm = c3_params()
+    prm = params()
     pairs = ctx.icp_run_pairs(prm, frames, [park_map] * len(frames), T_init, want_log=True)
     ctx.set_target(park_map, RADIUS)
     scans = ctx.icp_run_scans(prm, frames, T_init, want_log=True)
@@ -118,7 +81,7 @@ def test_pairs_match_oracle(ctx, scene):
     import dcreg_oracle_c as oc
     src, tgt, _, T_init = scene
     pick = [0, 3, 5, 7, 9, 14]                              # 6 pairs of 4 k - 8 k source points
-    batch = ctx.icp_run_pairs(c3_params(), [src[k] for k in pick], [tgt[k] for k in pick], T_init[pick], want_log=True)
+    batch = ctx.icp_run_pairs(params(), [src[k] for k in pick], [tgt[k] for k in pick], T_init[pick], want_log=True)
     cp = oc.make_params(search_radius=RADIUS, max_iterations=30, conv_rot=1e-5, conv_trans=1e-3, kappa_target=10.0)
     for b, k in zip(batch, pick):
         sc = oc.Scene(src[k], tgt[k])
@@ -138,7 +101,7 @@ def test_pairs_reproducible_and_context_intact(ctx, scene, cylinder):
     from dcreg_b200.scenes import g2_initial_pose, make_parking_frames
     src, tgt, _, T_init = scene
     frames, _, Tf, park_map = make_parking_frames(4, seed=58, n_map=200_000, n_scan=3_000)
-    prm = c3_params()
+    prm = params()
     ctx.set_target(park_map, RADIUS)
     ctx.set_source(frames[0])
     one = ctx.icp_run(prm, Tf[0])
@@ -157,7 +120,7 @@ def test_pairs_reproducible_and_context_intact(ctx, scene, cylinder):
     assert all(same_bits(x, y) for x, y in zip(sc1, sc2))
     # a smaller call after the large one: the grown arenas do not leak into it
     small = ([cylinder[:3000], cylinder[3000:]], [cylinder, cylinder[::2]], [g2_initial_pose()] * 2)
-    p1 = c3_params(search_radius=1.0)
+    p1 = params(search_radius=1.0)
     r1 = ctx.icp_run_pairs(p1, *small, want_log=True, metrics_threshold=1.0)
     with Context(0) as fresh:
         r2 = fresh.icp_run_pairs(p1, *small, want_log=True, metrics_threshold=1.0)
@@ -170,7 +133,7 @@ def test_pairs_mixed_outcomes(ctx, scene):
     returns it; its neighbours still equal their single runs."""
     from dcreg_b200 import api
     src, tgt, _, T_init = scene
-    prm = c3_params()
+    prm = params()
     Ts = T_init[:5].copy()
     Ts[2] = o.pose6d_to_matrix(500.0, 0, 0, 0, 0, 0)
     batch = ctx.icp_run_pairs(prm, src[:5], tgt[:5], Ts, want_log=True)
@@ -182,7 +145,7 @@ def test_pairs_mixed_outcomes(ctx, scene):
 
 def test_pairs_covariance(ctx, scene):
     src, tgt, _, T_init = scene
-    prm = c3_params()
+    prm = params()
     Ts = T_init[:6].copy()
     Ts[4] = o.pose6d_to_matrix(500.0, 0, 0, 0, 0, 0)        # not converged: 1e6 I
     batch = ctx.icp_run_pairs(prm, src[:6], tgt[:6], Ts, want_cov=True)
@@ -200,7 +163,7 @@ def test_pairs_covariance(ctx, scene):
 @pytest.mark.parametrize("threshold", [0.5, 0.05])
 def test_pairs_metrics(ctx, scene, threshold):
     src, tgt, _, T_init = scene
-    batch = ctx.icp_run_pairs(c3_params(), src, tgt, T_init, metrics_threshold=threshold)
+    batch = ctx.icp_run_pairs(params(), src, tgt, T_init, metrics_threshold=threshold)
     for k, b in enumerate(batch):
         ctx.set_target(tgt[k], RADIUS)
         ctx.set_source(src[k])
@@ -212,7 +175,7 @@ def test_pairs_metrics(ctx, scene, threshold):
 
 def test_pairs_launch_count_does_not_grow(ctx, scene):
     src, tgt, _, T_init = scene
-    prm = c3_params(max_iterations=3, fixed_iterations=1)
+    prm = params(max_iterations=3, fixed_iterations=1)
     deltas = []
     for n in (2, 16, 2):
         l0 = ctx.launch_count
@@ -224,7 +187,7 @@ def test_pairs_launch_count_does_not_grow(ctx, scene):
 def test_pairs_bad_arguments(ctx, scene, cylinder):
     from dcreg_b200 import api
     src, tgt, _, T_init = scene
-    prm = c3_params()
+    prm = params()
     lib, h = ctx.lib, ctx._h
     xs = np.ascontiguousarray(np.concatenate(src[:3]), dtype=np.float32)
     xt = np.ascontiguousarray(np.concatenate(tgt[:3]), dtype=np.float32)
@@ -250,7 +213,7 @@ def test_pairs_bad_arguments(ctx, scene, cylinder):
            dict(to=np.array([2, 10, 20, 30], np.int64)), dict(to=np.array([0, 100, 50, len(xt)], np.int64)),
            dict(to=np.array([0, 100, 100, len(xt)], np.int64)),
            dict(n=1, so=np.array([0, huge], np.int64)), dict(n=1, to=np.array([0, huge], np.int64)),   # int32 totals
-           dict(params=c3_params(weight_gate=1.5)), dict(params=c3_params(max_iterations=-1))]      # check_run_args
+           dict(params=params(weight_gate=1.5)), dict(params=params(max_iterations=-1))]      # check_run_args
     for kw in bad:
         assert call(**kw) == api.BAD_ARG, kw
         assert lib.dcreg_last_error(h).decode(), kw

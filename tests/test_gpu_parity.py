@@ -11,17 +11,9 @@ import numpy as np
 import pytest
 
 import dcreg_oracle as o
-from test_oracle_golden import METHODS, init_T, params_from
+from harness import METHODS, ctx, init_T, params_from  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
 
 
 @pytest.fixture(scope="module")

@@ -11,18 +11,9 @@ import numpy as np
 import pytest
 
 import dcreg_oracle as o
+from harness import RADIUS, assert_same_run, ctx, params, rel_err  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-RADIUS = 0.5
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
 
 
 @pytest.fixture(scope="module")
@@ -37,39 +28,11 @@ def scene():
     return cut, T_true, T_init, tgt
 
 
-def c3_params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
-
-
-def rel_err(a, b):
-    a = np.asarray(a, dtype=np.float64); b = np.asarray(b, dtype=np.float64)
-    return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-300))
-
-
-def assert_same_run(b, single, logs=True):
-    assert (b.status, b.iterations, b.converged) == (single.status, single.iterations, single.converged)
-    assert o.se3_log_distance(single.T, b.T) < 1e-8
-    if not logs:
-        return
-    assert len(b.logs) == len(single.logs)
-    for x, y in zip(b.logs, single.logs):
-        assert x.n_effective == y.n_effective and x.n_corr_pt == y.n_corr_pt
-        assert list(x.analysis.degenerate_mask) == list(y.analysis.degenerate_mask)
-        if x.status == 0:
-            assert rel_err(np.array(x.H27), np.array(y.H27)) < 1e-8
-            assert np.max(np.abs(np.array(x.dx) - np.array(y.dx))) < 1e-8
-
-
 @pytest.mark.parametrize("method", ["Ours", "ME-TSVD"])
 def test_scans_equal_single_runs(ctx, scene, method):
     """Ours folds the solve step into the loop kernel; ME-TSVD takes the separate solve kernel (k2_step_kernel)."""
     frames, _, T_init, tgt = scene
-    prm = c3_params(method)
+    prm = params(method)
     ctx.set_target(tgt, RADIUS)
     batch = ctx.icp_run_scans(prm, frames, T_init, want_log=True)
     assert len(batch) == len(frames)
@@ -87,7 +50,7 @@ def test_scans_match_oracle(ctx, scene):
     frames, _, T_init, tgt = scene
     pick = [0, 2, 3, 5, 7, 9, 10, 14]                       # 8 frames of 4 k - 8 k points
     ctx.set_target(tgt, RADIUS)
-    batch = ctx.icp_run_scans(c3_params(), [frames[k] for k in pick], T_init[pick], want_log=True)
+    batch = ctx.icp_run_scans(params(), [frames[k] for k in pick], T_init[pick], want_log=True)
     cp = oc.make_params(search_radius=RADIUS, max_iterations=30, conv_rot=1e-5, conv_trans=1e-3, kappa_target=10.0)
     for b, k in zip(batch, pick):
         sc = oc.Scene(frames[k], tgt)
@@ -104,7 +67,7 @@ def test_scans_match_oracle(ctx, scene):
 
 def test_scans_reproducible_and_context_intact(ctx, scene, cylinder):
     frames, _, T_init, tgt = scene
-    prm = c3_params()
+    prm = params()
     ctx.set_target(tgt, RADIUS)
     ctx.set_source(frames[0])
     one = ctx.icp_run(prm, T_init[0])
@@ -125,9 +88,9 @@ def test_scans_reproducible_and_context_intact(ctx, scene, cylinder):
     ctx.set_target(cylinder, 1.0)
     ctx.set_source(cylinder)
     from dcreg_b200.scenes import g2_initial_pose
-    r1 = ctx.icp_run(c3_params(search_radius=1.0), g2_initial_pose())
-    ctx.icp_run_scans(c3_params(search_radius=1.0), [cylinder[:3000], cylinder[3000:]], [g2_initial_pose()] * 2)
-    r2 = ctx.icp_run(c3_params(search_radius=1.0), g2_initial_pose())
+    r1 = ctx.icp_run(params(search_radius=1.0), g2_initial_pose())
+    ctx.icp_run_scans(params(search_radius=1.0), [cylinder[:3000], cylinder[3000:]], [g2_initial_pose()] * 2)
+    r2 = ctx.icp_run(params(search_radius=1.0), g2_initial_pose())
     assert r1.T.tobytes() == r2.T.tobytes()
 
 
@@ -136,7 +99,7 @@ def test_scans_mixed_outcomes(ctx, scene):
     returns it; its neighbours still equal their single runs."""
     from dcreg_b200 import api
     frames, _, T_init, tgt = scene
-    prm = c3_params()
+    prm = params()
     Ts = T_init[:5].copy()
     Ts[2] = o.pose6d_to_matrix(500.0, 0, 0, 0, 0, 0)
     ctx.set_target(tgt, RADIUS)
@@ -150,7 +113,7 @@ def test_scans_mixed_outcomes(ctx, scene):
 
 def test_scans_covariance(ctx, scene):
     frames, _, T_init, tgt = scene
-    prm = c3_params()
+    prm = params()
     Ts = T_init[:6].copy()
     Ts[4] = o.pose6d_to_matrix(500.0, 0, 0, 0, 0, 0)        # not converged: 1e6 I
     ctx.set_target(tgt, RADIUS)
@@ -170,7 +133,7 @@ def test_scans_covariance(ctx, scene):
 def test_scans_bad_arguments(ctx, scene, cylinder):
     from dcreg_b200 import api
     frames, _, T_init, tgt = scene
-    prm = c3_params()
+    prm = params()
     ctx.set_target(tgt, RADIUS)
     lib, h = ctx.lib, ctx._h
     xyz = np.ascontiguousarray(np.concatenate(frames[:3]), dtype=np.float32)
@@ -192,7 +155,7 @@ def test_scans_bad_arguments(ctx, scene, cylinder):
            dict(offsets=np.array([1, 10, 20, 30], np.int64)),                                   # not from 0
            dict(offsets=np.array([0, 100, 50, len(xyz)], np.int64)),                            # descending
            dict(offsets=np.array([0, 100, 100, len(xyz)], np.int64)),                           # an empty scan
-           dict(params=c3_params(weight_gate=1.5)), dict(params=c3_params(max_iterations=-1))]  # check_run_args
+           dict(params=params(weight_gate=1.5)), dict(params=params(max_iterations=-1))]  # check_run_args
     for kw in bad:
         assert call(**kw) == api.BAD_ARG, kw
         assert lib.dcreg_last_error(h).decode(), kw

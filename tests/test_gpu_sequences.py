@@ -12,18 +12,9 @@ import numpy as np
 import pytest
 
 import dcreg_oracle as o
+from harness import RADIUS, assert_same_run, ctx, params  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-RADIUS = 0.5
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
 
 
 @pytest.fixture(scope="module")
@@ -51,34 +42,6 @@ def chain():
     return seqs, cut, T_init[bounds[:-1]], deltas, T_true, tgt
 
 
-def c3_params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
-
-
-def rel_err(a, b):
-    a = np.asarray(a, dtype=np.float64); b = np.asarray(b, dtype=np.float64)
-    return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-300))
-
-
-def assert_same_run(b, single, logs=True):
-    assert (b.status, b.iterations, b.converged) == (single.status, single.iterations, single.converged)
-    assert o.se3_log_distance(single.T, b.T) < 1e-8
-    if not logs:
-        return
-    assert len(b.logs) == len(single.logs)
-    for x, y in zip(b.logs, single.logs):
-        assert x.n_effective == y.n_effective and x.n_corr_pt == y.n_corr_pt
-        assert list(x.analysis.degenerate_mask) == list(y.analysis.degenerate_mask)
-        if x.status == 0:
-            assert rel_err(np.array(x.H27), np.array(y.H27)) < 1e-8
-            assert np.max(np.abs(np.array(x.dx) - np.array(y.dx))) < 1e-8
-
-
 def assert_chained_priors(res, seqs, T_init, deltas):
     """First prior of every sequence = T_init byte for byte; every later prior = compose_prior(previous result, delta)."""
     from dcreg_b200.api import compose_prior
@@ -94,7 +57,7 @@ def assert_chained_priors(res, seqs, T_init, deltas):
 @pytest.mark.parametrize("method", ["Ours", "ME-TSVD"])
 def test_one_frame_sequences_equal_scan_batch(ctx, scene, method):
     frames, _, T_init, tgt = scene
-    prm = c3_params(method)
+    prm = params(method)
     ctx.set_target(tgt, RADIUS)
     scans = ctx.icp_run_scans(prm, frames, T_init, want_log=True, want_cov=True)
     seqs = ctx.icp_run_sequences(prm, [[f] for f in frames], T_init, want_log=True, want_cov=True)
@@ -111,7 +74,7 @@ def test_one_frame_sequences_equal_scan_batch(ctx, scene, method):
 def test_chained_frames_equal_their_own_runs(ctx, chain, method):
     """Ours advances the frame in the loop kernel's folded step; ME-TSVD in the separate solve kernel (k2_step_kernel)."""
     seqs, frames, T_init, deltas, _, tgt = chain
-    prm = c3_params(method)
+    prm = params(method)
     ctx.set_target(tgt, RADIUS)
     res = ctx.icp_run_sequences(prm, seqs, T_init, deltas, want_log=True)
     assert len(res) == len(frames) == 32
@@ -126,7 +89,7 @@ def test_chained_frames_match_oracle(ctx, chain):
     import dcreg_oracle_c as oc
     seqs, frames, T_init, deltas, _, tgt = chain
     ctx.set_target(tgt, RADIUS)
-    res = ctx.icp_run_sequences(c3_params(), seqs, T_init, deltas, want_log=True)
+    res = ctx.icp_run_sequences(params(), seqs, T_init, deltas, want_log=True)
     cp = oc.make_params(search_radius=RADIUS, max_iterations=30, conv_rot=1e-5, conv_trans=1e-3, kappa_target=10.0)
     for k in (9, 16, 23, 31):                               # frames deep in the 24-frame sequence
         b = res[k]
@@ -149,7 +112,7 @@ def test_abort_does_not_stop_the_sequence(ctx, chain):
     _, frames, T_init, deltas, _, tgt = chain
     seq = [frames[8], frames[9], frames[10][:5], frames[11], frames[12]]
     d = deltas[8:13]
-    prm = c3_params()
+    prm = params()
     ctx.set_target(tgt, RADIUS)
     res = ctx.icp_run_sequences(prm, [seq], T_init[2:3], d, want_log=True)
     assert res[2].status == api.NOT_ENOUGH_POINTS and res[2].iterations == 1 and not res[2].converged
@@ -164,7 +127,7 @@ def test_abort_does_not_stop_the_sequence(ctx, chain):
 @pytest.mark.parametrize("method", ["Ours", "ME-TSVD"])
 def test_fixed_iterations_run_every_frame_to_the_cap(ctx, chain, method):
     seqs, frames, T_init, deltas, _, tgt = chain
-    prm = c3_params(method, fixed_iterations=1, max_iterations=5)
+    prm = params(method, fixed_iterations=1, max_iterations=5)
     ctx.set_target(tgt, RADIUS)
     res = ctx.icp_run_sequences(prm, seqs, T_init, deltas)
     assert len(res) == len(frames)
@@ -177,14 +140,14 @@ def test_identity_increments(ctx, chain):
     seqs, frames, T_init, _, _, tgt = chain
     ctx.set_target(tgt, RADIUS)
     short = [s[:3] for s in seqs]
-    res = ctx.icp_run_sequences(c3_params(), short, T_init)
+    res = ctx.icp_run_sequences(params(), short, T_init)
     assert_chained_priors(res, short, T_init, None)
 
 
 def test_sequences_reproducible_and_context_intact(ctx, scene, chain):
     seqs, _, T_init, deltas, _, tgt = chain
     frames16, _, T16, _ = scene
-    prm = c3_params()
+    prm = params()
     ctx.set_target(tgt, RADIUS)
     ctx.set_source(frames16[0])
     one = ctx.icp_run(prm, T16[0])
@@ -207,7 +170,7 @@ def test_sequences_reproducible_and_context_intact(ctx, scene, chain):
 def test_sequences_bad_arguments(ctx, chain, cylinder):
     from dcreg_b200 import api
     _, frames, T_init, deltas, _, tgt = chain
-    prm = c3_params()
+    prm = params()
     ctx.set_target(tgt, RADIUS)
     lib, h = ctx.lib, ctx._h
     fr = frames[:4]
@@ -235,8 +198,8 @@ def test_sequences_bad_arguments(ctx, chain, cylinder):
            dict(seq_off=np.array([1, 2, 4], np.int32)),                                 # not from 0
            dict(seq_off=np.array([0, 1, 3], np.int32)),                                 # seq_offsets[n_seqs] != n_frames
            dict(offsets=np.array([0, off[1], off[1], off[3], off[4]], np.int64)),       # an empty frame
-           dict(params=c3_params(max_iterations=0)), dict(params=c3_params(max_iterations=-1)),
-           dict(params=c3_params(weight_gate=1.5))]
+           dict(params=params(max_iterations=0)), dict(params=params(max_iterations=-1)),
+           dict(params=params(weight_gate=1.5))]
     for kw in bad:
         assert call(**kw) == api.BAD_ARG, kw
         assert lib.dcreg_last_error(h).decode(), kw

@@ -23,28 +23,13 @@ import pytest
 
 import dcreg_oracle as o
 import dcreg_oracle_mp as m
-from test_gpu_k2_step import designed, run_designed
+from harness import METHODS, ctx, designed, run_designed  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-METHODS = {                       # the six methods of the CLI's SO(3) path, and the two handled as plain QR
-    "Ours": ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG"),
-    "NONE": ("NONE_DETE", "NONE_HAND"),
-    "ME-SR": ("FULL_EVD_MIN_EIGENVALUE", "SOLUTION_REMAPPING"),
-    "FCN-SR": ("FULL_SVD_CONDITION", "SOLUTION_REMAPPING"),
-    "ME-TSVD": ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD"),
-    "ME-TReg": ("FULL_EVD_MIN_EIGENVALUE", "STANDARD_REGULARIZATION"),
-}
+# besides harness.METHODS, the two settings the step handles as plain QR
 QR_LIKE = {"ADAPTIVE": ("NONE_DETE", "ADAPTIVE_REGULARIZATION"), "EVD_SUB": ("EVD_SUB_CONDITION", "NONE_HAND")}
 STATS = {}
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
 
 
 def params(method, **over):

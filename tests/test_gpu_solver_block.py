@@ -7,16 +7,9 @@ import numpy as np
 import pytest
 
 from dcreg_b200.scenes import g2_initial_pose, make_cylinder
+from harness import ctx  # noqa: F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
 
 
 def _run(ctx, prm, T0, **env):

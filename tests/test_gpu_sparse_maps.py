@@ -12,20 +12,12 @@ import numpy as np
 import pytest
 
 import dcreg_oracle as o
+from harness import ctx, log_bytes, params  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-RADIUS = 0.5
 CELL = 0.5
 FAR_CELL = 0.25          # the long-range scene's cell: rings = 2
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
 
 
 @pytest.fixture(scope="module")
@@ -42,23 +34,6 @@ def long_range():
     from dcreg_b200.scenes import make_long_range_sequence
     frames, T_true, deltas = make_long_range_sequence(16, seed=81, n_scan=4_000, n_far=1_500)
     return [frames[:8], frames[8:]], T_true[[0, 8]], deltas
-
-
-def params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
-
-
-def log_bytes(rec, fitness=True):
-    r = type(rec).from_buffer_copy(rec)
-    r.iter_time_ms = 0.0
-    if not fitness:
-        r.fitness = 0.0
-    return bytes(r)
 
 
 def assert_same(a, b, skip_counts=()):
@@ -298,12 +273,6 @@ def test_session_captures_setting_and_failed_push(ctx, odo):
 
 
 # ---- 5. pairs --------------------------------------------------------------------------------------------------------
-
-@pytest.fixture(scope="module")
-def cylinder():
-    import os
-    return o.read_pcd_xyz(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "cylinder_7562.pcd"))
-
 
 def test_pairs_far_target(ctx, cylinder, odo):
     from dcreg_b200 import api

@@ -13,17 +13,14 @@ both.  Contracts:
     keys of the cube, knn_search_lb's seven smallest inside the bound with their positions, knn_warp_search's
     got == (cube points inside the bound <= 64) and, when got, knn_search_lb's list.
 """
-import os
 import subprocess
 
 import numpy as np
 import pytest
 
-from test_gpu_corr_search import (CELLS, CLOUDS, RADIUS, WARP_CAP, F, Layout, Reference, bounds_for, cloud, first_bad,
-                                  make_queries, r2_up, rings_of, write_input)
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HARNESS = os.path.join(ROOT, "tools", "test_sparse_search.cu")
+from harness import tool_program
+from search_harness import (CELLS, CLOUDS, RADIUS, WARP_CAP, Layout, Reference, bounds_for, cloud, first_bad,
+                            make_queries, r2_up, rings_of, write_input)
 
 
 def read_output(path, nq, nrr):
@@ -54,11 +51,8 @@ def read_output(path, nq, nrr):
 
 @pytest.fixture(scope="module")
 def harness(tmp_path_factory):
-    from dcreg_b200.build import _nvcc
-    from test_host_la import device_program_flags
-    exe = tmp_path_factory.mktemp("sparse_search") / "test_sparse_search"
-    subprocess.run([_nvcc()] + device_program_flags() + ["-o", str(exe), HARNESS], check=True, capture_output=True, text=True)
-    return exe
+    return tool_program(tmp_path_factory.mktemp("sparse_search"), "test_sparse_search.cu", compiler="device",
+                        skip_missing=False)
 
 
 @pytest.mark.gpu
@@ -121,11 +115,4 @@ def test_sparse_searches_equal_dense(harness, tmp_path, name, cell):
 
 def test_sparse_harness_compiles_for_sm90a(tmp_path):
     """tools/test_sparse_search.cu builds with the library's flags (no GPU needed to compile)."""
-    from dcreg_b200.build import _nvcc
-    from test_host_la import device_program_flags
-    try:
-        nvcc = _nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc not available")
-    res = subprocess.run([nvcc] + device_program_flags() + ["-o", str(tmp_path / "h"), HARNESS], capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr
+    tool_program(tmp_path, "test_sparse_search.cu", compiler="device")

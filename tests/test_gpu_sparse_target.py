@@ -16,19 +16,11 @@ import numpy as np
 import pytest
 
 import dcreg_oracle as o
+from harness import RADIUS, ctx, log_bytes, params  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-RADIUS = 0.5
 FAR = np.array([[2000.0, 1500.0, 400.0], [3000.0, 3000.0, 500.0]], dtype=np.float32)
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from dcreg_b200 import Context
-    c = Context(0)
-    yield c
-    c.close()
 
 
 @pytest.fixture(scope="module")
@@ -50,24 +42,6 @@ def box_cells(xyz, cell):
     lo = np.floor(xyz.astype(np.float64).min(axis=0) / cell)
     hi = np.floor(xyz.astype(np.float64).max(axis=0) / cell)
     return float(np.prod(hi - lo + 1))
-
-
-def params(method="Ours", **over):
-    from dcreg_b200 import default_params
-    det, hand = ("SCHUR_CONDITION_NUMBER", "PRECONDITIONED_CG") if method == "Ours" else ("FULL_EVD_MIN_EIGENVALUE", "TRUNCATED_SVD")
-    kw = dict(search_radius=RADIUS, max_iterations=30, conv_thresh_rot=1e-5, conv_thresh_trans=1e-3, kappa_target=10.0,
-              detection=det, handling=hand)
-    kw.update(over)
-    return default_params(**kw)
-
-
-def log_bytes(L):
-    """a log record's bytes without iter_time_ms (a device clock reading)"""
-    from dcreg_b200.api import IterLog
-    b = bytearray(bytes(L))
-    off = IterLog.iter_time_ms.offset
-    b[off:off + 8] = bytes(8)
-    return bytes(b)
 
 
 def assert_identical(x, y):

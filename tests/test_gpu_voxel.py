@@ -8,8 +8,9 @@ tests/test_gpu_odometry.py."""
 import numpy as np
 import pytest
 
-from odom_harness import (CELL, assert_anchor, assert_priors, assert_same_run, clouds_of_every_case, ctx,  # noqa: F401
-                          parking, params, raw_downsample, raw_odometry, reconstruct, split)
+from harness import assert_same_run, ctx, params  # noqa: F401
+from odom_harness import (CELL, assert_anchor, assert_priors, clouds_of_every_case, parking,  # noqa: F401
+                          raw_downsample, raw_odometry, reconstruct, split)
 
 pytestmark = pytest.mark.gpu
 

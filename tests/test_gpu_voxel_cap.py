@@ -7,8 +7,9 @@ voxel_downsample(concatenation of map_points(T_out[j], filtered frame j) over th
 import numpy as np
 import pytest
 
-from odom_harness import (CELL, assert_anchor, assert_priors, assert_same_run, crowded_clouds, ctx, parking,  # noqa: F401
-                          params, raw_downsample, raw_odometry, reconstruct, split, window_map)
+from harness import assert_same_run, ctx, params  # noqa: F401
+from odom_harness import (CELL, assert_anchor, assert_priors, crowded_clouds, parking, raw_downsample,  # noqa: F401
+                          raw_odometry, reconstruct, split, window_map)
 
 pytestmark = pytest.mark.gpu
 

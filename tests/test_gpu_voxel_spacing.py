@@ -10,10 +10,10 @@ import math
 import numpy as np
 import pytest
 
+from harness import assert_same_run, ctx, params  # noqa: F401
 from odom_harness import (CELL, RAGGED, assert_anchor, assert_priors, assert_same, assert_same_flat,  # noqa: F401
-                          assert_same_run, crowded_clouds, ctx, map_call, odo, one_per_push, params, pushed,
-                          raw_downsample, raw_odometry, seq_results, source_points, split, sweeps, twin_maps,
-                          window_call, window_map)
+                          crowded_clouds, map_call, odo, one_per_push, pushed, raw_downsample, raw_odometry,
+                          seq_results, source_points, split, sweeps, twin_maps, window_call, window_map)
 
 pytestmark = pytest.mark.gpu
 

@@ -1,8 +1,6 @@
 """The gyroscope rotation of dcreg_icp_run_odometry_gyro: the NumPy twin (api.gyro_rotation, gyro_knots,
 deskew_points_gyro) against closed forms, a 50-digit evaluation, its clipping and bracketing rules and a scene whose gyro
 matches its trajectory; and dcreg_b200/csrc/se3.cuh built as host C++ against the twin, bit for bit."""
-import os
-import shutil
 import subprocess
 
 import mpmath
@@ -11,8 +9,7 @@ import pytest
 from scipy.spatial.transform import Rotation
 
 from dcreg_b200 import api, scenes
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from harness import tool_program
 
 
 def random_samples(rng, n=60, t0=-0.3, dt=0.01, scale=1.5):
@@ -145,12 +142,7 @@ def test_deskew_copies_what_does_not_move():
 
 
 def test_host_build_matches_the_twin(tmp_path):
-    cxx = shutil.which("g++") or shutil.which("c++")
-    if not cxx:
-        pytest.skip("no host C++ compiler")
-    exe = tmp_path / "test_gyro"
-    subprocess.run([cxx, "-O2", "-std=c++17", "-o", str(exe), os.path.join(ROOT, "tools", "test_gyro.cpp")], check=True,
-                   capture_output=True, text=True)
+    exe = tool_program(tmp_path, "test_gyro.cpp", compiler="c++")
     rng = np.random.default_rng(2026)
     R, bias = extrinsic(rng)
     S = random_samples(rng, n=300, scale=3.0)

@@ -1,33 +1,22 @@
 """Host side of per-lane solver settings (dcreg_set_lane_params): lane_plan.hpp compiled as plain host C++."""
-import os
-import shutil
 import subprocess
 
-import pytest
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from harness import dump, tool_program, write_config
 
 
 def test_lane_plan(tmp_path):
     """lane_plan: every parameter byte is common or per lane (reserved0 neither), a differing common field is named with
     its entry, the uniform case, and the fold mix (all fold, none, mixed, no fold without the in-kernel step)."""
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    exe = tmp_path / "test_lane_plan"
-    subprocess.run([gxx, "-O2", "-std=c++17", "-Wall", "-Wextra", "-o", str(exe),
-                    os.path.join(ROOT, "tools", "test_lane_plan.cpp")], check=True, capture_output=True, text=True)
+    exe = tool_program(tmp_path, "test_lane_plan.cpp", "-Wall", "-Wextra")
     res = subprocess.run([str(exe)], capture_output=True, text=True)
     assert res.returncode == 0, res.stdout + res.stderr
     assert "LANE_PLAN_OK" in res.stdout
-
 
 
 def test_cli_one_call_key(golden, tmp_path):
     """monte_carlo.one_call: off by default, parsed when given, and a YAML error past 65535 lanes (methods the SO(3) path
     recognises x trials)"""
     from dcreg_b200 import build as b
-    from test_cli_runner import dump, write_config
     runner = b.build_runner()
     cfg = tmp_path / "icp.yaml"
     setup = golden["G2"]["setup"]

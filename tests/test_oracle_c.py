@@ -4,7 +4,7 @@ import pytest
 
 import dcreg_oracle as o
 import dcreg_oracle_c as oc
-from test_oracle_golden import METHODS, init_T, params_from
+from harness import init_T, params_from
 
 
 def c_params(prm: o.Params, **kw):

@@ -4,38 +4,11 @@ Tolerances: the dumps print 8 decimals (dx, T, RMSE) / 3-6 decimals (eigenvalues
 G1 (released code path, every baseline handler) is reproduced to print precision (<= 1e-8);
 G2/G3 ("Ours", unreleased full code) to <= 5e-7 on dx/T - inside the 1e-6 pose contract.
 """
-import math
-
 import numpy as np
 import pytest
 
 import dcreg_oracle as o
-
-METHODS = {  # icp.yaml test_methods / icp_pk01.yaml:106
-    "ME-SR": (o.DET_FULL_EVD_MIN_EIGENVALUE, o.HAND_SOLUTION_REMAPPING),
-    "ME-TSVD": (o.DET_FULL_EVD_MIN_EIGENVALUE, o.HAND_TRUNCATED_SVD),
-    "ME-TReg": (o.DET_FULL_EVD_MIN_EIGENVALUE, o.HAND_STANDARD_REGULARIZATION),
-    "FCN-SR": (o.DET_FULL_SVD_CONDITION, o.HAND_SOLUTION_REMAPPING),
-    "Ours": (o.DET_SCHUR_CONDITION_NUMBER, o.HAND_PRECONDITIONED_CG),
-}
-
-
-def params_from(setup, method, **over):
-    det, hand = METHODS[method]
-    p = o.Params(search_radius=setup["search_radius"], max_iterations=setup["max_iterations"],
-                 conv_rot=setup["conv_rot"], conv_trans=setup["conv_trans"], cond_thresh=setup["cond_thresh"],
-                 eig_thresh=setup["eig_thresh"], kappa_target=setup["kappa_target"],
-                 std_reg_gamma=setup["std_reg_gamma"], use_weight_derivative=setup["use_weight_derivative"],
-                 detection=det, handling=hand)
-    for k, v in over.items():
-        setattr(p, k, v)
-    return p
-
-
-def init_T(setup):
-    x, y, z = setup["init_xyz"]
-    r, p, yw = [math.radians(a) for a in setup["init_rpy_deg"]]
-    return o.pose6d_to_matrix(x, y, z, r, p, yw)
+from harness import init_T, params_from
 
 
 @pytest.fixture(scope="module")

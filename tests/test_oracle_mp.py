@@ -13,6 +13,7 @@ import pytest
 
 import dcreg_oracle as o
 import dcreg_oracle_mp as m
+from harness import METHODS, oracle_method
 
 
 def _records(golden, cylinder, name, **over):
@@ -93,16 +94,6 @@ def test_mp_reference_reports_margins_and_branches():
 # every analysis field, the baseline methods, the pose update and the covariance (dcreg_oracle_mp.analysis_reference,
 # boxplus_reference, covariance_reference) against the FP64 oracle, and the slips those checks must catch
 # ------------------------------------------------------------------------------------------------------------------
-METHODS = {                      # the six methods of the CLI's SO(3) path: (detection, handling)
-    "Ours": (o.DET_SCHUR_CONDITION_NUMBER, o.HAND_PRECONDITIONED_CG),
-    "NONE": (o.DET_NONE, o.HAND_NONE),
-    "ME-SR": (o.DET_FULL_EVD_MIN_EIGENVALUE, o.HAND_SOLUTION_REMAPPING),
-    "FCN-SR": (o.DET_FULL_SVD_CONDITION, o.HAND_SOLUTION_REMAPPING),
-    "ME-TSVD": (o.DET_FULL_EVD_MIN_EIGENVALUE, o.HAND_TRUNCATED_SVD),
-    "ME-TReg": (o.DET_FULL_EVD_MIN_EIGENVALUE, o.HAND_STANDARD_REGULARIZATION),
-}
-
-
 def align_fp64(V, sign_fix=True):
     """FP64 twin of k2_solve.cuh's align_axes (V: 3x3, eigenvectors in columns)"""
     used_v, used_e, ind = set(), set(), [0, 0, 0]
@@ -142,7 +133,8 @@ def _method_runs(golden, cylinder):
     out = []
     for name in ("G1", "G2"):
         s = golden[name]["setup"]
-        for meth, (det, hand) in METHODS.items():
+        for meth in METHODS:
+            det, hand = oracle_method(meth)
             x, y, z = s["init_xyz"]
             r, p, yw = [math.radians(v) for v in s["init_rpy_deg"]]
             prm = o.Params(search_radius=s["search_radius"], max_iterations=s["max_iterations"], conv_rot=s["conv_rot"],

@@ -1,24 +1,16 @@
 """Host side of dcreg_icp_run_scans (a batch of different scans against one map): the ragged tile rule of loop_plan.hpp
 compiled as plain host C++, and the seeded C3-shaped frame generator the benchmark and the GPU tests use."""
-import os
-import shutil
 import subprocess
 
 import numpy as np
-import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from harness import tool_program
 
 
 def test_scan_tile_plan(tmp_path):
     """loop_plan::plan_scan_tiles: one grid for scans of ragged sizes, sized by the largest; every slot of every scan taken
     by exactly one block, the blocks past a smaller scan's end take none, full tiles, at most 64 blocks per scan."""
-    gxx = shutil.which("g++")
-    if not gxx:
-        pytest.skip("g++ not available")
-    exe = tmp_path / "test_scan_plan"
-    subprocess.run([gxx, "-O2", "-std=c++17", "-o", str(exe), os.path.join(ROOT, "tools", "test_scan_plan.cpp")], check=True,
-                   capture_output=True, text=True)
+    exe = tool_program(tmp_path, "test_scan_plan.cpp")
     res = subprocess.run([str(exe)], capture_output=True, text=True)
     assert res.returncode == 0, res.stdout + res.stderr
     assert "SCAN_PLAN_OK" in res.stdout

@@ -1,16 +1,12 @@
 """dcreg_b200/csrc/se3.cuh (the device's SE(3) log / exp of the odometry's motion compensation) built as host C++ and
 held against the NumPy twin on random motions: at most 4 FP64 ulp on every twist entry (of the twist's largest entry),
 and every deskewed point within the accuracy contract (one float32 ulp or 1e-12 m) of the twin."""
-import os
-import shutil
 import subprocess
 
 import numpy as np
-import pytest
 
 from dcreg_b200 import api
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from harness import tool_program
 
 
 def random_motions(rng, n):
@@ -27,12 +23,7 @@ def random_motions(rng, n):
 
 
 def test_host_build_matches_the_twin(tmp_path):
-    cxx = shutil.which("g++") or shutil.which("c++")
-    if not cxx:
-        pytest.skip("no host C++ compiler")
-    exe = tmp_path / "test_se3"
-    subprocess.run([cxx, "-O2", "-std=c++17", "-o", str(exe), os.path.join(ROOT, "tools", "test_se3.cpp")], check=True,
-                   capture_output=True, text=True)
+    exe = tool_program(tmp_path, "test_se3.cpp", compiler="c++")
     rng = np.random.default_rng(2024)
     D = random_motions(rng, 400)
     n_pts = 20_000

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 from dcreg_b200.api import VOXEL_LIMIT, voxel_downsample
-from test_voxel_twin import direct as first_per_voxel
+from harness import direct, holes, voxel_lattice
 
 
 def insertion_loop(P, voxel, max_points):
@@ -39,22 +39,6 @@ def check(P, voxel, max_points):
     return pts, idx
 
 
-def lattice(voxel):
-    """Points on voxel faces on both sides of 0, their float32 neighbours below, and their mirror images"""
-    g = np.arange(-6, 6, dtype=np.float64) * voxel
-    P = np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3).astype(np.float32)
-    return np.concatenate([P, np.nextafter(P, np.float32(-np.inf)), -P])
-
-
-def holes(rng, n=600):
-    P = rng.uniform(-3, 3, (n, 4)).astype(np.float32)
-    P[::7, 0] = np.nan
-    P[3::11, 1] = np.inf
-    P[5::13, 2] = -np.inf
-    P[::17, 3] = np.nan                                                      # a 4th column does not matter
-    return P
-
-
 CAPS = [1, 2, 3, 4, 20]
 
 
@@ -69,7 +53,7 @@ def test_random_clouds(voxel, max_points):
 @pytest.mark.parametrize("max_points", CAPS)
 @pytest.mark.parametrize("voxel", [0.25, 0.1])
 def test_lattice_on_voxel_boundaries(voxel, max_points):
-    pts, idx = check(lattice(voxel), voxel, max_points)
+    pts, idx = check(voxel_lattice(voxel), voxel, max_points)
     keys = np.floor(pts.astype(np.float64) * (1.0 / voxel))
     _, counts = np.unique(keys, axis=0, return_counts=True)
     assert counts.max() <= max_points and (keys < 0).any()
@@ -99,16 +83,16 @@ def test_one_voxel_holding_thousands(max_points):
 @pytest.mark.parametrize("voxel", [0.05, 0.25, 1.0])
 def test_one_point_per_voxel_is_the_first_point_filter(voxel):
     rng = np.random.default_rng(21)
-    for P in (rng.standard_normal((2000, 3)).astype(np.float32) * 4, lattice(voxel), holes(rng)):
+    for P in (rng.standard_normal((2000, 3)).astype(np.float32) * 4, voxel_lattice(voxel), holes(rng)):
         pts, idx = voxel_downsample(P, voxel, 1)
         pts0, idx0 = voxel_downsample(P, voxel)
-        assert np.array_equal(idx, first_per_voxel(P, voxel)) and np.array_equal(idx, idx0)
+        assert np.array_equal(idx, direct(P, voxel)) and np.array_equal(idx, idx0)
         assert pts.tobytes() == pts0.tobytes()
 
 
 def test_kept_sets_nest():
     rng = np.random.default_rng(22)
-    P = np.concatenate([(rng.standard_normal((4000, 3)) * 2).astype(np.float32), lattice(0.25)])
+    P = np.concatenate([(rng.standard_normal((4000, 3)) * 2).astype(np.float32), voxel_lattice(0.25)])
     prev = voxel_downsample(P, 0.25, 1)[1]
     for n in range(2, 12):
         idx = voxel_downsample(P, 0.25, n)[1]

@@ -9,7 +9,7 @@ import pytest
 
 from dcreg_b200 import api
 from dcreg_b200.api import voxel_downsample
-from test_voxel_cap_twin import holes, lattice
+from harness import holes, voxel_lattice
 
 
 def add_points(voxels, P, voxel, max_points, min_spacing, stamp0=0):
@@ -95,8 +95,8 @@ def test_pairs_at_the_spacing_and_one_ulp_either_side(max_points):
 @pytest.mark.parametrize("max_points", CAPS)
 @pytest.mark.parametrize("voxel", [0.25, 0.1])
 def test_points_on_voxel_faces(voxel, max_points):
-    check(lattice(voxel), voxel, max_points, voxel / math.sqrt(max_points))
-    check(lattice(voxel), voxel, max_points, 0.5 * voxel)
+    check(voxel_lattice(voxel), voxel, max_points, voxel / math.sqrt(max_points))
+    check(voxel_lattice(voxel), voxel, max_points, 0.5 * voxel)
 
 
 @pytest.mark.parametrize("max_points", CAPS)
@@ -108,7 +108,7 @@ def test_non_finite_rows(max_points):
 @pytest.mark.parametrize("max_points", CAPS)
 def test_zero_spacing_is_the_cap_rule(max_points):
     rng = np.random.default_rng(11)
-    for P in (rng.standard_normal((3000, 3)).astype(np.float32), lattice(0.25), holes(rng)):
+    for P in (rng.standard_normal((3000, 3)).astype(np.float32), voxel_lattice(0.25), holes(rng)):
         pts, idx = voxel_downsample(P, 0.25, max_points, 0.0)
         pts0, idx0 = voxel_downsample(P, 0.25, max_points)
         assert np.array_equal(idx, idx0) and pts.tobytes() == pts0.tobytes()
@@ -118,7 +118,7 @@ def test_zero_spacing_is_the_cap_rule(max_points):
 def test_spacing_above_twice_the_voxel_is_cap_one(max_points):
     rng = np.random.default_rng(12)
     for voxel in (0.1, 0.5):
-        P = np.concatenate([rng.standard_normal((3000, 3)).astype(np.float32), lattice(voxel), holes(rng)[:, :3]])
+        P = np.concatenate([rng.standard_normal((3000, 3)).astype(np.float32), voxel_lattice(voxel), holes(rng)[:, :3]])
         idx1 = voxel_downsample(P, voxel, 1)[1]
         for s in (np.nextafter(2 * voxel, np.inf), 3 * voxel):
             assert np.array_equal(voxel_downsample(P, voxel, max_points, s)[1], idx1)

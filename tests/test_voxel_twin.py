@@ -1,26 +1,10 @@
 """dcreg_b200.api.voxel_downsample, the NumPy twin of dcreg_voxel_downsample: against a direct per-point reading of the
 rule (a dict of the first index per voxel, one point at a time), on the CPU."""
-import math
-
 import numpy as np
 import pytest
 
-from dcreg_b200.api import VOXEL_LIMIT, voxel_downsample
-
-
-def direct(P, voxel):
-    """The rule read literally: walk the points in order, the voxel of a finite point is floor(float64(c) * (1 / voxel))
-    per axis, and the first point to reach a voxel keeps it."""
-    inv = 1.0 / voxel
-    first = {}
-    for i, p in enumerate(np.asarray(P, dtype=np.float32)):
-        c = [float(np.float64(v)) for v in p[:3]]
-        if not all(math.isfinite(v) for v in c):
-            continue
-        key = tuple(math.floor(v * inv) for v in c)
-        assert all(-VOXEL_LIMIT <= k < VOXEL_LIMIT for k in key)
-        first.setdefault(key, i)
-    return np.array(sorted(first.values()), dtype=np.int64)
+from dcreg_b200.api import voxel_downsample
+from harness import direct, voxel_lattice
 
 
 def check(P, voxel):
@@ -45,10 +29,7 @@ def test_random_clouds(voxel):
 def test_lattice_on_voxel_boundaries(voxel):
     """Points exactly on voxel faces, on both sides of 0, where floor and truncation differ for negative coordinates;
     0.1 is not a binary fraction, so some products round across a face."""
-    g = np.arange(-6, 6, dtype=np.float64) * voxel
-    P = np.stack(np.meshgrid(g, g, g, indexing="ij"), -1).reshape(-1, 3).astype(np.float32)
-    P = np.concatenate([P, np.nextafter(P, np.float32(-np.inf)), -P])
-    pts, idx = check(P, voxel)
+    pts, idx = check(voxel_lattice(voxel), voxel)
     keys = np.floor(pts.astype(np.float64) * (1.0 / voxel))
     assert len(np.unique(keys, axis=0)) == len(keys)
     assert (keys < 0).any()
