@@ -117,7 +117,7 @@ _lib = None
 EXPORTS = [
     "dcreg_abi_version", "dcreg_create", "dcreg_destroy", "dcreg_last_error", "dcreg_default_params",
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_set_target_sparse", "dcreg_set_sparse_maps",
-    "dcreg_set_lane_params", "dcreg_set_map_spacing",
+    "dcreg_set_lane_params", "dcreg_set_map_spacing", "dcreg_set_map_input_voxel",
     "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
@@ -150,6 +150,7 @@ def load_library():
     lib.dcreg_set_sparse_maps.argtypes = [vp, ci]
     lib.dcreg_set_lane_params.argtypes = [vp, ci]
     lib.dcreg_set_map_spacing.argtypes = [vp, C.c_double]
+    lib.dcreg_set_map_input_voxel.argtypes = [vp, C.c_double]
     lib.dcreg_find_planes.argtypes = [vp, dp, C.c_double, dp, C.POINTER(i64)]
     lib.dcreg_reduce_normal_equations.argtypes = [vp, vp, vp, i64, dp, ci, dp, dp]
     lib.dcreg_reduce_normal_equations_f64plane.argtypes = [vp, vp, vp, i64, dp, ci, dp, dp]
@@ -1014,6 +1015,8 @@ def _trial_results(st, conv, n_it, T_out, logs, cap, cov=None):
 class Context:
     """One engine context per GPU (owns the stream, device buffers and the optional NCCL comm)."""
 
+    _map_input_voxel = 0.0      # dcreg_set_map_input_voxel as set_map_input_voxel last set it
+
     def __init__(self, device: int = 0):
         self.lib = load_library()
         self._h = C.c_void_p()
@@ -1088,6 +1091,15 @@ class Context:
         default: the cap rule; KISS-ICP uses map_voxel / sqrt(map_max_points)).  A session keeps the value it had when it
         opened."""
         self._check(self.lib.dcreg_set_map_spacing(self._h, float(min_spacing)))
+
+    def set_map_input_voxel(self, voxel: float):
+        """The map-input filter of scan-to-map odometry (include/dcreg_b200.h, dcreg_set_map_input_voxel; KISS-ICP's
+        Voxelize): with voxel > 0 the frames enter the local maps as voxel_downsample(frame, voxel) and register with
+        voxel_downsample(voxel_downsample(frame, voxel), source_voxel, source_max_points), its NumPy twin (0, the
+        default: the maps take the source).  Applies to icp_run_odometry, icp_run_odometry_map and the sessions (which
+        keep the value they had when they opened), whatever their own voxel sizes."""
+        self._check(self.lib.dcreg_set_map_input_voxel(self._h, float(voxel)))
+        self._map_input_voxel = float(voxel)
 
     def set_lane_params(self, enable: bool):
         """Per-lane solver settings (include/dcreg_b200.h, dcreg_set_lane_params): the batched calls' params point to one
@@ -1390,7 +1402,8 @@ class Context:
         entry = _odometry_entry("icp_run_odometry", radius=with_radius, voxel_map=max_distance is not None,
                                 deskew=timestamps is not None or want_deskewed,
                                 capped=source_max_points != 1 or map_max_points != 1,
-                                filtered=source_voxel != 0.0 or map_voxel != 0.0, gyro=gyro is not None)
+                                filtered=source_voxel != 0.0 or map_voxel != 0.0 or self._map_input_voxel > 0.0,
+                                gyro=gyro is not None)
         ft, smp, smp_off = _pack_gyro(name, gyro, frame_times, gyro_samples, n, S)
         ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
                               off if off is not None else np.zeros(1, np.int64), name)

@@ -1343,7 +1343,9 @@ __global__ void odom_twist_kernel(const IcpState* __restrict__ states, int step_
 // Per step: the step's frames [step_first, step_first + active), points [base, base + n) of the packed (src) and the
 // sorted copy, deskewed in place by se3::deskew_point with their lane's twist.  A packed point's timestamp is ts[i]; a
 // sorted point's is that of its index in the frame (.w).  A point that does not move is not written.  The frame's lever
-// arm is taken again from the deskewed packed points with pack_points_kernel's rule.
+// arm is taken again from the deskewed packed points with pack_points_kernel's rule.  kSource = false (the map-input
+// points of dcreg_set_map_input_voxel, segments seg): the packed points alone, no sorted copy, no lever arm.
+template <bool kSource>
 __global__ void odom_deskew_kernel(float4* __restrict__ src, float4* __restrict__ sorted, const long long* __restrict__ seg,
                                    int step_first, int active, long long base, long long n, const float* __restrict__ ts,
                                    const double* __restrict__ xi, float* __restrict__ radius) {
@@ -1361,6 +1363,7 @@ __global__ void odom_deskew_kernel(float4* __restrict__ src, float4* __restrict_
             p.x = o[0]; p.y = o[1]; p.z = o[2];
             src[i] = p;
         }
+        if (!kSource) return;
         float4 q = sorted[i];
         const float qi[3] = {q.x, q.y, q.z};
         if (se3::deskew_point(x, ts[seg[b] + __float_as_int(q.w)], qi, o)) {
@@ -1371,6 +1374,7 @@ __global__ void odom_deskew_kernel(float4* __restrict__ src, float4* __restrict_
         r = sqrtf(px * px + py * py + pz * pz);
         if (!(r < 3.0e38f)) r = 0.0f;
     }
+    if (!kSource) return;
     const unsigned peers = __match_any_sync(0xffffffffu, b);
     const unsigned rmax = __reduce_max_sync(peers, __float_as_uint(r));
     if (b >= 0 && (int)(threadIdx.x & 31) == __ffs(peers) - 1 && rmax > 0u)
@@ -1397,7 +1401,8 @@ __global__ void odom_gyro_kernel(se3::Gyro g, const double* __restrict__ smp, co
 }
 
 // Per step, after odom_start_gyro_kernel: odom_deskew_kernel with se3::deskew_point_gyro, the lane's increment
-// translation tD[3 j ..] and its frame's knot table; the lever arm is taken again the same way.
+// translation tD[3 j ..] and its frame's knot table; the lever arm is taken again the same way (kSource as there).
+template <bool kSource>
 __global__ void odom_deskew_gyro_kernel(float4* __restrict__ src, float4* __restrict__ sorted,
                                         const long long* __restrict__ seg, int step_first, int active, long long base,
                                         long long n, const float* __restrict__ ts, const double* __restrict__ ft,
@@ -1420,6 +1425,7 @@ __global__ void odom_deskew_gyro_kernel(float4* __restrict__ src, float4* __rest
             p.x = o[0]; p.y = o[1]; p.z = o[2];
             src[i] = p;
         }
+        if (!kSource) return;
         float4 q = sorted[i];
         const float qi[3] = {q.x, q.y, q.z};
         if (se3::deskew_point_gyro(K, nk, f[0], f[1], f[2], f[3], t, ts[seg[b] + __float_as_int(q.w)], qi, o)) {
@@ -1430,6 +1436,7 @@ __global__ void odom_deskew_gyro_kernel(float4* __restrict__ src, float4* __rest
         r = sqrtf(px * px + py * py + pz * pz);
         if (!(r < 3.0e38f)) r = 0.0f;
     }
+    if (!kSource) return;
     const unsigned peers = __match_any_sync(0xffffffffu, b);
     const unsigned rmax = __reduce_max_sync(peers, __float_as_uint(r));
     if (b >= 0 && (int)(threadIdx.x & 31) == __ffs(peers) - 1 && rmax > 0u)
@@ -1556,6 +1563,9 @@ struct OdomSettings {
     // context's
     bool sparse_maps = false;
     double map_spacing = 0.0;
+    // dcreg_set_map_input_voxel (at open, for a session; at the call for the filtered one-shot calls; 0 for
+    // dcreg_icp_run_odometry): the frames enter the maps as F_in(frame), and register with F_s(F_in(frame))
+    double map_input_voxel = 0.0;
     // dcreg_set_lane_params on (at open, for a session): every sequence's settings [n_seqs], params being entry 0; off:
     // empty
     std::vector<dcreg_icp_params> lanes;
@@ -1634,6 +1644,12 @@ struct dcreg_ctx {
     // [points], and the step's twists [lanes][6]
     DevBuf<float> d_odom_ts_in, d_odom_ts;
     DevBuf<double> d_odom_xi;
+    // the map-input filter with a source filter after it (dcreg_set_map_input_voxel, voxel_filter_chain): F_in's kept
+    // xyz [input points][3] (NaN past the kept ones), their indices in their frames, its kept offsets [n_frames + 1];
+    // F_in's points packed in device order, and (timestamps) theirs
+    DevBuf<float> d_in_xyz; DevBuf<long long> d_in_index, d_in_seg;
+    DevBuf<float4> d_odom_in;
+    DevBuf<float> d_odom_ts_map;
     // gyroscope input: the call's samples [rows][4], every device frame's (start, span, tm, tm_prev) [n_frames][4], its
     // prior's rotation [n_frames][9] and the knot tables [knots][16] (odom_gyro_kernel)
     DevBuf<double> d_gyro_smp, d_gyro_ft, d_gyro_G, d_gyro_knots;
@@ -1696,6 +1712,9 @@ struct dcreg_ctx {
     // dcreg_set_map_spacing: the minimum point spacing of odometry's map filter (0: the cap rule; a session keeps the
     // value it had at open)
     double map_spacing = 0.0;
+    // dcreg_set_map_input_voxel: the voxel of odometry's map-input filter F_in (0: none; a session keeps the value it
+    // had at open)
+    double map_input_voxel = 0.0;
     // dcreg_set_lane_params: the batched calls' params point to one entry per lane (a session keeps the value it had at
     // open).  A call's entries [lanes] (plan_iteration), an odometry step's device lane -> sequence [lanes], and the log
     // fill's device trial -> lane [trials]
@@ -2161,6 +2180,53 @@ static int voxel_filter_host(dcreg_ctx* ctx, int n, const float* xyz, const int6
     return DCREG_OK;
 }
 
+// Odometry's map-input filter and the source filter after it (dcreg_set_map_input_voxel, KISS-ICP's Voxelize) on n
+// frames of host points, validated: F_in = the filter at voxel_in, one point per voxel, into ctx->d_in_xyz (indices in
+// the frame to ctx->d_in_index when `index`); then F_s = the filter at voxel with max_points over F_in's kept points,
+// through F_in's kept offsets on the device (ctx->d_in_seg), into ctx->d_vox_xyz (indices in F_in(frame) to
+// ctx->d_vox_index).  F_s runs over as many points as the input has: the rest of d_in_xyz is NaN, which has no voxel
+// and is never kept, so nothing waits for F_in's counts.  One host sync, after which kept_in / bad_in and kept / bad
+// ([n + 1] / [n]) hold F_in's and F_s's kept offsets and range flags.
+static int voxel_filter_chain(dcreg_ctx* ctx, int n, const float* xyz, const int64_t* offsets, int stride,
+                              double voxel_in, double voxel, int max_points, bool index, int64_t* kept_in, int* bad_in,
+                              int64_t* kept, int* bad) {
+    const long long total = offsets[n];
+    CK(ctx->d_stage.ensure(total * stride));
+    CK(ctx->d_vox_in_seg.ensure(n + 1));
+    CK(ctx->d_in_seg.ensure(n + 1));
+    CK(ctx->d_in_xyz.ensure(total * 3));
+    CK(ctx->d_vox_xyz.ensure(total * 3));
+    if (index) {
+        CK(ctx->d_in_index.ensure(total));
+        CK(ctx->d_vox_index.ensure(total));
+    }
+    // pinned: F_in's [n + 1] kept offsets and [n] flags (padded to 8 B), then F_s's
+    const size_t b_seg = (size_t)(n + 1) * sizeof(long long), b_bad = ((size_t)n * sizeof(int) + 7) / 8 * 8;
+    CK(ctx->h_pinned.ensure((long long)(2 * (b_seg + b_bad))));
+    unsigned char* h = ctx->h_pinned.p;
+    CK(cudaMemcpyAsync(ctx->d_stage, xyz, (size_t)total * stride * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_vox_in_seg, offsets, b_seg, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(ctx->d_in_xyz, 0xff, (size_t)total * 3 * sizeof(float), ctx->stream));   // NaN
+    int rc = voxel_filter(ctx, ctx->d_stage, total, stride, ctx->d_vox_in_seg, offsets, n, voxel_in, ctx->d_in_xyz, 3,
+                          index ? ctx->d_in_index.p : nullptr);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(ctx->d_in_seg, ctx->d_vox_seg, b_seg, cudaMemcpyDeviceToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(h, ctx->d_vox_seg, b_seg, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(h + b_seg, ctx->d_vox_bad, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    // the input offsets bound F_in's kept ones, so they size F_s's tables
+    if ((rc = voxel_filter(ctx, ctx->d_in_xyz, total, 3, ctx->d_in_seg, offsets, n, voxel, ctx->d_vox_xyz, 3,
+                           index ? ctx->d_vox_index.p : nullptr, max_points)))
+        return rc;
+    CK(cudaMemcpyAsync(h + b_seg + b_bad, ctx->d_vox_seg, b_seg, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(h + 2 * b_seg + b_bad, ctx->d_vox_bad, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    memcpy(kept_in, h, b_seg);
+    memcpy(bad_in, h + b_seg, (size_t)n * sizeof(int));
+    memcpy(kept, h + b_seg + b_bad, b_seg);
+    memcpy(bad, h + 2 * b_seg + b_bad, (size_t)n * sizeof(int));
+    return DCREG_OK;
+}
+
 // Grid arenas (dcreg_ctx::GridArena, planned by arena_plan.hpp): the dense grids of n clouds at once, cloud b being
 // d_pts[h_seg[b], h_seg[b+1]) (d_seg: the same offsets on the device).  One segmented bounds pass and one copy of the
 // n x 6 bounds to the host (arena_bounds: the only host sync), then one count, one exclusive scan, one scatter and one
@@ -2438,6 +2504,16 @@ int dcreg_set_map_spacing(dcreg_ctx* ctx, double min_spacing) {
         return DCREG_BAD_ARG;
     }
     ctx->map_spacing = min_spacing;
+    return DCREG_OK;
+}
+
+int dcreg_set_map_input_voxel(dcreg_ctx* ctx, double voxel) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!(voxel >= 0.0 && voxel < INFINITY)) {
+        ctx->err = "set_map_input_voxel: voxel must be finite and >= 0 (0: the maps take the source)";
+        return DCREG_BAD_ARG;
+    }
+    ctx->map_input_voxel = voxel;
     return DCREG_OK;
 }
 
@@ -3582,6 +3658,13 @@ static OdomSettings odom_settings(const dcreg_icp_params* params, int n_seqs, do
     return set;
 }
 
+// The settings of a filtered one-shot call (every dcreg_icp_run_odometry_* but dcreg_icp_run_odometry itself) with the
+// context's dcreg_set_map_input_voxel
+static OdomSettings with_map_input(OdomSettings set, const dcreg_ctx* ctx) {
+    if (ctx) set.map_input_voxel = ctx->map_input_voxel;
+    return set;
+}
+
 // How far R_sensor_imu^T R_sensor_imu may be from I, entry by entry
 constexpr double kGyroOrthoTol = 1e-6;
 
@@ -3653,6 +3736,15 @@ struct OdomCall {
     // the frames as the device gets them: the caller's, or the source filter's kept points (src_off: kept offsets)
     const float* src_xyz = xyz; int src_stride = stride; const int64_t* src_off = frame_offsets;
     std::vector<int64_t> kept;
+    // (dcreg_set_map_input_voxel) the frames' filter is the map-input filter F_in, whose kept points are the maps' input;
+    // split: a source filter F_s runs over them (voxel_filter_chain), and in_off (F_in's kept offsets) differs from
+    // src_off.  d_map_src: the points the maps and a session's window take, the packed sources or (split) d_odom_in
+    const bool split = set.map_input_voxel > 0.0 && set.source_voxel > 0.0;
+    const bool filtered = set.map_input_voxel > 0.0 || set.source_voxel > 0.0;
+    const int64_t* in_off = frame_offsets;
+    std::vector<int64_t> in_kept;
+    size_t in_ll = 0;                               // (split) where the map-input offsets are in d_odom_ll
+    const float4* d_map_src = nullptr;
     odom_plan::Push U;
     const odom_plan::Plan& P = U.plan;
     // where the tables are in d_odom_ll / d_odom_int: step i's map's (odom_plan::pack), then its int prev, prev2 and
@@ -3748,7 +3840,7 @@ int OdomCall::build_map(const odom_plan::MapInput& in, const long long* ll, cons
             return rc;
         const long long* d_dst = ll + segs + 1;
         map_points_kernel<<<(unsigned)((m + 255) / 256), 256, 0, ctx->stream>>>(
-            ctx->d_scan_src, d_win, d_old, n_frames, d_dst, pieces, d_dst + pieces + 1, ints, m, ctx->d_state, d_hist_T,
+            d_map_src, d_win, d_old, n_frames, d_dst, pieces, d_dst + pieces + 1, ints, m, ctx->d_state, d_hist_T,
             ctx->d_odom_map);
         ctx->launches++;
         CK(cudaGetLastError());
@@ -3817,23 +3909,40 @@ int OdomCall::check() {
                     return DCREG_BAD_ARG;
                 }
     if ((set.gyro || gi.frame_times || gi.samples || gi.sample_offsets) && (rc = check_gyro())) return rc;
-    if (set.source_voxel > 0.0) {
+    if (filtered) {
         kept.resize((size_t)n_frames + 1);
-        std::vector<int> bad((size_t)n_frames);
-        if ((rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, set.source_voxel, set.source_max_points,
-                                    0.0, timestamps != nullptr, false, kept.data(), bad.data())))
-            return rc;
+        std::vector<int> bad((size_t)n_frames), bad_in;
+        if (split) {
+            in_kept.resize((size_t)n_frames + 1);
+            bad_in.resize((size_t)n_frames);
+            rc = voxel_filter_chain(ctx, n_frames, xyz, frame_offsets, stride, set.map_input_voxel, set.source_voxel,
+                                    set.source_max_points, timestamps != nullptr, in_kept.data(), bad_in.data(),
+                                    kept.data(), bad.data());
+        } else if (set.map_input_voxel > 0.0) {     // F_s = none: the source is F_in(frame)
+            rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, set.map_input_voxel, 1, 0.0,
+                                   timestamps != nullptr, false, kept.data(), bad.data());
+        } else {
+            rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, set.source_voxel, set.source_max_points,
+                                   0.0, timestamps != nullptr, false, kept.data(), bad.data());
+        }
+        if (rc) return rc;
+        auto why = [](const std::vector<int64_t>& kp, const std::vector<int>& bd, int k, bool map_input) -> std::string {
+            const std::string f = map_input ? "the map-input filter" : "the source filter";
+            return bd[(size_t)k] ? "a voxel coordinate of " + f + " lies outside [-2^20, 2^20)"
+                   : kp[(size_t)k + 1] == kp[(size_t)k] ? "no point is left by " + f + " (no finite point)"
+                                                        : std::string();
+        };
         for (int s = 0; s < n_seqs; ++s)
             for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k) {
-                const char* why = bad[(size_t)k] ? "a voxel coordinate of the source filter lies outside [-2^20, 2^20)"
-                                  : kept[(size_t)k + 1] == kept[(size_t)k] ? "no point is left by the source filter (no finite point)"
-                                                                           : nullptr;
-                if (why) {
-                    ctx->err = std::string(name) + ": " + frame_name(s, k) + ": " + why;
+                std::string w = split ? why(in_kept, bad_in, k, true) : std::string();
+                if (w.empty()) w = why(kept, bad, k, set.map_input_voxel > 0.0 && !split);
+                if (!w.empty()) {
+                    ctx->err = std::string(name) + ": " + frame_name(s, k) + ": " + w;
                     return DCREG_BAD_ARG;
                 }
             }
         src_xyz = ctx->d_vox_xyz; src_stride = 3; src_off = kept.data();
+        in_off = split ? in_kept.data() : src_off;
     }
     if (frame_points)
         for (int k = 0; k < n_frames; ++k) frame_points[k] = src_off[k + 1] - src_off[k];
@@ -3918,7 +4027,8 @@ int OdomCall::upload() {
     int rc;
     {
         const std::string why = odom_plan::make_push(n_seqs, seq_offsets, n_frames, src_off,
-                                                     set.voxel_map ? 0 : set.map_frames, arena_plan::kMaxPoints, hist, &U);
+                                                     set.voxel_map ? 0 : set.map_frames, arena_plan::kMaxPoints, hist, &U,
+                                                     split ? in_off : nullptr);
         if (!why.empty()) { ctx->err = std::string(name) + ": " + why; return DCREG_BAD_ARG; }
     }
     const int n_steps = (int)P.steps.size();
@@ -3958,6 +4068,14 @@ int OdomCall::upload() {
         for (int d = 0; d < n_frames; ++d) hll.push_back(frame_offsets[P.input[(size_t)d]]);
         for (int d = 0; d < n_frames; ++d) hll.push_back(src_off[P.input[(size_t)d]]);
     }
+    // (split) then the map-input points' device offsets [n_frames + 1] and, with timestamps, F_in's kept offsets in
+    // device order [n_frames] (the first timestamp gather's kept_at)
+    in_ll = hll.size();
+    if (split) {
+        hll.insert(hll.end(), P.map_off.begin(), P.map_off.end());
+        if (timestamps)
+            for (int d = 0; d < n_frames; ++d) hll.push_back(in_off[P.input[(size_t)d]]);
+    }
     // (gyro input) then odom_gyro_kernel's: long long knot_off [n_frames + 1], range [n_frames][2] (device order)
     gyro_ll = hll.size();
     if (set.gyro && gi.samples) {
@@ -3984,7 +4102,7 @@ int OdomCall::upload() {
     // lane's frame range set by odom_start_kernel at every step; grids: the step's local maps
     S = Batch{n_frames, src_xyz, src_stride, P.dev_off.data()};
     S.order = P.input.data(); S.in_off = src_off;
-    if (set.source_voxel > 0.0) S.kind = cudaMemcpyDeviceToDevice;
+    if (filtered) S.kind = cudaMemcpyDeviceToDevice;
     S.sort = Batch::kBox;
     S.sort_box.inv_cell = 1.0 / set.cell_size;
     S.sort_box.ox = S.sort_box.oy = S.sort_box.oz = -512;
@@ -3994,6 +4112,8 @@ int OdomCall::upload() {
     S.lanes = n_seqs;
     if ((rc = stage_sources(ctx, S)) || (rc = stage_lanes(ctx, n_seqs, n_frames, &S.seq))) return rc;
     S.sort_T = ctx->d_seq_prior;
+    if (split) CK(ctx->d_odom_in.ensure(std::max<long long>(P.map_off[(size_t)n_frames], 1)));
+    d_map_src = split ? ctx->d_odom_in.p : ctx->d_scan_src.p;
     CK(ctx->d_odom_ll.ensure(std::max<long long>((long long)hll.size(), 1)));
     CK(ctx->d_odom_int.ensure(std::max<long long>((long long)hint.size(), 1)));
     CK(ctx->d_odom_map.ensure(std::max<long long>(P.max_map, 1)));
@@ -4053,7 +4173,12 @@ int OdomCall::start() {
         for (int c4 = 0; c4 < 4; ++c4) ident[(size_t)d * 16 + 5 * c4] = 1.0;
     CK(cudaMemcpyAsync(ctx->d_seq_prior, ident.data(), ident.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = start_loop(ctx, n_frames, T_dev.data(), R, &S, &dlog, &src_iter))) return rc;
-    const long long n_points = P.dev_off[(size_t)n_frames];
+    const long long n_points = P.dev_off[(size_t)n_frames], n_map_points = P.map_off[(size_t)n_frames];
+    const long long* d_map_seg = ctx->d_odom_ll + in_ll;
+    if (split &&                // F_in's kept points packed in device order, as the sources are
+        (rc = upload_points(ctx, ctx->d_in_xyz, n_map_points, 3, d_map_seg, n_frames, ctx->d_odom_in, nullptr,
+                            P.input.data(), in_off, cudaMemcpyDeviceToDevice)))
+        return rc;
     if (timestamps) {
         CK(ctx->d_odom_ts_in.ensure(std::max<long long>(frame_offsets[n_frames], 1)));
         CK(ctx->d_odom_ts.ensure(std::max<long long>(n_points, 1)));
@@ -4061,10 +4186,21 @@ int OdomCall::start() {
         CK(cudaMemcpyAsync(ctx->d_odom_ts_in, timestamps, (size_t)frame_offsets[n_frames] * sizeof(float),
                            cudaMemcpyHostToDevice, ctx->stream));
         const long long* d_in_at = ctx->d_odom_ll + ts_ll;
-        odom_ts_gather_kernel<<<(unsigned)((n_points + 255) / 256), 256, 0, ctx->stream>>>(
-            ctx->d_odom_ts_in, n_points, ctx->d_scan_seg, n_frames, d_in_at, d_in_at + n_frames,
-            set.source_voxel > 0.0 ? ctx->d_vox_index.p : nullptr, ctx->d_odom_ts);
-        ctx->launches++;
+        if (split) {            // the map-input points' timestamps, then the sources' from theirs
+            CK(ctx->d_odom_ts_map.ensure(std::max<long long>(n_map_points, 1)));
+            odom_ts_gather_kernel<<<(unsigned)((n_map_points + 255) / 256), 256, 0, ctx->stream>>>(
+                ctx->d_odom_ts_in, n_map_points, d_map_seg, n_frames, d_in_at, d_map_seg + n_frames + 1,
+                ctx->d_in_index, ctx->d_odom_ts_map);
+            odom_ts_gather_kernel<<<(unsigned)((n_points + 255) / 256), 256, 0, ctx->stream>>>(
+                ctx->d_odom_ts_map, n_points, ctx->d_scan_seg, n_frames, d_map_seg, d_in_at + n_frames,
+                ctx->d_vox_index, ctx->d_odom_ts);
+            ctx->launches += 2;
+        } else {
+            odom_ts_gather_kernel<<<(unsigned)((n_points + 255) / 256), 256, 0, ctx->stream>>>(
+                ctx->d_odom_ts_in, n_points, ctx->d_scan_seg, n_frames, d_in_at, d_in_at + n_frames,
+                filtered ? ctx->d_vox_index.p : nullptr, ctx->d_odom_ts);
+            ctx->launches++;
+        }
         CK(cudaGetLastError());
     }
     if (set.gyro && gi.samples) {   // every non-anchor frame's prior rotation and knot table, from one upload
@@ -4191,7 +4327,7 @@ int OdomCall::step(int i) {
     if (timestamps && set.gyro) {
         const long long a = P.dev_off[(size_t)st.first], np = P.dev_off[(size_t)(st.first + st.active)] - a;
         const long long* d_knot_off = ctx->d_odom_ll + gyro_ll;
-        odom_deskew_gyro_kernel<<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
+        odom_deskew_gyro_kernel<true><<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
             ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_seg, st.first, st.active, a, np, ctx->d_odom_ts,
             ctx->d_gyro_ft, d_knot_off, ctx->d_gyro_knots, ctx->d_odom_xi, ctx->d_scan_radius);
         ctx->launches++;
@@ -4201,10 +4337,26 @@ int OdomCall::step(int i) {
             ctx->d_state, st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T,
             ctx->d_odom_xi, ctx->d_scan_radius);
         const long long a = P.dev_off[(size_t)st.first], np = P.dev_off[(size_t)(st.first + st.active)] - a;
-        odom_deskew_kernel<<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
+        odom_deskew_kernel<true><<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
             ctx->d_scan_src, ctx->d_scan_sorted, ctx->d_scan_seg, st.first, st.active, a, np, ctx->d_odom_ts,
             ctx->d_odom_xi, ctx->d_scan_radius);
         ctx->launches += 2;
+        CK(cudaGetLastError());
+    }
+    // 3c. (split, timestamps) the step's map-input points deskewed with the same increments: every source point is a
+    // copy of one of them with the same timestamp, so the two passes agree on it bit for bit
+    if (timestamps && split) {
+        const long long a = P.map_off[(size_t)st.first], np = P.map_off[(size_t)(st.first + st.active)] - a;
+        const long long* d_map_seg = ctx->d_odom_ll + in_ll;
+        if (set.gyro)
+            odom_deskew_gyro_kernel<false><<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
+                ctx->d_odom_in, nullptr, d_map_seg, st.first, st.active, a, np, ctx->d_odom_ts_map, ctx->d_gyro_ft,
+                ctx->d_odom_ll + gyro_ll, ctx->d_gyro_knots, ctx->d_odom_xi, nullptr);
+        else
+            odom_deskew_kernel<false><<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
+                ctx->d_odom_in, nullptr, d_map_seg, st.first, st.active, a, np, ctx->d_odom_ts_map, ctx->d_odom_xi,
+                nullptr);
+        ctx->launches++;
         CK(cudaGetLastError());
     }
     // 4. the loop: the same chunks (and CUDA graphs) at every step - the grid table keeps its pointer (the first step
@@ -4248,7 +4400,7 @@ int OdomCall::finish() {
         const long long* d_keep_dst = ctx->d_odom_ll + keep_ll;
         const int keep = (int)U.keep_ref.size();
         retain_points_kernel<<<(unsigned)((kept_points + 255) / 256), 256, 0, ctx->stream>>>(
-            ctx->d_scan_src, sess->win[sess->cur], n_frames, d_keep_dst, keep, d_keep_dst + keep + 1,
+            d_map_src, sess->win[sess->cur], n_frames, d_keep_dst, keep, d_keep_dst + keep + 1,
             ctx->d_odom_int + keep_int, kept_points, sess->win[1 - sess->cur]);
         ctx->launches++;
         CK(cudaGetLastError());
@@ -4349,8 +4501,9 @@ int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params,
                                  double* T_out, int* n_iterations, int* converged, int* status, double* cov,
                                  dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_voxel",
-                        odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel, 1, 1, T_init,
-                                      ctx && ctx->lane_params),
+                        with_map_input(odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel,
+                                                     map_voxel, 1, 1, T_init, ctx && ctx->lane_params),
+                                       ctx),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, nullptr,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points, nullptr);
 }
@@ -4363,8 +4516,10 @@ int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* param
                                    int* n_iterations, int* converged, int* status, double* cov, dcreg_iter_log* log,
                                    int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_voxel_n",
-                        odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
-                                      source_max_points, map_max_points, T_init, ctx && ctx->lane_params),
+                        with_map_input(odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel,
+                                                     map_voxel, source_max_points, map_max_points, T_init,
+                                                     ctx && ctx->lane_params),
+                                       ctx),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, nullptr,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points, nullptr);
 }
@@ -4377,8 +4532,10 @@ int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params
                                   int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
                                   dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_deskew",
-                        odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
-                                      source_max_points, map_max_points, T_init, ctx && ctx->lane_params),
+                        with_map_input(odom_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel,
+                                                     map_voxel, source_max_points, map_max_points, T_init,
+                                                     ctx && ctx->lane_params),
+                                       ctx),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
                         deskewed_xyz);
@@ -4403,8 +4560,10 @@ int dcreg_icp_run_odometry_map(dcreg_ctx* ctx, const dcreg_icp_params* params, i
                                int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
                                dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_map",
-                        odom_map_settings(params, n_seqs, cell_size, motion, source_voxel, map_voxel, source_max_points,
-                                          map_max_points, max_distance, T_init, ctx && ctx->lane_params),
+                        with_map_input(odom_map_settings(params, n_seqs, cell_size, motion, source_voxel, map_voxel,
+                                                         source_max_points, map_max_points, max_distance, T_init,
+                                                         ctx && ctx->lane_params),
+                                       ctx),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
                         deskewed_xyz);
@@ -4436,9 +4595,11 @@ int dcreg_icp_run_odometry_adaptive(dcreg_ctx* ctx, const dcreg_icp_params* para
                                     int* n_iterations, int* converged, int* status, double* cov, float* deskewed_xyz,
                                     double* search_radius, dcreg_iter_log* log, int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_adaptive",
-                        odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion, source_voxel, map_voxel,
-                                               source_max_points, map_max_points, max_distance, adaptive, T_init,
-                                               ctx && ctx->lane_params),
+                        with_map_input(odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion,
+                                                              source_voxel, map_voxel, source_max_points,
+                                                              map_max_points, max_distance, adaptive, T_init,
+                                                              ctx && ctx->lane_params),
+                                       ctx),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
                         deskewed_xyz, search_radius);
@@ -4465,11 +4626,14 @@ int dcreg_icp_run_odometry_gyro(dcreg_ctx* ctx, const dcreg_icp_params* params, 
                                 double* cov, float* deskewed_xyz, double* search_radius, dcreg_iter_log* log,
                                 int log_cap) {
     return run_odometry(ctx, "icp_run_odometry_gyro",
-                        odom_gyro_settings(odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion,
-                                                                  source_voxel, map_voxel, source_max_points,
-                                                                  map_max_points, max_distance, adaptive, T_init,
-                                                                  ctx && ctx->lane_params),
-                                           gyro),
+                        with_map_input(odom_gyro_settings(odom_adaptive_settings(params, n_seqs, cell_size,
+                                                                                 map_frames, motion, source_voxel,
+                                                                                 map_voxel, source_max_points,
+                                                                                 map_max_points, max_distance,
+                                                                                 adaptive, T_init,
+                                                                                 ctx && ctx->lane_params),
+                                                          gyro),
+                                       ctx),
                         nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
                         Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
                         deskewed_xyz, search_radius,
@@ -4486,6 +4650,7 @@ static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     ss->set = set;
     ss->set.sparse_maps = ctx->sparse_maps;
     ss->set.map_spacing = ctx->map_spacing;
+    ss->set.map_input_voxel = ctx->map_input_voxel;
     const int n_seqs = set.n_seqs;
     BatchCheck c{name, !ss->set.T_init.empty(), "null pointer or n_seqs <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_seqs};

@@ -9,6 +9,9 @@
 // The map of frame k (since its sequence started) is the window frames [max(0, k - map_frames), k) of its sequence in
 // ascending order, each frame's points in their input order; the lanes' maps follow each other in one buffer.  Every
 // map input, a step's windows or a voxel-map update's, is one piece table (MapInput), which map_points_kernel lays out.
+// A frame has two point ranges in device order: the points it registers with (Plan::dev_off, the loop's segments) and
+// the points it gives the maps (Plan::map_off, the map input's pieces and a session's window).  They are one table
+// unless dcreg_set_map_input_voxel splits them: then a frame's map input is F_in(frame), its source F_s(F_in(frame)).
 // Everything here is plain C++ so tests/test_odom_plan.py, tests/test_odom_session_plan.py and
 // tests/test_odom_map_plan.py can check it on the CPU (tools/test_odom_*plan.cpp).
 #pragma once
@@ -58,6 +61,7 @@ struct Plan {
     std::vector<int> dev;               // [n_frames] device index of input frame k
     std::vector<int> input;             // [n_frames] input frame of device index d
     std::vector<int64_t> dev_off;       // [n_frames + 1] point offsets of the frames in device order
+    std::vector<int64_t> map_off;       // [n_frames + 1] ... of their map-input points (dev_off's values when not split)
     std::vector<Step> steps;            // steps[0]: the anchors (no map)
     long long max_map = 0;              // the most map points of one step
     int max_pieces = 0;                 // the most window frames of one step
@@ -66,7 +70,7 @@ struct Plan {
 // What a session carries, per sequence, from one push to the next: the frames pushed so far and the last of them: the
 // window frames the next frames' maps need, with their points, and the frames the constant-velocity model needs, by
 // pose alone.  Sequence s retains its last min(seen, max(map_frames, 2)) frames; the last min(seen, map_frames) of them
-// carry points (map_frames = 1 keeps the frame before the last as a pose alone).
+// carry their map-input points (map_frames = 1 keeps the frame before the last as a pose alone).
 struct History {
     std::vector<long long> seen;        // [n_seqs] frames of the sequence since the session opened
     std::vector<int> off;               // [n_seqs + 1] retained frames of sequence s: [off[s], off[s + 1]), oldest first
@@ -93,10 +97,11 @@ inline int retained_frames(long long seen, int map_frames) {
 }
 
 // seq_off: n_seqs + 1 non-decreasing frame offsets of the pushed frames (a sequence may have none), frame_off: n_frames
-// + 1 point offsets, both validated; h: the history before the push.  Fails (returns the reason) when the maps of one
-// step hold more than max_points points.
+// + 1 point offsets, both validated; h: the history before the push.  map_frame_off: n_frames + 1 offsets of the
+// frames' map-input points (null: frame_off, the points they register with).  Fails (returns the reason) when the maps
+// of one step hold more than max_points points.
 inline std::string make_push(int n_seqs, const int* seq_off, int n_frames, const int64_t* frame_off, int map_frames,
-                             long long max_points, const History& h, Push* out) {
+                             long long max_points, const History& h, Push* out, const int64_t* map_frame_off = nullptr) {
     Push& u = *out;
     u = Push{};
     Plan& p = u.plan;
@@ -124,18 +129,23 @@ inline std::string make_push(int n_seqs, const int* seq_off, int n_frames, const
         }
         st.active = (int)st.seq.size();
     }
-    p.dev_off.assign((size_t)n_frames + 1, 0);
-    for (int e = 0; e < n_frames; ++e) {
-        const int k = p.input[(size_t)e];
-        p.dev_off[(size_t)e + 1] = p.dev_off[(size_t)e] + (frame_off[k + 1] - frame_off[k]);
-    }
+    auto device_order = [&](const int64_t* off) {
+        std::vector<int64_t> o((size_t)n_frames + 1, 0);
+        for (int e = 0; e < n_frames; ++e) {
+            const int k = p.input[(size_t)e];
+            o[(size_t)e + 1] = o[(size_t)e] + (off[k + 1] - off[k]);
+        }
+        return o;
+    };
+    p.dev_off = device_order(frame_off);
+    p.map_off = map_frame_off ? device_order(map_frame_off) : p.dev_off;
     // frame w (since open) of sequence s: a pushed frame, or one the history retains
     auto ref = [&](int s, long long w) {
         const long long seen = h.seen[(size_t)s];
         return w >= seen ? p.dev[(size_t)(seq_off[s] + (w - seen))] : n_frames + h.off[(size_t)s + 1] - (int)(seen - w);
     };
-    auto points = [&](int r) { return r < n_frames ? p.dev_off[(size_t)r + 1] - p.dev_off[(size_t)r] : h.n[(size_t)(r - n_frames)]; };
-    auto first_point = [&](int r) { return r < n_frames ? p.dev_off[(size_t)r] : h.at[(size_t)(r - n_frames)]; };
+    auto points = [&](int r) { return r < n_frames ? p.map_off[(size_t)r + 1] - p.map_off[(size_t)r] : h.n[(size_t)(r - n_frames)]; };
+    auto first_point = [&](int r) { return r < n_frames ? p.map_off[(size_t)r] : h.at[(size_t)(r - n_frames)]; };
     for (int i = 1; i < n_steps; ++i) {
         Step& st = p.steps[(size_t)i];
         for (int j = 0; j < st.active; ++j) {
@@ -238,7 +248,7 @@ inline void map_step(const Plan& p, int i, bool carry, MapState& ms, MapInput* o
     for (int s : seq) {
         const int r = ms.last[(size_t)s];
         if (ms.n[(size_t)s] > 0) m.add_piece(ms.at[(size_t)s], -1, ms.n[(size_t)s]);
-        if (ms.pending[(size_t)s]) m.add_piece(p.dev_off[(size_t)r], r, p.dev_off[(size_t)r + 1] - p.dev_off[(size_t)r]);
+        if (ms.pending[(size_t)s]) m.add_piece(p.map_off[(size_t)r], r, p.map_off[(size_t)r + 1] - p.map_off[(size_t)r]);
         m.center.push_back(m.piece_dst.back() > m.seg.back() ? r : -1);
         m.end_segment(s);
     }

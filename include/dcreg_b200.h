@@ -203,6 +203,29 @@ int dcreg_set_lane_params(dcreg_ctx* ctx, int enable);
  * the value it had at dcreg_odometry_open*: changing it later does not change that session's pushes, and
  * dcreg_odometry_local_map returns the spaced map.  min_spacing NaN, negative or infinite: DCREG_BAD_ARG. */
 int dcreg_set_map_spacing(dcreg_ctx* ctx, double min_spacing);
+/* The map-input filter of scan-to-map odometry (KISS-ICP's Voxelize): with voxel > 0, frame k's points enter the maps
+ * as F_in(frame k) = dcreg_voxel_downsample(frame k, voxel), and frame k registers with F_s(F_in(frame k)).
+ * 0 (the default): the maps take F_s(frame k), as now.
+ * - Rule: F_in is applied to the raw frame in the sensor frame; F_s (source_voxel, source_max_points) to F_in's output
+ *   in F_in's order, so every source point is a bit-for-bit copy of one F_in point; source_voxel = 0: the source is
+ *   F_in(frame) itself.  Only the maps' input changes: the window of frame k is F_m(concatenation over the window frames
+ *   j of map_points(T_out[j], F_in(frame j))), the voxel map's update U(M_k, F_in(frame k), T_out[k]), anchors put
+ *   F_in(anchor) into the maps, a session retains the F_in points of its window frames and dcreg_odometry_local_map
+ *   returns the map built from them.  F_m, caps, dcreg_set_map_spacing, pruning, priors, the adaptive threshold, gyro
+ *   input and lane parameters are unchanged; frame_points and deskewed_xyz are still the registration source's.
+ * - Deskewing: each F_in point is deskewed with its own timestamp at its frame's step by the call's rule, and the
+ *   deskewed F_in points enter the maps; the source is deskewed the same way, so each source point is the deskewed copy
+ *   of its F_in point.  The frames are still filtered first, then deskewed.
+ * - Applies to dcreg_icp_run_odometry_voxel, _voxel_n, _deskew, _map, _adaptive and _gyro, and to sessions from every
+ *   dcreg_odometry_open*, which keep the value they had at open.  dcreg_icp_run_odometry (no downsampling),
+ *   _sequences, _scans, _pairs and the standalone filters ignore it.
+ * - Cost: the frames are filtered once per call: F_s runs on the device over F_in's output, and both filters' kept
+ *   counts come back in the one frame-filter sync.  A step keeps its one host sync and its launches (one more with
+ *   timestamps and a source filter: the F_in points' deskew), whatever the number of sequences.
+ * Errors (DCREG_BAD_ARG): voxel NaN, negative or infinite; at a call, before any loop launch and naming the sequence
+ * and frame, a frame with no finite point left by the map-input filter or a voxel coordinate of that filter outside
+ * [-2^20, 2^20).  A push that fails commits nothing. */
+int dcreg_set_map_input_voxel(dcreg_ctx* ctx, double voxel);
 
 /* ---- seam 1: correspondence stage (icp_test_runner.cpp:1714-1813) -------------------------
  * For every source slot: q = fl32(R p + t), exact 5-NN in the target, 5th d^2 < radius^2,
@@ -397,7 +420,8 @@ int dcreg_icp_run_odometry(dcreg_ctx* ctx, const dcreg_icp_params* params, int n
  * anything is launched); a frame with no finite point, or a voxel coordinate of the source filter outside [-2^20, 2^20)
  * (after the frames' filter, before any loop launch); a step's map with a voxel coordinate outside that range (at its
  * step, like a map too large for a dense grid: the earlier steps keep their outputs, the context stays usable).
- * dcreg_set_sparse_maps applies as in dcreg_icp_run_odometry. */
+ * dcreg_set_sparse_maps applies as in dcreg_icp_run_odometry.  With dcreg_set_map_input_voxel the maps take F_in(frame j)
+ * instead of F_s(frame j), and the source is F_s(F_in(frame k)); so in every call below that builds on this one. */
 int dcreg_icp_run_odometry_voxel(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
                                  int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
                                  double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
@@ -435,7 +459,8 @@ int dcreg_icp_run_odometry_voxel_n(dcreg_ctx* ctx, const dcreg_icp_params* param
  *   never deskewed (nothing is known of their motion).  Accuracy: within one float32 ulp of the exact value or 1e-12 m,
  *   whichever is larger (the device's sincos and libm's differ in the last FP64 bit).
  * - Order: the source filter runs first, on the raw points (the plan needs every frame's kept count before the loop);
- *   each kept point is then deskewed at its frame's step with its own timestamp.  KISS-ICP deskews, then filters; this
+ *   each kept point is then deskewed at its frame's step with its own timestamp (with dcreg_set_map_input_voxel, every
+ *   F_in point too: the maps take those).  KISS-ICP deskews, then filters; this
  *   call filters, then deskews.
  * - The deskewed frame is what frame k registers with, what enters the later maps (at T_out[k]) and what a session
  *   retains.  deskewed_xyz (out, may be NULL): every frame's kept points after deskewing, 3 floats each, frame_points[k]
@@ -465,7 +490,7 @@ int dcreg_icp_run_odometry_deskew(dcreg_ctx* ctx, const dcreg_icp_params* params
  *   pose it returned, aborted ones included, deskewed when timestamps are given.  Frame k registers against M_k and
  *   returns what dcreg_set_target(M_k, cell_size) + dcreg_set_source(F_s(frame k)) + dcreg_icp_run(T_prior[k]) returns,
  *   up to how the FP64 partial sums are grouped; priors, anchors, deskewing, covariances and logs as in
- *   dcreg_icp_run_odometry_deskew.
+ *   dcreg_icp_run_odometry_deskew.  With dcreg_set_map_input_voxel, F_in(frame) replaces F_s(frame) in the updates.
  * - max_distance = +inf prunes nothing; then, since cap(cap(A) ++ B) = cap(A ++ B), M_k is the window map of
  *   dcreg_icp_run_odometry_deskew with map_frames >= the longest sequence, and every output is the same bytes.
  * - Cost per step: one launch that lays out [old map | new frame] for every sequence, the capped filter and one prune
@@ -512,6 +537,7 @@ int dcreg_icp_run_odometry_map(dcreg_ctx* ctx, const dcreg_icp_params* params, i
  *   read-back) plus one launch that gathers the next windows; equal-shaped pushes reuse the buffers and the loop's CUDA
  *   graphs.  Other calls may run between pushes without changing the session's results, and a push leaves the
  *   context's source, target and grid as they were.
+ * dcreg_set_map_input_voxel, like dcreg_set_sparse_maps, is recorded at open: the window then retains F_in points.
  * dcreg_odometry_close: ends the session and frees its buffers; push or close without an open session is
  *   DCREG_BAD_ARG. */
 int dcreg_odometry_open(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
