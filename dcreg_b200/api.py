@@ -118,6 +118,7 @@ EXPORTS = [
     "dcreg_abi_version", "dcreg_create", "dcreg_destroy", "dcreg_last_error", "dcreg_default_params",
     "dcreg_stream", "dcreg_set_source", "dcreg_set_target", "dcreg_set_target_sparse", "dcreg_set_sparse_maps",
     "dcreg_set_lane_params", "dcreg_set_map_spacing", "dcreg_set_map_input_voxel",
+    "dcreg_set_prior_map",
     "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
@@ -151,6 +152,7 @@ def load_library():
     lib.dcreg_set_lane_params.argtypes = [vp, ci]
     lib.dcreg_set_map_spacing.argtypes = [vp, C.c_double]
     lib.dcreg_set_map_input_voxel.argtypes = [vp, C.c_double]
+    lib.dcreg_set_prior_map.argtypes = [vp, ci]
     lib.dcreg_find_planes.argtypes = [vp, dp, C.c_double, dp, C.POINTER(i64)]
     lib.dcreg_reduce_normal_equations.argtypes = [vp, vp, vp, i64, dp, ci, dp, dp]
     lib.dcreg_reduce_normal_equations_f64plane.argtypes = [vp, vp, vp, i64, dp, ci, dp, dp]
@@ -1100,6 +1102,13 @@ class Context:
         keep the value they had when they opened), whatever their own voxel sizes."""
         self._check(self.lib.dcreg_set_map_input_voxel(self._h, float(voxel)))
         self._map_input_voxel = float(voxel)
+
+    def set_prior_map(self, enable: int):
+        """Localisation in a prior map (include/dcreg_b200.h, dcreg_set_prior_map): with 1, icp_run_odometry (window
+        forms, map_frames >= 1) and the window sessions register every frame against the context's target instead of a
+        local map, each sequence's first frame from its T_init (0, the default: local maps).  Anything but 0 or 1
+        raises.  A session keeps the value it had when it opened, and local_map raises on it."""
+        self._check(self.lib.dcreg_set_prior_map(self._h, int(enable)))
 
     def set_lane_params(self, enable: bool):
         """Per-lane solver settings (include/dcreg_b200.h, dcreg_set_lane_params): the batched calls' params point to one

@@ -1203,7 +1203,7 @@ __global__ void map_points_kernel(const float4* __restrict__ src, const float4* 
 }
 
 // The increment D lane j's prior is composed with: delta[prev[j]] (null: identity), or with constant velocity the
-// increment from frame k-2 to frame k-1 (identity after the anchor).  The start kernel and odom_twist_kernel both take
+// increment from frame k-2 to frame k-1 (identity after the anchor); the identity for a first frame (prev[j] < 0).  The start kernel and odom_twist_kernel both take
 // it from here, so the deskew twist is the increment the prior used, bit for bit.
 __device__ __forceinline__ void odom_increment(int j, const IcpState* __restrict__ states, const int* __restrict__ prev,
                                                const int* __restrict__ prev2, const double* __restrict__ delta, int motion,
@@ -1216,7 +1216,7 @@ __device__ __forceinline__ void odom_increment(int j, const IcpState* __restrict
             ref_pose(prev2[j], n_frames, states, hist_T, Rb, tb);
             constant_velocity_increment(Rb, tb, Ra, ta, D);
         }
-    } else if (delta) {
+    } else if (delta && prev[j] >= 0) {
         for (int i = 0; i < 16; ++i) D[i] = delta[(size_t)prev[j] * 16 + i];
     }
 }
@@ -1226,7 +1226,8 @@ __device__ __forceinline__ void odom_increment(int j, const IcpState* __restrict
 // frame's prior is compose_prior(frame prev[j]'s pose, odom_increment); delta holds one entry per frame reference, or is
 // null.  kGyro (odom_start_gyro_kernel): the increment's rotation is the frame's gyro rotation G[9 f ..] instead, and
 // with tD the increment's translation goes to tD[3 j ..] and the frame's lever arm is zeroed, for
-// odom_deskew_gyro_kernel.
+// odom_deskew_gyro_kernel.  (prior map) A lane whose prev[j] < 0 runs its sequence's first frame from the state and
+// prior start_loop gave it, T_init: only its frame range is set.
 template <bool kGyro>
 __device__ __forceinline__ void odom_start(IcpState* states, const long long* __restrict__ seg, double* T_prior,
                                            int* cursor, int* first, unsigned int* n_active, int lanes, int step_first,
@@ -1239,7 +1240,7 @@ __device__ __forceinline__ void odom_start(IcpState* states, const long long* __
     if (j >= lanes) return;
     const int f = step_first + min(j, active);
     first[j] = f; cursor[j] = f;
-    if (j >= active) return;
+    if (j >= active || prev[j] < 0) return;
     double D[16], Ra[9], ta[3];
     odom_increment(j, states, prev, prev2, delta, motion, n_frames, hist_T, D);
     if (kGyro) {
@@ -1401,7 +1402,8 @@ __global__ void odom_gyro_kernel(se3::Gyro g, const double* __restrict__ smp, co
 }
 
 // Per step, after odom_start_gyro_kernel: odom_deskew_kernel with se3::deskew_point_gyro, the lane's increment
-// translation tD[3 j ..] and its frame's knot table; the lever arm is taken again the same way (kSource as there).
+// translation tD[3 j ..] and its frame's knot table; the lever arm is taken again the same way (kSource as there).  A
+// frame without knots (prior map: a sequence's first frame) is left as it is.
 template <bool kSource>
 __global__ void odom_deskew_gyro_kernel(float4* __restrict__ src, float4* __restrict__ sorted,
                                         const long long* __restrict__ seg, int step_first, int active, long long base,
@@ -1421,14 +1423,14 @@ __global__ void odom_deskew_gyro_kernel(float4* __restrict__ src, float4* __rest
         float o[3];
         float4 p = src[i];
         const float pi[3] = {p.x, p.y, p.z};
-        if (se3::deskew_point_gyro(K, nk, f[0], f[1], f[2], f[3], t, ts[i], pi, o)) {
+        if (nk > 0 && se3::deskew_point_gyro(K, nk, f[0], f[1], f[2], f[3], t, ts[i], pi, o)) {
             p.x = o[0]; p.y = o[1]; p.z = o[2];
             src[i] = p;
         }
         if (!kSource) return;
         float4 q = sorted[i];
         const float qi[3] = {q.x, q.y, q.z};
-        if (se3::deskew_point_gyro(K, nk, f[0], f[1], f[2], f[3], t, ts[seg[b] + __float_as_int(q.w)], qi, o)) {
+        if (nk > 0 && se3::deskew_point_gyro(K, nk, f[0], f[1], f[2], f[3], t, ts[seg[b] + __float_as_int(q.w)], qi, o)) {
             q.x = o[0]; q.y = o[1]; q.z = o[2];
             sorted[i] = q;
         }
@@ -1448,7 +1450,8 @@ __global__ void odom_deskew_gyro_kernel(float4* __restrict__ src, float4* __rest
 // stopped, is folded into its sequence's state, state[seq[j]], with the correction inv(T_prior) T_out, and the
 // sequence's next radius goes to lane_radius[next_lane[j]], the lane that runs the sequence at the next step (-1: none).
 // The lanes of a step keep their order into the next one, so next_lane[j] <= j is written by one thread and read by
-// none here.
+// none here.  (prior map) seq[j] < 0: the lane ran sequence ~seq[j]'s first frame, whose prior was the caller's guess,
+// not a prediction; its state is not folded.
 __global__ void odom_threshold_kernel(const IcpState* __restrict__ states, const double* __restrict__ T_prior,
                                       int step_first, int active, const int* __restrict__ seq,
                                       const int* __restrict__ next_lane, adaptive::Settings set, double ceiling,
@@ -1460,9 +1463,12 @@ __global__ void odom_threshold_kernel(const IcpState* __restrict__ states, const
     const double Ra[9] = {P[0], P[1], P[2], P[4], P[5], P[6], P[8], P[9], P[10]}, ta[3] = {P[3], P[7], P[11]};
     double D[16];
     constant_velocity_increment(Ra, ta, st->R, st->t, D);
-    adaptive::State x = state[seq[j]];
-    adaptive::fold(&x, adaptive::model_error(D, set.max_range), set.min_motion);
-    state[seq[j]] = x;
+    const int s = seq[j] < 0 ? ~seq[j] : seq[j];
+    adaptive::State x = state[s];
+    if (seq[j] >= 0) {
+        adaptive::fold(&x, adaptive::model_error(D, set.max_range), set.min_motion);
+        state[s] = x;
+    }
     if (next_lane[j] >= 0) lane_radius[next_lane[j]] = adaptive::radius(x, set.initial_threshold, ceiling);
 }
 
@@ -1569,6 +1575,8 @@ struct OdomSettings {
     // dcreg_set_lane_params on (at open, for a session): every sequence's settings [n_seqs], params being entry 0; off:
     // empty
     std::vector<dcreg_icp_params> lanes;
+    // (a session) dcreg_set_prior_map as it was at open; a one-shot call reads the context's
+    bool prior_map = false;
 };
 
 struct dcreg_ctx {
@@ -1674,6 +1682,9 @@ struct dcreg_ctx {
         std::vector<adaptive::State> thr_state;                        // [n_seqs]
         // (set.gyro) every sequence's last committed mid-sweep time (NaN: none yet, or pushed without frame times)
         std::vector<double> last_mid;                                  // [n_seqs]
+        // (set.prior_map) every sequence's dead-reckoned pose (T_init and the increments alone) of its last frame, the
+        // pose its next frame's points are sorted under
+        std::vector<double> dr_T;                                      // [n_seqs][16]
     };
     std::unique_ptr<OdomSession> odom;
     // the voxel filter (voxel_filter): table [slots] keys / first indices, [points] slots, [points + 1] flags and their
@@ -1719,6 +1730,9 @@ struct dcreg_ctx {
     // open).  A call's entries [lanes] (plan_iteration), an odometry step's device lane -> sequence [lanes], and the log
     // fill's device trial -> lane [trials]
     bool lane_params = false;
+    // dcreg_set_prior_map: odometry registers every frame against the context's target instead of a local map (a
+    // session keeps the value it had at open)
+    bool prior_map = false;
     DevBuf<dcreg_icp_params> d_lane_prm;
     DevBuf<int> d_lane_seq, d_trial_lane;
     DevBuf<float4> d_pair_tgt;                                   // targets, packed (w = global index)
@@ -2514,6 +2528,13 @@ int dcreg_set_map_input_voxel(dcreg_ctx* ctx, double voxel) {
         return DCREG_BAD_ARG;
     }
     ctx->map_input_voxel = voxel;
+    return DCREG_OK;
+}
+
+int dcreg_set_prior_map(dcreg_ctx* ctx, int enable) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (enable != 0 && enable != 1) { ctx->err = "set_prior_map: enable must be 0 or 1"; return DCREG_BAD_ARG; }
+    ctx->prior_map = enable == 1;
     return DCREG_OK;
 }
 
@@ -3736,11 +3757,17 @@ struct OdomCall {
     // the frames as the device gets them: the caller's, or the source filter's kept points (src_off: kept offsets)
     const float* src_xyz = xyz; int src_stride = stride; const int64_t* src_off = frame_offsets;
     std::vector<int64_t> kept;
-    // (dcreg_set_map_input_voxel) the frames' filter is the map-input filter F_in, whose kept points are the maps' input;
-    // split: a source filter F_s runs over them (voxel_filter_chain), and in_off (F_in's kept offsets) differs from
-    // src_off.  d_map_src: the points the maps and a session's window take, the packed sources or (split) d_odom_in
-    const bool split = set.map_input_voxel > 0.0 && set.source_voxel > 0.0;
-    const bool filtered = set.map_input_voxel > 0.0 || set.source_voxel > 0.0;
+    // (dcreg_set_prior_map) every frame registers against the context's target: no anchors, no maps (odom_plan.hpp)
+    const bool prior = sess ? set.prior_map : ctx->prior_map;
+    std::vector<double> next_dr;                    // (prior, sess) every sequence's dead-reckoned pose after the push
+    std::vector<double> first_r;                    // (prior, adaptive) the radii of step 0's lanes, from the host
+    // (dcreg_set_map_input_voxel, not read with a prior map) the frames' filter is the map-input filter F_in, whose
+    // kept points are the maps' input; split: a source filter F_s runs over them (voxel_filter_chain), and in_off
+    // (F_in's kept offsets) differs from src_off.  d_map_src: the points the maps and a session's window take, the
+    // packed sources or (split) d_odom_in
+    const double in_voxel = prior ? 0.0 : set.map_input_voxel;
+    const bool split = in_voxel > 0.0 && set.source_voxel > 0.0;
+    const bool filtered = in_voxel > 0.0 || set.source_voxel > 0.0;
     const int64_t* in_off = frame_offsets;
     std::vector<int64_t> in_kept;
     size_t in_ll = 0;                               // (split) where the map-input offsets are in d_odom_ll
@@ -3760,6 +3787,9 @@ struct OdomCall {
     // (sparse_maps) the plan of the steps whose maps are sparse row indexes, made at the first such step
     const bool sparse_maps = sess ? set.sparse_maps : ctx->sparse_maps;
     LoopPlan L_sparse; bool planned_sparse = false;
+    bool sparse = false;            // the step's grids are sparse row indexes (sparse_maps: a lane's box, or the step's
+                                    // boxes in all, too large for dense grids; prior: the target is one)
+    std::vector<int> lane_rings;    // (window, adaptive) the step's lanes' rings
     const double map_spacing = sess ? set.map_spacing : ctx->map_spacing;   // the map filter's minimum spacing
     int failed = -1;                                // the step whose maps failed (-1: none)
     // (voxel map) where every sequence's map is: the session's maps before the first update, then each update's output
@@ -3775,6 +3805,8 @@ struct OdomCall {
     long long gyro_knots = 0;
 
     int check(), check_gyro(), upload(), start(), step(int i), finish();
+    int prior_grids(int i), window_grids(int i), step_run(int i);
+    const char* prior_error() const;
     int build_map(const odom_plan::MapInput& in, const long long* ll, const int* ints, DevBuf<float4>& out, StepMap* sm);
 
     // the sequence of the caller's frame k
@@ -3891,7 +3923,8 @@ int OdomCall::check() {
     c.offsets = frame_offsets; c.item = "frame"; c.stride = stride; c.own_cell = true; c.cell_size = set.cell_size;
     c.need_target = false; c.one_iteration = true; c.n_seqs = n_seqs; c.seq_offsets = seq_offsets;
     c.empty_seqs = sess != nullptr;
-    c.own_msg = odometry_settings_error(set, deltas != nullptr);
+    c.own_msg = prior ? prior_error() : nullptr;
+    if (!c.own_msg) c.own_msg = odometry_settings_error(set, deltas != nullptr);
     c.lanes = (int)set.lanes.size();
     int rc = check_batch_call(ctx, set.lanes.empty() ? params : set.lanes.data(), c);
     if (rc) return rc;
@@ -3918,8 +3951,8 @@ int OdomCall::check() {
             rc = voxel_filter_chain(ctx, n_frames, xyz, frame_offsets, stride, set.map_input_voxel, set.source_voxel,
                                     set.source_max_points, timestamps != nullptr, in_kept.data(), bad_in.data(),
                                     kept.data(), bad.data());
-        } else if (set.map_input_voxel > 0.0) {     // F_s = none: the source is F_in(frame)
-            rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, set.map_input_voxel, 1, 0.0,
+        } else if (in_voxel > 0.0) {                // F_s = none: the source is F_in(frame)
+            rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, in_voxel, 1, 0.0,
                                    timestamps != nullptr, false, kept.data(), bad.data());
         } else {
             rc = voxel_filter_host(ctx, n_frames, xyz, frame_offsets, stride, set.source_voxel, set.source_max_points,
@@ -3935,7 +3968,7 @@ int OdomCall::check() {
         for (int s = 0; s < n_seqs; ++s)
             for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k) {
                 std::string w = split ? why(in_kept, bad_in, k, true) : std::string();
-                if (w.empty()) w = why(kept, bad, k, set.map_input_voxel > 0.0 && !split);
+                if (w.empty()) w = why(kept, bad, k, in_voxel > 0.0 && !split);
                 if (!w.empty()) {
                     ctx->err = std::string(name) + ": " + frame_name(s, k) + ": " + w;
                     return DCREG_BAD_ARG;
@@ -3947,6 +3980,16 @@ int OdomCall::check() {
     if (frame_points)
         for (int k = 0; k < n_frames; ++k) frame_points[k] = src_off[k + 1] - src_off[k];
     return DCREG_OK;
+}
+
+// (prior) What the prior map refuses, or null: the voxel map, a context without a target, a cell size other than the
+// target's, and a sharded context
+const char* OdomCall::prior_error() const {
+    if (set.voxel_map) return "the prior map (dcreg_set_prior_map) registers against the target: no voxel map (map_frames >= 1)";
+    if (!ctx->has_grid) return "the prior map (dcreg_set_prior_map) needs a target (dcreg_set_target)";
+    if (set.cell_size != ctx->cell_size) return "with the prior map (dcreg_set_prior_map) cell_size must be the target's";
+    if (ctx->comm) return "the prior map (dcreg_set_prior_map) does not run on a sharded context";
+    return nullptr;
 }
 
 // (gyro) The frame times and samples, before anything is launched: the samples finite and strictly ascending in time
@@ -4027,8 +4070,8 @@ int OdomCall::upload() {
     int rc;
     {
         const std::string why = odom_plan::make_push(n_seqs, seq_offsets, n_frames, src_off,
-                                                     set.voxel_map ? 0 : set.map_frames, arena_plan::kMaxPoints, hist, &U,
-                                                     split ? in_off : nullptr);
+                                                     set.voxel_map || prior ? 0 : set.map_frames, arena_plan::kMaxPoints,
+                                                     hist, &U, split ? in_off : nullptr, prior);
         if (!why.empty()) { ctx->err = std::string(name) + ": " + why; return DCREG_BAD_ARG; }
     }
     const int n_steps = (int)P.steps.size();
@@ -4036,14 +4079,14 @@ int OdomCall::upload() {
     std::vector<long long> hll;
     std::vector<int> hint;
     at_ll.assign((size_t)n_steps, 0); at_int.assign((size_t)n_steps, 0);
-    for (int i = 1; i < n_steps; ++i) {
+    for (int i = prior ? 0 : 1; i < n_steps; ++i) {
         const odom_plan::Step& st = P.steps[(size_t)i];
         at_ll[(size_t)i] = hll.size(); at_int[(size_t)i] = hint.size();
         odom_plan::pack(st.map, hll, hint);
         hint.insert(hint.end(), st.prev.begin(), st.prev.end());
         hint.insert(hint.end(), st.prev2.begin(), st.prev2.end());
-        if (set.adaptive) {     // lane j's sequence, and the lane that runs it at the next step
-            hint.insert(hint.end(), st.seq.begin(), st.seq.end());
+        if (set.adaptive) {     // lane j's sequence (~ it: a first frame), and the lane that runs it at the next step
+            for (int j = 0; j < st.active; ++j) hint.push_back(st.prev[(size_t)j] < 0 ? ~st.seq[(size_t)j] : st.seq[(size_t)j]);
             for (int s : st.seq) {
                 int next = -1;
                 if (i + 1 < n_steps) {
@@ -4099,15 +4142,22 @@ int OdomCall::upload() {
     }
     // the frames in device order, each sorted by its own cell in the sensor frame (identity poses, a box of 1024^3 cells
     // around the sensor: locality only, the chained priors are not known yet); lanes: grid y of the loop kernel, a
-    // lane's frame range set by odom_start_kernel at every step; grids: the step's local maps
+    // lane's frame range set by odom_start_kernel at every step; grids: the step's local maps.  (prior) Sorted as
+    // dcreg_icp_run_sequences sorts them, in the target's cells under their dead-reckoned poses (start()); grids: the
+    // target with each lane's rings
     S = Batch{n_frames, src_xyz, src_stride, P.dev_off.data()};
     S.order = P.input.data(); S.in_off = src_off;
     if (filtered) S.kind = cudaMemcpyDeviceToDevice;
-    S.sort = Batch::kBox;
-    S.sort_box.inv_cell = 1.0 / set.cell_size;
-    S.sort_box.ox = S.sort_box.oy = S.sort_box.oz = -512;
-    S.sort_box.nx = S.sort_box.ny = S.sort_box.nz = 1024;
-    S.sort_cells = 1ll << 30;
+    if (prior) {
+        S.sparse = ctx->grid.dense == corr::kSparseGrid;
+        CK(ctx->odom_maps.d_grids.ensure(n_seqs));
+    } else {
+        S.sort = Batch::kBox;
+        S.sort_box.inv_cell = 1.0 / set.cell_size;
+        S.sort_box.ox = S.sort_box.oy = S.sort_box.oz = -512;
+        S.sort_box.nx = S.sort_box.ny = S.sort_box.nz = 1024;
+        S.sort_cells = 1ll << 30;
+    }
     S.grid_table = true; S.cell_size = set.cell_size;
     S.lanes = n_seqs;
     if ((rc = stage_sources(ctx, S)) || (rc = stage_lanes(ctx, n_seqs, n_frames, &S.seq))) return rc;
@@ -4117,7 +4167,8 @@ int OdomCall::upload() {
     CK(ctx->d_odom_ll.ensure(std::max<long long>((long long)hll.size(), 1)));
     CK(ctx->d_odom_int.ensure(std::max<long long>((long long)hint.size(), 1)));
     CK(ctx->d_odom_map.ensure(std::max<long long>(P.max_map, 1)));
-    if (set.map_voxel > 0.0 && !set.voxel_map) {   // the maps' filter at its largest step: no regrowth inside the loop
+    if (set.map_voxel > 0.0 && !set.voxel_map && !prior) {  // the maps' filter at its largest step: no regrowth inside
+                                                              // the loop
         CK(ctx->d_vmap[0].ensure(std::max<long long>(P.max_map, 1)));
         long long slots = 0;
         std::vector<long long> tab;
@@ -4169,9 +4220,30 @@ int OdomCall::start() {
     for (int s = 0; s < n_seqs; ++s)
         for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k)
             memcpy(&T_dev[(size_t)P.dev[(size_t)k] * 16], &set.T_init[(size_t)s * 16], 16 * sizeof(double));
-    for (int d = 0; d < n_frames; ++d)
-        for (int c4 = 0; c4 < 4; ++c4) ident[(size_t)d * 16 + 5 * c4] = 1.0;
-    CK(cudaMemcpyAsync(ctx->d_seq_prior, ident.data(), ident.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    if (prior) {    // frame k's dead-reckoned pose: T_init (a sequence's first frame), then compose_prior with D_{k-1}
+        static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+        const bool inc = set.motion == DCREG_MOTION_INCREMENTS;
+        if (sess) next_dr = sess->dr_T;
+        for (int s = 0; s < n_seqs; ++s)
+            for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k) {
+                double* T = &T_dev[(size_t)P.dev[(size_t)k] * 16];
+                const bool first = k == seq_offsets[s] && hist.seen.at((size_t)s) == 0;
+                if (!first) {
+                    const double* A = k > seq_offsets[s] ? &T_dev[(size_t)P.dev[(size_t)(k - 1)] * 16] : &sess->dr_T[(size_t)s * 16];
+                    const double* D = !inc ? kIdentity
+                                      : k > seq_offsets[s] ? (deltas ? deltas + (size_t)(k - 1) * 16 : kIdentity)
+                                                           : &sess->last_delta[(size_t)s * 16];
+                    const double R[9] = {A[0], A[1], A[2], A[4], A[5], A[6], A[8], A[9], A[10]}, t[3] = {A[3], A[7], A[11]};
+                    compose_prior(R, t, D, T);
+                }
+                if (sess && k + 1 == seq_offsets[s + 1]) memcpy(&next_dr[(size_t)s * 16], T, 16 * sizeof(double));
+            }
+    } else {
+        for (int d = 0; d < n_frames; ++d)
+            for (int c4 = 0; c4 < 4; ++c4) ident[(size_t)d * 16 + 5 * c4] = 1.0;
+        CK(cudaMemcpyAsync(ctx->d_seq_prior, ident.data(), ident.size() * sizeof(double), cudaMemcpyHostToDevice,
+                           ctx->stream));
+    }
     if ((rc = start_loop(ctx, n_frames, T_dev.data(), R, &S, &dlog, &src_iter))) return rc;
     const long long n_points = P.dev_off[(size_t)n_frames], n_map_points = P.map_off[(size_t)n_frames];
     const long long* d_map_seg = ctx->d_odom_ll + in_ll;
@@ -4228,13 +4300,15 @@ int OdomCall::start() {
         if (sess) d_old = sess->win[sess->cur];
     }
     frame_radius.assign((size_t)n_frames, 0.0);
-    if (set.adaptive) {         // the sequences' committed states, and the radii step 1's lanes register with
+    if (set.adaptive) {         // the sequences' committed states, and the radii step 1's (prior: step 0's) lanes use
         const std::vector<adaptive::State> h =
             sess ? sess->thr_state : std::vector<adaptive::State>((size_t)n_seqs, adaptive::State{0.0, 0});
         std::vector<double> r;
-        if (P.steps.size() > 1)
-            for (int s : P.steps[1].seq)
+        const size_t i0 = prior ? 0 : 1;
+        if (P.steps.size() > i0)
+            for (int s : P.steps[i0].seq)
                 r.push_back(adaptive::radius(h[(size_t)s], set.threshold.initial_threshold, params->search_radius));
+        if (prior) first_r = r;
         CK(ctx->d_thr_state.ensure(n_seqs));
         CK(ctx->d_lane_radius.ensure(n_seqs));
         CK(cudaMemcpyAsync(ctx->d_thr_state, h.data(), h.size() * sizeof(adaptive::State), cudaMemcpyHostToDevice, ctx->stream));
@@ -4244,13 +4318,45 @@ int OdomCall::start() {
     return DCREG_OK;
 }
 
-// Step i >= 1; when its maps fail, ctx->err names the frame, `failed` the step, and nothing of it runs
+// Step i >= 1 (prior: i >= 0); when its maps fail, ctx->err names the frame, `failed` the step, and nothing of it runs
 int OdomCall::step(int i) {
     const odom_plan::Step& st = P.steps[(size_t)i];
     int rc;
+    if (prior && (rc = prior_grids(i))) return rc;
+    else if (!prior && (rc = window_grids(i))) return rc;
+    if (failed >= 0) return DCREG_OK;
     // 1. the lanes' local maps from the window frames' device-resident results and the retained frames, or (voxel map)
     // one update: every lane's map becomes its previous one with frame k-1 inserted at its pose, capped and pruned (with
     // a session, every other sequence's map is carried along); then the map filter, if any
+    return step_run(i);
+}
+
+// (prior) The step's grid table: the context's target with the rings of each lane's radius; with the adaptive threshold
+// the radii of step i >= 1 come back first (the step's one sync; step 0's are start()'s), else the table is the same at
+// every step and goes up once
+int OdomCall::prior_grids(int i) {
+    const odom_plan::Step& st = P.steps[(size_t)i];
+    std::vector<double> lane_r((size_t)st.active, params->search_radius);
+    if (set.adaptive && i == 0) {
+        lane_r = first_r;
+    } else if (set.adaptive) {
+        CK(cudaMemcpyAsync(lane_r.data(), ctx->d_lane_radius, lane_r.size() * sizeof(double), cudaMemcpyDeviceToHost,
+                           ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    sparse = ctx->grid.dense == corr::kSparseGrid;
+    for (int j = 0; j < st.active; ++j) frame_radius[(size_t)P.input[(size_t)(st.first + j)]] = lane_r[(size_t)j];
+    if (!set.adaptive && planned + planned_sparse > 0) return DCREG_OK;
+    std::vector<corr::Grid> g((size_t)st.active, ctx->grid);
+    for (int j = 0; j < st.active; ++j) g[(size_t)j].rings = std::max(1, search_rings(lane_r[(size_t)j], set.cell_size));
+    CK(cudaMemcpyAsync(ctx->odom_maps.d_grids, g.data(), g.size() * sizeof(corr::Grid), cudaMemcpyHostToDevice, ctx->stream));
+    return DCREG_OK;
+}
+
+// (window, voxel map) The step's maps and their grids; when the maps fail, ctx->err names the frame and `failed` the step
+int OdomCall::window_grids(int i) {
+    const odom_plan::Step& st = P.steps[(size_t)i];
+    int rc;
     odom_plan::MapInput update;
     const odom_plan::MapInput& in = set.voxel_map ? update : st.map;
     if (set.voxel_map) odom_plan::map_step(P, i, sess != nullptr, MS, &update);
@@ -4264,13 +4370,13 @@ int OdomCall::step(int i) {
     // which the last step's threshold kernel left, ride the same copy; each lane's grid gets its own ring count
     const double inv_cell = 1.0 / set.cell_size;
     std::vector<double> lane_r((size_t)st.active, params->search_radius);
-    std::vector<int> lane_rings;
+    lane_rings.clear();
     if (set.adaptive) sm.more.push_back(Readback{ctx->d_lane_radius.p, lane_r.size() * sizeof(double), lane_r.data()});
     std::vector<int> hb;
     std::vector<arena_plan::Box> boxes;
     long long cells = 0;
     std::string plan_why;
-    bool sparse = false;            // (sparse_maps) a lane's box, or the step's boxes in all, too large for dense grids
+    sparse = false;
     if (sm.map) {
         if ((rc = arena_bounds(ctx, ctx->odom_maps, sm.map, in.seg.data(), sm.d_seg, st.active, inv_cell, hb, sm.more)))
             return rc;
@@ -4309,6 +4415,13 @@ int OdomCall::step(int i) {
                                 set.adaptive ? lane_rings.data() : nullptr))) {
         return rc;
     }
+    return DCREG_OK;
+}
+
+// Step i's frames, after its grids: their priors, deskew, the loop, and (adaptive) the threshold states
+int OdomCall::step_run(int i) {
+    const odom_plan::Step& st = P.steps[(size_t)i];
+    int rc;
     // 3. every lane's frame of this step: its prior and a fresh loop state
     const int* d_prev = ctx->d_odom_int + at_int[(size_t)i] + st.map.piece_frame.size() + st.map.center.size();
     const int* d_prev2 = d_prev + st.active;
@@ -4323,8 +4436,9 @@ int OdomCall::step(int i) {
             st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T);
     ctx->launches++;
     CK(cudaGetLastError());
-    // 3b. (timestamps) the step's frames deskewed with the increments their priors used, outside the loop's graphs
-    if (timestamps && set.gyro) {
+    // 3b. (timestamps) the step's frames deskewed with the increments their priors used, outside the loop's graphs.
+    // (gyro) A push without gyro input holds first frames alone (check_gyro), which are not deskewed: no knot table
+    if (timestamps && set.gyro && gi.samples) {
         const long long a = P.dev_off[(size_t)st.first], np = P.dev_off[(size_t)(st.first + st.active)] - a;
         const long long* d_knot_off = ctx->d_odom_ll + gyro_ll;
         odom_deskew_gyro_kernel<true><<<(unsigned)((np + 255) / 256), 256, 0, ctx->stream>>>(
@@ -4332,7 +4446,7 @@ int OdomCall::step(int i) {
             ctx->d_gyro_ft, d_knot_off, ctx->d_gyro_knots, ctx->d_odom_xi, ctx->d_scan_radius);
         ctx->launches++;
         CK(cudaGetLastError());
-    } else if (timestamps) {
+    } else if (timestamps && !set.gyro) {
         odom_twist_kernel<<<(unsigned)((st.active + 127) / 128), 128, 0, ctx->stream>>>(
             ctx->d_state, st.first, st.active, d_prev, d_prev2, d_delta, set.motion, n_frames, d_hist_T,
             ctx->d_odom_xi, ctx->d_scan_radius);
@@ -4457,6 +4571,7 @@ int OdomCall::finish() {
         if (set.gyro)
             for (int s = 0; s < n_seqs; ++s)
                 if (seq_offsets[s + 1] > seq_offsets[s]) sess->last_mid[(size_t)s] = next_mid[(size_t)s];
+        if (prior) sess->dr_T.swap(next_dr);
     }
     return DCREG_OK;
 }
@@ -4476,7 +4591,7 @@ static int run_odometry(dcreg_ctx* ctx, const char* name, const OdomSettings& se
                frame_points, deskewed_xyz, search_radius, gi};
     int rc;
     if ((rc = o.check()) || (rc = o.upload()) || (rc = o.start())) return rc;
-    for (int i = 1; i < (int)o.P.steps.size() && o.failed < 0; ++i)
+    for (int i = o.prior ? 0 : 1; i < (int)o.P.steps.size() && o.failed < 0; ++i)
         if ((rc = o.step(i))) return rc;
     return o.finish();
 }
@@ -4651,11 +4766,17 @@ static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     ss->set.sparse_maps = ctx->sparse_maps;
     ss->set.map_spacing = ctx->map_spacing;
     ss->set.map_input_voxel = ctx->map_input_voxel;
+    ss->set.prior_map = ctx->prior_map;
     const int n_seqs = set.n_seqs;
     BatchCheck c{name, !ss->set.T_init.empty(), "null pointer or n_seqs <= 0",
                  "sequences are independent - give each rank its own, do not shard them", n_seqs};
     c.own_cell = true; c.cell_size = set.cell_size; c.need_target = false; c.one_iteration = true;
-    c.own_msg = odometry_settings_error(ss->set, false);
+    if (ss->set.prior_map && set.voxel_map)
+        c.own_msg = "the prior map (dcreg_set_prior_map) registers against the target: no voxel map (map_frames >= 1)";
+    else if (ss->set.prior_map && ctx->comm)
+        c.own_msg = "the prior map (dcreg_set_prior_map) does not run on a sharded context";
+    else
+        c.own_msg = odometry_settings_error(ss->set, false);
     c.lanes = (int)ss->set.lanes.size();
     const int rc = check_batch_call(ctx, ss->set.lanes.empty() ? &ss->set.params : ss->set.lanes.data(), c);
     if (rc) return rc;
@@ -4663,6 +4784,7 @@ static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     ss->map_off.assign((size_t)n_seqs + 1, 0);
     ss->thr_state.assign((size_t)n_seqs, adaptive::State{0.0, 0});
     ss->last_mid.assign((size_t)n_seqs, NAN);
+    if (ss->set.prior_map) ss->dr_T = ss->set.T_init;
     ss->last_delta.assign((size_t)n_seqs * 16, 0.0);
     for (int s = 0; s < n_seqs; ++s)
         for (int c4 = 0; c4 < 4; ++c4) ss->last_delta[(size_t)s * 16 + 5 * c4] = 1.0;
@@ -4716,6 +4838,10 @@ int dcreg_odometry_local_map(dcreg_ctx* ctx, int seq, float* xyz, int64_t cap, i
     if (!ctx) return DCREG_BAD_ARG;
     if (!ctx->odom) { ctx->err = "odometry_local_map: no session is open (dcreg_odometry_open_map)"; return DCREG_BAD_ARG; }
     const dcreg_ctx::OdomSession& ss = *ctx->odom;
+    if (ss.set.prior_map) {
+        ctx->err = "odometry_local_map: the session registers against the prior map (dcreg_set_prior_map): no local map";
+        return DCREG_BAD_ARG;
+    }
     if (!ss.set.voxel_map) {
         ctx->err = "odometry_local_map: the session keeps a window of frames, not a voxel map (dcreg_odometry_open_map)";
         return DCREG_BAD_ARG;

@@ -12,8 +12,11 @@
 // A frame has two point ranges in device order: the points it registers with (Plan::dev_off, the loop's segments) and
 // the points it gives the maps (Plan::map_off, the map input's pieces and a session's window).  They are one table
 // unless dcreg_set_map_input_voxel splits them: then a frame's map input is F_in(frame), its source F_s(F_in(frame)).
-// Everything here is plain C++ so tests/test_odom_plan.py, tests/test_odom_session_plan.py and
-// tests/test_odom_map_plan.py can check it on the CPU (tools/test_odom_*plan.cpp).
+// With a prior map (dcreg_set_prior_map) there are no anchors and no maps: every frame registers against the context's
+// target, step 0 holds every sequence's first frame in the push, a prev of -1 means "start from T_init", and the
+// history keeps poses alone (make_push with prior = true and map_frames = 0).
+// Everything here is plain C++ so tests/test_odom_plan.py, tests/test_odom_session_plan.py,
+// tests/test_odom_map_plan.py and tests/test_odom_prior_plan.py can check it on the CPU (tools/test_odom_*plan.cpp).
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -53,7 +56,8 @@ struct Step {
     int first = 0;                      // device index of the step's first frame; lane j runs first + j
     int active = 0;                     // lanes: the sequences with a frame at this step
     std::vector<int> seq;               // [active] sequence of lane j
-    std::vector<int> prev, prev2;       // [active] device index of frame k - 1, and of k - 2 (-1: k - 1 is the anchor)
+    std::vector<int> prev, prev2;       // [active] device index of frame k - 1, and of k - 2 (-1: k - 1 is the anchor;
+                                        // prior map: prev -1, frame k is its sequence's first and starts from T_init)
     MapInput map;                       // the lanes' window maps, one segment per lane (the voxel map: none)
 };
 
@@ -62,7 +66,7 @@ struct Plan {
     std::vector<int> input;             // [n_frames] input frame of device index d
     std::vector<int64_t> dev_off;       // [n_frames + 1] point offsets of the frames in device order
     std::vector<int64_t> map_off;       // [n_frames + 1] ... of their map-input points (dev_off's values when not split)
-    std::vector<Step> steps;            // steps[0]: the anchors (no map)
+    std::vector<Step> steps;            // steps[0]: the anchors (no map; prior map: registered like every step)
     long long max_map = 0;              // the most map points of one step
     int max_pieces = 0;                 // the most window frames of one step
 };
@@ -99,14 +103,16 @@ inline int retained_frames(long long seen, int map_frames) {
 // seq_off: n_seqs + 1 non-decreasing frame offsets of the pushed frames (a sequence may have none), frame_off: n_frames
 // + 1 point offsets, both validated; h: the history before the push.  map_frame_off: n_frames + 1 offsets of the
 // frames' map-input points (null: frame_off, the points they register with).  Fails (returns the reason) when the maps
-// of one step hold more than max_points points.
+// of one step hold more than max_points points.  prior (with map_frames = 0): no anchors, as described at the top.
 inline std::string make_push(int n_seqs, const int* seq_off, int n_frames, const int64_t* frame_off, int map_frames,
-                             long long max_points, const History& h, Push* out, const int64_t* map_frame_off = nullptr) {
+                             long long max_points, const History& h, Push* out, const int64_t* map_frame_off = nullptr,
+                             bool prior = false) {
     Push& u = *out;
     u = Push{};
     Plan& p = u.plan;
     // sequence s's pushed frame j is its frame seen[s] + j, at step j (a new sequence: j = 0 is its anchor) or j + 1
-    auto step_of = [&](int s, int j) { return h.seen[(size_t)s] > 0 ? j + 1 : j; };
+    // (prior map: at step j)
+    auto step_of = [&](int s, int j) { return !prior && h.seen[(size_t)s] > 0 ? j + 1 : j; };
     int n_steps = 0;
     for (int s = 0; s < n_seqs; ++s)
         if (seq_off[s + 1] > seq_off[s]) n_steps = std::max(n_steps, step_of(s, seq_off[s + 1] - seq_off[s] - 1) + 1);
@@ -146,12 +152,12 @@ inline std::string make_push(int n_seqs, const int* seq_off, int n_frames, const
     };
     auto points = [&](int r) { return r < n_frames ? p.map_off[(size_t)r + 1] - p.map_off[(size_t)r] : h.n[(size_t)(r - n_frames)]; };
     auto first_point = [&](int r) { return r < n_frames ? p.map_off[(size_t)r] : h.at[(size_t)(r - n_frames)]; };
-    for (int i = 1; i < n_steps; ++i) {
+    for (int i = prior ? 0 : 1; i < n_steps; ++i) {
         Step& st = p.steps[(size_t)i];
         for (int j = 0; j < st.active; ++j) {
             const int s = st.seq[(size_t)j];
             const long long k = h.seen[(size_t)s] + (i - step_of(s, 0));
-            st.prev.push_back(ref(s, k - 1));
+            st.prev.push_back(k > 0 ? ref(s, k - 1) : -1);
             st.prev2.push_back(k - 1 > 0 ? ref(s, k - 2) : -1);
             for (long long w = std::max<long long>(0, k - map_frames); w < k; ++w) {
                 const int r = ref(s, w);

@@ -226,6 +226,44 @@ int dcreg_set_map_spacing(dcreg_ctx* ctx, double min_spacing);
  * and frame, a frame with no finite point left by the map-input filter or a voxel coordinate of that filter outside
  * [-2^20, 2^20).  A push that fails commits nothing. */
 int dcreg_set_map_input_voxel(dcreg_ctx* ctx, double voxel);
+/* Localisation in a prior map through the odometry front end: with enable = 1, dcreg_icp_run_odometry, _voxel,
+ * _voxel_n, _deskew, _adaptive and _gyro (map_frames >= 1), and sessions from dcreg_odometry_open, _open_adaptive and
+ * _open_gyro with every _push* onto them, register every frame against the context's target (dcreg_set_target: a dense
+ * grid or a sparse row index) instead of a local map.  0 (the default): every call keeps its launches and bytes.
+ * - No anchors.  A sequence's first frame registers from T_prior = T_init[s], as in dcreg_icp_run_sequences, with real
+ *   iterations, status, covariance and log.  Every later frame k starts from compose_prior(T_out[k-1], D_k):
+ *   DCREG_MOTION_INCREMENTS: D_k = deltas[k-1] (NULL: the identity); DCREG_MOTION_CONSTANT_VELOCITY: the identity for
+ *   the second frame, then constant_velocity_increment(T_out[k-2], T_out[k-1]); gyro input: [G(tm_{k-1} -> tm_k) | t_D].
+ *   The first frame plays the anchor's part in the motion model: nothing is known of the motion before it.
+ * - A sequence's first frame is not deskewed, in every motion mode; later frames are, by the call's rule, when
+ *   timestamps are given.  The source filter F_s applies as always: filter first, then deskew.
+ * - Adaptive threshold: a sequence starts at (sse, n) = (0, 0), so its first frame registers at
+ *   min(3 initial_threshold, search_radius); the first frame does not update the state (its prior is the caller's
+ *   guess, not a prediction), every later frame does.
+ * - Target: cell_size must equal the target's cell size, and search_radius / cell_size must lie in (0, 4].  Frame k
+ *   returns what dcreg_set_source(F_s(frame k), deskewed) + dcreg_icp_run(T_prior[k]) returns on the target, up to how
+ *   the FP64 partial sums are grouped: counts, masks, iteration counts and status identical, poses equal to rounding.
+ *   The frames are sorted as dcreg_icp_run_sequences sorts them (in the target's cells, under T_init and the increments
+ *   alone), so with increments and no filter or timestamps a call returns _sequences' bytes.  A call reproduces bit
+ *   for bit.
+ * - Not read: map_frames (still checked >= 1), map_voxel, map_max_points, dcreg_set_map_spacing,
+ *   dcreg_set_map_input_voxel and dcreg_set_sparse_maps.  deskewed_xyz, frame_points, search_radius, T_prior and cov
+ *   keep their meaning.
+ * - Sessions record the setting at open.  A session keeps per sequence two poses, the dead-reckoned pose its next
+ *   frame is sorted under, the last increment and the last mid-sweep time, and no points; any chunking of a recording
+ *   gives one call's bytes (deskewed_xyz and search_radius included) as long as the target stays the same.  A push reads
+ *   the context's target at push time, so a caller may swap map tiles between pushes with dcreg_set_target: the one
+ *   exception to "other calls between pushes do not change a session's results".  A push leaves the context's source
+ *   and target as they were.
+ * - Cost: a step has no map-building launch: the start kernel, the deskew (one or two launches with timestamps), the
+ *   loop's chunks and, adaptive, the threshold kernel.  Without the adaptive threshold a step has no host sync besides
+ *   the loop's peeks; with it, one at every step after the first (the lanes' radii, for their search rings).
+ *   Neither depends on the number of sequences.
+ * Errors (DCREG_BAD_ARG, naming the prior map, before any launch): enable other than 0 or 1; at a call or push, no
+ * target, a cell_size other than the target's; the voxel-map forms (dcreg_icp_run_odometry_map,
+ * dcreg_odometry_open_map, and _adaptive / _gyro / _open_adaptive / _open_gyro with map_frames = 0); a sharded context;
+ * dcreg_odometry_local_map on a prior-map session.  A push that fails commits nothing. */
+int dcreg_set_prior_map(dcreg_ctx* ctx, int enable);
 
 /* ---- seam 1: correspondence stage (icp_test_runner.cpp:1714-1813) -------------------------
  * For every source slot: q = fl32(R p + t), exact 5-NN in the target, 5th d^2 < radius^2,
