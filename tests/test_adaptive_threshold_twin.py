@@ -1,7 +1,7 @@
 """The adaptive threshold of scan-to-map odometry (dcreg_icp_run_odometry_adaptive) on the CPU: the NumPy twin
 (api.adaptive_threshold_*) against a literal per-frame reading of KISS-ICP's AdaptiveThreshold, its error against a
-50-digit evaluation, the sample rule at min_motion, poses that are not finite, the radius rule, and
-dcreg_b200/csrc/adaptive_threshold.cuh built as host C++ against the twin."""
+50-digit evaluation (oracle/dcreg_oracle_motion_mp.py), the sample rule at min_motion, poses that are not finite, the
+radius rule, and dcreg_b200/csrc/adaptive_threshold.cuh built as host C++ against the twin."""
 import math
 import subprocess
 
@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from dcreg_b200 import api
+from dcreg_oracle_motion_mp import mp_model_error
 from harness import tool_program
 
 INIT, MIN_MOTION, MAX_RANGE, CEILING = 2.0, 0.1, 100.0, 2.0
@@ -88,21 +89,8 @@ def test_error_against_50_digits(theta):
         for j in range(3):
             T[i, j] = float((1 if i == j else 0) * c + s * K[i][j] + (1 - c) * a[i] * a[j])
     T[:3, 3] = [0.3, -0.2, 0.05]
-    # reference: the angle of the ROUNDED matrix through its quaternion (Shepperd's well-conditioned branch) in 50 digits
-    R = [[mp.mpf(float(T[i, j])) for j in range(3)] for i in range(3)]
-    tr = R[0][0] + R[1][1] + R[2][2]
-    if tr > 0:
-        w = mp.sqrt(tr + 1) / 2
-        vx, vy, vz = (R[2][1] - R[1][2]) / (4 * w), (R[0][2] - R[2][0]) / (4 * w), (R[1][0] - R[0][1]) / (4 * w)
-    else:
-        i = max(range(3), key=lambda d: R[d][d])
-        j, k = (i + 1) % 3, (i + 2) % 3
-        vi = mp.sqrt(R[i][i] - R[j][j] - R[k][k] + 1) / 2
-        w = abs(R[k][j] - R[j][k]) / (4 * vi)
-        vx, vy, vz = vi, (R[j][i] + R[i][j]) / (4 * vi), (R[k][i] + R[i][k]) / (4 * vi)
-    th = 2 * mp.atan2(mp.sqrt(vx * vx + vy * vy + vz * vz), w)
-    t = [mp.mpf(float(x)) for x in T[:3, 3]]
-    want = 2 * mp.mpf(MAX_RANGE) * mp.sin(th / 2) + mp.sqrt(sum(x * x for x in t))
+    # reference: the error of the ROUNDED matrix, its angle through Shepperd's quaternion, in 50 digits
+    want = mp_model_error(T.reshape(-1), MAX_RANGE)
     got = api.adaptive_threshold_error(np.eye(4), T, MAX_RANGE)
     # a few FP64 roundings of |v| and w, times the 200 m that turn half the angle into metres
     assert abs(mp.mpf(got) - want) <= mp.mpf(2e-13), (theta, got, float(want))

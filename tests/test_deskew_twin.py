@@ -1,5 +1,5 @@
 """The NumPy twin of the odometry's motion compensation (api.se3_log / se3_exp / deskew_points) on the CPU: against a
-50-digit mpmath evaluation of the same maps, its exact-copy rules, and the geometry of make_parking_sweeps (a sign or
+50-digit mpmath evaluation of the same maps (oracle/dcreg_oracle_motion_mp.py), its exact-copy rules, and the geometry of make_parking_sweeps (a sign or
 direction error that device-vs-twin parity cannot catch)."""
 import math
 
@@ -9,75 +9,10 @@ import pytest
 
 from dcreg_b200 import api
 from dcreg_b200.scenes import make_parking_sweeps
+from dcreg_oracle_motion_mp import mp_exp, mp_exp_apply, mp_log
 
 mp.mp.dps = 50
 THETAS = [0.0, 1e-12, 1e-6, 0.1, 1.0, math.pi - 1e-6]
-
-
-def mp_cross(a, b):
-    return [a[1] * b[2] - a[2] * b[1], a[2] * b[0] - a[0] * b[2], a[0] * b[1] - a[1] * b[0]]
-
-
-def mp_exp_coeffs(theta):
-    if theta == 0:
-        return mp.mpf(1), mp.mpf(1) / 2, mp.mpf(1) / 6
-    return mp.sin(theta) / theta, (1 - mp.cos(theta)) / theta ** 2, (theta - mp.sin(theta)) / theta ** 3
-
-
-def mp_exp_apply(xi, s, p):
-    """Exp(s xi) p in 50 digits"""
-    rho = [s * x for x in xi[:3]]
-    phi = [s * x for x in xi[3:]]
-    A, B, C = mp_exp_coeffs(mp.sqrt(sum(x * x for x in phi)))
-    a = mp_cross(phi, p)
-    c = mp_cross(phi, rho)
-    b, d = mp_cross(phi, a), mp_cross(phi, c)
-    return [p[r] + A * a[r] + B * b[r] + rho[r] + B * c[r] + C * d[r] for r in range(3)]
-
-
-def mp_exp(xi):
-    """Exp(xi) as a 4x4 of mpf"""
-    T = [[mp.mpf(int(r == c)) for c in range(4)] for r in range(4)]
-    for c in range(3):
-        e = [mp.mpf(int(r == c)) for r in range(3)]
-        col = mp_exp_apply(xi, 1, e)
-        t0 = mp_exp_apply(xi, 1, [mp.mpf(0)] * 3)
-        for r in range(3):
-            T[r][c] = col[r] - t0[r]
-    t0 = mp_exp_apply(xi, 1, [mp.mpf(0)] * 3)
-    for r in range(3):
-        T[r][3] = t0[r]
-    return T
-
-
-def mp_log(D):
-    """Log(D) in 50 digits: the rotation's quaternion (Shepperd, w >= 0), theta = 2 atan2(|v|, w), rho = V^-1 t"""
-    R = [[mp.mpf(float(D[r, c])) for c in range(3)] for r in range(3)]
-    t = [mp.mpf(float(D[r, 3])) for r in range(3)]
-    tr = R[0][0] + R[1][1] + R[2][2]
-    v = [mp.mpf(0)] * 3
-    if tr > 0:
-        r = mp.sqrt(tr + 1)
-        w = r / 2
-        v = [(R[2][1] - R[1][2]) / (2 * r), (R[0][2] - R[2][0]) / (2 * r), (R[1][0] - R[0][1]) / (2 * r)]
-    else:
-        i = max(range(3), key=lambda k: (R[k][k], -k))
-        j, k = (i + 1) % 3, (i + 2) % 3
-        r = mp.sqrt(R[i][i] - R[j][j] - R[k][k] + 1)
-        v[i] = r / 2
-        w = (R[k][j] - R[j][k]) / (2 * r)
-        v[j] = (R[j][i] + R[i][j]) / (2 * r)
-        v[k] = (R[k][i] + R[i][k]) / (2 * r)
-    if w < 0:
-        w, v = -w, [-x for x in v]
-    n = mp.sqrt(sum(x * x for x in v))
-    f = 2 / w if n == 0 else 2 * mp.atan2(n, w) / n
-    phi = [f * x for x in v]
-    theta = f * n
-    c = mp.mpf(1) / 12 if theta == 0 else (1 - theta * mp.cos(theta / 2) / (2 * mp.sin(theta / 2))) / theta ** 2
-    a = mp_cross(phi, t)
-    b = mp_cross(phi, a)
-    return [t[r] - a[r] / 2 + c * b[r] for r in range(3)] + phi
 
 
 def motion(theta, seed):

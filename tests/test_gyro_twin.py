@@ -1,14 +1,14 @@
 """The gyroscope rotation of dcreg_icp_run_odometry_gyro: the NumPy twin (api.gyro_rotation, gyro_knots,
-deskew_points_gyro) against closed forms, a 50-digit evaluation, its clipping and bracketing rules and a scene whose gyro
-matches its trajectory; and dcreg_b200/csrc/se3.cuh built as host C++ against the twin, bit for bit."""
+deskew_points_gyro) against closed forms, a 50-digit evaluation (oracle/dcreg_oracle_motion_mp.py), its clipping and
+bracketing rules and a scene whose gyro matches its trajectory; and dcreg_b200/csrc/se3.cuh built as host C++ against the twin, bit for bit."""
 import subprocess
 
-import mpmath
 import numpy as np
 import pytest
 from scipy.spatial.transform import Rotation
 
 from dcreg_b200 import api, scenes
+from dcreg_oracle_motion_mp import mp_gyro_rotation
 from harness import tool_program
 
 
@@ -33,25 +33,8 @@ def test_rotation_against_50_digits():
     rng = np.random.default_rng(5)
     R, bias = extrinsic(rng)
     S = random_samples(rng)
-    mpmath.mp.dps = 50
-
-    def mexp(phi):
-        th = mpmath.sqrt(sum(p * p for p in phi))
-        K = mpmath.matrix([[0, -phi[2], phi[1]], [phi[2], 0, -phi[0]], [-phi[1], phi[0], 0]])
-        if th == 0:
-            return mpmath.eye(3)
-        return mpmath.eye(3) + (mpmath.sin(th) / th) * K + ((1 - mpmath.cos(th)) / th ** 2) * (K * K)
-
-    Rm = mpmath.matrix(R.tolist())
     for a, b in [(S[3, 0], S[40, 0]), (S[5, 0] + 1e-3, S[30, 0] - 2e-3), (S[0, 0], S[-1, 0])]:
-        M = mpmath.eye(3)
-        cur = mpmath.mpf(a)
-        j = np.searchsorted(S[:, 0], a, side="right") - 1
-        while cur < b:
-            nxt = min(mpmath.mpf(S[j + 1, 0]), mpmath.mpf(b))
-            w = Rm * mpmath.matrix([mpmath.mpf(S[j, c + 1]) - mpmath.mpf(bias[c]) for c in range(3)])
-            M = M * mexp([w[c] * (nxt - cur) for c in range(3)])
-            cur, j = nxt, j + 1
+        M = mp_gyro_rotation(S, a, b, R, bias)
         G = api.gyro_rotation(S, a, b, R, bias)
         err = max(abs(float(M[r, c]) - G[r, c]) for r in range(3) for c in range(3))
         assert err < 1e-13, err
