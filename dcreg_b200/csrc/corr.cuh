@@ -945,13 +945,14 @@ __global__ void transform_points_kernel(const float4* __restrict__ in, long long
 // |x| >= min_norm and max_j (n.nb_j + d)^2 < thickness^2 (icp_test_runner.cpp:1727-1773).
 // Returns true and (n, d) when a valid plane exists.
 // The QR is the register-resident one (small_la.cuh: the same operations in the same order as the generic
-// colpiv_qr_solve, bit-identical results; tools/test_qr_reg.cu).  A separate function with its own register allocation:
-// it is called from the fit work list of the loop kernel, where almost nothing is live across the call (inlined into a
-// loop body full of live state it spills and ran several times slower during development; not re-measured on H100).
+// colpiv_qr_solve, bit-identical results; tools/test_qr_reg.cu).  Inlined into the fit list of the loop kernel: as a
+// separate function under the kernel's 80-register cap it saved and restored the caller's registers and its own spills
+// through local memory on every fit's chain, and its key array (kpos) lived in the stack frame; kpos is the fit list's
+// key row in shared memory (§3, "Fit keys from shared memory, fit inlined").
 // Rejected: a variant of the QR with hardware reciprocal / rsqrt seeds instead of the ~30 IEEE divisions and square
 // roots on the fit's dependent chain shortens a fit, but on exactly rank-deficient neighbourhoods (collinear lattice
 // points) its 1-ulp differences flip the pivoted QR's rank decision and change a correspondence.
-__device__ __noinline__ bool fit_plane_reg(const Grid& g, const int (&kpos)[5], double min_norm, double thickness,
+__device__ __forceinline__ bool fit_plane_reg(const Grid& g, const int* kpos, double min_norm, double thickness,
                                            double& nx, double& ny, double& nz, double& d) {
     double A[5][3], b[5], x[3];
 #pragma unroll

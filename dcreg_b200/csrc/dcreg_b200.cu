@@ -599,11 +599,8 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
             const int nF = sm.nF;
             for (int f = tid; f < nF; f += kBlock) {
                 const int t = sm.listF[f];
-                int key[5];
-#pragma unroll
-                for (int k = 0; k < 5; ++k) key[k] = sm.key[t][k];
                 double fx = 0.0, fy = 0.0, fz = 0.0, fd = 0.0;
-                const int fit = corr::fit_plane_reg(g, key, A.prm.min_normal_norm, A.prm.plane_thickness, fx, fy, fz, fd) ? 2 : 1;
+                const int fit = corr::fit_plane_reg(g, sm.key[t], A.prm.min_normal_norm, A.prm.plane_thickness, fx, fy, fz, fd) ? 2 : 1;
                 sm.plane[t] = make_double4(fx, fy, fz, fd);
                 sm.fitres[t] = (signed char)fit;
                 if (coherent) {
@@ -611,7 +608,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                     if (fit == 2) rec_plane[it] = make_double4(fx, fy, fz, fd);
                     int* kp = rec_key + 5 * it;
 #pragma unroll
-                    for (int k = 0; k < 5; ++k) kp[k] = key[k];
+                    for (int k = 0; k < 5; ++k) kp[k] = sm.key[t][k];
                     rec_fit[it] = (signed char)fit;
                 }
                 ++n_fit;
