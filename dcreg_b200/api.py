@@ -111,6 +111,38 @@ class Gyro(C.Structure):
         return np.array(self.bias[:])
 
 
+class Imu(C.Structure):
+    """dcreg_imu: R_sensor_imu (3, 3) maps IMU-frame vectors into the LiDAR frame, gyro_bias (3,) rad/s and accel_bias
+    (3,) m/s^2 are subtracted first, gravity (3,) m/s^2 is the world-frame (T_init's frame) gravity vector"""
+    _fields_ = [("R_sensor_imu", C.c_double * 9), ("gyro_bias", C.c_double * 3), ("accel_bias", C.c_double * 3),
+                ("gravity", C.c_double * 3)]
+
+    def __init__(self, R_sensor_imu=None, gyro_bias=(0.0, 0.0, 0.0), accel_bias=(0.0, 0.0, 0.0),
+                 gravity=(0.0, 0.0, -9.80665)):
+        super().__init__()
+        R = np.eye(3) if R_sensor_imu is None else np.asarray(R_sensor_imu, dtype=np.float64).reshape(3, 3)
+        self.R_sensor_imu[:] = [float(x) for x in R.reshape(-1)]
+        self.gyro_bias[:] = [float(x) for x in np.asarray(gyro_bias, dtype=np.float64).reshape(3)]
+        self.accel_bias[:] = [float(x) for x in np.asarray(accel_bias, dtype=np.float64).reshape(3)]
+        self.gravity[:] = [float(x) for x in np.asarray(gravity, dtype=np.float64).reshape(3)]
+
+    @property
+    def R(self):
+        return np.array(self.R_sensor_imu[:]).reshape(3, 3)
+
+    @property
+    def bg(self):
+        return np.array(self.gyro_bias[:])
+
+    @property
+    def ba(self):
+        return np.array(self.accel_bias[:])
+
+    @property
+    def g(self):
+        return np.array(self.gravity[:])
+
+
 _lib = None
 
 # every symbol include/dcreg_b200.h declares (checked by tests/test_abi.py)
@@ -122,7 +154,7 @@ EXPORTS = [
     "dcreg_find_planes",
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
-    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_icp_run_odometry_adaptive", "dcreg_odometry_open_adaptive", "dcreg_odometry_push_adaptive", "dcreg_icp_run_odometry_gyro", "dcreg_odometry_open_gyro", "dcreg_odometry_push_gyro", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_voxel_downsample_spaced", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
+    "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_icp_run_odometry_adaptive", "dcreg_odometry_open_adaptive", "dcreg_odometry_push_adaptive", "dcreg_icp_run_odometry_gyro", "dcreg_odometry_open_gyro", "dcreg_odometry_push_gyro", "dcreg_icp_run_odometry_imu", "dcreg_odometry_open_imu", "dcreg_odometry_push_imu", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_voxel_downsample_spaced", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
     "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
@@ -232,6 +264,18 @@ def load_library():
                                              C.POINTER(C.c_float), dp, dp, C.POINTER(i64), C.POINTER(i64), dp, dp,
                                              C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(C.c_float), dp,
                                              C.POINTER(IterLog), ci]
+    lib.dcreg_icp_run_odometry_imu.argtypes = [vp, C.POINTER(IcpParams), ci, C.POINTER(ci), ci, C.POINTER(C.c_float),
+                                               C.POINTER(i64), ci, C.c_double, ci, ci, C.c_double, C.c_double, ci, ci,
+                                               C.c_double, C.POINTER(AdaptiveThreshold), C.POINTER(Imu), dp, dp, dp,
+                                               C.POINTER(C.c_float), dp, dp, C.POINTER(i64), C.POINTER(i64), dp, dp,
+                                               C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(C.c_float), dp,
+                                               dp, C.POINTER(IterLog), ci]
+    lib.dcreg_odometry_open_imu.argtypes = [vp, C.POINTER(IcpParams), ci, C.c_double, ci, ci, C.c_double, C.c_double,
+                                            ci, ci, C.c_double, C.POINTER(AdaptiveThreshold), C.POINTER(Imu), dp, dp]
+    lib.dcreg_odometry_push_imu.argtypes = [vp, C.POINTER(ci), ci, C.POINTER(C.c_float), C.POINTER(i64), ci, dp,
+                                            C.POINTER(C.c_float), dp, dp, C.POINTER(i64), C.POINTER(i64), dp, dp,
+                                            C.POINTER(ci), C.POINTER(ci), C.POINTER(ci), dp, C.POINTER(C.c_float), dp, dp,
+                                            C.POINTER(IterLog), ci]
     lib.dcreg_comm_mode.argtypes = [vp]
     lib.dcreg_icp_enqueue.argtypes = [vp, C.POINTER(IcpParams), dp]
     lib.dcreg_icp_fetch.argtypes = [vp, dp, C.POINTER(ci), C.POINTER(ci)]
@@ -327,9 +371,10 @@ def _pack_timestamps(timestamps, off, name):
     return np.ascontiguousarray(np.concatenate(ts) if ts else np.zeros(0, np.float32))
 
 
-def _pack_gyro(name, gyro, frame_times, gyro_samples, n_frames, n_seqs):
-    """(frame_times (n_frames, 2), samples (rows, 4), sample_offsets int64 [n_seqs + 1]) as contiguous arrays, or Nones
-    without gyro input (a gyro session's push may leave both out; one without the other is refused)"""
+def _pack_gyro(name, gyro, frame_times, gyro_samples, n_frames, n_seqs, cols=4):
+    """(frame_times (n_frames, 2), samples (rows, cols), sample_offsets int64 [n_seqs + 1]) as contiguous arrays, or
+    Nones without gyro input (a gyro session's push may leave both out; one without the other is refused).  cols = 7:
+    IMU samples (t, wx, wy, wz, ax, ay, az)"""
     if gyro is None:
         if frame_times is not None or gyro_samples is not None:
             raise ValueError(f"{name}: frame_times and gyro_samples need gyro input")
@@ -343,10 +388,20 @@ def _pack_gyro(name, gyro, frame_times, gyro_samples, n_frames, n_seqs):
         raise ValueError(f"{name}: {n_frames} frames but {ft.shape[0]} frame times")
     if len(gyro_samples) != n_seqs:
         raise ValueError(f"{name}: {n_seqs} sequences but {len(gyro_samples)} sample arrays")
-    smp = [np.asarray(x, dtype=np.float64).reshape(-1, 4) for x in gyro_samples]
+    smp = [np.asarray(x, dtype=np.float64).reshape(-1, cols) for x in gyro_samples]
     off = np.zeros(n_seqs + 1, dtype=np.int64)
     off[1:] = np.cumsum([x.shape[0] for x in smp])
-    return ft, np.ascontiguousarray(np.concatenate(smp) if smp else np.zeros((0, 4))), off
+    return ft, np.ascontiguousarray(np.concatenate(smp) if smp else np.zeros((0, cols))), off
+
+
+def _pack_v_init(name, v_init, n_seqs):
+    """v_init as a contiguous (n_seqs, 3) float64 array, or None (every sequence starts at rest)"""
+    if v_init is None:
+        return None
+    v = np.ascontiguousarray(v_init, dtype=np.float64).reshape(-1, 3)
+    if v.shape[0] != n_seqs:
+        raise ValueError(f"{name}: {n_seqs} sequences but {v.shape[0]} initial velocities")
+    return v
 
 
 def _split_deskewed(out, npts):
@@ -387,6 +442,10 @@ _ODOMETRY_ARGS = {name: " ".join(args).split() for name, args in {
     "dcreg_icp_run_odometry_gyro": (_RUN, "map_frames motion", _FILTERS,
                                     "max_distance adaptive gyro T_init deltas timestamps frame_times samples",
                                     "sample_offsets frame_points", _OUTPUTS, "deskewed_xyz search_radius log log_cap"),
+    "dcreg_icp_run_odometry_imu": (_RUN, "map_frames motion", _FILTERS,
+                                   "max_distance adaptive imu T_init v_init deltas timestamps frame_times samples",
+                                   "sample_offsets frame_points", _OUTPUTS, "deskewed_xyz search_radius velocity log",
+                                   "log_cap"),
     "dcreg_odometry_open": ("params n_seqs cell_size map_frames motion", _FILTERS, "T_init"),
     "dcreg_odometry_open_map": ("params n_seqs cell_size motion", _FILTERS, "max_distance T_init"),
     "dcreg_odometry_open_adaptive": ("params n_seqs cell_size map_frames motion", _FILTERS,
@@ -399,6 +458,10 @@ _ODOMETRY_ARGS = {name: " ".join(args).split() for name, args in {
                                  "max_distance adaptive gyro T_init"),
     "dcreg_odometry_push_gyro": (_PUSH, "timestamps frame_times samples sample_offsets frame_points", _OUTPUTS,
                                  "deskewed_xyz search_radius log log_cap"),
+    "dcreg_odometry_open_imu": ("params n_seqs cell_size map_frames motion", _FILTERS,
+                                "max_distance adaptive imu T_init v_init"),
+    "dcreg_odometry_push_imu": (_PUSH, "timestamps frame_times samples sample_offsets frame_points", _OUTPUTS,
+                                "deskewed_xyz search_radius velocity log log_cap"),
     "dcreg_voxel_downsample": (_DOWNSAMPLE, "out_xyz out_offsets out_index"),
     "dcreg_voxel_downsample_n": (_DOWNSAMPLE, "max_points out_xyz out_offsets out_index"),
     "dcreg_voxel_downsample_spaced": (_DOWNSAMPLE, "max_points min_spacing out_xyz out_offsets out_index"),
@@ -416,9 +479,12 @@ def _odometry_call(lib, h, entry, **values):
     return getattr(lib, entry)(h, *(values.get(k) for k in _ODOMETRY_ARGS[entry]))
 
 
-def _odometry_entry(op, radius=False, voxel_map=False, deskew=False, capped=False, filtered=False, gyro=False):
+def _odometry_entry(op, radius=False, voxel_map=False, deskew=False, capped=False, filtered=False, gyro=False,
+                    imu=False):
     """The entry point of op ("icp_run_odometry", "odometry_open" or "odometry_push") for a call with these settings: the
     narrowest that takes them all.  Each entry point names itself in dcreg_last_error."""
+    if imu:
+        return f"dcreg_{op}_imu"
     if gyro:
         return f"dcreg_{op}_gyro"
     if radius:
@@ -836,7 +902,100 @@ def deskew_points_gyro(P, timestamps, frame_time, tm_prev, samples, t_D=(0.0, 0.
     return xyz
 
 
-VOXEL_LIMIT = 1 << 20     # voxel coordinates must lie in [-2^20, 2^20): 21 bits per axis in one 63-bit key
+# The accelerometer prior of dcreg_icp_run_odometry_imu (se3::gyro_rotation with acc_bias, se3::imu_translation,
+# se3::imu_velocity): the same formulas and operation order in Python floats (FP64, one rounding per operation, no FMA).
+# samples: (n, 7) rows (t, wx, wy, wz, ax, ay, az) in the IMU frame, t strictly ascending.
+def imu_preintegrate(samples, a, b, R_sensor_imu=np.eye(3), gyro_bias=(0.0, 0.0, 0.0), accel_bias=(0.0, 0.0, 0.0)):
+    """(G, alpha, beta, gamma) over [a, b], a <= b: G = gyro_rotation(samples, a, b) bit for bit, and over every piece
+    [u, u + d] of that walk, with M the walk's rotation at u and f = R_sensor_imu (acc_j - accel_bias) held over the
+    piece, m = M f d (each entry ((m0 f0 + m1 f1) + m2 f2) d), alpha += m, beta += m ((b - u) - 0.5 d), gamma += m ((u -
+    a) + 0.5 d).  It reads only the samples that bracket [a, b] (ValueError when they do not).  Returns (3, 3) and three
+    (3,) arrays."""
+    a, b = float(a), float(b)
+    S = np.asarray(samples, dtype=np.float64).reshape(-1, 7)
+    t = [float(x) for x in S[:, 0]]
+    R = [float(x) for x in np.asarray(R_sensor_imu, dtype=np.float64).reshape(9)]
+    bg = [float(x) for x in np.asarray(gyro_bias, dtype=np.float64).reshape(3)]
+    ba = [float(x) for x in np.asarray(accel_bias, dtype=np.float64).reshape(3)]
+    j = bisect.bisect_right(t, a) - 1
+    if not a <= b or j < 0 or not t or t[-1] < b:
+        raise ValueError(f"imu_preintegrate: the samples do not bracket [{a!r}, {b!r}]")
+    M = [1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0]
+    al, be, ga = [0.0] * 3, [0.0] * 3, [0.0] * 3
+    cur = a
+    while cur < b:
+        nxt = min(t[j + 1], b)
+        d = nxt - cur
+        row = S[j]
+        f = _gyro_rate(R, ba, [0.0, float(row[4]), float(row[5]), float(row[6])])
+        h = 0.5 * d
+        wb, wg = (b - cur) - h, (cur - a) + h
+        for r in range(3):
+            m = ((M[3 * r] * f[0] + M[3 * r + 1] * f[1]) + M[3 * r + 2] * f[2]) * d
+            al[r] = al[r] + m
+            be[r] = be[r] + m * wb
+            ga[r] = ga[r] + m * wg
+        M = _gyro_piece(M, _gyro_rate(R, bg, row), d)
+        cur = nxt
+        j += 1
+    return np.array(M).reshape(3, 3), np.array(al), np.array(be), np.array(ga)
+
+
+def imu_translation(T_prev, v_prev, gravity, beta, dt):
+    """t_D = dt R^T v + (0.5 dt^2) R^T g + beta, R = T_prev's rotation, every R^T x entry ((R_0r x0 + R_1r x1) + R_2r x2)
+    (se3::imu_translation).  Returns (3,)."""
+    R = [float(x) for x in np.asarray(T_prev, dtype=np.float64)[:3, :3].reshape(9)]
+    v = [float(x) for x in np.asarray(v_prev, dtype=np.float64).reshape(3)]
+    g = [float(x) for x in np.asarray(gravity, dtype=np.float64).reshape(3)]
+    be = [float(x) for x in np.asarray(beta, dtype=np.float64).reshape(3)]
+    dt = float(dt)
+    c2 = 0.5 * (dt * dt)
+    out = []
+    for r in range(3):
+        rv = (R[r] * v[0] + R[3 + r] * v[1]) + R[6 + r] * v[2]
+        rg = (R[r] * g[0] + R[3 + r] * g[1]) + R[6 + r] * g[2]
+        out.append((dt * rv + c2 * rg) + be[r])
+    return np.array(out)
+
+
+def imu_increment(samples, tm_prev, tm, T_prev, v_prev, gravity, R_sensor_imu=np.eye(3), gyro_bias=(0.0, 0.0, 0.0),
+                  accel_bias=(0.0, 0.0, 0.0)):
+    """The increment D a non-anchor frame's prior is composed with (dcreg_icp_run_odometry_imu): rotation G(tm_prev ->
+    tm), translation imu_translation(T_prev, v_prev, gravity, beta, tm - tm_prev).  T_prior = compose_prior(T_prev, D).
+    Returns (4, 4)."""
+    G, _, beta, _ = imu_preintegrate(samples, tm_prev, tm, R_sensor_imu, gyro_bias, accel_bias)
+    D = np.eye(4)
+    D[:3, :3] = G
+    D[:3, 3] = imu_translation(T_prev, v_prev, gravity, beta, float(tm) - float(tm_prev))
+    return D
+
+
+def imu_velocity(samples, tm_prev, tm, T_prev, T, gravity, R_sensor_imu=np.eye(3), gyro_bias=(0.0, 0.0, 0.0),
+                 accel_bias=(0.0, 0.0, 0.0)):
+    """A frame's velocity once it has stopped (dcreg_icp_run_odometry_imu): v = (t - t_prev) / dt + (R_prev gamma) / dt +
+    (0.5 dt) g, dt = tm - tm_prev, every R_prev gamma entry ((r0 g0 + r1 g1) + r2 g2) (se3::imu_velocity).  T_prev, T:
+    the two frames' poses.  Returns (3,)."""
+    _, _, _, gamma = imu_preintegrate(samples, tm_prev, tm, R_sensor_imu, gyro_bias, accel_bias)
+    return imu_velocity_from(T_prev, T, gravity, gamma, float(tm) - float(tm_prev))
+
+
+def imu_velocity_from(T_prev, T, gravity, gamma, dt):
+    """imu_velocity from a given gamma and dt"""
+    A = np.asarray(T_prev, dtype=np.float64)
+    B = np.asarray(T, dtype=np.float64)
+    Rp = [float(x) for x in A[:3, :3].reshape(9)]
+    g = [float(x) for x in np.asarray(gravity, dtype=np.float64).reshape(3)]
+    gm = [float(x) for x in np.asarray(gamma, dtype=np.float64).reshape(3)]
+    dt = float(dt)
+    h = 0.5 * dt
+    out = []
+    for r in range(3):
+        rg = (Rp[3 * r] * gm[0] + Rp[3 * r + 1] * gm[1]) + Rp[3 * r + 2] * gm[2]
+        out.append(((float(B[r, 3]) - float(A[r, 3])) / dt + rg / dt) + h * g[r])
+    return np.array(out)
+
+
+VOXEL_LIMIT = 1 << 20    # voxel coordinates must lie in [-2^20, 2^20): 21 bits per axis in one 63-bit key
 
 
 def _max_points(v, name="max_points"):
@@ -1352,7 +1511,8 @@ class Context:
                          map_frames: int = 10, cell_size=None, want_log: bool = False, want_cov: bool = False,
                          source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
                          map_max_points: int = 1, timestamps=None, want_deskewed: bool = False, adaptive=None,
-                         want_radius: bool = False, gyro=None, frame_times=None, gyro_samples=None):
+                         want_radius: bool = False, gyro=None, frame_times=None, gyro_samples=None, imu=None,
+                         imu_samples=None, v_init=None, want_velocity: bool = False):
         """Scan-to-map odometry (`sequences`: a list of lists of (N, >=3) point arrays): frame k of a sequence registers
         against the local map of the frames [k - map_frames, k) before it, each placed at its own registered pose
         (map_points), starting from compose_prior(frame k-1's result, D).  motion "increments": D = deltas[k-1]
@@ -1374,16 +1534,23 @@ class Context:
         gyro (a Gyro), frame_times ((n_frames, 2) (start, span) in seconds over all frames in order) and gyro_samples (one
         (n_s, 4) array (t, wx, wy, wz) per sequence): every non-anchor frame's prior rotation, and with timestamps its
         deskew rotation, come from the integrated rates (dcreg_icp_run_odometry_gyro; the twin is gyro_rotation,
-        gyro_increment and deskew_points_gyro); motion must be "constant_velocity".  .search_radius as with adaptive."""
+        gyro_increment and deskew_points_gyro); motion must be "constant_velocity".  .search_radius as with adaptive.
+        imu (an Imu), frame_times and imu_samples (one (n_s, 7) array (t, wx, wy, wz, ax, ay, az) per sequence) instead
+        of gyro: the gyro's rotation, and every non-anchor frame's prior translation from the previous frame's velocity
+        and the preintegrated specific force (dcreg_icp_run_odometry_imu; the twin is imu_preintegrate, imu_increment
+        and imu_velocity).  v_init ((n_seqs, 3), None: zero): every sequence's velocity at its first frame; want_velocity:
+        .velocity holds every frame's world-frame velocity at its mid-sweep time."""
         return self._odometry("icp_run_odometry", params, sequences, T_init, deltas, motion, map_frames, None, cell_size,
                               want_log, want_cov, source_voxel, map_voxel, source_max_points, map_max_points, timestamps,
-                              want_deskewed, adaptive, want_radius, gyro, frame_times, gyro_samples)
+                              want_deskewed, adaptive, want_radius, gyro, frame_times, gyro_samples, imu, imu_samples,
+                              v_init, want_velocity)
 
     def icp_run_odometry_map(self, params, sequences, T_init, deltas=None, motion: str = "increments", *,
                              map_voxel: float, max_distance: float, cell_size=None, want_log: bool = False,
                              want_cov: bool = False, source_voxel: float = 0.0, source_max_points: int = 1,
                              map_max_points: int = 1, timestamps=None, want_deskewed: bool = False, adaptive=None,
-                             want_radius: bool = False, gyro=None, frame_times=None, gyro_samples=None):
+                             want_radius: bool = False, gyro=None, frame_times=None, gyro_samples=None, imu=None,
+                             imu_samples=None, v_init=None, want_velocity: bool = False):
         """icp_run_odometry with a persistent voxel map per sequence instead of the window (dcreg_icp_run_odometry_map,
         KISS-ICP's VoxelHashMap): frame k registers against M_k, where M_1 = voxel_map_update(empty, F_s(anchor),
         T_init[s]) and M_{k+1} = voxel_map_update(M_k, F_s(frame k), T_out[k], map_voxel, map_max_points,
@@ -1393,11 +1560,12 @@ class Context:
         return self._odometry("icp_run_odometry_map", params, sequences, T_init, deltas, motion, 0,
                               float(max_distance), cell_size, want_log, want_cov, source_voxel, map_voxel,
                               source_max_points, map_max_points, timestamps, want_deskewed, adaptive, want_radius, gyro,
-                              frame_times, gyro_samples)
+                              frame_times, gyro_samples, imu, imu_samples, v_init, want_velocity)
 
     def _odometry(self, name, params, sequences, T_init, deltas, motion, map_frames, max_distance, cell_size, want_log,
                   want_cov, source_voxel, map_voxel, source_max_points, map_max_points, timestamps, want_deskewed,
-                  adaptive, want_radius, gyro=None, frame_times=None, gyro_samples=None):
+                  adaptive, want_radius, gyro=None, frame_times=None, gyro_samples=None, imu=None, imu_samples=None,
+                  v_init=None, want_velocity=False):
         """icp_run_odometry (max_distance None: the window of map_frames frames) and icp_run_odometry_map (map_frames
         0: the voxel map pruned at max_distance)"""
         motion = _motion(motion, name)
@@ -1407,13 +1575,22 @@ class Context:
         S, n = len(sequences), int(seq_off[-1])
         params, parg, per_lane = self._lanes(name, params, S)
         cell = float(params.search_radius if cell_size is None else cell_size)
-        with_radius = adaptive is not None or want_radius or gyro is not None
+        if imu is not None and (gyro is not None or gyro_samples is not None):
+            raise ValueError(f"{name}: imu and gyro input are exclusive (imu carries the gyro)")
+        if imu is None and (imu_samples is not None or v_init is not None or want_velocity):
+            raise ValueError(f"{name}: imu_samples, v_init and want_velocity need imu input")
+        with_radius = adaptive is not None or want_radius or gyro is not None or imu is not None
         entry = _odometry_entry("icp_run_odometry", radius=with_radius, voxel_map=max_distance is not None,
                                 deskew=timestamps is not None or want_deskewed,
                                 capped=source_max_points != 1 or map_max_points != 1,
                                 filtered=source_voxel != 0.0 or map_voxel != 0.0 or self._map_input_voxel > 0.0,
-                                gyro=gyro is not None)
-        ft, smp, smp_off = _pack_gyro(name, gyro, frame_times, gyro_samples, n, S)
+                                gyro=gyro is not None, imu=imu is not None)
+        if imu is not None:
+            ft, smp, smp_off = _pack_gyro(name, imu, frame_times, imu_samples, n, S, cols=7)
+        else:
+            ft, smp, smp_off = _pack_gyro(name, gyro, frame_times, gyro_samples, n, S)
+        v0 = _pack_v_init(name, v_init, S)
+        vel = np.zeros((max(n, 1), 3)) if want_velocity else None
         ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
                               off if off is not None else np.zeros(1, np.int64), name)
         npts = np.diff(off) if off is not None else np.zeros(0, dtype=np.int64)
@@ -1434,10 +1611,14 @@ class Context:
                 n_iterations=o.n_it, converged=o.conv, status=o.st, cov=_optr(o.cov), deskewed_xyz=_fptr(desk),
                 search_radius=_optr(radius), log=o.logs, log_cap=o.cap,
                 gyro=None if gyro is None else C.byref(gyro), frame_times=_optr(ft), samples=_optr(smp),
-                sample_offsets=_iptr(smp_off))
+                sample_offsets=_iptr(smp_off), imu=None if imu is None else C.byref(imu), v_init=_optr(v0),
+                velocity=_optr(vel))
         with self._lane_setting(per_lane):
             out = self._run_batched(name, call, params, n, S, "sequences", T_init, want_log, want_cov, deltas,
                                     want_prior=True)
+        if want_velocity:
+            for r, v in zip(out, vel):
+                r.velocity = v.copy()
         for r, c in zip(out, npts):
             r.n_points = int(c)
         if with_radius:
@@ -1450,27 +1631,32 @@ class Context:
 
     def odometry_map_session(self, params, n_seqs: int, T_init, motion: str = "increments", *,
                              map_voxel: float, max_distance: float, cell_size=None, source_voxel: float = 0.0,
-                             source_max_points: int = 1, map_max_points: int = 1, adaptive=None, gyro=None):
+                             source_max_points: int = 1, map_max_points: int = 1, adaptive=None, gyro=None, imu=None,
+                             v_init=None):
         """Open the context's odometry session with icp_run_odometry_map's voxel map (dcreg_odometry_open_map): the
         OdometrySession of odometry_session, whose pushes give byte for byte what one icp_run_odometry_map call over the
         recording gives, and whose local_map(s) returns sequence s's current map.  The arguments are odometry_session's
         in the same positions, without map_frames; map_voxel and max_distance are keyword-only."""
         return self._open_session("odometry_map_session", params, n_seqs, T_init, motion, 0, float(max_distance),
-                                  cell_size, source_voxel, map_voxel, source_max_points, map_max_points, adaptive, gyro)
+                                  cell_size, source_voxel, map_voxel, source_max_points, map_max_points, adaptive, gyro,
+                                  imu, v_init)
 
     def odometry_session(self, params, n_seqs: int, T_init, motion: str = "increments", map_frames: int = 10,
                          cell_size=None, source_voxel: float = 0.0, map_voxel: float = 0.0, source_max_points: int = 1,
-                         map_max_points: int = 1, adaptive=None, gyro=None):
+                         map_max_points: int = 1, adaptive=None, gyro=None, imu=None, v_init=None):
         """Open the context's odometry session (dcreg_odometry_open): icp_run_odometry's settings for n_seqs sequences
         whose frames come in pushes (OdometrySession.push).  T_init (n_seqs, 4, 4): the pose of each sequence's first
         frame.  Pushing a recording in any chunks gives byte for byte what one icp_run_odometry call over it gives.
         One session per context; use it as a context manager, or close() it.  gyro (a Gyro): dcreg_odometry_open_gyro,
-        whose pushes take frame_times and gyro_samples and return .search_radius."""
+        whose pushes take frame_times and gyro_samples and return .search_radius.  imu (an Imu) and v_init ((n_seqs, 3),
+        None: zero): dcreg_odometry_open_imu, whose pushes take frame_times and imu_samples and return .search_radius
+        and, with want_velocity, .velocity."""
         return self._open_session("odometry_session", params, n_seqs, T_init, motion, map_frames, None, cell_size,
-                                  source_voxel, map_voxel, source_max_points, map_max_points, adaptive, gyro)
+                                  source_voxel, map_voxel, source_max_points, map_max_points, adaptive, gyro, imu,
+                                  v_init)
 
     def _open_session(self, name, params, n_seqs, T_init, motion, map_frames, max_distance, cell_size, source_voxel,
-                      map_voxel, source_max_points, map_max_points, adaptive, gyro=None):
+                      map_voxel, source_max_points, map_max_points, adaptive, gyro=None, imu=None, v_init=None):
         """odometry_session (max_distance None) and odometry_map_session (map_frames 0), as in _odometry"""
         motion = _motion(motion, name)
         source_max_points = _max_points(source_max_points, "source_max_points")
@@ -1481,8 +1667,13 @@ class Context:
         params, parg, per_lane = self._lanes(name, params, int(n_seqs))
         cell = float(params.search_radius if cell_size is None else cell_size)
         # dcreg_odometry_open_adaptive's pushes return .search_radius
+        if imu is not None and gyro is not None:
+            raise ValueError(f"{name}: imu and gyro input are exclusive (imu carries the gyro)")
+        if imu is None and v_init is not None:
+            raise ValueError(f"{name}: v_init needs imu input")
         entry = _odometry_entry("odometry_open", radius=adaptive is not None, voxel_map=max_distance is not None,
-                                gyro=gyro is not None)
+                                gyro=gyro is not None, imu=imu is not None)
+        v0 = _pack_v_init(name, v_init, int(n_seqs))
         with self._lane_setting(per_lane):
             self._check(_odometry_call(
                 self.lib, self._h, entry, params=parg, n_seqs=int(n_seqs), cell_size=cell, map_frames=int(map_frames),
@@ -1490,8 +1681,9 @@ class Context:
                 source_max_points=source_max_points, map_max_points=map_max_points,
                 max_distance=0.0 if max_distance is None else float(max_distance),
                 adaptive=None if adaptive is None else C.byref(adaptive), gyro=None if gyro is None else C.byref(gyro),
-                T_init=_dptr(T0)))
-        return OdometrySession(self, params, int(n_seqs), adaptive=adaptive is not None, gyro=gyro is not None)
+                imu=None if imu is None else C.byref(imu), T_init=_dptr(T0), v_init=_optr(v0)))
+        return OdometrySession(self, params, int(n_seqs), adaptive=adaptive is not None, gyro=gyro is not None,
+                               imu=imu is not None)
 
     def icp_run_pairs(self, params, sources, targets, T_init, cell_size=None, want_log: bool = False,
                       want_cov: bool = False, metrics_threshold=None):
@@ -1590,14 +1782,17 @@ class OdometrySession:
     """The context's odometry session (Context.odometry_session): frames pushed as they arrive, each sequence's local-map
     window and motion-model state kept on the device from one push to the next."""
 
-    def __init__(self, ctx: Context, params: IcpParams, n_seqs: int, adaptive: bool = False, gyro: bool = False):
+    def __init__(self, ctx: Context, params: IcpParams, n_seqs: int, adaptive: bool = False, gyro: bool = False,
+                 imu: bool = False):
         self.ctx, self.params, self.n_seqs = ctx, params, n_seqs
         self.adaptive = adaptive        # opened with an AdaptiveThreshold: every push returns .search_radius
         self.gyro = gyro                # opened with a Gyro: pushes take frame_times and gyro_samples
+        self.imu = imu                  # opened with an Imu: pushes take frame_times and imu_samples
         self.open = True
 
     def push(self, frames_per_seq, deltas=None, want_log: bool = False, want_cov: bool = False, timestamps=None,
-             want_deskewed: bool = False, frame_times=None, gyro_samples=None):
+             want_deskewed: bool = False, frame_times=None, gyro_samples=None, imu_samples=None,
+             want_velocity: bool = False):
         """The next frames of every sequence (dcreg_odometry_push): frames_per_seq, a list of n_seqs lists, possibly
         empty, of (N, >=3) point arrays.  deltas: (frames, 4, 4) increments over the pushed frames in order (entry k maps
         frame k's result to the next frame's prior in its sequence, which may come in a later push), or None for
@@ -1605,8 +1800,10 @@ class OdometrySession:
         only when want_log, .cov when want_cov).  timestamps / want_deskewed: as in icp_run_odometry, nested like
         frames_per_seq (dcreg_odometry_push_deskew).  frame_times ((frames, 2) over the pushed frames in order) and
         gyro_samples (one (n_s, 4) array per sequence, holding the samples that bracket every pushed frame's interval
-        from the previous mid-sweep to its sweep's end): a gyro session's input (dcreg_odometry_push_gyro).  A push that
-        fails raises DcregError and leaves the session as it was."""
+        from the previous mid-sweep to its sweep's end): a gyro session's input (dcreg_odometry_push_gyro).
+        frame_times and imu_samples (one (n_s, 7) array per sequence, the same bracketing): an IMU session's input
+        (dcreg_odometry_push_imu); want_velocity: .velocity as in icp_run_odometry.  A push that fails raises DcregError
+        and leaves the session as it was."""
         ctx = self.ctx
         if len(frames_per_seq) != self.n_seqs:
             raise ValueError(f"odometry push: {self.n_seqs} sequences but {len(frames_per_seq)} frame lists")
@@ -1624,20 +1821,31 @@ class OdometrySession:
         cov = np.empty((m, 6, 6)) if want_cov else None
         cap = int(self.params.max_iterations) if want_log else 0
         logs = (IterLog * max(cap * n, 1))() if want_log else None
-        radius = np.zeros(m) if self.adaptive or self.gyro else None
-        ft, smp, smp_off = _pack_gyro("odometry push", self.gyro or None, frame_times, gyro_samples, n, self.n_seqs)
+        radius = np.zeros(m) if self.adaptive or self.gyro or self.imu else None
+        if not self.imu and (imu_samples is not None or want_velocity):
+            raise ValueError("odometry push: imu_samples and want_velocity need a session opened with imu input")
+        if self.imu:
+            if gyro_samples is not None:
+                raise ValueError("odometry push: an imu session takes imu_samples, not gyro_samples")
+            ft, smp, smp_off = _pack_gyro("odometry push", True, frame_times, imu_samples, n, self.n_seqs, cols=7)
+        else:
+            ft, smp, smp_off = _pack_gyro("odometry push", self.gyro or None, frame_times, gyro_samples, n, self.n_seqs)
+        vel = np.zeros((m, 3)) if want_velocity else None
         ts = _pack_timestamps([t for s in timestamps for t in s] if timestamps is not None else None,
                               off if off is not None else np.zeros(1, np.int64), "odometry push")
         desk = np.empty((max(int(off[-1]) if off is not None else 0, 1), 3), np.float32) if want_deskewed else None
         entry = _odometry_entry("odometry_push", radius=self.adaptive, deskew=timestamps is not None or want_deskewed,
-                                gyro=self.gyro)
+                                gyro=self.gyro, imu=self.imu)
         ctx._check(_odometry_call(
             ctx.lib, ctx._h, entry, seq_offsets=seq_off.ctypes.data_as(C.POINTER(C.c_int)), n_frames=n, xyz=_fptr(xyz),
             frame_offsets=_iptr(off), stride=3, deltas=_optr(D), timestamps=_fptr(ts), frame_points=_iptr(npts),
             T_prior=_dptr(T_prior), T_out=_dptr(T_out), n_iterations=n_it, converged=conv, status=st, cov=_optr(cov),
             deskewed_xyz=_fptr(desk), search_radius=_optr(radius), log=logs, log_cap=cap, frame_times=_optr(ft),
-            samples=_optr(smp), sample_offsets=_iptr(smp_off)))
+            samples=_optr(smp), sample_offsets=_iptr(smp_off), velocity=_optr(vel)))
         res = _trial_results(st[:n], conv[:n], n_it[:n], T_out, logs, cap, cov)
+        if want_velocity:
+            for r, v in zip(res, vel):
+                r.velocity = v.copy()
         for r, Tp, c in zip(res, T_prior, npts):
             r.T_prior, r.n_points = Tp, int(c)
         if radius is not None:

@@ -1199,6 +1199,16 @@ __global__ void map_points_kernel(const float4* __restrict__ src, const float4* 
     out[i] = make_float4(v[0], v[1], v[2], __int_as_float((int)i));
 }
 
+// Accelerometer input (dcreg_icp_run_odometry_imu): device frame d's (start, span, tm, tm_prev) ft[4 d ..] and its
+// (alpha, beta, gamma) abg[9 d ..] (odom_gyro_kernel), every frame reference r's velocity v[3 r ..] (world frame; a
+// step's velocity kernel writes its frames'), gravity in the world frame.  v null: gyro input alone.
+struct OdomImu {
+    const double* ft = nullptr;
+    const double* abg = nullptr;
+    double* v = nullptr;
+    double gravity[3] = {0.0, 0.0, 0.0};
+};
+
 // The increment D lane j's prior is composed with: delta[prev[j]] (null: identity), or with constant velocity the
 // increment from frame k-2 to frame k-1 (identity after the anchor); the identity for a first frame (prev[j] < 0).  The start kernel and odom_twist_kernel both take
 // it from here, so the deskew twist is the increment the prior used, bit for bit.
@@ -1223,15 +1233,18 @@ __device__ __forceinline__ void odom_increment(int j, const IcpState* __restrict
 // frame's prior is compose_prior(frame prev[j]'s pose, odom_increment); delta holds one entry per frame reference, or is
 // null.  kGyro (odom_start_gyro_kernel): the increment's rotation is the frame's gyro rotation G[9 f ..] instead, and
 // with tD the increment's translation goes to tD[3 j ..] and the frame's lever arm is zeroed, for
-// odom_deskew_gyro_kernel.  (prior map) A lane whose prev[j] < 0 runs its sequence's first frame from the state and
-// prior start_loop gave it, T_init: only its frame range is set.
+// odom_deskew_gyro_kernel.  With accelerometer input (imu.v not null) the increment's translation is
+// se3::imu_translation's instead, from frame prev[j]'s pose and velocity and the frame's beta.  (prior map) A lane whose
+// prev[j] < 0 runs its sequence's first frame from the state and prior start_loop gave it, T_init: only its frame range
+// is set.
 template <bool kGyro>
 __device__ __forceinline__ void odom_start(IcpState* states, const long long* __restrict__ seg, double* T_prior,
                                            int* cursor, int* first, unsigned int* n_active, int lanes, int step_first,
                                            int active, const int* __restrict__ prev, const int* __restrict__ prev2,
                                            const double* __restrict__ delta, int motion, int n_frames,
                                            const double* __restrict__ hist_T, const double* __restrict__ G,
-                                           double* __restrict__ tD, float* __restrict__ radius) {
+                                           double* __restrict__ tD, float* __restrict__ radius,
+                                           const OdomImu& imu) {
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j == 0) { *n_active = (unsigned)active; first[lanes] = step_first + active; }
     if (j >= lanes) return;
@@ -1240,15 +1253,22 @@ __device__ __forceinline__ void odom_start(IcpState* states, const long long* __
     if (j >= active || prev[j] < 0) return;
     double D[16], Ra[9], ta[3];
     odom_increment(j, states, prev, prev2, delta, motion, n_frames, hist_T, D);
+    ref_pose(prev[j], n_frames, states, hist_T, Ra, ta);
     if (kGyro) {
         for (int r = 0; r < 3; ++r)
             for (int c = 0; c < 3; ++c) D[4 * r + c] = G[(size_t)f * 9 + 3 * r + c];
+        if (imu.v) {
+            const double* ft = imu.ft + 4 * (size_t)f;
+            double t[3];
+            se3::imu_translation(Ra, imu.v + 3 * (size_t)prev[j], imu.gravity, imu.abg + 9 * (size_t)f + 3,
+                                 __dsub_rn(ft[2], ft[3]), t);
+            for (int r = 0; r < 3; ++r) D[4 * r + 3] = t[r];
+        }
         if (tD) {
             for (int r = 0; r < 3; ++r) tD[3 * (size_t)j + r] = D[4 * r + 3];
             radius[f] = 0.0f;
         }
     }
-    ref_pose(prev[j], n_frames, states, hist_T, Ra, ta);
     double T[16];
     compose_prior(Ra, ta, D, T);
     for (int i = 0; i < 16; ++i) T_prior[(size_t)f * 16 + i] = T[i];
@@ -1261,16 +1281,16 @@ __global__ void odom_start_kernel(IcpState* states, const long long* __restrict_
                                   const double* __restrict__ delta, int motion, int n_frames,
                                   const double* __restrict__ hist_T) {
     odom_start<false>(states, seg, T_prior, cursor, first, n_active, lanes, step_first, active, prev, prev2, delta,
-                      motion, n_frames, hist_T, nullptr, nullptr, nullptr);
+                      motion, n_frames, hist_T, nullptr, nullptr, nullptr, OdomImu{});
 }
 
 __global__ void odom_start_gyro_kernel(IcpState* states, const long long* __restrict__ seg, double* T_prior, int* cursor,
                                        int* first, unsigned int* n_active, int lanes, int step_first, int active,
                                        const int* __restrict__ prev, const int* __restrict__ prev2, int n_frames,
                                        const double* __restrict__ hist_T, const double* __restrict__ G,
-                                       double* __restrict__ tD, float* __restrict__ radius) {
+                                       double* __restrict__ tD, float* __restrict__ radius, OdomImu imu) {
     odom_start<true>(states, seg, T_prior, cursor, first, n_active, lanes, step_first, active, prev, prev2, nullptr,
-                     DCREG_MOTION_CONSTANT_VELOCITY, n_frames, hist_T, G, tD, radius);
+                     DCREG_MOTION_CONSTANT_VELOCITY, n_frames, hist_T, G, tD, radius, imu);
 }
 
 // The session's window after a push: m points in `pieces` retained frames, piece p being out[dst[p], dst[p+1]) = the
@@ -1385,17 +1405,38 @@ __global__ void odom_deskew_kernel(float4* __restrict__ src, float4* __restrict_
 // [kKnotStride knot_off[d] ..], empty for an anchor.
 //
 // Once per call, before the steps (one thread per device frame; the poses play no part): every non-anchor frame's
-// G(tm_prev -> tm), the rotation of its prior's increment, into G[9 d ..], and its sweep's knot table.
-__global__ void odom_gyro_kernel(se3::Gyro g, const double* __restrict__ smp, const double* __restrict__ ft,
-                                 const long long* __restrict__ range, const long long* __restrict__ knot_off,
-                                 int n_frames, double* __restrict__ G, double* __restrict__ knots) {
+// G(tm_prev -> tm), the rotation of its prior's increment, into G[9 d ..], and its sweep's knot table; samples `stride`
+// doubles a row.  With abg (IMU samples) the same walk's (alpha, beta, gamma) into abg[9 d ..], the specific force less
+// acc_bias.
+struct AccelBias { double b[3]; };
+__global__ void odom_gyro_kernel(se3::Gyro g, int stride, AccelBias acc, const double* __restrict__ smp,
+                                 const double* __restrict__ ft, const long long* __restrict__ range,
+                                 const long long* __restrict__ knot_off, int n_frames, double* __restrict__ G,
+                                 double* __restrict__ abg, double* __restrict__ knots) {
     const int d = blockIdx.x * blockDim.x + threadIdx.x;
     if (d >= n_frames || knot_off[d + 1] == knot_off[d]) return;
-    const double* s = smp + (size_t)range[2 * d] * se3::kSampleStride;
+    const double* s = smp + (size_t)range[2 * d] * stride;
     const long long n = range[2 * d + 1] - range[2 * d];
     const double* f = ft + 4 * (size_t)d;
-    se3::gyro_rotation(g, s, n, f[3], f[2], G + 9 * (size_t)d);
-    se3::gyro_knots(g, s, n, f[0], f[2], __dadd_rn(f[0], f[1]), knots + (size_t)knot_off[d] * se3::kKnotStride);
+    se3::gyro_rotation(g, s, n, f[3], f[2], G + 9 * (size_t)d, stride, abg ? acc.b : nullptr,
+                       abg ? abg + 9 * (size_t)d : nullptr);
+    se3::gyro_knots(g, s, n, f[0], f[2], __dadd_rn(f[0], f[1]), knots + (size_t)knot_off[d] * se3::kKnotStride, stride);
+}
+
+// (IMU) Per step, after its loop has ended (one thread per lane j < active): the velocity of the lane's frame
+// step_first + j, which has stopped, from its pose and frame prev[j]'s (se3::imu_velocity).  A sequence's first frame
+// (prior map: prev[j] < 0) keeps the velocity it was given.
+__global__ void odom_velocity_kernel(const IcpState* __restrict__ states, int step_first, int active,
+                                     const int* __restrict__ prev, int n_frames, const double* __restrict__ hist_T,
+                                     OdomImu imu) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= active || prev[j] < 0) return;
+    const int f = step_first + j;
+    double Ra[9], ta[3], R[9], t[3];
+    ref_pose(prev[j], n_frames, states, hist_T, Ra, ta);
+    ref_pose(f, n_frames, states, hist_T, R, t);
+    const double* ft = imu.ft + 4 * (size_t)f;
+    se3::imu_velocity(Ra, ta, t, imu.gravity, imu.abg + 9 * (size_t)f + 6, __dsub_rn(ft[2], ft[3]), imu.v + 3 * (size_t)f);
 }
 
 // Per step, after odom_start_gyro_kernel: odom_deskew_kernel with se3::deskew_point_gyro, the lane's increment
@@ -1562,6 +1603,12 @@ struct OdomSettings {
     // and deskew rotation come from integrated gyro rates
     bool gyro = false;
     se3::Gyro gyro_set{};
+    // accelerometer input (dcreg_icp_run_odometry_imu, dcreg_odometry_open_imu; gyro is set too): every non-anchor
+    // frame's prior translation from the previous frame's velocity and the preintegrated specific force (IMU samples:
+    // se3::kImuStride doubles a row).  v_init [n_seqs][3]: the velocity of every sequence's first frame
+    bool imu = false;
+    double accel_bias[3] = {0.0, 0.0, 0.0}, gravity[3] = {0.0, 0.0, 0.0};
+    std::vector<double> v_init;
     // (a session) dcreg_set_sparse_maps and dcreg_set_map_spacing as they were at open; a one-shot call reads the
     // context's
     bool sparse_maps = false;
@@ -1658,6 +1705,9 @@ struct dcreg_ctx {
     // gyroscope input: the call's samples [rows][4], every device frame's (start, span, tm, tm_prev) [n_frames][4], its
     // prior's rotation [n_frames][9] and the knot tables [knots][16] (odom_gyro_kernel)
     DevBuf<double> d_gyro_smp, d_gyro_ft, d_gyro_G, d_gyro_knots;
+    // accelerometer input: every device frame's (alpha, beta, gamma) [n_frames][9], and every frame reference's
+    // velocity [n_frames + retained][3] (OdomImu)
+    DevBuf<double> d_imu_abg, d_imu_v;
     // the adaptive threshold: every sequence's (sse, n) [n_seqs], and the radii of the coming step's lanes [lanes]
     DevBuf<adaptive::State> d_thr_state;
     DevBuf<double> d_lane_radius;
@@ -1679,6 +1729,8 @@ struct dcreg_ctx {
         std::vector<adaptive::State> thr_state;                        // [n_seqs]
         // (set.gyro) every sequence's last committed mid-sweep time (NaN: none yet, or pushed without frame times)
         std::vector<double> last_mid;                                  // [n_seqs]
+        // (set.imu) every sequence's last committed velocity (its v_init before its first frame)
+        std::vector<double> last_v;                                    // [n_seqs][3]
         // (set.prior_map) every sequence's dead-reckoned pose (T_init and the increments alone) of its last frame, the
         // pose its next frame's points are sorted under
         std::vector<double> dr_T;                                      // [n_seqs][16]
@@ -3717,7 +3769,22 @@ static const char* odometry_settings_error(const OdomSettings& set, bool deltas)
         if (!(std::isfinite(g.bias[0]) && std::isfinite(g.bias[1]) && std::isfinite(g.bias[2])))
             return "gyro: bias has an entry that is not finite";
     }
+    if (set.imu) {
+        bool finite = true;
+        for (int i = 0; i < 3; ++i) finite = finite && std::isfinite(set.accel_bias[i]);
+        if (!finite) return "imu: accel_bias has an entry that is not finite";
+        for (int i = 0; i < 3; ++i) finite = finite && std::isfinite(set.gravity[i]);
+        if (!finite) return "imu: gravity has an entry that is not finite";
+    }
     return nullptr;
+}
+
+// (IMU) The sequence whose v_init has an entry that is not finite, as a message, or empty
+static std::string v_init_error(const OdomSettings& set) {
+    for (size_t i = 0; set.imu && i < set.v_init.size(); ++i)
+        if (!std::isfinite(set.v_init[i]))
+            return "imu: v_init of sequence " + std::to_string(i / 3) + " has an entry that is not finite";
+    return std::string();
 }
 
 // A step's maps (or a session's final voxel-map update): segment b is points [d_seg[b], d_seg[b + 1]) of `map` (null:
@@ -3732,10 +3799,14 @@ struct StepMap {
 
 // The gyro input of a call or push (dcreg_icp_run_odometry_gyro, dcreg_odometry_push_gyro): frame_times [n_frames][2]
 // (start, span), samples [rows][4] (t, wx, wy, wz), sequence s's rows [sample_offsets[s], sample_offsets[s + 1])
+// (dcreg_icp_run_odometry_imu, dcreg_odometry_push_imu) samples [rows][7] (t, wx, wy, wz, ax, ay, az): stride
+// se3::kImuStride, and velocity (out, may be null) [n_frames][3]
 struct GyroInput {
     const double* frame_times = nullptr;
     const double* samples = nullptr;
     const int64_t* sample_offsets = nullptr;
+    int stride = se3::kSampleStride;
+    double* velocity = nullptr;
 };
 
 // One odometry call or push (run_odometry): its arguments, what its phases share, and the phases, in the order they run
@@ -3800,6 +3871,10 @@ struct OdomCall {
     std::vector<double> next_mid;
     size_t gyro_ll = 0;
     long long gyro_knots = 0;
+    // (set.imu) every frame reference's velocity in device order [n_frames + retained][3]: v_init (a first frame), the
+    // session's last (a sequence's last retained frame), then the frames' as the call computed them (finish)
+    std::vector<double> imu_v;
+    OdomImu imu_dev;                                // (set.imu, samples given) what the kernels read
 
     int check(), check_gyro(), upload(), start(), step(int i), finish();
     int prior_grids(int i), window_grids(int i), step_run(int i);
@@ -3925,7 +4000,11 @@ int OdomCall::check() {
     c.lanes = (int)set.lanes.size();
     int rc = check_batch_call(ctx, set.lanes.empty() ? params : set.lanes.data(), c);
     if (rc) return rc;
-    if (!sess) none = odom_plan::History(n_seqs);
+    if (!sess) {
+        const std::string why = v_init_error(set);
+        if (!why.empty()) { ctx->err = std::string(name) + ": " + why; return DCREG_BAD_ARG; }
+        none = odom_plan::History(n_seqs);
+    }
     CK(cudaSetDevice(ctx->device));
     if (timestamps)             // every point's fraction of its sweep, before anything is launched
         for (int s = 0; s < n_seqs; ++s)
@@ -4000,18 +4079,25 @@ int OdomCall::check_gyro() {
     if (!given && (gi.frame_times || gi.samples || gi.sample_offsets))
         return bad("frame_times, samples and sample_offsets are given together or not at all");
     if (!given && !sess) return bad("gyro input needs frame_times, samples and sample_offsets");
+    const int sw = gi.stride;
+    if (given && set.imu && sw != se3::kImuStride)
+        return bad("a session opened with IMU input takes 7-column samples (dcreg_odometry_push_imu)");
+    if (given && !set.imu && sw != se3::kSampleStride)
+        return bad("7-column IMU samples need a session opened with IMU input (dcreg_odometry_open_imu)");
     const int64_t* so = gi.sample_offsets;
     if (given) {
         if (so[0] != 0) return bad("sample_offsets[0] must be 0");
         for (int s = 0; s < n_seqs; ++s) {
             if (so[s + 1] < so[s]) return bad("sample_offsets must be non-decreasing");
             for (int64_t i = so[s]; i < so[s + 1]; ++i) {
-                const double* r = gi.samples + (size_t)i * se3::kSampleStride;
+                const double* r = gi.samples + (size_t)i * sw;
                 const std::string at = "sequence " + std::to_string(s) + ", sample " + std::to_string(i - so[s]) +
                                        " (row " + std::to_string(i) + ")";
                 if (!(std::isfinite(r[0]) && std::isfinite(r[1]) && std::isfinite(r[2]) && std::isfinite(r[3])))
                     return bad(at + ": a value that is not finite");
-                if (i > so[s] && !(r[0] > r[-se3::kSampleStride]))
+                for (int c = 4; c < sw; ++c)
+                    if (!std::isfinite(r[c])) return bad(at + ": an accelerometer value that is not finite");
+                if (i > so[s] && !(r[0] > r[-sw]))
                     return bad(at + ": its time is not after the previous sample's (times must be strictly ascending)");
             }
         }
@@ -4022,7 +4108,7 @@ int OdomCall::check_gyro() {
     for (int s = 0; s < n_seqs; ++s) {
         const bool started = sess && hist.seen[(size_t)s] > 0;
         double prev = sess ? sess->last_mid[(size_t)s] : NAN;
-        const double* sm = given ? gi.samples + (size_t)so[s] * se3::kSampleStride : nullptr;
+        const double* sm = given ? gi.samples + (size_t)so[s] * sw : nullptr;
         const long long ns = given ? so[s + 1] - so[s] : 0;
         for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k) {
             const bool anchor = !started && k == seq_offsets[s];
@@ -4046,10 +4132,10 @@ int OdomCall::check_gyro() {
                     return bad(frame_name(s, k) + ": its mid-sweep time " + std::to_string(tm) +
                                " is not after the previous frame's, " + std::to_string(prev));
                 const double lo = std::min(prev, start);
-                if (se3::gyro_last(sm, ns, lo, false) < 0)
+                if (se3::gyro_last(sm, ns, lo, false, sw) < 0)
                     return bad(frame_name(s, k) + ": no gyro sample at or before " + std::to_string(lo) +
                                " (the previous mid-sweep time or the sweep's start)");
-                if (ns == 0 || sm[(size_t)(ns - 1) * se3::kSampleStride] < end)
+                if (ns == 0 || sm[(size_t)(ns - 1) * sw] < end)
                     return bad(frame_name(s, k) + ": no gyro sample at or after the sweep's end, " + std::to_string(end));
             }
             const double f[4] = {start, span, tm, prev};
@@ -4127,8 +4213,9 @@ int OdomCall::upload() {
             const int64_t* so = gi.sample_offsets;
             const int s = frame_seq_of(k);
             hll.push_back(hll.back() + (gyro_anchor[(size_t)k] ? 0
-                                        : se3::gyro_knot_count(gi.samples + (size_t)so[s] * se3::kSampleStride,
-                                                               so[s + 1] - so[s], f[0], f[2], f[0] + f[1], &nb)));
+                                        : se3::gyro_knot_count(gi.samples + (size_t)so[s] * gi.stride,
+                                                               so[s + 1] - so[s], f[0], f[2], f[0] + f[1], &nb,
+                                                               gi.stride)));
         }
         gyro_knots = hll.back();
         for (int d = 0; d < n_frames; ++d) {
@@ -4213,6 +4300,17 @@ int OdomCall::upload() {
 // = T_init, no iteration, not converged), and (timestamps) the caller's timestamps beside the packed points
 int OdomCall::start() {
     int rc;
+    if (set.imu) {
+        const int n_hist = (int)hist.n.size();
+        imu_v.assign((size_t)(n_frames + n_hist) * 3, 0.0);
+        for (int s = 0; s < n_seqs; ++s) {
+            for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k)
+                std::copy(&set.v_init[(size_t)s * 3], &set.v_init[(size_t)s * 3] + 3, &imu_v[(size_t)P.dev[(size_t)k] * 3]);
+            if (hist.off[(size_t)s + 1] > hist.off[(size_t)s])
+                std::copy(&sess->last_v[(size_t)s * 3], &sess->last_v[(size_t)s * 3] + 3,
+                          &imu_v[(size_t)(n_frames + hist.off[(size_t)s + 1] - 1) * 3]);
+        }
+    }
     std::vector<double> T_dev((size_t)n_frames * 16), ident((size_t)n_frames * 16, 0.0);
     for (int s = 0; s < n_seqs; ++s)
         for (int k = seq_offsets[s]; k < seq_offsets[s + 1]; ++k)
@@ -4277,18 +4375,30 @@ int OdomCall::start() {
         std::vector<double> ft((size_t)n_frames * 4);
         for (int d = 0; d < n_frames; ++d)
             std::copy(&gyro_ft[(size_t)P.input[(size_t)d] * 4], &gyro_ft[(size_t)P.input[(size_t)d] * 4] + 4, &ft[(size_t)d * 4]);
-        CK(ctx->d_gyro_smp.ensure(std::max<long long>(rows * se3::kSampleStride, 1)));
+        CK(ctx->d_gyro_smp.ensure(std::max<long long>(rows * gi.stride, 1)));
         CK(ctx->d_gyro_ft.ensure((long long)ft.size()));
         CK(ctx->d_gyro_G.ensure((long long)n_frames * 9));
         CK(ctx->d_gyro_knots.ensure(std::max<long long>(gyro_knots * se3::kKnotStride, 1)));
         if (rows)
-            CK(cudaMemcpyAsync(ctx->d_gyro_smp, gi.samples, (size_t)rows * se3::kSampleStride * sizeof(double),
+            CK(cudaMemcpyAsync(ctx->d_gyro_smp, gi.samples, (size_t)rows * gi.stride * sizeof(double),
                                cudaMemcpyHostToDevice, ctx->stream));
         CK(cudaMemcpyAsync(ctx->d_gyro_ft, ft.data(), ft.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        if (set.imu) {          // (IMU) the preintegrals' room, and every frame reference's velocity as it starts
+            CK(ctx->d_imu_abg.ensure((long long)n_frames * 9));
+            CK(ctx->d_imu_v.ensure((long long)imu_v.size()));
+            CK(cudaMemcpyAsync(ctx->d_imu_v, imu_v.data(), imu_v.size() * sizeof(double), cudaMemcpyHostToDevice,
+                               ctx->stream));
+            imu_dev.ft = ctx->d_gyro_ft;
+            imu_dev.abg = ctx->d_imu_abg;
+            imu_dev.v = ctx->d_imu_v;
+            std::copy(set.gravity, set.gravity + 3, imu_dev.gravity);
+        }
+        AccelBias acc{};
+        std::copy(set.accel_bias, set.accel_bias + 3, acc.b);
         const long long* d_knot_off = ctx->d_odom_ll + gyro_ll;
         odom_gyro_kernel<<<(unsigned)((n_frames + 127) / 128), 128, 0, ctx->stream>>>(
-            set.gyro_set, ctx->d_gyro_smp, ctx->d_gyro_ft, d_knot_off + n_frames + 1, d_knot_off, n_frames,
-            ctx->d_gyro_G, ctx->d_gyro_knots);
+            set.gyro_set, gi.stride, acc, ctx->d_gyro_smp, ctx->d_gyro_ft, d_knot_off + n_frames + 1, d_knot_off,
+            n_frames, ctx->d_gyro_G, set.imu ? ctx->d_imu_abg.p : nullptr, ctx->d_gyro_knots);
         ctx->launches++;
         CK(cudaGetLastError());
     }
@@ -4426,7 +4536,7 @@ int OdomCall::step_run(int i) {
         odom_start_gyro_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
             ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active,
             n_seqs, st.first, st.active, d_prev, d_prev2, n_frames, d_hist_T, ctx->d_gyro_G,
-            timestamps ? ctx->d_odom_xi.p : nullptr, ctx->d_scan_radius);
+            timestamps ? ctx->d_odom_xi.p : nullptr, ctx->d_scan_radius, imu_dev);
     else
         odom_start_kernel<<<(unsigned)((n_seqs + 127) / 128), 128, 0, ctx->stream>>>(
             ctx->d_state, ctx->d_scan_seg, ctx->d_seq_prior, ctx->d_seq_cursor, ctx->d_seq_first, ctx->d_n_active, n_seqs,
@@ -4488,6 +4598,13 @@ int OdomCall::step_run(int i) {
     if (lanes.n)            // the sequence each lane of this step runs (the lanes' settings are the sequences')
         CK(cudaMemcpyAsync(ctx->d_lane_seq, st.seq.data(), st.seq.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = run_chunks(ctx, LP, params, dlog, dlog ? R.log_cap : 0, params->max_iterations, 16, true))) return rc;
+    // 4b. (IMU) the step's frames' velocities, which the next step's priors read
+    if (imu_dev.v) {
+        odom_velocity_kernel<<<(unsigned)((st.active + 127) / 128), 128, 0, ctx->stream>>>(
+            ctx->d_state, st.first, st.active, d_prev, n_frames, d_hist_T, imu_dev);
+        ctx->launches++;
+        CK(cudaGetLastError());
+    }
     // 5. (adaptive) the step's frames into their sequences' threshold states, and the next step's radii
     if (set.adaptive) {
         const int* d_seq = d_prev2 + st.active;
@@ -4561,8 +4678,21 @@ int OdomCall::finish() {
             }
         }
     }
+    if (imu_dev.v) {            // (IMU) the frames' velocities (imu_v keeps v_init without samples: anchors alone)
+        CK(cudaMemcpyAsync(imu_v.data(), ctx->d_imu_v, (size_t)n_frames * 3 * sizeof(double), cudaMemcpyDeviceToHost,
+                           ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+    }
+    if (set.imu && gi.velocity)
+        for (int k = 0; k < n_frames; ++k)
+            std::copy(&imu_v[(size_t)P.dev[(size_t)k] * 3], &imu_v[(size_t)P.dev[(size_t)k] * 3] + 3, gi.velocity + (size_t)k * 3);
     if (sess) {
         commit_push(*sess, U, n_frames, seq_offsets, R.T_out, deltas);
+        if (set.imu)
+            for (int s = 0; s < n_seqs; ++s)
+                if (seq_offsets[s + 1] > seq_offsets[s])
+                    std::copy(&imu_v[(size_t)P.dev[(size_t)(seq_offsets[s + 1] - 1)] * 3],
+                              &imu_v[(size_t)P.dev[(size_t)(seq_offsets[s + 1] - 1)] * 3] + 3, &sess->last_v[(size_t)s * 3]);
         if (set.voxel_map) sess->map_off.assign(sm.kept.begin(), sm.kept.end());
         if (set.adaptive) sess->thr_state.swap(thr);
         if (set.gyro)
@@ -4752,7 +4882,48 @@ int dcreg_icp_run_odometry_gyro(dcreg_ctx* ctx, const dcreg_icp_params* params, 
                         gyro ? GyroInput{frame_times, samples, sample_offsets} : GyroInput{});
 }
 
-// Opens the context's one session with the settings `set` (dcreg_odometry_open, _open_map, _open_adaptive, _open_gyro)
+// the settings of dcreg_icp_run_odometry_imu / dcreg_odometry_open_imu: the gyro call's, with the gyro and the
+// accelerometer when imu is given (v_init null: every sequence starts at rest)
+static OdomSettings odom_imu_settings(OdomSettings set, const dcreg_imu* imu, const double* v_init) {
+    if (!imu) return set;
+    dcreg_gyro g;
+    std::copy(imu->R_sensor_imu, imu->R_sensor_imu + 9, g.R_sensor_imu);
+    std::copy(imu->gyro_bias, imu->gyro_bias + 3, g.bias);
+    set = odom_gyro_settings(set, &g);
+    set.imu = true;
+    std::copy(imu->accel_bias, imu->accel_bias + 3, set.accel_bias);
+    std::copy(imu->gravity, imu->gravity + 3, set.gravity);
+    set.v_init.assign((size_t)std::max(set.n_seqs, 0) * 3, 0.0);
+    if (v_init) std::copy(v_init, v_init + set.v_init.size(), set.v_init.begin());
+    return set;
+}
+
+int dcreg_icp_run_odometry_imu(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                               int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                               double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                               int source_max_points, int map_max_points, double max_distance,
+                               const dcreg_adaptive_threshold* adaptive, const dcreg_imu* imu, const double* T_init,
+                               const double* v_init, const double* deltas, const float* timestamps,
+                               const double* frame_times, const double* samples, const int64_t* sample_offsets,
+                               int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                               int* status, double* cov, float* deskewed_xyz, double* search_radius, double* velocity,
+                               dcreg_iter_log* log, int log_cap) {
+    return run_odometry(ctx, "icp_run_odometry_imu",
+                        with_map_input(odom_imu_settings(odom_adaptive_settings(params, n_seqs, cell_size, map_frames,
+                                                                                motion, source_voxel, map_voxel,
+                                                                                source_max_points, map_max_points,
+                                                                                max_distance, adaptive, T_init,
+                                                                                ctx && ctx->lane_params),
+                                                         imu, v_init),
+                                       ctx),
+                        nullptr, seq_offsets, n_frames, xyz, frame_offsets, stride, deltas, timestamps,
+                        Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior}, frame_points,
+                        deskewed_xyz, search_radius,
+                        imu ? GyroInput{frame_times, samples, sample_offsets, se3::kImuStride, velocity} : GyroInput{});
+}
+
+// Opens the context's one session with the settings `set` (dcreg_odometry_open, _open_map, _open_adaptive, _open_gyro,
+// _open_imu)
 static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& set) {
     if (ctx->odom) {
         ctx->err = std::string(name) + ": a session is open already (dcreg_odometry_close it first)";
@@ -4777,6 +4948,9 @@ static int open_session(dcreg_ctx* ctx, const char* name, const OdomSettings& se
     c.lanes = (int)ss->set.lanes.size();
     const int rc = check_batch_call(ctx, ss->set.lanes.empty() ? &ss->set.params : ss->set.lanes.data(), c);
     if (rc) return rc;
+    const std::string why = v_init_error(ss->set);
+    if (!why.empty()) { ctx->err = std::string(name) + ": " + why; return DCREG_BAD_ARG; }
+    ss->last_v = ss->set.v_init;
     ss->hist = odom_plan::History(n_seqs);
     ss->map_off.assign((size_t)n_seqs + 1, 0);
     ss->thr_state.assign((size_t)n_seqs, adaptive::State{0.0, 0});
@@ -4829,6 +5003,19 @@ int dcreg_odometry_open_gyro(dcreg_ctx* ctx, const dcreg_icp_params* params, int
                                                                   map_max_points, max_distance, adaptive, T_init,
                                                                   ctx && ctx->lane_params),
                                            gyro));
+}
+
+int dcreg_odometry_open_imu(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
+                            int motion, double source_voxel, double map_voxel, int source_max_points, int map_max_points,
+                            double max_distance, const dcreg_adaptive_threshold* adaptive, const dcreg_imu* imu,
+                            const double* T_init, const double* v_init) {
+    if (!ctx) return DCREG_BAD_ARG;
+    return open_session(ctx, "odometry_open_imu",
+                        odom_imu_settings(odom_adaptive_settings(params, n_seqs, cell_size, map_frames, motion,
+                                                                 source_voxel, map_voxel, source_max_points,
+                                                                 map_max_points, max_distance, adaptive, T_init,
+                                                                 ctx && ctx->lane_params),
+                                          imu, v_init));
 }
 
 int dcreg_odometry_local_map(dcreg_ctx* ctx, int seq, float* xyz, int64_t cap, int64_t* n) {
@@ -4914,6 +5101,21 @@ int dcreg_odometry_push_gyro(dcreg_ctx* ctx, const int* seq_offsets, int n_frame
     return run_odometry(ctx, "odometry_push_gyro", ss.set, &ss, seq_offsets, n_frames, xyz, frame_offsets, stride,
                         deltas, timestamps, Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior},
                         frame_points, deskewed_xyz, search_radius, GyroInput{frame_times, samples, sample_offsets});
+}
+
+int dcreg_odometry_push_imu(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
+                            const int64_t* frame_offsets, int stride, const double* deltas, const float* timestamps,
+                            const double* frame_times, const double* samples, const int64_t* sample_offsets,
+                            int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                            int* status, double* cov, float* deskewed_xyz, double* search_radius, double* velocity,
+                            dcreg_iter_log* log, int log_cap) {
+    if (!ctx) return DCREG_BAD_ARG;
+    if (!ctx->odom) { ctx->err = "odometry_push_imu: no session is open (dcreg_odometry_open_imu)"; return DCREG_BAD_ARG; }
+    dcreg_ctx::OdomSession& ss = *ctx->odom;
+    return run_odometry(ctx, "odometry_push_imu", ss.set, &ss, seq_offsets, n_frames, xyz, frame_offsets, stride,
+                        deltas, timestamps, Results{T_out, n_iterations, converged, status, log, log_cap, cov, T_prior},
+                        frame_points, deskewed_xyz, search_radius,
+                        GyroInput{frame_times, samples, sample_offsets, se3::kImuStride, velocity});
 }
 
 // The session's buffers go with it; nothing queued may still read them

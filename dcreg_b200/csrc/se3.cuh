@@ -148,8 +148,10 @@ struct Gyro {
     double bias[3];
 };
 
-// Rows of a sample array: (t, wx, wy, wz), t strictly ascending
+// Rows of a sample array: (t, wx, wy, wz), t strictly ascending; with an accelerometer (dcreg_icp_run_odometry_imu)
+// (t, wx, wy, wz, ax, ay, az).  Every function below that reads samples takes the row stride, the gyro's by default
 constexpr int kSampleStride = 4;
+constexpr int kImuStride = 7;
 // One knot of a sweep's table: time, Q = G(t_m -> time) row-major, the rate after the knot, the rate before it
 constexpr int kKnotStride = 16;
 
@@ -190,11 +192,19 @@ SE3_HD void mat3_mul_right(double* M, const double* E) {
 }
 
 // The rate of sample j in the LiDAR frame: R_si (omega_j - bias), each entry ((r0 d0 + r1 d1) + r2 d2)
-SE3_HD void gyro_rate(const Gyro& g, const double* smp, long long j, double* w) {
-    const double* s = smp + (size_t)j * kSampleStride;
+SE3_HD void gyro_rate(const Gyro& g, const double* smp, long long j, double* w, int stride = kSampleStride) {
+    const double* s = smp + (size_t)j * stride;
     const double d[3] = {SE3_SUB(s[1], g.bias[0]), SE3_SUB(s[2], g.bias[1]), SE3_SUB(s[3], g.bias[2])};
     for (int r = 0; r < 3; ++r)
         w[r] = SE3_ADD(SE3_ADD(SE3_MUL(g.R_si[3 * r], d[0]), SE3_MUL(g.R_si[3 * r + 1], d[1])), SE3_MUL(g.R_si[3 * r + 2], d[2]));
+}
+
+// The specific force of IMU sample j (kImuStride rows) in the LiDAR frame: R_si (acc_j - acc_bias), gyro_rate's order
+SE3_HD void accel_force(const Gyro& g, const double* acc_bias, const double* smp, long long j, double* f) {
+    const double* s = smp + (size_t)j * kImuStride;
+    const double d[3] = {SE3_SUB(s[4], acc_bias[0]), SE3_SUB(s[5], acc_bias[1]), SE3_SUB(s[6], acc_bias[2])};
+    for (int r = 0; r < 3; ++r)
+        f[r] = SE3_ADD(SE3_ADD(SE3_MUL(g.R_si[3 * r], d[0]), SE3_MUL(g.R_si[3 * r + 1], d[1])), SE3_MUL(g.R_si[3 * r + 2], d[2]));
 }
 
 // M = M Exp(w d): one zero-order-hold piece of d seconds (d < 0: walked backwards)
@@ -206,11 +216,11 @@ SE3_HD void gyro_piece(double* M, const double* w, double d) {
 }
 
 // The last sample j in [0, n) with t_j <= t (strict: t_j < t), or -1
-SE3_HD long long gyro_last(const double* smp, long long n, double t, bool strict) {
+SE3_HD long long gyro_last(const double* smp, long long n, double t, bool strict, int stride = kSampleStride) {
     long long lo = 0, hi = n;           // the first sample past t is in [lo, hi]
     while (lo < hi) {
         const long long mid = lo + (hi - lo) / 2;
-        const double tm = smp[(size_t)mid * kSampleStride];
+        const double tm = smp[(size_t)mid * stride];
         if (strict ? tm < t : tm <= t) lo = mid + 1;
         else hi = mid;
     }
@@ -220,26 +230,76 @@ SE3_HD long long gyro_last(const double* smp, long long n, double t, bool strict
 // G(a -> b), a <= b, over n samples: the walk from a to b in time order, M = I then M = M Exp(w_j d_j) for every sample
 // interval [t_j, t_{j+1}) clipped to [a, b] with d_j > 0, w_j the rate of sample j (zero-order hold).  Needs a sample at
 // or before a and one at or after b (the caller checks); it reads no sample outside them.
-SE3_HD void gyro_rotation(const Gyro& g, const double* smp, long long n, double a, double b, double* G) {
+//
+// With acc_bias (IMU samples, stride kImuStride) the same walk preintegrates the accelerometer into abg[9] = (alpha,
+// beta, gamma): over every piece [u, u + d], M the walk's rotation at u (before the piece) and f = R_si (acc_j -
+// acc_bias) (accel_force), both held over the piece (a first-order rule), m = M f d (each entry ((m0 f0 + m1 f1) + m2
+// f2) d) and alpha += m, beta += m ((b - u) - 0.5 d), gamma += m ((u - a) + 0.5 d), from zero.  G is the gyro's walk,
+// bit for bit.
+SE3_HD void gyro_rotation(const Gyro& g, const double* smp, long long n, double a, double b, double* G,
+                          int stride = kSampleStride, const double* acc_bias = nullptr, double* abg = nullptr) {
     for (int i = 0; i < 9; ++i) G[i] = (i % 4 == 0) ? 1.0 : 0.0;
-    long long j = gyro_last(smp, n, a, false);
+    if (acc_bias)
+        for (int i = 0; i < 9; ++i) abg[i] = 0.0;
+    long long j = gyro_last(smp, n, a, false, stride);
     double cur = a;
     while (cur < b) {
-        const double t1 = smp[(size_t)(j + 1) * kSampleStride];
+        const double t1 = smp[(size_t)(j + 1) * stride];
         const double nxt = t1 < b ? t1 : b;
+        const double d = SE3_SUB(nxt, cur);
+        if (acc_bias) {
+            double f[3];
+            accel_force(g, acc_bias, smp, j, f);
+            const double h = SE3_MUL(0.5, d);
+            const double wb = SE3_SUB(SE3_SUB(b, cur), h), wg = SE3_ADD(SE3_SUB(cur, a), h);
+            for (int r = 0; r < 3; ++r) {
+                const double m = SE3_MUL(SE3_ADD(SE3_ADD(SE3_MUL(G[3 * r], f[0]), SE3_MUL(G[3 * r + 1], f[1])),
+                                                 SE3_MUL(G[3 * r + 2], f[2])),
+                                         d);
+                abg[r] = SE3_ADD(abg[r], m);
+                abg[3 + r] = SE3_ADD(abg[3 + r], SE3_MUL(m, wb));
+                abg[6 + r] = SE3_ADD(abg[6 + r], SE3_MUL(m, wg));
+            }
+        }
         double w[3];
-        gyro_rate(g, smp, j, w);
-        gyro_piece(G, w, SE3_SUB(nxt, cur));
+        gyro_rate(g, smp, j, w, stride);
+        gyro_piece(G, w, d);
         cur = nxt;
         ++j;
     }
 }
 
+// The accelerometer's prior translation (dcreg_icp_run_odometry_imu) over [tm_prev, tm], dt = tm - tm_prev, from the
+// previous frame's pose (R row-major) and velocity v, gravity grav (world frame) and beta: t_D = dt R^T v + (0.5 dt^2)
+// R^T g + beta, every R^T x entry ((R_0r x0 + R_1r x1) + R_2r x2), summed in that order
+SE3_HD void imu_translation(const double* R, const double* v, const double* grav, const double* beta, double dt,
+                            double* tD) {
+    const double c2 = SE3_MUL(0.5, SE3_MUL(dt, dt));
+    for (int r = 0; r < 3; ++r) {
+        const double rv = SE3_ADD(SE3_ADD(SE3_MUL(R[r], v[0]), SE3_MUL(R[3 + r], v[1])), SE3_MUL(R[6 + r], v[2]));
+        const double rg = SE3_ADD(SE3_ADD(SE3_MUL(R[r], grav[0]), SE3_MUL(R[3 + r], grav[1])), SE3_MUL(R[6 + r], grav[2]));
+        tD[r] = SE3_ADD(SE3_ADD(SE3_MUL(dt, rv), SE3_MUL(c2, rg)), beta[r]);
+    }
+}
+
+// A frame's velocity once it has stopped: v = (t - t_prev) / dt + (R_prev gamma) / dt + (0.5 dt) g (world frame), the
+// exact kinematic identity for the held inputs, every R gamma entry ((r0 g0 + r1 g1) + r2 g2)
+SE3_HD void imu_velocity(const double* R_prev, const double* t_prev, const double* t, const double* grav,
+                         const double* gamma, double dt, double* v) {
+    const double h = SE3_MUL(0.5, dt);
+    for (int r = 0; r < 3; ++r) {
+        const double rg = SE3_ADD(SE3_ADD(SE3_MUL(R_prev[3 * r], gamma[0]), SE3_MUL(R_prev[3 * r + 1], gamma[1])),
+                                  SE3_MUL(R_prev[3 * r + 2], gamma[2]));
+        v[r] = SE3_ADD(SE3_ADD(SE3_SUB(t[r], t_prev[r]) / dt, rg / dt), SE3_MUL(h, grav[r]));
+    }
+}
+
 // The knots of a sweep [start, end] with mid-sweep tm: tm, and every sample time strictly inside (start, end) other
 // than tm.  Returns how many lie before tm (*before) and in all.
-SE3_HD int gyro_knot_count(const double* smp, long long n, double start, double tm, double end, int* before) {
-    const long long lo = gyro_last(smp, n, start, false), m0 = gyro_last(smp, n, tm, true),
-                    m1 = gyro_last(smp, n, tm, false), hi = gyro_last(smp, n, end, true);
+SE3_HD int gyro_knot_count(const double* smp, long long n, double start, double tm, double end, int* before,
+                           int stride = kSampleStride) {
+    const long long lo = gyro_last(smp, n, start, false, stride), m0 = gyro_last(smp, n, tm, true, stride),
+                    m1 = gyro_last(smp, n, tm, false, stride), hi = gyro_last(smp, n, end, true, stride);
     *before = (int)(m0 - lo);
     return 1 + (int)(m0 - lo) + (int)(hi - m1);
 }
@@ -248,40 +308,41 @@ SE3_HD int gyro_knot_count(const double* smp, long long n, double start, double 
 // from tm to the knot forms it (forwards: M = M Exp(w d); backwards: the same with d < 0, which is G(time -> tm)^T up
 // to rounding), the rate after the knot (of the last sample at or before it) and the rate before it (of the last sample
 // strictly before it).  Needs a sample at or before start and one at or after end.
-SE3_HD void gyro_knots(const Gyro& g, const double* smp, long long n, double start, double tm, double end, double* K) {
+SE3_HD void gyro_knots(const Gyro& g, const double* smp, long long n, double start, double tm, double end, double* K,
+                       int stride = kSampleStride) {
     int nb = 0;
-    gyro_knot_count(smp, n, start, tm, end, &nb);
+    gyro_knot_count(smp, n, start, tm, end, &nb, stride);
     double Q[9];
     double* k = K + (size_t)nb * kKnotStride;           // tm's knot
     for (int i = 0; i < 9; ++i) Q[i] = (i % 4 == 0) ? 1.0 : 0.0;
-    long long ja = gyro_last(smp, n, tm, false), jb = gyro_last(smp, n, tm, true);
+    long long ja = gyro_last(smp, n, tm, false, stride), jb = gyro_last(smp, n, tm, true, stride);
     k[0] = tm;
     for (int i = 0; i < 9; ++i) k[1 + i] = Q[i];
-    gyro_rate(g, smp, ja, k + 10);
-    gyro_rate(g, smp, jb, k + 13);
+    gyro_rate(g, smp, ja, k + 10, stride);
+    gyro_rate(g, smp, jb, k + 13, stride);
     double cur = tm;                                    // backwards: the samples in (start, tm), newest first
     for (int i = nb - 1; i >= 0; --i) {
-        const double t = smp[(size_t)jb * kSampleStride];
+        const double t = smp[(size_t)jb * stride];
         double* o = K + (size_t)i * kKnotStride;
         gyro_piece(Q, K + (size_t)(i + 1) * kKnotStride + 13, SE3_SUB(t, cur));
         cur = t;
         o[0] = t;
         for (int c = 0; c < 9; ++c) o[1 + c] = Q[c];
-        gyro_rate(g, smp, jb, o + 10);
-        gyro_rate(g, smp, jb - 1, o + 13);
+        gyro_rate(g, smp, jb, o + 10, stride);
+        gyro_rate(g, smp, jb - 1, o + 13, stride);
         --jb;
     }
     for (int i = 0; i < 9; ++i) Q[i] = (i % 4 == 0) ? 1.0 : 0.0;
     cur = tm;                                           // forwards: the samples in (tm, end)
-    for (double* o = k + kKnotStride; ja + 1 < n && smp[(size_t)(ja + 1) * kSampleStride] < end; o += kKnotStride) {
-        const double t = smp[(size_t)(ja + 1) * kSampleStride];
+    for (double* o = k + kKnotStride; ja + 1 < n && smp[(size_t)(ja + 1) * stride] < end; o += kKnotStride) {
+        const double t = smp[(size_t)(ja + 1) * stride];
         gyro_piece(Q, o - kKnotStride + 10, SE3_SUB(t, cur));
         cur = t;
         ++ja;
         o[0] = t;
         for (int c = 0; c < 9; ++c) o[1 + c] = Q[c];
-        gyro_rate(g, smp, ja, o + 10);
-        gyro_rate(g, smp, ja - 1, o + 13);
+        gyro_rate(g, smp, ja, o + 10, stride);
+        gyro_rate(g, smp, ja - 1, o + 13, stride);
     }
 }
 

@@ -257,6 +257,88 @@ def make_parking_imu(n_frames, rate_hz=200, noise=0.0, bias=(0.0, 0.0, 0.0), see
     return skewed, stamps, frame_times, samples, T_true, frames
 
 
+def make_parking_imu_accel(n_frames, rate_hz=200, gyro_noise=0.0, accel_noise=0.0, gyro_bias=(0.0, 0.0, 0.0),
+                           accel_bias=(0.0, 0.0, 0.0), gravity=(0.0, 0.0, -9.80665), R_sensor_imu=None, seed=73,
+                           period=0.1, speed_swing=0.3, shake=0.05, shake_hz=3.0, yaw_swing=0.02, yaw_hz=1.3,
+                           n_scan=6_000, map_seed=43, n_map=500_000, extent=60.0, max_range=30.0,
+                           path_half_length=20.0):
+    """make_parking_frames' map and S-path as a C-infinity trajectory seen by a spinning LiDAR with an IMU at its origin.
+    Time runs over [0, n_frames period]; frame k's sweep is [k period, (k + 1) period), mid-sweep tm_k = (k + 0.5)
+    period.  With u = t / (n_frames period), the path parameter s = -1 + 2 u + speed_swing sin(2 pi u) / pi moves along
+    the path at a speed that varies by +-speed_swing; the position is (L s, L/4 sin(pi s) + shake sin(2 pi shake_hz t),
+    shake sin(2 pi 1.3 shake_hz t)) (L = path_half_length: a lateral and a vertical shake), the yaw follows the path's
+    tangent plus yaw_swing sin(2 pi yaw_hz t), roll and pitch are zero.  Every point is measured from the analytic pose
+    at its own time t = k period + tau period, tau = (azimuth + pi) / (2 pi) from the unskewed frame (the map points
+    within max_range of the mid-sweep pose, thinned to about n_scan, plus 5 mm noise, in the mid-sweep sensor frame).
+    The IMU samples, at t = j / rate_hz from one sample before 0 to one past the end, are the analytic body rate and
+    specific force R(t)^T (x''(t) - gravity) in the IMU frame (R_sensor_imu^T times the LiDAR-frame vectors), plus the
+    biases and seeded white noise.  Returns (skewed frames, timestamps, frame_times (n, 2) (start, span), samples (m, 7)
+    (t, wx, wy, wz, ax, ay, az), T_true (n, 4, 4) mid-sweep poses, v_true (n, 3) world-frame mid-sweep velocities,
+    unskewed frames)."""
+    tgt = _parking_map(np.random.default_rng(map_seed), n_map, extent)
+    rng = np.random.default_rng(seed)
+    L, total = float(path_half_length), n_frames * float(period)
+    g = np.asarray(gravity, dtype=np.float64).reshape(3)
+    a_c, wl, wz, wy = 0.25 * math.pi, 2 * math.pi * shake_hz, 2 * math.pi * 1.3 * shake_hz, 2 * math.pi * yaw_hz
+
+    def state(t):
+        """position, velocity, acceleration (each (len(t), 3)), yaw and yaw rate (each (len(t),)) at times t"""
+        t = np.asarray(t, dtype=np.float64)
+        u = t / total
+        s = -1.0 + 2.0 * u + speed_swing * np.sin(2 * math.pi * u) / math.pi
+        s1 = (2.0 + 2.0 * speed_swing * np.cos(2 * math.pi * u)) / total
+        s2 = -4.0 * math.pi * speed_swing * np.sin(2 * math.pi * u) / total ** 2
+        ps, pc = np.sin(math.pi * s), np.cos(math.pi * s)
+        x = np.stack([L * s, 0.25 * L * ps + shake * np.sin(wl * t), shake * np.sin(wz * t)], axis=1)
+        v = np.stack([L * s1, 0.25 * L * math.pi * pc * s1 + shake * wl * np.cos(wl * t), shake * wz * np.cos(wz * t)],
+                     axis=1)
+        a = np.stack([L * s2, 0.25 * L * math.pi * (-math.pi * ps * s1 ** 2 + pc * s2) - shake * wl ** 2 * np.sin(wl * t),
+                      -shake * wz ** 2 * np.sin(wz * t)], axis=1)
+        yaw = np.arctan(a_c * pc) + yaw_swing * np.sin(wy * t)
+        rate = -a_c * math.pi * ps * s1 / (1.0 + (a_c * pc) ** 2) + yaw_swing * wy * np.cos(wy * t)
+        return x, v, a, yaw, rate
+
+    def rot(yaw):
+        c, sn = np.cos(yaw), np.sin(yaw)
+        R = np.zeros((len(yaw), 3, 3))
+        R[:, 0, 0], R[:, 0, 1], R[:, 1, 0], R[:, 1, 1], R[:, 2, 2] = c, -sn, sn, c, 1.0
+        return R
+
+    frame_times = np.stack([np.arange(n_frames) * float(period), np.full(n_frames, float(period))], axis=1)
+    tm = frame_times[:, 0] + 0.5 * frame_times[:, 1]
+    x, v_true, _, yaw, _ = state(tm)
+    Rm = rot(yaw)
+    T_true = np.tile(np.eye(4), (n_frames, 1, 1))
+    T_true[:, :3, :3], T_true[:, :3, 3] = Rm, x
+    near0 = np.count_nonzero(np.hypot(tgt[:, 0] - x[0, 0], tgt[:, 1] - x[0, 1]) < max_range)
+    keep_p = min(1.0, n_scan / max(near0, 1))
+    frames, skewed, stamps = [], [], []
+    for k in range(n_frames):
+        near = np.nonzero(np.hypot(tgt[:, 0] - x[k, 0], tgt[:, 1] - x[k, 1]) < max_range)[0]
+        pick = near[rng.random(near.size) < keep_p]
+        pm = tgt[pick].astype(np.float64) + rng.normal(0, 0.005, (pick.size, 3))
+        p = (pm - x[k]) @ Rm[k]                                 # R^T (p - t), row by row
+        frames.append(np.ascontiguousarray(p.astype(np.float32)))
+        tau = np.clip(((np.arctan2(p[:, 1], p[:, 0]) + np.pi) / (2.0 * np.pi)).astype(np.float32), np.float32(0.0),
+                      np.float32(1.0))
+        xt, _, _, yt, _ = state(frame_times[k, 0] + tau.astype(np.float64) * frame_times[k, 1])
+        Rt = rot(yt)
+        q = np.einsum("nji,nj->ni", Rt, pm - xt)               # R(t)^T (p - x(t)) per point
+        skewed.append(np.ascontiguousarray(q.astype(np.float32)))
+        stamps.append(tau)
+    times = np.arange(-1, int(math.ceil(total * rate_hz)) + 2) / float(rate_hz)
+    _, _, a, ys, rate = state(times)
+    Rs = rot(ys)
+    f = np.einsum("nji,nj->ni", Rs, a - g)                      # R^T (x'' - g), the LiDAR frame
+    w = np.stack([np.zeros_like(rate), np.zeros_like(rate), rate], axis=1)
+    Rsi = np.eye(3) if R_sensor_imu is None else np.asarray(R_sensor_imu, dtype=np.float64).reshape(3, 3)
+    nrng = np.random.default_rng([seed, 5])
+    w_imu = w @ Rsi + np.asarray(gyro_bias, dtype=np.float64) + nrng.normal(0.0, gyro_noise, w.shape)
+    f_imu = f @ Rsi + np.asarray(accel_bias, dtype=np.float64) + nrng.normal(0.0, accel_noise, f.shape)
+    samples = np.concatenate([times[:, None], w_imu, f_imu], axis=1)
+    return skewed, stamps, frame_times, samples, T_true, v_true, frames
+
+
 def make_large_map(n_side=4, spacing=1000.0, n_map=500_000, map_seed=43, extent=60.0):
     """A prior map too large for a dense grid: n_side x n_side parking maps (_parking_map, tile t from seed map_seed + t),
     their centres spacing metres apart on a square lattice starting at the origin.  At 0.5 m cells the 4 x 4 default

@@ -735,6 +735,70 @@ int dcreg_odometry_push_gyro(dcreg_ctx* ctx, const int* seq_offsets, int n_frame
                              int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
                              int* status, double* cov, float* deskewed_xyz, double* search_radius, dcreg_iter_log* log,
                              int log_cap);
+/* ACCELEROMETER INPUT: a loosely coupled IMU prior on top of the gyro's.  R_sensor_imu and gyro_bias are dcreg_gyro's;
+ * the IMU sits at the LiDAR origin (no lever arm).  accel_bias (m/s^2) is subtracted from every accelerometer sample;
+ * gravity is the world-frame (T_init's frame) gravity vector, e.g. (0, 0, -9.80665).  Nothing is estimated: no bias, no
+ * gravity and no filter state.  Every frame's velocity comes from the registered poses and the integrated specific
+ * force, so registration corrects it at every frame. */
+typedef struct dcreg_imu {
+    double R_sensor_imu[9];
+    double gyro_bias[3];
+    double accel_bias[3];
+    double gravity[3];
+} dcreg_imu;
+/* dcreg_icp_run_odometry_gyro with accelerometer input.  imu == NULL is the gyro call with gyro == NULL (frame_times,
+ * samples, sample_offsets and v_init are not read, velocity is not written): the same launches and the same bytes.
+ * - Inputs (HOST memory): as the gyro call's, but samples are rows of 7 doubles (t, wx, wy, wz, ax, ay, az) in the IMU
+ *   frame.  v_init: n_seqs x 3, every sequence's world-frame velocity at its first frame's mid-sweep time (NULL: zero).
+ *   velocity (out, may be NULL): n_frames x 3, every frame's world-frame velocity at its mid-sweep time.
+ * - Preintegration of a non-anchor frame k over [a, b] = [tm_{k-1}, tm_k], dt = b - a: the gyro's walk over the same
+ *   zero-order-hold pieces with the same clipping (so G, the rotation, is the gyro call's, bit for bit, and only the
+ *   samples that bracket [a, b] are read).  Over every piece [u, u + d], with M the walk's rotation at u and f = R_si
+ *   (acc_j - accel_bias), both held over the piece (a first-order rule): alpha += M f d, beta += M f d (b - u - d/2),
+ *   gamma += M f d (u + d/2 - a).
+ * - Prior: with R_{k-1}, t_{k-1} = T_out[k-1] and v_{k-1} the previous frame's velocity, t_D = dt R_{k-1}^T v_{k-1} +
+ *   (dt^2 / 2) R_{k-1}^T g + beta and T_prior[k] = compose_prior(T_out[k-1], [G | t_D]).
+ * - Velocity, once frame k has stopped (converged, not converged or aborted: the pose it returned): v_k = (t_k -
+ *   t_{k-1}) / dt + R_{k-1} gamma / dt + (dt / 2) g, the exact kinematic identity for the held inputs.  v_{k-1} cancels
+ *   out of it, so the registered poses re-anchor the velocity at every frame.  An anchor, and a prior-map sequence's
+ *   first frame (dcreg_set_prior_map), has v = v_init[s]; the frame after it uses that velocity.
+ * - Deskew: the gyro's rule, p' = fl32(G(tm_k -> t) p + s t_D), with this t_D.  The translation inside a sweep stays
+ *   first order (no second-order term).
+ * - dcreg_b200.api.imu_preintegrate, imu_increment and imu_velocity are the NumPy twin (bit for bit on the host; the
+ *   device's sin and cos may differ in the last bit).  Everything else (filters, maps, spacing, sparse maps, the adaptive
+ *   threshold, lane params, the prior map, aborts, covariances, reproducibility, the context left untouched) is the gyro
+ *   call's; motion must be DCREG_MOTION_CONSTANT_VELOCITY and deltas NULL.
+ * - Cost over the gyro call: 7 doubles a sample uploaded instead of 4, 9 more doubles per frame written by the call's
+ *   one preintegration launch, one velocity upload, and one launch per step after the loop (one thread per lane).  No
+ *   host sync is added inside the steps; the velocities come back with the results.  Launches do not depend on n_seqs.
+ * Errors (DCREG_BAD_ARG before anything is launched, naming the sequence, frame or sample): every gyro error, and an
+ * accel_bias, gravity or v_init entry (naming the sequence) or an accelerometer value that is not finite. */
+int dcreg_icp_run_odometry_imu(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, const int* seq_offsets,
+                               int n_frames, const float* xyz, const int64_t* frame_offsets, int stride,
+                               double cell_size, int map_frames, int motion, double source_voxel, double map_voxel,
+                               int source_max_points, int map_max_points, double max_distance,
+                               const dcreg_adaptive_threshold* adaptive, const dcreg_imu* imu, const double* T_init,
+                               const double* v_init, const double* deltas, const float* timestamps,
+                               const double* frame_times, const double* samples, const int64_t* sample_offsets,
+                               int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                               int* status, double* cov, float* deskewed_xyz, double* search_radius, double* velocity,
+                               dcreg_iter_log* log, int log_cap);
+/* dcreg_odometry_open_gyro with accelerometer input (imu == NULL: the gyro open with gyro == NULL), and its push.  The
+ * session keeps every sequence's last velocity next to its last mid-sweep time.  Any chunking gives byte for byte the
+ * one dcreg_icp_run_odometry_imu call's outputs, velocity included, under the gyro's rule for bracketing samples.  A push
+ * that fails commits nothing.  Plain pushes (_push, _push_deskew, _push_adaptive, _push_imu without samples) onto an
+ * IMU session follow the gyro's rule: anchors only, which take v_init.  _push_gyro's 4-column samples on an IMU session,
+ * and _push_imu's samples on a session opened without IMU input, are DCREG_BAD_ARG. */
+int dcreg_odometry_open_imu(dcreg_ctx* ctx, const dcreg_icp_params* params, int n_seqs, double cell_size, int map_frames,
+                            int motion, double source_voxel, double map_voxel, int source_max_points, int map_max_points,
+                            double max_distance, const dcreg_adaptive_threshold* adaptive, const dcreg_imu* imu,
+                            const double* T_init, const double* v_init);
+int dcreg_odometry_push_imu(dcreg_ctx* ctx, const int* seq_offsets, int n_frames, const float* xyz,
+                            const int64_t* frame_offsets, int stride, const double* deltas, const float* timestamps,
+                            const double* frame_times, const double* samples, const int64_t* sample_offsets,
+                            int64_t* frame_points, double* T_prior, double* T_out, int* n_iterations, int* converged,
+                            int* status, double* cov, float* deskewed_xyz, double* search_radius, double* velocity,
+                            dcreg_iter_log* log, int log_cap);
 /* Voxel downsampling of many clouds in one call (KISS-ICP's VoxelDownsample rule: the first point of every voxel).
  * xyz / offsets / stride: HOST memory as in dcreg_icp_run_scans (n_clouds + 1 offsets, ascending strictly from 0, at
  * most 2^29 - 1 points).  With inv = 1.0 / voxel in FP64, point i's voxel is (floor((double)x inv), floor((double)y inv),
