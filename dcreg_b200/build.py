@@ -10,7 +10,7 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libdcreg_b200.so")
 SOURCES = ["dcreg_b200.cu"]
-HEADERS = ["corr.cuh", "k1_reduce.cuh", "k1_stream.cuh", "k2_solve.cuh", "k2_fast.cuh", "peer_reduce.cuh", "loop_plan.hpp", "lane_plan.hpp", "arena_plan.hpp", "odom_plan.hpp", "sparse_index.hpp", "se3.cuh", "adaptive_threshold.cuh",
+HEADERS = ["corr.cuh", "cr_fp64.cuh", "k1_reduce.cuh", "k1_stream.cuh", "k2_solve.cuh", "k2_fast.cuh", "peer_reduce.cuh", "loop_plan.hpp", "lane_plan.hpp", "arena_plan.hpp", "odom_plan.hpp", "sparse_index.hpp", "se3.cuh", "adaptive_threshold.cuh",
            "small_la.cuh",
            "../../include/dcreg_b200.h"]
 

@@ -22,6 +22,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "cr_fp64.cuh"
 #include "small_la.cuh"
 #include "sparse_index.hpp"
 
@@ -941,41 +942,85 @@ __global__ void transform_points_kernel(const float4* __restrict__ in, long long
                          (float)(T[8] * px + T[9] * py + T[10] * pz + T[11]), p.w);
 }
 
+// The fit's divisions and square roots by the correctly rounded primitives of cr_fp64.cuh: each ORs "operand outside
+// the exact range" into `bad` instead of branching to the library's slow path.
+struct CrArith {
+    bool& bad;
+    __device__ __forceinline__ double div(double a, double b) const { return crf::div(a, b, bad); }
+    __device__ __forceinline__ double rcp(double b) const { return crf::rcp_step(b, bad); }
+    __device__ __forceinline__ double div_by(double a, double b, double y) const { return crf::div_by(a, b, y, bad); }
+    __device__ __forceinline__ double sqrt(double a) const { return crf::sqrt(a, bad); }
+};
+
 // Plane through the 5 neighbours: least squares of [nb] x = -1, n = x/|x|, d = 1/|x|, gates
 // |x| >= min_norm and max_j (n.nb_j + d)^2 < thickness^2 (icp_test_runner.cpp:1727-1773).
-// Returns true and (n, d) when a valid plane exists.
+// Returns true and (n, d) when a valid plane exists; (n, d) is written whenever |x| >= min_norm.
 // The QR is the register-resident one (small_la.cuh: the same operations in the same order as the generic
-// colpiv_qr_solve, bit-identical results; tools/test_qr_reg.cu).  Inlined into the fit list of the loop kernel: as a
-// separate function under the kernel's 80-register cap it saved and restored the caller's registers and its own spills
-// through local memory on every fit's chain, and its key array (kpos) lived in the stack frame; kpos is the fit list's
-// key row in shared memory (§3, "Fit keys from shared memory, fit inlined").
-// Rejected: a variant of the QR with hardware reciprocal / rsqrt seeds instead of the ~30 IEEE divisions and square
-// roots on the fit's dependent chain shortens a fit, but on exactly rank-deficient neighbourhoods (collinear lattice
-// points) its 1-ulp differences flip the pivoted QR's rank decision and change a correspondence.
-__device__ __forceinline__ bool fit_plane_reg(const Grid& g, const int* kpos, double min_norm, double thickness,
-                                           double& nx, double& ny, double& nz, double& d) {
+// colpiv_qr_solve, bit-identical results; tools/test_qr_reg.cu).  Every division and square root goes through `ar`.
+template <class Ar>
+__device__ __forceinline__ bool fit_plane_ar(const float4* pts, const int* kpos, double min_norm, double thickness,
+                                             double& nx, double& ny, double& nz, double& d, Ar ar) {
     double A[5][3], b[5], x[3];
 #pragma unroll
     for (int j = 0; j < 5; ++j) {
-        const float4 p = __ldg(&g.pts[kpos[j]]);
+        const float4 p = __ldg(&pts[kpos[j]]);
         A[j][0] = (double)p.x;
         A[j][1] = (double)p.y;
         A[j][2] = (double)p.z;
         b[j] = -1.0;
     }
-    dla::colpiv_qr_solve_reg<5, 3>(A, b, x);
-    const double ps = sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
+    dla::colpiv_qr_solve_reg<5, 3>(A, b, x, ar);
+    const double ps = ar.sqrt(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
     if (!(ps >= min_norm)) return false;                 // :1752 (also rejects NaN)
-    nx = x[0] / ps; ny = x[1] / ps; nz = x[2] / ps; d = 1.0 / ps;
+    const double y = ar.rcp(ps);                         // the four divisions by ps share one reciprocal
+    nx = ar.div_by(x[0], ps, y); ny = ar.div_by(x[1], ps, y); nz = ar.div_by(x[2], ps, y); d = ar.div_by(1.0, ps, y);
     double worst = 0.0;
 #pragma unroll
     for (int j = 0; j < 5; ++j) {
-        const float4 p = __ldg(&g.pts[kpos[j]]);
+        const float4 p = __ldg(&pts[kpos[j]]);
         double e = nx * (double)p.x + ny * (double)p.y + nz * (double)p.z + d;
         e *= e;
         worst = fmax(worst, e);
     }
     return worst < thickness * thickness;                // :1772-1773
+}
+
+// The loop's plane fit.  It runs fit_plane_ar with the correctly rounded primitives, whose values are exactly those of
+// `/` and `sqrt` wherever their range flag stays clear, so the pivot choices, the rank cut and the gates see the same
+// bits as with plain arithmetic.  A fit that set the flag (an operand outside the primitives' range: in practice a
+// subnormal, huge or degenerate neighbourhood) discards what it computed and runs again with plain `/` and `sqrt`.
+// The primitives have no branch per operation, so the fit's ~30 serial divisions and square roots form one straight
+// dependent chain and the independent ones (the column norms, the downdates of two columns, the normalisation)
+// overlap.  Inlined into the fit list of the loop kernel: as a separate function under the kernel's 80-register cap
+// it saved and restored the caller's registers and its own spills through local memory on every fit's chain, and its
+// key array (kpos) lived in the stack frame; kpos is the fit list's key row in shared memory (§3, "Fit keys from
+// shared memory, fit inlined").
+// Rejected: a variant of the QR with hardware reciprocal / rsqrt seeds instead of the ~30 IEEE divisions and square
+// roots on the fit's dependent chain shortens a fit, but on exactly rank-deficient neighbourhoods (collinear lattice
+// points) its 1-ulp differences flip the pivoted QR's rank decision and change a correspondence.
+struct FitPlane { double nx, ny, nz, d; bool ok; };
+
+// The fallback, out of line: inlined, its registers shaped the allocation of the fast fit and of the kernel around it
+// (more spills in the loop kernel's per-trial-grid instantiations).  p carries the caller's (n, d) in and out, so an
+// early rejection leaves them as they were.
+__device__ __noinline__ FitPlane fit_plane_plain(const float4* pts, const int* kpos, double min_norm, double thickness,
+                                                 FitPlane p) {
+    p.ok = fit_plane_ar(pts, kpos, min_norm, thickness, p.nx, p.ny, p.nz, p.d, dla::PlainArith());
+    return p;
+}
+
+__device__ __forceinline__ bool fit_plane_reg(const Grid& g, const int* kpos, double min_norm, double thickness,
+                                           double& nx, double& ny, double& nz, double& d) {
+    bool bad = false;
+    double fx = nx, fy = ny, fz = nz, fd = d;
+    const bool ok = fit_plane_ar(g.pts, kpos, min_norm, thickness, fx, fy, fz, fd, CrArith{bad});
+    if (bad) {
+        const FitPlane p = fit_plane_plain(g.pts, kpos, min_norm, thickness, FitPlane{nx, ny, nz, d, false});
+        nx = p.nx; ny = p.ny; nz = p.nz; d = p.d;
+        return p.ok;
+    }
+    nx = fx; ny = fy; nz = fz; d = fd;
+    return ok;
 }
 
 }  // namespace corr

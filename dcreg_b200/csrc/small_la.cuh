@@ -247,12 +247,23 @@ __host__ __device__ __noinline__ void colpiv_qr_solve(double* A, double* b, doub
     for (int i = 0; i < nz; ++i) x[perm[i]] = c[i];
 }
 
+// Plain IEEE `/` and `sqrt`: the arithmetic of colpiv_qr_solve_reg unless the caller passes another with the same
+// members (the loop's plane fit passes correctly rounded primitives with a deferred range test, corr.cuh).  rcp and
+// div_by split a division whose divisor is shared: div_by(a, b, rcp(b)) is a / b.
+struct PlainArith {
+    __host__ __device__ __forceinline__ double div(double a, double b) const { return a / b; }
+    __host__ __device__ __forceinline__ double rcp(double) const { return 0.0; }
+    __host__ __device__ __forceinline__ double div_by(double a, double b, double) const { return a / b; }
+    __host__ __device__ __forceinline__ double sqrt(double a) const { return ::sqrt(a); }
+};
+
 // Same algorithm, same operations in the same order (bit-identical results, tools/test_qr_reg.cu), but every array
 // index is a compile-time constant after unrolling: the pivot column is brought to position k with conditional
 // swaps against each later column and the rank cut `nz` becomes a predicate, so A, b and the norms stay in registers
-// instead of local memory.  Used for the 5x3 plane fit, which runs once per source slot.
-template <int M, int N>
-__host__ __device__ __forceinline__ void colpiv_qr_solve_reg(double (&A)[M][N], double (&b)[M], double (&x)[N]) {
+// instead of local memory.  Used for the 5x3 plane fit, which runs once per source slot.  Every division and square
+// root goes through `ar`; with PlainArith they are the `/` and `sqrt` of colpiv_qr_solve.
+template <int M, int N, class Ar = PlainArith>
+__host__ __device__ __forceinline__ void colpiv_qr_solve_reg(double (&A)[M][N], double (&b)[M], double (&x)[N], Ar ar = Ar()) {
     const double eps = 2.220446049250313e-16;
     double normU[N], normD[N];
     int perm[N];
@@ -262,7 +273,7 @@ __host__ __device__ __forceinline__ void colpiv_qr_solve_reg(double (&A)[M][N], 
         double s = 0.0;
 #pragma unroll
         for (int i = 0; i < M; ++i) s += A[i][j] * A[i][j];
-        normU[j] = normD[j] = sqrt(s);
+        normU[j] = normD[j] = ar.sqrt(s);
         perm[j] = j;
         if (normU[j] > maxn) maxn = normU[j];
     }
@@ -298,12 +309,12 @@ __host__ __device__ __forceinline__ void colpiv_qr_solve_reg(double (&A)[M][N], 
 #pragma unroll
             for (int i = k + 1; i < M; ++i) A[i][k] = 0.0;
         } else {
-            beta = sqrt(c0 * c0 + tail);
+            beta = ar.sqrt(c0 * c0 + tail);
             if (c0 >= 0.0) beta = -beta;
-            const double inv = 1.0 / (c0 - beta);
+            const double inv = ar.div(1.0, c0 - beta);
 #pragma unroll
             for (int i = k + 1; i < M; ++i) A[i][k] *= inv;
-            tau = (beta - c0) / beta;
+            tau = ar.div(beta - c0, beta);
         }
         A[k][k] = beta;
         // apply to the remaining columns and to b
@@ -328,18 +339,18 @@ __host__ __device__ __forceinline__ void colpiv_qr_solve_reg(double (&A)[M][N], 
 #pragma unroll
         for (int j = k + 1; j < N; ++j) {
             if (normU[j] != 0.0) {
-                double t = fabs(A[k][j]) / normU[j];
+                double t = ar.div(fabs(A[k][j]), normU[j]);
                 t = (1.0 + t) * (1.0 - t);
                 if (t < 0.0) t = 0.0;
-                const double r = normU[j] / normD[j];
+                const double r = ar.div(normU[j], normD[j]);
                 const double t2 = t * r * r;
                 if (t2 <= downdate_thr) {
                     double s = 0.0;
 #pragma unroll
                     for (int i = k + 1; i < M; ++i) s += A[i][j] * A[i][j];
-                    normD[j] = normU[j] = sqrt(s);
+                    normD[j] = normU[j] = ar.sqrt(s);
                 } else {
-                    normU[j] *= sqrt(t);
+                    normU[j] *= ar.sqrt(t);
                 }
             }
         }
@@ -355,7 +366,7 @@ __host__ __device__ __forceinline__ void colpiv_qr_solve_reg(double (&A)[M][N], 
 #pragma unroll
             for (int j = i + 1; j < N; ++j)
                 if (j < nz) s -= A[i][j] * c[j];
-            c[i] = s / A[i][i];
+            c[i] = ar.div(s, A[i][i]);
         }
     }
 #pragma unroll
