@@ -37,6 +37,7 @@ HAND = {"NONE_HAND": 0, "STANDARD_REGULARIZATION": 1, "ADAPTIVE_REGULARIZATION":
 STATUS = {0: "OK", 1: "NOT_ENOUGH_POINTS", 2: "NONFINITE_UPDATE", 3: "SINGULAR_BLOCK", 4: "CUDA_ERROR",
           5: "NCCL_ERROR", 6: "BAD_ARG", 7: "NO_DEVICE"}
 OK, NOT_ENOUGH_POINTS, NONFINITE_UPDATE, SINGULAR_BLOCK, CUDA_ERROR, NCCL_ERROR, BAD_ARG, NO_DEVICE = range(8)
+LOOP_VARIANTS = 18          # instantiations of the iteration kernel (loop_plan.hpp kVariants)
 
 
 class IcpParams(C.Structure):
@@ -155,7 +156,8 @@ EXPORTS = [
     "dcreg_reduce_normal_equations", "dcreg_reduce_normal_equations_f64plane",
     "dcreg_reduce_normal_equations_host", "dcreg_analyze_and_solve", "dcreg_solve_pcg", "dcreg_icp_run",
     "dcreg_icp_run_batch", "dcreg_icp_run_scans", "dcreg_icp_run_pairs", "dcreg_icp_run_sequences", "dcreg_icp_run_odometry", "dcreg_icp_run_odometry_voxel", "dcreg_icp_run_odometry_voxel_n", "dcreg_icp_run_odometry_deskew", "dcreg_icp_run_odometry_map", "dcreg_odometry_open", "dcreg_odometry_open_map", "dcreg_odometry_push", "dcreg_odometry_push_deskew", "dcreg_odometry_local_map", "dcreg_odometry_close", "dcreg_icp_run_odometry_adaptive", "dcreg_odometry_open_adaptive", "dcreg_odometry_push_adaptive", "dcreg_icp_run_odometry_gyro", "dcreg_odometry_open_gyro", "dcreg_odometry_push_gyro", "dcreg_icp_run_odometry_imu", "dcreg_odometry_open_imu", "dcreg_odometry_push_imu", "dcreg_voxel_downsample", "dcreg_voxel_downsample_n", "dcreg_voxel_downsample_spaced", "dcreg_icp_enqueue", "dcreg_icp_fetch", "dcreg_icp_run_host_planes", "dcreg_comm_mode", "dcreg_last_covariance", "dcreg_point_to_point_metrics", "dcreg_comm_unique_id", "dcreg_comm_init",
-    "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_device_source",
+    "dcreg_comm_destroy", "dcreg_set_global_source_count", "dcreg_launch_count", "dcreg_loop_variant_launches",
+    "dcreg_device_source",
     "dcreg_device_planes_f64", "dcreg_device_planes_f32", "dcreg_freeze_planes_f32", "dcreg_time_reduce", "dcreg_time_iteration", "dcreg_iteration_counters", "dcreg_iteration_timeline",
 ]
 
@@ -288,6 +290,7 @@ def load_library():
     lib.dcreg_comm_destroy.argtypes = [vp]
     lib.dcreg_set_global_source_count.argtypes = [vp, i64]
     lib.dcreg_launch_count.argtypes = [vp]; lib.dcreg_launch_count.restype = i64
+    lib.dcreg_loop_variant_launches.argtypes = [vp, C.POINTER(i64)]
     for nm in ("dcreg_device_source", "dcreg_device_planes_f64", "dcreg_device_planes_f32"):
         getattr(lib, nm).argtypes = [vp]; getattr(lib, nm).restype = vp
     lib.dcreg_freeze_planes_f32.argtypes = [vp]
@@ -1221,6 +1224,14 @@ class Context:
     @property
     def launch_count(self) -> int:
         return int(self.lib.dcreg_launch_count(self._h))
+
+    @property
+    def loop_variant_launches(self) -> np.ndarray:
+        """Loop-kernel launches since the context was created, one count per loop_plan.hpp variant (18, int64): which
+        instantiation of the iteration kernel each call ran (include/dcreg_b200.h, dcreg_loop_variant_launches)."""
+        out = np.zeros(LOOP_VARIANTS, np.int64)
+        self._check(self.lib.dcreg_loop_variant_launches(self._h, out.ctypes.data_as(C.POINTER(C.c_int64))))
+        return out
 
     # -- clouds --
     def set_source(self, xyz):

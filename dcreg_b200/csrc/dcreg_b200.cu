@@ -1629,6 +1629,7 @@ struct dcreg_ctx {
     cudaStream_t stream = nullptr;
     std::string err;
     long long launches = 0;
+    long long loop_launches[loop_plan::kVariants] = {};   // loop kernels run, per loop_plan variant (graph replays too)
 
     DevBuf<float4> d_src; long long n_src = 0; long long n_src_total = 0;
     DevBuf<float> d_stage;                                                 // host point uploads before packing
@@ -2064,6 +2065,12 @@ int dcreg_destroy(dcreg_ctx* ctx) {
 const char* dcreg_last_error(const dcreg_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
 void* dcreg_stream(dcreg_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
 int64_t dcreg_launch_count(const dcreg_ctx* ctx) { return ctx ? ctx->launches : 0; }
+int dcreg_loop_variant_launches(const dcreg_ctx* ctx, int64_t counts[18]) {
+    static_assert(loop_plan::kVariants == 18, "dcreg_loop_variant_launches reports 18 counts");
+    if (!ctx || !counts) return DCREG_BAD_ARG;
+    for (int v = 0; v < loop_plan::kVariants; ++v) counts[v] = ctx->loop_launches[v];
+    return DCREG_OK;
+}
 void* dcreg_device_source(dcreg_ctx* ctx) { return ctx ? ctx->d_src.p : nullptr; }
 void* dcreg_device_planes_f64(dcreg_ctx* ctx) { return ctx ? ctx->d_planes64.p : nullptr; }
 void* dcreg_device_planes_f32(dcreg_ctx* ctx) { return ctx ? ctx->d_planes32.p : nullptr; }
@@ -3014,6 +3021,7 @@ static int launch_plan(dcreg_ctx* ctx, LoopPlan& L) {
     const LoopKernel& k = kLoopKernels[L.variant];
     CK(launch_pdl(k.kernel, dim3((unsigned)L.grid_x, (unsigned)L.trials), dim3(kBlock), k.smem, ctx->stream, L.b));
     ctx->launches++;
+    ctx->loop_launches[L.variant]++;
     CK(cudaGetLastError());
     return DCREG_OK;
 }
@@ -3346,7 +3354,7 @@ static int enqueue_iterations(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_param
         if (!exec) {
             cudaGraph_t graph = nullptr;
             const bool nn_valid0 = ctx->nn_valid;
-            const long long launches0 = ctx->launches;
+            const long long launches0 = ctx->launches, loop_launches0 = ctx->loop_launches[L.variant];
             cudaError_t e = cudaStreamBeginCapture(ctx->stream, cudaStreamCaptureModeRelaxed);
             int rc = DCREG_OK;
             if (e == cudaSuccess) {
@@ -3354,6 +3362,7 @@ static int enqueue_iterations(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_param
                 e = cudaStreamEndCapture(ctx->stream, &graph);
             }
             ctx->nn_valid = nn_valid0; ctx->launches = launches0;      // nothing has run yet
+            ctx->loop_launches[L.variant] = loop_launches0;
             if (e == cudaSuccess && rc == DCREG_OK && graph) e = cudaGraphInstantiate(&exec, graph, 0);
             if (graph) cudaGraphDestroy(graph);
             if (e != cudaSuccess || rc != DCREG_OK || !exec) {
@@ -3368,6 +3377,7 @@ static int enqueue_iterations(dcreg_ctx* ctx, LoopPlan& L, const dcreg_icp_param
             CK(cudaGraphLaunch(exec, ctx->stream));
             ctx->nn_valid = true;
             ctx->launches += (long long)iters * (L.k2 ? 2 : 1); ctx->graph_launches++;
+            ctx->loop_launches[L.variant] += iters;
             return DCREG_OK;
         }
     }

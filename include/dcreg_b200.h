@@ -874,6 +874,11 @@ int dcreg_set_global_source_count(dcreg_ctx* ctx, int64_t n_total);
 /* ---- instrumentation ----------------------------------------------------------------------- */
 /* Number of kernels this context has launched since creation (bench.py's gpu_launches). */
 int64_t dcreg_launch_count(const dcreg_ctx* ctx);
+/* Number of loop-kernel launches since creation, one count per instantiation of the iteration kernel: counts[v] for
+ * variant v of loop_plan.hpp (bit 0 weight derivative, bit 1 per-trial grids, bit 2 sequence lanes, bit 3 sparse row
+ * index; 16 and 17: dcreg_find_planes on a dense grid and on a sparse index).  A replayed CUDA graph counts every loop
+ * kernel it holds.  DCREG_BAD_ARG on a NULL context or array. */
+int dcreg_loop_variant_launches(const dcreg_ctx* ctx, int64_t counts[18]);
 /* Device pointers of the ctx-owned source float4 array and plane arrays (for the K1 seam). */
 void* dcreg_device_source(dcreg_ctx* ctx);
 void* dcreg_device_planes_f64(dcreg_ctx* ctx);

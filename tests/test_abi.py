@@ -1,9 +1,10 @@
 """The C-ABI library must exist in-tree, load, and export every symbol include/dcreg_b200.h declares.
-No compute calls here (no GPU on the build box)."""
+No compute calls here (no GPU on the build box); one GPU test opens a context and reads its counters."""
 import ctypes
 import os
 import re
 
+import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -55,6 +56,29 @@ def test_struct_sizes_match_c(tmp_path):
     from dcreg_b200 import api
     assert [int(x) for x in out] == [ctypes.sizeof(api.IcpParams), ctypes.sizeof(api.Analysis),
                                      ctypes.sizeof(api.IterLog)]
+
+
+def test_loop_variant_launches_symbol_and_null_context(lib):
+    """dcreg_loop_variant_launches: one count per loop_plan.hpp variant; a NULL context or array is BAD_ARG and leaves
+    the array as it was"""
+    from dcreg_b200 import api
+    assert "dcreg_loop_variant_launches" in api.EXPORTS and hasattr(lib, "dcreg_loop_variant_launches")
+    assert api.LOOP_VARIANTS == 18
+    out = np.full(api.LOOP_VARIANTS + 1, -7, np.int64)
+    assert lib.dcreg_loop_variant_launches(None, out.ctypes.data_as(ctypes.POINTER(ctypes.c_int64))) == api.BAD_ARG
+    assert (out == -7).all()
+    assert lib.dcreg_loop_variant_launches(None, None) == api.BAD_ARG
+
+
+@pytest.mark.gpu
+def test_loop_variant_launches_of_a_fresh_context(lib):
+    """A new context has launched no loop kernel: 18 zeros, and the entry after them is not written"""
+    from dcreg_b200 import api
+    with api.Context(0) as c:
+        assert c.loop_variant_launches.tolist() == [0] * api.LOOP_VARIANTS
+        out = np.full(api.LOOP_VARIANTS + 1, -7, np.int64)
+        assert lib.dcreg_loop_variant_launches(c._h, out.ctypes.data_as(ctypes.POINTER(ctypes.c_int64))) == api.OK
+        assert out[:-1].tolist() == [0] * api.LOOP_VARIANTS and out[-1] == -7
 
 
 def test_no_device_fails_loudly(lib):

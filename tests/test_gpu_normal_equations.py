@@ -25,63 +25,9 @@ from scipy.spatial import cKDTree
 import dcreg_oracle as o
 import dcreg_oracle_rows as rows
 from harness import METHODS, ctx, init_T, ties_lattice, tool_program  # noqa: F401
+from rows_harness import check_run, report
 
 F = np.float32
-STATS = {}             # label -> [records, slots, band counts {reason: n}, worst error / allowance]
-
-
-# ------------------------------------------------------------------------------------------------------------------
-# shared checks
-# ------------------------------------------------------------------------------------------------------------------
-def check_record(label, rec, src, tgt, tree, T, prm, n_total=None, lattice=False):
-    ref = rows.iteration_reference(src, tgt, tree, T, prm.search_radius, bool(prm.use_weight_derivative),
-                                   slope=prm.weight_slope, gate=prm.weight_gate, min_norm=prm.min_normal_norm,
-                                   thickness=prm.plane_thickness)
-    n_total = len(src) if n_total is None else n_total
-    H27 = np.array(rec.H27)
-    n_eff = rec.n_effective
-    sum_b2 = 2.0 * rec.objective
-    sum_r2 = rec.rmse * rec.rmse * n_eff
-    ref.allow[28] += 8 * rows.EPS * ref.sum_r2              # the rmse's square root and division
-    ratio = ref.check(H27, sum_b2, sum_r2)
-    where = (label, rec.iter)
-    assert abs(rec.n_corr_pt - ref.n_pt) <= ref.n_pt_band, where + (rec.n_corr_pt, ref.n_pt, ref.n_pt_band)
-    assert ref.n_eff_clear <= n_eff <= ref.n_eff_clear + ref.n_band, where + (n_eff, ref.n_eff_clear, ref.n_band)
-    assert np.array(rec.gradient).tobytes() == (-H27[21:]).tobytes(), where
-    assert rec.fitness == rec.n_corr_pt / n_total, where
-    worst = float(ratio.max())
-    assert worst <= 1.0, where + (int(ratio.argmax()), worst, ref.band_counts())
-    if not lattice:
-        assert ref.n_band <= 1e-3 * max(ref.n_slots, 1) + 1, where + (ref.band_counts(),)
-    st = STATS.setdefault(label, [0, 0, {}, 0.0])
-    st[0] += 1
-    st[1] += ref.n_slots
-    for k, v in ref.band_counts().items():
-        st[2][k] = st[2].get(k, 0) + v
-    st[3] = max(st[3], worst)
-    return ref
-
-
-def report(label):
-    n, slots, band, worst = STATS[label]
-    print(f"{label}: {n} records, {slots} slots, band {band or 'none'}, worst |error| / allowance {worst:.3g}")
-
-
-def poses_of(res, T0):
-    """the pose each record's iteration ran at"""
-    return [np.asarray(T0, np.float64)] + [np.array(r.T).reshape(4, 4) for r in res.logs[:-1]]
-
-
-def check_run(label, res, src, tgt, T0, prm, pick=None, tree=None, n_total=None, lattice=False):
-    tree = cKDTree(np.asarray(tgt, np.float64)) if tree is None else tree
-    poses = poses_of(res, T0)
-    done = 0
-    for i, rec in enumerate(res.logs):
-        if rec.status != 0 or (pick is not None and i not in pick):
-            continue
-        check_record(label, rec, src, tgt, tree, poses[i], prm, n_total=n_total, lattice=lattice)
-        done += 1
-    return done
 
 
 # ------------------------------------------------------------------------------------------------------------------

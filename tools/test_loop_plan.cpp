@@ -1,10 +1,12 @@
 // Host check of loop_plan.hpp (tests/test_host_la.py::test_loop_tile_plan).  plan_tiles: every slot is covered exactly
 // once per pass structure, tiles stay within the block, a single run never asks for more than the resident blocks.
 // variant / smem_class: the instantiation of the iteration kernel and its shared memory, against launch_plan's former
-// if-ladder, transcribed below, so that the table keeps launching what the ladder launched.
+// if-ladder, transcribed below, so that the table keeps launching what the ladder launched.  With --flags it prints
+// variant_flags of every variant instead.
 #include <cstdio>
 #include <cstdlib>
 #include <set>
+#include <string>
 #include <tuple>
 #include "../dcreg_b200/csrc/loop_plan.hpp"
 
@@ -78,7 +80,16 @@ static void check_variants() {
     CHECK((int)reached.size() == loop_plan::kVariants);
 }
 
-int main() {
+int main(int argc, char** argv) {
+    if (argc > 1 && std::string(argv[1]) == "--flags") {
+        // the instantiation table alone, one line per variant: v use_wd grids seq planes sparse
+        // (tests/test_gpu_loop_variants.py reads it to check its cases' expected variants)
+        for (int v = 0; v < loop_plan::kVariants; ++v) {
+            const loop_plan::Variant f = loop_plan::variant_flags(v);
+            std::printf("%d %d %d %d %d %d\n", v, f.use_wd, f.grids, f.seq, f.planes, f.sparse);
+        }
+        return 0;
+    }
     check_variants();
     const int sms[] = {1, 8, 132, 148, 160};
     long long cases = 0;
