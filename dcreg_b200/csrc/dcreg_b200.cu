@@ -59,15 +59,6 @@ constexpr int kBlock = 256;
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_release() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-__device__ __forceinline__ k1::Pose load_pose(const IcpState* st) {
-    k1::Pose P;
-#pragma unroll
-    for (int i = 0; i < 9; ++i) P.R[i] = st->R[i];
-#pragma unroll
-    for (int i = 0; i < 3; ++i) P.t[i] = st->t[i];
-    return P;
-}
-
 // K2 executed by warp 0 of the block that finished a trial's reduction (k2_solve.cuh).  A separate function with its
 // own register allocation and stack frame: the iteration kernels are capped at 85 registers for 3 blocks per SM and
 // must not pay for the solve's live state.  acc: the body-frame sums in shared memory.
@@ -244,6 +235,9 @@ struct Iter2Smem {
     int listS[kBlock], listF[kBlock];
     corr::RowRange rowtab[kSearchListMax][9];   // cell rows of the tile's listed searches (cell = radius)
     int nS, nF;
+    k1::Pose pose;                              // the trial's pose, read by the query and the row of every tile: held in
+                                                // registers across the tile it spilled (§3, "Tile loop state off the registers")
+    // (every instantiation has the members up to here: the ones without kGrids are launched with offsetof(., grid) bytes)
     corr::Grid grid;                            // this trial's own target grid (Iter2Args::grids)
     // odometry (kGrids and kSeq): the search radius of the lane's frame (Iter2Args::lane_radius, or the parameters'), its
     // square rounded up to float, and for the solve step the parameters with that radius
@@ -385,7 +379,10 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
         solver_block(a, st, sm, *a.row_epoch, peer::load_epoch(a.peer));
         return;
     }
-    const k1::Pose P = load_pose(st);
+    // (read after the first barrier of the tile loop, or of the grid copy)
+    if (tid < 9) sm.pose.R[tid] = st->R[tid];
+    else if (tid < 12) sm.pose.t[tid - 9] = st->t[tid - 9];
+    const k1::Pose& P = sm.pose;
     if constexpr (kGrids) {
         static_assert(sizeof(corr::Grid) % sizeof(int) == 0 && sizeof(corr::Grid) / sizeof(int) <= kBlock, "grid copy");
         if (tid < (int)(sizeof(corr::Grid) / sizeof(int)))
@@ -419,10 +416,8 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     const bool use_seeds = a.force ? (a.use_seeds != 0) : (coherent && st->seeds != 0);
     double c0 = 0.0, c1 = 0.0, e0 = 0.0, e1 = 0.0;
     int neff = 0, npt = 0;
-    unsigned n_search = 0, n_fit = 0;
-    double radius = A.prm.search_radius;
-    if constexpr (kGrids && kSeq) radius = sm.radius;
-    const double r2max = radius * radius;
+    // (formed where it is used: a loop-wide register spilled)
+    const auto r2max = [&]() { const double r = (kGrids && kSeq) ? sm.radius : A.prm.search_radius; return r * r; };
     {
         // ---- tiles of a.tile (<= 256) slots with per-tile work lists, so that searches and fits run densely packed.  Lean mode (the
         // pose still moves a lot) uses the same phases: every slot searches (plain 5-NN), every accepted slot fits.
@@ -432,11 +427,10 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
             if (tid == 0) { sm.nS = 0; sm.nF = 0; }
             __syncthreads();
             // -- 1. query, previous seven, certificate
-            double px = 0.0, py = 0.0, pz = 0.0;
             bool need = false;
             if (valid) {
                 const float4 p4 = __ldg(&src[i]);
-                px = (double)p4.x; py = (double)p4.y; pz = (double)p4.z;
+                const double px = (double)p4.x, py = (double)p4.y, pz = (double)p4.z;
                 // q = fl32(R p + t)  (utils.hpp:630-636)
                 const float qx = (float)(P.R[0] * px + P.R[1] * py + P.R[2] * pz + P.t[0]);
                 const float qy = (float)(P.R[3] * px + P.R[4] * py + P.R[5] * pz + P.t[1]);
@@ -474,7 +468,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                     }
                 }
                 sm.q[tid] = make_float4(qx, qy, qz, B);
-                if (need) { sm.res[tid][9] = 2; ++n_search; }
+                if (need) sm.res[tid][9] = 2;
             }
             {   // search list of the tile (slot order)
                 const unsigned bits = __ballot_sync(0xffffffffu, need);
@@ -488,6 +482,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
             // -- 2. searches: few -> one warp per listed slot (the other slots' threads are not held up by a
             //       long sequential search); many -> every thread searches for its own slot
             const int nS = sm.nS;
+            if (a.stats && tid == 0 && nS) atomicAdd(&a.stats[0], (unsigned)nS);
             if (coherent && nS <= kSearchListMax) {
                 corr::WarpKnnSmem& W = *reinterpret_cast<corr::WarpKnnSmem*>(sm.tbuf[warp]);
                 // cell = radius: the 9 cell rows of EVERY listed search are set up by all threads first (one memory round
@@ -541,15 +536,14 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                 }
                 sm.res[tid][9] = 0;
             }
-            // -- 3a. record; which five; cached plane?
-            double nx = 0.0, ny = 0.0, nz = 0.0, d = 0.0;
-            bool ok = false, want_fit = false, have5 = false;
-            float d5 = 0.0f;
+            // -- 3a. record; which five; cached plane?  The slot's plane and fit state go to sm.plane / sm.fitres, as the
+            //        fit list's do: the row reads them there, so nothing but `inr` stays live across the fits
+            bool want_fit = false, inr = false;
             if (valid) {
                 int pos[corr::kSeeds];
 #pragma unroll
                 for (int k = 0; k < corr::kSeeds; ++k) pos[k] = sm.res[tid][k];
-                d5 = __int_as_float(sm.res[tid][8]);
+                const float d5 = __int_as_float(sm.res[tid][8]);
                 if (coherent) {
                     rec_nn[kNnRec * i] = make_int4(pos[0], pos[1], pos[2], pos[3]);
                     rec_nn[kNnRec * i + 1] = make_int4(pos[4], pos[5], pos[6], sm.res[tid][7]);
@@ -559,7 +553,9 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                     }
                 }
                 // (a lean search is not bounded by the radius: its five may lie outside and then need no plane)
-                have5 = pos[4] >= 0 && (coherent || (double)d5 < r2max);
+                const bool have5 = pos[4] >= 0 && (coherent || (double)d5 < r2max());
+                inr = have5 && (double)d5 < r2max();                          // icp_test_runner.cpp:1726, 1731
+                npt += inr ? 1 : 0;
                 // The plane is a function of the five target points IN THEIR ORDER (the rows of the 5x3 system keep the
                 // reference's distance order, so the QR rounds exactly as a fresh fit would): the cache key is the
                 // ordered list.  A pure re-ranking therefore refits; the fit list keeps that cheap.
@@ -573,8 +569,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                             cached = (int)rec_fit[i];
                     }
                     if (cached == 2) {
-                        const double4 c = rec_plane[i];
-                        nx = c.x; ny = c.y; nz = c.z; d = c.w;
+                        sm.plane[tid] = rec_plane[i];
                         fit = 2;
                     } else if (cached == 1) {
                         fit = 1;
@@ -584,7 +579,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                         for (int k = 0; k < 5; ++k) sm.key[tid][k] = key[k];
                     }
                 }
-                if (!want_fit) { if (coherent) rec_fit[i] = (signed char)fit; ok = fit == 2; }
+                if (!want_fit) { if (coherent) rec_fit[i] = (signed char)fit; sm.fitres[tid] = (signed char)fit; }
             }
             {   // fit list of the tile
                 const unsigned bits = __ballot_sync(0xffffffffu, want_fit);
@@ -597,6 +592,7 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
             __syncthreads();
             // -- 3b. fits, densely packed into the first warps
             const int nF = sm.nF;
+            if (a.stats && tid == 0 && nF) atomicAdd(&a.stats[1], (unsigned)nF);
             for (int f = tid; f < nF; f += kBlock) {
                 const int t = sm.listF[f];
                 double fx = 0.0, fy = 0.0, fz = 0.0, fd = 0.0;
@@ -611,21 +607,19 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
                     for (int k = 0; k < 5; ++k) kp[k] = sm.key[t][k];
                     rec_fit[it] = (signed char)fit;
                 }
-                ++n_fit;
             }
             __syncthreads();
             DCREG_STAMP(4);
             // -- 3c. gate, row, Gram
+            double px = 0.0, py = 0.0, pz = 0.0;     // (loaded again: live across the phases they spilled)
+            double nx = 0.0, ny = 0.0, nz = 0.0, d = 0.0;
+            bool ok = false;
             if (valid) {
-                if (want_fit) {
-                    const double4 c = sm.plane[tid];
-                    nx = c.x; ny = c.y; nz = c.z; d = c.w;
-                    ok = sm.fitres[tid] == 2;
-                }
-                if (have5 && (double)d5 < r2max) npt += 1;                    // icp_test_runner.cpp:1726, 1731
-                else ok = false;
-                if (!ok) { nx = 0.0; ny = 0.0; nz = 0.0; d = 0.0; }
-                if constexpr (kPlanes) A.planes_out[__float_as_int(src[i].w)] = make_double4(nx, ny, nz, d);
+                const float4 p4 = __ldg(&src[i]);
+                px = (double)p4.x; py = (double)p4.y; pz = (double)p4.z;
+                ok = inr && sm.fitres[tid] == 2;
+                if (ok) { const double4 c = sm.plane[tid]; nx = c.x; ny = c.y; nz = c.z; d = c.w; }
+                if constexpr (kPlanes) A.planes_out[__float_as_int(p4.w)] = make_double4(nx, ny, nz, d);
             }
             double c[8];
             k1::slot_front<kUseWd>(P, px, py, pz, nx, ny, nz, d, ok, c, neff, A.prm.weight_slope, A.prm.weight_gate);
@@ -637,11 +631,6 @@ __global__ void __launch_bounds__(kBlock, 3) icp_iter2_kernel(const __grid_const
     DCREG_STAMP(5);
     // (the solver block advances the counter only after it has seen this block's flag, which carries the value read here)
     const unsigned long long row_want = solver_path ? *a.row_epoch + 1 : 0ull;
-    if (a.stats) {
-        n_search = __reduce_add_sync(0xffffffffu, n_search);
-        n_fit = __reduce_add_sync(0xffffffffu, n_fit);
-        if (lane == 0 && (n_search | n_fit)) { atomicAdd(&a.stats[0], n_search); atomicAdd(&a.stats[1], n_fit); }
-    }
     // ---- tail: the warp's 8x8 Gram -> packed totals (k1s::kPk layout), then the grid reduction
     c0 += e0; c1 += e1;
 #pragma unroll
